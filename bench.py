@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py - CTR inferences/s of the DIN forward path (BASELINE.json configs[2]).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 What is scored: DIN ranking instances (T=50, E=32, MovieLens-20M-shaped vocabularies, synthetic
 Zipf inputs, seeded random-init weights of the reference architecture) in batches of `--batch`
@@ -14,8 +14,8 @@ number of launches are in the line (`step`, `gpu_launches`).
 
 * `value`  : rows scored per second with the dataset already resident in HBM, device-timed with
              CUDA events around exactly K steps (K replays of a CUDA graph of the R launches),
-             max over ranks.  The dataset's footprint far exceeds the 126 MB L2, so every
-             launch's ids / numerics come from HBM; the 21 MB of embedding tables stay L2
+             max over ranks.  The dataset's footprint far exceeds the 50 MB L2 of the H100, so
+             every launch's ids / numerics come from HBM; the 21 MB of embedding tables stay L2
              resident by size (that is the workload's nature, see `detail.l2`).
 * `e2e`    : the same metric through the reference-facing C-ABI call with HOST buffers: one
              `srs_predict_host_batches` call per step over a pinned host dataset (H2D of each
@@ -25,7 +25,7 @@ number of launches are in the line (`step`, `gpu_launches`).
              (`srs_batch::hist16`, opt-in in the Python surface too).
 * `roofline`: algorithmic bytes per launch (SURVEY.md 8d: 7160 B/row) / device time per launch
              (timed region / launches), against the measured HBM copy bandwidth in
-             MEASURED_PEAKS.json.
+             MEASURED_PEAKS.json, or the H100 SXM data-sheet 3.35 TB/s when that file is absent.
 * `cpu_baseline`: the CPU restatement of the Keras graph (TensorFlow is not installable here)
              timed on this box's host cores on a bounded sample: oracle/ctr_oracle_c.c (plain C,
              OpenMP over rows) for DIN, the row-chunked numpy oracle for the other models.
@@ -38,9 +38,13 @@ collective (weak scaling: 4096 rows per GPU per launch); `--gather` adds the exc
 that a ranking call spanning GPUs needs (`--gather nccl`: torch NCCL all-gather per launch;
 `--gather fused`: the kernel's epilogue stores its scores into every peer's gather buffer over
 NVLink).  Each rank binds to the CPUs of its GPU's NUMA node before it allocates pinned memory.
-`--workload cfg5_din` (10^8-row table) launches directly instead of replaying a graph (`--graph`
-restores the replay; why: DESIGN.md section 6).  stdout carries the one JSON line and nothing else;
-an outer `timeout` (SIGTERM) makes the script dump its Python stacks to stderr first.
+stdout carries the one JSON line and nothing else; an outer `timeout` (SIGTERM) makes the script
+dump its Python stacks to stderr first.
+
+`--dump-outputs DIR` writes, after the timed steps, the scores the timed path computed in its last
+step as DIR/scores.npy (float32, [batches of the dataset, rows per batch]; above 60 MB a fixed
+seeded sample of the scores, with their flat indices in DIR/scores_index.npy).  The inputs and weights
+are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -64,7 +68,7 @@ for _k, _v in (("OMP_WAIT_POLICY", "PASSIVE"), ("GOMP_SPINCOUNT", "0"), ("OMP_PR
 
 METRIC = "CTR inferences/sec (DIN, batch=4096, hist_len=50)"
 WORKLOAD = "cfg3_din"
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024          # H100 SXM
 DTYPE = "bf16x3 (fp32 accumulate)"      # every MMA operand is split hi + lo, three products, fp32 accumulators
 
 # BASELINE.json configs -> (default rows per GPU per launch, metric label).  cfg3_din is the
@@ -107,8 +111,6 @@ def parse_args(argv=None):
                     help="exchange the scores after every launch (N > 1): torch NCCL all-gather, or the "
                          "kernel storing into the peers' gather buffers (fused)")
     ap.add_argument("--no-graph", action="store_true", help="launch directly instead of CUDA graphs")
-    ap.add_argument("--graph", action="store_true",
-                    help="cfg5_din only: replay a CUDA graph although that is off by default there (see below)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--streams", type=int, default=None,
@@ -122,13 +124,11 @@ def parse_args(argv=None):
                     help="distribution of the history ids (default: uniform for cfg 5 - the L2-defeating worst case "
                          "BASELINE.md asks for - Zipf(1.05) otherwise)")
     ap.add_argument("--cpu-seconds", type=float, default=10.0)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the scores of the last timed step to DIR/scores.npy (see above)")
     args = ap.parse_args(argv)
     if args.batch is None:
         args.batch = WORKLOADS[args.workload][0]
-    # cfg 5 launches directly: CUDA-graph replays of din_rt64_kernel on the 10^8-row table did not finish in
-    # 11 of 18 runs on the B200 (direct launches: 4 of 4 finished, same throughput; profiles/r02/rt64_hang/)
-    if args.workload == "cfg5_din" and not args.graph:
-        args.no_graph = True
     if args.streams is None:
         # batches in flight side by side (BASELINE.md section 3 (iii): steady-state throughput is quoted
         # with batches in flight, single-call latency separately).  cfg 5 launches fill the machine.
@@ -303,22 +303,23 @@ def measured_peaks():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s; MEASURED_PEAKS.json absent)"
+        return 3350.0, "H100 SXM data sheet 3.35 TB/s (MEASURED_PEAKS.json absent)"
 
 
-def ncu_traffic(workload, kernel_name, batch):
-    """dram read+write bytes per launch of the dominant kernel from the committed ncu summary of this
-    workload (profiles/ncu_bench_summary.json, written by profiles/summarize_r02.py from one
-    `ncu --set full` capture of `bench.py --workload W`), or None when the capture was of another
-    kernel or batch size."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_bench_summary.json")) as f:
-            rec = json.load(f)[workload]
-        if rec.get("kernel") != kernel_name or int(rec.get("batch", -1)) != int(batch):
-            return None
-        return rec.get("dram_bytes_per_launch")
-    except Exception:
-        return None
+DUMP_LIMIT_BYTES = 60 * 10 ** 6        # values + indices: the two files stay under 64 MB with headers
+
+
+def dump_outputs(directory, scores):
+    """DIR/scores.npy: float32 scores of the last timed step; above 60 MB a fixed seeded sample of
+    them, flat indices in DIR/scores_index.npy."""
+    os.makedirs(directory, exist_ok=True)
+    scores = np.ascontiguousarray(scores, dtype=np.float32)
+    if scores.nbytes > DUMP_LIMIT_BYTES:
+        n = DUMP_LIMIT_BYTES // 8                                   # values + int32 indices stay under the limit
+        idx = np.sort(np.random.default_rng(0).choice(scores.size, n, replace=False)).astype(np.int32)
+        np.save(os.path.join(directory, "scores_index.npy"), idx)
+        scores = scores.reshape(-1)[idx]
+    np.save(os.path.join(directory, "scores.npy"), scores)
 
 
 # ----------------------------------------------------------------------------------------
@@ -577,7 +578,7 @@ def run_ours(args):
     S = max(1, args.streams) if gather_mode is None else 1
     n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
     side = [torch.cuda.Stream(device=dev) for _ in range(S - 1)]
-    half_sm_kernel = False                                         # (no kernel fits two CTAs per SM at present)
+    half_sm_kernel = False                                         # (no persistent kernel fits two CTAs per SM)
     if args.sm_limit is not None:
         sm_limit = args.sm_limit
     else:
@@ -658,6 +659,8 @@ def run_ours(args):
         torch.cuda.synchronize()
         ms = ev0.elapsed_time(ev1)
     model.status()                                     # no id was out of range
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(args.dump_outputs, out.cpu().numpy())
     if S > 1:
         model.set_sm_limit(0)                          # the host legs below are single launches again
 
@@ -772,7 +775,7 @@ def run_ours(args):
             "detail": {
                 "parallelism": "dp%d: rows sharded by user-batch, weights replicated, %s" % (world, gather_note),
                 "kernel": model.kernel_name, "launch": launch_mode,
-                "l2": "the dataset (%d batches, %.0f MB) exceeds the 126 MB L2: ids / numerics are read from "
+                "l2": "the dataset (%d batches, %.0f MB) exceeds the 50 MB L2: ids / numerics are read from "
                       "HBM every launch; embedding tables total %.1f MB (%s)"
                       % (ring, ring * bytes_per_batch / 1e6,
                          4 * spec.emb_dim * (spec.n_movies + spec.n_users) / 1e6,
@@ -785,7 +788,6 @@ def run_ours(args):
             "clocks": sampler.summary(),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                          "frac": achieved / peak,
-                         "traffic": ncu_traffic(args.workload, model.kernel_name, B),
                          "algorithmic_bytes_per_launch": bpi * B, "launch_us": launch_us,
                          "peak_source": peak_src},
         }

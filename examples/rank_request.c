@@ -4,7 +4,7 @@
  * (online/recprocess/RecForYouProcess.java:40-59,113-138: candidates -> scores from the model ->
  * sort -> cut to `size`) as ONE call into libsrs_ctr.so.  This is the body a JNI shim would wrap
  * (INTEGRATION.md section B); it is compiled and linked by tests/test_host_logic.py so that the
- * header stays usable from C, and it runs on a machine with a B200:
+ * header stays usable from C, and it runs on a machine with an H100:
  *
  *   gcc -std=c99 -Iinclude examples/rank_request.c -Lsparrowrecsys_b200 -lsrs_ctr \
  *       -Wl,-rpath,$PWD/sparrowrecsys_b200 -o rank_request && ./rank_request

@@ -1,5 +1,5 @@
 /*
- * srs_ctr.h - C ABI of the B200-native SparrowRecSys CTR ranking forward path.
+ * srs_ctr.h - C ABI of the H100-native SparrowRecSys CTR ranking forward path.
  *
  * The reference has no FFI: its hot path is `model.predict(feature_dict)` on a
  * Keras graph (TFRecModel/src/com/sparrowrecsys/offline/tensorflow/<Model>.py) and, at
@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define SRS_ABI_VERSION 3
+#define SRS_ABI_VERSION 4
 
 enum srs_status {
   SRS_OK = 0,
@@ -130,7 +130,8 @@ const char* srs_last_error(void);
 int srs_model_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors,
                      int32_t device, srs_model** out);
 
-/* Same, with kernel-variant options "key=value;key=value": din_impl = rt | rtp | tc | cudacore,
+/* Same, with kernel-variant options "key=value;key=value": din_impl = tc | cudacore (rt and rtp,
+ * the names of earlier tensor-core DIN kernels, select the tc kernel),
  * embmlp_impl / deepfm_impl = tc | cudacore, zero_copy_scores = 0 | 1.  Unknown keys are ignored; a
  * forced variant that does not support the shape makes the call fail.  NULL / "" = the defaults
  * (which srs_model_kernel_name reports).  The environment variables SRS_DIN_IMPL, SRS_EMBMLP_IMPL,
@@ -206,22 +207,18 @@ int srs_model_status(srs_model* m);
 /* Algorithmic bytes per inference of this model (SURVEY.md section 8d definition). */
 int64_t srs_model_bytes_per_inference(const srs_model* m);
 
-/* Name of the kernel variant srs_predict_* dispatches to for this model.  DIN has four
- * (din_rt_kernel / din_rt64_kernel: tcgen05 row tiles; din_tc_kernel: tcgen05 per pair;
- * din_kernel: CUDA cores); the choice follows the shape and can be forced with the environment
- * variable SRS_DIN_IMPL = rt | rtp | tc | cudacore read by srs_model_create (a forced variant that does
- * not support the shape makes srs_model_create fail; rtp selects din_rtp_kernel, the row-tile kernel with
- * the phases of consecutive row groups pipelined, see csrc/din_rtp.cu).  SRS_EMBMLP_IMPL and SRS_DEEPFM_IMPL
- * (tc | cudacore) do the same for EmbeddingMLP / Wide&Deep and DeepFM. */
+/* Name of the kernel variant srs_predict_* dispatches to for this model.  DIN has two
+ * (din_wg_kernel: activation unit on warpgroup MMAs; din_kernel: CUDA cores); the choice follows
+ * the shape and can be forced with the environment variable SRS_DIN_IMPL = tc | cudacore read by
+ * srs_model_create (a forced variant that does not support the shape makes srs_model_create fail).
+ * SRS_EMBMLP_IMPL and SRS_DEEPFM_IMPL (tc | cudacore) do the same for EmbeddingMLP / Wide&Deep
+ * and DeepFM. */
 const char* srs_model_kernel_name(const srs_model* m);
 
-/* Limit the persistent tensor-core kernels of this model (din_rt / din_rt64 / din_tc /
- * embmlp_tc / deepfm_tc) to at most n_sms CTAs per launch (n_sms <= 0: every SM of the device,
- * the default).  A launch then leaves the other SMs to launches of other streams: with
- * 148 / S CTAs per launch, S consecutive batches of a pipeline run side by side on disjoint SM
- * sets, each CTA walking several row groups, so the per-launch latency chain (prologue, first
- * ids, launch gap) is paid once per S batches per SM instead of once per batch.  Takes effect
- * at the next srs_predict_* call; results do not depend on it. */
+/* Limit the persistent tensor-core kernels of this model (din_wg / embmlp_tc / deepfm_tc) to at most
+ * n_sms CTAs per launch (n_sms <= 0: every SM of the device, the default).  A launch then leaves the
+ * other SMs to launches of other streams.  Takes effect at the next srs_predict_* call; results
+ * do not depend on it. */
 int srs_model_set_sm_limit(srs_model* m, int32_t n_sms);
 
 /* Number of kernels this library has launched in this process (all models). */
@@ -279,32 +276,12 @@ int srs_model_set_movie_features(srs_model* m, int32_t n_movies, const int32_t* 
 int srs_rank_user_host(srs_model* m, const srs_user_row* user, const int32_t* candidate_movie_ids,
                        int32_t n, int32_t k, int32_t* top_idx, float* top_scores, float* probs);
 
-/* Debug aid for kernel tuning: enable/disable recording of per-phase SM-clock timestamps
- * in the tensor-core DIN kernels (CTA 0; slot meaning: profiles/trace_din_rt.py,
- * profiles/trace_din_tc.py) and, if out40 != NULL, synchronise and copy the 40 recorded values
- * out.  No effect on results. */
-int srs_debug_din_trace(srs_model* m, int32_t enable, uint64_t* out40);
-
-/* din_rtp_kernel only, with tracing enabled (srs_debug_din_trace): per-tile SM-clock timestamps of CTA 0,
- * out[kind * 64 + tile] (12 x 64 values), kinds 0 gather issued, 1 delivered, 2 weight operand built, 3 activation-unit
- * MMAs issued, 4 consumer sees the accumulators, 5 gate done, 6 pooling MMAs issued, 7 pooled rows read,
- * 8-11 inside the issuer (wait passed, MMAs issued, commits done, iteration start). */
-int srs_debug_din_timeline(srs_model* m, uint64_t* out512);
-
-/* Micro-benchmark behind the DIN kernel's MMA shape choice: SM cycles for a chain of n_mma
- * tcgen05.mma (M = 128, K = 16 bf16) with N in {32, 64, 128}, A from shared (0) or tensor (1)
- * memory, into one accumulator (two_acc bit 0 = 0) or alternating two (bit 0 = 1); bit 1 of
- * two_acc selects warp-uniform issue through elect.sync instead of a divergent single thread.
- * out2[0] = issue cycles, out2[1] = cycles until the commit barrier completes. */
-int srs_debug_umma_bench(int32_t N, int32_t n_mma, int32_t a_in_tmem, int32_t two_acc,
-                         int32_t device, uint64_t* out2);
-
-/* Known-answer self test of the tcgen05 / TMEM plumbing the DIN kernel is built on:
+/* Known-answer self test of the warpgroup-MMA (wgmma) plumbing the tensor-core kernels are built on:
  * D[128][N] = bf16(A[128][K]) * bf16(B[N][K])^T (inputs truncated to bf16, fp32 accumulate),
- * K = 64 * k_blocks (1..3), N = 16 or 32, A staged through shared memory (a_in_tmem = 0)
- * or written to tensor memory (a_in_tmem = 1).  Device pointers; synchronous. */
-int srs_selftest_umma(const float* A, const float* B, float* D, int32_t N, int32_t k_blocks,
-                      int32_t a_in_tmem, int32_t device);
+ * K = 64 * k_blocks (1..4), N = 16 or 32, A read from shared memory (a_in_regs = 0) or from
+ * registers (a_in_regs = 1).  Device pointers; synchronous. */
+int srs_selftest_wgmma(const float* A, const float* B, float* D, int32_t N, int32_t k_blocks,
+                       int32_t a_in_regs, int32_t device);
 
 #ifdef __cplusplus
 }

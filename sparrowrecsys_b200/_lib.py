@@ -14,7 +14,7 @@ SRS_OK = 0
 SRS_ERR_INVALID, SRS_ERR_MISSING, SRS_ERR_SHAPE = -1, -2, -3
 SRS_ERR_CUDA, SRS_ERR_RANGE, SRS_ERR_NOMEM = -4, -5, -6
 SRS_HOST, SRS_DEVICE_BORROWED = 0, 1
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 
 class SrsSpec(C.Structure):
@@ -42,7 +42,7 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_cosine_scores_device", "srs_topk_device", "srs_rank_host", "srs_gather_create", "srs_gather_export",
            "srs_gather_connect", "srs_gather_destroy", "srs_predict_device_gather", "srs_gather_wait",
            "srs_gather_scores", "srs_gather_copy_scores", "srs_model_set_movie_features", "srs_rank_user_host",
-           "srs_selftest_umma", "srs_debug_din_trace", "srs_debug_din_timeline", "srs_debug_umma_bench")
+           "srs_selftest_wgmma")
 
 _lib = None
 
@@ -60,7 +60,7 @@ class SrsError(RuntimeError):
 
 
 def lib_path() -> str:
-    # SRS_CTR_LIB: an alternative build of the library (kernel-tuning experiments: profiles/exp/build_variants.py)
+    # SRS_CTR_LIB: an alternative build of the library (kernel-tuning experiments)
     return os.environ.get("SRS_CTR_LIB") or _build.LIB
 
 
@@ -141,14 +141,8 @@ def load():
     lib.srs_rank_user_host.restype = C.c_int
     lib.srs_rank_user_host.argtypes = [C.c_void_p, C.POINTER(SrsUserRow), C.c_void_p, C.c_int32, C.c_int32,
                                        C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.srs_debug_din_trace.restype = C.c_int
-    lib.srs_debug_din_trace.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
-    lib.srs_debug_din_timeline.restype = C.c_int
-    lib.srs_debug_din_timeline.argtypes = [C.c_void_p, C.c_void_p]
-    lib.srs_debug_umma_bench.restype = C.c_int
-    lib.srs_debug_umma_bench.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
-    lib.srs_selftest_umma.restype = C.c_int
-    lib.srs_selftest_umma.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+    lib.srs_selftest_wgmma.restype = C.c_int
+    lib.srs_selftest_wgmma.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                       C.c_int32, C.c_int32]
     if lib.srs_abi_version() != ABI_VERSION:
         raise ImportError("libsrs_ctr.so ABI version %d != %d" % (lib.srs_abi_version(), ABI_VERSION))

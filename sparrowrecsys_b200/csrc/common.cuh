@@ -1,4 +1,4 @@
-// common.cuh - device helpers shared by the fused CTR forward kernels (sm_100a).
+// common.cuh - device helpers shared by the fused CTR forward kernels (sm_90a).
 //
 // The kernels restate the reference graphs
 // (TFRecModel/src/com/sparrowrecsys/offline/tensorflow/*.py) on a private device

@@ -1,4 +1,4 @@
-// deepfm_tc.cu - DeepFM forward with the deep MLP on the tensor cores (tcgen05 + TMEM), for
+// deepfm_tc.cu - DeepFM forward with the deep MLP on the tensor cores (warpgroup MMAs), for
 // emb_dim 13..16 (EP = 16; BASELINE cfg 2: E = 16, ML-20M vocabularies).
 //
 // Reference: TFRecModel/src/com/sparrowrecsys/offline/tensorflow/DeepFM.py:91-113.
@@ -6,17 +6,19 @@
 //   FM          : four embedding dots <item,user> <ig,ug> <ig,user> <item,ug>  (CUDA cores)
 //   deep        : [deep_item | deep_user | 7 numerics] -> Dense64-relu -> Dense64-relu
 // The two Dense(64) layers are computed transposed, D[units x rows] = W^T . X^T, with the 32
-// rows of a CTA's super-group as the MMA's N (activations hi/lo stacked along N -> N = 64) and
-// the weights (bf16 hi/lo images resident in shared memory) as its M - same scheme and same
-// bf16x3 precision as embmlp_tc.cu / din_tc.cu; the raw-scale numerics stay in fp32.
+// rows of a CTA's super-group as the MMA's N (activations hi/lo stacked along N -> m64n64k16)
+// and the 64 units (bf16 hi/lo weight images resident in shared memory) as its M - same scheme
+// and same bf16x3 precision as embmlp_tc.cu; the raw-scale numerics stay in fp32.  The CTA is
+// one warpgroup.
 #include "kernels.h"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace srs {
-using namespace umma;
+using namespace wg;
 
 constexpr int kFtRows = 32;                              // rows per super-group
-// shared-memory image: [128 (64 used) units][64 k] bf16 SW128 tiles, 16 KB each
+// shared-memory image: [128 (64 used) units][64 k] bf16 SW128 tiles, 16 KB each (layout shared with
+// model.cu's image builder; rows 64..127 are zero and not read)
 constexpr uint32_t FIMG_W1_HI = 0, FIMG_W1_LO = 16384, FIMG_W2_HI = 32768, FIMG_W2_LO = 49152;
 constexpr uint32_t FIMG_BYTES = 65536;
 // scratch
@@ -31,9 +33,8 @@ constexpr uint32_t FS_BYTES = 27648;
 __global__ void __launch_bounds__(128) deepfm_tc_kernel(const __grid_constant__ DeepFmTcParams p,
                                                         BatchView b) {
   extern __shared__ uint8_t raw[];
-  __shared__ uint64_t wbar, mbar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, warp = tid >> 5;
+  __shared__ uint64_t wbar;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, cq = lane & 3;
   uint8_t* base = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
   uint8_t* img = base;
   uint8_t* sc = base + FIMG_BYTES;
@@ -45,10 +46,8 @@ __global__ void __launch_bounds__(128) deepfm_tc_kernel(const __grid_constant__ 
   float* zp = reinterpret_cast<float*>(sc + FS_ZP);
 
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  if (tid < 32) tmem_alloc(&tmem_slot, 64);
   if (tid == 0) {
     mbar_init(&wbar, 1);
-    mbar_init(&mbar, 1);
     fence_mbar_init();
     mbar_arrive_expect_tx(&wbar, FIMG_BYTES);
     bulk_g2s(img, p.image, 32768u, &wbar);
@@ -60,20 +59,18 @@ __global__ void __launch_bounds__(128) deepfm_tc_kernel(const __grid_constant__ 
     *reinterpret_cast<uint4*>(sc + FS_X + sw128_offset(r, ch)) = make_uint4(0, 0, 0, 0);
   }
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tD = tmem_slot;
-  const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-  const uint32_t idesc = idesc_bf16(128, 2 * kFtRows);
   const uint32_t s_img = smem_u32(img), s_x = smem_u32(sc + FS_X);
-  uint32_t phase = 0;
   bool weights_ready = false;
-  const int unit = tid & 63;                             // lanes 64..127 carry zero-padded units
-  const float b1 = __ldg(p.b1 + unit), b2 = __ldg(p.b2 + unit), wdeep = __ldg(p.wdeep + unit);
-  float w1n[kNumNumerics];
+  // this thread's accumulator rows are units u_i = 16 warp + g + 8 i of both layers
+  float b1[2], b2[2], wdeep[2], w1n[2][kNumNumerics];
 #pragma unroll
-  for (int n = 0; n < kNumNumerics; ++n) w1n[n] = __ldg(p.w1num + n * 64 + unit);
+  for (int i = 0; i < 2; ++i) {
+    const int u = 16 * warp + g + 8 * i;
+    b1[i] = __ldg(p.b1 + u); b2[i] = __ldg(p.b2 + u); wdeep[i] = __ldg(p.wdeep + u);
+#pragma unroll
+    for (int n = 0; n < kNumNumerics; ++n) w1n[i][n] = __ldg(p.w1num + n * 64 + u);
+  }
 
   const int n_sg = (b.B + kFtRows - 1) / kFtRows;
   for (int sg = blockIdx.x; sg < n_sg; sg += gridDim.x) {
@@ -117,99 +114,87 @@ __global__ void __launch_bounds__(128) deepfm_tc_kernel(const __grid_constant__ 
       nums[i] = (j < kNumNumerics && row < b.B) ? __ldg(b.numerics + row * kNumNumerics + j) : 0.f;
     }
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
     if (!weights_ready) { mbar_wait(&wbar, 0); weights_ready = true; }
 
     // ---- layer 1: K = 32 (two K steps) ----------------------------------------------------------
-    if (tid == 0) {
-      tc_fence_after();
-      const uint64_t ah = smem_desc_sw128(s_img + FIMG_W1_HI), al = smem_desc_sw128(s_img + FIMG_W1_LO);
-      const uint64_t xs = smem_desc_sw128(s_x);                              // [X hi | X lo], N = 64
+    float d[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) d[i] = 0.f;
+    {
+      const uint64_t ah = desc_sw128(s_img + FIMG_W1_HI), al = desc_sw128(s_img + FIMG_W1_LO);
+      const uint64_t xs = desc_sw128(s_x);                                   // [X hi | X lo], N = 64
+      mma_fence();
 #pragma unroll
       for (int ks = 0; ks < 2; ++ks) {
-        mma_ss(tD, ah + 2 * ks, xs + 2 * ks, idesc, ks > 0);
-        mma_ss(tD, al + 2 * ks, xs + 2 * ks, idesc, 1);
+        mma_m64n64_ss(d, ah + 2 * ks, xs + 2 * ks, ks > 0);
+        mma_m64n64_ss(d, al + 2 * ks, xs + 2 * ks, 1);
       }
-      mma_commit(&mbar);
+      mma_commit();
     }
-    __syncwarp();
     {  // FM dots while the MMAs run (DeepFM.py:100-103): <item,user> <ig,ug> <ig,user> <item,ug>
-      const int r = tid >> 2, d = tid & 3;
+      const int r = tid >> 2, dd = tid & 3;
       const float* f = Fs + r * LDF;
-      const float* a = (d == 0 || d == 3) ? f : f + 32;                      // item or item_genre
-      const float* c = (d == 0 || d == 2) ? f + 16 : f + 48;                 // user or user_genre
+      const float* a = (dd == 0 || dd == 3) ? f : f + 32;                    // item or item_genre
+      const float* c = (dd == 0 || dd == 2) ? f + 16 : f + 48;               // user or user_genre
       float s = 0.f;
 #pragma unroll
       for (int k = 0; k < 16; ++k) s = fmaf(a[k], c[k], s);
       dots[tid] = s;
     }
-    mbar_wait(&mbar, phase);
-    phase ^= 1;
-    __syncwarp();
-    tc_fence_after();
-    {
-      uint32_t dh[32], dl[32];
-      tmem_ld32(tD + lane_base, dh);                     // W1 . X hi   (columns = rows 0..31)
-      tmem_ld32(tD + kFtRows + lane_base, dl);           // W1 . X lo
-      tmem_ld_wait();
-      const uint32_t chunk = (tid & 63) >> 3, within = (tid & 7) * 2;
-      if (tid < 64) {
+    mma_wait<0>();
+    reg_fence(d);
+    __syncthreads();                                     // every warp's MMAs have read X
+    // epilogue: units u_i, rows r = 8 j + 2 cq + c (X hi: column r, X lo: column 32 + r) -> H1[r][k = u_i]
 #pragma unroll
-        for (int r = 0; r < kFtRows; ++r) {
+    for (int i = 0; i < 2; ++i) {
+      const int u = 16 * warp + g + 8 * i;
+      const uint32_t chunk = u >> 3, within = (u & 7) * 2;
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int r = 8 * j + 2 * cq + c;
           const float4 n0 = *reinterpret_cast<const float4*>(nums + r * 8);
           const float4 n1 = *reinterpret_cast<const float4*>(nums + r * 8 + 4);
-          float v = (__uint_as_float(dh[r]) + __uint_as_float(dl[r])) + b1;
-          v = fmaf(n0.x, w1n[0], v); v = fmaf(n0.y, w1n[1], v); v = fmaf(n0.z, w1n[2], v);
-          v = fmaf(n0.w, w1n[3], v); v = fmaf(n1.x, w1n[4], v); v = fmaf(n1.y, w1n[5], v);
-          v = fmaf(n1.z, w1n[6], v);
+          float v = (d[4 * j + 2 * i + c] + d[4 * (j + 4) + 2 * i + c]) + b1[i];
+          v = fmaf(n0.x, w1n[i][0], v); v = fmaf(n0.y, w1n[i][1], v); v = fmaf(n0.z, w1n[i][2], v);
+          v = fmaf(n0.w, w1n[i][3], v); v = fmaf(n1.x, w1n[i][4], v); v = fmaf(n1.y, w1n[i][5], v);
+          v = fmaf(n1.z, w1n[i][6], v);
           v = fmaxf(v, 0.f);
-          const uint32_t off = sw128_offset(r, chunk) + within;               // H1[row r][k = unit]
+          const uint32_t off = sw128_offset(r, chunk) + within;
           const __nv_bfloat16 vh = __float2bfloat16_rn(v);
           *reinterpret_cast<__nv_bfloat16*>(sc + FS_X + off) = vh;
-          *reinterpret_cast<__nv_bfloat16*>(sc + FS_X + off + 4096u) =
-              __float2bfloat16_rn(v - __bfloat162float(vh));
+          *reinterpret_cast<__nv_bfloat16*>(sc + FS_X + off + 4096u) = __float2bfloat16_rn(v - __bfloat162float(vh));
         }
-      }
     }
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
     // ---- layer 2: K = 64 ----------------------------------------------------------------------------
-    if (tid == 0) {
-      tc_fence_after();
-      const uint64_t ah = smem_desc_sw128(s_img + FIMG_W2_HI), al = smem_desc_sw128(s_img + FIMG_W2_LO);
-      const uint64_t hs = smem_desc_sw128(s_x);
+    {
+      const uint64_t ah = desc_sw128(s_img + FIMG_W2_HI), al = desc_sw128(s_img + FIMG_W2_LO);
+      const uint64_t hs = desc_sw128(s_x);
+      mma_fence();
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
-        mma_ss(tD, ah + 2 * ks, hs + 2 * ks, idesc, ks > 0);
-        mma_ss(tD, al + 2 * ks, hs + 2 * ks, idesc, 1);
+        mma_m64n64_ss(d, ah + 2 * ks, hs + 2 * ks, ks > 0);
+        mma_m64n64_ss(d, al + 2 * ks, hs + 2 * ks, 1);
       }
-      mma_commit(&mbar);
+      mma_commit();
+      mma_wait<0>();
+      reg_fence(d);
     }
-    __syncwarp();
-    mbar_wait(&mbar, phase);
-    phase ^= 1;
-    __syncwarp();
-    tc_fence_after();
-    {
-      uint32_t dh[32], dl[32];
-      tmem_ld32(tD + lane_base, dh);
-      tmem_ld32(tD + kFtRows + lane_base, dl);
-      tmem_ld_wait();
-      if (tid < 64) {
 #pragma unroll
-        for (int r = 0; r < kFtRows; r += 4) {
-          float4 o;
-          o.x = fmaxf((__uint_as_float(dh[r]) + __uint_as_float(dl[r])) + b2, 0.f) * wdeep;
-          o.y = fmaxf((__uint_as_float(dh[r + 1]) + __uint_as_float(dl[r + 1])) + b2, 0.f) * wdeep;
-          o.z = fmaxf((__uint_as_float(dh[r + 2]) + __uint_as_float(dl[r + 2])) + b2, 0.f) * wdeep;
-          o.w = fmaxf((__uint_as_float(dh[r + 3]) + __uint_as_float(dl[r + 3])) + b2, 0.f) * wdeep;
-          *reinterpret_cast<float4*>(red + tid * kFtRows + r) = o;
+    for (int i = 0; i < 2; ++i) {
+      const int u = 16 * warp + g + 8 * i;
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int r = 8 * j + 2 * cq + c;
+          red[u * kFtRows + r] = fmaxf((d[4 * j + 2 * i + c] + d[4 * (j + 4) + 2 * i + c]) + b2[i], 0.f) * wdeep[i];
         }
-      }
     }
-    tc_fence_before();
     __syncthreads();
     {  // 32 rows x 4 partial sums of 16 units
       const int r = tid & 31, part = tid >> 5;
@@ -249,9 +234,6 @@ __global__ void __launch_bounds__(128) deepfm_tc_kernel(const __grid_constant__ 
     }
   }
   if (!weights_ready) mbar_wait(&wbar, 0);
-  tc_fence_before();
-  __syncthreads();
-  if (tid < 32) tmem_dealloc(tmem_slot, 64);
 }
 
 static size_t deepfm_tc_smem() { return 1024 + FIMG_BYTES + FS_BYTES; }

@@ -1,0 +1,334 @@
+// din_wg.cu - DIN forward with the activation unit on Hopper warpgroup MMAs (wgmma), E padded
+// to 32 or 64, any history length (64-position MMA tiles).
+//
+// Reference: TFRecModel/src/com/sparrowrecsys/offline/tensorflow/DIN.py:125-167.  Same math as
+// din.cu; what changes is where the per-(row, position) work of the activation unit runs:
+//
+//   * the movie table is stored pre-split, one row [EP x bf16 hi | EP x bf16 lo] per movie
+//     (x = hi + lo, both round-to-nearest), so a gathered row IS an MMA operand row: history
+//     rows go HBM/L2 -> shared memory by cp.async and are never touched by a CUDA core before
+//     the MMA;
+//   * activation unit: (h*c).Wp = h.(diag(c) Wp), so per batch row r the B operand
+//         W_r = (Wsub + Wh) + diag(c_r) Wp            [32 units x EP]
+//     is built once (fp32, then split to bf16 hi/lo) and 64 positions form one M = 64 tile:
+//         D[64 x 32] = H_hi W_hi + H_lo W_hi + H_hi W_lo    (bf16x3, fp32 accumulate)
+//   * gate (PReLU per position, Dense(1), sigmoid) on the accumulator registers, one quad of
+//     lanes per position;
+//   * pooling sum_t w_t h_t from the same shared-memory tile (h = hi + lo);
+//   * top MLP on CUDA cores over the CTA's 32-row tile, as in din.cu.
+//
+// CTA = 256 threads = two warpgroups, 32 batch rows; warpgroup q owns rows q, q + 2, ... and
+// double-buffers its history tiles (the next tile's cp.async runs under this tile's MMA and
+// epilogue; the ids of the tile after it are already on their way from HBM).  Shared memory:
+// ~105 KB (E <= 32) / ~180 KB (E <= 64).
+#include "kernels.h"
+#include "wgmma.cuh"
+
+namespace srs {
+using namespace wg;
+
+constexpr int kWgRows = 32;       // rows per CTA (top-MLP tile height, as din.cu)
+constexpr int kWgPos = 64;        // history positions per MMA tile
+
+template <int EP>
+struct DinWgLayout {
+  static constexpr int KB = EP / 32;                          // 128-byte K blocks of a [hi | lo] row
+  static constexpr uint32_t A_BYTES = KB * kWgPos * 128;      // one history tile
+  static constexpr uint32_t B_BYTES = KB * 32 * 128;          // W_r, 32 unit rows
+  static constexpr uint32_t WG_BYTES = 2 * A_BYTES + B_BYTES; // per warpgroup
+  static constexpr int KP = 5 * EP + kNumPad, LDX = KP + 4, LDH1 = 128 + 4, LDH2 = 64 + 4;
+  // fp32 region behind the operand tiles
+  static constexpr int F_X = 0;
+  static constexpr int F_H1 = F_X + kWgRows * LDX;
+  static constexpr int F_H2 = F_H1 + kWgRows * LDH1;
+  static constexpr int F_WH = F_H2 + kWgRows * LDH2;          // [EP][32] Wsub + Wh
+  static constexpr int F_WP = F_WH + EP * 32;                 // [EP][32] Wp
+  static constexpr int F_WC = F_WP + EP * 32;                 // [EP][32] Wc - Wsub
+  static constexpr int F_CST = F_WC + EP * 32;                // [32 rows][32 units] activation-unit constants
+  static constexpr int F_WG = F_CST + kWgRows * 32;           // per warpgroup: w[64] | part[128]
+  static constexpr int F_WG_STRIDE = kWgPos + 128;
+  static constexpr int F_END = F_WG + 2 * F_WG_STRIDE;
+  static constexpr size_t SMEM = 1024 + 2 * WG_BYTES + (size_t)F_END * sizeof(float);
+};
+
+// byte offset of K byte `kb` (hi part: 2 e, lo part: 2 (EP + e)) of operand row `row` in a tile of
+// `rows` rows: K blocks are `rows * 128` bytes apart
+__device__ __forceinline__ uint32_t wg_kbyte(uint32_t row, uint32_t kb, uint32_t rows) {
+  return (kb >> 7) * rows * 128u + sw128_offset(row, (kb & 127u) >> 4) + (kb & 15u);
+}
+
+template <int EP>
+__global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchView b) {
+  using L = DinWgLayout<EP>;
+  constexpr int KB = L::KB;
+  constexpr int KS = EP / 16;                     // K steps per part (hi or lo)
+  constexpr int CP = 8 * KB;                      // 16-byte chunks per split row
+  constexpr int NCOPY = kWgPos * CP / 128;        // cp.async per thread per tile
+  constexpr int PARTS = 128 / EP, PP = kWgPos / PARTS;
+  constexpr int OFF_UG = 0, OFF_U = EP, OFF_POOL = 2 * EP, OFF_C = 3 * EP, OFF_MG = 4 * EP, OFF_NUM = 5 * EP;
+  extern __shared__ uint8_t raw[];
+  uint8_t* base = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
+  float* fs = reinterpret_cast<float*>(base + 2 * L::WG_BYTES);
+  float* Xs = fs + L::F_X;
+  float* H1 = fs + L::F_H1;
+  float* H2 = fs + L::F_H2;
+  const float* wh = fs + L::F_WH;
+  const float* wp = fs + L::F_WP;
+  const float* wc = fs + L::F_WC;
+  float* cst_all = fs + L::F_CST;
+  const int tid = threadIdx.x;
+  const int q = tid >> 7, tw = tid & 127;
+  const int warp = tw >> 5, lane = tw & 31, g = lane >> 2, cq = lane & 3;
+  const int T = p.T, nch = (T + kWgPos - 1) / kWgPos;
+  uint8_t* tiles = base + q * L::WG_BYTES;        // history tiles 0, 1 | W_r
+  uint8_t* Bt = tiles + 2 * L::A_BYTES;
+  float* wsm = fs + L::F_WG + q * L::F_WG_STRIDE;
+  float* part = wsm + kWgPos;
+
+  stage_weights(fs + L::F_WH, p.au_wh, EP * 32);
+  stage_weights(fs + L::F_WP, p.au_wp, EP * 32);
+  stage_weights(fs + L::F_WC, p.au_wc, EP * 32);
+  // persistent over the batch's 32-row tiles: one tile per CTA unless srs_model_set_sm_limit caps the grid
+  const int n_tiles = (b.B + kWgRows - 1) / kWgRows;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int row0 = tile * kWgRows;
+    tile_side_features<EP, kWgRows>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users, p.n_genres,
+                                    OFF_UG, OFF_U, OFF_MG, OFF_NUM);
+    // candidate rows of the tile (ids pass through float32, DIN.py:95,125); rows past the batch end are zero
+    for (int i = tid; i < kWgRows * EP / 4; i += kThreads) {
+      const int r = i / (EP / 4), c4 = i % (EP / 4), row = row0 + r;
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (row < b.B) {
+        const int cid = checked_id(__float2int_rz(__int2float_rn(__ldg(b.movie_id + row))), p.n_movies, b.err_flag);
+        v = ldg4(p.movie + (size_t)cid * EP + 4 * c4);
+      } else {
+        *reinterpret_cast<float4*>(Xs + r * L::LDX + OFF_POOL + 4 * c4) = v;
+      }
+      *reinterpret_cast<float4*>(Xs + r * L::LDX + OFF_C + 4 * c4) = v;
+    }
+    stage_wait();
+    __syncthreads();
+    // activation-unit constant of every row: cst[r][j] = au_b[j] + sum_e c_r[e] (Wc - Wsub)[e][j]
+    for (int i = tid; i < kWgRows * 32; i += kThreads) {
+      const int r = i >> 5, j = i & 31;
+      const float* cv = Xs + r * L::LDX + OFF_C;
+      float acc = __ldg(p.au_b + j);
+  #pragma unroll 8
+      for (int e = 0; e < EP; ++e) acc = fmaf(cv[e], wc[e * 32 + j], acc);
+      cst_all[i] = acc;
+    }
+    __syncthreads();
+    // rows of this warpgroup: q, q + 2, ...; the valid ones are a prefix
+    int nrows = 0;
+    for (int r = q; r < kWgRows; r += 2)
+      if (row0 + r < b.B) ++nrows;
+
+    // gate constants of this thread's 8 accumulator columns 8 j + 2 cq + c
+    float wout[8];
+  #pragma unroll
+    for (int j = 0; j < 4; ++j)
+  #pragma unroll
+      for (int c = 0; c < 2; ++c) wout[2 * j + c] = __ldg(p.au_wout + 8 * j + 2 * cq + c);
+
+    const int n_items = nrows * nch;                // (row, 64-position chunk) pairs, chunk fastest
+    // The history ids of an item are requested (into registers) two items before its rows are gathered,
+    // so the HBM latency of the ids is not on the item chain.  Whether a slot is live is decided from its
+    // position, never from the id value: every live id goes through the range check.
+    auto item_nt = [&](int k) { return k < n_items ? min(kWgPos, T - (k % nch) * kWgPos) : 0; };
+    auto load_ids = [&](int k, int (&ids)[NCOPY]) {
+      const int row = row0 + q + 2 * (k / nch), t0 = (k % nch) * kWgPos, nt = item_nt(k);
+      const int32_t* hrow = b.hist + (size_t)row * b.hist_stride + t0;
+  #pragma unroll
+      for (int n = 0; n < NCOPY; ++n) {
+        const int pos = (tw + 128 * n) / CP;
+        ids[n] = pos < nt ? __ldg(hrow + pos) : 0;
+      }
+    };
+    auto gather = [&](int k, const int (&ids)[NCOPY]) {
+      uint8_t* A = tiles + (k & 1) * L::A_BYTES;
+      const int nt = item_nt(k);
+  #pragma unroll
+      for (int n = 0; n < NCOPY; ++n) {
+        const int i = tw + 128 * n, pos = i / CP, c = i % CP;
+        if (pos < nt) {
+          const int id = checked_id(__float2int_rz(__int2float_rn(ids[n])), p.n_movies, b.err_flag);
+          cp_async16(A + (c >> 3) * (kWgPos * 128) + sw128_offset(pos, c & 7),
+                     p.movie_split + (size_t)id * (CP * 16) + c * 16);
+        }
+      }
+    };
+
+    int ids_next[NCOPY];
+    {
+      int ids0[NCOPY];
+      load_ids(0, ids0);
+      load_ids(1, ids_next);
+      gather(0, ids0);
+    }
+    cp_async_commit();
+    float pool_acc = 0.f;
+    for (int k = 0; k < n_items; ++k) {
+      const int r = q + 2 * (k / nch), ch = k % nch, t0 = ch * kWgPos;
+      const int nt = min(kWgPos, T - t0);
+      float* xrow = Xs + r * L::LDX;
+      const float* cst = cst_all + r * 32;
+      if (ch == 0) {
+        // B operand of the row: W_r = (Wsub + Wh) + diag(c_r) Wp, split to bf16 hi / lo
+        const float* cv = xrow + OFF_C;
+        for (int i = tw; i < 32 * EP / 2; i += 128) {          // (unit j, element pair e, e + 1)
+          const int j = i / (EP / 2), e = 2 * (i % (EP / 2));
+          const float v0 = fmaf(cv[e], wp[e * 32 + j], wh[e * 32 + j]);
+          const float v1 = fmaf(cv[e + 1], wp[(e + 1) * 32 + j], wh[(e + 1) * 32 + j]);
+          const Split2 s = split_pack(v0, v1);
+          *reinterpret_cast<uint32_t*>(Bt + wg_kbyte(j, 2 * e, 32)) = s.hi;
+          *reinterpret_cast<uint32_t*>(Bt + wg_kbyte(j, 2 * (EP + e), 32)) = s.lo;
+        }
+        pool_acc = 0.f;
+      }
+      gather(k + 1, ids_next);                                // its buffer's last reader finished before the
+      cp_async_commit();                                      // closing barrier of item k - 1
+      load_ids(k + 2, ids_next);
+      // PReLU slopes of this thread's positions pr = 16 warp + g + 8 i and columns 8 j + 2 cq + c,
+      // requested before the waits below
+      float slope[2][8];
+  #pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const float* alpha = p.au_alpha + (size_t)min(t0 + 16 * warp + g + 8 * i, T - 1) * 32;
+  #pragma unroll
+        for (int j = 0; j < 4; ++j)
+  #pragma unroll
+          for (int c = 0; c < 2; ++c) slope[i][2 * j + c] = __ldg(alpha + 8 * j + 2 * cq + c);
+      }
+      cp_async_wait<1>();
+      fence_async_smem();
+      named_sync(1 + q, 128);                                 // tile k and W_r in place
+
+      // ---- activation unit: D[64 positions x 32 units], bf16x3
+      float d[16];
+  #pragma unroll
+      for (int i = 0; i < 16; ++i) d[i] = 0.f;
+      {
+        const uint32_t sa = smem_u32(tiles + (k & 1) * L::A_BYTES), sb = smem_u32(Bt);
+        mma_fence();
+  #pragma unroll
+        for (int s = 0; s < KS; ++s) {
+          const uint32_t kh = 32 * s, kl = 2 * EP + 32 * s;   // K byte of the hi / lo step
+          const uint64_t ah = desc_sw128(sa + (kh >> 7) * (kWgPos * 128) + (kh & 127));
+          const uint64_t al = desc_sw128(sa + (kl >> 7) * (kWgPos * 128) + (kl & 127));
+          const uint64_t bh = desc_sw128(sb + (kh >> 7) * (32 * 128) + (kh & 127));
+          const uint64_t bl = desc_sw128(sb + (kl >> 7) * (32 * 128) + (kl & 127));
+          mma_m64n32_ss(d, ah, bh, s > 0);
+          mma_m64n32_ss(d, al, bh, 1);
+          mma_m64n32_ss(d, ah, bl, 1);
+        }
+        mma_commit();
+        mma_wait<0>();
+        reg_fence(d);
+      }
+      // ---- gate: positions pr = 16 warp + g + 8 i; the quad of lanes sharing a position sums its 32 units
+  #pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int pr = 16 * warp + g + 8 * i;
+        float s = 0.f;
+  #pragma unroll
+        for (int j = 0; j < 4; ++j)
+  #pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int col = 8 * j + 2 * cq + c;
+            const float z = d[4 * j + 2 * i + c] + cst[col];
+            const float a = z > 0.f ? z : slope[i][2 * j + c] * z;
+            s = fmaf(a, wout[2 * j + c], s);
+          }
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        if (cq == 0) wsm[pr] = pr < nt ? 1.f / (1.f + __expf(-(s + p.au_bout))) : 0.f;
+      }
+      named_sync(1 + q, 128);
+      // ---- pooling: thread (part, e) sums positions part * PP .. + PP of element e
+      {
+        const int e = tw % EP, pt = tw / EP;
+        const uint8_t* A = tiles + (k & 1) * L::A_BYTES;
+        const uint32_t oh = 2 * e, ol = 2 * (EP + e);
+        const int pend = min(nt, (pt + 1) * PP);
+        for (int pos = pt * PP; pos < pend; ++pos) {
+          const float h = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(A + wg_kbyte(pos, oh, kWgPos))) +
+                          __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(A + wg_kbyte(pos, ol, kWgPos)));
+          pool_acc = fmaf(wsm[pos], h, pool_acc);
+        }
+        if (ch == nch - 1) {
+          part[tw] = pool_acc;
+          named_sync(1 + q, 128);
+          if (tw < EP) {
+            float v = 0.f;
+  #pragma unroll
+            for (int u = 0; u < PARTS; ++u) v += part[u * EP + tw];
+            xrow[OFF_POOL + tw] = v;
+          }
+        }
+      }
+      named_sync(1 + q, 128);                                 // tile k, wsm, part and W_r free again
+    }
+    cp_async_wait<0>();
+    __syncthreads();
+
+    // ---- top MLP on the tile ----------------------------------------------------------
+    dense_layer<kWgRows, 128, 2, 8>(Xs, L::LDX, L::KP, p.W1, p.b1, ACT_PRELU, p.a1, H1, L::LDH1);
+    __syncthreads();
+    dense_layer<kWgRows, 64, 1, 8>(H1, L::LDH1, 128, p.W2, p.b2, ACT_PRELU, p.a2, H2, L::LDH2);
+    __syncthreads();
+    row_dot<kWgRows>(H2, L::LDH2, 64, p.w3, [&](int r, float s) {
+      const int row = row0 + r;
+      if (row >= b.B) return;
+      const float z = s + p.b3;
+      store_score(b, row, sigmoidf_acc(z));
+      if (b.logits) b.logits[row] = z;
+    });
+    __syncthreads();                              // the next tile reuses every buffer
+  }
+  gather_signal_tail(b);                          // spanning ranking call: publish "slice complete"
+}
+
+// fp32 table [rows][EP] -> [rows][EP x bf16 hi | EP x bf16 lo]
+template <int EP>
+__global__ void split_table_kernel(const float* __restrict__ src, uint32_t* __restrict__ dst, int64_t n_pairs) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;   // pair index: row * EP / 2 + pair
+  if (i >= n_pairs) return;
+  const int64_t row = i / (EP / 2);
+  const int pr = (int)(i % (EP / 2));
+  const float2 v = *reinterpret_cast<const float2*>(src + row * EP + 2 * pr);
+  const Split2 s = split_pack(v.x, v.y);
+  dst[row * EP + pr] = s.hi;
+  dst[row * EP + EP / 2 + pr] = s.lo;
+}
+
+cudaError_t launch_split_table(const float* src, void* dst, int64_t rows, int EP, cudaStream_t s) {
+  const int64_t n_pairs = rows * (EP / 2);
+  const int threads = 256;
+  const int64_t blocks = (n_pairs + threads - 1) / threads;
+  if (EP == 32) split_table_kernel<32><<<(unsigned)blocks, threads, 0, s>>>(src, reinterpret_cast<uint32_t*>(dst), n_pairs);
+  else if (EP == 64) split_table_kernel<64><<<(unsigned)blocks, threads, 0, s>>>(src, reinterpret_cast<uint32_t*>(dst), n_pairs);
+  else return cudaErrorInvalidValue;
+  ++g_launch_count;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_din_wg(const DinParams& p, const BatchView& b, cudaStream_t s) {
+  if (b.B <= 0) return cudaSuccess;
+  const int n_tiles = (b.B + kWgRows - 1) / kWgRows;
+  const int blocks = p.max_ctas > 0 && p.max_ctas < n_tiles ? p.max_ctas : n_tiles;
+  ++g_launch_count;
+  if (p.EP == 32) din_wg_kernel<32><<<blocks, kThreads, DinWgLayout<32>::SMEM, s>>>(p, b);
+  else if (p.EP == 64) din_wg_kernel<64><<<blocks, kThreads, DinWgLayout<64>::SMEM, s>>>(p, b);
+  else return cudaErrorInvalidValue;
+  return cudaGetLastError();
+}
+
+cudaError_t setup_din_wg_attributes() {
+  cudaError_t e = cudaFuncSetAttribute(din_wg_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)DinWgLayout<32>::SMEM);
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(din_wg_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              (int)DinWgLayout<64>::SMEM);
+}
+
+}  // namespace srs

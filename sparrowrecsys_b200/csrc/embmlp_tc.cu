@@ -1,23 +1,24 @@
-// embmlp_tc.cu - EmbeddingMLP / Wide&Deep forward on the tensor cores (tcgen05 + TMEM) for the
-// reference shape (E <= 12: ten 12-float embedding slots = 120 of 128 K columns).
+// embmlp_tc.cu - EmbeddingMLP / Wide&Deep forward on the tensor cores (warpgroup MMAs, wgmma) for
+// the reference shape (E <= 12: ten 12-float embedding slots = 120 of 128 K columns).
 //
 // Reference: EmbeddingMLP.py:72-77 and WideNDeep.py:101-107
-// (TFRecModel/src/com/sparrowrecsys/offline/tensorflow/).  Same structure as phase 2 of
-// din_tc.cu: both Dense(128) layers are computed transposed - D[128 units x rows] =
-// W^T[128 x 128] . X^T - so the 64 rows of a super-group are the MMA's N and the weights,
-// resident in shared memory as bf16 hi/lo images, its M.  Operands are split x = hi + lo
-// (bf16x3, see din_tc.cu); the activations' hi and lo halves are stacked along N
-// ([64 rows hi | 64 rows lo]), so a layer is 8 K steps x 2 MMAs of N = 128.  The 7 raw-scale
+// (TFRecModel/src/com/sparrowrecsys/offline/tensorflow/).  Both Dense(128) layers are computed
+// transposed - D[128 units x rows] = W^T[128 x 128] . X^T - so the 64 rows of a super-group are
+// the MMA's N and the weights, resident in shared memory as bf16 hi/lo images, its M (warpgroup
+// q issues units 64 q .. 64 q + 63).  Operands are split x = hi + lo (bf16x3: hi*hi + lo*hi +
+// hi*lo, fp32 accumulate); the activations' hi and lo halves are stacked along N ([64 rows hi |
+// 64 rows lo]), so a layer is 8 K steps x 2 MMAs of m64n128k16 per warpgroup.  The 7 raw-scale
 // numerics never enter an MMA: their contribution is added in fp32 in the layer-1 epilogue.
 //
 // One persistent CTA per SM, 256 threads; per super-group of 64 rows: 30 row gathers per row
-// straight into the X operand tile, 16 MMAs, epilogue (thread = unit, 32 rows each) -> H1
-// operand tile over the X tile, 16 MMAs, epilogue, Dense(1) (+ the W&D wide weight), sigmoid.
+// straight into the X operand tile, MMAs, epilogue on the accumulator registers (thread = 2
+// units x 16 rows) -> H1 operand tile over the X tile, MMAs, epilogue, Dense(1) (+ the W&D
+// wide weight), sigmoid.
 #include "kernels.h"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace srs {
-using namespace umma;
+using namespace wg;
 
 constexpr int kEtRows = 64;                              // rows per super-group = half of the MMA N
 // shared-memory image: four 32 KB operands, each 2 K blocks x [128 units][64 k] bf16 SW128
@@ -33,9 +34,9 @@ constexpr uint32_t ES_BYTES = 68608;
 __global__ void __launch_bounds__(256, 1) embmlp_tc_kernel(const __grid_constant__ EmbMlpTcParams p,
                                                             BatchView b) {
   extern __shared__ uint8_t raw[];
-  __shared__ uint64_t wbar, mbar;
-  __shared__ uint32_t tmem_slot;
-  const int tid = threadIdx.x, wg = tid >> 7, tw = tid & 127, warp_w = tw >> 5;
+  __shared__ uint64_t wbar;
+  const int tid = threadIdx.x, q = tid >> 7, tw = tid & 127, warp_w = tw >> 5;
+  const int lane = tw & 31, g = lane >> 2, cq = lane & 3;
   uint8_t* base = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
   uint8_t* img = base;
   uint8_t* sc = base + EIMG_BYTES;
@@ -44,29 +45,25 @@ __global__ void __launch_bounds__(256, 1) embmlp_tc_kernel(const __grid_constant
   float* zp = reinterpret_cast<float*>(sc + ES_ZP);
 
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  if (tid < 32) tmem_alloc(&tmem_slot, 128);
   if (tid == 0) {
     mbar_init(&wbar, 1);
-    mbar_init(&mbar, 1);
     fence_mbar_init();
     mbar_arrive_expect_tx(&wbar, EIMG_BYTES);
     for (uint32_t off = 0; off < EIMG_BYTES; off += 32768u) bulk_g2s(img + off, p.image + off, 32768u, &wbar);
   }
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tD = tmem_slot;
-  const uint32_t lane_base = (uint32_t)(warp_w * 32) << 16;
-  const uint32_t idesc = idesc_bf16(128, 2 * kEtRows);
   const uint32_t s_img = smem_u32(img), s_x = smem_u32(sc + ES_X);
-  uint32_t phase = 0;
   bool weights_ready = false;
-  // this thread is unit `tw` of both layers
-  const float b1 = __ldg(p.b1 + tw), b2 = __ldg(p.b2 + tw), w3 = __ldg(p.w3 + tw);
-  float w1n[kNumNumerics];
+  // this thread's accumulator rows are units u_i = 64 q + 16 warp_w + g + 8 i of both layers
+  float b1[2], b2[2], w3[2], w1n[2][kNumNumerics];
 #pragma unroll
-  for (int n = 0; n < kNumNumerics; ++n) w1n[n] = __ldg(p.w1num + n * 128 + tw);
+  for (int i = 0; i < 2; ++i) {
+    const int u = 64 * q + 16 * warp_w + g + 8 * i;
+    b1[i] = __ldg(p.b1 + u); b2[i] = __ldg(p.b2 + u); w3[i] = __ldg(p.w3 + u);
+#pragma unroll
+    for (int n = 0; n < kNumNumerics; ++n) w1n[i][n] = __ldg(p.w1num + n * 128 + u);
+  }
 
   const int n_sg = (b.B + kEtRows - 1) / kEtRows;
   for (int sg = blockIdx.x; sg < n_sg; sg += gridDim.x) {
@@ -110,87 +107,63 @@ __global__ void __launch_bounds__(256, 1) embmlp_tc_kernel(const __grid_constant
       nums[i] = (j < kNumNumerics && row < b.B) ? __ldg(b.numerics + row * kNumNumerics + j) : 0.f;
     }
     fence_async_smem();
-    tc_fence_before();
     __syncthreads();
     if (!weights_ready) { mbar_wait(&wbar, 0); weights_ready = true; }
 
     // ---- two Dense(128, relu) layers ----------------------------------------------------
 #pragma unroll 1
     for (int layer = 0; layer < 2; ++layer) {
-      if (tid == 0) {
-        tc_fence_after();
-        const uint32_t a_hi = s_img + (layer == 0 ? EIMG_W1_HI : EIMG_W2_HI);
-        const uint32_t a_lo = s_img + (layer == 0 ? EIMG_W1_LO : EIMG_W2_LO);
-        uint32_t acc = 0;
+      float d[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) d[i] = 0.f;
+      {
+        const uint32_t a_hi = s_img + (layer == 0 ? EIMG_W1_HI : EIMG_W2_HI) + q * 8192;   // units 64 q ..
+        const uint32_t a_lo = s_img + (layer == 0 ? EIMG_W1_LO : EIMG_W2_LO) + q * 8192;
+        mma_fence();
 #pragma unroll
         for (int kb = 0; kb < 2; ++kb) {
-          const uint64_t ah = smem_desc_sw128(a_hi + kb * 16384), al = smem_desc_sw128(a_lo + kb * 16384);
-          const uint64_t xs = smem_desc_sw128(s_x + kb * 16384);            // [X hi | X lo], N = 128
+          const uint64_t ah = desc_sw128(a_hi + kb * 16384), al = desc_sw128(a_lo + kb * 16384);
+          const uint64_t xs = desc_sw128(s_x + kb * 16384);                 // [X hi | X lo], N = 128
 #pragma unroll
           for (int ks = 0; ks < 4; ++ks) {
-            mma_ss(tD, ah + 2 * ks, xs + 2 * ks, idesc, acc);
-            acc = 1;
-            mma_ss(tD, al + 2 * ks, xs + 2 * ks, idesc, 1);
+            mma_m64n128_ss(d, ah + 2 * ks, xs + 2 * ks, kb > 0 || ks > 0);
+            mma_m64n128_ss(d, al + 2 * ks, xs + 2 * ks, 1);
           }
         }
-        mma_commit(&mbar);
+        mma_commit();
+        mma_wait<0>();
+        reg_fence(d);
       }
-      __syncwarp();
-      mbar_wait(&mbar, phase);
-      phase ^= 1;
-      __syncwarp();
-      tc_fence_after();
-      // epilogue: unit tw, rows 32*wg .. 32*wg+31, in two halves of 16 rows
-      const uint32_t koff = (uint32_t)(tw >> 6) * 16384u;
-      const uint32_t chunk = (tw & 63) >> 3, within = (tw & 7) * 2;
+      __syncthreads();                                     // both warpgroups' MMAs have read X
+      // epilogue: units u_i, rows r = 8 j + 2 cq + c (X hi: column r, X lo: column 64 + r)
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        uint32_t dh[16], dl[16];
-        const int rbase = 32 * wg + 16 * half;
-        tmem_ld16(tD + rbase + lane_base, dh);               // W . X hi
-        tmem_ld16(tD + kEtRows + rbase + lane_base, dl);     // W . X lo
-        tmem_ld_wait();
-        if (layer == 0) {
+      for (int i = 0; i < 2; ++i) {
+        const int u = 64 * q + 16 * warp_w + g + 8 * i;
+        const uint32_t koff = (uint32_t)(u >> 6) * 16384u, chunk = (u & 63) >> 3, within = (u & 7) * 2;
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int r = rbase + i;
-            const float4 n0 = *reinterpret_cast<const float4*>(nums + r * 8);
-            const float4 n1 = *reinterpret_cast<const float4*>(nums + r * 8 + 4);
-            float v = (__uint_as_float(dh[i]) + __uint_as_float(dl[i])) + b1;
-            v = fmaf(n0.x, w1n[0], v); v = fmaf(n0.y, w1n[1], v); v = fmaf(n0.z, w1n[2], v);
-            v = fmaf(n0.w, w1n[3], v); v = fmaf(n1.x, w1n[4], v); v = fmaf(n1.y, w1n[5], v);
-            v = fmaf(n1.z, w1n[6], v);
-            v = fmaxf(v, 0.f);
-            dh[i] = __float_as_uint(v);
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int r = 8 * j + 2 * cq + c;
+            float v = d[4 * j + 2 * i + c] + d[4 * (j + 8) + 2 * i + c];
+            if (layer == 0) {
+              const float4 n0 = *reinterpret_cast<const float4*>(nums + r * 8);
+              const float4 n1 = *reinterpret_cast<const float4*>(nums + r * 8 + 4);
+              v += b1[i];
+              v = fmaf(n0.x, w1n[i][0], v); v = fmaf(n0.y, w1n[i][1], v); v = fmaf(n0.z, w1n[i][2], v);
+              v = fmaf(n0.w, w1n[i][3], v); v = fmaf(n1.x, w1n[i][4], v); v = fmaf(n1.y, w1n[i][5], v);
+              v = fmaf(n1.z, w1n[i][6], v);
+              v = fmaxf(v, 0.f);
+              const uint32_t off = koff + sw128_offset(r, chunk) + within;   // H1[row r][k = unit u]
+              const __nv_bfloat16 vh = __float2bfloat16_rn(v);
+              *reinterpret_cast<__nv_bfloat16*>(sc + ES_X + off) = vh;
+              *reinterpret_cast<__nv_bfloat16*>(sc + ES_X + off + 8192u) = __float2bfloat16_rn(v - __bfloat162float(vh));
+            } else {
+              red[u * kEtRows + r] = fmaxf(v + b2[i], 0.f) * w3[i];
+            }
           }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i)
-            dh[i] = __float_as_uint(fmaxf((__uint_as_float(dh[i]) + __uint_as_float(dl[i])) + b2, 0.f) * w3);
-        }
-        if (layer == 0) {
-          // the X tile's MMAs have completed (every thread waited on mbar), but other threads may
-          // still be reading D; H1 only overwrites shared memory, which is safe
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int r = rbase + i;
-            const float v = __uint_as_float(dh[i]);
-            const uint32_t off = koff + sw128_offset(r, chunk) + within;
-            const __nv_bfloat16 vh = __float2bfloat16_rn(v);
-            *reinterpret_cast<__nv_bfloat16*>(sc + ES_X + off) = vh;
-            *reinterpret_cast<__nv_bfloat16*>(sc + ES_X + off + 8192u) =
-                __float2bfloat16_rn(v - __bfloat162float(vh));
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; i += 4)
-            *reinterpret_cast<float4*>(red + tw * kEtRows + rbase + i) =
-                make_float4(__uint_as_float(dh[i]), __uint_as_float(dh[i + 1]), __uint_as_float(dh[i + 2]),
-                            __uint_as_float(dh[i + 3]));
-        }
       }
       fence_async_smem();
-      tc_fence_before();
       __syncthreads();
     }
     // ---- Dense(1): sum over the 128 units, + wide weight (W&D), sigmoid ------------------------
@@ -218,9 +191,6 @@ __global__ void __launch_bounds__(256, 1) embmlp_tc_kernel(const __grid_constant
     __syncthreads();
   }
   if (!weights_ready) mbar_wait(&wbar, 0);
-  tc_fence_before();
-  __syncthreads();
-  if (tid < 32) tmem_dealloc(tmem_slot, 128);
 }
 
 static size_t embmlp_tc_smem() { return 1024 + EIMG_BYTES + ES_BYTES; }

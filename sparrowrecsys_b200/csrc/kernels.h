@@ -153,6 +153,8 @@ struct DinParams {
   int n_movies, n_users, n_genres;
   int T;
   int EP;
+  const uint8_t* movie_split;  // din_wg.cu: [n_movies][EP x bf16 hi | EP x bf16 lo] (history rows)
+  int max_ctas;                // din_wg.cu: CTAs per launch, 0 = one per 32-row tile (srs_model_set_sm_limit)
 };
 
 // ---- DIEN (DIEN.py:154-256), CUDA-core kernel for E <= 32 -------------------------------------
@@ -177,83 +179,9 @@ struct DienParams {
   int EP;
 };
 
-// ---- DIN on tensor cores (din_tc.cu): E padded to 32, T <= 128 -----------------------------
-struct DinTcParams {
-  const float* movie;      // [n_movies][32]
-  const float* user;       // [n_users][32]
-  const float* ugenre;     // [19][32]
-  const float* mgenre;     // [19][32]
-  const uint8_t* image;    // shared-memory image: bf16 hi/lo SW128 operand tiles + P/Q epilogue tables
-  const float* au_wc;      // [32][32]  W_c - W_sub
-  const float* au_b;       // [32]
-  const float* b1;         // [128]
-  const float* a1;         // [128]
-  const float* w1num;      // [8][128] rows of dense/kernel that multiply the 7 numerics
-  const float* b2;         // [64]
-  const float* a2;         // [64]
-  const float* w3;         // [64]
-  float au_wout[32];
-  float au_bout;
-  float b3;
-  int n_movies, n_users, n_genres;
-  int T;
-  int CPR;                 // 32-position chunks per row = ceil(T / 32)
-  int num_sms;
-  int trace;               // debug: record phase timestamps of worker 0 (srs_debug_din_trace)
-};
-
-// din_rt.cu (E padded to 32, T <= 64) and din_rt64.cu (E padded to 64, T <= 256): history rows gathered
-// by cp.async into tcgen05 operand tiles; table pitches and the P/Q row length follow the padded E
-struct DinRtParams {
-  const float* movie;        // [n_movies][32] fp32 (candidate rows)
-  const uint8_t* movie_split;// [n_movies][32 bf16 hi | 32 bf16 lo]  (history rows)
-  const float* user;         // [n_users][32]
-  const float* ugenre;       // [19][32]
-  const float* mgenre;       // [19][32]
-  const uint8_t* image;      // W2 | W1 hi | W1 lo operand images (131072 bytes)
-  const float* waT;          // [32 units][32 e]  (Wsub + Wh)^T
-  const float* wpT;          // [32 units][32 e]  Wp^T
-  const float* pq;           // [T][64]: P_t[0..31] | Q_t[0..31]
-  const float* au_wc;        // [32][32]  W_c - W_sub
-  const float* au_b;         // [32]
-  const float* b1;           // [128]
-  const float* a1;           // [128]
-  const float* w1num;        // [8][128]
-  const float* b2;           // [64]
-  const float* a2;           // [64]
-  const float* w3;           // [64]
-  float au_bout;
-  float b3;
-  int n_movies, n_users, n_genres;
-  int T;
-  int rows_per_group;        // set by the launcher
-  int nch;                   // din_rt64: 128-position chunks per row (1 or 2)
-  int num_sms;
-  int trace;
-  // din_rtp (pipelined row-tile kernel): layer-1 weights as a tensor-memory A operand and the genre
-  // columns of the top MLP folded into fp32 tables
-  const uint32_t* w1_tmem;   // [128 units][48 words hi | 48 words lo]: packed bf16 pairs of W1^T over
-                             // K = [userId 32 | pooled 32 | candidate 32]
-  const float* gtab_u;       // [n_genres][128]: userGenre1 embedding row . its rows of dense/kernel
-  const float* gtab_m;       // [n_genres][128]: movieGenre1 likewise
-};
-
 // launchers (defined next to their kernels); return cudaGetLastError()
-cudaError_t launch_din_rt(const DinRtParams& p, const BatchView& b, cudaStream_t s);
-cudaError_t launch_split_table(const float* src, void* dst, int64_t rows, cudaStream_t s);
-cudaError_t read_din_rt_trace(unsigned long long* out40);
-cudaError_t setup_din_rt_attributes();
-cudaError_t launch_din_rtp(const DinRtParams& p, const BatchView& b, cudaStream_t s);
-cudaError_t setup_din_rtp_attributes();
-cudaError_t read_din_rtp_trace(unsigned long long* out40);
-cudaError_t take_din_rtp_abort(int* aborted, unsigned long long* rec4);
-cudaError_t read_din_rtp_timeline(unsigned long long* out768);
-cudaError_t launch_din_rt64(const DinRtParams& p, const BatchView& b, cudaStream_t s);
-cudaError_t take_din_rt64_abort(int* n, unsigned long long* rec64);   // debugging builds (-DRT64_WATCHDOG) only
-cudaError_t launch_split_table64(const float* src, void* dst, int64_t rows, cudaStream_t s);
-cudaError_t setup_din_rt64_attributes();
-cudaError_t launch_din_tc(const DinTcParams& p, const BatchView& b, cudaStream_t s);
-cudaError_t read_din_tc_trace(unsigned long long* out40);
+cudaError_t launch_din_wg(const DinParams& p, const BatchView& b, cudaStream_t s);
+cudaError_t launch_split_table(const float* src, void* dst, int64_t rows, int EP, cudaStream_t s);
 cudaError_t launch_ncf(const NcfParams& p, const BatchView& b, cudaStream_t s);
 cudaError_t launch_embmlp(const EmbMlpParams& p, const BatchView& b, cudaStream_t s);
 cudaError_t launch_embmlp_tc(const EmbMlpTcParams& p, const BatchView& b, cudaStream_t s);
@@ -266,10 +194,8 @@ int dien_seq_floats(int EP);     // size of DienParams::seq for a padded width, 
 cudaError_t setup_dien_attributes();
 cudaError_t launch_fill_uniform(float* x, int64_t n, uint64_t seed, float lo, float hi,
                                 cudaStream_t s);
-cudaError_t launch_umma_selftest(const float* A, const float* B, float* D, int N, int KB,
-                                 int a_in_tmem, cudaStream_t s);
-cudaError_t launch_umma_bench(unsigned long long* out, int N, int n_mma, int a_in_tmem, int two_acc,
-                              int uniform, cudaStream_t s);
+cudaError_t launch_wgmma_selftest(const float* A, const float* B, float* D, int N, int KB,
+                                  int a_in_regs, cudaStream_t s);
 cudaError_t launch_cosine(const float* q, const float* c, int n, int dim, float* out,
                           cudaStream_t s);
 cudaError_t launch_widen_u16(const uint16_t* src, int32_t* dst, int64_t n, cudaStream_t s);

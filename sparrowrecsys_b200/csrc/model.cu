@@ -20,10 +20,7 @@ cudaError_t setup_embmlp_attributes();
 cudaError_t setup_deepfm_attributes();
 cudaError_t setup_din_attributes();
 cudaError_t setup_dien_attributes();
-cudaError_t setup_din_tc_attributes();
-cudaError_t setup_din_rt_attributes();
-cudaError_t setup_din_rtp_attributes();
-cudaError_t setup_din_rt64_attributes();
+cudaError_t setup_din_wg_attributes();
 cudaError_t setup_embmlp_tc_attributes();
 cudaError_t setup_deepfm_tc_attributes();
 // gather.cu
@@ -129,12 +126,7 @@ struct srs_model {
   DeepFm2Params fm2{};
   DinParams din{};
   DienParams dien{};
-  DinTcParams din_tc{};
-  bool use_din_tc = false;
-  DinRtParams din_rt{};
-  bool use_din_rt = false;
-  bool use_din_rt64 = false;         // din_rt holds the parameters of din_rt64_kernel
-  bool use_din_rtp = false;          // din_rt holds the parameters; the pipelined row-tile kernel runs them
+  bool use_din_wg = false;           // din holds the parameters of din_wg_kernel
   EmbMlpTcParams emb_tc{};
   bool use_emb_tc = false;
   DeepFmTcParams fm_tc{};
@@ -145,7 +137,7 @@ struct srs_model {
                                      // of a host batch straight into the caller's pinned buffer
   void* movie_feats = nullptr;       // srs_model_set_movie_features: [n][8 words] movie-side features in HBM
   int movie_feats_rows = 0;
-  int device_sms = 148;
+  int device_sms = 132;
   int64_t bytes_per_inf = 0;
   Slot slots[kSlots + 1];
   std::mutex mu;
@@ -708,307 +700,19 @@ void write_sw128(uint8_t* dst, int rows, int kblocks, bool lo_part, F get) {
         }
 }
 
-// Fills m->din_tc from the same reference tensors build_din validated.
-int build_din_tc(Builder& B) {
+// Tensor-core DIN kernel (din_wg.cu): the movie table pre-split into bf16 hi / lo rows; every other
+// tensor is the one build_din uploaded.
+int build_din_wg(Builder& B) {
   srs_model* m = B.m;
-  const srs_spec& s = m->spec;
-  const int E = s.emb_dim, T = s.hist_len, A = 32;
-  const int h0 = s.hidden[0], h1 = s.hidden[1];
-  const int CPR = (T + 31) / 32, TP = CPR * 32;
-  const float* au = B.host("au_dense/kernel", 4 * E, A);
-  const float* alpha = B.host("au_prelu/alpha", T, A);
-  const float* auo = B.host("au_out/kernel", A, 1);
-  const float* k1 = B.host("dense/kernel", 5 * E + 7, h0);
-  const float* k2 = B.host("dense_1/kernel", h0, h1);
-  if (B.status != SRS_OK) return B.status;
-  // image offsets mirror the constants in din_tc.cu
-  const uint32_t IMG_AUB_HI = 0, IMG_AUB_LO = 4096, IMG_W1_HI = 8192, IMG_W1_LO = IMG_W1_HI + 3 * 16384,
-                 IMG_W2 = IMG_W1_LO + 3 * 16384, IMG_PQ = IMG_W2 + 2 * 16384;
-  const uint32_t kPqStride = 68;
-  const uint32_t bytes = IMG_PQ + (uint32_t)TP * kPqStride * 4u;
-  std::vector<uint8_t> img(bytes, 0);
-  // activation unit B operand: row j = [ (Wsub+Wh)[e][j], e<32 | Wp[e][j], e<32 ]
-  auto au_get = [&](int j, int k) -> float {
-    const int e = k & 31;
-    if (e >= E) return 0.f;
-    if (k < 32) return au[(size_t)e * A + j] + au[(size_t)(E + e) * A + j];
-    return au[(size_t)(3 * E + e) * A + j];
-  };
-  write_sw128(img.data() + IMG_AUB_HI, 32, 1, false, au_get);
-  write_sw128(img.data() + IMG_AUB_LO, 32, 1, true, au_get);
-  // layer 1 A operand: row = unit j, K = [userGenre1 | userId | pooled | candidate | movieGenre1 | 0] x 32
-  const int base = 3 + 4 * E;
-  const int slot_start[6] = {1, 1 + E, 3 + 2 * E, 3 + 3 * E, base + 1, -1};
-  auto w1_get = [&](int j, int k) -> float {
-    const int slot = k >> 5, e = k & 31;
-    if (j >= h0 || slot >= 5 || e >= E) return 0.f;
-    return k1[(size_t)(slot_start[slot] + e) * h0 + j];
-  };
-  write_sw128(img.data() + IMG_W1_HI, 128, 3, false, w1_get);
-  write_sw128(img.data() + IMG_W1_LO, 128, 3, true, w1_get);
-  // layer 2 A operand: rows 0..63 = hi halves of W2^T, rows 64..127 = lo halves
-  auto w2_raw = [&](int i, int k) -> float { return (i < h1 && k < h0) ? k2[(size_t)k * h1 + i] : 0.f; };
-  {
-    std::vector<uint8_t> hi(2 * 64 * 128), lo(2 * 64 * 128);
-    // build as two 64-row matrices, then interleave into 128-row tiles
-    for (int kb = 0; kb < 2; ++kb)
-      for (int r = 0; r < 128; ++r)
-        for (int c = 0; c < 8; ++c)
-          for (int i = 0; i < 8; ++i) {
-            const float x = w2_raw(r & 63, kb * 64 + c * 8 + i);
-            const uint16_t hb = bf16_rn_bits(x);
-            const uint16_t v = (r < 64) ? hb : bf16_rn_bits(x - u2f((uint32_t)hb << 16));
-            memcpy(img.data() + IMG_W2 + (size_t)kb * 16384 + sw128_off(r, c) + i * 2, &v, 2);
-          }
-  }
-  // PReLU + Dense(1) folded into two tables, one 68-float row per position t (zero beyond T):
-  //   wout_j max(v,0) + alpha_tj wout_j min(v,0) = v P_tj + |v| Q_tj
-  // stored as 16 x (P_2m, P_2m+1, Q_2m, Q_2m+1) so one 128-bit load feeds two packed FMAs
-  float* PQ = reinterpret_cast<float*>(img.data() + IMG_PQ);
-  for (int t = 0; t < T; ++t)
-    for (int j = 0; j < A; ++j) {
-      const float wo = auo[j], aw = alpha[(size_t)t * A + j] * auo[j];
-      float* cell = PQ + (size_t)t * kPqStride + (j >> 1) * 4 + (j & 1);
-      cell[0] = 0.5f * (wo + aw);
-      cell[2] = 0.5f * (wo - aw);
-    }
-  uint8_t* d_img = nullptr;
-  cudaError_t e = cudaMalloc(&d_img, bytes);
-  if (e != cudaSuccess) return fail(SRS_ERR_NOMEM, "cudaMalloc(%u) failed: %s", bytes, cudaGetErrorString(e));
-  m->owned.push_back(d_img);
-  e = cudaMemcpy(d_img, img.data(), bytes, cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "image upload failed: %s", cudaGetErrorString(e));
-  // numerics rows of dense/kernel in NUMERIC_KEYS order
-  const int nrows[7] = {base, base + 1 + E, base + 2 + E, base + 3 + E, 0, 1 + 2 * E, 2 + 2 * E};
-  std::vector<float> w1num(8 * 128, 0.f);
-  for (int n = 0; n < 7; ++n)
-    for (int j = 0; j < h0; ++j) w1num[(size_t)n * 128 + j] = k1[(size_t)nrows[n] * h0 + j];
-  DinTcParams& p = m->din_tc;
-  const DinParams& v1 = m->din;                 // reuse tables / vectors uploaded by build_din
-  p.movie = v1.movie; p.user = v1.user; p.ugenre = v1.ugenre; p.mgenre = v1.mgenre;
-  p.image = d_img;
-  p.au_wc = v1.au_wc; p.au_b = v1.au_b;
-  p.b1 = v1.b1; p.a1 = v1.a1; p.w1num = B.upload(w1num);
-  p.b2 = v1.b2; p.a2 = v1.a2; p.w3 = v1.w3;
-  for (int j = 0; j < A; ++j) p.au_wout[j] = auo[j];
-  p.au_bout = v1.au_bout; p.b3 = v1.b3;
-  p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres;
-  p.T = T; p.CPR = CPR;
-  int sms = 0;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
-  p.num_sms = sms > 0 ? sms : 148;
-  return B.status;
-}
-
-// Row-tile DIN kernel (din_rt.cu): pre-split movie table, transposed activation-unit weights,
-// P/Q gate tables and the top-MLP operand images, from the tensors build_din validated.
-int build_din_rt(Builder& B) {
-  srs_model* m = B.m;
-  const srs_spec& s = m->spec;
-  const int E = s.emb_dim, T = s.hist_len, A = 32;
-  const int h0 = s.hidden[0], h1 = s.hidden[1];
-  const float* au = B.host("au_dense/kernel", 4 * E, A);
-  const float* alpha = B.host("au_prelu/alpha", T, A);
-  const float* auo = B.host("au_out/kernel", A, 1);
-  const float* k1 = B.host("dense/kernel", 5 * E + 7, h0);
-  const float* k2 = B.host("dense_1/kernel", h0, h1);
-  if (B.status != SRS_OK) return B.status;
-  const uint32_t RI_W2 = 0, RI_W1_HI = 32768, RI_W1_LO = RI_W1_HI + 49152, RI_BYTES = RI_W1_LO + 49152;
-  std::vector<uint8_t> img(RI_BYTES, 0);
-  const int base = 3 + 4 * E;
-  const int slot_start[6] = {1, 1 + E, 3 + 2 * E, 3 + 3 * E, base + 1, -1};
-  auto w1_get = [&](int j, int k) -> float {
-    const int slot = k >> 5, e = k & 31;
-    if (j >= h0 || slot >= 5 || e >= E) return 0.f;
-    return k1[(size_t)(slot_start[slot] + e) * h0 + j];
-  };
-  write_sw128(img.data() + RI_W1_HI, 128, 3, false, w1_get);
-  write_sw128(img.data() + RI_W1_LO, 128, 3, true, w1_get);
-  auto w2_raw = [&](int i, int k) -> float { return (i < h1 && k < h0) ? k2[(size_t)k * h1 + i] : 0.f; };
-  for (int kb = 0; kb < 2; ++kb)
-    for (int r = 0; r < 128; ++r)
-      for (int c = 0; c < 8; ++c)
-        for (int i = 0; i < 8; ++i) {
-          const float x = w2_raw(r & 63, kb * 64 + c * 8 + i);
-          const uint16_t hb = bf16_rn_bits(x);
-          const uint16_t v = (r < 64) ? hb : bf16_rn_bits(x - u2f((uint32_t)hb << 16));
-          memcpy(img.data() + RI_W2 + (size_t)kb * 16384 + sw128_off(r, c) + i * 2, &v, 2);
-        }
-  uint8_t* d_img = nullptr;
-  cudaError_t e = cudaMalloc(&d_img, RI_BYTES);
-  if (e != cudaSuccess) return fail(SRS_ERR_NOMEM, "cudaMalloc(%u) failed: %s", RI_BYTES, cudaGetErrorString(e));
-  m->owned.push_back(d_img);
-  e = cudaMemcpy(d_img, img.data(), RI_BYTES, cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "image upload failed: %s", cudaGetErrorString(e));
-  // activation unit: (Wsub + Wh)^T and Wp^T, [unit j][e], zero beyond E
-  std::vector<float> waT(32 * 32, 0.f), wpT(32 * 32, 0.f);
-  for (int j = 0; j < A; ++j)
-    for (int ee = 0; ee < E; ++ee) {
-      waT[(size_t)j * 32 + ee] = au[(size_t)ee * A + j] + au[(size_t)(E + ee) * A + j];
-      wpT[(size_t)j * 32 + ee] = au[(size_t)(3 * E + ee) * A + j];
-    }
-  // PReLU + Dense(1) folded: wout_j max(v,0) + alpha_tj wout_j min(v,0) = v P_tj + |v| Q_tj
-  std::vector<float> pq((size_t)T * 64, 0.f);
-  for (int t = 0; t < T; ++t)
-    for (int j = 0; j < A; ++j) {
-      const float wo = auo[j], aw = alpha[(size_t)t * A + j] * auo[j];
-      pq[(size_t)t * 64 + j] = 0.5f * (wo + aw);
-      pq[(size_t)t * 64 + 32 + j] = 0.5f * (wo - aw);
-    }
-  const int nrows[7] = {base, base + 1 + E, base + 2 + E, base + 3 + E, 0, 1 + 2 * E, 2 + 2 * E};
-  std::vector<float> w1num(8 * 128, 0.f);
-  for (int n = 0; n < 7; ++n)
-    for (int j = 0; j < h0; ++j) w1num[(size_t)n * 128 + j] = k1[(size_t)nrows[n] * h0 + j];
-  // din_rtp: W1^T over K = [userId | pooled | candidate] as a tensor-memory A operand (lane = unit,
-  // one 32-bit column per pair of consecutive k: 48 hi words, then 48 lo words), and the two genre
-  // blocks of dense/kernel folded into fp32 tables G[genre][unit] = emb[genre] . rows (exact: 19 values)
-  std::vector<float> w1t_words((size_t)128 * 96, 0.f);
-  {
-    const int kstart[3] = {1 + E, 3 + 2 * E, 3 + 3 * E};
-    auto w1k = [&](int j, int k) -> float {
-      const int f = k >> 5, ee = k & 31;
-      if (j >= h0 || ee >= E) return 0.f;
-      return k1[(size_t)(kstart[f] + ee) * h0 + j];
-    };
-    uint32_t* words = reinterpret_cast<uint32_t*>(w1t_words.data());
-    for (int j = 0; j < 128; ++j)
-      for (int w = 0; w < 48; ++w) {
-        uint32_t hi = 0, lo = 0;
-        for (int half = 0; half < 2; ++half) {
-          const float x = w1k(j, 2 * w + half);
-          const uint16_t hb = bf16_rn_bits(x);
-          const uint16_t lb = bf16_rn_bits(x - u2f((uint32_t)hb << 16));
-          hi |= (uint32_t)hb << (16 * half);
-          lo |= (uint32_t)lb << (16 * half);
-        }
-        words[(size_t)j * 96 + w] = hi;
-        words[(size_t)j * 96 + 48 + w] = lo;
-      }
-  }
-  std::vector<float> gtab_u((size_t)s.n_genres * 128, 0.f), gtab_m((size_t)s.n_genres * 128, 0.f);
-  {
-    const float* ug = B.host("userGenre1_embedding", s.n_genres, E);
-    const float* mg = B.host("movieGenre1_embedding", s.n_genres, E);
-    if (B.status != SRS_OK) return B.status;
-    for (int g = 0; g < s.n_genres; ++g)
-      for (int j = 0; j < h0; ++j) {
-        double su = 0.0, sm = 0.0;
-        for (int ee = 0; ee < E; ++ee) {
-          su += (double)ug[(size_t)g * E + ee] * (double)k1[(size_t)(1 + ee) * h0 + j];
-          sm += (double)mg[(size_t)g * E + ee] * (double)k1[(size_t)(base + 1 + ee) * h0 + j];
-        }
-        gtab_u[(size_t)g * 128 + j] = (float)su;
-        gtab_m[(size_t)g * 128 + j] = (float)sm;
-      }
-  }
-  DinRtParams& p = m->din_rt;
-  const DinParams& v1 = m->din;                 // tables / vectors uploaded by build_din
-  p.w1_tmem = reinterpret_cast<const uint32_t*>(B.upload(w1t_words));
-  p.gtab_u = B.upload(gtab_u);
-  p.gtab_m = B.upload(gtab_m);
-  // history rows: [n_movies][32 bf16 hi | 32 bf16 lo]
+  DinParams& p = m->din;
   void* d_split = nullptr;
-  const size_t split_bytes = (size_t)s.n_movies * 128;
-  e = cudaMalloc(&d_split, split_bytes);
+  const size_t split_bytes = (size_t)m->spec.n_movies * m->EP * 4;
+  cudaError_t e = cudaMalloc(&d_split, split_bytes);
   if (e != cudaSuccess) return fail(SRS_ERR_NOMEM, "cudaMalloc(%zu) failed: %s", split_bytes, cudaGetErrorString(e));
   m->owned.push_back(d_split);
-  e = launch_split_table(v1.movie, d_split, s.n_movies, nullptr);
+  e = launch_split_table(p.movie, d_split, m->spec.n_movies, m->EP, nullptr);
   if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "table split failed: %s", cudaGetErrorString(e));
-  p.movie = v1.movie; p.movie_split = static_cast<const uint8_t*>(d_split);
-  p.user = v1.user; p.ugenre = v1.ugenre; p.mgenre = v1.mgenre;
-  p.image = d_img;
-  p.waT = B.upload(waT); p.wpT = B.upload(wpT); p.pq = B.upload(pq);
-  p.au_wc = v1.au_wc; p.au_b = v1.au_b;
-  p.b1 = v1.b1; p.a1 = v1.a1; p.w1num = B.upload(w1num);
-  p.b2 = v1.b2; p.a2 = v1.a2; p.w3 = v1.w3;
-  p.au_bout = v1.au_bout; p.b3 = v1.b3;
-  p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres;
-  p.T = T; p.rows_per_group = 32;
-  int sms = 0;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
-  p.num_sms = sms > 0 ? sms : 148;
-  return B.status;
-}
-
-// Row-tile DIN kernel for E padded to 64 (din_rt64.cu): pre-split movie table (256-byte rows),
-// transposed activation-unit weights, P/Q gate tables, top-MLP images with one K block per feature.
-int build_din_rt64(Builder& B) {
-  srs_model* m = B.m;
-  const srs_spec& s = m->spec;
-  const int E = s.emb_dim, T = s.hist_len, A = 32;
-  const int h0 = s.hidden[0], h1 = s.hidden[1];
-  const float* au = B.host("au_dense/kernel", 4 * E, A);
-  const float* alpha = B.host("au_prelu/alpha", T, A);
-  const float* auo = B.host("au_out/kernel", A, 1);
-  const float* k1 = B.host("dense/kernel", 5 * E + 7, h0);
-  const float* k2 = B.host("dense_1/kernel", h0, h1);
-  if (B.status != SRS_OK) return B.status;
-  const uint32_t W1HI = 0, W1LO = 81920, W2OFF = 163840, BYTES = 196608;
-  std::vector<uint8_t> img(BYTES, 0);
-  const int base = 3 + 4 * E;
-  const int slot_start[5] = {1, 1 + E, 3 + 2 * E, 3 + 3 * E, base + 1};   // userGenre1, userId, pooled, candidate, movieGenre1
-  auto w1_get = [&](int j, int k) -> float {
-    const int slot = k >> 6, e = k & 63;
-    if (j >= h0 || slot >= 5 || e >= E) return 0.f;
-    return k1[(size_t)(slot_start[slot] + e) * h0 + j];
-  };
-  write_sw128(img.data() + W1HI, 128, 5, false, w1_get);
-  write_sw128(img.data() + W1LO, 128, 5, true, w1_get);
-  auto w2_raw = [&](int i, int k) -> float { return (i < h1 && k < h0) ? k2[(size_t)k * h1 + i] : 0.f; };
-  for (int kb = 0; kb < 2; ++kb)
-    for (int r = 0; r < 128; ++r)
-      for (int c = 0; c < 8; ++c)
-        for (int i = 0; i < 8; ++i) {
-          const float x = w2_raw(r & 63, kb * 64 + c * 8 + i);
-          const uint16_t hb = bf16_rn_bits(x);
-          const uint16_t v = (r < 64) ? hb : bf16_rn_bits(x - u2f((uint32_t)hb << 16));
-          memcpy(img.data() + W2OFF + (size_t)kb * 16384 + sw128_off(r, c) + i * 2, &v, 2);
-        }
-  uint8_t* d_img = nullptr;
-  cudaError_t e = cudaMalloc(&d_img, BYTES);
-  if (e != cudaSuccess) return fail(SRS_ERR_NOMEM, "cudaMalloc(%u) failed: %s", BYTES, cudaGetErrorString(e));
-  m->owned.push_back(d_img);
-  e = cudaMemcpy(d_img, img.data(), BYTES, cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "image upload failed: %s", cudaGetErrorString(e));
-  std::vector<float> waT(32 * 64, 0.f), wpT(32 * 64, 0.f);
-  for (int j = 0; j < A; ++j)
-    for (int ee = 0; ee < E; ++ee) {
-      waT[(size_t)j * 64 + ee] = au[(size_t)ee * A + j] + au[(size_t)(E + ee) * A + j];
-      wpT[(size_t)j * 64 + ee] = au[(size_t)(3 * E + ee) * A + j];
-    }
-  std::vector<float> pq((size_t)T * 64, 0.f);
-  for (int t = 0; t < T; ++t)
-    for (int j = 0; j < A; ++j) {
-      const float wo = auo[j], aw = alpha[(size_t)t * A + j] * auo[j];
-      pq[(size_t)t * 64 + j] = 0.5f * (wo + aw);
-      pq[(size_t)t * 64 + 32 + j] = 0.5f * (wo - aw);
-    }
-  const int nrows[7] = {base, base + 1 + E, base + 2 + E, base + 3 + E, 0, 1 + 2 * E, 2 + 2 * E};
-  std::vector<float> w1num(8 * 128, 0.f);
-  for (int n = 0; n < 7; ++n)
-    for (int j = 0; j < h0; ++j) w1num[(size_t)n * 128 + j] = k1[(size_t)nrows[n] * h0 + j];
-  DinRtParams& p = m->din_rt;
-  const DinParams& v1 = m->din;                 // tables / vectors uploaded (or borrowed) by build_din, pitch 64
-  void* d_split = nullptr;
-  const size_t split_bytes = (size_t)s.n_movies * 256;
-  e = cudaMalloc(&d_split, split_bytes);
-  if (e != cudaSuccess) return fail(SRS_ERR_NOMEM, "cudaMalloc(%zu) failed: %s", split_bytes, cudaGetErrorString(e));
-  m->owned.push_back(d_split);
-  e = launch_split_table64(v1.movie, d_split, s.n_movies, nullptr);
-  if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "table split failed: %s", cudaGetErrorString(e));
-  p.movie = v1.movie; p.movie_split = static_cast<const uint8_t*>(d_split);
-  p.user = v1.user; p.ugenre = v1.ugenre; p.mgenre = v1.mgenre;
-  p.image = d_img;
-  p.waT = B.upload(waT); p.wpT = B.upload(wpT); p.pq = B.upload(pq);
-  p.au_wc = v1.au_wc; p.au_b = v1.au_b;
-  p.b1 = v1.b1; p.a1 = v1.a1; p.w1num = B.upload(w1num);
-  p.b2 = v1.b2; p.a2 = v1.a2; p.w3 = v1.w3;
-  p.au_bout = v1.au_bout; p.b3 = v1.b3;
-  p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres;
-  p.T = T; p.rows_per_group = 32; p.nch = T > 128 ? 2 : 1;
-  int sms = 0;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
-  p.num_sms = sms > 0 ? sms : 148;
+  p.movie_split = static_cast<const uint8_t*>(d_split);
   return B.status;
 }
 
@@ -1057,7 +761,7 @@ int build_embmlp_tc(Builder& B) {
   p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres; p.cross_buckets = s.cross_buckets;
   int sms = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
-  p.num_sms = sms > 0 ? sms : 148;
+  p.num_sms = sms > 0 ? sms : 132;
   return B.status;
 }
 
@@ -1103,7 +807,7 @@ int build_deepfm_tc(Builder& B) {
   p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres;
   int sms = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
-  p.num_sms = sms > 0 ? sms : 148;
+  p.num_sms = sms > 0 ? sms : 132;
   return B.status;
 }
 
@@ -1155,11 +859,7 @@ int launch(srs_model* m, const BatchView& v, cudaStream_t stream) {
       break;
     case SRS_DEEPFM_V2: e = launch_deepfm2(m->fm2, v, stream); break;
     case SRS_DIN:
-      e = m->use_din_rt64 ? launch_din_rt64(m->din_rt, v, stream)
-          : m->use_din_rtp ? launch_din_rtp(m->din_rt, v, stream)
-          : m->use_din_rt ? launch_din_rt(m->din_rt, v, stream)
-          : m->use_din_tc ? launch_din_tc(m->din_tc, v, stream)
-                          : launch_din(m->din, v, stream);
+      e = m->use_din_wg ? launch_din_wg(m->din, v, stream) : launch_din(m->din, v, stream);
       break;
     case SRS_DIEN: e = launch_dien(m->dien, v, stream); break;
     default: return fail(SRS_ERR_INVALID, "unknown model kind");
@@ -1383,9 +1083,7 @@ int srs_model_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_
   CUDA_TRY(setup_deepfm_attributes());
   CUDA_TRY(setup_din_attributes());
   CUDA_TRY(setup_dien_attributes());
-  CUDA_TRY(setup_din_tc_attributes());
-  CUDA_TRY(setup_din_rt_attributes());
-  CUDA_TRY(setup_din_rt64_attributes());
+  CUDA_TRY(setup_din_wg_attributes());
   CUDA_TRY(setup_embmlp_tc_attributes());
   CUDA_TRY(setup_deepfm_tc_attributes());
 
@@ -1399,7 +1097,7 @@ int srs_model_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_
   {
     int sms = 0;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    m->device_sms = sms > 0 ? sms : 148;
+    m->device_sms = sms > 0 ? sms : 132;
   }
   m->EP = round_ep(spec->emb_dim);
   m->hist_cols = (spec->kind == SRS_DIN || spec->kind == SRS_DIEN) ? spec->hist_len
@@ -1458,50 +1156,25 @@ int srs_model_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_
     case SRS_DIEN: rc = build_dien(B); break;
     default: {
       rc = build_din(B);
-      // kernel selection (SRS_DIN_IMPL=cudacore|tc|rt overrides; tc / rt fail loudly on an unsupported shape):
-      //   rt  row-tile kernels: E padded to 32 and T in 9..64 (din_rt), E padded to 64 and T in 9..256 (din_rt64)
-      //   tc  per-pair tensor-core kernel, E padded to 32 and T in 9..128
+      // kernel selection (SRS_DIN_IMPL=cudacore|tc overrides; tc fails loudly on an unsupported shape):
+      //   tc  activation unit on warpgroup MMAs (din_wg.cu): E padded to 32 or 64.  The default for E
+      //       padded to 64 and T > 8, where it measured faster on the H100 (BASELINE cfg 5: 12.6 vs 8.6 M
+      //       inferences/s); for E <= 32 the CUDA-core kernel measured slightly faster (cfg 3: 58.0 vs 57.3 M).
+      //   rt, rtp  the names of the earlier row-tile tensor-core kernels; callers that pass them get the
+      //       same tensor-core kernel as tc.
       const char* impl_c = opt("din_impl", "SRS_DIN_IMPL");
       const std::string impl_s = impl_c ? impl_c : "";
       const char* impl = impl_c ? impl_s.c_str() : nullptr;
-      const bool fits_tc = m->EP == 32 && spec->hist_len <= 128;
-      const bool fits_rt32 = m->EP == 32 && spec->hist_len <= 64;
-      const bool fits_rt64 = m->EP == 64 && spec->hist_len <= 256;
-      const bool fits_rt = fits_rt32 || fits_rt64;
-      bool want_rt = fits_rt && spec->hist_len > 8;
-      bool want_tc = !want_rt && fits_tc && spec->hist_len > 8;
-      if (impl && !strcmp(impl, "cudacore")) want_rt = want_tc = false;
-      if (impl && !strcmp(impl, "tc")) {
-        if (!fits_tc && rc == SRS_OK) rc = fail(SRS_ERR_INVALID, "SRS_DIN_IMPL=tc needs 16 < emb_dim <= 32 and hist_len <= 128");
-        want_tc = true; want_rt = false;
-      }
-      const bool want_rtp = impl && !strcmp(impl, "rtp");       // pipelined row-tile kernel (din_rtp.cu)
-      if (want_rtp) {
-        if (!fits_rt32 && rc == SRS_OK)
-          rc = fail(SRS_ERR_INVALID, "SRS_DIN_IMPL=rtp needs 16 < emb_dim <= 32 and hist_len <= 64");
-        want_rt = true; want_tc = false;
-      }
-      if (impl && !strcmp(impl, "rt")) {
-        if (!fits_rt && rc == SRS_OK)
-          rc = fail(SRS_ERR_INVALID, "SRS_DIN_IMPL=rt needs 16 < emb_dim <= 32 and hist_len <= 64, or 32 < emb_dim <= 64 and hist_len <= 256");
-        want_rt = true; want_tc = false;
+      const bool fits_tc = m->EP == 32 || m->EP == 64;
+      bool want_tc = m->EP == 64 && spec->hist_len > 8;
+      if (impl && !strcmp(impl, "cudacore")) want_tc = false;
+      if (impl && (!strcmp(impl, "tc") || !strcmp(impl, "rt") || !strcmp(impl, "rtp"))) {
+        if (!fits_tc && rc == SRS_OK) rc = fail(SRS_ERR_INVALID, "SRS_DIN_IMPL=%s needs 16 < emb_dim <= 64", impl);
+        want_tc = true;
       }
       if (rc == SRS_OK && want_tc) {
-        rc = build_din_tc(B);
-        if (rc == SRS_OK) { m->use_din_tc = true; m->kernel_name = "din_tc_kernel"; }
-      }
-      if (rc == SRS_OK && want_rt && fits_rt32) {
-        rc = build_din_rt(B);
-        if (rc == SRS_OK) { m->use_din_rt = true; m->kernel_name = "din_rt_kernel"; }
-        if (rc == SRS_OK && want_rtp) {
-          cudaError_t ea = setup_din_rtp_attributes();
-          if (ea != cudaSuccess) rc = fail(SRS_ERR_CUDA, "din_rtp attribute setup failed: %s", cudaGetErrorString(ea));
-          m->use_din_rt = false; m->use_din_rtp = true; m->kernel_name = "din_rtp_kernel";
-        }
-      }
-      if (rc == SRS_OK && want_rt && fits_rt64) {
-        rc = build_din_rt64(B);
-        if (rc == SRS_OK) { m->use_din_rt64 = true; m->kernel_name = "din_rt64_kernel"; }
+        rc = build_din_wg(B);
+        if (rc == SRS_OK) { m->use_din_wg = true; m->kernel_name = "din_wg_kernel"; }
       }
       break;
     }
@@ -1609,7 +1282,7 @@ int srs_predict_device_gather(srs_model* m, const srs_batch* b, srs_gather* gg, 
   v.movie_id = b->movie_id; v.user_id = b->user_id; v.hist = b->hist;
   v.movie_genre = b->movie_genre; v.user_genre = b->user_genre; v.numerics = b->numerics;
   v.logits = nullptr; v.err_flag = m->err_flag;
-  const bool in_kernel = m->spec.kind == SRS_DIN && (m->use_din_rtp || m->use_din_rt) ;   // kernels ending in gather_signal_tail()
+  const bool in_kernel = m->spec.kind == SRS_DIN && m->use_din_wg;   // kernels ending in gather_signal_tail()
   gather_begin_step(g, v, in_kernel);
   rc = launch(m, v, static_cast<cudaStream_t>(stream));
   if (rc != SRS_OK) return rc;
@@ -1727,27 +1400,6 @@ int srs_model_status(srs_model* m) {
   if (!m) return fail(SRS_ERR_INVALID, "null model");
   CUDA_TRY(cudaSetDevice(m->device));
   CUDA_TRY(cudaDeviceSynchronize());
-  if (m->use_din_rtp) {                              // a protocol error in din_rtp_kernel ends the launch, see rtp_wait
-    int aborted = 0;
-    unsigned long long rec[4] = {0, 0, 0, 0};
-    CUDA_TRY(take_din_rtp_abort(&aborted, rec));
-    if (aborted)
-      return fail(SRS_ERR_CUDA, "din_rtp_kernel: an mbarrier wait timed out (wait code %llu, block %llu, thread %llu, "
-                  "parity %llu); the scores of that launch are invalid", rec[0], rec[1], rec[2], rec[3]);
-  }
-  if (m->spec.kind == SRS_DIN) {                     // -DRT64_WATCHDOG builds of din_rt64.cu only
-    int n = 0;
-    unsigned long long rec[64];
-    CUDA_TRY(take_din_rt64_abort(&n, rec));
-    if (n > 0) {
-      char msg[900];
-      int at = snprintf(msg, sizeof(msg), "din_rt64_kernel: %d mbarrier wait(s) timed out [line/block/thread/parity]:", n);
-      for (int i = 0; i < n && at < (int)sizeof(msg) - 60; ++i)
-        at += snprintf(msg + at, sizeof(msg) - at, " %llu/%llu/%llu/%llu", rec[4 * i], rec[4 * i + 1],
-                       rec[4 * i + 2] & 0xffffffffull, rec[4 * i + 3]);
-      return fail(SRS_ERR_CUDA, "%s", msg);
-    }
-  }
   int flags[kErrWords] = {0};
   CUDA_TRY(cudaMemcpy(flags, m->err_flag, kErrWords * sizeof(int), cudaMemcpyDeviceToHost));
   bool any = false;
@@ -1767,10 +1419,9 @@ int srs_model_set_sm_limit(srs_model* m, int32_t n_sms) {
   if (!m) return fail(SRS_ERR_INVALID, "null model");
   const int n = (n_sms <= 0 || n_sms > m->device_sms) ? m->device_sms : n_sms;
   std::lock_guard<std::mutex> lock(m->mu);
-  m->din_rt.num_sms = n;
-  m->din_tc.num_sms = n;
   m->emb_tc.num_sms = n;
   m->fm_tc.num_sms = n;
+  m->din.max_ctas = n < m->device_sms ? n : 0;
   return SRS_OK;
 }
 
@@ -1953,49 +1604,11 @@ int srs_rank_user_host(srs_model* m, const srs_user_row* user, const int32_t* ca
   return rc;
 }
 
-int srs_debug_din_trace(srs_model* m, int32_t enable, uint64_t* out40) {
-  if (!m) return fail(SRS_ERR_INVALID, "null model");
-  CUDA_TRY(cudaSetDevice(m->device));
-  m->din_tc.trace = enable;
-  m->din_rt.trace = enable;
-  if (out40) {
-    CUDA_TRY(cudaDeviceSynchronize());
-    if (m->use_din_rtp) CUDA_TRY(read_din_rtp_trace(reinterpret_cast<unsigned long long*>(out40)));
-    else if (m->use_din_rt) CUDA_TRY(read_din_rt_trace(reinterpret_cast<unsigned long long*>(out40)));
-    else CUDA_TRY(read_din_tc_trace(reinterpret_cast<unsigned long long*>(out40)));
-  }
-  return SRS_OK;
-}
-
-int srs_debug_din_timeline(srs_model* m, uint64_t* out512) {   /* 12 x 64 values */
-  if (!m || !out512) return fail(SRS_ERR_INVALID, "null argument");
-  if (!m->use_din_rtp) return fail(SRS_ERR_INVALID, "the per-tile timeline exists for din_rtp_kernel only");
-  CUDA_TRY(cudaSetDevice(m->device));
-  CUDA_TRY(cudaDeviceSynchronize());
-  CUDA_TRY(read_din_rtp_timeline(reinterpret_cast<unsigned long long*>(out512)));
-  return SRS_OK;
-}
-
-int srs_debug_umma_bench(int32_t N, int32_t n_mma, int32_t a_in_tmem, int32_t two_acc,
-                         int32_t device, uint64_t* out2) {
-  if (!out2 || (N != 32 && N != 64 && N != 128) || n_mma < 1 || n_mma > 4096)
-    return fail(SRS_ERR_INVALID, "bad argument");
-  CUDA_TRY(cudaSetDevice(device));
-  unsigned long long* d = nullptr;
-  CUDA_TRY(cudaMalloc(&d, 16));
-  cudaError_t e = launch_umma_bench(d, N, n_mma, a_in_tmem & 1, two_acc & 1, (two_acc >> 1) & 1, nullptr);
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e == cudaSuccess) e = cudaMemcpy(out2, d, 16, cudaMemcpyDeviceToHost);
-  cudaFree(d);
-  if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "umma bench failed: %s", cudaGetErrorString(e));
-  return SRS_OK;
-}
-
-int srs_selftest_umma(const float* A, const float* B, float* D, int32_t N, int32_t k_blocks,
-                      int32_t a_in_tmem, int32_t device) {
+int srs_selftest_wgmma(const float* A, const float* B, float* D, int32_t N, int32_t k_blocks,
+                       int32_t a_in_regs, int32_t device) {
   if (!A || !B || !D) return fail(SRS_ERR_INVALID, "null pointer");
   CUDA_TRY(cudaSetDevice(device));
-  CUDA_TRY(launch_umma_selftest(A, B, D, N, k_blocks, a_in_tmem, nullptr));
+  CUDA_TRY(launch_wgmma_selftest(A, B, D, N, k_blocks, a_in_regs, nullptr));
   CUDA_TRY(cudaDeviceSynchronize());
   return SRS_OK;
 }

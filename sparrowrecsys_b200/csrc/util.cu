@@ -27,7 +27,7 @@ cudaError_t launch_fill_uniform(float* x, int64_t n, uint64_t seed, float lo, fl
   if (n <= 0) return cudaSuccess;
   const int threads = 256;
   int64_t blocks = (n + threads - 1) / threads;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   fill_uniform_kernel<<<(int)blocks, threads, 0, s>>>(x, n, seed, lo, hi);
   ++g_launch_count;
   return cudaGetLastError();
@@ -51,7 +51,7 @@ cudaError_t launch_widen_u16(const uint16_t* src, int32_t* dst, int64_t n, cudaS
   const int threads = 256;
   int64_t blocks = ((n >> 1) + threads - 1) / threads;
   if (blocks < 1) blocks = 1;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   widen_u16_kernel<<<(int)blocks, threads, 0, s>>>(src, dst, n);
   ++g_launch_count;
   return cudaGetLastError();
@@ -104,7 +104,7 @@ cudaError_t launch_assemble_request(const int32_t* req, const void* movie_feats,
   const int words = 2 + hc + (dense ? 15 : 0);
   const int threads = 256;
   int64_t blocks = ((int64_t)n * words + threads - 1) / threads;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   assemble_request_kernel<<<(int)blocks, threads, 0, s>>>(req, static_cast<const int4*>(movie_feats), n_table, n, hc,
                                                          dense, movie_id, user_id, hist, movie_genre, user_genre,
                                                          numerics, err_flag);

@@ -90,7 +90,7 @@ class CTRModel:
         torch CUDA tensor for an embedding table that is already in HBM (used in
         place, see SRS_DEVICE_BORROWED in include/srs_ctr.h).  `narrow_ids`: host batches
         carry the history ids as uint16 (`srs_batch::hist16`, n_movies <= 65536).  `options`:
-        kernel-variant choices for `srs_model_create_ex`, e.g. {"din_impl": "rt"}."""
+        kernel-variant choices for `srs_model_create_ex`, e.g. {"din_impl": "tc"}."""
         self.spec = spec
         self.narrow_ids = bool(narrow_ids) and spec.n_movies <= 65536
         self.device = int(device)

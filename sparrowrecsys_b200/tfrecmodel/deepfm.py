@@ -1,4 +1,4 @@
-"""tfrecmodel.deepfm - B200 drop-in for the reference's `DeepFM.py` model
+"""tfrecmodel.deepfm - H100 drop-in for the reference's `DeepFM.py` model
 (TFRecModel/src/com/sparrowrecsys/offline/tensorflow/DeepFM.py:91-131).
 
     from tfrecmodel import deepfm

@@ -1,4 +1,4 @@
-"""tfrecmodel.deepfm_v2 - B200 drop-in for the reference's `DeepFM_v2.py` model
+"""tfrecmodel.deepfm_v2 - H100 drop-in for the reference's `DeepFM_v2.py` model
 (TFRecModel/src/com/sparrowrecsys/offline/tensorflow/DeepFM_v2.py:98-173).
 
     from tfrecmodel import deepfm_v2

@@ -1,4 +1,4 @@
-"""tfrecmodel.dien - B200 drop-in for the forward pass (`y_pred`) of the reference's `DIEN.py`
+"""tfrecmodel.dien - H100 drop-in for the forward pass (`y_pred`) of the reference's `DIEN.py`
 model (TFRecModel/src/com/sparrowrecsys/offline/tensorflow/DIEN.py:154-256), with the AUGRU's
 initial state a stored weight (`augru_h0`) instead of a fresh random draw per call (:235-236).
 

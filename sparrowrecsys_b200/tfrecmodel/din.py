@@ -1,4 +1,4 @@
-"""tfrecmodel.din - B200 drop-in for the reference's `DIN.py` model
+"""tfrecmodel.din - H100 drop-in for the reference's `DIN.py` model
 (TFRecModel/src/com/sparrowrecsys/offline/tensorflow/DIN.py:125-185).
 
     from tfrecmodel import din

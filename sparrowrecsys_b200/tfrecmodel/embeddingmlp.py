@@ -1,4 +1,4 @@
-"""tfrecmodel.embeddingmlp - B200 drop-in for the reference's `EmbeddingMLP.py` model
+"""tfrecmodel.embeddingmlp - H100 drop-in for the reference's `EmbeddingMLP.py` model
 (TFRecModel/src/com/sparrowrecsys/offline/tensorflow/EmbeddingMLP.py:72-94).
 
     from tfrecmodel import embeddingmlp

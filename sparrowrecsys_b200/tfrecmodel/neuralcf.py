@@ -1,4 +1,4 @@
-"""tfrecmodel.neuralcf - B200 drop-in for the reference's `NeuralCF.py` model
+"""tfrecmodel.neuralcf - H100 drop-in for the reference's `NeuralCF.py` model
 (TFRecModel/src/com/sparrowrecsys/offline/tensorflow/NeuralCF.py:45-53,74,91).
 
     from tfrecmodel import neuralcf

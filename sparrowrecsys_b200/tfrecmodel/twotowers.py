@@ -1,4 +1,4 @@
-"""tfrecmodel.twotowers - B200 drop-in for the reference's `NeuralCF.py` model
+"""tfrecmodel.twotowers - H100 drop-in for the reference's `NeuralCF.py` model
 (TFRecModel/src/com/sparrowrecsys/offline/tensorflow/NeuralCF.py:57-70).
 
     from tfrecmodel import twotowers

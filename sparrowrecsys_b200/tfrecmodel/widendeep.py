@@ -1,4 +1,4 @@
-"""tfrecmodel.widendeep - B200 drop-in for the reference's `WideNDeep.py` model
+"""tfrecmodel.widendeep - H100 drop-in for the reference's `WideNDeep.py` model
 (TFRecModel/src/com/sparrowrecsys/offline/tensorflow/WideNDeep.py:101-125).
 
     from tfrecmodel import widendeep

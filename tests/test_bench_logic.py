@@ -46,19 +46,6 @@ def test_tiled_dataset_holds_the_same_rows_in_other_orders():
     assert bench.tile_encoded(enc, 1, np.random.default_rng(0)) is enc
 
 
-def test_ncu_traffic_is_only_quoted_for_the_captured_kernel_and_batch():
-    import bench
-    summary = json.load(open(os.path.join(ROOT, "profiles", "ncu_bench_summary.json")))
-    rec = summary["cfg3_din"]
-    assert rec["kernel"] == "din_rt_kernel" and rec["batch"] == bench.WORKLOADS["cfg3_din"][0]
-    assert bench.ncu_traffic("cfg3_din", "din_rt_kernel", rec["batch"]) == rec["dram_bytes_per_launch"]
-    assert bench.ncu_traffic("cfg3_din", "din_rtp_kernel", rec["batch"]) is None    # another kernel
-    assert bench.ncu_traffic("cfg3_din", "din_rt_kernel", 2 * rec["batch"]) is None  # another batch size
-    assert bench.ncu_traffic("no_such_workload", "din_rt_kernel", 1) is None
-    for w, r in summary.items():                                   # every capture is of that workload's own kernel
-        assert w in bench.WORKLOADS and r["dram_bytes_per_launch"] > 0 and r["duration_us"] > 0
-
-
 def test_both_arms_print_the_same_config():
     import bench
     a = bench.parse_args(["--workload", "cfg3_din"])
@@ -68,8 +55,8 @@ def test_both_arms_print_the_same_config():
     assert bench.shared_config(a, spec, 1) == bench.shared_config(b, spec, 1)
     c = bench.shared_config(a, spec, 4)
     assert c["global_batch"] == 4 * c["batch_per_gpu"] and "workload" in c
-    assert bench.parse_args(["--workload", "cfg5_din"]).no_graph          # cfg 5 launches directly (DESIGN section 6)
-    assert not bench.parse_args(["--workload", "cfg5_din", "--graph"]).no_graph
+    assert not bench.parse_args(["--workload", "cfg5_din"]).no_graph      # every workload replays a CUDA graph
+    assert bench.parse_args(["--workload", "cfg5_din", "--no-graph"]).no_graph
     assert not bench.parse_args([]).no_graph
 
 
@@ -84,3 +71,20 @@ def test_stdout_of_the_reference_arm_is_one_json_line():
     assert d["impl"] == "reference" and d["unit"] == "inferences/s" and d["value"] > 0
     assert d["e2e"]["h2d_bytes_per_step"] == 0 and d["cpu_baseline"]["kind"] == "port"
     assert d["dtype"] == "f32" and d["higher_is_better"] is True
+
+
+def test_dump_outputs_writes_float32_scores_and_a_fixed_sample_above_the_limit(tmp_path, monkeypatch):
+    import bench
+    small = np.random.default_rng(1).random((3, 5), dtype=np.float32)
+    bench.dump_outputs(str(tmp_path / "a"), small)
+    got = np.load(tmp_path / "a" / "scores.npy")
+    assert got.dtype == np.float32 and np.array_equal(got, small)
+    assert not (tmp_path / "a" / "scores_index.npy").exists()
+    monkeypatch.setattr(bench, "DUMP_LIMIT_BYTES", 64)              # 8 values + their indices
+    big = np.arange(1000, dtype=np.float32).reshape(10, 100)
+    for d in ("b", "c"):
+        bench.dump_outputs(str(tmp_path / d), big)
+    idx, vals = np.load(tmp_path / "b" / "scores_index.npy"), np.load(tmp_path / "b" / "scores.npy")
+    assert len(idx) == 8 and np.array_equal(vals, big.reshape(-1)[idx])
+    assert np.array_equal(idx, np.load(tmp_path / "c" / "scores_index.npy"))   # the same sample every run
+    assert vals.nbytes + idx.nbytes <= 64

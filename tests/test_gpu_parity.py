@@ -1,4 +1,4 @@
-"""CUDA path vs oracle, through the C ABI (run on the B200 box: pytest -m gpu).
+"""CUDA path vs oracle, through the C ABI (needs a GPU: pytest -m gpu).
 
 Tolerance: BASELINE.json's north_star asks for predictions within 1e-4 of the
 reference float32 `model.predict`; these tests hold the CUDA path to PROB_ATOL = 2e-5
@@ -146,7 +146,7 @@ def test_din_cfg5_at_the_real_vocabulary():
     Wd = dict(W)
     Wd["embedding"] = table
     with _model(spec, Wd) as m:
-        assert m.kernel_name == "din_rt64_kernel"
+        assert m.kernel_name == "din_wg_kernel"
         p, z = m.predict_with_logits(feats)
     del table
     torch.cuda.empty_cache()
@@ -397,9 +397,12 @@ def test_launch_counter_counts_kernels():
         assert launch_count() == before + 1
 
 
-# ---- DIN tensor-core kernels (csrc/din_tc.cu per-pair, csrc/din_rt.cu row tiles) vs CUDA-core
-#      kernel vs oracle ----------------------------------------------------------------------
-KERNEL_OF = {"tc": "din_tc_kernel", "rt": "din_rt_kernel"}
+# ---- DIN tensor-core kernel (csrc/din_wg.cu, warpgroup MMAs) vs CUDA-core kernel vs oracle ----
+#      the option values tc, rt and rtp all select it.  "tc" runs it with one CTA per 32-row tile;
+#      "rt" (the row-tile option value) runs it with the grid capped at SM_CAP CTAs, so that every CTA
+#      walks several tiles in its grid-stride loop.
+KERNEL_OF = {"tc": "din_wg_kernel", "rt": "din_wg_kernel"}
+SM_CAP = {"tc": 0, "rt": 7}
 
 @pytest.fixture
 def din_impl(monkeypatch):
@@ -413,14 +416,13 @@ def din_impl(monkeypatch):
                                    (24, 100, 1), (32, 50, 4097)])
 @pytest.mark.parametrize("impl", ["tc", "rt"])
 def test_din_tensor_core_kernel(E, T, B, impl, din_impl):
-    if impl == "rt" and T > 64:
-        pytest.skip("row-tile kernel covers hist_len <= 64")
     spec = default_spec("din", emb_dim=E, hist_len=T, n_movies=27279, n_users=5000)
     W = init_weights(spec, E * 1000 + T)
     feats = synthetic_features(spec, B, seed=T)
     din_impl(impl)
     with _model(spec, W) as m:
         assert m.kernel_name == KERNEL_OF[impl]
+        m.set_sm_limit(SM_CAP[impl])
         p_tc, z_tc = m.predict_with_logits(feats)
         p_tc2 = m.predict(feats)
     assert np.array_equal(p_tc, p_tc2)                       # deterministic
@@ -438,13 +440,14 @@ def test_din_tensor_core_kernel(E, T, B, impl, din_impl):
 @pytest.mark.parametrize("E,T,B", [(64, 200, 512), (64, 128, 100), (48, 129, 33), (33, 9, 17), (64, 256, 65),
                                    (40, 64, 4097), (64, 200, 1), (64, 130, 148 * 32 + 5)])
 def test_din_row_tile_kernel_wide_embeddings(E, T, B, din_impl):
-    """din_rt64_kernel (csrc/din_rt64.cu): 32 < E <= 64, T <= 256, one or two 128-position chunks per row."""
+    """din_wg_kernel (csrc/din_wg.cu) with E padded to 64: two K blocks per history row, several 64-position
+    tiles per row."""
     spec = default_spec("din", emb_dim=E, hist_len=T, n_movies=50_000, n_users=5000)
     W = init_weights(spec, E * 1000 + T)
     feats = synthetic_features(spec, B, seed=T, uniform_history=(T == 200))
     din_impl("rt")
     with _model(spec, W) as m:
-        assert m.kernel_name == "din_rt64_kernel"
+        assert m.kernel_name == "din_wg_kernel"
         p_rt, z_rt = m.predict_with_logits(feats)
         p_rt2 = m.predict(feats)
     assert np.array_equal(p_rt, p_rt2)                       # deterministic
@@ -466,7 +469,7 @@ def test_din_row_tile_kernel_wide_row_independence(din_impl):
     feats = synthetic_features(spec, B, seed=7, uniform_history=True)
     perm = np.random.default_rng(2).permutation(B)
     with _model(spec, W) as m:
-        assert m.kernel_name == "din_rt64_kernel"
+        assert m.kernel_name == "din_wg_kernel"
         p = m.predict(feats)[:, 0]
         pp = m.predict({k: v[perm] for k, v in feats.items()})[:, 0]
         assert np.array_equal(pp, p[perm])                   # bit-exact under row permutation
@@ -484,6 +487,7 @@ def test_din_tensor_core_row_independence(impl, din_impl):
     feats = synthetic_features(spec, B, seed=3)
     perm = np.random.default_rng(1).permutation(B)
     with _model(spec, W) as m:
+        m.set_sm_limit(SM_CAP[impl])
         p = m.predict(feats)[:, 0]
         pp = m.predict({k: v[perm] for k, v in feats.items()})[:, 0]
         assert np.array_equal(pp, p[perm])                   # bit-exact under row permutation
@@ -504,6 +508,7 @@ def test_din_tensor_core_large_magnitudes(impl, din_impl):
     W["dense_2/kernel"] = (W["dense_2/kernel"] * 4).astype(np.float32)
     feats = synthetic_features(spec, 2048, seed=5)
     with _model(spec, W) as m:
+        m.set_sm_limit(SM_CAP[impl])
         p, z = m.predict_with_logits(feats)
     po, zo = O.forward(spec, W, feats)
     assert np.abs(zo).max() > 2.0
@@ -587,10 +592,10 @@ def test_deepfm_tensor_core_kernel(E, B, monkeypatch):
         assert np.abs(m.predict(feats) - po).max() <= PROB_ATOL
 
 
-# ---- pipelined row-tile kernel (csrc/din_rtp.cu) ----------------------------------------------
-# Every role is a persistent loop over the CTA's row groups; the SM limit decides how many groups a
-# CTA walks (1 SM: every group of the batch on one CTA - staging by the loader warp, both staging
-# buffers, pooled-buffer reuse, odd last tiles, one-tile groups all get exercised).
+# ---- the tensor-core DIN kernel under an SM limit (option value rtp) -----------------------------
+# din_wg_kernel walks the batch's 32-row tiles in a grid-stride loop; the SM limit decides how many tiles a
+# CTA walks (1 SM: every tile of the batch on one CTA - buffer reuse across tiles, odd last tiles, one-row
+# tiles all get exercised).
 @pytest.mark.parametrize("E,T,B,sms", [(32, 50, 28, 0), (32, 50, 4096, 0), (32, 50, 4096, 74), (32, 50, 4096, 37),
                                        (32, 50, 1500, 3), (32, 9, 100, 1), (32, 31, 17, 0), (32, 64, 333, 2),
                                        (20, 33, 15, 0), (32, 50, 2 * 148 * 32 + 77, 0), (32, 50, 1, 0),
@@ -601,7 +606,7 @@ def test_din_rtp_kernel(E, T, B, sms, din_impl):
     feats = synthetic_features(spec, B, seed=T + B)
     din_impl("rtp")
     with _model(spec, W) as m:
-        assert m.kernel_name == "din_rtp_kernel"
+        assert m.kernel_name == "din_wg_kernel"
         if sms:
             m.set_sm_limit(sms)
         p, z = m.predict_with_logits(feats)
@@ -626,6 +631,28 @@ def test_din_rtp_out_of_range_ids_latch_the_error_flag(din_impl):
         import torch
         d.hist[17, 3] = spec.n_movies + 5                          # device path: no host pre-validation
         out = torch.empty(300, dtype=torch.float32, device="cuda:0")
+        m.predict_device(d, out)
+        with pytest.raises((SrsError, ValueError)):
+            m.status()
+
+
+@pytest.mark.parametrize("E,T,pos", [(64, 200, 3), (64, 200, 130), (32, 50, 49)])
+def test_din_tensor_core_negative_history_id_latches_the_error_flag(E, T, pos, din_impl):
+    """-1 is a value a caller can put into a history slot: the tensor-core DIN kernel (the default when E pads
+    to 64) range-checks it like every other live id instead of taking it for an empty slot."""
+    import torch
+    from sparrowrecsys_b200._lib import SrsError
+    spec = default_spec("din", emb_dim=E, hist_len=T, n_movies=27279, n_users=5000)
+    W = init_weights(spec, 2)
+    feats = synthetic_features(spec, 300, seed=4)
+    din_impl("tc")
+    with _model(spec, W) as m:
+        assert m.kernel_name == "din_wg_kernel"
+        d = m.to_device(feats)
+        out = torch.empty(300, dtype=torch.float32, device="cuda:0")
+        m.predict_device(d, out)
+        m.status()                                                 # the valid batch raises nothing
+        d.hist[17, pos] = -1                                       # device path: no host pre-validation
         m.predict_device(d, out)
         with pytest.raises((SrsError, ValueError)):
             m.status()

@@ -145,9 +145,14 @@ def test_abi_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), "libsrs_ctr.so does not export %s" % name
     assert set(declared) == set(_lib.EXPORTS)
-    assert lib.srs_abi_version() == _lib.ABI_VERSION == 3
+    assert lib.srs_abi_version() == _lib.ABI_VERSION == 4
     assert lib.srs_num_slots() >= 2
-    assert lib.srs_launch_count() == 0
+    # a freshly loaded library has launched nothing (this process may already have run GPU tests)
+    import subprocess
+    import sys
+    r = subprocess.run([sys.executable, "-c", "from sparrowrecsys_b200 import _lib; print(_lib.load().srs_launch_count())"],
+                       capture_output=True, text=True, cwd=ROOT, timeout=120)
+    assert r.returncode == 0 and r.stdout.strip() == "0", r.stdout + r.stderr
 
 
 def test_struct_layouts_match_header():
@@ -219,38 +224,6 @@ def test_abi_argument_validation_needs_no_device():
     assert b"unknown model kind" in lib.srs_last_error() and not h.value
     with pytest.raises(ValueError):
         default_spec("dien", emb_dim=33)                     # one lane per state element
-
-
-def test_din_rtp_barrier_protocol_model():
-    """din_rtp_kernel (csrc/din_rtp.cu) orders seven roles with nothing but mbarriers across group
-    boundaries; its protocol is checked on a CPU model under random interleavings
-    (profiles/exp/rtp_protocol_sim.py: no deadlock, no parity aliasing, no operand / staging hazard).
-    One-tile groups are the case that deadlocked the first draft."""
-    import importlib.util
-    spec = importlib.util.spec_from_file_location(
-        "rtp_protocol_sim", os.path.join(ROOT, "profiles", "exp", "rtp_protocol_sim.py"))
-    sim = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(sim)
-    for shape in ([1], [14], [14, 14, 14], [1, 1, 1, 1, 1, 1], [2, 1, 3, 1, 1, 2], [16, 1, 5, 16, 1, 1, 7]):
-        for seed in range(10):
-            sim.Sim(shape, seed).run()
-
-
-def test_row_tile_barrier_protocol_model():
-    """din_rt_kernel / din_rt64_kernel share one mbarrier protocol; profiles/exp/rt_protocol_sim.py runs it on the
-    CPU with warp-level actors under random interleavings.  The shipped kernels keep ONE pooling-weights barrier
-    per consumer (w_ready[q]); the model shows what that allows when a consumer warp lags its siblings by a tile
-    or the issuer is late - a phase completed by arrivals of two different tiles, then parity aliasing and a
-    deadlock - and that one barrier per (consumer, pooled buffer) (-DSRS_WREADY_SPLIT, the form din_rtp uses)
-    has none of it.  DESIGN.md section 9 item 1."""
-    import importlib.util
-    spec = importlib.util.spec_from_file_location(
-        "rt_protocol_sim", os.path.join(ROOT, "profiles", "exp", "rt_protocol_sim.py"))
-    sim = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(sim)
-    assert sim.check(False, runs=21) == []
-    broken = sim.check(True, runs=21)
-    assert broken and any("different tiles" in m or "Deadlock" in m or "meant completion" in m for _, _, m in broken)
 
 
 def test_c_example_builds_against_the_public_header(tmp_path, have_gpu):

@@ -7,7 +7,7 @@ import os
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, REFERENCE_WEBROOT, load_golden_weights
+from conftest import GOLDEN, load_golden_weights
 from oracle import ctr_oracle as O
 from sparrowrecsys_b200.spec import default_spec
 
@@ -63,31 +63,65 @@ def test_full_file_stats_recorded():
     assert abs(s["roc_auc"] - 0.73208) < 1e-5
 
 
-@pytest.mark.skipif(not os.path.isdir(REFERENCE_WEBROOT), reason="reference checkout not present")
-def test_bundle_reader_matches_fixture():
-    """The TF-free bundle reader on the real SavedModel dirs equals the committed fixture."""
+def _rebuilt_bundle(tmp_path, name):
+    """A SavedModel directory rebuilt from tests/golden/bundle_pins.npz: the reference's variables.index as it
+    is, and a sparse copy of its data file holding the byte ranges of the model variables (the user table at
+    the rows of the users the weight fixtures hold)."""
+    z = np.load(os.path.join(GOLDEN, "bundle_pins.npz"))
+    vdir = tmp_path / name / "variables"
+    vdir.mkdir(parents=True)
+    (vdir / "variables.index").write_bytes(z[name + "__index"].tobytes())
+    blob = z[name + "__bytes"].tobytes()
+    with open(vdir / "variables.data-00000-of-00001", "wb") as f:
+        f.truncate(int(z[name + "__size"]))
+        at = 0
+        for off, n in zip(z[name + "__offsets"].tolist(), z[name + "__lengths"].tolist()):
+            f.seek(off)
+            f.write(blob[at:at + n])
+            at += n
+    return str(tmp_path / name)
+
+
+def test_bundle_reader_matches_fixture(tmp_path):
+    """The TF-free bundle reader on the SavedModel variable files equals the committed fixture."""
     from sparrowrecsys_b200 import bundle
-    W = bundle.load_neuralcf(REFERENCE_WEBROOT + "modeldata/neuralcf/002")
+    d = _rebuilt_bundle(tmp_path, "neuralcf_002")
+    W = bundle.load_neuralcf(d)
     G = load_golden_weights("neuralcf_002")
     for k in ("movieId_embedding", "dense_0/kernel", "dense_0/bias", "dense_1/kernel",
               "dense_2/kernel", "dense_2/bias"):
         assert np.array_equal(W[k], G[k]), k
     nz = np.flatnonzero(np.abs(G["userId_embedding"]).sum(axis=1))
     assert np.array_equal(W["userId_embedding"][nz], G["userId_embedding"][nz])
-    idx = bundle.read_index(REFERENCE_WEBROOT + "modeldata/neuralcf/002/variables/variables.index")
+    idx = bundle.read_index(os.path.join(d, "variables", "variables.index"))
     e = idx["layer_with_weights-2/kernel/.ATTRIBUTES/VARIABLE_VALUE"]
     assert (e["shape"], e["offset"]) == ((20, 10), 1240080)       # SURVEY.md 8c offsets
-    W5 = bundle.load_twotowers(REFERENCE_WEBROOT + "modeldata/MLPRec/005")
+    W5 = bundle.load_twotowers(_rebuilt_bundle(tmp_path, "mlprec_005"))
     assert W5["item_dense_0/kernel"].shape == (10, 10)
+    G5 = load_golden_weights("mlprec_005")
+    for k in ("item_dense_0/kernel", "item_dense_0/bias", "user_dense_0/kernel", "user_dense_0/bias"):
+        assert np.array_equal(W5[k], G5[k]), k
 
 
-@pytest.mark.skipif(not os.path.isdir(REFERENCE_WEBROOT), reason="reference checkout not present")
+def _pins():
+    """What the reference's files and serialised graphs gave (tests/golden/make_reference_pins.py)."""
+    return np.load(os.path.join(GOLDEN, "reference_pins.npz"))
+
+
+def _neuralcf_002_with_pinned_users():
+    z = _pins()
+    W = load_golden_weights("neuralcf_002")
+    W["userId_embedding"][z["user_ids"]] = z["user_rows"]
+    return W
+
+
 def test_head_fixture_is_prefix_of_reference_file():
-    with open(REFERENCE_WEBROOT + "sampledata/testSamples.csv", "rb") as f:
-        ref = f.read(200000)
+    import hashlib
+    z = _pins()
     with open(os.path.join(GOLDEN, "samples_head.csv"), "rb") as f:
         head = f.read()
-    assert ref.startswith(head)
+    assert len(head) == int(z["head_bytes"])
+    assert hashlib.sha256(head).hexdigest() == str(z["head_sha256"])
 
 
 # ---- the reference's own serialised graphs (tests/golden/make_savedmodel_graph_vectors.py) ----------------
@@ -187,55 +221,37 @@ def test_feature_column_semantics_read_off_the_older_exports():
     assert O.genre_index(f, "movieGenre1").tolist() == [0, 18, -1, -1, 1]
 
 
-@pytest.mark.skipif(not os.path.isdir(REFERENCE_WEBROOT), reason="reference checkout not present")
 def test_identity_column_edge_cases_of_the_serialised_graph():
     """What the reference's graph itself does with odd ids: an id >= num_buckets trips the graph's own assert (our
     ValueError / SRS_ERR_RANGE), the last valid id works, and -1 is the column's "missing" value: its embedding is
     the zero vector (we reject -1 instead: INTEGRATION.md, error table)."""
-    from oracle import savedmodel_graph as SG
-    from sparrowrecsys_b200 import bundle
-    g = SG.ServingGraph(REFERENCE_WEBROOT + "modeldata/neuralcf/002", bundle.read_variables)
-    with pytest.raises(ValueError):
-        g.run({"movieId": np.array([5, 1001]), "userId": np.array([7, 7])})
-    with pytest.raises(ValueError):
-        g.run({"movieId": np.array([5, 5]), "userId": np.array([7, 30001])})
-    ok = g.run({"movieId": np.array([5, 1000]), "userId": np.array([7, 30000])})
-    assert ok.shape == (2, 1)
-    W = bundle.load_neuralcf(REFERENCE_WEBROOT + "modeldata/neuralcf/002")
-    missing = g.run({"movieId": np.array([-1]), "userId": np.array([7])})
+    z = _pins()
+    assert bool(z["edge_raises_movie_1001"]) and bool(z["edge_raises_user_30001"])
+    W = _neuralcf_002_with_pinned_users()
+    spec = default_spec("neuralcf")
+    ok, _ = O.neuralcf_forward(spec, W, {"movieId": np.array([5, 1000], np.int32), "userId": np.array([7, 30000], np.int32)})
+    np.testing.assert_allclose(ok[:, 0], z["edge_last_valid"], rtol=0, atol=5e-7)
     Wz = dict(W)
     Wz["movieId_embedding"] = W["movieId_embedding"].copy()
     Wz["movieId_embedding"][0] = 0                            # row 0 zeroed = what a zero vector does
-    p, _ = O.neuralcf_forward(default_spec("neuralcf"), Wz, {"movieId": np.array([0], np.int32), "userId": np.array([7], np.int32)})
-    np.testing.assert_allclose(missing[:, 0], p[:, 0], rtol=0, atol=5e-7)
-    assert np.array_equal(g.run({"movieId": np.array([3, 9]), "userId": np.array([7, 8])}),
-                          g.run({"movieId": np.array([3, 9]), "userId": np.array([7, 8])}, full=False))
+    p, _ = O.neuralcf_forward(spec, Wz, {"movieId": np.array([0], np.int32), "userId": np.array([7], np.int32)})
+    np.testing.assert_allclose(z["edge_missing_movie"], p[:, 0], rtol=0, atol=5e-7)
+    assert bool(z["edge_full_equals_partial"])
+    pair, _ = O.neuralcf_forward(spec, W, {"movieId": np.array([3, 9], np.int32), "userId": np.array([7, 8], np.int32)})
+    np.testing.assert_allclose(pair[:, 0], z["edge_pair_output"], rtol=0, atol=5e-7)
 
 
-@pytest.mark.skipif(not os.path.isdir(REFERENCE_WEBROOT), reason="reference checkout not present")
-def test_graph_vectors_regenerate_from_the_reference_exports():
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("mk", os.path.join(GOLDEN, "make_savedmodel_graph_vectors.py"))
-    mk = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mk)
-    fresh = json.loads(json.dumps(mk.vectors()))
-    assert fresh == _graph_vectors()
-
-
-@pytest.mark.skipif(not os.path.isdir(REFERENCE_WEBROOT), reason="reference checkout not present")
 def test_whole_test_file_through_the_serialised_graph():
     """All 22 440 rows of the reference's testSamples.csv through the serialised neuralcf/002 graph: the oracle agrees
-    row by row, and the accuracy / ROC-AUC recorded in full_file_stats.json (SURVEY.md 8c) are the graph's."""
-    from oracle import savedmodel_graph as SG
-    from sparrowrecsys_b200 import bundle
-    from sparrowrecsys_b200.features import load_samples_csv
-    full = load_samples_csv(REFERENCE_WEBROOT + "sampledata/testSamples.csv")
-    g = SG.ServingGraph(REFERENCE_WEBROOT + "modeldata/neuralcf/002", bundle.read_variables)
-    pg = g.run({"movieId": np.asarray(full["movieId"]), "userId": np.asarray(full["userId"])})[:, 0]
-    W = bundle.load_neuralcf(REFERENCE_WEBROOT + "modeldata/neuralcf/002")
-    po = O.predict(default_spec("neuralcf"), W, full)[:, 0]
-    assert len(pg) == 22440 and np.abs(pg - po).max() <= 5e-7
-    lab = np.asarray(full["label"])
+    row by row on a fixed sample of 2000 of them, and the accuracy / ROC-AUC recorded in full_file_stats.json
+    (SURVEY.md 8c) are the graph's."""
+    z = _pins()
+    pg = z["graph_output"]
+    idx = z["sample_index"]
+    W = _neuralcf_002_with_pinned_users()
+    po, _ = O.neuralcf_forward(default_spec("neuralcf"), W, {"movieId": z["sample_movieId"], "userId": z["sample_userId"]})
+    assert len(pg) == 22440 and np.abs(pg[idx] - po[:, 0]).max() <= 5e-7
+    lab = z["label"].astype(np.int64)
     with open(os.path.join(GOLDEN, "full_file_stats.json")) as f:
         s = json.load(f)
     assert abs(float(((pg > 0.5) == (lab == 1)).mean()) - s["accuracy"]) < 1e-9
