@@ -208,8 +208,9 @@ int srs_model_status(srs_model* m);
 int64_t srs_model_bytes_per_inference(const srs_model* m);
 
 /* Name of the kernel variant srs_predict_* dispatches to for this model.  DIN has two
- * (din_wg_kernel: activation unit on warpgroup MMAs; din_kernel: CUDA cores); the choice follows
- * the shape and can be forced with the environment variable SRS_DIN_IMPL = tc | cudacore read by
+ * (din_wg_kernel: activation unit - and for emb_dim <= 32 the top MLP - on warpgroup MMAs, the
+ * default for 16 < emb_dim <= 64 and hist_len > 8; din_kernel: CUDA cores, every other shape); the
+ * choice follows the shape and can be forced with the environment variable SRS_DIN_IMPL = tc | cudacore read by
  * srs_model_create (a forced variant that does not support the shape makes srs_model_create fail).
  * SRS_EMBMLP_IMPL and SRS_DEEPFM_IMPL (tc | cudacore) do the same for EmbeddingMLP / Wide&Deep
  * and DeepFM. */

@@ -42,14 +42,19 @@ def needs_build() -> bool:
     return any(os.path.getmtime(d) > t for d in sources() + headers())
 
 
-def build(force: bool = False, verbose: bool = False) -> str:
-    if not force and not needs_build():
+def build(force: bool = False, verbose: bool = False, defines=(), out_dir: str = None) -> str:
+    """Compile and link the library; returns its path.  `defines` (e.g. ["SRS_DIN_PHASES"]) build a
+    variant, which needs `out_dir`: its objects and library go there, never over the in-tree build."""
+    if defines and not out_dir:
+        raise ValueError("a build with extra defines needs its own out_dir")
+    lib = os.path.join(out_dir, "libsrs_ctr.so") if out_dir else LIB
+    if not out_dir and not force and not needs_build():
         return LIB
-    objdir = os.path.join(HERE, "build", ARCH[1].split("code=")[1])     # objects of another arch never mix in
+    objdir = os.path.join(out_dir or os.path.join(HERE, "build"), ARCH[1].split("code=")[1])   # objects of another arch never mix in
     os.makedirs(objdir, exist_ok=True)
     nvcc = nvcc_path()
     common = [nvcc, *ARCH, "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
-              "--expt-relaxed-constexpr", "--extended-lambda"]
+              "--expt-relaxed-constexpr", "--extended-lambda"] + ["-D" + d for d in defines]
     if verbose:
         common += ["-Xptxas", "-v"]
     procs = []
@@ -72,10 +77,10 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(out)
     if failed:
         raise RuntimeError("CUDA build failed")
-    tmp = LIB + ".tmp%d" % os.getpid()                   # link aside, then rename: a reader (or a copy of
+    tmp = lib + ".tmp%d" % os.getpid()                   # link aside, then rename: a reader (or a copy of
     subprocess.check_call([nvcc, *ARCH, "-shared", "-o", tmp, *objs])   # the tree) never sees a half-written library
-    os.replace(tmp, LIB)
-    return LIB
+    os.replace(tmp, lib)
+    return lib
 
 
 if __name__ == "__main__":

@@ -70,6 +70,54 @@ __device__ __forceinline__ void gather_signal_tail(const BatchView& b) {
   }
 }
 
+// ---- opt-in phase timing of the DIN kernels (tools/din_phases.py builds the library with -DSRS_DIN_PHASES) ----
+// One lead thread per timing unit (a warpgroup of din_wg_kernel, warp 0 of din_kernel) adds the clock64()
+// cycles since its previous lap to g_din_phases[phase]; in the default build a lap compiles to nothing.
+enum DinPhase {
+  PH_TILE_INPUTS = 0,   // side features, candidate rows, activation-unit constants
+  PH_W_BUILD,           // per-row B operand W_r (wgmma) / folded column (CUDA cores)
+  PH_GATHER_ISSUE,      // history ids and history-row gathers issued
+  PH_GATHER_WAIT,       // waiting for the gathers of the current row
+  PH_AU_MMA,            // activation-unit MMAs, issue to completion
+  PH_GATE,              // PReLU, Dense(1), sigmoid per position
+  PH_POOL,              // weighted sum of the history rows
+  PH_AU_LOOP,           // CUDA-core kernel: activation unit + gate + pooling per position
+  PH_ROW_IMBALANCE,     // waiting at the barrier before the top MLP
+  PH_TOP_MLP,           // Dense(128) / Dense(64) / Dense(1) + sigmoid
+  kDinPhases
+};
+#ifdef SRS_DIN_PHASES
+static __device__ unsigned long long g_din_phases[kDinPhases];
+struct PhaseClock {
+  long long t = 0;
+  bool lead;
+  __device__ explicit PhaseClock(bool lead_) : lead(lead_) {
+#ifdef __CUDA_ARCH__
+    t = clock64();
+#endif
+  }
+  __device__ void lap(int ph) {
+#ifdef __CUDA_ARCH__
+    const long long n = clock64();
+    if (lead) atomicAdd(&g_din_phases[ph], (unsigned long long)(n - t));
+    t = n;
+#endif
+  }
+};
+// copy the counters of this translation unit's kernel to the host and clear them
+static inline cudaError_t din_phases_take(unsigned long long* out) {
+  cudaError_t e = cudaMemcpyFromSymbol(out, g_din_phases, sizeof(unsigned long long) * kDinPhases);
+  if (e != cudaSuccess) return e;
+  static const unsigned long long zero[kDinPhases] = {};
+  return cudaMemcpyToSymbol(g_din_phases, zero, sizeof zero);
+}
+#else
+struct PhaseClock {
+  __device__ explicit PhaseClock(bool) {}
+  __device__ void lap(int) {}
+};
+#endif
+
 __device__ __forceinline__ float4 ldg4(const float* p) {
   return __ldg(reinterpret_cast<const float4*>(p));
 }

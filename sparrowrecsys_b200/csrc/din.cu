@@ -44,10 +44,12 @@ __global__ void __launch_bounds__(kThreads) din_kernel(DinParams p, BatchView b)
   const int warp = tid >> 5, lane = tid & 31;
   const int row0 = blockIdx.x * R;
   float* hc = Hc + warp * TC * EP;
+  PhaseClock clk(tid == 0);
 
   // ---- side features: user genre, user, movie genre rows and numerics ------------
   tile_side_features<EP, R>(Xs, LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users, p.n_genres,
                             OFF_UG, OFF_U, OFF_MG, OFF_NUM);
+  clk.lap(PH_TILE_INPUTS);
 
   // ---- activation unit + pooling: one warp per row ---------------------------------
   const float wout = __ldg(p.au_wout + lane);
@@ -73,6 +75,7 @@ __global__ void __launch_bounds__(kThreads) din_kernel(DinParams p, BatchView b)
       M[e] = fmaf(c, __ldg(p.au_wp + e * 32 + lane), __ldg(p.au_wh + e * 32 + lane));
       cst = fmaf(c, __ldg(p.au_wc + e * 32 + lane), cst);
     }
+    clk.lap(PH_W_BUILD);
     float pooled[NE];
 #pragma unroll
     for (int n = 0; n < NE; ++n) pooled[n] = 0.f;
@@ -95,6 +98,7 @@ __global__ void __launch_bounds__(kThreads) din_kernel(DinParams p, BatchView b)
               ldg4(p.movie + (size_t)id * EP + 4 * q);
       }
       __syncwarp();
+      clk.lap(PH_GATHER_WAIT);
       for (int t = 0; t < nt; ++t) {
         const float* h = hc + t * EP;
         float z0 = cst, z1 = 0.f;
@@ -116,6 +120,7 @@ __global__ void __launch_bounds__(kThreads) din_kernel(DinParams p, BatchView b)
           if (e < EP) pooled[n] = fmaf(w, h[e], pooled[n]);
         }
       }
+      clk.lap(PH_AU_LOOP);
     }
 #pragma unroll
     for (int n = 0; n < NE; ++n) {
@@ -123,7 +128,9 @@ __global__ void __launch_bounds__(kThreads) din_kernel(DinParams p, BatchView b)
       if (e < EP) xrow[OFF_POOL + e] = pooled[n];
     }
   }
+  clk.lap(PH_AU_LOOP);
   __syncthreads();
+  clk.lap(PH_ROW_IMBALANCE);
 
   // ---- top MLP on the tile ----------------------------------------------------------
   dense_layer<R, 128, 2, 8>(Xs, LDX, KP, p.W1, p.b1, ACT_PRELU, p.a1, H1, LDH1);
@@ -137,6 +144,7 @@ __global__ void __launch_bounds__(kThreads) din_kernel(DinParams p, BatchView b)
     store_score(b, row, sigmoidf_acc(z));
     if (b.logits) b.logits[row] = z;
   });
+  clk.lap(PH_TOP_MLP);
 }
 
 template <int EP>
@@ -174,5 +182,9 @@ cudaError_t setup_din_attributes() {
 #undef SRS_ATTR
   return cudaSuccess;
 }
+
+#ifdef SRS_DIN_PHASES
+cudaError_t din_take_phases(unsigned long long* out) { return din_phases_take(out); }
+#endif
 
 }  // namespace srs

@@ -15,12 +15,18 @@
 //   * gate (PReLU per position, Dense(1), sigmoid) on the accumulator registers, one quad of
 //     lanes per position;
 //   * pooling sum_t w_t h_t from the same shared-memory tile (h = hi + lo);
-//   * top MLP on CUDA cores over the CTA's 32-row tile, as in din.cu.
+//   * top MLP over the CTA's 32-row tile.  E <= 32: on wgmma, computed transposed like
+//     embmlp_tc.cu - D[units x rows] = W^T X^T with W1^T (the 160 embedding columns of the tile) and
+//     W2^T resident in shared memory as bf16 hi / lo images (one bulk copy per CTA), the tile's hi
+//     and lo halves stacked along N, the 7 raw-scale numerics added in fp32 in the layer-1
+//     epilogue, PReLU / Dense(1) / sigmoid on the accumulator registers.  E <= 64: on CUDA cores
+//     (common.cuh::dense_layer); its W1 image would be ~160 KB, and at cfg 5's T = 200 the
+//     activation unit dominates the tile.
 //
 // CTA = 256 threads = two warpgroups, 32 batch rows; warpgroup q owns rows q, q + 2, ... and
 // double-buffers its history tiles (the next tile's cp.async runs under this tile's MMA and
 // epilogue; the ids of the tile after it are already on their way from HBM).  Shared memory:
-// ~105 KB (E <= 32) / ~180 KB (E <= 64).
+// ~209 KB with the MLP images (E <= 32) / ~180 KB (E <= 64): one CTA per SM.
 #include "kernels.h"
 #include "wgmma.cuh"
 
@@ -32,29 +38,175 @@ constexpr int kWgPos = 64;        // history positions per MMA tile
 
 template <int EP>
 struct DinWgLayout {
+  static constexpr bool TC_MLP = EP == 32;                    // top MLP on wgmma
   static constexpr int KB = EP / 32;                          // 128-byte K blocks of a [hi | lo] row
   static constexpr uint32_t A_BYTES = KB * kWgPos * 128;      // one history tile
   static constexpr uint32_t B_BYTES = KB * 32 * 128;          // W_r, 32 unit rows
   static constexpr uint32_t WG_BYTES = 2 * A_BYTES + B_BYTES; // per warpgroup
+  static constexpr uint32_t AU_BYTES = 2 * WG_BYTES;
+  // top-MLP operand images (TC_MLP): W1^T [128 units][160 k] in 3 K blocks (the third half used) and
+  // W2^T [64 units][128 k] in 2, each as a hi and a lo image
+  static constexpr uint32_t IMG_W1_HI = 0, IMG_W1_LO = 49152, IMG_W2_HI = 98304, IMG_W2_LO = 114688;
+  static constexpr uint32_t IMG_BYTES = TC_MLP ? 131072 : 0;
+  // X operand [32 rows hi | 32 rows lo][160 k] (3 K blocks), then the H1 operand [.. ][128 k] (2 K blocks):
+  // both over the history tiles, which are free once the tile's activation unit is done
+  static constexpr uint32_t OP_KB_BYTES = 2 * kWgRows * 128;
+  static_assert(!TC_MLP || 3 * OP_KB_BYTES <= AU_BYTES, "X operand must fit over the history tiles");
   static constexpr int KP = 5 * EP + kNumPad, LDX = KP + 4, LDH1 = 128 + 4, LDH2 = 64 + 4;
-  // fp32 region behind the operand tiles
+  // fp32 region behind the operand tiles and images
   static constexpr int F_X = 0;
-  static constexpr int F_H1 = F_X + kWgRows * LDX;
-  static constexpr int F_H2 = F_H1 + kWgRows * LDH1;
-  static constexpr int F_WH = F_H2 + kWgRows * LDH2;          // [EP][32] Wsub + Wh
+  static constexpr int F_H1 = F_X + kWgRows * LDX;                       // CUDA-core MLP only
+  static constexpr int F_H2 = F_H1 + (TC_MLP ? 0 : kWgRows * LDH1);
+  static constexpr int F_WH = F_H2 + (TC_MLP ? 0 : kWgRows * LDH2);    // [EP][32] Wsub + Wh
   static constexpr int F_WP = F_WH + EP * 32;                 // [EP][32] Wp
   static constexpr int F_WC = F_WP + EP * 32;                 // [EP][32] Wc - Wsub
   static constexpr int F_CST = F_WC + EP * 32;                // [32 rows][32 units] activation-unit constants
   static constexpr int F_WG = F_CST + kWgRows * 32;           // per warpgroup: w[64] | part[128]
   static constexpr int F_WG_STRIDE = kWgPos + 128;
-  static constexpr int F_END = F_WG + 2 * F_WG_STRIDE;
-  static constexpr size_t SMEM = 1024 + 2 * WG_BYTES + (size_t)F_END * sizeof(float);
+  static constexpr int F_RED = F_WG + 2 * F_WG_STRIDE;        // [4 warps][32 rows] Dense(1) partial sums
+  static constexpr int F_END = F_RED + 4 * kWgRows;
+  static constexpr size_t SMEM = 1024 + AU_BYTES + IMG_BYTES + (size_t)F_END * sizeof(float);
+  static_assert(SMEM <= 227 * 1024, "one CTA per SM must fit");
 };
 
 // byte offset of K byte `kb` (hi part: 2 e, lo part: 2 (EP + e)) of operand row `row` in a tile of
 // `rows` rows: K blocks are `rows * 128` bytes apart
 __device__ __forceinline__ uint32_t wg_kbyte(uint32_t row, uint32_t kb, uint32_t rows) {
   return (kb >> 7) * rows * 128u + sw128_offset(row, (kb & 127u) >> 4) + (kb & 15u);
+}
+
+// Top MLP of a 32-row tile on wgmma (E <= 32).  Xs holds the fp32 input tile; the X and H1 operands go
+// over the history tiles at `ops`; `img` holds the W1^T / W2^T images, which have landed once `wbar` (if
+// not null) completes.  Ends with every score of the tile stored.
+template <int EP>
+__device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& b, int row0, const float* Xs,
+                                           uint8_t* ops, const uint8_t* img, float* red, uint64_t* wbar) {
+  using L = DinWgLayout<EP>;
+  constexpr int KE = 5 * EP;                       // embedding columns of the tile: the MMAs' K
+  constexpr uint32_t KBB = L::OP_KB_BYTES, LO = kWgRows * 128;   // operand K block; lo rows follow the hi rows
+  const int tid = threadIdx.x, q = tid >> 7, tw = tid & 127;
+  const int warp = tw >> 5, lane = tw & 31, g = lane >> 2, cq = lane & 3;
+  // X operand: tile columns 0 .. KE - 1 split to bf16 hi (operand rows 0..31) and lo (rows 32..63)
+  for (int i = tid; i < kWgRows * KE / 2; i += kThreads) {
+    const int r = i / (KE / 2), k = 2 * (i % (KE / 2));
+    const float2 v = *reinterpret_cast<const float2*>(Xs + r * L::LDX + k);
+    const Split2 s = split_pack(v.x, v.y);
+    const uint32_t off = (uint32_t)(k >> 6) * KBB + sw128_offset(r, (k & 63) >> 3) + (k & 7) * 2;
+    *reinterpret_cast<uint32_t*>(ops + off) = s.hi;
+    *reinterpret_cast<uint32_t*>(ops + off + LO) = s.lo;
+  }
+  fence_async_smem();
+  __syncthreads();
+  if (wbar) mbar_wait(wbar, 0);
+  const uint32_t s_img = smem_u32(img), s_op = smem_u32(ops);
+
+  // ---- Dense(128) + PReLU: warpgroup q owns units 64 q .. 64 q + 63; D[64 units x (32 rows hi | 32 rows lo)]
+  {
+    float d[32];
+  #pragma unroll
+    for (int i = 0; i < 32; ++i) d[i] = 0.f;
+    mma_fence();
+  #pragma unroll
+    for (int kb = 0; kb < (KE + 63) / 64; ++kb) {
+      const uint64_t ah = desc_sw128(s_img + L::IMG_W1_HI + kb * 16384 + q * 8192);
+      const uint64_t al = desc_sw128(s_img + L::IMG_W1_LO + kb * 16384 + q * 8192);
+      const uint64_t xs = desc_sw128(s_op + kb * KBB);
+  #pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        if (64 * kb + 16 * ks < KE) {              // the third K block is half used
+          mma_m64n64_ss(d, ah + 2 * ks, xs + 2 * ks, kb > 0 || ks > 0);
+          mma_m64n64_ss(d, al + 2 * ks, xs + 2 * ks, 1);
+        }
+      }
+    }
+    mma_commit();
+    mma_wait<0>();
+    reg_fence(d);
+    __syncthreads();                               // both warpgroups' MMAs have read X: H1 goes over it
+    // epilogue: units u = 64 q + 16 warp + g + 8 i, tile rows r = 8 j + 2 cq + c (hi: column r, lo: 32 + r)
+  #pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int u = 64 * q + 16 * warp + g + 8 * i;
+      const float bias = __ldg(p.b1 + u), slope = __ldg(p.a1 + u);
+      float wn[kNumNumerics];
+  #pragma unroll
+      for (int n = 0; n < kNumNumerics; ++n) wn[n] = __ldg(p.W1 + (size_t)(KE + n) * 128 + u);
+      const uint32_t koff = (uint32_t)(u >> 6) * KBB, chunk = (u & 63) >> 3, within = (u & 7) * 2;
+  #pragma unroll
+      for (int j = 0; j < 4; ++j)
+  #pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int r = 8 * j + 2 * cq + c;
+          const float* num = Xs + r * L::LDX + KE;
+          float v = d[4 * j + 2 * i + c] + d[4 * (j + 4) + 2 * i + c] + bias;
+  #pragma unroll
+          for (int n = 0; n < kNumNumerics; ++n) v = fmaf(num[n], wn[n], v);
+          v = v > 0.f ? v : slope * v;
+          const __nv_bfloat16 vh = __float2bfloat16_rn(v);
+          const uint32_t off = koff + sw128_offset(r, chunk) + within;
+          *reinterpret_cast<__nv_bfloat16*>(ops + off) = vh;
+          *reinterpret_cast<__nv_bfloat16*>(ops + off + LO) = __float2bfloat16_rn(v - __bfloat162float(vh));
+        }
+    }
+    fence_async_smem();
+    __syncthreads();
+  }
+  // ---- Dense(64) + PReLU, Dense(1), sigmoid: warpgroup 0, D[64 units x (32 rows hi | 32 rows lo)]
+  if (q != 0) return;
+  float d[32];
+  #pragma unroll
+  for (int i = 0; i < 32; ++i) d[i] = 0.f;
+  mma_fence();
+  #pragma unroll
+  for (int kb = 0; kb < 2; ++kb) {
+    const uint64_t ah = desc_sw128(s_img + L::IMG_W2_HI + kb * 8192);
+    const uint64_t al = desc_sw128(s_img + L::IMG_W2_LO + kb * 8192);
+    const uint64_t hs = desc_sw128(s_op + kb * KBB);
+  #pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      mma_m64n64_ss(d, ah + 2 * ks, hs + 2 * ks, kb > 0 || ks > 0);
+      mma_m64n64_ss(d, al + 2 * ks, hs + 2 * ks, 1);
+    }
+  }
+  mma_commit();
+  mma_wait<0>();
+  reg_fence(d);
+  float s[4][2];
+  #pragma unroll
+  for (int j = 0; j < 4; ++j) s[j][0] = s[j][1] = 0.f;
+  #pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int u = 16 * warp + g + 8 * i;
+    const float bias = __ldg(p.b2 + u), slope = __ldg(p.a2 + u), w3 = __ldg(p.w3 + u);
+  #pragma unroll
+    for (int j = 0; j < 4; ++j)
+  #pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        float v = d[4 * j + 2 * i + c] + d[4 * (j + 4) + 2 * i + c] + bias;
+        v = v > 0.f ? v : slope * v;
+        s[j][c] = fmaf(v, w3, s[j][c]);
+      }
+  }
+  // sum over the 8 lanes of a column quad (g), then over the 4 warps in a fixed order
+  #pragma unroll
+  for (int j = 0; j < 4; ++j)
+  #pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      float v = s[j][c];
+      v += __shfl_xor_sync(0xffffffffu, v, 4);
+      v += __shfl_xor_sync(0xffffffffu, v, 8);
+      v += __shfl_xor_sync(0xffffffffu, v, 16);
+      if (g == 0) red[warp * kWgRows + 8 * j + 2 * cq + c] = v;
+    }
+  named_sync(1, 128);
+  if (tw < kWgRows) {
+    const int row = row0 + tw;
+    if (row < b.B) {
+      const float z = ((red[tw] + red[kWgRows + tw]) + (red[2 * kWgRows + tw] + red[3 * kWgRows + tw])) + p.b3;
+      store_score(b, row, sigmoidf_acc(z));
+      if (b.logits) b.logits[row] = z;
+    }
+  }
 }
 
 template <int EP>
@@ -67,8 +219,10 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
   constexpr int PARTS = 128 / EP, PP = kWgPos / PARTS;
   constexpr int OFF_UG = 0, OFF_U = EP, OFF_POOL = 2 * EP, OFF_C = 3 * EP, OFF_MG = 4 * EP, OFF_NUM = 5 * EP;
   extern __shared__ uint8_t raw[];
+  __shared__ uint64_t wbar;                       // top-MLP images landed (TC_MLP)
   uint8_t* base = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
-  float* fs = reinterpret_cast<float*>(base + 2 * L::WG_BYTES);
+  uint8_t* img = base + L::AU_BYTES;
+  float* fs = reinterpret_cast<float*>(base + L::AU_BYTES + L::IMG_BYTES);
   float* Xs = fs + L::F_X;
   float* H1 = fs + L::F_H1;
   float* H2 = fs + L::F_H2;
@@ -84,7 +238,17 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
   uint8_t* Bt = tiles + 2 * L::A_BYTES;
   float* wsm = fs + L::F_WG + q * L::F_WG_STRIDE;
   float* part = wsm + kWgPos;
+  PhaseClock clk(tw == 0);
 
+  bool weights_ready = !L::TC_MLP;
+  if constexpr (L::TC_MLP) {
+    if (tid == 0) {                               // visible to the waiters through the tile loop's first barrier
+      mbar_init(&wbar, 1);
+      fence_mbar_init();
+      mbar_arrive_expect_tx(&wbar, L::IMG_BYTES);
+      for (uint32_t off = 0; off < L::IMG_BYTES; off += 32768u) bulk_g2s(img + off, p.mlp_image + off, 32768u, &wbar);
+    }
+  }
   stage_weights(fs + L::F_WH, p.au_wh, EP * 32);
   stage_weights(fs + L::F_WP, p.au_wp, EP * 32);
   stage_weights(fs + L::F_WC, p.au_wc, EP * 32);
@@ -118,6 +282,7 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
       cst_all[i] = acc;
     }
     __syncthreads();
+    clk.lap(PH_TILE_INPUTS);
     // rows of this warpgroup: q, q + 2, ...; the valid ones are a prefix
     int nrows = 0;
     for (int r = q; r < kWgRows; r += 2)
@@ -167,6 +332,7 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
     }
     cp_async_commit();
     float pool_acc = 0.f;
+    float slope[2][8], cstv[8];
     for (int k = 0; k < n_items; ++k) {
       const int r = q + 2 * (k / nch), ch = k % nch, t0 = ch * kWgPos;
       const int nt = min(kWgPos, T - t0);
@@ -175,33 +341,41 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
       if (ch == 0) {
         // B operand of the row: W_r = (Wsub + Wh) + diag(c_r) Wp, split to bf16 hi / lo
         const float* cv = xrow + OFF_C;
-        for (int i = tw; i < 32 * EP / 2; i += 128) {          // (unit j, element pair e, e + 1)
-          const int j = i / (EP / 2), e = 2 * (i % (EP / 2));
+        for (int i = tw; i < 32 * EP / 2; i += 128) {          // (unit j, element pair e, e + 1): the lanes
+          const int j = i & 31, e = 2 * (i >> 5);               // of a warp read 32 consecutive banks
           const float v0 = fmaf(cv[e], wp[e * 32 + j], wh[e * 32 + j]);
           const float v1 = fmaf(cv[e + 1], wp[(e + 1) * 32 + j], wh[(e + 1) * 32 + j]);
           const Split2 s = split_pack(v0, v1);
           *reinterpret_cast<uint32_t*>(Bt + wg_kbyte(j, 2 * e, 32)) = s.hi;
           *reinterpret_cast<uint32_t*>(Bt + wg_kbyte(j, 2 * (EP + e), 32)) = s.lo;
         }
+  #pragma unroll
+        for (int j = 0; j < 4; ++j)
+  #pragma unroll
+          for (int c = 0; c < 2; ++c) cstv[2 * j + c] = cst[8 * j + 2 * cq + c];
         pool_acc = 0.f;
+        clk.lap(PH_W_BUILD);
       }
       gather(k + 1, ids_next);                                // its buffer's last reader finished before the
       cp_async_commit();                                      // closing barrier of item k - 1
       load_ids(k + 2, ids_next);
       // PReLU slopes of this thread's positions pr = 16 warp + g + 8 i and columns 8 j + 2 cq + c,
-      // requested before the waits below
-      float slope[2][8];
+      // requested before the waits below; with one chunk per row (T <= 64) they are the same for every row
+      if (nch > 1 || k == 0) {
   #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const float* alpha = p.au_alpha + (size_t)min(t0 + 16 * warp + g + 8 * i, T - 1) * 32;
+        for (int i = 0; i < 2; ++i) {
+          const float* alpha = p.au_alpha + (size_t)min(t0 + 16 * warp + g + 8 * i, T - 1) * 32;
   #pragma unroll
-        for (int j = 0; j < 4; ++j)
+          for (int j = 0; j < 4; ++j)
   #pragma unroll
-          for (int c = 0; c < 2; ++c) slope[i][2 * j + c] = __ldg(alpha + 8 * j + 2 * cq + c);
+            for (int c = 0; c < 2; ++c) slope[i][2 * j + c] = __ldg(alpha + 8 * j + 2 * cq + c);
+        }
       }
+      clk.lap(PH_GATHER_ISSUE);
       cp_async_wait<1>();
       fence_async_smem();
       named_sync(1 + q, 128);                                 // tile k and W_r in place
+      clk.lap(PH_GATHER_WAIT);
 
       // ---- activation unit: D[64 positions x 32 units], bf16x3
       float d[16];
@@ -225,6 +399,7 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
         mma_wait<0>();
         reg_fence(d);
       }
+      clk.lap(PH_AU_MMA);
       // ---- gate: positions pr = 16 warp + g + 8 i; the quad of lanes sharing a position sums its 32 units
   #pragma unroll
       for (int i = 0; i < 2; ++i) {
@@ -234,8 +409,7 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
         for (int j = 0; j < 4; ++j)
   #pragma unroll
           for (int c = 0; c < 2; ++c) {
-            const int col = 8 * j + 2 * cq + c;
-            const float z = d[4 * j + 2 * i + c] + cst[col];
+            const float z = d[4 * j + 2 * i + c] + cstv[2 * j + c];
             const float a = z > 0.f ? z : slope[i][2 * j + c] * z;
             s = fmaf(a, wout[2 * j + c], s);
           }
@@ -244,6 +418,7 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
         if (cq == 0) wsm[pr] = pr < nt ? 1.f / (1.f + __expf(-(s + p.au_bout))) : 0.f;
       }
       named_sync(1 + q, 128);
+      clk.lap(PH_GATE);
       // ---- pooling: thread (part, e) sums positions part * PP .. + PP of element e
       {
         const int e = tw % EP, pt = tw / EP;
@@ -267,24 +442,33 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
         }
       }
       named_sync(1 + q, 128);                                 // tile k, wsm, part and W_r free again
+      clk.lap(PH_POOL);
     }
     cp_async_wait<0>();
     __syncthreads();
+    clk.lap(PH_ROW_IMBALANCE);
 
     // ---- top MLP on the tile ----------------------------------------------------------
-    dense_layer<kWgRows, 128, 2, 8>(Xs, L::LDX, L::KP, p.W1, p.b1, ACT_PRELU, p.a1, H1, L::LDH1);
-    __syncthreads();
-    dense_layer<kWgRows, 64, 1, 8>(H1, L::LDH1, 128, p.W2, p.b2, ACT_PRELU, p.a2, H2, L::LDH2);
-    __syncthreads();
-    row_dot<kWgRows>(H2, L::LDH2, 64, p.w3, [&](int r, float s) {
-      const int row = row0 + r;
-      if (row >= b.B) return;
-      const float z = s + p.b3;
-      store_score(b, row, sigmoidf_acc(z));
-      if (b.logits) b.logits[row] = z;
-    });
+    if constexpr (L::TC_MLP) {
+      top_mlp_wg<EP>(p, b, row0, Xs, base, img, fs + L::F_RED, weights_ready ? nullptr : &wbar);
+      weights_ready = true;
+    } else {
+      dense_layer<kWgRows, 128, 2, 8>(Xs, L::LDX, L::KP, p.W1, p.b1, ACT_PRELU, p.a1, H1, L::LDH1);
+      __syncthreads();
+      dense_layer<kWgRows, 64, 1, 8>(H1, L::LDH1, 128, p.W2, p.b2, ACT_PRELU, p.a2, H2, L::LDH2);
+      __syncthreads();
+      row_dot<kWgRows>(H2, L::LDH2, 64, p.w3, [&](int r, float s) {
+        const int row = row0 + r;
+        if (row >= b.B) return;
+        const float z = s + p.b3;
+        store_score(b, row, sigmoidf_acc(z));
+        if (b.logits) b.logits[row] = z;
+      });
+    }
     __syncthreads();                              // the next tile reuses every buffer
+    clk.lap(PH_TOP_MLP);
   }
+  if (!weights_ready) mbar_wait(&wbar, 0);        // no bulk copy may outlive the CTA
   gather_signal_tail(b);                          // spanning ranking call: publish "slice complete"
 }
 
@@ -322,6 +506,10 @@ cudaError_t launch_din_wg(const DinParams& p, const BatchView& b, cudaStream_t s
   else return cudaErrorInvalidValue;
   return cudaGetLastError();
 }
+
+#ifdef SRS_DIN_PHASES
+cudaError_t din_wg_take_phases(unsigned long long* out) { return din_phases_take(out); }
+#endif
 
 cudaError_t setup_din_wg_attributes() {
   cudaError_t e = cudaFuncSetAttribute(din_wg_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize,

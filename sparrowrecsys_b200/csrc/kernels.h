@@ -155,6 +155,7 @@ struct DinParams {
   int EP;
   const uint8_t* movie_split;  // din_wg.cu: [n_movies][EP x bf16 hi | EP x bf16 lo] (history rows)
   int max_ctas;                // din_wg.cu: CTAs per launch, 0 = one per 32-row tile (srs_model_set_sm_limit)
+  const uint8_t* mlp_image;    // din_wg.cu, EP = 32: W1^T / W2^T bf16 hi / lo images (DinWgLayout<32>::IMG_*)
 };
 
 // ---- DIEN (DIEN.py:154-256), CUDA-core kernel for E <= 32 -------------------------------------

@@ -21,6 +21,10 @@ cudaError_t setup_deepfm_attributes();
 cudaError_t setup_din_attributes();
 cudaError_t setup_dien_attributes();
 cudaError_t setup_din_wg_attributes();
+#ifdef SRS_DIN_PHASES
+cudaError_t din_take_phases(unsigned long long* out);
+cudaError_t din_wg_take_phases(unsigned long long* out);
+#endif
 cudaError_t setup_embmlp_tc_attributes();
 cudaError_t setup_deepfm_tc_attributes();
 // gather.cu
@@ -700,11 +704,34 @@ void write_sw128(uint8_t* dst, int rows, int kblocks, bool lo_part, F get) {
         }
 }
 
-// Tensor-core DIN kernel (din_wg.cu): the movie table pre-split into bf16 hi / lo rows; every other
-// tensor is the one build_din uploaded.
+// Tensor-core DIN kernel (din_wg.cu): the movie table pre-split into bf16 hi / lo rows and, for EP = 32,
+// the top MLP's operand images; every other tensor is the one build_din uploaded.
 int build_din_wg(Builder& B) {
   srs_model* m = B.m;
   DinParams& p = m->din;
+  if (m->EP == 32) {
+    // W1^T over the 160 embedding columns of the tile (K blocks 64 | 64 | 32 + zeros), W2^T; units are the
+    // MMA rows, zero-padded to 128 / 64 like the permuted fp32 weights they are read back from
+    constexpr int KE = 5 * 32;
+    std::vector<float> w1((size_t)(KE + 8) * 128), w2((size_t)128 * 64);
+    cudaError_t e = cudaMemcpy(w1.data(), p.W1, w1.size() * sizeof(float), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(w2.data(), p.W2, w2.size() * sizeof(float), cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "weight read-back failed: %s", cudaGetErrorString(e));
+    auto w1_get = [&](int u, int k) -> float { return k < KE ? w1[(size_t)k * 128 + u] : 0.f; };
+    auto w2_get = [&](int u, int k) -> float { return w2[(size_t)k * 64 + u]; };
+    std::vector<uint8_t> img(131072, 0);
+    write_sw128(img.data() + 0, 128, 3, false, w1_get);
+    write_sw128(img.data() + 49152, 128, 3, true, w1_get);
+    write_sw128(img.data() + 98304, 64, 2, false, w2_get);
+    write_sw128(img.data() + 114688, 64, 2, true, w2_get);
+    uint8_t* d_img = nullptr;
+    e = cudaMalloc(&d_img, img.size());
+    if (e != cudaSuccess) return fail(SRS_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(e));
+    m->owned.push_back(d_img);
+    e = cudaMemcpy(d_img, img.data(), img.size(), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "image upload failed: %s", cudaGetErrorString(e));
+    p.mlp_image = d_img;
+  }
   void* d_split = nullptr;
   const size_t split_bytes = (size_t)m->spec.n_movies * m->EP * 4;
   cudaError_t e = cudaMalloc(&d_split, split_bytes);
@@ -1157,16 +1184,17 @@ int srs_model_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_
     default: {
       rc = build_din(B);
       // kernel selection (SRS_DIN_IMPL=cudacore|tc overrides; tc fails loudly on an unsupported shape):
-      //   tc  activation unit on warpgroup MMAs (din_wg.cu): E padded to 32 or 64.  The default for E
-      //       padded to 64 and T > 8, where it measured faster on the H100 (BASELINE cfg 5: 12.6 vs 8.6 M
-      //       inferences/s); for E <= 32 the CUDA-core kernel measured slightly faster (cfg 3: 58.0 vs 57.3 M).
+      //   tc  activation unit on warpgroup MMAs (din_wg.cu): E padded to 32 or 64.  The default for T > 8,
+      //       where it measured faster on the H100 (DESIGN.md section 6): BASELINE cfg 5 (E padded to 64)
+      //       and cfg 3 (E = 32, where the top MLP runs on wgmma too).  cudacore stays the only kernel for
+      //       E <= 16.
       //   rt, rtp  the names of the earlier row-tile tensor-core kernels; callers that pass them get the
       //       same tensor-core kernel as tc.
       const char* impl_c = opt("din_impl", "SRS_DIN_IMPL");
       const std::string impl_s = impl_c ? impl_c : "";
       const char* impl = impl_c ? impl_s.c_str() : nullptr;
       const bool fits_tc = m->EP == 32 || m->EP == 64;
-      bool want_tc = m->EP == 64 && spec->hist_len > 8;
+      bool want_tc = fits_tc && spec->hist_len > 8;
       if (impl && !strcmp(impl, "cudacore")) want_tc = false;
       if (impl && (!strcmp(impl, "tc") || !strcmp(impl, "rt") || !strcmp(impl, "rtp"))) {
         if (!fits_tc && rc == SRS_OK) rc = fail(SRS_ERR_INVALID, "SRS_DIN_IMPL=%s needs 16 < emb_dim <= 64", impl);
@@ -1612,5 +1640,19 @@ int srs_selftest_wgmma(const float* A, const float* B, float* D, int32_t N, int3
   CUDA_TRY(cudaDeviceSynchronize());
   return SRS_OK;
 }
+
+#ifdef SRS_DIN_PHASES
+// Phase-timing builds only (tools/din_phases.py): the cycles the DIN kernel of this model spent in each
+// srs::DinPhase since the previous call, summed over timing units; the counters are cleared.
+int srs_debug_din_phases(const srs_model* m, uint64_t* out, int32_t n) {
+  if (!m || !out || n < kDinPhases) return fail(SRS_ERR_INVALID, "need %d counters", (int)kDinPhases);
+  CUDA_TRY(cudaSetDevice(m->device));
+  CUDA_TRY(cudaDeviceSynchronize());
+  unsigned long long c[kDinPhases];
+  CUDA_TRY(m->use_din_wg ? din_wg_take_phases(c) : din_take_phases(c));
+  for (int i = 0; i < kDinPhases; ++i) out[i] = c[i];
+  return SRS_OK;
+}
+#endif
 
 }  // extern "C"
