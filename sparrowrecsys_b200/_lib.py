@@ -59,6 +59,10 @@ class SrsError(RuntimeError):
         self.code = code
 
 
+class SrsInvalidError(SrsError, ValueError):
+    """SRS_ERR_INVALID: an argument the library does not support (e.g. a hidden width past a builder's limit)."""
+
+
 def lib_path() -> str:
     # SRS_CTR_LIB: an alternative build of the library (kernel-tuning experiments)
     return os.environ.get("SRS_CTR_LIB") or _build.LIB
@@ -158,4 +162,6 @@ def check(rc: int):
         raise ValueError(msg)            # mirrors TF's assert on identity columns
     if rc == SRS_ERR_MISSING:
         raise KeyError(msg)
+    if rc == SRS_ERR_INVALID:
+        raise SrsInvalidError(rc, msg)
     raise SrsError(rc, msg)
