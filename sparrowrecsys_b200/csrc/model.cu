@@ -1570,8 +1570,6 @@ int srs_rank_user_host(srs_model* m, const srs_user_row* user, const int32_t* ca
   if (n > s.req_capacity || !s.d_req) {
     cudaFree(s.d_req);
     if (s.h_req) cudaFreeHost(s.h_req);
-    if (s.h_done) cudaFreeHost(s.h_done);
-    if (s.h_res) cudaFreeHost(s.h_res);
     s.d_req = nullptr; s.h_req = nullptr; s.req_capacity = 0;
     const size_t words = 16 + (size_t)hc + (size_t)s.capacity;
     CUDA_TRY(cudaMalloc(&s.d_req, words * 4));
