@@ -277,6 +277,52 @@ int srs_model_set_movie_features(srs_model* m, int32_t n_movies, const int32_t* 
 int srs_rank_user_host(srs_model* m, const srs_user_row* user, const int32_t* candidate_movie_ids,
                        int32_t n, int32_t k, int32_t* top_idx, float* top_scores, float* probs);
 
+/* ---- `model.evaluate(dataset)`: the four numbers every CTR script of the reference prints
+ * (loss='binary_crossentropy', metrics=['accuracy', AUC(curve='ROC'), AUC(curve='PR')],
+ * e.g. DIN.py:171-185, EmbeddingMLP.py:80-91, NeuralCF.py:77-88), with Keras's (TF 2.0) semantics:
+ *   loss      mean over rows of the logit-path sigmoid cross-entropy max(x,0) - x*z + log1p(exp(-|x|)),
+ *             each row in float32 (for a sigmoid output layer Keras does not clip the probability);
+ *   accuracy  binary_accuracy: label == (p > 0.5);
+ *   roc_auc, pr_auc   AUC(num_thresholds=200, summation_method='interpolation'): p counts as positive at
+ *             threshold t when float32(p) > t; PR by interpolate_pr_auc (Davis & Goadrich).  The
+ *             TP/FP/TN/FN counts are exact 64-bit integers (Keras keeps them in float32, which is exact
+ *             only up to 2^24 rows).  A single-class input gives an AUC of 0.
+ * Labels must be 0 or 1 and probabilities in [0, 1] (Keras asserts this): anything else latches the
+ * state's error word and the result call returns SRS_ERR_INVALID. */
+typedef struct srs_eval_result {
+  int64_t rows, positives, correct;
+  double loss, accuracy, roc_auc, pr_auc;
+} srs_eval_result;
+
+/* Device-resident metric state on one device: 2 x 201 (label, threshold bin) counts, the correct rows,
+ * the loss sum and the error word.  Updates are asynchronous and can be captured in a CUDA graph; the
+ * updates of one state must be ordered (one stream, or streams joined by events).  The loss is summed
+ * in a fixed order, so it has the same bits on every run over the same batches. */
+typedef struct srs_metrics srs_metrics;
+int srs_metrics_create(int32_t device, srs_metrics** out);
+void srs_metrics_destroy(srs_metrics* mt);
+/* zero the state, asynchronous on `stream` */
+int srs_metrics_reset(srs_metrics* mt, void* stream);
+/* fold n >= 1 rows of device buffers (probs, logits [n] float32, labels [n] int32) into the state,
+ * asynchronous on `stream` */
+int srs_metrics_update_device(srs_metrics* mt, const float* probs, const float* logits,
+                              const int32_t* labels, int32_t n, void* stream);
+/* synchronise the device and summarise: AUCs computed on the host in double from the counts.
+ * `confusion`: NULL or int64[4][200] = tp, fp, tn, fn per threshold.  SRS_ERR_INVALID if an update saw
+ * a bad label or probability (the error stays until srs_metrics_reset) or if no row was folded. */
+int srs_metrics_result(srs_metrics* mt, srs_eval_result* out, int64_t* confusion);
+
+/* `model.evaluate(dataset)` over host batches: each batch is scored and folded into the metrics on the
+ * device the way srs_predict_host_batches pipelines it (batch i on slot i % srs_num_slots()); only its
+ * labels [B] int32 go in beside the features and no score comes back.  The loss sums of the batches are
+ * added in batch order, so the result does not depend on which slot finishes first.  Synchronous.
+ * SRS_ERR_RANGE for an out-of-range id, SRS_ERR_INVALID for a bad label or probability, for no rows,
+ * and for the models evaluate does not cover - DIEN (its Keras evaluate loss includes the training-only
+ * auxiliary loss) and two towers without the final Dense (its output is a raw dot, not a probability).
+ * `out` is written only on success. */
+int srs_evaluate_host_batches(srs_model* m, int32_t n_batches, const srs_batch* batches,
+                              const int32_t* const* labels, srs_eval_result* out);
+
 /* Known-answer self test of the warpgroup-MMA (wgmma) plumbing the tensor-core kernels are built on:
  * D[128][N] = bf16(A[128][K]) * bf16(B[N][K])^T (inputs truncated to bf16, fp32 accumulate),
  * K = 64 * k_blocks (1..4), N = 16 or 32, A read from shared memory (a_in_regs = 0) or from

@@ -42,7 +42,8 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_cosine_scores_device", "srs_topk_device", "srs_rank_host", "srs_gather_create", "srs_gather_export",
            "srs_gather_connect", "srs_gather_destroy", "srs_predict_device_gather", "srs_gather_wait",
            "srs_gather_scores", "srs_gather_copy_scores", "srs_model_set_movie_features", "srs_rank_user_host",
-           "srs_selftest_wgmma")
+           "srs_selftest_wgmma", "srs_metrics_create", "srs_metrics_destroy", "srs_metrics_reset",
+           "srs_metrics_update_device", "srs_metrics_result", "srs_evaluate_host_batches")
 
 _lib = None
 
@@ -51,6 +52,12 @@ class SrsUserRow(C.Structure):
     """`srs_user_row` (include/srs_ctr.h): the typed `uf:<userId>` hash of one user."""
     _fields_ = [("user_id", C.c_int32), ("user_genre", C.c_int32 * 5), ("user_numerics", C.c_float * 3),
                 ("n_hist", C.c_int32), ("hist", C.c_void_p)]
+
+
+class SrsEvalResult(C.Structure):
+    """`srs_eval_result` (include/srs_ctr.h): what `model.evaluate` reports, with its counts."""
+    _fields_ = [("rows", C.c_int64), ("positives", C.c_int64), ("correct", C.c_int64), ("loss", C.c_double),
+                ("accuracy", C.c_double), ("roc_auc", C.c_double), ("pr_auc", C.c_double)]
 
 
 class SrsError(RuntimeError):
@@ -148,6 +155,20 @@ def load():
     lib.srs_selftest_wgmma.restype = C.c_int
     lib.srs_selftest_wgmma.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                       C.c_int32, C.c_int32]
+    lib.srs_metrics_create.restype = C.c_int
+    lib.srs_metrics_create.argtypes = [C.c_int32, C.POINTER(C.c_void_p)]
+    lib.srs_metrics_destroy.restype = None
+    lib.srs_metrics_destroy.argtypes = [C.c_void_p]
+    lib.srs_metrics_reset.restype = C.c_int
+    lib.srs_metrics_reset.argtypes = [C.c_void_p, C.c_void_p]
+    lib.srs_metrics_update_device.restype = C.c_int
+    lib.srs_metrics_update_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                              C.c_void_p]
+    lib.srs_metrics_result.restype = C.c_int
+    lib.srs_metrics_result.argtypes = [C.c_void_p, C.POINTER(SrsEvalResult), C.c_void_p]
+    lib.srs_evaluate_host_batches.restype = C.c_int
+    lib.srs_evaluate_host_batches.argtypes = [C.c_void_p, C.c_int32, C.POINTER(SrsBatch), C.POINTER(C.c_void_p),
+                                              C.POINTER(SrsEvalResult)]
     if lib.srs_abi_version() != ABI_VERSION:
         raise ImportError("libsrs_ctr.so ABI version %d != %d" % (lib.srs_abi_version(), ABI_VERSION))
     _lib = lib

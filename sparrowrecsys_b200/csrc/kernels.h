@@ -7,6 +7,8 @@
 
 #include "common.cuh"
 
+struct srs_eval_result;
+
 namespace srs {
 
 // ---- NeuralCF / two towers (NeuralCF.py:45-70) ------------------------------------
@@ -212,6 +214,33 @@ cudaError_t launch_topk(const float* scores, int n, int k, int32_t* top_idx, flo
 cudaError_t launch_topk_done(const float* scores, int n, int k, int32_t* top_idx, float* top_scores,
                              void* scratch, int* err_flag, uint32_t* done, uint32_t seq, cudaStream_t s);
 cudaError_t launch_finish(int* err_flag, uint32_t* done, uint32_t seq, cudaStream_t s);
+
+// ---- metrics.cu: Keras's evaluate metrics (loss, accuracy, ROC / PR AUC) over labelled batches -----------
+constexpr int kMetThresholds = 200;        // Keras AUC num_thresholds
+constexpr int kMetBins = kMetThresholds + 1;   // bin k = #{j : p > t_j}, 0..200
+constexpr int kMetMaxCtas = 264;           // CTAs of one update launch (fixed by n alone: the loss bits do not
+                                           // depend on the SM count or an SM limit)
+constexpr int kMetErrLabel = 1;            // MetricsCounters::err bits: a label other than 0 / 1
+constexpr int kMetErrProb = 2;             //   a probability that is NaN or outside [0, 1]
+struct MetricsCounters {                   // device, zeroed by a reset; integer atomics only
+  unsigned long long hist[2 * kMetBins];   // [label 0 | label 1][bin]
+  unsigned long long correct;
+  int err;
+  int pad_;
+};
+struct MetricsReduce {                     // per stream of updates: the last CTA sums partial[] in CTA order
+  unsigned int ticket;
+  unsigned int pad_;
+  double partial[kMetMaxCtas];
+};
+// Fold n rows into `cnt`; the rows' loss sum goes to *loss_dst (added to it when `accumulate`).  Launches
+// sharing one `red` must be stream-ordered.
+cudaError_t launch_metrics_update(const float* probs, const float* logits, const int32_t* labels, int n,
+                                  MetricsCounters* cnt, MetricsReduce* red, double* loss_dst, int accumulate,
+                                  cudaStream_t s);
+// host: the counts -> srs_eval_result (AUCs in double); `confusion` NULL or [4][200] tp, fp, tn, fn
+void metrics_summarise(const unsigned long long* hist, unsigned long long correct, double loss_sum,
+                       srs_eval_result* out, int64_t* confusion);
 
 // one-time per-device kernel attribute setup (dynamic shared memory opt-in)
 cudaError_t setup_kernel_attributes();

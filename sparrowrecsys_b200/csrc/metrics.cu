@@ -1,0 +1,186 @@
+// metrics.cu - the metrics of Keras's `model.evaluate` over labelled batches (the reference compiles
+// every CTR model with loss='binary_crossentropy' and metrics=['accuracy', AUC(curve='ROC'),
+// AUC(curve='PR')], e.g. DIN.py:171-181): one kernel folds a batch's scores into a device-resident
+// state; the AUCs are computed on the host from that state's 2 x 201 integer counts.
+//
+// Per row (DESIGN.md section 4, "Metrics"):
+//   bin k = #{j : p > t_j} over Keras's 200 float32 thresholds, counted per (label, k);
+//   correct = (label == (p > 0.5)), Keras's binary_accuracy;
+//   loss = max(x, 0) - x*z + log1p(exp(-|x|)) on the logit x in float32: for a sigmoid output layer
+//   Keras's binary_crossentropy takes this logit path, not the clipped-probability formula.
+// Counts are integer atomics (exact, order-free).  The loss is reduced in double in a fixed order inside
+// each CTA; the last CTA (ticket counter) sums the CTA partials in CTA order, so it has the same bits on
+// every run for the same rows.
+#include <cmath>
+
+#include "../../include/srs_ctr.h"
+#include "kernels.h"
+
+namespace srs {
+
+namespace {
+
+constexpr int kMetThreads = 256;
+constexpr int kMetRowsPerCta = 4 * kMetThreads;
+
+// Keras's thresholds: [0 - 1e-7] + [(i + 1) / 199 for i in range(198)] + [1 + 1e-7] in double, each cast
+// to float32 (IEEE double division and rounding are the same on the device and on the host).
+__device__ __forceinline__ float keras_threshold(int j) {
+  if (j == 0) return (float)(0.0 - 1e-7);
+  if (j == kMetThresholds - 1) return (float)(1.0 + 1e-7);
+  return (float)((double)j * 1.0 / (double)(kMetThresholds - 1));
+}
+
+// the row's logit-path binary cross-entropy in float32 (sigmoid_cross_entropy_with_logits)
+__device__ __forceinline__ float row_loss(float x, int z) {
+  const float relu = fmaxf(x, 0.f);
+  const float xz = z ? x : 0.f;                    // x * z, z in {0, 1}
+  return __fadd_rn(__fsub_rn(relu, xz), log1pf(expf(-fabsf(x))));
+}
+
+__global__ void __launch_bounds__(kMetThreads)
+metrics_update_kernel(const float* __restrict__ probs, const float* __restrict__ logits,
+                      const int32_t* __restrict__ labels, int n, MetricsCounters* cnt, MetricsReduce* red,
+                      double* loss_dst, int accumulate) {
+  __shared__ float s_t[kMetThresholds];
+  __shared__ unsigned int s_hist[2 * kMetBins];
+  __shared__ double s_loss[kMetThreads / 32];
+  __shared__ unsigned int s_correct;
+  __shared__ int s_err;
+  __shared__ int s_last;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int j = tid; j < kMetThresholds; j += kMetThreads) s_t[j] = keras_threshold(j);
+  for (int j = tid; j < 2 * kMetBins; j += kMetThreads) s_hist[j] = 0u;
+  if (tid == 0) { s_correct = 0u; s_err = 0; }
+  __syncthreads();
+
+  double loss = 0.0;
+  unsigned int correct = 0u;
+  int err = 0;
+  for (int64_t base = (int64_t)blockIdx.x * kMetThreads; base < n; base += (int64_t)gridDim.x * kMetThreads) {
+    const int64_t i = base + tid;
+    int key = -1;
+    if (i < n) {
+      const float p = __ldg(probs + i);
+      const int z = __ldg(labels + i);
+      const bool ok_p = p >= 0.f && p <= 1.f;             // false for NaN
+      const bool ok_z = z == 0 || z == 1;
+      err |= (ok_z ? 0 : kMetErrLabel) | (ok_p ? 0 : kMetErrProb);
+      if (ok_p && ok_z) {
+        int lo = 0, hi = kMetThresholds;                   // k = #{j : p > t_j}, thresholds ascending
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          if (p > s_t[mid]) lo = mid + 1; else hi = mid;
+        }
+        key = z * kMetBins + lo;
+        correct += (unsigned int)((z == 1) == (p > 0.5f));
+        loss += (double)row_loss(__ldg(logits + i), z);
+      }
+    }
+    // scores cluster: one shared atomic per distinct (label, bin) in the warp
+    const unsigned int active = __ballot_sync(0xffffffffu, key >= 0);
+    if (key >= 0) {
+      const unsigned int peers = __match_any_sync(active, key);
+      if (lane == __ffs(peers) - 1) atomicAdd(&s_hist[key], (unsigned int)__popc(peers));
+    }
+  }
+
+  correct = __reduce_add_sync(0xffffffffu, correct);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) loss += __shfl_xor_sync(0xffffffffu, loss, o);
+  err = __reduce_or_sync(0xffffffffu, (unsigned int)err);
+  if (lane == 0) {
+    s_loss[warp] = loss;
+    if (correct) atomicAdd(&s_correct, correct);
+    if (err) atomicOr(&s_err, err);
+  }
+  __syncthreads();
+
+  for (int j = tid; j < 2 * kMetBins; j += kMetThreads) {
+    const unsigned int v = s_hist[j];
+    if (v) atomicAdd(&cnt->hist[j], (unsigned long long)v);
+  }
+  if (tid == 0) {
+    if (s_correct) atomicAdd(&cnt->correct, (unsigned long long)s_correct);
+    if (s_err) atomicOr(&cnt->err, s_err);
+    double cta = 0.0;
+    for (int w = 0; w < kMetThreads / 32; ++w) cta += s_loss[w];
+    red->partial[blockIdx.x] = cta;
+    __threadfence();
+    s_last = atomicAdd(&red->ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!s_last || warp != 0) return;
+  __threadfence();
+  double tot = 0.0;                                        // CTA partials in a fixed order
+  for (int b = lane; b < (int)gridDim.x; b += 32) tot += __ldcg(red->partial + b);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, o);
+  if (lane == 0) {
+    *loss_dst = accumulate ? *loss_dst + tot : tot;
+    red->ticket = 0u;                                      // ready for the next launch on this stream
+  }
+}
+
+inline double div_no_nan(double a, double b) { return b == 0.0 ? 0.0 : a / b; }
+
+}  // namespace
+
+cudaError_t launch_metrics_update(const float* probs, const float* logits, const int32_t* labels, int n,
+                                  MetricsCounters* cnt, MetricsReduce* red, double* loss_dst, int accumulate,
+                                  cudaStream_t s) {
+  if (n <= 0) return cudaSuccess;
+  int64_t blocks = ((int64_t)n + kMetRowsPerCta - 1) / kMetRowsPerCta;
+  if (blocks > kMetMaxCtas) blocks = kMetMaxCtas;
+  metrics_update_kernel<<<(int)blocks, kMetThreads, 0, s>>>(probs, logits, labels, n, cnt, red, loss_dst,
+                                                            accumulate);
+  ++g_launch_count;
+  return cudaGetLastError();
+}
+
+// Keras's AUC(num_thresholds=200, summation_method='interpolation') from the (label, bin) counts.  Keras
+// keeps TP/FP/TN/FN in float32 variables, which stop being exact above 2^24 rows; these are exact integers.
+void metrics_summarise(const unsigned long long* hist, unsigned long long correct, double loss_sum,
+                       srs_eval_result* out, int64_t* confusion) {
+  const unsigned long long* neg = hist;
+  const unsigned long long* pos = hist + kMetBins;
+  double tp[kMetThresholds], fp[kMetThresholds], tn[kMetThresholds], fn[kMetThresholds];
+  unsigned long long P = 0, N = 0;
+  for (int k = 0; k < kMetBins; ++k) { P += pos[k]; N += neg[k]; }
+  unsigned long long above_p = P, above_n = N;             // rows with bin > j, i.e. p > t_j
+  for (int j = 0; j < kMetThresholds; ++j) {
+    above_p -= pos[j]; above_n -= neg[j];
+    tp[j] = (double)above_p; fp[j] = (double)above_n;
+    fn[j] = (double)(P - above_p); tn[j] = (double)(N - above_n);
+    if (confusion) {
+      confusion[j] = (int64_t)above_p;
+      confusion[kMetThresholds + j] = (int64_t)above_n;
+      confusion[2 * kMetThresholds + j] = (int64_t)(N - above_n);
+      confusion[3 * kMetThresholds + j] = (int64_t)(P - above_p);
+    }
+  }
+  double roc = 0.0, pr = 0.0;
+  for (int j = 0; j + 1 < kMetThresholds; ++j) {
+    const double r0 = div_no_nan(tp[j], tp[j] + fn[j]), r1 = div_no_nan(tp[j + 1], tp[j + 1] + fn[j + 1]);
+    const double f0 = div_no_nan(fp[j], fp[j] + tn[j]), f1 = div_no_nan(fp[j + 1], fp[j + 1] + tn[j + 1]);
+    roc += (f0 - f1) * ((r0 + r1) / 2.0);
+    // interpolate_pr_auc (Davis & Goadrich 2006)
+    const double dtp = tp[j] - tp[j + 1];
+    const double p0 = tp[j] + fp[j], p1 = tp[j + 1] + fp[j + 1];
+    const double dp = p0 - p1;
+    const double slope = div_no_nan(dtp, std::fmax(dp, 0.0));
+    const double intercept = tp[j + 1] - slope * p1;
+    const double ratio = (p0 > 0.0 && p1 > 0.0) ? div_no_nan(p0, std::fmax(p1, 0.0)) : 1.0;
+    pr += div_no_nan(slope * (dtp + intercept * std::log(ratio)), std::fmax(tp[j + 1] + fn[j + 1], 0.0));
+  }
+  const unsigned long long rows = P + N;
+  out->rows = (int64_t)rows;
+  out->positives = (int64_t)P;
+  out->correct = (int64_t)correct;
+  out->loss = rows ? loss_sum / (double)rows : 0.0;
+  out->accuracy = rows ? (double)correct / (double)rows : 0.0;
+  out->roc_auc = roc;
+  out->pr_auc = pr;
+}
+
+}  // namespace srs

@@ -111,6 +111,9 @@ struct Slot {
   int req_capacity = 0;             // srs_rank_user_host only: candidates the request staging holds
   int32_t* d_req = nullptr;         // [user row | history | candidate ids] on the device
   int32_t* h_req = nullptr;         // pinned copy of it
+  int label_capacity = 0;           // srs_evaluate_host_batches only (ensure_labels): labels d_labels can hold
+  int32_t* d_labels = nullptr;
+  MetricsReduce* d_mred = nullptr;  // the metrics kernel's CTA partials and ticket for this slot's stream
 };
 
 }  // namespace
@@ -144,7 +147,21 @@ struct srs_model {
   int device_sms = 132;
   int64_t bytes_per_inf = 0;
   Slot slots[kSlots + 1];
+  MetricsCounters* eval_cnt = nullptr;  // srs_evaluate_host_batches (ensure_eval): counts shared by the slots
+  double* eval_loss = nullptr;          //   and one loss sum per batch, added in batch order on the host
+  int eval_loss_capacity = 0;
   std::mutex mu;
+};
+
+// srs_metrics_*: one allocation on the device
+struct MetricsState {
+  MetricsCounters cnt;
+  double loss;
+  MetricsReduce red;
+};
+struct srs_metrics {
+  int device = 0;
+  MetricsState* d = nullptr;
 };
 
 namespace {
@@ -1080,6 +1097,44 @@ int wait_done(srs_model* m, Slot& s) {
   return SRS_OK;
 }
 
+// srs_evaluate_host_batches: the slot's label staging and metrics-reduction scratch.  Only this function
+// allocates or frees them (and srs_model_destroy at the end).
+int ensure_labels(Slot& s, int B) {
+  if (!s.d_mred) {
+    CUDA_TRY(cudaMalloc(&s.d_mred, sizeof(MetricsReduce)));
+    CUDA_TRY(cudaMemsetAsync(s.d_mred, 0, sizeof(MetricsReduce), s.stream));
+  }
+  if (B <= s.label_capacity) return SRS_OK;
+  cudaFree(s.d_labels);
+  s.d_labels = nullptr; s.label_capacity = 0;
+  const int cap = std::max(B, 1024);
+  CUDA_TRY(cudaMalloc(&s.d_labels, (size_t)cap * sizeof(int32_t)));
+  s.label_capacity = cap;
+  return SRS_OK;
+}
+
+// srs_evaluate_host_batches: the model's shared counts and per-batch loss sums for n batches
+int ensure_eval(srs_model* m, int n) {
+  if (!m->eval_cnt) CUDA_TRY(cudaMalloc(&m->eval_cnt, sizeof(MetricsCounters)));
+  if (n <= m->eval_loss_capacity) return SRS_OK;
+  cudaFree(m->eval_loss);
+  m->eval_loss = nullptr; m->eval_loss_capacity = 0;
+  const int cap = std::max(n, 64);
+  CUDA_TRY(cudaMalloc(&m->eval_loss, (size_t)cap * sizeof(double)));
+  m->eval_loss_capacity = cap;
+  return SRS_OK;
+}
+
+// the model kinds whose output is a probability Keras's evaluate metrics apply to
+int check_evaluable(const srs_model* m) {
+  if (m->spec.kind == SRS_DIEN)
+    return fail(SRS_ERR_INVALID, "evaluate does not cover DIEN: its Keras evaluate loss includes the auxiliary "
+                                 "negative-sample loss, which is training-only and not computed here");
+  if (m->spec.kind == SRS_TWOTOWERS && !m->spec.final_dense)
+    return fail(SRS_ERR_INVALID, "evaluate needs a probability: two towers without the final Dense output a raw dot");
+  return SRS_OK;
+}
+
 }  // namespace
 
 // ======================================================================================
@@ -1246,7 +1301,9 @@ void srs_model_destroy(srs_model* m) {
     if (s.h_done) cudaFreeHost(s.h_done);
     if (s.h_res) cudaFreeHost(s.h_res);
     cudaFree(s.d_req);
+    cudaFree(s.d_labels); cudaFree(s.d_mred);
   }
+  cudaFree(m->eval_cnt); cudaFree(m->eval_loss);
   for (void* p : m->owned) cudaFree(p);
   if (m->err_flag) cudaFree(m->err_flag);
   cudaFree(m->movie_feats);
@@ -1628,6 +1685,139 @@ int srs_rank_user_host(srs_model* m, const srs_user_row* user, const int32_t* ca
     if (top_scores) memcpy(top_scores, r_top, (size_t)k * 4);
   }
   return rc;
+}
+
+// ---- evaluate: Keras's loss / accuracy / ROC AUC / PR AUC (metrics.cu) ----------------------------------
+int srs_metrics_create(int32_t device, srs_metrics** out) {
+  if (!out) return fail(SRS_ERR_INVALID, "null argument");
+  *out = nullptr;
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0)
+    return fail(SRS_ERR_CUDA, "no CUDA device available (%s); this library has no CPU path", cudaGetErrorString(e));
+  if (device < 0 || device >= ndev) return fail(SRS_ERR_INVALID, "device %d out of range", device);
+  CUDA_TRY(cudaSetDevice(device));
+  srs_metrics* mt = new srs_metrics();
+  mt->device = device;
+  e = cudaMalloc(&mt->d, sizeof(MetricsState));
+  if (e == cudaSuccess) e = cudaMemset(mt->d, 0, sizeof(MetricsState));
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {
+    cudaFree(mt->d);
+    delete mt;
+    return fail(SRS_ERR_CUDA, "metrics state allocation failed: %s", cudaGetErrorString(e));
+  }
+  *out = mt;
+  return SRS_OK;
+}
+
+void srs_metrics_destroy(srs_metrics* mt) {
+  if (!mt) return;
+  cudaSetDevice(mt->device);
+  cudaFree(mt->d);
+  delete mt;
+}
+
+int srs_metrics_reset(srs_metrics* mt, void* stream) {
+  if (!mt) return fail(SRS_ERR_INVALID, "null metrics state");
+  CUDA_TRY(cudaSetDevice(mt->device));
+  CUDA_TRY(cudaMemsetAsync(mt->d, 0, sizeof(MetricsState), static_cast<cudaStream_t>(stream)));
+  return SRS_OK;
+}
+
+int srs_metrics_update_device(srs_metrics* mt, const float* probs, const float* logits, const int32_t* labels,
+                              int32_t n, void* stream) {
+  if (!mt) return fail(SRS_ERR_INVALID, "null metrics state");
+  if (n < 1) return fail(SRS_ERR_INVALID, "n must be at least 1");
+  if (!probs || !logits || !labels) return fail(SRS_ERR_INVALID, "probs, logits and labels are required");
+  CUDA_TRY(cudaSetDevice(mt->device));
+  CUDA_TRY(launch_metrics_update(probs, logits, labels, n, &mt->d->cnt, &mt->d->red, &mt->d->loss, 1,
+                                 static_cast<cudaStream_t>(stream)));
+  return SRS_OK;
+}
+
+int srs_metrics_result(srs_metrics* mt, srs_eval_result* out, int64_t* confusion) {
+  if (!mt || !out) return fail(SRS_ERR_INVALID, "null argument");
+  CUDA_TRY(cudaSetDevice(mt->device));
+  CUDA_TRY(cudaDeviceSynchronize());
+  MetricsCounters c;
+  double loss = 0.0;
+  CUDA_TRY(cudaMemcpy(&c, &mt->d->cnt, sizeof(c), cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(&loss, &mt->d->loss, sizeof(loss), cudaMemcpyDeviceToHost));
+  if (c.err & kMetErrLabel) return fail(SRS_ERR_INVALID, "a label is not 0 or 1");
+  if (c.err & kMetErrProb) return fail(SRS_ERR_INVALID, "a probability is NaN or outside [0, 1]");
+  srs_eval_result r{};
+  metrics_summarise(c.hist, c.correct, loss, &r, confusion);
+  if (r.rows == 0) return fail(SRS_ERR_INVALID, "no rows have been folded into the metrics");
+  *out = r;
+  return SRS_OK;
+}
+
+int srs_evaluate_host_batches(srs_model* m, int32_t n, const srs_batch* batches, const int32_t* const* labels,
+                              srs_eval_result* out) {
+  if (!m) return fail(SRS_ERR_INVALID, "null model");
+  if (n < 0 || (n > 0 && (!batches || !labels)) || !out) return fail(SRS_ERR_INVALID, "null argument");
+  int rc = check_evaluable(m);
+  if (rc != SRS_OK) return rc;
+  int64_t rows = 0;
+  for (int i = 0; i < n; ++i) {
+    rc = check_batch(m, &batches[i]);
+    if (rc != SRS_OK) return rc;
+    if (batches[i].B > 0 && !labels[i]) return fail(SRS_ERR_INVALID, "labels of batch %d are null", i);
+    rows += batches[i].B;
+  }
+  if (rows == 0) return fail(SRS_ERR_INVALID, "evaluate needs at least one row");
+  std::lock_guard<std::mutex> lock(m->mu);
+  CUDA_TRY(cudaSetDevice(m->device));
+  rc = ensure_eval(m, n);
+  if (rc != SRS_OK) return rc;
+  {
+    Slot& s0 = m->slots[0];
+    rc = ensure_slot(m, s0, 0);
+    if (rc != SRS_OK) return rc;
+    CUDA_TRY(cudaMemsetAsync(m->eval_cnt, 0, sizeof(MetricsCounters), s0.stream));
+    CUDA_TRY(cudaStreamSynchronize(s0.stream));               // before any slot folds into the counts
+  }
+  for (int i = 0; i < n && rc == SRS_OK; ++i) {
+    Slot& s = m->slots[i % kSlots];
+    if (i >= kSlots && s.stream) CUDA_TRY(cudaStreamSynchronize(s.stream));     // slot's previous batch is done
+    const srs_batch* b = &batches[i];
+    if (b->B == 0) continue;
+    rc = stage_and_launch(m, s, b, true);
+    if (rc == SRS_OK) rc = ensure_labels(s, b->B);
+    if (rc != SRS_OK) break;
+    CUDA_TRY(cudaMemcpyAsync(s.d_labels, labels[i], (size_t)b->B * sizeof(int32_t), cudaMemcpyHostToDevice,
+                             s.stream));
+    // the batch's loss sum goes to its own entry: the batch order, not the slot completion order, fixes the sum
+    CUDA_TRY(launch_metrics_update(s.d_probs, s.d_logits, s.d_labels, b->B, m->eval_cnt, s.d_mred,
+                                   m->eval_loss + i, 0, s.stream));
+  }
+  for (int k = 0; k < kSlots; ++k)
+    if (m->slots[k].stream) {
+      cudaError_t e = cudaStreamSynchronize(m->slots[k].stream);
+      if (e != cudaSuccess && rc == SRS_OK)
+        rc = fail(SRS_ERR_CUDA, "stream synchronize failed: %s", cudaGetErrorString(e));
+    }
+  if (rc != SRS_OK) return rc;
+  int flags[kSlots] = {0};
+  CUDA_TRY(cudaMemcpy(flags, m->err_flag + 1, kSlots * sizeof(int), cudaMemcpyDeviceToHost));
+  bool any = false;
+  for (int k = 0; k < kSlots; ++k) any = any || flags[k] != 0;
+  if (any) {
+    CUDA_TRY(cudaMemset(m->err_flag + 1, 0, kSlots * sizeof(int)));
+    return fail(SRS_ERR_RANGE, "an id in a batch was outside its vocabulary");
+  }
+  MetricsCounters c;
+  std::vector<double> batch_loss((size_t)n);
+  CUDA_TRY(cudaMemcpy(&c, m->eval_cnt, sizeof(c), cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(batch_loss.data(), m->eval_loss, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost));
+  if (c.err & kMetErrLabel) return fail(SRS_ERR_INVALID, "a label is not 0 or 1");
+  if (c.err & kMetErrProb) return fail(SRS_ERR_INVALID, "a probability is NaN or outside [0, 1]");
+  double loss = 0.0;
+  for (int i = 0; i < n; ++i)
+    if (batches[i].B > 0) loss += batch_loss[(size_t)i];
+  metrics_summarise(c.hist, c.correct, loss, out, nullptr);
+  return SRS_OK;
 }
 
 int srs_selftest_wgmma(const float* A, const float* B, float* D, int32_t N, int32_t k_blocks,

@@ -243,6 +243,51 @@ class CTRModel:
                                            top.ctypes.data))
         return idx, top
 
+    def evaluate(self, features: Mapping[str, object], labels=None, batch_size: Optional[int] = None):
+        """`model.evaluate(x)` of a model compiled as every reference script compiles it
+        (loss='binary_crossentropy', metrics=['accuracy', AUC(curve='ROC'), AUC(curve='PR')]):
+        returns (loss, accuracy, roc_auc, pr_auc), Keras's order.  `labels` defaults to
+        `features["label"]` (KeyError if missing); they must be 0 or 1.  Batches of `batch_size` rows
+        (default: one) are scored and folded into the metrics on the device
+        (`srs_evaluate_host_batches`); no score comes back.  ValueError for an out-of-range id, a bad
+        label, a NaN or out-of-range probability, no rows, and the models evaluate does not cover
+        (DIEN; two towers without the final Dense)."""
+        r = self.evaluate_result(features, labels, batch_size)
+        return r.loss, r.accuracy, r.roc_auc, r.pr_auc
+
+    def evaluate_result(self, features, labels=None, batch_size: Optional[int] = None) -> _lib.SrsEvalResult:
+        """`evaluate` with the counts: the `srs_eval_result` (rows, positives, correct and the four metrics)."""
+        if labels is None:
+            if "label" not in features:
+                raise KeyError("missing required feature 'label' (or pass labels=)")
+            labels = features["label"]
+        lab = np.asarray(labels)
+        if lab.ndim == 2 and lab.shape[1] == 1:
+            lab = lab[:, 0]
+        if lab.ndim != 1:
+            raise ValueError("labels must be 1-D [N], got shape %s" % (lab.shape,))
+        if lab.dtype.kind == "f" and not np.all(lab == np.trunc(lab)):
+            raise ValueError("labels must be 0 or 1")
+        if lab.dtype.kind not in "biuf":
+            raise ValueError("labels must be numeric 0 or 1")
+        if lab.size and (lab.min() < np.iinfo(np.int32).min or lab.max() > np.iinfo(np.int32).max):
+            raise ValueError("labels must be 0 or 1")
+        lab = np.ascontiguousarray(lab, np.int32)            # the library rejects anything but 0 and 1
+        enc = encode_batch(self.spec, features, narrow_ids=self.narrow_ids)
+        n = enc.B
+        if lab.shape[0] != n:
+            raise ValueError("labels have %d rows, the features %d" % (lab.shape[0], n))
+        if n == 0:
+            raise ValueError("evaluate needs at least one row")
+        step = n if not batch_size else max(int(batch_size), 1)
+        bounds = [(lo, min(n, lo + step)) for lo in range(0, n, step)]
+        keep = []
+        structs = (_lib.SrsBatch * len(bounds))(*[_host_struct(enc.slice(lo, hi), keep) for lo, hi in bounds])
+        lp = (C.c_void_p * len(bounds))(*[lab[lo:hi].ctypes.data for lo, hi in bounds])
+        out = _lib.SrsEvalResult()
+        _lib.check(self._lib.srs_evaluate_host_batches(self._h, len(bounds), structs, lp, C.byref(out)))
+        return out
+
     # ---- one user x n candidates, movie features resident in HBM ----------------------------
     def set_movie_table(self, table):
         """Upload the movie side of the serving feature store (`featurestore.MovieFeatureTable`,
@@ -325,6 +370,65 @@ class CTRModel:
     def status(self):
         """Synchronise; raises ValueError if a device batch carried an out-of-range id."""
         _lib.check(self._lib.srs_model_status(self._h))
+
+
+class Metrics:
+    """Keras's evaluate metrics accumulated on the device (`srs_metrics`): fold batches whose scores are
+    already in HBM - e.g. straight after `CTRModel.predict_device`, in the same CUDA graph - and read
+    the four numbers once at the end."""
+
+    def __init__(self, device: int = 0):
+        self._lib = _lib.load()
+        self.device = int(device)
+        self._h = None
+        h = C.c_void_p()
+        _lib.check(self._lib.srs_metrics_create(self.device, C.byref(h)))
+        self._h = h
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.srs_metrics_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def _stream(self, stream):
+        import torch
+        return (stream if stream is not None else torch.cuda.current_stream(self.device)).cuda_stream
+
+    def update_device(self, probs, logits, labels, stream=None):
+        """Fold n rows: `probs`, `logits` float32 and `labels` int32 CUDA tensors [n], asynchronous on
+        `stream` (a torch stream; default: torch's current stream)."""
+        n = int(probs.numel())
+        for name, t, dt in (("probs", probs, "torch.float32"), ("logits", logits, "torch.float32"),
+                            ("labels", labels, "torch.int32")):
+            if str(t.dtype) != dt or not t.is_cuda or not t.is_contiguous() or int(t.numel()) != n:
+                raise ValueError("%s must be a contiguous %s CUDA tensor of %d elements" % (name, dt[6:], n))
+        _lib.check(self._lib.srs_metrics_update_device(self._h, probs.data_ptr(), logits.data_ptr(),
+                                                       labels.data_ptr(), n, self._stream(stream)))
+
+    def reset(self, stream=None):
+        _lib.check(self._lib.srs_metrics_reset(self._h, self._stream(stream)))
+
+    def result(self) -> dict:
+        """Synchronise and summarise: loss, accuracy, roc_auc, pr_auc, rows, positives, correct, and the
+        confusion counts tp, fp, tn, fn (int64 [200] each, one per Keras threshold)."""
+        out = _lib.SrsEvalResult()
+        conf = np.zeros((4, 200), np.int64)
+        _lib.check(self._lib.srs_metrics_result(self._h, C.byref(out), conf.ctypes.data))
+        r = {k: getattr(out, k) for k, _ in _lib.SrsEvalResult._fields_}
+        r.update(tp=conf[0], fp=conf[1], tn=conf[2], fn=conf[3])
+        return r
 
 
 def launch_count() -> int:

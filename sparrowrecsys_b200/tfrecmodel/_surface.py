@@ -5,7 +5,8 @@ module-level Keras `model` and the call `model.predict(feature_dict)`
 (`TFRecModel/src/com/sparrowrecsys/offline/tensorflow/<Name>.py`).  The modules in
 this package keep that surface: `load(...)` builds the module-level `model` (a
 `sparrowrecsys_b200.model.CTRModel` living on one GPU), `predict(features)` is
-`model.predict(features)`.
+`model.predict(features)` and `evaluate(features)` is `model.evaluate(test_dataset)`, the last
+call of each script (e.g. DIN.py:171-185).
 """
 from __future__ import annotations
 
@@ -49,3 +50,9 @@ class Surface:
         if self.model is None:
             raise RuntimeError("tfrecmodel.%s: call load() before predict()" % self.name)
         return self.model.predict(features, batch_size)
+
+    def evaluate(self, features, batch_size: Optional[int] = None):
+        """(loss, accuracy, roc_auc, pr_auc) over the labelled rows (`features["label"]`)."""
+        if self.model is None:
+            raise RuntimeError("tfrecmodel.%s: call load() before evaluate()" % self.name)
+        return self.model.evaluate(features, batch_size=batch_size)

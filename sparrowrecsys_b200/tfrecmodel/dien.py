@@ -21,3 +21,10 @@ def load(weights=None, spec=None, seed=None, savedmodel=None, device=0):
 
 def predict(features, batch_size=None):
     return _surface.predict(features, batch_size)
+
+
+def evaluate(features, batch_size=None):
+    """Not covered: the reference's DIEN `model.evaluate` returns (loss, roc_auc) with a loss that includes
+    the auxiliary negative-sample loss (DIEN.py:261-304), which is training-only and not computed here."""
+    raise NotImplementedError("tfrecmodel.dien.evaluate: DIEN's Keras evaluate loss includes the auxiliary "
+                              "negative-sample loss, which is training-only and not computed by this library")

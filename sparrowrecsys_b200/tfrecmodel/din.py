@@ -4,6 +4,7 @@
     from tfrecmodel import din
     din.load(weights)            # or load(savedmodel=...), load(spec=..., seed=...)
     p = din.predict(features)    # dict of 1-D columns -> float32 [N,1]
+    loss, acc, roc_auc, pr_auc = din.evaluate(test_features)   # rows labelled by "label"
 """
 from ._surface import Surface
 
@@ -20,3 +21,7 @@ def load(weights=None, spec=None, seed=None, savedmodel=None, device=0):
 
 def predict(features, batch_size=None):
     return _surface.predict(features, batch_size)
+
+
+def evaluate(features, batch_size=None):
+    return _surface.evaluate(features, batch_size)
