@@ -242,9 +242,6 @@ cudaError_t launch_metrics_update(const float* probs, const float* logits, const
 void metrics_summarise(const unsigned long long* hist, unsigned long long correct, double loss_sum,
                        srs_eval_result* out, int64_t* confusion);
 
-// one-time per-device kernel attribute setup (dynamic shared memory opt-in)
-cudaError_t setup_kernel_attributes();
-
 extern int64_t g_launch_count;   // kernels launched by this library
 
 }  // namespace srs

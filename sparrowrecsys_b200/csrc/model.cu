@@ -19,7 +19,6 @@ namespace srs {
 cudaError_t setup_embmlp_attributes();
 cudaError_t setup_deepfm_attributes();
 cudaError_t setup_din_attributes();
-cudaError_t setup_dien_attributes();
 cudaError_t setup_din_wg_attributes();
 #ifdef SRS_DIN_PHASES
 cudaError_t din_take_phases(unsigned long long* out);
@@ -92,28 +91,56 @@ constexpr int kSlots = 4;           // public pipelining slots; slot kSlots is p
                                     // the synchronous srs_predict_host
 constexpr int kErrWords = kSlots + 2;
 
+// The single owner of one device (cudaMalloc) or pinned host (cudaMallocHost) buffer and its capacity in
+// rows.  grow(n, first, bytes) makes room for n rows: when it holds fewer it frees, then allocates
+// max(n, first) rows of bytes(rows) bytes; a failed allocation leaves it empty ({nullptr, 0}).
+template <class T, bool Pinned = false>
+struct Buffer {
+  T* p = nullptr;
+  int cap = 0;
+  Buffer() = default;
+  Buffer(const Buffer&) = delete;
+  Buffer& operator=(const Buffer&) = delete;
+  ~Buffer() { release(); }
+  template <class F>
+  cudaError_t grow(int n, int first, F bytes) {
+    if (n <= cap) return cudaSuccess;
+    release();
+    const int c = std::max(n, first);
+    void* q = nullptr;
+    const cudaError_t e = Pinned ? cudaMallocHost(&q, bytes(c)) : cudaMalloc(&q, bytes(c));
+    if (e == cudaSuccess) { p = static_cast<T*>(q); cap = c; }
+    return e;
+  }
+
+ private:
+  void release() {
+    if (p) { if (Pinned) cudaFreeHost(p); else cudaFree(p); }
+    p = nullptr; cap = 0;
+  }
+};
+template <class T> using PinnedBuffer = Buffer<T, true>;
+
+inline size_t word_bytes(int rows) { return (size_t)rows * 4; }     // one 4-byte word per row
+
 struct Slot {
   cudaStream_t stream = nullptr;
-  int capacity = 0;                 // rows the device staging can hold
-  uint8_t* d_block = nullptr;       // one allocation: [movie|user|hist|movie_genre|user_genre|numerics]
-  float* d_probs = nullptr;
-  float* d_logits = nullptr;
-  int32_t* d_hist32 = nullptr;      // widened history ids when the batch came with hist16
-  int rank_capacity = 0;            // srs_rank_host only: rows d_rank can rank
-  uint8_t* d_rank = nullptr;        // [top_idx cap | top_scores cap | sort scratch]
-  int* h_err = nullptr;             // pinned mirror of the device error flag
+  int capacity = 0;                 // rows d_block, d_probs, d_logits and d_hist32 all hold
+  Buffer<uint8_t> d_block;          // one allocation: [movie|user|hist|movie_genre|user_genre|numerics]
+  Buffer<float> d_probs;
+  Buffer<float> d_logits;
+  Buffer<int32_t> d_hist32;         // widened history ids when the batch came with hist16
+  Buffer<uint8_t> d_rank;           // ranking only: [top_idx cap | top_scores cap | sort scratch]
+  PinnedBuffer<int> h_err;          // pinned mirror of the device error flag
   // latency path (synchronous single calls): the last kernel of the call writes {sequence number, error
   // word} into a pinned record the caller spins on - no device-to-host copy, no stream synchronise
-  uint32_t* h_done = nullptr;       // pinned [4]
+  PinnedBuffer<uint32_t> h_done;    // [4]
   uint32_t seq = 0;
-  int res_capacity = 0;
-  int32_t* h_res = nullptr;         // pinned: top positions [cap] | top scores [cap]
-  int req_capacity = 0;             // srs_rank_user_host only: candidates the request staging holds
-  int32_t* d_req = nullptr;         // [user row | history | candidate ids] on the device
-  int32_t* h_req = nullptr;         // pinned copy of it
-  int label_capacity = 0;           // srs_evaluate_host_batches only (ensure_labels): labels d_labels can hold
-  int32_t* d_labels = nullptr;
-  MetricsReduce* d_mred = nullptr;  // the metrics kernel's CTA partials and ticket for this slot's stream
+  PinnedBuffer<int32_t> h_res;      // top positions [cap] | top scores [cap]
+  Buffer<int32_t> d_req;            // srs_rank_user_host only: [user row | history | candidate ids]
+  PinnedBuffer<int32_t> h_req;      //   and its pinned copy
+  Buffer<int32_t> d_labels;         // srs_evaluate_host_batches only (ensure_labels)
+  Buffer<MetricsReduce> d_mred;     // the metrics kernel's CTA partials and ticket for this slot's stream
 };
 
 }  // namespace
@@ -139,17 +166,16 @@ struct srs_model {
   DeepFmTcParams fm_tc{};
   bool use_fm_tc = false;
   const char* kernel_name = "";
-  bool no_zero_copy = false;         // SRS_ZERO_COPY_SCORES=0 switches the latency path of srs_predict_host off
-  bool zero_copy_scores = false;     // SRS_ZERO_COPY_SCORES=1 (experimental): kernels write the scores
-                                     // of a host batch straight into the caller's pinned buffer
+  int zero_copy_scores = -1;         // the zero_copy_scores option: 0 switches the latency path of srs_predict_host
+                                     // off; 1 (experimental): kernels write the scores of every host batch
+                                     // straight into the caller's pinned buffer; anything else: the default
   void* movie_feats = nullptr;       // srs_model_set_movie_features: [n][8 words] movie-side features in HBM
   int movie_feats_rows = 0;
   int device_sms = 132;
   int64_t bytes_per_inf = 0;
   Slot slots[kSlots + 1];
-  MetricsCounters* eval_cnt = nullptr;  // srs_evaluate_host_batches (ensure_eval): counts shared by the slots
-  double* eval_loss = nullptr;          //   and one loss sum per batch, added in batch order on the host
-  int eval_loss_capacity = 0;
+  Buffer<MetricsCounters> eval_cnt;  // srs_evaluate_host_batches (ensure_eval): counts shared by the slots
+  Buffer<double> eval_loss;          //   and one loss sum per batch, added in batch order on the host
   std::mutex mu;
 };
 
@@ -182,6 +208,7 @@ struct Builder {
   srs_model* m;
   std::map<std::string, const srs_tensor*> by_name;
   int status = SRS_OK;
+  std::vector<float> din_w1, din_w2;    // the permuted DIN top-MLP weights build_din uploaded, for build_din_wg
 
   const srs_tensor* need(const char* name, int64_t rows, int64_t cols) {
     if (status != SRS_OK) return nullptr;
@@ -214,10 +241,12 @@ struct Builder {
     return t->data;
   }
 
-  float* upload(const std::vector<float>& v) {
+  // host weights, or a tensor-core operand image (write_sw128 tiles) -> a device copy the model owns
+  template <class T>
+  T* upload(const std::vector<T>& v) {
     if (status != SRS_OK) return nullptr;
-    float* d = nullptr;
-    size_t bytes = (v.size() ? v.size() : 1) * sizeof(float);
+    T* d = nullptr;
+    size_t bytes = (v.size() ? v.size() : 1) * sizeof(T);
     cudaError_t e = cudaMalloc(&d, bytes);
     if (e != cudaSuccess) {
       status = fail(SRS_ERR_NOMEM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
@@ -225,7 +254,7 @@ struct Builder {
     }
     m->owned.push_back(d);
     if (!v.empty()) {
-      e = cudaMemcpy(d, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice);
+      e = cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
       if (e != cudaSuccess) {
         status = fail(SRS_ERR_CUDA, "cudaMemcpy H2D failed: %s", cudaGetErrorString(e));
         return nullptr;
@@ -582,10 +611,12 @@ int build_din(Builder& B) {
   append(map, iota_map(base + 1, E, EP));        // movieGenre1 emb
   const int nums[8] = {base, base + 1 + E, base + 2 + E, base + 3 + E, 0, 1 + 2 * E, 2 + 2 * E, -1};
   for (int j = 0; j < 8; ++j) map.push_back(nums[j]);
-  p.W1 = B.upload(B.permute(k1, h0, map, 128));
+  B.din_w1 = B.permute(k1, h0, map, 128);
+  B.din_w2 = B.permute(k2, h1, iota_map(0, h0, 128), 64);
+  p.W1 = B.upload(B.din_w1);
   p.b1 = B.upload(B.padvec(b1, h0, 128));
   p.a1 = B.upload(B.padvec(a1, h0, 128));
-  p.W2 = B.upload(B.permute(k2, h1, iota_map(0, h0, 128), 64));
+  p.W2 = B.upload(B.din_w2);
   p.b2 = B.upload(B.padvec(b2, h1, 64));
   p.a2 = B.upload(B.padvec(a2, h1, 64));
   p.w3 = B.upload(B.padvec(k3, h1, 64));
@@ -728,12 +759,10 @@ int build_din_wg(Builder& B) {
   DinParams& p = m->din;
   if (m->EP == 32) {
     // W1^T over the 160 embedding columns of the tile (K blocks 64 | 64 | 32 + zeros), W2^T; units are the
-    // MMA rows, zero-padded to 128 / 64 like the permuted fp32 weights they are read back from
+    // MMA rows, zero-padded to 128 / 64 like the permuted fp32 weights build_din uploaded
     constexpr int KE = 5 * 32;
-    std::vector<float> w1((size_t)(KE + 8) * 128), w2((size_t)128 * 64);
-    cudaError_t e = cudaMemcpy(w1.data(), p.W1, w1.size() * sizeof(float), cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(w2.data(), p.W2, w2.size() * sizeof(float), cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "weight read-back failed: %s", cudaGetErrorString(e));
+    const std::vector<float>& w1 = B.din_w1;     // [KE + 8][128]
+    const std::vector<float>& w2 = B.din_w2;     // [128][64]
     auto w1_get = [&](int u, int k) -> float { return k < KE ? w1[(size_t)k * 128 + u] : 0.f; };
     auto w2_get = [&](int u, int k) -> float { return w2[(size_t)k * 64 + u]; };
     std::vector<uint8_t> img(131072, 0);
@@ -741,13 +770,8 @@ int build_din_wg(Builder& B) {
     write_sw128(img.data() + 49152, 128, 3, true, w1_get);
     write_sw128(img.data() + 98304, 64, 2, false, w2_get);
     write_sw128(img.data() + 114688, 64, 2, true, w2_get);
-    uint8_t* d_img = nullptr;
-    e = cudaMalloc(&d_img, img.size());
-    if (e != cudaSuccess) return fail(SRS_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(e));
-    m->owned.push_back(d_img);
-    e = cudaMemcpy(d_img, img.data(), img.size(), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "image upload failed: %s", cudaGetErrorString(e));
-    p.mlp_image = d_img;
+    p.mlp_image = B.upload(img);
+    if (B.status != SRS_OK) return B.status;
   }
   void* d_split = nullptr;
   const size_t split_bytes = (size_t)m->spec.n_movies * m->EP * 4;
@@ -757,6 +781,8 @@ int build_din_wg(Builder& B) {
   e = launch_split_table(p.movie, d_split, m->spec.n_movies, m->EP, nullptr);
   if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "table split failed: %s", cudaGetErrorString(e));
   p.movie_split = static_cast<const uint8_t*>(d_split);
+  m->use_din_wg = true;
+  m->kernel_name = "din_wg_kernel";
   return B.status;
 }
 
@@ -785,12 +811,6 @@ int build_embmlp_tc(Builder& B) {
   write_sw128(img.data() + 32768, 128, 2, true, w1_get);
   write_sw128(img.data() + 65536, 128, 2, false, w2_get);
   write_sw128(img.data() + 98304, 128, 2, true, w2_get);
-  uint8_t* d_img = nullptr;
-  cudaError_t e = cudaMalloc(&d_img, img.size());
-  if (e != cudaSuccess) return fail(SRS_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(e));
-  m->owned.push_back(d_img);
-  e = cudaMemcpy(d_img, img.data(), img.size(), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "image upload failed: %s", cudaGetErrorString(e));
   const int nrows[7] = {0, 1 + 4 * E, 2 + 4 * E, 3 + 4 * E, 4 + 4 * E, 5 + 10 * E, 6 + 10 * E};
   std::vector<float> w1num(8 * 128, 0.f);
   for (int n = 0; n < 7; ++n)
@@ -799,13 +819,13 @@ int build_embmlp_tc(Builder& B) {
   const EmbMlpParams& v1 = m->emb;
   for (int k = 0; k < 8; ++k) p.genre[k] = v1.genre[k];
   p.movie = v1.movie; p.user = v1.user;
-  p.image = d_img;
+  p.image = B.upload(img);
   p.b1 = v1.b1; p.b2 = v1.b2; p.w3 = v1.w3; p.wide = v1.wide; p.b3 = v1.b3;
   p.w1num = B.upload(w1num);
   p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres; p.cross_buckets = s.cross_buckets;
-  int sms = 0;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
-  p.num_sms = sms > 0 ? sms : 132;
+  p.num_sms = m->device_sms;
+  m->use_emb_tc = true;
+  m->kernel_name = s.kind == SRS_WIDENDEEP ? "embmlp_tc_kernel<wide&deep>" : "embmlp_tc_kernel";
   return B.status;
 }
 
@@ -829,12 +849,6 @@ int build_deepfm_tc(Builder& B) {
   write_sw128(img.data() + 16384, 128, 1, true, w1_get);
   write_sw128(img.data() + 32768, 128, 1, false, w2_get);
   write_sw128(img.data() + 49152, 128, 1, true, w2_get);
-  uint8_t* d_img = nullptr;
-  cudaError_t e = cudaMalloc(&d_img, img.size());
-  if (e != cudaSuccess) return fail(SRS_ERR_NOMEM, "cudaMalloc failed: %s", cudaGetErrorString(e));
-  m->owned.push_back(d_img);
-  e = cudaMemcpy(d_img, img.data(), img.size(), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "image upload failed: %s", cudaGetErrorString(e));
   const int nrows[7] = {0, 1 + E, 2 + E, 3 + E, 4 + E, 5 + 2 * E, 6 + 2 * E};
   std::vector<float> w1num(8 * 64, 0.f);
   for (int n = 0; n < 7; ++n)
@@ -843,16 +857,41 @@ int build_deepfm_tc(Builder& B) {
   const DeepFmParams& v1 = m->fm;
   p.fm_movie = v1.fm_movie; p.fm_user = v1.fm_user; p.fm_mgenre = v1.fm_mgenre; p.fm_ugenre = v1.fm_ugenre;
   p.deep_movie = v1.deep_movie; p.deep_user = v1.deep_user;
-  p.image = d_img;
+  p.image = B.upload(img);
   p.b1 = v1.b1; p.b2 = v1.b2; p.first = v1.first; p.wdeep = v1.wdeep;
   p.w1num = B.upload(w1num);
   for (int d = 0; d < 4; ++d) p.wdot[d] = v1.wdot[d];
   p.bout = v1.bout;
   p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres;
-  int sms = 0;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device);
-  p.num_sms = sms > 0 ? sms : 132;
+  p.num_sms = m->device_sms;
+  m->use_fm_tc = true;
+  m->kernel_name = "deepfm_tc_kernel";
   return B.status;
+}
+
+// Kernel variant of a model kind whose CUDA-core kernel build_* has built: the tensor-core one (its builder
+// `build_tc`) when the shape `fits` it and `by_default`.  The option `key` (environment variable `env`)
+// overrides: cudacore keeps the CUDA-core kernel; tc (and with `rt_alias`, rt / rtp: the names of the earlier
+// row-tile tensor-core DIN kernels) builds the tensor-core one, or fails loudly on a shape that does not fit.
+int choose_kernel(Builder& B, const char* key, const char* env, bool fits, bool by_default, const char* fit_rule,
+                  bool rt_alias, int (*build_tc)(Builder&)) {
+  const char* impl = opt(key, env);
+  bool tc = fits && by_default;
+  if (impl && !strcmp(impl, "cudacore")) tc = false;
+  if (impl && (!strcmp(impl, "tc") || (rt_alias && (!strcmp(impl, "rt") || !strcmp(impl, "rtp"))))) {
+    if (!fits) return fail(SRS_ERR_INVALID, "%s=%s needs %s", env, impl, fit_rule);
+    tc = true;
+  }
+  return tc ? build_tc(B) : SRS_OK;
+}
+
+int check_device(int device) {
+  int ndev = 0;
+  const cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0)
+    return fail(SRS_ERR_CUDA, "no CUDA device available (%s); this library has no CPU path", cudaGetErrorString(e));
+  if (device < 0 || device >= ndev) return fail(SRS_ERR_INVALID, "device %d out of range", device);
+  return SRS_OK;
 }
 
 int64_t bytes_per_inference(const srs_spec& s) {
@@ -886,6 +925,31 @@ int check_batch(const srs_model* m, const srs_batch* b) {
     if (b->hist_stride < m->hist_cols)
       return fail(SRS_ERR_INVALID, "hist_stride %d < history columns %d", b->hist_stride, m->hist_cols);
   }
+  return SRS_OK;
+}
+
+// The batches of a multi-batch call, all checked before its first launch: a call that failed on an argument
+// after launching would leave that launch's error word behind for the next call.  `out[i]` (batch i's probs
+// or labels, named `what`) must be non-null when the batch has rows.
+template <class T>
+int check_batches(const srs_model* m, int n, const srs_batch* batches, T* const* out, const char* what) {
+  for (int i = 0; i < n; ++i) {
+    const int rc = check_batch(m, &batches[i]);
+    if (rc != SRS_OK) return rc;
+    if (batches[i].B > 0 && !out[i]) return fail(SRS_ERR_INVALID, "%s of batch %d are null", what, i);
+  }
+  return SRS_OK;
+}
+
+// The BatchView of a caller's device batch (srs_predict_device, srs_predict_device_gather)
+int device_view(const srs_model* m, const srs_batch* b, float* probs, float* logits, BatchView* v) {
+  if (m->hist_cols > 0 && !b->hist)
+    return fail(SRS_ERR_INVALID, "device batches carry int32 history ids (hist16 is for host batches)");
+  *v = BatchView{};
+  v->B = b->B; v->hist_stride = b->hist_stride;
+  v->movie_id = b->movie_id; v->user_id = b->user_id; v->hist = b->hist;
+  v->movie_genre = b->movie_genre; v->user_genre = b->user_genre; v->numerics = b->numerics;
+  v->probs = probs; v->logits = logits; v->err_flag = m->err_flag;
   return SRS_OK;
 }
 
@@ -936,22 +1000,35 @@ PackedLayout packed_layout(const srs_model* m, size_t B, bool narrow_hist = fals
 
 int ensure_slot(srs_model* m, Slot& s, int B) {
   if (!s.stream) CUDA_TRY(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
-  if (!s.h_err) {
-    CUDA_TRY(cudaMallocHost(&s.h_err, sizeof(int)));
-    *s.h_err = 0;
+  if (!s.h_err.p) {
+    CUDA_TRY(s.h_err.grow(1, 1, [](int) { return sizeof(int); }));
+    *s.h_err.p = 0;
   }
   if (B <= s.capacity) return SRS_OK;
-  int cap = std::max(B, 1024);
-  cudaFree(s.d_block); cudaFree(s.d_probs); cudaFree(s.d_logits); cudaFree(s.d_hist32);
-  s.d_block = nullptr; s.d_probs = nullptr; s.d_logits = nullptr; s.d_hist32 = nullptr;
+  const int cap = std::max(B, 1024);
   s.capacity = 0;
-  CUDA_TRY(cudaMalloc(&s.d_block, packed_layout(m, (size_t)cap).total + 256));
-  CUDA_TRY(cudaMalloc(&s.d_probs, (size_t)cap * 4));
-  CUDA_TRY(cudaMalloc(&s.d_logits, (size_t)cap * 4));
+  CUDA_TRY(s.d_block.grow(cap, cap, [&](int c) { return packed_layout(m, (size_t)c).total + 256; }));
+  CUDA_TRY(s.d_probs.grow(cap, cap, word_bytes));
+  CUDA_TRY(s.d_logits.grow(cap, cap, word_bytes));
   if (m->hist_cols > 0 && m->spec.n_movies <= 65536)
-    CUDA_TRY(cudaMalloc(&s.d_hist32, (size_t)cap * m->hist_cols * 4));
+    CUDA_TRY(s.d_hist32.grow(cap, cap, [&](int c) { return (size_t)c * m->hist_cols * 4; }));
   s.capacity = cap;
   return SRS_OK;
+}
+
+// The BatchView of n rows staged in the slot's block in the packed order; the scores go to the slot's buffer.
+BatchView staged_view(srs_model* m, Slot& s, size_t n, const PackedLayout& L) {
+  const uint8_t* d = s.d_block.p;
+  BatchView v{};
+  v.B = (int)n; v.hist_stride = m->hist_cols;
+  v.movie_id = reinterpret_cast<const int32_t*>(d + L.movie);
+  v.user_id = reinterpret_cast<const int32_t*>(d + L.user);
+  v.hist = reinterpret_cast<const int32_t*>(d + L.hist);
+  v.movie_genre = reinterpret_cast<const int32_t*>(d + L.mg);
+  v.user_genre = reinterpret_cast<const int32_t*>(d + L.ug);
+  v.numerics = reinterpret_cast<const float*>(d + L.num);
+  v.probs = s.d_probs.p; v.logits = nullptr; v.err_flag = slot_err(m, s);
+  return v;
 }
 
 // H2D of the batch into the slot's staging and the forward kernel, on the slot's stream;
@@ -970,7 +1047,7 @@ int stage_and_launch(srs_model* m, Slot& s, const srs_batch* b, bool want_logits
   const bool dense_feats = !(k == SRS_NEURALCF || k == SRS_TWOTOWERS);
   const bool narrow = m->hist_cols > 0 && b->hist16 != nullptr;
   const PackedLayout L = packed_layout(m, B, narrow);
-  uint8_t* d = s.d_block;
+  uint8_t* d = s.d_block.p;
   const uint8_t* h0 = reinterpret_cast<const uint8_t*>(b->movie_id);
   bool packed = reinterpret_cast<const uint8_t*>(b->user_id) == h0 + L.user;
   if (m->hist_cols > 0)
@@ -1002,46 +1079,42 @@ int stage_and_launch(srs_model* m, Slot& s, const srs_batch* b, bool want_logits
       CUDA_TRY(cudaMemcpyAsync(d + L.num, b->numerics, B * 7 * 4, cudaMemcpyHostToDevice, s.stream));
     }
   }
-  BatchView v{};
-  v.B = b->B; v.hist_stride = m->hist_cols;
-  v.movie_id = reinterpret_cast<const int32_t*>(d + L.movie);
-  v.user_id = reinterpret_cast<const int32_t*>(d + L.user);
-  v.hist = reinterpret_cast<const int32_t*>(d + L.hist);
+  BatchView v = staged_view(m, s, B, L);
   if (narrow) {
-    CUDA_TRY(launch_widen_u16(reinterpret_cast<const uint16_t*>(d + L.hist), s.d_hist32,
+    CUDA_TRY(launch_widen_u16(reinterpret_cast<const uint16_t*>(d + L.hist), s.d_hist32.p,
                               (int64_t)B * m->hist_cols, s.stream));
-    v.hist = s.d_hist32;
+    v.hist = s.d_hist32.p;
   }
-  v.movie_genre = reinterpret_cast<const int32_t*>(d + L.mg);
-  v.user_genre = reinterpret_cast<const int32_t*>(d + L.ug);
-  v.numerics = reinterpret_cast<const float*>(d + L.num);
-  v.probs = probs_out ? probs_out : s.d_probs;
-  v.logits = want_logits ? (logits_out ? logits_out : s.d_logits) : nullptr; v.err_flag = slot_err(m, s);
+  if (probs_out) v.probs = probs_out;
+  if (want_logits) v.logits = logits_out ? logits_out : s.d_logits.p;
   return launch(m, v, s.stream);
+}
+
+// device-visible alias of a host pointer if it is pinned (page-locked) memory, else nullptr
+float* pinned_alias(float* p) {
+  if (!p) return nullptr;
+  cudaPointerAttributes at{};
+  if (cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer)
+    return static_cast<float*>(at.devicePointer);
+  cudaGetLastError();                                   // pageable memory: not an error
+  return nullptr;
 }
 
 int enqueue_host(srs_model* m, Slot& s, const srs_batch* b, float* probs, float* logits,
                  bool copy_err = true) {
   if (!probs) return fail(SRS_ERR_INVALID, "probs is null");
-  // Experimental (SRS_ZERO_COPY_SCORES=1): a pinned output buffer is device-addressable under
+  // Experimental (zero_copy_scores=1): a pinned output buffer is device-addressable under
   // unified addressing, so the kernel can write the 4 B per row over PCIe itself and the
   // device-to-host copy - one driver call and one copy-engine operation per batch - goes away.
-  float* direct = nullptr;
-  if (m->zero_copy_scores && b && b->B > 0) {
-    cudaPointerAttributes at{};
-    if (cudaPointerGetAttributes(&at, probs) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer)
-      direct = static_cast<float*>(at.devicePointer);
-    else
-      cudaGetLastError();                                 // pageable memory: not an error, use the copy
-  }
+  float* direct = m->zero_copy_scores == 1 && b && b->B > 0 ? pinned_alias(probs) : nullptr;
   int rc = stage_and_launch(m, s, b, logits != nullptr, direct);
   if (rc != SRS_OK) return rc;
   if (b->B == 0) return SRS_OK;
   const size_t B = (size_t)b->B;
-  if (!direct) CUDA_TRY(cudaMemcpyAsync(probs, s.d_probs, B * 4, cudaMemcpyDeviceToHost, s.stream));
-  if (logits) CUDA_TRY(cudaMemcpyAsync(logits, s.d_logits, B * 4, cudaMemcpyDeviceToHost, s.stream));
+  if (!direct) CUDA_TRY(cudaMemcpyAsync(probs, s.d_probs.p, B * 4, cudaMemcpyDeviceToHost, s.stream));
+  if (logits) CUDA_TRY(cudaMemcpyAsync(logits, s.d_logits.p, B * 4, cudaMemcpyDeviceToHost, s.stream));
   if (copy_err)
-    CUDA_TRY(cudaMemcpyAsync(s.h_err, slot_err(m, s), sizeof(int), cudaMemcpyDeviceToHost, s.stream));
+    CUDA_TRY(cudaMemcpyAsync(s.h_err.p, slot_err(m, s), sizeof(int), cudaMemcpyDeviceToHost, s.stream));
   return SRS_OK;
 }
 
@@ -1049,8 +1122,8 @@ int wait_slot(srs_model* m, Slot& s) {
   if (!s.stream) return SRS_OK;
   CUDA_TRY(cudaSetDevice(m->device));
   CUDA_TRY(cudaStreamSynchronize(s.stream));
-  if (s.h_err && *s.h_err) {
-    *s.h_err = 0;
+  if (s.h_err.p && *s.h_err.p) {
+    *s.h_err.p = 0;
     CUDA_TRY(cudaMemsetAsync(slot_err(m, s), 0, sizeof(int), s.stream));
     CUDA_TRY(cudaStreamSynchronize(s.stream));
     return fail(SRS_ERR_RANGE, "an id in the batch is outside its vocabulary");
@@ -1058,25 +1131,20 @@ int wait_slot(srs_model* m, Slot& s) {
   return SRS_OK;
 }
 
+// The completion record of the latency path and room for k ranking results (positions | scores).
 int ensure_done(Slot& s, int k) {
-  if (!s.h_done) {
-    CUDA_TRY(cudaMallocHost(&s.h_done, 4 * sizeof(uint32_t)));
-    memset(s.h_done, 0, 4 * sizeof(uint32_t));
+  if (!s.h_done.p) {
+    CUDA_TRY(s.h_done.grow(1, 1, [](int) { return 4 * sizeof(uint32_t); }));
+    memset(s.h_done.p, 0, 4 * sizeof(uint32_t));
   }
-  if (k > s.res_capacity) {
-    if (s.h_res) cudaFreeHost(s.h_res);
-    s.h_res = nullptr; s.res_capacity = 0;
-    const int cap = std::max(k, 1024);
-    CUDA_TRY(cudaMallocHost(&s.h_res, (size_t)cap * 8));
-    s.res_capacity = cap;
-  }
+  CUDA_TRY(s.h_res.grow(k, std::max(k, 1024), [](int c) { return (size_t)c * 8; }));
   return SRS_OK;
 }
 
 // Spin until the call's last kernel has published sequence number `s.seq` (the stream is polled now
 // and then so that a failed launch or a faulting kernel ends the wait with an error, not a hang).
-int wait_done(srs_model* m, Slot& s) {
-  volatile uint32_t* d = s.h_done;
+int wait_done(Slot& s) {
+  volatile uint32_t* d = s.h_done.p;
   uint64_t spins = 0;
   while (d[0] != s.seq) {
     if ((++spins & 0x1FFF) == 0) {
@@ -1093,36 +1161,78 @@ int wait_done(srs_model* m, Slot& s) {
   }
   std::atomic_thread_fence(std::memory_order_acquire);
   if (d[1]) return fail(SRS_ERR_RANGE, "an id in the batch is outside its vocabulary");
-  (void)m;
   return SRS_OK;
 }
 
-// srs_evaluate_host_batches: the slot's label staging and metrics-reduction scratch.  Only this function
-// allocates or frees them (and srs_model_destroy at the end).
-int ensure_labels(Slot& s, int B) {
-  if (!s.d_mred) {
-    CUDA_TRY(cudaMalloc(&s.d_mred, sizeof(MetricsReduce)));
-    CUDA_TRY(cudaMemsetAsync(s.d_mred, 0, sizeof(MetricsReduce), s.stream));
+// The ranking tail of srs_rank_host / srs_rank_user_host: the k best of the n scores in s.d_probs.  The ranking
+// kernel writes the k positions / scores into pinned host memory and then the completion record the caller
+// spins on: no device-to-host copy, no stream synchronise.
+int rank_and_wait(srs_model* m, Slot& s, int n, int k, int32_t* top_idx, float* top_scores) {
+  int rc = ensure_done(s, k);
+  if (rc != SRS_OK) return rc;
+  if (k > 0)
+    CUDA_TRY(s.d_rank.grow(n, s.capacity, [](int c) { return (size_t)c * 8 + topk_scratch_bytes(c) + 256; }));
+  int32_t* r_idx = s.h_res.p;
+  float* r_top = reinterpret_cast<float*>(s.h_res.p + s.h_res.cap);
+  void* scratch = s.d_rank.p ? s.d_rank.p + (size_t)s.d_rank.cap * 8 : nullptr;
+  s.seq += 1;
+  CUDA_TRY(launch_topk_done(s.d_probs.p, n, k, r_idx, r_top, scratch, slot_err(m, s), s.h_done.p, s.seq, s.stream));
+  rc = wait_done(s);
+  if (k > 0) {
+    memcpy(top_idx, r_idx, (size_t)k * 4);
+    if (top_scores) memcpy(top_scores, r_top, (size_t)k * 4);
   }
-  if (B <= s.label_capacity) return SRS_OK;
-  cudaFree(s.d_labels);
-  s.d_labels = nullptr; s.label_capacity = 0;
-  const int cap = std::max(B, 1024);
-  CUDA_TRY(cudaMalloc(&s.d_labels, (size_t)cap * sizeof(int32_t)));
-  s.label_capacity = cap;
+  return rc;
+}
+
+// srs_evaluate_host_batches: the slot's label staging and metrics-reduction scratch
+int ensure_labels(Slot& s, int B) {
+  if (!s.d_mred.p) {
+    CUDA_TRY(s.d_mred.grow(1, 1, [](int) { return sizeof(MetricsReduce); }));
+    CUDA_TRY(cudaMemsetAsync(s.d_mred.p, 0, sizeof(MetricsReduce), s.stream));
+  }
+  CUDA_TRY(s.d_labels.grow(B, 1024, word_bytes));
   return SRS_OK;
 }
 
 // srs_evaluate_host_batches: the model's shared counts and per-batch loss sums for n batches
 int ensure_eval(srs_model* m, int n) {
-  if (!m->eval_cnt) CUDA_TRY(cudaMalloc(&m->eval_cnt, sizeof(MetricsCounters)));
-  if (n <= m->eval_loss_capacity) return SRS_OK;
-  cudaFree(m->eval_loss);
-  m->eval_loss = nullptr; m->eval_loss_capacity = 0;
-  const int cap = std::max(n, 64);
-  CUDA_TRY(cudaMalloc(&m->eval_loss, (size_t)cap * sizeof(double)));
-  m->eval_loss_capacity = cap;
+  CUDA_TRY(m->eval_cnt.grow(1, 1, [](int) { return sizeof(MetricsCounters); }));
+  CUDA_TRY(m->eval_loss.grow(n, 64, [](int c) { return (size_t)c * sizeof(double); }));
   return SRS_OK;
+}
+
+// Reads the error words [first, first + n), and clears them when one is set.
+int read_error_words(int* first, int n) {
+  int flags[kErrWords] = {0};
+  CUDA_TRY(cudaMemcpy(flags, first, n * sizeof(int), cudaMemcpyDeviceToHost));
+  for (int k = 0; k < n; ++k)
+    if (flags[k]) {
+      CUDA_TRY(cudaMemset(first, 0, n * sizeof(int)));
+      return fail(SRS_ERR_RANGE, "an id in a batch was outside its vocabulary");
+    }
+  return SRS_OK;
+}
+
+// Runs step(slot, i) for the batches i = 0..n-1 round-robin over the public slots, each slot taking its next
+// batch once its previous one is done.  Then every slot is synchronised, the first failure is kept, and - when
+// there is none - the slots' error words are read.
+template <class Step>
+int run_pipelined(srs_model* m, int n, Step step) {
+  int rc = SRS_OK;
+  for (int i = 0; i < n && rc == SRS_OK; ++i) {
+    Slot& s = m->slots[i % kSlots];
+    if (i >= kSlots && s.stream) CUDA_TRY(cudaStreamSynchronize(s.stream));     // slot's previous batch is done
+    rc = step(s, i);
+  }
+  for (int k = 0; k < kSlots; ++k)
+    if (m->slots[k].stream) {
+      cudaError_t e = cudaStreamSynchronize(m->slots[k].stream);
+      if (e != cudaSuccess && rc == SRS_OK)
+        rc = fail(SRS_ERR_CUDA, "stream synchronize failed: %s", cudaGetErrorString(e));
+    }
+  if (rc != SRS_OK) return rc;
+  return read_error_words(m->err_flag + 1, kSlots);
 }
 
 // the model kinds whose output is a probability Keras's evaluate metrics apply to
@@ -1154,12 +1264,8 @@ int srs_model_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_
   if (spec->n_movies < 1 || spec->n_users < 1 || spec->n_genres < 1)
     return fail(SRS_ERR_INVALID, "vocabulary sizes must be positive");
   if (spec->n_hidden < 0 || spec->n_hidden > 4) return fail(SRS_ERR_INVALID, "n_hidden must be in 0..4");
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0)
-    return fail(SRS_ERR_CUDA, "no CUDA device available (%s); this library has no CPU path",
-                cudaGetErrorString(e));
-  if (device < 0 || device >= ndev) return fail(SRS_ERR_INVALID, "device %d out of range", device);
+  int rc = check_device(device);
+  if (rc != SRS_OK) return rc;
   CUDA_TRY(cudaSetDevice(device));
   CUDA_TRY(setup_embmlp_attributes());
   CUDA_TRY(setup_deepfm_attributes());
@@ -1172,15 +1278,10 @@ int srs_model_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_
   srs_model* m = new srs_model();
   m->spec = *spec;
   m->device = device;
-  if (const char* zc = opt("zero_copy_scores", "SRS_ZERO_COPY_SCORES")) {
-    m->zero_copy_scores = atoi(zc) == 1;              // pipelined paths too (experimental)
-    m->no_zero_copy = atoi(zc) == 0;
-  }
-  {
-    int sms = 0;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    m->device_sms = sms > 0 ? sms : 132;
-  }
+  if (const char* zc = opt("zero_copy_scores", "SRS_ZERO_COPY_SCORES")) m->zero_copy_scores = atoi(zc);
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+  m->device_sms = sms > 0 ? sms : 132;
   m->EP = round_ep(spec->emb_dim);
   m->hist_cols = (spec->kind == SRS_DIN || spec->kind == SRS_DIEN) ? spec->hist_len
                  : spec->kind == SRS_WIDENDEEP ? 1 : 0;
@@ -1188,80 +1289,37 @@ int srs_model_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_
   Builder B{m};
   for (int i = 0; i < n_tensors; ++i)
     if (tensors[i].name) B.by_name[tensors[i].name] = &tensors[i];
-  int rc;
   switch (spec->kind) {
     case SRS_NEURALCF:
     case SRS_TWOTOWERS: rc = build_ncf(B); break;
     case SRS_EMBEDDINGMLP:
-    case SRS_WIDENDEEP: {
+    case SRS_WIDENDEEP:
+      // tensor cores for the reference shape (E <= 12)
       rc = build_embmlp(B);
-      // tensor-core path for the reference shape (E <= 12); SRS_EMBMLP_IMPL=cudacore|tc overrides
-      const char* impl_c = opt("embmlp_impl", "SRS_EMBMLP_IMPL");
-      const std::string impl_s = impl_c ? impl_c : "";
-      const char* impl = impl_c ? impl_s.c_str() : nullptr;
-      const bool fits = m->EP == 12;
-      bool want = fits;
-      if (impl && !strcmp(impl, "cudacore")) want = false;
-      if (impl && !strcmp(impl, "tc")) {
-        if (!fits && rc == SRS_OK) rc = fail(SRS_ERR_INVALID, "SRS_EMBMLP_IMPL=tc needs emb_dim <= 12");
-        want = true;
-      }
-      if (rc == SRS_OK && want) {
-        rc = build_embmlp_tc(B);
-        if (rc == SRS_OK) {
-          m->use_emb_tc = true;
-          m->kernel_name = spec->kind == SRS_WIDENDEEP ? "embmlp_tc_kernel<wide&deep>" : "embmlp_tc_kernel";
-        }
-      }
+      if (rc == SRS_OK)
+        rc = choose_kernel(B, "embmlp_impl", "SRS_EMBMLP_IMPL", m->EP == 12, true, "emb_dim <= 12", false,
+                           build_embmlp_tc);
       break;
-    }
-    case SRS_DEEPFM: {
+    case SRS_DEEPFM:
+      // tensor-core deep MLP when emb_dim pads to 16
       rc = build_deepfm(B);
-      // tensor-core deep MLP when emb_dim pads to 16; SRS_DEEPFM_IMPL=cudacore|tc overrides
-      const char* impl_c = opt("deepfm_impl", "SRS_DEEPFM_IMPL");
-      const std::string impl_s = impl_c ? impl_c : "";
-      const char* impl = impl_c ? impl_s.c_str() : nullptr;
-      const bool fits = m->EP == 16;
-      bool want = fits;
-      if (impl && !strcmp(impl, "cudacore")) want = false;
-      if (impl && !strcmp(impl, "tc")) {
-        if (!fits && rc == SRS_OK) rc = fail(SRS_ERR_INVALID, "SRS_DEEPFM_IMPL=tc needs 12 < emb_dim <= 16");
-        want = true;
-      }
-      if (rc == SRS_OK && want) {
-        rc = build_deepfm_tc(B);
-        if (rc == SRS_OK) { m->use_fm_tc = true; m->kernel_name = "deepfm_tc_kernel"; }
-      }
+      if (rc == SRS_OK)
+        rc = choose_kernel(B, "deepfm_impl", "SRS_DEEPFM_IMPL", m->EP == 16, true, "12 < emb_dim <= 16", false,
+                           build_deepfm_tc);
       break;
-    }
     case SRS_DEEPFM_V2: rc = build_deepfm2(B); break;
     case SRS_DIEN: rc = build_dien(B); break;
-    default: {
+    default:
+      // the activation unit on warpgroup MMAs (din_wg.cu) for E padded to 32 or 64; the default for T > 8,
+      // where it measured faster on the H100 (DESIGN.md section 6): BASELINE cfg 5 (E padded to 64) and
+      // cfg 3 (E = 32, where the top MLP runs on wgmma too).  cudacore stays the only kernel for E <= 16.
       rc = build_din(B);
-      // kernel selection (SRS_DIN_IMPL=cudacore|tc overrides; tc fails loudly on an unsupported shape):
-      //   tc  activation unit on warpgroup MMAs (din_wg.cu): E padded to 32 or 64.  The default for T > 8,
-      //       where it measured faster on the H100 (DESIGN.md section 6): BASELINE cfg 5 (E padded to 64)
-      //       and cfg 3 (E = 32, where the top MLP runs on wgmma too).  cudacore stays the only kernel for
-      //       E <= 16.
-      //   rt, rtp  the names of the earlier row-tile tensor-core kernels; callers that pass them get the
-      //       same tensor-core kernel as tc.
-      const char* impl_c = opt("din_impl", "SRS_DIN_IMPL");
-      const std::string impl_s = impl_c ? impl_c : "";
-      const char* impl = impl_c ? impl_s.c_str() : nullptr;
-      const bool fits_tc = m->EP == 32 || m->EP == 64;
-      bool want_tc = fits_tc && spec->hist_len > 8;
-      if (impl && !strcmp(impl, "cudacore")) want_tc = false;
-      if (impl && (!strcmp(impl, "tc") || !strcmp(impl, "rt") || !strcmp(impl, "rtp"))) {
-        if (!fits_tc && rc == SRS_OK) rc = fail(SRS_ERR_INVALID, "SRS_DIN_IMPL=%s needs 16 < emb_dim <= 64", impl);
-        want_tc = true;
-      }
-      if (rc == SRS_OK && want_tc) {
-        rc = build_din_wg(B);
-        if (rc == SRS_OK) { m->use_din_wg = true; m->kernel_name = "din_wg_kernel"; }
-      }
+      if (rc == SRS_OK)
+        rc = choose_kernel(B, "din_impl", "SRS_DIN_IMPL", m->EP == 32 || m->EP == 64, spec->hist_len > 8,
+                           "16 < emb_dim <= 64", true, build_din_wg);
       break;
-    }
   }
+  cudaError_t e = cudaSuccess;
   if (rc == SRS_OK) {
     e = cudaMalloc(&m->err_flag, kErrWords * sizeof(int));
     if (e == cudaSuccess) e = cudaMemset(m->err_flag, 0, kErrWords * sizeof(int));
@@ -1292,22 +1350,12 @@ int srs_model_create_ex(const srs_spec* spec, const srs_tensor* tensors, int32_t
 void srs_model_destroy(srs_model* m) {
   if (!m) return;
   cudaSetDevice(m->device);
-  for (Slot& s : m->slots) {
+  for (Slot& s : m->slots)
     if (s.stream) { cudaStreamSynchronize(s.stream); cudaStreamDestroy(s.stream); }
-    cudaFree(s.d_block); cudaFree(s.d_probs); cudaFree(s.d_logits); cudaFree(s.d_rank);
-    cudaFree(s.d_hist32);
-    if (s.h_err) cudaFreeHost(s.h_err);
-    if (s.h_req) cudaFreeHost(s.h_req);
-    if (s.h_done) cudaFreeHost(s.h_done);
-    if (s.h_res) cudaFreeHost(s.h_res);
-    cudaFree(s.d_req);
-    cudaFree(s.d_labels); cudaFree(s.d_mred);
-  }
-  cudaFree(m->eval_cnt); cudaFree(m->eval_loss);
   for (void* p : m->owned) cudaFree(p);
   if (m->err_flag) cudaFree(m->err_flag);
   cudaFree(m->movie_feats);
-  delete m;
+  delete m;                                             // the slot and evaluate buffers free themselves
 }
 
 int srs_predict_device(srs_model* m, const srs_batch* b, float* probs, float* logits, void* stream) {
@@ -1315,14 +1363,10 @@ int srs_predict_device(srs_model* m, const srs_batch* b, float* probs, float* lo
   if (rc != SRS_OK) return rc;
   if (!probs) return fail(SRS_ERR_INVALID, "probs is null");
   if (b->B == 0) return SRS_OK;
-  if (m->hist_cols > 0 && !b->hist)
-    return fail(SRS_ERR_INVALID, "device batches carry int32 history ids (hist16 is for host batches)");
+  BatchView v;
+  rc = device_view(m, b, probs, logits, &v);
+  if (rc != SRS_OK) return rc;
   CUDA_TRY(cudaSetDevice(m->device));
-  BatchView v{};
-  v.B = b->B; v.hist_stride = b->hist_stride;
-  v.movie_id = b->movie_id; v.user_id = b->user_id; v.hist = b->hist;
-  v.movie_genre = b->movie_genre; v.user_genre = b->user_genre; v.numerics = b->numerics;
-  v.probs = probs; v.logits = logits; v.err_flag = m->err_flag;
   return launch(m, v, static_cast<cudaStream_t>(stream));
 }
 
@@ -1359,14 +1403,10 @@ int srs_predict_device_gather(srs_model* m, const srs_batch* b, srs_gather* gg, 
   if (!gather_connected(g)) return fail(SRS_ERR_INVALID, "srs_gather_connect has not been called");
   if (gather_device(g) != m->device) return fail(SRS_ERR_INVALID, "gather object lives on another device");
   if (b->B < 1 || b->B > gather_slice_rows(g)) return fail(SRS_ERR_INVALID, "batch rows must be in 1..slice_rows");
-  if (m->hist_cols > 0 && !b->hist)
-    return fail(SRS_ERR_INVALID, "device batches carry int32 history ids (hist16 is for host batches)");
+  BatchView v;
+  rc = device_view(m, b, nullptr, nullptr, &v);          // gather_begin_step points the scores at the exchange
+  if (rc != SRS_OK) return rc;
   CUDA_TRY(cudaSetDevice(m->device));
-  BatchView v{};
-  v.B = b->B; v.hist_stride = b->hist_stride;
-  v.movie_id = b->movie_id; v.user_id = b->user_id; v.hist = b->hist;
-  v.movie_genre = b->movie_genre; v.user_genre = b->user_genre; v.numerics = b->numerics;
-  v.logits = nullptr; v.err_flag = m->err_flag;
   const bool in_kernel = m->spec.kind == SRS_DIN && m->use_din_wg;   // kernels ending in gather_signal_tail()
   gather_begin_step(g, v, in_kernel);
   rc = launch(m, v, static_cast<cudaStream_t>(stream));
@@ -1400,16 +1440,6 @@ int srs_gather_copy_scores(srs_gather* gg, float* dst, int32_t dst_on_host, void
   return SRS_OK;
 }
 
-// device-visible alias of a host pointer if it is pinned (page-locked) memory, else nullptr
-static float* pinned_alias(float* p) {
-  if (!p) return nullptr;
-  cudaPointerAttributes at{};
-  if (cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer)
-    return static_cast<float*>(at.devicePointer);
-  cudaGetLastError();                                   // pageable memory: not an error
-  return nullptr;
-}
-
 int srs_predict_host(srs_model* m, const srs_batch* b, float* probs, float* logits) {
   if (!m) return fail(SRS_ERR_INVALID, "null model");
   std::lock_guard<std::mutex> lock(m->mu);
@@ -1417,7 +1447,7 @@ int srs_predict_host(srs_model* m, const srs_batch* b, float* probs, float* logi
   // Latency path: when the caller's output buffers are pinned, the kernel writes the scores (4 B per row)
   // straight into them over PCIe and a one-warp kernel publishes the completion record: two copy-engine
   // operations, two driver calls and the stream synchronise of the general path go away.
-  if (probs && b && b->B > 0 && !m->no_zero_copy) {
+  if (probs && b && b->B > 0 && m->zero_copy_scores != 0) {
     float* dp = pinned_alias(probs);
     float* dl = logits ? pinned_alias(logits) : nullptr;
     if (dp && (!logits || dl)) {
@@ -1427,8 +1457,8 @@ int srs_predict_host(srs_model* m, const srs_batch* b, float* probs, float* logi
       rc = stage_and_launch(m, s, b, logits != nullptr, dp, dl);
       if (rc != SRS_OK) return rc;
       s.seq += 1;
-      CUDA_TRY(launch_finish(slot_err(m, s), s.h_done, s.seq, s.stream));
-      return wait_done(m, s);
+      CUDA_TRY(launch_finish(slot_err(m, s), s.h_done.p, s.seq, s.stream));
+      return wait_done(s);
     }
   }
   int rc = enqueue_host(m, s, b, probs, logits);
@@ -1440,30 +1470,14 @@ int srs_predict_host_batches(srs_model* m, int32_t n, const srs_batch* batches,
                              float* const* probs, float* const* logits) {
   if (!m) return fail(SRS_ERR_INVALID, "null model");
   if (n < 0 || (n > 0 && (!batches || !probs))) return fail(SRS_ERR_INVALID, "null argument");
+  int rc = check_batches(m, n, batches, probs, "probs");
+  if (rc != SRS_OK) return rc;
   std::lock_guard<std::mutex> lock(m->mu);
   CUDA_TRY(cudaSetDevice(m->device));
-  int rc = SRS_OK;
-  for (int i = 0; i < n && rc == SRS_OK; ++i) {
-    Slot& s = m->slots[i % kSlots];
-    if (i >= kSlots) CUDA_TRY(cudaStreamSynchronize(s.stream));     // slot's previous batch is out
-    rc = enqueue_host(m, s, &batches[i], probs[i], logits ? logits[i] : nullptr, false);
-  }
-  for (int k = 0; k < kSlots; ++k)
-    if (m->slots[k].stream) {
-      cudaError_t e = cudaStreamSynchronize(m->slots[k].stream);
-      if (e != cudaSuccess && rc == SRS_OK)
-        rc = fail(SRS_ERR_CUDA, "stream synchronize failed: %s", cudaGetErrorString(e));
-    }
-  if (rc != SRS_OK) return rc;
-  int flags[kSlots] = {0};
-  CUDA_TRY(cudaMemcpy(flags, m->err_flag + 1, kSlots * sizeof(int), cudaMemcpyDeviceToHost));
-  bool any = false;
-  for (int k = 0; k < kSlots; ++k) any = any || flags[k] != 0;
-  if (any) {
-    CUDA_TRY(cudaMemset(m->err_flag + 1, 0, kSlots * sizeof(int)));
-    return fail(SRS_ERR_RANGE, "an id in a batch was outside its vocabulary");
-  }
-  return SRS_OK;
+  return run_pipelined(m, n, [&](Slot& s, int i) -> int {
+    if (batches[i].B == 0) return SRS_OK;                // nothing to stage, and its probs may be null
+    return enqueue_host(m, s, &batches[i], probs[i], logits ? logits[i] : nullptr, false);
+  });
 }
 
 int srs_num_slots(void) { return kSlots; }
@@ -1485,15 +1499,7 @@ int srs_model_status(srs_model* m) {
   if (!m) return fail(SRS_ERR_INVALID, "null model");
   CUDA_TRY(cudaSetDevice(m->device));
   CUDA_TRY(cudaDeviceSynchronize());
-  int flags[kErrWords] = {0};
-  CUDA_TRY(cudaMemcpy(flags, m->err_flag, kErrWords * sizeof(int), cudaMemcpyDeviceToHost));
-  bool any = false;
-  for (int k = 0; k < kErrWords; ++k) any = any || flags[k] != 0;
-  if (any) {
-    CUDA_TRY(cudaMemset(m->err_flag, 0, kErrWords * sizeof(int)));
-    return fail(SRS_ERR_RANGE, "an id in a batch was outside its vocabulary");
-  }
-  return SRS_OK;
+  return read_error_words(m->err_flag, kErrWords);
 }
 
 int64_t srs_model_bytes_per_inference(const srs_model* m) { return m ? m->bytes_per_inf : 0; }
@@ -1550,37 +1556,14 @@ int srs_rank_host(srs_model* m, const srs_batch* b, int32_t k, int32_t* top_idx,
                   float* top_scores) {
   if (!m) return fail(SRS_ERR_INVALID, "null model");
   if (k < 0) return fail(SRS_ERR_INVALID, "negative k");
+  if (b && std::min(k, b->B) > 0 && !top_idx) return fail(SRS_ERR_INVALID, "top_idx is null");
   std::lock_guard<std::mutex> lock(m->mu);
   Slot& s = m->slots[kSlots];
-  int rc = stage_and_launch(m, s, b, false);
+  const int rc = stage_and_launch(m, s, b, false);
   if (rc != SRS_OK) return rc;
   const int n = b->B;
   if (n == 0) return SRS_OK;
-  if (k > n) k = n;
-  if (k > 0 && !top_idx) return fail(SRS_ERR_INVALID, "top_idx is null");
-  rc = ensure_done(s, k);
-  if (rc != SRS_OK) return rc;
-  if (k > 0 && n > s.rank_capacity) {
-    cudaFree(s.d_rank);
-    s.d_rank = nullptr;
-    s.rank_capacity = 0;
-    const int cap = s.capacity;     // >= n after stage_and_launch
-    CUDA_TRY(cudaMalloc(&s.d_rank, (size_t)cap * 8 + topk_scratch_bytes(cap) + 256));
-    s.rank_capacity = cap;
-  }
-  // the ranking kernel writes the k positions / scores into pinned host memory and then the completion
-  // record the caller spins on: no device-to-host copy, no stream synchronise
-  int32_t* r_idx = s.h_res;
-  float* r_top = reinterpret_cast<float*>(s.h_res + s.res_capacity);
-  void* scratch = s.d_rank ? s.d_rank + (size_t)s.rank_capacity * 8 : nullptr;
-  s.seq += 1;
-  CUDA_TRY(launch_topk_done(s.d_probs, n, k, r_idx, r_top, scratch, slot_err(m, s), s.h_done, s.seq, s.stream));
-  rc = wait_done(m, s);
-  if (k > 0) {
-    memcpy(top_idx, r_idx, (size_t)k * 4);
-    if (top_scores) memcpy(top_scores, r_top, (size_t)k * 4);
-  }
-  return rc;
+  return rank_and_wait(m, s, n, std::min(k, n), top_idx, top_scores);
 }
 
 int srs_model_set_movie_features(srs_model* m, int32_t n_movies, const int32_t* genres, const float* numerics) {
@@ -1616,25 +1599,18 @@ int srs_rank_user_host(srs_model* m, const srs_user_row* user, const int32_t* ca
   const int hc = m->hist_cols;
   if (user->n_hist < 0 || user->n_hist > hc || (user->n_hist > 0 && !user->hist))
     return fail(SRS_ERR_INVALID, "n_hist must be in 0..%d", hc);
+  if (std::min(k, n) > 0 && !top_idx) return fail(SRS_ERR_INVALID, "top_idx is null");
   std::lock_guard<std::mutex> lock(m->mu);
   Slot& s = m->slots[kSlots];
   CUDA_TRY(cudaSetDevice(m->device));
   int rc = ensure_slot(m, s, n);
   if (rc != SRS_OK) return rc;
   if (n == 0) return SRS_OK;
-  if (k > n) k = n;
-  if (k > 0 && !top_idx) return fail(SRS_ERR_INVALID, "top_idx is null");
-  if (n > s.req_capacity || !s.d_req) {
-    cudaFree(s.d_req);
-    if (s.h_req) cudaFreeHost(s.h_req);
-    s.d_req = nullptr; s.h_req = nullptr; s.req_capacity = 0;
-    const size_t words = 16 + (size_t)hc + (size_t)s.capacity;
-    CUDA_TRY(cudaMalloc(&s.d_req, words * 4));
-    CUDA_TRY(cudaMallocHost(&s.h_req, words * 4));
-    s.req_capacity = s.capacity;
-  }
+  auto req_bytes = [&](int c) { return (16 + (size_t)hc + (size_t)c) * 4; };
+  CUDA_TRY(s.d_req.grow(n, s.capacity, req_bytes));
+  CUDA_TRY(s.h_req.grow(n, s.capacity, req_bytes));
   // request block: [userId | userGenre1..5 | 3 user numerics | hist[hc] | candidate ids[n]]
-  int32_t* h = s.h_req;
+  int32_t* h = s.h_req.p;
   h[0] = user->user_id;
   for (int g = 0; g < 5; ++g) h[1 + g] = user->user_genre[g] < 0 ? -1 : user->user_genre[g];
   memcpy(h + 6, user->user_numerics, 12);
@@ -1642,64 +1618,30 @@ int srs_rank_user_host(srs_model* m, const srs_user_row* user, const int32_t* ca
   memcpy(h + 9 + hc, cand, (size_t)n * 4);
   // one small copy: (9 + T + n) words instead of n full feature rows.  (Letting the assemble kernel read the
   // pinned block over PCIe itself was measured slower: every row re-reads the user part from host memory.)
-  CUDA_TRY(cudaMemcpyAsync(s.d_req, s.h_req, (9 + (size_t)hc + (size_t)n) * 4, cudaMemcpyHostToDevice, s.stream));
-  rc = ensure_done(s, k);
-  if (rc != SRS_OK) return rc;
+  CUDA_TRY(cudaMemcpyAsync(s.d_req.p, h, (9 + (size_t)hc + (size_t)n) * 4, cudaMemcpyHostToDevice, s.stream));
   const PackedLayout L = packed_layout(m, (size_t)n);
-  uint8_t* d = s.d_block;
-  BatchView v{};
-  v.B = n; v.hist_stride = hc;
-  v.movie_id = reinterpret_cast<const int32_t*>(d + L.movie);
-  v.user_id = reinterpret_cast<const int32_t*>(d + L.user);
-  v.hist = reinterpret_cast<const int32_t*>(d + L.hist);
-  v.movie_genre = reinterpret_cast<const int32_t*>(d + L.mg);
-  v.user_genre = reinterpret_cast<const int32_t*>(d + L.ug);
-  v.numerics = reinterpret_cast<const float*>(d + L.num);
-  v.probs = s.d_probs; v.logits = nullptr; v.err_flag = slot_err(m, s);
-  CUDA_TRY(launch_assemble_request(s.d_req, m->movie_feats, m->movie_feats_rows, n, hc, dense_feats ? 1 : 0,
+  uint8_t* d = s.d_block.p;
+  CUDA_TRY(launch_assemble_request(s.d_req.p, m->movie_feats, m->movie_feats_rows, n, hc, dense_feats ? 1 : 0,
                                    reinterpret_cast<int32_t*>(d + L.movie), reinterpret_cast<int32_t*>(d + L.user),
                                    reinterpret_cast<int32_t*>(d + L.hist), reinterpret_cast<int32_t*>(d + L.mg),
                                    reinterpret_cast<int32_t*>(d + L.ug), reinterpret_cast<float*>(d + L.num),
                                    slot_err(m, s), s.stream));
-  rc = launch(m, v, s.stream);
+  rc = launch(m, staged_view(m, s, (size_t)n, L), s.stream);
   if (rc != SRS_OK) return rc;
-  if (probs) CUDA_TRY(cudaMemcpyAsync(probs, s.d_probs, (size_t)n * 4, cudaMemcpyDeviceToHost, s.stream));
-  if (k > 0 && n > s.rank_capacity) {
-    cudaFree(s.d_rank);
-    s.d_rank = nullptr;
-    s.rank_capacity = 0;
-    const int cap = s.capacity;
-    CUDA_TRY(cudaMalloc(&s.d_rank, (size_t)cap * 8 + topk_scratch_bytes(cap) + 256));
-    s.rank_capacity = cap;
-  }
-  // positions and scores are written into pinned host memory by the ranking kernel itself, followed by the
-  // completion record
-  int32_t* r_idx = s.h_res;
-  float* r_top = reinterpret_cast<float*>(s.h_res + s.res_capacity);
-  void* scratch = s.d_rank ? s.d_rank + (size_t)s.rank_capacity * 8 : nullptr;
-  s.seq += 1;
-  CUDA_TRY(launch_topk_done(s.d_probs, n, k, r_idx, r_top, scratch, slot_err(m, s), s.h_done, s.seq, s.stream));
-  rc = wait_done(m, s);
-  if (k > 0) {
-    memcpy(top_idx, r_idx, (size_t)k * 4);
-    if (top_scores) memcpy(top_scores, r_top, (size_t)k * 4);
-  }
-  return rc;
+  if (probs) CUDA_TRY(cudaMemcpyAsync(probs, s.d_probs.p, (size_t)n * 4, cudaMemcpyDeviceToHost, s.stream));
+  return rank_and_wait(m, s, n, std::min(k, n), top_idx, top_scores);
 }
 
 // ---- evaluate: Keras's loss / accuracy / ROC AUC / PR AUC (metrics.cu) ----------------------------------
 int srs_metrics_create(int32_t device, srs_metrics** out) {
   if (!out) return fail(SRS_ERR_INVALID, "null argument");
   *out = nullptr;
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0)
-    return fail(SRS_ERR_CUDA, "no CUDA device available (%s); this library has no CPU path", cudaGetErrorString(e));
-  if (device < 0 || device >= ndev) return fail(SRS_ERR_INVALID, "device %d out of range", device);
+  const int rc = check_device(device);
+  if (rc != SRS_OK) return rc;
   CUDA_TRY(cudaSetDevice(device));
   srs_metrics* mt = new srs_metrics();
   mt->device = device;
-  e = cudaMalloc(&mt->d, sizeof(MetricsState));
+  cudaError_t e = cudaMalloc(&mt->d, sizeof(MetricsState));
   if (e == cudaSuccess) e = cudaMemset(mt->d, 0, sizeof(MetricsState));
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
@@ -1759,13 +1701,10 @@ int srs_evaluate_host_batches(srs_model* m, int32_t n, const srs_batch* batches,
   if (n < 0 || (n > 0 && (!batches || !labels)) || !out) return fail(SRS_ERR_INVALID, "null argument");
   int rc = check_evaluable(m);
   if (rc != SRS_OK) return rc;
+  rc = check_batches(m, n, batches, labels, "labels");
+  if (rc != SRS_OK) return rc;
   int64_t rows = 0;
-  for (int i = 0; i < n; ++i) {
-    rc = check_batch(m, &batches[i]);
-    if (rc != SRS_OK) return rc;
-    if (batches[i].B > 0 && !labels[i]) return fail(SRS_ERR_INVALID, "labels of batch %d are null", i);
-    rows += batches[i].B;
-  }
+  for (int i = 0; i < n; ++i) rows += batches[i].B;
   if (rows == 0) return fail(SRS_ERR_INVALID, "evaluate needs at least one row");
   std::lock_guard<std::mutex> lock(m->mu);
   CUDA_TRY(cudaSetDevice(m->device));
@@ -1775,42 +1714,27 @@ int srs_evaluate_host_batches(srs_model* m, int32_t n, const srs_batch* batches,
     Slot& s0 = m->slots[0];
     rc = ensure_slot(m, s0, 0);
     if (rc != SRS_OK) return rc;
-    CUDA_TRY(cudaMemsetAsync(m->eval_cnt, 0, sizeof(MetricsCounters), s0.stream));
+    CUDA_TRY(cudaMemsetAsync(m->eval_cnt.p, 0, sizeof(MetricsCounters), s0.stream));
     CUDA_TRY(cudaStreamSynchronize(s0.stream));               // before any slot folds into the counts
   }
-  for (int i = 0; i < n && rc == SRS_OK; ++i) {
-    Slot& s = m->slots[i % kSlots];
-    if (i >= kSlots && s.stream) CUDA_TRY(cudaStreamSynchronize(s.stream));     // slot's previous batch is done
+  rc = run_pipelined(m, n, [&](Slot& s, int i) -> int {
     const srs_batch* b = &batches[i];
-    if (b->B == 0) continue;
-    rc = stage_and_launch(m, s, b, true);
-    if (rc == SRS_OK) rc = ensure_labels(s, b->B);
-    if (rc != SRS_OK) break;
-    CUDA_TRY(cudaMemcpyAsync(s.d_labels, labels[i], (size_t)b->B * sizeof(int32_t), cudaMemcpyHostToDevice,
+    if (b->B == 0) return SRS_OK;
+    int r = stage_and_launch(m, s, b, true);
+    if (r == SRS_OK) r = ensure_labels(s, b->B);
+    if (r != SRS_OK) return r;
+    CUDA_TRY(cudaMemcpyAsync(s.d_labels.p, labels[i], (size_t)b->B * sizeof(int32_t), cudaMemcpyHostToDevice,
                              s.stream));
     // the batch's loss sum goes to its own entry: the batch order, not the slot completion order, fixes the sum
-    CUDA_TRY(launch_metrics_update(s.d_probs, s.d_logits, s.d_labels, b->B, m->eval_cnt, s.d_mred,
-                                   m->eval_loss + i, 0, s.stream));
-  }
-  for (int k = 0; k < kSlots; ++k)
-    if (m->slots[k].stream) {
-      cudaError_t e = cudaStreamSynchronize(m->slots[k].stream);
-      if (e != cudaSuccess && rc == SRS_OK)
-        rc = fail(SRS_ERR_CUDA, "stream synchronize failed: %s", cudaGetErrorString(e));
-    }
+    CUDA_TRY(launch_metrics_update(s.d_probs.p, s.d_logits.p, s.d_labels.p, b->B, m->eval_cnt.p, s.d_mred.p,
+                                   m->eval_loss.p + i, 0, s.stream));
+    return SRS_OK;
+  });
   if (rc != SRS_OK) return rc;
-  int flags[kSlots] = {0};
-  CUDA_TRY(cudaMemcpy(flags, m->err_flag + 1, kSlots * sizeof(int), cudaMemcpyDeviceToHost));
-  bool any = false;
-  for (int k = 0; k < kSlots; ++k) any = any || flags[k] != 0;
-  if (any) {
-    CUDA_TRY(cudaMemset(m->err_flag + 1, 0, kSlots * sizeof(int)));
-    return fail(SRS_ERR_RANGE, "an id in a batch was outside its vocabulary");
-  }
   MetricsCounters c;
   std::vector<double> batch_loss((size_t)n);
-  CUDA_TRY(cudaMemcpy(&c, m->eval_cnt, sizeof(c), cudaMemcpyDeviceToHost));
-  CUDA_TRY(cudaMemcpy(batch_loss.data(), m->eval_loss, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(&c, m->eval_cnt.p, sizeof(c), cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(batch_loss.data(), m->eval_loss.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost));
   if (c.err & kMetErrLabel) return fail(SRS_ERR_INVALID, "a label is not 0 or 1");
   if (c.err & kMetErrProb) return fail(SRS_ERR_INVALID, "a probability is NaN or outside [0, 1]");
   double loss = 0.0;

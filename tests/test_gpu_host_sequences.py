@@ -15,6 +15,7 @@ scores, and a sample of at most 256 rows must match the float64 oracle.
   - `SCRIPT`: every ordered pair of the five synchronous-slot calls on a fresh model, the second call growing the slot;
   - a seeded random walk of 150 calls per model, with one out-of-range id in one row at fixed steps;
   - the error words of the host slots and of the device path do not leak into each other;
+  - srs_rank_host and srs_predict_host_batches reject a bad argument before their first launch;
   - srs_rank_user_host through the raw ABI: history lengths, genres below -1, duplicate candidates, a table upload
     that fails;
   - two threads on one model give the bits of a serial run.
@@ -557,6 +558,42 @@ def test_error_words_stay_with_their_path(rig):
             m.predict_device(m.to_device(good), out)
             _assert_status_clean(rig, m, "device batch after a bad %s call" % ep)
             assert _same_bits(out.cpu().numpy(), rig.ref_scores(good)[0])
+
+
+@pytest.mark.gpu
+def test_rank_host_rejects_a_null_top_idx_before_it_launches(rig):
+    """srs_rank_host with k > 0 and no top_idx fails before it stages the batch, so an out-of-range id in that
+    batch leaves no error word behind for the next call on the private slot."""
+    from sparrowrecsys_b200.model import _host_struct
+    with rig.model() as m:
+        keep = []
+        b = _host_struct(Call(rig, "rank", 600, 5, rig.seed + 80, bad="user").enc, keep)
+        top = np.full(5, np.nan, np.float32)
+        rc, launches = _launches(lambda: rig.lib.srs_rank_host(m._h, C.byref(b), 5, None, top.ctypes.data))
+        assert rc == _lib.SRS_ERR_INVALID, _last_error()
+        assert launches == 0
+        for i, ep in enumerate(("host", "host_pinned", "rank", "rank_user")):
+            Call(rig, ep, 300, 5, rig.seed + 81 + i)(rig, m)
+        _assert_status_clean(rig, m, "after the rejected srs_rank_host")
+
+
+@pytest.mark.gpu
+def test_predict_host_batches_checks_every_batch_before_it_launches(rig):
+    """A srs_predict_host_batches call whose batch 1 has no movie_id fails before batch 0, which holds an
+    out-of-range id, is launched: the next call and srs_model_status are clean."""
+    from sparrowrecsys_b200.model import _host_struct
+    with rig.model() as m:
+        keep = []
+        calls = [Call(rig, "host", 500, 0, rig.seed + 90, bad="user"), Call(rig, "host", 400, 0, rig.seed + 91)]
+        structs = (_lib.SrsBatch * 2)(*[_host_struct(c.enc, keep) for c in calls])
+        structs[1].movie_id = None
+        out = [np.full(c.n, np.nan, np.float32) for c in calls]
+        pp = (C.c_void_p * 2)(*[p.ctypes.data for p in out])
+        rc, launches = _launches(lambda: rig.lib.srs_predict_host_batches(m._h, 2, structs, pp, None))
+        assert rc == _lib.SRS_ERR_INVALID, _last_error()
+        assert launches == 0
+        Call(rig, "batches", 700, 0, rig.seed + 92)(rig, m)
+        _assert_status_clean(rig, m, "after the rejected srs_predict_host_batches")
 
 
 @pytest.mark.gpu
