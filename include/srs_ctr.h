@@ -317,11 +317,57 @@ int srs_metrics_result(srs_metrics* mt, srs_eval_result* out, int64_t* confusion
  * labels [B] int32 go in beside the features and no score comes back.  The loss sums of the batches are
  * added in batch order, so the result does not depend on which slot finishes first.  Synchronous.
  * SRS_ERR_RANGE for an out-of-range id, SRS_ERR_INVALID for a bad label or probability, for no rows,
- * and for the models evaluate does not cover - DIEN (its Keras evaluate loss includes the training-only
- * auxiliary loss) and two towers without the final Dense (its output is a raw dot, not a probability).
- * `out` is written only on success. */
+ * and for the models evaluate does not cover - DIEN (its Keras evaluate reports the loss with the auxiliary
+ * term and its AUC metrics instead: srs_dien_evaluate_host_batches) and two towers without the final Dense
+ * (its output is a raw dot, not a probability).  `out` is written only on success. */
 int srs_evaluate_host_batches(srs_model* m, int32_t n_batches, const srs_batch* batches,
                               const int32_t* const* labels, srs_eval_result* out);
+
+/* ---- DIEN's second output and its Keras evaluate.  The reference's DIEN is a two-output model,
+ * `tf.keras.Model(inputs, outputs=[y_pred, auxiliary_loss_value])` (DIEN.py:296): `model.predict(dataset)`
+ * (:312) returns both arrays and `model.evaluate(dataset)` (:304) reports the `add_loss` value and the
+ * auxiliary layer's AUC metrics.  The second output comes from `auxiliary_loss_layer` (:261-292), which needs
+ * the optional weight group aux_pos_dense/kernel [2E,32], aux_pos_dense/bias [32], aux_pos_out/kernel [32,1],
+ * aux_pos_out/bias [1] and the same four aux_neg_* (all eight or none at srs_model_create); without it, and
+ * for any other model, these calls return SRS_ERR_INVALID.  Per row, with g_t the GRU output and e() a row of
+ * the shared movie embedding (1-based positions t = 1..T-1, no mask):
+ *   aux = sum_t sigmoid(Dense1_pos(sigmoid(Dense32_pos([g_t | e(hist_{t+1})]))))
+ *             + sigmoid(Dense1_neg(sigmoid(Dense32_neg([g_t | e(neg_{t+1})]))))           (:276-285)
+ * and per Keras batch (:287), in float32:
+ *   final_loss_i = bce_i - 0.5 * mean_{j in batch}(aux_j),  bce_i = max(x,0) - x*y + log1p(exp(-|x|))
+ * on the logit x and the 0/1 label y, the batch mean summed in a fixed order.  `neg_hist` holds the ids
+ * negtive_userRatedMovie2..T [B][T-1] in graph order (:83-86,123-128): they pass through float32 like the
+ * history and an id outside the vocabulary gives SRS_ERR_RANGE (read as row 0).  With T = 1 aux is 0 and
+ * neg_hist may be NULL. */
+typedef struct srs_dien_eval_result {
+  int64_t rows, batches;
+  double loss;        /* the Mean of every row's final_loss: sum over all rows / rows                         */
+  double auc;         /* the layer's tf.keras.metrics.AUC() over all (label, y_pred): the roc_auc of evaluate  */
+  double auc_value;   /* add_metric(auc.result(), aggregation="mean"): the mean over batches k of the ROC AUC   */
+                      /* of batches 0..k, so it depends on the batch order; exact counts, AUCs in double       */
+} srs_dien_eval_result;
+
+/* One device batch = one Keras batch, asynchronous on `stream`: probs / logits [B] with the bits of
+ * srs_predict_device, aux [B], and final_loss [B] from labels [B] int32.  Device pointers, all required when
+ * B > 0; neg_hist has neg_stride >= T-1 elements per row.  A label other than 0 / 1 gives a NaN final_loss;
+ * an out-of-range id is reported by srs_model_status. */
+int srs_dien_outputs_device(srs_model* m, const srs_batch* batch, const int32_t* neg_hist, int32_t neg_stride,
+                            const int32_t* labels, float* probs, float* logits, float* aux, float* final_loss,
+                            void* stream);
+
+/* `model.predict(dataset)` of the two-output model (DIEN.py:312) over host batches, pipelined over the slots
+ * as srs_predict_host_batches: batch i (one Keras batch) with neg_hist[i] [B][T-1] and labels[i] [B] int32
+ * gives probs[i] [B] (y_pred) and final_loss[i] [B].  Synchronous.  Labels must be 0 or 1 (SRS_ERR_INVALID,
+ * checked before any launch). */
+int srs_dien_outputs_host_batches(srs_model* m, int32_t n_batches, const srs_batch* batches,
+                                  const int32_t* const* neg_hist, const int32_t* const* labels,
+                                  float* const* probs, float* const* final_loss);
+
+/* `model.evaluate(dataset)` of DIEN (DIEN.py:304) with Keras >= 2.3 semantics, over host batches pipelined as
+ * srs_dien_outputs_host_batches; no score comes back.  Synchronous; `out` is written only on success. */
+int srs_dien_evaluate_host_batches(srs_model* m, int32_t n_batches, const srs_batch* batches,
+                                   const int32_t* const* neg_hist, const int32_t* const* labels,
+                                   srs_dien_eval_result* out);
 
 /* Known-answer self test of the warpgroup-MMA (wgmma) plumbing the tensor-core kernels are built on:
  * D[128][N] = bf16(A[128][K]) * bf16(B[N][K])^T (inputs truncated to bf16, fp32 accumulate),

@@ -43,7 +43,8 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_gather_connect", "srs_gather_destroy", "srs_predict_device_gather", "srs_gather_wait",
            "srs_gather_scores", "srs_gather_copy_scores", "srs_model_set_movie_features", "srs_rank_user_host",
            "srs_selftest_wgmma", "srs_metrics_create", "srs_metrics_destroy", "srs_metrics_reset",
-           "srs_metrics_update_device", "srs_metrics_result", "srs_evaluate_host_batches")
+           "srs_metrics_update_device", "srs_metrics_result", "srs_evaluate_host_batches",
+           "srs_dien_outputs_device", "srs_dien_outputs_host_batches", "srs_dien_evaluate_host_batches")
 
 _lib = None
 
@@ -58,6 +59,12 @@ class SrsEvalResult(C.Structure):
     """`srs_eval_result` (include/srs_ctr.h): what `model.evaluate` reports, with its counts."""
     _fields_ = [("rows", C.c_int64), ("positives", C.c_int64), ("correct", C.c_int64), ("loss", C.c_double),
                 ("accuracy", C.c_double), ("roc_auc", C.c_double), ("pr_auc", C.c_double)]
+
+
+class SrsDienEvalResult(C.Structure):
+    """`srs_dien_eval_result` (include/srs_ctr.h): what DIEN's `model.evaluate` reports (DIEN.py:304)."""
+    _fields_ = [("rows", C.c_int64), ("batches", C.c_int64), ("loss", C.c_double), ("auc", C.c_double),
+                ("auc_value", C.c_double)]
 
 
 class SrsError(RuntimeError):
@@ -169,6 +176,16 @@ def load():
     lib.srs_evaluate_host_batches.restype = C.c_int
     lib.srs_evaluate_host_batches.argtypes = [C.c_void_p, C.c_int32, C.POINTER(SrsBatch), C.POINTER(C.c_void_p),
                                               C.POINTER(SrsEvalResult)]
+    lib.srs_dien_outputs_device.restype = C.c_int
+    lib.srs_dien_outputs_device.argtypes = [C.c_void_p, C.POINTER(SrsBatch), C.c_void_p, C.c_int32, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.srs_dien_outputs_host_batches.restype = C.c_int
+    lib.srs_dien_outputs_host_batches.argtypes = [C.c_void_p, C.c_int32, C.POINTER(SrsBatch), C.POINTER(C.c_void_p),
+                                                  C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                                  C.POINTER(C.c_void_p)]
+    lib.srs_dien_evaluate_host_batches.restype = C.c_int
+    lib.srs_dien_evaluate_host_batches.argtypes = [C.c_void_p, C.c_int32, C.POINTER(SrsBatch), C.POINTER(C.c_void_p),
+                                                   C.POINTER(C.c_void_p), C.POINTER(SrsDienEvalResult)]
     if lib.srs_abi_version() != ABI_VERSION:
         raise ImportError("libsrs_ctr.so ABI version %d != %d" % (lib.srs_abi_version(), ABI_VERSION))
     _lib = lib

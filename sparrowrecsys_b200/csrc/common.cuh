@@ -129,6 +129,14 @@ __device__ __forceinline__ float sigmoidf_acc(float x) {
   return e / (1.f + e);
 }
 
+// Keras's binary_crossentropy of one row of a sigmoid output layer in float32: the logit path
+// max(x, 0) - x*z + log1p(exp(-|x|)) (sigmoid_cross_entropy_with_logits), label z in {0, 1}
+__device__ __forceinline__ float logit_bce(float x, int z) {
+  const float relu = fmaxf(x, 0.f);
+  const float xz = z ? x : 0.f;                    // x * z, z in {0, 1}
+  return __fadd_rn(__fsub_rn(relu, xz), log1pf(expf(-fabsf(x))));
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -15,6 +15,18 @@
 // 15 EP^2 + 45 EP + 68 floats, is staged once per CTA).  GRU step, attention and AUGRU step
 // of position t are fused in one loop, so no [T,E] intermediate exists.  The top MLP is the
 // 32-row tile code DIN uses (common.cuh::dense_layer).
+//
+// The AUX variant (dien_kernel<EP, true>) also computes the second output's per-row term, the auxiliary
+// head of DIEN.py:261-292 (DESIGN.md section 4.7).  For t = 1..T-1 (1-based positions):
+//   pos_t = sigmoid(Dense1_pos(sigmoid(Dense32_pos([g_t | e(h_{t+1})]))))
+//   neg_t = sigmoid(Dense1_neg(sigmoid(Dense32_neg([g_t | e(n_{t+1})]))))
+//   aux   = sum_t (pos_t + neg_t)             no mask: the slices drop it, padded positions count
+// At the kernel's 0-based step t >= 1, h still holds the GRU output of step t-1 while x holds the row of
+// hist[t]: they are g_t and e(h_{t+1}) above, and the negative row e(neg[t-1]) is gathered beside x.  Lane
+// j owns unit j of both Dense32 layers; their weights (aux_pos_* / aux_neg_*, 2 (64 EP + 66) floats: 16.5 KB
+// at EP = 32) are staged after the sequence part.  The plain variant compiles without any of it.
+#include <cmath>
+
 #include "kernels.h"
 
 namespace srs {
@@ -41,7 +53,40 @@ struct DienBlob {                 // float offsets inside DienParams::seq (see m
 };
 
 template <int EP>
-__global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView b) {
+struct DienAuxBlob {              // float offsets inside DienAuxView::w (see model.cu::build_dien)
+  static constexpr int PW = 0;                       // aux_pos_dense/kernel  [2EP k][32]: g_t rows, then e rows
+  static constexpr int NW = PW + 64 * EP;            // aux_neg_dense/kernel  [2EP k][32]
+  static constexpr int PB = NW + 64 * EP;            // aux_pos_dense/bias    [32]
+  static constexpr int NB = PB + 32;                 // aux_neg_dense/bias    [32]
+  static constexpr int PO = NB + 32;                 // aux_pos_out/kernel    [32]
+  static constexpr int NO = PO + 32;                 // aux_neg_out/kernel    [32]
+  static constexpr int POB = NO + 32;                // aux_pos_out/bias      [1]
+  static constexpr int NOB = POB + 1;                // aux_neg_out/bias      [1] (+2 pad)
+  static constexpr int TOTAL = POB + 4;
+};
+
+// pos_t + neg_t of one position: g = g_t, e = e(h_{t+1}), n = e(n_{t+1}), lane k holding element k
+template <int EP>
+__device__ __forceinline__ float dien_aux_step(const float* Sa, float g, float e, float n, int lane) {
+  using A = DienAuxBlob<EP>;
+  float ap = Sa[A::PB + lane], an = Sa[A::NB + lane];
+#pragma unroll
+  for (int k = 0; k < EP; ++k) {
+    const float gk = __shfl_sync(0xffffffffu, g, k);
+    const float ek = __shfl_sync(0xffffffffu, e, k);
+    const float nk = __shfl_sync(0xffffffffu, n, k);
+    ap = fmaf(gk, Sa[A::PW + k * 32 + lane], ap);
+    an = fmaf(gk, Sa[A::NW + k * 32 + lane], an);
+    ap = fmaf(ek, Sa[A::PW + (EP + k) * 32 + lane], ap);
+    an = fmaf(nk, Sa[A::NW + (EP + k) * 32 + lane], an);
+  }
+  const float pos = sigmoidf_acc(warp_sum(sigmoidf_acc(ap) * Sa[A::PO + lane]) + Sa[A::POB]);
+  const float neg = sigmoidf_acc(warp_sum(sigmoidf_acc(an) * Sa[A::NO + lane]) + Sa[A::NOB]);
+  return pos + neg;
+}
+
+template <int EP, bool AUX>
+__global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView b, DienAuxView ax) {
   static_assert(EP <= 32, "one lane per state element");
   using L = DienBlob<EP>;
   constexpr int R = kDienRows;
@@ -57,11 +102,13 @@ __global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView 
   float* H1 = Xs + R * LDX;              // [R][LDH1]
   float* H2 = H1 + R * LDH1;             // [R][LDH2]
   float* Sq = H2 + R * LDH2;             // [L::TOTAL] sequence-part weights
+  float* Sa = Sq + L::TOTAL;             // AUX: [DienAuxBlob<EP>::TOTAL] auxiliary-head weights
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
   const int row0 = blockIdx.x * R;
 
   stage_weights(Sq, p.seq, L::TOTAL);
+  if constexpr (AUX) stage_weights(Sa, ax.w, DienAuxBlob<EP>::TOTAL);
 
   // ---- side features: user genre, user, movie genre rows and numerics ------------
   tile_side_features<EP, R>(Xs, LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users, p.n_genres,
@@ -93,6 +140,7 @@ __global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView 
     float h = 0.f;                                         // GRU state = its output g_t
     float u = Sq[L::H0 + le];                              // AUGRU state
     int hid_next = __ldg(hrow);
+    float aux_row = 0.f;                                   // AUX: sum of pos_t + neg_t
     for (int t = 0; t < p.T; ++t) {
       const int raw = hid_next;
       if (t + 1 < p.T) hid_next = __ldg(hrow + t + 1);
@@ -100,6 +148,15 @@ __global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView 
       const bool valid = hid != 0;                         // Embedding(mask_zero=True) mask
       hid = checked_id(hid, p.n_movies, b.err_flag);
       const float x = lane < EP ? __ldg(p.movie + (size_t)hid * EP + lane) : 0.f;
+      float g_prev = 0.f, xn = 0.f;                        // AUX: g_t and the negative row beside x
+      if constexpr (AUX) {
+        if (t > 0) {
+          g_prev = h;
+          int nid = __float2int_rz(__int2float_rn(__ldg(ax.neg + (size_t)row * ax.neg_stride + t - 1)));
+          nid = checked_id(nid, p.n_movies, b.err_flag);
+          xn = lane < EP ? __ldg(p.movie + (size_t)nid * EP + lane) : 0.f;
+        }
+      }
       // -- GRU step (Keras: z | r | h, reset_after)
       float xz = Sq[L::BX + le], xr = Sq[L::BX + EP + le], xh = Sq[L::BX + 2 * EP + le];
       float rz = Sq[L::BH + le], rr = Sq[L::BH + EP + le], rh = Sq[L::BH + 2 * EP + le];
@@ -120,6 +177,9 @@ __global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView 
         const float hh = tanhf(xh + rg * rh);
         const float hn = z * h + (1.f - z) * hh;
         if (valid) h = hn;                                 // masked step: state and output carried
+      }
+      if constexpr (AUX) {
+        if (t > 0) aux_row += dien_aux_step<EP>(Sa, g_prev, x, xn, lane);
       }
       // -- attention score of position t
       const float pc = h * c;
@@ -160,6 +220,9 @@ __global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView 
       u = (1.f - ra) * u + ra * hn;
     }
     if (lane < EP) { xrow[OFF_C + lane] = c; xrow[OFF_ST + lane] = u; }
+    if constexpr (AUX) {
+      if (lane == 0) ax.aux[row] = aux_row;
+    }
   }
   __syncthreads();
 
@@ -177,9 +240,12 @@ __global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView 
   });
 }
 
-template <int EP>
+// Dynamic shared memory: input tile, two hidden tiles, sequence weights (+ the AUX head's weights).
+// EP = 32: 115 088 B plain, 132 000 B AUX.
+template <int EP, bool AUX>
 static size_t dien_smem() {
-  return (size_t)(kDienRows * ((5 * EP + kNumPad + 4) + 132 + 68) + DienBlob<EP>::TOTAL) *
+  return (size_t)(kDienRows * ((5 * EP + kNumPad + 4) + 132 + 68) + DienBlob<EP>::TOTAL +
+                  (AUX ? DienAuxBlob<EP>::TOTAL : 0)) *
          sizeof(float);
 }
 
@@ -192,10 +258,20 @@ int dien_seq_floats(int EP) {
   return -1;
 }
 
-template <int EP>
-static cudaError_t launch_dien_t(const DienParams& p, const BatchView& b, cudaStream_t s) {
+int dien_aux_floats(int EP) {
+  switch (EP) {
+    case 12: return DienAuxBlob<12>::TOTAL;
+    case 16: return DienAuxBlob<16>::TOTAL;
+    case 32: return DienAuxBlob<32>::TOTAL;
+  }
+  return -1;
+}
+
+template <int EP, bool AUX = false>
+static cudaError_t launch_dien_t(const DienParams& p, const BatchView& b, cudaStream_t s,
+                                 const DienAuxView& a = DienAuxView{}) {
   const int blocks = (b.B + kDienRows - 1) / kDienRows;
-  dien_kernel<EP><<<blocks, kThreads, dien_smem<EP>(), s>>>(p, b);
+  dien_kernel<EP, AUX><<<blocks, kThreads, dien_smem<EP, AUX>(), s>>>(p, b, a);
   ++g_launch_count;
   return cudaGetLastError();
 }
@@ -210,13 +286,68 @@ cudaError_t launch_dien(const DienParams& p, const BatchView& b, cudaStream_t s)
   return cudaErrorInvalidValue;
 }
 
+cudaError_t launch_dien_aux(const DienParams& p, const DienAuxView& a, const BatchView& b, cudaStream_t s) {
+  if (b.B <= 0) return cudaSuccess;
+  switch (p.EP) {
+    case 12: return launch_dien_t<12, true>(p, b, s, a);
+    case 16: return launch_dien_t<16, true>(p, b, s, a);
+    case 32: return launch_dien_t<32, true>(p, b, s, a);
+  }
+  return cudaErrorInvalidValue;
+}
+
+// ---- DIEN.py:287: final_loss = binary_crossentropy(y_true, y_pred) - 0.5 * reduce_mean(aux) ----------
+constexpr int kFinalThreads = 1024;
+
+// a double summed by every thread of the CTA, reduced in a fixed order (the same bits on every run)
+__device__ double cta_sum(double v, double* s_part) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if (lane == 0) s_part[warp] = v;
+  __syncthreads();
+  double t = lane < kFinalThreads / 32 ? s_part[lane] : 0.0;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+  __syncthreads();                                       // s_part may be reused
+  return t;
+}
+
+__global__ void __launch_bounds__(kFinalThreads)
+dien_final_loss_kernel(const float* __restrict__ logits, const int32_t* __restrict__ labels,
+                       const float* __restrict__ aux, int n, float* __restrict__ final_loss, double* sum_dst) {
+  __shared__ double s_part[kFinalThreads / 32];
+  double a = 0.0;
+  for (int i = threadIdx.x; i < n; i += kFinalThreads) a += (double)__ldg(aux + i);
+  const float half_mean = 0.5f * (float)(cta_sum(a, s_part) / (double)n);   // alpha * reduce_mean, float32
+  double f = 0.0;
+  for (int i = threadIdx.x; i < n; i += kFinalThreads) {
+    const int z = __ldg(labels + i);
+    const float v = (z == 0 || z == 1) ? __fsub_rn(logit_bce(__ldg(logits + i), z), half_mean) : NAN;
+    final_loss[i] = v;
+    f += (double)v;
+  }
+  if (!sum_dst) return;
+  f = cta_sum(f, s_part);
+  if (threadIdx.x == 0) *sum_dst = f;
+}
+
+cudaError_t launch_dien_final_loss(const float* logits, const int32_t* labels, const float* aux, int n,
+                                   float* final_loss, double* sum_dst, cudaStream_t s) {
+  if (n <= 0) return cudaSuccess;
+  dien_final_loss_kernel<<<1, kFinalThreads, 0, s>>>(logits, labels, aux, n, final_loss, sum_dst);
+  ++g_launch_count;
+  return cudaGetLastError();
+}
+
 cudaError_t setup_dien_attributes() {
   cudaError_t e;
-#define SRS_ATTR(E_)                                                                     \
-  e = cudaFuncSetAttribute(dien_kernel<E_>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                           (int)dien_smem<E_>());                                        \
+#define SRS_ATTR(E_, AUX_)                                                                     \
+  e = cudaFuncSetAttribute(dien_kernel<E_, AUX_>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                           (int)dien_smem<E_, AUX_>());                                        \
   if (e != cudaSuccess) return e;
-  SRS_ATTR(12) SRS_ATTR(16) SRS_ATTR(32)
+  SRS_ATTR(12, false) SRS_ATTR(16, false) SRS_ATTR(32, false)
+  SRS_ATTR(12, true) SRS_ATTR(16, true) SRS_ATTR(32, true)
 #undef SRS_ATTR
   return cudaSuccess;
 }

@@ -182,6 +182,22 @@ struct DienParams {
   int EP;
 };
 
+// ---- DIEN's auxiliary head (DIEN.py:261-292), the AUX variant of dien_kernel --------------------------
+struct DienAuxView {
+  const float* w;          // aux_pos_* / aux_neg_* weights, layout dien.cu::DienAuxBlob<EP>
+  const int32_t* neg;      // [B][neg_stride] negtive_userRatedMovie2..T in graph order
+  int neg_stride;
+  float* aux;              // [B] out: sum over t of pos_t + neg_t
+};
+int dien_aux_floats(int EP);     // size of DienAuxView::w for a padded width, -1 if unsupported
+// the AUX variant of dien_kernel: probs / logits with the bits of launch_dien, plus aux[B]
+cudaError_t launch_dien_aux(const DienParams& p, const DienAuxView& a, const BatchView& b, cudaStream_t s);
+// final_loss[i] = bce(logits[i], labels[i]) - 0.5 * mean(aux[0..n)) in float32 (DIEN.py:287), the mean summed
+// in double in a fixed order; NaN for a label other than 0 / 1.  sum_dst (or null) gets the double sum of
+// final_loss[0..n) in a fixed order.  One CTA.
+cudaError_t launch_dien_final_loss(const float* logits, const int32_t* labels, const float* aux, int n,
+                                   float* final_loss, double* sum_dst, cudaStream_t s);
+
 // launchers (defined next to their kernels); return cudaGetLastError()
 cudaError_t launch_din_wg(const DinParams& p, const BatchView& b, cudaStream_t s);
 cudaError_t launch_split_table(const float* src, void* dst, int64_t rows, int EP, cudaStream_t s);
@@ -233,11 +249,16 @@ struct MetricsReduce {                     // per stream of updates: the last CT
   unsigned int pad_;
   double partial[kMetMaxCtas];
 };
-// Fold n rows into `cnt`; the rows' loss sum goes to *loss_dst (added to it when `accumulate`).  Launches
-// sharing one `red` must be stream-ordered.
+// Fold n rows into `cnt`; the rows' loss sum goes to *loss_dst (added to it when `accumulate`; not written
+// when loss_dst is null).  `own_hist` (zeroed by the caller, or null): the batch's own 2 x 201 (label, bin)
+// counts are added to it as well.  Launches sharing one `red` must be stream-ordered.
 cudaError_t launch_metrics_update(const float* probs, const float* logits, const int32_t* labels, int n,
                                   MetricsCounters* cnt, MetricsReduce* red, double* loss_dst, int accumulate,
-                                  cudaStream_t s);
+                                  cudaStream_t s, unsigned long long* own_hist = nullptr);
+// DIEN's auc_value: `hist` holds K batch histograms [K][2 x 201] in batch order and is turned into their
+// prefix sums in place; auc[k] (K doubles) = the ROC AUC of batches 0..k in double, *sum_dst = their sum,
+// added in batch order.  Three launches on `s`.
+cudaError_t launch_auc_value(unsigned long long* hist, int K, double* auc, double* sum_dst, cudaStream_t s);
 // host: the counts -> srs_eval_result (AUCs in double); `confusion` NULL or [4][200] tp, fp, tn, fn
 void metrics_summarise(const unsigned long long* hist, unsigned long long correct, double loss_sum,
                        srs_eval_result* out, int64_t* confusion);

@@ -11,6 +11,9 @@
 // Counts are integer atomics (exact, order-free).  The loss is reduced in double in a fixed order inside
 // each CTA; the last CTA (ticket counter) sums the CTA partials in CTA order, so it has the same bits on
 // every run for the same rows.
+//
+// DIEN's evaluate (DESIGN.md section 4.7) also needs each batch's own histogram (`own_hist`) and, from those,
+// auc_value: the mean over batches k of the ROC AUC of batches 0..k (launch_auc_value).
 #include <cmath>
 
 #include "../../include/srs_ctr.h"
@@ -31,17 +34,10 @@ __device__ __forceinline__ float keras_threshold(int j) {
   return (float)((double)j * 1.0 / (double)(kMetThresholds - 1));
 }
 
-// the row's logit-path binary cross-entropy in float32 (sigmoid_cross_entropy_with_logits)
-__device__ __forceinline__ float row_loss(float x, int z) {
-  const float relu = fmaxf(x, 0.f);
-  const float xz = z ? x : 0.f;                    // x * z, z in {0, 1}
-  return __fadd_rn(__fsub_rn(relu, xz), log1pf(expf(-fabsf(x))));
-}
-
 __global__ void __launch_bounds__(kMetThreads)
 metrics_update_kernel(const float* __restrict__ probs, const float* __restrict__ logits,
                       const int32_t* __restrict__ labels, int n, MetricsCounters* cnt, MetricsReduce* red,
-                      double* loss_dst, int accumulate) {
+                      double* loss_dst, int accumulate, unsigned long long* own_hist) {
   __shared__ float s_t[kMetThresholds];
   __shared__ unsigned int s_hist[2 * kMetBins];
   __shared__ double s_loss[kMetThreads / 32];
@@ -74,7 +70,7 @@ metrics_update_kernel(const float* __restrict__ probs, const float* __restrict__
         }
         key = z * kMetBins + lo;
         correct += (unsigned int)((z == 1) == (p > 0.5f));
-        loss += (double)row_loss(__ldg(logits + i), z);
+        loss += (double)logit_bce(__ldg(logits + i), z);
       }
     }
     // scores cluster: one shared atomic per distinct (label, bin) in the warp
@@ -99,6 +95,7 @@ metrics_update_kernel(const float* __restrict__ probs, const float* __restrict__
   for (int j = tid; j < 2 * kMetBins; j += kMetThreads) {
     const unsigned int v = s_hist[j];
     if (v) atomicAdd(&cnt->hist[j], (unsigned long long)v);
+    if (v && own_hist) atomicAdd(&own_hist[j], (unsigned long long)v);
   }
   if (tid == 0) {
     if (s_correct) atomicAdd(&cnt->correct, (unsigned long long)s_correct);
@@ -117,24 +114,75 @@ metrics_update_kernel(const float* __restrict__ probs, const float* __restrict__
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, o);
   if (lane == 0) {
-    *loss_dst = accumulate ? *loss_dst + tot : tot;
+    if (loss_dst) *loss_dst = accumulate ? *loss_dst + tot : tot;
     red->ticket = 0u;                                      // ready for the next launch on this stream
   }
 }
 
-inline double div_no_nan(double a, double b) { return b == 0.0 ? 0.0 : a / b; }
+inline __host__ __device__ double div_no_nan(double a, double b) { return b == 0.0 ? 0.0 : a / b; }
+
+// auc_value of DIEN's evaluate: hist[k] becomes the sum of the batch histograms 0..k (one thread per bin,
+// batches in batch order; integer sums, so exact)
+__global__ void hist_prefix_kernel(unsigned long long* hist, int K) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= 2 * kMetBins) return;
+  unsigned long long c = 0;
+  for (int k = 0; k < K; ++k) {
+    unsigned long long* h = hist + (size_t)k * 2 * kMetBins + j;
+    c += *h;
+    *h = c;
+  }
+}
+
+// auc[k] = the ROC AUC of prefix histogram k, in double: the ROC sum of metrics_summarise, one thread per prefix
+__global__ void prefix_auc_kernel(const unsigned long long* __restrict__ hist, int K, double* __restrict__ auc) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= K) return;
+  const unsigned long long* neg = hist + (size_t)k * 2 * kMetBins;
+  const unsigned long long* pos = neg + kMetBins;
+  unsigned long long P = 0, N = 0;
+  for (int j = 0; j < kMetBins; ++j) { P += pos[j]; N += neg[j]; }
+  unsigned long long above_p = P - pos[0], above_n = N - neg[0];
+  double r0 = div_no_nan((double)above_p, (double)P), f0 = div_no_nan((double)above_n, (double)N);
+  double roc = 0.0;
+  for (int j = 1; j < kMetThresholds; ++j) {
+    above_p -= pos[j]; above_n -= neg[j];
+    const double r1 = div_no_nan((double)above_p, (double)P), f1 = div_no_nan((double)above_n, (double)N);
+    roc += (f0 - f1) * ((r0 + r1) / 2.0);
+    r0 = r1; f0 = f1;
+  }
+  auc[k] = roc;
+}
+
+// *dst = sum of v[0..K) in a fixed order (one warp: strided lane sums, then a fixed butterfly)
+__global__ void ordered_sum_kernel(const double* __restrict__ v, int K, double* dst) {
+  double s = 0.0;
+  for (int k = threadIdx.x; k < K; k += 32) s += v[k];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (threadIdx.x == 0) *dst = s;
+}
 
 }  // namespace
 
 cudaError_t launch_metrics_update(const float* probs, const float* logits, const int32_t* labels, int n,
                                   MetricsCounters* cnt, MetricsReduce* red, double* loss_dst, int accumulate,
-                                  cudaStream_t s) {
+                                  cudaStream_t s, unsigned long long* own_hist) {
   if (n <= 0) return cudaSuccess;
   int64_t blocks = ((int64_t)n + kMetRowsPerCta - 1) / kMetRowsPerCta;
   if (blocks > kMetMaxCtas) blocks = kMetMaxCtas;
   metrics_update_kernel<<<(int)blocks, kMetThreads, 0, s>>>(probs, logits, labels, n, cnt, red, loss_dst,
-                                                            accumulate);
+                                                            accumulate, own_hist);
   ++g_launch_count;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_auc_value(unsigned long long* hist, int K, double* auc, double* sum_dst, cudaStream_t s) {
+  if (K <= 0) return cudaSuccess;
+  hist_prefix_kernel<<<(2 * kMetBins + 127) / 128, 128, 0, s>>>(hist, K);
+  prefix_auc_kernel<<<(K + 127) / 128, 128, 0, s>>>(hist, K, auc);
+  ordered_sum_kernel<<<1, 32, 0, s>>>(auc, K, sum_dst);
+  g_launch_count += 3;
   return cudaGetLastError();
 }
 

@@ -141,6 +141,9 @@ struct Slot {
   PinnedBuffer<int32_t> h_req;      //   and its pinned copy
   Buffer<int32_t> d_labels;         // srs_evaluate_host_batches only (ensure_labels)
   Buffer<MetricsReduce> d_mred;     // the metrics kernel's CTA partials and ticket for this slot's stream
+  Buffer<int32_t> d_neg;            // srs_dien_*_host_batches only (ensure_dien): negative ids [B][T-1],
+  Buffer<float> d_aux;              //   the auxiliary head's per-row sums [B]
+  Buffer<float> d_final;            //   and final_loss [B]
 };
 
 }  // namespace
@@ -160,6 +163,7 @@ struct srs_model {
   DeepFm2Params fm2{};
   DinParams din{};
   DienParams dien{};
+  DienAuxView dien_aux{};            // DIEN's auxiliary-head weights (w == nullptr: built without them)
   bool use_din_wg = false;           // din holds the parameters of din_wg_kernel
   EmbMlpTcParams emb_tc{};
   bool use_emb_tc = false;
@@ -176,6 +180,8 @@ struct srs_model {
   Slot slots[kSlots + 1];
   Buffer<MetricsCounters> eval_cnt;  // srs_evaluate_host_batches (ensure_eval): counts shared by the slots
   Buffer<double> eval_loss;          //   and one loss sum per batch, added in batch order on the host
+  Buffer<unsigned long long> eval_bhist;   // srs_dien_evaluate_host_batches (ensure_dien_eval): each batch's
+  Buffer<double> eval_auc;                 //   own histogram, the prefix AUCs and (last entry) their sum
   std::mutex mu;
 };
 
@@ -627,6 +633,44 @@ int build_din(Builder& B) {
   return B.status;
 }
 
+// ---- DIEN's auxiliary head (DIEN.py:261-292): an optional group of eight tensors, all or none; the blob
+// in the layout of dien.cu::DienAuxBlob<EP> ---------------------------------------------------------------
+const char* const kDienAuxNames[8] = {"aux_pos_dense/kernel", "aux_pos_dense/bias", "aux_pos_out/kernel",
+                                      "aux_pos_out/bias",     "aux_neg_dense/kernel", "aux_neg_dense/bias",
+                                      "aux_neg_out/kernel",   "aux_neg_out/bias"};
+
+int build_dien_aux(Builder& B) {
+  srs_model* m = B.m;
+  const int E = m->spec.emb_dim, EP = m->EP;
+  int present = 0;
+  for (const char* n : kDienAuxNames) present += B.by_name.count(n) ? 1 : 0;
+  if (present == 0) return SRS_OK;
+  const float* w[2][4];
+  for (int side = 0; side < 2; ++side) {
+    w[side][0] = B.host(kDienAuxNames[4 * side + 0], 2 * E, 32);
+    w[side][1] = B.host(kDienAuxNames[4 * side + 1], 32, 1);
+    w[side][2] = B.host(kDienAuxNames[4 * side + 2], 32, 1);
+    w[side][3] = B.host(kDienAuxNames[4 * side + 3], 1, 1);
+  }
+  if (B.status != SRS_OK) return B.status;
+  const int total = dien_aux_floats(EP);
+  if (total < 0) return fail(SRS_ERR_INVALID, "DIEN: unsupported padded width %d", EP);
+  std::vector<float> q((size_t)total, 0.f);
+  const int PW = 0, NW = 64 * EP, PB = 128 * EP, NB = PB + 32, PO = NB + 32, NO = PO + 32, POB = NO + 32;
+  for (int side = 0; side < 2; ++side) {
+    const int W = side ? NW : PW, Bs = side ? NB : PB, O = side ? NO : PO;
+    for (int k = 0; k < E; ++k)                  // concat order: hidden state rows, then embedding rows
+      for (int j = 0; j < 32; ++j) {
+        q[W + (size_t)k * 32 + j] = w[side][0][(size_t)k * 32 + j];
+        q[W + (size_t)(EP + k) * 32 + j] = w[side][0][(size_t)(E + k) * 32 + j];
+      }
+    for (int j = 0; j < 32; ++j) { q[Bs + j] = w[side][1][j]; q[O + j] = w[side][2][j]; }
+    q[POB + side] = w[side][3][0];
+  }
+  m->dien_aux.w = B.upload(q);
+  return B.status;
+}
+
 // ---- DIEN (DIEN.py:154-256): sequence-part blob in the layout of dien.cu::DienBlob<EP> ---------
 int build_dien(Builder& B) {
   srs_model* m = B.m;
@@ -725,7 +769,8 @@ int build_dien(Builder& B) {
   p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres;
   p.T = T; p.EP = EP;
   m->kernel_name = "dien_kernel";
-  return B.status;
+  if (B.status != SRS_OK) return B.status;
+  return build_dien_aux(B);
 }
 
 // ---- tensor-core DIN: shared-memory image ------------------------------------------------
@@ -1031,11 +1076,9 @@ BatchView staged_view(srs_model* m, Slot& s, size_t n, const PackedLayout& L) {
   return v;
 }
 
-// H2D of the batch into the slot's staging and the forward kernel, on the slot's stream;
-// the scores are left in s.d_probs (and s.d_logits).
-// `probs_out`: where the kernel writes the scores (default: the slot's device buffer).
-int stage_and_launch(srs_model* m, Slot& s, const srs_batch* b, bool want_logits,
-                     float* probs_out = nullptr, float* logits_out = nullptr) {
+// H2D of the batch into the slot's staging, on the slot's stream; *v is the view of the staged rows (left
+// as it is for an empty batch), its scores going to s.d_probs.
+int stage(srs_model* m, Slot& s, const srs_batch* b, BatchView* v) {
   int rc = check_batch(m, b);
   if (rc != SRS_OK) return rc;
   CUDA_TRY(cudaSetDevice(m->device));
@@ -1079,12 +1122,22 @@ int stage_and_launch(srs_model* m, Slot& s, const srs_batch* b, bool want_logits
       CUDA_TRY(cudaMemcpyAsync(d + L.num, b->numerics, B * 7 * 4, cudaMemcpyHostToDevice, s.stream));
     }
   }
-  BatchView v = staged_view(m, s, B, L);
+  *v = staged_view(m, s, B, L);
   if (narrow) {
     CUDA_TRY(launch_widen_u16(reinterpret_cast<const uint16_t*>(d + L.hist), s.d_hist32.p,
                               (int64_t)B * m->hist_cols, s.stream));
-    v.hist = s.d_hist32.p;
+    v->hist = s.d_hist32.p;
   }
+  return SRS_OK;
+}
+
+// stage() and the forward kernel, on the slot's stream; the scores are left in s.d_probs (and s.d_logits).
+// `probs_out`: where the kernel writes the scores (default: the slot's device buffer).
+int stage_and_launch(srs_model* m, Slot& s, const srs_batch* b, bool want_logits,
+                     float* probs_out = nullptr, float* logits_out = nullptr) {
+  BatchView v;
+  const int rc = stage(m, s, b, &v);
+  if (rc != SRS_OK || b->B == 0) return rc;
   if (probs_out) v.probs = probs_out;
   if (want_logits) v.logits = logits_out ? logits_out : s.d_logits.p;
   return launch(m, v, s.stream);
@@ -1238,10 +1291,74 @@ int run_pipelined(srs_model* m, int n, Step step) {
 // the model kinds whose output is a probability Keras's evaluate metrics apply to
 int check_evaluable(const srs_model* m) {
   if (m->spec.kind == SRS_DIEN)
-    return fail(SRS_ERR_INVALID, "evaluate does not cover DIEN: its Keras evaluate loss includes the auxiliary "
-                                 "negative-sample loss, which is training-only and not computed here");
+    return fail(SRS_ERR_INVALID, "evaluate does not cover DIEN: its Keras evaluate reports the loss with the "
+                                 "auxiliary negative-sample term and its AUC metrics, not these four numbers; "
+                                 "use srs_dien_evaluate_host_batches");
   if (m->spec.kind == SRS_TWOTOWERS && !m->spec.final_dense)
     return fail(SRS_ERR_INVALID, "evaluate needs a probability: two towers without the final Dense output a raw dot");
+  return SRS_OK;
+}
+
+// srs_dien_*: a DIEN model built with the auxiliary-head group
+int check_dien_aux(const srs_model* m) {
+  if (m->spec.kind != SRS_DIEN)
+    return fail(SRS_ERR_INVALID, "the auxiliary-loss output belongs to DIEN (DIEN.py:261-296); this model is not DIEN");
+  if (!m->dien_aux.w)
+    return fail(SRS_ERR_INVALID, "this DIEN model was built without the auxiliary-head weights "
+                                 "(aux_pos_dense/kernel ... aux_neg_out/bias)");
+  return SRS_OK;
+}
+
+// The negatives and labels of a srs_dien_*_host_batches call, all checked before its first launch; labels must be
+// 0 or 1 (Keras's evaluate asserts the same).
+int check_dien_batches(const srs_model* m, int n, const srs_batch* batches, const int32_t* const* neg_hist,
+                       const int32_t* const* labels) {
+  for (int i = 0; i < n; ++i) {
+    const int B = batches[i].B;
+    if (B == 0) continue;
+    if (!labels[i]) return fail(SRS_ERR_INVALID, "labels of batch %d are null", i);
+    if (m->hist_cols > 1 && !neg_hist[i]) return fail(SRS_ERR_INVALID, "neg_hist of batch %d is null", i);
+    for (int r = 0; r < B; ++r)
+      if (labels[i][r] != 0 && labels[i][r] != 1)
+        return fail(SRS_ERR_INVALID, "a label is not 0 or 1 (batch %d, row %d)", i, r);
+  }
+  return SRS_OK;
+}
+
+// srs_dien_*_host_batches: the slot's staging of negatives and labels and its aux / final_loss outputs
+int ensure_dien(const srs_model* m, Slot& s, int B) {
+  const size_t cols = (size_t)std::max(m->hist_cols - 1, 1);
+  CUDA_TRY(s.d_neg.grow(B, 1024, [&](int c) { return (size_t)c * cols * 4; }));
+  CUDA_TRY(s.d_aux.grow(B, 1024, word_bytes));
+  CUDA_TRY(s.d_final.grow(B, 1024, word_bytes));
+  return ensure_labels(s, B);
+}
+
+// srs_dien_evaluate_host_batches: K batch histograms, K prefix AUCs and their sum
+int ensure_dien_eval(srs_model* m, int K) {
+  CUDA_TRY(m->eval_bhist.grow(K, 64, [](int c) { return (size_t)c * 2 * kMetBins * sizeof(unsigned long long); }));
+  CUDA_TRY(m->eval_auc.grow(K + 1, 65, [](int c) { return (size_t)c * sizeof(double); }));
+  return SRS_OK;
+}
+
+// One Keras batch of a srs_dien_*_host_batches call on slot s: the batch, its negatives and its labels go in; the
+// AUX kernel leaves probs / logits / aux in the slot and the final-loss kernel final_loss in s.d_final (and its
+// sum in *loss_sum when that is not null).
+int dien_stage_and_launch(srs_model* m, Slot& s, const srs_batch* b, const int32_t* neg, const int32_t* labels,
+                          double* loss_sum) {
+  BatchView v;
+  int rc = stage(m, s, b, &v);
+  if (rc == SRS_OK) rc = ensure_dien(m, s, b->B);
+  if (rc != SRS_OK) return rc;
+  const size_t B = (size_t)b->B;
+  const int cols = m->hist_cols - 1;
+  if (cols > 0) CUDA_TRY(cudaMemcpyAsync(s.d_neg.p, neg, B * cols * 4, cudaMemcpyHostToDevice, s.stream));
+  CUDA_TRY(cudaMemcpyAsync(s.d_labels.p, labels, B * 4, cudaMemcpyHostToDevice, s.stream));
+  v.logits = s.d_logits.p;
+  DienAuxView a = m->dien_aux;
+  a.neg = s.d_neg.p; a.neg_stride = cols; a.aux = s.d_aux.p;
+  CUDA_TRY(launch_dien_aux(m->dien, a, v, s.stream));
+  CUDA_TRY(launch_dien_final_loss(s.d_logits.p, s.d_labels.p, s.d_aux.p, (int)B, s.d_final.p, loss_sum, s.stream));
   return SRS_OK;
 }
 
@@ -1741,6 +1858,116 @@ int srs_evaluate_host_batches(srs_model* m, int32_t n, const srs_batch* batches,
   for (int i = 0; i < n; ++i)
     if (batches[i].B > 0) loss += batch_loss[(size_t)i];
   metrics_summarise(c.hist, c.correct, loss, out, nullptr);
+  return SRS_OK;
+}
+
+// ---- DIEN's second output and its Keras evaluate (DIEN.py:261-304) ---------------------------------------
+int srs_dien_outputs_device(srs_model* m, const srs_batch* b, const int32_t* neg_hist, int32_t neg_stride,
+                            const int32_t* labels, float* probs, float* logits, float* aux, float* final_loss,
+                            void* stream) {
+  int rc = check_batch(m, b);
+  if (rc == SRS_OK) rc = check_dien_aux(m);
+  if (rc != SRS_OK) return rc;
+  if (b->B == 0) return SRS_OK;
+  if (!labels || !probs || !logits || !aux || !final_loss)
+    return fail(SRS_ERR_INVALID, "labels, probs, logits, aux and final_loss are required");
+  const int cols = m->hist_cols - 1;
+  if (cols > 0 && (!neg_hist || neg_stride < cols))
+    return fail(SRS_ERR_INVALID, "neg_hist [B][neg_stride >= %d] is required", cols);
+  BatchView v;
+  rc = device_view(m, b, probs, logits, &v);
+  if (rc != SRS_OK) return rc;
+  CUDA_TRY(cudaSetDevice(m->device));
+  DienAuxView a = m->dien_aux;
+  a.neg = neg_hist; a.neg_stride = neg_stride; a.aux = aux;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(launch_dien_aux(m->dien, a, v, st));
+  CUDA_TRY(launch_dien_final_loss(logits, labels, aux, b->B, final_loss, nullptr, st));
+  return SRS_OK;
+}
+
+int srs_dien_outputs_host_batches(srs_model* m, int32_t n, const srs_batch* batches, const int32_t* const* neg_hist,
+                                  const int32_t* const* labels, float* const* probs, float* const* final_loss) {
+  if (!m) return fail(SRS_ERR_INVALID, "null model");
+  if (n < 0 || (n > 0 && (!batches || !labels || !probs || !final_loss || (m->hist_cols > 1 && !neg_hist))))
+    return fail(SRS_ERR_INVALID, "null argument");
+  int rc = check_dien_aux(m);
+  if (rc == SRS_OK) rc = check_batches(m, n, batches, probs, "probs");
+  if (rc == SRS_OK) rc = check_batches(m, n, batches, final_loss, "final_loss");
+  if (rc == SRS_OK) rc = check_dien_batches(m, n, batches, neg_hist, labels);
+  if (rc != SRS_OK) return rc;
+  std::lock_guard<std::mutex> lock(m->mu);
+  CUDA_TRY(cudaSetDevice(m->device));
+  return run_pipelined(m, n, [&](Slot& s, int i) -> int {
+    const srs_batch* b = &batches[i];
+    if (b->B == 0) return SRS_OK;
+    const int r = dien_stage_and_launch(m, s, b, neg_hist ? neg_hist[i] : nullptr, labels[i], nullptr);
+    if (r != SRS_OK) return r;
+    CUDA_TRY(cudaMemcpyAsync(probs[i], s.d_probs.p, (size_t)b->B * 4, cudaMemcpyDeviceToHost, s.stream));
+    CUDA_TRY(cudaMemcpyAsync(final_loss[i], s.d_final.p, (size_t)b->B * 4, cudaMemcpyDeviceToHost, s.stream));
+    return SRS_OK;
+  });
+}
+
+int srs_dien_evaluate_host_batches(srs_model* m, int32_t n, const srs_batch* batches, const int32_t* const* neg_hist,
+                                   const int32_t* const* labels, srs_dien_eval_result* out) {
+  if (!m) return fail(SRS_ERR_INVALID, "null model");
+  if (n < 0 || (n > 0 && (!batches || !labels || (m->hist_cols > 1 && !neg_hist))) || !out)
+    return fail(SRS_ERR_INVALID, "null argument");
+  int rc = check_dien_aux(m);
+  if (rc == SRS_OK) rc = check_batches(m, n, batches, labels, "labels");
+  if (rc == SRS_OK) rc = check_dien_batches(m, n, batches, neg_hist, labels);
+  if (rc != SRS_OK) return rc;
+  int64_t rows = 0;
+  std::vector<int> nth((size_t)n, -1);                  // position of batch i among the batches with rows
+  int K = 0;
+  for (int i = 0; i < n; ++i) {
+    rows += batches[i].B;
+    if (batches[i].B > 0) nth[(size_t)i] = K++;
+  }
+  if (rows == 0) return fail(SRS_ERR_INVALID, "evaluate needs at least one row");
+  std::lock_guard<std::mutex> lock(m->mu);
+  CUDA_TRY(cudaSetDevice(m->device));
+  rc = ensure_eval(m, n);
+  if (rc == SRS_OK) rc = ensure_dien_eval(m, K);
+  if (rc != SRS_OK) return rc;
+  Slot& s0 = m->slots[0];
+  rc = ensure_slot(m, s0, 0);
+  if (rc != SRS_OK) return rc;
+  CUDA_TRY(cudaMemsetAsync(m->eval_cnt.p, 0, sizeof(MetricsCounters), s0.stream));
+  CUDA_TRY(cudaMemsetAsync(m->eval_bhist.p, 0, (size_t)K * 2 * kMetBins * sizeof(unsigned long long), s0.stream));
+  CUDA_TRY(cudaStreamSynchronize(s0.stream));               // before any slot folds into the counts
+  rc = run_pipelined(m, n, [&](Slot& s, int i) -> int {
+    const srs_batch* b = &batches[i];
+    if (b->B == 0) return SRS_OK;
+    // each batch's final_loss sum and histogram go to its own entry: batch order, not slot completion, fixes them
+    const int r = dien_stage_and_launch(m, s, b, neg_hist ? neg_hist[i] : nullptr, labels[i], m->eval_loss.p + i);
+    if (r != SRS_OK) return r;
+    CUDA_TRY(launch_metrics_update(s.d_probs.p, s.d_logits.p, s.d_labels.p, b->B, m->eval_cnt.p, s.d_mred.p, nullptr,
+                                   0, s.stream, m->eval_bhist.p + (size_t)nth[(size_t)i] * 2 * kMetBins));
+    return SRS_OK;
+  });
+  if (rc != SRS_OK) return rc;
+  CUDA_TRY(launch_auc_value(m->eval_bhist.p, K, m->eval_auc.p, m->eval_auc.p + K, s0.stream));
+  CUDA_TRY(cudaStreamSynchronize(s0.stream));
+  MetricsCounters c;
+  std::vector<double> batch_loss((size_t)n);
+  double auc_sum = 0.0;
+  CUDA_TRY(cudaMemcpy(&c, m->eval_cnt.p, sizeof(c), cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(batch_loss.data(), m->eval_loss.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(&auc_sum, m->eval_auc.p + K, sizeof(double), cudaMemcpyDeviceToHost));
+  if (c.err & kMetErrLabel) return fail(SRS_ERR_INVALID, "a label is not 0 or 1");
+  if (c.err & kMetErrProb) return fail(SRS_ERR_INVALID, "a probability is NaN or outside [0, 1]");
+  double loss = 0.0;
+  for (int i = 0; i < n; ++i)
+    if (batches[i].B > 0) loss += batch_loss[(size_t)i];
+  srs_eval_result r{};
+  metrics_summarise(c.hist, c.correct, loss, &r, nullptr);
+  out->rows = rows;
+  out->batches = K;
+  out->loss = r.loss;
+  out->auc = r.roc_auc;
+  out->auc_value = auc_sum / (double)K;
   return SRS_OK;
 }
 

@@ -180,6 +180,49 @@ def encode_batch(spec: ModelSpec, features: Mapping[str, object], arena_alloc=No
     return EncodedBatch(B, movie_id, user_id, hist, movie_genre, user_genre, numerics)
 
 
+def negative_history_keys(T: int):
+    """The DIEN negative-sample inputs `negtive_userRatedMovie2..T` (sic, DIEN.py:83-86), graph order."""
+    return ["negtive_userRatedMovie%d" % k for k in range(2, T + 1)]
+
+
+def negative_history(features: Mapping[str, object], T: int, seed: int, n_movies: int = 1001) -> Dict[str, np.ndarray]:
+    """The negative samples of the reference's `get_dataset_with_negtive_movie` (DIEN.py:30-47), draw for draw:
+    `negtive_userRatedMovie<k>` (int32 [N], k = 2..T) for the feature dict's `userRatedMovie<k>` columns.
+
+    The reference does, on the test file with seed 2021 (:50):
+      1. `tmp_df.fillna(0)` - a missing history id becomes 0 (NaN here);
+      2. `random.seed(seed)` - the module-level Mersenne Twister, seeded from the int;
+      3. `tmp_df.loc[:, 'userRatedMovie2':'userRatedMovie5'].applymap(lambda x: random.sample(
+         set(range(0, 1001)) - set([int(x)]), 1)[0])`.
+    pandas >= 1.1 runs `applymap` as one `map` per column, columns left to right, rows in order, so the draws
+    go column by column.  Python 3.8's `random.sample` turns a set population into `tuple(population)`; a set of
+    small ints iterates in ascending order (each int hashes to itself and the table is larger than 1000), so
+    that tuple is the sorted list used here (Python 3.11+ rejects a set population).  With n = 999 or 1000
+    elements and k = 1, `sample` takes its set-selection branch (n > 21) and returns population[randbelow(n)]
+    on both versions: one `_randbelow` per cell, the same words of the generator.  A fresh `random.Random(seed)`
+    is the state `random.seed(seed)` gives the module generator.
+
+    Caveat: pandas < 1.1 ran `applymap` through `apply`, which called the function on the first column twice
+    (once to infer the result type); under those versions every draw after the first column's is shifted and
+    this does not reproduce them."""
+    import random
+    rng = random.Random(seed)
+    pops: Dict[int, list] = {}
+    out: Dict[str, np.ndarray] = {}
+    for k, key in zip(range(2, T + 1), negative_history_keys(T)):
+        col = np.asarray(_as_1d(features, "userRatedMovie%d" % k), np.float64)
+        col = np.where(np.isnan(col), 0.0, col)                                  # fillna(0)
+        vals = np.empty(col.shape[0], np.int32)
+        for i, x in enumerate(col.tolist()):
+            x = int(x)
+            pop = pops.get(x)
+            if pop is None:
+                pop = pops[x] = sorted(set(range(0, n_movies)) - {x})
+            vals[i] = rng.sample(pop, 1)[0]
+        out[key] = vals
+    return out
+
+
 def synthetic_features(spec: ModelSpec, batch: int, seed: int, *, zipf_a: float = 1.05,
                        missing_genre: float = 0.10, uniform_history: bool = False,
                        pad_history: bool = True) -> Dict[str, np.ndarray]:

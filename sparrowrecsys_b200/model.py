@@ -20,9 +20,9 @@ from typing import Dict, Mapping, Optional
 import numpy as np
 
 from . import _lib
-from .features import EncodedBatch, encode_batch
+from .features import EncodedBatch, _as_ids, encode_batch, negative_history_keys
 from .spec import ModelSpec, default_spec
-from .weights import check_weights, init_weights, weight_shapes
+from .weights import aux_weight_shapes, check_weights, has_aux_weights, init_weights, weight_shapes
 
 
 def _spec_struct(spec: ModelSpec) -> _lib.SrsSpec:
@@ -89,7 +89,9 @@ class CTRModel:
         """`weights`: canonical name -> float32 numpy array (reference shapes), or a
         torch CUDA tensor for an embedding table that is already in HBM (used in
         place, see SRS_DEVICE_BORROWED in include/srs_ctr.h).  `narrow_ids`: host batches
-        carry the history ids as uint16 (`srs_batch::hist16`, n_movies <= 65536).  `options`:
+        carry the history ids as uint16 (`srs_batch::hist16`, n_movies <= 65536).  A DIEN model may also
+        be given the eight auxiliary-head tensors (`weights.aux_weight_shapes`) for `dien_outputs` /
+        `dien_evaluate`.  `options`:
         kernel-variant choices for `srs_model_create_ex`, e.g. {"din_impl": "tc"}."""
         self.spec = spec
         self.narrow_ids = bool(narrow_ids) and spec.n_movies <= 65536
@@ -101,6 +103,9 @@ class CTRModel:
         check_weights(spec, {k: v for k, v in weights.items() if k not in borrowed},
                       skip=tuple(borrowed))
         shapes = dict(weight_shapes(spec))
+        self.has_aux = has_aux_weights(spec, weights)      # DIEN's optional auxiliary-head group
+        if self.has_aux:
+            shapes.update(aux_weight_shapes(spec))
         tensors = (_lib.SrsTensor * len(shapes))()
         self._keep = []
         for i, (name, shape) in enumerate(shapes.items()):
@@ -257,22 +262,7 @@ class CTRModel:
 
     def evaluate_result(self, features, labels=None, batch_size: Optional[int] = None) -> _lib.SrsEvalResult:
         """`evaluate` with the counts: the `srs_eval_result` (rows, positives, correct and the four metrics)."""
-        if labels is None:
-            if "label" not in features:
-                raise KeyError("missing required feature 'label' (or pass labels=)")
-            labels = features["label"]
-        lab = np.asarray(labels)
-        if lab.ndim == 2 and lab.shape[1] == 1:
-            lab = lab[:, 0]
-        if lab.ndim != 1:
-            raise ValueError("labels must be 1-D [N], got shape %s" % (lab.shape,))
-        if lab.dtype.kind == "f" and not np.all(lab == np.trunc(lab)):
-            raise ValueError("labels must be 0 or 1")
-        if lab.dtype.kind not in "biuf":
-            raise ValueError("labels must be numeric 0 or 1")
-        if lab.size and (lab.min() < np.iinfo(np.int32).min or lab.max() > np.iinfo(np.int32).max):
-            raise ValueError("labels must be 0 or 1")
-        lab = np.ascontiguousarray(lab, np.int32)            # the library rejects anything but 0 and 1
+        lab = _label_array(features, labels)
         enc = encode_batch(self.spec, features, narrow_ids=self.narrow_ids)
         n = enc.B
         if lab.shape[0] != n:
@@ -287,6 +277,66 @@ class CTRModel:
         out = _lib.SrsEvalResult()
         _lib.check(self._lib.srs_evaluate_host_batches(self._h, len(bounds), structs, lp, C.byref(out)))
         return out
+
+    # ---- DIEN's second output (DIEN.py:261-296) ---------------------------------------------------
+    def _dien_batches(self, features, batch_size):
+        """The Keras batches of a DIEN two-output call: (encoded batch, negatives, labels) structs and bounds."""
+        lab = _label_array(features, None)
+        if not np.all((lab == 0) | (lab == 1)):
+            raise ValueError("labels must be 0 or 1")
+        enc = encode_batch(self.spec, features, narrow_ids=self.narrow_ids)
+        n = enc.B
+        if lab.shape[0] != n:
+            raise ValueError("labels have %d rows, the features %d" % (lab.shape[0], n))
+        keys = negative_history_keys(self.spec.hist_len)
+        neg = np.empty((n, max(len(keys), 1)), np.int32)
+        for j, k in enumerate(keys):          # numeric_column ids like the history (DIEN.py:123-128), range-checked
+            neg[:, j] = _as_ids(features, k, self.spec.n_movies, "negative movie id")
+        neg = np.ascontiguousarray(neg[:, :len(keys)])
+        step = n if not batch_size else max(int(batch_size), 1)
+        bounds = [(lo, min(n, lo + step)) for lo in range(0, n, step)]
+        keep = [neg, lab]
+        structs = (_lib.SrsBatch * len(bounds))(*[_host_struct(enc.slice(lo, hi), keep) for lo, hi in bounds])
+        negs = [np.ascontiguousarray(neg[lo:hi]) for lo, hi in bounds]
+        keep += negs
+        np_ = (C.c_void_p * len(bounds))(*[a.ctypes.data if a.size else None for a in negs])
+        lp = (C.c_void_p * len(bounds))(*[lab[lo:hi].ctypes.data for lo, hi in bounds])
+        return n, bounds, structs, np_, lp, keep
+
+    def dien_outputs(self, features, batch_size: Optional[int] = None):
+        """`model.predict(x)` of the reference's two-output DIEN (DIEN.py:296,312): `[y_pred float32 [N,1],
+        final_loss float32 [N]]`.  `features` also carries `negtive_userRatedMovie2..T` (e.g. from
+        `features.negative_history`) and `label` (0 or 1); a missing one raises KeyError, as Keras does for a
+        missing input.  final_loss_i = bce_i - 0.5 * mean_j aux_j over the Keras batch of row i (DIEN.py:287),
+        so it depends on `batch_size` (None: one batch).  y_pred has the bits of `predict`.  Needs the
+        auxiliary-head weights (ValueError otherwise)."""
+        n, bounds, structs, negs, lp, keep = self._dien_batches(features, batch_size)
+        probs = np.empty(n, np.float32)
+        final = np.empty(n, np.float32)
+        pp = (C.c_void_p * len(bounds))(*[probs[lo:hi].ctypes.data for lo, hi in bounds])
+        fp = (C.c_void_p * len(bounds))(*[final[lo:hi].ctypes.data for lo, hi in bounds])
+        _lib.check(self._lib.srs_dien_outputs_host_batches(self._h, len(bounds), structs, negs, lp, pp, fp))
+        return [probs.reshape(n, 1), final]
+
+    def dien_evaluate(self, features, batch_size: Optional[int] = None) -> dict:
+        """`model.evaluate(x, return_dict=True)` of the reference's DIEN (DIEN.py:298-304): {"loss", "auc",
+        "auc_value"}, with Keras >= 2.3 semantics - the model is compiled without a loss or metrics, so Keras
+        reports the `add_loss` value and the layer's own metrics:
+          loss       the compile-less loss Mean over every element of each batch's final_loss: the sum over all
+                     rows / N;
+          auc        the layer's `tf.keras.metrics.AUC()` over all (label, y_pred) (200 thresholds, exact counts;
+                     the roc_auc of `evaluate`);
+          auc_value  `add_metric(self.auc.result(), aggregation="mean")`: the mean over batches k of the AUC of
+                     batches 0..k, so it depends on the batch order.
+        Keras >= 2.3 because DIEN.py:41-42 drops the last partial batch only for TF < 2.3, whose loss is aggregated
+        per batch position; this keeps every row.  Batches of `batch_size` rows (None: one batch).  Inputs and
+        errors as `dien_outputs`."""
+        n, bounds, structs, negs, lp, keep = self._dien_batches(features, batch_size)
+        if n == 0:
+            raise ValueError("evaluate needs at least one row")
+        out = _lib.SrsDienEvalResult()
+        _lib.check(self._lib.srs_dien_evaluate_host_batches(self._h, len(bounds), structs, negs, lp, C.byref(out)))
+        return {"loss": out.loss, "auc": out.auc, "auc_value": out.auc_value}
 
     # ---- one user x n candidates, movie features resident in HBM ----------------------------
     def set_movie_table(self, table):
@@ -429,6 +479,26 @@ class Metrics:
         r = {k: getattr(out, k) for k, _ in _lib.SrsEvalResult._fields_}
         r.update(tp=conf[0], fp=conf[1], tn=conf[2], fn=conf[3])
         return r
+
+
+def _label_array(features, labels=None) -> np.ndarray:
+    """`labels` (default: `features["label"]`, KeyError if missing) as int32 [N]; ValueError unless integral."""
+    if labels is None:
+        if "label" not in features:
+            raise KeyError("missing required feature 'label' (or pass labels=)")
+        labels = features["label"]
+    lab = np.asarray(labels)
+    if lab.ndim == 2 and lab.shape[1] == 1:
+        lab = lab[:, 0]
+    if lab.ndim != 1:
+        raise ValueError("labels must be 1-D [N], got shape %s" % (lab.shape,))
+    if lab.dtype.kind == "f" and not np.all(lab == np.trunc(lab)):
+        raise ValueError("labels must be 0 or 1")
+    if lab.dtype.kind not in "biuf":
+        raise ValueError("labels must be numeric 0 or 1")
+    if lab.size and (lab.min() < np.iinfo(np.int32).min or lab.max() > np.iinfo(np.int32).max):
+        raise ValueError("labels must be 0 or 1")
+    return np.ascontiguousarray(lab, np.int32)            # the library rejects anything but 0 and 1
 
 
 def launch_count() -> int:

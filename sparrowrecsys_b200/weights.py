@@ -216,6 +216,30 @@ def init_weights(spec: ModelSpec, seed: int = 0, *, for_test: bool = True,
     return W
 
 
+def aux_weight_shapes(spec: ModelSpec) -> List[Tuple[str, Tuple[int, ...]]]:
+    """DIEN's optional auxiliary-head group (`auxiliary_loss_layer`, DIEN.py:261-270): two Dense(32, sigmoid)
+    over [g_t | e] and two Dense(1, sigmoid), for the positive and the negative next item.  A DIEN model takes
+    all eight or none; without them it serves `y_pred` only.  Kept apart from `weight_shapes` so that the
+    model's base inventory - and the seeded draws of `init_weights` - stay what they are."""
+    if spec.model != "dien":
+        raise ValueError("the auxiliary-head weights belong to DIEN, not %r" % spec.model)
+    E = spec.emb_dim
+    out: List[Tuple[str, Tuple[int, ...]]] = []
+    for side in ("pos", "neg"):                 # DIEN.py:265-268
+        out += [("aux_%s_dense/kernel" % side, (2 * E, 32)), ("aux_%s_dense/bias" % side, (32,)),
+                ("aux_%s_out/kernel" % side, (32, 1)), ("aux_%s_out/bias" % side, (1,))]
+    return out
+
+
+def init_aux_weights(spec: ModelSpec, seed: int = 0) -> Dict[str, np.ndarray]:
+    """Seeded auxiliary-head weights with Keras's Dense defaults: glorot_uniform kernels, zero biases.  The draws
+    come from their own generator, so adding the group leaves `init_weights(spec, seed)` unchanged."""
+    rng = np.random.default_rng(seed)
+    return {name: (_glorot(rng, shape[0], shape[1], shape) if name.endswith("/kernel")
+                   else np.zeros(shape, np.float32))
+            for name, shape in aux_weight_shapes(spec)}
+
+
 def check_weights(spec: ModelSpec, W: Dict[str, np.ndarray], skip: Tuple[str, ...] = ()) -> None:
     for name, shape in weight_shapes(spec):
         if name in skip:
@@ -227,3 +251,23 @@ def check_weights(spec: ModelSpec, W: Dict[str, np.ndarray], skip: Tuple[str, ..
                              % (name, tuple(W[name].shape), shape))
         if W[name].dtype != np.float32:
             raise ValueError("weight %r must be float32" % name)
+
+
+def has_aux_weights(spec: ModelSpec, W) -> bool:
+    """True when `W` carries DIEN's auxiliary-head group (checked: all eight tensors with their shapes, float32),
+    False when it carries none of it; KeyError / ValueError for a partial or malformed group."""
+    if spec.model != "dien":
+        return False
+    shapes = aux_weight_shapes(spec)
+    present = [n for n, _ in shapes if n in W]
+    if not present:
+        return False
+    for name, shape in shapes:
+        if name not in W:
+            raise KeyError("missing weight tensor %r: the auxiliary-head group is all eight tensors or none" % name)
+        a = W[name]
+        if tuple(a.shape) != shape:
+            raise ValueError("weight %r has shape %s, expected %s" % (name, tuple(a.shape), shape))
+        if not isinstance(a, np.ndarray) or a.dtype != np.float32:
+            raise ValueError("weight %r must be a float32 host array" % name)
+    return True
