@@ -369,6 +369,49 @@ int srs_dien_evaluate_host_batches(srs_model* m, int32_t n_batches, const srs_ba
                                    const int32_t* const* neg_hist, const int32_t* const* labels,
                                    srs_dien_eval_result* out);
 
+/* ---- `model.fit` of NeuralCF (neural_cf_model_1): NeuralCF.py:74-91 compiles with loss='binary_crossentropy',
+ * optimizer='adam' and calls `fit(train_dataset, epochs=5)` over make_csv_dataset batches of 12.  A trainer owns
+ * fp32 weights and Adam's slots on one device; it never touches an srs_model: a serving model is built from the
+ * weights srs_trainer_get_weights exports.  Per step of B_b rows (DESIGN.md section 4.8):
+ *   loss      the mean over the batch of max(z,0) - z*y + log1p(exp(-|z|)), so dL/dz_i = (sigmoid(z_i) - y_i) / B_b;
+ *   gradient  through the Dense layers (relu' = [a > 0]) into both embedding rows of each row; an id that occurs
+ *             several times in the batch gets the sum of its rows' gradients (TF's _deduplicate_indexed_slices);
+ *   Adam      Keras's, t = iterations + 1, alpha = lr * sqrt(1 - beta_2^t) / (1 - beta_1^t) in float32.  Dense
+ *             kernels and biases: m += (g - m)(1 - beta_1), v += (g^2 - v)(1 - beta_2) (TF's ApplyAdam).  The two
+ *             embedding tables (IndexedSlices gradients, _resource_apply_sparse): m and v of EVERY row decay,
+ *             m = beta_1 m + (1 - beta_1) G, v = beta_2 v + (1 - beta_2) G^2 with G = 0 off the batch, and every
+ *             row is updated - not "lazy Adam".  All: w -= alpha m / (sqrt(v) + epsilon).
+ * Every sum has a fixed order: the same weights, data and order give the same bits.
+ * Supported: emb_dim 1..64, 1..3 hidden layers of width 1..32, any batch size >= 1. */
+typedef struct srs_adam {
+  float lr, beta_1, beta_2, epsilon;   /* Keras's defaults: 0.001, 0.9, 0.999, 1e-7 */
+} srs_adam;
+typedef struct srs_trainer srs_trainer;
+
+/* `tensors`: the initial weights in Keras shapes (host, the names and shapes srs_model_create takes for
+ * SRS_NEURALCF); `hp` NULL = Keras's defaults.  A model kind other than SRS_NEURALCF, an unsupported shape or bad
+ * hyper-parameters give SRS_ERR_INVALID. */
+int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
+                       const srs_adam* hp, srs_trainer** out);
+void srs_trainer_destroy(srs_trainer* tr);
+
+/* `epochs` epochs over the n = batch->B rows of `batch` (movie_id, user_id; host) with labels [n] int32: epoch e
+ * takes the rows order[e * n + 0 .. n) (each a permutation of 0..n-1) in batches of `batch_size`, the last one
+ * partial.  The dataset is uploaded once and the steps run on the device with no host synchronisation between
+ * them.  history (NULL or [epochs]) receives each epoch's loss (mean over its rows), accuracy and ROC / PR AUC, as
+ * srs_eval_result, each computed on the step's outputs before that step's update (Keras >= 2.2 `fit` logs).
+ * Synchronous.  A label other than 0 / 1 or an order row that is not a permutation gives SRS_ERR_INVALID, an id
+ * outside the vocabulary SRS_ERR_RANGE; all of them are checked before any launch, so a rejected call leaves the
+ * trainer as it was. */
+int srs_trainer_fit_host(srs_trainer* tr, const srs_batch* batch, const int32_t* labels, const int32_t* order,
+                         int32_t batch_size, int32_t epochs, srs_eval_result* history);
+
+/* Copy one trained tensor, in its Keras shape, to host memory `dst` (SRS_ERR_MISSING for an unknown name). */
+int srs_trainer_get_weights(const srs_trainer* tr, const char* name, float* dst);
+
+/* Adam steps taken so far (Keras's optimizer.iterations). */
+int64_t srs_trainer_iterations(const srs_trainer* tr);
+
 /* Known-answer self test of the warpgroup-MMA (wgmma) plumbing the tensor-core kernels are built on:
  * D[128][N] = bf16(A[128][K]) * bf16(B[N][K])^T (inputs truncated to bf16, fp32 accumulate),
  * K = 64 * k_blocks (1..4), N = 16 or 32, A read from shared memory (a_in_regs = 0) or from

@@ -44,7 +44,9 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_gather_scores", "srs_gather_copy_scores", "srs_model_set_movie_features", "srs_rank_user_host",
            "srs_selftest_wgmma", "srs_metrics_create", "srs_metrics_destroy", "srs_metrics_reset",
            "srs_metrics_update_device", "srs_metrics_result", "srs_evaluate_host_batches",
-           "srs_dien_outputs_device", "srs_dien_outputs_host_batches", "srs_dien_evaluate_host_batches")
+           "srs_dien_outputs_device", "srs_dien_outputs_host_batches", "srs_dien_evaluate_host_batches",
+           "srs_trainer_create", "srs_trainer_destroy", "srs_trainer_fit_host", "srs_trainer_get_weights",
+           "srs_trainer_iterations")
 
 _lib = None
 
@@ -65,6 +67,11 @@ class SrsDienEvalResult(C.Structure):
     """`srs_dien_eval_result` (include/srs_ctr.h): what DIEN's `model.evaluate` reports (DIEN.py:304)."""
     _fields_ = [("rows", C.c_int64), ("batches", C.c_int64), ("loss", C.c_double), ("auc", C.c_double),
                 ("auc_value", C.c_double)]
+
+
+class SrsAdam(C.Structure):
+    """`srs_adam` (include/srs_ctr.h): Keras Adam's hyper-parameters."""
+    _fields_ = [("lr", C.c_float), ("beta_1", C.c_float), ("beta_2", C.c_float), ("epsilon", C.c_float)]
 
 
 class SrsError(RuntimeError):
@@ -186,6 +193,18 @@ def load():
     lib.srs_dien_evaluate_host_batches.restype = C.c_int
     lib.srs_dien_evaluate_host_batches.argtypes = [C.c_void_p, C.c_int32, C.POINTER(SrsBatch), C.POINTER(C.c_void_p),
                                                    C.POINTER(C.c_void_p), C.POINTER(SrsDienEvalResult)]
+    lib.srs_trainer_create.restype = C.c_int
+    lib.srs_trainer_create.argtypes = [C.POINTER(SrsSpec), C.POINTER(SrsTensor), C.c_int32, C.c_int32,
+                                       C.POINTER(SrsAdam), C.POINTER(C.c_void_p)]
+    lib.srs_trainer_destroy.restype = None
+    lib.srs_trainer_destroy.argtypes = [C.c_void_p]
+    lib.srs_trainer_fit_host.restype = C.c_int
+    lib.srs_trainer_fit_host.argtypes = [C.c_void_p, C.POINTER(SrsBatch), C.c_void_p, C.c_void_p, C.c_int32,
+                                         C.c_int32, C.POINTER(SrsEvalResult)]
+    lib.srs_trainer_get_weights.restype = C.c_int
+    lib.srs_trainer_get_weights.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
+    lib.srs_trainer_iterations.restype = C.c_int64
+    lib.srs_trainer_iterations.argtypes = [C.c_void_p]
     if lib.srs_abi_version() != ABI_VERSION:
         raise ImportError("libsrs_ctr.so ABI version %d != %d" % (lib.srs_abi_version(), ABI_VERSION))
     _lib = lib

@@ -265,4 +265,7 @@ void metrics_summarise(const unsigned long long* hist, unsigned long long correc
 
 extern int64_t g_launch_count;   // kernels launched by this library
 
+// model.cu: set the message srs_last_error() reports on this thread; returns `code`
+int set_last_error(int code, const char* msg);
+
 }  // namespace srs

@@ -200,6 +200,11 @@ namespace {
 inline int* slot_err(srs_model* m, const Slot& s) { return m->err_flag + 1 + (&s - m->slots); }
 }  // namespace
 
+int srs::set_last_error(int code, const char* msg) {
+  g_err = msg;
+  return code;
+}
+
 
 namespace {
 

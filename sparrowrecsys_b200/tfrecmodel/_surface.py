@@ -23,6 +23,7 @@ class Surface:
     def __init__(self, name: str):
         self.name = name
         self.model: Optional[CTRModel] = None
+        self.weights = None       # the host weights `model` was built from (None: a shipped export of another model)
 
     def spec(self, **overrides) -> ModelSpec:
         """The reference script's own constants unless overridden."""
@@ -34,8 +35,14 @@ class Surface:
         if self.model is not None:
             self.model.close()
             self.model = None
+        self.weights = None
         if savedmodel is not None:
-            self.model = CTRModel.from_savedmodel(savedmodel, self.name, device)
+            if self.name == "neuralcf":                 # kept on the host, so that fit() can start from them
+                from ..bundle import load_neuralcf
+                self.weights = load_neuralcf(savedmodel)
+                self.model = CTRModel(default_spec("neuralcf"), self.weights, device)
+            else:
+                self.model = CTRModel.from_savedmodel(savedmodel, self.name, device)
             return self.model
         spec = spec or self.spec()
         if spec.model != self.name:
@@ -44,6 +51,7 @@ class Surface:
             # untrained model: the reference's initialisers (what `model` holds before fit)
             weights = init_weights(spec, 0 if seed is None else seed, for_test=False)
         self.model = CTRModel(spec, weights, device)
+        self.weights = weights
         return self.model
 
     def predict(self, features, batch_size: Optional[int] = None) -> np.ndarray:
@@ -56,3 +64,21 @@ class Surface:
         if self.model is None:
             raise RuntimeError("tfrecmodel.%s: call load() before evaluate()" % self.name)
         return self.model.evaluate(features, batch_size=batch_size)
+
+    def fit(self, features, epochs: int = 5, batch_size: int = 12, seed: int = 0) -> dict:
+        """`model.fit(train_dataset, epochs=5)` (NeuralCF.py:91): train from the weights `model` was loaded with,
+        then rebuild `model` from the trained weights.  Returns Keras's history dict.  NeuralCF only."""
+        if self.name != "neuralcf":
+            raise NotImplementedError("tfrecmodel.%s: fit is implemented for NeuralCF (tfrecmodel.neuralcf) only"
+                                      % self.name)
+        if self.model is None or self.weights is None:
+            raise RuntimeError("tfrecmodel.%s: call load() before fit()" % self.name)
+        from ..training import Trainer
+        spec, device = self.model.spec, self.model.device
+        with Trainer(spec, self.weights, device) as tr:
+            history = tr.fit(features, epochs=epochs, batch_size=batch_size, seed=seed)
+            trained = tr.weights()
+        self.model.close()
+        self.model = CTRModel(spec, trained, device)
+        self.weights = trained
+        return history

@@ -25,3 +25,8 @@ def predict(features, batch_size=None):
 
 def evaluate(features, batch_size=None):
     return _surface.evaluate(features, batch_size)
+
+
+def fit(features, epochs=5, batch_size=12, seed=0):
+    """Not implemented for this model: `fit` covers NeuralCF (tfrecmodel.neuralcf) only."""
+    return _surface.fit(features, epochs, batch_size, seed)

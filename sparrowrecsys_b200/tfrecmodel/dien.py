@@ -56,3 +56,8 @@ def evaluate(features, batch_size=None):
     raise NotImplementedError("tfrecmodel.dien.evaluate: DIEN's Keras evaluate reports the loss with the auxiliary "
                               "negative-sample term and its AUC metrics, not the four compile metrics; use "
                               "tfrecmodel.dien.evaluate_outputs (CTRModel.dien_evaluate)")
+
+
+def fit(features, epochs=5, batch_size=12, seed=0):
+    """Not implemented for this model: `fit` covers NeuralCF (tfrecmodel.neuralcf) only."""
+    return _surface.fit(features, epochs, batch_size, seed)

@@ -5,6 +5,7 @@
     neuralcf.load(weights)            # or load(savedmodel=...), load(spec=..., seed=...)
     p = neuralcf.predict(features)    # dict of 1-D columns -> float32 [N,1]
     loss, acc, roc_auc, pr_auc = neuralcf.evaluate(test_features)   # rows labelled by "label"
+    history = neuralcf.fit(train_features, epochs=5)   # NeuralCF.py:91; rebuilds `model` from the result
 """
 from ._surface import Surface
 
@@ -25,3 +26,12 @@ def predict(features, batch_size=None):
 
 def evaluate(features, batch_size=None):
     return _surface.evaluate(features, batch_size)
+
+
+def fit(features, epochs=5, batch_size=12, seed=0):
+    """`model.fit(train_dataset, epochs=5)`: train from the loaded weights on the GPU, then rebuild `model` from the
+    trained weights; returns Keras's history dict {"loss", "accuracy", "auc", "auc_1"} (one value per epoch)."""
+    global model
+    history = _surface.fit(features, epochs, batch_size, seed)
+    model = _surface.model
+    return history
