@@ -8,109 +8,20 @@
 // both kernels evaluate the first-order term.  Everything else per 64-row tile:
 // row gathers straight into shared memory, FM interaction on the tile, the deep MLP
 // with register-tiled FFMA, one score per row out.
-#include "kernels.h"
+#include "deepfm_layers.cuh"
 
 namespace srs {
 
 constexpr int kFmRows = 64;      // DeepFM_v2 tile
-constexpr int kFm1Rows = 32;     // DeepFM tile: 4096 rows -> 128 CTAs
-
-__device__ __forceinline__ int genre_id(const int32_t* col, int row, int stride, int n_genres,
-                                        int* err_flag) {
-  int id = __ldg(col + row * stride);
-  if (id >= n_genres) { atomicExch(err_flag, 1); id = -1; }
-  return id < 0 ? -1 : id;
-}
 
 // ------------------------------------------------------------------------------------
-// DeepFM (v1)
+// DeepFM (v1): the tile forward of deepfm_layers.cuh
 // ------------------------------------------------------------------------------------
 template <int EP>
 __global__ void __launch_bounds__(kThreads) deepfm_kernel(DeepFmParams p, BatchView b) {
-  constexpr int R = kFm1Rows;
-  constexpr int Q = EP / 4;
-  constexpr int KP = 2 * EP + kNumPad;
-  constexpr int LDX = KP + 4;
-  constexpr int LDF = 4 * EP + 4;
-  constexpr int LDH = 64 + 4;
-  extern __shared__ __align__(16) float smem[];
-  float* Xs = smem;                    // [R][LDX]  deep input: deep_item | deep_user | numerics
-  float* Fs = Xs + R * LDX;            // [R][LDF]  fm rows: item | user | item_genre | user_genre
-  float* H1 = Fs + R * LDF;            // [R][LDH]
-  float* H2 = H1 + R * LDH;            // [R][LDH]
-  float* Ds = H2 + R * LDH;            // [R][4]    the four FM dots
-  float* W1s = Ds + R * 4;             // [KP][64] staged deep kernels
-  float* W2s = W1s + KP * 64;          // [64][64]
-  const int tid = threadIdx.x;
-  const int row0 = blockIdx.x * R;
-  stage_weights(W1s, p.W1, KP * 64);
-  stage_weights(W2s, p.W2, 64 * 64);
-
-  for (int i = tid; i < R * 6 * Q; i += kThreads) {
-    const int q = i % Q;
-    const int t = i / Q;
-    const int slot = t % 6;
-    const int r = t / 6;
-    const int row = row0 + r;
-    int id = -1;
-    const float* table = p.fm_movie;
-    float* dst = Fs + r * LDF;
-    if (row < b.B) {
-      const int mid = checked_id(__ldg(b.movie_id + row), p.n_movies, b.err_flag);
-      const int uid = checked_id(__ldg(b.user_id + row), p.n_users, b.err_flag);
-      switch (slot) {
-        case 0: id = mid; table = p.fm_movie; break;
-        case 1: id = uid; table = p.fm_user; break;
-        case 2: id = genre_id(b.movie_genre, row, 3, p.n_genres, b.err_flag); table = p.fm_mgenre; break;
-        case 3: id = genre_id(b.user_genre, row, 5, p.n_genres, b.err_flag); table = p.fm_ugenre; break;
-        case 4: id = mid; table = p.deep_movie; break;
-        default: id = uid; table = p.deep_user; break;
-      }
-    }
-    if (slot < 4) dst = Fs + r * LDF + slot * EP;
-    else dst = Xs + r * LDX + (slot - 4) * EP;
-    gather_row<EP>(dst, table, id, q);
-  }
-  for (int i = tid; i < R * kNumPad; i += kThreads) {
-    const int r = i / kNumPad, j = i % kNumPad;
-    const int row = row0 + r;
-    float v = 0.f;
-    if (j < kNumNumerics && row < b.B) v = __ldg(b.numerics + row * kNumNumerics + j);
-    Xs[r * LDX + 2 * EP + j] = v;
-  }
-  stage_wait();
-  __syncthreads();
-  if (tid < R * 4) {  // four dots per row (DeepFM.py:100-103): <item,user> <ig,ug> <ig,user> <item,ug>
-    const int r = tid >> 2, d = tid & 3;
-    const float* f = Fs + r * LDF;
-    const float* a = (d == 0 || d == 3) ? f : f + 2 * EP;            // item or item_genre
-    const float* c = (d == 0 || d == 2) ? f + EP : f + 3 * EP;       // user or user_genre
-    float s = 0.f;
-#pragma unroll
-    for (int k = 0; k < EP; ++k) s = fmaf(a[k], c[k], s);
-    Ds[r * 4 + d] = s;
-  }
-  dense_layer<R, 64, 1, 8, true>(Xs, LDX, KP, W1s, p.b1, ACT_RELU, nullptr, H1, LDH);
-  __syncthreads();
-  dense_layer<R, 64, 1, 8, true>(H1, LDH, 64, W2s, p.b2, ACT_RELU, nullptr, H2, LDH);
-  __syncthreads();
-  row_dot<R>(H2, LDH, 64, p.wdeep, [&](int r, float s) {
-    const int row = row0 + r;
-    if (row >= b.B) return;
-    const int G = p.n_genres;
-    const int mid = checked_id(__ldg(b.movie_id + row), p.n_movies, b.err_flag);
-    const int uid = checked_id(__ldg(b.user_id + row), p.n_users, b.err_flag);
-    const int ig = genre_id(b.movie_genre, row, 3, G, b.err_flag);
-    const int ug = genre_id(b.user_genre, row, 5, G, b.err_flag);
-    // one-hot block order (sorted column names): movieGenre1 | movieId | userGenre1 | userId
-    float z = 0.f;
-    if (ig >= 0) z += __ldg(p.first + ig);
-    z += __ldg(p.first + G + mid);
-    if (ug >= 0) z += __ldg(p.first + G + p.n_movies + ug);
-    z += __ldg(p.first + (size_t)(2 * G + p.n_movies) + uid);
-#pragma unroll
-    for (int d = 0; d < 4; ++d) z = fmaf(Ds[r * 4 + d], p.wdot[d], z);
-    z += s + p.bout;
+  const int row0 = blockIdx.x * kFm1Rows;
+  deepfm_tile_forward<EP>(p, b, row0);
+  deepfm_tile_logits<EP>(p, b, row0, [&](int, int row, float z) {
     store_score(b, row, sigmoidf_acc(z));
     if (b.logits) b.logits[row] = z;
   });
@@ -118,8 +29,7 @@ __global__ void __launch_bounds__(kThreads) deepfm_kernel(DeepFmParams p, BatchV
 
 template <int EP>
 static size_t deepfm_smem() {
-  return ((size_t)kFm1Rows * ((2 * EP + kNumPad + 4) + (4 * EP + 4) + 68 + 68 + 4) +
-          (size_t)(2 * EP + kNumPad) * 64 + 64 * 64) * sizeof(float);
+  return (size_t)DeepFmTile<EP>::kFloats * sizeof(float);
 }
 
 template <int EP>

@@ -84,6 +84,52 @@ struct DeepFmParams {
   int EP;
 };
 
+// ---- DeepFM's training step (deepfm_train.cu; DESIGN.md section 4.9) ----------------------------
+// The Dense weights of a DeepFM trainer as one blob, offsets in floats: W1 [2EP + 8][64] and W2 [64][64] in
+// build_deepfm's tile order and padding, b1 [64], b2 [64], wdeep [64] (the deep rows of dense_2/kernel), wdot [4]
+// (its dot rows), bout (dense_2/bias) and 3 floats of padding.  The one-hot rows of dense_2/kernel live apart.
+struct DeepFmBlob {
+  int W1, b1, W2, b2, wdeep, wdot, bout, floats;
+  __host__ __device__ static DeepFmBlob of(int EP) {
+    DeepFmBlob l;
+    l.W1 = 0;
+    l.b1 = (2 * EP + kNumPad) * 64;
+    l.W2 = l.b1 + 64;
+    l.b2 = l.W2 + 64 * 64;
+    l.wdeep = l.b2 + 64;
+    l.wdot = l.wdeep + 64;
+    l.bout = l.wdot + 4;
+    l.floats = l.bout + 4;
+    return l;
+  }
+};
+constexpr int kDeepFmTables = 6;   // fm movieId, fm userId, fm movieGenre1, fm userGenre1, deep movieId, deep userId
+struct DeepFmStepArgs {
+  DeepFmParams p;          // the trainer's tables and Dense weights (wdot and bout are read from `blob`)
+  const float* blob;       // DeepFmBlob layout
+  BatchView b;             // the step's B rows in order; probs / logits receive its outputs before the update
+  const int32_t* label;    // [B]
+  int64_t tab_row0[kDeepFmTables];   // first row of each table in the trainer's table array
+  int32_t* trow;           // [6B] table row of entry s * B + r (slot s in kDeepFmTables order), -1 = none
+  float* gemb;             // [6B][EP] the entries' gradients
+  int32_t* frow;           // [4B] one-hot row of dense_2/kernel of entry s * B + r, -1 = none (a missing genre)
+  float* fgrad;            // [4B] its gradient (the row's dL/dz)
+  float* part;             // [ctas][DeepFmBlob::floats] per-CTA Dense gradient sums
+};
+int deepfm_train_ctas(int B);
+cudaError_t launch_deepfm_train_step(const DeepFmStepArgs& a, cudaStream_t s);
+struct DeepFmRows {        // a DeepFM dataset on the device, in the srs_batch layout
+  int32_t* movie;          // [n]
+  int32_t* user;           // [n]
+  int32_t* mgenre;         // [n][3], column 0 read
+  int32_t* ugenre;         // [n][5], column 0 read
+  float* numerics;         // [n][7]
+  int32_t* label;          // [n]
+};
+// dst row i = src row order[i], i < n (genres: column 0 only)
+cudaError_t launch_deepfm_permute(const DeepFmRows& src, const DeepFmRows& dst, const int32_t* order, int n,
+                                  cudaStream_t s);
+
 // ---- DeepFM with the deep MLP on tensor cores (deepfm_tc.cu): emb_dim 13..16 --------------------
 struct DeepFmTcParams {
   const float* fm_movie;   // [n_movies][16]

@@ -1,17 +1,21 @@
-// ncf_train.cu - `model.fit` of NeuralCF (neural_cf_model_1, NeuralCF.py:74-91) on the device: the C ABI's
-// srs_trainer (include/srs_ctr.h) and its kernels.  DESIGN.md section 4.8.
+// ncf_train.cu - `model.fit` on the device: the C ABI's srs_trainer (include/srs_ctr.h), which trains NeuralCF
+// (neural_cf_model_1, NeuralCF.py:74-91; DESIGN.md section 4.8) and DeepFM (DeepFM.py; section 4.9, its step kernel
+// in deepfm_train.cu), and the kernels both models share: dedupe, the two forms of Adam, metrics.
 //
-// One step of batch B_b (rows order[off .. off + B_b) of the uploaded dataset), five launches, no host sync:
+// NeuralCF's step of batch B_b (rows order[off .. off + B_b) of the uploaded dataset), five launches, no host sync:
 //   ncf_train_step_kernel  forward (the arithmetic of ncf_kernel) and backward, one thread per row; the Dense
 //                          gradients as per-CTA partials summed over the CTA's rows in row order; each row's two
 //                          embedding gradients and table rows to a list
 //   table_grad_kernel      the table gradient of each distinct id of the batch: its rows' gradients added in row
 //                          order by the thread of its first row (TF's _deduplicate_indexed_slices), into G
-//   table_adam_kernel      Keras's sparse Adam on EVERY row of both tables (decay m and v, add the batch's G, update
+//   table_adam_kernel<false>  Keras's sparse Adam on EVERY row of both tables (decay m and v, add the batch's G, update
 //                          w); clears G
 //   dense_adam_kernel      the CTA partials summed in CTA order, then TF's ApplyAdam on the Dense weights; advances
 //                          the device-resident iteration counter
 //   metrics_update_kernel  the step's probs / logits / labels into the epoch's history (metrics.cu)
+// DeepFM's step is seven launches: deepfm_train_step_kernel, table_grad_kernel over its table entries and again over
+// its one-hot entries, table_adam_kernel<false> over the six tables and <true> over dense_2/kernel's one-hot rows,
+// dense_adam_kernel, metrics_update_kernel; plus deepfm_permute_kernel once per epoch.
 // No float atomics: every sum has a fixed order, so a fit is bitwise reproducible.
 #include <cuda_runtime.h>
 
@@ -172,12 +176,13 @@ __global__ void __launch_bounds__(kTrainRows) ncf_train_step_kernel(StepArgs a, 
 }
 
 // G[t] = the sum, in entry order, of the gradients of the entries whose table row is t; entry e owns row t when
-// no earlier entry has it.  G is zero on entry (table_adam_kernel clears what it reads).
+// no earlier entry has it; t = -1 is no entry.  G is zero on entry (table_adam_kernel clears what it reads).
 __global__ void table_grad_kernel(const int32_t* __restrict__ trow, const float* __restrict__ gemb, int n,
                                   int EP, float* __restrict__ G) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n) return;
   const int t = trow[e];
+  if (t < 0) return;                                  // no entry (a missing genre)
   for (int j = 0; j < e; ++j)
     if (trow[j] == t) return;
   float* g = G + (size_t)t * EP;
@@ -187,8 +192,11 @@ __global__ void table_grad_kernel(const int32_t* __restrict__ trow, const float*
   }
 }
 
-// Keras's _resource_apply_sparse on every element of both tables: m = b1 m + (1-b1) G, v = b2 v + (1-b2) G^2,
-// w -= alpha m / (sqrt(v) + eps), each operation rounded on its own (no contraction)
+// Keras Adam on every element of an array whose gradient table_grad_kernel deduped into G (cleared behind it):
+// kApplyAdam = false, _resource_apply_sparse (the embedding tables): m = b1 m + (1-b1) G, v = b2 v + (1-b2) G^2;
+// kApplyAdam = true, ApplyAdam's dense form (DeepFM's one-hot rows of dense_2/kernel): m += (G - m)(1-b1),
+// v += (G^2 - v)(1-b2).  Then w -= alpha m / (sqrt(v) + eps).  Each operation is rounded on its own (no contraction).
+template <bool kApplyAdam>
 __global__ void table_adam_kernel(float* __restrict__ w, float* __restrict__ m, float* __restrict__ v,
                                   float* __restrict__ G, int64_t n, AdamHp h, const long long* __restrict__ it) {
   const float alpha = adam_alpha(h, *it);
@@ -196,8 +204,10 @@ __global__ void table_adam_kernel(float* __restrict__ w, float* __restrict__ m, 
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float g = G[i];
     if (g != 0.f) G[i] = 0.f;
-    const float mi = __fadd_rn(__fmul_rn(h.b1, m[i]), __fmul_rn(c1, g));
-    const float vi = __fadd_rn(__fmul_rn(h.b2, v[i]), __fmul_rn(c2, __fmul_rn(g, g)));
+    const float mi = kApplyAdam ? __fadd_rn(m[i], __fmul_rn(__fsub_rn(g, m[i]), c1))
+                                : __fadd_rn(__fmul_rn(h.b1, m[i]), __fmul_rn(c1, g));
+    const float vi = kApplyAdam ? __fadd_rn(v[i], __fmul_rn(__fsub_rn(__fmul_rn(g, g), v[i]), c2))
+                                : __fadd_rn(__fmul_rn(h.b2, v[i]), __fmul_rn(c2, __fmul_rn(g, g)));
     m[i] = mi;
     v[i] = vi;
     w[i] = __fsub_rn(w[i], __fdiv_rn(__fmul_rn(alpha, mi), __fadd_rn(__fsqrt_rn(vi), h.eps)));
@@ -289,6 +299,13 @@ struct DeviceScratch {
   }
 };
 
+struct TrainTensor {                  // one Keras tensor of a trainer
+  std::string name;
+  int64_t rows, cols;
+  int64_t row0;                       // an embedding table: its first row in the trainer's table array; else -1
+  std::vector<int64_t> at;            // a Dense tensor: element i * cols + j -> blob offset, or -1 - r for one-hot row r
+};
+
 }  // namespace
 }  // namespace srs
 
@@ -298,11 +315,16 @@ struct srs_trainer {
   srs_spec spec{};
   int device = 0;
   int E = 0, EP = 0, HP = 0;
-  TrainLayout ly{};
+  TrainLayout ly{};                   // NeuralCF's blob layout
+  int blob_floats = 0;
   AdamHp hp{};
-  int64_t tab_floats = 0;             // (n_movies + n_users) * EP
-  float* tab[4] = {};                 // w, m, v, G   [n_movies + n_users][EP], padding zero
+  std::vector<TrainTensor> tensors;   // the Keras tensors, in srs_model_create's order
+  int64_t tab_row0[kDeepFmTables] = {};   // first row of each table in tab (DeepFM)
+  int64_t tab_floats = 0;             // (sum of the tables' rows) * EP
+  float* tab[4] = {};                 // w, m, v, G   [rows][EP], padding zero
   float* blob[3] = {};                // w, m, v      [blob_floats]
+  int64_t onehot = 0;                 // DeepFM: the one-hot rows of dense_2/kernel (fm1_width)
+  float* fo[4] = {};                  // w, m, v, G   [onehot]
   long long* d_it = nullptr;          // Adam's iteration counter, on the device
   int64_t iterations = 0;             // its host mirror
   cudaStream_t stream = nullptr;
@@ -315,6 +337,7 @@ void trainer_free(srs_trainer* t) {
   cudaSetDevice(t->device);
   for (float* p : t->tab) cudaFree(p);
   for (float* p : t->blob) cudaFree(p);
+  for (float* p : t->fo) cudaFree(p);
   cudaFree(t->d_it);
   if (t->stream) cudaStreamDestroy(t->stream);
   delete t;
@@ -338,30 +361,100 @@ const srs_tensor* find_tensor(const srs_tensor* ts, int n, const char* name, int
   return nullptr;
 }
 
-// the Keras shape of a trainer tensor: table (layer -1), Dense kernel / bias of layer l; false if unknown
-bool tensor_shape(const srs_trainer* t, const char* name, int* layer, int* is_bias, int64_t* rows, int64_t* cols) {
+TrainTensor table_tensor(const char* name, int64_t rows, int E, int64_t row0) {
+  TrainTensor x;
+  x.name = name; x.rows = rows; x.cols = E; x.row0 = row0;
+  return x;
+}
+
+TrainTensor dense_tensor(const char* name, int64_t rows, int64_t cols) {
+  TrainTensor x;
+  x.name = name; x.rows = rows; x.cols = cols; x.row0 = -1;
+  x.at.assign((size_t)(rows * cols), -1);
+  return x;
+}
+
+// NeuralCF: the two tables (movie rows, then user rows) and dense_l/kernel, dense_l/bias in build_ncf's blob layout
+void ncf_tensors(srs_trainer* t) {
   const srs_spec& s = t->spec;
-  if (!strcmp(name, "movieId_embedding")) { *layer = -1; *is_bias = 0; *rows = s.n_movies; *cols = t->E; return true; }
-  if (!strcmp(name, "userId_embedding")) { *layer = -1; *is_bias = 1; *rows = s.n_users; *cols = t->E; return true; }
-  const int L = s.n_hidden;
+  const int L = s.n_hidden, E = t->E, EP = t->EP, HP = t->HP;
+  t->tensors.push_back(table_tensor("movieId_embedding", s.n_movies, E, 0));
+  t->tensors.push_back(table_tensor("userId_embedding", s.n_users, E, s.n_movies));
   for (int l = 0; l <= L; ++l) {
     char k[32], b[32];
     snprintf(k, sizeof(k), "dense_%d/kernel", l);
     snprintf(b, sizeof(b), "dense_%d/bias", l);
-    const int in = l == 0 ? 2 * t->E : s.hidden[l - 1], out = l == L ? 1 : s.hidden[l];
-    if (!strcmp(name, k)) { *layer = l; *is_bias = 0; *rows = in; *cols = out; return true; }
-    if (!strcmp(name, b)) { *layer = l; *is_bias = 1; *rows = out; *cols = 1; return true; }
+    const int in = l == 0 ? 2 * E : s.hidden[l - 1], out = l == L ? 1 : s.hidden[l];
+    TrainTensor K = dense_tensor(k, in, out), B = dense_tensor(b, out, 1);
+    for (int i = 0; i < in; ++i)
+      for (int j = 0; j < out; ++j) {
+        if (l == L) { K.at[(size_t)i * out + j] = t->ly.out_w + i; continue; }
+        const int row = l == 0 ? (i < E ? i : EP + (i - E)) : i;
+        K.at[(size_t)i * out + j] = t->ly.w_off[l] + row * HP + j;
+      }
+    for (int i = 0; i < out; ++i) B.at[i] = l == L ? t->ly.out_b : t->ly.b_off[l] + i;
+    t->tensors.push_back(std::move(K));
+    t->tensors.push_back(std::move(B));
   }
-  return false;
 }
 
-// element (i, j) of a Dense tensor -> its blob offset (build_ncf's layout), -1 for none
-int blob_index(const srs_trainer* t, int layer, int is_bias, int64_t i, int64_t j) {
-  const int L = t->spec.n_hidden, E = t->E, EP = t->EP, HP = t->HP;
-  if (layer == L) return is_bias ? t->ly.out_b : t->ly.out_w + (int)i;
-  if (is_bias) return t->ly.b_off[layer] + (int)i;
-  const int row = layer == 0 ? (i < E ? (int)i : EP + (int)(i - E)) : (int)i;
-  return t->ly.w_off[layer] + row * HP + (int)j;
+// DeepFM: the six tables one after another, the Dense tensors in DeepFmBlob's layout (build_deepfm's tile order
+// and padding) and dense_2/kernel's one-hot rows in fo (at = -1 - row)
+void deepfm_tensors(srs_trainer* t) {
+  const srs_spec& s = t->spec;
+  const int E = t->E, EP = t->EP, h0 = s.hidden[0], h1 = s.hidden[1];
+  const DeepFmBlob ly = DeepFmBlob::of(EP);
+  const char* names[kDeepFmTables] = {"fm_movieId_embedding", "fm_userId_embedding", "fm_movieGenre1_embedding",
+                                      "fm_userGenre1_embedding", "deep_movieId_embedding", "deep_userId_embedding"};
+  const int64_t rows[kDeepFmTables] = {s.n_movies, s.n_users, s.n_genres, s.n_genres, s.n_movies, s.n_users};
+  int64_t row0 = 0;
+  for (int k = 0; k < kDeepFmTables; ++k) {
+    t->tab_row0[k] = row0;
+    t->tensors.push_back(table_tensor(names[k], rows[k], E, row0));
+    row0 += rows[k];
+  }
+  // dense/kernel rows, sorted DenseFeatures concat: movieAvgRating | deep movieId | 4 numerics | deep userId | 2
+  TrainTensor K1 = dense_tensor("dense/kernel", 7 + 2 * E, h0);
+  for (int i = 0; i < 7 + 2 * E; ++i) {
+    int tr;                                            // the tile row (deep movie | deep user | numerics)
+    if (i == 0) tr = 2 * EP;
+    else if (i <= E) tr = i - 1;
+    else if (i <= E + 4) tr = 2 * EP + (i - E);
+    else if (i <= 2 * E + 4) tr = EP + (i - E - 5);
+    else tr = 2 * EP + (i - 2 * E);
+    for (int j = 0; j < h0; ++j) K1.at[(size_t)i * h0 + j] = ly.W1 + tr * 64 + j;
+  }
+  TrainTensor B1 = dense_tensor("dense/bias", h0, 1), K2 = dense_tensor("dense_1/kernel", h0, h1),
+              B2 = dense_tensor("dense_1/bias", h1, 1);
+  for (int i = 0; i < h0; ++i) {
+    B1.at[i] = ly.b1 + i;
+    for (int j = 0; j < h1; ++j) K2.at[(size_t)i * h1 + j] = ly.W2 + i * 64 + j;
+  }
+  for (int j = 0; j < h1; ++j) B2.at[j] = ly.b2 + j;
+  const int64_t fm1 = t->onehot;
+  TrainTensor K3 = dense_tensor("dense_2/kernel", fm1 + 4 + h1, 1), B3 = dense_tensor("dense_2/bias", 1, 1);
+  for (int64_t i = 0; i < fm1 + 4 + h1; ++i)
+    K3.at[i] = i < fm1 ? -1 - i : i < fm1 + 4 ? ly.wdot + (i - fm1) : ly.wdeep + (i - fm1 - 4);
+  B3.at[0] = ly.bout;
+  for (TrainTensor* x : {&K1, &B1, &K2, &B2, &K3, &B3}) t->tensors.push_back(std::move(*x));
+}
+
+const TrainTensor* trainer_tensor(const srs_trainer* t, const char* name) {
+  for (const TrainTensor& x : t->tensors)
+    if (x.name == name) return &x;
+  return nullptr;
+}
+
+// a DeepFM dataset of n rows on the device
+DeepFmRows deepfm_rows(DeviceScratch& sc, int n, cudaError_t* e) {
+  DeepFmRows r{};
+  *e = sc.alloc(&r.movie, n);
+  if (*e == cudaSuccess) *e = sc.alloc(&r.user, n);
+  if (*e == cudaSuccess) *e = sc.alloc(&r.mgenre, (size_t)n * 3);
+  if (*e == cudaSuccess) *e = sc.alloc(&r.ugenre, (size_t)n * 5);
+  if (*e == cudaSuccess) *e = sc.alloc(&r.numerics, (size_t)n * kNumNumerics);
+  if (*e == cudaSuccess) *e = sc.alloc(&r.label, n);
+  return r;
 }
 
 }  // namespace
@@ -373,14 +466,23 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
   if (!spec || !out) return failf(SRS_ERR_INVALID, "null argument");
   *out = nullptr;
   const srs_spec& s = *spec;
-  if (s.kind != SRS_NEURALCF) return failf(SRS_ERR_INVALID, "fit is implemented for NeuralCF (neural_cf_model_1) only");
+  const bool fm = s.kind == SRS_DEEPFM;
+  if (s.kind != SRS_NEURALCF && !fm)
+    return failf(SRS_ERR_INVALID, "fit is implemented for NeuralCF (neural_cf_model_1) and DeepFM only");
   if (s.emb_dim < 1 || s.emb_dim > 64) return failf(SRS_ERR_INVALID, "emb_dim must be in 1..64");
   if (s.n_movies < 1 || s.n_users < 1) return failf(SRS_ERR_INVALID, "empty vocabulary");
-  if (s.n_hidden < 1 || s.n_hidden > 3) return failf(SRS_ERR_INVALID, "1..3 hidden layers supported");
   int hmax = 0;
-  for (int i = 0; i < s.n_hidden; ++i) {
-    if (s.hidden[i] < 1 || s.hidden[i] > 32) return failf(SRS_ERR_INVALID, "hidden widths must be in 1..32");
-    hmax = std::max(hmax, s.hidden[i]);
+  if (fm) {
+    if (s.n_hidden != 2) return failf(SRS_ERR_INVALID, "DeepFM's fit needs exactly 2 hidden layers");
+    if (s.n_genres < 1) return failf(SRS_ERR_INVALID, "empty genre vocabulary");
+    for (int i = 0; i < 2; ++i)
+      if (s.hidden[i] < 1 || s.hidden[i] > 64) return failf(SRS_ERR_INVALID, "DeepFM's hidden widths must be in 1..64");
+  } else {
+    if (s.n_hidden < 1 || s.n_hidden > 3) return failf(SRS_ERR_INVALID, "1..3 hidden layers supported");
+    for (int i = 0; i < s.n_hidden; ++i) {
+      if (s.hidden[i] < 1 || s.hidden[i] > 32) return failf(SRS_ERR_INVALID, "hidden widths must be in 1..32");
+      hmax = std::max(hmax, s.hidden[i]);
+    }
   }
   AdamHp h{0.001f, 0.9f, 0.999f, 1e-7f};              // Keras's Adam defaults
   if (hp) h = AdamHp{hp->lr, hp->beta_1, hp->beta_2, hp->epsilon};
@@ -400,38 +502,44 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
   t->hp = h;
   t->E = s.emb_dim;
   t->EP = s.emb_dim <= 12 ? 12 : s.emb_dim <= 16 ? 16 : s.emb_dim <= 32 ? 32 : 64;
-  t->HP = hmax <= 16 ? 16 : 32;
-  const int E = t->E, EP = t->EP, HP = t->HP, L = s.n_hidden;
-  // the blob layout of build_ncf: kernels [2EP or HP][HP] and biases [HP] per hidden layer, then out [HP], [4]
-  int off = 0;
-  t->ly.n_layers = L;
-  for (int l = 0; l < L; ++l) {
-    t->ly.w_off[l] = off; off += (l == 0 ? 2 * EP : HP) * HP;
-    t->ly.b_off[l] = off; off += HP;
+  const int EP = t->EP;
+  int64_t tab_rows;
+  if (fm) {
+    t->HP = 64;
+    t->blob_floats = DeepFmBlob::of(EP).floats;
+    t->onehot = (int64_t)2 * s.n_genres + s.n_movies + s.n_users;
+    tab_rows = 2 * ((int64_t)s.n_movies + s.n_users) + 2 * (int64_t)s.n_genres;
+    deepfm_tensors(t);
+  } else {
+    t->HP = hmax <= 16 ? 16 : 32;
+    const int HP = t->HP, L = s.n_hidden;
+    // the blob layout of build_ncf: kernels [2EP or HP][HP] and biases [HP] per hidden layer, then out [HP], [4]
+    int off = 0;
+    t->ly.n_layers = L;
+    for (int l = 0; l < L; ++l) {
+      t->ly.w_off[l] = off; off += (l == 0 ? 2 * EP : HP) * HP;
+      t->ly.b_off[l] = off; off += HP;
+    }
+    t->ly.out_w = off; off += HP;
+    t->ly.out_b = off; off += 4;
+    t->ly.blob_floats = off;
+    t->blob_floats = off;
+    tab_rows = (int64_t)s.n_movies + s.n_users;
+    ncf_tensors(t);
   }
-  t->ly.out_w = off; off += HP;
-  t->ly.out_b = off; off += 4;
-  t->ly.blob_floats = off;
-  t->tab_floats = ((int64_t)s.n_movies + s.n_users) * EP;
+  t->tab_floats = tab_rows * EP;
+  const int nb = t->blob_floats;
 
-  std::vector<float> blob(off, 0.f);
-  std::vector<std::pair<const float*, int64_t>> tabs;      // host source, rows
+  std::vector<float> blob(nb, 0.f), onehot(t->onehot, 0.f);
+  std::vector<std::pair<const srs_tensor*, int64_t>> tabs;   // host source, first row
   int rc = SRS_OK;
-  for (int which = 0; which < 2 && rc == SRS_OK; ++which) {
-    const char* name = which ? "userId_embedding" : "movieId_embedding";
-    const srs_tensor* x = find_tensor(tensors, n_tensors, name, which ? s.n_users : s.n_movies, E, &rc);
-    if (x) tabs.push_back({x->data, x->rows});
-  }
-  for (int l = 0; l <= L && rc == SRS_OK; ++l) {
-    for (int is_bias = 0; is_bias < 2 && rc == SRS_OK; ++is_bias) {
-      char name[32];
-      snprintf(name, sizeof(name), is_bias ? "dense_%d/bias" : "dense_%d/kernel", l);
-      int layer, b; int64_t rows, cols;
-      tensor_shape(t, name, &layer, &b, &rows, &cols);
-      const srs_tensor* x = find_tensor(tensors, n_tensors, name, rows, cols, &rc);
-      if (!x) break;
-      for (int64_t i = 0; i < rows; ++i)
-        for (int64_t j = 0; j < cols; ++j) blob[blob_index(t, layer, b, i, j)] = x->data[i * cols + j];
+  for (const TrainTensor& x : t->tensors) {
+    const srs_tensor* src = find_tensor(tensors, n_tensors, x.name.c_str(), x.rows, x.cols, &rc);
+    if (!src) break;
+    if (x.row0 >= 0) { tabs.push_back({src, x.row0}); continue; }
+    for (size_t i = 0; i < x.at.size(); ++i) {
+      if (x.at[i] >= 0) blob[x.at[i]] = src->data[i];
+      else onehot[-1 - x.at[i]] = src->data[i];
     }
   }
   if (rc != SRS_OK) { delete t; return rc; }
@@ -439,17 +547,21 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
   ce = cudaSetDevice(device);
   if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking);
   for (int k = 0; k < 4 && ce == cudaSuccess; ++k) ce = cudaMalloc(&t->tab[k], t->tab_floats * sizeof(float));
-  for (int k = 0; k < 3 && ce == cudaSuccess; ++k) ce = cudaMalloc(&t->blob[k], (size_t)off * sizeof(float));
+  for (int k = 0; k < 3 && ce == cudaSuccess; ++k) ce = cudaMalloc(&t->blob[k], (size_t)nb * sizeof(float));
+  for (int k = 0; k < 4 && ce == cudaSuccess && t->onehot; ++k) ce = cudaMalloc(&t->fo[k], t->onehot * sizeof(float));
   if (ce == cudaSuccess) ce = cudaMalloc(&t->d_it, sizeof(long long));
   for (int k = 0; k < 4 && ce == cudaSuccess; ++k) ce = cudaMemset(t->tab[k], 0, t->tab_floats * sizeof(float));
-  for (int k = 1; k < 3 && ce == cudaSuccess; ++k) ce = cudaMemset(t->blob[k], 0, (size_t)off * sizeof(float));
+  for (int k = 1; k < 3 && ce == cudaSuccess; ++k) ce = cudaMemset(t->blob[k], 0, (size_t)nb * sizeof(float));
+  for (int k = 1; k < 4 && ce == cudaSuccess && t->onehot; ++k) ce = cudaMemset(t->fo[k], 0, t->onehot * sizeof(float));
   if (ce == cudaSuccess) ce = cudaMemset(t->d_it, 0, sizeof(long long));
-  if (ce == cudaSuccess) ce = cudaMemcpy(t->blob[0], blob.data(), (size_t)off * sizeof(float), cudaMemcpyHostToDevice);
-  int64_t row0 = 0;
+  if (ce == cudaSuccess) ce = cudaMemcpy(t->blob[0], blob.data(), (size_t)nb * sizeof(float), cudaMemcpyHostToDevice);
+  if (ce == cudaSuccess && t->onehot)
+    ce = cudaMemcpy(t->fo[0], onehot.data(), t->onehot * sizeof(float), cudaMemcpyHostToDevice);
   for (size_t k = 0; k < tabs.size() && ce == cudaSuccess; ++k) {   // [V][E] -> [V][EP], padding stays zero
-    ce = cudaMemcpy2D(t->tab[0] + row0 * EP, (size_t)EP * sizeof(float), tabs[k].first, (size_t)E * sizeof(float),
-                      (size_t)E * sizeof(float), (size_t)tabs[k].second, cudaMemcpyHostToDevice);
-    row0 += tabs[k].second;
+    const srs_tensor* x = tabs[k].first;
+    ce = cudaMemcpy2D(t->tab[0] + tabs[k].second * EP, (size_t)EP * sizeof(float), x->data,
+                      (size_t)x->cols * sizeof(float), (size_t)x->cols * sizeof(float), (size_t)x->rows,
+                      cudaMemcpyHostToDevice);
   }
   if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
   if (ce != cudaSuccess) {
@@ -468,11 +580,14 @@ int64_t srs_trainer_iterations(const srs_trainer* t) { return t ? t->iterations 
 int srs_trainer_fit_host(srs_trainer* t, const srs_batch* batch, const int32_t* labels, const int32_t* order,
                          int32_t batch_size, int32_t epochs, srs_eval_result* history) {
   if (!t || !batch || !labels || !order) return failf(SRS_ERR_INVALID, "null argument");
+  const bool fm = t->spec.kind == SRS_DEEPFM;
   const int n = batch->B;
   if (n < 1) return failf(SRS_ERR_INVALID, "fit needs at least one row");
   if (batch_size < 1) return failf(SRS_ERR_INVALID, "batch_size must be at least 1");
   if (epochs < 1) return failf(SRS_ERR_INVALID, "epochs must be at least 1");
   if (!batch->movie_id || !batch->user_id) return failf(SRS_ERR_INVALID, "movie_id and user_id are required");
+  if (fm && (!batch->movie_genre || !batch->user_genre || !batch->numerics))
+    return failf(SRS_ERR_INVALID, "DeepFM needs movie_genre, user_genre and numerics");
   // every check before the first launch: a rejected call leaves the trainer as it was
   for (int i = 0; i < n; ++i)
     if (labels[i] != 0 && labels[i] != 1) return failf(SRS_ERR_INVALID, "label of row %d is %d, not 0 or 1", i, labels[i]);
@@ -481,6 +596,14 @@ int srs_trainer_fit_host(srs_trainer* t, const srs_batch* batch, const int32_t* 
       return failf(SRS_ERR_RANGE, "movieId %d of row %d is outside [0, %d)", batch->movie_id[i], i, t->spec.n_movies);
     if ((unsigned)batch->user_id[i] >= (unsigned)t->spec.n_users)
       return failf(SRS_ERR_RANGE, "userId %d of row %d is outside [0, %d)", batch->user_id[i], i, t->spec.n_users);
+  }
+  for (int i = 0; fm && i < n; ++i) {                  // a negative genre is missing (deepfm_kernel's genre_id)
+    if (batch->movie_genre[(size_t)i * 3] >= t->spec.n_genres)
+      return failf(SRS_ERR_RANGE, "movieGenre1 index %d of row %d is outside [0, %d)", batch->movie_genre[(size_t)i * 3],
+                   i, t->spec.n_genres);
+    if (batch->user_genre[(size_t)i * 5] >= t->spec.n_genres)
+      return failf(SRS_ERR_RANGE, "userGenre1 index %d of row %d is outside [0, %d)", batch->user_genre[(size_t)i * 5],
+                   i, t->spec.n_genres);
   }
   {
     std::vector<char> seen(n);
@@ -495,52 +618,117 @@ int srs_trainer_fit_host(srs_trainer* t, const srs_batch* batch, const int32_t* 
   }
   TRAIN_TRY(cudaSetDevice(t->device));
   const int EP = t->EP, Bmax = std::min(batch_size, n);
-  const int n_cta = (Bmax + kTrainRows - 1) / kTrainRows;
+  const int n_ent = fm ? kDeepFmTables : 2;            // table entries per row
+  const int n_cta = fm ? deepfm_train_ctas(Bmax) : (Bmax + kTrainRows - 1) / kTrainRows;
   cudaStream_t s = t->stream;
   DeviceScratch sc;
-  int32_t *d_movie, *d_user, *d_label, *d_order, *d_lab_b, *d_trow;
-  float *d_probs, *d_logits, *d_gemb, *d_part;
+  int32_t *d_order, *d_trow, *d_lab_b = nullptr, *d_frow = nullptr;
+  float *d_probs, *d_logits, *d_gemb, *d_part, *d_fgrad = nullptr;
+  int* d_err = nullptr;
   EpochMetrics* d_met;
-  TRAIN_TRY(sc.alloc(&d_movie, n));
-  TRAIN_TRY(sc.alloc(&d_user, n));
-  TRAIN_TRY(sc.alloc(&d_label, n));
   TRAIN_TRY(sc.alloc(&d_order, (size_t)epochs * n));
-  TRAIN_TRY(sc.alloc(&d_lab_b, Bmax));
-  TRAIN_TRY(sc.alloc(&d_trow, 2 * (size_t)Bmax));
+  TRAIN_TRY(sc.alloc(&d_trow, (size_t)n_ent * Bmax));
   TRAIN_TRY(sc.alloc(&d_probs, Bmax));
   TRAIN_TRY(sc.alloc(&d_logits, Bmax));
-  TRAIN_TRY(sc.alloc(&d_gemb, 2 * (size_t)Bmax * EP));
-  TRAIN_TRY(sc.alloc(&d_part, (size_t)n_cta * t->ly.blob_floats));
+  TRAIN_TRY(sc.alloc(&d_gemb, (size_t)n_ent * Bmax * EP));
+  TRAIN_TRY(sc.alloc(&d_part, (size_t)n_cta * t->blob_floats));
   TRAIN_TRY(sc.alloc(&d_met, epochs));
-  TRAIN_TRY(cudaMemcpyAsync(d_movie, batch->movie_id, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-  TRAIN_TRY(cudaMemcpyAsync(d_user, batch->user_id, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-  TRAIN_TRY(cudaMemcpyAsync(d_label, labels, (size_t)n * 4, cudaMemcpyHostToDevice, s));
   TRAIN_TRY(cudaMemcpyAsync(d_order, order, (size_t)epochs * n * 4, cudaMemcpyHostToDevice, s));
   TRAIN_TRY(cudaMemsetAsync(d_met, 0, sizeof(EpochMetrics) * epochs, s));
+  DeepFmRows src{}, rows{};                            // DeepFM: the dataset, and the epoch's rows in order
+  int32_t *d_movie = nullptr, *d_user = nullptr, *d_label = nullptr;
+  if (fm) {
+    cudaError_t e;
+    src = deepfm_rows(sc, n, &e);
+    TRAIN_TRY(e);
+    rows = deepfm_rows(sc, n, &e);
+    TRAIN_TRY(e);
+    TRAIN_TRY(sc.alloc(&d_frow, 4 * (size_t)Bmax));
+    TRAIN_TRY(sc.alloc(&d_fgrad, 4 * (size_t)Bmax));
+    TRAIN_TRY(sc.alloc(&d_err, 1));
+    TRAIN_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), s));
+    TRAIN_TRY(cudaMemcpyAsync(src.movie, batch->movie_id, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    TRAIN_TRY(cudaMemcpyAsync(src.user, batch->user_id, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    TRAIN_TRY(cudaMemcpyAsync(src.mgenre, batch->movie_genre, (size_t)n * 3 * 4, cudaMemcpyHostToDevice, s));
+    TRAIN_TRY(cudaMemcpyAsync(src.ugenre, batch->user_genre, (size_t)n * 5 * 4, cudaMemcpyHostToDevice, s));
+    TRAIN_TRY(cudaMemcpyAsync(src.numerics, batch->numerics, (size_t)n * kNumNumerics * 4, cudaMemcpyHostToDevice, s));
+    TRAIN_TRY(cudaMemcpyAsync(src.label, labels, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  } else {
+    TRAIN_TRY(sc.alloc(&d_movie, n));
+    TRAIN_TRY(sc.alloc(&d_user, n));
+    TRAIN_TRY(sc.alloc(&d_label, n));
+    TRAIN_TRY(sc.alloc(&d_lab_b, Bmax));
+    TRAIN_TRY(cudaMemcpyAsync(d_movie, batch->movie_id, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    TRAIN_TRY(cudaMemcpyAsync(d_user, batch->user_id, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    TRAIN_TRY(cudaMemcpyAsync(d_label, labels, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  }
 
   int dev_sms = 132;
   cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, t->device);
   const int adam_blocks = (int)std::min<int64_t>((t->tab_floats + 255) / 256, (int64_t)dev_sms * 8);
+  const int fo_blocks = (int)std::min<int64_t>((t->onehot + 255) / 256, (int64_t)dev_sms * 8);
   StepArgs a{};
   a.tab = t->tab[0]; a.blob = t->blob[0];
   a.movie = d_movie; a.user = d_user; a.label = d_label;
   a.n_movies = t->spec.n_movies;
   a.probs = d_probs; a.logits = d_logits; a.labels = d_lab_b; a.trow = d_trow; a.gemb = d_gemb; a.part = d_part;
+  DeepFmStepArgs f{};
+  if (fm) {
+    const DeepFmBlob ly = DeepFmBlob::of(EP);
+    DeepFmParams& p = f.p;
+    float* tabs[kDeepFmTables];
+    for (int k = 0; k < kDeepFmTables; ++k) {
+      f.tab_row0[k] = t->tab_row0[k];
+      tabs[k] = t->tab[0] + t->tab_row0[k] * EP;
+    }
+    p.fm_movie = tabs[0]; p.fm_user = tabs[1]; p.fm_mgenre = tabs[2]; p.fm_ugenre = tabs[3];
+    p.deep_movie = tabs[4]; p.deep_user = tabs[5];
+    p.W1 = t->blob[0] + ly.W1; p.b1 = t->blob[0] + ly.b1; p.W2 = t->blob[0] + ly.W2; p.b2 = t->blob[0] + ly.b2;
+    p.first = t->fo[0]; p.wdeep = t->blob[0] + ly.wdeep;
+    p.n_movies = t->spec.n_movies; p.n_users = t->spec.n_users; p.n_genres = t->spec.n_genres; p.EP = EP;
+    f.blob = t->blob[0];
+    f.b.probs = d_probs; f.b.logits = d_logits; f.b.err_flag = d_err;
+    f.trow = d_trow; f.gemb = d_gemb; f.frow = d_frow; f.fgrad = d_fgrad; f.part = d_part;
+  }
   int64_t steps = 0;
   for (int e = 0; e < epochs; ++e) {
+    if (fm) TRAIN_TRY(launch_deepfm_permute(src, rows, d_order + (size_t)e * n, n, s));
     for (int off = 0; off < n; off += batch_size) {
-      a.B = std::min(batch_size, n - off);
-      a.order = d_order + (size_t)e * n + off;
-      TRAIN_TRY(launch_step(EP, t->HP, a, t->ly, s));
-      table_grad_kernel<<<(2 * a.B + 127) / 128, 128, 0, s>>>(d_trow, d_gemb, 2 * a.B, EP, t->tab[3]);
-      table_adam_kernel<<<adam_blocks, 256, 0, s>>>(t->tab[0], t->tab[1], t->tab[2], t->tab[3], t->tab_floats, t->hp,
-                                                   t->d_it);
-      dense_adam_kernel<<<1, kAdamThreads, 0, s>>>(d_part, (a.B + kTrainRows - 1) / kTrainRows, t->ly.blob_floats,
-                                                   t->blob[0], t->blob[1], t->blob[2], t->hp, t->d_it);
-      g_launch_count += 3;
+      const int B = std::min(batch_size, n - off);
+      const int32_t* step_labels;
+      if (fm) {
+        f.b.B = B;
+        f.b.movie_id = rows.movie + off; f.b.user_id = rows.user + off;
+        f.b.movie_genre = rows.mgenre + (size_t)off * 3; f.b.user_genre = rows.ugenre + (size_t)off * 5;
+        f.b.numerics = rows.numerics + (size_t)off * kNumNumerics;
+        f.label = rows.label + off;
+        step_labels = f.label;
+        TRAIN_TRY(launch_deepfm_train_step(f, s));
+        table_grad_kernel<<<(kDeepFmTables * B + 127) / 128, 128, 0, s>>>(d_trow, d_gemb, kDeepFmTables * B, EP,
+                                                                          t->tab[3]);
+        table_grad_kernel<<<(4 * B + 127) / 128, 128, 0, s>>>(d_frow, d_fgrad, 4 * B, 1, t->fo[3]);
+        table_adam_kernel<false><<<adam_blocks, 256, 0, s>>>(t->tab[0], t->tab[1], t->tab[2], t->tab[3],
+                                                             t->tab_floats, t->hp, t->d_it);
+        table_adam_kernel<true><<<fo_blocks, 256, 0, s>>>(t->fo[0], t->fo[1], t->fo[2], t->fo[3], t->onehot, t->hp,
+                                                          t->d_it);
+        dense_adam_kernel<<<1, kAdamThreads, 0, s>>>(d_part, deepfm_train_ctas(B), t->blob_floats, t->blob[0],
+                                                     t->blob[1], t->blob[2], t->hp, t->d_it);
+        g_launch_count += 5;
+      } else {
+        a.B = B;
+        a.order = d_order + (size_t)e * n + off;
+        step_labels = d_lab_b;
+        TRAIN_TRY(launch_step(EP, t->HP, a, t->ly, s));
+        table_grad_kernel<<<(2 * a.B + 127) / 128, 128, 0, s>>>(d_trow, d_gemb, 2 * a.B, EP, t->tab[3]);
+        table_adam_kernel<false><<<adam_blocks, 256, 0, s>>>(t->tab[0], t->tab[1], t->tab[2], t->tab[3],
+                                                             t->tab_floats, t->hp, t->d_it);
+        dense_adam_kernel<<<1, kAdamThreads, 0, s>>>(d_part, (a.B + kTrainRows - 1) / kTrainRows, t->ly.blob_floats,
+                                                     t->blob[0], t->blob[1], t->blob[2], t->hp, t->d_it);
+        g_launch_count += 3;
+      }
       TRAIN_TRY(cudaGetLastError());
-      TRAIN_TRY(launch_metrics_update(d_probs, d_logits, d_lab_b, a.B, &d_met[e].cnt, &d_met[e].red, &d_met[e].loss, 1,
-                                      s));
+      TRAIN_TRY(launch_metrics_update(d_probs, d_logits, step_labels, B, &d_met[e].cnt, &d_met[e].red, &d_met[e].loss,
+                                      1, s));
       ++steps;
     }
   }
@@ -557,22 +745,23 @@ int srs_trainer_fit_host(srs_trainer* t, const srs_batch* batch, const int32_t* 
 
 int srs_trainer_get_weights(const srs_trainer* t, const char* name, float* dst) {
   if (!t || !name || !dst) return failf(SRS_ERR_INVALID, "null argument");
-  int layer, is_bias;
-  int64_t rows, cols;
-  if (!tensor_shape(t, name, &layer, &is_bias, &rows, &cols))
-    return failf(SRS_ERR_MISSING, "the trainer has no tensor '%s'", name);
+  const TrainTensor* x = trainer_tensor(t, name);
+  if (!x) return failf(SRS_ERR_MISSING, "the trainer has no tensor '%s'", name);
   TRAIN_TRY(cudaSetDevice(t->device));
   TRAIN_TRY(cudaStreamSynchronize(t->stream));
-  if (layer < 0) {
-    const int64_t row0 = is_bias ? t->spec.n_movies : 0;      // is_bias marks the user table here
-    TRAIN_TRY(cudaMemcpy2D(dst, (size_t)cols * sizeof(float), t->tab[0] + row0 * t->EP, (size_t)t->EP * sizeof(float),
-                           (size_t)cols * sizeof(float), (size_t)rows, cudaMemcpyDeviceToHost));
+  if (x->row0 >= 0) {
+    TRAIN_TRY(cudaMemcpy2D(dst, (size_t)x->cols * sizeof(float), t->tab[0] + x->row0 * t->EP,
+                           (size_t)t->EP * sizeof(float), (size_t)x->cols * sizeof(float), (size_t)x->rows,
+                           cudaMemcpyDeviceToHost));
     return SRS_OK;
   }
-  std::vector<float> blob(t->ly.blob_floats);
+  std::vector<float> blob(t->blob_floats), onehot;
   TRAIN_TRY(cudaMemcpy(blob.data(), t->blob[0], blob.size() * sizeof(float), cudaMemcpyDeviceToHost));
-  for (int64_t i = 0; i < rows; ++i)
-    for (int64_t j = 0; j < cols; ++j) dst[i * cols + j] = blob[blob_index(t, layer, is_bias, i, j)];
+  if (t->onehot && std::any_of(x->at.begin(), x->at.end(), [](int64_t i) { return i < 0; })) {
+    onehot.resize(t->onehot);
+    TRAIN_TRY(cudaMemcpy(onehot.data(), t->fo[0], onehot.size() * sizeof(float), cudaMemcpyDeviceToHost));
+  }
+  for (size_t i = 0; i < x->at.size(); ++i) dst[i] = x->at[i] >= 0 ? blob[x->at[i]] : onehot[-1 - x->at[i]];
   return SRS_OK;
 }
 

@@ -66,11 +66,12 @@ class Surface:
         return self.model.evaluate(features, batch_size=batch_size)
 
     def fit(self, features, epochs: int = 5, batch_size: int = 12, seed: int = 0) -> dict:
-        """`model.fit(train_dataset, epochs=5)` (NeuralCF.py:91): train from the weights `model` was loaded with,
-        then rebuild `model` from the trained weights.  Returns Keras's history dict.  NeuralCF only."""
-        if self.name != "neuralcf":
-            raise NotImplementedError("tfrecmodel.%s: fit is implemented for NeuralCF (tfrecmodel.neuralcf) only"
-                                      % self.name)
+        """`model.fit(train_dataset, epochs=5)` (NeuralCF.py:91, DeepFM.py): train from the weights `model` was
+        loaded with, then rebuild `model` from the trained weights.  Returns Keras's history dict.  NeuralCF and
+        DeepFM only."""
+        if self.name not in ("neuralcf", "deepfm"):
+            raise NotImplementedError("tfrecmodel.%s: fit is implemented for NeuralCF (tfrecmodel.neuralcf) and "
+                                      "DeepFM (tfrecmodel.deepfm) only" % self.name)
         if self.model is None or self.weights is None:
             raise RuntimeError("tfrecmodel.%s: call load() before fit()" % self.name)
         from ..training import Trainer

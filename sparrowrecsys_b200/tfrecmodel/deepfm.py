@@ -5,6 +5,7 @@
     deepfm.load(weights)            # or load(savedmodel=...), load(spec=..., seed=...)
     p = deepfm.predict(features)    # dict of 1-D columns -> float32 [N,1]
     loss, acc, roc_auc, pr_auc = deepfm.evaluate(test_features)   # rows labelled by "label"
+    history = deepfm.fit(train_features, epochs=5)   # rebuilds `model` from the result
 """
 from ._surface import Surface
 
@@ -28,5 +29,9 @@ def evaluate(features, batch_size=None):
 
 
 def fit(features, epochs=5, batch_size=12, seed=0):
-    """Not implemented for this model: `fit` covers NeuralCF (tfrecmodel.neuralcf) only."""
-    return _surface.fit(features, epochs, batch_size, seed)
+    """`model.fit(train_dataset, epochs=5)`: train from the loaded weights on the GPU, then rebuild `model` from the
+    trained weights; returns Keras's history dict {"loss", "accuracy", "auc", "auc_1"} (one value per epoch)."""
+    global model
+    history = _surface.fit(features, epochs, batch_size, seed)
+    model = _surface.model
+    return history

@@ -59,5 +59,6 @@ def evaluate(features, batch_size=None):
 
 
 def fit(features, epochs=5, batch_size=12, seed=0):
-    """Not implemented for this model: `fit` covers NeuralCF (tfrecmodel.neuralcf) only."""
+    """Not implemented for this model: `fit` covers NeuralCF (tfrecmodel.neuralcf) and DeepFM (tfrecmodel.deepfm)
+    only."""
     return _surface.fit(features, epochs, batch_size, seed)

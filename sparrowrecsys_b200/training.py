@@ -1,5 +1,5 @@
-"""`model.fit` of NeuralCF on the GPU (NeuralCF.py:74-91: compile(loss='binary_crossentropy', optimizer='adam'),
-then fit(train_dataset, epochs=5) over make_csv_dataset batches of 12).
+"""`model.fit` of NeuralCF and DeepFM on the GPU (NeuralCF.py:74-91, DeepFM.py: compile(loss='binary_crossentropy',
+optimizer='adam'), then fit(train_dataset, epochs=5) over make_csv_dataset batches of 12).
 
     from sparrowrecsys_b200.training import Trainer
     tr = Trainer(spec, weights, device=0)                 # initial weights in Keras shapes
@@ -7,7 +7,7 @@ then fit(train_dataset, epochs=5) over make_csv_dataset batches of 12).
     model = tr.to_model()                                 # a serving CTRModel built from the trained weights
 
 The forward, backward and Keras Adam run in the CUDA library (`srs_trainer_*`, include/srs_ctr.h; DESIGN.md
-section 4.8).  TF's shuffle (buffer 10 000, unseeded) cannot be reproduced, so `fit` takes a seed instead: the host
+sections 4.8 and 4.9).  TF's shuffle (buffer 10 000, unseeded) cannot be reproduced, so `fit` takes a seed instead: the host
 draws one `numpy.random.default_rng(seed).permutation(n)` per epoch and the library trains in that row order.
 """
 from __future__ import annotations
@@ -18,7 +18,8 @@ from typing import Dict, Mapping, Optional
 import numpy as np
 
 from . import _lib
-from .model import CTRModel, _label_array, _spec_struct
+from .features import encode_batch
+from .model import CTRModel, _host_struct, _label_array, _spec_struct
 from .spec import ModelSpec
 from .weights import check_weights, weight_shapes
 
@@ -30,16 +31,19 @@ def epoch_orders(n: int, epochs: int, seed: int) -> np.ndarray:
 
 
 class Trainer:
-    """Trainable NeuralCF weights and Keras Adam's state on one GPU."""
+    """Trainable NeuralCF or DeepFM weights and Keras Adam's state on one GPU."""
+
+    MODELS = ("neuralcf", "deepfm")
 
     def __init__(self, spec: ModelSpec, weights: Mapping[str, np.ndarray], device: int = 0,
                  adam: Optional[Mapping[str, float]] = None):
         """`weights`: the initial weights (canonical names, Keras shapes, float32 host arrays), e.g.
         `init_weights(spec, seed, for_test=False)` for an untrained model.  `adam`: Keras Adam's lr, beta_1,
         beta_2, epsilon (default: Keras's 0.001, 0.9, 0.999, 1e-7).  NotImplementedError for any model but
-        NeuralCF."""
-        if spec.model != "neuralcf":
-            raise NotImplementedError("fit is implemented for NeuralCF (neural_cf_model_1) only, not %r" % spec.model)
+        NeuralCF and DeepFM."""
+        if spec.model not in self.MODELS:
+            raise NotImplementedError("fit is implemented for NeuralCF (neural_cf_model_1) and DeepFM only, not %r"
+                                      % spec.model)
         self.spec = spec
         self.device = int(device)
         self._h = None
@@ -87,19 +91,28 @@ class Trainer:
 
     def fit(self, features: Mapping[str, object], labels=None, epochs: int = 5, batch_size: int = 12, seed: int = 0,
             order=None) -> Dict[str, list]:
-        """`model.fit(dataset, epochs)`: train on the rows of `features` (`movieId`, `userId`; labels default to
+        """`model.fit(dataset, epochs)`: train on the rows of `features` (the model's `predict` columns: `movieId`,
+        `userId` for NeuralCF, also the 7 numerics, `movieGenre1` and `userGenre1` for DeepFM; labels default to
         `features["label"]`) in batches of `batch_size`, the last one partial.  The row order of epoch e is
         `epoch_orders(n, epochs, seed)[e]` unless `order` ([epochs][n], each a permutation) is given.  Returns
         Keras's history dict {"loss", "accuracy", "auc", "auc_1"}: one value per epoch, each computed on the
         steps' forward outputs before their updates (`auc` ROC, `auc_1` PR, the compile line's metric names).
-        ValueError for an out-of-range id, a label other than 0 / 1, or a bad order; the weights are then
-        unchanged."""
+        ValueError for an out-of-range id or genre, a label other than 0 / 1, or a bad order, KeyError for a
+        missing column; the weights are then unchanged."""
         lab = _label_array(features, labels)
         n = lab.shape[0]
-        movie = _ids(features, "movieId")
-        user = _ids(features, "userId")
-        if movie.shape[0] != n or user.shape[0] != n:
-            raise ValueError("labels have %d rows, the features %d" % (n, movie.shape[0]))
+        keep = []
+        if self.spec.model == "neuralcf":
+            movie = _ids(features, "movieId")
+            user = _ids(features, "userId")
+            if movie.shape[0] != n or user.shape[0] != n:
+                raise ValueError("labels have %d rows, the features %d" % (n, movie.shape[0]))
+            batch = _lib.SrsBatch(n, 0, movie.ctypes.data, user.ctypes.data, None, None, None, None, None)
+        else:                                           # predict's encoding: keys, dtypes, genre strings, errors
+            enc = encode_batch(self.spec, features)
+            if enc.B != n:
+                raise ValueError("labels have %d rows, the features %d" % (n, enc.B))
+            batch = _host_struct(enc, keep)
         if n == 0:
             raise ValueError("fit needs at least one row")
         epochs, batch_size = int(epochs), int(batch_size)
@@ -108,7 +121,6 @@ class Trainer:
         order = np.ascontiguousarray(order, np.int32)
         if order.shape != (epochs, n):
             raise ValueError("order must be [epochs=%d][n=%d], got %s" % (epochs, n, order.shape))
-        batch = _lib.SrsBatch(n, 0, movie.ctypes.data, user.ctypes.data, None, None, None, None, None)
         hist = (_lib.SrsEvalResult * max(epochs, 1))()
         _lib.check(self._lib.srs_trainer_fit_host(self._h, C.byref(batch), lab.ctypes.data, order.ctypes.data,
                                                   batch_size, epochs, hist))
