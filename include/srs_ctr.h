@@ -413,6 +413,26 @@ void srs_trainer_destroy(srs_trainer* tr);
 int srs_trainer_fit_host(srs_trainer* tr, const srs_batch* batch, const int32_t* labels, const int32_t* order,
                          int32_t batch_size, int32_t epochs, srs_eval_result* history);
 
+/* srs_trainer_fit_host with Keras's `fit(..., validation_data=(x_val, y_val), validation_freq=val_freq)`: at the
+ * end of every epoch e with (e + 1) % val_freq == 0, after its last update, `model.evaluate` of the current weights
+ * over all val_batch->B rows of `val_batch` (host, the columns `batch` has) with `val_labels` [B] int32, in file
+ * order.  val_history (NULL or [epochs]) receives those results as srs_trainer_evaluate_host would report them, and
+ * a zeroed entry (rows = 0) for every epoch not validated.  Validation changes no weight, no Adam state and no
+ * training history; its rows are uploaded once and each validated epoch adds two launches on the trainer's stream
+ * (the forward and one metrics update), with no host synchronisation.  Synchronous.  val_batch NULL: no validation,
+ * srs_trainer_fit_host exactly.  The validation rows are checked like the training rows, and val_freq >= 1, before
+ * any launch; a validation probability that is NaN or outside [0, 1] gives SRS_ERR_INVALID naming the epoch. */
+int srs_trainer_fit_validate_host(srs_trainer* tr, const srs_batch* batch, const int32_t* labels, const int32_t* order,
+                                  int32_t batch_size, int32_t epochs, srs_eval_result* history,
+                                  const srs_batch* val_batch, const int32_t* val_labels, int32_t val_freq,
+                                  srs_eval_result* val_history);
+
+/* `model.evaluate(x)` of the trainer's current weights (srs_evaluate_host_batches' metrics over the n rows as one
+ * batch), with no export and no srs_model: the rows (as srs_trainer_fit_host takes them) are uploaded, scored by
+ * the serving CUDA-core forward over the trainer's arrays and folded into the metrics on the device.  Synchronous;
+ * the checks and errors of srs_trainer_fit_host's rows, before any launch. */
+int srs_trainer_evaluate_host(srs_trainer* tr, const srs_batch* batch, const int32_t* labels, srs_eval_result* out);
+
 /* Copy one trained tensor, in its Keras shape, to host memory `dst` (SRS_ERR_MISSING for an unknown name). */
 int srs_trainer_get_weights(const srs_trainer* tr, const char* name, float* dst);
 

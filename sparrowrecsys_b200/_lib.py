@@ -46,7 +46,7 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_metrics_update_device", "srs_metrics_result", "srs_evaluate_host_batches",
            "srs_dien_outputs_device", "srs_dien_outputs_host_batches", "srs_dien_evaluate_host_batches",
            "srs_trainer_create", "srs_trainer_destroy", "srs_trainer_fit_host", "srs_trainer_get_weights",
-           "srs_trainer_iterations")
+           "srs_trainer_iterations", "srs_trainer_fit_validate_host", "srs_trainer_evaluate_host")
 
 _lib = None
 
@@ -205,6 +205,12 @@ def load():
     lib.srs_trainer_get_weights.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
     lib.srs_trainer_iterations.restype = C.c_int64
     lib.srs_trainer_iterations.argtypes = [C.c_void_p]
+    lib.srs_trainer_fit_validate_host.restype = C.c_int
+    lib.srs_trainer_fit_validate_host.argtypes = [C.c_void_p, C.POINTER(SrsBatch), C.c_void_p, C.c_void_p, C.c_int32,
+                                                  C.c_int32, C.POINTER(SrsEvalResult), C.POINTER(SrsBatch),
+                                                  C.c_void_p, C.c_int32, C.POINTER(SrsEvalResult)]
+    lib.srs_trainer_evaluate_host.restype = C.c_int
+    lib.srs_trainer_evaluate_host.argtypes = [C.c_void_p, C.POINTER(SrsBatch), C.c_void_p, C.POINTER(SrsEvalResult)]
     if lib.srs_abi_version() != ABI_VERSION:
         raise ImportError("libsrs_ctr.so ABI version %d != %d" % (lib.srs_abi_version(), ABI_VERSION))
     _lib = lib

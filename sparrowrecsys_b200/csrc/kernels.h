@@ -118,6 +118,9 @@ struct DeepFmStepArgs {
 };
 int deepfm_train_ctas(int B);
 cudaError_t launch_deepfm_train_step(const DeepFmStepArgs& a, cudaStream_t s);
+// deepfm_kernel's forward (probs and logits, both required) with p.wdot and p.bout taken from `blob` (DeepFmBlob
+// layout) on the device
+cudaError_t launch_deepfm_blob_forward(const DeepFmParams& p, const float* blob, const BatchView& b, cudaStream_t s);
 struct DeepFmRows {        // a DeepFM dataset on the device, in the srs_batch layout
   int32_t* movie;          // [n]
   int32_t* user;           // [n]

@@ -17,6 +17,10 @@
 // its one-hot entries, table_adam_kernel<false> over the six tables and <true> over dense_2/kernel's one-hot rows,
 // dense_adam_kernel, metrics_update_kernel; plus deepfm_permute_kernel once per epoch.
 // No float atomics: every sum has a fixed order, so a fit is bitwise reproducible.
+//
+// Validation (srs_trainer_fit_validate_host) and srs_trainer_evaluate_host run the serving forward over the
+// trainer's arrays (ncf_kernel; deepfm_kernel's forward reading wdot / bout from the blob) and one
+// metrics_update_kernel over all the rows: two launches, with the bits of a CTRModel built from the exported weights.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -457,6 +461,111 @@ DeepFmRows deepfm_rows(DeviceScratch& sc, int n, cudaError_t* e) {
   return r;
 }
 
+// The checks of rows the trainer reads (fit, validation, evaluate), all made before any launch.  `what` prefixes
+// the messages: "" or "validation data: ".
+int check_rows(const srs_trainer* t, const srs_batch* batch, const int32_t* labels, const char* what) {
+  const bool fm = t->spec.kind == SRS_DEEPFM;
+  const int n = batch->B;
+  if (!batch->movie_id || !batch->user_id) return failf(SRS_ERR_INVALID, "%smovie_id and user_id are required", what);
+  if (fm && (!batch->movie_genre || !batch->user_genre || !batch->numerics))
+    return failf(SRS_ERR_INVALID, "%sDeepFM needs movie_genre, user_genre and numerics", what);
+  for (int i = 0; i < n; ++i)
+    if (labels[i] != 0 && labels[i] != 1)
+      return failf(SRS_ERR_INVALID, "%slabel of row %d is %d, not 0 or 1", what, i, labels[i]);
+  for (int i = 0; i < n; ++i) {
+    if ((unsigned)batch->movie_id[i] >= (unsigned)t->spec.n_movies)
+      return failf(SRS_ERR_RANGE, "%smovieId %d of row %d is outside [0, %d)", what, batch->movie_id[i], i,
+                   t->spec.n_movies);
+    if ((unsigned)batch->user_id[i] >= (unsigned)t->spec.n_users)
+      return failf(SRS_ERR_RANGE, "%suserId %d of row %d is outside [0, %d)", what, batch->user_id[i], i,
+                   t->spec.n_users);
+  }
+  for (int i = 0; fm && i < n; ++i) {                  // a negative genre is missing (deepfm_kernel's genre_id)
+    if (batch->movie_genre[(size_t)i * 3] >= t->spec.n_genres)
+      return failf(SRS_ERR_RANGE, "%smovieGenre1 index %d of row %d is outside [0, %d)", what,
+                   batch->movie_genre[(size_t)i * 3], i, t->spec.n_genres);
+    if (batch->user_genre[(size_t)i * 5] >= t->spec.n_genres)
+      return failf(SRS_ERR_RANGE, "%suserGenre1 index %d of row %d is outside [0, %d)", what,
+                   batch->user_genre[(size_t)i * 5], i, t->spec.n_genres);
+  }
+  return SRS_OK;
+}
+
+// batch->B rows on the device, uploaded on s: the columns the trainer's model reads (NeuralCF: movie and user only)
+// and the labels
+cudaError_t upload_rows(DeviceScratch& sc, bool fm, const srs_batch* b, const int32_t* labels, DeepFmRows* r,
+                        cudaStream_t s) {
+  const size_t n = (size_t)b->B;
+  cudaError_t e;
+  if (fm) {
+    *r = deepfm_rows(sc, (int)n, &e);
+  } else {
+    *r = DeepFmRows{};
+    e = sc.alloc(&r->movie, n);
+    if (e == cudaSuccess) e = sc.alloc(&r->user, n);
+    if (e == cudaSuccess) e = sc.alloc(&r->label, n);
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(r->movie, b->movie_id, n * 4, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(r->user, b->user_id, n * 4, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(r->label, labels, n * 4, cudaMemcpyHostToDevice, s);
+  if (fm && e == cudaSuccess) e = cudaMemcpyAsync(r->mgenre, b->movie_genre, n * 3 * 4, cudaMemcpyHostToDevice, s);
+  if (fm && e == cudaSuccess) e = cudaMemcpyAsync(r->ugenre, b->user_genre, n * 5 * 4, cudaMemcpyHostToDevice, s);
+  if (fm && e == cudaSuccess)
+    e = cudaMemcpyAsync(r->numerics, b->numerics, n * kNumNumerics * 4, cudaMemcpyHostToDevice, s);
+  return e;
+}
+
+// The serving kernels' parameters over the trainer's arrays.  The blob is build_ncf's layout (TrainLayout's offsets
+// are build_ncf's, every segment a multiple of 4 floats) and the tables are movie rows, then user rows.
+NcfParams ncf_params(const srs_trainer* t) {
+  NcfParams p{};
+  p.movie = t->tab[0];
+  p.user = t->tab[0] + (size_t)t->spec.n_movies * t->EP;
+  p.blob = t->blob[0];
+  p.blob_floats = t->blob_floats;
+  p.n_movies = t->spec.n_movies; p.n_users = t->spec.n_users;
+  p.EP = t->EP; p.HP = t->HP; p.n_layers = t->ly.n_layers;
+  for (int l = 0; l < t->ly.n_layers; ++l) { p.w_off[l] = t->ly.w_off[l]; p.b_off[l] = t->ly.b_off[l]; }
+  p.out_w = t->ly.out_w; p.out_b = t->ly.out_b;
+  return p;
+}
+
+// DeepFmBlob's W1 / W2 / b1 / b2 / wdeep are build_deepfm's tile order and padding; wdot and bout stay in the blob
+// (the step kernel and deepfm_blob_forward_kernel read them there), so they are zero here
+DeepFmParams deepfm_params(const srs_trainer* t) {
+  const int EP = t->EP;
+  const DeepFmBlob ly = DeepFmBlob::of(EP);
+  DeepFmParams p{};
+  const float* tabs[kDeepFmTables];
+  for (int k = 0; k < kDeepFmTables; ++k) tabs[k] = t->tab[0] + t->tab_row0[k] * EP;
+  p.fm_movie = tabs[0]; p.fm_user = tabs[1]; p.fm_mgenre = tabs[2]; p.fm_ugenre = tabs[3];
+  p.deep_movie = tabs[4]; p.deep_user = tabs[5];
+  p.W1 = t->blob[0] + ly.W1; p.b1 = t->blob[0] + ly.b1; p.W2 = t->blob[0] + ly.W2; p.b2 = t->blob[0] + ly.b2;
+  p.first = t->fo[0]; p.wdeep = t->blob[0] + ly.wdeep;
+  p.n_movies = t->spec.n_movies; p.n_users = t->spec.n_users; p.n_genres = t->spec.n_genres; p.EP = EP;
+  return p;
+}
+
+// `model.evaluate` of the trainer's current weights over n device rows, two launches on s: the serving forward
+// (ncf_kernel, or deepfm_kernel's forward with the blob's wdot / bout), then one metrics_update_kernel over all
+// the rows into em.  `err` may be null for NeuralCF only (DeepFM's genre check writes it).
+cudaError_t eval_rows(const srs_trainer* t, const DeepFmRows& r, int n, float* probs, float* logits, int* err,
+                      EpochMetrics* em, cudaStream_t s) {
+  BatchView b{};
+  b.B = n;
+  b.movie_id = r.movie; b.user_id = r.user;
+  b.probs = probs; b.logits = logits; b.err_flag = err;
+  cudaError_t e;
+  if (t->spec.kind == SRS_DEEPFM) {
+    b.movie_genre = r.mgenre; b.user_genre = r.ugenre; b.numerics = r.numerics;
+    e = launch_deepfm_blob_forward(deepfm_params(t), t->blob[0], b, s);
+  } else {
+    e = launch_ncf(ncf_params(t), b, s);
+  }
+  if (e != cudaSuccess) return e;
+  return launch_metrics_update(probs, logits, r.label, n, &em->cnt, &em->red, &em->loss, 1, s);
+}
+
 }  // namespace
 
 extern "C" {
@@ -579,32 +688,23 @@ int64_t srs_trainer_iterations(const srs_trainer* t) { return t ? t->iterations 
 
 int srs_trainer_fit_host(srs_trainer* t, const srs_batch* batch, const int32_t* labels, const int32_t* order,
                          int32_t batch_size, int32_t epochs, srs_eval_result* history) {
+  return srs_trainer_fit_validate_host(t, batch, labels, order, batch_size, epochs, history, nullptr, nullptr, 1,
+                                       nullptr);
+}
+
+int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const int32_t* labels, const int32_t* order,
+                                  int32_t batch_size, int32_t epochs, srs_eval_result* history,
+                                  const srs_batch* val_batch, const int32_t* val_labels, int32_t val_freq,
+                                  srs_eval_result* val_history) {
   if (!t || !batch || !labels || !order) return failf(SRS_ERR_INVALID, "null argument");
   const bool fm = t->spec.kind == SRS_DEEPFM;
   const int n = batch->B;
   if (n < 1) return failf(SRS_ERR_INVALID, "fit needs at least one row");
   if (batch_size < 1) return failf(SRS_ERR_INVALID, "batch_size must be at least 1");
   if (epochs < 1) return failf(SRS_ERR_INVALID, "epochs must be at least 1");
-  if (!batch->movie_id || !batch->user_id) return failf(SRS_ERR_INVALID, "movie_id and user_id are required");
-  if (fm && (!batch->movie_genre || !batch->user_genre || !batch->numerics))
-    return failf(SRS_ERR_INVALID, "DeepFM needs movie_genre, user_genre and numerics");
   // every check before the first launch: a rejected call leaves the trainer as it was
-  for (int i = 0; i < n; ++i)
-    if (labels[i] != 0 && labels[i] != 1) return failf(SRS_ERR_INVALID, "label of row %d is %d, not 0 or 1", i, labels[i]);
-  for (int i = 0; i < n; ++i) {
-    if ((unsigned)batch->movie_id[i] >= (unsigned)t->spec.n_movies)
-      return failf(SRS_ERR_RANGE, "movieId %d of row %d is outside [0, %d)", batch->movie_id[i], i, t->spec.n_movies);
-    if ((unsigned)batch->user_id[i] >= (unsigned)t->spec.n_users)
-      return failf(SRS_ERR_RANGE, "userId %d of row %d is outside [0, %d)", batch->user_id[i], i, t->spec.n_users);
-  }
-  for (int i = 0; fm && i < n; ++i) {                  // a negative genre is missing (deepfm_kernel's genre_id)
-    if (batch->movie_genre[(size_t)i * 3] >= t->spec.n_genres)
-      return failf(SRS_ERR_RANGE, "movieGenre1 index %d of row %d is outside [0, %d)", batch->movie_genre[(size_t)i * 3],
-                   i, t->spec.n_genres);
-    if (batch->user_genre[(size_t)i * 5] >= t->spec.n_genres)
-      return failf(SRS_ERR_RANGE, "userGenre1 index %d of row %d is outside [0, %d)", batch->user_genre[(size_t)i * 5],
-                   i, t->spec.n_genres);
-  }
+  int rc = check_rows(t, batch, labels, "");
+  if (rc != SRS_OK) return rc;
   {
     std::vector<char> seen(n);
     for (int e = 0; e < epochs; ++e) {
@@ -615,6 +715,14 @@ int srs_trainer_fit_host(srs_trainer* t, const srs_batch* batch, const int32_t* 
         seen[r] = 1;
       }
     }
+  }
+  const int nv = val_batch ? val_batch->B : 0;         // validation rows; 0: no validation
+  if (val_batch) {
+    if (!val_labels) return failf(SRS_ERR_INVALID, "validation data: null labels");
+    if (nv < 1) return failf(SRS_ERR_INVALID, "validation data: needs at least one row");
+    if (val_freq < 1) return failf(SRS_ERR_INVALID, "validation_freq must be at least 1");
+    rc = check_rows(t, val_batch, val_labels, "validation data: ");
+    if (rc != SRS_OK) return rc;
   }
   TRAIN_TRY(cudaSetDevice(t->device));
   const int EP = t->EP, Bmax = std::min(batch_size, n);
@@ -635,32 +743,29 @@ int srs_trainer_fit_host(srs_trainer* t, const srs_batch* batch, const int32_t* 
   TRAIN_TRY(sc.alloc(&d_met, epochs));
   TRAIN_TRY(cudaMemcpyAsync(d_order, order, (size_t)epochs * n * 4, cudaMemcpyHostToDevice, s));
   TRAIN_TRY(cudaMemsetAsync(d_met, 0, sizeof(EpochMetrics) * epochs, s));
-  DeepFmRows src{}, rows{};                            // DeepFM: the dataset, and the epoch's rows in order
-  int32_t *d_movie = nullptr, *d_user = nullptr, *d_label = nullptr;
+  DeepFmRows src{}, rows{};                            // the dataset, and (DeepFM) the epoch's rows in order
+  TRAIN_TRY(upload_rows(sc, fm, batch, labels, &src, s));
   if (fm) {
     cudaError_t e;
-    src = deepfm_rows(sc, n, &e);
-    TRAIN_TRY(e);
     rows = deepfm_rows(sc, n, &e);
     TRAIN_TRY(e);
     TRAIN_TRY(sc.alloc(&d_frow, 4 * (size_t)Bmax));
     TRAIN_TRY(sc.alloc(&d_fgrad, 4 * (size_t)Bmax));
     TRAIN_TRY(sc.alloc(&d_err, 1));
     TRAIN_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), s));
-    TRAIN_TRY(cudaMemcpyAsync(src.movie, batch->movie_id, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    TRAIN_TRY(cudaMemcpyAsync(src.user, batch->user_id, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    TRAIN_TRY(cudaMemcpyAsync(src.mgenre, batch->movie_genre, (size_t)n * 3 * 4, cudaMemcpyHostToDevice, s));
-    TRAIN_TRY(cudaMemcpyAsync(src.ugenre, batch->user_genre, (size_t)n * 5 * 4, cudaMemcpyHostToDevice, s));
-    TRAIN_TRY(cudaMemcpyAsync(src.numerics, batch->numerics, (size_t)n * kNumNumerics * 4, cudaMemcpyHostToDevice, s));
-    TRAIN_TRY(cudaMemcpyAsync(src.label, labels, (size_t)n * 4, cudaMemcpyHostToDevice, s));
   } else {
-    TRAIN_TRY(sc.alloc(&d_movie, n));
-    TRAIN_TRY(sc.alloc(&d_user, n));
-    TRAIN_TRY(sc.alloc(&d_label, n));
     TRAIN_TRY(sc.alloc(&d_lab_b, Bmax));
-    TRAIN_TRY(cudaMemcpyAsync(d_movie, batch->movie_id, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    TRAIN_TRY(cudaMemcpyAsync(d_user, batch->user_id, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    TRAIN_TRY(cudaMemcpyAsync(d_label, labels, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  }
+  // validation: its rows uploaded once, in file order; each validated epoch's metrics in its own state
+  DeepFmRows vrows{};
+  float *d_vprobs = nullptr, *d_vlogits = nullptr;
+  EpochMetrics* d_vmet = nullptr;
+  if (nv) {
+    TRAIN_TRY(upload_rows(sc, fm, val_batch, val_labels, &vrows, s));
+    TRAIN_TRY(sc.alloc(&d_vprobs, nv));
+    TRAIN_TRY(sc.alloc(&d_vlogits, nv));
+    TRAIN_TRY(sc.alloc(&d_vmet, epochs));
+    TRAIN_TRY(cudaMemsetAsync(d_vmet, 0, sizeof(EpochMetrics) * epochs, s));
   }
 
   int dev_sms = 132;
@@ -669,23 +774,13 @@ int srs_trainer_fit_host(srs_trainer* t, const srs_batch* batch, const int32_t* 
   const int fo_blocks = (int)std::min<int64_t>((t->onehot + 255) / 256, (int64_t)dev_sms * 8);
   StepArgs a{};
   a.tab = t->tab[0]; a.blob = t->blob[0];
-  a.movie = d_movie; a.user = d_user; a.label = d_label;
+  a.movie = src.movie; a.user = src.user; a.label = src.label;
   a.n_movies = t->spec.n_movies;
   a.probs = d_probs; a.logits = d_logits; a.labels = d_lab_b; a.trow = d_trow; a.gemb = d_gemb; a.part = d_part;
   DeepFmStepArgs f{};
   if (fm) {
-    const DeepFmBlob ly = DeepFmBlob::of(EP);
-    DeepFmParams& p = f.p;
-    float* tabs[kDeepFmTables];
-    for (int k = 0; k < kDeepFmTables; ++k) {
-      f.tab_row0[k] = t->tab_row0[k];
-      tabs[k] = t->tab[0] + t->tab_row0[k] * EP;
-    }
-    p.fm_movie = tabs[0]; p.fm_user = tabs[1]; p.fm_mgenre = tabs[2]; p.fm_ugenre = tabs[3];
-    p.deep_movie = tabs[4]; p.deep_user = tabs[5];
-    p.W1 = t->blob[0] + ly.W1; p.b1 = t->blob[0] + ly.b1; p.W2 = t->blob[0] + ly.W2; p.b2 = t->blob[0] + ly.b2;
-    p.first = t->fo[0]; p.wdeep = t->blob[0] + ly.wdeep;
-    p.n_movies = t->spec.n_movies; p.n_users = t->spec.n_users; p.n_genres = t->spec.n_genres; p.EP = EP;
+    f.p = deepfm_params(t);
+    for (int k = 0; k < kDeepFmTables; ++k) f.tab_row0[k] = t->tab_row0[k];
     f.blob = t->blob[0];
     f.b.probs = d_probs; f.b.logits = d_logits; f.b.err_flag = d_err;
     f.trow = d_trow; f.gemb = d_gemb; f.frow = d_frow; f.fgrad = d_fgrad; f.part = d_part;
@@ -731,15 +826,55 @@ int srs_trainer_fit_host(srs_trainer* t, const srs_batch* batch, const int32_t* 
                                       1, s));
       ++steps;
     }
+    // after the epoch's last update, on the same stream: no host synchronisation
+    if (nv && (e + 1) % val_freq == 0) TRAIN_TRY(eval_rows(t, vrows, nv, d_vprobs, d_vlogits, d_err, &d_vmet[e], s));
   }
-  std::vector<EpochMetrics> met(epochs);
+  std::vector<EpochMetrics> met(epochs), vmet(nv ? epochs : 0);
   TRAIN_TRY(cudaMemcpyAsync(met.data(), d_met, sizeof(EpochMetrics) * epochs, cudaMemcpyDeviceToHost, s));
+  if (nv) TRAIN_TRY(cudaMemcpyAsync(vmet.data(), d_vmet, sizeof(EpochMetrics) * epochs, cudaMemcpyDeviceToHost, s));
   TRAIN_TRY(cudaStreamSynchronize(s));
   t->iterations += steps;
   for (int e = 0; e < epochs; ++e) {
+    const bool validated = nv && (e + 1) % val_freq == 0;
     if (met[e].cnt.err) return failf(SRS_ERR_INVALID, "epoch %d produced a probability that is NaN or outside [0, 1]", e);
+    if (validated && vmet[e].cnt.err)
+      return failf(SRS_ERR_INVALID, "the validation of epoch %d produced a probability that is NaN or outside [0, 1]",
+                   e);
     if (history) metrics_summarise(met[e].cnt.hist, met[e].cnt.correct, met[e].loss, &history[e], nullptr);
+    if (val_history) {
+      val_history[e] = srs_eval_result{};
+      if (validated) metrics_summarise(vmet[e].cnt.hist, vmet[e].cnt.correct, vmet[e].loss, &val_history[e], nullptr);
+    }
   }
+  return SRS_OK;
+}
+
+int srs_trainer_evaluate_host(srs_trainer* t, const srs_batch* batch, const int32_t* labels, srs_eval_result* out) {
+  if (!t || !batch || !labels || !out) return failf(SRS_ERR_INVALID, "null argument");
+  const int n = batch->B;
+  if (n < 1) return failf(SRS_ERR_INVALID, "evaluate needs at least one row");
+  const int rc = check_rows(t, batch, labels, "");
+  if (rc != SRS_OK) return rc;
+  TRAIN_TRY(cudaSetDevice(t->device));
+  cudaStream_t s = t->stream;
+  DeviceScratch sc;
+  DeepFmRows rows{};
+  float *d_probs, *d_logits;
+  int* d_err;
+  EpochMetrics* d_met;
+  TRAIN_TRY(upload_rows(sc, t->spec.kind == SRS_DEEPFM, batch, labels, &rows, s));
+  TRAIN_TRY(sc.alloc(&d_probs, n));
+  TRAIN_TRY(sc.alloc(&d_logits, n));
+  TRAIN_TRY(sc.alloc(&d_err, 1));
+  TRAIN_TRY(sc.alloc(&d_met, 1));
+  TRAIN_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), s));
+  TRAIN_TRY(cudaMemsetAsync(d_met, 0, sizeof(EpochMetrics), s));
+  TRAIN_TRY(eval_rows(t, rows, n, d_probs, d_logits, d_err, d_met, s));
+  EpochMetrics met;
+  TRAIN_TRY(cudaMemcpyAsync(&met, d_met, sizeof(met), cudaMemcpyDeviceToHost, s));
+  TRAIN_TRY(cudaStreamSynchronize(s));
+  if (met.cnt.err) return failf(SRS_ERR_INVALID, "evaluate produced a probability that is NaN or outside [0, 1]");
+  metrics_summarise(met.cnt.hist, met.cnt.correct, met.loss, out, nullptr);
   return SRS_OK;
 }
 

@@ -65,9 +65,11 @@ class Surface:
             raise RuntimeError("tfrecmodel.%s: call load() before evaluate()" % self.name)
         return self.model.evaluate(features, batch_size=batch_size)
 
-    def fit(self, features, epochs: int = 5, batch_size: int = 12, seed: int = 0) -> dict:
+    def fit(self, features, epochs: int = 5, batch_size: int = 12, seed: int = 0, validation_data=None,
+            validation_split: float = 0.0, validation_freq: int = 1) -> dict:
         """`model.fit(train_dataset, epochs=5)` (NeuralCF.py:91, DeepFM.py): train from the weights `model` was
-        loaded with, then rebuild `model` from the trained weights.  Returns Keras's history dict.  NeuralCF and
+        loaded with, then rebuild `model` from the trained weights.  Returns Keras's history dict, with the
+        `val_*` lists when `validation_data` or `validation_split` is given (`Trainer.fit`).  NeuralCF and
         DeepFM only."""
         if self.name not in ("neuralcf", "deepfm"):
             raise NotImplementedError("tfrecmodel.%s: fit is implemented for NeuralCF (tfrecmodel.neuralcf) and "
@@ -77,7 +79,9 @@ class Surface:
         from ..training import Trainer
         spec, device = self.model.spec, self.model.device
         with Trainer(spec, self.weights, device) as tr:
-            history = tr.fit(features, epochs=epochs, batch_size=batch_size, seed=seed)
+            history = tr.fit(features, epochs=epochs, batch_size=batch_size, seed=seed,
+                             validation_data=validation_data, validation_split=validation_split,
+                             validation_freq=validation_freq)
             trained = tr.weights()
         self.model.close()
         self.model = CTRModel(spec, trained, device)

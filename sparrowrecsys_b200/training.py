@@ -3,7 +3,9 @@ optimizer='adam'), then fit(train_dataset, epochs=5) over make_csv_dataset batch
 
     from sparrowrecsys_b200.training import Trainer
     tr = Trainer(spec, weights, device=0)                 # initial weights in Keras shapes
-    history = tr.fit(train_features, epochs=5, batch_size=12, seed=0)
+    history = tr.fit(train_features, epochs=5, batch_size=12, seed=0,
+                     validation_data=test_features)       # optional: adds val_loss, val_accuracy, val_auc, val_auc_1
+    loss, accuracy, roc_auc, pr_auc = tr.evaluate(test_features)   # the current weights, no export
     model = tr.to_model()                                 # a serving CTRModel built from the trained weights
 
 The forward, backward and Keras Adam run in the CUDA library (`srs_trainer_*`, include/srs_ctr.h; DESIGN.md
@@ -90,7 +92,8 @@ class Trainer:
         return int(self._lib.srs_trainer_iterations(self._h))
 
     def fit(self, features: Mapping[str, object], labels=None, epochs: int = 5, batch_size: int = 12, seed: int = 0,
-            order=None) -> Dict[str, list]:
+            order=None, validation_data=None, validation_split: float = 0.0,
+            validation_freq: int = 1) -> Dict[str, list]:
         """`model.fit(dataset, epochs)`: train on the rows of `features` (the model's `predict` columns: `movieId`,
         `userId` for NeuralCF, also the 7 numerics, `movieGenre1` and `userGenre1` for DeepFM; labels default to
         `features["label"]`) in batches of `batch_size`, the last one partial.  The row order of epoch e is
@@ -98,23 +101,46 @@ class Trainer:
         Keras's history dict {"loss", "accuracy", "auc", "auc_1"}: one value per epoch, each computed on the
         steps' forward outputs before their updates (`auc` ROC, `auc_1` PR, the compile line's metric names).
         ValueError for an out-of-range id or genre, a label other than 0 / 1, or a bad order, KeyError for a
-        missing column; the weights are then unchanged."""
-        lab = _label_array(features, labels)
-        n = lab.shape[0]
+        missing column; the weights are then unchanged.
+
+        Validation, as Keras's `fit`: `validation_data` is `(x_val, y_val)` or a feature dict with "label";
+        otherwise `validation_split` = f in (0, 1) holds out the last floor(n * f) rows, taken before any
+        shuffling (training then uses the first n - floor(n * f) rows, and `order` is over those).  The epochs e
+        with (e + 1) % `validation_freq` == 0 end, after their last update, with `evaluate` of the current weights
+        on the validation rows (one batch, in file order), logged as "val_loss", "val_accuracy", "val_auc" and
+        "val_auc_1" for those epochs only.  Validation changes no weight, no Adam state and no training log.  Its
+        rows are checked like the training rows before anything runs."""
+        res, vres, validated = self._fit(features, labels, epochs, batch_size, seed, order, validation_data,
+                                         validation_split, validation_freq)
+        out = _logs(res, "")
+        if validated:
+            out.update(_logs([vres[e] for e in validated], "val_"))
+        return out
+
+    def _fit(self, features, labels=None, epochs=5, batch_size=12, seed=0, order=None, validation_data=None,
+             validation_split=0.0, validation_freq=1):
+        """`fit`, returning the library's results: (the epochs' srs_eval_result, the validation's [epochs] with
+        zeroed entries for epochs not validated, the validated epochs)."""
+        val = None
+        if validation_data is not None:
+            val = _validation_pair(validation_data)
+        elif validation_split:
+            split = float(validation_split)
+            if not 0.0 < split < 1.0:
+                raise ValueError("validation_split must be in (0, 1), got %r" % (validation_split,))
+            lab = _label_array(features, labels)
+            n = lab.shape[0]
+            split_at = int(np.floor(n * (1.0 - split)))       # Keras's train_validation_split
+            if split_at == 0 or split_at == n:
+                raise ValueError("%d rows are not enough to split into a training and a validation part with "
+                                 "validation_split=%r" % (n, validation_split))
+            val = (_take(features, split_at, n), lab[split_at:])
+            features, labels = _take(features, 0, split_at), lab[:split_at]
+        if isinstance(validation_freq, bool) or not isinstance(validation_freq, (int, np.integer)) \
+                or validation_freq < 1:
+            raise ValueError("validation_freq must be an integer >= 1, got %r" % (validation_freq,))
         keep = []
-        if self.spec.model == "neuralcf":
-            movie = _ids(features, "movieId")
-            user = _ids(features, "userId")
-            if movie.shape[0] != n or user.shape[0] != n:
-                raise ValueError("labels have %d rows, the features %d" % (n, movie.shape[0]))
-            batch = _lib.SrsBatch(n, 0, movie.ctypes.data, user.ctypes.data, None, None, None, None, None)
-        else:                                           # predict's encoding: keys, dtypes, genre strings, errors
-            enc = encode_batch(self.spec, features)
-            if enc.B != n:
-                raise ValueError("labels have %d rows, the features %d" % (n, enc.B))
-            batch = _host_struct(enc, keep)
-        if n == 0:
-            raise ValueError("fit needs at least one row")
+        batch, lab, n = self._rows(features, labels, keep, "fit")
         epochs, batch_size = int(epochs), int(batch_size)
         if order is None:
             order = epoch_orders(n, epochs, seed)
@@ -122,10 +148,52 @@ class Trainer:
         if order.shape != (epochs, n):
             raise ValueError("order must be [epochs=%d][n=%d], got %s" % (epochs, n, order.shape))
         hist = (_lib.SrsEvalResult * max(epochs, 1))()
-        _lib.check(self._lib.srs_trainer_fit_host(self._h, C.byref(batch), lab.ctypes.data, order.ctypes.data,
-                                                  batch_size, epochs, hist))
-        return {"loss": [h.loss for h in hist[:epochs]], "accuracy": [h.accuracy for h in hist[:epochs]],
-                "auc": [h.roc_auc for h in hist[:epochs]], "auc_1": [h.pr_auc for h in hist[:epochs]]}
+        vhist = (_lib.SrsEvalResult * max(epochs, 1))()
+        vbatch, vlab = None, None
+        if val is not None:
+            vb, vlab, _ = self._rows(val[0], val[1], keep, "validation")
+            vbatch = C.byref(vb)
+        _lib.check(self._lib.srs_trainer_fit_validate_host(
+            self._h, C.byref(batch), lab.ctypes.data, order.ctypes.data, batch_size, epochs, hist, vbatch,
+            None if vlab is None else vlab.ctypes.data, int(validation_freq), vhist))
+        validated = [e for e in range(epochs) if val is not None and (e + 1) % validation_freq == 0]
+        return list(hist[:epochs]), list(vhist[:epochs]), validated
+
+    def evaluate(self, features: Mapping[str, object], labels=None):
+        """`model.evaluate(x)` of the current weights: (loss, accuracy, roc_auc, pr_auc) over the rows of
+        `features` in one batch, as `CTRModel.evaluate` of `to_model()` reports them (on CUDA cores), without
+        exporting the weights.  Errors as `fit`'s."""
+        r = self.evaluate_result(features, labels)
+        return r.loss, r.accuracy, r.roc_auc, r.pr_auc
+
+    def evaluate_result(self, features, labels=None) -> _lib.SrsEvalResult:
+        """`evaluate` with the counts: the `srs_eval_result` (rows, positives, correct and the four metrics)."""
+        keep = []
+        batch, lab, _ = self._rows(features, labels, keep, "evaluate")
+        out = _lib.SrsEvalResult()
+        _lib.check(self._lib.srs_trainer_evaluate_host(self._h, C.byref(batch), lab.ctypes.data, C.byref(out)))
+        return out
+
+    def _rows(self, features, labels, keep: list, what: str):
+        """(srs_batch over host arrays kept alive in `keep`, int32 labels, rows) of the model's columns."""
+        lab = _label_array(features, labels)
+        n = lab.shape[0]
+        if self.spec.model == "neuralcf":
+            movie = _ids(features, "movieId")
+            user = _ids(features, "userId")
+            if movie.shape[0] != n or user.shape[0] != n:
+                raise ValueError("labels have %d rows, the features %d" % (n, movie.shape[0]))
+            keep += [movie, user]
+            batch = _lib.SrsBatch(n, 0, movie.ctypes.data, user.ctypes.data, None, None, None, None, None)
+        else:                                           # predict's encoding: keys, dtypes, genre strings, errors
+            enc = encode_batch(self.spec, features)
+            if enc.B != n:
+                raise ValueError("labels have %d rows, the features %d" % (n, enc.B))
+            batch = _host_struct(enc, keep)
+        if n == 0:
+            raise ValueError("%s needs at least one row" % what)
+        keep.append(lab)
+        return batch, lab, n
 
     def weights(self) -> Dict[str, np.ndarray]:
         """The current weights, canonical names and Keras shapes (float32 host arrays)."""
@@ -139,6 +207,27 @@ class Trainer:
     def to_model(self, device: Optional[int] = None) -> CTRModel:
         """A serving `CTRModel` built from the current weights (the trainer is not shared with it)."""
         return CTRModel(self.spec, self.weights(), self.device if device is None else device)
+
+
+def _logs(results, prefix: str) -> Dict[str, list]:
+    """Keras's History lists of srs_eval_results: loss, accuracy, auc (ROC), auc_1 (PR)."""
+    return {prefix + "loss": [r.loss for r in results], prefix + "accuracy": [r.accuracy for r in results],
+            prefix + "auc": [r.roc_auc for r in results], prefix + "auc_1": [r.pr_auc for r in results]}
+
+
+def _validation_pair(validation_data):
+    """(features, labels) of `validation_data`: `(x_val, y_val)`, or a feature dict whose "label" holds the labels."""
+    if isinstance(validation_data, Mapping):
+        return validation_data, None
+    if isinstance(validation_data, (tuple, list)) and len(validation_data) == 2 \
+            and isinstance(validation_data[0], Mapping):
+        return validation_data[0], validation_data[1]
+    raise ValueError("validation_data must be (features, labels) or a feature dict with 'label'")
+
+
+def _take(features, lo: int, hi: int) -> Dict[str, np.ndarray]:
+    """Rows lo .. hi of every column of a feature dict."""
+    return {k: np.asarray(v)[lo:hi] for k, v in features.items()}
 
 
 def _ids(features, key) -> np.ndarray:

@@ -1,12 +1,17 @@
 """Time NeuralCF's or DeepFM's `fit` on the GPU against the numpy oracle on the host.
 
     python tools/fit_throughput.py [--model neuralcf|deepfm] [--epochs 5] [--batch-sizes 12,4096] [--cpu-epochs 1]
+                                   [--validate [--repeats 5]]
 
 Trains the reference script's run - the untrained model of `init_weights(default_spec(model), 0, for_test=False)`
 over the 88 827 rows of `tests/golden/<model>_trainset.npz` - for `--epochs` epochs at each batch size, and reports
 the wall time of `Trainer.fit` (upload, every step, the history read-back) and µs per step.  The CPU column is the
 float32 oracle (`oracle.ncf_train.fit` / `oracle.deepfm_train.fit`) over `--cpu-epochs` epochs at the same batch
-size, scaled to µs per step.  Prints one JSON object with the card name and power limit read from nvidia-smi in the
+size, scaled to µs per step (`--cpu-epochs 0` leaves it out).  `--validate` adds the cost of validating on the
+22 440 rows of `tests/golden/dien_testset.npz` every epoch, next to the epoch time: `validation_s_per_epoch` from
+fits of `--val-epochs` one-step epochs (the first batch of rows) with and without validation, where the two validation
+launches are a large part of each epoch, and `validated_minus_plain_s_per_epoch` from full-size fits (below the
+noise of a 7 403-step epoch).  Plain and validated fits alternate, `--repeats` pairs, medians.  Prints one JSON object with the card name and power limit read from nvidia-smi in the
 same run (and the model's name unless it is the default, NeuralCF).  Writes nothing.
 """
 import argparse
@@ -38,6 +43,10 @@ def main():
     ap.add_argument("--epochs", type=int, default=5)
     ap.add_argument("--batch-sizes", default="12,4096")
     ap.add_argument("--cpu-epochs", type=int, default=1)
+    ap.add_argument("--validate", action="store_true",
+                    help="also report the cost per epoch of validating on dien_testset.npz every epoch")
+    ap.add_argument("--val-epochs", type=int, default=500)
+    ap.add_argument("--repeats", type=int, default=5)
     args = ap.parse_args()
     from oracle import deepfm_train, ncf_train
     from sparrowrecsys_b200.spec import default_spec
@@ -61,23 +70,45 @@ def main():
     res = {"rows": n, "epochs": args.epochs, **card(), "runs": []}
     if args.model != "neuralcf":
         res = {"model": args.model, **res}
+    val = None
+    if args.validate:
+        t = np.load(os.path.join(ROOT, "tests", "golden", "dien_testset.npz"))
+        val = {k: t[k] for k in (("movieId", "userId", "label") if args.model == "neuralcf" else t.files)}
+        res["validation_rows"] = len(val["label"])
+
+    def timed_fit(B, validation_data=None, rows=None, epochs=args.epochs):
+        f = feats if rows is None else {k: v[:rows] for k, v in feats.items()}
+        with Trainer(spec, W0) as tr:
+            t0 = time.perf_counter()
+            hist = tr.fit(f, epochs=epochs, batch_size=B, seed=0, validation_data=validation_data)
+            return time.perf_counter() - t0, hist
+
+    def paired(B, **kw):
+        """median over --repeats alternating pairs of the validated fit's wall minus the plain fit's"""
+        pairs = [(timed_fit(B, **kw)[0], timed_fit(B, val, **kw)[0]) for _ in range(args.repeats)]
+        return float(np.median([p for p, _ in pairs])), float(np.median([v - p for p, v in pairs]))
+
     for B in (int(b) for b in args.batch_sizes.split(",")):
         steps = args.epochs * -(-n // B)
         with Trainer(spec, W0) as tr:
-            tr.fit(feats, epochs=1, batch_size=B, seed=1)          # warm-up: module load, first launches
-        with Trainer(spec, W0) as tr:
+            tr.fit(feats, epochs=1, batch_size=B, seed=1, validation_data=val)   # warm-up: module load, first launches
+        wall, hist = timed_fit(B)
+        run = {"batch_size": B, "steps": steps, "gpu_wall_s": wall, "gpu_us_per_step": 1e6 * wall / steps}
+        if val is not None:                       # plain and validated fits alternate, so drift hits both alike
+            plain, extra = paired(B)
+            _, extra_small = paired(B, rows=B, epochs=args.val_epochs)
+            run.update({"gpu_epoch_s": plain / args.epochs, "validation_s_per_epoch": extra_small / args.val_epochs,
+                        "validated_minus_plain_s_per_epoch": extra / args.epochs})
+        if args.cpu_epochs:
+            orders = ncf_train.epoch_orders(n, args.cpu_epochs, 0)
             t0 = time.perf_counter()
-            hist = tr.fit(feats, epochs=args.epochs, batch_size=B, seed=0)
-            wall = time.perf_counter() - t0
-        orders = ncf_train.epoch_orders(n, args.cpu_epochs, 0)
-        t0 = time.perf_counter()
-        oracle_fit(orders, B)
-        cpu = time.perf_counter() - t0
-        cpu_steps = args.cpu_epochs * -(-n // B)
-        res["runs"].append({"batch_size": B, "steps": steps, "gpu_wall_s": wall, "gpu_us_per_step": 1e6 * wall / steps,
-                            "cpu_oracle_us_per_step": 1e6 * cpu / cpu_steps,
-                            "cpu_oracle_wall_s_scaled": cpu * steps / cpu_steps,
-                            "final_epoch": {k: v[-1] for k, v in hist.items()}})
+            oracle_fit(orders, B)
+            cpu = time.perf_counter() - t0
+            cpu_steps = args.cpu_epochs * -(-n // B)
+            run.update({"cpu_oracle_us_per_step": 1e6 * cpu / cpu_steps,
+                        "cpu_oracle_wall_s_scaled": cpu * steps / cpu_steps})
+        run["final_epoch"] = {k: v[-1] for k, v in hist.items()}
+        res["runs"].append(run)
     print(json.dumps(res))
 
 
