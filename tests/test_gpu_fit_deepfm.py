@@ -63,14 +63,6 @@ def test_parity_batch_of_one_movie(trainset, B, n, epochs):
     _parity(trainset, default_spec("deepfm"), B, n, epochs, one_movie=True, multiple=6.0)
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("E", [16, 64])
-@pytest.mark.parametrize("B,n,epochs", [(12, 115, 1), (33, 330, 1)])
-def test_parity_padded_widths(trainset, E, B, n, epochs):
-    """E = 16 and 64 with hidden (37, 5): the table padding and the hidden padding to 64 must stay zero."""
-    _parity(trainset, default_spec("deepfm", emb_dim=E, hidden=(37, 5)), B, n, epochs)
-
-
 def _parity(trainset, spec, B, n, epochs, one_movie=False, multiple=SPREAD_MULTIPLE):
     from sparrowrecsys_b200.training import Trainer
     W0 = init_weights(spec, 3, for_test=True)
