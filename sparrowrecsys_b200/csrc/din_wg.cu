@@ -23,10 +23,14 @@
 //     (common.cuh::dense_layer); its W1 image would be ~160 KB, and at cfg 5's T = 200 the
 //     activation unit dominates the tile.
 //
-// CTA = 256 threads = two warpgroups, 32 batch rows; warpgroup q owns rows q, q + 2, ... and
+// CTA = 384 threads = three warpgroups, 32 batch rows; warpgroup q owns rows q, q + 3, ... and
 // double-buffers its history tiles (the next tile's cp.async runs under this tile's MMA and
-// epilogue; the ids of the tile after it are already on their way from HBM).  Shared memory:
-// ~209 KB with the MLP images (E <= 32) / ~180 KB (E <= 64): one CTA per SM.
+// epilogue; the ids of the tile after it are already on their way from HBM).  The per-row chain
+// is latency-bound, so a third warpgroup (12 warps per SM instead of 8) shortens each warpgroup's
+// walk from 16 rows to 11 without lengthening the chain.  The shared tile helpers
+// (tile_side_features, dense_layer, ...) map 256 threads; the third warpgroup skips them, and
+// only warpgroups 0 and 1 issue the top MLP's Dense(128).  Shared memory: ~213 KB with the MLP
+// images (E <= 32) / ~218 KB (E <= 64): one CTA per SM.
 #include "kernels.h"
 #include "wgmma.cuh"
 
@@ -35,6 +39,8 @@ using namespace wg;
 
 constexpr int kWgRows = 32;       // rows per CTA (top-MLP tile height, as din.cu)
 constexpr int kWgPos = 64;        // history positions per MMA tile
+constexpr int kWgGroups = 3;      // warpgroups per CTA: each walks every third row of the tile
+constexpr int kWgThreads = 128 * kWgGroups;
 
 template <int EP>
 struct DinWgLayout {
@@ -43,11 +49,15 @@ struct DinWgLayout {
   static constexpr uint32_t A_BYTES = KB * kWgPos * 128;      // one history tile
   static constexpr uint32_t B_BYTES = KB * 32 * 128;          // W_r, 32 unit rows
   static constexpr uint32_t WG_BYTES = 2 * A_BYTES + B_BYTES; // per warpgroup
-  static constexpr uint32_t AU_BYTES = 2 * WG_BYTES;
-  // top-MLP operand images (TC_MLP): W1^T [128 units][160 k] in 3 K blocks (the third half used) and
-  // W2^T [64 units][128 k] in 2, each as a hi and a lo image
-  static constexpr uint32_t IMG_W1_HI = 0, IMG_W1_LO = 49152, IMG_W2_HI = 98304, IMG_W2_LO = 114688;
-  static constexpr uint32_t IMG_BYTES = TC_MLP ? 131072 : 0;
+  static constexpr uint32_t AU_BYTES = kWgGroups * WG_BYTES;
+  // top-MLP operand images (TC_MLP, written by model.cu::build_din_wg): W1^T [128 units][160 k] as k 0..127
+  // in 2 K blocks, a hi and a lo image, then one tail K block whose 128-byte rows are [hi k 128..159 |
+  // lo k 128..159]; W2^T [64 units][128 k] in 2 K blocks, a hi and a lo image
+  static constexpr uint32_t IMG_W1_HI = 0, IMG_W1_LO = 32768, IMG_W1_TAIL = 65536;
+  static constexpr uint32_t IMG_W2_HI = 81920, IMG_W2_LO = 98304;
+  static constexpr uint32_t IMG_BYTES = TC_MLP ? 114688 : 0;
+  static_assert(!TC_MLP || (IMG_W1_TAIL == 2 * 16384 * 2 && IMG_W2_HI == IMG_W1_TAIL + 16384 &&
+                            IMG_BYTES == IMG_W2_LO + 2 * 8192), "top-MLP image layout");
   // X operand [32 rows hi | 32 rows lo][160 k] (3 K blocks), then the H1 operand [.. ][128 k] (2 K blocks):
   // both over the history tiles, which are free once the tile's activation unit is done
   static constexpr uint32_t OP_KB_BYTES = 2 * kWgRows * 128;
@@ -63,7 +73,7 @@ struct DinWgLayout {
   static constexpr int F_CST = F_WC + EP * 32;                // [32 rows][32 units] activation-unit constants
   static constexpr int F_WG = F_CST + kWgRows * 32;           // per warpgroup: w[64] | part[128]
   static constexpr int F_WG_STRIDE = kWgPos + 128;
-  static constexpr int F_RED = F_WG + 2 * F_WG_STRIDE;        // [4 warps][32 rows] Dense(1) partial sums
+  static constexpr int F_RED = F_WG + kWgGroups * F_WG_STRIDE;  // [4 warps][32 rows] Dense(1) partial sums
   static constexpr int F_END = F_RED + 4 * kWgRows;
   static constexpr size_t SMEM = 1024 + AU_BYTES + IMG_BYTES + (size_t)F_END * sizeof(float);
   static_assert(SMEM <= 227 * 1024, "one CTA per SM must fit");
@@ -83,11 +93,12 @@ __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& 
                                            uint8_t* ops, const uint8_t* img, float* red, uint64_t* wbar) {
   using L = DinWgLayout<EP>;
   constexpr int KE = 5 * EP;                       // embedding columns of the tile: the MMAs' K
+  static_assert(KE == 160, "W1 image: two full K blocks and a 32-wide tail");
   constexpr uint32_t KBB = L::OP_KB_BYTES, LO = kWgRows * 128;   // operand K block; lo rows follow the hi rows
   const int tid = threadIdx.x, q = tid >> 7, tw = tid & 127;
   const int warp = tw >> 5, lane = tw & 31, g = lane >> 2, cq = lane & 3;
   // X operand: tile columns 0 .. KE - 1 split to bf16 hi (operand rows 0..31) and lo (rows 32..63)
-  for (int i = tid; i < kWgRows * KE / 2; i += kThreads) {
+  for (int i = tid; i < kWgRows * KE / 2; i += kWgThreads) {
     const int r = i / (KE / 2), k = 2 * (i % (KE / 2));
     const float2 v = *reinterpret_cast<const float2*>(Xs + r * L::LDX + k);
     const Split2 s = split_pack(v.x, v.y);
@@ -100,32 +111,35 @@ __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& 
   if (wbar) mbar_wait(wbar, 0);
   const uint32_t s_img = smem_u32(img), s_op = smem_u32(ops);
 
-  // ---- Dense(128) + PReLU: warpgroup q owns units 64 q .. 64 q + 63; D[64 units x (32 rows hi | 32 rows lo)]
+  // ---- Dense(128) + PReLU: warpgroups 0 and 1, warpgroup q owns units 64 q .. 64 q + 63;
+  // D[64 units x (32 rows hi | 32 rows lo)]
   {
     float d[32];
   #pragma unroll
     for (int i = 0; i < 32; ++i) d[i] = 0.f;
-    mma_fence();
-  #pragma unroll
-    for (int kb = 0; kb < (KE + 63) / 64; ++kb) {
-      const uint64_t ah = desc_sw128(s_img + L::IMG_W1_HI + kb * 16384 + q * 8192);
-      const uint64_t al = desc_sw128(s_img + L::IMG_W1_LO + kb * 16384 + q * 8192);
-      const uint64_t xs = desc_sw128(s_op + kb * KBB);
-  #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        if (64 * kb + 16 * ks < KE) {              // the third K block is half used
+    if (q < 2) {
+      mma_fence();
+    #pragma unroll
+      for (int kb = 0; kb < 3; ++kb) {
+        // k 0..127: hi and lo images; k 128..159: the tail block, hi at K byte 0 and lo at K byte 64 of its rows
+        const uint64_t ah = kb < 2 ? desc_sw128(s_img + L::IMG_W1_HI + kb * 16384 + q * 8192)
+                                   : desc_sw128(s_img + L::IMG_W1_TAIL + q * 8192);
+        const uint64_t al = kb < 2 ? desc_sw128(s_img + L::IMG_W1_LO + kb * 16384 + q * 8192) : ah + 4;
+        const uint64_t xs = desc_sw128(s_op + kb * KBB);
+    #pragma unroll
+        for (int ks = 0; ks < (kb < 2 ? 4 : 2); ++ks) {
           mma_m64n64_ss(d, ah + 2 * ks, xs + 2 * ks, kb > 0 || ks > 0);
           mma_m64n64_ss(d, al + 2 * ks, xs + 2 * ks, 1);
         }
       }
+      mma_commit();
+      mma_wait<0>();
+      reg_fence(d);
     }
-    mma_commit();
-    mma_wait<0>();
-    reg_fence(d);
     __syncthreads();                               // both warpgroups' MMAs have read X: H1 goes over it
     // epilogue: units u = 64 q + 16 warp + g + 8 i, tile rows r = 8 j + 2 cq + c (hi: column r, lo: 32 + r)
   #pragma unroll
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < 2 * (q < 2); ++i) {
       const int u = 64 * q + 16 * warp + g + 8 * i;
       const float bias = __ldg(p.b1 + u), slope = __ldg(p.a1 + u);
       float wn[kNumNumerics];
@@ -210,7 +224,7 @@ __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& 
 }
 
 template <int EP>
-__global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchView b) {
+__global__ void __launch_bounds__(kWgThreads, 1) din_wg_kernel(DinParams p, BatchView b) {
   using L = DinWgLayout<EP>;
   constexpr int KB = L::KB;
   constexpr int KS = EP / 16;                     // K steps per part (hi or lo)
@@ -246,20 +260,24 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
       mbar_init(&wbar, 1);
       fence_mbar_init();
       mbar_arrive_expect_tx(&wbar, L::IMG_BYTES);
-      for (uint32_t off = 0; off < L::IMG_BYTES; off += 32768u) bulk_g2s(img + off, p.mlp_image + off, 32768u, &wbar);
+      for (uint32_t off = 0; off < L::IMG_BYTES; off += 32768u)
+        bulk_g2s(img + off, p.mlp_image + off, min(32768u, L::IMG_BYTES - off), &wbar);
     }
   }
-  stage_weights(fs + L::F_WH, p.au_wh, EP * 32);
-  stage_weights(fs + L::F_WP, p.au_wp, EP * 32);
-  stage_weights(fs + L::F_WC, p.au_wc, EP * 32);
+  if (tid < kThreads) {                           // the shared tile helpers map kThreads threads
+    stage_weights(fs + L::F_WH, p.au_wh, EP * 32);
+    stage_weights(fs + L::F_WP, p.au_wp, EP * 32);
+    stage_weights(fs + L::F_WC, p.au_wc, EP * 32);
+  }
   // persistent over the batch's 32-row tiles: one tile per CTA unless srs_model_set_sm_limit caps the grid
   const int n_tiles = (b.B + kWgRows - 1) / kWgRows;
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int row0 = tile * kWgRows;
-    tile_side_features<EP, kWgRows>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users, p.n_genres,
-                                    OFF_UG, OFF_U, OFF_MG, OFF_NUM);
+    if (tid < kThreads)
+      tile_side_features<EP, kWgRows>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users, p.n_genres,
+                                      OFF_UG, OFF_U, OFF_MG, OFF_NUM);
     // candidate rows of the tile (ids pass through float32, DIN.py:95,125); rows past the batch end are zero
-    for (int i = tid; i < kWgRows * EP / 4; i += kThreads) {
+    for (int i = tid; i < kWgRows * EP / 4; i += kWgThreads) {
       const int r = i / (EP / 4), c4 = i % (EP / 4), row = row0 + r;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
       if (row < b.B) {
@@ -273,7 +291,7 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
     stage_wait();
     __syncthreads();
     // activation-unit constant of every row: cst[r][j] = au_b[j] + sum_e c_r[e] (Wc - Wsub)[e][j]
-    for (int i = tid; i < kWgRows * 32; i += kThreads) {
+    for (int i = tid; i < kWgRows * 32; i += kWgThreads) {
       const int r = i >> 5, j = i & 31;
       const float* cv = Xs + r * L::LDX + OFF_C;
       float acc = __ldg(p.au_b + j);
@@ -283,9 +301,9 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
     }
     __syncthreads();
     clk.lap(PH_TILE_INPUTS);
-    // rows of this warpgroup: q, q + 2, ...; the valid ones are a prefix
+    // rows of this warpgroup: q, q + kWgGroups, ...; the valid ones are a prefix
     int nrows = 0;
-    for (int r = q; r < kWgRows; r += 2)
+    for (int r = q; r < kWgRows; r += kWgGroups)
       if (row0 + r < b.B) ++nrows;
 
     // gate constants of this thread's 8 accumulator columns 8 j + 2 cq + c
@@ -301,7 +319,7 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
     // position, never from the id value: every live id goes through the range check.
     auto item_nt = [&](int k) { return k < n_items ? min(kWgPos, T - (k % nch) * kWgPos) : 0; };
     auto load_ids = [&](int k, int (&ids)[NCOPY]) {
-      const int row = row0 + q + 2 * (k / nch), t0 = (k % nch) * kWgPos, nt = item_nt(k);
+      const int row = row0 + q + kWgGroups * (k / nch), t0 = (k % nch) * kWgPos, nt = item_nt(k);
       const int32_t* hrow = b.hist + (size_t)row * b.hist_stride + t0;
   #pragma unroll
       for (int n = 0; n < NCOPY; ++n) {
@@ -334,7 +352,7 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
     float pool_acc = 0.f;
     float slope[2][8], cstv[8];
     for (int k = 0; k < n_items; ++k) {
-      const int r = q + 2 * (k / nch), ch = k % nch, t0 = ch * kWgPos;
+      const int r = q + kWgGroups * (k / nch), ch = k % nch, t0 = ch * kWgPos;
       const int nt = min(kWgPos, T - t0);
       float* xrow = Xs + r * L::LDX;
       const float* cst = cst_all + r * 32;
@@ -453,11 +471,11 @@ __global__ void __launch_bounds__(kThreads, 1) din_wg_kernel(DinParams p, BatchV
       top_mlp_wg<EP>(p, b, row0, Xs, base, img, fs + L::F_RED, weights_ready ? nullptr : &wbar);
       weights_ready = true;
     } else {
-      dense_layer<kWgRows, 128, 2, 8>(Xs, L::LDX, L::KP, p.W1, p.b1, ACT_PRELU, p.a1, H1, L::LDH1);
+      if (tid < kThreads) dense_layer<kWgRows, 128, 2, 8>(Xs, L::LDX, L::KP, p.W1, p.b1, ACT_PRELU, p.a1, H1, L::LDH1);
       __syncthreads();
-      dense_layer<kWgRows, 64, 1, 8>(H1, L::LDH1, 128, p.W2, p.b2, ACT_PRELU, p.a2, H2, L::LDH2);
+      if (tid < kThreads) dense_layer<kWgRows, 64, 1, 8>(H1, L::LDH1, 128, p.W2, p.b2, ACT_PRELU, p.a2, H2, L::LDH2);
       __syncthreads();
-      row_dot<kWgRows>(H2, L::LDH2, 64, p.w3, [&](int r, float s) {
+      if (tid < kThreads) row_dot<kWgRows>(H2, L::LDH2, 64, p.w3, [&](int r, float s) {
         const int row = row0 + r;
         if (row >= b.B) return;
         const float z = s + p.b3;
@@ -501,8 +519,8 @@ cudaError_t launch_din_wg(const DinParams& p, const BatchView& b, cudaStream_t s
   const int n_tiles = (b.B + kWgRows - 1) / kWgRows;
   const int blocks = p.max_ctas > 0 && p.max_ctas < n_tiles ? p.max_ctas : n_tiles;
   ++g_launch_count;
-  if (p.EP == 32) din_wg_kernel<32><<<blocks, kThreads, DinWgLayout<32>::SMEM, s>>>(p, b);
-  else if (p.EP == 64) din_wg_kernel<64><<<blocks, kThreads, DinWgLayout<64>::SMEM, s>>>(p, b);
+  if (p.EP == 32) din_wg_kernel<32><<<blocks, kWgThreads, DinWgLayout<32>::SMEM, s>>>(p, b);
+  else if (p.EP == 64) din_wg_kernel<64><<<blocks, kWgThreads, DinWgLayout<64>::SMEM, s>>>(p, b);
   else return cudaErrorInvalidValue;
   return cudaGetLastError();
 }

@@ -787,18 +787,21 @@ inline uint16_t bf16_rn_bits(float x) {
 }
 inline uint32_t sw128_off(uint32_t row, uint32_t chunk) { return row * 128u + ((chunk ^ (row & 7u)) << 4); }
 
-// Write logical matrix M[rows][64*kblocks] (via getter) as K-major SW128 bf16 tiles; `part`
-// selects the hi half (x rounded to bf16) or the lo half (x - hi rounded to bf16).
+// Write logical matrix M[rows][k0 + 64*kblocks] (via getter) from column k0 on as K-major SW128 bf16
+// tiles; `part` selects the hi half (x rounded to bf16) or the lo half (x - hi rounded to bf16).  With
+// `chunks` < 8 only that many 16-byte chunks (8 k each) of every 128-byte row are written, from chunk
+// `chunk0` on: a 32-wide K tail at bytes 0..63 or 64..127 of a K block.
 template <class F>
-void write_sw128(uint8_t* dst, int rows, int kblocks, bool lo_part, F get) {
+void write_sw128(uint8_t* dst, int rows, int kblocks, bool lo_part, F get, int k0 = 0, int chunk0 = 0,
+                 int chunks = 8) {
   for (int kb = 0; kb < kblocks; ++kb)
     for (int r = 0; r < rows; ++r)
-      for (int c = 0; c < 8; ++c)
+      for (int c = 0; c < chunks; ++c)
         for (int i = 0; i < 8; ++i) {
-          const float x = get(r, kb * 64 + c * 8 + i);
+          const float x = get(r, k0 + kb * 64 + c * 8 + i);
           const uint16_t hb = bf16_rn_bits(x);
           const uint16_t v = lo_part ? bf16_rn_bits(x - u2f((uint32_t)hb << 16)) : hb;
-          memcpy(dst + (size_t)kb * rows * 128 + sw128_off(r, c) + i * 2, &v, 2);
+          memcpy(dst + (size_t)kb * rows * 128 + sw128_off(r, chunk0 + c) + i * 2, &v, 2);
         }
 }
 
@@ -808,18 +811,21 @@ int build_din_wg(Builder& B) {
   srs_model* m = B.m;
   DinParams& p = m->din;
   if (m->EP == 32) {
-    // W1^T over the 160 embedding columns of the tile (K blocks 64 | 64 | 32 + zeros), W2^T; units are the
-    // MMA rows, zero-padded to 128 / 64 like the permuted fp32 weights build_din uploaded
-    constexpr int KE = 5 * 32;
-    const std::vector<float>& w1 = B.din_w1;     // [KE + 8][128]
+    // W1^T over the 160 embedding columns of the tile: K blocks 0..63 and 64..127 as a hi and a lo image, then
+    // one tail block whose rows are [hi k 128..159 | lo k 128..159]; W2^T as a hi and a lo image.  Units are
+    // the MMA rows, zero-padded to 128 / 64 like the permuted fp32 weights build_din uploaded.  Offsets:
+    // din_wg.cu::DinWgLayout::IMG_*
+    const std::vector<float>& w1 = B.din_w1;     // [5 * 32 + 8][128]
     const std::vector<float>& w2 = B.din_w2;     // [128][64]
-    auto w1_get = [&](int u, int k) -> float { return k < KE ? w1[(size_t)k * 128 + u] : 0.f; };
+    auto w1_get = [&](int u, int k) -> float { return w1[(size_t)k * 128 + u]; };
     auto w2_get = [&](int u, int k) -> float { return w2[(size_t)k * 64 + u]; };
-    std::vector<uint8_t> img(131072, 0);
-    write_sw128(img.data() + 0, 128, 3, false, w1_get);
-    write_sw128(img.data() + 49152, 128, 3, true, w1_get);
-    write_sw128(img.data() + 98304, 64, 2, false, w2_get);
-    write_sw128(img.data() + 114688, 64, 2, true, w2_get);
+    std::vector<uint8_t> img(114688, 0);
+    write_sw128(img.data() + 0, 128, 2, false, w1_get);
+    write_sw128(img.data() + 32768, 128, 2, true, w1_get);
+    write_sw128(img.data() + 65536, 128, 1, false, w1_get, 128, 0, 4);
+    write_sw128(img.data() + 65536, 128, 1, true, w1_get, 128, 4, 4);
+    write_sw128(img.data() + 81920, 64, 2, false, w2_get);
+    write_sw128(img.data() + 98304, 64, 2, true, w2_get);
     p.mlp_image = B.upload(img);
     if (B.status != SRS_OK) return B.status;
   }
