@@ -446,6 +446,42 @@ int64_t srs_trainer_iterations(const srs_trainer* tr);
 int srs_selftest_wgmma(const float* A, const float* B, float* D, int32_t N, int32_t k_blocks,
                        int32_t a_in_regs, int32_t device);
 
+/* ---- Sample building: FeatureEngForRecModel.scala:21-130 on the device (DESIGN.md section 4.11) ----
+ * Every output column has capacity n_ratings rows (user_rated_movie, user_genre: [n_ratings][5], movie_genre:
+ * [n_ratings][3]); the first *n_kept rows are written, in input (file) order.  `row` is each kept row's index in
+ * the input, so userId, movieId, rating and timestamp are the caller's own.  Genre columns hold word indices,
+ * -1 = none; user_rated_movie 0 = none.  The two-decimal columns hold the float32 nearest format_number's text. */
+typedef struct srs_samples {
+  int32_t* row;
+  int32_t* label;                     /* rating >= 3.5 */
+  int32_t* release_year;
+  int32_t* movie_genre;               /* [3] movieGenre1..3 */
+  int32_t* movie_rating_count;
+  float* movie_avg_rating;
+  float* movie_rating_stddev;
+  int32_t* user_rated_movie;          /* [5] the window's positive movies, most recent first */
+  int32_t* user_rating_count;         /* > 1 on every kept row */
+  float* user_avg_release_year;       /* integral: the average truncated */
+  float* user_release_year_stddev;
+  float* user_avg_rating;
+  float* user_rating_stddev;
+  int32_t* user_genre;                /* [5] by descending count, ties in the reference's hash-map order */
+} srs_samples;
+
+/* The samples of n_ratings ratings (host arrays): user_id >= 0, movie_id in [0, n_movie_slots), half = rating in
+ * half-stars (1..10), timestamp > 0 (int32 seconds; ordered as its decimal string, as the reference orders it).
+ * Per movie id (host, n_movie_slots rows): movie_year (the title rule's year, in -999..9999; 1990 for a movie
+ * missing from movies.csv) and movie_genres [n_movie_slots][genres_per_movie], the movie's genre word indices in
+ * string order, then -1.  genre_hash [n_genres]: java.lang.String.hashCode of each genre word (the reference's
+ * genre counting runs in a Scala hash map, whose order breaks count ties).  Bounds: n_ratings <= 21 000 000,
+ * n_movie_slots <= 2^24, genres_per_movie 1..24, n_genres 0..24.  Every input is checked before any device call;
+ * a violation gives SRS_ERR_INVALID.  The inputs are uploaded once and the job runs on `device` with no host round
+ * trip; synchronous.  The same inputs give the same bits. */
+int srs_featureeng_host(const int32_t* user_id, const int32_t* movie_id, const int8_t* half, const int32_t* timestamp,
+                        int64_t n_ratings, const int32_t* movie_year, const int32_t* movie_genres,
+                        int32_t n_movie_slots, int32_t genres_per_movie, const int32_t* genre_hash, int32_t n_genres,
+                        int32_t device, srs_samples* out, int64_t* n_kept);
+
 #ifdef __cplusplus
 }
 #endif

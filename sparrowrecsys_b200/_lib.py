@@ -46,7 +46,8 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_metrics_update_device", "srs_metrics_result", "srs_evaluate_host_batches",
            "srs_dien_outputs_device", "srs_dien_outputs_host_batches", "srs_dien_evaluate_host_batches",
            "srs_trainer_create", "srs_trainer_destroy", "srs_trainer_fit_host", "srs_trainer_get_weights",
-           "srs_trainer_iterations", "srs_trainer_fit_validate_host", "srs_trainer_evaluate_host")
+           "srs_trainer_iterations", "srs_trainer_fit_validate_host", "srs_trainer_evaluate_host",
+           "srs_featureeng_host")
 
 _lib = None
 
@@ -72,6 +73,14 @@ class SrsDienEvalResult(C.Structure):
 class SrsAdam(C.Structure):
     """`srs_adam` (include/srs_ctr.h): Keras Adam's hyper-parameters."""
     _fields_ = [("lr", C.c_float), ("beta_1", C.c_float), ("beta_2", C.c_float), ("epsilon", C.c_float)]
+
+
+class SrsSamples(C.Structure):
+    """`srs_samples` (include/srs_ctr.h): the output columns of srs_featureeng_host."""
+    _fields_ = [(name, C.c_void_p) for name in (
+        "row", "label", "release_year", "movie_genre", "movie_rating_count", "movie_avg_rating",
+        "movie_rating_stddev", "user_rated_movie", "user_rating_count", "user_avg_release_year",
+        "user_release_year_stddev", "user_avg_rating", "user_rating_stddev", "user_genre")]
 
 
 class SrsError(RuntimeError):
@@ -211,6 +220,10 @@ def load():
                                                   C.c_void_p, C.c_int32, C.POINTER(SrsEvalResult)]
     lib.srs_trainer_evaluate_host.restype = C.c_int
     lib.srs_trainer_evaluate_host.argtypes = [C.c_void_p, C.POINTER(SrsBatch), C.c_void_p, C.POINTER(SrsEvalResult)]
+    lib.srs_featureeng_host.restype = C.c_int
+    lib.srs_featureeng_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                        C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
+                                        C.POINTER(SrsSamples), C.POINTER(C.c_int64)]
     if lib.srs_abi_version() != ABI_VERSION:
         raise ImportError("libsrs_ctr.so ABI version %d != %d" % (lib.srs_abi_version(), ABI_VERSION))
     _lib = lib
