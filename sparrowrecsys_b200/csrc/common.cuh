@@ -84,6 +84,7 @@ enum DinPhase {
   PH_AU_LOOP,           // CUDA-core kernel: activation unit + gate + pooling per position
   PH_ROW_IMBALANCE,     // waiting at the barrier before the top MLP
   PH_TOP_MLP,           // Dense(128) / Dense(64) / Dense(1) + sigmoid
+  PH_IMAGE_WAIT,        // waiting for the top-MLP weight image (din_wg_kernel, E <= 32)
   kDinPhases
 };
 #ifdef SRS_DIN_PHASES
@@ -240,10 +241,12 @@ __device__ __forceinline__ void dense_layer(const float* __restrict__ xs, int ld
 
 // Asynchronous global -> shared copy of a dense weight array (floats multiple of 4, 16-byte
 // aligned both sides) by the whole CTA: the per-K-step L2 latency of reading weights in place
-// becomes one bulk latency that overlaps the embedding gathers.  Pair with stage_wait().
+// becomes one bulk latency that overlaps the embedding gathers.  Pair with stage_wait().  NT: the
+// CTA's thread count.
+template <int NT = kThreads>
 __device__ __forceinline__ void stage_weights(float* dst_smem, const float* __restrict__ src, int n_floats) {
   const uint32_t dst = static_cast<uint32_t>(__cvta_generic_to_shared(dst_smem));
-  for (int i = threadIdx.x * 4; i < n_floats; i += kThreads * 4)
+  for (int i = threadIdx.x * 4; i < n_floats; i += NT * 4)
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst + i * 4), "l"(src + i) : "memory");
 }
 __device__ __forceinline__ void stage_wait() {
@@ -277,15 +280,15 @@ __device__ __forceinline__ void gather_row(float* dst, const float* __restrict__
 // userId and movieGenre1 embedding rows (DenseFeatures columns of the user-profile / context
 // layers, e.g. DIN.py:108-123) land at tile columns off_ug / off_u / off_mg, the 7 numerics
 // (+ one zero pad) at off_num.  Rows past the batch end and missing / OOV genres (-1) are zero;
-// an id outside its vocabulary latches the error flag.
-template <int EP, int R>
+// an id outside its vocabulary latches the error flag.  NT: the CTA's thread count.
+template <int EP, int R, int NT = kThreads>
 __device__ __forceinline__ void tile_side_features(float* __restrict__ Xs, int ldx, int row0,
                                                    const BatchView& b, const float* user,
                                                    const float* ugenre, const float* mgenre,
                                                    int n_users, int n_genres, int off_ug, int off_u,
                                                    int off_mg, int off_num) {
   constexpr int Q = EP / 4;
-  for (int i = threadIdx.x; i < R * 3 * Q; i += kThreads) {
+  for (int i = threadIdx.x; i < R * 3 * Q; i += NT) {
     const int q = i % Q;
     const int t = i / Q;
     const int slot = t % 3;
@@ -306,7 +309,7 @@ __device__ __forceinline__ void tile_side_features(float* __restrict__ Xs, int l
     }
     gather_row<EP>(Xs + r * ldx + off, table, id, q);
   }
-  for (int i = threadIdx.x; i < R * kNumPad; i += kThreads) {
+  for (int i = threadIdx.x; i < R * kNumPad; i += NT) {
     const int r = i / kNumPad, j = i % kNumPad;
     const int row = row0 + r;
     float v = 0.f;

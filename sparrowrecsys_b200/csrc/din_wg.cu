@@ -17,20 +17,22 @@
 //   * pooling sum_t w_t h_t from the same shared-memory tile (h = hi + lo);
 //   * top MLP over the CTA's 32-row tile.  E <= 32: on wgmma, computed transposed like
 //     embmlp_tc.cu - D[units x rows] = W^T X^T with W1^T (the 160 embedding columns of the tile) and
-//     W2^T resident in shared memory as bf16 hi / lo images (one bulk copy per CTA), the tile's hi
-//     and lo halves stacked along N, the 7 raw-scale numerics added in fp32 in the layer-1
-//     epilogue, PReLU / Dense(1) / sigmoid on the accumulator registers.  E <= 64: on CUDA cores
-//     (common.cuh::dense_layer); its W1 image would be ~160 KB, and at cfg 5's T = 200 the
-//     activation unit dominates the tile.
+//     W2^T in shared memory as bf16 hi / lo images, the tile's hi and lo halves stacked along N, the
+//     7 raw-scale numerics added in fp32 in the layer-1 epilogue, PReLU / Dense(1) / sigmoid on the
+//     accumulator registers.  E <= 64: on CUDA cores (common.cuh::dense_layer); its W1 image would be
+//     ~160 KB, and at cfg 5's T = 200 the activation unit dominates the tile.
 //
-// CTA = 384 threads = three warpgroups, 32 batch rows; warpgroup q owns rows q, q + 3, ... and
-// double-buffers its history tiles (the next tile's cp.async runs under this tile's MMA and
-// epilogue; the ids of the tile after it are already on their way from HBM).  The per-row chain
-// is latency-bound, so a third warpgroup (12 warps per SM instead of 8) shortens each warpgroup's
-// walk from 16 rows to 11 without lengthening the chain.  The shared tile helpers
-// (tile_side_features, dense_layer, ...) map 256 threads; the third warpgroup skips them, and
-// only warpgroups 0 and 1 issue the top MLP's Dense(128).  Shared memory: ~213 KB with the MLP
-// images (E <= 32) / ~218 KB (E <= 64): one CTA per SM.
+// CTA = G warpgroups (DinWgLayout::G: 5 at E <= 32, 3 at E <= 64), 32 batch rows; warpgroup q owns rows
+// q, q + G, ... and double-buffers its history tiles (the next tile's cp.async runs under this tile's MMA
+// and epilogue; the ids of the tile after it are already on their way from HBM).  The per-row chain is
+// latency-bound, so more warpgroups shorten each warpgroup's walk (7 or 6 rows at G = 5) without
+// lengthening the chain.  At E <= 32 the 112 KB MLP image is not resident beside the warpgroups' buffers:
+// they share one region, the image at its bottom and the buffers at its top, and the image bytes under the
+// buffers are copied again in each tile once its activation unit is done (28 KB of W2^T at G = 5, in
+// flight under Dense(128)).  The shared tile helpers that map threads generically (tile_side_features,
+// stage_weights) use every warpgroup; dense_layer and row_dot (E <= 64) map 256 threads, and only
+// warpgroups 0 and 1 issue the top MLP's Dense(128).  Shared memory: ~227 KB (E <= 32) / ~218 KB
+// (E <= 64): one CTA per SM.
 #include "kernels.h"
 #include "wgmma.cuh"
 
@@ -39,17 +41,23 @@ using namespace wg;
 
 constexpr int kWgRows = 32;       // rows per CTA (top-MLP tile height, as din.cu)
 constexpr int kWgPos = 64;        // history positions per MMA tile
-constexpr int kWgGroups = 3;      // warpgroups per CTA: each walks every third row of the tile
-constexpr int kWgThreads = 128 * kWgGroups;
+// warpgroups per CTA at E <= 32 (DESIGN §6 has the measurements that chose 5; a build with
+// -DSRS_DIN_WG_GROUPS32=N measures another count)
+#ifndef SRS_DIN_WG_GROUPS32
+#define SRS_DIN_WG_GROUPS32 5
+#endif
 
 template <int EP>
 struct DinWgLayout {
   static constexpr bool TC_MLP = EP == 32;                    // top MLP on wgmma
+  // warpgroups per CTA: warpgroup q walks rows q, q + G, ... of the tile
+  static constexpr int G = TC_MLP ? SRS_DIN_WG_GROUPS32 : 3;
+  static constexpr int THREADS = 128 * G;
   static constexpr int KB = EP / 32;                          // 128-byte K blocks of a [hi | lo] row
   static constexpr uint32_t A_BYTES = KB * kWgPos * 128;      // one history tile
   static constexpr uint32_t B_BYTES = KB * 32 * 128;          // W_r, 32 unit rows
   static constexpr uint32_t WG_BYTES = 2 * A_BYTES + B_BYTES; // per warpgroup
-  static constexpr uint32_t AU_BYTES = kWgGroups * WG_BYTES;
+  static constexpr uint32_t AU_BYTES = G * WG_BYTES;
   // top-MLP operand images (TC_MLP, written by model.cu::build_din_wg): W1^T [128 units][160 k] as k 0..127
   // in 2 K blocks, a hi and a lo image, then one tail K block whose 128-byte rows are [hi k 128..159 |
   // lo k 128..159]; W2^T [64 units][128 k] in 2 K blocks, a hi and a lo image
@@ -58,10 +66,8 @@ struct DinWgLayout {
   static constexpr uint32_t IMG_BYTES = TC_MLP ? 114688 : 0;
   static_assert(!TC_MLP || (IMG_W1_TAIL == 2 * 16384 * 2 && IMG_W2_HI == IMG_W1_TAIL + 16384 &&
                             IMG_BYTES == IMG_W2_LO + 2 * 8192), "top-MLP image layout");
-  // X operand [32 rows hi | 32 rows lo][160 k] (3 K blocks), then the H1 operand [.. ][128 k] (2 K blocks):
-  // both over the history tiles, which are free once the tile's activation unit is done
+  // X operand [32 rows hi | 32 rows lo][160 k] (3 K blocks), then the H1 operand [.. ][128 k] (2 K blocks)
   static constexpr uint32_t OP_KB_BYTES = 2 * kWgRows * 128;
-  static_assert(!TC_MLP || 3 * OP_KB_BYTES <= AU_BYTES, "X operand must fit over the history tiles");
   static constexpr int KP = 5 * EP + kNumPad, LDX = KP + 4, LDH1 = 128 + 4, LDH2 = 64 + 4;
   // fp32 region behind the operand tiles and images
   static constexpr int F_X = 0;
@@ -73,10 +79,25 @@ struct DinWgLayout {
   static constexpr int F_CST = F_WC + EP * 32;                // [32 rows][32 units] activation-unit constants
   static constexpr int F_WG = F_CST + kWgRows * 32;           // per warpgroup: w[64] | part[128]
   static constexpr int F_WG_STRIDE = kWgPos + 128;
-  static constexpr int F_RED = F_WG + kWgGroups * F_WG_STRIDE;  // [4 warps][32 rows] Dense(1) partial sums
+  static constexpr int F_RED = F_WG + G * F_WG_STRIDE;        // [4 warps][32 rows] Dense(1) partial sums
   static constexpr int F_END = F_RED + 4 * kWgRows;
-  static constexpr size_t SMEM = 1024 + AU_BYTES + IMG_BYTES + (size_t)F_END * sizeof(float);
-  static_assert(SMEM <= 227 * 1024, "one CTA per SM must fit");
+  static constexpr uint32_t FS_BYTES = (uint32_t)F_END * sizeof(float);
+  // Byte region at the aligned base, in front of the fp32 region.  E <= 64: the warpgroups' history tiles and
+  // W_r.  E <= 32: every byte that one CTA per SM leaves (kSmemStatic: the static mbarriers), the image at its
+  // bottom and the warpgroups' buffers at its top, the X / H1 operand over the last of those.  The image bytes
+  // under the buffers (IMG_RELOAD) are copied again in every tile once its activation unit is done; the rest
+  // (IMG_RESIDENT) is copied once per CTA.
+  static constexpr uint32_t kSmemStatic = 64;
+  static constexpr uint32_t REGION = TC_MLP ? (227u * 1024 - 1024 - kSmemStatic - FS_BYTES) / 1024 * 1024 : AU_BYTES;
+  static constexpr uint32_t AU_OFF = REGION - AU_BYTES;         // warpgroup q's buffers at AU_OFF + q WG_BYTES
+  static constexpr uint32_t OPS_OFF = REGION - 3 * OP_KB_BYTES; // X / H1 operand
+  static constexpr uint32_t IMG_RESIDENT = AU_OFF < IMG_BYTES ? AU_OFF : IMG_BYTES;
+  static constexpr uint32_t IMG_RELOAD = IMG_BYTES - IMG_RESIDENT;
+  static constexpr bool RELOAD_IN_W2 = IMG_RESIDENT >= IMG_W2_HI;  // Dense(128) never waits for the reload
+  static_assert(REGION >= AU_BYTES && AU_OFF % 1024 == 0 && IMG_RESIDENT % 16 == 0, "buffer alignment");
+  static_assert(!TC_MLP || OPS_OFF >= IMG_BYTES, "the X / H1 operand must not overlap the image");
+  static constexpr size_t SMEM = 1024 + REGION + FS_BYTES;
+  static_assert(SMEM + kSmemStatic <= 227 * 1024, "one CTA per SM must fit");
 };
 
 // byte offset of K byte `kb` (hi part: 2 e, lo part: 2 (EP + e)) of operand row `row` in a tile of
@@ -86,11 +107,13 @@ __device__ __forceinline__ uint32_t wg_kbyte(uint32_t row, uint32_t kb, uint32_t
 }
 
 // Top MLP of a 32-row tile on wgmma (E <= 32).  Xs holds the fp32 input tile; the X and H1 operands go
-// over the history tiles at `ops`; `img` holds the W1^T / W2^T images, which have landed once `wbar` (if
-// not null) completes.  Ends with every score of the tile stored.
+// over the history tiles at `ops`; `img` holds the W1^T / W2^T images: the resident part has landed once
+// `res_bar` (if not null) completes, the reloaded part once `reload_bar` completes phase `parity`.  Ends
+// with every score of the tile stored.
 template <int EP>
 __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& b, int row0, const float* Xs,
-                                           uint8_t* ops, const uint8_t* img, float* red, uint64_t* wbar) {
+                                           uint8_t* ops, const uint8_t* img, float* red, uint64_t* res_bar,
+                                           uint64_t* reload_bar, uint32_t parity, PhaseClock& clk) {
   using L = DinWgLayout<EP>;
   constexpr int KE = 5 * EP;                       // embedding columns of the tile: the MMAs' K
   static_assert(KE == 160, "W1 image: two full K blocks and a 32-wide tail");
@@ -98,7 +121,7 @@ __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& 
   const int tid = threadIdx.x, q = tid >> 7, tw = tid & 127;
   const int warp = tw >> 5, lane = tw & 31, g = lane >> 2, cq = lane & 3;
   // X operand: tile columns 0 .. KE - 1 split to bf16 hi (operand rows 0..31) and lo (rows 32..63)
-  for (int i = tid; i < kWgRows * KE / 2; i += kWgThreads) {
+  for (int i = tid; i < kWgRows * KE / 2; i += L::THREADS) {
     const int r = i / (KE / 2), k = 2 * (i % (KE / 2));
     const float2 v = *reinterpret_cast<const float2*>(Xs + r * L::LDX + k);
     const Split2 s = split_pack(v.x, v.y);
@@ -108,7 +131,10 @@ __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& 
   }
   fence_async_smem();
   __syncthreads();
-  if (wbar) mbar_wait(wbar, 0);
+  clk.lap(PH_TOP_MLP);
+  if (res_bar) mbar_wait(res_bar, 0);
+  if (L::IMG_RELOAD > 0 && !L::RELOAD_IN_W2) mbar_wait(reload_bar, parity);
+  clk.lap(PH_IMAGE_WAIT);
   const uint32_t s_img = smem_u32(img), s_op = smem_u32(ops);
 
   // ---- Dense(128) + PReLU: warpgroups 0 and 1, warpgroup q owns units 64 q .. 64 q + 63;
@@ -167,6 +193,11 @@ __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& 
   }
   // ---- Dense(64) + PReLU, Dense(1), sigmoid: warpgroup 0, D[64 units x (32 rows hi | 32 rows lo)]
   if (q != 0) return;
+  if (L::IMG_RELOAD > 0 && L::RELOAD_IN_W2) {      // the reloaded part is W2's: it flew under Dense(128)
+    clk.lap(PH_TOP_MLP);
+    mbar_wait(reload_bar, parity);
+    clk.lap(PH_IMAGE_WAIT);
+  }
   float d[32];
   #pragma unroll
   for (int i = 0; i < 32; ++i) d[i] = 0.f;
@@ -224,8 +255,9 @@ __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& 
 }
 
 template <int EP>
-__global__ void __launch_bounds__(kWgThreads, 1) din_wg_kernel(DinParams p, BatchView b) {
+__global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(DinParams p, BatchView b) {
   using L = DinWgLayout<EP>;
+  constexpr int G = L::G, NT = L::THREADS;
   constexpr int KB = L::KB;
   constexpr int KS = EP / 16;                     // K steps per part (hi or lo)
   constexpr int CP = 8 * KB;                      // 16-byte chunks per split row
@@ -233,10 +265,10 @@ __global__ void __launch_bounds__(kWgThreads, 1) din_wg_kernel(DinParams p, Batc
   constexpr int PARTS = 128 / EP, PP = kWgPos / PARTS;
   constexpr int OFF_UG = 0, OFF_U = EP, OFF_POOL = 2 * EP, OFF_C = 3 * EP, OFF_MG = 4 * EP, OFF_NUM = 5 * EP;
   extern __shared__ uint8_t raw[];
-  __shared__ uint64_t wbar;                       // top-MLP images landed (TC_MLP)
+  __shared__ uint64_t res_bar, reload_bar;        // top-MLP image (TC_MLP): resident part / this tile's reload landed
   uint8_t* base = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
-  uint8_t* img = base + L::AU_BYTES;
-  float* fs = reinterpret_cast<float*>(base + L::AU_BYTES + L::IMG_BYTES);
+  uint8_t* img = base;
+  float* fs = reinterpret_cast<float*>(base + L::REGION);
   float* Xs = fs + L::F_X;
   float* H1 = fs + L::F_H1;
   float* H2 = fs + L::F_H2;
@@ -248,36 +280,35 @@ __global__ void __launch_bounds__(kWgThreads, 1) din_wg_kernel(DinParams p, Batc
   const int q = tid >> 7, tw = tid & 127;
   const int warp = tw >> 5, lane = tw & 31, g = lane >> 2, cq = lane & 3;
   const int T = p.T, nch = (T + kWgPos - 1) / kWgPos;
-  uint8_t* tiles = base + q * L::WG_BYTES;        // history tiles 0, 1 | W_r
+  uint8_t* tiles = base + L::AU_OFF + q * L::WG_BYTES;   // history tiles 0, 1 | W_r
   uint8_t* Bt = tiles + 2 * L::A_BYTES;
   float* wsm = fs + L::F_WG + q * L::F_WG_STRIDE;
   float* part = wsm + kWgPos;
   PhaseClock clk(tw == 0);
 
   bool weights_ready = !L::TC_MLP;
+  uint32_t reload_parity = 0;
   if constexpr (L::TC_MLP) {
     if (tid == 0) {                               // visible to the waiters through the tile loop's first barrier
-      mbar_init(&wbar, 1);
+      mbar_init(&res_bar, 1);
+      mbar_init(&reload_bar, 1);
       fence_mbar_init();
-      mbar_arrive_expect_tx(&wbar, L::IMG_BYTES);
-      for (uint32_t off = 0; off < L::IMG_BYTES; off += 32768u)
-        bulk_g2s(img + off, p.mlp_image + off, min(32768u, L::IMG_BYTES - off), &wbar);
+      mbar_arrive_expect_tx(&res_bar, L::IMG_RESIDENT);
+      for (uint32_t off = 0; off < L::IMG_RESIDENT; off += 32768u)
+        bulk_g2s(img + off, p.mlp_image + off, min(32768u, L::IMG_RESIDENT - off), &res_bar);
     }
   }
-  if (tid < kThreads) {                           // the shared tile helpers map kThreads threads
-    stage_weights(fs + L::F_WH, p.au_wh, EP * 32);
-    stage_weights(fs + L::F_WP, p.au_wp, EP * 32);
-    stage_weights(fs + L::F_WC, p.au_wc, EP * 32);
-  }
+  stage_weights<NT>(fs + L::F_WH, p.au_wh, EP * 32);
+  stage_weights<NT>(fs + L::F_WP, p.au_wp, EP * 32);
+  stage_weights<NT>(fs + L::F_WC, p.au_wc, EP * 32);
   // persistent over the batch's 32-row tiles: one tile per CTA unless srs_model_set_sm_limit caps the grid
   const int n_tiles = (b.B + kWgRows - 1) / kWgRows;
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int row0 = tile * kWgRows;
-    if (tid < kThreads)
-      tile_side_features<EP, kWgRows>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users, p.n_genres,
-                                      OFF_UG, OFF_U, OFF_MG, OFF_NUM);
+    tile_side_features<EP, kWgRows, NT>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users, p.n_genres,
+                                        OFF_UG, OFF_U, OFF_MG, OFF_NUM);
     // candidate rows of the tile (ids pass through float32, DIN.py:95,125); rows past the batch end are zero
-    for (int i = tid; i < kWgRows * EP / 4; i += kWgThreads) {
+    for (int i = tid; i < kWgRows * EP / 4; i += NT) {
       const int r = i / (EP / 4), c4 = i % (EP / 4), row = row0 + r;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
       if (row < b.B) {
@@ -291,7 +322,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) din_wg_kernel(DinParams p, Batc
     stage_wait();
     __syncthreads();
     // activation-unit constant of every row: cst[r][j] = au_b[j] + sum_e c_r[e] (Wc - Wsub)[e][j]
-    for (int i = tid; i < kWgRows * 32; i += kWgThreads) {
+    for (int i = tid; i < kWgRows * 32; i += NT) {
       const int r = i >> 5, j = i & 31;
       const float* cv = Xs + r * L::LDX + OFF_C;
       float acc = __ldg(p.au_b + j);
@@ -301,9 +332,9 @@ __global__ void __launch_bounds__(kWgThreads, 1) din_wg_kernel(DinParams p, Batc
     }
     __syncthreads();
     clk.lap(PH_TILE_INPUTS);
-    // rows of this warpgroup: q, q + kWgGroups, ...; the valid ones are a prefix
+    // rows of this warpgroup: q, q + G, ...; the valid ones are a prefix
     int nrows = 0;
-    for (int r = q; r < kWgRows; r += kWgGroups)
+    for (int r = q; r < kWgRows; r += G)
       if (row0 + r < b.B) ++nrows;
 
     // gate constants of this thread's 8 accumulator columns 8 j + 2 cq + c
@@ -319,7 +350,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) din_wg_kernel(DinParams p, Batc
     // position, never from the id value: every live id goes through the range check.
     auto item_nt = [&](int k) { return k < n_items ? min(kWgPos, T - (k % nch) * kWgPos) : 0; };
     auto load_ids = [&](int k, int (&ids)[NCOPY]) {
-      const int row = row0 + q + kWgGroups * (k / nch), t0 = (k % nch) * kWgPos, nt = item_nt(k);
+      const int row = row0 + q + G * (k / nch), t0 = (k % nch) * kWgPos, nt = item_nt(k);
       const int32_t* hrow = b.hist + (size_t)row * b.hist_stride + t0;
   #pragma unroll
       for (int n = 0; n < NCOPY; ++n) {
@@ -352,7 +383,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) din_wg_kernel(DinParams p, Batc
     float pool_acc = 0.f;
     float slope[2][8], cstv[8];
     for (int k = 0; k < n_items; ++k) {
-      const int r = q + kWgGroups * (k / nch), ch = k % nch, t0 = ch * kWgPos;
+      const int r = q + G * (k / nch), ch = k % nch, t0 = ch * kWgPos;
       const int nt = min(kWgPos, T - t0);
       float* xrow = Xs + r * L::LDX;
       const float* cst = cst_all + r * 32;
@@ -468,8 +499,18 @@ __global__ void __launch_bounds__(kWgThreads, 1) din_wg_kernel(DinParams p, Batc
 
     // ---- top MLP on the tile ----------------------------------------------------------
     if constexpr (L::TC_MLP) {
-      top_mlp_wg<EP>(p, b, row0, Xs, base, img, fs + L::F_RED, weights_ready ? nullptr : &wbar);
+      if (L::IMG_RELOAD > 0 && tid == 0) {
+        // every warpgroup is past its last wgmma and shared-memory access of the history tiles (the barrier
+        // above); the fence orders those before the bulk copy that writes the image's top over them
+        fence_async_smem();
+        mbar_arrive_expect_tx(&reload_bar, L::IMG_RELOAD);
+        for (uint32_t off = L::IMG_RESIDENT; off < L::IMG_BYTES; off += 32768u)
+          bulk_g2s(img + off, p.mlp_image + off, min(32768u, L::IMG_BYTES - off), &reload_bar);
+      }
+      top_mlp_wg<EP>(p, b, row0, Xs, base + L::OPS_OFF, img, fs + L::F_RED, weights_ready ? nullptr : &res_bar,
+                     &reload_bar, reload_parity, clk);
       weights_ready = true;
+      reload_parity ^= 1u;
     } else {
       if (tid < kThreads) dense_layer<kWgRows, 128, 2, 8>(Xs, L::LDX, L::KP, p.W1, p.b1, ACT_PRELU, p.a1, H1, L::LDH1);
       __syncthreads();
@@ -486,7 +527,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) din_wg_kernel(DinParams p, Batc
     __syncthreads();                              // the next tile reuses every buffer
     clk.lap(PH_TOP_MLP);
   }
-  if (!weights_ready) mbar_wait(&wbar, 0);        // no bulk copy may outlive the CTA
+  // no bulk copy may outlive the CTA: each tile waited for its reload, and the first for the resident part
+  // (the grid never exceeds the tile count, so every CTA has a tile)
   gather_signal_tail(b);                          // spanning ranking call: publish "slice complete"
 }
 
@@ -519,8 +561,8 @@ cudaError_t launch_din_wg(const DinParams& p, const BatchView& b, cudaStream_t s
   const int n_tiles = (b.B + kWgRows - 1) / kWgRows;
   const int blocks = p.max_ctas > 0 && p.max_ctas < n_tiles ? p.max_ctas : n_tiles;
   ++g_launch_count;
-  if (p.EP == 32) din_wg_kernel<32><<<blocks, kWgThreads, DinWgLayout<32>::SMEM, s>>>(p, b);
-  else if (p.EP == 64) din_wg_kernel<64><<<blocks, kWgThreads, DinWgLayout<64>::SMEM, s>>>(p, b);
+  if (p.EP == 32) din_wg_kernel<32><<<blocks, DinWgLayout<32>::THREADS, DinWgLayout<32>::SMEM, s>>>(p, b);
+  else if (p.EP == 64) din_wg_kernel<64><<<blocks, DinWgLayout<64>::THREADS, DinWgLayout<64>::SMEM, s>>>(p, b);
   else return cudaErrorInvalidValue;
   return cudaGetLastError();
 }

@@ -22,7 +22,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 PHASES = ["tile inputs", "W_r / folded column", "gather issue", "gather wait", "AU MMA", "gate", "pooling",
-          "AU position loop", "row imbalance", "top MLP"]
+          "AU position loop", "row imbalance", "top MLP", "image wait"]
 IMPLS = (("tc", "din_wg_kernel"), ("cudacore", "din_kernel"))
 
 
