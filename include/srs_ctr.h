@@ -482,6 +482,44 @@ int srs_featureeng_host(const int32_t* user_id, const int32_t* movie_id, const i
                         int32_t n_movie_slots, int32_t genres_per_movie, const int32_t* genre_hash, int32_t n_genres,
                         int32_t device, srs_samples* out, int64_t* n_kept);
 
+/* ---- Embeddings: Embedding.scala:27-138 on the device (DESIGN.md section 4.12) ----
+ * srs_item2vec_host is Spark MLlib's Word2Vec.fit over each user's positive ratings: a hierarchical-softmax
+ * skip-gram trained by SGD, minCount 5, learning rate 0.025, sentences cut at 1000 words.  The ratings are host
+ * arrays as srs_featureeng_host takes them: user_id >= 0, movie_id in [0, 2^24), half = rating in half-stars
+ * (1..10), timestamp > 0; n_ratings <= 21 000 000.  A sentence is one user's movies rated >= 3.5 (users ascending),
+ * ordered by the timestamp's decimal string with ties in input order.  Each of `partitions` partitions trains
+ * sentences i = p, p + P, ... on its own copy of the tables; at the end of an iteration each row modified by one or
+ * more partitions becomes their rows' sum in partition order times 1.0f / count (partitions = 1: the reference's
+ * run).  Random numbers come from a counter-based generator keyed by `seed`.  Every sum has a fixed order and
+ * there are no float atomics: the same inputs give the same bits.
+ * Output: *vocab_size = V, vocab_ids [V] (movie ids by positive count descending, ties by id ascending) and
+ * vectors [V][vector_size]; `capacity` is the room in both, and V is at most the number of distinct movie ids rated
+ * >= 3.5.  Every input is checked before any device call (SRS_ERR_INVALID).  A vocabulary that is empty
+ * (SRS_ERR_INVALID, as Spark's require), larger than `capacity` (SRS_ERR_RANGE) or with a Huffman code longer
+ * than 32 (SRS_ERR_INVALID) is reported after the counting step, with nothing written.  Synchronous. */
+typedef struct srs_item2vec_params {
+  int32_t vector_size;                /* 1..64 (the reference: 10) */
+  int32_t window;                     /* 1..65536 (the reference: 5) */
+  int32_t iterations;                 /* 1..100000 (the reference: 10) */
+  int32_t partitions;                 /* 1..65536 (the reference: 1) */
+  uint64_t seed;
+} srs_item2vec_params;
+int srs_item2vec_host(const int32_t* user_id, const int32_t* movie_id, const int8_t* half, const int32_t* timestamp,
+                      int64_t n_ratings, const srs_item2vec_params* params, int32_t device, int32_t capacity,
+                      int32_t* vocab_ids, float* vectors, int32_t* vocab_size);
+
+/* generateUserEmb (Embedding.scala:53-101) as the reference's shipped userEmb.csv was made: per user, the float32
+ * sum of the vectors of every movie the user rated (any rating) that has one, taken in reverse input order, with
+ * no division; a user with none gets a zero row.  Ratings: user_id >= 0, movie_id in [0, 2^24), n_ratings <=
+ * 21 000 000 (host).  Items: n_items distinct ids in [0, 2^24) and vectors [n_items][vector_size] (host),
+ * vector_size 1..64.  Output: *n_users = U distinct users, ascending, in user_ids [U] and user_vectors
+ * [U][vector_size]; `capacity` is the room in both (U > capacity: SRS_ERR_RANGE, nothing written).  Every input is
+ * checked before any device call (SRS_ERR_INVALID).  Synchronous; the same inputs give the same bits. */
+int srs_user_embeddings_host(const int32_t* user_id, const int32_t* movie_id, int64_t n_ratings,
+                             const int32_t* item_ids, const float* item_vectors, int32_t n_items,
+                             int32_t vector_size, int32_t device, int32_t capacity, int32_t* user_ids,
+                             float* user_vectors, int32_t* n_users);
+
 #ifdef __cplusplus
 }
 #endif

@@ -47,7 +47,7 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_dien_outputs_device", "srs_dien_outputs_host_batches", "srs_dien_evaluate_host_batches",
            "srs_trainer_create", "srs_trainer_destroy", "srs_trainer_fit_host", "srs_trainer_get_weights",
            "srs_trainer_iterations", "srs_trainer_fit_validate_host", "srs_trainer_evaluate_host",
-           "srs_featureeng_host")
+           "srs_featureeng_host", "srs_item2vec_host", "srs_user_embeddings_host")
 
 _lib = None
 
@@ -81,6 +81,12 @@ class SrsSamples(C.Structure):
         "row", "label", "release_year", "movie_genre", "movie_rating_count", "movie_avg_rating",
         "movie_rating_stddev", "user_rated_movie", "user_rating_count", "user_avg_release_year",
         "user_release_year_stddev", "user_avg_rating", "user_rating_stddev", "user_genre")]
+
+
+class SrsItem2vecParams(C.Structure):
+    """`srs_item2vec_params` (include/srs_ctr.h): Word2Vec's settings."""
+    _fields_ = [("vector_size", C.c_int32), ("window", C.c_int32), ("iterations", C.c_int32),
+                ("partitions", C.c_int32), ("seed", C.c_uint64)]
 
 
 class SrsError(RuntimeError):
@@ -224,6 +230,14 @@ def load():
     lib.srs_featureeng_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                         C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
                                         C.POINTER(SrsSamples), C.POINTER(C.c_int64)]
+    lib.srs_item2vec_host.restype = C.c_int
+    lib.srs_item2vec_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                      C.POINTER(SrsItem2vecParams), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                      C.POINTER(C.c_int32)]
+    lib.srs_user_embeddings_host.restype = C.c_int
+    lib.srs_user_embeddings_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,
+                                             C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                             C.POINTER(C.c_int32)]
     if lib.srs_abi_version() != ABI_VERSION:
         raise ImportError("libsrs_ctr.so ABI version %d != %d" % (lib.srs_abi_version(), ABI_VERSION))
     _lib = lib

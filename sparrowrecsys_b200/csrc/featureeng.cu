@@ -5,9 +5,10 @@
 // with fewer than two earlier ratings of the same user dropped.  DESIGN.md section 4.11 gives the semantics.
 //
 // Launches, all on one stream, with no host round trip between them:
-//   1. fe_prepare_kernel   sort keys (timestamp in *string* order) and the movies' exact integer moments
-//                          (count, sum h, sum h^2 of half-stars; 64-bit integer atomics, so order-free);
-//   2. two stable CUB radix sorts: by timestamp key, then by user - ties keep file order;
+//   1. fe_prepare_kernel   the movies' exact integer moments (count, sum h, sum h^2 of half-stars; 64-bit
+//                          integer atomics, so order-free);
+//   2. user_time_order     sort keys (timestamp in *string* order), then two stable CUB radix sorts: by
+//                          timestamp key, then by user - ties keep file order (item2vec.cu's sentences use it too);
 //   3. fe_movie_kernel     per movie: count, format_number(avg), format_number(stddev);
 //   4. fe_window_kernel    one thread per rating scans its <= 100 predecessors of the same user, oldest first;
 //   5. CUB DeviceSelect    the kept rows (userRatingCount > 1), in file order;
@@ -55,19 +56,6 @@ int fe_fail(int code, const char* fmt, ...) {
       return fe_fail(SRS_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
   } while (0)
 
-struct Scratch {                       // device allocations of one call, freed when it ends
-  std::vector<void*> ptrs;
-  ~Scratch() { for (void* p : ptrs) cudaFree(p); }
-  template <class T>
-  cudaError_t alloc(T** p, size_t count) {
-    void* q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, (count ? count : 1) * sizeof(T));
-    if (e == cudaSuccess) ptrs.push_back(q);
-    *p = static_cast<T*>(q);
-    return e;
-  }
-};
-
 // java.text.DecimalFormat("#,##0.00") with HALF_EVEN on the exact binary value of x (>= 0): the k it prints as
 // k/100.  100 x = p + e exactly (e from the fma), so the comparisons with the half-way point are exact.
 __device__ __forceinline__ long long hundredths_half_even(double x) {
@@ -109,9 +97,8 @@ struct Welford {
   }
 };
 
-__global__ void fe_prepare_kernel(const int32_t* __restrict__ movie, const int8_t* __restrict__ half,
-                                  const int32_t* __restrict__ ts, int n, uint64_t* __restrict__ ts_key,
-                                  int32_t* __restrict__ iota, unsigned long long* __restrict__ mmom) {
+__global__ void fe_ts_key_kernel(const int32_t* __restrict__ ts, int n, uint64_t* __restrict__ ts_key,
+                                 int32_t* __restrict__ iota) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const int64_t t = ts[i];
     int digits = 1;
@@ -120,6 +107,13 @@ __global__ void fe_prepare_kernel(const int32_t* __restrict__ movie, const int8_
     int64_t aligned = t;
     for (int d = digits; d < 10; ++d) aligned *= 10;
     ts_key[i] = ((uint64_t)aligned << 4) | (uint64_t)digits;   // a string prefix sorts first
+    iota[i] = i;
+  }
+}
+
+__global__ void fe_prepare_kernel(const int32_t* __restrict__ movie, const int8_t* __restrict__ half, int n,
+                                  int32_t* __restrict__ iota, unsigned long long* __restrict__ mmom) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     iota[i] = i;
     const unsigned long long h = (unsigned long long)half[i];
     unsigned long long* m = mmom + 3 * (size_t)movie[i];
@@ -256,6 +250,46 @@ int grid_for(int64_t n, int threads) {
 }
 
 }  // namespace
+
+cudaError_t user_time_order(const int32_t* d_user, const int32_t* d_ts, int n, int32_t* d_order,
+                            uint32_t* d_user_sorted, cudaStream_t s) {
+  if (n <= 0) return cudaSuccess;
+  uint64_t *tskey = nullptr, *tskey2 = nullptr;
+  int32_t *iota = nullptr, *order = nullptr;
+  uint32_t* ukey = nullptr;
+  void* tmp = nullptr;
+  size_t tmp_ts = 0, tmp_u = 0;
+  cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, tmp_ts, tskey, tskey2, iota, order, n, 0, kTsBits, s);
+  if (e == cudaSuccess)
+    e = cub::DeviceRadixSort::SortPairs(nullptr, tmp_u, ukey, d_user_sorted, order, d_order, n, 0, 31, s);
+  const size_t tmp_bytes = std::max(tmp_ts, tmp_u);
+  if (e == cudaSuccess) e = cudaMallocAsync(&tskey, sizeof(uint64_t) * n, s);
+  if (e == cudaSuccess) e = cudaMallocAsync(&tskey2, sizeof(uint64_t) * n, s);
+  if (e == cudaSuccess) e = cudaMallocAsync(&iota, sizeof(int32_t) * n, s);
+  if (e == cudaSuccess) e = cudaMallocAsync(&order, sizeof(int32_t) * n, s);
+  if (e == cudaSuccess) e = cudaMallocAsync(&ukey, sizeof(uint32_t) * n, s);
+  if (e == cudaSuccess) e = cudaMallocAsync(&tmp, tmp_bytes ? tmp_bytes : 1, s);
+  if (e == cudaSuccess) {
+    const int T = 256;
+    fe_ts_key_kernel<<<grid_for(n, T), T, 0, s>>>(d_ts, n, tskey, iota);
+    ++g_launch_count;
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess)
+    e = cub::DeviceRadixSort::SortPairs(tmp, tmp_ts, tskey, tskey2, iota, order, n, 0, kTsBits, s);
+  if (e == cudaSuccess) {
+    const int T = 256;
+    fe_gather_user_kernel<<<grid_for(n, T), T, 0, s>>>(order, d_user, n, ukey);
+    ++g_launch_count;
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess)
+    e = cub::DeviceRadixSort::SortPairs(tmp, tmp_u, ukey, d_user_sorted, order, d_order, n, 0, 31, s);
+  for (void* p : {(void*)tskey, (void*)tskey2, (void*)iota, (void*)order, (void*)ukey, tmp})
+    if (p) cudaFreeAsync(p, s);
+  return e;
+}
+
 }  // namespace srs
 
 using namespace srs;
@@ -324,35 +358,29 @@ extern "C" int srs_featureeng_host(const int32_t* user_id, const int32_t* movie_
   FE_TRY(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
   struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamSynchronize(s); cudaStreamDestroy(s); } } sg{s};
   const size_t slots = (size_t)n_movie_slots;
-  int32_t *d_user, *d_movie, *d_ts, *d_year, *d_genres, *d_iota, *d_order, *d_order2, *d_mcount, *d_wcount;
+  int32_t *d_user, *d_movie, *d_ts, *d_year, *d_genres, *d_iota, *d_order2, *d_mcount, *d_wcount;
   int32_t *d_wrated, *d_wgenre, *d_kept, *d_oi32, *d_omgenre, *d_orated, *d_ogenre;
   int8_t* d_half;
-  uint64_t *d_tskey, *d_tskey2;
-  uint32_t *d_ukey, *d_ukey2;
+  uint32_t* d_ukey2;
   unsigned long long* d_mmom;
   float *d_mavg, *d_mstd, *d_wf32, *d_of32;
   uint8_t* d_keep;
   int* d_nkept;
   FE_TRY(sc.alloc(&d_user, n)); FE_TRY(sc.alloc(&d_movie, n)); FE_TRY(sc.alloc(&d_ts, n));
   FE_TRY(sc.alloc(&d_half, n)); FE_TRY(sc.alloc(&d_year, slots)); FE_TRY(sc.alloc(&d_genres, slots * L));
-  FE_TRY(sc.alloc(&d_iota, n)); FE_TRY(sc.alloc(&d_order, n)); FE_TRY(sc.alloc(&d_order2, n));
-  FE_TRY(sc.alloc(&d_tskey, n)); FE_TRY(sc.alloc(&d_tskey2, n)); FE_TRY(sc.alloc(&d_ukey, n));
-  FE_TRY(sc.alloc(&d_ukey2, n)); FE_TRY(sc.alloc(&d_mmom, 3 * slots)); FE_TRY(sc.alloc(&d_mcount, slots));
+  FE_TRY(sc.alloc(&d_iota, n)); FE_TRY(sc.alloc(&d_order2, n)); FE_TRY(sc.alloc(&d_ukey2, n)); FE_TRY(sc.alloc(&d_mmom, 3 * slots)); FE_TRY(sc.alloc(&d_mcount, slots));
   FE_TRY(sc.alloc(&d_mavg, slots)); FE_TRY(sc.alloc(&d_mstd, slots)); FE_TRY(sc.alloc(&d_wcount, n));
   FE_TRY(sc.alloc(&d_wf32, 4 * (size_t)n)); FE_TRY(sc.alloc(&d_wrated, 5 * (size_t)n));
   FE_TRY(sc.alloc(&d_wgenre, 5 * (size_t)n)); FE_TRY(sc.alloc(&d_keep, n)); FE_TRY(sc.alloc(&d_kept, n));
   FE_TRY(sc.alloc(&d_nkept, 1)); FE_TRY(sc.alloc(&d_oi32, 5 * (size_t)n)); FE_TRY(sc.alloc(&d_omgenre, 3 * (size_t)n)); FE_TRY(sc.alloc(&d_of32, 6 * (size_t)n));
   FE_TRY(sc.alloc(&d_orated, 5 * (size_t)n)); FE_TRY(sc.alloc(&d_ogenre, 5 * (size_t)n));
 
-  size_t tmp_sort_ts = 0, tmp_sort_u = 0, tmp_sel = 0;
-  FE_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort_ts, d_tskey, d_tskey2, d_iota, d_order, n, 0, kTsBits, s));
-  FE_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort_u, d_ukey, d_ukey2, d_order, d_order2, n, 0, 31, s));
+  size_t tmp_sel = 0;
   FE_TRY(cub::DeviceSelect::Flagged(nullptr, tmp_sel, d_iota, d_keep, d_kept, d_nkept, n, s));
-  size_t tmp_bytes = std::max(tmp_sort_ts, std::max(tmp_sort_u, tmp_sel));
   void* d_tmp = nullptr;
   {
     uint8_t* t8 = nullptr;
-    FE_TRY(sc.alloc(&t8, tmp_bytes));
+    FE_TRY(sc.alloc(&t8, tmp_sel));
     d_tmp = t8;
   }
 
@@ -365,14 +393,10 @@ extern "C" int srs_featureeng_host(const int32_t* user_id, const int32_t* movie_
   FE_TRY(cudaMemsetAsync(d_mmom, 0, sizeof(unsigned long long) * 3 * slots, s));
 
   const int T = 256;
-  fe_prepare_kernel<<<grid_for(n, T), T, 0, s>>>(d_movie, d_half, d_ts, n, d_tskey, d_iota, d_mmom);
+  fe_prepare_kernel<<<grid_for(n, T), T, 0, s>>>(d_movie, d_half, n, d_iota, d_mmom);
   ++g_launch_count;
   FE_TRY(cudaGetLastError());
-  FE_TRY(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_sort_ts, d_tskey, d_tskey2, d_iota, d_order, n, 0, kTsBits, s));
-  fe_gather_user_kernel<<<grid_for(n, T), T, 0, s>>>(d_order, d_user, n, d_ukey);
-  ++g_launch_count;
-  FE_TRY(cudaGetLastError());
-  FE_TRY(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_sort_u, d_ukey, d_ukey2, d_order, d_order2, n, 0, 31, s));
+  FE_TRY(user_time_order(d_user, d_ts, n, d_order2, d_ukey2, s));
   fe_movie_kernel<<<grid_for(n_movie_slots, T), T, 0, s>>>(d_mmom, n_movie_slots, d_mcount, d_mavg, d_mstd);
   ++g_launch_count;
   FE_TRY(cudaGetLastError());

@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <vector>
+
 #include "common.cuh"
 
 struct srs_eval_result;
@@ -311,6 +313,25 @@ cudaError_t launch_auc_value(unsigned long long* hist, int K, double* auc, doubl
 // host: the counts -> srs_eval_result (AUCs in double); `confusion` NULL or [4][200] tp, fp, tn, fn
 void metrics_summarise(const unsigned long long* hist, unsigned long long correct, double loss_sum,
                        srs_eval_result* out, int64_t* confusion);
+
+// featureeng.cu: the (user, timestamp string, file index) order of n ratings (device arrays), as the reference's
+// jobs order a user's ratings: d_order[i] = file index of the i-th, d_user_sorted[i] = its user.  Stable radix
+// sorts on `s`; temporaries are stream-ordered allocations.
+cudaError_t user_time_order(const int32_t* d_user, const int32_t* d_ts, int n, int32_t* d_order,
+                            uint32_t* d_user_sorted, cudaStream_t s);
+
+struct Scratch {                       // device allocations of one host call, freed when it ends
+  std::vector<void*> ptrs;
+  ~Scratch() { for (void* p : ptrs) cudaFree(p); }
+  template <class T>
+  cudaError_t alloc(T** p, size_t count) {
+    void* q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, (count ? count : 1) * sizeof(T));
+    if (e == cudaSuccess) ptrs.push_back(q);
+    *p = static_cast<T*>(q);
+    return e;
+  }
+};
 
 extern int64_t g_launch_count;   // kernels launched by this library
 
