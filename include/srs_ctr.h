@@ -520,6 +520,36 @@ int srs_user_embeddings_host(const int32_t* user_id, const int32_t* movie_id, in
                              int32_t vector_size, int32_t device, int32_t capacity, int32_t* user_ids,
                              float* user_vectors, int32_t* n_users);
 
+/* ---- Collaborative filtering: CollaborativeFiltering.scala on the device (DESIGN.md section 4.13) ----
+ * srs_als_fit_host is Spark ML's ALS.fit with explicit feedback: `max_iter` times, the movie factors and then the
+ * user factors, each entity's from its double-precision normal equations (its ratings in ascending counterpart id,
+ * duplicates in input order) plus reg_param * (its rating count) on the diagonal, solved by Cholesky (LAPACK dppsv's
+ * loops) and rounded to float.  The users' initial factors come from a Gaussian generator keyed by `seed` and the
+ * user id, scaled to unit norm.  Ratings are host arrays: user_id >= 0, movie_id >= 0, rating finite; 1 <=
+ * n_ratings <= 21 000 000.  Output: *n_users = U distinct user ids, ascending, in user_ids [U] and user_factors
+ * [U][rank]; *n_movies = M, likewise.  Every input is checked before any device call (SRS_ERR_INVALID).  More
+ * entities than a capacity give SRS_ERR_RANGE, and a system with a pivot <= 0 or NaN gives SRS_ERR_INVALID naming
+ * the user or movie; either way nothing is written.  Synchronous; the same inputs give the same bits. */
+typedef struct srs_als_params {
+  int32_t rank;                       /* 1..64 (Spark's default: 10) */
+  int32_t max_iter;                   /* >= 1 (the reference: 5) */
+  double reg_param;                   /* finite, >= 0 (the reference: 0.01) */
+  uint64_t seed;
+} srs_als_params;
+int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id, const float* rating, int64_t n_ratings,
+                     const srs_als_params* params, int32_t device, int32_t user_capacity, int32_t movie_capacity,
+                     int32_t* user_ids, float* user_factors, int32_t* n_users, int32_t* movie_ids,
+                     float* movie_factors, int32_t* n_movies);
+
+/* ALSModel.recommendForAll: for each of n_src source factors [n_src][rank] (host), the L = min(num, n_dst)
+ * destinations of highest score, best first, in out_ids / out_scores [n_src][L].  The score is the float dot
+ * sum += src(d) * dst(d) from 0.0f, d ascending, each operation rounded once.  Ties go to the lower destination id
+ * (dst_ids must be strictly ascending); a NaN score ranks as -inf.  rank 1..64, num 1..128, factors finite;
+ * checked before any device call (SRS_ERR_INVALID).  Synchronous; the same inputs give the same bits. */
+int srs_als_recommend_host(const float* src_factors, int32_t n_src, const int32_t* dst_ids, const float* dst_factors,
+                           int32_t n_dst, int32_t rank, int32_t num, int32_t device, int32_t* out_ids,
+                           float* out_scores);
+
 #ifdef __cplusplus
 }
 #endif

@@ -47,7 +47,8 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_dien_outputs_device", "srs_dien_outputs_host_batches", "srs_dien_evaluate_host_batches",
            "srs_trainer_create", "srs_trainer_destroy", "srs_trainer_fit_host", "srs_trainer_get_weights",
            "srs_trainer_iterations", "srs_trainer_fit_validate_host", "srs_trainer_evaluate_host",
-           "srs_featureeng_host", "srs_item2vec_host", "srs_user_embeddings_host")
+           "srs_featureeng_host", "srs_item2vec_host", "srs_user_embeddings_host", "srs_als_fit_host",
+           "srs_als_recommend_host")
 
 _lib = None
 
@@ -87,6 +88,11 @@ class SrsItem2vecParams(C.Structure):
     """`srs_item2vec_params` (include/srs_ctr.h): Word2Vec's settings."""
     _fields_ = [("vector_size", C.c_int32), ("window", C.c_int32), ("iterations", C.c_int32),
                 ("partitions", C.c_int32), ("seed", C.c_uint64)]
+
+
+class SrsAlsParams(C.Structure):
+    """`srs_als_params` (include/srs_ctr.h): ALS's settings."""
+    _fields_ = [("rank", C.c_int32), ("max_iter", C.c_int32), ("reg_param", C.c_double), ("seed", C.c_uint64)]
 
 
 class SrsError(RuntimeError):
@@ -238,6 +244,13 @@ def load():
     lib.srs_user_embeddings_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,
                                              C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                              C.POINTER(C.c_int32)]
+    lib.srs_als_fit_host.restype = C.c_int
+    lib.srs_als_fit_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(SrsAlsParams),
+                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32),
+                                     C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]
+    lib.srs_als_recommend_host.restype = C.c_int
+    lib.srs_als_recommend_host.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                           C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     if lib.srs_abi_version() != ABI_VERSION:
         raise ImportError("libsrs_ctr.so ABI version %d != %d" % (lib.srs_abi_version(), ABI_VERSION))
     _lib = lib

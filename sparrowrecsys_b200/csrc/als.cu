@@ -1,0 +1,606 @@
+// als.cu - the reference's CollaborativeFiltering job (Spark ML ALS, explicit feedback) on one device: the factors
+// from double-precision normal equations solved by Cholesky, and the fused top-k recommendations.  DESIGN.md
+// section 4.13 gives the semantics, the orders Spark leaves open and the bounds.
+//
+// srs_als_fit_host, on one stream, inputs uploaded once:
+//   1. four stable radix sorts: by user and by movie (the dense, ascending ids: run-length encodings), then the
+//      user-ordered ratings by movie - the by-movie layout (movie, user, input order) - and that by user - the
+//      by-user layout (user, movie, input order);
+//   2. als_gather_kernel: each layout's counterpart index and rating; each side's entities sorted longest first;
+//   -- the ids come to the host once: the users' initial factors are drawn there (O(users * rank)) --
+//   3. per iteration, with no host round trip: als_solve_kernel over the movies, then over the users.
+// als_solve_kernel runs one block per entity, longest first.  The block stages 32 of the entity's ratings at a time
+// in shared memory; each thread owns elements of the packed upper ata and of atb and adds each rating's term to
+// them in rating order (dspr / daxpy).  Then thread c owns column c: row r of the Cholesky factor is computed in
+// step r (dpptrf's elements, each in its own order), then the two triangular solves (dpptrs).  Every double
+// operation is an explicitly rounded intrinsic and there are no atomics on data: the same inputs give the same
+// bits as oracle/als_c.c.  A non-positive or NaN pivot latches (half-step, entity) in an error word (atomicMin:
+// the first half-step, then the lowest entity).
+//
+// als_recommend_kernel (srs_als_recommend_host): 32 sources per block, 4 per warp; destinations stream through
+// shared memory in tiles of 128, transposed so that each lane reads its own 4.  Each lane computes 4 x 4 exact
+// sequential float dots (__fmul_rn / __fadd_rn from 0.0f, no fma); the warp keeps a sorted list of `num` per
+// source, inserting a candidate only when it beats the list's last entry.  The top-k under a strict total order
+// does not depend on the order candidates arrive in.
+#include <cuda_runtime.h>
+#include <cub/cub.cuh>
+
+#include <algorithm>
+#include <climits>
+#include <cmath>
+#include <cstdarg>
+#include <cstdio>
+#include <vector>
+
+#include "../../include/srs_ctr.h"
+#include "kernels.h"
+
+namespace srs {
+namespace {
+
+constexpr int kMaxRank = 64;           // one thread per factor column
+constexpr int kMaxNum = 128;           // four list entries per lane
+constexpr int64_t kMaxRatings = 21000000;
+constexpr int kSolveThreads = 128;
+constexpr int kChunk = 32;             // ratings staged per step of the accumulation
+constexpr int kRecWarps = 8;
+constexpr int kSrcPerWarp = 4;
+constexpr int kSrcPerBlock = kRecWarps * kSrcPerWarp;
+constexpr int kTile = 128;             // destinations per shared-memory tile, 4 per lane
+constexpr unsigned kFull = 0xffffffffu;
+
+int als_fail(int code, const char* fmt, ...) {
+  char buf[512];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof(buf), fmt, ap);
+  va_end(ap);
+  return set_last_error(code, buf);
+}
+
+#define ALS_TRY(expr)                                                                                     \
+  do {                                                                                                    \
+    cudaError_t e__ = (expr);                                                                             \
+    if (e__ != cudaSuccess)                                                                               \
+      return als_fail(SRS_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
+  } while (0)
+
+#define ALS_LAUNCHED()                                                                                    \
+  do {                                                                                                    \
+    ++g_launch_count;                                                                                     \
+    ALS_TRY(cudaGetLastError());                                                                          \
+  } while (0)
+
+uint64_t splitmix(uint64_t x, uint64_t i) {
+  uint64_t z = x + (i + 1) * 0x9E3779B97F4A7C15ULL;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
+  return z ^ (z >> 31);
+}
+
+// The initial factor of the user with id `user`: `rank` draws of java.util.Random.nextGaussian's polar method on
+// uniforms (top 53 bits of splitmix(splitmix(seed, user), c)) / 2^53, each cast to float, then scaled by
+// 1.0f / snrm2 (reference BLAS's scaled sum of squares).  oracle/als_c.c restates this function line for line.
+void init_factor(uint64_t seed, int32_t user, int rank, float* out) {
+  const uint64_t key = splitmix(seed, (uint64_t)(uint32_t)user);
+  uint64_t c = 0;
+  for (int d = 0; d < rank; d += 2) {
+    double v1, v2, s;
+    do {
+      v1 = 2 * ((double)(splitmix(key, c++) >> 11) * 0x1p-53) - 1;
+      v2 = 2 * ((double)(splitmix(key, c++) >> 11) * 0x1p-53) - 1;
+      s = v1 * v1 + v2 * v2;
+    } while (s >= 1 || s == 0);
+    const double m = std::sqrt(-2 * std::log(s) / s);
+    out[d] = (float)(v1 * m);
+    if (d + 1 < rank) out[d + 1] = (float)(v2 * m);
+  }
+  float scale = 0.0f, ssq = 1.0f;
+  for (int d = 0; d < rank; ++d) {
+    if (out[d] == 0.0f) continue;
+    const float a = std::fabs(out[d]);
+    if (scale < a) {
+      const float t = scale / a;
+      ssq = 1.0f + ssq * (t * t);
+      scale = a;
+    } else {
+      const float t = a / scale;
+      ssq = ssq + t * t;
+    }
+  }
+  const float inv = 1.0f / (scale * std::sqrt(ssq));
+  for (int d = 0; d < rank; ++d) out[d] = out[d] * inv;
+}
+
+int grid_for(int64_t n, int threads) {
+  int64_t b = (n + threads - 1) / threads;
+  return (int)(b < 1 ? 1 : b > 132 * 64 ? 132 * 64 : b);
+}
+
+__global__ void als_iota_kernel(int32_t* __restrict__ out, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = i;
+}
+
+// head[p] = 1 where the sorted key changes (the first rating of an entity)
+__global__ void als_head_kernel(const int32_t* __restrict__ key, int n, int32_t* __restrict__ head) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    head[i] = (i == 0 || key[i] != key[i - 1]) ? 1 : 0;
+}
+
+// dense[perm[p]] = seg[p] - 1 (seg: the inclusive sum of the heads)
+__global__ void als_scatter_kernel(const int32_t* __restrict__ perm, const int32_t* __restrict__ seg, int n,
+                                   int32_t* __restrict__ dense) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) dense[perm[i]] = seg[i] - 1;
+}
+
+// key[p] = dense[perm[p]]
+__global__ void als_key_kernel(const int32_t* __restrict__ perm, const int32_t* __restrict__ dense, int n,
+                               int32_t* __restrict__ key) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) key[i] = dense[perm[i]];
+}
+
+// a layout's counterpart (source) index and rating, in layout order
+__global__ void als_gather_kernel(const int32_t* __restrict__ perm, const int32_t* __restrict__ src_dense,
+                                  const float* __restrict__ rating, int n, int32_t* __restrict__ src,
+                                  float* __restrict__ r) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const int q = perm[i];
+    src[i] = src_dense[q];
+    r[i] = rating[q];
+  }
+}
+
+struct Side {
+  const int32_t* off;                  // [nE + 1] first rating of each entity in the layout
+  const int32_t* src;                  // [n] counterpart index of each rating, in accumulation order
+  const float* r;                      // [n] its rating
+  const int32_t* order;                // [nE] entities, longest first
+  int nE;
+};
+
+// One block per entity (blockIdx.x-th longest): NormalEquation.add over its ratings, then
+// CholeskySolver.solve(ne, n * regParam) (dppsv "U": dpptrf, then dpptrs's two dtpsv).
+__global__ void __launch_bounds__(kSolveThreads) als_solve_kernel(Side sd, const float* __restrict__ srcF,
+                                                                  float* __restrict__ dstF, int k, double reg,
+                                                                  unsigned long long* __restrict__ err,
+                                                                  unsigned long long half_step) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int nA = k * (k + 1) / 2;
+  double* P = reinterpret_cast<double*>(smem);          // [nA] packed upper ata, then [k] atb
+  double* B = P + nA;
+  double* s_y = B + k;                                  // [k] the solves' published values
+  float* s_x = reinterpret_cast<float*>(s_y + k);       // [kChunk][k] staged source factors
+  float* s_r = s_x + kChunk * k;                        // [kChunk]
+  uint8_t* s_i = reinterpret_cast<uint8_t*>(s_r + kChunk);   // [nA] row of each packed element
+  uint8_t* s_j = s_i + nA;                                   // [nA] its column
+  __shared__ int s_bad;
+  __shared__ int s_nz[kMaxRank];
+  const int tid = threadIdx.x;
+  const int ent = sd.order[blockIdx.x];
+  const int lo0 = sd.off[ent], hi = sd.off[ent + 1];
+  for (int e = tid; e < nA; e += kSolveThreads) {
+    int j = 0;
+    while ((j + 1) * (j + 2) / 2 <= e) ++j;
+    s_j[e] = (uint8_t)j;
+    s_i[e] = (uint8_t)(e - j * (j + 1) / 2);
+  }
+  for (int e = tid; e < nA + k; e += kSolveThreads) P[e] = 0.0;
+  if (tid == 0) s_bad = 0;
+  for (int lo = lo0; lo < hi; lo += kChunk) {
+    const int cn = min(kChunk, hi - lo);
+    __syncthreads();                                    // the previous chunk is consumed
+    for (int t = tid; t < cn * k; t += kSolveThreads) {
+      const int c = t / k;
+      s_x[t] = srcF[(size_t)sd.src[lo + c] * k + (t - c * k)];
+    }
+    for (int t = tid; t < cn; t += kSolveThreads) s_r[t] = sd.r[lo + t];
+    __syncthreads();
+    for (int e = tid; e < nA + k; e += kSolveThreads) {
+      double a = P[e];
+      if (e < nA) {                                     // dspr: ap(i,j) += x(i) * (1.0 * x(j)), skipped for x(j) == 0
+        const int i = s_i[e], j = s_j[e];
+        for (int c = 0; c < cn; ++c) {
+          const float xj = s_x[c * k + j];
+          if (xj != 0.0f) a = __dadd_rn(a, __dmul_rn((double)s_x[c * k + i], (double)xj));
+        }
+      } else {                                          // daxpy: atb(i) += rating * x(i), skipped for rating == 0
+        const int i = e - nA;
+        for (int c = 0; c < cn; ++c) {
+          const float rv = s_r[c];
+          if (rv != 0.0f) a = __dadd_rn(a, __dmul_rn((double)rv, (double)s_x[c * k + i]));
+        }
+      }
+      P[e] = a;
+    }
+  }
+  __syncthreads();
+  const double lambda = __dmul_rn((double)(hi - lo0), reg);
+  if (tid < k) P[tid * (tid + 1) / 2 + tid] = __dadd_rn(P[tid * (tid + 1) / 2 + tid], lambda);
+  __syncthreads();
+  // dpptrf "U": in step r, U(r,r) = sqrt(a(r,r) - ddot(U(0:r,r), U(0:r,r))), then for c > r
+  // U(r,c) = (a(r,c) - U(0,r) U(0,c) - ... - U(r-1,r) U(r-1,c)) / U(r,r): dtpsv's element, subtracted in order
+  const int c = tid;
+  const int bc = c * (c + 1) / 2;
+  for (int r = 0; r < k; ++r) {
+    const int br = r * (r + 1) / 2;
+    if (c == r) {
+      double dd = 0.0;
+      for (int i = 0; i < r; ++i) dd = __dadd_rn(dd, __dmul_rn(P[br + i], P[br + i]));
+      const double ajj = __dsub_rn(P[br + r], dd);
+      if (!(ajj > 0.0)) s_bad = 1;                      // a non-positive or NaN pivot
+      else P[br + r] = __dsqrt_rn(ajj);
+    }
+    __syncthreads();
+    if (s_bad) {
+      if (tid == 0) atomicMin(err, (half_step << 32) | (unsigned long long)ent);
+      return;
+    }
+    if (c > r && c < k) {
+      double t = P[bc + r];
+      for (int i = 0; i < r; ++i) t = __dsub_rn(t, __dmul_rn(P[br + i], P[bc + i]));
+      P[bc + r] = __ddiv_rn(t, P[br + r]);
+    }
+    __syncthreads();
+  }
+  // dtpsv "U", "T": y(j) = (b(j) - U(0,j) y(0) - ... - U(j-1,j) y(j-1)) / U(j,j); thread j keeps its running value
+  double x = c < k ? B[c] : 0.0;
+  for (int i = 0; i < k; ++i) {
+    if (c == i) {
+      x = __ddiv_rn(x, P[bc + c]);
+      s_y[i] = x;
+    }
+    __syncthreads();
+    if (c > i && c < k) x = __dsub_rn(x, __dmul_rn(P[bc + i], s_y[i]));
+  }
+  __syncthreads();
+  // dtpsv "U", "N": for j = k-1 .. 0, if x(j) != 0: x(j) /= U(j,j), then x(i) -= x(j) U(i,j) for i < j
+  for (int j = k - 1; j >= 0; --j) {
+    if (c == j) {
+      s_nz[j] = x != 0.0;
+      if (x != 0.0) x = __ddiv_rn(x, P[bc + c]);
+      s_y[j] = x;
+    }
+    __syncthreads();
+    if (c < j && s_nz[j]) x = __dsub_rn(x, __dmul_rn(s_y[j], P[j * (j + 1) / 2 + c]));
+  }
+  if (c < k) dstF[(size_t)ent * k + c] = __double2float_rn(x);
+}
+
+size_t solve_smem(int k) {
+  const int nA = k * (k + 1) / 2;
+  return sizeof(double) * (nA + 2 * k) + sizeof(float) * (kChunk * k + kChunk) + 2 * nA;
+}
+
+// candidate a ranks before b: higher score (NaN as -inf), then lower destination position
+__device__ __forceinline__ bool rec_better(float sa, int ia, float sb, int ib) {
+  const float ka = sa != sa ? -INFINITY : sa, kb = sb != sb ? -INFINITY : sb;
+  return ka > kb || (ka == kb && ia < ib);
+}
+
+__global__ void __launch_bounds__(kRecWarps * 32) als_recommend_kernel(const float* __restrict__ src, int n_src,
+                                                                       const int32_t* __restrict__ dst_ids,
+                                                                       const float* __restrict__ dst, int n_dst,
+                                                                       int k, int L, int32_t* __restrict__ out_ids,
+                                                                       float* __restrict__ out_scores) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  float* s_dst = reinterpret_cast<float*>(smem);        // [k][kTile]
+  float4* s_src = reinterpret_cast<float4*>(s_dst + k * kTile);   // [k][kRecWarps] 4 sources of a warp
+  float* s_score = reinterpret_cast<float*>(s_src + k * kRecWarps);   // [kSrcPerBlock][L]
+  int* s_pos = reinterpret_cast<int*>(s_score + kSrcPerBlock * L);
+  const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
+  const int s0 = blockIdx.x * kSrcPerBlock;
+  float* srcw = reinterpret_cast<float*>(s_src);
+  for (int e = tid; e < kSrcPerBlock * k; e += blockDim.x) {   // source q's factor d at [d][q]
+    const int q = e / k, d = e - q * k;
+    srcw[d * kSrcPerBlock + q] = s0 + q < n_src ? src[(size_t)(s0 + q) * k + d] : 0.0f;
+  }
+  int cnt[kSrcPerWarp];
+#pragma unroll
+  for (int q = 0; q < kSrcPerWarp; ++q) cnt[q] = 0;
+  for (int t0 = 0; t0 < n_dst; t0 += kTile) {
+    const int tn = min(kTile, n_dst - t0);
+    __syncthreads();
+    for (int e = tid; e < tn * k; e += blockDim.x) {
+      const int j = e / k, d = e - j * k;
+      s_dst[d * kTile + j] = dst[(size_t)(t0 + j) * k + d];
+    }
+    __syncthreads();
+    float acc[kSrcPerWarp][4];
+#pragma unroll
+    for (int q = 0; q < kSrcPerWarp; ++q)
+#pragma unroll
+      for (int t = 0; t < 4; ++t) acc[q][t] = 0.0f;
+    for (int d = 0; d < k; ++d) {                       // dot += a(d) * b(d), in order from d = 0
+      const float4 sv = s_src[d * kRecWarps + w];
+      const float sq[4] = {sv.x, sv.y, sv.z, sv.w};
+#pragma unroll
+      for (int t = 0; t < 4; ++t) {
+        const float x = s_dst[d * kTile + lane + 32 * t];
+#pragma unroll
+        for (int q = 0; q < kSrcPerWarp; ++q) acc[q][t] = __fadd_rn(acc[q][t], __fmul_rn(sq[q], x));
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < kSrcPerWarp; ++q) {
+      float* sc = s_score + (w * kSrcPerWarp + q) * L;
+      int* ps = s_pos + (w * kSrcPerWarp + q) * L;
+#pragma unroll
+      for (int t = 0; t < 4; ++t) {
+        const int jj = lane + 32 * t;
+        const int pos = t0 + jj;
+        const bool in = jj < tn && (cnt[q] < L || rec_better(acc[q][t], pos, sc[L - 1], ps[L - 1]));
+        unsigned m = __ballot_sync(kFull, in);
+        while (m) {
+          const int from = __ffs(m) - 1;
+          m &= m - 1;
+          const float cs = __shfl_sync(kFull, acc[q][t], from);
+          const int cp = __shfl_sync(kFull, pos, from);
+          if (cnt[q] == L && !rec_better(cs, cp, sc[L - 1], ps[L - 1])) continue;   // the list moved on
+          int at = 0;
+          for (int b = 0; b < cnt[q]; b += 32) {
+            const int e = b + lane;
+            at += __popc(__ballot_sync(kFull, e < cnt[q] && rec_better(sc[e], ps[e], cs, cp)));
+          }
+          const int nc = min(cnt[q] + 1, L);
+          float mv_s[kMaxNum / 32];
+          int mv_p[kMaxNum / 32];
+#pragma unroll
+          for (int u = 0; u < kMaxNum / 32; ++u) {
+            const int e = lane + 32 * u;
+            if (e >= at && e + 1 < nc) { mv_s[u] = sc[e]; mv_p[u] = ps[e]; }
+          }
+          __syncwarp();
+#pragma unroll
+          for (int u = 0; u < kMaxNum / 32; ++u) {
+            const int e = lane + 32 * u;
+            if (e >= at && e + 1 < nc) { sc[e + 1] = mv_s[u]; ps[e + 1] = mv_p[u]; }
+          }
+          if (lane == 0) { sc[at] = cs; ps[at] = cp; }
+          __syncwarp();
+          cnt[q] = nc;
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int q = 0; q < kSrcPerWarp; ++q) {
+    const int s = s0 + w * kSrcPerWarp + q;
+    if (s >= n_src) continue;
+    const float* sc = s_score + (w * kSrcPerWarp + q) * L;
+    const int* ps = s_pos + (w * kSrcPerWarp + q) * L;
+    for (int e = lane; e < L; e += 32) {
+      out_ids[(size_t)s * L + e] = dst_ids[ps[e]];
+      out_scores[(size_t)s * L + e] = sc[e];
+    }
+  }
+}
+
+int select_device(int32_t device) {
+  int ndev = 0;
+  cudaError_t ce = cudaGetDeviceCount(&ndev);
+  if (ce != cudaSuccess || ndev == 0)
+    return als_fail(SRS_ERR_CUDA, "no CUDA device available (%s); this library has no CPU path", cudaGetErrorString(ce));
+  if (device < 0 || device >= ndev) return als_fail(SRS_ERR_INVALID, "device %d out of range", device);
+  ALS_TRY(cudaSetDevice(device));
+  return SRS_OK;
+}
+
+struct StreamGuard {
+  cudaStream_t s = nullptr;
+  ~StreamGuard() {
+    if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
+  }
+};
+
+// CUB's temporary storage, grown as the calls ask
+struct CubTemp {
+  Scratch* sc;
+  void* p = nullptr;
+  size_t bytes = 0;
+  cudaError_t need(size_t b) {
+    if (b <= bytes) return cudaSuccess;
+    uint8_t* q = nullptr;
+    cudaError_t e = sc->alloc(&q, b);
+    p = q;
+    bytes = b;
+    return e;
+  }
+};
+
+#define ALS_CUB(call_with_tmp)                                                                            \
+  do {                                                                                                    \
+    size_t need__ = 0;                                                                                    \
+    { void* tmp__ = nullptr; size_t& tb__ = need__; ALS_TRY(call_with_tmp); }                            \
+    ALS_TRY(ct.need(need__));                                                                             \
+    { void* tmp__ = ct.p; size_t tb__ = ct.bytes; ALS_TRY(call_with_tmp); }                              \
+  } while (0)
+
+int bits_for(int n) {
+  int b = 1;
+  while (b < 31 && (1 << b) < n) ++b;
+  return b;
+}
+
+}  // namespace
+}  // namespace srs
+
+using namespace srs;
+
+extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
+                                int64_t n_ratings, const srs_als_params* params, int32_t device,
+                                int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
+                                float* user_factors, int32_t* n_users, int32_t* movie_ids, float* movie_factors,
+                                int32_t* n_movies) {
+  if (!n_users || !n_movies) return als_fail(SRS_ERR_INVALID, "null n_users or n_movies");
+  *n_users = 0;
+  *n_movies = 0;
+  if (!params) return als_fail(SRS_ERR_INVALID, "null params");
+  const srs_als_params hp = *params;
+  if (hp.rank < 1 || hp.rank > kMaxRank) return als_fail(SRS_ERR_INVALID, "rank %d outside 1..%d", hp.rank, kMaxRank);
+  if (hp.max_iter < 1) return als_fail(SRS_ERR_INVALID, "max_iter %d is not positive", hp.max_iter);
+  if (!std::isfinite(hp.reg_param) || hp.reg_param < 0)
+    return als_fail(SRS_ERR_INVALID, "reg_param %g is not finite and >= 0", hp.reg_param);
+  if (n_ratings < 1 || n_ratings > kMaxRatings)
+    return als_fail(SRS_ERR_INVALID, "n_ratings %lld outside 1..%lld", (long long)n_ratings, (long long)kMaxRatings);
+  if (!user_id || !movie_id || !rating) return als_fail(SRS_ERR_INVALID, "null ratings");
+  if (user_capacity < 0 || movie_capacity < 0 || (user_capacity > 0 && (!user_ids || !user_factors)) ||
+      (movie_capacity > 0 && (!movie_ids || !movie_factors)))
+    return als_fail(SRS_ERR_INVALID, "negative capacity or null outputs");
+  const int n = (int)n_ratings;
+  for (int i = 0; i < n; ++i) {
+    if (user_id[i] < 0 || movie_id[i] < 0)
+      return als_fail(SRS_ERR_INVALID, "rating %d: negative id (user %d, movie %d)", i, user_id[i], movie_id[i]);
+    if (!std::isfinite(rating[i])) return als_fail(SRS_ERR_INVALID, "rating %d is not finite", i);
+  }
+  if (int rc = select_device(device)) return rc;
+
+  Scratch sc;
+  CubTemp ct{&sc};
+  StreamGuard sg;
+  ALS_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+  cudaStream_t s = sg.s;
+  const int T = 256, G = grid_for(n, T), k = hp.rank;
+  int32_t *d_user, *d_movie, *d_iota, *d_key, *d_perm_u, *d_perm_m, *d_head, *d_seg, *d_du, *d_dm;
+  int32_t *d_uids, *d_ucnt, *d_mids, *d_mcnt, *d_bm, *d_bu, *d_src_m, *d_src_u;
+  float *d_rating, *d_r_m, *d_r_u;
+  int* d_count;
+  ALS_TRY(sc.alloc(&d_user, n)); ALS_TRY(sc.alloc(&d_movie, n)); ALS_TRY(sc.alloc(&d_rating, n));
+  ALS_TRY(sc.alloc(&d_iota, n)); ALS_TRY(sc.alloc(&d_key, n)); ALS_TRY(sc.alloc(&d_perm_u, n));
+  ALS_TRY(sc.alloc(&d_perm_m, n)); ALS_TRY(sc.alloc(&d_head, n)); ALS_TRY(sc.alloc(&d_seg, n));
+  ALS_TRY(sc.alloc(&d_du, n)); ALS_TRY(sc.alloc(&d_dm, n)); ALS_TRY(sc.alloc(&d_uids, n));
+  ALS_TRY(sc.alloc(&d_ucnt, n + 1)); ALS_TRY(sc.alloc(&d_mids, n)); ALS_TRY(sc.alloc(&d_mcnt, n + 1));
+  ALS_TRY(sc.alloc(&d_bm, n)); ALS_TRY(sc.alloc(&d_bu, n)); ALS_TRY(sc.alloc(&d_src_m, n));
+  ALS_TRY(sc.alloc(&d_src_u, n)); ALS_TRY(sc.alloc(&d_r_m, n)); ALS_TRY(sc.alloc(&d_r_u, n));
+  ALS_TRY(sc.alloc(&d_count, 2));
+  ALS_TRY(cudaMemcpyAsync(d_user, user_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  ALS_TRY(cudaMemcpyAsync(d_movie, movie_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  ALS_TRY(cudaMemcpyAsync(d_rating, rating, sizeof(float) * n, cudaMemcpyHostToDevice, s));
+  als_iota_kernel<<<G, T, 0, s>>>(d_iota, n);
+  ALS_LAUNCHED();
+
+  // the dense ids: a stable sort by raw id, its run-length encoding, and each rating's segment
+  const int32_t* raw[2] = {d_user, d_movie};
+  int32_t* perm[2] = {d_perm_u, d_perm_m};
+  int32_t* uniq[2] = {d_uids, d_mids};
+  int32_t* cnt[2] = {d_ucnt, d_mcnt};
+  int32_t* dense[2] = {d_du, d_dm};
+  for (int side = 0; side < 2; ++side) {
+    ALS_CUB(cub::DeviceRadixSort::SortPairs(tmp__, tb__, raw[side], d_key, d_iota, perm[side], n, 0, 31, s));
+    ALS_CUB(cub::DeviceRunLengthEncode::Encode(tmp__, tb__, d_key, uniq[side], cnt[side], d_count + side, n, s));
+    als_head_kernel<<<G, T, 0, s>>>(d_key, n, d_head);
+    ALS_LAUNCHED();
+    ALS_CUB(cub::DeviceScan::InclusiveSum(tmp__, tb__, d_head, d_seg, n, s));
+    als_scatter_kernel<<<G, T, 0, s>>>(perm[side], d_seg, n, dense[side]);
+    ALS_LAUNCHED();
+  }
+  int counts[2];
+  ALS_TRY(cudaMemcpyAsync(counts, d_count, sizeof(counts), cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaStreamSynchronize(s));
+  const int nU = counts[0], nM = counts[1];
+  if (nU > user_capacity) return als_fail(SRS_ERR_RANGE, "%d users exceed capacity %d", nU, user_capacity);
+  if (nM > movie_capacity) return als_fail(SRS_ERR_RANGE, "%d movies exceed capacity %d", nM, movie_capacity);
+  std::vector<int32_t> uid(nU);
+  ALS_TRY(cudaMemcpyAsync(uid.data(), d_uids, sizeof(int32_t) * nU, cudaMemcpyDeviceToHost, s));
+
+  // by-movie layout: the (user, input)-ordered ratings stably sorted by dense movie; by-user: that by dense user
+  als_key_kernel<<<G, T, 0, s>>>(d_perm_u, d_dm, n, d_key);
+  ALS_LAUNCHED();
+  ALS_CUB(cub::DeviceRadixSort::SortPairs(tmp__, tb__, d_key, d_head, d_perm_u, d_bm, n, 0, bits_for(nM), s));
+  als_key_kernel<<<G, T, 0, s>>>(d_bm, d_du, n, d_key);
+  ALS_LAUNCHED();
+  ALS_CUB(cub::DeviceRadixSort::SortPairs(tmp__, tb__, d_key, d_head, d_bm, d_bu, n, 0, bits_for(nU), s));
+  als_gather_kernel<<<G, T, 0, s>>>(d_bm, d_du, d_rating, n, d_src_m, d_r_m);
+  ALS_LAUNCHED();
+  als_gather_kernel<<<G, T, 0, s>>>(d_bu, d_dm, d_rating, n, d_src_u, d_r_u);
+  ALS_LAUNCHED();
+  // each side's offsets and its entities longest first (ties: lower index first)
+  int32_t *d_moff, *d_uoff, *d_morder, *d_uorder;
+  ALS_TRY(sc.alloc(&d_moff, nM + 1)); ALS_TRY(sc.alloc(&d_uoff, nU + 1));
+  ALS_TRY(sc.alloc(&d_morder, nM)); ALS_TRY(sc.alloc(&d_uorder, nU));
+  ALS_TRY(cudaMemsetAsync(d_mcnt + nM, 0, sizeof(int32_t), s));
+  ALS_TRY(cudaMemsetAsync(d_ucnt + nU, 0, sizeof(int32_t), s));
+  ALS_CUB(cub::DeviceScan::ExclusiveSum(tmp__, tb__, d_mcnt, d_moff, nM + 1, s));
+  ALS_CUB(cub::DeviceScan::ExclusiveSum(tmp__, tb__, d_ucnt, d_uoff, nU + 1, s));
+  ALS_CUB(cub::DeviceRadixSort::SortPairsDescending(tmp__, tb__, d_mcnt, d_key, d_iota, d_morder, nM, 0, 31, s));
+  ALS_CUB(cub::DeviceRadixSort::SortPairsDescending(tmp__, tb__, d_ucnt, d_key, d_iota, d_uorder, nU, 0, 31, s));
+
+  // the users' initial factors, drawn on the host
+  std::vector<float> init((size_t)nU * k);
+  for (int u = 0; u < nU; ++u) init_factor(hp.seed, uid[u], k, init.data() + (size_t)u * k);
+  float *d_uf, *d_mf;
+  unsigned long long* d_err;
+  ALS_TRY(sc.alloc(&d_uf, (size_t)nU * k)); ALS_TRY(sc.alloc(&d_mf, (size_t)nM * k)); ALS_TRY(sc.alloc(&d_err, 1));
+  ALS_TRY(cudaMemcpyAsync(d_uf, init.data(), sizeof(float) * init.size(), cudaMemcpyHostToDevice, s));
+  ALS_TRY(cudaMemsetAsync(d_err, 0xff, sizeof(unsigned long long), s));
+  const Side movies{d_moff, d_src_m, d_r_m, d_morder, nM};
+  const Side users{d_uoff, d_src_u, d_r_u, d_uorder, nU};
+  const size_t sm = solve_smem(k);
+  for (int it = 0; it < hp.max_iter; ++it) {
+    als_solve_kernel<<<nM, kSolveThreads, sm, s>>>(movies, d_uf, d_mf, k, hp.reg_param, d_err, 2ull * it);
+    ALS_LAUNCHED();
+    als_solve_kernel<<<nU, kSolveThreads, sm, s>>>(users, d_mf, d_uf, k, hp.reg_param, d_err, 2ull * it + 1);
+    ALS_LAUNCHED();
+  }
+  unsigned long long err = 0;
+  ALS_TRY(cudaMemcpyAsync(&err, d_err, sizeof(err), cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaStreamSynchronize(s));
+  if (err != ~0ull) {
+    const int hs = (int)(err >> 32), ent = (int)(err & 0xffffffffu);
+    int32_t id = 0;
+    ALS_TRY(cudaMemcpy(&id, (hs & 1 ? d_uids : d_mids) + ent, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return als_fail(SRS_ERR_INVALID, "singular normal equations for %s %d in iteration %d (a pivot <= 0 or NaN)",
+                    hs & 1 ? "user" : "movie", id, hs / 2 + 1);
+  }
+  ALS_TRY(cudaMemcpyAsync(user_ids, d_uids, sizeof(int32_t) * nU, cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaMemcpyAsync(user_factors, d_uf, sizeof(float) * nU * k, cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaMemcpyAsync(movie_ids, d_mids, sizeof(int32_t) * nM, cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaMemcpyAsync(movie_factors, d_mf, sizeof(float) * nM * k, cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaStreamSynchronize(s));
+  *n_users = nU;
+  *n_movies = nM;
+  return SRS_OK;
+}
+
+extern "C" int srs_als_recommend_host(const float* src_factors, int32_t n_src, const int32_t* dst_ids,
+                                      const float* dst_factors, int32_t n_dst, int32_t rank, int32_t num,
+                                      int32_t device, int32_t* out_ids, float* out_scores) {
+  if (rank < 1 || rank > kMaxRank) return als_fail(SRS_ERR_INVALID, "rank %d outside 1..%d", rank, kMaxRank);
+  if (num < 1 || num > kMaxNum) return als_fail(SRS_ERR_INVALID, "num %d outside 1..%d", num, kMaxNum);
+  if (n_src < 0 || n_dst < 0) return als_fail(SRS_ERR_INVALID, "negative n_src or n_dst");
+  if ((n_src && !src_factors) || (n_dst && (!dst_ids || !dst_factors)) ||
+      (n_src && n_dst && (!out_ids || !out_scores)))
+    return als_fail(SRS_ERR_INVALID, "null factors, ids or outputs");
+  for (int32_t i = 1; i < n_dst; ++i)
+    if (dst_ids[i] <= dst_ids[i - 1])
+      return als_fail(SRS_ERR_INVALID, "destination ids are not strictly ascending at %d", i);
+  for (int64_t i = 0; i < (int64_t)n_src * rank; ++i)
+    if (!std::isfinite(src_factors[i])) return als_fail(SRS_ERR_INVALID, "source factor element %lld is not finite", (long long)i);
+  for (int64_t i = 0; i < (int64_t)n_dst * rank; ++i)
+    if (!std::isfinite(dst_factors[i]))
+      return als_fail(SRS_ERR_INVALID, "destination factor element %lld is not finite", (long long)i);
+  if (n_src == 0 || n_dst == 0) return SRS_OK;
+  if (int rc = select_device(device)) return rc;
+  const int L = std::min(num, n_dst), k = rank;
+  Scratch sc;
+  StreamGuard sg;
+  ALS_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+  cudaStream_t s = sg.s;
+  float *d_src, *d_dst, *d_scores;
+  int32_t *d_dids, *d_ids;
+  ALS_TRY(sc.alloc(&d_src, (size_t)n_src * k)); ALS_TRY(sc.alloc(&d_dst, (size_t)n_dst * k));
+  ALS_TRY(sc.alloc(&d_dids, n_dst)); ALS_TRY(sc.alloc(&d_ids, (size_t)n_src * L));
+  ALS_TRY(sc.alloc(&d_scores, (size_t)n_src * L));
+  ALS_TRY(cudaMemcpyAsync(d_src, src_factors, sizeof(float) * n_src * k, cudaMemcpyHostToDevice, s));
+  ALS_TRY(cudaMemcpyAsync(d_dst, dst_factors, sizeof(float) * n_dst * k, cudaMemcpyHostToDevice, s));
+  ALS_TRY(cudaMemcpyAsync(d_dids, dst_ids, sizeof(int32_t) * n_dst, cudaMemcpyHostToDevice, s));
+  const size_t sm = sizeof(float) * k * kTile + sizeof(float4) * k * kRecWarps + (sizeof(float) + sizeof(int)) *
+                    kSrcPerBlock * L;
+  ALS_TRY(cudaFuncSetAttribute(als_recommend_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  als_recommend_kernel<<<(n_src + kSrcPerBlock - 1) / kSrcPerBlock, kRecWarps * 32, sm, s>>>(
+      d_src, n_src, d_dids, d_dst, n_dst, k, L, d_ids, d_scores);
+  ALS_LAUNCHED();
+  ALS_TRY(cudaMemcpyAsync(out_ids, d_ids, sizeof(int32_t) * n_src * L, cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaMemcpyAsync(out_scores, d_scores, sizeof(float) * n_src * L, cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaStreamSynchronize(s));
+  return SRS_OK;
+}
