@@ -520,6 +520,55 @@ int srs_user_embeddings_host(const int32_t* user_id, const int32_t* movie_id, in
                              int32_t vector_size, int32_t device, int32_t capacity, int32_t* user_ids,
                              float* user_vectors, int32_t* n_users);
 
+/* ---- Graph embedding and LSH: the rest of Embedding.scala on the device (DESIGN.md section 4.14) ----
+ * The ratings are host arrays as srs_item2vec_host takes them, with its checks, and its sentences (positive ratings
+ * by user, in timestamp-string order).  Every consecutive (a, b) of a sentence is a pair; count(a, b) per distinct
+ * pair, out(a) = sum over b, pairTotal = sum of out.  A source is a movie with an outgoing pair.
+ * srs_item_transitions_host (generateTransitionMatrix): *n_sources = S sources ascending in sources [S], their out(a)
+ * in out_counts [S] and dist(a) = out(a) / pairTotal (a double division) in source_probs [S]; row s's pairs are
+ * entries row_offsets[s] .. row_offsets[s + 1] - 1 (row_offsets [S + 1]) of targets / counts / probs [E], targets
+ * ascending, probs = count / out(a) in double; *n_edges = E.  S or E beyond its capacity: SRS_ERR_RANGE, nothing
+ * written.  Synchronous; the same inputs give the same bits. */
+int srs_item_transitions_host(const int32_t* user_id, const int32_t* movie_id, const int8_t* half,
+                              const int32_t* timestamp, int64_t n_ratings, int32_t device, int32_t source_capacity,
+                              int32_t edge_capacity, int32_t* sources, int32_t* row_offsets, int32_t* out_counts,
+                              double* source_probs, int32_t* targets, int32_t* counts, double* probs,
+                              int32_t* n_sources, int32_t* n_edges);
+
+/* randomWalk (Embedding.scala:140-184): num_walks walks of at most walk_length items, in walks [num_walks]
+ * [walk_length] (-1 past a walk's end) and lengths [num_walks].  Walk w draws u_t = (splitmix(splitmix(splitmix(~seed,
+ * 0), w), t) >> 11) / 2^53 at step t; a draw picks the first entry whose cumulative sum (the probabilities added
+ * left to right in double, sources and targets ascending) is >= u.  Step 0 draws the first item from dist; each
+ * later step stops the walk at an item with no outgoing pair, else draws from its row.  A u past the last sum
+ * leaves the current item (it repeats), or at step 0 makes the walk empty.  num_walks, walk_length >= 1 and
+ * num_walks * walk_length <= 21 000 000, checked before any device call (SRS_ERR_INVALID).  Synchronous. */
+int srs_random_walks_host(const int32_t* user_id, const int32_t* movie_id, const int8_t* half,
+                          const int32_t* timestamp, int64_t n_ratings, int32_t num_walks, int32_t walk_length,
+                          uint64_t seed, int32_t device, int32_t* walks, int32_t* lengths);
+
+/* graphEmb (Embedding.scala:254-266): srs_random_walks_host's walks with params->seed, each non-empty walk one
+ * sentence, trained by srs_item2vec_host's Word2Vec with `params`; outputs, capacity and errors as there. */
+int srs_graph_embedding_host(const int32_t* user_id, const int32_t* movie_id, const int8_t* half,
+                             const int32_t* timestamp, int64_t n_ratings, const srs_item2vec_params* params,
+                             int32_t num_walks, int32_t walk_length, int32_t device, int32_t capacity,
+                             int32_t* vocab_ids, float* vectors, int32_t* vocab_size);
+
+/* BucketedRandomProjectionLSHModel.transform: buckets [n][num_tables] (double) = floor(dot(x, v_j) / bucket_length)
+ * of the float vectors [n][dim] (host) and the unit vectors [num_tables][dim] (double, host); the dot is summed left
+ * to right in double from 0.0, one rounding per operation.  dim 1..1024, num_tables 1..64, bucket_length finite and
+ * > 0, every entry finite, n <= 2^31 - 1; checked before any device call (SRS_ERR_INVALID).  Synchronous. */
+int srs_lsh_transform_host(const float* vectors, int64_t n, int32_t dim, const double* unit_vectors,
+                           int32_t num_tables, double bucket_length, int32_t device, double* buckets);
+
+/* approxNearestNeighbors(dataset, key, k), single probe, for num_keys keys [num_keys][dim] (double) at once: the
+ * candidates are the rows sharing the key's bucket in at least one table; the distance is sqrt of the sum of (x - key)^2
+ * in double, left to right.  Per key q, out_count[q] = min(k, candidates) rows in out_ids / out_dist [q][k] by
+ * distance ascending, ties by id then row ascending; entries past out_count[q] are not written.  k 1..256, keys
+ * finite, and srs_lsh_transform_host's checks, before any device call (SRS_ERR_INVALID).  Synchronous. */
+int srs_lsh_query_host(const int32_t* ids, const float* vectors, int64_t n, int32_t dim, const double* unit_vectors,
+                       int32_t num_tables, double bucket_length, const double* keys, int32_t num_keys, int32_t k,
+                       int32_t device, int32_t* out_ids, double* out_dist, int32_t* out_count);
+
 /* ---- Collaborative filtering: CollaborativeFiltering.scala on the device (DESIGN.md section 4.13) ----
  * srs_als_fit_host is Spark ML's ALS.fit with explicit feedback: `max_iter` times, the movie factors and then the
  * user factors, each entity's from its double-precision normal equations (its ratings in ascending counterpart id,

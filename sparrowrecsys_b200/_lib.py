@@ -48,7 +48,8 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_trainer_create", "srs_trainer_destroy", "srs_trainer_fit_host", "srs_trainer_get_weights",
            "srs_trainer_iterations", "srs_trainer_fit_validate_host", "srs_trainer_evaluate_host",
            "srs_featureeng_host", "srs_item2vec_host", "srs_user_embeddings_host", "srs_als_fit_host",
-           "srs_als_recommend_host")
+           "srs_als_recommend_host", "srs_item_transitions_host", "srs_random_walks_host",
+           "srs_graph_embedding_host", "srs_lsh_transform_host", "srs_lsh_query_host")
 
 _lib = None
 
@@ -251,6 +252,24 @@ def load():
     lib.srs_als_recommend_host.restype = C.c_int
     lib.srs_als_recommend_host.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                            C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.srs_item_transitions_host.restype = C.c_int
+    lib.srs_item_transitions_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
+                                              C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32),
+                                              C.POINTER(C.c_int32)]
+    lib.srs_random_walks_host.restype = C.c_int
+    lib.srs_random_walks_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
+                                          C.c_int32, C.c_uint64, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.srs_graph_embedding_host.restype = C.c_int
+    lib.srs_graph_embedding_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                             C.POINTER(SrsItem2vecParams), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                             C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]
+    lib.srs_lsh_transform_host.restype = C.c_int
+    lib.srs_lsh_transform_host.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_double,
+                                           C.c_int32, C.c_void_p]
+    lib.srs_lsh_query_host.restype = C.c_int
+    lib.srs_lsh_query_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_double,
+                                       C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     if lib.srs_abi_version() != ABI_VERSION:
         raise ImportError("libsrs_ctr.so ABI version %d != %d" % (lib.srs_abi_version(), ABI_VERSION))
     _lib = lib

@@ -2,10 +2,13 @@
 // (hierarchical-softmax skip-gram, SGD) over each user's positive ratings, and the user embeddings.  DESIGN.md
 // section 4.12 gives the semantics, the orders Spark leaves open and the bounds.
 //
-// srs_item2vec_host, on one stream:
+// srs_item2vec_host, on one stream.  i2v_positive_corpus (steps 1-2) builds the sentences; word2vec_fit (steps 3-7)
+// is Word2Vec.fit over any device corpus given as movie ids plus sentence keys, and graphemb.cu trains it on random
+// walks as well:
 //   1. user_time_order (featureeng.cu)   (user, timestamp string, file index) order of the ratings;
-//   2. i2v_flag_kernel + DeviceSelect    the positive ratings (>= 3.5) in that order: the sentences;
-//   3. i2v_count_kernel                  each positive's movie and user, and a per-movie count (integer atomics);
+//   2. i2v_flag_kernel + DeviceSelect    the positive ratings (>= 3.5) in that order, and i2v_gather_kernel their
+//                                        movies and users: the words and their sentence keys;
+//   3. i2v_count_kernel                  a per-movie count (integer atomics);
 //   -- the counts come to the host: vocabulary (count >= 5, count descending, id ascending) and Huffman tree --
 //   4. i2v_map_kernel + two selects      the in-vocabulary words and their users;
 //   5. i2v_user_start_kernel, a max-scan, i2v_chunk_kernel + select: sentence starts, cut every 1000 words;
@@ -94,18 +97,22 @@ __global__ void i2v_flag_kernel(const int32_t* __restrict__ order, const int8_t*
   }
 }
 
-__global__ void i2v_count_kernel(const int32_t* __restrict__ sel, const int* __restrict__ n_sel,
-                                 const int32_t* __restrict__ order, const uint32_t* __restrict__ suser,
-                                 const int32_t* __restrict__ movie, int32_t* __restrict__ pmovie,
-                                 uint32_t* __restrict__ puser, int32_t* __restrict__ count) {
+__global__ void i2v_gather_kernel(const int32_t* __restrict__ sel, const int* __restrict__ n_sel,
+                                  const int32_t* __restrict__ order, const uint32_t* __restrict__ suser,
+                                  const int32_t* __restrict__ movie, int32_t* __restrict__ pmovie,
+                                  uint32_t* __restrict__ puser) {
   const int n = *n_sel;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const int s = sel[i];
-    const int m = movie[order[s]];
-    pmovie[i] = m;
+    pmovie[i] = movie[order[s]];
     puser[i] = suser[s];
-    atomicAdd(count + m, 1);
   }
+}
+
+__global__ void i2v_count_kernel(const int32_t* __restrict__ words, const int* __restrict__ n_words,
+                                 int32_t* __restrict__ count) {
+  const int n = *n_words;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) atomicAdd(count + words[i], 1);
 }
 
 // flags every one of the n entries: those past the positives are cleared for the selects that follow
@@ -365,18 +372,10 @@ struct StreamGuard {
 };
 
 }  // namespace
-}  // namespace srs
 
-using namespace srs;
-
-extern "C" int srs_item2vec_host(const int32_t* user_id, const int32_t* movie_id, const int8_t* half,
-                                 const int32_t* timestamp, int64_t n_ratings, const srs_item2vec_params* params,
-                                 int32_t device, int32_t capacity, int32_t* vocab_ids, float* vectors,
-                                 int32_t* vocab_size) {
-  if (!vocab_size) return i2v_fail(SRS_ERR_INVALID, "null vocab_size");
-  *vocab_size = 0;
+int i2v_check_params(const srs_item2vec_params* params) {
   if (!params) return i2v_fail(SRS_ERR_INVALID, "null params");
-  const srs_item2vec_params hp = *params;
+  const srs_item2vec_params& hp = *params;
   if (hp.vector_size < 1 || hp.vector_size > kMaxDim)
     return i2v_fail(SRS_ERR_INVALID, "vector_size %d outside 1..%d", hp.vector_size, kMaxDim);
   if (hp.window < 1 || hp.window > kMaxWindow)
@@ -385,10 +384,12 @@ extern "C" int srs_item2vec_host(const int32_t* user_id, const int32_t* movie_id
     return i2v_fail(SRS_ERR_INVALID, "iterations %d outside 1..%d", hp.iterations, kMaxIterations);
   if (hp.partitions < 1 || hp.partitions > kMaxPartitions)
     return i2v_fail(SRS_ERR_INVALID, "partitions %d outside 1..%d", hp.partitions, kMaxPartitions);
-  if (capacity < 0 || (capacity > 0 && (!vocab_ids || !vectors)))
-    return i2v_fail(SRS_ERR_INVALID, "negative capacity or null outputs");
-  int32_t n_slots = 0;
-  if (int rc = check_ratings(user_id, movie_id, n_ratings, &n_slots)) return rc;
+  return SRS_OK;
+}
+
+int i2v_check_ratings(const int32_t* user_id, const int32_t* movie_id, const int8_t* half, const int32_t* timestamp,
+                      int64_t n_ratings, int32_t* n_slots) {
+  if (int rc = check_ratings(user_id, movie_id, n_ratings, n_slots)) return rc;
   if (n_ratings && (!half || !timestamp)) return i2v_fail(SRS_ERR_INVALID, "null ratings");
   const int n = (int)n_ratings;
   for (int i = 0; i < n; ++i) {
@@ -397,41 +398,58 @@ extern "C" int srs_item2vec_host(const int32_t* user_id, const int32_t* movie_id
     if (timestamp[i] <= 0) return i2v_fail(SRS_ERR_INVALID, "rating %d: timestamp %d is not positive", i, timestamp[i]);
   }
   if (n == 0) return i2v_fail(SRS_ERR_INVALID, "no ratings: the vocabulary would be empty");
-  if (int rc = select_device(device)) return rc;
+  return SRS_OK;
+}
 
-  Scratch sc;
-  StreamGuard sg;
-  I2V_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
-  cudaStream_t s = sg.s;
-  int32_t *d_user, *d_movie, *d_ts, *d_order, *d_iota, *d_sel, *d_pmovie, *d_count;
-  uint32_t *d_suser, *d_puser;
+int i2v_select_device(int32_t device) { return select_device(device); }
+
+int i2v_positive_corpus(Scratch& sc, cudaStream_t s, const int32_t* user_id, const int32_t* movie_id,
+                        const int8_t* half, const int32_t* timestamp, int n, I2vCorpus* out) {
+  int32_t *d_user, *d_movie, *d_ts, *d_order, *d_iota, *d_sel;
+  uint32_t* d_suser;
   int8_t* d_half;
   uint8_t* d_flag;
-  int* d_nsel;
   I2V_TRY(sc.alloc(&d_user, n)); I2V_TRY(sc.alloc(&d_movie, n)); I2V_TRY(sc.alloc(&d_ts, n));
   I2V_TRY(sc.alloc(&d_half, n)); I2V_TRY(sc.alloc(&d_order, n)); I2V_TRY(sc.alloc(&d_suser, n));
   I2V_TRY(sc.alloc(&d_iota, n)); I2V_TRY(sc.alloc(&d_sel, n)); I2V_TRY(sc.alloc(&d_flag, n));
-  I2V_TRY(sc.alloc(&d_pmovie, n)); I2V_TRY(sc.alloc(&d_puser, n)); I2V_TRY(sc.alloc(&d_count, n_slots));
-  I2V_TRY(sc.alloc(&d_nsel, 2));
+  I2V_TRY(sc.alloc(&out->movie, n)); I2V_TRY(sc.alloc(&out->user, n)); I2V_TRY(sc.alloc(&out->n, 1));
   I2V_TRY(cudaMemcpyAsync(d_user, user_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
   I2V_TRY(cudaMemcpyAsync(d_movie, movie_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
   I2V_TRY(cudaMemcpyAsync(d_ts, timestamp, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
   I2V_TRY(cudaMemcpyAsync(d_half, half, n, cudaMemcpyHostToDevice, s));
-  I2V_TRY(cudaMemsetAsync(d_count, 0, sizeof(int32_t) * n_slots, s));
-
   const int T = 256;
   I2V_TRY(user_time_order(d_user, d_ts, n, d_order, d_suser, s));
   i2v_flag_kernel<<<grid_for(n, T), T, 0, s>>>(d_order, d_half, n, d_flag, d_iota);
   I2V_LAUNCHED();
+  size_t tmp_bytes = 0;
+  I2V_TRY(cub::DeviceSelect::Flagged(nullptr, tmp_bytes, d_iota, d_flag, d_sel, out->n, n, s));
+  uint8_t* d_tmp;
+  I2V_TRY(sc.alloc(&d_tmp, tmp_bytes));
+  I2V_TRY(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_iota, d_flag, d_sel, out->n, n, s));
+  i2v_gather_kernel<<<grid_for(n, T), T, 0, s>>>(d_sel, out->n, d_order, d_suser, d_movie, out->movie, out->user);
+  I2V_LAUNCHED();
+  return SRS_OK;
+}
+
+int word2vec_fit(Scratch& sc, cudaStream_t s, const int32_t* d_pmovie, const uint32_t* d_puser, const int* d_npos,
+                 int n, int32_t n_slots, const srs_item2vec_params& hp, const char* what, int32_t capacity,
+                 int32_t* vocab_ids, float* vectors, int32_t* vocab_size) {
+  int32_t *d_count, *d_iota, *d_pword, *d_vidx, *d_words, *d_ustart, *d_offs, *d_points, *d_codelen;
+  uint32_t *d_wuser, *d_code;
+  uint8_t* d_flag;
+  int* d_nsel;
+  I2V_TRY(sc.alloc(&d_count, n_slots)); I2V_TRY(sc.alloc(&d_iota, n)); I2V_TRY(sc.alloc(&d_flag, n));
+  I2V_TRY(sc.alloc(&d_nsel, 2));
+  I2V_TRY(cudaMemsetAsync(d_count, 0, sizeof(int32_t) * n_slots, s));
+  const int T = 256;
+  i2v_count_kernel<<<grid_for(n, T), T, 0, s>>>(d_pmovie, d_npos, d_count);
+  I2V_LAUNCHED();
   size_t tmp_bytes = 0, t2 = 0;
-  I2V_TRY(cub::DeviceSelect::Flagged(nullptr, tmp_bytes, d_iota, d_flag, d_sel, d_nsel, n, s));
-  I2V_TRY(cub::DeviceScan::InclusiveScan(nullptr, t2, d_iota, d_sel, MaxOp(), n, s));
+  I2V_TRY(cub::DeviceSelect::Flagged(nullptr, tmp_bytes, d_iota, d_flag, d_iota, d_nsel, n, s));
+  I2V_TRY(cub::DeviceScan::InclusiveScan(nullptr, t2, d_iota, d_iota, MaxOp(), n, s));
   tmp_bytes = std::max(tmp_bytes, t2);
   uint8_t* d_tmp;
   I2V_TRY(sc.alloc(&d_tmp, tmp_bytes));
-  I2V_TRY(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_iota, d_flag, d_sel, d_nsel, n, s));
-  i2v_count_kernel<<<grid_for(n, T), T, 0, s>>>(d_sel, d_nsel, d_order, d_suser, d_movie, d_pmovie, d_puser, d_count);
-  I2V_LAUNCHED();
   std::vector<int32_t> counts(n_slots);
   I2V_TRY(cudaMemcpyAsync(counts.data(), d_count, sizeof(int32_t) * n_slots, cudaMemcpyDeviceToHost, s));
   I2V_TRY(cudaStreamSynchronize(s));
@@ -442,7 +460,7 @@ extern "C" int srs_item2vec_host(const int32_t* user_id, const int32_t* movie_id
     if (counts[m] >= kMinCount) vocab.push_back(m);
   std::stable_sort(vocab.begin(), vocab.end(), [&](int32_t x, int32_t y) { return counts[x] > counts[y]; });
   const int V = (int)vocab.size();
-  if (V == 0) return i2v_fail(SRS_ERR_INVALID, "the vocabulary is empty: no movie has %d ratings >= 3.5", kMinCount);
+  if (V == 0) return i2v_fail(SRS_ERR_INVALID, "the vocabulary is empty: no movie has %d %s", kMinCount, what);
   if (V > capacity) return i2v_fail(SRS_ERR_RANGE, "vocabulary of %d words exceeds capacity %d", V, capacity);
   std::vector<int64_t> cn(V);
   std::vector<int32_t> vocab_index(n_slots, -1);
@@ -466,8 +484,6 @@ extern "C" int srs_item2vec_host(const int32_t* user_id, const int32_t* movie_id
   const int D = hp.vector_size, P = hp.partitions;
   const int nw = (int)train_words;
   const int64_t vd = (int64_t)V * D;
-  int32_t *d_vidx, *d_pword, *d_words, *d_ustart, *d_offs, *d_points, *d_codelen;
-  uint32_t *d_wuser, *d_code;
   float *d_exp, *d_syn0, *d_syn1, *d_l0 = nullptr, *d_l1 = nullptr;
   uint8_t *d_mod0 = nullptr, *d_mod1 = nullptr;
   I2V_TRY(sc.alloc(&d_vidx, n_slots)); I2V_TRY(sc.alloc(&d_pword, n)); I2V_TRY(sc.alloc(&d_words, nw));
@@ -485,8 +501,8 @@ extern "C" int srs_item2vec_host(const int32_t* user_id, const int32_t* movie_id
   I2V_TRY(cudaMemcpyAsync(d_code, code_bits.data(), sizeof(uint32_t) * V, cudaMemcpyHostToDevice, s));
   I2V_TRY(cudaMemcpyAsync(d_exp, exp_table.data(), sizeof(float) * kExpTable, cudaMemcpyHostToDevice, s));
 
-  // the in-vocabulary words and their users, then the sentence starts
-  i2v_map_kernel<<<grid_for(n, T), T, 0, s>>>(d_pmovie, d_nsel, n, d_vidx, d_pword, d_flag);
+  // the in-vocabulary words and their sentence keys, then the sentence starts
+  i2v_map_kernel<<<grid_for(n, T), T, 0, s>>>(d_pmovie, d_npos, n, d_vidx, d_pword, d_flag);
   I2V_LAUNCHED();
   I2V_TRY(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_pword, d_flag, d_words, d_nsel + 1, n, s));
   I2V_TRY(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_puser, d_flag, d_wuser, d_nsel + 1, n, s));
@@ -531,6 +547,33 @@ extern "C" int srs_item2vec_host(const int32_t* user_id, const int32_t* movie_id
   std::copy(vocab.begin(), vocab.end(), vocab_ids);
   *vocab_size = V;
   return SRS_OK;
+}
+
+}  // namespace srs
+
+using namespace srs;
+
+extern "C" int srs_item2vec_host(const int32_t* user_id, const int32_t* movie_id, const int8_t* half,
+                                 const int32_t* timestamp, int64_t n_ratings, const srs_item2vec_params* params,
+                                 int32_t device, int32_t capacity, int32_t* vocab_ids, float* vectors,
+                                 int32_t* vocab_size) {
+  if (!vocab_size) return i2v_fail(SRS_ERR_INVALID, "null vocab_size");
+  *vocab_size = 0;
+  if (int rc = i2v_check_params(params)) return rc;
+  if (capacity < 0 || (capacity > 0 && (!vocab_ids || !vectors)))
+    return i2v_fail(SRS_ERR_INVALID, "negative capacity or null outputs");
+  int32_t n_slots = 0;
+  if (int rc = i2v_check_ratings(user_id, movie_id, half, timestamp, n_ratings, &n_slots)) return rc;
+  if (int rc = select_device(device)) return rc;
+
+  Scratch sc;
+  StreamGuard sg;
+  I2V_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+  const int n = (int)n_ratings;
+  I2vCorpus pos;
+  if (int rc = i2v_positive_corpus(sc, sg.s, user_id, movie_id, half, timestamp, n, &pos)) return rc;
+  return word2vec_fit(sc, sg.s, pos.movie, pos.user, pos.n, n, n_slots, *params, "ratings >= 3.5", capacity,
+                      vocab_ids, vectors, vocab_size);
 }
 
 extern "C" int srs_user_embeddings_host(const int32_t* user_id, const int32_t* movie_id, int64_t n_ratings,

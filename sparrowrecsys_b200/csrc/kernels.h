@@ -10,6 +10,7 @@
 #include "common.cuh"
 
 struct srs_eval_result;
+struct srs_item2vec_params;
 
 namespace srs {
 
@@ -332,6 +333,29 @@ struct Scratch {                       // device allocations of one host call, f
     return e;
   }
 };
+
+// ---- item2vec.cu: the Embedding job's sentences and Word2Vec, shared with graphemb.cu ---------------------------
+// Each returns an SRS_* code and sets the last error message.
+int i2v_check_params(const srs_item2vec_params* params);
+// the ratings' checks of srs_item2vec_host (ids, half-stars, timestamps, at least one rating); *n_slots = max movie + 1
+int i2v_check_ratings(const int32_t* user_id, const int32_t* movie_id, const int8_t* half, const int32_t* timestamp,
+                      int64_t n_ratings, int32_t* n_slots);
+int i2v_select_device(int32_t device);
+struct I2vCorpus {                     // device: *n words, movie[i] in sentence order, user[i] its sentence's key
+  int32_t* movie;
+  uint32_t* user;
+  int* n;
+};
+// processItemSequence: the n ratings (host) uploaded, and their positives (>= 3.5) grouped by user ascending, each
+// user's in (timestamp string, input index) order; arrays of n entries allocated in `sc`
+int i2v_positive_corpus(Scratch& sc, cudaStream_t s, const int32_t* user_id, const int32_t* movie_id,
+                        const int8_t* half, const int32_t* timestamp, int n, I2vCorpus* out);
+// Word2Vec.fit over the device corpus of *d_n <= n words (movie ids < n_slots) whose sentences are the runs of
+// equal keys: vocabulary, Huffman tree, exp table, the 1000-word cut and training; the outputs as srs_item2vec_host.
+// `what` names the words in the empty-vocabulary message.  Synchronises `s`.
+int word2vec_fit(Scratch& sc, cudaStream_t s, const int32_t* d_words, const uint32_t* d_keys, const int* d_n, int n,
+                 int32_t n_slots, const srs_item2vec_params& hp, const char* what, int32_t capacity,
+                 int32_t* vocab_ids, float* vectors, int32_t* vocab_size);
 
 extern int64_t g_launch_count;   // kernels launched by this library
 
