@@ -442,7 +442,8 @@ int64_t srs_trainer_iterations(const srs_trainer* tr);
 /* Known-answer self test of the warpgroup-MMA (wgmma) plumbing the tensor-core kernels are built on:
  * D[128][N] = bf16(A[128][K]) * bf16(B[N][K])^T (inputs truncated to bf16, fp32 accumulate),
  * K = 64 * k_blocks (1..4), N = 16 or 32, A read from shared memory (a_in_regs = 0) or from
- * registers (a_in_regs = 1).  Device pointers; synchronous. */
+ * registers (a_in_regs = 1); N = 8: A read MN-major from shared memory (a_in_regs = 0).  Device
+ * pointers; synchronous. */
 int srs_selftest_wgmma(const float* A, const float* B, float* D, int32_t N, int32_t k_blocks,
                        int32_t a_in_regs, int32_t device);
 

@@ -14,7 +14,9 @@
 //         D[64 x 32] = H_hi W_hi + H_lo W_hi + H_hi W_lo    (bf16x3, fp32 accumulate)
 //   * gate (PReLU per position, Dense(1), sigmoid) on the accumulator registers, one quad of
 //     lanes per position;
-//   * pooling sum_t w_t h_t from the same shared-memory tile (h = hi + lo);
+//   * pooling sum_t w_t h_t on a warpgroup MMA from the same shared-memory tile, read MN-major
+//     (its 128-byte rows are positions): D[e'][n] = sum_t A[t][e'] Pb[n][t] with Pb's rows w hi and
+//     w lo, so pooled = h_hi w_hi + h_lo w_hi + h_hi w_lo (bf16x3, as the activation unit);
 //   * top MLP over the CTA's 32-row tile.  E <= 32: on wgmma, computed transposed like
 //     embmlp_tc.cu - D[units x rows] = W^T X^T with W1^T (the 160 embedding columns of the tile) and
 //     W2^T in shared memory as bf16 hi / lo images, the tile's hi and lo halves stacked along N, the
@@ -38,6 +40,14 @@
 
 namespace srs {
 using namespace wg;
+
+// 1 / x to about 1 ulp (rcp.approx): the gate weight it forms is rounded to 16 significant bits (bf16 hi + lo)
+// before it is used, so the correctly rounded reciprocal's Newton steps and slow path buy nothing
+__device__ __forceinline__ float rcp_approx(float x) {
+  float r;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+  return r;
+}
 
 constexpr int kWgRows = 32;       // rows per CTA (top-MLP tile height, as din.cu)
 constexpr int kWgPos = 64;        // history positions per MMA tile
@@ -77,18 +87,25 @@ struct DinWgLayout {
   static constexpr int F_WP = F_WH + EP * 32;                 // [EP][32] Wp
   static constexpr int F_WC = F_WP + EP * 32;                 // [EP][32] Wc - Wsub
   static constexpr int F_CST = F_WC + EP * 32;                // [32 rows][32 units] activation-unit constants
-  static constexpr int F_WG = F_CST + kWgRows * 32;           // per warpgroup: w[64] | part[128]
-  static constexpr int F_WG_STRIDE = kWgPos + 128;
+  static constexpr int F_WG = F_CST + kWgRows * 32;           // per warpgroup: pooled lo sums (EP = 32)
+  static constexpr int F_WG_STRIDE = 32;
   static constexpr int F_RED = F_WG + G * F_WG_STRIDE;        // [4 warps][32 rows] Dense(1) partial sums
   static constexpr int F_END = F_RED + 4 * kWgRows;
   static constexpr uint32_t FS_BYTES = (uint32_t)F_END * sizeof(float);
-  // Byte region at the aligned base, in front of the fp32 region.  E <= 64: the warpgroups' history tiles and
-  // W_r.  E <= 32: every byte that one CTA per SM leaves (kSmemStatic: the static mbarriers), the image at its
-  // bottom and the warpgroups' buffers at its top, the X / H1 operand over the last of those.  The image bytes
-  // under the buffers (IMG_RELOAD) are copied again in every tile once its activation unit is done; the rest
-  // (IMG_RESIDENT) is copied once per CTA.
+  // pooling B operand per warpgroup, K-major [8 rows][64 positions] bf16: row 0 w hi, row 1 w lo, rows 2-7 zero.
+  // They sit between the byte region and the fp32 region, where neither the image nor the X / H1 operand
+  // reaches, so their zero rows are written once per CTA.
+  static constexpr uint32_t PB_BYTES = 1024;
+  // Byte region at the aligned base, in front of the pooling operands and the fp32 region.  E <= 64: the
+  // warpgroups' history tiles and W_r.  E <= 32: every byte that one CTA per SM leaves (kSmemStatic: the static
+  // mbarriers), the image at its bottom and the warpgroups' buffers at its top, the X / H1 operand over the last
+  // of those.  The image bytes under the buffers (IMG_RELOAD) are copied again in every tile once its
+  // activation unit is done; the rest (IMG_RESIDENT) is copied once per CTA.
   static constexpr uint32_t kSmemStatic = 64;
-  static constexpr uint32_t REGION = TC_MLP ? (227u * 1024 - 1024 - kSmemStatic - FS_BYTES) / 1024 * 1024 : AU_BYTES;
+  static constexpr uint32_t REGION =
+      TC_MLP ? (227u * 1024 - 1024 - kSmemStatic - G * PB_BYTES - FS_BYTES) / 1024 * 1024 : AU_BYTES;
+  static constexpr uint32_t PB_OFF = REGION;                    // warpgroup q's pooling operand at PB_OFF + q PB_BYTES
+  static constexpr uint32_t FS_OFF = PB_OFF + G * PB_BYTES;
   static constexpr uint32_t AU_OFF = REGION - AU_BYTES;         // warpgroup q's buffers at AU_OFF + q WG_BYTES
   static constexpr uint32_t OPS_OFF = REGION - 3 * OP_KB_BYTES; // X / H1 operand
   static constexpr uint32_t IMG_RESIDENT = AU_OFF < IMG_BYTES ? AU_OFF : IMG_BYTES;
@@ -96,7 +113,7 @@ struct DinWgLayout {
   static constexpr bool RELOAD_IN_W2 = IMG_RESIDENT >= IMG_W2_HI;  // Dense(128) never waits for the reload
   static_assert(REGION >= AU_BYTES && AU_OFF % 1024 == 0 && IMG_RESIDENT % 16 == 0, "buffer alignment");
   static_assert(!TC_MLP || OPS_OFF >= IMG_BYTES, "the X / H1 operand must not overlap the image");
-  static constexpr size_t SMEM = 1024 + REGION + FS_BYTES;
+  static constexpr size_t SMEM = 1024 + FS_OFF + FS_BYTES;
   static_assert(SMEM + kSmemStatic <= 227 * 1024, "one CTA per SM must fit");
 };
 
@@ -201,6 +218,14 @@ __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& 
   float d[32];
   #pragma unroll
   for (int i = 0; i < 32; ++i) d[i] = 0.f;
+  float bias[2], slope[2], w3[2];                  // units u = 16 warp + g + 8 i, requested before the MMAs
+  #pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int u = 16 * warp + g + 8 * i;
+    bias[i] = __ldg(p.b2 + u);
+    slope[i] = __ldg(p.a2 + u);
+    w3[i] = __ldg(p.w3 + u);
+  }
   mma_fence();
   #pragma unroll
   for (int kb = 0; kb < 2; ++kb) {
@@ -221,15 +246,13 @@ __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& 
   for (int j = 0; j < 4; ++j) s[j][0] = s[j][1] = 0.f;
   #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    const int u = 16 * warp + g + 8 * i;
-    const float bias = __ldg(p.b2 + u), slope = __ldg(p.a2 + u), w3 = __ldg(p.w3 + u);
   #pragma unroll
     for (int j = 0; j < 4; ++j)
   #pragma unroll
       for (int c = 0; c < 2; ++c) {
-        float v = d[4 * j + 2 * i + c] + d[4 * (j + 4) + 2 * i + c] + bias;
-        v = v > 0.f ? v : slope * v;
-        s[j][c] = fmaf(v, w3, s[j][c]);
+        float v = d[4 * j + 2 * i + c] + d[4 * (j + 4) + 2 * i + c] + bias[i];
+        v = v > 0.f ? v : slope[i] * v;
+        s[j][c] = fmaf(v, w3[i], s[j][c]);
       }
   }
   // sum over the 8 lanes of a column quad (g), then over the 4 warps in a fixed order
@@ -262,13 +285,12 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
   constexpr int KS = EP / 16;                     // K steps per part (hi or lo)
   constexpr int CP = 8 * KB;                      // 16-byte chunks per split row
   constexpr int NCOPY = kWgPos * CP / 128;        // cp.async per thread per tile
-  constexpr int PARTS = 128 / EP, PP = kWgPos / PARTS;
   constexpr int OFF_UG = 0, OFF_U = EP, OFF_POOL = 2 * EP, OFF_C = 3 * EP, OFF_MG = 4 * EP, OFF_NUM = 5 * EP;
   extern __shared__ uint8_t raw[];
   __shared__ uint64_t res_bar, reload_bar;        // top-MLP image (TC_MLP): resident part / this tile's reload landed
   uint8_t* base = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
   uint8_t* img = base;
-  float* fs = reinterpret_cast<float*>(base + L::REGION);
+  float* fs = reinterpret_cast<float*>(base + L::FS_OFF);
   float* Xs = fs + L::F_X;
   float* H1 = fs + L::F_H1;
   float* H2 = fs + L::F_H2;
@@ -282,9 +304,9 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
   const int T = p.T, nch = (T + kWgPos - 1) / kWgPos;
   uint8_t* tiles = base + L::AU_OFF + q * L::WG_BYTES;   // history tiles 0, 1 | W_r
   uint8_t* Bt = tiles + 2 * L::A_BYTES;
-  float* wsm = fs + L::F_WG + q * L::F_WG_STRIDE;
-  float* part = wsm + kWgPos;
   PhaseClock clk(tw == 0);
+  // pooling B operand: w hi | w lo | 6 zero rows (128 threads x 8 B: the whole operand)
+  reinterpret_cast<uint2*>(base + L::PB_OFF + q * L::PB_BYTES)[tw] = make_uint2(0u, 0u);
 
   bool weights_ready = !L::TC_MLP;
   uint32_t reload_parity = 0;
@@ -305,6 +327,21 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
   const int n_tiles = (b.B + kWgRows - 1) / kWgRows;
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const int row0 = tile * kWgRows;
+    // Warp 0 brings the lines of the tile's ids into L1 at once: the steps below that each wait for ids (side
+    // features -> their rows, candidate id -> its row, history ids -> the first gathers) then find them there
+    // instead of making their own HBM round trips one after the other.
+    if (tid < kWgRows && row0 + tid < b.B) {
+      const int row = row0 + tid, n = min(T, kWgPos);
+      const int32_t* h = b.hist + (size_t)row * b.hist_stride;
+      prefetch_l1(b.user_id + row);
+      prefetch_l1(b.user_genre + row * 5);
+      prefetch_l1(b.movie_genre + row * 3);
+      prefetch_l1(b.movie_id + row);
+      prefetch_l1(b.numerics + row * kNumNumerics);
+      prefetch_l1(h);                                        // the first chunk's ids: at most 3 lines
+      prefetch_l1(h + (n - 1) / 2);
+      prefetch_l1(h + n - 1);
+    }
     tile_side_features<EP, kWgRows, NT>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users, p.n_genres,
                                         OFF_UG, OFF_U, OFF_MG, OFF_NUM);
     // candidate rows of the tile (ids pass through float32, DIN.py:95,125); rows past the batch end are zero
@@ -348,9 +385,12 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
     // The history ids of an item are requested (into registers) two items before its rows are gathered,
     // so the HBM latency of the ids is not on the item chain.  Whether a slot is live is decided from its
     // position, never from the id value: every live id goes through the range check.
-    auto item_nt = [&](int k) { return k < n_items ? min(kWgPos, T - (k % nch) * kWgPos) : 0; };
+    // item k is chunk k % nch of the warpgroup's row k / nch; with one chunk per row (T <= 64) no division
+    auto item_row = [&](int k) { return nch == 1 ? k : k / nch; };
+    auto item_ch = [&](int k) { return nch == 1 ? 0 : k % nch; };
+    auto item_nt = [&](int k) { return k < n_items ? min(kWgPos, T - item_ch(k) * kWgPos) : 0; };
     auto load_ids = [&](int k, int (&ids)[NCOPY]) {
-      const int row = row0 + q + G * (k / nch), t0 = (k % nch) * kWgPos, nt = item_nt(k);
+      const int row = row0 + q + G * item_row(k), t0 = item_ch(k) * kWgPos, nt = item_nt(k);
       const int32_t* hrow = b.hist + (size_t)row * b.hist_stride + t0;
   #pragma unroll
       for (int n = 0; n < NCOPY; ++n) {
@@ -358,18 +398,24 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
         ids[n] = pos < nt ? __ldg(hrow + pos) : 0;
       }
     };
+    // Every position of the tile is written: positions past nt are zero-filled, because the pooling MMA
+    // reads them (with w = 0, which a stale NaN would still turn into NaN).  An out-of-range id is read as
+    // row 0 and latches the error word, once per warp and item.
     auto gather = [&](int k, const int (&ids)[NCOPY]) {
+      if (k >= n_items) return;
       uint8_t* A = tiles + (k & 1) * L::A_BYTES;
       const int nt = item_nt(k);
+      bool bad = false;
   #pragma unroll
       for (int n = 0; n < NCOPY; ++n) {
         const int i = tw + 128 * n, pos = i / CP, c = i % CP;
-        if (pos < nt) {
-          const int id = checked_id(__float2int_rz(__int2float_rn(ids[n])), p.n_movies, b.err_flag);
-          cp_async16(A + (c >> 3) * (kWgPos * 128) + sw128_offset(pos, c & 7),
-                     p.movie_split + (size_t)id * (CP * 16) + c * 16);
-        }
+        const int id = __float2int_rz(__int2float_rn(ids[n]));
+        const bool in_range = static_cast<unsigned>(id) < static_cast<unsigned>(p.n_movies);
+        bad |= !in_range;                                     // ids past nt are 0: never out of range
+        cp_async16_zfill(A + (c >> 3) * (kWgPos * 128) + sw128_offset(pos, c & 7),
+                         p.movie_split + (size_t)(in_range ? id : 0) * (CP * 16) + c * 16, pos < nt ? 16u : 0u);
       }
+      if (__any_sync(0xffffffffu, bad) && lane == 0 && b.err_flag) atomicExch(b.err_flag, 1);
     };
 
     int ids_next[NCOPY];
@@ -380,36 +426,49 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
       gather(0, ids0);
     }
     cp_async_commit();
-    float pool_acc = 0.f;
+    const uint32_t pb_s = smem_u32(base + L::PB_OFF + q * L::PB_BYTES);
+    float* pool_lo = fs + L::F_WG + q * L::F_WG_STRIDE;
+    // W_r destinations of this thread (unit j = lane, element pair e = 2 warp + 8 n, K byte 4 warp + 16 n), the
+    // same in every row: chunk n of row `lane`, byte 4 warp within it; its sources wh / wp [e][j]
+    const uint32_t wr_row = smem_u32(Bt) + lane * 128u + 4u * warp, wr_sw = lane & 7u;
+    const int wr_src = 2 * warp * 32 + lane;
     float slope[2][8], cstv[8];
+    // pooled sums of the row so far: D[e'][n] = sum_t A[t][e'] Pb[n][t] for the operand columns e' of K block kb
+    // (EP = 32: hi e | lo e; EP = 64: block 0 hi, block 1 lo) and n = w hi, w lo, added chunk by chunk
+    float pacc[KB][4];
     for (int k = 0; k < n_items; ++k) {
-      const int r = q + G * (k / nch), ch = k % nch, t0 = ch * kWgPos;
+      const int r = q + G * item_row(k), ch = item_ch(k), t0 = ch * kWgPos;
       const int nt = min(kWgPos, T - t0);
       float* xrow = Xs + r * L::LDX;
       const float* cst = cst_all + r * 32;
       if (ch == 0) {
-        // B operand of the row: W_r = (Wsub + Wh) + diag(c_r) Wp, split to bf16 hi / lo
-        const float* cv = xrow + OFF_C;
-        for (int i = tw; i < 32 * EP / 2; i += 128) {          // (unit j, element pair e, e + 1): the lanes
-          const int j = i & 31, e = 2 * (i >> 5);               // of a warp read 32 consecutive banks
-          const float v0 = fmaf(cv[e], wp[e * 32 + j], wh[e * 32 + j]);
-          const float v1 = fmaf(cv[e + 1], wp[(e + 1) * 32 + j], wh[(e + 1) * 32 + j]);
+        // B operand of the row: W_r = (Wsub + Wh) + diag(c_r) Wp, split to bf16 hi / lo.  Thread (warp, lane)
+        // writes unit j = lane, element pairs e = 2 warp + 8 n: the lanes of a warp read 32 consecutive banks
+        const float* cv = xrow + OFF_C + 2 * warp;
+  #pragma unroll
+        for (int n = 0; n < EP / 8; ++n) {
+          const float2 c2 = *reinterpret_cast<const float2*>(cv + 8 * n);
+          const float v0 = fmaf(c2.x, wp[wr_src + 256 * n], wh[wr_src + 256 * n]);
+          const float v1 = fmaf(c2.y, wp[wr_src + 256 * n + 32], wh[wr_src + 256 * n + 32]);
           const Split2 s = split_pack(v0, v1);
-          *reinterpret_cast<uint32_t*>(Bt + wg_kbyte(j, 2 * e, 32)) = s.hi;
-          *reinterpret_cast<uint32_t*>(Bt + wg_kbyte(j, 2 * (EP + e), 32)) = s.lo;
+          // the lo half of K byte kb sits at K byte 2 EP + kb: 64 bytes on in the same row (EP = 32, the
+          // chunk index gains bit 2), or the next K block (EP = 64)
+          const uint32_t dst = wr_row + ((n ^ wr_sw) << 4);
+          st_shared_u32(dst, s.hi);
+          st_shared_u32(EP == 32 ? dst ^ 64u : dst + 32u * 128u, s.lo);
         }
   #pragma unroll
         for (int j = 0; j < 4; ++j)
   #pragma unroll
           for (int c = 0; c < 2; ++c) cstv[2 * j + c] = cst[8 * j + 2 * cq + c];
-        pool_acc = 0.f;
         clk.lap(PH_W_BUILD);
       }
       gather(k + 1, ids_next);                                // its buffer's last reader finished before the
       cp_async_commit();                                      // closing barrier of item k - 1
       load_ids(k + 2, ids_next);
-      // PReLU slopes of this thread's positions pr = 16 warp + g + 8 i and columns 8 j + 2 cq + c,
-      // requested before the waits below; with one chunk per row (T <= 64) they are the same for every row
+      // PReLU slopes of this thread's positions pr = 16 warp + g + 8 i and columns 8 j + 2 cq + c, times the
+      // Dense(1) weights (the gate adds z wout or z slope wout), requested before the waits below; with one chunk
+      // per row (T <= 64) they are the same for every row
       if (nch > 1 || k == 0) {
   #pragma unroll
         for (int i = 0; i < 2; ++i) {
@@ -417,7 +476,7 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
   #pragma unroll
           for (int j = 0; j < 4; ++j)
   #pragma unroll
-            for (int c = 0; c < 2; ++c) slope[i][2 * j + c] = __ldg(alpha + 8 * j + 2 * cq + c);
+            for (int c = 0; c < 2; ++c) slope[i][2 * j + c] = __ldg(alpha + 8 * j + 2 * cq + c) * wout[2 * j + c];
         }
       }
       clk.lap(PH_GATHER_ISSUE);
@@ -459,39 +518,71 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
   #pragma unroll
           for (int c = 0; c < 2; ++c) {
             const float z = d[4 * j + 2 * i + c] + cstv[2 * j + c];
-            const float a = z > 0.f ? z : slope[i][2 * j + c] * z;
-            s = fmaf(a, wout[2 * j + c], s);
+            s = fmaf(z, z > 0.f ? wout[2 * j + c] : slope[i][2 * j + c], s);
           }
         s += __shfl_xor_sync(0xffffffffu, s, 1);
         s += __shfl_xor_sync(0xffffffffu, s, 2);
-        if (cq == 0) wsm[pr] = pr < nt ? 1.f / (1.f + __expf(-(s + p.au_bout))) : 0.f;
+        // w split to bf16 hi / lo into rows 0 and 1 of the pooling operand (K byte 2 pr); w = 0 past nt
+        const float w = pr < nt ? rcp_approx(1.f + __expf(-(s + p.au_bout))) : 0.f;
+        if (cq == 0) {
+          const __nv_bfloat16 wh16 = __float2bfloat16_rn(w);
+          const __nv_bfloat16 wl16 = __float2bfloat16_rn(w - __bfloat162float(wh16));
+          st_shared_u16(pb_s + sw128_offset(0, pr >> 3) + 2 * (pr & 7), __bfloat16_as_ushort(wh16));
+          st_shared_u16(pb_s + sw128_offset(1, pr >> 3) + 2 * (pr & 7), __bfloat16_as_ushort(wl16));
+        }
       }
-      named_sync(1 + q, 128);
+      fence_async_smem();
+      named_sync(1 + q, 128);                                 // w in place
       clk.lap(PH_GATE);
-      // ---- pooling: thread (part, e) sums positions part * PP .. + PP of element e
+      // ---- pooling: D (+)= A^T Pb over the tile's 64 positions, A read MN-major (its 128-byte rows are
+      // positions); products h_hi w_hi, h_lo w_hi, h_hi w_lo as in the activation unit
       {
-        const int e = tw % EP, pt = tw / EP;
-        const uint8_t* A = tiles + (k & 1) * L::A_BYTES;
-        const uint32_t oh = 2 * e, ol = 2 * (EP + e);
-        const int pend = min(nt, (pt + 1) * PP);
-        for (int pos = pt * PP; pos < pend; ++pos) {
-          const float h = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(A + wg_kbyte(pos, oh, kWgPos))) +
-                          __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(A + wg_kbyte(pos, ol, kWgPos)));
-          pool_acc = fmaf(wsm[pos], h, pool_acc);
-        }
-        if (ch == nch - 1) {
-          part[tw] = pool_acc;
-          named_sync(1 + q, 128);
-          if (tw < EP) {
-            float v = 0.f;
+        // (an accumulator set that stayed live across the next activation-unit MMAs would make ptxas spill)
+        const uint32_t sa = smem_u32(tiles + (k & 1) * L::A_BYTES), sp = pb_s;
+        float pd[KB][4];
+        mma_fence();
   #pragma unroll
-            for (int u = 0; u < PARTS; ++u) v += part[u * EP + tw];
-            xrow[OFF_POOL + tw] = v;
-          }
+        for (int s = 0; s < kWgPos / 16; ++s)
+  #pragma unroll
+          for (int kb = 0; kb < KB; ++kb)
+            mma_m64n8_ss_amn(pd[kb], desc_sw128_mn(sa + kb * (kWgPos * 128) + s * 2048), desc_sw128(sp + 32 * s),
+                             s > 0);
+        mma_commit();
+        mma_wait<0>();
+  #pragma unroll
+        for (int kb = 0; kb < KB; ++kb) {
+          reg_fence(pd[kb]);
+  #pragma unroll
+          for (int i = 0; i < 4; ++i) pacc[kb][i] = ch > 0 ? pacc[kb][i] + pd[kb][i] : pd[kb][i];
         }
       }
-      named_sync(1 + q, 128);                                 // tile k, wsm, part and W_r free again
+      // lanes cq = 0 hold columns w hi (pacc[.][0], [2]) and w lo ([1], [3]) of operand columns 16 warp + g (+ 8);
+      // at EP = 32 the lo elements' sums (columns 32 + e) are in warps 2 and 3 and go through shared memory
+      const bool last = ch == nch - 1;
+      if (EP == 32 && last && warp >= 2 && cq == 0) {
+        pool_lo[16 * (warp - 2) + g] = pacc[0][0];
+        pool_lo[16 * (warp - 2) + g + 8] = pacc[0][2];
+      }
+      named_sync(1 + q, 128);                                 // tile k, Pb and W_r free again
+      if (last && cq == 0 && (EP == 64 || warp < 2)) {
+  #pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int e = 16 * warp + g + 8 * i;
+          const float lo_whi = EP == 32 ? pool_lo[e] : pacc[KB - 1][2 * i];
+          xrow[OFF_POOL + e] = (pacc[0][2 * i] + lo_whi) + pacc[0][2 * i + 1];
+        }
+      }
       clk.lap(PH_POOL);
+    }
+    if constexpr (L::TC_MLP) {
+      // the top MLP's epilogue constants (b1, a1, the numerics' rows of W1, b2, a2, w3: 42 lines) come into L1
+      // while the warpgroups wait for the one with the most rows
+      if (tw < 42) {
+        const float* src = tw < 4 ? p.b1 + 32 * tw : tw < 8 ? p.a1 + 32 * (tw - 4)
+                         : tw < 36 ? p.W1 + (size_t)(5 * EP + (tw - 8) / 4) * 128 + 32 * ((tw - 8) % 4)
+                         : tw < 38 ? p.b2 + 32 * (tw - 36) : tw < 40 ? p.a2 + 32 * (tw - 38) : p.w3 + 32 * (tw - 40);
+        prefetch_l1(src);
+      }
     }
     cp_async_wait<0>();
     __syncthreads();

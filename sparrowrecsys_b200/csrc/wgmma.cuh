@@ -23,6 +23,13 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
+__device__ __forceinline__ void st_shared_u32(uint32_t smem_addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(smem_addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_shared_u16(uint32_t smem_addr, unsigned short v) {
+  asm volatile("st.shared.u16 [%0], %1;" ::"r"(smem_addr), "h"(v) : "memory");
+}
+
 // byte offset of (row, 16-byte chunk c) inside a SW128 K-major tile
 __host__ __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t chunk) {
   return row * 128u + ((chunk ^ (row & 7u)) << 4);
@@ -34,6 +41,19 @@ __device__ __forceinline__ uint64_t desc_sw128(uint32_t smem_addr_bytes) {
   d |= (uint64_t)((smem_addr_bytes & 0x3FFFF) >> 4);   // start address
   d |= (uint64_t)1 << 16;                               // leading byte offset (unused for SW128 K-major)
   d |= (uint64_t)(1024 >> 4) << 32;                     // stride byte offset: 8 rows * 128 B
+  d |= (uint64_t)1 << 62;                               // SWIZZLE_128B
+  return d;
+}
+
+// wgmma shared-memory matrix descriptor: MN-major, SWIZZLE_128B.  Each 128-byte row holds 64 consecutive
+// M (or N) elements of one K index, rows swizzled as in a K-major tile, so a K-major tile read this way is its
+// own transpose.  Stride byte offset: 8 K rows (1024 B) to the next 8; leading byte offset: one 64-element MN
+// block to the next, never reached by a 64-wide operand.  One K = 16 step advances the start by 2048 B.
+__device__ __forceinline__ uint64_t desc_sw128_mn(uint32_t smem_addr_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr_bytes & 0x3FFFF) >> 4);   // start address
+  d |= (uint64_t)(1024 >> 4) << 16;                     // leading byte offset (unused at 64 MN elements)
+  d |= (uint64_t)(1024 >> 4) << 32;                     // stride byte offset: 8 K rows * 128 B
   d |= (uint64_t)1 << 62;                               // SWIZZLE_128B
   return d;
 }
@@ -96,6 +116,15 @@ __device__ __forceinline__ void mma_m64n16_rs(float (&d)[8], const uint32_t (&a)
       "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(accumulate));
+}
+// D[64 x 8] (+)= A[smem desc, MN-major: desc_sw128_mn] * B[smem desc, K-major]
+__device__ __forceinline__ void mma_m64n8_ss_amn(float (&d)[4], uint64_t a, uint64_t b, int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3}, %4, %5, p, 1, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "l"(a), "l"(b), "r"(accumulate));
 }
 
 // D[64 x 64] (+)= A[smem desc] * B[smem desc]
@@ -163,9 +192,19 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
                : "memory");
 }
 
+// brings the line holding p into L1 (and L2); no register waits for it
+__device__ __forceinline__ void prefetch_l1(const void* p) {
+  asm volatile("prefetch.global.L1 [%0];" ::"l"(p));
+}
+
 // ---- cp.async, named barriers --------------------------------------------------------------
 __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+// copies the first src_bytes (0 or 16) of src and zero-fills the rest of the 16 bytes; 0 reads nothing
+__device__ __forceinline__ void cp_async16_zfill(void* dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(src_bytes)
+               : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
