@@ -591,6 +591,29 @@ int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id, const floa
                      int32_t* user_ids, float* user_factors, int32_t* n_users, int32_t* movie_ids,
                      float* movie_factors, int32_t* n_movies);
 
+/* Many ALS fits over one rating set in one pass (CrossValidator's fold x grid models, DESIGN.md section 4.15).
+ * fold [n_ratings] gives each rating a fold in 0..n_folds-1 (2 <= n_folds <= 65536).  Model m of the n_models
+ * (1..64) trains on the ratings outside fold models[m].exclude_fold (-1: on all of them) with its own rank,
+ * max_iter and reg_param and the shared `seed`; its result is bit for bit what srs_als_fit_host returns on those
+ * ratings in input order.  A model's users and movies are those with a training rating in it.  Output of model m,
+ * with R_m = the sum of the ranks of models 0..m-1: n_users[m] user ids at user_ids + m * user_capacity and their
+ * factors at user_factors + user_capacity * R_m ([n_users[m]][rank]); movies likewise.  The capacities must hold
+ * every distinct id of the whole set (else SRS_ERR_RANGE).  Every input is checked before any device call,
+ * including that no model's training set is empty (SRS_ERR_INVALID).  A singular system gives SRS_ERR_INVALID
+ * naming the lowest failing model and its user or movie, and nothing is written.  Synchronous; the same inputs give
+ * the same bits. */
+typedef struct srs_als_model {
+  int32_t rank;                       /* 1..64 */
+  int32_t max_iter;                   /* >= 1 */
+  double reg_param;                   /* finite, >= 0 */
+  int32_t exclude_fold;               /* -1 or 0..n_folds-1 */
+} srs_als_model;
+int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* movie_id, const float* rating, const int32_t* fold,
+                           int64_t n_ratings, int32_t n_folds, const srs_als_model* models, int32_t n_models,
+                           uint64_t seed, int32_t device, int32_t user_capacity, int32_t movie_capacity,
+                           int32_t* user_ids, float* user_factors, int32_t* n_users, int32_t* movie_ids,
+                           float* movie_factors, int32_t* n_movies);
+
 /* ALSModel.recommendForAll: for each of n_src source factors [n_src][rank] (host), the L = min(num, n_dst)
  * destinations of highest score, best first, in out_ids / out_scores [n_src][L].  The score is the float dot
  * sum += src(d) * dst(d) from 0.0f, d ascending, each operation rounded once.  Ties go to the lower destination id

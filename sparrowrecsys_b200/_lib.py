@@ -48,7 +48,7 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_trainer_create", "srs_trainer_destroy", "srs_trainer_fit_host", "srs_trainer_get_weights",
            "srs_trainer_iterations", "srs_trainer_fit_validate_host", "srs_trainer_evaluate_host",
            "srs_featureeng_host", "srs_item2vec_host", "srs_user_embeddings_host", "srs_als_fit_host",
-           "srs_als_recommend_host", "srs_item_transitions_host", "srs_random_walks_host",
+           "srs_als_fit_folds_host", "srs_als_recommend_host", "srs_item_transitions_host", "srs_random_walks_host",
            "srs_graph_embedding_host", "srs_lsh_transform_host", "srs_lsh_query_host")
 
 _lib = None
@@ -94,6 +94,12 @@ class SrsItem2vecParams(C.Structure):
 class SrsAlsParams(C.Structure):
     """`srs_als_params` (include/srs_ctr.h): ALS's settings."""
     _fields_ = [("rank", C.c_int32), ("max_iter", C.c_int32), ("reg_param", C.c_double), ("seed", C.c_uint64)]
+
+
+class SrsAlsModel(C.Structure):
+    """`srs_als_model` (include/srs_ctr.h): one model of a batched ALS fit."""
+    _fields_ = [("rank", C.c_int32), ("max_iter", C.c_int32), ("reg_param", C.c_double),
+                ("exclude_fold", C.c_int32)]
 
 
 class SrsError(RuntimeError):
@@ -249,6 +255,10 @@ def load():
     lib.srs_als_fit_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(SrsAlsParams),
                                      C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32),
                                      C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]
+    lib.srs_als_fit_folds_host.restype = C.c_int
+    lib.srs_als_fit_folds_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
+                                           C.c_void_p, C.c_int32, C.c_uint64, C.c_int32, C.c_int32, C.c_int32,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.srs_als_recommend_host.restype = C.c_int
     lib.srs_als_recommend_host.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                            C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]

@@ -10,15 +10,19 @@ them.
 * `als` trains on one device (`srs_als_fit_host`) and returns an `AlsModel`.
 * `AlsModel.transform` predicts on the host with ALSModel's float dot; `rmse` is RegressionEvaluator("rmse").
 * `AlsModel.recommend_for_*` score and keep the top `num` on one device (`srs_als_recommend_host`).
+* `cross_validate` is the job's last step, `CrossValidator` over a `ParamGridBuilder` grid: every fold x grid model
+  trained in one batched device pass (`als_folds`, `srs_als_fit_folds_host`; DESIGN.md section 4.15).
 
-    python -m sparrowrecsys_b200.collab ratings.csv
+    python -m sparrowrecsys_b200.collab ratings.csv [--cv]
 """
 from __future__ import annotations
 
 import ctypes as C
 import math
+import struct
 import sys
-from typing import Mapping, Sequence, Tuple
+from dataclasses import dataclass
+from typing import List, Mapping, Sequence, Tuple
 
 import numpy as np
 
@@ -83,21 +87,38 @@ class AlsModel:
         self.rank = user_factors.shape[1]
         self.device = device
 
-    def transform(self, ratings: Mapping[str, np.ndarray]) -> Tuple[np.ndarray, np.ndarray]:
-        """ALSModel.transform with coldStartStrategy "drop": rows whose user or movie has no factor are dropped.
-        Returns (kept row indices int64, predictions float32): dot += u(d) * m(d) from 0.0f, d ascending."""
+    def _lookup(self, ratings):
+        """(user factor row, movie factor row, both known) of each rating row."""
         user = np.asarray(ratings["userId"], np.int64)
         movie = np.asarray(ratings["movieId"], np.int64)
         ui = np.searchsorted(self.user_ids, user)
         mi = np.searchsorted(self.item_ids, movie)
         ok = (ui < len(self.user_ids)) & (mi < len(self.item_ids))
         ok[ok] &= (self.user_ids[ui[ok]] == user[ok]) & (self.item_ids[mi[ok]] == movie[ok])
+        return ui, mi, ok
+
+    def cold_rows(self, ratings: Mapping[str, np.ndarray]) -> int:
+        """The number of rows whose user or movie has no factor."""
+        return int(np.count_nonzero(~self._lookup(ratings)[2]))
+
+    def transform(self, ratings: Mapping[str, np.ndarray],
+                  cold_start_strategy: str = "drop") -> Tuple[np.ndarray, np.ndarray]:
+        """ALSModel.transform: dot += u(d) * m(d) from 0.0f, d ascending, for rows whose user and movie have
+        factors.  coldStartStrategy "drop" drops the other rows; "nan" (Spark's default) keeps them with a NaN
+        prediction.  Returns (row indices int64, predictions float32)."""
+        if cold_start_strategy not in ("drop", "nan"):
+            raise ValueError("cold_start_strategy must be 'drop' or 'nan', not %r" % (cold_start_strategy,))
+        ui, mi, ok = self._lookup(ratings)
         rows = np.flatnonzero(ok)
         uf, mf = self.user_factors[ui[rows]], self.item_factors[mi[rows]]
         pred = np.zeros(len(rows), np.float32)
         for d in range(self.rank):
             pred = pred + uf[:, d] * mf[:, d]
-        return rows, pred
+        if cold_start_strategy == "drop":
+            return rows, pred
+        out = np.full(len(ok), np.nan, np.float32)
+        out[rows] = pred
+        return np.arange(len(ok), dtype=np.int64), out
 
     def recommend_for_all_users(self, num: int):
         """(user ids [U], movie ids [U][L], scores [U][L]), L = min(num, movies)."""
@@ -153,14 +174,204 @@ def als(ratings: Mapping[str, np.ndarray], rank: int = 10, max_iter: int = 5, re
                     device)
 
 
+MAX_BATCH_MODELS = 64
+
+
+def als_folds(ratings: Mapping[str, np.ndarray], fold, n_folds: int, models: Sequence[Mapping], seed: int = 0,
+              device: int = 0) -> List[AlsModel]:
+    """Many ALS.fit calls over one rating set in one device pass (`srs_als_fit_folds_host`).  `fold` [n] gives each
+    row a fold in 0..n_folds-1; each of the (at most 64) `models` is a mapping with rank, max_iter, reg_param and
+    exclude_fold (-1: train on every row).  Model m trains on the rows outside its excluded fold, and its factors
+    are bit for bit `als` on those rows in input order with its settings and `seed`."""
+    user = np.ascontiguousarray(ratings["userId"], np.int32)
+    movie = np.ascontiguousarray(ratings["movieId"], np.int32)
+    rating = np.ascontiguousarray(ratings["rating"], np.float32)
+    fold = np.ascontiguousarray(fold, np.int32)
+    n = user.shape[0]
+    if movie.shape[0] != n or rating.shape[0] != n or fold.shape[0] != n:
+        raise ValueError("ratings columns and fold differ in length")
+    M = len(models)
+    specs = (_lib.SrsAlsModel * max(M, 1))()
+    for i, p in enumerate(models):
+        specs[i] = _lib.SrsAlsModel(int(p["rank"]), int(p["max_iter"]), float(p["reg_param"]),
+                                    int(p["exclude_fold"]))
+    cu, cm = max(1, int(np.unique(user).size)), max(1, int(np.unique(movie).size))
+    ranks = [max(1, int(p["rank"])) for p in models] or [1]
+    uids, mids = np.zeros((len(ranks), cu), np.int32), np.zeros((len(ranks), cm), np.int32)
+    uf, mf = np.zeros(cu * sum(ranks), np.float32), np.zeros(cm * sum(ranks), np.float32)
+    nu, nm = np.zeros(len(ranks), np.int32), np.zeros(len(ranks), np.int32)
+    _lib.check(_lib.load().srs_als_fit_folds_host(_p(user), _p(movie), _p(rating), _p(fold), n, int(n_folds), specs,
+                                                  M, int(seed) & _M64, device, cu, cm, _p(uids), _p(uf), _p(nu),
+                                                  _p(mids), _p(mf), _p(nm)))
+    out, r0 = [], 0
+    for m, k in enumerate(ranks[:M]):
+        U = uf[cu * r0:cu * (r0 + k)].reshape(cu, k)
+        V = mf[cm * r0:cm * (r0 + k)].reshape(cm, k)
+        out.append(AlsModel(uids[m, :nu[m]].copy(), U[:nu[m]].copy(), mids[m, :nm[m]].copy(), V[:nm[m]].copy(),
+                            device))
+        r0 += k
+    return out
+
+
+def _sum_sq(labels, predictions):
+    d = np.asarray(labels, np.float32).astype(np.float64) - np.asarray(predictions, np.float32).astype(np.float64)
+    return d, (float(np.cumsum(d * d)[-1]) if d.size else 0.0)
+
+
 def rmse(labels, predictions) -> float:
     """RegressionEvaluator("rmse") as Spark 2.4's RegressionMetrics computes it: the L2 norm of (label -
     prediction) in double, summed in row order, squared, over the count, then the square root."""
-    d = np.asarray(labels, np.float32).astype(np.float64) - np.asarray(predictions, np.float32).astype(np.float64)
+    d, ss = _sum_sq(labels, predictions)
     if d.size == 0:
         return float("nan")
-    norm = math.sqrt(float(np.cumsum(d * d)[-1]))
+    norm = math.sqrt(ss)
     return math.sqrt(norm * norm / d.size)
+
+
+def mse(labels, predictions) -> float:
+    """RegressionEvaluator("mse"): rmse's value before the square root, the squared L2 norm over the count."""
+    d, ss = _sum_sq(labels, predictions)
+    if d.size == 0:
+        return float("nan")
+    norm = math.sqrt(ss)
+    return norm * norm / d.size
+
+
+def mae(labels, predictions) -> float:
+    """RegressionEvaluator("mae"): |label - prediction| in double, summed in row order, over the count."""
+    d, _ = _sum_sq(labels, predictions)
+    if d.size == 0:
+        return float("nan")
+    return float(np.cumsum(np.abs(d))[-1]) / d.size
+
+
+METRICS = {"rmse": rmse, "mse": mse, "mae": mae}
+_GRID_PARAMS = ("rank", "reg_param", "max_iter")
+
+
+def fold_ids(n: int, num_folds: int, seed: int = 0) -> np.ndarray:
+    """MLUtils.kFold's fold of each row (0-based): row i draws `_uniforms(seed, n)[i]` once, the same draw for every
+    fold, and fold f validates the rows with lb <= u < ub, lb = (f - 1) / k and ub = f / k (f = 1..k) computed as
+    float32 quotients (Spark's `(fold - 1) / numFolds.toFloat`) and widened to double.  Returns int32 [n]."""
+    if int(num_folds) < 2:
+        raise ValueError("num_folds must be >= 2, not %d" % int(num_folds))
+    return _fold_of(_uniforms(int(seed), int(n)), int(num_folds))
+
+
+def _fold_of(u, k):
+    out = np.full(len(u), -1, np.int32)
+    for f in range(1, k + 1):
+        lb = float(np.float32(f - 1) / np.float32(k))
+        ub = float(np.float32(f) / np.float32(k))
+        out[(u >= lb) & (u < ub)] = f - 1
+    return out
+
+
+def k_fold(n: int, num_folds: int, seed: int = 0):
+    """MLUtils.kFold: one (training rows, validation rows) pair of ascending int64 indices per fold, the training
+    rows the complement of the validation rows (see `fold_ids`)."""
+    f = fold_ids(n, num_folds, seed)
+    return [(np.flatnonzero(f != i), np.flatnonzero(f == i)) for i in range(int(num_folds))]
+
+
+def param_maps(param_grid) -> List[dict]:
+    """ParamGridBuilder.build over an ordered list of (param, values) pairs (or a dict, in its order) of "rank",
+    "reg_param" and "max_iter": every combination, the first param varying fastest.  No params give one empty
+    map, as Spark's builder does; a param with no values gives none, which is an error here."""
+    pairs = list(param_grid.items()) if isinstance(param_grid, Mapping) else [tuple(p) for p in param_grid]
+    names = [p[0] for p in pairs]
+    if any(name not in _GRID_PARAMS for name in names) or len(set(names)) != len(names):
+        raise ValueError("grid params must be distinct names from %s, not %s" % (_GRID_PARAMS, names))
+    maps = [{}]
+    for name, values in pairs:
+        maps = [dict(m, **{name: v}) for v in values for m in maps]
+    if not maps:
+        raise ValueError("the parameter grid is empty")
+    return maps
+
+
+def _java_compare(a: float, b: float) -> int:
+    """java.lang.Double.compare: numeric order, then the bits (-0.0 < 0.0, NaN above everything)."""
+    if a < b:
+        return -1
+    if a > b:
+        return 1
+
+    def bits(x):
+        return 0x7FF8000000000000 if math.isnan(x) else struct.unpack("<q", struct.pack("<d", x))[0]
+    return (bits(a) > bits(b)) - (bits(a) < bits(b))
+
+
+def average_metrics(fold_metrics) -> List[float]:
+    """CrossValidator's avgMetrics from fold_metrics [k][P]: per grid point the sum over folds in fold order, in
+    double from 0.0, over k."""
+    k = len(fold_metrics)
+    avg = []
+    for p in range(len(fold_metrics[0])):
+        s = 0.0
+        for f in range(k):
+            s += float(fold_metrics[f][p])
+        avg.append(s / k)
+    return avg
+
+
+def best_index(metrics: Sequence[float]) -> int:
+    """CrossValidator's minBy over the average metrics (rmse, mse and mae are smaller-is-better) in
+    java.lang.Double.compare's order: NaN ranks last, and the first index wins a tie."""
+    best = 0
+    for i in range(1, len(metrics)):
+        if _java_compare(float(metrics[i]), float(metrics[best])) < 0:
+            best = i
+    return best
+
+
+@dataclass
+class CrossValidation:
+    """What `cross_validate` returns.  avg_metrics [P] and fold_metrics [k][P] follow param_maps' order;
+    param_maps holds each grid point's full settings; cold_rows [k] counts each fold's validation rows whose user or
+    movie has no factor in that fold's models."""
+    avg_metrics: List[float]
+    fold_metrics: List[List[float]]
+    best_index: int
+    best_params: dict
+    best_model: AlsModel
+    param_maps: List[dict]
+    cold_rows: List[int]
+
+
+def cross_validate(ratings: Mapping[str, np.ndarray], param_grid, num_folds: int = 10, metric: str = "rmse",
+                   cold_start_strategy: str = "nan", seed: int = 0, rank: int = 10, max_iter: int = 5,
+                   reg_param: float = 0.01, als_seed: int = 0, device: int = 0) -> CrossValidation:
+    """CrossValidator(ALS, RegressionEvaluator(metric), param_grid, num_folds).fit(ratings) on the device.  Every
+    fold x grid model is trained in batched passes of at most 64 models (`als_folds`); params not in the grid take
+    rank, max_iter and reg_param, and every fit uses `als_seed`.  Each model predicts its validation rows with
+    `cold_start_strategy` ("nan", the estimator's default, makes a fold with a cold row score NaN), avg_metrics[p]
+    is the fold-order sum over k, and the best point (`best_index`) is refit on all rows by `als`."""
+    if metric not in METRICS:
+        raise ValueError("metric must be one of %s, not %r" % (sorted(METRICS), metric))
+    if cold_start_strategy not in ("drop", "nan"):
+        raise ValueError("cold_start_strategy must be 'drop' or 'nan', not %r" % (cold_start_strategy,))
+    points = [dict(dict(rank=rank, max_iter=max_iter, reg_param=reg_param), **pm) for pm in param_maps(param_grid)]
+    k, P = int(num_folds), len(points)
+    n = len(ratings["userId"])
+    fold = fold_ids(n, k, seed)
+    specs = [dict(p, exclude_fold=f) for f in range(k) for p in points]
+    models = []
+    for i in range(0, len(specs), MAX_BATCH_MODELS):
+        models += als_folds(ratings, fold, k, specs[i:i + MAX_BATCH_MODELS], als_seed, device)
+    fold_metrics, cold = [], []
+    for f in range(k):
+        val = {c: np.asarray(v)[fold == f] for c, v in ratings.items()}
+        cold.append(models[f * P].cold_rows(val))
+        row = []
+        for p in range(P):
+            rows, pred = models[f * P + p].transform(val, cold_start_strategy)
+            row.append(METRICS[metric](np.asarray(val["rating"])[rows], pred))
+        fold_metrics.append(row)
+    avg = average_metrics(fold_metrics)
+    best = best_index(avg)
+    model = als(ratings, points[best]["rank"], points[best]["max_iter"], points[best]["reg_param"], als_seed, device)
+    return CrossValidation(avg, fold_metrics, best, dict(points[best]), model, points, cold)
 
 
 def _show(title, ids, rec, sc, rows=10):
@@ -171,11 +382,13 @@ def _show(title, ids, rec, sc, rows=10):
 
 def main(argv=None) -> int:
     argv = sys.argv[1:] if argv is None else argv
-    if len(argv) != 1:
-        sys.stderr.write("usage: python -m sparrowrecsys_b200.collab ratings.csv\n")
+    cv = "--cv" in argv
+    args = [a for a in argv if a != "--cv"]
+    if len(args) != 1:
+        sys.stderr.write("usage: python -m sparrowrecsys_b200.collab ratings.csv [--cv]\n")
         return 2
     from .featureeng import load_ratings_csv
-    r = load_ratings_csv(argv[0])
+    r = load_ratings_csv(args[0])
     train_rows, test_rows = random_split(len(r["userId"]), (0.8, 0.2), seed=0)
     train = {k: v[train_rows] for k, v in r.items()}
     test = {k: v[test_rows] for k, v in r.items()}
@@ -195,6 +408,10 @@ def main(argv=None) -> int:
     movies = r["movieId"][np.sort(first_movies)[:3]]
     _show("userSubsetRecs", *model.recommend_for_user_subset(users, 10))
     _show("movieSubSetRecs", *model.recommend_for_item_subset(movies, 10))
+    if cv:                                                  # cv.fit(test): regParam grid [0.01], 10 folds
+        res = cross_validate(test, [("reg_param", [0.01])], num_folds=10)
+        print("avgMetrics = %r" % res.avg_metrics)
+        print("cold validation rows per fold = %r" % res.cold_rows)
     return 0
 
 

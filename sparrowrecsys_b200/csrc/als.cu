@@ -17,6 +17,11 @@
 // bits as oracle/als_c.c.  A non-positive or NaN pivot latches (half-step, entity) in an error word (atomicMin:
 // the first half-step, then the lowest entity).
 //
+// srs_als_fit_folds_host (DESIGN.md section 4.15) fits up to 64 models - each its own rank, max_iter, reg_param and
+// excluded fold - over one rating set: the layouts of steps 1-2 once, each rating's fold gathered into both, then one
+// als_solve_kernel<true> launch per half-step for every model.  A fold's subset of a layout keeps its order, so
+// each model's results are bit for bit srs_als_fit_host's on its training ratings.
+//
 // als_recommend_kernel (srs_als_recommend_host): 32 sources per block, 4 per warp; destinations stream through
 // shared memory in tiles of 128, transposed so that each lane reads its own 4.  Each lane computes 4 x 4 exact
 // sequential float dots (__fmul_rn / __fadd_rn from 0.0f, no fma); the warp keeps a sorted list of `num` per
@@ -41,6 +46,8 @@ namespace {
 constexpr int kMaxRank = 64;           // one thread per factor column
 constexpr int kMaxNum = 128;           // four list entries per lane
 constexpr int64_t kMaxRatings = 21000000;
+constexpr int kMaxModels = 64;         // models of one batched fit
+constexpr int kMaxFolds = 65536;
 constexpr int kSolveThreads = 128;
 constexpr int kChunk = 32;             // ratings staged per step of the accumulation
 constexpr int kRecWarps = 8;
@@ -158,13 +165,47 @@ struct Side {
   int nE;
 };
 
-// One block per entity (blockIdx.x-th longest): NormalEquation.add over its ratings, then
-// CholeskySolver.solve(ne, n * regParam) (dppsv "U": dpptrf, then dpptrs's two dtpsv).
+// One model of a batched fit (srs_als_fit_folds_host)
+struct BatchModel {
+  int k;
+  int half_steps;                      // 2 * max_iter
+  double reg;
+  int exclude;                         // the fold whose ratings it skips; -1: none
+  size_t user_off, movie_off;          // its [nU][k] user and [nM][k] movie factors in the shared arrays
+};
+
+struct Batch {
+  const BatchModel* models;            // [M]
+  const int32_t* fold;                 // [n] fold of each rating, in the side's layout order
+  int32_t* count;                      // [M][nE] each entity's training ratings in each model
+  int M;
+  bool to_users;                       // this half-step solves the users from the movies
+};
+
+// One block per entity (the blockIdx.x-th longest; batched: block b is model b % M's (b / M)-th longest entity):
+// NormalEquation.add over its ratings, then CholeskySolver.solve(ne, n * regParam) (dppsv "U": dpptrf, then
+// dpptrs's two dtpsv).  A batched model skips its excluded fold's ratings, so its n counts the rest; an entity with
+// none is not in that model and its block writes nothing but the count.
+template <bool kBatch>
 __global__ void __launch_bounds__(kSolveThreads) als_solve_kernel(Side sd, const float* __restrict__ srcF,
                                                                   float* __restrict__ dstF, int k, double reg,
                                                                   unsigned long long* __restrict__ err,
-                                                                  unsigned long long half_step) {
+                                                                  unsigned long long half_step, Batch bt) {
   extern __shared__ __align__(16) unsigned char smem[];
+  __shared__ uint8_t s_keep[kChunk];
+  int m = 0, exclude = -1, pos = blockIdx.x;
+  if (kBatch) {
+    m = blockIdx.x % bt.M;
+    pos = blockIdx.x / bt.M;
+    const BatchModel md = bt.models[m];
+    if (half_step >= (unsigned long long)md.half_steps) return;   // this model has finished
+    k = md.k;
+    reg = md.reg;
+    exclude = md.exclude;
+    srcF += bt.to_users ? md.movie_off : md.user_off;
+    dstF += bt.to_users ? md.user_off : md.movie_off;
+    err += m;
+  }
   const int nA = k * (k + 1) / 2;
   double* P = reinterpret_cast<double*>(smem);          // [nA] packed upper ata, then [k] atb
   double* B = P + nA;
@@ -176,8 +217,9 @@ __global__ void __launch_bounds__(kSolveThreads) als_solve_kernel(Side sd, const
   __shared__ int s_bad;
   __shared__ int s_nz[kMaxRank];
   const int tid = threadIdx.x;
-  const int ent = sd.order[blockIdx.x];
+  const int ent = sd.order[pos];
   const int lo0 = sd.off[ent], hi = sd.off[ent + 1];
+  int n_train = hi - lo0;
   for (int e = tid; e < nA; e += kSolveThreads) {
     int j = 0;
     while ((j + 1) * (j + 2) / 2 <= e) ++j;
@@ -186,6 +228,7 @@ __global__ void __launch_bounds__(kSolveThreads) als_solve_kernel(Side sd, const
   }
   for (int e = tid; e < nA + k; e += kSolveThreads) P[e] = 0.0;
   if (tid == 0) s_bad = 0;
+  if (kBatch) n_train = 0;
   for (int lo = lo0; lo < hi; lo += kChunk) {
     const int cn = min(kChunk, hi - lo);
     __syncthreads();                                    // the previous chunk is consumed
@@ -193,19 +236,26 @@ __global__ void __launch_bounds__(kSolveThreads) als_solve_kernel(Side sd, const
       const int c = t / k;
       s_x[t] = srcF[(size_t)sd.src[lo + c] * k + (t - c * k)];
     }
-    for (int t = tid; t < cn; t += kSolveThreads) s_r[t] = sd.r[lo + t];
+    for (int t = tid; t < cn; t += kSolveThreads) {
+      s_r[t] = sd.r[lo + t];
+      if (kBatch) s_keep[t] = bt.fold[lo + t] != exclude;
+    }
     __syncthreads();
+    if (kBatch)
+      for (int c = 0; c < cn; ++c) n_train += s_keep[c];
     for (int e = tid; e < nA + k; e += kSolveThreads) {
       double a = P[e];
       if (e < nA) {                                     // dspr: ap(i,j) += x(i) * (1.0 * x(j)), skipped for x(j) == 0
         const int i = s_i[e], j = s_j[e];
         for (int c = 0; c < cn; ++c) {
+          if (kBatch && !s_keep[c]) continue;
           const float xj = s_x[c * k + j];
           if (xj != 0.0f) a = __dadd_rn(a, __dmul_rn((double)s_x[c * k + i], (double)xj));
         }
       } else {                                          // daxpy: atb(i) += rating * x(i), skipped for rating == 0
         const int i = e - nA;
         for (int c = 0; c < cn; ++c) {
+          if (kBatch && !s_keep[c]) continue;
           const float rv = s_r[c];
           if (rv != 0.0f) a = __dadd_rn(a, __dmul_rn((double)rv, (double)s_x[c * k + i]));
         }
@@ -214,7 +264,11 @@ __global__ void __launch_bounds__(kSolveThreads) als_solve_kernel(Side sd, const
     }
   }
   __syncthreads();
-  const double lambda = __dmul_rn((double)(hi - lo0), reg);
+  if (kBatch) {
+    if (tid == 0) bt.count[(size_t)m * sd.nE + ent] = n_train;
+    if (n_train == 0) return;                           // not in this model (every thread has the same count)
+  }
+  const double lambda = __dmul_rn((double)n_train, reg);
   if (tid < k) P[tid * (tid + 1) / 2 + tid] = __dadd_rn(P[tid * (tid + 1) / 2 + tid], lambda);
   __syncthreads();
   // dpptrf "U": in step r, U(r,r) = sqrt(a(r,r) - ddot(U(0:r,r), U(0:r,r))), then for c > r
@@ -421,45 +475,38 @@ int bits_for(int n) {
   return b;
 }
 
-}  // namespace
-}  // namespace srs
+int check_params(int32_t rank, int32_t max_iter, double reg_param) {
+  if (rank < 1 || rank > kMaxRank) return als_fail(SRS_ERR_INVALID, "rank %d outside 1..%d", rank, kMaxRank);
+  if (max_iter < 1) return als_fail(SRS_ERR_INVALID, "max_iter %d is not positive", max_iter);
+  if (!std::isfinite(reg_param) || reg_param < 0)
+    return als_fail(SRS_ERR_INVALID, "reg_param %g is not finite and >= 0", reg_param);
+  return SRS_OK;
+}
 
-using namespace srs;
-
-extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
-                                int64_t n_ratings, const srs_als_params* params, int32_t device,
-                                int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
-                                float* user_factors, int32_t* n_users, int32_t* movie_ids, float* movie_factors,
-                                int32_t* n_movies) {
-  if (!n_users || !n_movies) return als_fail(SRS_ERR_INVALID, "null n_users or n_movies");
-  *n_users = 0;
-  *n_movies = 0;
-  if (!params) return als_fail(SRS_ERR_INVALID, "null params");
-  const srs_als_params hp = *params;
-  if (hp.rank < 1 || hp.rank > kMaxRank) return als_fail(SRS_ERR_INVALID, "rank %d outside 1..%d", hp.rank, kMaxRank);
-  if (hp.max_iter < 1) return als_fail(SRS_ERR_INVALID, "max_iter %d is not positive", hp.max_iter);
-  if (!std::isfinite(hp.reg_param) || hp.reg_param < 0)
-    return als_fail(SRS_ERR_INVALID, "reg_param %g is not finite and >= 0", hp.reg_param);
+int check_ratings(const int32_t* user_id, const int32_t* movie_id, const float* rating, int64_t n_ratings) {
   if (n_ratings < 1 || n_ratings > kMaxRatings)
     return als_fail(SRS_ERR_INVALID, "n_ratings %lld outside 1..%lld", (long long)n_ratings, (long long)kMaxRatings);
   if (!user_id || !movie_id || !rating) return als_fail(SRS_ERR_INVALID, "null ratings");
-  if (user_capacity < 0 || movie_capacity < 0 || (user_capacity > 0 && (!user_ids || !user_factors)) ||
-      (movie_capacity > 0 && (!movie_ids || !movie_factors)))
-    return als_fail(SRS_ERR_INVALID, "negative capacity or null outputs");
-  const int n = (int)n_ratings;
-  for (int i = 0; i < n; ++i) {
+  for (int64_t i = 0; i < n_ratings; ++i) {
     if (user_id[i] < 0 || movie_id[i] < 0)
-      return als_fail(SRS_ERR_INVALID, "rating %d: negative id (user %d, movie %d)", i, user_id[i], movie_id[i]);
-    if (!std::isfinite(rating[i])) return als_fail(SRS_ERR_INVALID, "rating %d is not finite", i);
+      return als_fail(SRS_ERR_INVALID, "rating %d: negative id (user %d, movie %d)", (int)i, user_id[i], movie_id[i]);
+    if (!std::isfinite(rating[i])) return als_fail(SRS_ERR_INVALID, "rating %d is not finite", (int)i);
   }
-  if (int rc = select_device(device)) return rc;
+  return SRS_OK;
+}
 
-  Scratch sc;
-  CubTemp ct{&sc};
-  StreamGuard sg;
-  ALS_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
-  cudaStream_t s = sg.s;
-  const int T = 256, G = grid_for(n, T), k = hp.rank;
+// One rating set's dense ids and both layouts on the device (steps 1 and 2 of srs_als_fit_host)
+struct Layouts {
+  int nU = 0, nM = 0;
+  int32_t *d_uids, *d_mids;            // the dense ids' raw ids, ascending
+  int32_t *d_bm, *d_bu;                // input row of each by-movie / by-user layout position
+  Side movies, users;
+  std::vector<int32_t> uid;            // d_uids on the host
+};
+
+int build_layouts(Scratch& sc, CubTemp& ct, cudaStream_t s, const int32_t* user_id, const int32_t* movie_id,
+                  const float* rating, int n, int32_t user_capacity, int32_t movie_capacity, Layouts* L) {
+  const int T = 256, G = grid_for(n, T);
   int32_t *d_user, *d_movie, *d_iota, *d_key, *d_perm_u, *d_perm_m, *d_head, *d_seg, *d_du, *d_dm;
   int32_t *d_uids, *d_ucnt, *d_mids, *d_mcnt, *d_bm, *d_bu, *d_src_m, *d_src_u;
   float *d_rating, *d_r_m, *d_r_u;
@@ -499,8 +546,8 @@ extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id,
   const int nU = counts[0], nM = counts[1];
   if (nU > user_capacity) return als_fail(SRS_ERR_RANGE, "%d users exceed capacity %d", nU, user_capacity);
   if (nM > movie_capacity) return als_fail(SRS_ERR_RANGE, "%d movies exceed capacity %d", nM, movie_capacity);
-  std::vector<int32_t> uid(nU);
-  ALS_TRY(cudaMemcpyAsync(uid.data(), d_uids, sizeof(int32_t) * nU, cudaMemcpyDeviceToHost, s));
+  L->uid.resize(nU);
+  ALS_TRY(cudaMemcpyAsync(L->uid.data(), d_uids, sizeof(int32_t) * nU, cudaMemcpyDeviceToHost, s));
 
   // by-movie layout: the (user, input)-ordered ratings stably sorted by dense movie; by-user: that by dense user
   als_key_kernel<<<G, T, 0, s>>>(d_perm_u, d_dm, n, d_key);
@@ -523,22 +570,65 @@ extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id,
   ALS_CUB(cub::DeviceScan::ExclusiveSum(tmp__, tb__, d_ucnt, d_uoff, nU + 1, s));
   ALS_CUB(cub::DeviceRadixSort::SortPairsDescending(tmp__, tb__, d_mcnt, d_key, d_iota, d_morder, nM, 0, 31, s));
   ALS_CUB(cub::DeviceRadixSort::SortPairsDescending(tmp__, tb__, d_ucnt, d_key, d_iota, d_uorder, nU, 0, 31, s));
+  L->nU = nU;
+  L->nM = nM;
+  L->d_uids = d_uids;
+  L->d_mids = d_mids;
+  L->d_bm = d_bm;
+  L->d_bu = d_bu;
+  L->movies = Side{d_moff, d_src_m, d_r_m, d_morder, nM};
+  L->users = Side{d_uoff, d_src_u, d_r_u, d_uorder, nU};
+  return SRS_OK;
+}
+
+}  // namespace
+}  // namespace srs
+
+using namespace srs;
+
+extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
+                                int64_t n_ratings, const srs_als_params* params, int32_t device,
+                                int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
+                                float* user_factors, int32_t* n_users, int32_t* movie_ids, float* movie_factors,
+                                int32_t* n_movies) {
+  if (!n_users || !n_movies) return als_fail(SRS_ERR_INVALID, "null n_users or n_movies");
+  *n_users = 0;
+  *n_movies = 0;
+  if (!params) return als_fail(SRS_ERR_INVALID, "null params");
+  const srs_als_params hp = *params;
+  if (int rc = check_params(hp.rank, hp.max_iter, hp.reg_param)) return rc;
+  if (int rc = check_ratings(user_id, movie_id, rating, n_ratings)) return rc;
+  if (user_capacity < 0 || movie_capacity < 0 || (user_capacity > 0 && (!user_ids || !user_factors)) ||
+      (movie_capacity > 0 && (!movie_ids || !movie_factors)))
+    return als_fail(SRS_ERR_INVALID, "negative capacity or null outputs");
+  if (int rc = select_device(device)) return rc;
+
+  Scratch sc;
+  CubTemp ct{&sc};
+  StreamGuard sg;
+  ALS_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+  cudaStream_t s = sg.s;
+  const int k = hp.rank;
+  Layouts L;
+  if (int rc = build_layouts(sc, ct, s, user_id, movie_id, rating, (int)n_ratings, user_capacity, movie_capacity, &L))
+    return rc;
+  const int nU = L.nU, nM = L.nM;
 
   // the users' initial factors, drawn on the host
   std::vector<float> init((size_t)nU * k);
-  for (int u = 0; u < nU; ++u) init_factor(hp.seed, uid[u], k, init.data() + (size_t)u * k);
+  for (int u = 0; u < nU; ++u) init_factor(hp.seed, L.uid[u], k, init.data() + (size_t)u * k);
   float *d_uf, *d_mf;
   unsigned long long* d_err;
   ALS_TRY(sc.alloc(&d_uf, (size_t)nU * k)); ALS_TRY(sc.alloc(&d_mf, (size_t)nM * k)); ALS_TRY(sc.alloc(&d_err, 1));
   ALS_TRY(cudaMemcpyAsync(d_uf, init.data(), sizeof(float) * init.size(), cudaMemcpyHostToDevice, s));
   ALS_TRY(cudaMemsetAsync(d_err, 0xff, sizeof(unsigned long long), s));
-  const Side movies{d_moff, d_src_m, d_r_m, d_morder, nM};
-  const Side users{d_uoff, d_src_u, d_r_u, d_uorder, nU};
   const size_t sm = solve_smem(k);
   for (int it = 0; it < hp.max_iter; ++it) {
-    als_solve_kernel<<<nM, kSolveThreads, sm, s>>>(movies, d_uf, d_mf, k, hp.reg_param, d_err, 2ull * it);
+    als_solve_kernel<false><<<nM, kSolveThreads, sm, s>>>(L.movies, d_uf, d_mf, k, hp.reg_param, d_err, 2ull * it,
+                                                          Batch{});
     ALS_LAUNCHED();
-    als_solve_kernel<<<nU, kSolveThreads, sm, s>>>(users, d_mf, d_uf, k, hp.reg_param, d_err, 2ull * it + 1);
+    als_solve_kernel<false><<<nU, kSolveThreads, sm, s>>>(L.users, d_mf, d_uf, k, hp.reg_param, d_err,
+                                                          2ull * it + 1, Batch{});
     ALS_LAUNCHED();
   }
   unsigned long long err = 0;
@@ -547,17 +637,158 @@ extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id,
   if (err != ~0ull) {
     const int hs = (int)(err >> 32), ent = (int)(err & 0xffffffffu);
     int32_t id = 0;
-    ALS_TRY(cudaMemcpy(&id, (hs & 1 ? d_uids : d_mids) + ent, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    ALS_TRY(cudaMemcpy(&id, (hs & 1 ? L.d_uids : L.d_mids) + ent, sizeof(int32_t), cudaMemcpyDeviceToHost));
     return als_fail(SRS_ERR_INVALID, "singular normal equations for %s %d in iteration %d (a pivot <= 0 or NaN)",
                     hs & 1 ? "user" : "movie", id, hs / 2 + 1);
   }
-  ALS_TRY(cudaMemcpyAsync(user_ids, d_uids, sizeof(int32_t) * nU, cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaMemcpyAsync(user_ids, L.d_uids, sizeof(int32_t) * nU, cudaMemcpyDeviceToHost, s));
   ALS_TRY(cudaMemcpyAsync(user_factors, d_uf, sizeof(float) * nU * k, cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaMemcpyAsync(movie_ids, d_mids, sizeof(int32_t) * nM, cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaMemcpyAsync(movie_ids, L.d_mids, sizeof(int32_t) * nM, cudaMemcpyDeviceToHost, s));
   ALS_TRY(cudaMemcpyAsync(movie_factors, d_mf, sizeof(float) * nM * k, cudaMemcpyDeviceToHost, s));
   ALS_TRY(cudaStreamSynchronize(s));
   *n_users = nU;
   *n_movies = nM;
+  return SRS_OK;
+}
+
+extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
+                                      const int32_t* fold, int64_t n_ratings, int32_t n_folds,
+                                      const srs_als_model* models, int32_t n_models, uint64_t seed, int32_t device,
+                                      int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
+                                      float* user_factors, int32_t* n_users, int32_t* movie_ids,
+                                      float* movie_factors, int32_t* n_movies) {
+  if (n_models < 1 || n_models > kMaxModels)
+    return als_fail(SRS_ERR_INVALID, "n_models %d outside 1..%d", n_models, kMaxModels);
+  if (!models || !n_users || !n_movies) return als_fail(SRS_ERR_INVALID, "null models, n_users or n_movies");
+  for (int m = 0; m < n_models; ++m) n_users[m] = n_movies[m] = 0;
+  if (n_folds < 2 || n_folds > kMaxFolds)
+    return als_fail(SRS_ERR_INVALID, "n_folds %d outside 2..%d", n_folds, kMaxFolds);
+  const std::vector<srs_als_model> md(models, models + n_models);
+  for (int m = 0; m < n_models; ++m) {
+    if (int rc = check_params(md[m].rank, md[m].max_iter, md[m].reg_param))
+      return als_fail(rc, "model %d: %s", m, srs_last_error());
+    if (md[m].exclude_fold < -1 || md[m].exclude_fold >= n_folds)
+      return als_fail(SRS_ERR_INVALID, "model %d: exclude_fold %d outside -1..%d", m, md[m].exclude_fold, n_folds - 1);
+  }
+  if (int rc = check_ratings(user_id, movie_id, rating, n_ratings)) return rc;
+  if (!fold) return als_fail(SRS_ERR_INVALID, "null fold");
+  if (user_capacity < 0 || movie_capacity < 0 || (user_capacity > 0 && (!user_ids || !user_factors)) ||
+      (movie_capacity > 0 && (!movie_ids || !movie_factors)))
+    return als_fail(SRS_ERR_INVALID, "negative capacity or null outputs");
+  const int n = (int)n_ratings;
+  std::vector<int64_t> in_fold(n_folds, 0);
+  for (int i = 0; i < n; ++i) {
+    if (fold[i] < 0 || fold[i] >= n_folds)
+      return als_fail(SRS_ERR_INVALID, "rating %d: fold %d outside 0..%d", i, fold[i], n_folds - 1);
+    ++in_fold[fold[i]];
+  }
+  for (int m = 0; m < n_models; ++m)
+    if (md[m].exclude_fold >= 0 && in_fold[md[m].exclude_fold] == n)
+      return als_fail(SRS_ERR_INVALID, "model %d: no training ratings (every rating is in fold %d)", m,
+                      md[m].exclude_fold);
+  if (int rc = select_device(device)) return rc;
+
+  Scratch sc;
+  CubTemp ct{&sc};
+  StreamGuard sg;
+  ALS_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+  cudaStream_t s = sg.s;
+  Layouts L;
+  if (int rc = build_layouts(sc, ct, s, user_id, movie_id, rating, n, user_capacity, movie_capacity, &L)) return rc;
+  const int nU = L.nU, nM = L.nM, M = n_models, T = 256, G = grid_for(n, T);
+
+  // each model's factors over every dense id of the whole set; the initial user factors depend on the rank only
+  std::vector<BatchModel> bm(M);
+  size_t uf_total = 0, mf_total = 0;
+  int kmax = 1, half_steps = 0;
+  for (int m = 0; m < M; ++m) {
+    bm[m] = BatchModel{md[m].rank, 2 * md[m].max_iter, md[m].reg_param, md[m].exclude_fold, uf_total, mf_total};
+    uf_total += (size_t)nU * md[m].rank;
+    mf_total += (size_t)nM * md[m].rank;
+    kmax = std::max(kmax, md[m].rank);
+    half_steps = std::max(half_steps, 2 * md[m].max_iter);
+  }
+  std::vector<float> init(uf_total);
+  std::vector<int> drawn(kMaxRank + 1, -1);            // the first model of each rank
+  for (int m = 0; m < M; ++m) {
+    const int k = md[m].rank;
+    float* dst = init.data() + bm[m].user_off;
+    if (drawn[k] >= 0) {
+      std::copy_n(init.data() + bm[drawn[k]].user_off, (size_t)nU * k, dst);
+      continue;
+    }
+    drawn[k] = m;
+    for (int u = 0; u < nU; ++u) init_factor(seed, L.uid[u], k, dst + (size_t)u * k);
+  }
+  int32_t *d_fold, *d_fold_m, *d_fold_u, *d_cnt_m, *d_cnt_u;
+  float *d_uf, *d_mf;
+  BatchModel* d_models;
+  unsigned long long* d_err;
+  ALS_TRY(sc.alloc(&d_fold, n)); ALS_TRY(sc.alloc(&d_fold_m, n)); ALS_TRY(sc.alloc(&d_fold_u, n));
+  ALS_TRY(sc.alloc(&d_cnt_m, (size_t)M * nM)); ALS_TRY(sc.alloc(&d_cnt_u, (size_t)M * nU));
+  ALS_TRY(sc.alloc(&d_uf, uf_total)); ALS_TRY(sc.alloc(&d_mf, mf_total));
+  ALS_TRY(sc.alloc(&d_models, M)); ALS_TRY(sc.alloc(&d_err, M));
+  ALS_TRY(cudaMemcpyAsync(d_fold, fold, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  ALS_TRY(cudaMemcpyAsync(d_uf, init.data(), sizeof(float) * uf_total, cudaMemcpyHostToDevice, s));
+  ALS_TRY(cudaMemcpyAsync(d_models, bm.data(), sizeof(BatchModel) * M, cudaMemcpyHostToDevice, s));
+  ALS_TRY(cudaMemsetAsync(d_err, 0xff, sizeof(unsigned long long) * M, s));
+  als_key_kernel<<<G, T, 0, s>>>(L.d_bm, d_fold, n, d_fold_m);      // each layout's fold ids
+  ALS_LAUNCHED();
+  als_key_kernel<<<G, T, 0, s>>>(L.d_bu, d_fold, n, d_fold_u);
+  ALS_LAUNCHED();
+  // one launch per half-step for every model: a model past its max_iter exits at once
+  const size_t sm = solve_smem(kmax);
+  for (int h = 0; h < half_steps; ++h) {
+    const bool to_users = h & 1;
+    const Batch bt{d_models, to_users ? d_fold_u : d_fold_m, to_users ? d_cnt_u : d_cnt_m, M, to_users};
+    const int nE = to_users ? nU : nM;
+    als_solve_kernel<true><<<(unsigned)((int64_t)nE * M), kSolveThreads, sm, s>>>(
+        to_users ? L.users : L.movies, to_users ? d_mf : d_uf, to_users ? d_uf : d_mf, 0, 0.0, d_err,
+        (unsigned long long)h, bt);
+    ALS_LAUNCHED();
+  }
+  std::vector<unsigned long long> err(M);
+  ALS_TRY(cudaMemcpyAsync(err.data(), d_err, sizeof(unsigned long long) * M, cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaStreamSynchronize(s));
+  for (int m = 0; m < M; ++m) {
+    if (err[m] == ~0ull) continue;
+    const int hs = (int)(err[m] >> 32), ent = (int)(err[m] & 0xffffffffu);
+    int32_t id = 0;
+    ALS_TRY(cudaMemcpy(&id, (hs & 1 ? L.d_uids : L.d_mids) + ent, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return als_fail(SRS_ERR_INVALID,
+                    "model %d: singular normal equations for %s %d in iteration %d (a pivot <= 0 or NaN)", m,
+                    hs & 1 ? "user" : "movie", id, hs / 2 + 1);
+  }
+  std::vector<int32_t> mid(nM), cnt_u((size_t)M * nU), cnt_m((size_t)M * nM);
+  std::vector<float> uf(uf_total), mf(mf_total);
+  ALS_TRY(cudaMemcpyAsync(mid.data(), L.d_mids, sizeof(int32_t) * nM, cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaMemcpyAsync(cnt_u.data(), d_cnt_u, sizeof(int32_t) * cnt_u.size(), cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaMemcpyAsync(cnt_m.data(), d_cnt_m, sizeof(int32_t) * cnt_m.size(), cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaMemcpyAsync(uf.data(), d_uf, sizeof(float) * uf_total, cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaMemcpyAsync(mf.data(), d_mf, sizeof(float) * mf_total, cudaMemcpyDeviceToHost, s));
+  ALS_TRY(cudaStreamSynchronize(s));
+  // model m's entities are those with a training rating in it, ascending; its outputs start after the models before
+  size_t uo = 0, mo = 0;
+  for (int m = 0; m < M; ++m) {
+    const int k = md[m].rank;
+    int32_t nu = 0, nm = 0;
+    for (int u = 0; u < nU; ++u) {
+      if (!cnt_u[(size_t)m * nU + u]) continue;
+      user_ids[(size_t)m * user_capacity + nu] = L.uid[u];
+      std::copy_n(uf.data() + bm[m].user_off + (size_t)u * k, k, user_factors + uo + (size_t)nu * k);
+      ++nu;
+    }
+    for (int e = 0; e < nM; ++e) {
+      if (!cnt_m[(size_t)m * nM + e]) continue;
+      movie_ids[(size_t)m * movie_capacity + nm] = mid[e];
+      std::copy_n(mf.data() + bm[m].movie_off + (size_t)e * k, k, movie_factors + mo + (size_t)nm * k);
+      ++nm;
+    }
+    n_users[m] = nu;
+    n_movies[m] = nm;
+    uo += (size_t)user_capacity * k;
+    mo += (size_t)movie_capacity * k;
+  }
   return SRS_OK;
 }
 
