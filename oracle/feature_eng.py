@@ -245,10 +245,10 @@ def _windows(S, lo_all, a, b, year_of, genres_of, G, b16, b32, out):
     nd = present.sum(axis=1, keepdims=True)
     ok = _genre_order_keys(ins, nd, b16[None, :], b32[None, :])
     key = np.where(present, ((1000 - cnt) << 24) | ok, 1 << 50)
-    order = np.argsort(key, axis=1, kind="stable")[:, :5]
+    order = np.argsort(key, axis=1, kind="stable")[:, :5]                 # fewer than 5 columns if G < 5
     got = np.take_along_axis(present, order, axis=1)
     for k in range(5):
-        out["userGenre%d_i" % (k + 1)][a:b] = np.where(got[:, k], order[:, k], -1)
+        out["userGenre%d_i" % (k + 1)][a:b] = np.where(got[:, k], order[:, k], -1) if k < G else -1
 
 
 def build_samples(ratings: Dict[str, np.ndarray], movies: Dict[str, Sequence]) -> Dict[str, np.ndarray]:
