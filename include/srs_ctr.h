@@ -623,6 +623,78 @@ int srs_als_recommend_host(const float* src_factors, int32_t n_src, const int32_
                            int32_t n_dst, int32_t rank, int32_t num, int32_t device, int32_t* out_ids,
                            float* out_scores);
 
+/* ---- The FeatureEngineering job and the sample split on the device (DESIGN.md section 4.16) ----
+ * Every entry checks its inputs before any device call (SRS_ERR_INVALID) and writes its outputs only on success.
+ * Synchronous; the same inputs give the same bits.  Values are never NaN.
+ *
+ * approxQuantile as Spark 2.4.3's QuantileSummaries answers it with every value in one summary: the n values
+ * (1 <= n <= 2^31 - 1) sorted in Double's total order, withHeadBufferInserted, compressImmut with mergeThreshold
+ * 2 eps n, then query (targetError = ceil(eps n)) at each probability in [0, 1] (1..65536 of them) -> out.
+ * NaN values are rejected (Spark's approxQuantile skips them).  Besides the sort, the compress takes at most
+ * min(n, 2 eps n + 4) sequential steps and each query O(log n). */
+int srs_approx_quantile_host(const double* values, int64_t n, const double* probabilities, int32_t n_probabilities,
+                             double relative_error, int32_t device, double* out);
+
+/* QuantileDiscretizer(num_buckets 2..10000, relative_error 0..1).fit: approxQuantile at the elements of Scala's
+ * (0.0 to 1.0 by 1.0 / num_buckets), 0.0 + step * k (num_buckets + 1 of them, or num_buckets when the step's decimal
+ * exceeds 1 / num_buckets), the first and last replaced by -inf / +inf, distinct values in order -> splits
+ * [<= num_buckets + 1], *n_splits.  `buckets` (or NULL)
+ * [n] receives Bucketizer's bucket of each value.  Splits that are not >= 3 strictly increasing values give
+ * SRS_ERR_INVALID after the device run. */
+int srs_quantile_discretizer_host(const double* values, int64_t n, int32_t num_buckets, double relative_error,
+                                  int32_t device, double* splits, int32_t* n_splits, int32_t* buckets);
+
+/* Bucketizer(splits).transform (handleInvalid "error"): 3..10001 strictly increasing splits; every value must lie in
+ * [splits[0], splits[n_splits - 1]].  A value on a split goes to the bucket above it; the last bucket includes the
+ * last split. */
+int srs_bucketize_host(const double* splits, int32_t n_splits, const double* values, int64_t n, int32_t device,
+                       int32_t* buckets);
+
+/* MinMaxScaler (min 0, max 1): out[i] = (x - Emin) / (Emax - Emin), 0.5 when Emax == Emin.  Emin / Emax are
+ * fit_min_max[0..1] when given, else the values' minimum and maximum in Double's total order; min_max (or NULL)
+ * receives the ones used. */
+int srs_minmax_scale_host(const double* values, int64_t n, const double* fit_min_max, int32_t device, double* out,
+                          double* min_max);
+
+/* groupBy(movieId).agg(count, avg(rating), variance(rating)) over 1..21 000 000 ratings (movie ids 0..2^24 - 1,
+ * half-stars 1..10): *n_movies rows, ascending movie id, of the movies with a rating.  avg and var_samp are each
+ * one correctly rounded division of exact integer moments; a one-rating movie's variance is NaN (null).  More
+ * movies than `capacity` give SRS_ERR_RANGE. */
+int srs_rating_features_host(const int32_t* movie_id, const int8_t* half, int64_t n_ratings, int32_t device,
+                             int32_t capacity, int32_t* movie_ids, int64_t* counts, double* avg, double* var,
+                             int32_t* n_movies);
+
+/* StringIndexer.fit (frequencyDesc) over tokens [n_tokens] (word ids 0..n_words - 1, each word occurring; 1 <=
+ * n_words <= 2^20) whose strings have the Java hashCodes word_hash [n_words]: label k is word label_words[k], with
+ * label_counts[k] occurrences; by descending count, ties in the iteration order of a Scala 2.11 immutable.HashMap.
+ * Two words whose improved hashes are equal are rejected. */
+int srs_string_indexer_host(const int32_t* tokens, int64_t n_tokens, const int32_t* word_hash, int32_t n_words,
+                            int32_t device, int32_t* label_words, int64_t* label_counts);
+
+/* The multi-hot genre vectors: movie r (distinct ids 0..2^24 - 1) lists the words words[offsets[r] ..
+ * offsets[r + 1]) (1..256 distinct words); the labels as srs_string_indexer_host, then per movie in ascending id
+ * (out_movie_ids [n_movies]) its label indices ascending, in CSR form: out_offsets [n_movies + 1], out_indices
+ * [offsets[n_movies]]. */
+int srs_genre_multihot_host(const int32_t* movie_id, const int32_t* offsets, const int32_t* words, int32_t n_movies,
+                            const int32_t* word_hash, int32_t n_words, int32_t device, int32_t* label_words,
+                            int64_t* label_counts, int32_t* out_movie_ids, int32_t* out_offsets,
+                            int32_t* out_indices);
+
+/* sample(fraction) then randomSplit(weights [n_parts], 1..64, finite, >= 0, sum > 0) of rows 0..n - 1: row i is
+ * sampled when the top 53 bits of splitmix(splitmix(seed, 0), i) / 2^53 < fraction, and goes to part j when
+ * lb_j <= u < ub_j for u from splitmix(splitmix(seed, 1), i), the bounds the running sums of the normalised weights.
+ * rows [n] receives part 0's rows, then part 1's, ..., each ascending; part_counts [n_parts] their counts. */
+int srs_sample_split_host(int64_t n, uint64_t seed, double fraction, const double* weights, int32_t n_parts,
+                          int32_t device, int32_t* rows, int64_t* part_counts);
+
+/* The same sample, then approxQuantile(timestamp, 0.8, relative_error) of the sampled rows (as
+ * srs_approx_quantile_host) -> *split_timestamp (NaN when no row is sampled): sampled rows with timestamp <= it
+ * are part 0 (training), the rest part 1 (test); rows and part_counts [2] as srs_sample_split_host.  Timestamps
+ * within +-2^53. */
+int srs_sample_split_by_timestamp_host(const int64_t* timestamp, int64_t n, uint64_t seed, double fraction,
+                                       double relative_error, int32_t device, int32_t* rows, int64_t* part_counts,
+                                       double* split_timestamp);
+
 #ifdef __cplusplus
 }
 #endif

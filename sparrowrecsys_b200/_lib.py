@@ -49,7 +49,10 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_trainer_iterations", "srs_trainer_fit_validate_host", "srs_trainer_evaluate_host",
            "srs_featureeng_host", "srs_item2vec_host", "srs_user_embeddings_host", "srs_als_fit_host",
            "srs_als_fit_folds_host", "srs_als_recommend_host", "srs_item_transitions_host", "srs_random_walks_host",
-           "srs_graph_embedding_host", "srs_lsh_transform_host", "srs_lsh_query_host")
+           "srs_graph_embedding_host", "srs_lsh_transform_host", "srs_lsh_query_host", "srs_approx_quantile_host",
+           "srs_quantile_discretizer_host", "srs_bucketize_host", "srs_minmax_scale_host", "srs_rating_features_host",
+           "srs_string_indexer_host", "srs_genre_multihot_host", "srs_sample_split_host",
+           "srs_sample_split_by_timestamp_host")
 
 _lib = None
 
@@ -280,6 +283,20 @@ def load():
     lib.srs_lsh_query_host.restype = C.c_int
     lib.srs_lsh_query_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_double,
                                        C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    V, I32, I64, F64 = C.c_void_p, C.c_int32, C.c_int64, C.c_double
+    for name, args in (
+            ("srs_approx_quantile_host", [V, I64, V, I32, F64, I32, V]),
+            ("srs_quantile_discretizer_host", [V, I64, I32, F64, I32, V, C.POINTER(I32), V]),
+            ("srs_bucketize_host", [V, I32, V, I64, I32, V]),
+            ("srs_minmax_scale_host", [V, I64, V, I32, V, V]),
+            ("srs_rating_features_host", [V, V, I64, I32, I32, V, V, V, V, C.POINTER(I32)]),
+            ("srs_string_indexer_host", [V, I64, V, I32, I32, V, V]),
+            ("srs_genre_multihot_host", [V, V, V, I32, V, I32, I32, V, V, V, V, V]),
+            ("srs_sample_split_host", [I64, C.c_uint64, F64, V, I32, I32, V, V]),
+            ("srs_sample_split_by_timestamp_host", [V, I64, C.c_uint64, F64, F64, I32, V, V, C.POINTER(F64)])):
+        f = getattr(lib, name)
+        f.restype = C.c_int
+        f.argtypes = args
     if lib.srs_abi_version() != ABI_VERSION:
         raise ImportError("libsrs_ctr.so ABI version %d != %d" % (lib.srs_abi_version(), ABI_VERSION))
     _lib = lib

@@ -290,6 +290,15 @@ cudaError_t user_time_order(const int32_t* d_user, const int32_t* d_ts, int n, i
   return e;
 }
 
+cudaError_t launch_movie_moments(const int32_t* d_movie, const int8_t* d_half, int n, int32_t* d_iota,
+                                 unsigned long long* d_mmom, cudaStream_t s) {
+  if (n <= 0) return cudaSuccess;
+  const int T = 256;
+  fe_prepare_kernel<<<grid_for(n, T), T, 0, s>>>(d_movie, d_half, n, d_iota, d_mmom);
+  ++g_launch_count;
+  return cudaGetLastError();
+}
+
 }  // namespace srs
 
 using namespace srs;

@@ -320,6 +320,10 @@ void metrics_summarise(const unsigned long long* hist, unsigned long long correc
 // sorts on `s`; temporaries are stream-ordered allocations.
 cudaError_t user_time_order(const int32_t* d_user, const int32_t* d_ts, int n, int32_t* d_order,
                             uint32_t* d_user_sorted, cudaStream_t s);
+// featureeng.cu: the movies' exact integer moments of n ratings (device arrays): d_mmom[3 m .. 3 m + 2] += count,
+// sum h, sum h^2 of movie m's half-stars (64-bit integer atomics; the caller zeroes d_mmom); d_iota[i] = i.
+cudaError_t launch_movie_moments(const int32_t* d_movie, const int8_t* d_half, int n, int32_t* d_iota,
+                                 unsigned long long* d_mmom, cudaStream_t s);
 
 struct Scratch {                       // device allocations of one host call, freed when it ends
   std::vector<void*> ptrs;

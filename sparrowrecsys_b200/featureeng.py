@@ -11,6 +11,13 @@ order rules; `oracle/feature_eng.py` restates them in numpy.
   keyed and typed exactly as `features.load_samples_csv` returns them, so the result goes straight into
   `predict`, `evaluate` and `Trainer.fit`.
 * `write_samples_csv` writes rows in the reference's text format.
+* `feature_engineering`, `split_samples` and `split_samples_by_timestamp` (from `featurejob`, DESIGN.md section
+  4.16) run the FeatureEngineering job and the sample / split that turns these rows into trainingSamples.csv and
+  testSamples.csv.
+
+    python -m sparrowrecsys_b200.featureeng samples RATINGS MOVIES OUT.csv
+    python -m sparrowrecsys_b200.featureeng job RATINGS MOVIES
+    python -m sparrowrecsys_b200.featureeng split RATINGS MOVIES OUT_DIR [--by-timestamp] [--seed S]
 """
 from __future__ import annotations
 
@@ -22,6 +29,7 @@ from typing import Dict, List, Mapping, Sequence
 import numpy as np
 
 from . import _lib
+from .featurejob import feature_engineering, split_samples, split_samples_by_timestamp  # noqa: F401
 
 DEFAULT_YEAR = 1990
 MAX_GENRE_WORDS = 24
@@ -191,3 +199,61 @@ def write_samples_csv(path: str, samples: Mapping[str, Sequence]) -> None:
         f.write(",".join(COLUMNS) + "\n")
         for row in zip(*cols):
             f.write(",".join(row) + "\n")
+
+
+def _show(title: str, cols: Mapping[str, Sequence], rows: int = 10) -> None:
+    names = list(cols)
+    print(title)
+    print("|".join(names))
+    for i in range(min(rows, len(cols[names[0]]))):
+        print("|".join(str(cols[c][i]) for c in names))
+    print()
+
+
+def main(argv: Sequence[str]) -> int:
+    """`samples`: build_samples -> OUT.csv; `job`: the FeatureEngineering job, printing the first 10 rows of each
+    result as its show(10) calls do; `split`: build the samples, sample 10 % and write OUT_DIR/trainingSamples.csv
+    and OUT_DIR/testSamples.csv (0.8 / 0.2 at random, or at the 0.8 timestamp quantile with --by-timestamp)."""
+    import argparse
+    import os
+    ap = argparse.ArgumentParser(prog="python -m sparrowrecsys_b200.featureeng")
+    ap.add_argument("mode", choices=("samples", "job", "split"))
+    ap.add_argument("ratings")
+    ap.add_argument("movies")
+    ap.add_argument("out", nargs="?")
+    ap.add_argument("--by-timestamp", action="store_true")
+    ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--device", type=int, default=0)
+    a = ap.parse_args(argv)
+    ratings, movies = load_ratings_csv(a.ratings), load_movies_csv(a.movies)
+    if a.mode == "job":
+        r = feature_engineering(ratings, movies, a.device)
+        oh, mh, mf = r["one_hot"], r["multi_hot"], r["movie_features"]
+        _show("OneHotEncoder Example:", {"movieId": movies["movieId"], "movieIdVector": [
+            "(%d,[%d],[1.0])" % (oh["size"], i) for i in oh["index"][:10]]})
+        vec = ["(%d,[%s],[%s])" % (mh["size"], ",".join(map(str, mh["indices"][b:e])), ",".join(["1.0"] * (e - b)))
+               for b, e in zip(mh["offsets"][:10], mh["offsets"][1:11])]
+        _show("MultiHotEncoder Example:", {"movieId": mh["movieId"], "vector": vec})
+        _show("Numerical features Example:", {k: mf[k] for k in ("movieId", "ratingCount", "avgRating", "ratingVar",
+                                                                 "ratingCountBucket", "scaleAvgRating")})
+        return 0
+    if not a.out:
+        ap.error("%s needs an output path" % a.mode)
+    samples = build_samples(ratings, movies, a.device)
+    if a.mode == "samples":
+        write_samples_csv(a.out, samples)
+        return 0
+    if a.by_timestamp:
+        train, test = split_samples_by_timestamp(samples, a.seed, device=a.device)
+    else:
+        train, test = split_samples(samples, a.seed, device=a.device)
+    os.makedirs(a.out, exist_ok=True)
+    write_samples_csv(os.path.join(a.out, "trainingSamples.csv"), train)
+    write_samples_csv(os.path.join(a.out, "testSamples.csv"), test)
+    print("%d training and %d test rows in %s" % (len(train["movieId"]), len(test["movieId"]), a.out))
+    return 0
+
+
+if __name__ == "__main__":
+    import sys
+    sys.exit(main(sys.argv[1:]))
