@@ -24,15 +24,18 @@
 //     accumulator registers.  E <= 64: on CUDA cores (common.cuh::dense_layer); its W1 image would be
 //     ~160 KB, and at cfg 5's T = 200 the activation unit dominates the tile.
 //
-// CTA = G warpgroups (DinWgLayout::G: 5 at E <= 32, 3 at E <= 64), 32 batch rows; warpgroup q owns rows
-// q, q + G, ... and double-buffers its history tiles (the next tile's cp.async runs under this tile's MMA
-// and epilogue; the ids of the tile after it are already on their way from HBM).  The per-row chain is
-// latency-bound, so more warpgroups shorten each warpgroup's walk (7 or 6 rows at G = 5) without
-// lengthening the chain.  At E <= 32 the 112 KB MLP image is not resident beside the warpgroups' buffers:
-// they share one region, the image at its bottom and the buffers at its top, and the image bytes under the
-// buffers are copied again in each tile once its activation unit is done (28 KB of W2^T at G = 5, in
-// flight under Dense(128)).  The shared tile helpers that map threads generically (tile_side_features,
-// stage_weights) use every warpgroup; dense_layer and row_dot (E <= 64) map 256 threads, and only
+// CTA = G warpgroups (DinWgLayout::G: 4 at E <= 32, 3 at E <= 64), 32 batch rows; warpgroup q owns rows
+// q, q + G, ... and walks them in items of R rows at one 64-position chunk (DinWgLayout::R: 2 at E <= 32, 1 at
+// E <= 64), double-buffering the items' history tiles.  The rows of a pair share its barriers, its gather wait
+// and its two MMA round trips (both rows' MMAs in one commit group, waited with wait_group 0).  The work that
+// does not depend on those MMAs runs while they are in flight: the next item's gathers (and the ids of the item
+// after it) are issued under the activation-unit MMAs, the next row's W_r is built under the pooling MMAs.
+// At E <= 32 the 112 KB MLP image is not resident beside the warpgroups' buffers: they share one region, the
+// image at its bottom and the buffers at its top, and the image bytes under the buffers (94 KB at G = 4,
+// R = 2) are copied again in each tile once its activation unit is done, W1^T's
+// part (if any) first on its own barrier so that W2^T's flies under Dense(128).  The shared tile
+// helpers that map threads generically (tile_side_features, stage_weights) use every warpgroup; dense_layer
+// and row_dot (E <= 64) map 256 threads, and only
 // warpgroups 0 and 1 issue the top MLP's Dense(128).  Shared memory: ~227 KB (E <= 32) / ~218 KB
 // (E <= 64): one CTA per SM.
 #include "kernels.h"
@@ -51,22 +54,28 @@ __device__ __forceinline__ float rcp_approx(float x) {
 
 constexpr int kWgRows = 32;       // rows per CTA (top-MLP tile height, as din.cu)
 constexpr int kWgPos = 64;        // history positions per MMA tile
-// warpgroups per CTA at E <= 32 (DESIGN §6 has the measurements that chose 5; a build with
-// -DSRS_DIN_WG_GROUPS32=N measures another count)
+// warpgroups per CTA and batch rows per warpgroup item at E <= 32 (DESIGN §6 has the measurements that chose
+// 4 and 2; a build with -DSRS_DIN_WG_GROUPS32=N or -DSRS_DIN_WG_ROWS32=N measures another count)
 #ifndef SRS_DIN_WG_GROUPS32
-#define SRS_DIN_WG_GROUPS32 5
+#define SRS_DIN_WG_GROUPS32 4
+#endif
+#ifndef SRS_DIN_WG_ROWS32
+#define SRS_DIN_WG_ROWS32 2
 #endif
 
 template <int EP>
 struct DinWgLayout {
   static constexpr bool TC_MLP = EP == 32;                    // top MLP on wgmma
-  // warpgroups per CTA: warpgroup q walks rows q, q + G, ... of the tile
+  // warpgroups per CTA: warpgroup q walks rows q, q + G, ... of the tile, R of them per item
   static constexpr int G = TC_MLP ? SRS_DIN_WG_GROUPS32 : 3;
+  static constexpr int R = TC_MLP ? SRS_DIN_WG_ROWS32 : 1;
+  static_assert(R >= 1 && R <= 2, "one or two rows per item");
   static constexpr int THREADS = 128 * G;
   static constexpr int KB = EP / 32;                          // 128-byte K blocks of a [hi | lo] row
   static constexpr uint32_t A_BYTES = KB * kWgPos * 128;      // one history tile
   static constexpr uint32_t B_BYTES = KB * 32 * 128;          // W_r, 32 unit rows
-  static constexpr uint32_t WG_BYTES = 2 * A_BYTES + B_BYTES; // per warpgroup
+  // per warpgroup: two item buffers of R history tiles each, then R W_r operands
+  static constexpr uint32_t WG_BYTES = 2 * R * A_BYTES + R * B_BYTES;
   static constexpr uint32_t AU_BYTES = G * WG_BYTES;
   // top-MLP operand images (TC_MLP, written by model.cu::build_din_wg): W1^T [128 units][160 k] as k 0..127
   // in 2 K blocks, a hi and a lo image, then one tail K block whose 128-byte rows are [hi k 128..159 |
@@ -87,32 +96,39 @@ struct DinWgLayout {
   static constexpr int F_WP = F_WH + EP * 32;                 // [EP][32] Wp
   static constexpr int F_WC = F_WP + EP * 32;                 // [EP][32] Wc - Wsub
   static constexpr int F_CST = F_WC + EP * 32;                // [32 rows][32 units] activation-unit constants
-  static constexpr int F_WG = F_CST + kWgRows * 32;           // per warpgroup: pooled lo sums (EP = 32)
-  static constexpr int F_WG_STRIDE = 32;
+  static constexpr int F_WG = F_CST + kWgRows * 32;           // per warpgroup: pooled lo sums of R rows (EP = 32)
+  static constexpr int F_WG_STRIDE = 32 * R;
   static constexpr int F_RED = F_WG + G * F_WG_STRIDE;        // [4 warps][32 rows] Dense(1) partial sums
   static constexpr int F_END = F_RED + 4 * kWgRows;
   static constexpr uint32_t FS_BYTES = (uint32_t)F_END * sizeof(float);
-  // pooling B operand per warpgroup, K-major [8 rows][64 positions] bf16: row 0 w hi, row 1 w lo, rows 2-7 zero.
+  // pooling B operand per item row, K-major [8 rows][64 positions] bf16: row 0 w hi, row 1 w lo, rows 2-7 zero.
   // They sit between the byte region and the fp32 region, where neither the image nor the X / H1 operand
   // reaches, so their zero rows are written once per CTA.
   static constexpr uint32_t PB_BYTES = 1024;
+  static constexpr uint32_t PB_WG_BYTES = R * PB_BYTES;        // per warpgroup
   // Byte region at the aligned base, in front of the pooling operands and the fp32 region.  E <= 64: the
   // warpgroups' history tiles and W_r.  E <= 32: every byte that one CTA per SM leaves (kSmemStatic: the static
   // mbarriers), the image at its bottom and the warpgroups' buffers at its top, the X / H1 operand over the last
   // of those.  The image bytes under the buffers (IMG_RELOAD) are copied again in every tile once its
-  // activation unit is done; the rest (IMG_RESIDENT) is copied once per CTA.
+  // activation unit is done, W1^T's part (RELOAD_W1) first and on its own barrier, so that the copy of W2^T's
+  // part (RELOAD_W2) still flies under Dense(128); the rest (IMG_RESIDENT) is copied once per CTA.
   static constexpr uint32_t kSmemStatic = 64;
   static constexpr uint32_t REGION =
-      TC_MLP ? (227u * 1024 - 1024 - kSmemStatic - G * PB_BYTES - FS_BYTES) / 1024 * 1024 : AU_BYTES;
-  static constexpr uint32_t PB_OFF = REGION;                    // warpgroup q's pooling operand at PB_OFF + q PB_BYTES
-  static constexpr uint32_t FS_OFF = PB_OFF + G * PB_BYTES;
+      TC_MLP ? (227u * 1024 - 1024 - kSmemStatic - G * PB_WG_BYTES - FS_BYTES) / 1024 * 1024 : AU_BYTES;
+  static constexpr uint32_t PB_OFF = REGION;                    // row s of warpgroup q: PB_OFF + q PB_WG_BYTES + s PB_BYTES
+  static constexpr uint32_t FS_OFF = PB_OFF + G * PB_WG_BYTES;
   static constexpr uint32_t AU_OFF = REGION - AU_BYTES;         // warpgroup q's buffers at AU_OFF + q WG_BYTES
   static constexpr uint32_t OPS_OFF = REGION - 3 * OP_KB_BYTES; // X / H1 operand
   static constexpr uint32_t IMG_RESIDENT = AU_OFF < IMG_BYTES ? AU_OFF : IMG_BYTES;
   static constexpr uint32_t IMG_RELOAD = IMG_BYTES - IMG_RESIDENT;
-  static constexpr bool RELOAD_IN_W2 = IMG_RESIDENT >= IMG_W2_HI;  // Dense(128) never waits for the reload
+  static constexpr uint32_t RELOAD_W1 = TC_MLP && IMG_RESIDENT < IMG_W2_HI ? IMG_W2_HI - IMG_RESIDENT : 0;
+  static constexpr uint32_t RELOAD_W2_OFF = IMG_RESIDENT + RELOAD_W1;
+  static constexpr uint32_t RELOAD_W2 = IMG_RELOAD - RELOAD_W1;
   static_assert(REGION >= AU_BYTES && AU_OFF % 1024 == 0 && IMG_RESIDENT % 16 == 0, "buffer alignment");
+  static_assert(WG_BYTES % 1024 == 0 && (2 * R * A_BYTES) % 1024 == 0, "SW128 operands sit on 1 KB boundaries");
   static_assert(!TC_MLP || OPS_OFF >= IMG_BYTES, "the X / H1 operand must not overlap the image");
+  static_assert(!TC_MLP || (RELOAD_W2_OFF >= IMG_W2_HI && RELOAD_W2_OFF + RELOAD_W2 == IMG_BYTES &&
+                            RELOAD_W2_OFF % 16 == 0), "reload split at W2^T");
   static constexpr size_t SMEM = 1024 + FS_OFF + FS_BYTES;
   static_assert(SMEM + kSmemStatic <= 227 * 1024, "one CTA per SM must fit");
 };
@@ -125,8 +141,8 @@ __device__ __forceinline__ uint32_t wg_kbyte(uint32_t row, uint32_t kb, uint32_t
 
 // Top MLP of a 32-row tile on wgmma (E <= 32).  Xs holds the fp32 input tile; the X and H1 operands go
 // over the history tiles at `ops`; `img` holds the W1^T / W2^T images: the resident part has landed once
-// `res_bar` (if not null) completes, the reloaded part once `reload_bar` completes phase `parity`.  Ends
-// with every score of the tile stored.
+// `res_bar` (if not null) completes, the reloaded parts of W1^T and W2^T once `reload_bar[0]` and
+// `reload_bar[1]` complete phase `parity`.  Ends with every score of the tile stored.
 template <int EP>
 __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& b, int row0, const float* Xs,
                                            uint8_t* ops, const uint8_t* img, float* red, uint64_t* res_bar,
@@ -150,7 +166,7 @@ __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& 
   __syncthreads();
   clk.lap(PH_TOP_MLP);
   if (res_bar) mbar_wait(res_bar, 0);
-  if (L::IMG_RELOAD > 0 && !L::RELOAD_IN_W2) mbar_wait(reload_bar, parity);
+  if (L::RELOAD_W1 > 0) mbar_wait(&reload_bar[0], parity);
   clk.lap(PH_IMAGE_WAIT);
   const uint32_t s_img = smem_u32(img), s_op = smem_u32(ops);
 
@@ -210,9 +226,9 @@ __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& 
   }
   // ---- Dense(64) + PReLU, Dense(1), sigmoid: warpgroup 0, D[64 units x (32 rows hi | 32 rows lo)]
   if (q != 0) return;
-  if (L::IMG_RELOAD > 0 && L::RELOAD_IN_W2) {      // the reloaded part is W2's: it flew under Dense(128)
+  if (L::RELOAD_W2 > 0) {                          // W2's reloaded part flew under Dense(128)
     clk.lap(PH_TOP_MLP);
-    mbar_wait(reload_bar, parity);
+    mbar_wait(&reload_bar[1], parity);
     clk.lap(PH_IMAGE_WAIT);
   }
   float d[32];
@@ -280,14 +296,15 @@ __device__ __forceinline__ void top_mlp_wg(const DinParams& p, const BatchView& 
 template <int EP>
 __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(DinParams p, BatchView b) {
   using L = DinWgLayout<EP>;
-  constexpr int G = L::G, NT = L::THREADS;
+  constexpr int G = L::G, R = L::R, NT = L::THREADS;
   constexpr int KB = L::KB;
   constexpr int KS = EP / 16;                     // K steps per part (hi or lo)
   constexpr int CP = 8 * KB;                      // 16-byte chunks per split row
   constexpr int NCOPY = kWgPos * CP / 128;        // cp.async per thread per tile
   constexpr int OFF_UG = 0, OFF_U = EP, OFF_POOL = 2 * EP, OFF_C = 3 * EP, OFF_MG = 4 * EP, OFF_NUM = 5 * EP;
   extern __shared__ uint8_t raw[];
-  __shared__ uint64_t res_bar, reload_bar;        // top-MLP image (TC_MLP): resident part / this tile's reload landed
+  // top-MLP image (TC_MLP): resident part / this tile's reload of W1^T's and of W2^T's part landed
+  __shared__ uint64_t res_bar, reload_bar[2];
   uint8_t* base = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
   uint8_t* img = base;
   float* fs = reinterpret_cast<float*>(base + L::FS_OFF);
@@ -302,18 +319,22 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
   const int q = tid >> 7, tw = tid & 127;
   const int warp = tw >> 5, lane = tw & 31, g = lane >> 2, cq = lane & 3;
   const int T = p.T, nch = (T + kWgPos - 1) / kWgPos;
-  uint8_t* tiles = base + L::AU_OFF + q * L::WG_BYTES;   // history tiles 0, 1 | W_r
-  uint8_t* Bt = tiles + 2 * L::A_BYTES;
+  // history tiles of item buffer 0 (rows 0 .. R - 1), of buffer 1 | W_r of rows 0 .. R - 1
+  uint8_t* tiles = base + L::AU_OFF + q * L::WG_BYTES;
+  uint8_t* Bt = tiles + 2 * R * L::A_BYTES;
   PhaseClock clk(tw == 0);
-  // pooling B operand: w hi | w lo | 6 zero rows (128 threads x 8 B: the whole operand)
-  reinterpret_cast<uint2*>(base + L::PB_OFF + q * L::PB_BYTES)[tw] = make_uint2(0u, 0u);
+  // pooling B operands: w hi | w lo | 6 zero rows (128 threads x 8 B: one whole operand)
+  #pragma unroll
+  for (int s = 0; s < R; ++s)
+    reinterpret_cast<uint2*>(base + L::PB_OFF + q * L::PB_WG_BYTES + s * L::PB_BYTES)[tw] = make_uint2(0u, 0u);
 
   bool weights_ready = !L::TC_MLP;
   uint32_t reload_parity = 0;
   if constexpr (L::TC_MLP) {
     if (tid == 0) {                               // visible to the waiters through the tile loop's first barrier
       mbar_init(&res_bar, 1);
-      mbar_init(&reload_bar, 1);
+      mbar_init(&reload_bar[0], 1);
+      mbar_init(&reload_bar[1], 1);
       fence_mbar_init();
       mbar_arrive_expect_tx(&res_bar, L::IMG_RESIDENT);
       for (uint32_t off = 0; off < L::IMG_RESIDENT; off += 32768u)
@@ -381,195 +402,261 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
   #pragma unroll
       for (int c = 0; c < 2; ++c) wout[2 * j + c] = __ldg(p.au_wout + 8 * j + 2 * cq + c);
 
-    const int n_items = nrows * nch;                // (row, 64-position chunk) pairs, chunk fastest
+    // An item is a pair (R = 2) of the warpgroup's rows at one 64-position chunk, chunk fastest: item k is chunk
+    // k % nch of rows q + G (R i + s), s < R, with i = k / nch.  Row s of the pair is live if R i + s < nrows; the
+    // pair's first row always is.  A row that is not (the last pair of a warpgroup with an odd row count) has no
+    // W_r build, gathers, gate or stores; nothing reads its buffers.  Its MMAs are still issued, on row 0's
+    // operands, and their sums dropped: wgmmas skipped in a branch make ptxas serialise every wgmma (C7520).
+    const int n_items = (nrows + R - 1) / R * nch;
     // The history ids of an item are requested (into registers) two items before its rows are gathered,
     // so the HBM latency of the ids is not on the item chain.  Whether a slot is live is decided from its
     // position, never from the id value: every live id goes through the range check.
-    // item k is chunk k % nch of the warpgroup's row k / nch; with one chunk per row (T <= 64) no division
-    auto item_row = [&](int k) { return nch == 1 ? k : k / nch; };
+    // With one chunk per row (T <= 64) the item is the pair: no division
+    auto item_pair = [&](int k) { return nch == 1 ? k : k / nch; };
     auto item_ch = [&](int k) { return nch == 1 ? 0 : k % nch; };
+    auto row_live = [&](int i, int s) { return s == 0 || R * i + s < nrows; };
     auto item_nt = [&](int k) { return k < n_items ? min(kWgPos, T - item_ch(k) * kWgPos) : 0; };
-    auto load_ids = [&](int k, int (&ids)[NCOPY]) {
-      const int row = row0 + q + G * item_row(k), t0 = item_ch(k) * kWgPos, nt = item_nt(k);
-      const int32_t* hrow = b.hist + (size_t)row * b.hist_stride + t0;
+    auto load_ids = [&](int k, int (&ids)[R][NCOPY]) {
+      const int i = item_pair(k), t0 = item_ch(k) * kWgPos, nt = item_nt(k);
   #pragma unroll
-      for (int n = 0; n < NCOPY; ++n) {
-        const int pos = (tw + 128 * n) / CP;
-        ids[n] = pos < nt ? __ldg(hrow + pos) : 0;
+      for (int s = 0; s < R; ++s) {
+        const int row = row0 + q + G * (R * i + s), nts = row_live(i, s) ? nt : 0;
+        const int32_t* hrow = b.hist + (size_t)row * b.hist_stride + t0;
+  #pragma unroll
+        for (int n = 0; n < NCOPY; ++n) {
+          const int pos = (tw + 128 * n) / CP;
+          ids[s][n] = pos < nts ? __ldg(hrow + pos) : 0;
+        }
       }
     };
-    // Every position of the tile is written: positions past nt are zero-filled, because the pooling MMA
+    // Every position of a live row's tile is written: positions past nt are zero-filled, because the pooling MMA
     // reads them (with w = 0, which a stale NaN would still turn into NaN).  An out-of-range id is read as
     // row 0 and latches the error word, once per warp and item.
-    auto gather = [&](int k, const int (&ids)[NCOPY]) {
+    auto gather = [&](int k, const int (&ids)[R][NCOPY]) {
       if (k >= n_items) return;
-      uint8_t* A = tiles + (k & 1) * L::A_BYTES;
-      const int nt = item_nt(k);
+      uint8_t* A = tiles + (k & 1) * (R * L::A_BYTES);
+      const int i = item_pair(k), nt = item_nt(k);
       bool bad = false;
   #pragma unroll
-      for (int n = 0; n < NCOPY; ++n) {
-        const int i = tw + 128 * n, pos = i / CP, c = i % CP;
-        const int id = __float2int_rz(__int2float_rn(ids[n]));
-        const bool in_range = static_cast<unsigned>(id) < static_cast<unsigned>(p.n_movies);
-        bad |= !in_range;                                     // ids past nt are 0: never out of range
-        cp_async16_zfill(A + (c >> 3) * (kWgPos * 128) + sw128_offset(pos, c & 7),
-                         p.movie_split + (size_t)(in_range ? id : 0) * (CP * 16) + c * 16, pos < nt ? 16u : 0u);
+      for (int s = 0; s < R; ++s) {
+        if (!row_live(i, s)) continue;
+  #pragma unroll
+        for (int n = 0; n < NCOPY; ++n) {
+          const int t = tw + 128 * n, pos = t / CP, c = t % CP;
+          const int id = __float2int_rz(__int2float_rn(ids[s][n]));
+          const bool in_range = static_cast<unsigned>(id) < static_cast<unsigned>(p.n_movies);
+          bad |= !in_range;                                   // ids past nt are 0: never out of range
+          cp_async16_zfill(A + s * L::A_BYTES + (c >> 3) * (kWgPos * 128) + sw128_offset(pos, c & 7),
+                           p.movie_split + (size_t)(in_range ? id : 0) * (CP * 16) + c * 16, pos < nt ? 16u : 0u);
+        }
       }
       if (__any_sync(0xffffffffu, bad) && lane == 0 && b.err_flag) atomicExch(b.err_flag, 1);
     };
 
-    int ids_next[NCOPY];
+    int ids_next[R][NCOPY];
     {
-      int ids0[NCOPY];
+      int ids0[R][NCOPY];
       load_ids(0, ids0);
       load_ids(1, ids_next);
       gather(0, ids0);
     }
     cp_async_commit();
-    const uint32_t pb_s = smem_u32(base + L::PB_OFF + q * L::PB_BYTES);
+    // per item row s: pooling operand at pb_s + s PB_BYTES, pooled lo sums at pool_lo + 32 s, W_r at + s B_BYTES
+    const uint32_t pb_s = smem_u32(base + L::PB_OFF + q * L::PB_WG_BYTES);
     float* pool_lo = fs + L::F_WG + q * L::F_WG_STRIDE;
     // W_r destinations of this thread (unit j = lane, element pair e = 2 warp + 8 n, K byte 4 warp + 16 n), the
     // same in every row: chunk n of row `lane`, byte 4 warp within it; its sources wh / wp [e][j]
     const uint32_t wr_row = smem_u32(Bt) + lane * 128u + 4u * warp, wr_sw = lane & 7u;
     const int wr_src = 2 * warp * 32 + lane;
-    float slope[2][8], cstv[8];
-    // pooled sums of the row so far: D[e'][n] = sum_t A[t][e'] Pb[n][t] for the operand columns e' of K block kb
-    // (EP = 32: hi e | lo e; EP = 64: block 0 hi, block 1 lo) and n = w hi, w lo, added chunk by chunk
-    float pacc[KB][4];
-    for (int k = 0; k < n_items; ++k) {
-      const int r = q + G * item_row(k), ch = item_ch(k), t0 = ch * kWgPos;
-      const int nt = min(kWgPos, T - t0);
-      float* xrow = Xs + r * L::LDX;
-      const float* cst = cst_all + r * 32;
-      if (ch == 0) {
-        // B operand of the row: W_r = (Wsub + Wh) + diag(c_r) Wp, split to bf16 hi / lo.  Thread (warp, lane)
-        // writes unit j = lane, element pairs e = 2 warp + 8 n: the lanes of a warp read 32 consecutive banks
-        const float* cv = xrow + OFF_C + 2 * warp;
+    float slope[2][8], cstv[R][8];
+    // B operand of each live row of item k: W_r = (Wsub + Wh) + diag(c_r) Wp, split to bf16 hi / lo, and the row's
+    // gate constants.  Thread (warp, lane) writes unit j = lane, element pairs e = 2 warp + 8 n: the lanes of a
+    // warp read 32 consecutive banks
+    auto build_wr = [&](int k) {
+      const int i = item_pair(k);
+  #pragma unroll
+      for (int s = 0; s < R; ++s) {
+        if (!row_live(i, s)) continue;
+        const int r = q + G * (R * i + s);
+        const float* cv = Xs + r * L::LDX + OFF_C + 2 * warp;
   #pragma unroll
         for (int n = 0; n < EP / 8; ++n) {
           const float2 c2 = *reinterpret_cast<const float2*>(cv + 8 * n);
           const float v0 = fmaf(c2.x, wp[wr_src + 256 * n], wh[wr_src + 256 * n]);
           const float v1 = fmaf(c2.y, wp[wr_src + 256 * n + 32], wh[wr_src + 256 * n + 32]);
-          const Split2 s = split_pack(v0, v1);
+          const Split2 sp = split_pack(v0, v1);
           // the lo half of K byte kb sits at K byte 2 EP + kb: 64 bytes on in the same row (EP = 32, the
           // chunk index gains bit 2), or the next K block (EP = 64)
-          const uint32_t dst = wr_row + ((n ^ wr_sw) << 4);
-          st_shared_u32(dst, s.hi);
-          st_shared_u32(EP == 32 ? dst ^ 64u : dst + 32u * 128u, s.lo);
+          const uint32_t dst = wr_row + s * L::B_BYTES + ((n ^ wr_sw) << 4);
+          st_shared_u32(dst, sp.hi);
+          st_shared_u32(EP == 32 ? dst ^ 64u : dst + 32u * 128u, sp.lo);
         }
+        const float* cst = cst_all + r * 32;
   #pragma unroll
         for (int j = 0; j < 4; ++j)
   #pragma unroll
-          for (int c = 0; c < 2; ++c) cstv[2 * j + c] = cst[8 * j + 2 * cq + c];
-        clk.lap(PH_W_BUILD);
+          for (int c = 0; c < 2; ++c) cstv[s][2 * j + c] = cst[8 * j + 2 * cq + c];
       }
-      gather(k + 1, ids_next);                                // its buffer's last reader finished before the
-      cp_async_commit();                                      // closing barrier of item k - 1
-      load_ids(k + 2, ids_next);
+    };
+    if (n_items > 0) build_wr(0);
+    clk.lap(PH_W_BUILD);
+    // pooled sums of each row so far: D[e'][n] = sum_t A[t][e'] Pb[n][t] for the operand columns e' of K block kb
+    // (EP = 32: hi e | lo e; EP = 64: block 0 hi, block 1 lo) and n = w hi, w lo, added chunk by chunk
+    float pacc[R][KB][4];
+    for (int k = 0; k < n_items; ++k) {
+      const int i = item_pair(k), ch = item_ch(k), t0 = ch * kWgPos;
+      const int nt = min(kWgPos, T - t0);
+      bool live[R];
+      int r[R];
+  #pragma unroll
+      for (int s = 0; s < R; ++s) {
+        live[s] = row_live(i, s);
+        r[s] = q + G * (R * i + s);
+      }
       // PReLU slopes of this thread's positions pr = 16 warp + g + 8 i and columns 8 j + 2 cq + c, times the
-      // Dense(1) weights (the gate adds z wout or z slope wout), requested before the waits below; with one chunk
-      // per row (T <= 64) they are the same for every row
+      // Dense(1) weights (the gate adds z wout or z slope wout), requested before the waits below; the same for
+      // both rows of an item, and with one chunk per row (T <= 64) for every item
       if (nch > 1 || k == 0) {
   #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const float* alpha = p.au_alpha + (size_t)min(t0 + 16 * warp + g + 8 * i, T - 1) * 32;
+        for (int h = 0; h < 2; ++h) {
+          const float* alpha = p.au_alpha + (size_t)min(t0 + 16 * warp + g + 8 * h, T - 1) * 32;
   #pragma unroll
           for (int j = 0; j < 4; ++j)
   #pragma unroll
-            for (int c = 0; c < 2; ++c) slope[i][2 * j + c] = __ldg(alpha + 8 * j + 2 * cq + c) * wout[2 * j + c];
+            for (int c = 0; c < 2; ++c) slope[h][2 * j + c] = __ldg(alpha + 8 * j + 2 * cq + c) * wout[2 * j + c];
         }
       }
-      clk.lap(PH_GATHER_ISSUE);
-      cp_async_wait<1>();
+      cp_async_wait<0>();
       fence_async_smem();
-      named_sync(1 + q, 128);                                 // tile k and W_r in place
+      named_sync(1 + q, 128);                                 // tiles of item k and W_r in place
       clk.lap(PH_GATHER_WAIT);
 
-      // ---- activation unit: D[64 positions x 32 units], bf16x3
-      float d[16];
+      const uint32_t sa = smem_u32(tiles + (k & 1) * (R * L::A_BYTES));
+      // ---- activation unit: D[64 positions x 32 units] per row, bf16x3; the rows' MMAs in one commit group
+      float d[R][16];
   #pragma unroll
-      for (int i = 0; i < 16; ++i) d[i] = 0.f;
+      for (int s = 0; s < R; ++s)
+  #pragma unroll
+        for (int e = 0; e < 16; ++e) d[s][e] = 0.f;
       {
-        const uint32_t sa = smem_u32(tiles + (k & 1) * L::A_BYTES), sb = smem_u32(Bt);
         mma_fence();
   #pragma unroll
-        for (int s = 0; s < KS; ++s) {
-          const uint32_t kh = 32 * s, kl = 2 * EP + 32 * s;   // K byte of the hi / lo step
-          const uint64_t ah = desc_sw128(sa + (kh >> 7) * (kWgPos * 128) + (kh & 127));
-          const uint64_t al = desc_sw128(sa + (kl >> 7) * (kWgPos * 128) + (kl & 127));
-          const uint64_t bh = desc_sw128(sb + (kh >> 7) * (32 * 128) + (kh & 127));
-          const uint64_t bl = desc_sw128(sb + (kl >> 7) * (32 * 128) + (kl & 127));
-          mma_m64n32_ss(d, ah, bh, s > 0);
-          mma_m64n32_ss(d, al, bh, 1);
-          mma_m64n32_ss(d, ah, bl, 1);
+        for (int s = 0; s < R; ++s) {
+          // a row that is not live reads row 0's operands (so does its pooling below)
+          const uint32_t sas = live[s] ? sa + s * L::A_BYTES : sa;
+          const uint32_t sb = smem_u32(Bt) + (live[s] ? s * L::B_BYTES : 0u);
+  #pragma unroll
+          for (int ks = 0; ks < KS; ++ks) {
+            const uint32_t kh = 32 * ks, kl = 2 * EP + 32 * ks;   // K byte of the hi / lo step
+            const uint64_t ah = desc_sw128(sas + (kh >> 7) * (kWgPos * 128) + (kh & 127));
+            const uint64_t al = desc_sw128(sas + (kl >> 7) * (kWgPos * 128) + (kl & 127));
+            const uint64_t bh = desc_sw128(sb + (kh >> 7) * (32 * 128) + (kh & 127));
+            const uint64_t bl = desc_sw128(sb + (kl >> 7) * (32 * 128) + (kl & 127));
+            mma_m64n32_ss(d[s], ah, bh, ks > 0);
+            mma_m64n32_ss(d[s], al, bh, 1);
+            mma_m64n32_ss(d[s], ah, bl, 1);
+          }
         }
         mma_commit();
+        // item k + 1's gathers fly under the MMAs: its buffer's last reader finished before the closing barrier
+        // of item k - 1; the ids of item k + 2 are requested behind them
+        gather(k + 1, ids_next);
+        cp_async_commit();
+        load_ids(k + 2, ids_next);
+        clk.lap(PH_GATHER_ISSUE);
         mma_wait<0>();
-        reg_fence(d);
+  #pragma unroll
+        for (int s = 0; s < R; ++s) reg_fence(d[s]);
       }
       clk.lap(PH_AU_MMA);
-      // ---- gate: positions pr = 16 warp + g + 8 i; the quad of lanes sharing a position sums its 32 units
+      // ---- gate: positions pr = 16 warp + g + 8 h; the quad of lanes sharing a position sums its 32 units
   #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int pr = 16 * warp + g + 8 * i;
-        float s = 0.f;
+      for (int s = 0; s < R; ++s) {
+        if (!live[s]) continue;
   #pragma unroll
-        for (int j = 0; j < 4; ++j)
+        for (int h = 0; h < 2; ++h) {
+          const int pr = 16 * warp + g + 8 * h;
+          float acc = 0.f;
   #pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const float z = d[4 * j + 2 * i + c] + cstv[2 * j + c];
-            s = fmaf(z, z > 0.f ? wout[2 * j + c] : slope[i][2 * j + c], s);
+          for (int j = 0; j < 4; ++j)
+  #pragma unroll
+            for (int c = 0; c < 2; ++c) {
+              const float z = d[s][4 * j + 2 * h + c] + cstv[s][2 * j + c];
+              acc = fmaf(z, z > 0.f ? wout[2 * j + c] : slope[h][2 * j + c], acc);
+            }
+          acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+          acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+          // w split to bf16 hi / lo into rows 0 and 1 of the row's pooling operand (K byte 2 pr); w = 0 past nt
+          const float w = pr < nt ? rcp_approx(1.f + __expf(-(acc + p.au_bout))) : 0.f;
+          if (cq == 0) {
+            const uint32_t pb = pb_s + s * L::PB_BYTES;
+            const __nv_bfloat16 wh16 = __float2bfloat16_rn(w);
+            const __nv_bfloat16 wl16 = __float2bfloat16_rn(w - __bfloat162float(wh16));
+            st_shared_u16(pb + sw128_offset(0, pr >> 3) + 2 * (pr & 7), __bfloat16_as_ushort(wh16));
+            st_shared_u16(pb + sw128_offset(1, pr >> 3) + 2 * (pr & 7), __bfloat16_as_ushort(wl16));
           }
-        s += __shfl_xor_sync(0xffffffffu, s, 1);
-        s += __shfl_xor_sync(0xffffffffu, s, 2);
-        // w split to bf16 hi / lo into rows 0 and 1 of the pooling operand (K byte 2 pr); w = 0 past nt
-        const float w = pr < nt ? rcp_approx(1.f + __expf(-(s + p.au_bout))) : 0.f;
-        if (cq == 0) {
-          const __nv_bfloat16 wh16 = __float2bfloat16_rn(w);
-          const __nv_bfloat16 wl16 = __float2bfloat16_rn(w - __bfloat162float(wh16));
-          st_shared_u16(pb_s + sw128_offset(0, pr >> 3) + 2 * (pr & 7), __bfloat16_as_ushort(wh16));
-          st_shared_u16(pb_s + sw128_offset(1, pr >> 3) + 2 * (pr & 7), __bfloat16_as_ushort(wl16));
         }
       }
       fence_async_smem();
       named_sync(1 + q, 128);                                 // w in place
       clk.lap(PH_GATE);
       // ---- pooling: D (+)= A^T Pb over the tile's 64 positions, A read MN-major (its 128-byte rows are
-      // positions); products h_hi w_hi, h_lo w_hi, h_hi w_lo as in the activation unit
+      // positions); products h_hi w_hi, h_lo w_hi, h_hi w_lo as in the activation unit; the rows' MMAs in one
+      // commit group
       {
         // (an accumulator set that stayed live across the next activation-unit MMAs would make ptxas spill)
-        const uint32_t sa = smem_u32(tiles + (k & 1) * L::A_BYTES), sp = pb_s;
-        float pd[KB][4];
+        float pd[R][KB][4];
         mma_fence();
   #pragma unroll
-        for (int s = 0; s < kWgPos / 16; ++s)
+        for (int s = 0; s < R; ++s) {
+          const uint32_t as = live[s] ? sa + s * L::A_BYTES : sa, ps = live[s] ? pb_s + s * L::PB_BYTES : pb_s;
   #pragma unroll
-          for (int kb = 0; kb < KB; ++kb)
-            mma_m64n8_ss_amn(pd[kb], desc_sw128_mn(sa + kb * (kWgPos * 128) + s * 2048), desc_sw128(sp + 32 * s),
-                             s > 0);
+          for (int ks = 0; ks < kWgPos / 16; ++ks)
+  #pragma unroll
+            for (int kb = 0; kb < KB; ++kb)
+              mma_m64n8_ss_amn(pd[s][kb], desc_sw128_mn(as + kb * (kWgPos * 128) + ks * 2048),
+                               desc_sw128(ps + 32 * ks), ks > 0);
+        }
         mma_commit();
+        // the next row's W_r and gate constants under the MMAs: every warp of the warpgroup has waited for this
+        // row's activation-unit MMAs (the gate barrier) and used its gate constants
+        if (k + 1 < n_items && item_ch(k + 1) == 0) build_wr(k + 1);
+        clk.lap(PH_W_BUILD);
         mma_wait<0>();
   #pragma unroll
-        for (int kb = 0; kb < KB; ++kb) {
-          reg_fence(pd[kb]);
+        for (int s = 0; s < R; ++s) {
+          if (!live[s]) continue;
   #pragma unroll
-          for (int i = 0; i < 4; ++i) pacc[kb][i] = ch > 0 ? pacc[kb][i] + pd[kb][i] : pd[kb][i];
+          for (int kb = 0; kb < KB; ++kb) {
+            reg_fence(pd[s][kb]);
+  #pragma unroll
+            for (int e = 0; e < 4; ++e) pacc[s][kb][e] = ch > 0 ? pacc[s][kb][e] + pd[s][kb][e] : pd[s][kb][e];
+          }
         }
       }
-      // lanes cq = 0 hold columns w hi (pacc[.][0], [2]) and w lo ([1], [3]) of operand columns 16 warp + g (+ 8);
+      // lanes cq = 0 hold columns w hi (pacc[s][.][0], [2]) and w lo ([1], [3]) of operand columns 16 warp + g (+ 8);
       // at EP = 32 the lo elements' sums (columns 32 + e) are in warps 2 and 3 and go through shared memory
       const bool last = ch == nch - 1;
       if (EP == 32 && last && warp >= 2 && cq == 0) {
-        pool_lo[16 * (warp - 2) + g] = pacc[0][0];
-        pool_lo[16 * (warp - 2) + g + 8] = pacc[0][2];
+  #pragma unroll
+        for (int s = 0; s < R; ++s) {
+          if (!live[s]) continue;
+          pool_lo[32 * s + 16 * (warp - 2) + g] = pacc[s][0][0];
+          pool_lo[32 * s + 16 * (warp - 2) + g + 8] = pacc[s][0][2];
+        }
       }
-      named_sync(1 + q, 128);                                 // tile k, Pb and W_r free again
+      named_sync(1 + q, 128);                                 // tiles of item k, Pb and W_r free again
       if (last && cq == 0 && (EP == 64 || warp < 2)) {
   #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int e = 16 * warp + g + 8 * i;
-          const float lo_whi = EP == 32 ? pool_lo[e] : pacc[KB - 1][2 * i];
-          xrow[OFF_POOL + e] = (pacc[0][2 * i] + lo_whi) + pacc[0][2 * i + 1];
+        for (int s = 0; s < R; ++s) {
+          if (!live[s]) continue;
+          float* xrow = Xs + r[s] * L::LDX;
+  #pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int e = 16 * warp + g + 8 * h;
+            const float lo_whi = EP == 32 ? pool_lo[32 * s + e] : pacc[s][KB - 1][2 * h];
+            xrow[OFF_POOL + e] = (pacc[s][0][2 * h] + lo_whi) + pacc[s][0][2 * h + 1];
+          }
         }
       }
       clk.lap(PH_POOL);
@@ -593,13 +680,21 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
       if (L::IMG_RELOAD > 0 && tid == 0) {
         // every warpgroup is past its last wgmma and shared-memory access of the history tiles (the barrier
         // above); the fence orders those before the bulk copy that writes the image's top over them
+        // (W1^T's part first: Dense(128) waits for it, Dense(64) for W2^T's)
         fence_async_smem();
-        mbar_arrive_expect_tx(&reload_bar, L::IMG_RELOAD);
-        for (uint32_t off = L::IMG_RESIDENT; off < L::IMG_BYTES; off += 32768u)
-          bulk_g2s(img + off, p.mlp_image + off, min(32768u, L::IMG_BYTES - off), &reload_bar);
+        if (L::RELOAD_W1 > 0) {
+          mbar_arrive_expect_tx(&reload_bar[0], L::RELOAD_W1);
+          for (uint32_t off = L::IMG_RESIDENT; off < L::RELOAD_W2_OFF; off += 32768u)
+            bulk_g2s(img + off, p.mlp_image + off, min(32768u, L::RELOAD_W2_OFF - off), &reload_bar[0]);
+        }
+        if (L::RELOAD_W2 > 0) {
+          mbar_arrive_expect_tx(&reload_bar[1], L::RELOAD_W2);
+          for (uint32_t off = L::RELOAD_W2_OFF; off < L::IMG_BYTES; off += 32768u)
+            bulk_g2s(img + off, p.mlp_image + off, min(32768u, L::IMG_BYTES - off), &reload_bar[1]);
+        }
       }
       top_mlp_wg<EP>(p, b, row0, Xs, base + L::OPS_OFF, img, fs + L::F_RED, weights_ready ? nullptr : &res_bar,
-                     &reload_bar, reload_parity, clk);
+                     reload_bar, reload_parity, clk);
       weights_ready = true;
       reload_parity ^= 1u;
     } else {
