@@ -33,12 +33,10 @@
 #include <algorithm>
 #include <climits>
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
 #include <vector>
 
 #include "../../include/srs_ctr.h"
-#include "kernels.h"
+#include "hostcall.h"
 
 namespace srs {
 namespace {
@@ -56,37 +54,8 @@ constexpr int kSrcPerBlock = kRecWarps * kSrcPerWarp;
 constexpr int kTile = 128;             // destinations per shared-memory tile, 4 per lane
 constexpr unsigned kFull = 0xffffffffu;
 
-int als_fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  return set_last_error(code, buf);
-}
-
-#define ALS_TRY(expr)                                                                                     \
-  do {                                                                                                    \
-    cudaError_t e__ = (expr);                                                                             \
-    if (e__ != cudaSuccess)                                                                               \
-      return als_fail(SRS_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
-
-#define ALS_LAUNCHED()                                                                                    \
-  do {                                                                                                    \
-    ++g_launch_count;                                                                                     \
-    ALS_TRY(cudaGetLastError());                                                                          \
-  } while (0)
-
-uint64_t splitmix(uint64_t x, uint64_t i) {
-  uint64_t z = x + (i + 1) * 0x9E3779B97F4A7C15ULL;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-  return z ^ (z >> 31);
-}
-
 // The initial factor of the user with id `user`: `rank` draws of java.util.Random.nextGaussian's polar method on
-// uniforms (top 53 bits of splitmix(splitmix(seed, user), c)) / 2^53, each cast to float, then scaled by
+// uniforms uniform53(splitmix(seed, user), c), each cast to float, then scaled by
 // 1.0f / snrm2 (reference BLAS's scaled sum of squares).  oracle/als_c.c restates this function line for line.
 void init_factor(uint64_t seed, int32_t user, int rank, float* out) {
   const uint64_t key = splitmix(seed, (uint64_t)(uint32_t)user);
@@ -94,8 +63,8 @@ void init_factor(uint64_t seed, int32_t user, int rank, float* out) {
   for (int d = 0; d < rank; d += 2) {
     double v1, v2, s;
     do {
-      v1 = 2 * ((double)(splitmix(key, c++) >> 11) * 0x1p-53) - 1;
-      v2 = 2 * ((double)(splitmix(key, c++) >> 11) * 0x1p-53) - 1;
+      v1 = 2 * uniform53(key, c++) - 1;
+      v2 = 2 * uniform53(key, c++) - 1;
       s = v1 * v1 + v2 * v2;
     } while (s >= 1 || s == 0);
     const double m = std::sqrt(-2 * std::log(s) / s);
@@ -117,11 +86,6 @@ void init_factor(uint64_t seed, int32_t user, int rank, float* out) {
   }
   const float inv = 1.0f / (scale * std::sqrt(ssq));
   for (int d = 0; d < rank; ++d) out[d] = out[d] * inv;
-}
-
-int grid_for(int64_t n, int threads) {
-  int64_t b = (n + threads - 1) / threads;
-  return (int)(b < 1 ? 1 : b > 132 * 64 ? 132 * 64 : b);
 }
 
 __global__ void als_iota_kernel(int32_t* __restrict__ out, int n) {
@@ -429,46 +393,6 @@ __global__ void __launch_bounds__(kRecWarps * 32) als_recommend_kernel(const flo
   }
 }
 
-int select_device(int32_t device) {
-  int ndev = 0;
-  cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev == 0)
-    return als_fail(SRS_ERR_CUDA, "no CUDA device available (%s); this library has no CPU path", cudaGetErrorString(ce));
-  if (device < 0 || device >= ndev) return als_fail(SRS_ERR_INVALID, "device %d out of range", device);
-  ALS_TRY(cudaSetDevice(device));
-  return SRS_OK;
-}
-
-struct StreamGuard {
-  cudaStream_t s = nullptr;
-  ~StreamGuard() {
-    if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
-  }
-};
-
-// CUB's temporary storage, grown as the calls ask
-struct CubTemp {
-  Scratch* sc;
-  void* p = nullptr;
-  size_t bytes = 0;
-  cudaError_t need(size_t b) {
-    if (b <= bytes) return cudaSuccess;
-    uint8_t* q = nullptr;
-    cudaError_t e = sc->alloc(&q, b);
-    p = q;
-    bytes = b;
-    return e;
-  }
-};
-
-#define ALS_CUB(call_with_tmp)                                                                            \
-  do {                                                                                                    \
-    size_t need__ = 0;                                                                                    \
-    { void* tmp__ = nullptr; size_t& tb__ = need__; ALS_TRY(call_with_tmp); }                            \
-    ALS_TRY(ct.need(need__));                                                                             \
-    { void* tmp__ = ct.p; size_t tb__ = ct.bytes; ALS_TRY(call_with_tmp); }                              \
-  } while (0)
-
 int bits_for(int n) {
   int b = 1;
   while (b < 31 && (1 << b) < n) ++b;
@@ -476,21 +400,21 @@ int bits_for(int n) {
 }
 
 int check_params(int32_t rank, int32_t max_iter, double reg_param) {
-  if (rank < 1 || rank > kMaxRank) return als_fail(SRS_ERR_INVALID, "rank %d outside 1..%d", rank, kMaxRank);
-  if (max_iter < 1) return als_fail(SRS_ERR_INVALID, "max_iter %d is not positive", max_iter);
+  if (rank < 1 || rank > kMaxRank) return failf(SRS_ERR_INVALID, "rank %d outside 1..%d", rank, kMaxRank);
+  if (max_iter < 1) return failf(SRS_ERR_INVALID, "max_iter %d is not positive", max_iter);
   if (!std::isfinite(reg_param) || reg_param < 0)
-    return als_fail(SRS_ERR_INVALID, "reg_param %g is not finite and >= 0", reg_param);
+    return failf(SRS_ERR_INVALID, "reg_param %g is not finite and >= 0", reg_param);
   return SRS_OK;
 }
 
 int check_ratings(const int32_t* user_id, const int32_t* movie_id, const float* rating, int64_t n_ratings) {
   if (n_ratings < 1 || n_ratings > kMaxRatings)
-    return als_fail(SRS_ERR_INVALID, "n_ratings %lld outside 1..%lld", (long long)n_ratings, (long long)kMaxRatings);
-  if (!user_id || !movie_id || !rating) return als_fail(SRS_ERR_INVALID, "null ratings");
+    return failf(SRS_ERR_INVALID, "n_ratings %lld outside 1..%lld", (long long)n_ratings, (long long)kMaxRatings);
+  if (!user_id || !movie_id || !rating) return failf(SRS_ERR_INVALID, "null ratings");
   for (int64_t i = 0; i < n_ratings; ++i) {
     if (user_id[i] < 0 || movie_id[i] < 0)
-      return als_fail(SRS_ERR_INVALID, "rating %d: negative id (user %d, movie %d)", (int)i, user_id[i], movie_id[i]);
-    if (!std::isfinite(rating[i])) return als_fail(SRS_ERR_INVALID, "rating %d is not finite", (int)i);
+      return failf(SRS_ERR_INVALID, "rating %d: negative id (user %d, movie %d)", (int)i, user_id[i], movie_id[i]);
+    if (!std::isfinite(rating[i])) return failf(SRS_ERR_INVALID, "rating %d is not finite", (int)i);
   }
   return SRS_OK;
 }
@@ -504,26 +428,28 @@ struct Layouts {
   std::vector<int32_t> uid;            // d_uids on the host
 };
 
-int build_layouts(Scratch& sc, CubTemp& ct, cudaStream_t s, const int32_t* user_id, const int32_t* movie_id,
-                  const float* rating, int n, int32_t user_capacity, int32_t movie_capacity, Layouts* L) {
+int build_layouts(HostCall& c, const int32_t* user_id, const int32_t* movie_id, const float* rating, int n,
+                  int32_t user_capacity, int32_t movie_capacity, Layouts* L) {
+  Scratch& sc = c.sc;
+  cudaStream_t s = c.s;
   const int T = 256, G = grid_for(n, T);
   int32_t *d_user, *d_movie, *d_iota, *d_key, *d_perm_u, *d_perm_m, *d_head, *d_seg, *d_du, *d_dm;
   int32_t *d_uids, *d_ucnt, *d_mids, *d_mcnt, *d_bm, *d_bu, *d_src_m, *d_src_u;
   float *d_rating, *d_r_m, *d_r_u;
   int* d_count;
-  ALS_TRY(sc.alloc(&d_user, n)); ALS_TRY(sc.alloc(&d_movie, n)); ALS_TRY(sc.alloc(&d_rating, n));
-  ALS_TRY(sc.alloc(&d_iota, n)); ALS_TRY(sc.alloc(&d_key, n)); ALS_TRY(sc.alloc(&d_perm_u, n));
-  ALS_TRY(sc.alloc(&d_perm_m, n)); ALS_TRY(sc.alloc(&d_head, n)); ALS_TRY(sc.alloc(&d_seg, n));
-  ALS_TRY(sc.alloc(&d_du, n)); ALS_TRY(sc.alloc(&d_dm, n)); ALS_TRY(sc.alloc(&d_uids, n));
-  ALS_TRY(sc.alloc(&d_ucnt, n + 1)); ALS_TRY(sc.alloc(&d_mids, n)); ALS_TRY(sc.alloc(&d_mcnt, n + 1));
-  ALS_TRY(sc.alloc(&d_bm, n)); ALS_TRY(sc.alloc(&d_bu, n)); ALS_TRY(sc.alloc(&d_src_m, n));
-  ALS_TRY(sc.alloc(&d_src_u, n)); ALS_TRY(sc.alloc(&d_r_m, n)); ALS_TRY(sc.alloc(&d_r_u, n));
-  ALS_TRY(sc.alloc(&d_count, 2));
-  ALS_TRY(cudaMemcpyAsync(d_user, user_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-  ALS_TRY(cudaMemcpyAsync(d_movie, movie_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-  ALS_TRY(cudaMemcpyAsync(d_rating, rating, sizeof(float) * n, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(sc.alloc(&d_user, n)); CUDA_TRY(sc.alloc(&d_movie, n)); CUDA_TRY(sc.alloc(&d_rating, n));
+  CUDA_TRY(sc.alloc(&d_iota, n)); CUDA_TRY(sc.alloc(&d_key, n)); CUDA_TRY(sc.alloc(&d_perm_u, n));
+  CUDA_TRY(sc.alloc(&d_perm_m, n)); CUDA_TRY(sc.alloc(&d_head, n)); CUDA_TRY(sc.alloc(&d_seg, n));
+  CUDA_TRY(sc.alloc(&d_du, n)); CUDA_TRY(sc.alloc(&d_dm, n)); CUDA_TRY(sc.alloc(&d_uids, n));
+  CUDA_TRY(sc.alloc(&d_ucnt, n + 1)); CUDA_TRY(sc.alloc(&d_mids, n)); CUDA_TRY(sc.alloc(&d_mcnt, n + 1));
+  CUDA_TRY(sc.alloc(&d_bm, n)); CUDA_TRY(sc.alloc(&d_bu, n)); CUDA_TRY(sc.alloc(&d_src_m, n));
+  CUDA_TRY(sc.alloc(&d_src_u, n)); CUDA_TRY(sc.alloc(&d_r_m, n)); CUDA_TRY(sc.alloc(&d_r_u, n));
+  CUDA_TRY(sc.alloc(&d_count, 2));
+  CUDA_TRY(cudaMemcpyAsync(d_user, user_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_movie, movie_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_rating, rating, sizeof(float) * n, cudaMemcpyHostToDevice, s));
   als_iota_kernel<<<G, T, 0, s>>>(d_iota, n);
-  ALS_LAUNCHED();
+  LAUNCHED();
 
   // the dense ids: a stable sort by raw id, its run-length encoding, and each rating's segment
   const int32_t* raw[2] = {d_user, d_movie};
@@ -532,44 +458,44 @@ int build_layouts(Scratch& sc, CubTemp& ct, cudaStream_t s, const int32_t* user_
   int32_t* cnt[2] = {d_ucnt, d_mcnt};
   int32_t* dense[2] = {d_du, d_dm};
   for (int side = 0; side < 2; ++side) {
-    ALS_CUB(cub::DeviceRadixSort::SortPairs(tmp__, tb__, raw[side], d_key, d_iota, perm[side], n, 0, 31, s));
-    ALS_CUB(cub::DeviceRunLengthEncode::Encode(tmp__, tb__, d_key, uniq[side], cnt[side], d_count + side, n, s));
+    CUB_RUN(c, cub::DeviceRadixSort::SortPairs(tmp__, tb__, raw[side], d_key, d_iota, perm[side], n, 0, 31, s));
+    CUB_RUN(c, cub::DeviceRunLengthEncode::Encode(tmp__, tb__, d_key, uniq[side], cnt[side], d_count + side, n, s));
     als_head_kernel<<<G, T, 0, s>>>(d_key, n, d_head);
-    ALS_LAUNCHED();
-    ALS_CUB(cub::DeviceScan::InclusiveSum(tmp__, tb__, d_head, d_seg, n, s));
+    LAUNCHED();
+    CUB_RUN(c, cub::DeviceScan::InclusiveSum(tmp__, tb__, d_head, d_seg, n, s));
     als_scatter_kernel<<<G, T, 0, s>>>(perm[side], d_seg, n, dense[side]);
-    ALS_LAUNCHED();
+    LAUNCHED();
   }
   int counts[2];
-  ALS_TRY(cudaMemcpyAsync(counts, d_count, sizeof(counts), cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(counts, d_count, sizeof(counts), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   const int nU = counts[0], nM = counts[1];
-  if (nU > user_capacity) return als_fail(SRS_ERR_RANGE, "%d users exceed capacity %d", nU, user_capacity);
-  if (nM > movie_capacity) return als_fail(SRS_ERR_RANGE, "%d movies exceed capacity %d", nM, movie_capacity);
+  if (nU > user_capacity) return failf(SRS_ERR_RANGE, "%d users exceed capacity %d", nU, user_capacity);
+  if (nM > movie_capacity) return failf(SRS_ERR_RANGE, "%d movies exceed capacity %d", nM, movie_capacity);
   L->uid.resize(nU);
-  ALS_TRY(cudaMemcpyAsync(L->uid.data(), d_uids, sizeof(int32_t) * nU, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(L->uid.data(), d_uids, sizeof(int32_t) * nU, cudaMemcpyDeviceToHost, s));
 
   // by-movie layout: the (user, input)-ordered ratings stably sorted by dense movie; by-user: that by dense user
   als_key_kernel<<<G, T, 0, s>>>(d_perm_u, d_dm, n, d_key);
-  ALS_LAUNCHED();
-  ALS_CUB(cub::DeviceRadixSort::SortPairs(tmp__, tb__, d_key, d_head, d_perm_u, d_bm, n, 0, bits_for(nM), s));
+  LAUNCHED();
+  CUB_RUN(c, cub::DeviceRadixSort::SortPairs(tmp__, tb__, d_key, d_head, d_perm_u, d_bm, n, 0, bits_for(nM), s));
   als_key_kernel<<<G, T, 0, s>>>(d_bm, d_du, n, d_key);
-  ALS_LAUNCHED();
-  ALS_CUB(cub::DeviceRadixSort::SortPairs(tmp__, tb__, d_key, d_head, d_bm, d_bu, n, 0, bits_for(nU), s));
+  LAUNCHED();
+  CUB_RUN(c, cub::DeviceRadixSort::SortPairs(tmp__, tb__, d_key, d_head, d_bm, d_bu, n, 0, bits_for(nU), s));
   als_gather_kernel<<<G, T, 0, s>>>(d_bm, d_du, d_rating, n, d_src_m, d_r_m);
-  ALS_LAUNCHED();
+  LAUNCHED();
   als_gather_kernel<<<G, T, 0, s>>>(d_bu, d_dm, d_rating, n, d_src_u, d_r_u);
-  ALS_LAUNCHED();
+  LAUNCHED();
   // each side's offsets and its entities longest first (ties: lower index first)
   int32_t *d_moff, *d_uoff, *d_morder, *d_uorder;
-  ALS_TRY(sc.alloc(&d_moff, nM + 1)); ALS_TRY(sc.alloc(&d_uoff, nU + 1));
-  ALS_TRY(sc.alloc(&d_morder, nM)); ALS_TRY(sc.alloc(&d_uorder, nU));
-  ALS_TRY(cudaMemsetAsync(d_mcnt + nM, 0, sizeof(int32_t), s));
-  ALS_TRY(cudaMemsetAsync(d_ucnt + nU, 0, sizeof(int32_t), s));
-  ALS_CUB(cub::DeviceScan::ExclusiveSum(tmp__, tb__, d_mcnt, d_moff, nM + 1, s));
-  ALS_CUB(cub::DeviceScan::ExclusiveSum(tmp__, tb__, d_ucnt, d_uoff, nU + 1, s));
-  ALS_CUB(cub::DeviceRadixSort::SortPairsDescending(tmp__, tb__, d_mcnt, d_key, d_iota, d_morder, nM, 0, 31, s));
-  ALS_CUB(cub::DeviceRadixSort::SortPairsDescending(tmp__, tb__, d_ucnt, d_key, d_iota, d_uorder, nU, 0, 31, s));
+  CUDA_TRY(sc.alloc(&d_moff, nM + 1)); CUDA_TRY(sc.alloc(&d_uoff, nU + 1));
+  CUDA_TRY(sc.alloc(&d_morder, nM)); CUDA_TRY(sc.alloc(&d_uorder, nU));
+  CUDA_TRY(cudaMemsetAsync(d_mcnt + nM, 0, sizeof(int32_t), s));
+  CUDA_TRY(cudaMemsetAsync(d_ucnt + nU, 0, sizeof(int32_t), s));
+  CUB_RUN(c, cub::DeviceScan::ExclusiveSum(tmp__, tb__, d_mcnt, d_moff, nM + 1, s));
+  CUB_RUN(c, cub::DeviceScan::ExclusiveSum(tmp__, tb__, d_ucnt, d_uoff, nU + 1, s));
+  CUB_RUN(c, cub::DeviceRadixSort::SortPairsDescending(tmp__, tb__, d_mcnt, d_key, d_iota, d_morder, nM, 0, 31, s));
+  CUB_RUN(c, cub::DeviceRadixSort::SortPairsDescending(tmp__, tb__, d_ucnt, d_key, d_iota, d_uorder, nU, 0, 31, s));
   L->nU = nU;
   L->nM = nM;
   L->d_uids = d_uids;
@@ -591,27 +517,24 @@ extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id,
                                 int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
                                 float* user_factors, int32_t* n_users, int32_t* movie_ids, float* movie_factors,
                                 int32_t* n_movies) {
-  if (!n_users || !n_movies) return als_fail(SRS_ERR_INVALID, "null n_users or n_movies");
+  if (!n_users || !n_movies) return failf(SRS_ERR_INVALID, "null n_users or n_movies");
   *n_users = 0;
   *n_movies = 0;
-  if (!params) return als_fail(SRS_ERR_INVALID, "null params");
+  if (!params) return failf(SRS_ERR_INVALID, "null params");
   const srs_als_params hp = *params;
-  if (int rc = check_params(hp.rank, hp.max_iter, hp.reg_param)) return rc;
-  if (int rc = check_ratings(user_id, movie_id, rating, n_ratings)) return rc;
+  PROPAGATE(check_params(hp.rank, hp.max_iter, hp.reg_param));
+  PROPAGATE(check_ratings(user_id, movie_id, rating, n_ratings));
   if (user_capacity < 0 || movie_capacity < 0 || (user_capacity > 0 && (!user_ids || !user_factors)) ||
       (movie_capacity > 0 && (!movie_ids || !movie_factors)))
-    return als_fail(SRS_ERR_INVALID, "negative capacity or null outputs");
-  if (int rc = select_device(device)) return rc;
+    return failf(SRS_ERR_INVALID, "negative capacity or null outputs");
 
-  Scratch sc;
-  CubTemp ct{&sc};
-  StreamGuard sg;
-  ALS_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
-  cudaStream_t s = sg.s;
+  HostCall c;
+  PROPAGATE(c.begin(device));
+  Scratch& sc = c.sc;
+  cudaStream_t s = c.s;
   const int k = hp.rank;
   Layouts L;
-  if (int rc = build_layouts(sc, ct, s, user_id, movie_id, rating, (int)n_ratings, user_capacity, movie_capacity, &L))
-    return rc;
+  PROPAGATE(build_layouts(c, user_id, movie_id, rating, (int)n_ratings, user_capacity, movie_capacity, &L));
   const int nU = L.nU, nM = L.nM;
 
   // the users' initial factors, drawn on the host
@@ -619,33 +542,33 @@ extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id,
   for (int u = 0; u < nU; ++u) init_factor(hp.seed, L.uid[u], k, init.data() + (size_t)u * k);
   float *d_uf, *d_mf;
   unsigned long long* d_err;
-  ALS_TRY(sc.alloc(&d_uf, (size_t)nU * k)); ALS_TRY(sc.alloc(&d_mf, (size_t)nM * k)); ALS_TRY(sc.alloc(&d_err, 1));
-  ALS_TRY(cudaMemcpyAsync(d_uf, init.data(), sizeof(float) * init.size(), cudaMemcpyHostToDevice, s));
-  ALS_TRY(cudaMemsetAsync(d_err, 0xff, sizeof(unsigned long long), s));
+  CUDA_TRY(sc.alloc(&d_uf, (size_t)nU * k)); CUDA_TRY(sc.alloc(&d_mf, (size_t)nM * k)); CUDA_TRY(sc.alloc(&d_err, 1));
+  CUDA_TRY(cudaMemcpyAsync(d_uf, init.data(), sizeof(float) * init.size(), cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemsetAsync(d_err, 0xff, sizeof(unsigned long long), s));
   const size_t sm = solve_smem(k);
   for (int it = 0; it < hp.max_iter; ++it) {
     als_solve_kernel<false><<<nM, kSolveThreads, sm, s>>>(L.movies, d_uf, d_mf, k, hp.reg_param, d_err, 2ull * it,
                                                           Batch{});
-    ALS_LAUNCHED();
+    LAUNCHED();
     als_solve_kernel<false><<<nU, kSolveThreads, sm, s>>>(L.users, d_mf, d_uf, k, hp.reg_param, d_err,
                                                           2ull * it + 1, Batch{});
-    ALS_LAUNCHED();
+    LAUNCHED();
   }
   unsigned long long err = 0;
-  ALS_TRY(cudaMemcpyAsync(&err, d_err, sizeof(err), cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(&err, d_err, sizeof(err), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   if (err != ~0ull) {
     const int hs = (int)(err >> 32), ent = (int)(err & 0xffffffffu);
     int32_t id = 0;
-    ALS_TRY(cudaMemcpy(&id, (hs & 1 ? L.d_uids : L.d_mids) + ent, sizeof(int32_t), cudaMemcpyDeviceToHost));
-    return als_fail(SRS_ERR_INVALID, "singular normal equations for %s %d in iteration %d (a pivot <= 0 or NaN)",
+    CUDA_TRY(cudaMemcpy(&id, (hs & 1 ? L.d_uids : L.d_mids) + ent, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return failf(SRS_ERR_INVALID, "singular normal equations for %s %d in iteration %d (a pivot <= 0 or NaN)",
                     hs & 1 ? "user" : "movie", id, hs / 2 + 1);
   }
-  ALS_TRY(cudaMemcpyAsync(user_ids, L.d_uids, sizeof(int32_t) * nU, cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaMemcpyAsync(user_factors, d_uf, sizeof(float) * nU * k, cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaMemcpyAsync(movie_ids, L.d_mids, sizeof(int32_t) * nM, cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaMemcpyAsync(movie_factors, d_mf, sizeof(float) * nM * k, cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(user_ids, L.d_uids, sizeof(int32_t) * nU, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(user_factors, d_uf, sizeof(float) * nU * k, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(movie_ids, L.d_mids, sizeof(int32_t) * nM, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(movie_factors, d_mf, sizeof(float) * nM * k, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   *n_users = nU;
   *n_movies = nM;
   return SRS_OK;
@@ -658,43 +581,41 @@ extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* mov
                                       float* user_factors, int32_t* n_users, int32_t* movie_ids,
                                       float* movie_factors, int32_t* n_movies) {
   if (n_models < 1 || n_models > kMaxModels)
-    return als_fail(SRS_ERR_INVALID, "n_models %d outside 1..%d", n_models, kMaxModels);
-  if (!models || !n_users || !n_movies) return als_fail(SRS_ERR_INVALID, "null models, n_users or n_movies");
+    return failf(SRS_ERR_INVALID, "n_models %d outside 1..%d", n_models, kMaxModels);
+  if (!models || !n_users || !n_movies) return failf(SRS_ERR_INVALID, "null models, n_users or n_movies");
   for (int m = 0; m < n_models; ++m) n_users[m] = n_movies[m] = 0;
   if (n_folds < 2 || n_folds > kMaxFolds)
-    return als_fail(SRS_ERR_INVALID, "n_folds %d outside 2..%d", n_folds, kMaxFolds);
+    return failf(SRS_ERR_INVALID, "n_folds %d outside 2..%d", n_folds, kMaxFolds);
   const std::vector<srs_als_model> md(models, models + n_models);
   for (int m = 0; m < n_models; ++m) {
     if (int rc = check_params(md[m].rank, md[m].max_iter, md[m].reg_param))
-      return als_fail(rc, "model %d: %s", m, srs_last_error());
+      return failf(rc, "model %d: %s", m, srs_last_error());
     if (md[m].exclude_fold < -1 || md[m].exclude_fold >= n_folds)
-      return als_fail(SRS_ERR_INVALID, "model %d: exclude_fold %d outside -1..%d", m, md[m].exclude_fold, n_folds - 1);
+      return failf(SRS_ERR_INVALID, "model %d: exclude_fold %d outside -1..%d", m, md[m].exclude_fold, n_folds - 1);
   }
-  if (int rc = check_ratings(user_id, movie_id, rating, n_ratings)) return rc;
-  if (!fold) return als_fail(SRS_ERR_INVALID, "null fold");
+  PROPAGATE(check_ratings(user_id, movie_id, rating, n_ratings));
+  if (!fold) return failf(SRS_ERR_INVALID, "null fold");
   if (user_capacity < 0 || movie_capacity < 0 || (user_capacity > 0 && (!user_ids || !user_factors)) ||
       (movie_capacity > 0 && (!movie_ids || !movie_factors)))
-    return als_fail(SRS_ERR_INVALID, "negative capacity or null outputs");
+    return failf(SRS_ERR_INVALID, "negative capacity or null outputs");
   const int n = (int)n_ratings;
   std::vector<int64_t> in_fold(n_folds, 0);
   for (int i = 0; i < n; ++i) {
     if (fold[i] < 0 || fold[i] >= n_folds)
-      return als_fail(SRS_ERR_INVALID, "rating %d: fold %d outside 0..%d", i, fold[i], n_folds - 1);
+      return failf(SRS_ERR_INVALID, "rating %d: fold %d outside 0..%d", i, fold[i], n_folds - 1);
     ++in_fold[fold[i]];
   }
   for (int m = 0; m < n_models; ++m)
     if (md[m].exclude_fold >= 0 && in_fold[md[m].exclude_fold] == n)
-      return als_fail(SRS_ERR_INVALID, "model %d: no training ratings (every rating is in fold %d)", m,
+      return failf(SRS_ERR_INVALID, "model %d: no training ratings (every rating is in fold %d)", m,
                       md[m].exclude_fold);
-  if (int rc = select_device(device)) return rc;
 
-  Scratch sc;
-  CubTemp ct{&sc};
-  StreamGuard sg;
-  ALS_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
-  cudaStream_t s = sg.s;
+  HostCall c;
+  PROPAGATE(c.begin(device));
+  Scratch& sc = c.sc;
+  cudaStream_t s = c.s;
   Layouts L;
-  if (int rc = build_layouts(sc, ct, s, user_id, movie_id, rating, n, user_capacity, movie_capacity, &L)) return rc;
+  PROPAGATE(build_layouts(c, user_id, movie_id, rating, n, user_capacity, movie_capacity, &L));
   const int nU = L.nU, nM = L.nM, M = n_models, T = 256, G = grid_for(n, T);
 
   // each model's factors over every dense id of the whole set; the initial user factors depend on the rank only
@@ -724,18 +645,18 @@ extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* mov
   float *d_uf, *d_mf;
   BatchModel* d_models;
   unsigned long long* d_err;
-  ALS_TRY(sc.alloc(&d_fold, n)); ALS_TRY(sc.alloc(&d_fold_m, n)); ALS_TRY(sc.alloc(&d_fold_u, n));
-  ALS_TRY(sc.alloc(&d_cnt_m, (size_t)M * nM)); ALS_TRY(sc.alloc(&d_cnt_u, (size_t)M * nU));
-  ALS_TRY(sc.alloc(&d_uf, uf_total)); ALS_TRY(sc.alloc(&d_mf, mf_total));
-  ALS_TRY(sc.alloc(&d_models, M)); ALS_TRY(sc.alloc(&d_err, M));
-  ALS_TRY(cudaMemcpyAsync(d_fold, fold, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-  ALS_TRY(cudaMemcpyAsync(d_uf, init.data(), sizeof(float) * uf_total, cudaMemcpyHostToDevice, s));
-  ALS_TRY(cudaMemcpyAsync(d_models, bm.data(), sizeof(BatchModel) * M, cudaMemcpyHostToDevice, s));
-  ALS_TRY(cudaMemsetAsync(d_err, 0xff, sizeof(unsigned long long) * M, s));
+  CUDA_TRY(sc.alloc(&d_fold, n)); CUDA_TRY(sc.alloc(&d_fold_m, n)); CUDA_TRY(sc.alloc(&d_fold_u, n));
+  CUDA_TRY(sc.alloc(&d_cnt_m, (size_t)M * nM)); CUDA_TRY(sc.alloc(&d_cnt_u, (size_t)M * nU));
+  CUDA_TRY(sc.alloc(&d_uf, uf_total)); CUDA_TRY(sc.alloc(&d_mf, mf_total));
+  CUDA_TRY(sc.alloc(&d_models, M)); CUDA_TRY(sc.alloc(&d_err, M));
+  CUDA_TRY(cudaMemcpyAsync(d_fold, fold, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_uf, init.data(), sizeof(float) * uf_total, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_models, bm.data(), sizeof(BatchModel) * M, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemsetAsync(d_err, 0xff, sizeof(unsigned long long) * M, s));
   als_key_kernel<<<G, T, 0, s>>>(L.d_bm, d_fold, n, d_fold_m);      // each layout's fold ids
-  ALS_LAUNCHED();
+  LAUNCHED();
   als_key_kernel<<<G, T, 0, s>>>(L.d_bu, d_fold, n, d_fold_u);
-  ALS_LAUNCHED();
+  LAUNCHED();
   // one launch per half-step for every model: a model past its max_iter exits at once
   const size_t sm = solve_smem(kmax);
   for (int h = 0; h < half_steps; ++h) {
@@ -745,28 +666,28 @@ extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* mov
     als_solve_kernel<true><<<(unsigned)((int64_t)nE * M), kSolveThreads, sm, s>>>(
         to_users ? L.users : L.movies, to_users ? d_mf : d_uf, to_users ? d_uf : d_mf, 0, 0.0, d_err,
         (unsigned long long)h, bt);
-    ALS_LAUNCHED();
+    LAUNCHED();
   }
   std::vector<unsigned long long> err(M);
-  ALS_TRY(cudaMemcpyAsync(err.data(), d_err, sizeof(unsigned long long) * M, cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(err.data(), d_err, sizeof(unsigned long long) * M, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   for (int m = 0; m < M; ++m) {
     if (err[m] == ~0ull) continue;
     const int hs = (int)(err[m] >> 32), ent = (int)(err[m] & 0xffffffffu);
     int32_t id = 0;
-    ALS_TRY(cudaMemcpy(&id, (hs & 1 ? L.d_uids : L.d_mids) + ent, sizeof(int32_t), cudaMemcpyDeviceToHost));
-    return als_fail(SRS_ERR_INVALID,
+    CUDA_TRY(cudaMemcpy(&id, (hs & 1 ? L.d_uids : L.d_mids) + ent, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return failf(SRS_ERR_INVALID,
                     "model %d: singular normal equations for %s %d in iteration %d (a pivot <= 0 or NaN)", m,
                     hs & 1 ? "user" : "movie", id, hs / 2 + 1);
   }
   std::vector<int32_t> mid(nM), cnt_u((size_t)M * nU), cnt_m((size_t)M * nM);
   std::vector<float> uf(uf_total), mf(mf_total);
-  ALS_TRY(cudaMemcpyAsync(mid.data(), L.d_mids, sizeof(int32_t) * nM, cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaMemcpyAsync(cnt_u.data(), d_cnt_u, sizeof(int32_t) * cnt_u.size(), cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaMemcpyAsync(cnt_m.data(), d_cnt_m, sizeof(int32_t) * cnt_m.size(), cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaMemcpyAsync(uf.data(), d_uf, sizeof(float) * uf_total, cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaMemcpyAsync(mf.data(), d_mf, sizeof(float) * mf_total, cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(mid.data(), L.d_mids, sizeof(int32_t) * nM, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(cnt_u.data(), d_cnt_u, sizeof(int32_t) * cnt_u.size(), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(cnt_m.data(), d_cnt_m, sizeof(int32_t) * cnt_m.size(), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(uf.data(), d_uf, sizeof(float) * uf_total, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(mf.data(), d_mf, sizeof(float) * mf_total, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   // model m's entities are those with a training rating in it, ascending; its outputs start after the models before
   size_t uo = 0, mo = 0;
   for (int m = 0; m < M; ++m) {
@@ -795,43 +716,42 @@ extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* mov
 extern "C" int srs_als_recommend_host(const float* src_factors, int32_t n_src, const int32_t* dst_ids,
                                       const float* dst_factors, int32_t n_dst, int32_t rank, int32_t num,
                                       int32_t device, int32_t* out_ids, float* out_scores) {
-  if (rank < 1 || rank > kMaxRank) return als_fail(SRS_ERR_INVALID, "rank %d outside 1..%d", rank, kMaxRank);
-  if (num < 1 || num > kMaxNum) return als_fail(SRS_ERR_INVALID, "num %d outside 1..%d", num, kMaxNum);
-  if (n_src < 0 || n_dst < 0) return als_fail(SRS_ERR_INVALID, "negative n_src or n_dst");
+  if (rank < 1 || rank > kMaxRank) return failf(SRS_ERR_INVALID, "rank %d outside 1..%d", rank, kMaxRank);
+  if (num < 1 || num > kMaxNum) return failf(SRS_ERR_INVALID, "num %d outside 1..%d", num, kMaxNum);
+  if (n_src < 0 || n_dst < 0) return failf(SRS_ERR_INVALID, "negative n_src or n_dst");
   if ((n_src && !src_factors) || (n_dst && (!dst_ids || !dst_factors)) ||
       (n_src && n_dst && (!out_ids || !out_scores)))
-    return als_fail(SRS_ERR_INVALID, "null factors, ids or outputs");
+    return failf(SRS_ERR_INVALID, "null factors, ids or outputs");
   for (int32_t i = 1; i < n_dst; ++i)
     if (dst_ids[i] <= dst_ids[i - 1])
-      return als_fail(SRS_ERR_INVALID, "destination ids are not strictly ascending at %d", i);
+      return failf(SRS_ERR_INVALID, "destination ids are not strictly ascending at %d", i);
   for (int64_t i = 0; i < (int64_t)n_src * rank; ++i)
-    if (!std::isfinite(src_factors[i])) return als_fail(SRS_ERR_INVALID, "source factor element %lld is not finite", (long long)i);
+    if (!std::isfinite(src_factors[i])) return failf(SRS_ERR_INVALID, "source factor element %lld is not finite", (long long)i);
   for (int64_t i = 0; i < (int64_t)n_dst * rank; ++i)
     if (!std::isfinite(dst_factors[i]))
-      return als_fail(SRS_ERR_INVALID, "destination factor element %lld is not finite", (long long)i);
+      return failf(SRS_ERR_INVALID, "destination factor element %lld is not finite", (long long)i);
   if (n_src == 0 || n_dst == 0) return SRS_OK;
-  if (int rc = select_device(device)) return rc;
+  HostCall c;
+  PROPAGATE(c.begin(device));
+  Scratch& sc = c.sc;
+  cudaStream_t s = c.s;
   const int L = std::min(num, n_dst), k = rank;
-  Scratch sc;
-  StreamGuard sg;
-  ALS_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
-  cudaStream_t s = sg.s;
   float *d_src, *d_dst, *d_scores;
   int32_t *d_dids, *d_ids;
-  ALS_TRY(sc.alloc(&d_src, (size_t)n_src * k)); ALS_TRY(sc.alloc(&d_dst, (size_t)n_dst * k));
-  ALS_TRY(sc.alloc(&d_dids, n_dst)); ALS_TRY(sc.alloc(&d_ids, (size_t)n_src * L));
-  ALS_TRY(sc.alloc(&d_scores, (size_t)n_src * L));
-  ALS_TRY(cudaMemcpyAsync(d_src, src_factors, sizeof(float) * n_src * k, cudaMemcpyHostToDevice, s));
-  ALS_TRY(cudaMemcpyAsync(d_dst, dst_factors, sizeof(float) * n_dst * k, cudaMemcpyHostToDevice, s));
-  ALS_TRY(cudaMemcpyAsync(d_dids, dst_ids, sizeof(int32_t) * n_dst, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(sc.alloc(&d_src, (size_t)n_src * k)); CUDA_TRY(sc.alloc(&d_dst, (size_t)n_dst * k));
+  CUDA_TRY(sc.alloc(&d_dids, n_dst)); CUDA_TRY(sc.alloc(&d_ids, (size_t)n_src * L));
+  CUDA_TRY(sc.alloc(&d_scores, (size_t)n_src * L));
+  CUDA_TRY(cudaMemcpyAsync(d_src, src_factors, sizeof(float) * n_src * k, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_dst, dst_factors, sizeof(float) * n_dst * k, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_dids, dst_ids, sizeof(int32_t) * n_dst, cudaMemcpyHostToDevice, s));
   const size_t sm = sizeof(float) * k * kTile + sizeof(float4) * k * kRecWarps + (sizeof(float) + sizeof(int)) *
                     kSrcPerBlock * L;
-  ALS_TRY(cudaFuncSetAttribute(als_recommend_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  CUDA_TRY(cudaFuncSetAttribute(als_recommend_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
   als_recommend_kernel<<<(n_src + kSrcPerBlock - 1) / kSrcPerBlock, kRecWarps * 32, sm, s>>>(
       d_src, n_src, d_dids, d_dst, n_dst, k, L, d_ids, d_scores);
-  ALS_LAUNCHED();
-  ALS_TRY(cudaMemcpyAsync(out_ids, d_ids, sizeof(int32_t) * n_src * L, cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaMemcpyAsync(out_scores, d_scores, sizeof(float) * n_src * L, cudaMemcpyDeviceToHost, s));
-  ALS_TRY(cudaStreamSynchronize(s));
+  LAUNCHED();
+  CUDA_TRY(cudaMemcpyAsync(out_ids, d_ids, sizeof(int32_t) * n_src * L, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(out_scores, d_scores, sizeof(float) * n_src * L, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   return SRS_OK;
 }

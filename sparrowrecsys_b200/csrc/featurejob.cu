@@ -18,12 +18,11 @@
 #include <algorithm>
 #include <charconv>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 #include <vector>
 
 #include "../../include/srs_ctr.h"
-#include "kernels.h"
+#include "hostcall.h"
 
 namespace srs {
 namespace {
@@ -38,32 +37,9 @@ constexpr int kMaxParts = 64;
 constexpr int32_t kMaxMovieId = (1 << 24) - 1;
 constexpr int64_t kMaxRatings = 21000000;       // featureeng.cu's bound: every Q and 4n(n-1) below 2^53
 
-int fj_fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  return set_last_error(code, buf);
-}
-
-#define FJ_TRY(expr)                                                                                     \
-  do {                                                                                                   \
-    cudaError_t e__ = (expr);                                                                            \
-    if (e__ != cudaSuccess)                                                                              \
-      return fj_fail(SRS_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
-
-#define FJ_LAUNCHED() do { ++g_launch_count; FJ_TRY(cudaGetLastError()); } while (0)
-
 // a grid-stride loop over 0..n-1 with a 64-bit index: n may come within one grid stride of INT32_MAX
 #define FJ_GRID_STRIDE(i, n) \
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < (n); i += (int64_t)gridDim.x * blockDim.x)
-
-int grid_for(int64_t n, int threads) {
-  int64_t b = (n + threads - 1) / threads;
-  return (int)(b < 1 ? 1 : b > 132 * 64 ? 132 * 64 : b);
-}
 
 // java.lang.Double.compare's total order (-0.0 < 0.0) as unsigned keys; no key of a non-NaN value is ~0
 __host__ __device__ __forceinline__ uint64_t order_key(double x) {
@@ -76,18 +52,6 @@ __host__ __device__ __forceinline__ double key_value(uint64_t k) {
   double x;
   memcpy(&x, &b, 8);
   return x;
-}
-
-// splitmix64's finaliser of x + (i + 1) * golden (collab.random_split's and srs_fill_uniform's hash)
-__host__ __device__ __forceinline__ uint64_t splitmix(uint64_t x, uint64_t i) {
-  uint64_t z = x + (i + 1) * 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
-__device__ __forceinline__ double uniform53(uint64_t key, uint64_t i) {
-  return (double)(splitmix(key, i) >> 11) * 0x1p-53;
 }
 
 // scala.collection.immutable.HashMap.improve (2.11)
@@ -425,41 +389,9 @@ __global__ void fj_flag_count_kernel(const uint8_t* __restrict__ flag, int n, in
 }
 
 // ------------------------------------------------------------------------------------------------- host side
-struct Run {                           // one host call's device, stream and allocations
-  Scratch sc;
-  cudaStream_t s = nullptr;
-  ~Run() {
-    if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
-  }
-};
-
-int begin(Run& r, int32_t device) {
-  int ndev = 0;
-  cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev == 0)
-    return fj_fail(SRS_ERR_CUDA, "no CUDA device available (%s); this library has no CPU path", cudaGetErrorString(ce));
-  if (device < 0 || device >= ndev) return fj_fail(SRS_ERR_INVALID, "device %d out of range", device);
-  FJ_TRY(cudaSetDevice(device));
-  FJ_TRY(cudaStreamCreateWithFlags(&r.s, cudaStreamNonBlocking));
-  return SRS_OK;
-}
-
-template <class T>
-int upload(Run& r, T** d, const T* h, size_t count) {
-  FJ_TRY(r.sc.alloc(d, count));
-  if (count) FJ_TRY(cudaMemcpyAsync(*d, h, sizeof(T) * count, cudaMemcpyHostToDevice, r.s));
-  return SRS_OK;
-}
-
-#define FJ_OK(expr)                       \
-  do {                                    \
-    const int rc__ = (expr);              \
-    if (rc__ != SRS_OK) return rc__;      \
-  } while (0)
-
 // approxQuantile of the first *d_n of n_cap device keys (sorted in place) at np device probabilities -> d_out
-int quantiles_of_keys(Run& r, uint64_t* d_keys, int n_cap, const int* d_n, const double* d_probs, int np, double eps,
-                      double* d_out) {
+int quantiles_of_keys(HostCall& r, uint64_t* d_keys, int n_cap, const int* d_n, const double* d_probs, int np,
+                      double eps, double* d_out) {
   // segments: at most min(heads, runs + 3), runs <= 2 eps n + 1 (fj_compress_kernel)
   const long long by_runs = (long long)(2.0 * eps * (double)n_cap) + 8;
   const int seg_cap = (int)std::min<long long>(n_cap, by_runs) + 2;
@@ -468,123 +400,113 @@ int quantiles_of_keys(Run& r, uint64_t* d_keys, int n_cap, const int* d_n, const
   long long *s_g, *s_minr, *s_d, *d_m;
   QSegment* d_seg;
   int *d_nseg, *d_err;
-  FJ_TRY(r.sc.alloc(&d_sorted, n_cap));
-  FJ_TRY(r.sc.alloc(&s_idx, n_cap));
-  FJ_TRY(r.sc.alloc(&s_g, n_cap));
-  FJ_TRY(r.sc.alloc(&s_minr, n_cap));
-  FJ_TRY(r.sc.alloc(&s_d, n_cap));
-  FJ_TRY(r.sc.alloc(&d_m, 1));
-  FJ_TRY(r.sc.alloc(&d_seg, seg_cap));
-  FJ_TRY(r.sc.alloc(&d_nseg, 1));
-  FJ_TRY(r.sc.alloc(&d_err, 1));
-  size_t t1 = 0, t2 = 0;
-  FJ_TRY(cub::DeviceRadixSort::SortKeys(nullptr, t1, d_keys, d_sorted, n_cap, 0, 64, r.s));
-  FJ_TRY(cub::DeviceScan::InclusiveSum(nullptr, t2, s_g, s_minr, n_cap, r.s));
-  uint8_t* d_tmp;
-  t1 = std::max(t1, t2);
-  FJ_TRY(r.sc.alloc(&d_tmp, t1));
-  FJ_TRY(cub::DeviceRadixSort::SortKeys(d_tmp, t1, d_keys, d_sorted, n_cap, 0, 64, r.s));
+  CUDA_TRY(r.sc.alloc(&d_sorted, n_cap));
+  CUDA_TRY(r.sc.alloc(&s_idx, n_cap));
+  CUDA_TRY(r.sc.alloc(&s_g, n_cap));
+  CUDA_TRY(r.sc.alloc(&s_minr, n_cap));
+  CUDA_TRY(r.sc.alloc(&s_d, n_cap));
+  CUDA_TRY(r.sc.alloc(&d_m, 1));
+  CUDA_TRY(r.sc.alloc(&d_seg, seg_cap));
+  CUDA_TRY(r.sc.alloc(&d_nseg, 1));
+  CUDA_TRY(r.sc.alloc(&d_err, 1));
+  CUB_RUN(r, cub::DeviceRadixSort::SortKeys(tmp__, tb__, d_keys, d_sorted, n_cap, 0, 64, r.s));
   fj_compress_kernel<<<1, 1, 0, r.s>>>(d_n, eps, d_seg, seg_cap, d_nseg, d_m, d_err);
-  FJ_LAUNCHED();
+  LAUNCHED();
   fj_expand_kernel<<<grid_for(n_cap, 256), 256, 0, r.s>>>(d_seg, d_nseg, d_m, d_n, s_idx, s_g, s_d);
-  FJ_LAUNCHED();
+  LAUNCHED();
   // entries past m are never read: the prefix sums below m do not depend on them
-  FJ_TRY(cub::DeviceScan::InclusiveSum(d_tmp, t1, s_g, s_minr, n_cap, r.s));
+  CUB_RUN(r, cub::DeviceScan::InclusiveSum(tmp__, tb__, s_g, s_minr, n_cap, r.s));
   fj_query_kernel<<<(np + 127) / 128, 128, 0, r.s>>>(d_sorted, d_n, s_idx, s_minr, s_d, d_m, d_probs, np, eps, d_out);
-  FJ_LAUNCHED();
+  LAUNCHED();
   int err = 0;
-  FJ_TRY(cudaMemcpyAsync(&err, d_err, sizeof(int), cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaStreamSynchronize(r.s));
-  if (err) return fj_fail(SRS_ERR_INVALID, "approxQuantile: more compress segments than the bound %d", seg_cap);
+  CUDA_TRY(cudaMemcpyAsync(&err, d_err, sizeof(int), cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaStreamSynchronize(r.s));
+  if (err) return failf(SRS_ERR_INVALID, "approxQuantile: more compress segments than the bound %d", seg_cap);
   return SRS_OK;
 }
 
 int check_values(const double* v, int64_t n, const char* what) {
-  if (n < 1 || n > kMaxValues) return fj_fail(SRS_ERR_INVALID, "%s: n %lld outside 1..%lld", what, (long long)n,
+  if (n < 1 || n > kMaxValues) return failf(SRS_ERR_INVALID, "%s: n %lld outside 1..%lld", what, (long long)n,
                                               (long long)kMaxValues);
-  if (!v) return fj_fail(SRS_ERR_INVALID, "%s: null values", what);
+  if (!v) return failf(SRS_ERR_INVALID, "%s: null values", what);
   for (int64_t i = 0; i < n; ++i)
-    if (std::isnan(v[i])) return fj_fail(SRS_ERR_INVALID, "%s: value %lld is NaN", what, (long long)i);
+    if (std::isnan(v[i])) return failf(SRS_ERR_INVALID, "%s: value %lld is NaN", what, (long long)i);
   return SRS_OK;
 }
 
 int check_eps(double eps) {
-  if (!(eps >= 0.0 && eps <= 1.0)) return fj_fail(SRS_ERR_INVALID, "relative_error %g outside [0, 1]", eps);
+  if (!(eps >= 0.0 && eps <= 1.0)) return failf(SRS_ERR_INVALID, "relative_error %g outside [0, 1]", eps);
   return SRS_OK;
 }
 
 // device values -> keys, then the quantiles at host probabilities into d_out
-int quantiles_of_values(Run& r, const double* d_v, int n, const double* probs, int np, double eps, double* d_out) {
+int quantiles_of_values(HostCall& r, const double* d_v, int n, const double* probs, int np, double eps, double* d_out) {
   uint64_t* d_keys;
   double* d_probs;
   int* d_n;
-  FJ_TRY(r.sc.alloc(&d_keys, n));
-  FJ_OK(upload(r, &d_probs, probs, np));
-  FJ_OK(upload(r, &d_n, &n, 1));
+  CUDA_TRY(r.sc.alloc(&d_keys, n));
+  PROPAGATE(r.upload(&d_probs, probs, np));
+  PROPAGATE(r.upload(&d_n, &n, 1));
   fj_keys_kernel<<<grid_for(n, 256), 256, 0, r.s>>>(d_v, n, d_keys);
-  FJ_LAUNCHED();
+  LAUNCHED();
   return quantiles_of_keys(r, d_keys, n, d_n, d_probs, np, eps, d_out);
 }
 
 int check_splits(const double* splits, int32_t n_splits) {
   if (!splits || n_splits < 3 || n_splits > kMaxBuckets + 1)
-    return fj_fail(SRS_ERR_INVALID, "splits: need 3..%d values", kMaxBuckets + 1);
+    return failf(SRS_ERR_INVALID, "splits: need 3..%d values", kMaxBuckets + 1);
   for (int k = 0; k < n_splits; ++k) {
-    if (std::isnan(splits[k])) return fj_fail(SRS_ERR_INVALID, "split %d is NaN", k);
-    if (k && !(splits[k - 1] < splits[k])) return fj_fail(SRS_ERR_INVALID, "splits must be strictly increasing");
+    if (std::isnan(splits[k])) return failf(SRS_ERR_INVALID, "split %d is NaN", k);
+    if (k && !(splits[k - 1] < splits[k])) return failf(SRS_ERR_INVALID, "splits must be strictly increasing");
   }
   return SRS_OK;
 }
 
 // the word-histogram and label order shared by the StringIndexer and the multi-hot encoder; d_label_of [W] and
 // d_label_word / d_label_cnt [W] on the device
-int index_labels(Run& r, const int32_t* d_tok, int n_tok, const int32_t* hash, int W, int32_t** d_label_of,
+int index_labels(HostCall& r, const int32_t* d_tok, int n_tok, const int32_t* hash, int W, int32_t** d_label_of,
                  int32_t** d_label_word, int64_t** d_label_cnt) {
   unsigned long long* d_cnt;
   int32_t *d_hash, *d_word;
   uint64_t *d_key, *d_key2;
-  FJ_TRY(r.sc.alloc(&d_cnt, W));
-  FJ_OK(upload(r, &d_hash, hash, W));
-  FJ_TRY(r.sc.alloc(&d_word, W));
-  FJ_TRY(r.sc.alloc(&d_key, W));
-  FJ_TRY(r.sc.alloc(&d_key2, W));
-  FJ_TRY(r.sc.alloc(d_label_of, W));
-  FJ_TRY(r.sc.alloc(d_label_word, W));
-  FJ_TRY(r.sc.alloc(d_label_cnt, W));
-  FJ_TRY(cudaMemsetAsync(d_cnt, 0, sizeof(unsigned long long) * W, r.s));
+  CUDA_TRY(r.sc.alloc(&d_cnt, W));
+  PROPAGATE(r.upload(&d_hash, hash, W));
+  CUDA_TRY(r.sc.alloc(&d_word, W));
+  CUDA_TRY(r.sc.alloc(&d_key, W));
+  CUDA_TRY(r.sc.alloc(&d_key2, W));
+  CUDA_TRY(r.sc.alloc(d_label_of, W));
+  CUDA_TRY(r.sc.alloc(d_label_word, W));
+  CUDA_TRY(r.sc.alloc(d_label_cnt, W));
+  CUDA_TRY(cudaMemsetAsync(d_cnt, 0, sizeof(unsigned long long) * W, r.s));
   fj_hist_kernel<<<grid_for(n_tok, 256), 256, 0, r.s>>>(d_tok, n_tok, d_cnt);
-  FJ_LAUNCHED();
+  LAUNCHED();
   fj_label_key_kernel<<<grid_for(W, 256), 256, 0, r.s>>>(d_cnt, d_hash, W, d_key, d_word);
-  FJ_LAUNCHED();
-  size_t tmp_bytes = 0;
-  FJ_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d_key, d_key2, d_word, *d_label_word, W, 0, 64, r.s));
-  uint8_t* d_tmp;
-  FJ_TRY(r.sc.alloc(&d_tmp, tmp_bytes));
-  FJ_TRY(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, d_key, d_key2, d_word, *d_label_word, W, 0, 64, r.s));
+  LAUNCHED();
+  CUB_RUN(r, cub::DeviceRadixSort::SortPairs(tmp__, tb__, d_key, d_key2, d_word, *d_label_word, W, 0, 64, r.s));
   fj_label_index_kernel<<<grid_for(W, 256), 256, 0, r.s>>>(*d_label_word, d_cnt, W, *d_label_of, *d_label_cnt);
-  FJ_LAUNCHED();
+  LAUNCHED();
   return SRS_OK;
 }
 
 int check_tokens(const int32_t* tok, int64_t n_tok, const int32_t* hash, int32_t W) {
   if (n_tok < 1 || n_tok > kMaxTokens)
-    return fj_fail(SRS_ERR_INVALID, "n_tokens %lld outside 1..%lld", (long long)n_tok, (long long)kMaxTokens);
-  if (W < 1 || W > kMaxWords) return fj_fail(SRS_ERR_INVALID, "n_words %d outside 1..%d", W, kMaxWords);
-  if (!tok || !hash) return fj_fail(SRS_ERR_INVALID, "null tokens or hashes");
+    return failf(SRS_ERR_INVALID, "n_tokens %lld outside 1..%lld", (long long)n_tok, (long long)kMaxTokens);
+  if (W < 1 || W > kMaxWords) return failf(SRS_ERR_INVALID, "n_words %d outside 1..%d", W, kMaxWords);
+  if (!tok || !hash) return failf(SRS_ERR_INVALID, "null tokens or hashes");
   std::vector<uint8_t> seen(W, 0);
   for (int64_t i = 0; i < n_tok; ++i) {
     if (tok[i] < 0 || tok[i] >= W)
-      return fj_fail(SRS_ERR_INVALID, "token %lld: word %d outside 0..%d", (long long)i, tok[i], W - 1);
+      return failf(SRS_ERR_INVALID, "token %lld: word %d outside 0..%d", (long long)i, tok[i], W - 1);
     seen[tok[i]] = 1;
   }
   for (int w = 0; w < W; ++w)
-    if (!seen[w]) return fj_fail(SRS_ERR_INVALID, "word %d never occurs", w);
+    if (!seen[w]) return failf(SRS_ERR_INVALID, "word %d never occurs", w);
   std::vector<uint64_t> keys(W);
   for (int w = 0; w < W; ++w) keys[w] = trie_key(hash[w]);
   std::sort(keys.begin(), keys.end());
   for (int w = 1; w < W; ++w)
     if (keys[w] == keys[w - 1])
-      return fj_fail(SRS_ERR_INVALID, "two words share improve(hashCode); their hash-trie order is not supported");
+      return failf(SRS_ERR_INVALID, "two words share improve(hashCode); their hash-trie order is not supported");
   return SRS_OK;
 }
 
@@ -618,30 +540,26 @@ uint64_t stream_key(uint64_t seed, uint64_t stream) { return splitmix(seed, stre
 
 // the rows of each part of d_part (device, n) into rows (host), part after part, in input order: one stable radix
 // sort of (part, row) over the part's 8 bits
-int gather_parts(Run& r, const int8_t* d_part, int n, int n_parts, int32_t* rows, int64_t* part_counts) {
+int gather_parts(HostCall& r, const int8_t* d_part, int n, int n_parts, int32_t* rows, int64_t* part_counts) {
   uint8_t *d_key, *d_key2;
   int32_t *d_iota, *d_rows;
   unsigned long long* d_cnt;
-  FJ_TRY(r.sc.alloc(&d_key, n));
-  FJ_TRY(r.sc.alloc(&d_key2, n));
-  FJ_TRY(r.sc.alloc(&d_iota, n));
-  FJ_TRY(r.sc.alloc(&d_rows, n));
-  FJ_TRY(r.sc.alloc(&d_cnt, n_parts));
-  size_t tmp_bytes = 0;
-  FJ_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d_key, d_key2, d_iota, d_rows, n, 0, 8, r.s));
-  uint8_t* d_tmp;
-  FJ_TRY(r.sc.alloc(&d_tmp, tmp_bytes));
-  FJ_TRY(cudaMemsetAsync(d_cnt, 0, sizeof(unsigned long long) * n_parts, r.s));
+  CUDA_TRY(r.sc.alloc(&d_key, n));
+  CUDA_TRY(r.sc.alloc(&d_key2, n));
+  CUDA_TRY(r.sc.alloc(&d_iota, n));
+  CUDA_TRY(r.sc.alloc(&d_rows, n));
+  CUDA_TRY(r.sc.alloc(&d_cnt, n_parts));
+  CUDA_TRY(cudaMemsetAsync(d_cnt, 0, sizeof(unsigned long long) * n_parts, r.s));
   fj_part_count_kernel<<<grid_for(n, 256), 256, 0, r.s>>>(d_part, n, n_parts, d_key, d_iota, d_cnt);
-  FJ_LAUNCHED();
-  FJ_TRY(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, d_key, d_key2, d_iota, d_rows, n, 0, 8, r.s));
+  LAUNCHED();
+  CUB_RUN(r, cub::DeviceRadixSort::SortPairs(tmp__, tb__, d_key, d_key2, d_iota, d_rows, n, 0, 8, r.s));
   std::vector<unsigned long long> cnt(n_parts);
-  FJ_TRY(cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(unsigned long long) * n_parts, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaStreamSynchronize(r.s));
+  CUDA_TRY(cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(unsigned long long) * n_parts, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaStreamSynchronize(r.s));
   unsigned long long total = 0;
   for (int j = 0; j < n_parts; ++j) total += cnt[j];
-  if (total) FJ_TRY(cudaMemcpyAsync(rows, d_rows, sizeof(int32_t) * total, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaStreamSynchronize(r.s));
+  if (total) CUDA_TRY(cudaMemcpyAsync(rows, d_rows, sizeof(int32_t) * total, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaStreamSynchronize(r.s));
   for (int j = 0; j < n_parts; ++j) part_counts[j] = (int64_t)cnt[j];
   return SRS_OK;
 }
@@ -653,67 +571,67 @@ using namespace srs;
 
 extern "C" int srs_approx_quantile_host(const double* values, int64_t n, const double* probabilities,
                                         int32_t n_probabilities, double relative_error, int32_t device, double* out) {
-  FJ_OK(check_values(values, n, "approx_quantile"));
-  FJ_OK(check_eps(relative_error));
+  PROPAGATE(check_values(values, n, "approx_quantile"));
+  PROPAGATE(check_eps(relative_error));
   if (n_probabilities < 1 || n_probabilities > kMaxProbs || !probabilities || !out)
-    return fj_fail(SRS_ERR_INVALID, "need 1..%d probabilities and an output", kMaxProbs);
+    return failf(SRS_ERR_INVALID, "need 1..%d probabilities and an output", kMaxProbs);
   for (int q = 0; q < n_probabilities; ++q)
     if (!(probabilities[q] >= 0.0 && probabilities[q] <= 1.0))
-      return fj_fail(SRS_ERR_INVALID, "probability %d (%g) outside [0, 1]", q, probabilities[q]);
-  Run r;
-  FJ_OK(begin(r, device));
+      return failf(SRS_ERR_INVALID, "probability %d (%g) outside [0, 1]", q, probabilities[q]);
+  HostCall r;
+  PROPAGATE(r.begin(device));
   double *d_v, *d_out;
-  FJ_OK(upload(r, &d_v, values, (size_t)n));
-  FJ_TRY(r.sc.alloc(&d_out, n_probabilities));
-  FJ_OK(quantiles_of_values(r, d_v, (int)n, probabilities, n_probabilities, relative_error, d_out));
-  FJ_TRY(cudaMemcpyAsync(out, d_out, sizeof(double) * n_probabilities, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaStreamSynchronize(r.s));
+  PROPAGATE(r.upload(&d_v, values, (size_t)n));
+  CUDA_TRY(r.sc.alloc(&d_out, n_probabilities));
+  PROPAGATE(quantiles_of_values(r, d_v, (int)n, probabilities, n_probabilities, relative_error, d_out));
+  CUDA_TRY(cudaMemcpyAsync(out, d_out, sizeof(double) * n_probabilities, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaStreamSynchronize(r.s));
   return SRS_OK;
 }
 
 extern "C" int srs_quantile_discretizer_host(const double* values, int64_t n, int32_t num_buckets,
                                              double relative_error, int32_t device, double* splits, int32_t* n_splits,
                                              int32_t* buckets) {
-  FJ_OK(check_values(values, n, "quantile_discretizer"));
-  FJ_OK(check_eps(relative_error));
+  PROPAGATE(check_values(values, n, "quantile_discretizer"));
+  PROPAGATE(check_eps(relative_error));
   if (num_buckets < 2 || num_buckets > kMaxBuckets)
-    return fj_fail(SRS_ERR_INVALID, "num_buckets %d outside 2..%d", num_buckets, kMaxBuckets);
-  if (!splits || !n_splits) return fj_fail(SRS_ERR_INVALID, "null output");
+    return failf(SRS_ERR_INVALID, "num_buckets %d outside 2..%d", num_buckets, kMaxBuckets);
+  if (!splits || !n_splits) return failf(SRS_ERR_INVALID, "null output");
   const std::vector<double> probs = discretizer_probabilities(num_buckets);
   const int nq = (int)probs.size();
   if (nq < 2 || nq > num_buckets + 1)
-    return fj_fail(SRS_ERR_INVALID, "num_buckets %d: %d probabilities from the step's decimal", num_buckets, nq);
-  Run r;
-  FJ_OK(begin(r, device));
+    return failf(SRS_ERR_INVALID, "num_buckets %d: %d probabilities from the step's decimal", num_buckets, nq);
+  HostCall r;
+  PROPAGATE(r.begin(device));
   double *d_v, *d_q, *d_splits;
   int *d_ns, *d_err;
   uint8_t* d_dup;
   int32_t* d_b;
-  FJ_OK(upload(r, &d_v, values, (size_t)n));
-  FJ_TRY(r.sc.alloc(&d_q, nq));
-  FJ_TRY(r.sc.alloc(&d_splits, nq));
-  FJ_TRY(r.sc.alloc(&d_ns, 1));
-  FJ_TRY(r.sc.alloc(&d_err, 1));
-  FJ_TRY(r.sc.alloc(&d_dup, nq));
-  FJ_TRY(r.sc.alloc(&d_b, buckets ? (size_t)n : 1));
-  FJ_OK(quantiles_of_values(r, d_v, (int)n, probs.data(), nq, relative_error, d_q));
+  PROPAGATE(r.upload(&d_v, values, (size_t)n));
+  CUDA_TRY(r.sc.alloc(&d_q, nq));
+  CUDA_TRY(r.sc.alloc(&d_splits, nq));
+  CUDA_TRY(r.sc.alloc(&d_ns, 1));
+  CUDA_TRY(r.sc.alloc(&d_err, 1));
+  CUDA_TRY(r.sc.alloc(&d_dup, nq));
+  CUDA_TRY(r.sc.alloc(&d_b, buckets ? (size_t)n : 1));
+  PROPAGATE(quantiles_of_values(r, d_v, (int)n, probs.data(), nq, relative_error, d_q));
   fj_splits_kernel<<<1, 1024, 0, r.s>>>(d_q, nq, d_splits, d_ns, d_err, d_dup);
-  FJ_LAUNCHED();
+  LAUNCHED();
   if (buckets) {
     fj_bucket_kernel<<<grid_for(n, 256), 256, 0, r.s>>>(d_v, (int)n, d_splits, d_ns, d_b);
-    FJ_LAUNCHED();
+    LAUNCHED();
   }
   int ns = 0, err = 0;
   std::vector<double> h_splits(nq);
-  FJ_TRY(cudaMemcpyAsync(&ns, d_ns, sizeof(int), cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaMemcpyAsync(&err, d_err, sizeof(int), cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaMemcpyAsync(h_splits.data(), d_splits, sizeof(double) * nq, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaStreamSynchronize(r.s));
+  CUDA_TRY(cudaMemcpyAsync(&ns, d_ns, sizeof(int), cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaMemcpyAsync(&err, d_err, sizeof(int), cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaMemcpyAsync(h_splits.data(), d_splits, sizeof(double) * nq, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaStreamSynchronize(r.s));
   if (err)
-    return fj_fail(SRS_ERR_INVALID, "the %d distinct splits are not >= 3 strictly increasing values (Bucketizer)", ns);
+    return failf(SRS_ERR_INVALID, "the %d distinct splits are not >= 3 strictly increasing values (Bucketizer)", ns);
   if (buckets) {
-    FJ_TRY(cudaMemcpyAsync(buckets, d_b, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, r.s));
-    FJ_TRY(cudaStreamSynchronize(r.s));
+    CUDA_TRY(cudaMemcpyAsync(buckets, d_b, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, r.s));
+    CUDA_TRY(cudaStreamSynchronize(r.s));
   }
   std::copy(h_splits.begin(), h_splits.begin() + ns, splits);
   *n_splits = ns;
@@ -722,68 +640,62 @@ extern "C" int srs_quantile_discretizer_host(const double* values, int64_t n, in
 
 extern "C" int srs_bucketize_host(const double* splits, int32_t n_splits, const double* values, int64_t n,
                                   int32_t device, int32_t* buckets) {
-  FJ_OK(check_splits(splits, n_splits));
-  FJ_OK(check_values(values, n, "bucketize"));
-  if (!buckets) return fj_fail(SRS_ERR_INVALID, "null output");
+  PROPAGATE(check_splits(splits, n_splits));
+  PROPAGATE(check_values(values, n, "bucketize"));
+  if (!buckets) return failf(SRS_ERR_INVALID, "null output");
   const uint64_t lo = order_key(splits[0]), hi = order_key(splits[n_splits - 1]);
   for (int64_t i = 0; i < n; ++i) {
     const uint64_t k = order_key(values[i]);
     if (values[i] != splits[n_splits - 1] && (k < lo || k > hi))
-      return fj_fail(SRS_ERR_INVALID, "value %lld (%g) outside the splits [%g, %g]", (long long)i, values[i], splits[0],
+      return failf(SRS_ERR_INVALID, "value %lld (%g) outside the splits [%g, %g]", (long long)i, values[i], splits[0],
                      splits[n_splits - 1]);
   }
-  Run r;
-  FJ_OK(begin(r, device));
+  HostCall r;
+  PROPAGATE(r.begin(device));
   double *d_v, *d_s;
   int* d_ns;
   int32_t* d_b;
-  FJ_OK(upload(r, &d_v, values, (size_t)n));
-  FJ_OK(upload(r, &d_s, splits, (size_t)n_splits));
-  FJ_OK(upload(r, &d_ns, &n_splits, 1));
-  FJ_TRY(r.sc.alloc(&d_b, n));
+  PROPAGATE(r.upload(&d_v, values, (size_t)n));
+  PROPAGATE(r.upload(&d_s, splits, (size_t)n_splits));
+  PROPAGATE(r.upload(&d_ns, &n_splits, 1));
+  CUDA_TRY(r.sc.alloc(&d_b, n));
   fj_bucket_kernel<<<grid_for(n, 256), 256, 0, r.s>>>(d_v, (int)n, d_s, d_ns, d_b);
-  FJ_LAUNCHED();
-  FJ_TRY(cudaMemcpyAsync(buckets, d_b, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaStreamSynchronize(r.s));
+  LAUNCHED();
+  CUDA_TRY(cudaMemcpyAsync(buckets, d_b, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaStreamSynchronize(r.s));
   return SRS_OK;
 }
 
 extern "C" int srs_minmax_scale_host(const double* values, int64_t n, const double* fit_min_max, int32_t device,
                                      double* out, double* min_max) {
-  FJ_OK(check_values(values, n, "minmax_scale"));
-  if (!out) return fj_fail(SRS_ERR_INVALID, "null output");
+  PROPAGATE(check_values(values, n, "minmax_scale"));
+  if (!out) return failf(SRS_ERR_INVALID, "null output");
   if (fit_min_max && (std::isnan(fit_min_max[0]) || std::isnan(fit_min_max[1])))
-    return fj_fail(SRS_ERR_INVALID, "fitted min / max is NaN");
-  Run r;
-  FJ_OK(begin(r, device));
+    return failf(SRS_ERR_INVALID, "fitted min / max is NaN");
+  HostCall r;
+  PROPAGATE(r.begin(device));
   double *d_v, *d_out;
   uint64_t *d_keys, *d_kmm;
-  FJ_OK(upload(r, &d_v, values, (size_t)n));
-  FJ_TRY(r.sc.alloc(&d_out, n));
-  FJ_TRY(r.sc.alloc(&d_kmm, 2));
+  PROPAGATE(r.upload(&d_v, values, (size_t)n));
+  CUDA_TRY(r.sc.alloc(&d_out, n));
+  CUDA_TRY(r.sc.alloc(&d_kmm, 2));
   if (fit_min_max) {
     const uint64_t k[2] = {order_key(fit_min_max[0]), order_key(fit_min_max[1])};
-    FJ_TRY(cudaMemcpyAsync(d_kmm, k, sizeof(k), cudaMemcpyHostToDevice, r.s));
-    FJ_TRY(cudaStreamSynchronize(r.s));         // k lives on this stack frame
+    CUDA_TRY(cudaMemcpyAsync(d_kmm, k, sizeof(k), cudaMemcpyHostToDevice, r.s));
+    CUDA_TRY(cudaStreamSynchronize(r.s));         // k lives on this stack frame
   } else {
-    FJ_TRY(r.sc.alloc(&d_keys, n));
+    CUDA_TRY(r.sc.alloc(&d_keys, n));
     fj_keys_kernel<<<grid_for(n, 256), 256, 0, r.s>>>(d_v, (int)n, d_keys);
-    FJ_LAUNCHED();
-    size_t t1 = 0, t2 = 0;
-    FJ_TRY(cub::DeviceReduce::Min(nullptr, t1, d_keys, d_kmm, (int)n, r.s));
-    FJ_TRY(cub::DeviceReduce::Max(nullptr, t2, d_keys, d_kmm + 1, (int)n, r.s));
-    uint8_t* d_tmp;
-    t1 = std::max(t1, t2);
-    FJ_TRY(r.sc.alloc(&d_tmp, t1));
-    FJ_TRY(cub::DeviceReduce::Min(d_tmp, t1, d_keys, d_kmm, (int)n, r.s));
-    FJ_TRY(cub::DeviceReduce::Max(d_tmp, t1, d_keys, d_kmm + 1, (int)n, r.s));
+    LAUNCHED();
+    CUB_RUN(r, cub::DeviceReduce::Min(tmp__, tb__, d_keys, d_kmm, (int)n, r.s));
+    CUB_RUN(r, cub::DeviceReduce::Max(tmp__, tb__, d_keys, d_kmm + 1, (int)n, r.s));
   }
   fj_scale_kernel<<<grid_for(n, 256), 256, 0, r.s>>>(d_v, (int)n, d_kmm, d_kmm + 1, d_out);
-  FJ_LAUNCHED();
+  LAUNCHED();
   uint64_t kmm[2];
-  FJ_TRY(cudaMemcpyAsync(kmm, d_kmm, sizeof(kmm), cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaMemcpyAsync(out, d_out, sizeof(double) * n, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaStreamSynchronize(r.s));
+  CUDA_TRY(cudaMemcpyAsync(kmm, d_kmm, sizeof(kmm), cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaMemcpyAsync(out, d_out, sizeof(double) * n, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaStreamSynchronize(r.s));
   if (min_max) {
     min_max[0] = key_value(kmm[0]);
     min_max[1] = key_value(kmm[1]);
@@ -795,22 +707,22 @@ extern "C" int srs_rating_features_host(const int32_t* movie_id, const int8_t* h
                                         int32_t device, int32_t capacity, int32_t* movie_ids, int64_t* counts,
                                         double* avg, double* var, int32_t* n_movies) {
   if (n_ratings < 1 || n_ratings > kMaxRatings)
-    return fj_fail(SRS_ERR_INVALID, "n_ratings %lld outside 1..%lld", (long long)n_ratings, (long long)kMaxRatings);
-  if (!movie_id || !half) return fj_fail(SRS_ERR_INVALID, "null ratings");
+    return failf(SRS_ERR_INVALID, "n_ratings %lld outside 1..%lld", (long long)n_ratings, (long long)kMaxRatings);
+  if (!movie_id || !half) return failf(SRS_ERR_INVALID, "null ratings");
   if (!movie_ids || !counts || !avg || !var || !n_movies || capacity < 1)
-    return fj_fail(SRS_ERR_INVALID, "null output or capacity < 1");
+    return failf(SRS_ERR_INVALID, "null output or capacity < 1");
   int32_t top = 0;
   for (int64_t i = 0; i < n_ratings; ++i) {
     if (movie_id[i] < 0 || movie_id[i] > kMaxMovieId)
-      return fj_fail(SRS_ERR_INVALID, "rating %lld: movie id %d outside 0..%d", (long long)i, movie_id[i], kMaxMovieId);
+      return failf(SRS_ERR_INVALID, "rating %lld: movie id %d outside 0..%d", (long long)i, movie_id[i], kMaxMovieId);
     if (half[i] < 1 || half[i] > 10)
-      return fj_fail(SRS_ERR_INVALID, "rating %lld: %d half-stars is not a rating in [0.5, 5]", (long long)i,
+      return failf(SRS_ERR_INVALID, "rating %lld: %d half-stars is not a rating in [0.5, 5]", (long long)i,
                      (int)half[i]);
     top = std::max(top, movie_id[i]);
   }
   const int n = (int)n_ratings, slots = top + 1;
-  Run r;
-  FJ_OK(begin(r, device));
+  HostCall r;
+  PROPAGATE(r.begin(device));
   int32_t *d_movie, *d_iota, *d_slot, *d_ids;
   int8_t* d_half;
   unsigned long long* d_mmom;
@@ -818,54 +730,50 @@ extern "C" int srs_rating_features_host(const int32_t* movie_id, const int8_t* h
   int* d_count;
   int64_t* d_cnt;
   double *d_avg, *d_var;
-  FJ_OK(upload(r, &d_movie, movie_id, n));
-  FJ_OK(upload(r, &d_half, half, n));
-  FJ_TRY(r.sc.alloc(&d_iota, n));
-  FJ_TRY(r.sc.alloc(&d_mmom, 3 * (size_t)slots));
-  FJ_TRY(r.sc.alloc(&d_slot, slots));
-  FJ_TRY(r.sc.alloc(&d_flag, slots));
-  FJ_TRY(r.sc.alloc(&d_ids, slots));
-  FJ_TRY(r.sc.alloc(&d_count, 1));
-  FJ_TRY(r.sc.alloc(&d_cnt, slots));
-  FJ_TRY(r.sc.alloc(&d_avg, slots));
-  FJ_TRY(r.sc.alloc(&d_var, slots));
-  FJ_TRY(cudaMemsetAsync(d_mmom, 0, sizeof(unsigned long long) * 3 * slots, r.s));
-  FJ_TRY(launch_movie_moments(d_movie, d_half, n, d_iota, d_mmom, r.s));
+  PROPAGATE(r.upload(&d_movie, movie_id, n));
+  PROPAGATE(r.upload(&d_half, half, n));
+  CUDA_TRY(r.sc.alloc(&d_iota, n));
+  CUDA_TRY(r.sc.alloc(&d_mmom, 3 * (size_t)slots));
+  CUDA_TRY(r.sc.alloc(&d_slot, slots));
+  CUDA_TRY(r.sc.alloc(&d_flag, slots));
+  CUDA_TRY(r.sc.alloc(&d_ids, slots));
+  CUDA_TRY(r.sc.alloc(&d_count, 1));
+  CUDA_TRY(r.sc.alloc(&d_cnt, slots));
+  CUDA_TRY(r.sc.alloc(&d_avg, slots));
+  CUDA_TRY(r.sc.alloc(&d_var, slots));
+  CUDA_TRY(cudaMemsetAsync(d_mmom, 0, sizeof(unsigned long long) * 3 * slots, r.s));
+  CUDA_TRY(launch_movie_moments(d_movie, d_half, n, d_iota, d_mmom, r.s));
   fj_rated_kernel<<<grid_for(slots, 256), 256, 0, r.s>>>(d_mmom, slots, d_slot, d_flag);
-  FJ_LAUNCHED();
-  size_t tmp_bytes = 0;
-  FJ_TRY(cub::DeviceSelect::Flagged(nullptr, tmp_bytes, d_slot, d_flag, d_ids, d_count, slots, r.s));
-  uint8_t* d_tmp;
-  FJ_TRY(r.sc.alloc(&d_tmp, tmp_bytes));
-  FJ_TRY(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_slot, d_flag, d_ids, d_count, slots, r.s));
+  LAUNCHED();
+  CUB_RUN(r, cub::DeviceSelect::Flagged(tmp__, tb__, d_slot, d_flag, d_ids, d_count, slots, r.s));
   fj_rating_kernel<<<grid_for(slots, 256), 256, 0, r.s>>>(d_mmom, d_ids, d_count, d_cnt, d_avg, d_var);
-  FJ_LAUNCHED();
+  LAUNCHED();
   int m = 0;
-  FJ_TRY(cudaMemcpyAsync(&m, d_count, sizeof(int), cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaStreamSynchronize(r.s));
-  if (m > capacity) return fj_fail(SRS_ERR_RANGE, "%d rated movies exceed the capacity %d", m, capacity);
-  FJ_TRY(cudaMemcpyAsync(movie_ids, d_ids, sizeof(int32_t) * m, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaMemcpyAsync(counts, d_cnt, sizeof(int64_t) * m, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaMemcpyAsync(avg, d_avg, sizeof(double) * m, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaMemcpyAsync(var, d_var, sizeof(double) * m, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaStreamSynchronize(r.s));
+  CUDA_TRY(cudaMemcpyAsync(&m, d_count, sizeof(int), cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaStreamSynchronize(r.s));
+  if (m > capacity) return failf(SRS_ERR_RANGE, "%d rated movies exceed the capacity %d", m, capacity);
+  CUDA_TRY(cudaMemcpyAsync(movie_ids, d_ids, sizeof(int32_t) * m, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaMemcpyAsync(counts, d_cnt, sizeof(int64_t) * m, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaMemcpyAsync(avg, d_avg, sizeof(double) * m, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaMemcpyAsync(var, d_var, sizeof(double) * m, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaStreamSynchronize(r.s));
   *n_movies = m;
   return SRS_OK;
 }
 
 extern "C" int srs_string_indexer_host(const int32_t* tokens, int64_t n_tokens, const int32_t* word_hash,
                                        int32_t n_words, int32_t device, int32_t* label_words, int64_t* label_counts) {
-  FJ_OK(check_tokens(tokens, n_tokens, word_hash, n_words));
-  if (!label_words || !label_counts) return fj_fail(SRS_ERR_INVALID, "null output");
-  Run r;
-  FJ_OK(begin(r, device));
+  PROPAGATE(check_tokens(tokens, n_tokens, word_hash, n_words));
+  if (!label_words || !label_counts) return failf(SRS_ERR_INVALID, "null output");
+  HostCall r;
+  PROPAGATE(r.begin(device));
   int32_t *d_tok, *d_label_of, *d_label_word;
   int64_t* d_label_cnt;
-  FJ_OK(upload(r, &d_tok, tokens, (size_t)n_tokens));
-  FJ_OK(index_labels(r, d_tok, (int)n_tokens, word_hash, n_words, &d_label_of, &d_label_word, &d_label_cnt));
-  FJ_TRY(cudaMemcpyAsync(label_words, d_label_word, sizeof(int32_t) * n_words, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaMemcpyAsync(label_counts, d_label_cnt, sizeof(int64_t) * n_words, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaStreamSynchronize(r.s));
+  PROPAGATE(r.upload(&d_tok, tokens, (size_t)n_tokens));
+  PROPAGATE(index_labels(r, d_tok, (int)n_tokens, word_hash, n_words, &d_label_of, &d_label_word, &d_label_cnt));
+  CUDA_TRY(cudaMemcpyAsync(label_words, d_label_word, sizeof(int32_t) * n_words, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaMemcpyAsync(label_counts, d_label_cnt, sizeof(int64_t) * n_words, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaStreamSynchronize(r.s));
   return SRS_OK;
 }
 
@@ -874,108 +782,102 @@ extern "C" int srs_genre_multihot_host(const int32_t* movie_id, const int32_t* o
                                        int32_t* label_words, int64_t* label_counts, int32_t* out_movie_ids,
                                        int32_t* out_offsets, int32_t* out_indices) {
   if (n_movies < 1 || n_movies > kMaxMovieId + 1)
-    return fj_fail(SRS_ERR_INVALID, "n_movies %d outside 1..%d", n_movies, kMaxMovieId + 1);
-  if (!movie_id || !offsets) return fj_fail(SRS_ERR_INVALID, "null movies");
+    return failf(SRS_ERR_INVALID, "n_movies %d outside 1..%d", n_movies, kMaxMovieId + 1);
+  if (!movie_id || !offsets) return failf(SRS_ERR_INVALID, "null movies");
   if (!label_words || !label_counts || !out_movie_ids || !out_offsets || !out_indices)
-    return fj_fail(SRS_ERR_INVALID, "null output");
-  if (offsets[0] != 0) return fj_fail(SRS_ERR_INVALID, "offsets[0] must be 0");
+    return failf(SRS_ERR_INVALID, "null output");
+  if (offsets[0] != 0) return failf(SRS_ERR_INVALID, "offsets[0] must be 0");
   std::vector<uint8_t> id_seen((size_t)kMaxMovieId + 1, 0);
   for (int r = 0; r < n_movies; ++r) {
     const int len = offsets[r + 1] - offsets[r];
     if (len < 1 || len > kMaxWordsPerRow)
-      return fj_fail(SRS_ERR_INVALID, "movie row %d: %d words, need 1..%d", r, len, kMaxWordsPerRow);
+      return failf(SRS_ERR_INVALID, "movie row %d: %d words, need 1..%d", r, len, kMaxWordsPerRow);
     if (movie_id[r] < 0 || movie_id[r] > kMaxMovieId)
-      return fj_fail(SRS_ERR_INVALID, "movie row %d: id %d outside 0..%d", r, movie_id[r], kMaxMovieId);
-    if (id_seen[movie_id[r]]++) return fj_fail(SRS_ERR_INVALID, "movie %d listed twice", movie_id[r]);
+      return failf(SRS_ERR_INVALID, "movie row %d: id %d outside 0..%d", r, movie_id[r], kMaxMovieId);
+    if (id_seen[movie_id[r]]++) return failf(SRS_ERR_INVALID, "movie %d listed twice", movie_id[r]);
   }
   const int64_t nnz = offsets[n_movies];
-  FJ_OK(check_tokens(words, nnz, word_hash, n_words));
+  PROPAGATE(check_tokens(words, nnz, word_hash, n_words));
   for (int r = 0; r < n_movies; ++r)
     for (int a = offsets[r]; a < offsets[r + 1]; ++a)
       for (int b = offsets[r]; b < a; ++b)
-        if (words[a] == words[b]) return fj_fail(SRS_ERR_INVALID, "movie %d lists a genre twice", movie_id[r]);
-  Run r;
-  FJ_OK(begin(r, device));
+        if (words[a] == words[b]) return failf(SRS_ERR_INVALID, "movie %d lists a genre twice", movie_id[r]);
+  HostCall r;
+  PROPAGATE(r.begin(device));
   const int n = n_movies;
   int32_t *d_tok, *d_label_of, *d_label_word, *d_movie, *d_off, *d_iota, *d_order, *d_len, *d_ooff, *d_oidx;
   uint32_t *d_key, *d_key2;
   int64_t* d_label_cnt;
-  FJ_OK(upload(r, &d_tok, words, (size_t)nnz));
-  FJ_OK(upload(r, &d_movie, movie_id, n));
-  FJ_OK(upload(r, &d_off, offsets, (size_t)n + 1));
-  FJ_TRY(r.sc.alloc(&d_iota, n));
-  FJ_TRY(r.sc.alloc(&d_order, n));
-  FJ_TRY(r.sc.alloc(&d_key, n));
-  FJ_TRY(r.sc.alloc(&d_key2, n));
-  FJ_TRY(r.sc.alloc(&d_len, n));
-  FJ_TRY(r.sc.alloc(&d_ooff, (size_t)n + 1));
-  FJ_TRY(r.sc.alloc(&d_oidx, (size_t)nnz));
-  FJ_OK(index_labels(r, d_tok, (int)nnz, word_hash, n_words, &d_label_of, &d_label_word, &d_label_cnt));
+  PROPAGATE(r.upload(&d_tok, words, (size_t)nnz));
+  PROPAGATE(r.upload(&d_movie, movie_id, n));
+  PROPAGATE(r.upload(&d_off, offsets, (size_t)n + 1));
+  CUDA_TRY(r.sc.alloc(&d_iota, n));
+  CUDA_TRY(r.sc.alloc(&d_order, n));
+  CUDA_TRY(r.sc.alloc(&d_key, n));
+  CUDA_TRY(r.sc.alloc(&d_key2, n));
+  CUDA_TRY(r.sc.alloc(&d_len, n));
+  CUDA_TRY(r.sc.alloc(&d_ooff, (size_t)n + 1));
+  CUDA_TRY(r.sc.alloc(&d_oidx, (size_t)nnz));
+  PROPAGATE(index_labels(r, d_tok, (int)nnz, word_hash, n_words, &d_label_of, &d_label_word, &d_label_cnt));
   fj_row_iota_kernel<<<grid_for(n, 256), 256, 0, r.s>>>(d_movie, n, d_key, d_iota);
-  FJ_LAUNCHED();
-  size_t t1 = 0, t2 = 0;
-  FJ_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t1, d_key, d_key2, d_iota, d_order, n, 0, 24, r.s));
-  FJ_TRY(cub::DeviceScan::InclusiveSum(nullptr, t2, d_len, d_ooff + 1, n, r.s));
-  uint8_t* d_tmp;
-  t1 = std::max(t1, t2);
-  FJ_TRY(r.sc.alloc(&d_tmp, t1));
-  FJ_TRY(cub::DeviceRadixSort::SortPairs(d_tmp, t1, d_key, d_key2, d_iota, d_order, n, 0, 24, r.s));
+  LAUNCHED();
+  CUB_RUN(r, cub::DeviceRadixSort::SortPairs(tmp__, tb__, d_key, d_key2, d_iota, d_order, n, 0, 24, r.s));
   fj_row_len_kernel<<<grid_for(n, 256), 256, 0, r.s>>>(d_order, d_off, n, d_len);
-  FJ_LAUNCHED();
-  FJ_TRY(cudaMemsetAsync(d_ooff, 0, sizeof(int32_t), r.s));
-  FJ_TRY(cub::DeviceScan::InclusiveSum(d_tmp, t1, d_len, d_ooff + 1, n, r.s));
+  LAUNCHED();
+  CUDA_TRY(cudaMemsetAsync(d_ooff, 0, sizeof(int32_t), r.s));
+  CUB_RUN(r, cub::DeviceScan::InclusiveSum(tmp__, tb__, d_len, d_ooff + 1, n, r.s));
   fj_csr_kernel<<<grid_for(n, 128), 128, 0, r.s>>>(d_order, d_off, d_tok, d_label_of, n, d_ooff, d_oidx);
-  FJ_LAUNCHED();
-  FJ_TRY(cudaMemcpyAsync(label_words, d_label_word, sizeof(int32_t) * n_words, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaMemcpyAsync(label_counts, d_label_cnt, sizeof(int64_t) * n_words, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaMemcpyAsync(out_movie_ids, d_key2, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaMemcpyAsync(out_offsets, d_ooff, sizeof(int32_t) * ((size_t)n + 1), cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaMemcpyAsync(out_indices, d_oidx, sizeof(int32_t) * nnz, cudaMemcpyDeviceToHost, r.s));
-  FJ_TRY(cudaStreamSynchronize(r.s));
+  LAUNCHED();
+  CUDA_TRY(cudaMemcpyAsync(label_words, d_label_word, sizeof(int32_t) * n_words, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaMemcpyAsync(label_counts, d_label_cnt, sizeof(int64_t) * n_words, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaMemcpyAsync(out_movie_ids, d_key2, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaMemcpyAsync(out_offsets, d_ooff, sizeof(int32_t) * ((size_t)n + 1), cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaMemcpyAsync(out_indices, d_oidx, sizeof(int32_t) * nnz, cudaMemcpyDeviceToHost, r.s));
+  CUDA_TRY(cudaStreamSynchronize(r.s));
   return SRS_OK;
 }
 
 extern "C" int srs_sample_split_host(int64_t n, uint64_t seed, double fraction, const double* weights,
                                      int32_t n_parts, int32_t device, int32_t* rows, int64_t* part_counts) {
-  if (n < 1 || n > kMaxValues) return fj_fail(SRS_ERR_INVALID, "n %lld outside 1..%lld", (long long)n,
+  if (n < 1 || n > kMaxValues) return failf(SRS_ERR_INVALID, "n %lld outside 1..%lld", (long long)n,
                                               (long long)kMaxValues);
-  if (!(fraction >= 0.0 && fraction <= 1.0)) return fj_fail(SRS_ERR_INVALID, "fraction %g outside [0, 1]", fraction);
+  if (!(fraction >= 0.0 && fraction <= 1.0)) return failf(SRS_ERR_INVALID, "fraction %g outside [0, 1]", fraction);
   if (n_parts < 1 || n_parts > kMaxParts || !weights)
-    return fj_fail(SRS_ERR_INVALID, "need 1..%d weights", kMaxParts);
-  if (!rows || !part_counts) return fj_fail(SRS_ERR_INVALID, "null output");
+    return failf(SRS_ERR_INVALID, "need 1..%d weights", kMaxParts);
+  if (!rows || !part_counts) return failf(SRS_ERR_INVALID, "null output");
   double total = 0.0;
   for (int j = 0; j < n_parts; ++j) {
     if (!std::isfinite(weights[j]) || weights[j] < 0)
-      return fj_fail(SRS_ERR_INVALID, "weight %d (%g) is not finite and >= 0", j, weights[j]);
+      return failf(SRS_ERR_INVALID, "weight %d (%g) is not finite and >= 0", j, weights[j]);
     total += weights[j];
   }
-  if (!(total > 0.0)) return fj_fail(SRS_ERR_INVALID, "the weights sum to 0");
+  if (!(total > 0.0)) return failf(SRS_ERR_INVALID, "the weights sum to 0");
   Bounds b{};
   for (int j = 0; j < n_parts; ++j) b.b[j + 1] = b.b[j] + weights[j] / total;
-  Run r;
-  FJ_OK(begin(r, device));
+  HostCall r;
+  PROPAGATE(r.begin(device));
   int8_t* d_part;
-  FJ_TRY(r.sc.alloc(&d_part, n));
+  CUDA_TRY(r.sc.alloc(&d_part, n));
   fj_part_kernel<<<grid_for(n, 256), 256, 0, r.s>>>((int)n, stream_key(seed, 0), stream_key(seed, 1), fraction, b,
                                                     n_parts, d_part);
-  FJ_LAUNCHED();
+  LAUNCHED();
   return gather_parts(r, d_part, (int)n, n_parts, rows, part_counts);
 }
 
 extern "C" int srs_sample_split_by_timestamp_host(const int64_t* timestamp, int64_t n, uint64_t seed, double fraction,
                                                   double relative_error, int32_t device, int32_t* rows,
                                                   int64_t* part_counts, double* split_timestamp) {
-  if (n < 1 || n > kMaxValues) return fj_fail(SRS_ERR_INVALID, "n %lld outside 1..%lld", (long long)n,
+  if (n < 1 || n > kMaxValues) return failf(SRS_ERR_INVALID, "n %lld outside 1..%lld", (long long)n,
                                               (long long)kMaxValues);
-  if (!timestamp) return fj_fail(SRS_ERR_INVALID, "null timestamps");
-  if (!(fraction >= 0.0 && fraction <= 1.0)) return fj_fail(SRS_ERR_INVALID, "fraction %g outside [0, 1]", fraction);
-  FJ_OK(check_eps(relative_error));
-  if (!rows || !part_counts || !split_timestamp) return fj_fail(SRS_ERR_INVALID, "null output");
+  if (!timestamp) return failf(SRS_ERR_INVALID, "null timestamps");
+  if (!(fraction >= 0.0 && fraction <= 1.0)) return failf(SRS_ERR_INVALID, "fraction %g outside [0, 1]", fraction);
+  PROPAGATE(check_eps(relative_error));
+  if (!rows || !part_counts || !split_timestamp) return failf(SRS_ERR_INVALID, "null output");
   for (int64_t i = 0; i < n; ++i)
     if (timestamp[i] < -(1ll << 53) || timestamp[i] > (1ll << 53))
-      return fj_fail(SRS_ERR_INVALID, "timestamp %lld is not exact as a double", (long long)timestamp[i]);
-  Run r;
-  FJ_OK(begin(r, device));
+      return failf(SRS_ERR_INVALID, "timestamp %lld is not exact as a double", (long long)timestamp[i]);
+  HostCall r;
+  PROPAGATE(r.begin(device));
   const int nn = (int)n;
   int64_t* d_ts;
   uint64_t* d_keys;
@@ -984,24 +886,24 @@ extern "C" int srs_sample_split_by_timestamp_host(const int64_t* timestamp, int6
   int8_t* d_part;
   double *d_prob, *d_split;
   const double p08 = 0.8;
-  FJ_OK(upload(r, &d_ts, timestamp, (size_t)n));
-  FJ_TRY(r.sc.alloc(&d_keys, n));
-  FJ_TRY(r.sc.alloc(&d_flag, n));
-  FJ_TRY(r.sc.alloc(&d_count, 1));
-  FJ_TRY(r.sc.alloc(&d_part, n));
-  FJ_OK(upload(r, &d_prob, &p08, 1));
-  FJ_TRY(r.sc.alloc(&d_split, 1));
-  FJ_TRY(cudaMemsetAsync(d_count, 0, sizeof(int), r.s));
+  PROPAGATE(r.upload(&d_ts, timestamp, (size_t)n));
+  CUDA_TRY(r.sc.alloc(&d_keys, n));
+  CUDA_TRY(r.sc.alloc(&d_flag, n));
+  CUDA_TRY(r.sc.alloc(&d_count, 1));
+  CUDA_TRY(r.sc.alloc(&d_part, n));
+  PROPAGATE(r.upload(&d_prob, &p08, 1));
+  CUDA_TRY(r.sc.alloc(&d_split, 1));
+  CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int), r.s));
   fj_ts_keys_kernel<<<grid_for(n, 256), 256, 0, r.s>>>(d_ts, nn, stream_key(seed, 0), fraction, d_keys, d_flag);
-  FJ_LAUNCHED();
+  LAUNCHED();
   fj_flag_count_kernel<<<grid_for(n, 256), 256, 0, r.s>>>(d_flag, nn, d_count);
-  FJ_LAUNCHED();
-  FJ_OK(quantiles_of_keys(r, d_keys, nn, d_count, d_prob, 1, relative_error, d_split));
+  LAUNCHED();
+  PROPAGATE(quantiles_of_keys(r, d_keys, nn, d_count, d_prob, 1, relative_error, d_split));
   fj_ts_part_kernel<<<grid_for(n, 256), 256, 0, r.s>>>(d_ts, d_flag, nn, d_split, d_part);
-  FJ_LAUNCHED();
+  LAUNCHED();
   double split = 0.0;
-  FJ_TRY(cudaMemcpyAsync(&split, d_split, sizeof(double), cudaMemcpyDeviceToHost, r.s));
-  FJ_OK(gather_parts(r, d_part, nn, 2, rows, part_counts));
+  CUDA_TRY(cudaMemcpyAsync(&split, d_split, sizeof(double), cudaMemcpyDeviceToHost, r.s));
+  PROPAGATE(gather_parts(r, d_part, nn, 2, rows, part_counts));
   *split_timestamp = split;
   return SRS_OK;
 }

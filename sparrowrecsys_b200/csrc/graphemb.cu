@@ -17,13 +17,10 @@
 #include <cuda_runtime.h>
 #include <cub/cub.cuh>
 
-#include <algorithm>
-#include <cstdarg>
-#include <cstdio>
 #include <vector>
 
 #include "../../include/srs_ctr.h"
-#include "kernels.h"
+#include "hostcall.h"
 
 namespace srs {
 namespace {
@@ -31,48 +28,6 @@ namespace {
 constexpr int64_t kMaxWalkWords = 21000000;   // num_walks * walk_length: item2vec's bound on the corpus
 constexpr uint64_t kSentinel = 1ull << 48;
 constexpr uint32_t kIdMask = (1u << 24) - 1;
-
-int ge_fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  return set_last_error(code, buf);
-}
-
-#define GE_TRY(expr)                                                                                      \
-  do {                                                                                                    \
-    cudaError_t e__ = (expr);                                                                             \
-    if (e__ != cudaSuccess)                                                                               \
-      return ge_fail(SRS_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
-
-#define GE_LAUNCHED()                                                                                     \
-  do {                                                                                                    \
-    ++g_launch_count;                                                                                     \
-    GE_TRY(cudaGetLastError());                                                                           \
-  } while (0)
-
-// item2vec.cu's counter-based hash: splitmix64's finaliser of x + (i + 1) * golden
-__host__ __device__ __forceinline__ uint64_t splitmix(uint64_t x, uint64_t i) {
-  uint64_t z = x + (i + 1) * 0x9E3779B97F4A7C15ULL;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-  return z ^ (z >> 31);
-}
-
-int grid_for(int64_t n, int threads) {
-  int64_t b = (n + threads - 1) / threads;
-  return (int)(b < 1 ? 1 : b > 132 * 64 ? 132 * 64 : b);
-}
-
-struct StreamGuard {
-  cudaStream_t s = nullptr;
-  ~StreamGuard() {
-    if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
-  }
-};
 
 __global__ void ge_pair_kernel(const int32_t* __restrict__ movie, const uint32_t* __restrict__ user,
                                const int* __restrict__ n_pos, int n, uint64_t* __restrict__ key,
@@ -167,9 +122,9 @@ __device__ __forceinline__ int first_at_least(const double* __restrict__ a, int 
   return lo;
 }
 
-// u of walk w, step t: the top 53 bits of splitmix(splitmix(root, w), t) over 2^53, root = splitmix(~seed, 0)
+// u of walk w, step t, root = splitmix(~seed, 0)
 __device__ __forceinline__ double walk_uniform(uint64_t root, int w, int t) {
-  return (double)(splitmix(splitmix(root, (uint64_t)w), (uint64_t)t) >> 11) * 0x1p-53;
+  return uniform53(splitmix(root, (uint64_t)w), (uint64_t)t);
 }
 
 __global__ void ge_walk_kernel(Transitions t, uint64_t root, int W, int L, int32_t* __restrict__ walks,
@@ -206,63 +161,55 @@ __global__ void ge_flat_kernel(const int32_t* __restrict__ lengths, int64_t n, i
   }
 }
 
-int build_transitions(Scratch& sc, cudaStream_t s, const I2vCorpus& c, int n, int32_t n_slots, Transitions* t) {
+int build_transitions(HostCall& hc, const I2vCorpus& c, int n, int32_t n_slots, Transitions* t) {
+  Scratch& sc = hc.sc;
+  cudaStream_t s = hc.s;
   uint64_t *d_key, *d_skey, *d_ukey;
   int32_t *d_iota, *d_runs, *d_rstart;
   uint8_t* d_flag;
   int* d_nruns;
-  GE_TRY(sc.alloc(&d_key, n)); GE_TRY(sc.alloc(&d_skey, n)); GE_TRY(sc.alloc(&d_ukey, n));
-  GE_TRY(sc.alloc(&d_iota, n)); GE_TRY(sc.alloc(&d_runs, n)); GE_TRY(sc.alloc(&d_rstart, n));
-  GE_TRY(sc.alloc(&d_flag, n)); GE_TRY(sc.alloc(&d_nruns, 1));
-  GE_TRY(sc.alloc(&t->source, n)); GE_TRY(sc.alloc(&t->row_ptr, n + 1)); GE_TRY(sc.alloc(&t->out, n));
-  GE_TRY(sc.alloc(&t->dist, n)); GE_TRY(sc.alloc(&t->cdf, n)); GE_TRY(sc.alloc(&t->target, n));
-  GE_TRY(sc.alloc(&t->count, n)); GE_TRY(sc.alloc(&t->prob, n)); GE_TRY(sc.alloc(&t->cum, n));
-  GE_TRY(sc.alloc(&t->row_of, n_slots)); GE_TRY(sc.alloc(&t->n_rows, 2));
-  GE_TRY(cudaMemsetAsync(t->row_of, 0xff, sizeof(int32_t) * n_slots, s));
+  CUDA_TRY(sc.alloc(&d_key, n)); CUDA_TRY(sc.alloc(&d_skey, n)); CUDA_TRY(sc.alloc(&d_ukey, n));
+  CUDA_TRY(sc.alloc(&d_iota, n)); CUDA_TRY(sc.alloc(&d_runs, n)); CUDA_TRY(sc.alloc(&d_rstart, n));
+  CUDA_TRY(sc.alloc(&d_flag, n)); CUDA_TRY(sc.alloc(&d_nruns, 1));
+  CUDA_TRY(sc.alloc(&t->source, n)); CUDA_TRY(sc.alloc(&t->row_ptr, n + 1)); CUDA_TRY(sc.alloc(&t->out, n));
+  CUDA_TRY(sc.alloc(&t->dist, n)); CUDA_TRY(sc.alloc(&t->cdf, n)); CUDA_TRY(sc.alloc(&t->target, n));
+  CUDA_TRY(sc.alloc(&t->count, n)); CUDA_TRY(sc.alloc(&t->prob, n)); CUDA_TRY(sc.alloc(&t->cum, n));
+  CUDA_TRY(sc.alloc(&t->row_of, n_slots)); CUDA_TRY(sc.alloc(&t->n_rows, 2));
+  CUDA_TRY(cudaMemsetAsync(t->row_of, 0xff, sizeof(int32_t) * n_slots, s));
   const int T = 256;
   ge_pair_kernel<<<grid_for(n, T), T, 0, s>>>(c.movie, c.user, c.n, n, d_key, d_iota);
-  GE_LAUNCHED();
-  size_t b1 = 0, b2 = 0, b3 = 0;
-  GE_TRY(cub::DeviceRadixSort::SortKeys(nullptr, b1, d_key, d_skey, n, 0, 49, s));
-  GE_TRY(cub::DeviceRunLengthEncode::Encode(nullptr, b2, d_skey, d_ukey, d_runs, d_nruns, n, s));
-  GE_TRY(cub::DeviceSelect::Flagged(nullptr, b3, d_iota, d_flag, d_rstart, t->n_rows, n, s));
-  const size_t tmp_bytes = std::max(b1, std::max(b2, b3));
-  uint8_t* d_tmp;
-  GE_TRY(sc.alloc(&d_tmp, tmp_bytes));
-  GE_TRY(cub::DeviceRadixSort::SortKeys(d_tmp, b1, d_key, d_skey, n, 0, 49, s));
-  GE_TRY(cub::DeviceRunLengthEncode::Encode(d_tmp, b2, d_skey, d_ukey, d_runs, d_nruns, n, s));
+  LAUNCHED();
+  CUB_RUN(hc, cub::DeviceRadixSort::SortKeys(tmp__, tb__, d_key, d_skey, n, 0, 49, s));
+  CUB_RUN(hc, cub::DeviceRunLengthEncode::Encode(tmp__, tb__, d_skey, d_ukey, d_runs, d_nruns, n, s));
   ge_row_flag_kernel<<<grid_for(n, T), T, 0, s>>>(d_ukey, d_nruns, n, d_flag);
-  GE_LAUNCHED();
-  GE_TRY(cub::DeviceSelect::Flagged(d_tmp, b3, d_iota, d_flag, d_rstart, t->n_rows, n, s));
+  LAUNCHED();
+  CUB_RUN(hc, cub::DeviceSelect::Flagged(tmp__, tb__, d_iota, d_flag, d_rstart, t->n_rows, n, s));
   ge_row_kernel<<<grid_for(n, T), T, 0, s>>>(d_ukey, d_runs, d_nruns, d_rstart, *t);
-  GE_LAUNCHED();
+  LAUNCHED();
   ge_dist_kernel<<<1, 32, 0, s>>>(d_ukey, d_nruns, *t);
-  GE_LAUNCHED();
+  LAUNCHED();
   return SRS_OK;
 }
 
-// the ratings' checks, the device, the sentences and the transitions
-struct GraphCall {
-  Scratch sc;
-  StreamGuard sg;
+// a host call with the sentences and the transitions of its ratings
+struct GraphCall : HostCall {
   I2vCorpus corpus;
   Transitions t;
   int32_t n_slots = 0;
   int n = 0;
 };
 
-int begin(GraphCall& g, const int32_t* user_id, const int32_t* movie_id, const int8_t* half,
-          const int32_t* timestamp, int64_t n_ratings, int32_t device) {
-  if (int rc = i2v_select_device(device)) return rc;
-  GE_TRY(cudaStreamCreateWithFlags(&g.sg.s, cudaStreamNonBlocking));
+int begin_graph(GraphCall& g, const int32_t* user_id, const int32_t* movie_id, const int8_t* half,
+                const int32_t* timestamp, int64_t n_ratings, int32_t device) {
+  PROPAGATE(g.begin(device));
   g.n = (int)n_ratings;
-  if (int rc = i2v_positive_corpus(g.sc, g.sg.s, user_id, movie_id, half, timestamp, g.n, &g.corpus)) return rc;
-  return build_transitions(g.sc, g.sg.s, g.corpus, g.n, g.n_slots, &g.t);
+  PROPAGATE(i2v_positive_corpus(g, user_id, movie_id, half, timestamp, g.n, &g.corpus));
+  return build_transitions(g, g.corpus, g.n, g.n_slots, &g.t);
 }
 
 int check_walks(int32_t num_walks, int32_t walk_length) {
   if (num_walks < 1 || walk_length < 1 || (int64_t)num_walks * walk_length > kMaxWalkWords)
-    return ge_fail(SRS_ERR_INVALID, "%d walks of length %d: both must be >= 1 and their product <= %lld", num_walks,
+    return failf(SRS_ERR_INVALID, "%d walks of length %d: both must be >= 1 and their product <= %lld", num_walks,
                    walk_length, (long long)kMaxWalkWords);
   return SRS_OK;
 }
@@ -270,12 +217,12 @@ int check_walks(int32_t num_walks, int32_t walk_length) {
 int run_walks(GraphCall& g, int32_t num_walks, int32_t walk_length, uint64_t seed, int32_t** d_walks,
               int32_t** d_len) {
   const int64_t nw = (int64_t)num_walks * walk_length;
-  GE_TRY(g.sc.alloc(d_walks, nw));
-  GE_TRY(g.sc.alloc(d_len, num_walks));
+  CUDA_TRY(g.sc.alloc(d_walks, nw));
+  CUDA_TRY(g.sc.alloc(d_len, num_walks));
   const int T = 128;
-  ge_walk_kernel<<<grid_for(num_walks, T), T, 0, g.sg.s>>>(g.t, splitmix(~seed, 0), num_walks, walk_length,
+  ge_walk_kernel<<<grid_for(num_walks, T), T, 0, g.s>>>(g.t, splitmix(~seed, 0), num_walks, walk_length,
                                                            *d_walks, *d_len);
-  GE_LAUNCHED();
+  LAUNCHED();
   return SRS_OK;
 }
 
@@ -290,30 +237,30 @@ extern "C" int srs_item_transitions_host(const int32_t* user_id, const int32_t* 
                                          int32_t* row_offsets, int32_t* out_counts, double* source_probs,
                                          int32_t* targets, int32_t* counts, double* probs, int32_t* n_sources,
                                          int32_t* n_edges) {
-  if (!n_sources || !n_edges) return ge_fail(SRS_ERR_INVALID, "null n_sources or n_edges");
+  if (!n_sources || !n_edges) return failf(SRS_ERR_INVALID, "null n_sources or n_edges");
   *n_sources = *n_edges = 0;
   if (source_capacity < 0 || edge_capacity < 0 ||
       (source_capacity > 0 && (!sources || !row_offsets || !out_counts || !source_probs)) ||
       (edge_capacity > 0 && (!targets || !counts || !probs)))
-    return ge_fail(SRS_ERR_INVALID, "negative capacity or null outputs");
+    return failf(SRS_ERR_INVALID, "negative capacity or null outputs");
   GraphCall g;
-  if (int rc = i2v_check_ratings(user_id, movie_id, half, timestamp, n_ratings, &g.n_slots)) return rc;
-  if (int rc = begin(g, user_id, movie_id, half, timestamp, n_ratings, device)) return rc;
-  cudaStream_t s = g.sg.s;
+  PROPAGATE(i2v_check_ratings(user_id, movie_id, half, timestamp, n_ratings, &g.n_slots));
+  PROPAGATE(begin_graph(g, user_id, movie_id, half, timestamp, n_ratings, device));
+  cudaStream_t s = g.s;
   int se[2];
-  GE_TRY(cudaMemcpyAsync(se, g.t.n_rows, sizeof(se), cudaMemcpyDeviceToHost, s));
-  GE_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(se, g.t.n_rows, sizeof(se), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   if (se[0] > source_capacity || se[1] > edge_capacity)
-    return ge_fail(SRS_ERR_RANGE, "%d sources and %d pairs exceed the capacities %d and %d", se[0], se[1],
+    return failf(SRS_ERR_RANGE, "%d sources and %d pairs exceed the capacities %d and %d", se[0], se[1],
                    source_capacity, edge_capacity);
-  GE_TRY(cudaMemcpyAsync(sources, g.t.source, sizeof(int32_t) * se[0], cudaMemcpyDeviceToHost, s));
-  GE_TRY(cudaMemcpyAsync(row_offsets, g.t.row_ptr, sizeof(int32_t) * (se[0] + 1), cudaMemcpyDeviceToHost, s));
-  GE_TRY(cudaMemcpyAsync(out_counts, g.t.out, sizeof(int32_t) * se[0], cudaMemcpyDeviceToHost, s));
-  GE_TRY(cudaMemcpyAsync(source_probs, g.t.dist, sizeof(double) * se[0], cudaMemcpyDeviceToHost, s));
-  GE_TRY(cudaMemcpyAsync(targets, g.t.target, sizeof(int32_t) * se[1], cudaMemcpyDeviceToHost, s));
-  GE_TRY(cudaMemcpyAsync(counts, g.t.count, sizeof(int32_t) * se[1], cudaMemcpyDeviceToHost, s));
-  GE_TRY(cudaMemcpyAsync(probs, g.t.prob, sizeof(double) * se[1], cudaMemcpyDeviceToHost, s));
-  GE_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(sources, g.t.source, sizeof(int32_t) * se[0], cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(row_offsets, g.t.row_ptr, sizeof(int32_t) * (se[0] + 1), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(out_counts, g.t.out, sizeof(int32_t) * se[0], cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(source_probs, g.t.dist, sizeof(double) * se[0], cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(targets, g.t.target, sizeof(int32_t) * se[1], cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(counts, g.t.count, sizeof(int32_t) * se[1], cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(probs, g.t.prob, sizeof(double) * se[1], cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   *n_sources = se[0];
   *n_edges = se[1];
   return SRS_OK;
@@ -323,18 +270,18 @@ extern "C" int srs_random_walks_host(const int32_t* user_id, const int32_t* movi
                                      const int32_t* timestamp, int64_t n_ratings, int32_t num_walks,
                                      int32_t walk_length, uint64_t seed, int32_t device, int32_t* walks,
                                      int32_t* lengths) {
-  if (int rc = check_walks(num_walks, walk_length)) return rc;
-  if (!walks || !lengths) return ge_fail(SRS_ERR_INVALID, "null outputs");
+  PROPAGATE(check_walks(num_walks, walk_length));
+  if (!walks || !lengths) return failf(SRS_ERR_INVALID, "null outputs");
   GraphCall g;
-  if (int rc = i2v_check_ratings(user_id, movie_id, half, timestamp, n_ratings, &g.n_slots)) return rc;
-  if (int rc = begin(g, user_id, movie_id, half, timestamp, n_ratings, device)) return rc;
+  PROPAGATE(i2v_check_ratings(user_id, movie_id, half, timestamp, n_ratings, &g.n_slots));
+  PROPAGATE(begin_graph(g, user_id, movie_id, half, timestamp, n_ratings, device));
   int32_t *d_walks, *d_len;
-  if (int rc = run_walks(g, num_walks, walk_length, seed, &d_walks, &d_len)) return rc;
-  cudaStream_t s = g.sg.s;
-  GE_TRY(cudaMemcpyAsync(walks, d_walks, sizeof(int32_t) * num_walks * (int64_t)walk_length, cudaMemcpyDeviceToHost,
+  PROPAGATE(run_walks(g, num_walks, walk_length, seed, &d_walks, &d_len));
+  cudaStream_t s = g.s;
+  CUDA_TRY(cudaMemcpyAsync(walks, d_walks, sizeof(int32_t) * num_walks * (int64_t)walk_length, cudaMemcpyDeviceToHost,
                          s));
-  GE_TRY(cudaMemcpyAsync(lengths, d_len, sizeof(int32_t) * num_walks, cudaMemcpyDeviceToHost, s));
-  GE_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(lengths, d_len, sizeof(int32_t) * num_walks, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   return SRS_OK;
 }
 
@@ -343,33 +290,30 @@ extern "C" int srs_graph_embedding_host(const int32_t* user_id, const int32_t* m
                                         const srs_item2vec_params* params, int32_t num_walks, int32_t walk_length,
                                         int32_t device, int32_t capacity, int32_t* vocab_ids, float* vectors,
                                         int32_t* vocab_size) {
-  if (!vocab_size) return ge_fail(SRS_ERR_INVALID, "null vocab_size");
+  if (!vocab_size) return failf(SRS_ERR_INVALID, "null vocab_size");
   *vocab_size = 0;
-  if (int rc = i2v_check_params(params)) return rc;
-  if (int rc = check_walks(num_walks, walk_length)) return rc;
+  PROPAGATE(i2v_check_params(params));
+  PROPAGATE(check_walks(num_walks, walk_length));
   if (capacity < 0 || (capacity > 0 && (!vocab_ids || !vectors)))
-    return ge_fail(SRS_ERR_INVALID, "negative capacity or null outputs");
+    return failf(SRS_ERR_INVALID, "negative capacity or null outputs");
   GraphCall g;
-  if (int rc = i2v_check_ratings(user_id, movie_id, half, timestamp, n_ratings, &g.n_slots)) return rc;
-  if (int rc = begin(g, user_id, movie_id, half, timestamp, n_ratings, device)) return rc;
+  PROPAGATE(i2v_check_ratings(user_id, movie_id, half, timestamp, n_ratings, &g.n_slots));
+  PROPAGATE(begin_graph(g, user_id, movie_id, half, timestamp, n_ratings, device));
   int32_t *d_walks, *d_len;
-  if (int rc = run_walks(g, num_walks, walk_length, params->seed, &d_walks, &d_len)) return rc;
-  cudaStream_t s = g.sg.s;
+  PROPAGATE(run_walks(g, num_walks, walk_length, params->seed, &d_walks, &d_len));
+  cudaStream_t s = g.s;
   const int64_t nw = (int64_t)num_walks * walk_length;
-  uint8_t *d_flag, *d_tmp;
+  uint8_t* d_flag;
   uint32_t *d_key, *d_wkey;
   int32_t* d_words;
   int* d_n;
-  GE_TRY(g.sc.alloc(&d_flag, nw)); GE_TRY(g.sc.alloc(&d_key, nw)); GE_TRY(g.sc.alloc(&d_wkey, nw));
-  GE_TRY(g.sc.alloc(&d_words, nw)); GE_TRY(g.sc.alloc(&d_n, 1));
+  CUDA_TRY(g.sc.alloc(&d_flag, nw)); CUDA_TRY(g.sc.alloc(&d_key, nw)); CUDA_TRY(g.sc.alloc(&d_wkey, nw));
+  CUDA_TRY(g.sc.alloc(&d_words, nw)); CUDA_TRY(g.sc.alloc(&d_n, 1));
   const int T = 256;
   ge_flat_kernel<<<grid_for(nw, T), T, 0, s>>>(d_len, nw, walk_length, d_flag, d_key);
-  GE_LAUNCHED();
-  size_t tmp_bytes = 0;
-  GE_TRY(cub::DeviceSelect::Flagged(nullptr, tmp_bytes, d_walks, d_flag, d_words, d_n, (int)nw, s));
-  GE_TRY(g.sc.alloc(&d_tmp, tmp_bytes));
-  GE_TRY(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_walks, d_flag, d_words, d_n, (int)nw, s));
-  GE_TRY(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_key, d_flag, d_wkey, d_n, (int)nw, s));
-  return word2vec_fit(g.sc, s, d_words, d_wkey, d_n, (int)nw, g.n_slots, *params, "occurrences in the walks",
+  LAUNCHED();
+  CUB_RUN(g, cub::DeviceSelect::Flagged(tmp__, tb__, d_walks, d_flag, d_words, d_n, (int)nw, s));
+  CUB_RUN(g, cub::DeviceSelect::Flagged(tmp__, tb__, d_key, d_flag, d_wkey, d_n, (int)nw, s));
+  return word2vec_fit(g, d_words, d_wkey, d_n, (int)nw, g.n_slots, *params, "occurrences in the walks",
                       capacity, vocab_ids, vectors, vocab_size);
 }

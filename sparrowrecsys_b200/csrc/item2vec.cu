@@ -26,12 +26,10 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
 #include <vector>
 
 #include "../../include/srs_ctr.h"
-#include "kernels.h"
+#include "hostcall.h"
 
 namespace srs {
 namespace {
@@ -49,41 +47,6 @@ constexpr int kMaxWindow = 1 << 16;
 constexpr int kMaxIterations = 100000;
 constexpr int kMaxPartitions = 1 << 16;
 constexpr unsigned kFull = 0xffffffffu;
-
-int i2v_fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  return set_last_error(code, buf);
-}
-
-#define I2V_TRY(expr)                                                                                     \
-  do {                                                                                                    \
-    cudaError_t e__ = (expr);                                                                             \
-    if (e__ != cudaSuccess)                                                                               \
-      return i2v_fail(SRS_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
-
-#define I2V_LAUNCHED()                                                                                    \
-  do {                                                                                                    \
-    ++g_launch_count;                                                                                     \
-    I2V_TRY(cudaGetLastError());                                                                          \
-  } while (0)
-
-// srs_fill_uniform's hash: splitmix64's finaliser of x + (i + 1) * golden
-__host__ __device__ __forceinline__ uint64_t splitmix(uint64_t x, uint64_t i) {
-  uint64_t z = x + (i + 1) * 0x9E3779B97F4A7C15ULL;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-  return z ^ (z >> 31);
-}
-
-int grid_for(int64_t n, int threads) {
-  int64_t b = (n + threads - 1) / threads;
-  return (int)(b < 1 ? 1 : b > 132 * 64 ? 132 * 64 : b);
-}
 
 struct MaxOp {
   __device__ __forceinline__ int32_t operator()(int32_t a, int32_t b) const { return a > b ? a : b; }
@@ -339,120 +302,95 @@ int huffman(const std::vector<int64_t>& cn, std::vector<uint32_t>& code_bits, st
 
 int check_ratings(const int32_t* user_id, const int32_t* movie_id, int64_t n_ratings, int32_t* n_slots) {
   if (n_ratings < 0 || n_ratings > kMaxRatings)
-    return i2v_fail(SRS_ERR_INVALID, "n_ratings %lld outside 0..%lld", (long long)n_ratings, (long long)kMaxRatings);
-  if (n_ratings && (!user_id || !movie_id)) return i2v_fail(SRS_ERR_INVALID, "null ratings");
+    return failf(SRS_ERR_INVALID, "n_ratings %lld outside 0..%lld", (long long)n_ratings, (long long)kMaxRatings);
+  if (n_ratings && (!user_id || !movie_id)) return failf(SRS_ERR_INVALID, "null ratings");
   int32_t mx = -1;
   for (int64_t i = 0; i < n_ratings; ++i) {
     if (user_id[i] < 0 || movie_id[i] < 0)
-      return i2v_fail(SRS_ERR_INVALID, "rating %lld: negative id (user %d, movie %d)", (long long)i, user_id[i],
+      return failf(SRS_ERR_INVALID, "rating %lld: negative id (user %d, movie %d)", (long long)i, user_id[i],
                       movie_id[i]);
     if (movie_id[i] >= kMaxMovieSlots)
-      return i2v_fail(SRS_ERR_INVALID, "rating %lld: movie id %d is not below 2^24", (long long)i, movie_id[i]);
+      return failf(SRS_ERR_INVALID, "rating %lld: movie id %d is not below 2^24", (long long)i, movie_id[i]);
     mx = std::max(mx, movie_id[i]);
   }
   *n_slots = mx + 1;
   return SRS_OK;
 }
 
-int select_device(int32_t device) {
-  int ndev = 0;
-  cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev == 0)
-    return i2v_fail(SRS_ERR_CUDA, "no CUDA device available (%s); this library has no CPU path", cudaGetErrorString(ce));
-  if (device < 0 || device >= ndev) return i2v_fail(SRS_ERR_INVALID, "device %d out of range", device);
-  I2V_TRY(cudaSetDevice(device));
-  return SRS_OK;
-}
-
-struct StreamGuard {
-  cudaStream_t s = nullptr;
-  ~StreamGuard() {
-    if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
-  }
-};
-
 }  // namespace
 
 int i2v_check_params(const srs_item2vec_params* params) {
-  if (!params) return i2v_fail(SRS_ERR_INVALID, "null params");
+  if (!params) return failf(SRS_ERR_INVALID, "null params");
   const srs_item2vec_params& hp = *params;
   if (hp.vector_size < 1 || hp.vector_size > kMaxDim)
-    return i2v_fail(SRS_ERR_INVALID, "vector_size %d outside 1..%d", hp.vector_size, kMaxDim);
+    return failf(SRS_ERR_INVALID, "vector_size %d outside 1..%d", hp.vector_size, kMaxDim);
   if (hp.window < 1 || hp.window > kMaxWindow)
-    return i2v_fail(SRS_ERR_INVALID, "window %d outside 1..%d", hp.window, kMaxWindow);
+    return failf(SRS_ERR_INVALID, "window %d outside 1..%d", hp.window, kMaxWindow);
   if (hp.iterations < 1 || hp.iterations > kMaxIterations)
-    return i2v_fail(SRS_ERR_INVALID, "iterations %d outside 1..%d", hp.iterations, kMaxIterations);
+    return failf(SRS_ERR_INVALID, "iterations %d outside 1..%d", hp.iterations, kMaxIterations);
   if (hp.partitions < 1 || hp.partitions > kMaxPartitions)
-    return i2v_fail(SRS_ERR_INVALID, "partitions %d outside 1..%d", hp.partitions, kMaxPartitions);
+    return failf(SRS_ERR_INVALID, "partitions %d outside 1..%d", hp.partitions, kMaxPartitions);
   return SRS_OK;
 }
 
 int i2v_check_ratings(const int32_t* user_id, const int32_t* movie_id, const int8_t* half, const int32_t* timestamp,
                       int64_t n_ratings, int32_t* n_slots) {
-  if (int rc = check_ratings(user_id, movie_id, n_ratings, n_slots)) return rc;
-  if (n_ratings && (!half || !timestamp)) return i2v_fail(SRS_ERR_INVALID, "null ratings");
+  PROPAGATE(check_ratings(user_id, movie_id, n_ratings, n_slots));
+  if (n_ratings && (!half || !timestamp)) return failf(SRS_ERR_INVALID, "null ratings");
   const int n = (int)n_ratings;
   for (int i = 0; i < n; ++i) {
     if (half[i] < 1 || half[i] > 10)
-      return i2v_fail(SRS_ERR_INVALID, "rating %d: %d half-stars is not a rating in [0.5, 5]", i, (int)half[i]);
-    if (timestamp[i] <= 0) return i2v_fail(SRS_ERR_INVALID, "rating %d: timestamp %d is not positive", i, timestamp[i]);
+      return failf(SRS_ERR_INVALID, "rating %d: %d half-stars is not a rating in [0.5, 5]", i, (int)half[i]);
+    if (timestamp[i] <= 0) return failf(SRS_ERR_INVALID, "rating %d: timestamp %d is not positive", i, timestamp[i]);
   }
-  if (n == 0) return i2v_fail(SRS_ERR_INVALID, "no ratings: the vocabulary would be empty");
+  if (n == 0) return failf(SRS_ERR_INVALID, "no ratings: the vocabulary would be empty");
   return SRS_OK;
 }
 
-int i2v_select_device(int32_t device) { return select_device(device); }
-
-int i2v_positive_corpus(Scratch& sc, cudaStream_t s, const int32_t* user_id, const int32_t* movie_id,
-                        const int8_t* half, const int32_t* timestamp, int n, I2vCorpus* out) {
+int i2v_positive_corpus(HostCall& c, const int32_t* user_id, const int32_t* movie_id, const int8_t* half,
+                        const int32_t* timestamp, int n, I2vCorpus* out) {
+  Scratch& sc = c.sc;
+  cudaStream_t s = c.s;
   int32_t *d_user, *d_movie, *d_ts, *d_order, *d_iota, *d_sel;
   uint32_t* d_suser;
   int8_t* d_half;
   uint8_t* d_flag;
-  I2V_TRY(sc.alloc(&d_user, n)); I2V_TRY(sc.alloc(&d_movie, n)); I2V_TRY(sc.alloc(&d_ts, n));
-  I2V_TRY(sc.alloc(&d_half, n)); I2V_TRY(sc.alloc(&d_order, n)); I2V_TRY(sc.alloc(&d_suser, n));
-  I2V_TRY(sc.alloc(&d_iota, n)); I2V_TRY(sc.alloc(&d_sel, n)); I2V_TRY(sc.alloc(&d_flag, n));
-  I2V_TRY(sc.alloc(&out->movie, n)); I2V_TRY(sc.alloc(&out->user, n)); I2V_TRY(sc.alloc(&out->n, 1));
-  I2V_TRY(cudaMemcpyAsync(d_user, user_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-  I2V_TRY(cudaMemcpyAsync(d_movie, movie_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-  I2V_TRY(cudaMemcpyAsync(d_ts, timestamp, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-  I2V_TRY(cudaMemcpyAsync(d_half, half, n, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(sc.alloc(&d_user, n)); CUDA_TRY(sc.alloc(&d_movie, n)); CUDA_TRY(sc.alloc(&d_ts, n));
+  CUDA_TRY(sc.alloc(&d_half, n)); CUDA_TRY(sc.alloc(&d_order, n)); CUDA_TRY(sc.alloc(&d_suser, n));
+  CUDA_TRY(sc.alloc(&d_iota, n)); CUDA_TRY(sc.alloc(&d_sel, n)); CUDA_TRY(sc.alloc(&d_flag, n));
+  CUDA_TRY(sc.alloc(&out->movie, n)); CUDA_TRY(sc.alloc(&out->user, n)); CUDA_TRY(sc.alloc(&out->n, 1));
+  CUDA_TRY(cudaMemcpyAsync(d_user, user_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_movie, movie_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_ts, timestamp, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_half, half, n, cudaMemcpyHostToDevice, s));
   const int T = 256;
-  I2V_TRY(user_time_order(d_user, d_ts, n, d_order, d_suser, s));
+  PROPAGATE(user_time_order(s, d_user, d_ts, n, d_order, d_suser));
   i2v_flag_kernel<<<grid_for(n, T), T, 0, s>>>(d_order, d_half, n, d_flag, d_iota);
-  I2V_LAUNCHED();
-  size_t tmp_bytes = 0;
-  I2V_TRY(cub::DeviceSelect::Flagged(nullptr, tmp_bytes, d_iota, d_flag, d_sel, out->n, n, s));
-  uint8_t* d_tmp;
-  I2V_TRY(sc.alloc(&d_tmp, tmp_bytes));
-  I2V_TRY(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_iota, d_flag, d_sel, out->n, n, s));
+  LAUNCHED();
+  CUB_RUN(c, cub::DeviceSelect::Flagged(tmp__, tb__, d_iota, d_flag, d_sel, out->n, n, s));
   i2v_gather_kernel<<<grid_for(n, T), T, 0, s>>>(d_sel, out->n, d_order, d_suser, d_movie, out->movie, out->user);
-  I2V_LAUNCHED();
+  LAUNCHED();
   return SRS_OK;
 }
 
-int word2vec_fit(Scratch& sc, cudaStream_t s, const int32_t* d_pmovie, const uint32_t* d_puser, const int* d_npos,
-                 int n, int32_t n_slots, const srs_item2vec_params& hp, const char* what, int32_t capacity,
+int word2vec_fit(HostCall& c, const int32_t* d_pmovie, const uint32_t* d_puser, const int* d_npos, int n,
+                 int32_t n_slots, const srs_item2vec_params& hp, const char* what, int32_t capacity,
                  int32_t* vocab_ids, float* vectors, int32_t* vocab_size) {
+  Scratch& sc = c.sc;
+  cudaStream_t s = c.s;
   int32_t *d_count, *d_iota, *d_pword, *d_vidx, *d_words, *d_ustart, *d_offs, *d_points, *d_codelen;
   uint32_t *d_wuser, *d_code;
   uint8_t* d_flag;
   int* d_nsel;
-  I2V_TRY(sc.alloc(&d_count, n_slots)); I2V_TRY(sc.alloc(&d_iota, n)); I2V_TRY(sc.alloc(&d_flag, n));
-  I2V_TRY(sc.alloc(&d_nsel, 2));
-  I2V_TRY(cudaMemsetAsync(d_count, 0, sizeof(int32_t) * n_slots, s));
+  CUDA_TRY(sc.alloc(&d_count, n_slots)); CUDA_TRY(sc.alloc(&d_iota, n)); CUDA_TRY(sc.alloc(&d_flag, n));
+  CUDA_TRY(sc.alloc(&d_nsel, 2));
+  CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(int32_t) * n_slots, s));
   const int T = 256;
   i2v_count_kernel<<<grid_for(n, T), T, 0, s>>>(d_pmovie, d_npos, d_count);
-  I2V_LAUNCHED();
-  size_t tmp_bytes = 0, t2 = 0;
-  I2V_TRY(cub::DeviceSelect::Flagged(nullptr, tmp_bytes, d_iota, d_flag, d_iota, d_nsel, n, s));
-  I2V_TRY(cub::DeviceScan::InclusiveScan(nullptr, t2, d_iota, d_iota, MaxOp(), n, s));
-  tmp_bytes = std::max(tmp_bytes, t2);
-  uint8_t* d_tmp;
-  I2V_TRY(sc.alloc(&d_tmp, tmp_bytes));
+  LAUNCHED();
   std::vector<int32_t> counts(n_slots);
-  I2V_TRY(cudaMemcpyAsync(counts.data(), d_count, sizeof(int32_t) * n_slots, cudaMemcpyDeviceToHost, s));
-  I2V_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(counts.data(), d_count, sizeof(int32_t) * n_slots, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
 
   // vocabulary: count >= minCount, count descending, ties by movie id ascending
   std::vector<int32_t> vocab;
@@ -460,8 +398,8 @@ int word2vec_fit(Scratch& sc, cudaStream_t s, const int32_t* d_pmovie, const uin
     if (counts[m] >= kMinCount) vocab.push_back(m);
   std::stable_sort(vocab.begin(), vocab.end(), [&](int32_t x, int32_t y) { return counts[x] > counts[y]; });
   const int V = (int)vocab.size();
-  if (V == 0) return i2v_fail(SRS_ERR_INVALID, "the vocabulary is empty: no movie has %d %s", kMinCount, what);
-  if (V > capacity) return i2v_fail(SRS_ERR_RANGE, "vocabulary of %d words exceeds capacity %d", V, capacity);
+  if (V == 0) return failf(SRS_ERR_INVALID, "the vocabulary is empty: no movie has %d %s", kMinCount, what);
+  if (V > capacity) return failf(SRS_ERR_RANGE, "vocabulary of %d words exceeds capacity %d", V, capacity);
   std::vector<int64_t> cn(V);
   std::vector<int32_t> vocab_index(n_slots, -1);
   int64_t train_words = 0;
@@ -474,7 +412,7 @@ int word2vec_fit(Scratch& sc, cudaStream_t s, const int32_t* d_pmovie, const uin
   std::vector<int32_t> points, codelen;
   const int deepest = huffman(cn, code_bits, points, codelen);
   if (deepest > kMaxCode)
-    return i2v_fail(SRS_ERR_INVALID, "Huffman code of length %d: at most %d are supported", deepest, kMaxCode);
+    return failf(SRS_ERR_INVALID, "Huffman code of length %d: at most %d are supported", deepest, kMaxCode);
   std::vector<float> exp_table(kExpTable);
   for (int i = 0; i < kExpTable; ++i) {
     const double t = std::exp((2.0 * i / kExpTable - 1.0) * kMaxExp);
@@ -486,36 +424,36 @@ int word2vec_fit(Scratch& sc, cudaStream_t s, const int32_t* d_pmovie, const uin
   const int64_t vd = (int64_t)V * D;
   float *d_exp, *d_syn0, *d_syn1, *d_l0 = nullptr, *d_l1 = nullptr;
   uint8_t *d_mod0 = nullptr, *d_mod1 = nullptr;
-  I2V_TRY(sc.alloc(&d_vidx, n_slots)); I2V_TRY(sc.alloc(&d_pword, n)); I2V_TRY(sc.alloc(&d_words, nw));
-  I2V_TRY(sc.alloc(&d_wuser, nw)); I2V_TRY(sc.alloc(&d_ustart, nw)); I2V_TRY(sc.alloc(&d_offs, nw));
-  I2V_TRY(sc.alloc(&d_points, (size_t)V * kMaxCode)); I2V_TRY(sc.alloc(&d_codelen, V));
-  I2V_TRY(sc.alloc(&d_code, V)); I2V_TRY(sc.alloc(&d_exp, kExpTable));
-  I2V_TRY(sc.alloc(&d_syn0, vd)); I2V_TRY(sc.alloc(&d_syn1, vd));
+  CUDA_TRY(sc.alloc(&d_vidx, n_slots)); CUDA_TRY(sc.alloc(&d_pword, n)); CUDA_TRY(sc.alloc(&d_words, nw));
+  CUDA_TRY(sc.alloc(&d_wuser, nw)); CUDA_TRY(sc.alloc(&d_ustart, nw)); CUDA_TRY(sc.alloc(&d_offs, nw));
+  CUDA_TRY(sc.alloc(&d_points, (size_t)V * kMaxCode)); CUDA_TRY(sc.alloc(&d_codelen, V));
+  CUDA_TRY(sc.alloc(&d_code, V)); CUDA_TRY(sc.alloc(&d_exp, kExpTable));
+  CUDA_TRY(sc.alloc(&d_syn0, vd)); CUDA_TRY(sc.alloc(&d_syn1, vd));
   if (P > 1) {
-    I2V_TRY(sc.alloc(&d_l0, vd * P)); I2V_TRY(sc.alloc(&d_l1, vd * P));
-    I2V_TRY(sc.alloc(&d_mod0, (size_t)V * P)); I2V_TRY(sc.alloc(&d_mod1, (size_t)V * P));
+    CUDA_TRY(sc.alloc(&d_l0, vd * P)); CUDA_TRY(sc.alloc(&d_l1, vd * P));
+    CUDA_TRY(sc.alloc(&d_mod0, (size_t)V * P)); CUDA_TRY(sc.alloc(&d_mod1, (size_t)V * P));
   }
-  I2V_TRY(cudaMemcpyAsync(d_vidx, vocab_index.data(), sizeof(int32_t) * n_slots, cudaMemcpyHostToDevice, s));
-  I2V_TRY(cudaMemcpyAsync(d_points, points.data(), sizeof(int32_t) * points.size(), cudaMemcpyHostToDevice, s));
-  I2V_TRY(cudaMemcpyAsync(d_codelen, codelen.data(), sizeof(int32_t) * V, cudaMemcpyHostToDevice, s));
-  I2V_TRY(cudaMemcpyAsync(d_code, code_bits.data(), sizeof(uint32_t) * V, cudaMemcpyHostToDevice, s));
-  I2V_TRY(cudaMemcpyAsync(d_exp, exp_table.data(), sizeof(float) * kExpTable, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_vidx, vocab_index.data(), sizeof(int32_t) * n_slots, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_points, points.data(), sizeof(int32_t) * points.size(), cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_codelen, codelen.data(), sizeof(int32_t) * V, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_code, code_bits.data(), sizeof(uint32_t) * V, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_exp, exp_table.data(), sizeof(float) * kExpTable, cudaMemcpyHostToDevice, s));
 
   // the in-vocabulary words and their sentence keys, then the sentence starts
   i2v_map_kernel<<<grid_for(n, T), T, 0, s>>>(d_pmovie, d_npos, n, d_vidx, d_pword, d_flag);
-  I2V_LAUNCHED();
-  I2V_TRY(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_pword, d_flag, d_words, d_nsel + 1, n, s));
-  I2V_TRY(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_puser, d_flag, d_wuser, d_nsel + 1, n, s));
+  LAUNCHED();
+  CUB_RUN(c, cub::DeviceSelect::Flagged(tmp__, tb__, d_pword, d_flag, d_words, d_nsel + 1, n, s));
+  CUB_RUN(c, cub::DeviceSelect::Flagged(tmp__, tb__, d_puser, d_flag, d_wuser, d_nsel + 1, n, s));
   i2v_user_start_kernel<<<grid_for(nw, T), T, 0, s>>>(d_wuser, nw, d_iota);
-  I2V_LAUNCHED();
-  I2V_TRY(cub::DeviceScan::InclusiveScan(d_tmp, tmp_bytes, d_iota, d_ustart, MaxOp(), nw, s));
+  LAUNCHED();
+  CUB_RUN(c, cub::DeviceScan::InclusiveScan(tmp__, tb__, d_iota, d_ustart, MaxOp(), nw, s));
   i2v_chunk_kernel<<<grid_for(nw, T), T, 0, s>>>(d_ustart, nw, d_flag, d_iota);
-  I2V_LAUNCHED();
-  I2V_TRY(cub::DeviceSelect::Flagged(d_tmp, tmp_bytes, d_iota, d_flag, d_offs, d_nsel, nw, s));
+  LAUNCHED();
+  CUB_RUN(c, cub::DeviceSelect::Flagged(tmp__, tb__, d_iota, d_flag, d_offs, d_nsel, nw, s));
 
   i2v_init_kernel<<<grid_for(vd, T), T, 0, s>>>(d_syn0, vd, hp.seed, D);
-  I2V_LAUNCHED();
-  I2V_TRY(cudaMemsetAsync(d_syn1, 0, sizeof(float) * vd, s));
+  LAUNCHED();
+  CUDA_TRY(cudaMemsetAsync(d_syn1, 0, sizeof(float) * vd, s));
   TrainArgs ta;
   ta.words = d_words; ta.chunk_offs = d_offs; ta.n_chunks = d_nsel; ta.n_words = nw;
   ta.code_bits = d_code; ta.points = d_points; ta.codelen = d_codelen; ta.exp_table = d_exp;
@@ -527,23 +465,23 @@ int word2vec_fit(Scratch& sc, cudaStream_t s, const int32_t* d_pmovie, const uin
   for (int k = 1; k <= hp.iterations; ++k) {
     if (P > 1) {
       i2v_broadcast_kernel<<<grid_for(vd * P, T), T, 0, s>>>(d_syn0, vd, P, d_l0);
-      I2V_LAUNCHED();
+      LAUNCHED();
       i2v_broadcast_kernel<<<grid_for(vd * P, T), T, 0, s>>>(d_syn1, vd, P, d_l1);
-      I2V_LAUNCHED();
-      I2V_TRY(cudaMemsetAsync(d_mod0, 0, (size_t)V * P, s));
-      I2V_TRY(cudaMemsetAsync(d_mod1, 0, (size_t)V * P, s));
+      LAUNCHED();
+      CUDA_TRY(cudaMemsetAsync(d_mod0, 0, (size_t)V * P, s));
+      CUDA_TRY(cudaMemsetAsync(d_mod1, 0, (size_t)V * P, s));
     }
     i2v_train_kernel<<<train_blocks, 128, 0, s>>>(ta, k);
-    I2V_LAUNCHED();
+    LAUNCHED();
     if (P > 1) {
       i2v_merge_kernel<<<grid_for(vd, T), T, 0, s>>>(d_l0, d_mod0, V, D, P, d_syn0);
-      I2V_LAUNCHED();
+      LAUNCHED();
       i2v_merge_kernel<<<grid_for(vd, T), T, 0, s>>>(d_l1, d_mod1, V, D, P, d_syn1);
-      I2V_LAUNCHED();
+      LAUNCHED();
     }
   }
-  I2V_TRY(cudaMemcpyAsync(vectors, d_syn0, sizeof(float) * vd, cudaMemcpyDeviceToHost, s));
-  I2V_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(vectors, d_syn0, sizeof(float) * vd, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   std::copy(vocab.begin(), vocab.end(), vocab_ids);
   *vocab_size = V;
   return SRS_OK;
@@ -557,98 +495,88 @@ extern "C" int srs_item2vec_host(const int32_t* user_id, const int32_t* movie_id
                                  const int32_t* timestamp, int64_t n_ratings, const srs_item2vec_params* params,
                                  int32_t device, int32_t capacity, int32_t* vocab_ids, float* vectors,
                                  int32_t* vocab_size) {
-  if (!vocab_size) return i2v_fail(SRS_ERR_INVALID, "null vocab_size");
+  if (!vocab_size) return failf(SRS_ERR_INVALID, "null vocab_size");
   *vocab_size = 0;
-  if (int rc = i2v_check_params(params)) return rc;
+  PROPAGATE(i2v_check_params(params));
   if (capacity < 0 || (capacity > 0 && (!vocab_ids || !vectors)))
-    return i2v_fail(SRS_ERR_INVALID, "negative capacity or null outputs");
+    return failf(SRS_ERR_INVALID, "negative capacity or null outputs");
   int32_t n_slots = 0;
-  if (int rc = i2v_check_ratings(user_id, movie_id, half, timestamp, n_ratings, &n_slots)) return rc;
-  if (int rc = select_device(device)) return rc;
+  PROPAGATE(i2v_check_ratings(user_id, movie_id, half, timestamp, n_ratings, &n_slots));
 
-  Scratch sc;
-  StreamGuard sg;
-  I2V_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+  HostCall c;
+  PROPAGATE(c.begin(device));
   const int n = (int)n_ratings;
   I2vCorpus pos;
-  if (int rc = i2v_positive_corpus(sc, sg.s, user_id, movie_id, half, timestamp, n, &pos)) return rc;
-  return word2vec_fit(sc, sg.s, pos.movie, pos.user, pos.n, n, n_slots, *params, "ratings >= 3.5", capacity,
-                      vocab_ids, vectors, vocab_size);
+  PROPAGATE(i2v_positive_corpus(c, user_id, movie_id, half, timestamp, n, &pos));
+  return word2vec_fit(c, pos.movie, pos.user, pos.n, n, n_slots, *params, "ratings >= 3.5", capacity, vocab_ids,
+                      vectors, vocab_size);
 }
 
 extern "C" int srs_user_embeddings_host(const int32_t* user_id, const int32_t* movie_id, int64_t n_ratings,
                                         const int32_t* item_ids, const float* item_vectors, int32_t n_items,
                                         int32_t vector_size, int32_t device, int32_t capacity, int32_t* user_ids,
                                         float* user_vectors, int32_t* n_users) {
-  if (!n_users) return i2v_fail(SRS_ERR_INVALID, "null n_users");
+  if (!n_users) return failf(SRS_ERR_INVALID, "null n_users");
   *n_users = 0;
   if (vector_size < 1 || vector_size > kMaxDim)
-    return i2v_fail(SRS_ERR_INVALID, "vector_size %d outside 1..%d", vector_size, kMaxDim);
+    return failf(SRS_ERR_INVALID, "vector_size %d outside 1..%d", vector_size, kMaxDim);
   if (n_items < 0 || (n_items && (!item_ids || !item_vectors)))
-    return i2v_fail(SRS_ERR_INVALID, "negative n_items or null items");
+    return failf(SRS_ERR_INVALID, "negative n_items or null items");
   if (capacity < 0 || (capacity > 0 && (!user_ids || !user_vectors)))
-    return i2v_fail(SRS_ERR_INVALID, "negative capacity or null outputs");
+    return failf(SRS_ERR_INVALID, "negative capacity or null outputs");
   int32_t n_slots = 0;
-  if (int rc = check_ratings(user_id, movie_id, n_ratings, &n_slots)) return rc;
+  PROPAGATE(check_ratings(user_id, movie_id, n_ratings, &n_slots));
   for (int32_t i = 0; i < n_items; ++i) {
     if (item_ids[i] < 0 || item_ids[i] >= kMaxMovieSlots)
-      return i2v_fail(SRS_ERR_INVALID, "item %d: id %d outside 0..2^24-1", i, item_ids[i]);
+      return failf(SRS_ERR_INVALID, "item %d: id %d outside 0..2^24-1", i, item_ids[i]);
     n_slots = std::max(n_slots, item_ids[i] + 1);
   }
   std::vector<int32_t> row_of(std::max(n_slots, 1), -1);
   for (int32_t i = 0; i < n_items; ++i) {
-    if (row_of[item_ids[i]] >= 0) return i2v_fail(SRS_ERR_INVALID, "item id %d appears twice", item_ids[i]);
+    if (row_of[item_ids[i]] >= 0) return failf(SRS_ERR_INVALID, "item id %d appears twice", item_ids[i]);
     row_of[item_ids[i]] = i;
   }
   const int n = (int)n_ratings;
   if (n == 0) return SRS_OK;
-  if (int rc = select_device(device)) return rc;
 
-  Scratch sc;
-  StreamGuard sg;
-  I2V_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
-  cudaStream_t s = sg.s;
+  HostCall c;
+  PROPAGATE(c.begin(device));
+  Scratch& sc = c.sc;
+  cudaStream_t s = c.s;
   const int D = vector_size;
   const size_t slots = row_of.size();
   int32_t *d_movie, *d_iota, *d_order, *d_uniq, *d_cnt, *d_start, *d_row;
   uint32_t *d_user, *d_suser;
   float *d_vec, *d_out;
   int* d_nu;
-  I2V_TRY(sc.alloc(&d_user, n)); I2V_TRY(sc.alloc(&d_movie, n)); I2V_TRY(sc.alloc(&d_iota, n));
-  I2V_TRY(sc.alloc(&d_order, n)); I2V_TRY(sc.alloc(&d_suser, n)); I2V_TRY(sc.alloc(&d_uniq, n));
-  I2V_TRY(sc.alloc(&d_cnt, n)); I2V_TRY(sc.alloc(&d_start, n)); I2V_TRY(sc.alloc(&d_row, slots));
-  I2V_TRY(sc.alloc(&d_vec, (size_t)std::max(n_items, 1) * D)); I2V_TRY(sc.alloc(&d_out, (size_t)n * D));
-  I2V_TRY(sc.alloc(&d_nu, 1));
+  CUDA_TRY(sc.alloc(&d_user, n)); CUDA_TRY(sc.alloc(&d_movie, n)); CUDA_TRY(sc.alloc(&d_iota, n));
+  CUDA_TRY(sc.alloc(&d_order, n)); CUDA_TRY(sc.alloc(&d_suser, n)); CUDA_TRY(sc.alloc(&d_uniq, n));
+  CUDA_TRY(sc.alloc(&d_cnt, n)); CUDA_TRY(sc.alloc(&d_start, n)); CUDA_TRY(sc.alloc(&d_row, slots));
+  CUDA_TRY(sc.alloc(&d_vec, (size_t)std::max(n_items, 1) * D)); CUDA_TRY(sc.alloc(&d_out, (size_t)n * D));
+  CUDA_TRY(sc.alloc(&d_nu, 1));
   std::vector<int32_t> iota(n);
   for (int i = 0; i < n; ++i) iota[i] = i;
-  I2V_TRY(cudaMemcpyAsync(d_user, user_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-  I2V_TRY(cudaMemcpyAsync(d_movie, movie_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-  I2V_TRY(cudaMemcpyAsync(d_iota, iota.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-  I2V_TRY(cudaMemcpyAsync(d_row, row_of.data(), sizeof(int32_t) * slots, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_user, user_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_movie, movie_id, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_iota, iota.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_row, row_of.data(), sizeof(int32_t) * slots, cudaMemcpyHostToDevice, s));
   if (n_items)
-    I2V_TRY(cudaMemcpyAsync(d_vec, item_vectors, sizeof(float) * n_items * D, cudaMemcpyHostToDevice, s));
-  I2V_TRY(cudaMemsetAsync(d_cnt, 0, sizeof(int32_t) * n, s));
-  size_t b1 = 0, b2 = 0, b3 = 0;
-  I2V_TRY(cub::DeviceRadixSort::SortPairs(nullptr, b1, d_user, d_suser, d_iota, d_order, n, 0, 31, s));
-  I2V_TRY(cub::DeviceRunLengthEncode::Encode(nullptr, b2, d_suser, d_uniq, d_cnt, d_nu, n, s));
-  I2V_TRY(cub::DeviceScan::ExclusiveSum(nullptr, b3, d_cnt, d_start, n, s));
-  uint8_t* d_tmp;
-  const size_t tmp_bytes = std::max(b1, std::max(b2, b3));
-  I2V_TRY(sc.alloc(&d_tmp, tmp_bytes));
+    CUDA_TRY(cudaMemcpyAsync(d_vec, item_vectors, sizeof(float) * n_items * D, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemsetAsync(d_cnt, 0, sizeof(int32_t) * n, s));
   // a stable sort by user: each user's ratings stay in file order
-  I2V_TRY(cub::DeviceRadixSort::SortPairs(d_tmp, b1, d_user, d_suser, d_iota, d_order, n, 0, 31, s));
-  I2V_TRY(cub::DeviceRunLengthEncode::Encode(d_tmp, b2, d_suser, d_uniq, d_cnt, d_nu, n, s));
-  I2V_TRY(cub::DeviceScan::ExclusiveSum(d_tmp, b3, d_cnt, d_start, n, s));
+  CUB_RUN(c, cub::DeviceRadixSort::SortPairs(tmp__, tb__, d_user, d_suser, d_iota, d_order, n, 0, 31, s));
+  CUB_RUN(c, cub::DeviceRunLengthEncode::Encode(tmp__, tb__, d_suser, d_uniq, d_cnt, d_nu, n, s));
+  CUB_RUN(c, cub::DeviceScan::ExclusiveSum(tmp__, tb__, d_cnt, d_start, n, s));
   i2v_user_kernel<<<(int)(((int64_t)n * 32 + 127) / 128), 128, 0, s>>>(d_order, d_start, d_cnt, d_nu, d_movie, d_row,
                                                                      d_vec, D, d_out);
-  I2V_LAUNCHED();
+  LAUNCHED();
   int nu = 0;
-  I2V_TRY(cudaMemcpyAsync(&nu, d_nu, sizeof(int), cudaMemcpyDeviceToHost, s));
-  I2V_TRY(cudaStreamSynchronize(s));
-  if (nu > capacity) return i2v_fail(SRS_ERR_RANGE, "%d users exceed capacity %d", nu, capacity);
-  I2V_TRY(cudaMemcpyAsync(user_ids, d_uniq, sizeof(int32_t) * nu, cudaMemcpyDeviceToHost, s));
-  I2V_TRY(cudaMemcpyAsync(user_vectors, d_out, sizeof(float) * nu * D, cudaMemcpyDeviceToHost, s));
-  I2V_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(&nu, d_nu, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  if (nu > capacity) return failf(SRS_ERR_RANGE, "%d users exceed capacity %d", nu, capacity);
+  CUDA_TRY(cudaMemcpyAsync(user_ids, d_uniq, sizeof(int32_t) * nu, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(user_vectors, d_out, sizeof(float) * nu * D, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   *n_users = nu;
   return SRS_OK;
 }

@@ -1,5 +1,6 @@
-// kernels.h - parameter blocks (device pointers into the model's private weight
-// layout) and launch entry points of the fused per-model forward kernels.
+// kernels.h - what model.cu and ncf_train.cu need of the kernel files: the parameter blocks (device pointers into
+// the model's private weight layout) and launch entry points of the fused per-model forward kernels, of the
+// training steps, the ranking tail and the metrics.  The offline jobs' shared declarations are in hostcall.h.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -10,7 +11,6 @@
 #include "common.cuh"
 
 struct srs_eval_result;
-struct srs_item2vec_params;
 
 namespace srs {
 
@@ -315,55 +315,6 @@ cudaError_t launch_auc_value(unsigned long long* hist, int K, double* auc, doubl
 void metrics_summarise(const unsigned long long* hist, unsigned long long correct, double loss_sum,
                        srs_eval_result* out, int64_t* confusion);
 
-// featureeng.cu: the (user, timestamp string, file index) order of n ratings (device arrays), as the reference's
-// jobs order a user's ratings: d_order[i] = file index of the i-th, d_user_sorted[i] = its user.  Stable radix
-// sorts on `s`; temporaries are stream-ordered allocations.
-cudaError_t user_time_order(const int32_t* d_user, const int32_t* d_ts, int n, int32_t* d_order,
-                            uint32_t* d_user_sorted, cudaStream_t s);
-// featureeng.cu: the movies' exact integer moments of n ratings (device arrays): d_mmom[3 m .. 3 m + 2] += count,
-// sum h, sum h^2 of movie m's half-stars (64-bit integer atomics; the caller zeroes d_mmom); d_iota[i] = i.
-cudaError_t launch_movie_moments(const int32_t* d_movie, const int8_t* d_half, int n, int32_t* d_iota,
-                                 unsigned long long* d_mmom, cudaStream_t s);
-
-struct Scratch {                       // device allocations of one host call, freed when it ends
-  std::vector<void*> ptrs;
-  ~Scratch() { for (void* p : ptrs) cudaFree(p); }
-  template <class T>
-  cudaError_t alloc(T** p, size_t count) {
-    void* q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, (count ? count : 1) * sizeof(T));
-    if (e == cudaSuccess) ptrs.push_back(q);
-    *p = static_cast<T*>(q);
-    return e;
-  }
-};
-
-// ---- item2vec.cu: the Embedding job's sentences and Word2Vec, shared with graphemb.cu ---------------------------
-// Each returns an SRS_* code and sets the last error message.
-int i2v_check_params(const srs_item2vec_params* params);
-// the ratings' checks of srs_item2vec_host (ids, half-stars, timestamps, at least one rating); *n_slots = max movie + 1
-int i2v_check_ratings(const int32_t* user_id, const int32_t* movie_id, const int8_t* half, const int32_t* timestamp,
-                      int64_t n_ratings, int32_t* n_slots);
-int i2v_select_device(int32_t device);
-struct I2vCorpus {                     // device: *n words, movie[i] in sentence order, user[i] its sentence's key
-  int32_t* movie;
-  uint32_t* user;
-  int* n;
-};
-// processItemSequence: the n ratings (host) uploaded, and their positives (>= 3.5) grouped by user ascending, each
-// user's in (timestamp string, input index) order; arrays of n entries allocated in `sc`
-int i2v_positive_corpus(Scratch& sc, cudaStream_t s, const int32_t* user_id, const int32_t* movie_id,
-                        const int8_t* half, const int32_t* timestamp, int n, I2vCorpus* out);
-// Word2Vec.fit over the device corpus of *d_n <= n words (movie ids < n_slots) whose sentences are the runs of
-// equal keys: vocabulary, Huffman tree, exp table, the 1000-word cut and training; the outputs as srs_item2vec_host.
-// `what` names the words in the empty-vocabulary message.  Synchronises `s`.
-int word2vec_fit(Scratch& sc, cudaStream_t s, const int32_t* d_words, const uint32_t* d_keys, const int* d_n, int n,
-                 int32_t n_slots, const srs_item2vec_params& hp, const char* what, int32_t capacity,
-                 int32_t* vocab_ids, float* vectors, int32_t* vocab_size);
-
 extern int64_t g_launch_count;   // kernels launched by this library
-
-// model.cu: set the message srs_last_error() reports on this thread; returns `code`
-int set_last_error(int code, const char* msg);
 
 }  // namespace srs

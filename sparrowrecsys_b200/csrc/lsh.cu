@@ -12,11 +12,9 @@
 #include <cuda_runtime.h>
 
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
 
 #include "../../include/srs_ctr.h"
-#include "kernels.h"
+#include "hostcall.h"
 
 namespace srs {
 namespace {
@@ -26,40 +24,6 @@ constexpr int kMaxLshDim = 1024;
 constexpr int kMaxK = 256;
 constexpr int kQueryWarps = 8;
 constexpr unsigned kFull = 0xffffffffu;
-
-int lsh_fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  return set_last_error(code, buf);
-}
-
-#define LSH_TRY(expr)                                                                                     \
-  do {                                                                                                    \
-    cudaError_t e__ = (expr);                                                                             \
-    if (e__ != cudaSuccess)                                                                               \
-      return lsh_fail(SRS_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__); \
-  } while (0)
-
-#define LSH_LAUNCHED()                                                                                    \
-  do {                                                                                                    \
-    ++g_launch_count;                                                                                     \
-    LSH_TRY(cudaGetLastError());                                                                          \
-  } while (0)
-
-int grid_for(int64_t n, int threads) {
-  int64_t b = (n + threads - 1) / threads;
-  return (int)(b < 1 ? 1 : b > 132 * 64 ? 132 * 64 : b);
-}
-
-struct StreamGuard {
-  cudaStream_t s = nullptr;
-  ~StreamGuard() {
-    if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
-  }
-};
 
 // BLAS.dot(x, v) / bucketLength, floored: F2J's ddot adds the products left to right from 0.0
 template <class X>
@@ -187,39 +151,29 @@ bool finite_d(const double* p, int64_t n) {
 
 int check_model(const float* vectors, int64_t n, int32_t dim, const double* unit_vectors, int32_t num_tables,
                 double bucket_length) {
-  if (dim < 1 || dim > kMaxLshDim) return lsh_fail(SRS_ERR_INVALID, "dim %d outside 1..%d", dim, kMaxLshDim);
+  if (dim < 1 || dim > kMaxLshDim) return failf(SRS_ERR_INVALID, "dim %d outside 1..%d", dim, kMaxLshDim);
   if (num_tables < 1 || num_tables > kMaxTables)
-    return lsh_fail(SRS_ERR_INVALID, "num_hash_tables %d outside 1..%d", num_tables, kMaxTables);
+    return failf(SRS_ERR_INVALID, "num_hash_tables %d outside 1..%d", num_tables, kMaxTables);
   if (!(bucket_length > 0) || !std::isfinite(bucket_length))
-    return lsh_fail(SRS_ERR_INVALID, "bucket_length %g is not finite and > 0", bucket_length);
-  if (n < 0 || n > INT32_MAX) return lsh_fail(SRS_ERR_INVALID, "n %lld outside 0..2^31-1", (long long)n);
-  if (!unit_vectors || (n && !vectors)) return lsh_fail(SRS_ERR_INVALID, "null inputs");
+    return failf(SRS_ERR_INVALID, "bucket_length %g is not finite and > 0", bucket_length);
+  if (n < 0 || n > INT32_MAX) return failf(SRS_ERR_INVALID, "n %lld outside 0..2^31-1", (long long)n);
+  if (!unit_vectors || (n && !vectors)) return failf(SRS_ERR_INVALID, "null inputs");
   if (!finite_d(unit_vectors, (int64_t)num_tables * dim))
-    return lsh_fail(SRS_ERR_INVALID, "a unit vector entry is not finite");
-  if (!finite_f(vectors, n * dim)) return lsh_fail(SRS_ERR_INVALID, "a vector entry is not finite");
-  return SRS_OK;
-}
-
-int select_device(int32_t device) {
-  int ndev = 0;
-  cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev == 0)
-    return lsh_fail(SRS_ERR_CUDA, "no CUDA device available (%s); this library has no CPU path", cudaGetErrorString(ce));
-  if (device < 0 || device >= ndev) return lsh_fail(SRS_ERR_INVALID, "device %d out of range", device);
-  LSH_TRY(cudaSetDevice(device));
+    return failf(SRS_ERR_INVALID, "a unit vector entry is not finite");
+  if (!finite_f(vectors, n * dim)) return failf(SRS_ERR_INVALID, "a vector entry is not finite");
   return SRS_OK;
 }
 
 // the rows and unit vectors uploaded, and the rows' bucket ids [n][L] on the device
-int hash_rows(Scratch& sc, cudaStream_t s, const float* vectors, int64_t n, int32_t dim, const double* unit_vectors,
-              int32_t L, double bl, float** d_x, double** d_uv, double** d_buckets) {
-  LSH_TRY(sc.alloc(d_x, n * dim)); LSH_TRY(sc.alloc(d_uv, (int64_t)L * dim)); LSH_TRY(sc.alloc(d_buckets, n * L));
-  if (n) LSH_TRY(cudaMemcpyAsync(*d_x, vectors, sizeof(float) * n * dim, cudaMemcpyHostToDevice, s));
-  LSH_TRY(cudaMemcpyAsync(*d_uv, unit_vectors, sizeof(double) * L * dim, cudaMemcpyHostToDevice, s));
+int hash_rows(HostCall& c, const float* vectors, int64_t n, int32_t dim, const double* unit_vectors, int32_t L,
+              double bl, float** d_x, double** d_uv, double** d_buckets) {
+  PROPAGATE(c.upload(d_x, vectors, n * dim));
+  PROPAGATE(c.upload(d_uv, unit_vectors, (int64_t)L * dim));
+  CUDA_TRY(c.sc.alloc(d_buckets, n * L));
   if (n) {
     const int T = 256;
-    lsh_hash_kernel<<<grid_for(n * L, T), T, 0, s>>>(*d_x, n, dim, *d_uv, L, bl, *d_buckets);
-    LSH_LAUNCHED();
+    lsh_hash_kernel<<<grid_for(n * L, T), T, 0, c.s>>>(*d_x, n, dim, *d_uv, L, bl, *d_buckets);
+    LAUNCHED();
   }
   return SRS_OK;
 }
@@ -231,19 +185,16 @@ using namespace srs;
 
 extern "C" int srs_lsh_transform_host(const float* vectors, int64_t n, int32_t dim, const double* unit_vectors,
                                       int32_t num_tables, double bucket_length, int32_t device, double* buckets) {
-  if (int rc = check_model(vectors, n, dim, unit_vectors, num_tables, bucket_length)) return rc;
-  if (n && !buckets) return lsh_fail(SRS_ERR_INVALID, "null buckets");
+  PROPAGATE(check_model(vectors, n, dim, unit_vectors, num_tables, bucket_length));
+  if (n && !buckets) return failf(SRS_ERR_INVALID, "null buckets");
   if (n == 0) return SRS_OK;
-  if (int rc = select_device(device)) return rc;
-  Scratch sc;
-  StreamGuard sg;
-  LSH_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
+  HostCall c;
+  PROPAGATE(c.begin(device));
   float* d_x;
   double *d_uv, *d_b;
-  if (int rc = hash_rows(sc, sg.s, vectors, n, dim, unit_vectors, num_tables, bucket_length, &d_x, &d_uv, &d_b))
-    return rc;
-  LSH_TRY(cudaMemcpyAsync(buckets, d_b, sizeof(double) * n * num_tables, cudaMemcpyDeviceToHost, sg.s));
-  LSH_TRY(cudaStreamSynchronize(sg.s));
+  PROPAGATE(hash_rows(c, vectors, n, dim, unit_vectors, num_tables, bucket_length, &d_x, &d_uv, &d_b));
+  CUDA_TRY(cudaMemcpyAsync(buckets, d_b, sizeof(double) * n * num_tables, cudaMemcpyDeviceToHost, c.s));
+  CUDA_TRY(cudaStreamSynchronize(c.s));
   return SRS_OK;
 }
 
@@ -251,37 +202,33 @@ extern "C" int srs_lsh_query_host(const int32_t* ids, const float* vectors, int6
                                   const double* unit_vectors, int32_t num_tables, double bucket_length,
                                   const double* keys, int32_t num_keys, int32_t k, int32_t device, int32_t* out_ids,
                                   double* out_dist, int32_t* out_count) {
-  if (int rc = check_model(vectors, n, dim, unit_vectors, num_tables, bucket_length)) return rc;
-  if (n && !ids) return lsh_fail(SRS_ERR_INVALID, "null ids");
-  if (k < 1 || k > kMaxK) return lsh_fail(SRS_ERR_INVALID, "k %d outside 1..%d", k, kMaxK);
-  if (num_keys < 0) return lsh_fail(SRS_ERR_INVALID, "num_keys %d is negative", num_keys);
+  PROPAGATE(check_model(vectors, n, dim, unit_vectors, num_tables, bucket_length));
+  if (n && !ids) return failf(SRS_ERR_INVALID, "null ids");
+  if (k < 1 || k > kMaxK) return failf(SRS_ERR_INVALID, "k %d outside 1..%d", k, kMaxK);
+  if (num_keys < 0) return failf(SRS_ERR_INVALID, "num_keys %d is negative", num_keys);
   if (num_keys && (!keys || !out_ids || !out_dist || !out_count))
-    return lsh_fail(SRS_ERR_INVALID, "null keys or outputs");
-  if (!finite_d(keys, (int64_t)num_keys * dim)) return lsh_fail(SRS_ERR_INVALID, "a key entry is not finite");
+    return failf(SRS_ERR_INVALID, "null keys or outputs");
+  if (!finite_d(keys, (int64_t)num_keys * dim)) return failf(SRS_ERR_INVALID, "a key entry is not finite");
   if (num_keys == 0) return SRS_OK;
-  if (int rc = select_device(device)) return rc;
-  Scratch sc;
-  StreamGuard sg;
-  LSH_TRY(cudaStreamCreateWithFlags(&sg.s, cudaStreamNonBlocking));
-  cudaStream_t s = sg.s;
+  HostCall c;
+  PROPAGATE(c.begin(device));
+  cudaStream_t s = c.s;
   float* d_x;
   double *d_uv, *d_b, *d_keys, *d_dist;
   int32_t *d_ids, *d_oid, *d_cnt;
-  if (int rc = hash_rows(sc, s, vectors, n, dim, unit_vectors, num_tables, bucket_length, &d_x, &d_uv, &d_b))
-    return rc;
-  LSH_TRY(sc.alloc(&d_ids, n)); LSH_TRY(sc.alloc(&d_keys, (int64_t)num_keys * dim));
-  LSH_TRY(sc.alloc(&d_oid, (int64_t)num_keys * k)); LSH_TRY(sc.alloc(&d_dist, (int64_t)num_keys * k));
-  LSH_TRY(sc.alloc(&d_cnt, num_keys));
-  if (n) LSH_TRY(cudaMemcpyAsync(d_ids, ids, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-  LSH_TRY(cudaMemcpyAsync(d_keys, keys, sizeof(double) * num_keys * dim, cudaMemcpyHostToDevice, s));
+  PROPAGATE(hash_rows(c, vectors, n, dim, unit_vectors, num_tables, bucket_length, &d_x, &d_uv, &d_b));
+  PROPAGATE(c.upload(&d_ids, ids, n));
+  PROPAGATE(c.upload(&d_keys, keys, (int64_t)num_keys * dim));
+  CUDA_TRY(c.sc.alloc(&d_oid, (int64_t)num_keys * k)); CUDA_TRY(c.sc.alloc(&d_dist, (int64_t)num_keys * k));
+  CUDA_TRY(c.sc.alloc(&d_cnt, num_keys));
   const size_t smem = sizeof(Entry) * kQueryWarps * k + sizeof(double) * (dim + num_tables);
-  LSH_TRY(cudaFuncSetAttribute(lsh_query_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CUDA_TRY(cudaFuncSetAttribute(lsh_query_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   lsh_query_kernel<<<num_keys, kQueryWarps * 32, smem, s>>>(d_ids, d_x, d_b, (int)n, dim, d_uv, num_tables,
                                                              bucket_length, d_keys, k, d_oid, d_dist, d_cnt);
-  LSH_LAUNCHED();
-  LSH_TRY(cudaMemcpyAsync(out_ids, d_oid, sizeof(int32_t) * num_keys * k, cudaMemcpyDeviceToHost, s));
-  LSH_TRY(cudaMemcpyAsync(out_dist, d_dist, sizeof(double) * num_keys * k, cudaMemcpyDeviceToHost, s));
-  LSH_TRY(cudaMemcpyAsync(out_count, d_cnt, sizeof(int32_t) * num_keys, cudaMemcpyDeviceToHost, s));
-  LSH_TRY(cudaStreamSynchronize(s));
+  LAUNCHED();
+  CUDA_TRY(cudaMemcpyAsync(out_ids, d_oid, sizeof(int32_t) * num_keys * k, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(out_dist, d_dist, sizeof(double) * num_keys * k, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(out_count, d_cnt, sizeof(int32_t) * num_keys, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   return SRS_OK;
 }

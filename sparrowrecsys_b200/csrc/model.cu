@@ -13,7 +13,7 @@
 #include <vector>
 
 #include "../../include/srs_ctr.h"
-#include "kernels.h"
+#include "hostcall.h"
 
 namespace srs {
 cudaError_t setup_embmlp_attributes();
@@ -46,10 +46,10 @@ int64_t gather_slice_rows(const PeerGather* g);
 using namespace srs;
 
 namespace {
-
 thread_local std::string g_err;
+}  // namespace
 
-int fail(int code, const char* fmt, ...) {
+int srs::failf(int code, const char* fmt, ...) {
   char buf[512];
   va_list ap;
   va_start(ap, fmt);
@@ -58,6 +58,19 @@ int fail(int code, const char* fmt, ...) {
   g_err = buf;
   return code;
 }
+
+int srs::check_device(int device) {
+  int ndev = 0;
+  const cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0)
+    return failf(SRS_ERR_CUDA, "no CUDA device available (%s); this library has no CPU path", cudaGetErrorString(e));
+  if (device < 0 || device >= ndev) return failf(SRS_ERR_INVALID, "device %d out of range", device);
+  return SRS_OK;
+}
+
+namespace {
+
+constexpr auto fail = failf;        // this file's name for it
 
 // Kernel-variant options of the model being created: "key=value;key=value" handed to
 // srs_model_create_ex (keys: din_impl, embmlp_impl, deepfm_impl, zero_copy_scores).  The environment variables SRS_<KEY> remain as a tuning override of last resort.
@@ -78,14 +91,6 @@ const char* opt(const char* key, const char* env_name) {
   }
   return getenv(env_name);
 }
-
-#define CUDA_TRY(expr)                                                                   \
-  do {                                                                                   \
-    cudaError_t e__ = (expr);                                                            \
-    if (e__ != cudaSuccess)                                                              \
-      return fail(SRS_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), \
-                  __FILE__, __LINE__);                                                   \
-  } while (0)
 
 constexpr int kSlots = 4;           // public pipelining slots; slot kSlots is private to
                                     // the synchronous srs_predict_host
@@ -199,12 +204,6 @@ struct srs_metrics {
 namespace {
 inline int* slot_err(srs_model* m, const Slot& s) { return m->err_flag + 1 + (&s - m->slots); }
 }  // namespace
-
-int srs::set_last_error(int code, const char* msg) {
-  g_err = msg;
-  return code;
-}
-
 
 namespace {
 
@@ -939,15 +938,6 @@ int choose_kernel(Builder& B, const char* key, const char* env, bool fits, bool 
     tc = true;
   }
   return tc ? build_tc(B) : SRS_OK;
-}
-
-int check_device(int device) {
-  int ndev = 0;
-  const cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0)
-    return fail(SRS_ERR_CUDA, "no CUDA device available (%s); this library has no CPU path", cudaGetErrorString(e));
-  if (device < 0 || device >= ndev) return fail(SRS_ERR_INVALID, "device %d out of range", device);
-  return SRS_OK;
 }
 
 int64_t bytes_per_inference(const srs_spec& s) {

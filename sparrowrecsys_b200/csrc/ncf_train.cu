@@ -24,14 +24,13 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <string>
 #include <vector>
 
 #include "../../include/srs_ctr.h"
-#include "kernels.h"
+#include "hostcall.h"
 #include "ncf_layers.cuh"
 
 namespace srs {
@@ -272,37 +271,6 @@ struct EpochMetrics {                 // one epoch's history state (the layout o
   MetricsReduce red;
 };
 
-int failf(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  return set_last_error(code, buf);
-}
-
-#define TRAIN_TRY(expr)                                                                           \
-  do {                                                                                            \
-    cudaError_t e__ = (expr);                                                                     \
-    if (e__ != cudaSuccess)                                                                       \
-      return failf(SRS_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, \
-                   __LINE__);                                                                     \
-  } while (0)
-
-// device allocations of one scope, freed when it ends
-struct DeviceScratch {
-  std::vector<void*> ptrs;
-  ~DeviceScratch() { for (void* p : ptrs) cudaFree(p); }
-  template <class T>
-  cudaError_t alloc(T** p, size_t count) {
-    void* q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, std::max<size_t>(count, 1) * sizeof(T));
-    if (e == cudaSuccess) ptrs.push_back(q);
-    *p = static_cast<T*>(q);
-    return e;
-  }
-};
-
 struct TrainTensor {                  // one Keras tensor of a trainer
   std::string name;
   int64_t rows, cols;
@@ -450,7 +418,7 @@ const TrainTensor* trainer_tensor(const srs_trainer* t, const char* name) {
 }
 
 // a DeepFM dataset of n rows on the device
-DeepFmRows deepfm_rows(DeviceScratch& sc, int n, cudaError_t* e) {
+DeepFmRows deepfm_rows(Scratch& sc, int n, cudaError_t* e) {
   DeepFmRows r{};
   *e = sc.alloc(&r.movie, n);
   if (*e == cudaSuccess) *e = sc.alloc(&r.user, n);
@@ -493,7 +461,7 @@ int check_rows(const srs_trainer* t, const srs_batch* batch, const int32_t* labe
 
 // batch->B rows on the device, uploaded on s: the columns the trainer's model reads (NeuralCF: movie and user only)
 // and the labels
-cudaError_t upload_rows(DeviceScratch& sc, bool fm, const srs_batch* b, const int32_t* labels, DeepFmRows* r,
+cudaError_t upload_rows(Scratch& sc, bool fm, const srs_batch* b, const int32_t* labels, DeepFmRows* r,
                         cudaStream_t s) {
   const size_t n = (size_t)b->B;
   cudaError_t e;
@@ -599,11 +567,7 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
       !(h.eps > 0.f && h.eps < 1e30f))
     return failf(SRS_ERR_INVALID, "Adam needs lr > 0, 0 <= beta_1, beta_2 < 1 and epsilon > 0");
   if (n_tensors < 0 || (n_tensors > 0 && !tensors)) return failf(SRS_ERR_INVALID, "null tensors");
-  int ndev = 0;
-  cudaError_t ce = cudaGetDeviceCount(&ndev);
-  if (ce != cudaSuccess || ndev == 0)
-    return failf(SRS_ERR_CUDA, "no CUDA device available (%s); this library has no CPU path", cudaGetErrorString(ce));
-  if (device < 0 || device >= ndev) return failf(SRS_ERR_INVALID, "device %d out of range", device);
+  PROPAGATE(check_device(device));
 
   srs_trainer* t = new srs_trainer();
   t->spec = s;
@@ -653,7 +617,7 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
   }
   if (rc != SRS_OK) { delete t; return rc; }
 
-  ce = cudaSetDevice(device);
+  cudaError_t ce = cudaSetDevice(device);
   if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking);
   for (int k = 0; k < 4 && ce == cudaSuccess; ++k) ce = cudaMalloc(&t->tab[k], t->tab_floats * sizeof(float));
   for (int k = 0; k < 3 && ce == cudaSuccess; ++k) ce = cudaMalloc(&t->blob[k], (size_t)nb * sizeof(float));
@@ -724,48 +688,48 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
     rc = check_rows(t, val_batch, val_labels, "validation data: ");
     if (rc != SRS_OK) return rc;
   }
-  TRAIN_TRY(cudaSetDevice(t->device));
+  CUDA_TRY(cudaSetDevice(t->device));
   const int EP = t->EP, Bmax = std::min(batch_size, n);
   const int n_ent = fm ? kDeepFmTables : 2;            // table entries per row
   const int n_cta = fm ? deepfm_train_ctas(Bmax) : (Bmax + kTrainRows - 1) / kTrainRows;
   cudaStream_t s = t->stream;
-  DeviceScratch sc;
+  Scratch sc;
   int32_t *d_order, *d_trow, *d_lab_b = nullptr, *d_frow = nullptr;
   float *d_probs, *d_logits, *d_gemb, *d_part, *d_fgrad = nullptr;
   int* d_err = nullptr;
   EpochMetrics* d_met;
-  TRAIN_TRY(sc.alloc(&d_order, (size_t)epochs * n));
-  TRAIN_TRY(sc.alloc(&d_trow, (size_t)n_ent * Bmax));
-  TRAIN_TRY(sc.alloc(&d_probs, Bmax));
-  TRAIN_TRY(sc.alloc(&d_logits, Bmax));
-  TRAIN_TRY(sc.alloc(&d_gemb, (size_t)n_ent * Bmax * EP));
-  TRAIN_TRY(sc.alloc(&d_part, (size_t)n_cta * t->blob_floats));
-  TRAIN_TRY(sc.alloc(&d_met, epochs));
-  TRAIN_TRY(cudaMemcpyAsync(d_order, order, (size_t)epochs * n * 4, cudaMemcpyHostToDevice, s));
-  TRAIN_TRY(cudaMemsetAsync(d_met, 0, sizeof(EpochMetrics) * epochs, s));
+  CUDA_TRY(sc.alloc(&d_order, (size_t)epochs * n));
+  CUDA_TRY(sc.alloc(&d_trow, (size_t)n_ent * Bmax));
+  CUDA_TRY(sc.alloc(&d_probs, Bmax));
+  CUDA_TRY(sc.alloc(&d_logits, Bmax));
+  CUDA_TRY(sc.alloc(&d_gemb, (size_t)n_ent * Bmax * EP));
+  CUDA_TRY(sc.alloc(&d_part, (size_t)n_cta * t->blob_floats));
+  CUDA_TRY(sc.alloc(&d_met, epochs));
+  CUDA_TRY(cudaMemcpyAsync(d_order, order, (size_t)epochs * n * 4, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemsetAsync(d_met, 0, sizeof(EpochMetrics) * epochs, s));
   DeepFmRows src{}, rows{};                            // the dataset, and (DeepFM) the epoch's rows in order
-  TRAIN_TRY(upload_rows(sc, fm, batch, labels, &src, s));
+  CUDA_TRY(upload_rows(sc, fm, batch, labels, &src, s));
   if (fm) {
     cudaError_t e;
     rows = deepfm_rows(sc, n, &e);
-    TRAIN_TRY(e);
-    TRAIN_TRY(sc.alloc(&d_frow, 4 * (size_t)Bmax));
-    TRAIN_TRY(sc.alloc(&d_fgrad, 4 * (size_t)Bmax));
-    TRAIN_TRY(sc.alloc(&d_err, 1));
-    TRAIN_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), s));
+    CUDA_TRY(e);
+    CUDA_TRY(sc.alloc(&d_frow, 4 * (size_t)Bmax));
+    CUDA_TRY(sc.alloc(&d_fgrad, 4 * (size_t)Bmax));
+    CUDA_TRY(sc.alloc(&d_err, 1));
+    CUDA_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), s));
   } else {
-    TRAIN_TRY(sc.alloc(&d_lab_b, Bmax));
+    CUDA_TRY(sc.alloc(&d_lab_b, Bmax));
   }
   // validation: its rows uploaded once, in file order; each validated epoch's metrics in its own state
   DeepFmRows vrows{};
   float *d_vprobs = nullptr, *d_vlogits = nullptr;
   EpochMetrics* d_vmet = nullptr;
   if (nv) {
-    TRAIN_TRY(upload_rows(sc, fm, val_batch, val_labels, &vrows, s));
-    TRAIN_TRY(sc.alloc(&d_vprobs, nv));
-    TRAIN_TRY(sc.alloc(&d_vlogits, nv));
-    TRAIN_TRY(sc.alloc(&d_vmet, epochs));
-    TRAIN_TRY(cudaMemsetAsync(d_vmet, 0, sizeof(EpochMetrics) * epochs, s));
+    CUDA_TRY(upload_rows(sc, fm, val_batch, val_labels, &vrows, s));
+    CUDA_TRY(sc.alloc(&d_vprobs, nv));
+    CUDA_TRY(sc.alloc(&d_vlogits, nv));
+    CUDA_TRY(sc.alloc(&d_vmet, epochs));
+    CUDA_TRY(cudaMemsetAsync(d_vmet, 0, sizeof(EpochMetrics) * epochs, s));
   }
 
   int dev_sms = 132;
@@ -787,7 +751,7 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
   }
   int64_t steps = 0;
   for (int e = 0; e < epochs; ++e) {
-    if (fm) TRAIN_TRY(launch_deepfm_permute(src, rows, d_order + (size_t)e * n, n, s));
+    if (fm) CUDA_TRY(launch_deepfm_permute(src, rows, d_order + (size_t)e * n, n, s));
     for (int off = 0; off < n; off += batch_size) {
       const int B = std::min(batch_size, n - off);
       const int32_t* step_labels;
@@ -798,7 +762,7 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
         f.b.numerics = rows.numerics + (size_t)off * kNumNumerics;
         f.label = rows.label + off;
         step_labels = f.label;
-        TRAIN_TRY(launch_deepfm_train_step(f, s));
+        CUDA_TRY(launch_deepfm_train_step(f, s));
         table_grad_kernel<<<(kDeepFmTables * B + 127) / 128, 128, 0, s>>>(d_trow, d_gemb, kDeepFmTables * B, EP,
                                                                           t->tab[3]);
         table_grad_kernel<<<(4 * B + 127) / 128, 128, 0, s>>>(d_frow, d_fgrad, 4 * B, 1, t->fo[3]);
@@ -813,7 +777,7 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
         a.B = B;
         a.order = d_order + (size_t)e * n + off;
         step_labels = d_lab_b;
-        TRAIN_TRY(launch_step(EP, t->HP, a, t->ly, s));
+        CUDA_TRY(launch_step(EP, t->HP, a, t->ly, s));
         table_grad_kernel<<<(2 * a.B + 127) / 128, 128, 0, s>>>(d_trow, d_gemb, 2 * a.B, EP, t->tab[3]);
         table_adam_kernel<false><<<adam_blocks, 256, 0, s>>>(t->tab[0], t->tab[1], t->tab[2], t->tab[3],
                                                              t->tab_floats, t->hp, t->d_it);
@@ -821,18 +785,18 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
                                                      t->blob[0], t->blob[1], t->blob[2], t->hp, t->d_it);
         g_launch_count += 3;
       }
-      TRAIN_TRY(cudaGetLastError());
-      TRAIN_TRY(launch_metrics_update(d_probs, d_logits, step_labels, B, &d_met[e].cnt, &d_met[e].red, &d_met[e].loss,
+      CUDA_TRY(cudaGetLastError());
+      CUDA_TRY(launch_metrics_update(d_probs, d_logits, step_labels, B, &d_met[e].cnt, &d_met[e].red, &d_met[e].loss,
                                       1, s));
       ++steps;
     }
     // after the epoch's last update, on the same stream: no host synchronisation
-    if (nv && (e + 1) % val_freq == 0) TRAIN_TRY(eval_rows(t, vrows, nv, d_vprobs, d_vlogits, d_err, &d_vmet[e], s));
+    if (nv && (e + 1) % val_freq == 0) CUDA_TRY(eval_rows(t, vrows, nv, d_vprobs, d_vlogits, d_err, &d_vmet[e], s));
   }
   std::vector<EpochMetrics> met(epochs), vmet(nv ? epochs : 0);
-  TRAIN_TRY(cudaMemcpyAsync(met.data(), d_met, sizeof(EpochMetrics) * epochs, cudaMemcpyDeviceToHost, s));
-  if (nv) TRAIN_TRY(cudaMemcpyAsync(vmet.data(), d_vmet, sizeof(EpochMetrics) * epochs, cudaMemcpyDeviceToHost, s));
-  TRAIN_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(met.data(), d_met, sizeof(EpochMetrics) * epochs, cudaMemcpyDeviceToHost, s));
+  if (nv) CUDA_TRY(cudaMemcpyAsync(vmet.data(), d_vmet, sizeof(EpochMetrics) * epochs, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   t->iterations += steps;
   for (int e = 0; e < epochs; ++e) {
     const bool validated = nv && (e + 1) % val_freq == 0;
@@ -855,24 +819,24 @@ int srs_trainer_evaluate_host(srs_trainer* t, const srs_batch* batch, const int3
   if (n < 1) return failf(SRS_ERR_INVALID, "evaluate needs at least one row");
   const int rc = check_rows(t, batch, labels, "");
   if (rc != SRS_OK) return rc;
-  TRAIN_TRY(cudaSetDevice(t->device));
+  CUDA_TRY(cudaSetDevice(t->device));
   cudaStream_t s = t->stream;
-  DeviceScratch sc;
+  Scratch sc;
   DeepFmRows rows{};
   float *d_probs, *d_logits;
   int* d_err;
   EpochMetrics* d_met;
-  TRAIN_TRY(upload_rows(sc, t->spec.kind == SRS_DEEPFM, batch, labels, &rows, s));
-  TRAIN_TRY(sc.alloc(&d_probs, n));
-  TRAIN_TRY(sc.alloc(&d_logits, n));
-  TRAIN_TRY(sc.alloc(&d_err, 1));
-  TRAIN_TRY(sc.alloc(&d_met, 1));
-  TRAIN_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), s));
-  TRAIN_TRY(cudaMemsetAsync(d_met, 0, sizeof(EpochMetrics), s));
-  TRAIN_TRY(eval_rows(t, rows, n, d_probs, d_logits, d_err, d_met, s));
+  CUDA_TRY(upload_rows(sc, t->spec.kind == SRS_DEEPFM, batch, labels, &rows, s));
+  CUDA_TRY(sc.alloc(&d_probs, n));
+  CUDA_TRY(sc.alloc(&d_logits, n));
+  CUDA_TRY(sc.alloc(&d_err, 1));
+  CUDA_TRY(sc.alloc(&d_met, 1));
+  CUDA_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), s));
+  CUDA_TRY(cudaMemsetAsync(d_met, 0, sizeof(EpochMetrics), s));
+  CUDA_TRY(eval_rows(t, rows, n, d_probs, d_logits, d_err, d_met, s));
   EpochMetrics met;
-  TRAIN_TRY(cudaMemcpyAsync(&met, d_met, sizeof(met), cudaMemcpyDeviceToHost, s));
-  TRAIN_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(cudaMemcpyAsync(&met, d_met, sizeof(met), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
   if (met.cnt.err) return failf(SRS_ERR_INVALID, "evaluate produced a probability that is NaN or outside [0, 1]");
   metrics_summarise(met.cnt.hist, met.cnt.correct, met.loss, out, nullptr);
   return SRS_OK;
@@ -882,19 +846,19 @@ int srs_trainer_get_weights(const srs_trainer* t, const char* name, float* dst) 
   if (!t || !name || !dst) return failf(SRS_ERR_INVALID, "null argument");
   const TrainTensor* x = trainer_tensor(t, name);
   if (!x) return failf(SRS_ERR_MISSING, "the trainer has no tensor '%s'", name);
-  TRAIN_TRY(cudaSetDevice(t->device));
-  TRAIN_TRY(cudaStreamSynchronize(t->stream));
+  CUDA_TRY(cudaSetDevice(t->device));
+  CUDA_TRY(cudaStreamSynchronize(t->stream));
   if (x->row0 >= 0) {
-    TRAIN_TRY(cudaMemcpy2D(dst, (size_t)x->cols * sizeof(float), t->tab[0] + x->row0 * t->EP,
+    CUDA_TRY(cudaMemcpy2D(dst, (size_t)x->cols * sizeof(float), t->tab[0] + x->row0 * t->EP,
                            (size_t)t->EP * sizeof(float), (size_t)x->cols * sizeof(float), (size_t)x->rows,
                            cudaMemcpyDeviceToHost));
     return SRS_OK;
   }
   std::vector<float> blob(t->blob_floats), onehot;
-  TRAIN_TRY(cudaMemcpy(blob.data(), t->blob[0], blob.size() * sizeof(float), cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(blob.data(), t->blob[0], blob.size() * sizeof(float), cudaMemcpyDeviceToHost));
   if (t->onehot && std::any_of(x->at.begin(), x->at.end(), [](int64_t i) { return i < 0; })) {
     onehot.resize(t->onehot);
-    TRAIN_TRY(cudaMemcpy(onehot.data(), t->fo[0], onehot.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(onehot.data(), t->fo[0], onehot.size() * sizeof(float), cudaMemcpyDeviceToHost));
   }
   for (size_t i = 0; i < x->at.size(); ++i) dst[i] = x->at[i] >= 0 ? blob[x->at[i]] : onehot[-1 - x->at[i]];
   return SRS_OK;

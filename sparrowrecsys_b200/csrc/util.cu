@@ -1,11 +1,11 @@
 // util.cu - small device utilities around the forward path.
-#include "kernels.h"
+#include "hostcall.h"
 
 namespace srs {
 
 int64_t g_launch_count = 0;
 
-// Counter-based uniform fill (splitmix64 of seed + (i+1)*golden): the synthetic
+// Counter-based uniform fill (splitmix(seed, i)): the synthetic
 // 10^8-row movie table of BASELINE cfg 5 is generated in place in HBM; the oracle
 // regenerates any row it needs from the same formula.
 __global__ void fill_uniform_kernel(float* __restrict__ x, int64_t n, uint64_t seed, float lo,
@@ -13,11 +13,7 @@ __global__ void fill_uniform_kernel(float* __restrict__ x, int64_t n, uint64_t s
   const float span = hi - lo;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (int64_t)gridDim.x * blockDim.x) {
-    uint64_t z = seed + (uint64_t)(i + 1) * 0x9E3779B97F4A7C15ULL;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-    z = z ^ (z >> 31);
-    const float u = (float)(uint32_t)(z >> 40) * (1.0f / 16777216.0f);
+    const float u = (float)(uint32_t)(splitmix(seed, (uint64_t)i) >> 40) * (1.0f / 16777216.0f);
     x[i] = __fadd_rn(lo, __fmul_rn(span, u));
   }
 }
