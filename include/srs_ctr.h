@@ -591,6 +591,18 @@ int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id, const floa
                      int32_t* user_ids, float* user_factors, int32_t* n_users, int32_t* movie_ids,
                      float* movie_factors, int32_t* n_movies);
 
+/* ALS.fit with implicitPrefs (DESIGN.md section 4.17): srs_als_fit_host's arguments, layouts, init, order and
+ * solve, with `alpha` (finite, >= 0; Spark's default 1.0).  Before each half-step, YtY = the sum of y y^T over every
+ * source factor, in double: each of Spark's ten blocks (raw id mod 10, ascending id) summed from zero, then the
+ * blocks added in block order.  Each entity's system starts from YtY; each rating r adds c1 y y^T (c1 = alpha |r|)
+ * and, when r > 0, (1 + c1) y to the right-hand side; reg_param * (its count of ratings > 0) goes on the diagonal.
+ * Checks, errors and outputs as srs_als_fit_host's (alpha's before any device call).  Synchronous; the same inputs
+ * give the same bits. */
+int srs_als_fit_implicit_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
+                              int64_t n_ratings, const srs_als_params* params, int32_t device, int32_t user_capacity,
+                              int32_t movie_capacity, int32_t* user_ids, float* user_factors, int32_t* n_users,
+                              int32_t* movie_ids, float* movie_factors, int32_t* n_movies, double alpha);
+
 /* Many ALS fits over one rating set in one pass (CrossValidator's fold x grid models, DESIGN.md section 4.15).
  * fold [n_ratings] gives each rating a fold in 0..n_folds-1 (2 <= n_folds <= 65536).  Model m of the n_models
  * (1..64) trains on the ratings outside fold models[m].exclude_fold (-1: on all of them) with its own rank,
@@ -622,6 +634,17 @@ int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* movie_id, cons
 int srs_als_recommend_host(const float* src_factors, int32_t n_src, const int32_t* dst_ids, const float* dst_factors,
                            int32_t n_dst, int32_t rank, int32_t num, int32_t device, int32_t* out_ids,
                            float* out_scores);
+
+/* mllib RankingMetrics (Spark 2.4) over n_queries queries: pred_ids [n_queries][pred_len] best first, and query q's
+ * relevant ids label_ids[label_off[q] .. label_off[q + 1]) (a set: duplicates count once).  Per query, with
+ * |lab| its distinct labels: precision@k = hits in the first min(pred_len, k) / k; NDCG@k = dcg / maxDcg over
+ * i < min(max(pred_len, |lab|), k) with gain 1 / ln(i + 2), dcg taking the hits and maxDcg the first |lab|
+ * positions; average precision = the sum over every hit of (hits so far) / (i + 1), over |lab|.  An empty label
+ * set scores 0.  means [3] = precision@k, NDCG@k, MAP: StatCounter's mu += (x - mu) / n in query order (NaN for no
+ * query); per_query [3][n_queries], when not null, the values.  k >= 1, label_off[0] = 0 and non-decreasing;
+ * checked before any device call (SRS_ERR_INVALID).  Synchronous; the same inputs give the same bits. */
+int srs_ranking_metrics_host(const int32_t* pred_ids, int32_t n_queries, int32_t pred_len, const int32_t* label_off,
+                             const int32_t* label_ids, int32_t k, int32_t device, double* per_query, double* means);
 
 /* ---- The FeatureEngineering job and the sample split on the device (DESIGN.md section 4.16) ----
  * Every entry checks its inputs before any device call (SRS_ERR_INVALID) and writes its outputs only on success.

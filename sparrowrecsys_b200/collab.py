@@ -1,4 +1,5 @@
-"""Collaborative filtering on the GPU: ALS factors, test RMSE and top-k recommendations.
+"""Collaborative filtering on the GPU: ALS factors (explicit or implicit feedback), test RMSE or ranking metrics,
+and top-k recommendations.
 
 This is the reference's Spark job `OFF/model/CollaborativeFiltering.scala` (and its PySpark twin): split ratings.csv
 0.8 / 0.2, train Spark ML's `ALS` (explicit feedback, maxIter 5, regParam 0.01, rank 10) on the first part, take
@@ -12,8 +13,11 @@ them.
 * `AlsModel.recommend_for_*` score and keep the top `num` on one device (`srs_als_recommend_host`).
 * `cross_validate` is the job's last step, `CrossValidator` over a `ParamGridBuilder` grid: every fold x grid model
   trained in one batched device pass (`als_folds`, `srs_als_fit_folds_host`; DESIGN.md section 4.15).
+* `als(..., implicit_prefs=True, alpha=...)` is the estimator's implicit-feedback mode (`srs_als_fit_implicit_host`),
+  and `ranking_metrics` / `AlsModel.ranking_metrics` are mllib's `RankingMetrics` - precision@k, NDCG@k and MAP -
+  with the per-query values on the device (`srs_ranking_metrics_host`; DESIGN.md section 4.17).
 
-    python -m sparrowrecsys_b200.collab ratings.csv [--cv]
+    python -m sparrowrecsys_b200.collab ratings.csv [--cv | --implicit [--alpha A]]
 """
 from __future__ import annotations
 
@@ -130,6 +134,33 @@ class AlsModel:
         ids, sc = recommend(self.item_factors, self.user_ids, self.user_factors, num, self.device)
         return self.item_ids, ids, sc
 
+    def ranking_queries(self, ratings: Mapping[str, np.ndarray], threshold: float = 0.0):
+        """The queries of `ranking_metrics`: (the users of `ratings` that have factors, ascending; their rows in
+        user_factors; a CSR tuple (offsets, movie ids) of each one's movies rated above `threshold`)."""
+        user = np.asarray(ratings["userId"], np.int64)
+        movie = np.asarray(ratings["movieId"], np.int64)
+        rel = np.asarray(ratings["rating"], np.float32) > np.float32(threshold)
+        at = self._subset(user, self.user_ids)
+        order = np.lexsort((movie, user))
+        user, movie = user[order][rel[order]], movie[order][rel[order]]
+        users = self.user_ids[at].astype(np.int64)
+        lo = np.searchsorted(user, users, "left")
+        hi = np.searchsorted(user, users, "right")
+        off = np.zeros(len(users) + 1, np.int32)
+        off[1:] = np.cumsum(hi - lo)
+        ids = np.concatenate([movie[a:b] for a, b in zip(lo, hi)]) if len(users) else np.zeros(0)
+        return self.user_ids[at], at, (off, ids.astype(np.int32))
+
+    def ranking_metrics(self, ratings: Mapping[str, np.ndarray], k: int, threshold: float = 0.0) -> dict:
+        """RankingMetrics of recommend_for_user_subset(users, k) against held-out `ratings` (Spark 2.4 has no
+        ranking evaluator for ALS; this is how its users score implicit models): the queries are the users of
+        `ratings` that have factors, ascending; each one's relevant items are its movies rated above `threshold`
+        (preference [rating > 0] by default; a movie without a factor stays relevant and is never recommended).  A
+        user with none scores 0 and still counts.  Returns `ranking_metrics`' dict."""
+        users, _, labels = self.ranking_queries(ratings, threshold)
+        _, pred, _ = self.recommend_for_user_subset(users, k)
+        return ranking_metrics(pred, labels, k, self.device)
+
     @staticmethod
     def _subset(ids, known):
         q = np.unique(np.asarray(ids, np.int64))
@@ -152,10 +183,11 @@ class AlsModel:
 
 
 def als(ratings: Mapping[str, np.ndarray], rank: int = 10, max_iter: int = 5, reg_param: float = 0.01,
-        seed: int = 0, device: int = 0) -> AlsModel:
-    """ALS.fit (explicit feedback) on `ratings` (userId, movieId, rating; as `featureeng.load_ratings_csv` returns)
-    on `device`.  Ratings are cast to float32 as Spark casts its rating column.  The same inputs give the same
-    bits."""
+        seed: int = 0, device: int = 0, implicit_prefs: bool = False, alpha: float = 1.0) -> AlsModel:
+    """ALS.fit on `ratings` (userId, movieId, rating; as `featureeng.load_ratings_csv` returns) on `device`:
+    explicit feedback, or with `implicit_prefs` the implicit mode with confidence 1 + alpha |rating| and
+    preference [rating > 0] (DESIGN.md section 4.17).  Ratings are cast to float32 as Spark casts its rating
+    column.  The same inputs give the same bits."""
     user = np.ascontiguousarray(ratings["userId"], np.int32)
     movie = np.ascontiguousarray(ratings["movieId"], np.int32)
     rating = np.ascontiguousarray(ratings["rating"], np.float32)
@@ -168,10 +200,44 @@ def als(ratings: Mapping[str, np.ndarray], rank: int = 10, max_iter: int = 5, re
     mids, mf = np.zeros(cm, np.int32), np.zeros((cm, max(k, 1)), np.float32)
     params = _lib.SrsAlsParams(k, int(max_iter), float(reg_param), int(seed) & _M64)
     nu, nm = C.c_int32(0), C.c_int32(0)
-    _lib.check(_lib.load().srs_als_fit_host(_p(user), _p(movie), _p(rating), n, C.byref(params), device, cu, cm,
-                                            _p(uids), _p(uf), C.byref(nu), _p(mids), _p(mf), C.byref(nm)))
+    args = (_p(user), _p(movie), _p(rating), n, C.byref(params), device, cu, cm, _p(uids), _p(uf), C.byref(nu),
+            _p(mids), _p(mf), C.byref(nm))
+    if implicit_prefs:
+        _lib.check(_lib.load().srs_als_fit_implicit_host(*args, float(alpha)))
+    else:
+        _lib.check(_lib.load().srs_als_fit_host(*args))
     return AlsModel(uids[:nu.value].copy(), uf[:nu.value].copy(), mids[:nm.value].copy(), mf[:nm.value].copy(),
                     device)
+
+
+def ranking_metrics(pred_ids, labels, k: int, device: int = 0) -> dict:
+    """mllib RankingMetrics (Spark 2.4) on the device: `pred_ids` [n][L] best first, `labels` the relevant ids of
+    each query - a list of n sequences, or a CSR tuple (offsets [n + 1], ids) - taken as sets.  Returns
+    precision_at_k (hits in the first min(L, k) over k), ndcg_at_k and mean_average_precision (over the whole
+    list, as Spark 2.4's is), each StatCounter's mean over the queries in order; an empty label set scores 0."""
+    pred = np.ascontiguousarray(pred_ids, np.int32)
+    if pred.ndim == 1 and pred.size == 0:
+        pred = pred.reshape(0, 0)
+    if pred.ndim != 2:
+        raise ValueError("pred_ids must be [n_queries][L]")
+    if isinstance(labels, tuple):
+        off, ids = (np.ascontiguousarray(x, np.int32) for x in labels)
+        if off.shape != (pred.shape[0] + 1,) or ids.ndim != 1 or (len(off) and (off[0] != 0 or off[-1] != len(ids))):
+            raise ValueError("CSR labels need offsets [n + 1] from 0 to len(ids)")
+    else:
+        if len(labels) != pred.shape[0]:
+            raise ValueError("%d label sets for %d queries" % (len(labels), pred.shape[0]))
+        sizes = [len(x) for x in labels]
+        off = np.zeros(len(sizes) + 1, np.int32)
+        off[1:] = np.cumsum(sizes)
+        ids = np.ascontiguousarray(np.concatenate([np.asarray(x, np.int64) for x in labels]) if sizes
+                                   else np.zeros(0), np.int32)
+    means = np.zeros(3)
+    _lib.check(_lib.load().srs_ranking_metrics_host(_p(pred), pred.shape[0], pred.shape[1], _p(off),
+                                                    _p(ids if ids.size else np.zeros(1, np.int32)), int(k), device,
+                                                    None, _p(means)))
+    return {"precision_at_k": float(means[0]), "ndcg_at_k": float(means[1]),
+            "mean_average_precision": float(means[2])}
 
 
 MAX_BATCH_MODELS = 64
@@ -381,25 +447,44 @@ def _show(title, ids, rec, sc, rows=10):
 
 
 def main(argv=None) -> int:
-    argv = sys.argv[1:] if argv is None else argv
-    cv = "--cv" in argv
-    args = [a for a in argv if a != "--cv"]
-    if len(args) != 1:
-        sys.stderr.write("usage: python -m sparrowrecsys_b200.collab ratings.csv [--cv]\n")
+    argv = list(sys.argv[1:] if argv is None else argv)
+    usage = "usage: python -m sparrowrecsys_b200.collab ratings.csv [--cv | --implicit [--alpha A]]\n"
+    alpha = 1.0
+    if "--alpha" in argv:
+        at = argv.index("--alpha")
+        try:
+            alpha = float(argv[at + 1])
+        except (IndexError, ValueError):
+            sys.stderr.write(usage)
+            return 2
+        del argv[at:at + 2]
+        if "--implicit" not in argv:
+            sys.stderr.write(usage)
+            return 2
+    cv, implicit = "--cv" in argv, "--implicit" in argv
+    args = [a for a in argv if a not in ("--cv", "--implicit")]
+    if len(args) != 1 or (cv and implicit):                 # CrossValidator has no ranking evaluator
+        sys.stderr.write(usage)
         return 2
     from .featureeng import load_ratings_csv
     r = load_ratings_csv(args[0])
     train_rows, test_rows = random_split(len(r["userId"]), (0.8, 0.2), seed=0)
     train = {k: v[train_rows] for k, v in r.items()}
     test = {k: v[test_rows] for k, v in r.items()}
-    model = als(train, rank=10, max_iter=5, reg_param=0.01, seed=0)
+    model = als(train, rank=10, max_iter=5, reg_param=0.01, seed=0, implicit_prefs=implicit, alpha=alpha)
     for name, ids, f in (("itemFactors", model.item_ids, model.item_factors),
                          ("userFactors", model.user_ids, model.user_factors)):
         print(name)
         for i in range(min(10, len(ids))):
             print("%d\t[%s]" % (ids[i], ", ".join(repr(float(v)) for v in f[i])))
-    kept, pred = model.transform(test)
-    print("Root-mean-square error = %r" % rmse(test["rating"][kept], pred))
+    if implicit:                                            # preferences, not ratings: rank the held-out items
+        m = model.ranking_metrics(test, 10)
+        print("precisionAt(10) = %r" % m["precision_at_k"])
+        print("ndcgAt(10) = %r" % m["ndcg_at_k"])
+        print("meanAveragePrecision = %r" % m["mean_average_precision"])
+    else:
+        kept, pred = model.transform(test)
+        print("Root-mean-square error = %r" % rmse(test["rating"][kept], pred))
     _show("userRecs", *model.recommend_for_all_users(10))
     _show("movieRecs", *model.recommend_for_all_items(10))
     _, first_users = np.unique(r["userId"], return_index=True)

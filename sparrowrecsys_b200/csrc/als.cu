@@ -1,6 +1,7 @@
-// als.cu - the reference's CollaborativeFiltering job (Spark ML ALS, explicit feedback) on one device: the factors
-// from double-precision normal equations solved by Cholesky, and the fused top-k recommendations.  DESIGN.md
-// section 4.13 gives the semantics, the orders Spark leaves open and the bounds.
+// als.cu - the reference's CollaborativeFiltering job (Spark ML ALS, explicit or implicit feedback) on one device:
+// the factors from double-precision normal equations solved by Cholesky, the fused top-k recommendations and the
+// ranking metrics that score them.  DESIGN.md sections 4.13 and 4.17 give the semantics, the orders Spark leaves
+// open and the bounds.
 //
 // srs_als_fit_host, on one stream, inputs uploaded once:
 //   1. four stable radix sorts: by user and by movie (the dense, ascending ids: run-length encodings), then the
@@ -21,6 +22,15 @@
 // excluded fold - over one rating set: the layouts of steps 1-2 once, each rating's fold gathered into both, then one
 // als_solve_kernel<true> launch per half-step for every model.  A fold's subset of a layout keeps its order, so
 // each model's results are bit for bit srs_als_fit_host's on its training ratings.
+//
+// srs_als_fit_implicit_host (DESIGN.md section 4.17) is the same fit with Spark's implicitPrefs: before each
+// half-step als_yty_kernel sums YtY over the source factors in Spark's ten blocks (entity id mod 10, ascending id;
+// one block of elements per thread slice, each element owned by one thread), als_yty_merge_kernel adds the blocks
+// in block order, and als_solve_kernel<false, true> starts each entity's ata from YtY and adds each rating's
+// confidence and preference terms.
+//
+// srs_ranking_metrics_host: RankingMetrics' per-query precision@k, NDCG@k and average precision, one warp per
+// query (ranking_metrics_kernel), over each query's labels sorted on the device; the means on the host.
 //
 // als_recommend_kernel (srs_als_recommend_host): 32 sources per block, 4 per warp; destinations stream through
 // shared memory in tiles of 128, transposed so that each lane reads its own 4.  Each lane computes 4 x 4 exact
@@ -53,6 +63,9 @@ constexpr int kSrcPerWarp = 4;
 constexpr int kSrcPerBlock = kRecWarps * kSrcPerWarp;
 constexpr int kTile = 128;             // destinations per shared-memory tile, 4 per lane
 constexpr unsigned kFull = 0xffffffffu;
+constexpr int kYtyBlocks = 10;         // Spark's default number of ALS blocks
+constexpr int kYtyThreads = 128;       // packed YtY elements per thread slice
+constexpr int kRankWarps = 8;          // queries per block of ranking_metrics_kernel
 
 // The initial factor of the user with id `user`: `rank` draws of java.util.Random.nextGaussian's polar method on
 // uniforms uniform53(splitmix(seed, user), c), each cast to float, then scaled by
@@ -146,15 +159,24 @@ struct Batch {
   bool to_users;                       // this half-step solves the users from the movies
 };
 
+// The implicit-feedback settings of a half-step (srs_als_fit_implicit_host)
+struct Implicit {
+  const double* yty;                   // [k (k + 1) / 2] packed YtY of the source factors
+  double alpha;
+};
+
 // One block per entity (the blockIdx.x-th longest; batched: block b is model b % M's (b / M)-th longest entity):
 // NormalEquation.add over its ratings, then CholeskySolver.solve(ne, n * regParam) (dppsv "U": dpptrf, then
 // dpptrs's two dtpsv).  A batched model skips its excluded fold's ratings, so its n counts the rest; an entity with
-// none is not in that model and its block writes nothing but the count.
-template <bool kBatch>
+// none is not in that model and its block writes nothing but the count.  Implicit: ata starts as YtY, each rating
+// adds dspr(c1) and, when positive, daxpy(1 + c1) (c1 = alpha |r|), and n counts the positive ratings.
+template <bool kBatch, bool kImplicit = false>
 __global__ void __launch_bounds__(kSolveThreads) als_solve_kernel(Side sd, const float* __restrict__ srcF,
                                                                   float* __restrict__ dstF, int k, double reg,
                                                                   unsigned long long* __restrict__ err,
-                                                                  unsigned long long half_step, Batch bt) {
+                                                                  unsigned long long half_step, Batch bt,
+                                                                  Implicit im) {
+  static_assert(!(kBatch && kImplicit), "the batched fit is explicit only");
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ uint8_t s_keep[kChunk];
   int m = 0, exclude = -1, pos = blockIdx.x;
@@ -190,9 +212,9 @@ __global__ void __launch_bounds__(kSolveThreads) als_solve_kernel(Side sd, const
     s_j[e] = (uint8_t)j;
     s_i[e] = (uint8_t)(e - j * (j + 1) / 2);
   }
-  for (int e = tid; e < nA + k; e += kSolveThreads) P[e] = 0.0;
+  for (int e = tid; e < nA + k; e += kSolveThreads) P[e] = kImplicit && e < nA ? im.yty[e] : 0.0;   // merge(YtY)
   if (tid == 0) s_bad = 0;
-  if (kBatch) n_train = 0;
+  if (kBatch || kImplicit) n_train = 0;
   for (int lo = lo0; lo < hi; lo += kChunk) {
     const int cn = min(kChunk, hi - lo);
     __syncthreads();                                    // the previous chunk is consumed
@@ -207,9 +229,30 @@ __global__ void __launch_bounds__(kSolveThreads) als_solve_kernel(Side sd, const
     __syncthreads();
     if (kBatch)
       for (int c = 0; c < cn; ++c) n_train += s_keep[c];
+    if (kImplicit)
+      for (int c = 0; c < cn; ++c) n_train += s_r[c] > 0.0f;   // numExplicits
     for (int e = tid; e < nA + k; e += kSolveThreads) {
       double a = P[e];
-      if (e < nA) {                                     // dspr: ap(i,j) += x(i) * (1.0 * x(j)), skipped for x(j) == 0
+      if (kImplicit) {
+        if (e < nA) {                                   // dspr(c1): ap(i,j) += x(i) * (c1 * x(j)); none when c1 == 0
+          const int i = s_i[e], j = s_j[e];
+          for (int c = 0; c < cn; ++c) {
+            const double c1 = __dmul_rn(im.alpha, (double)fabsf(s_r[c]));
+            const float xj = s_x[c * k + j];
+            if (c1 != 0.0 && xj != 0.0f)
+              a = __dadd_rn(a, __dmul_rn((double)s_x[c * k + i], __dmul_rn(c1, (double)xj)));
+          }
+        } else {                                        // daxpy(1 + c1): atb(i) += (1 + c1) * x(i), for rating > 0
+          const int i = e - nA;
+          for (int c = 0; c < cn; ++c) {
+            const float rv = s_r[c];
+            if (rv > 0.0f) {
+              const double b = __dadd_rn(1.0, __dmul_rn(im.alpha, (double)rv));
+              a = __dadd_rn(a, __dmul_rn(b, (double)s_x[c * k + i]));
+            }
+          }
+        }
+      } else if (e < nA) {                              // dspr: ap(i,j) += x(i) * (1.0 * x(j)), skipped for x(j) == 0
         const int i = s_i[e], j = s_j[e];
         for (int c = 0; c < cn; ++c) {
           if (kBatch && !s_keep[c]) continue;
@@ -282,6 +325,49 @@ __global__ void __launch_bounds__(kSolveThreads) als_solve_kernel(Side sd, const
     if (c < j && s_nz[j]) x = __dsub_rn(x, __dmul_rn(s_y[j], P[j * (j + 1) / 2 + c]));
   }
   if (c < k) dstF[(size_t)ent * k + c] = __double2float_rn(x);
+}
+
+// Spark's computeYtY: block b = blockIdx.y of the ten sums NormalEquation.add(y, 0.0) - dspr("U", k, 1.0, y, ap),
+// skipped for y(j) == 0 - over its source entities members[boff[b] .. boff[b + 1]) (ascending id), from zero in
+// double; thread blockIdx.x * kYtyThreads + threadIdx.x owns one packed element.  part [10][nA].
+__global__ void __launch_bounds__(kYtyThreads) als_yty_kernel(const float* __restrict__ srcF, int k,
+                                                              const int32_t* __restrict__ members,
+                                                              const int32_t* __restrict__ boff,
+                                                              double* __restrict__ part) {
+  __shared__ float s_x[kChunk * kMaxRank];
+  const int nA = k * (k + 1) / 2, b = blockIdx.y, tid = threadIdx.x;
+  const int e = blockIdx.x * kYtyThreads + tid;
+  int i = 0, j = 0;
+  if (e < nA) {
+    while ((j + 1) * (j + 2) / 2 <= e) ++j;
+    i = e - j * (j + 1) / 2;
+  }
+  double a = 0.0;
+  const int hi = boff[b + 1];
+  for (int lo = boff[b]; lo < hi; lo += kChunk) {
+    const int cn = min(kChunk, hi - lo);
+    __syncthreads();                                    // the previous chunk is consumed
+    for (int t = tid; t < cn * k; t += kYtyThreads) {
+      const int c = t / k;
+      s_x[t] = srcF[(size_t)members[lo + c] * k + (t - c * k)];
+    }
+    __syncthreads();
+    if (e < nA)
+      for (int c = 0; c < cn; ++c) {
+        const float xj = s_x[c * k + j];
+        if (xj != 0.0f) a = __dadd_rn(a, __dmul_rn((double)s_x[c * k + i], (double)xj));
+      }
+  }
+  if (e < nA) part[(size_t)b * nA + e] = a;
+}
+
+// YtY = ((0 + B0) + B1) + ... + B9: NormalEquation.merge's daxpy(1.0) in block order
+__global__ void als_yty_merge_kernel(const double* __restrict__ part, int nA, double* __restrict__ yty) {
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < nA; e += gridDim.x * blockDim.x) {
+    double y = 0.0;
+    for (int b = 0; b < kYtyBlocks; ++b) y = __dadd_rn(y, part[(size_t)b * nA + e]);
+    yty[e] = y;
+  }
 }
 
 size_t solve_smem(int k) {
@@ -389,6 +475,66 @@ __global__ void __launch_bounds__(kRecWarps * 32) als_recommend_kernel(const flo
     for (int e = lane; e < L; e += 32) {
       out_ids[(size_t)s * L + e] = dst_ids[ps[e]];
       out_scores[(size_t)s * L + e] = sc[e];
+    }
+  }
+}
+
+// RankingMetrics per query, one warp per query: q's labels lab[off[q] .. off[q + 1]) sorted ascending (a set:
+// equal neighbours count once), its predictions pred [q][L] best first.  Lane t looks up position base + t by
+// binary search; lane 0 then walks the positions in order, summing in double with Spark's expressions: hits in the
+// first min(L, k) over k, dcg and maxDcg over min(max(L, |lab|), k) positions with gain[i] = 1 / ln(i + 2), and
+// the sum of (hits so far) / (i + 1) over every hit, over |lab|.  An empty label set scores 0.  out [3][n].
+__global__ void __launch_bounds__(kRankWarps * 32) ranking_metrics_kernel(const int32_t* __restrict__ pred, int n,
+                                                                          int L, const int32_t* __restrict__ off,
+                                                                          const int32_t* __restrict__ lab, int k,
+                                                                          const double* __restrict__ gain,
+                                                                          double* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  for (int q = blockIdx.x * kRankWarps + (threadIdx.x >> 5); q < n; q += gridDim.x * kRankWarps) {
+    const int lo = off[q], hi = off[q + 1];
+    int distinct = 0;
+    for (int j = lo + lane; j < hi; j += 32) distinct += j == lo || lab[j] != lab[j - 1];
+    distinct = __reduce_add_sync(kFull, distinct);
+    if (distinct == 0) {
+      if (lane == 0) out[q] = out[n + q] = out[2 * n + q] = 0.0;
+      continue;
+    }
+    const int n_prec = min(L, k), n_ndcg = min(max(L, distinct), k), steps = max(L, n_ndcg);
+    int cnt = 0, cnt_k = 0;
+    double prec_sum = 0.0, dcg = 0.0, max_dcg = 0.0;
+    for (int base = 0; base < steps; base += 32) {
+      const int i = base + lane;
+      bool hit = false;
+      if (i < L) {
+        const int32_t x = pred[(size_t)q * L + i];
+        int a = lo, b = hi;                             // the first label >= x
+        while (a < b) {
+          const int m = (a + b) >> 1;
+          if (lab[m] < x) a = m + 1;
+          else b = m;
+        }
+        hit = a < hi && lab[a] == x;
+      }
+      const unsigned hits = __ballot_sync(kFull, hit);
+      if (lane == 0)
+        for (int t = 0; t < 32 && base + t < steps; ++t) {
+          const int p = base + t;
+          const bool h = (hits >> t) & 1u;
+          if (h) {
+            ++cnt;
+            if (p < n_prec) ++cnt_k;
+            prec_sum = __dadd_rn(prec_sum, __ddiv_rn((double)cnt, (double)(p + 1)));
+          }
+          if (p < n_ndcg) {
+            if (h) dcg = __dadd_rn(dcg, gain[p]);
+            if (p < distinct) max_dcg = __dadd_rn(max_dcg, gain[p]);
+          }
+        }
+    }
+    if (lane == 0) {
+      out[q] = __ddiv_rn((double)cnt_k, (double)k);
+      out[n + q] = __ddiv_rn(dcg, max_dcg);
+      out[2 * n + q] = __ddiv_rn(prec_sum, (double)distinct);
     }
   }
 }
@@ -507,22 +653,19 @@ int build_layouts(HostCall& c, const int32_t* user_id, const int32_t* movie_id, 
   return SRS_OK;
 }
 
-}  // namespace
-}  // namespace srs
-
-using namespace srs;
-
-extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
-                                int64_t n_ratings, const srs_als_params* params, int32_t device,
-                                int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
-                                float* user_factors, int32_t* n_users, int32_t* movie_ids, float* movie_factors,
-                                int32_t* n_movies) {
+// srs_als_fit_host and srs_als_fit_implicit_host: every check, then the fit.  `alpha` null: explicit feedback.
+int fit_single(const int32_t* user_id, const int32_t* movie_id, const float* rating, int64_t n_ratings,
+               const srs_als_params* params, const double* alpha, int32_t device, int32_t user_capacity,
+               int32_t movie_capacity, int32_t* user_ids, float* user_factors, int32_t* n_users, int32_t* movie_ids,
+               float* movie_factors, int32_t* n_movies) {
   if (!n_users || !n_movies) return failf(SRS_ERR_INVALID, "null n_users or n_movies");
   *n_users = 0;
   *n_movies = 0;
   if (!params) return failf(SRS_ERR_INVALID, "null params");
   const srs_als_params hp = *params;
   PROPAGATE(check_params(hp.rank, hp.max_iter, hp.reg_param));
+  if (alpha && (!std::isfinite(*alpha) || *alpha < 0))
+    return failf(SRS_ERR_INVALID, "alpha %g is not finite and >= 0", *alpha);
   PROPAGATE(check_ratings(user_id, movie_id, rating, n_ratings));
   if (user_capacity < 0 || movie_capacity < 0 || (user_capacity > 0 && (!user_ids || !user_factors)) ||
       (movie_capacity > 0 && (!movie_ids || !movie_factors)))
@@ -546,13 +689,55 @@ extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id,
   CUDA_TRY(cudaMemcpyAsync(d_uf, init.data(), sizeof(float) * init.size(), cudaMemcpyHostToDevice, s));
   CUDA_TRY(cudaMemsetAsync(d_err, 0xff, sizeof(unsigned long long), s));
   const size_t sm = solve_smem(k);
-  for (int it = 0; it < hp.max_iter; ++it) {
-    als_solve_kernel<false><<<nM, kSolveThreads, sm, s>>>(L.movies, d_uf, d_mf, k, hp.reg_param, d_err, 2ull * it,
-                                                          Batch{});
-    LAUNCHED();
-    als_solve_kernel<false><<<nU, kSolveThreads, sm, s>>>(L.users, d_mf, d_uf, k, hp.reg_param, d_err,
-                                                          2ull * it + 1, Batch{});
-    LAUNCHED();
+  if (!alpha) {
+    for (int it = 0; it < hp.max_iter; ++it) {
+      als_solve_kernel<false><<<nM, kSolveThreads, sm, s>>>(L.movies, d_uf, d_mf, k, hp.reg_param, d_err, 2ull * it,
+                                                            Batch{}, Implicit{});
+      LAUNCHED();
+      als_solve_kernel<false><<<nU, kSolveThreads, sm, s>>>(L.users, d_mf, d_uf, k, hp.reg_param, d_err,
+                                                            2ull * it + 1, Batch{}, Implicit{});
+      LAUNCHED();
+    }
+  } else {
+    // YtY's blocks: each side's dense entities grouped by raw id mod 10, ascending id within a block
+    std::vector<int32_t> mid(nM);
+    CUDA_TRY(cudaMemcpyAsync(mid.data(), L.d_mids, sizeof(int32_t) * nM, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    int32_t *d_umem, *d_mmem, *d_uboff, *d_mboff;
+    const std::vector<int32_t>* ids[2] = {&L.uid, &mid};
+    int32_t** mem[2] = {&d_umem, &d_mmem};
+    int32_t** boff[2] = {&d_uboff, &d_mboff};
+    for (int side = 0; side < 2; ++side) {
+      const std::vector<int32_t>& id = *ids[side];
+      std::vector<int32_t> members, off(kYtyBlocks + 1, 0);
+      members.reserve(id.size());
+      for (int b = 0; b < kYtyBlocks; ++b) {
+        for (size_t e = 0; e < id.size(); ++e)
+          if (id[e] % kYtyBlocks == b) members.push_back((int32_t)e);
+        off[b + 1] = (int32_t)members.size();
+      }
+      PROPAGATE(c.upload(mem[side], members.data(), members.size()));
+      PROPAGATE(c.upload(boff[side], off.data(), off.size()));
+    }
+    const int nA = k * (k + 1) / 2;
+    double *d_part, *d_yty;
+    CUDA_TRY(sc.alloc(&d_part, (size_t)kYtyBlocks * nA)); CUDA_TRY(sc.alloc(&d_yty, nA));
+    const dim3 yg((nA + kYtyThreads - 1) / kYtyThreads, kYtyBlocks);
+    const Implicit im{d_yty, *alpha};
+    for (int it = 0; it < hp.max_iter; ++it)
+      for (int half = 0; half < 2; ++half) {            // the movies from the users, then the users from the movies
+        const bool to_users = half == 1;
+        const float* src = to_users ? d_mf : d_uf;
+        als_yty_kernel<<<yg, kYtyThreads, 0, s>>>(src, k, to_users ? d_mmem : d_umem, to_users ? d_mboff : d_uboff,
+                                                  d_part);
+        LAUNCHED();
+        als_yty_merge_kernel<<<grid_for(nA, 256), 256, 0, s>>>(d_part, nA, d_yty);
+        LAUNCHED();
+        als_solve_kernel<false, true><<<to_users ? nU : nM, kSolveThreads, sm, s>>>(
+            to_users ? L.users : L.movies, src, to_users ? d_uf : d_mf, k, hp.reg_param, d_err, 2ull * it + half,
+            Batch{}, im);
+        LAUNCHED();
+      }
   }
   unsigned long long err = 0;
   CUDA_TRY(cudaMemcpyAsync(&err, d_err, sizeof(err), cudaMemcpyDeviceToHost, s));
@@ -573,6 +758,29 @@ extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id,
   *n_movies = nM;
   return SRS_OK;
 }
+
+}  // namespace
+}  // namespace srs
+
+extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
+                                int64_t n_ratings, const srs_als_params* params, int32_t device,
+                                int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
+                                float* user_factors, int32_t* n_users, int32_t* movie_ids, float* movie_factors,
+                                int32_t* n_movies) {
+  return srs::fit_single(user_id, movie_id, rating, n_ratings, params, nullptr, device, user_capacity,
+                         movie_capacity, user_ids, user_factors, n_users, movie_ids, movie_factors, n_movies);
+}
+
+extern "C" int srs_als_fit_implicit_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
+                                         int64_t n_ratings, const srs_als_params* params, int32_t device,
+                                         int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
+                                         float* user_factors, int32_t* n_users, int32_t* movie_ids,
+                                         float* movie_factors, int32_t* n_movies, double alpha) {
+  return srs::fit_single(user_id, movie_id, rating, n_ratings, params, &alpha, device, user_capacity,
+                         movie_capacity, user_ids, user_factors, n_users, movie_ids, movie_factors, n_movies);
+}
+
+using namespace srs;
 
 extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
                                       const int32_t* fold, int64_t n_ratings, int32_t n_folds,
@@ -665,7 +873,7 @@ extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* mov
     const int nE = to_users ? nU : nM;
     als_solve_kernel<true><<<(unsigned)((int64_t)nE * M), kSolveThreads, sm, s>>>(
         to_users ? L.users : L.movies, to_users ? d_mf : d_uf, to_users ? d_uf : d_mf, 0, 0.0, d_err,
-        (unsigned long long)h, bt);
+        (unsigned long long)h, bt, Implicit{});
     LAUNCHED();
   }
   std::vector<unsigned long long> err(M);
@@ -753,5 +961,65 @@ extern "C" int srs_als_recommend_host(const float* src_factors, int32_t n_src, c
   CUDA_TRY(cudaMemcpyAsync(out_ids, d_ids, sizeof(int32_t) * n_src * L, cudaMemcpyDeviceToHost, s));
   CUDA_TRY(cudaMemcpyAsync(out_scores, d_scores, sizeof(float) * n_src * L, cudaMemcpyDeviceToHost, s));
   CUDA_TRY(cudaStreamSynchronize(s));
+  return SRS_OK;
+}
+
+extern "C" int srs_ranking_metrics_host(const int32_t* pred_ids, int32_t n_queries, int32_t pred_len,
+                                        const int32_t* label_off, const int32_t* label_ids, int32_t k,
+                                        int32_t device, double* per_query, double* means) {
+  if (!means) return failf(SRS_ERR_INVALID, "null means");
+  if (n_queries < 0 || pred_len < 0) return failf(SRS_ERR_INVALID, "negative n_queries or pred_len");
+  if (k < 1) return failf(SRS_ERR_INVALID, "k %d is not positive", k);
+  if ((int64_t)n_queries * pred_len > INT32_MAX)
+    return failf(SRS_ERR_INVALID, "%d x %d predictions exceed %d", n_queries, pred_len, INT32_MAX);
+  if (n_queries > 0 && (!label_off || (pred_len > 0 && !pred_ids)))
+    return failf(SRS_ERR_INVALID, "null predictions or label offsets");
+  int32_t max_lab = 0;
+  if (n_queries > 0) {
+    if (label_off[0] != 0) return failf(SRS_ERR_INVALID, "label_off[0] is %d, not 0", label_off[0]);
+    for (int32_t q = 0; q < n_queries; ++q) {
+      if (label_off[q + 1] < label_off[q])
+        return failf(SRS_ERR_INVALID, "label offsets decrease at query %d", q);
+      max_lab = std::max(max_lab, label_off[q + 1] - label_off[q]);
+    }
+    if (label_off[n_queries] > 0 && !label_ids) return failf(SRS_ERR_INVALID, "null label ids");
+  }
+  if (n_queries == 0) {                               // no query: the means are undefined
+    means[0] = means[1] = means[2] = NAN;
+    return SRS_OK;
+  }
+  const int nnz = label_off[n_queries];
+  // gain[i] = 1 / ln(i + 2) for every position an NDCG loop can reach, on the host (no device transcendental)
+  const int n_gain = std::min(k, std::max(pred_len, max_lab));
+  std::vector<double> gain(std::max(n_gain, 1), 0.0);
+  for (int i = 0; i < n_gain; ++i) gain[i] = 1.0 / std::log((double)(i + 2));
+
+  HostCall c;
+  PROPAGATE(c.begin(device));
+  cudaStream_t s = c.s;
+  int32_t *d_pred, *d_off, *d_lab_in, *d_lab;
+  double *d_gain, *d_out;
+  PROPAGATE(c.upload(&d_pred, pred_ids, (size_t)n_queries * pred_len));
+  PROPAGATE(c.upload(&d_off, label_off, (size_t)n_queries + 1));
+  PROPAGATE(c.upload(&d_lab_in, label_ids, (size_t)nnz));
+  PROPAGATE(c.upload(&d_gain, gain.data(), gain.size()));
+  CUDA_TRY(c.sc.alloc(&d_lab, (size_t)nnz));
+  CUDA_TRY(c.sc.alloc(&d_out, (size_t)3 * n_queries));
+  if (nnz > 0)                                        // each query's labels ascending: a set by its runs
+    CUB_RUN(c, cub::DeviceSegmentedRadixSort::SortKeys(tmp__, tb__, d_lab_in, d_lab, nnz, n_queries, d_off,
+                                                       d_off + 1, 0, 32, s));
+  const int blocks = (int)std::min<int64_t>(((int64_t)n_queries + kRankWarps - 1) / kRankWarps, kMaxGridBlocks);
+  ranking_metrics_kernel<<<blocks, kRankWarps * 32, 0, s>>>(d_pred, n_queries, pred_len, d_off, d_lab, k, d_gain,
+                                                           d_out);
+  LAUNCHED();
+  std::vector<double> v((size_t)3 * n_queries);
+  CUDA_TRY(cudaMemcpyAsync(v.data(), d_out, sizeof(double) * v.size(), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  for (int m = 0; m < 3; ++m) {                       // StatCounter's mean, in query order: mu += (x - mu) / n
+    double mu = 0.0;
+    for (int32_t q = 0; q < n_queries; ++q) mu = mu + (v[(size_t)m * n_queries + q] - mu) / (double)(q + 1);
+    means[m] = mu;
+  }
+  if (per_query) std::copy(v.begin(), v.end(), per_query);
   return SRS_OK;
 }
