@@ -21,6 +21,7 @@ template <int EP>
 __global__ void __launch_bounds__(kThreads) deepfm_kernel(DeepFmParams p, BatchView b) {
   const int row0 = blockIdx.x * kFm1Rows;
   deepfm_tile_forward<EP>(p, b, row0);
+  deepfm_load_out<EP>(p);                 // after the forward: the five floats are not held across its tiles
   deepfm_tile_logits<EP>(p, b, row0, [&](int, int row, float z) {
     store_score(b, row, sigmoidf_acc(z));
     if (b.logits) b.logits[row] = z;

@@ -1,7 +1,7 @@
 // deepfm_layers.cuh - the 32-row tile forward of DeepFM (DeepFM.py:91-113), shared by the forward kernel
 // (deepfm.cu) and the training step (deepfm_train.cu), so that a step's forward is the serving forward bit for bit.
 // Tables are padded to EP floats per row; W1 is [KP = 2*EP + 8][64] in tile order (deep movie | deep user |
-// numerics), W2 [64][64], hidden widths zero-padded to 64 (build_deepfm's layout).
+// numerics), W2 [64][64], hidden widths zero-padded to 64 (DeepFmBlob, placed by placement.h).
 #pragma once
 
 #include "kernels.h"
@@ -15,6 +15,16 @@ __device__ __forceinline__ int genre_id(const int32_t* col, int row, int stride,
   int id = __ldg(col + row * stride);
   if (id >= n_genres) { atomicExch(err_flag, 1); id = -1; }
   return id < 0 ? -1 : id;
+}
+
+// dense_2's four dot weights and its bias, from the blob: in a trainer they change on the device every step, so
+// the forward reads them where the step's Adam writes them, with no host read between steps
+template <int EP>
+__device__ __forceinline__ void deepfm_load_out(DeepFmParams& p) {
+  const DeepFmBlob ly = DeepFmBlob::of(EP);
+#pragma unroll
+  for (int d = 0; d < 4; ++d) p.wdot[d] = __ldg(p.blob + ly.wdot + d);
+  p.bout = __ldg(p.blob + ly.bout);
 }
 
 // The tile's regions of the kernel's dynamic shared memory (`smem`, which the kernel may extend past kFloats), in

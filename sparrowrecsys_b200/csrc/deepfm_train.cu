@@ -10,10 +10,7 @@
 //   entries the 6 table rows of each row (4 FM, 2 deep; a missing genre writes none) with their gradients, and
 //           the 4 one-hot rows of dense_2/kernel (scalar dz), for table_grad_kernel to dedupe in row order
 //   partial thread q sums Dense parameter q's gradient over the CTA's rows in row order
-// No float atomics.
-//
-// deepfm_blob_forward_kernel<EP>: the trainer's forward for validation and evaluate (deepfm_kernel's, reading
-// dense_2's dot weights and bias from the blob).
+// No float atomics.  The trainer's forward for validation and evaluate is deepfm_kernel itself (launch_deepfm).
 #include "deepfm_layers.cuh"
 
 namespace srs {
@@ -43,9 +40,7 @@ __global__ void __launch_bounds__(kThreads) deepfm_train_step_kernel(DeepFmStepA
   const DeepFmBlob ly = DeepFmBlob::of(EP);
   const BatchView& b = a.b;
   DeepFmParams p = a.p;
-#pragma unroll
-  for (int d = 0; d < 4; ++d) p.wdot[d] = __ldg(a.blob + ly.wdot + d);
-  p.bout = __ldg(a.blob + ly.bout);
+  deepfm_load_out<EP>(p);
   const int tid = threadIdx.x;
   const int row0 = blockIdx.x * R;
   const int nv = min(R, b.B - row0);
@@ -157,39 +152,6 @@ cudaError_t launch_step_t(const DeepFmStepArgs& a, cudaStream_t s) {
   return cudaGetLastError();
 }
 
-// deepfm_kernel with wdot and bout read from the trainer's blob: the serving forward (the same tile code, so the
-// same bits) of weights that change on the device every step.  deepfm_kernel takes them by value, which would need
-// a host read, and so a host synchronisation, before each validation of a fit.
-template <int EP>
-__global__ void __launch_bounds__(kThreads) deepfm_blob_forward_kernel(DeepFmParams p, const float* __restrict__ blob,
-                                                                       BatchView b) {
-  const DeepFmBlob ly = DeepFmBlob::of(EP);
-#pragma unroll
-  for (int d = 0; d < 4; ++d) p.wdot[d] = __ldg(blob + ly.wdot + d);
-  p.bout = __ldg(blob + ly.bout);
-  const int row0 = blockIdx.x * kFm1Rows;
-  deepfm_tile_forward<EP>(p, b, row0);
-  deepfm_tile_logits<EP>(p, b, row0, [&](int, int row, float z) {
-    b.probs[row] = sigmoidf_acc(z);
-    b.logits[row] = z;
-  });
-}
-
-template <int EP>
-cudaError_t launch_blob_forward_t(const DeepFmParams& p, const float* blob, const BatchView& b, cudaStream_t s) {
-  constexpr int smem = DeepFmTile<EP>::kFloats * (int)sizeof(float);
-  static bool attr_set = false;
-  if (!attr_set) {
-    const cudaError_t e = cudaFuncSetAttribute(deepfm_blob_forward_kernel<EP>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
-  deepfm_blob_forward_kernel<EP><<<(b.B + kFm1Rows - 1) / kFm1Rows, kThreads, smem, s>>>(p, blob, b);
-  ++g_launch_count;
-  return cudaGetLastError();
-}
-
 __global__ void deepfm_permute_kernel(DeepFmRows src, DeepFmRows dst, const int32_t* __restrict__ order, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -212,15 +174,6 @@ cudaError_t launch_deepfm_train_step(const DeepFmStepArgs& a, cudaStream_t s) {
   if (a.p.EP == E_) return launch_step_t<E_>(a, s);
   SRS_DEEPFM_TRAIN_CASE(12) SRS_DEEPFM_TRAIN_CASE(16) SRS_DEEPFM_TRAIN_CASE(32) SRS_DEEPFM_TRAIN_CASE(64)
 #undef SRS_DEEPFM_TRAIN_CASE
-  return cudaErrorInvalidValue;
-}
-
-cudaError_t launch_deepfm_blob_forward(const DeepFmParams& p, const float* blob, const BatchView& b, cudaStream_t s) {
-  if (b.B <= 0) return cudaSuccess;
-#define SRS_DEEPFM_FWD_CASE(E_) \
-  if (p.EP == E_) return launch_blob_forward_t<E_>(p, blob, b, s);
-  SRS_DEEPFM_FWD_CASE(12) SRS_DEEPFM_FWD_CASE(16) SRS_DEEPFM_FWD_CASE(32) SRS_DEEPFM_FWD_CASE(64)
-#undef SRS_DEEPFM_FWD_CASE
   return cudaErrorInvalidValue;
 }
 

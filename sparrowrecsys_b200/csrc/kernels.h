@@ -75,22 +75,23 @@ struct DeepFmParams {
   const float* fm_ugenre;  // [19][EP]
   const float* deep_movie; // [n_movies][EP]
   const float* deep_user;  // [n_users][EP]
+  const float* blob;       // the Dense weights, DeepFmBlob layout; W1, b1, W2, b2 and wdeep point into it
   const float* W1;         // [KP = 2*EP + 8][64]
   const float* b1;
   const float* W2;         // [64][64]
   const float* b2;
   const float* first;      // [fm1_width] one-hot rows of dense_2 (movieGenre1|movieId|userGenre1|userId)
   const float* wdeep;      // [64]
-  float wdot[4];
-  float bout;
+  float wdot[4];           // dense_2's dot rows and bias: deepfm_kernel and the training step load them from the
+  float bout;              //   blob (deepfm_load_out), deepfm_tc_kernel takes them from here
   int n_movies, n_users, n_genres;
   int EP;
 };
 
-// ---- DeepFM's training step (deepfm_train.cu; DESIGN.md section 4.9) ----------------------------
-// The Dense weights of a DeepFM trainer as one blob, offsets in floats: W1 [2EP + 8][64] and W2 [64][64] in
-// build_deepfm's tile order and padding, b1 [64], b2 [64], wdeep [64] (the deep rows of dense_2/kernel), wdot [4]
-// (its dot rows), bout (dense_2/bias) and 3 floats of padding.  The one-hot rows of dense_2/kernel live apart.
+// The Dense weights of DeepFM (a model's and a trainer's) as one blob, offsets in floats: W1 [2EP + 8][64] and
+// W2 [64][64] in the tile order and padding of deepfm_layers.cuh, b1 [64], b2 [64], wdeep [64] (the deep rows of
+// dense_2/kernel), wdot [4] (its dot rows), bout (dense_2/bias) and 3 floats of padding; every array up to wdeep
+// starts at a multiple of 64 floats.  The one-hot rows of dense_2/kernel live apart (placement.h).
 struct DeepFmBlob {
   int W1, b1, W2, b2, wdeep, wdot, bout, floats;
   __host__ __device__ static DeepFmBlob of(int EP) {
@@ -106,10 +107,12 @@ struct DeepFmBlob {
     return l;
   }
 };
+cudaError_t setup_deepfm_attributes();   // deepfm_kernel's (and deepfm2_kernel's) dynamic shared memory opt-in
+
+// ---- DeepFM's training step (deepfm_train.cu; DESIGN.md section 4.9) ----------------------------
 constexpr int kDeepFmTables = 6;   // fm movieId, fm userId, fm movieGenre1, fm userGenre1, deep movieId, deep userId
 struct DeepFmStepArgs {
-  DeepFmParams p;          // the trainer's tables and Dense weights (wdot and bout are read from `blob`)
-  const float* blob;       // DeepFmBlob layout
+  DeepFmParams p;          // the trainer's tables and Dense weights
   BatchView b;             // the step's B rows in order; probs / logits receive its outputs before the update
   const int32_t* label;    // [B]
   int64_t tab_row0[kDeepFmTables];   // first row of each table in the trainer's table array
@@ -121,9 +124,6 @@ struct DeepFmStepArgs {
 };
 int deepfm_train_ctas(int B);
 cudaError_t launch_deepfm_train_step(const DeepFmStepArgs& a, cudaStream_t s);
-// deepfm_kernel's forward (probs and logits, both required) with p.wdot and p.bout taken from `blob` (DeepFmBlob
-// layout) on the device
-cudaError_t launch_deepfm_blob_forward(const DeepFmParams& p, const float* blob, const BatchView& b, cudaStream_t s);
 struct DeepFmRows {        // a DeepFM dataset on the device, in the srs_batch layout
   int32_t* movie;          // [n]
   int32_t* user;           // [n]
@@ -300,6 +300,11 @@ struct MetricsReduce {                     // per stream of updates: the last CT
   unsigned int ticket;
   unsigned int pad_;
   double partial[kMetMaxCtas];
+};
+struct MetricsState {                      // one history (srs_metrics, an epoch of a fit): counts, loss sum, reduce
+  MetricsCounters cnt;
+  double loss;
+  MetricsReduce red;
 };
 // Fold n rows into `cnt`; the rows' loss sum goes to *loss_dst (added to it when `accumulate`; not written
 // when loss_dst is null).  `own_hist` (zeroed by the caller, or null): the batch's own 2 x 201 (label, bin)

@@ -14,10 +14,10 @@
 
 #include "../../include/srs_ctr.h"
 #include "hostcall.h"
+#include "placement.h"
 
 namespace srs {
 cudaError_t setup_embmlp_attributes();
-cudaError_t setup_deepfm_attributes();
 cudaError_t setup_din_attributes();
 cudaError_t setup_din_wg_attributes();
 #ifdef SRS_DIN_PHASES
@@ -191,11 +191,6 @@ struct srs_model {
 };
 
 // srs_metrics_*: one allocation on the device
-struct MetricsState {
-  MetricsCounters cnt;
-  double loss;
-  MetricsReduce red;
-};
 struct srs_metrics {
   int device = 0;
   MetricsState* d = nullptr;
@@ -207,49 +202,11 @@ inline int* slot_err(srs_model* m, const Slot& s) { return m->err_flag + 1 + (&s
 
 namespace {
 
-int round_ep(int E) {
-  if (E <= 12) return 12;
-  if (E <= 16) return 16;
-  if (E <= 32) return 32;
-  return 64;
-}
-
-struct Builder {
+struct Builder : TensorLookup {
   srs_model* m;
-  std::map<std::string, const srs_tensor*> by_name;
-  int status = SRS_OK;
   std::vector<float> din_w1, din_w2;    // the permuted DIN top-MLP weights build_din uploaded, for build_din_wg
 
-  const srs_tensor* need(const char* name, int64_t rows, int64_t cols) {
-    if (status != SRS_OK) return nullptr;
-    auto it = by_name.find(name);
-    if (it == by_name.end()) {
-      status = fail(SRS_ERR_MISSING, "missing weight tensor '%s'", name);
-      return nullptr;
-    }
-    const srs_tensor* t = it->second;
-    if (t->rows != rows || t->cols != cols) {
-      status = fail(SRS_ERR_SHAPE, "weight '%s' has shape [%lld,%lld], expected [%lld,%lld]", name,
-                    (long long)t->rows, (long long)t->cols, (long long)rows, (long long)cols);
-      return nullptr;
-    }
-    if (t->data == nullptr) {
-      status = fail(SRS_ERR_INVALID, "weight '%s' has a null data pointer", name);
-      return nullptr;
-    }
-    return t;
-  }
-
-  // dense host tensor -> float vector (must be SRS_HOST)
-  const float* host(const char* name, int64_t rows, int64_t cols) {
-    const srs_tensor* t = need(name, rows, cols);
-    if (!t) return nullptr;
-    if (t->location != SRS_HOST) {
-      status = fail(SRS_ERR_INVALID, "weight '%s' must be a host tensor", name);
-      return nullptr;
-    }
-    return t->data;
-  }
+  Builder(srs_model* m, const srs_tensor* ts, int n) : TensorLookup(ts, n), m(m) {}
 
   // host weights, or a tensor-core operand image (write_sw128 tiles) -> a device copy the model owns
   template <class T>
@@ -336,88 +293,38 @@ struct Builder {
   }
 };
 
-std::vector<int> iota_map(int start, int n, int padded) {
-  std::vector<int> v(padded, -1);
-  for (int i = 0; i < n; ++i) v[i] = start + i;
-  return v;
+// The tensors of a trainable model through its placement (placement.h): the Dense tensors scattered into the host
+// blob and one-hot arrays; the tables uploaded as the model's own arrays, tables[k] the k-th in placement order
+void place_host(Builder& B, const Placement& pl, const float** tables, float* blob, float* onehot) {
+  int k = 0;
+  for (const Placed& x : pl) {
+    if (x.table_row >= 0) {
+      tables[k++] = B.table(x.name.c_str(), x.rows, (int)x.cols);
+    } else if (const float* src = B.host(x.name.c_str(), x.rows, x.cols)) {
+      scatter(x, src, blob, onehot);
+    }
+  }
 }
-
-void append(std::vector<int>& a, const std::vector<int>& b) { a.insert(a.end(), b.begin(), b.end()); }
 
 // ------------------------------------------------------------------------------------
 int build_ncf(Builder& B) {
   srs_model* m = B.m;
   const srs_spec& s = m->spec;
-  const int E = s.emb_dim, EP = m->EP;
   const bool two = s.kind == SRS_TWOTOWERS;
   if (s.n_hidden < 1 || s.n_hidden > 3) return fail(SRS_ERR_INVALID, "1..3 hidden layers supported");
   int hmax = 0;
   for (int i = 0; i < s.n_hidden; ++i) hmax = std::max(hmax, s.hidden[i]);
   if (hmax > 32 || hmax < 1) return fail(SRS_ERR_INVALID, "hidden widths must be in 1..32");
-  const int HP = hmax <= 16 ? 16 : 32;
   NcfParams& p = m->ncf;
-  p.movie = B.table("movieId_embedding", s.n_movies, E);
-  p.user = B.table("userId_embedding", s.n_users, E);
-  p.n_movies = s.n_movies; p.n_users = s.n_users;
-  p.EP = EP; p.HP = HP; p.n_layers = s.n_hidden; p.two_towers = two; p.final_dense = s.final_dense;
-  std::vector<float> blob;
-  auto push = [&](const std::vector<float>& v) {
-    int off = (int)blob.size();
-    blob.insert(blob.end(), v.begin(), v.end());
-    while (blob.size() % 4) blob.push_back(0.f);
-    return off;
-  };
-  char name[64];
-  if (!two) {
-    int in = 2 * E;
-    for (int l = 0; l < s.n_hidden; ++l) {
-      const int out = s.hidden[l];
-      snprintf(name, sizeof(name), "dense_%d/kernel", l);
-      const float* k = B.host(name, in, out);
-      snprintf(name, sizeof(name), "dense_%d/bias", l);
-      const float* bias = B.host(name, out, 1);
-      std::vector<int> map;
-      if (l == 0) { append(map, iota_map(0, E, EP)); append(map, iota_map(E, E, EP)); }
-      else map = iota_map(0, in, HP);
-      p.w_off[l] = push(B.permute(k, out, map, HP));
-      p.b_off[l] = push(B.padvec(bias, out, HP));
-      in = out;
-    }
-    snprintf(name, sizeof(name), "dense_%d/kernel", s.n_hidden);
-    const float* k = B.host(name, in, 1);
-    snprintf(name, sizeof(name), "dense_%d/bias", s.n_hidden);
-    const float* bias = B.host(name, 1, 1);
-    p.out_w = push(B.padvec(k, in, HP));
-    p.out_b = push(B.padvec(bias, 1, 4));
-  } else {
-    const char* sides[2] = {"item", "user"};
-    for (int t = 0; t < 2; ++t) {
-      int in = E;
-      for (int l = 0; l < s.n_hidden; ++l) {
-        const int out = s.hidden[l];
-        snprintf(name, sizeof(name), "%s_dense_%d/kernel", sides[t], l);
-        const float* k = B.host(name, in, out);
-        snprintf(name, sizeof(name), "%s_dense_%d/bias", sides[t], l);
-        const float* bias = B.host(name, out, 1);
-        std::vector<int> map = l == 0 ? iota_map(0, E, EP) : iota_map(0, in, HP);
-        p.w_off[3 * t + l] = push(B.permute(k, out, map, HP));
-        p.b_off[3 * t + l] = push(B.padvec(bias, out, HP));
-        in = out;
-      }
-    }
-    if (s.final_dense) {
-      const float* k = B.host("dense_out/kernel", 1, 1);
-      const float* bias = B.host("dense_out/bias", 1, 1);
-      p.out_w = push(B.padvec(k, 1, 4));
-      p.out_b = push(B.padvec(bias, 1, 4));
-    } else {
-      p.out_w = push(std::vector<float>(4, 1.f));
-      p.out_b = push(std::vector<float>(4, 0.f));
-    }
-  }
+  const Placement pl = place_ncf(s, m->EP, hmax <= 16 ? 16 : 32, &p);
+  std::vector<float> blob(p.blob_floats, 0.f);
+  if (two && !s.final_dense) std::fill_n(blob.begin() + p.out_w, 4, 1.f);   // no dense_out: z = 1 * dot + 0
+  const float* tables[2];
+  place_host(B, pl, tables, blob.data(), nullptr);
   if (B.status != SRS_OK) return B.status;
+  p.movie = tables[0];
+  p.user = tables[1];
   p.blob = B.upload(blob);
-  p.blob_floats = (int)blob.size();
   m->kernel_name = two ? "ncf_kernel<two_towers>" : "ncf_kernel<neural_cf_model_1>";
   return B.status;
 }
@@ -475,39 +382,21 @@ int build_embmlp(Builder& B) {
 int build_deepfm(Builder& B) {
   srs_model* m = B.m;
   const srs_spec& s = m->spec;
-  const int E = s.emb_dim, EP = m->EP;
   if (s.n_hidden != 2 || s.hidden[0] > 64 || s.hidden[1] > 64 || s.hidden[0] < 1 || s.hidden[1] < 1)
     return fail(SRS_ERR_INVALID, "DeepFM needs two hidden layers of width <= 64");
-  const int h0 = s.hidden[0], h1 = s.hidden[1];
-  const int64_t fm1 = (int64_t)2 * s.n_genres + s.n_movies + s.n_users;
   DeepFmParams& p = m->fm;
-  p.fm_movie = B.table("fm_movieId_embedding", s.n_movies, E);
-  p.fm_user = B.table("fm_userId_embedding", s.n_users, E);
-  p.fm_mgenre = B.table("fm_movieGenre1_embedding", s.n_genres, E);
-  p.fm_ugenre = B.table("fm_userGenre1_embedding", s.n_genres, E);
-  p.deep_movie = B.table("deep_movieId_embedding", s.n_movies, E);
-  p.deep_user = B.table("deep_userId_embedding", s.n_users, E);
-  std::vector<int> map;
-  append(map, iota_map(1, E, EP));            // deep movieId emb
-  append(map, iota_map(5 + E, E, EP));        // deep userId emb
-  const int nums[8] = {0, 1 + E, 2 + E, 3 + E, 4 + E, 5 + 2 * E, 6 + 2 * E, -1};
-  for (int j = 0; j < 8; ++j) map.push_back(nums[j]);
-  const float* k1 = B.host("dense/kernel", 7 + 2 * E, h0);
-  const float* b1 = B.host("dense/bias", h0, 1);
-  const float* k2 = B.host("dense_1/kernel", h0, h1);
-  const float* b2 = B.host("dense_1/bias", h1, 1);
-  const float* k3 = B.host("dense_2/kernel", fm1 + 4 + h1, 1);
-  const float* b3 = B.host("dense_2/bias", 1, 1);
+  const Placement pl = place_deepfm(s, m->EP, &p);
+  const DeepFmBlob ly = DeepFmBlob::of(m->EP);
+  std::vector<float> blob(ly.floats, 0.f), first((size_t)2 * s.n_genres + s.n_movies + s.n_users, 0.f);
+  const float* tables[kDeepFmTables];
+  place_host(B, pl, tables, blob.data(), first.data());
   if (B.status != SRS_OK) return B.status;
-  p.W1 = B.upload(B.permute(k1, h0, map, 64));
-  p.b1 = B.upload(B.padvec(b1, h0, 64));
-  p.W2 = B.upload(B.permute(k2, h1, iota_map(0, h0, 64), 64));
-  p.b2 = B.upload(B.padvec(b2, h1, 64));
-  p.first = B.upload(std::vector<float>(k3, k3 + fm1));
-  for (int d = 0; d < 4; ++d) p.wdot[d] = k3[fm1 + d];
-  p.wdeep = B.upload(B.padvec(k3 + fm1 + 4, h1, 64));
-  p.bout = b3[0];
-  p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres; p.EP = EP;
+  p.fm_movie = tables[0]; p.fm_user = tables[1]; p.fm_mgenre = tables[2]; p.fm_ugenre = tables[3];
+  p.deep_movie = tables[4]; p.deep_user = tables[5];
+  point_into_blob(&p, B.upload(blob));
+  p.first = B.upload(first);
+  for (int d = 0; d < 4; ++d) p.wdot[d] = blob[ly.wdot + d];
+  p.bout = blob[ly.bout];
   m->kernel_name = "deepfm_kernel";
   return B.status;
 }
@@ -1404,9 +1293,7 @@ int srs_model_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_
   m->hist_cols = (spec->kind == SRS_DIN || spec->kind == SRS_DIEN) ? spec->hist_len
                  : spec->kind == SRS_WIDENDEEP ? 1 : 0;
   m->bytes_per_inf = bytes_per_inference(*spec);
-  Builder B{m};
-  for (int i = 0; i < n_tensors; ++i)
-    if (tensors[i].name) B.by_name[tensors[i].name] = &tensors[i];
+  Builder B(m, tensors, n_tensors);
   switch (spec->kind) {
     case SRS_NEURALCF:
     case SRS_TWOTOWERS: rc = build_ncf(B); break;

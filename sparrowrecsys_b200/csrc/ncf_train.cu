@@ -19,19 +19,18 @@
 // No float atomics: every sum has a fixed order, so a fit is bitwise reproducible.
 //
 // Validation (srs_trainer_fit_validate_host) and srs_trainer_evaluate_host run the serving forward over the
-// trainer's arrays (ncf_kernel; deepfm_kernel's forward reading wdot / bout from the blob) and one
-// metrics_update_kernel over all the rows: two launches, with the bits of a CTRModel built from the exported weights.
+// trainer's arrays (ncf_kernel, deepfm_kernel) and one metrics_update_kernel over all the rows: two launches, with the
+// bits of a CTRModel built from the exported weights.  The trainer's arrays hold the weights where the serving
+// builders put them: both place them through placement.h.
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdio>
-#include <cstring>
-#include <string>
 #include <vector>
 
 #include "../../include/srs_ctr.h"
 #include "hostcall.h"
 #include "ncf_layers.cuh"
+#include "placement.h"
 
 namespace srs {
 
@@ -40,10 +39,20 @@ namespace {
 constexpr int kTrainRows = 64;        // rows (threads) per CTA of the step kernel
 constexpr int kAdamThreads = 512;     // the one CTA of dense_adam_kernel
 
-struct TrainLayout {                  // the NcfParams blob layout (build_ncf), offsets in floats
+struct TrainLayout {                  // the step kernel's view of NcfParams' blob layout, offsets in floats
   int n_layers, blob_floats;
   int w_off[3], b_off[3], out_w, out_b;
 };
+
+TrainLayout train_layout(const NcfParams& p) {
+  TrainLayout ly{};
+  ly.n_layers = p.n_layers;
+  ly.blob_floats = p.blob_floats;
+  for (int l = 0; l < p.n_layers; ++l) { ly.w_off[l] = p.w_off[l]; ly.b_off[l] = p.b_off[l]; }
+  ly.out_w = p.out_w;
+  ly.out_b = p.out_b;
+  return ly;
+}
 
 struct StepArgs {
   const float* tab;                   // [n_movies + n_users][EP]: movie rows, then user rows
@@ -265,19 +274,6 @@ cudaError_t launch_step(int EP, int HP, const StepArgs& a, const TrainLayout& ly
   return cudaErrorInvalidValue;
 }
 
-struct EpochMetrics {                 // one epoch's history state (the layout of srs_metrics' state)
-  MetricsCounters cnt;
-  double loss;
-  MetricsReduce red;
-};
-
-struct TrainTensor {                  // one Keras tensor of a trainer
-  std::string name;
-  int64_t rows, cols;
-  int64_t row0;                       // an embedding table: its first row in the trainer's table array; else -1
-  std::vector<int64_t> at;            // a Dense tensor: element i * cols + j -> blob offset, or -1 - r for one-hot row r
-};
-
 }  // namespace
 }  // namespace srs
 
@@ -286,12 +282,12 @@ using namespace srs;
 struct srs_trainer {
   srs_spec spec{};
   int device = 0;
-  int E = 0, EP = 0, HP = 0;
-  TrainLayout ly{};                   // NeuralCF's blob layout
+  int EP = 0, HP = 0;
   int blob_floats = 0;
   AdamHp hp{};
-  std::vector<TrainTensor> tensors;   // the Keras tensors, in srs_model_create's order
-  int64_t tab_row0[kDeepFmTables] = {};   // first row of each table in tab (DeepFM)
+  Placement place;                    // where the Keras tensors live in tab, blob and fo
+  NcfParams ncf{};                    // the serving parameters over the trainer's arrays (NeuralCF)
+  DeepFmParams fm{};                  //   (DeepFM)
   int64_t tab_floats = 0;             // (sum of the tables' rows) * EP
   float* tab[4] = {};                 // w, m, v, G   [rows][EP], padding zero
   float* blob[3] = {};                // w, m, v      [blob_floats]
@@ -313,108 +309,6 @@ void trainer_free(srs_trainer* t) {
   cudaFree(t->d_it);
   if (t->stream) cudaStreamDestroy(t->stream);
   delete t;
-}
-
-const srs_tensor* find_tensor(const srs_tensor* ts, int n, const char* name, int64_t rows, int64_t cols, int* rc) {
-  for (int i = 0; i < n; ++i) {
-    if (!ts[i].name || strcmp(ts[i].name, name) != 0) continue;
-    if (ts[i].rows != rows || ts[i].cols != cols) {
-      *rc = failf(SRS_ERR_SHAPE, "weight '%s' has shape [%lld,%lld], expected [%lld,%lld]", name,
-                  (long long)ts[i].rows, (long long)ts[i].cols, (long long)rows, (long long)cols);
-      return nullptr;
-    }
-    if (!ts[i].data || ts[i].location != SRS_HOST) {
-      *rc = failf(SRS_ERR_INVALID, "weight '%s' must be a non-null host tensor", name);
-      return nullptr;
-    }
-    return &ts[i];
-  }
-  *rc = failf(SRS_ERR_MISSING, "missing weight tensor '%s'", name);
-  return nullptr;
-}
-
-TrainTensor table_tensor(const char* name, int64_t rows, int E, int64_t row0) {
-  TrainTensor x;
-  x.name = name; x.rows = rows; x.cols = E; x.row0 = row0;
-  return x;
-}
-
-TrainTensor dense_tensor(const char* name, int64_t rows, int64_t cols) {
-  TrainTensor x;
-  x.name = name; x.rows = rows; x.cols = cols; x.row0 = -1;
-  x.at.assign((size_t)(rows * cols), -1);
-  return x;
-}
-
-// NeuralCF: the two tables (movie rows, then user rows) and dense_l/kernel, dense_l/bias in build_ncf's blob layout
-void ncf_tensors(srs_trainer* t) {
-  const srs_spec& s = t->spec;
-  const int L = s.n_hidden, E = t->E, EP = t->EP, HP = t->HP;
-  t->tensors.push_back(table_tensor("movieId_embedding", s.n_movies, E, 0));
-  t->tensors.push_back(table_tensor("userId_embedding", s.n_users, E, s.n_movies));
-  for (int l = 0; l <= L; ++l) {
-    char k[32], b[32];
-    snprintf(k, sizeof(k), "dense_%d/kernel", l);
-    snprintf(b, sizeof(b), "dense_%d/bias", l);
-    const int in = l == 0 ? 2 * E : s.hidden[l - 1], out = l == L ? 1 : s.hidden[l];
-    TrainTensor K = dense_tensor(k, in, out), B = dense_tensor(b, out, 1);
-    for (int i = 0; i < in; ++i)
-      for (int j = 0; j < out; ++j) {
-        if (l == L) { K.at[(size_t)i * out + j] = t->ly.out_w + i; continue; }
-        const int row = l == 0 ? (i < E ? i : EP + (i - E)) : i;
-        K.at[(size_t)i * out + j] = t->ly.w_off[l] + row * HP + j;
-      }
-    for (int i = 0; i < out; ++i) B.at[i] = l == L ? t->ly.out_b : t->ly.b_off[l] + i;
-    t->tensors.push_back(std::move(K));
-    t->tensors.push_back(std::move(B));
-  }
-}
-
-// DeepFM: the six tables one after another, the Dense tensors in DeepFmBlob's layout (build_deepfm's tile order
-// and padding) and dense_2/kernel's one-hot rows in fo (at = -1 - row)
-void deepfm_tensors(srs_trainer* t) {
-  const srs_spec& s = t->spec;
-  const int E = t->E, EP = t->EP, h0 = s.hidden[0], h1 = s.hidden[1];
-  const DeepFmBlob ly = DeepFmBlob::of(EP);
-  const char* names[kDeepFmTables] = {"fm_movieId_embedding", "fm_userId_embedding", "fm_movieGenre1_embedding",
-                                      "fm_userGenre1_embedding", "deep_movieId_embedding", "deep_userId_embedding"};
-  const int64_t rows[kDeepFmTables] = {s.n_movies, s.n_users, s.n_genres, s.n_genres, s.n_movies, s.n_users};
-  int64_t row0 = 0;
-  for (int k = 0; k < kDeepFmTables; ++k) {
-    t->tab_row0[k] = row0;
-    t->tensors.push_back(table_tensor(names[k], rows[k], E, row0));
-    row0 += rows[k];
-  }
-  // dense/kernel rows, sorted DenseFeatures concat: movieAvgRating | deep movieId | 4 numerics | deep userId | 2
-  TrainTensor K1 = dense_tensor("dense/kernel", 7 + 2 * E, h0);
-  for (int i = 0; i < 7 + 2 * E; ++i) {
-    int tr;                                            // the tile row (deep movie | deep user | numerics)
-    if (i == 0) tr = 2 * EP;
-    else if (i <= E) tr = i - 1;
-    else if (i <= E + 4) tr = 2 * EP + (i - E);
-    else if (i <= 2 * E + 4) tr = EP + (i - E - 5);
-    else tr = 2 * EP + (i - 2 * E);
-    for (int j = 0; j < h0; ++j) K1.at[(size_t)i * h0 + j] = ly.W1 + tr * 64 + j;
-  }
-  TrainTensor B1 = dense_tensor("dense/bias", h0, 1), K2 = dense_tensor("dense_1/kernel", h0, h1),
-              B2 = dense_tensor("dense_1/bias", h1, 1);
-  for (int i = 0; i < h0; ++i) {
-    B1.at[i] = ly.b1 + i;
-    for (int j = 0; j < h1; ++j) K2.at[(size_t)i * h1 + j] = ly.W2 + i * 64 + j;
-  }
-  for (int j = 0; j < h1; ++j) B2.at[j] = ly.b2 + j;
-  const int64_t fm1 = t->onehot;
-  TrainTensor K3 = dense_tensor("dense_2/kernel", fm1 + 4 + h1, 1), B3 = dense_tensor("dense_2/bias", 1, 1);
-  for (int64_t i = 0; i < fm1 + 4 + h1; ++i)
-    K3.at[i] = i < fm1 ? -1 - i : i < fm1 + 4 ? ly.wdot + (i - fm1) : ly.wdeep + (i - fm1 - 4);
-  B3.at[0] = ly.bout;
-  for (TrainTensor* x : {&K1, &B1, &K2, &B2, &K3, &B3}) t->tensors.push_back(std::move(*x));
-}
-
-const TrainTensor* trainer_tensor(const srs_trainer* t, const char* name) {
-  for (const TrainTensor& x : t->tensors)
-    if (x.name == name) return &x;
-  return nullptr;
 }
 
 // a DeepFM dataset of n rows on the device
@@ -483,42 +377,11 @@ cudaError_t upload_rows(Scratch& sc, bool fm, const srs_batch* b, const int32_t*
   return e;
 }
 
-// The serving kernels' parameters over the trainer's arrays.  The blob is build_ncf's layout (TrainLayout's offsets
-// are build_ncf's, every segment a multiple of 4 floats) and the tables are movie rows, then user rows.
-NcfParams ncf_params(const srs_trainer* t) {
-  NcfParams p{};
-  p.movie = t->tab[0];
-  p.user = t->tab[0] + (size_t)t->spec.n_movies * t->EP;
-  p.blob = t->blob[0];
-  p.blob_floats = t->blob_floats;
-  p.n_movies = t->spec.n_movies; p.n_users = t->spec.n_users;
-  p.EP = t->EP; p.HP = t->HP; p.n_layers = t->ly.n_layers;
-  for (int l = 0; l < t->ly.n_layers; ++l) { p.w_off[l] = t->ly.w_off[l]; p.b_off[l] = t->ly.b_off[l]; }
-  p.out_w = t->ly.out_w; p.out_b = t->ly.out_b;
-  return p;
-}
-
-// DeepFmBlob's W1 / W2 / b1 / b2 / wdeep are build_deepfm's tile order and padding; wdot and bout stay in the blob
-// (the step kernel and deepfm_blob_forward_kernel read them there), so they are zero here
-DeepFmParams deepfm_params(const srs_trainer* t) {
-  const int EP = t->EP;
-  const DeepFmBlob ly = DeepFmBlob::of(EP);
-  DeepFmParams p{};
-  const float* tabs[kDeepFmTables];
-  for (int k = 0; k < kDeepFmTables; ++k) tabs[k] = t->tab[0] + t->tab_row0[k] * EP;
-  p.fm_movie = tabs[0]; p.fm_user = tabs[1]; p.fm_mgenre = tabs[2]; p.fm_ugenre = tabs[3];
-  p.deep_movie = tabs[4]; p.deep_user = tabs[5];
-  p.W1 = t->blob[0] + ly.W1; p.b1 = t->blob[0] + ly.b1; p.W2 = t->blob[0] + ly.W2; p.b2 = t->blob[0] + ly.b2;
-  p.first = t->fo[0]; p.wdeep = t->blob[0] + ly.wdeep;
-  p.n_movies = t->spec.n_movies; p.n_users = t->spec.n_users; p.n_genres = t->spec.n_genres; p.EP = EP;
-  return p;
-}
-
 // `model.evaluate` of the trainer's current weights over n device rows, two launches on s: the serving forward
-// (ncf_kernel, or deepfm_kernel's forward with the blob's wdot / bout), then one metrics_update_kernel over all
-// the rows into em.  `err` may be null for NeuralCF only (DeepFM's genre check writes it).
+// (ncf_kernel or deepfm_kernel), then one metrics_update_kernel over all the rows into em.  `err` may be null for
+// NeuralCF only (DeepFM's genre check writes it).
 cudaError_t eval_rows(const srs_trainer* t, const DeepFmRows& r, int n, float* probs, float* logits, int* err,
-                      EpochMetrics* em, cudaStream_t s) {
+                      MetricsState* em, cudaStream_t s) {
   BatchView b{};
   b.B = n;
   b.movie_id = r.movie; b.user_id = r.user;
@@ -526,9 +389,9 @@ cudaError_t eval_rows(const srs_trainer* t, const DeepFmRows& r, int n, float* p
   cudaError_t e;
   if (t->spec.kind == SRS_DEEPFM) {
     b.movie_genre = r.mgenre; b.user_genre = r.ugenre; b.numerics = r.numerics;
-    e = launch_deepfm_blob_forward(deepfm_params(t), t->blob[0], b, s);
+    e = launch_deepfm(t->fm, b, s);
   } else {
-    e = launch_ncf(ncf_params(t), b, s);
+    e = launch_ncf(t->ncf, b, s);
   }
   if (e != cudaSuccess) return e;
   return launch_metrics_update(probs, logits, r.label, n, &em->cnt, &em->red, &em->loss, 1, s);
@@ -573,51 +436,33 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
   t->spec = s;
   t->device = device;
   t->hp = h;
-  t->E = s.emb_dim;
-  t->EP = s.emb_dim <= 12 ? 12 : s.emb_dim <= 16 ? 16 : s.emb_dim <= 32 ? 32 : 64;
+  t->EP = round_ep(s.emb_dim);
   const int EP = t->EP;
-  int64_t tab_rows;
   if (fm) {
     t->HP = 64;
+    t->place = place_deepfm(s, EP, &t->fm);
     t->blob_floats = DeepFmBlob::of(EP).floats;
     t->onehot = (int64_t)2 * s.n_genres + s.n_movies + s.n_users;
-    tab_rows = 2 * ((int64_t)s.n_movies + s.n_users) + 2 * (int64_t)s.n_genres;
-    deepfm_tensors(t);
   } else {
     t->HP = hmax <= 16 ? 16 : 32;
-    const int HP = t->HP, L = s.n_hidden;
-    // the blob layout of build_ncf: kernels [2EP or HP][HP] and biases [HP] per hidden layer, then out [HP], [4]
-    int off = 0;
-    t->ly.n_layers = L;
-    for (int l = 0; l < L; ++l) {
-      t->ly.w_off[l] = off; off += (l == 0 ? 2 * EP : HP) * HP;
-      t->ly.b_off[l] = off; off += HP;
-    }
-    t->ly.out_w = off; off += HP;
-    t->ly.out_b = off; off += 4;
-    t->ly.blob_floats = off;
-    t->blob_floats = off;
-    tab_rows = (int64_t)s.n_movies + s.n_users;
-    ncf_tensors(t);
+    t->place = place_ncf(s, EP, t->HP, &t->ncf);
+    t->blob_floats = t->ncf.blob_floats;
   }
-  t->tab_floats = tab_rows * EP;
+  t->tab_floats = table_rows(t->place) * EP;
   const int nb = t->blob_floats;
 
+  // every tensor looked up, and the Dense ones placed, before the first device call
   std::vector<float> blob(nb, 0.f), onehot(t->onehot, 0.f);
-  std::vector<std::pair<const srs_tensor*, int64_t>> tabs;   // host source, first row
-  int rc = SRS_OK;
-  for (const TrainTensor& x : t->tensors) {
-    const srs_tensor* src = find_tensor(tensors, n_tensors, x.name.c_str(), x.rows, x.cols, &rc);
-    if (!src) break;
-    if (x.row0 >= 0) { tabs.push_back({src, x.row0}); continue; }
-    for (size_t i = 0; i < x.at.size(); ++i) {
-      if (x.at[i] >= 0) blob[x.at[i]] = src->data[i];
-      else onehot[-1 - x.at[i]] = src->data[i];
-    }
+  std::vector<const float*> src;                       // each tensor's data, in placement order
+  TensorLookup lookup(tensors, n_tensors);
+  for (const Placed& x : t->place) {
+    src.push_back(lookup.host(x.name.c_str(), x.rows, x.cols));
+    if (!src.back()) { delete t; return lookup.status; }
+    scatter(x, src.back(), blob.data(), onehot.data());
   }
-  if (rc != SRS_OK) { delete t; return rc; }
 
   cudaError_t ce = cudaSetDevice(device);
+  if (ce == cudaSuccess && fm) ce = setup_deepfm_attributes();   // validation and evaluate run deepfm_kernel
   if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking);
   for (int k = 0; k < 4 && ce == cudaSuccess; ++k) ce = cudaMalloc(&t->tab[k], t->tab_floats * sizeof(float));
   for (int k = 0; k < 3 && ce == cudaSuccess; ++k) ce = cudaMalloc(&t->blob[k], (size_t)nb * sizeof(float));
@@ -630,17 +475,29 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
   if (ce == cudaSuccess) ce = cudaMemcpy(t->blob[0], blob.data(), (size_t)nb * sizeof(float), cudaMemcpyHostToDevice);
   if (ce == cudaSuccess && t->onehot)
     ce = cudaMemcpy(t->fo[0], onehot.data(), t->onehot * sizeof(float), cudaMemcpyHostToDevice);
-  for (size_t k = 0; k < tabs.size() && ce == cudaSuccess; ++k) {   // [V][E] -> [V][EP], padding stays zero
-    const srs_tensor* x = tabs[k].first;
-    ce = cudaMemcpy2D(t->tab[0] + tabs[k].second * EP, (size_t)EP * sizeof(float), x->data,
-                      (size_t)x->cols * sizeof(float), (size_t)x->cols * sizeof(float), (size_t)x->rows,
-                      cudaMemcpyHostToDevice);
+  for (size_t k = 0; k < t->place.size() && ce == cudaSuccess; ++k) {   // [V][E] -> [V][EP], padding stays zero
+    const Placed& x = t->place[k];
+    if (x.table_row < 0) continue;
+    ce = cudaMemcpy2D(t->tab[0] + x.table_row * EP, (size_t)EP * sizeof(float), src[k], (size_t)x.cols * sizeof(float),
+                      (size_t)x.cols * sizeof(float), (size_t)x.rows, cudaMemcpyHostToDevice);
   }
   if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
   if (ce != cudaSuccess) {
     trainer_free(t);
     return failf(ce == cudaErrorMemoryAllocation ? SRS_ERR_NOMEM : SRS_ERR_CUDA, "trainer setup failed: %s",
                  cudaGetErrorString(ce));
+  }
+  // the serving parameters over the trainer's arrays
+  auto table = [&](int k) { return t->tab[0] + t->place[k].table_row * EP; };
+  if (fm) {
+    t->fm.fm_movie = table(0); t->fm.fm_user = table(1); t->fm.fm_mgenre = table(2); t->fm.fm_ugenre = table(3);
+    t->fm.deep_movie = table(4); t->fm.deep_user = table(5);
+    point_into_blob(&t->fm, t->blob[0]);
+    t->fm.first = t->fo[0];
+  } else {
+    t->ncf.movie = table(0);
+    t->ncf.user = table(1);
+    t->ncf.blob = t->blob[0];
   }
   *out = t;
   return SRS_OK;
@@ -697,7 +554,7 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
   int32_t *d_order, *d_trow, *d_lab_b = nullptr, *d_frow = nullptr;
   float *d_probs, *d_logits, *d_gemb, *d_part, *d_fgrad = nullptr;
   int* d_err = nullptr;
-  EpochMetrics* d_met;
+  MetricsState* d_met;
   CUDA_TRY(sc.alloc(&d_order, (size_t)epochs * n));
   CUDA_TRY(sc.alloc(&d_trow, (size_t)n_ent * Bmax));
   CUDA_TRY(sc.alloc(&d_probs, Bmax));
@@ -706,7 +563,7 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
   CUDA_TRY(sc.alloc(&d_part, (size_t)n_cta * t->blob_floats));
   CUDA_TRY(sc.alloc(&d_met, epochs));
   CUDA_TRY(cudaMemcpyAsync(d_order, order, (size_t)epochs * n * 4, cudaMemcpyHostToDevice, s));
-  CUDA_TRY(cudaMemsetAsync(d_met, 0, sizeof(EpochMetrics) * epochs, s));
+  CUDA_TRY(cudaMemsetAsync(d_met, 0, sizeof(MetricsState) * epochs, s));
   DeepFmRows src{}, rows{};                            // the dataset, and (DeepFM) the epoch's rows in order
   CUDA_TRY(upload_rows(sc, fm, batch, labels, &src, s));
   if (fm) {
@@ -723,19 +580,20 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
   // validation: its rows uploaded once, in file order; each validated epoch's metrics in its own state
   DeepFmRows vrows{};
   float *d_vprobs = nullptr, *d_vlogits = nullptr;
-  EpochMetrics* d_vmet = nullptr;
+  MetricsState* d_vmet = nullptr;
   if (nv) {
     CUDA_TRY(upload_rows(sc, fm, val_batch, val_labels, &vrows, s));
     CUDA_TRY(sc.alloc(&d_vprobs, nv));
     CUDA_TRY(sc.alloc(&d_vlogits, nv));
     CUDA_TRY(sc.alloc(&d_vmet, epochs));
-    CUDA_TRY(cudaMemsetAsync(d_vmet, 0, sizeof(EpochMetrics) * epochs, s));
+    CUDA_TRY(cudaMemsetAsync(d_vmet, 0, sizeof(MetricsState) * epochs, s));
   }
 
   int dev_sms = 132;
   cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, t->device);
   const int adam_blocks = (int)std::min<int64_t>((t->tab_floats + 255) / 256, (int64_t)dev_sms * 8);
   const int fo_blocks = (int)std::min<int64_t>((t->onehot + 255) / 256, (int64_t)dev_sms * 8);
+  const TrainLayout ly = train_layout(t->ncf);
   StepArgs a{};
   a.tab = t->tab[0]; a.blob = t->blob[0];
   a.movie = src.movie; a.user = src.user; a.label = src.label;
@@ -743,9 +601,8 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
   a.probs = d_probs; a.logits = d_logits; a.labels = d_lab_b; a.trow = d_trow; a.gemb = d_gemb; a.part = d_part;
   DeepFmStepArgs f{};
   if (fm) {
-    f.p = deepfm_params(t);
-    for (int k = 0; k < kDeepFmTables; ++k) f.tab_row0[k] = t->tab_row0[k];
-    f.blob = t->blob[0];
+    f.p = t->fm;
+    for (int k = 0; k < kDeepFmTables; ++k) f.tab_row0[k] = t->place[k].table_row;   // the tables come first
     f.b.probs = d_probs; f.b.logits = d_logits; f.b.err_flag = d_err;
     f.trow = d_trow; f.gemb = d_gemb; f.frow = d_frow; f.fgrad = d_fgrad; f.part = d_part;
   }
@@ -777,11 +634,11 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
         a.B = B;
         a.order = d_order + (size_t)e * n + off;
         step_labels = d_lab_b;
-        CUDA_TRY(launch_step(EP, t->HP, a, t->ly, s));
+        CUDA_TRY(launch_step(EP, t->HP, a, ly, s));
         table_grad_kernel<<<(2 * a.B + 127) / 128, 128, 0, s>>>(d_trow, d_gemb, 2 * a.B, EP, t->tab[3]);
         table_adam_kernel<false><<<adam_blocks, 256, 0, s>>>(t->tab[0], t->tab[1], t->tab[2], t->tab[3],
                                                              t->tab_floats, t->hp, t->d_it);
-        dense_adam_kernel<<<1, kAdamThreads, 0, s>>>(d_part, (a.B + kTrainRows - 1) / kTrainRows, t->ly.blob_floats,
+        dense_adam_kernel<<<1, kAdamThreads, 0, s>>>(d_part, (a.B + kTrainRows - 1) / kTrainRows, t->blob_floats,
                                                      t->blob[0], t->blob[1], t->blob[2], t->hp, t->d_it);
         g_launch_count += 3;
       }
@@ -793,9 +650,9 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
     // after the epoch's last update, on the same stream: no host synchronisation
     if (nv && (e + 1) % val_freq == 0) CUDA_TRY(eval_rows(t, vrows, nv, d_vprobs, d_vlogits, d_err, &d_vmet[e], s));
   }
-  std::vector<EpochMetrics> met(epochs), vmet(nv ? epochs : 0);
-  CUDA_TRY(cudaMemcpyAsync(met.data(), d_met, sizeof(EpochMetrics) * epochs, cudaMemcpyDeviceToHost, s));
-  if (nv) CUDA_TRY(cudaMemcpyAsync(vmet.data(), d_vmet, sizeof(EpochMetrics) * epochs, cudaMemcpyDeviceToHost, s));
+  std::vector<MetricsState> met(epochs), vmet(nv ? epochs : 0);
+  CUDA_TRY(cudaMemcpyAsync(met.data(), d_met, sizeof(MetricsState) * epochs, cudaMemcpyDeviceToHost, s));
+  if (nv) CUDA_TRY(cudaMemcpyAsync(vmet.data(), d_vmet, sizeof(MetricsState) * epochs, cudaMemcpyDeviceToHost, s));
   CUDA_TRY(cudaStreamSynchronize(s));
   t->iterations += steps;
   for (int e = 0; e < epochs; ++e) {
@@ -825,16 +682,16 @@ int srs_trainer_evaluate_host(srs_trainer* t, const srs_batch* batch, const int3
   DeepFmRows rows{};
   float *d_probs, *d_logits;
   int* d_err;
-  EpochMetrics* d_met;
+  MetricsState* d_met;
   CUDA_TRY(upload_rows(sc, t->spec.kind == SRS_DEEPFM, batch, labels, &rows, s));
   CUDA_TRY(sc.alloc(&d_probs, n));
   CUDA_TRY(sc.alloc(&d_logits, n));
   CUDA_TRY(sc.alloc(&d_err, 1));
   CUDA_TRY(sc.alloc(&d_met, 1));
   CUDA_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), s));
-  CUDA_TRY(cudaMemsetAsync(d_met, 0, sizeof(EpochMetrics), s));
+  CUDA_TRY(cudaMemsetAsync(d_met, 0, sizeof(MetricsState), s));
   CUDA_TRY(eval_rows(t, rows, n, d_probs, d_logits, d_err, d_met, s));
-  EpochMetrics met;
+  MetricsState met;
   CUDA_TRY(cudaMemcpyAsync(&met, d_met, sizeof(met), cudaMemcpyDeviceToHost, s));
   CUDA_TRY(cudaStreamSynchronize(s));
   if (met.cnt.err) return failf(SRS_ERR_INVALID, "evaluate produced a probability that is NaN or outside [0, 1]");
@@ -844,23 +701,25 @@ int srs_trainer_evaluate_host(srs_trainer* t, const srs_batch* batch, const int3
 
 int srs_trainer_get_weights(const srs_trainer* t, const char* name, float* dst) {
   if (!t || !name || !dst) return failf(SRS_ERR_INVALID, "null argument");
-  const TrainTensor* x = trainer_tensor(t, name);
+  const Placed* x = nullptr;
+  for (const Placed& y : t->place)
+    if (y.name == name) x = &y;
   if (!x) return failf(SRS_ERR_MISSING, "the trainer has no tensor '%s'", name);
   CUDA_TRY(cudaSetDevice(t->device));
   CUDA_TRY(cudaStreamSynchronize(t->stream));
-  if (x->row0 >= 0) {
-    CUDA_TRY(cudaMemcpy2D(dst, (size_t)x->cols * sizeof(float), t->tab[0] + x->row0 * t->EP,
+  if (x->table_row >= 0) {
+    CUDA_TRY(cudaMemcpy2D(dst, (size_t)x->cols * sizeof(float), t->tab[0] + x->table_row * t->EP,
                            (size_t)t->EP * sizeof(float), (size_t)x->cols * sizeof(float), (size_t)x->rows,
                            cudaMemcpyDeviceToHost));
     return SRS_OK;
   }
   std::vector<float> blob(t->blob_floats), onehot;
   CUDA_TRY(cudaMemcpy(blob.data(), t->blob[0], blob.size() * sizeof(float), cudaMemcpyDeviceToHost));
-  if (t->onehot && std::any_of(x->at.begin(), x->at.end(), [](int64_t i) { return i < 0; })) {
+  if (std::any_of(x->blocks.begin(), x->blocks.end(), [](const Block& k) { return k.onehot; })) {
     onehot.resize(t->onehot);
     CUDA_TRY(cudaMemcpy(onehot.data(), t->fo[0], onehot.size() * sizeof(float), cudaMemcpyDeviceToHost));
   }
-  for (size_t i = 0; i < x->at.size(); ++i) dst[i] = x->at[i] >= 0 ? blob[x->at[i]] : onehot[-1 - x->at[i]];
+  gather(*x, blob.data(), onehot.data(), dst);
   return SRS_OK;
 }
 

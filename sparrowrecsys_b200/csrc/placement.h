@@ -1,0 +1,235 @@
+// placement.h - where the Keras tensors of the trainable models (NeuralCF's neural_cf_model_1 and two towers, and
+// DeepFM) live on the device, written once for the serving builders (build_ncf, build_deepfm in model.cu) and the
+// trainer (srs_trainer_create, srs_trainer_get_weights in ncf_train.cu): the builders and the trainer scatter the
+// caller's host tensors through it, and the trainer gathers its weights back through it.  Also the by-name lookup of
+// the caller's tensors that both use.  Host code only.
+#pragma once
+
+#include <stdint.h>
+#include <stdio.h>
+
+#include <map>
+#include <string>
+#include <vector>
+
+#include "../../include/srs_ctr.h"
+#include "hostcall.h"
+
+namespace srs {
+
+// an embedding width padded to the kernels' instantiations
+inline int round_ep(int E) {
+  if (E <= 12) return 12;
+  if (E <= 16) return 16;
+  if (E <= 32) return 32;
+  return 64;
+}
+
+// n rows start, start + 1, ... then padded - n rows of -1
+inline std::vector<int> iota_map(int start, int n, int padded) {
+  std::vector<int> v(padded, -1);
+  for (int i = 0; i < n; ++i) v[i] = start + i;
+  return v;
+}
+
+inline void append(std::vector<int>& a, const std::vector<int>& b) { a.insert(a.end(), b.begin(), b.end()); }
+
+// The caller's tensors by name (a name given twice: the last one).  A failed lookup sets `status` and the error
+// message; every later lookup then returns null and keeps them.
+struct TensorLookup {
+  std::map<std::string, const srs_tensor*> by_name;
+  int status = SRS_OK;
+
+  TensorLookup(const srs_tensor* ts, int n) {
+    for (int i = 0; i < n; ++i)
+      if (ts[i].name) by_name[ts[i].name] = &ts[i];
+  }
+
+  const srs_tensor* need(const char* name, int64_t rows, int64_t cols) {
+    if (status != SRS_OK) return nullptr;
+    auto it = by_name.find(name);
+    if (it == by_name.end()) {
+      status = failf(SRS_ERR_MISSING, "missing weight tensor '%s'", name);
+      return nullptr;
+    }
+    const srs_tensor* t = it->second;
+    if (t->rows != rows || t->cols != cols) {
+      status = failf(SRS_ERR_SHAPE, "weight '%s' has shape [%lld,%lld], expected [%lld,%lld]", name,
+                     (long long)t->rows, (long long)t->cols, (long long)rows, (long long)cols);
+      return nullptr;
+    }
+    if (t->data == nullptr) {
+      status = failf(SRS_ERR_INVALID, "weight '%s' has a null data pointer", name);
+      return nullptr;
+    }
+    return t;
+  }
+
+  // a tensor the caller holds in host memory: its data
+  const float* host(const char* name, int64_t rows, int64_t cols) {
+    const srs_tensor* t = need(name, rows, cols);
+    if (!t) return nullptr;
+    if (t->location != SRS_HOST) {
+      status = failf(SRS_ERR_INVALID, "weight '%s' must be a host tensor", name);
+      return nullptr;
+    }
+    return t->data;
+  }
+};
+
+// Rows of a Dense tensor [rows][cols] in one zero-padded block of the Dense-weight blob or of DeepFM's one-hot array
+struct Block {
+  bool onehot;                   // false: the blob; true: the [fm1_width] one-hot rows of DeepFM's dense_2/kernel
+  int at;                        // the block's first float
+  int width;                     // floats per block row: the tensor's cols, zero padded
+  std::vector<int> map;          // block row i holds tensor row map[i]; -1: a zero row
+};
+
+struct Placed {                  // one Keras tensor [rows][cols]
+  std::string name;
+  int64_t rows, cols;
+  int64_t table_row;             // an embedding table: its first row in a trainer's [sum of rows][EP] array; else -1
+  std::vector<Block> blocks;     // a Dense tensor: where its rows go
+};
+
+// a model's tensors in the order they are looked up: its tables, then its Dense tensors
+using Placement = std::vector<Placed>;
+
+inline void place_table(Placement& pl, const char* name, int64_t rows, int E) {
+  const int64_t row = pl.empty() ? 0 : pl.back().table_row + pl.back().rows;
+  pl.push_back(Placed{name, rows, E, row, {}});
+}
+
+inline void place_dense(Placement& pl, const char* name, int64_t rows, int64_t cols, std::vector<Block> blocks) {
+  pl.push_back(Placed{name, rows, cols, -1, std::move(blocks)});
+}
+
+// The rows of a trainer's table array: the tables' rows, one table after another
+inline int64_t table_rows(const Placement& pl) {
+  int64_t n = 0;
+  for (const Placed& x : pl)
+    if (x.table_row >= 0) n += x.rows;
+  return n;
+}
+
+// NeuralCF and two towers.  The blob: per hidden layer its kernel [2EP (two towers: EP) or HP][HP] and its bias
+// [HP] (two towers: the item tower's layers, then the user tower's), then the output kernel and bias, each block a
+// multiple of 4 floats.  Fills p's layout: EP, HP, n_layers, the offsets and blob_floats.  Without dense_out, two
+// towers' out_w and out_b are 4 floats each that no tensor fills (build_ncf writes 1 and 0).
+inline Placement place_ncf(const srs_spec& s, int EP, int HP, NcfParams* p) {
+  const int E = s.emb_dim, L = s.n_hidden;
+  const bool two = s.kind == SRS_TWOTOWERS;
+  Placement pl;
+  place_table(pl, "movieId_embedding", s.n_movies, E);
+  place_table(pl, "userId_embedding", s.n_users, E);
+  int off = 0;
+  auto dense = [&](const char* name, int64_t rows, int64_t cols, std::vector<int> map, int width) {
+    const int at = off;
+    off += ((int)map.size() * width + 3) / 4 * 4;
+    place_dense(pl, name, rows, cols, {Block{false, at, width, std::move(map)}});
+    return at;
+  };
+  char k[48], b[48];
+  for (int t = 0; t < (two ? 2 : 1); ++t) {
+    int in = two ? E : 2 * E;
+    for (int l = 0; l < L; ++l) {
+      const int out = s.hidden[l];
+      if (two) {
+        snprintf(k, sizeof k, "%s_dense_%d/kernel", t ? "user" : "item", l);
+        snprintf(b, sizeof b, "%s_dense_%d/bias", t ? "user" : "item", l);
+      } else {
+        snprintf(k, sizeof k, "dense_%d/kernel", l);
+        snprintf(b, sizeof b, "dense_%d/bias", l);
+      }
+      std::vector<int> map;
+      if (l == 0) {                                     // the embedding rows, each side padded to EP
+        map = iota_map(0, E, EP);
+        if (!two) append(map, iota_map(E, E, EP));
+      } else {
+        map = iota_map(0, in, HP);
+      }
+      p->w_off[3 * t + l] = dense(k, in, out, map, HP);
+      p->b_off[3 * t + l] = dense(b, out, 1, iota_map(0, out, HP), 1);
+      in = out;
+    }
+    if (!two) {
+      snprintf(k, sizeof k, "dense_%d/kernel", L);
+      snprintf(b, sizeof b, "dense_%d/bias", L);
+      p->out_w = dense(k, in, 1, iota_map(0, in, HP), 1);
+      p->out_b = dense(b, 1, 1, iota_map(0, 1, 4), 1);
+    }
+  }
+  if (two && s.final_dense) {
+    p->out_w = dense("dense_out/kernel", 1, 1, iota_map(0, 1, 4), 1);
+    p->out_b = dense("dense_out/bias", 1, 1, iota_map(0, 1, 4), 1);
+  } else if (two) {
+    p->out_w = off; off += 4;
+    p->out_b = off; off += 4;
+  }
+  p->blob_floats = off;
+  p->n_movies = s.n_movies; p->n_users = s.n_users;
+  p->EP = EP; p->HP = HP; p->n_layers = L; p->two_towers = two; p->final_dense = s.final_dense;
+  return pl;
+}
+
+// DeepFM: the six tables in kDeepFmTables order, the Dense tensors in a DeepFmBlob::of(EP) and the one-hot rows of
+// dense_2/kernel in their own [fm1_width] array.  Fills p's sizes and EP.
+inline Placement place_deepfm(const srs_spec& s, int EP, DeepFmParams* p) {
+  const int E = s.emb_dim, h0 = s.hidden[0], h1 = s.hidden[1];
+  const int fm1 = 2 * s.n_genres + s.n_movies + s.n_users;
+  const DeepFmBlob ly = DeepFmBlob::of(EP);
+  Placement pl;
+  place_table(pl, "fm_movieId_embedding", s.n_movies, E);
+  place_table(pl, "fm_userId_embedding", s.n_users, E);
+  place_table(pl, "fm_movieGenre1_embedding", s.n_genres, E);
+  place_table(pl, "fm_userGenre1_embedding", s.n_genres, E);
+  place_table(pl, "deep_movieId_embedding", s.n_movies, E);
+  place_table(pl, "deep_userId_embedding", s.n_users, E);
+  // dense/kernel's rows are DenseFeatures' sorted concat (movieAvgRating | deep movieId | 4 numerics | deep userId |
+  // 2 numerics); its tile rows are deep movieId | deep userId | the 7 numerics and one zero row
+  std::vector<int> map;
+  append(map, iota_map(1, E, EP));
+  append(map, iota_map(5 + E, E, EP));
+  for (int r : {0, 1 + E, 2 + E, 3 + E, 4 + E, 5 + 2 * E, 6 + 2 * E, -1}) map.push_back(r);
+  place_dense(pl, "dense/kernel", 7 + 2 * E, h0, {Block{false, ly.W1, 64, map}});
+  place_dense(pl, "dense/bias", h0, 1, {Block{false, ly.b1, 1, iota_map(0, h0, 64)}});
+  place_dense(pl, "dense_1/kernel", h0, h1, {Block{false, ly.W2, 64, iota_map(0, h0, 64)}});
+  place_dense(pl, "dense_1/bias", h1, 1, {Block{false, ly.b2, 1, iota_map(0, h1, 64)}});
+  // dense_2/kernel: the one-hot rows (movieGenre1 | movieId | userGenre1 | userId), the four dot rows, the deep rows
+  place_dense(pl, "dense_2/kernel", fm1 + 4 + h1, 1,
+              {Block{true, 0, 1, iota_map(0, fm1, fm1)}, Block{false, ly.wdot, 1, iota_map(fm1, 4, 4)},
+               Block{false, ly.wdeep, 1, iota_map(fm1 + 4, h1, 64)}});
+  place_dense(pl, "dense_2/bias", 1, 1, {Block{false, ly.bout, 1, iota_map(0, 1, 1)}});
+  p->n_movies = s.n_movies; p->n_users = s.n_users; p->n_genres = s.n_genres; p->EP = EP;
+  return pl;
+}
+
+// p's Dense-weight pointers into a DeepFmBlob on the device
+inline void point_into_blob(DeepFmParams* p, const float* blob) {
+  const DeepFmBlob ly = DeepFmBlob::of(p->EP);
+  p->blob = blob;
+  p->W1 = blob + ly.W1; p->b1 = blob + ly.b1; p->W2 = blob + ly.W2; p->b2 = blob + ly.b2;
+  p->wdeep = blob + ly.wdeep;
+}
+
+// a Dense tensor's data [rows][cols] into its blocks; what no block row takes stays as it was (zero)
+inline void scatter(const Placed& x, const float* src, float* blob, float* onehot) {
+  for (const Block& k : x.blocks) {
+    float* dst = (k.onehot ? onehot : blob) + k.at;
+    for (size_t i = 0; i < k.map.size(); ++i)
+      if (k.map[i] >= 0)
+        for (int64_t j = 0; j < x.cols; ++j) dst[i * k.width + j] = src[(size_t)k.map[i] * x.cols + j];
+  }
+}
+
+// the inverse: a Dense tensor's data [rows][cols] from its blocks
+inline void gather(const Placed& x, const float* blob, const float* onehot, float* dst) {
+  for (const Block& k : x.blocks) {
+    const float* src = (k.onehot ? onehot : blob) + k.at;
+    for (size_t i = 0; i < k.map.size(); ++i)
+      if (k.map[i] >= 0)
+        for (int64_t j = 0; j < x.cols; ++j) dst[(size_t)k.map[i] * x.cols + j] = src[i * k.width + j];
+  }
+}
+
+}  // namespace srs

@@ -2,10 +2,10 @@
 
 NeuralCF's step is `ncf_train_step_kernel<EP, HP>` (EP in {12, 16, 32, 64}, HP in {16, 32}; csrc/ncf_train.cu) over
 1 to 3 hidden layers; it asks for more than 48 KiB of dynamic shared memory only when a shape needs it, and asks
-again when a later shape of the same instantiation needs more.  DeepFM's is `deepfm_train_step_kernel<EP>`, with
-`deepfm_blob_forward_kernel<EP>` for validation and `Trainer.evaluate` (csrc/deepfm_train.cu).  The trainer keeps its
-own copy of the serving builders' weight layout (`ncf_tensors`, `deepfm_tensors`, `ncf_params`, `deepfm_params`).
-The defects such code invites - a padded column read as data, the last real column or unit dropped, the wrong
+again when a later shape of the same instantiation needs more.  DeepFM's is `deepfm_train_step_kernel<EP>`
+(csrc/deepfm_train.cu), with the serving `deepfm_kernel<EP>` for validation and `Trainer.evaluate`.  The trainer places
+its weights through the serving builders' placement (csrc/placement.h) and gathers its exports back through it, and
+its step kernels restate the layout's offsets.  The defects such code invites - a padded column read as data, the last real column or unit dropped, the wrong
 template, a tail tile mishandled - compound over a fit's steps.  `FIT_MATRIX` names one case per (model,
 instantiation, width regime): the smallest E of a bucket, a partial pad and the exact bucket width, hidden width 1
 and each model's limit, batches one row past the step's row tile or its double (64 rows for NeuralCF, 32 for DeepFM),
@@ -74,7 +74,7 @@ FIT_MATRIX = [
     # measured on an H100 at 700 W: dense_2/bias lands 5.8x the float32 spread from float64, but that spread is
     # 0.3 ulp and the error 1.7 ulp, inside the rule's one-ulp term
     _ncf(64, (32, 17), 200, 1877, 9, ADAM, **TINY),              # <64, 32>   84.6 KiB, below the size opted in
-    # ---- deepfm_train_step_kernel<EP> and deepfm_blob_forward_kernel<EP>: every EP; widths 1 and 64 ----
+    # ---- deepfm_train_step_kernel<EP> and deepfm_kernel<EP>: every EP; widths 1 and 64 ----
     _fm(1, (1, 1), 33, 314, 0),                                  # EP 12
     _fm(12, (64, 64), 65, 615, 1, ADAM),                         # EP 12
     _fm(13, (17, 33), 33, 314, 2, ADAM_NO_MOMENTUM),             # EP 16
@@ -124,11 +124,12 @@ def instantiations(c):
     EP = round_ep(spec.emb_dim)
     if c.model == "neuralcf":
         return {("ncf_train_step_kernel", EP, 16 if max(spec.hidden) <= 16 else 32)}
-    return {("deepfm_train_step_kernel", EP), ("deepfm_blob_forward_kernel", EP)}
+    return {("deepfm_train_step_kernel", EP), ("deepfm_kernel", EP)}
 
 
 def dispatched_instantiations():
-    """Every instantiation the trainer's launchers in csrc/*.cu can dispatch, read from their dispatch lines."""
+    """Every instantiation the trainer's launchers in csrc/*.cu can dispatch, read from their dispatch lines: the step
+    kernels' cases, and the cases of `launch_deepfm`'s switch (the trainer's DeepFM forward)."""
     found = set()
     for path in sorted(glob.glob(os.path.join(CSRC, "*.cu"))):
         with open(path) as f:
@@ -137,8 +138,10 @@ def dispatched_instantiations():
             found.add(("ncf_train_step_kernel", int(ep), int(hp)))
         for ep in re.findall(r"SRS_DEEPFM_TRAIN_CASE\((\d+)\)", src):
             found.add(("deepfm_train_step_kernel", int(ep)))
-        for ep in re.findall(r"SRS_DEEPFM_FWD_CASE\((\d+)\)", src):
-            found.add(("deepfm_blob_forward_kernel", int(ep)))
+        launcher = re.search(r"cudaError_t launch_deepfm\(const DeepFmParams& p.*?\n}", src, re.S)
+        if launcher:
+            for ep in re.findall(r"case (\d+): return launch_deepfm_t<(?:\d+)>", launcher.group(0)):
+                found.add(("deepfm_kernel", int(ep)))
     return found
 
 
@@ -223,10 +226,12 @@ def _distance(Wa, Wb, tol):
 
 
 # ---- CPU: the matrix is complete, and its tolerances see the defects -------------------------------------
-def test_matrix_reaches_every_dispatched_instantiation():
+def test_matrix_reaches_every_step_and_forward_instantiation():
+    """Every step-kernel instantiation the trainer dispatches, and every `deepfm_kernel` instantiation (the trainer's
+    DeepFM forward for validation and evaluate), is run by some FIT_MATRIX case."""
     dispatched = dispatched_instantiations()
     assert {d[0] for d in dispatched} == {"ncf_train_step_kernel", "deepfm_train_step_kernel",
-                                          "deepfm_blob_forward_kernel"}, dispatched
+                                          "deepfm_kernel"}, dispatched
     reached = set().union(*(instantiations(c) for c in FIT_MATRIX))
     missing = sorted(dispatched - reached)
     assert not missing, "no FIT_MATRIX case runs %s" % ", ".join("%s<%s>" % (d[0], ", ".join(map(str, d[1:])))
@@ -408,8 +413,8 @@ def test_step_forward_is_the_serving_forward(case):
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", FIT_MATRIX, ids=_case_id)
 def test_padding_stays_zero(case):
-    """After the fit, the trainer's evaluate (its own padded arrays through `ncf_params` / `deepfm_params`) is the
-    evaluate of a serving model built from the exported weights, whose padding is zero by construction."""
+    """After the fit, the trainer's evaluate (its own padded arrays, through the NcfParams / DeepFmParams it keeps over
+    them) is the evaluate of a serving model built from the exported weights, whose padding is zero by construction."""
     W0, f, orders = _inputs(case)
     with _trainer(case, W0) as tr:
         tr.fit(f, epochs=case.epochs, batch_size=case.B, order=orders)

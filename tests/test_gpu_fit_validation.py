@@ -233,6 +233,40 @@ def test_rejected_validation_leaves_the_trainer_unchanged(data, model):
         assert tr.iterations == it + 9 and len(h["val_loss"]) == 1
 
 
+_FRESH_EVALUATE = """
+import json, os, sys
+import numpy as np
+from sparrowrecsys_b200.model import CTRModel
+from sparrowrecsys_b200.spec import default_spec
+from sparrowrecsys_b200.training import Trainer
+from sparrowrecsys_b200.weights import init_weights
+test = dict(np.load(os.path.join(sys.argv[1], "dien_testset.npz")))
+val = {k: np.ascontiguousarray(v[:500]) for k, v in test.items()}
+spec = default_spec("deepfm", emb_dim=64)
+with Trainer(spec, init_weights(spec, 3, for_test=True)) as tr:
+    got = tr.evaluate(val)
+    W = tr.weights()
+with CTRModel(spec, W, options={"deepfm_impl": "cudacore"}) as m:
+    ref = m.evaluate(val, batch_size=500)
+print(json.dumps([list(got), list(ref)]))
+"""
+
+
+@pytest.mark.gpu
+def test_deepfm_trainer_evaluates_in_a_process_without_a_model():
+    """The trainer's DeepFM forward is deepfm_kernel, whose dynamic shared memory opt-in (at E = 64, above the 48 KiB
+    default) srs_model_create also sets: a trainer created in a fresh process, before any CTRModel, must set it itself.
+    Its evaluate then equals that of a model rebuilt from its weights."""
+    import subprocess
+    import sys
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    r = subprocess.run([sys.executable, "-c", _FRESH_EVALUATE, GOLDEN], capture_output=True, text=True, cwd=root,
+                       timeout=300)
+    assert r.returncode == 0, r.stdout + r.stderr
+    got, ref = json.loads(r.stdout.strip().splitlines()[-1])
+    assert got == ref
+
+
 @pytest.mark.gpu
 def test_abi_rejects_bad_validation_rows_before_any_launch(data):
     """The library's own checks past encode_batch: a validation genre >= n_genres is SRS_ERR_RANGE naming the
