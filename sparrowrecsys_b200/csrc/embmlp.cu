@@ -9,8 +9,9 @@
 //
 // A CTA owns a tile of 64 rows: the gathers land directly in the shared-memory
 // input tile (slot-major, 128-bit stores), the three Dense layers run on the tile
-// with register-tiled FFMA, only the scores leave the SM.
-#include "kernels.h"
+// with register-tiled FFMA, only the scores leave the SM.  The tile forward is
+// embmlp_layers.cuh's, shared with Wide&Deep's training step.
+#include "embmlp_layers.cuh"
 
 namespace srs {
 
@@ -19,10 +20,9 @@ constexpr int kEmbRows = 64;
 template <int EP>
 __global__ void __launch_bounds__(kThreads) embmlp_kernel(EmbMlpParams p, BatchView b) {
   constexpr int R = kEmbRows;
-  constexpr int Q = EP / 4;
-  constexpr int KP = 10 * EP + kNumPad;
-  constexpr int LDX = KP + 4;
-  constexpr int LDH = 128 + 4;
+  constexpr int KP = EmbMlpTile<EP>::KP;
+  constexpr int LDX = EmbMlpTile<EP>::LDX;
+  constexpr int LDH = EmbMlpTile<EP>::LDH;
   static_assert(LDX >= LDH, "second hidden tile aliases the input tile");
   constexpr bool STAGE_W1 = EP == 12;      // 64 KB: fits next to the tiles only for the reference shape
   constexpr bool STAGE_W2 = EP <= 32;      // 64 KB
@@ -31,65 +31,16 @@ __global__ void __launch_bounds__(kThreads) embmlp_kernel(EmbMlpParams p, BatchV
   float* H1 = smem + R * LDX;
   float* W2s = H1 + R * LDH;               // [128][128] if STAGE_W2
   float* W1s = W2s + (STAGE_W2 ? 128 * 128 : 0);   // [KP][128] if STAGE_W1
-  const int tid = threadIdx.x;
   const int row0 = blockIdx.x * R;
   if (STAGE_W1) stage_weights(W1s, p.W1, KP * 128);
   if (STAGE_W2) stage_weights(W2s, p.W2, 128 * 128);
 
-  for (int i = tid; i < R * 10 * Q; i += kThreads) {
-    const int q = i % Q;
-    const int t = i / Q;
-    const int slot = t % 10;
-    const int r = t / 10;
-    const int row = row0 + r;
-    int id = -1;
-    const float* table = p.movie;
-    if (row < b.B) {
-      if (slot < 3) {
-        id = __ldg(b.movie_genre + row * 3 + slot);
-        table = p.genre[slot];
-      } else if (slot == 3) {
-        id = checked_id(__ldg(b.movie_id + row), p.n_movies, b.err_flag);
-      } else if (slot < 9) {
-        id = __ldg(b.user_genre + row * 5 + (slot - 4));
-        table = p.genre[slot - 1];
-      } else {
-        id = checked_id(__ldg(b.user_id + row), p.n_users, b.err_flag);
-        table = p.user;
-      }
-      if (slot != 3 && slot != 9) {                 // vocabulary column: -1 = missing / OOV
-        if (id >= p.n_genres) { atomicExch(b.err_flag, 1); id = -1; }
-        if (id < 0) id = -1;
-      }
-    }
-    gather_row<EP>(Xs + r * LDX + slot * EP, table, id, q);
-  }
-  for (int i = tid; i < R * kNumPad; i += kThreads) {
-    const int r = i / kNumPad, j = i % kNumPad;
-    const int row = row0 + r;
-    float v = 0.f;
-    if (j < kNumNumerics && row < b.B) v = __ldg(b.numerics + row * kNumNumerics + j);
-    Xs[r * LDX + 10 * EP + j] = v;
-  }
+  embmlp_tile_gather<EP, R>(p, b, row0, Xs);
   if (STAGE_W1 || STAGE_W2) stage_wait();
   __syncthreads();
-  if (STAGE_W1) dense_layer<R, 128, 4, 8, true>(Xs, LDX, KP, W1s, p.b1, ACT_RELU, nullptr, H1, LDH);
-  else dense_layer<R, 128, 4, 8>(Xs, LDX, KP, p.W1, p.b1, ACT_RELU, nullptr, H1, LDH);
-  __syncthreads();
   float* H2 = Xs;
-  if (STAGE_W2) dense_layer<R, 128, 4, 8, true>(H1, LDH, 128, W2s, p.b2, ACT_RELU, nullptr, H2, LDX);
-  else dense_layer<R, 128, 4, 8>(H1, LDH, 128, p.W2, p.b2, ACT_RELU, nullptr, H2, LDX);
-  __syncthreads();
-  row_dot<R>(H2, LDX, 128, p.w3, [&](int r, float s) {
-    const int row = row0 + r;
-    if (row >= b.B) return;
-    float z = s + p.b3;
-    if (p.wide) {
-      const int mid = checked_id(__ldg(b.movie_id + row), p.n_movies, b.err_flag);
-      const int rated = checked_id(__ldg(b.hist + (size_t)row * b.hist_stride), p.n_movies,
-                                   b.err_flag);
-      z += __ldg(p.wide + crossed_bucket(mid, rated, (uint32_t)p.cross_buckets));
-    }
+  embmlp_tile_mlp<EP, R, STAGE_W1, STAGE_W2>(p, Xs, STAGE_W1 ? W1s : p.W1, STAGE_W2 ? W2s : p.W2, H1, H2, LDX);
+  embmlp_tile_logits<R>(p, b, row0, H2, LDX, [&](int, int row, float z, int) {
     store_score(b, row, sigmoidf_acc(z));
     if (b.logits) b.logits[row] = z;
   });

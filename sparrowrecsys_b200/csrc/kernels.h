@@ -45,11 +45,48 @@ struct EmbMlpParams {
   const float* W2;         // [128][128]
   const float* b2;         // [128]
   const float* w3;         // [128] deep rows of dense_2
+  const float* b3;         // [1] dense_2/bias, on the device: a trainer's Adam writes it there every step
   const float* wide;       // [cross_buckets] wide rows of dense_2 (nullptr for EmbeddingMLP)
-  float b3;
   int n_movies, n_users, n_genres, cross_buckets;
   int EP;
 };
+
+// The Dense weights of EmbeddingMLP and Wide&Deep (a model's and a trainer's) as one blob, offsets in floats:
+// W1 [10EP + 8][128] in the tile order of embmlp_layers.cuh, b1 [128], W2 [128][128], b2 [128], w3 [128] (the deep
+// rows of dense_2/kernel), b3 (dense_2/bias) and 3 floats of padding; hidden widths zero padded to 128, every array
+// 16-byte aligned.  Wide&Deep's wide rows of dense_2/kernel live apart (placement.h).
+struct EmbMlpBlob {
+  int W1, b1, W2, b2, w3, b3, floats;
+  __host__ __device__ static EmbMlpBlob of(int EP) {
+    EmbMlpBlob l;
+    l.W1 = 0;
+    l.b1 = (10 * EP + kNumPad) * 128;
+    l.W2 = l.b1 + 128;
+    l.b2 = l.W2 + 128 * 128;
+    l.w3 = l.b2 + 128;
+    l.b3 = l.w3 + 128;
+    l.floats = l.b3 + 4;
+    return l;
+  }
+};
+cudaError_t setup_embmlp_attributes();   // embmlp_kernel's dynamic shared memory opt-in
+
+// ---- Wide&Deep's training step (widendeep_train.cu; DESIGN.md section 4.18) ---------------------------------------
+constexpr int kWideDeepTables = 10;   // the kernel's slots: movieGenre1..3, movieId, userGenre1..5, userId
+struct WideDeepStepArgs {
+  EmbMlpParams p;          // the trainer's tables, Dense weights and wide rows
+  BatchView b;             // the step's B rows in order (hist: userRatedMovie1, stride 1); probs / logits receive
+                           // its outputs before the update
+  const int32_t* label;    // [B]
+  int64_t tab_row0[kWideDeepTables];   // first row of each slot's table in the trainer's table array
+  int32_t* trow;           // [10B] table row of entry s * B + r, -1 = none (a missing genre)
+  float* gemb;             // [10B][EP] the entries' gradients
+  int32_t* wrow;           // [B] wide row (crossed bucket) of row r
+  float* wgrad;            // [B] its gradient (the row's dL/dz)
+  float* part;             // [ctas][EmbMlpBlob::floats] per-CTA Dense gradient sums
+};
+int widendeep_train_ctas(int B);
+cudaError_t launch_widendeep_train_step(const WideDeepStepArgs& a, cudaStream_t s);
 
 // ---- EmbeddingMLP / Wide&Deep on tensor cores (embmlp_tc.cu): E <= 12 ------------------------
 struct EmbMlpTcParams {
@@ -124,17 +161,21 @@ struct DeepFmStepArgs {
 };
 int deepfm_train_ctas(int B);
 cudaError_t launch_deepfm_train_step(const DeepFmStepArgs& a, cudaStream_t s);
-struct DeepFmRows {        // a DeepFM dataset on the device, in the srs_batch layout
+struct DeepFmRows {        // a DeepFM or Wide&Deep dataset on the device, in the srs_batch layout
   int32_t* movie;          // [n]
   int32_t* user;           // [n]
-  int32_t* mgenre;         // [n][3], column 0 read
-  int32_t* ugenre;         // [n][5], column 0 read
+  int32_t* mgenre;         // [n][3], column 0 read (DeepFM)
+  int32_t* ugenre;         // [n][5], column 0 read (DeepFM)
   float* numerics;         // [n][7]
   int32_t* label;          // [n]
+  int32_t* rated;          // [n] userRatedMovie1 (Wide&Deep; null otherwise)
 };
 // dst row i = src row order[i], i < n (genres: column 0 only)
 cudaError_t launch_deepfm_permute(const DeepFmRows& src, const DeepFmRows& dst, const int32_t* order, int n,
                                   cudaStream_t s);
+// the same for Wide&Deep: every genre column and userRatedMovie1
+cudaError_t launch_widendeep_permute(const DeepFmRows& src, const DeepFmRows& dst, const int32_t* order, int n,
+                                     cudaStream_t s);
 
 // ---- DeepFM with the deep MLP on tensor cores (deepfm_tc.cu): emb_dim 13..16 --------------------
 struct DeepFmTcParams {

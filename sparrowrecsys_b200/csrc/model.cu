@@ -332,49 +332,17 @@ int build_ncf(Builder& B) {
 int build_embmlp(Builder& B) {
   srs_model* m = B.m;
   const srs_spec& s = m->spec;
-  const int E = s.emb_dim, EP = m->EP;
   const bool wide = s.kind == SRS_WIDENDEEP;
   if (s.n_hidden != 2 || s.hidden[0] > 128 || s.hidden[1] > 128 || s.hidden[0] < 1 || s.hidden[1] < 1)
     return fail(SRS_ERR_INVALID, "EmbeddingMLP/W&D need two hidden layers of width <= 128");
-  const int h0 = s.hidden[0], h1 = s.hidden[1];
   EmbMlpParams& p = m->emb;
-  char name[64];
-  for (int k = 0; k < 3; ++k) {
-    snprintf(name, sizeof(name), "movieGenre%d_embedding", k + 1);
-    p.genre[k] = B.table(name, s.n_genres, E);
-  }
-  for (int k = 0; k < 5; ++k) {
-    snprintf(name, sizeof(name), "userGenre%d_embedding", k + 1);
-    p.genre[3 + k] = B.table(name, s.n_genres, E);
-  }
-  p.movie = B.table("movieId_embedding", s.n_movies, E);
-  p.user = B.table("userId_embedding", s.n_users, E);
-  // reference row order of dense/kernel: DenseFeatures sorted concat (SURVEY.md 8a row a2)
-  std::vector<int> map;
-  for (int k = 0; k < 3; ++k) append(map, iota_map(1 + k * E, E, EP));         // movieGenre1..3
-  append(map, iota_map(1 + 3 * E, E, EP));                                        // movieId
-  for (int k = 0; k < 5; ++k) append(map, iota_map(5 + 4 * E + k * E, E, EP));   // userGenre1..5
-  append(map, iota_map(5 + 9 * E, E, EP));                                        // userId
-  const int nums[8] = {0, 1 + 4 * E, 2 + 4 * E, 3 + 4 * E, 4 + 4 * E, 5 + 10 * E, 6 + 10 * E, -1};
-  for (int j = 0; j < 8; ++j) map.push_back(nums[j]);
-  const float* k1 = B.host("dense/kernel", 7 + 10 * E, h0);
-  const float* b1 = B.host("dense/bias", h0, 1);
-  const float* k2 = B.host("dense_1/kernel", h0, h1);
-  const float* b2 = B.host("dense_1/bias", h1, 1);
-  const int last_in = h1 + (wide ? s.cross_buckets : 0);
-  const float* k3 = B.host("dense_2/kernel", last_in, 1);
-  const float* b3 = B.host("dense_2/bias", 1, 1);
+  const Placement pl = place_embmlp(s, m->EP, &p);
+  std::vector<float> blob(EmbMlpBlob::of(m->EP).floats, 0.f), wide_rows(wide ? s.cross_buckets : 0, 0.f);
+  const float* tables[kWideDeepTables];
+  place_host(B, pl, tables, blob.data(), wide_rows.data());
   if (B.status != SRS_OK) return B.status;
-  p.W1 = B.upload(B.permute(k1, h0, map, 128));
-  p.b1 = B.upload(B.padvec(b1, h0, 128));
-  p.W2 = B.upload(B.permute(k2, h1, iota_map(0, h0, 128), 128));
-  p.b2 = B.upload(B.padvec(b2, h1, 128));
-  p.w3 = B.upload(B.padvec(k3, h1, 128));
-  p.wide = nullptr;
-  if (wide) p.wide = B.upload(std::vector<float>(k3 + h1, k3 + h1 + s.cross_buckets));
-  p.b3 = b3[0];
-  p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres;
-  p.cross_buckets = s.cross_buckets; p.EP = EP;
+  point_into_blob(&p, tables, B.upload(blob));
+  p.wide = wide ? B.upload(wide_rows) : nullptr;
   m->kernel_name = wide ? "embmlp_kernel<wide&deep>" : "embmlp_kernel";
   return B.status;
 }
@@ -737,6 +705,7 @@ int build_embmlp_tc(Builder& B) {
   const int E = s.emb_dim, h0 = s.hidden[0], h1 = s.hidden[1];
   const float* k1 = B.host("dense/kernel", 7 + 10 * E, h0);
   const float* k2 = B.host("dense_1/kernel", h0, h1);
+  const float* b3 = B.host("dense_2/bias", 1, 1);
   if (B.status != SRS_OK) return B.status;
   // K = slot * 12 + e; slot order of the kernel's gather: movieGenre1..3, movieId, userGenre1..5, userId
   int slot_start[10];
@@ -764,7 +733,7 @@ int build_embmlp_tc(Builder& B) {
   for (int k = 0; k < 8; ++k) p.genre[k] = v1.genre[k];
   p.movie = v1.movie; p.user = v1.user;
   p.image = B.upload(img);
-  p.b1 = v1.b1; p.b2 = v1.b2; p.w3 = v1.w3; p.wide = v1.wide; p.b3 = v1.b3;
+  p.b1 = v1.b1; p.b2 = v1.b2; p.w3 = v1.w3; p.wide = v1.wide; p.b3 = b3[0];
   p.w1num = B.upload(w1num);
   p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres; p.cross_buckets = s.cross_buckets;
   p.num_sms = m->device_sms;

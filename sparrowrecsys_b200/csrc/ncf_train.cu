@@ -1,6 +1,7 @@
 // ncf_train.cu - `model.fit` on the device: the C ABI's srs_trainer (include/srs_ctr.h), which trains NeuralCF
-// (neural_cf_model_1, NeuralCF.py:74-91; DESIGN.md section 4.8) and DeepFM (DeepFM.py; section 4.9, its step kernel
-// in deepfm_train.cu), and the kernels both models share: dedupe, the two forms of Adam, metrics.
+// (neural_cf_model_1, NeuralCF.py:74-91; DESIGN.md section 4.8), DeepFM (DeepFM.py; section 4.9, its step kernel
+// in deepfm_train.cu) and Wide&Deep (WideNDeep.py; section 4.18, its step kernel in widendeep_train.cu), and the
+// kernels the models share: dedupe, the two forms of Adam, metrics.
 //
 // NeuralCF's step of batch B_b (rows order[off .. off + B_b) of the uploaded dataset), five launches, no host sync:
 //   ncf_train_step_kernel  forward (the arithmetic of ncf_kernel) and backward, one thread per row; the Dense
@@ -16,10 +17,14 @@
 // DeepFM's step is seven launches: deepfm_train_step_kernel, table_grad_kernel over its table entries and again over
 // its one-hot entries, table_adam_kernel<false> over the six tables and <true> over dense_2/kernel's one-hot rows,
 // dense_adam_kernel, metrics_update_kernel; plus deepfm_permute_kernel once per epoch.
+// Wide&Deep's step is seven launches of the same shape: widendeep_train_step_kernel, table_grad_kernel over its ten
+// tables' entries and again (width 1) over its wide entries, table_adam_kernel<false> over the ten tables and <true>
+// over the cross_buckets wide rows of dense_2/kernel, dense_adam_kernel, metrics_update_kernel; plus
+// widendeep_permute_kernel once per epoch.
 // No float atomics: every sum has a fixed order, so a fit is bitwise reproducible.
 //
 // Validation (srs_trainer_fit_validate_host) and srs_trainer_evaluate_host run the serving forward over the
-// trainer's arrays (ncf_kernel, deepfm_kernel) and one metrics_update_kernel over all the rows: two launches, with the
+// trainer's arrays (ncf_kernel, deepfm_kernel, embmlp_kernel) and one metrics_update_kernel over all the rows: two launches, with the
 // bits of a CTRModel built from the exported weights.  The trainer's arrays hold the weights where the serving
 // builders put them: both place them through placement.h.
 #include <cuda_runtime.h>
@@ -288,10 +293,11 @@ struct srs_trainer {
   Placement place;                    // where the Keras tensors live in tab, blob and fo
   NcfParams ncf{};                    // the serving parameters over the trainer's arrays (NeuralCF)
   DeepFmParams fm{};                  //   (DeepFM)
+  EmbMlpParams emb{};                 //   (Wide&Deep)
   int64_t tab_floats = 0;             // (sum of the tables' rows) * EP
   float* tab[4] = {};                 // w, m, v, G   [rows][EP], padding zero
   float* blob[3] = {};                // w, m, v      [blob_floats]
-  int64_t onehot = 0;                 // DeepFM: the one-hot rows of dense_2/kernel (fm1_width)
+  int64_t onehot = 0;                 // the one-hot rows of dense_2/kernel: DeepFM's fm1_width, Wide&Deep's wide rows
   float* fo[4] = {};                  // w, m, v, G   [onehot]
   long long* d_it = nullptr;          // Adam's iteration counter, on the device
   int64_t iterations = 0;             // its host mirror
@@ -311,10 +317,11 @@ void trainer_free(srs_trainer* t) {
   delete t;
 }
 
-// a DeepFM dataset of n rows on the device
-DeepFmRows deepfm_rows(Scratch& sc, int n, cudaError_t* e) {
+// a DeepFM (wd: Wide&Deep) dataset of n rows on the device
+DeepFmRows deepfm_rows(Scratch& sc, int n, bool wd, cudaError_t* e) {
   DeepFmRows r{};
   *e = sc.alloc(&r.movie, n);
+  if (*e == cudaSuccess && wd) *e = sc.alloc(&r.rated, n);
   if (*e == cudaSuccess) *e = sc.alloc(&r.user, n);
   if (*e == cudaSuccess) *e = sc.alloc(&r.mgenre, (size_t)n * 3);
   if (*e == cudaSuccess) *e = sc.alloc(&r.ugenre, (size_t)n * 5);
@@ -326,11 +333,14 @@ DeepFmRows deepfm_rows(Scratch& sc, int n, cudaError_t* e) {
 // The checks of rows the trainer reads (fit, validation, evaluate), all made before any launch.  `what` prefixes
 // the messages: "" or "validation data: ".
 int check_rows(const srs_trainer* t, const srs_batch* batch, const int32_t* labels, const char* what) {
-  const bool fm = t->spec.kind == SRS_DEEPFM;
+  const bool fm = t->spec.kind == SRS_DEEPFM, wd = t->spec.kind == SRS_WIDENDEEP;
   const int n = batch->B;
   if (!batch->movie_id || !batch->user_id) return failf(SRS_ERR_INVALID, "%smovie_id and user_id are required", what);
   if (fm && (!batch->movie_genre || !batch->user_genre || !batch->numerics))
     return failf(SRS_ERR_INVALID, "%sDeepFM needs movie_genre, user_genre and numerics", what);
+  if (wd && (!batch->movie_genre || !batch->user_genre || !batch->numerics || !batch->hist || batch->hist_stride < 1))
+    return failf(SRS_ERR_INVALID, "%sWide&Deep needs movie_genre, user_genre, numerics and hist (userRatedMovie1)",
+                 what);
   for (int i = 0; i < n; ++i)
     if (labels[i] != 0 && labels[i] != 1)
       return failf(SRS_ERR_INVALID, "%slabel of row %d is %d, not 0 or 1", what, i, labels[i]);
@@ -350,17 +360,32 @@ int check_rows(const srs_trainer* t, const srs_batch* batch, const int32_t* labe
       return failf(SRS_ERR_RANGE, "%suserGenre1 index %d of row %d is outside [0, %d)", what,
                    batch->user_genre[(size_t)i * 5], i, t->spec.n_genres);
   }
+  for (int i = 0; wd && i < n; ++i) {                  // every genre slot; a negative genre is missing
+    for (int k = 0; k < 3; ++k)
+      if (batch->movie_genre[(size_t)i * 3 + k] >= t->spec.n_genres)
+        return failf(SRS_ERR_RANGE, "%smovieGenre%d index %d of row %d is outside [0, %d)", what, k + 1,
+                     batch->movie_genre[(size_t)i * 3 + k], i, t->spec.n_genres);
+    for (int k = 0; k < 5; ++k)
+      if (batch->user_genre[(size_t)i * 5 + k] >= t->spec.n_genres)
+        return failf(SRS_ERR_RANGE, "%suserGenre%d index %d of row %d is outside [0, %d)", what, k + 1,
+                     batch->user_genre[(size_t)i * 5 + k], i, t->spec.n_genres);
+    const int rated = batch->hist[(size_t)i * batch->hist_stride];
+    if ((unsigned)rated >= (unsigned)t->spec.n_movies)
+      return failf(SRS_ERR_RANGE, "%suserRatedMovie1 %d of row %d is outside [0, %d)", what, rated, i,
+                   t->spec.n_movies);
+  }
   return SRS_OK;
 }
 
-// batch->B rows on the device, uploaded on s: the columns the trainer's model reads (NeuralCF: movie and user only)
-// and the labels
-cudaError_t upload_rows(Scratch& sc, bool fm, const srs_batch* b, const int32_t* labels, DeepFmRows* r,
+// batch->B rows on the device, uploaded on s: the columns the trainer's model reads (NeuralCF: movie and user only;
+// Wide&Deep: also hist's column 0) and the labels
+cudaError_t upload_rows(Scratch& sc, int kind, const srs_batch* b, const int32_t* labels, DeepFmRows* r,
                         cudaStream_t s) {
   const size_t n = (size_t)b->B;
+  const bool wd = kind == SRS_WIDENDEEP, fm = kind == SRS_DEEPFM || wd;
   cudaError_t e;
   if (fm) {
-    *r = deepfm_rows(sc, (int)n, &e);
+    *r = deepfm_rows(sc, (int)n, wd, &e);
   } else {
     *r = DeepFmRows{};
     e = sc.alloc(&r->movie, n);
@@ -374,12 +399,14 @@ cudaError_t upload_rows(Scratch& sc, bool fm, const srs_batch* b, const int32_t*
   if (fm && e == cudaSuccess) e = cudaMemcpyAsync(r->ugenre, b->user_genre, n * 5 * 4, cudaMemcpyHostToDevice, s);
   if (fm && e == cudaSuccess)
     e = cudaMemcpyAsync(r->numerics, b->numerics, n * kNumNumerics * 4, cudaMemcpyHostToDevice, s);
+  if (wd && e == cudaSuccess)
+    e = cudaMemcpy2DAsync(r->rated, 4, b->hist, (size_t)b->hist_stride * 4, 4, n, cudaMemcpyHostToDevice, s);
   return e;
 }
 
 // `model.evaluate` of the trainer's current weights over n device rows, two launches on s: the serving forward
-// (ncf_kernel or deepfm_kernel), then one metrics_update_kernel over all the rows into em.  `err` may be null for
-// NeuralCF only (DeepFM's genre check writes it).
+// (ncf_kernel, deepfm_kernel or embmlp_kernel), then one metrics_update_kernel over all the rows into em.  `err` may
+// be null for NeuralCF only (the genre checks of the others write it).
 cudaError_t eval_rows(const srs_trainer* t, const DeepFmRows& r, int n, float* probs, float* logits, int* err,
                       MetricsState* em, cudaStream_t s) {
   BatchView b{};
@@ -390,6 +417,10 @@ cudaError_t eval_rows(const srs_trainer* t, const DeepFmRows& r, int n, float* p
   if (t->spec.kind == SRS_DEEPFM) {
     b.movie_genre = r.mgenre; b.user_genre = r.ugenre; b.numerics = r.numerics;
     e = launch_deepfm(t->fm, b, s);
+  } else if (t->spec.kind == SRS_WIDENDEEP) {
+    b.movie_genre = r.mgenre; b.user_genre = r.ugenre; b.numerics = r.numerics;
+    b.hist = r.rated; b.hist_stride = 1;
+    e = launch_embmlp(t->emb, b, s);
   } else {
     e = launch_ncf(t->ncf, b, s);
   }
@@ -401,14 +432,25 @@ cudaError_t eval_rows(const srs_trainer* t, const DeepFmRows& r, int n, float* p
 
 extern "C" {
 
+// NeuralCF and DeepFM only, as this entry point has always been documented; srs_trainer_create_ex takes Wide&Deep too
 int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
                        const srs_adam* hp, srs_trainer** out) {
   if (!spec || !out) return failf(SRS_ERR_INVALID, "null argument");
   *out = nullptr;
+  if (spec->kind != SRS_NEURALCF && spec->kind != SRS_DEEPFM)
+    return failf(SRS_ERR_INVALID, "srs_trainer_create trains NeuralCF (neural_cf_model_1) and DeepFM only; "
+                 "srs_trainer_create_ex also trains Wide&Deep");
+  return srs_trainer_create_ex(spec, tensors, n_tensors, device, hp, out);
+}
+
+int srs_trainer_create_ex(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
+                          const srs_adam* hp, srs_trainer** out) {
+  if (!spec || !out) return failf(SRS_ERR_INVALID, "null argument");
+  *out = nullptr;
   const srs_spec& s = *spec;
-  const bool fm = s.kind == SRS_DEEPFM;
-  if (s.kind != SRS_NEURALCF && !fm)
-    return failf(SRS_ERR_INVALID, "fit is implemented for NeuralCF (neural_cf_model_1) and DeepFM only");
+  const bool fm = s.kind == SRS_DEEPFM, wd = s.kind == SRS_WIDENDEEP;
+  if (s.kind != SRS_NEURALCF && !fm && !wd)
+    return failf(SRS_ERR_INVALID, "fit is implemented for NeuralCF (neural_cf_model_1), DeepFM and Wide&Deep only");
   if (s.emb_dim < 1 || s.emb_dim > 64) return failf(SRS_ERR_INVALID, "emb_dim must be in 1..64");
   if (s.n_movies < 1 || s.n_users < 1) return failf(SRS_ERR_INVALID, "empty vocabulary");
   int hmax = 0;
@@ -417,6 +459,13 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
     if (s.n_genres < 1) return failf(SRS_ERR_INVALID, "empty genre vocabulary");
     for (int i = 0; i < 2; ++i)
       if (s.hidden[i] < 1 || s.hidden[i] > 64) return failf(SRS_ERR_INVALID, "DeepFM's hidden widths must be in 1..64");
+  } else if (wd) {
+    if (s.n_hidden != 2) return failf(SRS_ERR_INVALID, "Wide&Deep's fit needs exactly 2 hidden layers");
+    if (s.n_genres < 1) return failf(SRS_ERR_INVALID, "empty genre vocabulary");
+    if (s.cross_buckets < 1) return failf(SRS_ERR_INVALID, "Wide&Deep needs cross_buckets >= 1");
+    for (int i = 0; i < 2; ++i)
+      if (s.hidden[i] < 1 || s.hidden[i] > 128)
+        return failf(SRS_ERR_INVALID, "Wide&Deep's hidden widths must be in 1..128");
   } else {
     if (s.n_hidden < 1 || s.n_hidden > 3) return failf(SRS_ERR_INVALID, "1..3 hidden layers supported");
     for (int i = 0; i < s.n_hidden; ++i) {
@@ -443,6 +492,11 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
     t->place = place_deepfm(s, EP, &t->fm);
     t->blob_floats = DeepFmBlob::of(EP).floats;
     t->onehot = (int64_t)2 * s.n_genres + s.n_movies + s.n_users;
+  } else if (wd) {
+    t->HP = 128;
+    t->place = place_embmlp(s, EP, &t->emb);
+    t->blob_floats = EmbMlpBlob::of(EP).floats;
+    t->onehot = s.cross_buckets;
   } else {
     t->HP = hmax <= 16 ? 16 : 32;
     t->place = place_ncf(s, EP, t->HP, &t->ncf);
@@ -463,6 +517,7 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
 
   cudaError_t ce = cudaSetDevice(device);
   if (ce == cudaSuccess && fm) ce = setup_deepfm_attributes();   // validation and evaluate run deepfm_kernel
+  if (ce == cudaSuccess && wd) ce = setup_embmlp_attributes();   //   (Wide&Deep: embmlp_kernel)
   if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking);
   for (int k = 0; k < 4 && ce == cudaSuccess; ++k) ce = cudaMalloc(&t->tab[k], t->tab_floats * sizeof(float));
   for (int k = 0; k < 3 && ce == cudaSuccess; ++k) ce = cudaMalloc(&t->blob[k], (size_t)nb * sizeof(float));
@@ -494,6 +549,11 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
     t->fm.deep_movie = table(4); t->fm.deep_user = table(5);
     point_into_blob(&t->fm, t->blob[0]);
     t->fm.first = t->fo[0];
+  } else if (wd) {
+    const float* tables[kWideDeepTables];
+    for (int k = 0; k < kWideDeepTables; ++k) tables[k] = table(k);
+    point_into_blob(&t->emb, tables, t->blob[0]);
+    t->emb.wide = t->fo[0];
   } else {
     t->ncf.movie = table(0);
     t->ncf.user = table(1);
@@ -518,7 +578,7 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
                                   const srs_batch* val_batch, const int32_t* val_labels, int32_t val_freq,
                                   srs_eval_result* val_history) {
   if (!t || !batch || !labels || !order) return failf(SRS_ERR_INVALID, "null argument");
-  const bool fm = t->spec.kind == SRS_DEEPFM;
+  const bool fm = t->spec.kind == SRS_DEEPFM, wd = t->spec.kind == SRS_WIDENDEEP;
   const int n = batch->B;
   if (n < 1) return failf(SRS_ERR_INVALID, "fit needs at least one row");
   if (batch_size < 1) return failf(SRS_ERR_INVALID, "batch_size must be at least 1");
@@ -547,8 +607,9 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
   }
   CUDA_TRY(cudaSetDevice(t->device));
   const int EP = t->EP, Bmax = std::min(batch_size, n);
-  const int n_ent = fm ? kDeepFmTables : 2;            // table entries per row
-  const int n_cta = fm ? deepfm_train_ctas(Bmax) : (Bmax + kTrainRows - 1) / kTrainRows;
+  const int n_ent = fm ? kDeepFmTables : wd ? kWideDeepTables : 2;   // table entries per row
+  const int n_cta = fm ? deepfm_train_ctas(Bmax) : wd ? widendeep_train_ctas(Bmax)
+                                                      : (Bmax + kTrainRows - 1) / kTrainRows;
   cudaStream_t s = t->stream;
   Scratch sc;
   int32_t *d_order, *d_trow, *d_lab_b = nullptr, *d_frow = nullptr;
@@ -564,14 +625,15 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
   CUDA_TRY(sc.alloc(&d_met, epochs));
   CUDA_TRY(cudaMemcpyAsync(d_order, order, (size_t)epochs * n * 4, cudaMemcpyHostToDevice, s));
   CUDA_TRY(cudaMemsetAsync(d_met, 0, sizeof(MetricsState) * epochs, s));
-  DeepFmRows src{}, rows{};                            // the dataset, and (DeepFM) the epoch's rows in order
-  CUDA_TRY(upload_rows(sc, fm, batch, labels, &src, s));
-  if (fm) {
+  DeepFmRows src{}, rows{};                            // the dataset, and (DeepFM, Wide&Deep) the epoch's rows in order
+  CUDA_TRY(upload_rows(sc, t->spec.kind, batch, labels, &src, s));
+  const int n_fent = fm ? 4 : 1;                       // one-hot entries per row (DeepFM, Wide&Deep)
+  if (fm || wd) {
     cudaError_t e;
-    rows = deepfm_rows(sc, n, &e);
+    rows = deepfm_rows(sc, n, wd, &e);
     CUDA_TRY(e);
-    CUDA_TRY(sc.alloc(&d_frow, 4 * (size_t)Bmax));
-    CUDA_TRY(sc.alloc(&d_fgrad, 4 * (size_t)Bmax));
+    CUDA_TRY(sc.alloc(&d_frow, n_fent * (size_t)Bmax));
+    CUDA_TRY(sc.alloc(&d_fgrad, n_fent * (size_t)Bmax));
     CUDA_TRY(sc.alloc(&d_err, 1));
     CUDA_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), s));
   } else {
@@ -582,7 +644,7 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
   float *d_vprobs = nullptr, *d_vlogits = nullptr;
   MetricsState* d_vmet = nullptr;
   if (nv) {
-    CUDA_TRY(upload_rows(sc, fm, val_batch, val_labels, &vrows, s));
+    CUDA_TRY(upload_rows(sc, t->spec.kind, val_batch, val_labels, &vrows, s));
     CUDA_TRY(sc.alloc(&d_vprobs, nv));
     CUDA_TRY(sc.alloc(&d_vlogits, nv));
     CUDA_TRY(sc.alloc(&d_vmet, epochs));
@@ -606,9 +668,17 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
     f.b.probs = d_probs; f.b.logits = d_logits; f.b.err_flag = d_err;
     f.trow = d_trow; f.gemb = d_gemb; f.frow = d_frow; f.fgrad = d_fgrad; f.part = d_part;
   }
+  WideDeepStepArgs w{};
+  if (wd) {
+    w.p = t->emb;
+    for (int k = 0; k < kWideDeepTables; ++k) w.tab_row0[k] = t->place[kEmbMlpSlotTable[k]].table_row;
+    w.b.probs = d_probs; w.b.logits = d_logits; w.b.err_flag = d_err; w.b.hist_stride = 1;
+    w.trow = d_trow; w.gemb = d_gemb; w.wrow = d_frow; w.wgrad = d_fgrad; w.part = d_part;
+  }
   int64_t steps = 0;
   for (int e = 0; e < epochs; ++e) {
     if (fm) CUDA_TRY(launch_deepfm_permute(src, rows, d_order + (size_t)e * n, n, s));
+    if (wd) CUDA_TRY(launch_widendeep_permute(src, rows, d_order + (size_t)e * n, n, s));
     for (int off = 0; off < n; off += batch_size) {
       const int B = std::min(batch_size, n - off);
       const int32_t* step_labels;
@@ -628,6 +698,24 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
         table_adam_kernel<true><<<fo_blocks, 256, 0, s>>>(t->fo[0], t->fo[1], t->fo[2], t->fo[3], t->onehot, t->hp,
                                                           t->d_it);
         dense_adam_kernel<<<1, kAdamThreads, 0, s>>>(d_part, deepfm_train_ctas(B), t->blob_floats, t->blob[0],
+                                                     t->blob[1], t->blob[2], t->hp, t->d_it);
+        g_launch_count += 5;
+      } else if (wd) {
+        w.b.B = B;
+        w.b.movie_id = rows.movie + off; w.b.user_id = rows.user + off; w.b.hist = rows.rated + off;
+        w.b.movie_genre = rows.mgenre + (size_t)off * 3; w.b.user_genre = rows.ugenre + (size_t)off * 5;
+        w.b.numerics = rows.numerics + (size_t)off * kNumNumerics;
+        w.label = rows.label + off;
+        step_labels = w.label;
+        CUDA_TRY(launch_widendeep_train_step(w, s));
+        table_grad_kernel<<<(kWideDeepTables * B + 127) / 128, 128, 0, s>>>(d_trow, d_gemb, kWideDeepTables * B, EP,
+                                                                            t->tab[3]);
+        table_grad_kernel<<<(B + 127) / 128, 128, 0, s>>>(d_frow, d_fgrad, B, 1, t->fo[3]);
+        table_adam_kernel<false><<<adam_blocks, 256, 0, s>>>(t->tab[0], t->tab[1], t->tab[2], t->tab[3],
+                                                             t->tab_floats, t->hp, t->d_it);
+        table_adam_kernel<true><<<fo_blocks, 256, 0, s>>>(t->fo[0], t->fo[1], t->fo[2], t->fo[3], t->onehot, t->hp,
+                                                          t->d_it);
+        dense_adam_kernel<<<1, kAdamThreads, 0, s>>>(d_part, widendeep_train_ctas(B), t->blob_floats, t->blob[0],
                                                      t->blob[1], t->blob[2], t->hp, t->d_it);
         g_launch_count += 5;
       } else {
@@ -683,7 +771,7 @@ int srs_trainer_evaluate_host(srs_trainer* t, const srs_batch* batch, const int3
   float *d_probs, *d_logits;
   int* d_err;
   MetricsState* d_met;
-  CUDA_TRY(upload_rows(sc, t->spec.kind == SRS_DEEPFM, batch, labels, &rows, s));
+  CUDA_TRY(upload_rows(sc, t->spec.kind, batch, labels, &rows, s));
   CUDA_TRY(sc.alloc(&d_probs, n));
   CUDA_TRY(sc.alloc(&d_logits, n));
   CUDA_TRY(sc.alloc(&d_err, 1));

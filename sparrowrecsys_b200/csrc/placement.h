@@ -1,5 +1,6 @@
-// placement.h - where the Keras tensors of the trainable models (NeuralCF's neural_cf_model_1 and two towers, and
-// DeepFM) live on the device, written once for the serving builders (build_ncf, build_deepfm in model.cu) and the
+// placement.h - where the Keras tensors of the trainable models (NeuralCF's neural_cf_model_1 and two towers, DeepFM,
+// and EmbeddingMLP / Wide&Deep) live on the device, written once for the serving builders (build_ncf, build_deepfm,
+// build_embmlp in model.cu) and the
 // trainer (srs_trainer_create, srs_trainer_get_weights in ncf_train.cu): the builders and the trainer scatter the
 // caller's host tensors through it, and the trainer gathers its weights back through it.  Also the by-name lookup of
 // the caller's tensors that both use.  Host code only.
@@ -77,9 +78,10 @@ struct TensorLookup {
   }
 };
 
-// Rows of a Dense tensor [rows][cols] in one zero-padded block of the Dense-weight blob or of DeepFM's one-hot array
+// Rows of a Dense tensor [rows][cols] in one zero-padded block of the Dense-weight blob or of the one-hot array
 struct Block {
-  bool onehot;                   // false: the blob; true: the [fm1_width] one-hot rows of DeepFM's dense_2/kernel
+  bool onehot;                   // false: the blob; true: the one-hot array, the [fm1_width] one-hot rows of DeepFM's
+                                 // dense_2/kernel or the [cross_buckets] wide rows of Wide&Deep's
   int at;                        // the block's first float
   int width;                     // floats per block row: the tensor's cols, zero padded
   std::vector<int> map;          // block row i holds tensor row map[i]; -1: a zero row
@@ -210,6 +212,61 @@ inline void point_into_blob(DeepFmParams* p, const float* blob) {
   p->blob = blob;
   p->W1 = blob + ly.W1; p->b1 = blob + ly.b1; p->W2 = blob + ly.W2; p->b2 = blob + ly.b2;
   p->wdeep = blob + ly.wdeep;
+}
+
+// EmbeddingMLP and Wide&Deep: the ten tables (movieGenre1..3, userGenre1..5, movieId, userId: the order the
+// builder has always looked them up in; EmbMlpSlotTable maps a kernel slot to it), the Dense tensors in an
+// EmbMlpBlob::of(EP) and, for Wide&Deep, the wide rows of dense_2/kernel in their own [cross_buckets] one-hot array.
+// Fills p's sizes and EP.
+constexpr int kEmbMlpSlotTable[10] = {0, 1, 2, 8, 3, 4, 5, 6, 7, 9};   // kernel slot -> placement index
+
+inline Placement place_embmlp(const srs_spec& s, int EP, EmbMlpParams* p) {
+  const int E = s.emb_dim, h0 = s.hidden[0], h1 = s.hidden[1];
+  const bool wide = s.kind == SRS_WIDENDEEP;
+  const EmbMlpBlob ly = EmbMlpBlob::of(EP);
+  Placement pl;
+  char name[48];
+  for (int k = 1; k <= 3; ++k) {
+    snprintf(name, sizeof name, "movieGenre%d_embedding", k);
+    place_table(pl, name, s.n_genres, E);
+  }
+  for (int k = 1; k <= 5; ++k) {
+    snprintf(name, sizeof name, "userGenre%d_embedding", k);
+    place_table(pl, name, s.n_genres, E);
+  }
+  place_table(pl, "movieId_embedding", s.n_movies, E);
+  place_table(pl, "userId_embedding", s.n_users, E);
+  // dense/kernel's rows are DenseFeatures' sorted concat (movieAvgRating | movieGenre1..3 | movieId | 4 numerics |
+  // userGenre1..5 | userId | 2 numerics); its tile rows are the ten slots, then the 7 numerics and one zero row
+  std::vector<int> map;
+  for (int k = 0; k < 3; ++k) append(map, iota_map(1 + k * E, E, EP));         // movieGenre1..3
+  append(map, iota_map(1 + 3 * E, E, EP));                                        // movieId
+  for (int k = 0; k < 5; ++k) append(map, iota_map(5 + 4 * E + k * E, E, EP));   // userGenre1..5
+  append(map, iota_map(5 + 9 * E, E, EP));                                        // userId
+  for (int r : {0, 1 + 4 * E, 2 + 4 * E, 3 + 4 * E, 4 + 4 * E, 5 + 10 * E, 6 + 10 * E, -1}) map.push_back(r);
+  place_dense(pl, "dense/kernel", 7 + 10 * E, h0, {Block{false, ly.W1, 128, map}});
+  place_dense(pl, "dense/bias", h0, 1, {Block{false, ly.b1, 1, iota_map(0, h0, 128)}});
+  place_dense(pl, "dense_1/kernel", h0, h1, {Block{false, ly.W2, 128, iota_map(0, h0, 128)}});
+  place_dense(pl, "dense_1/bias", h1, 1, {Block{false, ly.b2, 1, iota_map(0, h1, 128)}});
+  // dense_2/kernel: the deep rows, then (Wide&Deep) the wide rows
+  std::vector<Block> k3 = {Block{false, ly.w3, 1, iota_map(0, h1, 128)}};
+  if (wide) k3.push_back(Block{true, 0, 1, iota_map(h1, s.cross_buckets, s.cross_buckets)});
+  place_dense(pl, "dense_2/kernel", h1 + (wide ? s.cross_buckets : 0), 1, std::move(k3));
+  place_dense(pl, "dense_2/bias", 1, 1, {Block{false, ly.b3, 1, iota_map(0, 1, 1)}});
+  p->n_movies = s.n_movies; p->n_users = s.n_users; p->n_genres = s.n_genres;
+  p->cross_buckets = s.cross_buckets; p->EP = EP;
+  return pl;
+}
+
+// p's tables (tables[k]: the k-th table of place_embmlp's order) and Dense-weight pointers into an EmbMlpBlob on the
+// device
+inline void point_into_blob(EmbMlpParams* p, const float* const* tables, const float* blob) {
+  const EmbMlpBlob ly = EmbMlpBlob::of(p->EP);
+  for (int k = 0; k < 8; ++k) p->genre[k] = tables[k];
+  p->movie = tables[8];
+  p->user = tables[9];
+  p->W1 = blob + ly.W1; p->b1 = blob + ly.b1; p->W2 = blob + ly.W2; p->b2 = blob + ly.b2;
+  p->w3 = blob + ly.w3; p->b3 = blob + ly.b3;
 }
 
 // a Dense tensor's data [rows][cols] into its blocks; what no block row takes stays as it was (zero)

@@ -67,13 +67,14 @@ class Surface:
 
     def fit(self, features, epochs: int = 5, batch_size: int = 12, seed: int = 0, validation_data=None,
             validation_split: float = 0.0, validation_freq: int = 1) -> dict:
-        """`model.fit(train_dataset, epochs=5)` (NeuralCF.py:91, DeepFM.py): train from the weights `model` was
+        """`model.fit(train_dataset, epochs=5)` (NeuralCF.py:91, DeepFM.py, WideNDeep.py:117): train from the weights `model` was
         loaded with, then rebuild `model` from the trained weights.  Returns Keras's history dict, with the
-        `val_*` lists when `validation_data` or `validation_split` is given (`Trainer.fit`).  NeuralCF and
-        DeepFM only."""
-        if self.name not in ("neuralcf", "deepfm"):
-            raise NotImplementedError("tfrecmodel.%s: fit is implemented for NeuralCF (tfrecmodel.neuralcf) and "
-                                      "DeepFM (tfrecmodel.deepfm) only" % self.name)
+        `val_*` lists when `validation_data` or `validation_split` is given (`Trainer.fit`).  NeuralCF, DeepFM
+        and Wide&Deep only."""
+        if self.name not in ("neuralcf", "deepfm", "widendeep"):
+            raise NotImplementedError("tfrecmodel.%s: fit is implemented for NeuralCF (tfrecmodel.neuralcf), "
+                                      "DeepFM (tfrecmodel.deepfm) and Wide&Deep (tfrecmodel.widendeep) only"
+                                      % self.name)
         if self.model is None or self.weights is None:
             raise RuntimeError("tfrecmodel.%s: call load() before fit()" % self.name)
         from ..training import Trainer

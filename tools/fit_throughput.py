@@ -1,17 +1,19 @@
-"""Time NeuralCF's or DeepFM's `fit` on the GPU against the numpy oracle on the host.
+"""Time NeuralCF's, DeepFM's or Wide&Deep's `fit` on the GPU against the numpy oracle on the host.
 
-    python tools/fit_throughput.py [--model neuralcf|deepfm] [--epochs 5] [--batch-sizes 12,4096] [--cpu-epochs 1]
-                                   [--validate [--repeats 5]]
+    python tools/fit_throughput.py [--model neuralcf|deepfm|widendeep] [--epochs 5] [--batch-sizes 12,4096]
+                                   [--cpu-epochs 1] [--validate [--repeats 5]] [--kernels 4096]
 
 Trains the reference script's run - the untrained model of `init_weights(default_spec(model), 0, for_test=False)`
-over the 88 827 rows of `tests/golden/<model>_trainset.npz` - for `--epochs` epochs at each batch size, and reports
+over the 88 827 rows of `tests/golden/<model>_trainset.npz` (Wide&Deep: `deepfm_trainset.npz` with the columns of
+`widendeep_samples.npz`) - for `--epochs` epochs at each batch size, and reports
 the wall time of `Trainer.fit` (upload, every step, the history read-back) and µs per step.  The CPU column is the
-float32 oracle (`oracle.ncf_train.fit` / `oracle.deepfm_train.fit`) over `--cpu-epochs` epochs at the same batch
+float32 oracle (`oracle.ncf_train.fit` / `oracle.deepfm_train.fit` / `oracle.widendeep_train.fit`) over `--cpu-epochs` epochs at the same batch
 size, scaled to µs per step (`--cpu-epochs 0` leaves it out).  `--validate` adds the cost of validating on the
 22 440 rows of `tests/golden/dien_testset.npz` every epoch, next to the epoch time: `validation_s_per_epoch` from
 fits of `--val-epochs` one-step epochs (the first batch of rows) with and without validation, where the two validation
 launches are a large part of each epoch, and `validated_minus_plain_s_per_epoch` from full-size fits (below the
-noise of a 7 403-step epoch).  Plain and validated fits alternate, `--repeats` pairs, medians.  Prints one JSON object with the card name and power limit read from nvidia-smi in the
+noise of a 7 403-step epoch).  Plain and validated fits alternate, `--repeats` pairs, medians.  `--kernels B` adds
+the device time of each kernel over one epoch at batch B (torch.profiler), per step.  Prints one JSON object with the card name and power limit read from nvidia-smi in the
 same run (and the model's name unless it is the default, NeuralCF).  Writes nothing.
 """
 import argparse
@@ -39,7 +41,7 @@ def card():
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=("neuralcf", "deepfm"), default="neuralcf")
+    ap.add_argument("--model", choices=("neuralcf", "deepfm", "widendeep"), default="neuralcf")
     ap.add_argument("--epochs", type=int, default=5)
     ap.add_argument("--batch-sizes", default="12,4096")
     ap.add_argument("--cpu-epochs", type=int, default=1)
@@ -47,16 +49,22 @@ def main():
                     help="also report the cost per epoch of validating on dien_testset.npz every epoch")
     ap.add_argument("--val-epochs", type=int, default=500)
     ap.add_argument("--repeats", type=int, default=5)
+    ap.add_argument("--kernels", type=int, default=0, help="batch size of a per-kernel breakdown (0: none)")
     args = ap.parse_args()
-    from oracle import deepfm_train, ncf_train
+    from oracle import deepfm_train, ncf_train, widendeep_train
     from sparrowrecsys_b200.spec import default_spec
     from sparrowrecsys_b200.training import Trainer
     from sparrowrecsys_b200.weights import init_weights
-    z = np.load(os.path.join(ROOT, "tests", "golden", "%s_trainset.npz" % args.model))
+    golden = os.path.join(ROOT, "tests", "golden")
+    wd = args.model == "widendeep"
+    z = np.load(os.path.join(golden, "%s_trainset.npz" % ("deepfm" if wd else args.model)))
     if args.model == "neuralcf":
         feats = {k: z[k] for k in ("movieId", "userId", "label")}
     else:
         feats = dict(z)
+    if wd:
+        extra = np.load(os.path.join(golden, "widendeep_samples.npz"))
+        feats.update({k[6:]: extra[k] for k in extra.files if k.startswith("train_")})
     n = len(feats["label"])
     spec = default_spec(args.model)
     W0 = init_weights(spec, 0, for_test=False)
@@ -65,15 +73,19 @@ def main():
         if args.model == "neuralcf":
             ncf_train.fit(W0, feats["movieId"], feats["userId"], feats["label"], orders, B, np.float32)
         else:
-            deepfm_train.fit(W0, deepfm_train.Rows.from_features(feats), feats["label"], orders, B, np.float32)
+            m = widendeep_train if wd else deepfm_train
+            m.fit(W0, m.Rows.from_features(feats), feats["label"], orders, B, np.float32)
 
     res = {"rows": n, "epochs": args.epochs, **card(), "runs": []}
     if args.model != "neuralcf":
         res = {"model": args.model, **res}
     val = None
     if args.validate:
-        t = np.load(os.path.join(ROOT, "tests", "golden", "dien_testset.npz"))
+        t = np.load(os.path.join(golden, "dien_testset.npz"))
         val = {k: t[k] for k in (("movieId", "userId", "label") if args.model == "neuralcf" else t.files)}
+        if wd:
+            extra = np.load(os.path.join(golden, "widendeep_samples.npz"))
+            val.update({k[5:]: extra[k] for k in extra.files if k.startswith("test_")})
         res["validation_rows"] = len(val["label"])
 
     def timed_fit(B, validation_data=None, rows=None, epochs=args.epochs):
@@ -109,7 +121,31 @@ def main():
                         "cpu_oracle_wall_s_scaled": cpu * steps / cpu_steps})
         run["final_epoch"] = {k: v[-1] for k, v in hist.items()}
         res["runs"].append(run)
+    if args.kernels:
+        res["kernels"] = kernel_breakdown(spec, W0, feats, args.kernels)
     print(json.dumps(res))
+
+
+def kernel_breakdown(spec, W0, feats, B):
+    """{kernel: µs per step} of one epoch at batch B, from torch.profiler's CUDA activity (every kernel of the
+    process, the library's included)."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    from sparrowrecsys_b200.training import Trainer
+    n = len(feats["label"])
+    steps = -(-n // B)
+    with Trainer(spec, W0) as tr:
+        tr.fit(feats, epochs=1, batch_size=B, seed=2)             # warm-up
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            tr.fit(feats, epochs=1, batch_size=B, seed=3)
+    out = {}
+    for ev in prof.events():
+        if ev.device_type == torch.autograd.DeviceType.CUDA and "Memcpy" not in ev.name and "Memset" not in ev.name:
+            name = ev.name.replace("(anonymous namespace)::", "").replace("void ", "").replace("srs::", "")
+            name = name.split("(")[0].split("<")[0]
+            out[name] = out.get(name, 0.0) + ev.device_time / steps
+    return {"batch_size": B, "steps": steps, "us_per_step": dict(sorted(out.items(), key=lambda kv: -kv[1]))}
 
 
 if __name__ == "__main__":
