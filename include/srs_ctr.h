@@ -369,28 +369,34 @@ int srs_dien_evaluate_host_batches(srs_model* m, int32_t n_batches, const srs_ba
                                    const int32_t* const* neg_hist, const int32_t* const* labels,
                                    srs_dien_eval_result* out);
 
-/* ---- `model.fit` of NeuralCF (neural_cf_model_1, NeuralCF.py:74-91), DeepFM (DeepFM.py) and Wide&Deep
- * (WideNDeep.py:99-117): each script compiles
+/* ---- `model.fit` of NeuralCF (neural_cf_model_1, NeuralCF.py:74-91), DeepFM (DeepFM.py), Wide&Deep
+ * (WideNDeep.py:99-117) and DeepFM_v2 (DeepFM_v2.py:158-165): each script compiles
  * with loss='binary_crossentropy', optimizer='adam' and calls `fit(train_dataset, epochs=5)` over make_csv_dataset
  * batches of 12.  A trainer owns fp32 weights and Adam's slots on one device; it never touches an srs_model: a
  * serving model is built from the weights srs_trainer_get_weights exports.  Per step of B_b rows (DESIGN.md
- * sections 4.8, 4.9 and 4.18):
+ * sections 4.8, 4.9, 4.18 and 4.19):
  *   loss      the mean over the batch of max(z,0) - z*y + log1p(exp(-|z|)), so dL/dz_i = (sigmoid(z_i) - y_i) / B_b;
  *   gradient  through the Dense layers (relu' = [a > 0]) into the embedding rows of each row (DeepFM: also the four
  *             FM dots, and dz into the 4 one-hot rows of dense_2/kernel a row selects; Wide&Deep: its ten embedding
- *             columns, and dz into the wide row of dense_2/kernel at the row's crossed bucket; a missing genre gives
- *             no entry); an id that occurs several times in the batch gets the sum of its rows' gradients, in row
+ *             columns, and dz into the wide row of dense_2/kernel at the row's crossed bucket; DeepFM_v2: out/kernel
+ *             gets [first | fm | deep] . dz, dfirst = dz * out/kernel[0] goes to first_cat/bias, first_num/bias,
+ *             first_num/kernel (times the raw numerics) and the 4 one-hot rows of first_cat/kernel a row selects,
+ *             the FM (no 1/2) gives dF_fc = dz * out/kernel[1 + c] * 2 (sum_f F_fc - F_fc), the deep MLP adds
+ *             deep/kernel . delta1, and each field's proj_f/kernel gets x_f (x) dF_f, proj_f/bias dF_f (a row
+ *             whose genre is missing included) and its table row proj_f/kernel . dF_f; a missing genre gives no
+ *             entry); an id that occurs several times in the batch gets the sum of its rows' gradients, in row
  *             order (TF's _deduplicate_indexed_slices);
  *   Adam      Keras's, t = iterations + 1, alpha = lr * sqrt(1 - beta_2^t) / (1 - beta_1^t) in float32.  Dense
  *             kernels and biases - for DeepFM all 31 040 one-hot rows of dense_2/kernel included, for Wide&Deep all
- *             cross_buckets wide rows: m += (g - m)(1 -
+ *             cross_buckets wide rows, for DeepFM_v2 all fm1_width one-hot rows of first_cat/kernel: m += (g - m)(1 -
  *             beta_1), v += (g^2 - v)(1 - beta_2) (TF's ApplyAdam).  The embedding tables (IndexedSlices gradients,
  *             _resource_apply_sparse): m and v of EVERY row decay, m = beta_1 m + (1 - beta_1) G, v = beta_2 v +
  *             (1 - beta_2) G^2 with G = 0 off the batch, and every row is updated - not "lazy Adam".  All:
  *             w -= alpha m / (sqrt(v) + epsilon).
  * Every sum has a fixed order: the same weights, data and order give the same bits.
  * Supported: emb_dim 1..64; NeuralCF 1..3 hidden layers of width 1..32, DeepFM exactly 2 of width 1..64, Wide&Deep
- * exactly 2 of width 1..128 and cross_buckets >= 1; any batch size >= 1. */
+ * exactly 2 of width 1..128 and cross_buckets >= 1, DeepFM_v2 exactly 2 of widths 1..32 and 1..16, proj_dim 64 and
+ * n_genres >= 1; any batch size >= 1. */
 typedef struct srs_adam {
   float lr, beta_1, beta_2, epsilon;   /* Keras's defaults: 0.001, 0.9, 0.999, 1e-7 */
 } srs_adam;
@@ -406,9 +412,16 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
  * rely on its list. */
 int srs_trainer_create_ex(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
                           const srs_adam* hp, srs_trainer** out);
+/* srs_trainer_create for every kind this library can train; the list grows with the library, so a kind it rejects
+ * today (SRS_ERR_INVALID) may be accepted by a later version.  Today: SRS_NEURALCF, SRS_DEEPFM, SRS_WIDENDEEP and
+ * SRS_DEEPFM_V2 (its tensors as srs_model_create takes them).  Callers that rely on a fixed list use
+ * srs_trainer_create or srs_trainer_create_ex, whose lists do not change. */
+int srs_trainer_create_any(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
+                           const srs_adam* hp, srs_trainer** out);
 void srs_trainer_destroy(srs_trainer* tr);
 
-/* `epochs` epochs over the n = batch->B rows of `batch` (host; movie_id, user_id, and for DeepFM movie_genre [n][3]
+/* `epochs` epochs over the n = batch->B rows of `batch` (host; movie_id, user_id, and for DeepFM and DeepFM_v2
+ * movie_genre [n][3]
  * and user_genre [n][5], of which column 0 is read and a negative index is missing, and numerics [n][7]; for
  * Wide&Deep every genre column, numerics and hist, of which column 0 (userRatedMovie1) is read) with
  * labels [n] int32: epoch e

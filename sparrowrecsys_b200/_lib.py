@@ -45,7 +45,7 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_selftest_wgmma", "srs_metrics_create", "srs_metrics_destroy", "srs_metrics_reset",
            "srs_metrics_update_device", "srs_metrics_result", "srs_evaluate_host_batches",
            "srs_dien_outputs_device", "srs_dien_outputs_host_batches", "srs_dien_evaluate_host_batches",
-           "srs_trainer_create", "srs_trainer_create_ex", "srs_trainer_destroy", "srs_trainer_fit_host", "srs_trainer_get_weights",
+           "srs_trainer_create", "srs_trainer_create_ex", "srs_trainer_create_any", "srs_trainer_destroy", "srs_trainer_fit_host", "srs_trainer_get_weights",
            "srs_trainer_iterations", "srs_trainer_fit_validate_host", "srs_trainer_evaluate_host",
            "srs_featureeng_host", "srs_item2vec_host", "srs_user_embeddings_host", "srs_als_fit_host",
            "srs_als_fit_folds_host", "srs_als_recommend_host", "srs_item_transitions_host", "srs_random_walks_host",
@@ -224,7 +224,7 @@ def load():
     lib.srs_dien_evaluate_host_batches.restype = C.c_int
     lib.srs_dien_evaluate_host_batches.argtypes = [C.c_void_p, C.c_int32, C.POINTER(SrsBatch), C.POINTER(C.c_void_p),
                                                    C.POINTER(C.c_void_p), C.POINTER(SrsDienEvalResult)]
-    for f in (lib.srs_trainer_create, lib.srs_trainer_create_ex):
+    for f in (lib.srs_trainer_create, lib.srs_trainer_create_ex, lib.srs_trainer_create_any):
         f.restype = C.c_int
         f.argtypes = [C.POINTER(SrsSpec), C.POINTER(SrsTensor), C.c_int32, C.c_int32, C.POINTER(SrsAdam),
                       C.POINTER(C.c_void_p)]

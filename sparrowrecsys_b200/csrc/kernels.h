@@ -161,7 +161,7 @@ struct DeepFmStepArgs {
 };
 int deepfm_train_ctas(int B);
 cudaError_t launch_deepfm_train_step(const DeepFmStepArgs& a, cudaStream_t s);
-struct DeepFmRows {        // a DeepFM or Wide&Deep dataset on the device, in the srs_batch layout
+struct DeepFmRows {        // a DeepFM, DeepFM_v2 or Wide&Deep dataset on the device, in the srs_batch layout
   int32_t* movie;          // [n]
   int32_t* user;           // [n]
   int32_t* mgenre;         // [n][3], column 0 read (DeepFM)
@@ -203,9 +203,9 @@ struct DeepFm2Params {
   const float* movie;      // [n_movies][EP]
   const float* ugenre;     // [19][EP]
   const float* user;       // [n_users][EP]
+  const float* blob;       // the Dense weights, DeepFm2Blob layout; the pointers below (but `first`) point into it
   const float* first;      // [fm1_width] first_cat kernel
   const float* first_num;  // [8]
-  float first_bias;        // first_cat bias + first_num bias
   const float* proj[4];    // [EP][64] each, field order movieGenre1, movieId, userGenre1, userId
   const float* proj_b[4];  // [64]
   const float* proj_num;   // [8][64]
@@ -215,10 +215,54 @@ struct DeepFm2Params {
   const float* Wd1;        // [32][16]
   const float* bd1;        // [16]
   const float* wout;       // [1 + 64 + 16]
-  float bout;
   int n_movies, n_users, n_genres;
   int EP;
 };
+
+// The Dense weights of DeepFM_v2 (a model's and a trainer's) as one blob, offsets in floats: the four field
+// projections proj [4][EP][64] (rows past E zero), their biases proj_b [4][64], proj_num [8][64] (the 7 numerics'
+// rows and a zero row), proj_num_b [64], deep/kernel Wd [320][32], bd [32], deep_1/kernel Wd1 [32][16], bd1 [16]
+// (hidden widths zero padded to 32 and 16), out/kernel wout [84] (first | fm 64 | deep 16, zero padded),
+// first_num/kernel [8], then first_cat/bias, first_num/bias and out/bias (the forward reads the three biases here:
+// a trainer's Adam writes them every step) and one float of padding.  Every array is 16-byte aligned.  The one-hot
+// first_cat/kernel lives apart (placement.h).
+struct DeepFm2Blob {
+  int proj, proj_b, proj_num, proj_num_b, Wd, bd, Wd1, bd1, wout, first_num, first_cat_b, first_num_b, bout, floats;
+  __host__ __device__ static DeepFm2Blob of(int EP) {
+    DeepFm2Blob l;
+    l.proj = 0;
+    l.proj_b = 4 * EP * 64;
+    l.proj_num = l.proj_b + 4 * 64;
+    l.proj_num_b = l.proj_num + kNumPad * 64;
+    l.Wd = l.proj_num_b + 64;
+    l.bd = l.Wd + 5 * 64 * 32;
+    l.Wd1 = l.bd + 32;
+    l.bd1 = l.Wd1 + 32 * 16;
+    l.wout = l.bd1 + 16;
+    l.first_num = l.wout + 84;
+    l.first_cat_b = l.first_num + kNumPad;
+    l.first_num_b = l.first_cat_b + 1;
+    l.bout = l.first_num_b + 1;
+    l.floats = l.bout + 2;
+    return l;
+  }
+};
+
+// ---- DeepFM_v2's training step (deepfm2_train.cu; DESIGN.md section 4.19) ----------------------------------------
+constexpr int kDeepFm2Tables = 4;   // movieGenre1, movieId, userGenre1, userId: the field order
+struct DeepFm2StepArgs {
+  DeepFm2Params p;         // the trainer's tables, Dense weights and one-hot first_cat/kernel
+  BatchView b;             // the step's B rows in order; probs / logits receive its outputs before the update
+  const int32_t* label;    // [B]
+  int64_t tab_row0[kDeepFm2Tables];   // first row of each table in the trainer's table array
+  int32_t* trow;           // [4B] table row of entry s * B + r (field s), -1 = none (a missing genre)
+  float* gemb;             // [4B][EP] the entries' gradients
+  int32_t* frow;           // [4B] one-hot row of first_cat/kernel of entry s * B + r, -1 = none (a missing genre)
+  float* fgrad;            // [4B] its gradient (the row's dL/dz * out/kernel[0])
+  float* part;             // [ctas][DeepFm2Blob::floats] per-CTA Dense gradient sums
+};
+int deepfm2_train_ctas(int B);
+cudaError_t launch_deepfm2_train_step(const DeepFm2StepArgs& a, cudaStream_t s);
 
 // ---- DIN (DIN.py:125-167) ------------------------------------------------------------
 struct DinParams {

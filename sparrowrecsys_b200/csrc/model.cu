@@ -372,55 +372,18 @@ int build_deepfm(Builder& B) {
 int build_deepfm2(Builder& B) {
   srs_model* m = B.m;
   const srs_spec& s = m->spec;
-  const int E = s.emb_dim, EP = m->EP, P = 64;
-  if (s.proj_dim != P) return fail(SRS_ERR_INVALID, "DeepFM_v2 projection width must be 64");
+  const int EP = m->EP;
+  if (s.proj_dim != 64) return fail(SRS_ERR_INVALID, "DeepFM_v2 projection width must be 64");
   if (s.n_hidden != 2 || s.hidden[0] > 32 || s.hidden[1] > 16 || s.hidden[0] < 1 || s.hidden[1] < 1)
     return fail(SRS_ERR_INVALID, "DeepFM_v2 needs hidden widths <= (32, 16)");
-  const int h0 = s.hidden[0], h1 = s.hidden[1];
-  const int64_t fm1 = (int64_t)2 * s.n_genres + s.n_movies + s.n_users;
   DeepFm2Params& p = m->fm2;
-  p.mgenre = B.table("movieGenre1_embedding", s.n_genres, E);
-  p.movie = B.table("movieId_embedding", s.n_movies, E);
-  p.ugenre = B.table("userGenre1_embedding", s.n_genres, E);
-  p.user = B.table("userId_embedding", s.n_users, E);
-  const float* fc = B.host("first_cat/kernel", fm1, 1);
-  const float* fcb = B.host("first_cat/bias", 1, 1);
-  const float* fn = B.host("first_num/kernel", 7, 1);
-  const float* fnb = B.host("first_num/bias", 1, 1);
-  const char* fields[4] = {"movieGenre1", "movieId", "userGenre1", "userId"};
-  const float* pk[4]; const float* pb[4];
-  char name[64];
-  for (int f = 0; f < 4; ++f) {
-    snprintf(name, sizeof(name), "proj_%s/kernel", fields[f]);
-    pk[f] = B.host(name, E, P);
-    snprintf(name, sizeof(name), "proj_%s/bias", fields[f]);
-    pb[f] = B.host(name, P, 1);
-  }
-  const float* pnk = B.host("proj_num/kernel", 7, P);
-  const float* pnb = B.host("proj_num/bias", P, 1);
-  const float* dk = B.host("deep/kernel", 5 * P, h0);
-  const float* db = B.host("deep/bias", h0, 1);
-  const float* d1k = B.host("deep_1/kernel", h0, h1);
-  const float* d1b = B.host("deep_1/bias", h1, 1);
-  const float* ok = B.host("out/kernel", 1 + P + h1, 1);
-  const float* ob = B.host("out/bias", 1, 1);
+  const Placement pl = place_deepfm2(s, EP, &p);
+  std::vector<float> blob(DeepFm2Blob::of(EP).floats, 0.f), first((size_t)2 * s.n_genres + s.n_movies + s.n_users, 0.f);
+  const float* tables[kDeepFm2Tables];
+  place_host(B, pl, tables, blob.data(), first.data());
   if (B.status != SRS_OK) return B.status;
-  p.first = B.upload(std::vector<float>(fc, fc + fm1));
-  p.first_num = B.upload(B.padvec(fn, 7, 8));
-  p.first_bias = fcb[0] + fnb[0];
-  for (int f = 0; f < 4; ++f) {
-    p.proj[f] = B.upload(B.permute(pk[f], P, iota_map(0, E, EP), P));
-    p.proj_b[f] = B.upload(B.padvec(pb[f], P, P));
-  }
-  p.proj_num = B.upload(B.permute(pnk, P, iota_map(0, 7, 8), P));
-  p.proj_num_b = B.upload(B.padvec(pnb, P, P));
-  p.Wd = B.upload(B.permute(dk, h0, iota_map(0, 5 * P, 5 * P), 32));
-  p.bd = B.upload(B.padvec(db, h0, 32));
-  p.Wd1 = B.upload(B.permute(d1k, h1, iota_map(0, h0, 32), 16));
-  p.bd1 = B.upload(B.padvec(d1b, h1, 16));
-  p.wout = B.upload(B.padvec(ok, 1 + P + h1, 1 + P + 16));
-  p.bout = ob[0];
-  p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres; p.EP = EP;
+  point_into_blob(&p, tables, B.upload(blob));
+  p.first = B.upload(first);
   m->kernel_name = "deepfm2_kernel";
   return B.status;
 }

@@ -1,7 +1,8 @@
 // ncf_train.cu - `model.fit` on the device: the C ABI's srs_trainer (include/srs_ctr.h), which trains NeuralCF
 // (neural_cf_model_1, NeuralCF.py:74-91; DESIGN.md section 4.8), DeepFM (DeepFM.py; section 4.9, its step kernel
-// in deepfm_train.cu) and Wide&Deep (WideNDeep.py; section 4.18, its step kernel in widendeep_train.cu), and the
-// kernels the models share: dedupe, the two forms of Adam, metrics.
+// in deepfm_train.cu), Wide&Deep (WideNDeep.py; section 4.18, its step kernel in widendeep_train.cu) and DeepFM_v2
+// (DeepFM_v2.py; section 4.19, its step kernel in deepfm2_train.cu), and the kernels the models share: dedupe, the
+// two forms of Adam, metrics.
 //
 // NeuralCF's step of batch B_b (rows order[off .. off + B_b) of the uploaded dataset), five launches, no host sync:
 //   ncf_train_step_kernel  forward (the arithmetic of ncf_kernel) and backward, one thread per row; the Dense
@@ -21,10 +22,14 @@
 // tables' entries and again (width 1) over its wide entries, table_adam_kernel<false> over the ten tables and <true>
 // over the cross_buckets wide rows of dense_2/kernel, dense_adam_kernel, metrics_update_kernel; plus
 // widendeep_permute_kernel once per epoch.
+// DeepFM_v2's step is seven launches of the same shape again: deepfm2_train_step_kernel, table_grad_kernel over its
+// four tables' entries and (width 1) over its one-hot entries, table_adam_kernel<false> over the four tables and
+// <true> over first_cat/kernel's one-hot rows, dense_adam_kernel, metrics_update_kernel; plus deepfm_permute_kernel
+// (it reads DeepFM's columns) once per epoch.
 // No float atomics: every sum has a fixed order, so a fit is bitwise reproducible.
 //
 // Validation (srs_trainer_fit_validate_host) and srs_trainer_evaluate_host run the serving forward over the
-// trainer's arrays (ncf_kernel, deepfm_kernel, embmlp_kernel) and one metrics_update_kernel over all the rows: two launches, with the
+// trainer's arrays (ncf_kernel, deepfm_kernel, embmlp_kernel, deepfm2_kernel) and one metrics_update_kernel over all the rows: two launches, with the
 // bits of a CTRModel built from the exported weights.  The trainer's arrays hold the weights where the serving
 // builders put them: both place them through placement.h.
 #include <cuda_runtime.h>
@@ -294,10 +299,12 @@ struct srs_trainer {
   NcfParams ncf{};                    // the serving parameters over the trainer's arrays (NeuralCF)
   DeepFmParams fm{};                  //   (DeepFM)
   EmbMlpParams emb{};                 //   (Wide&Deep)
+  DeepFm2Params fm2{};                //   (DeepFM_v2)
   int64_t tab_floats = 0;             // (sum of the tables' rows) * EP
   float* tab[4] = {};                 // w, m, v, G   [rows][EP], padding zero
   float* blob[3] = {};                // w, m, v      [blob_floats]
-  int64_t onehot = 0;                 // the one-hot rows of dense_2/kernel: DeepFM's fm1_width, Wide&Deep's wide rows
+  int64_t onehot = 0;                 // the one-hot rows: DeepFM's dense_2/kernel and DeepFM_v2's first_cat/kernel
+                                      // (fm1_width), Wide&Deep's wide rows of dense_2/kernel
   float* fo[4] = {};                  // w, m, v, G   [onehot]
   long long* d_it = nullptr;          // Adam's iteration counter, on the device
   int64_t iterations = 0;             // its host mirror
@@ -333,11 +340,12 @@ DeepFmRows deepfm_rows(Scratch& sc, int n, bool wd, cudaError_t* e) {
 // The checks of rows the trainer reads (fit, validation, evaluate), all made before any launch.  `what` prefixes
 // the messages: "" or "validation data: ".
 int check_rows(const srs_trainer* t, const srs_batch* batch, const int32_t* labels, const char* what) {
-  const bool fm = t->spec.kind == SRS_DEEPFM, wd = t->spec.kind == SRS_WIDENDEEP;
+  const bool fm = t->spec.kind == SRS_DEEPFM || t->spec.kind == SRS_DEEPFM_V2, wd = t->spec.kind == SRS_WIDENDEEP;
   const int n = batch->B;
   if (!batch->movie_id || !batch->user_id) return failf(SRS_ERR_INVALID, "%smovie_id and user_id are required", what);
   if (fm && (!batch->movie_genre || !batch->user_genre || !batch->numerics))
-    return failf(SRS_ERR_INVALID, "%sDeepFM needs movie_genre, user_genre and numerics", what);
+    return failf(SRS_ERR_INVALID, "%s%s needs movie_genre, user_genre and numerics", what,
+                 t->spec.kind == SRS_DEEPFM ? "DeepFM" : "DeepFM_v2");
   if (wd && (!batch->movie_genre || !batch->user_genre || !batch->numerics || !batch->hist || batch->hist_stride < 1))
     return failf(SRS_ERR_INVALID, "%sWide&Deep needs movie_genre, user_genre, numerics and hist (userRatedMovie1)",
                  what);
@@ -378,11 +386,11 @@ int check_rows(const srs_trainer* t, const srs_batch* batch, const int32_t* labe
 }
 
 // batch->B rows on the device, uploaded on s: the columns the trainer's model reads (NeuralCF: movie and user only;
-// Wide&Deep: also hist's column 0) and the labels
+// DeepFM and DeepFM_v2: also the genres and numerics; Wide&Deep: also hist's column 0) and the labels
 cudaError_t upload_rows(Scratch& sc, int kind, const srs_batch* b, const int32_t* labels, DeepFmRows* r,
                         cudaStream_t s) {
   const size_t n = (size_t)b->B;
-  const bool wd = kind == SRS_WIDENDEEP, fm = kind == SRS_DEEPFM || wd;
+  const bool wd = kind == SRS_WIDENDEEP, fm = kind == SRS_DEEPFM || kind == SRS_DEEPFM_V2 || wd;
   cudaError_t e;
   if (fm) {
     *r = deepfm_rows(sc, (int)n, wd, &e);
@@ -405,7 +413,7 @@ cudaError_t upload_rows(Scratch& sc, int kind, const srs_batch* b, const int32_t
 }
 
 // `model.evaluate` of the trainer's current weights over n device rows, two launches on s: the serving forward
-// (ncf_kernel, deepfm_kernel or embmlp_kernel), then one metrics_update_kernel over all the rows into em.  `err` may
+// (ncf_kernel, deepfm_kernel, embmlp_kernel or deepfm2_kernel), then one metrics_update_kernel over all the rows into em.  `err` may
 // be null for NeuralCF only (the genre checks of the others write it).
 cudaError_t eval_rows(const srs_trainer* t, const DeepFmRows& r, int n, float* probs, float* logits, int* err,
                       MetricsState* em, cudaStream_t s) {
@@ -421,6 +429,9 @@ cudaError_t eval_rows(const srs_trainer* t, const DeepFmRows& r, int n, float* p
     b.movie_genre = r.mgenre; b.user_genre = r.ugenre; b.numerics = r.numerics;
     b.hist = r.rated; b.hist_stride = 1;
     e = launch_embmlp(t->emb, b, s);
+  } else if (t->spec.kind == SRS_DEEPFM_V2) {
+    b.movie_genre = r.mgenre; b.user_genre = r.ugenre; b.numerics = r.numerics;
+    e = launch_deepfm2(t->fm2, b, s);
   } else {
     e = launch_ncf(t->ncf, b, s);
   }
@@ -428,29 +439,11 @@ cudaError_t eval_rows(const srs_trainer* t, const DeepFmRows& r, int n, float* p
   return launch_metrics_update(probs, logits, r.label, n, &em->cnt, &em->red, &em->loss, 1, s);
 }
 
-}  // namespace
-
-extern "C" {
-
-// NeuralCF and DeepFM only, as this entry point has always been documented; srs_trainer_create_ex takes Wide&Deep too
-int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
-                       const srs_adam* hp, srs_trainer** out) {
-  if (!spec || !out) return failf(SRS_ERR_INVALID, "null argument");
-  *out = nullptr;
-  if (spec->kind != SRS_NEURALCF && spec->kind != SRS_DEEPFM)
-    return failf(SRS_ERR_INVALID, "srs_trainer_create trains NeuralCF (neural_cf_model_1) and DeepFM only; "
-                 "srs_trainer_create_ex also trains Wide&Deep");
-  return srs_trainer_create_ex(spec, tensors, n_tensors, device, hp, out);
-}
-
-int srs_trainer_create_ex(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
-                          const srs_adam* hp, srs_trainer** out) {
-  if (!spec || !out) return failf(SRS_ERR_INVALID, "null argument");
-  *out = nullptr;
+// The trainer of any trainable kind (the entry points below check the kind against their own lists first)
+int trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
+                   const srs_adam* hp, srs_trainer** out) {
   const srs_spec& s = *spec;
-  const bool fm = s.kind == SRS_DEEPFM, wd = s.kind == SRS_WIDENDEEP;
-  if (s.kind != SRS_NEURALCF && !fm && !wd)
-    return failf(SRS_ERR_INVALID, "fit is implemented for NeuralCF (neural_cf_model_1), DeepFM and Wide&Deep only");
+  const bool fm = s.kind == SRS_DEEPFM, wd = s.kind == SRS_WIDENDEEP, fm2 = s.kind == SRS_DEEPFM_V2;
   if (s.emb_dim < 1 || s.emb_dim > 64) return failf(SRS_ERR_INVALID, "emb_dim must be in 1..64");
   if (s.n_movies < 1 || s.n_users < 1) return failf(SRS_ERR_INVALID, "empty vocabulary");
   int hmax = 0;
@@ -466,6 +459,12 @@ int srs_trainer_create_ex(const srs_spec* spec, const srs_tensor* tensors, int32
     for (int i = 0; i < 2; ++i)
       if (s.hidden[i] < 1 || s.hidden[i] > 128)
         return failf(SRS_ERR_INVALID, "Wide&Deep's hidden widths must be in 1..128");
+  } else if (fm2) {
+    if (s.n_hidden != 2) return failf(SRS_ERR_INVALID, "DeepFM_v2's fit needs exactly 2 hidden layers");
+    if (s.proj_dim != 64) return failf(SRS_ERR_INVALID, "DeepFM_v2's fit needs proj_dim 64");
+    if (s.n_genres < 1) return failf(SRS_ERR_INVALID, "empty genre vocabulary");
+    if (s.hidden[0] < 1 || s.hidden[0] > 32 || s.hidden[1] < 1 || s.hidden[1] > 16)
+      return failf(SRS_ERR_INVALID, "DeepFM_v2's hidden widths must be in 1..32 and 1..16");
   } else {
     if (s.n_hidden < 1 || s.n_hidden > 3) return failf(SRS_ERR_INVALID, "1..3 hidden layers supported");
     for (int i = 0; i < s.n_hidden; ++i) {
@@ -497,6 +496,10 @@ int srs_trainer_create_ex(const srs_spec* spec, const srs_tensor* tensors, int32
     t->place = place_embmlp(s, EP, &t->emb);
     t->blob_floats = EmbMlpBlob::of(EP).floats;
     t->onehot = s.cross_buckets;
+  } else if (fm2) {
+    t->place = place_deepfm2(s, EP, &t->fm2);
+    t->blob_floats = DeepFm2Blob::of(EP).floats;
+    t->onehot = (int64_t)2 * s.n_genres + s.n_movies + s.n_users;
   } else {
     t->HP = hmax <= 16 ? 16 : 32;
     t->place = place_ncf(s, EP, t->HP, &t->ncf);
@@ -516,7 +519,8 @@ int srs_trainer_create_ex(const srs_spec* spec, const srs_tensor* tensors, int32
   }
 
   cudaError_t ce = cudaSetDevice(device);
-  if (ce == cudaSuccess && fm) ce = setup_deepfm_attributes();   // validation and evaluate run deepfm_kernel
+  if (ce == cudaSuccess && (fm || fm2)) ce = setup_deepfm_attributes();   // validation and evaluate run deepfm_kernel
+                                                                          //   (DeepFM_v2: deepfm2_kernel)
   if (ce == cudaSuccess && wd) ce = setup_embmlp_attributes();   //   (Wide&Deep: embmlp_kernel)
   if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&t->stream, cudaStreamNonBlocking);
   for (int k = 0; k < 4 && ce == cudaSuccess; ++k) ce = cudaMalloc(&t->tab[k], t->tab_floats * sizeof(float));
@@ -554,6 +558,11 @@ int srs_trainer_create_ex(const srs_spec* spec, const srs_tensor* tensors, int32
     for (int k = 0; k < kWideDeepTables; ++k) tables[k] = table(k);
     point_into_blob(&t->emb, tables, t->blob[0]);
     t->emb.wide = t->fo[0];
+  } else if (fm2) {
+    const float* tables[kDeepFm2Tables];
+    for (int k = 0; k < kDeepFm2Tables; ++k) tables[k] = table(k);
+    point_into_blob(&t->fm2, tables, t->blob[0]);
+    t->fm2.first = t->fo[0];
   } else {
     t->ncf.movie = table(0);
     t->ncf.user = table(1);
@@ -561,6 +570,44 @@ int srs_trainer_create_ex(const srs_spec* spec, const srs_tensor* tensors, int32
   }
   *out = t;
   return SRS_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+// NeuralCF and DeepFM only, as this entry point has always been documented
+int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
+                       const srs_adam* hp, srs_trainer** out) {
+  if (!spec || !out) return failf(SRS_ERR_INVALID, "null argument");
+  *out = nullptr;
+  if (spec->kind != SRS_NEURALCF && spec->kind != SRS_DEEPFM)
+    return failf(SRS_ERR_INVALID, "srs_trainer_create trains NeuralCF (neural_cf_model_1) and DeepFM only; "
+                 "srs_trainer_create_ex also trains Wide&Deep");
+  return trainer_create(spec, tensors, n_tensors, device, hp, out);
+}
+
+// NeuralCF, DeepFM and Wide&Deep, as this entry point has always been documented
+int srs_trainer_create_ex(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
+                          const srs_adam* hp, srs_trainer** out) {
+  if (!spec || !out) return failf(SRS_ERR_INVALID, "null argument");
+  *out = nullptr;
+  if (spec->kind != SRS_NEURALCF && spec->kind != SRS_DEEPFM && spec->kind != SRS_WIDENDEEP)
+    return failf(SRS_ERR_INVALID, "fit is implemented for NeuralCF (neural_cf_model_1), DeepFM and Wide&Deep only; "
+                 "srs_trainer_create_any trains every kind this library can train");
+  return trainer_create(spec, tensors, n_tensors, device, hp, out);
+}
+
+// every kind this library can train; the list grows with the library
+int srs_trainer_create_any(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
+                           const srs_adam* hp, srs_trainer** out) {
+  if (!spec || !out) return failf(SRS_ERR_INVALID, "null argument");
+  *out = nullptr;
+  const int k = spec->kind;
+  if (k != SRS_NEURALCF && k != SRS_DEEPFM && k != SRS_WIDENDEEP && k != SRS_DEEPFM_V2)
+    return failf(SRS_ERR_INVALID, "fit is implemented for NeuralCF (neural_cf_model_1), DeepFM, Wide&Deep and "
+                 "DeepFM_v2 only");
+  return trainer_create(spec, tensors, n_tensors, device, hp, out);
 }
 
 void srs_trainer_destroy(srs_trainer* t) { trainer_free(t); }
@@ -578,7 +625,7 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
                                   const srs_batch* val_batch, const int32_t* val_labels, int32_t val_freq,
                                   srs_eval_result* val_history) {
   if (!t || !batch || !labels || !order) return failf(SRS_ERR_INVALID, "null argument");
-  const bool fm = t->spec.kind == SRS_DEEPFM, wd = t->spec.kind == SRS_WIDENDEEP;
+  const bool fm = t->spec.kind == SRS_DEEPFM, wd = t->spec.kind == SRS_WIDENDEEP, fm2 = t->spec.kind == SRS_DEEPFM_V2;
   const int n = batch->B;
   if (n < 1) return failf(SRS_ERR_INVALID, "fit needs at least one row");
   if (batch_size < 1) return failf(SRS_ERR_INVALID, "batch_size must be at least 1");
@@ -607,9 +654,12 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
   }
   CUDA_TRY(cudaSetDevice(t->device));
   const int EP = t->EP, Bmax = std::min(batch_size, n);
-  const int n_ent = fm ? kDeepFmTables : wd ? kWideDeepTables : 2;   // table entries per row
-  const int n_cta = fm ? deepfm_train_ctas(Bmax) : wd ? widendeep_train_ctas(Bmax)
-                                                      : (Bmax + kTrainRows - 1) / kTrainRows;
+  const int n_ent = fm ? kDeepFmTables : wd ? kWideDeepTables : fm2 ? kDeepFm2Tables : 2;   // table entries per row
+  auto step_ctas = [&](int B) {
+    return fm ? deepfm_train_ctas(B) : wd ? widendeep_train_ctas(B) : fm2 ? deepfm2_train_ctas(B)
+                                                                         : (B + kTrainRows - 1) / kTrainRows;
+  };
+  const int n_cta = step_ctas(Bmax);
   cudaStream_t s = t->stream;
   Scratch sc;
   int32_t *d_order, *d_trow, *d_lab_b = nullptr, *d_frow = nullptr;
@@ -625,10 +675,10 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
   CUDA_TRY(sc.alloc(&d_met, epochs));
   CUDA_TRY(cudaMemcpyAsync(d_order, order, (size_t)epochs * n * 4, cudaMemcpyHostToDevice, s));
   CUDA_TRY(cudaMemsetAsync(d_met, 0, sizeof(MetricsState) * epochs, s));
-  DeepFmRows src{}, rows{};                            // the dataset, and (DeepFM, Wide&Deep) the epoch's rows in order
+  DeepFmRows src{}, rows{};                            // the dataset, and (but NeuralCF) the epoch's rows in order
   CUDA_TRY(upload_rows(sc, t->spec.kind, batch, labels, &src, s));
-  const int n_fent = fm ? 4 : 1;                       // one-hot entries per row (DeepFM, Wide&Deep)
-  if (fm || wd) {
+  const int n_fent = wd ? 1 : 4;                       // one-hot entries per row (DeepFM, DeepFM_v2, Wide&Deep)
+  if (fm || wd || fm2) {
     cudaError_t e;
     rows = deepfm_rows(sc, n, wd, &e);
     CUDA_TRY(e);
@@ -675,47 +725,37 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
     w.b.probs = d_probs; w.b.logits = d_logits; w.b.err_flag = d_err; w.b.hist_stride = 1;
     w.trow = d_trow; w.gemb = d_gemb; w.wrow = d_frow; w.wgrad = d_fgrad; w.part = d_part;
   }
+  DeepFm2StepArgs v{};
+  if (fm2) {
+    v.p = t->fm2;
+    for (int k = 0; k < kDeepFm2Tables; ++k) v.tab_row0[k] = t->place[k].table_row;   // the tables come first
+    v.b.probs = d_probs; v.b.logits = d_logits; v.b.err_flag = d_err;
+    v.trow = d_trow; v.gemb = d_gemb; v.frow = d_frow; v.fgrad = d_fgrad; v.part = d_part;
+  }
   int64_t steps = 0;
   for (int e = 0; e < epochs; ++e) {
-    if (fm) CUDA_TRY(launch_deepfm_permute(src, rows, d_order + (size_t)e * n, n, s));
+    if (fm || fm2) CUDA_TRY(launch_deepfm_permute(src, rows, d_order + (size_t)e * n, n, s));
     if (wd) CUDA_TRY(launch_widendeep_permute(src, rows, d_order + (size_t)e * n, n, s));
     for (int off = 0; off < n; off += batch_size) {
       const int B = std::min(batch_size, n - off);
       const int32_t* step_labels;
-      if (fm) {
-        f.b.B = B;
-        f.b.movie_id = rows.movie + off; f.b.user_id = rows.user + off;
-        f.b.movie_genre = rows.mgenre + (size_t)off * 3; f.b.user_genre = rows.ugenre + (size_t)off * 5;
-        f.b.numerics = rows.numerics + (size_t)off * kNumNumerics;
-        f.label = rows.label + off;
-        step_labels = f.label;
-        CUDA_TRY(launch_deepfm_train_step(f, s));
-        table_grad_kernel<<<(kDeepFmTables * B + 127) / 128, 128, 0, s>>>(d_trow, d_gemb, kDeepFmTables * B, EP,
-                                                                          t->tab[3]);
-        table_grad_kernel<<<(4 * B + 127) / 128, 128, 0, s>>>(d_frow, d_fgrad, 4 * B, 1, t->fo[3]);
+      if (fm || wd || fm2) {                           // the model's step, both dedupes, both forms of Adam
+        BatchView& b = fm ? f.b : wd ? w.b : v.b;
+        b.B = B;
+        b.movie_id = rows.movie + off; b.user_id = rows.user + off;
+        b.movie_genre = rows.mgenre + (size_t)off * 3; b.user_genre = rows.ugenre + (size_t)off * 5;
+        b.numerics = rows.numerics + (size_t)off * kNumNumerics;
+        if (wd) b.hist = rows.rated + off;
+        step_labels = f.label = w.label = v.label = rows.label + off;
+        CUDA_TRY(fm ? launch_deepfm_train_step(f, s) : wd ? launch_widendeep_train_step(w, s)
+                                                          : launch_deepfm2_train_step(v, s));
+        table_grad_kernel<<<(n_ent * B + 127) / 128, 128, 0, s>>>(d_trow, d_gemb, n_ent * B, EP, t->tab[3]);
+        table_grad_kernel<<<(n_fent * B + 127) / 128, 128, 0, s>>>(d_frow, d_fgrad, n_fent * B, 1, t->fo[3]);
         table_adam_kernel<false><<<adam_blocks, 256, 0, s>>>(t->tab[0], t->tab[1], t->tab[2], t->tab[3],
                                                              t->tab_floats, t->hp, t->d_it);
         table_adam_kernel<true><<<fo_blocks, 256, 0, s>>>(t->fo[0], t->fo[1], t->fo[2], t->fo[3], t->onehot, t->hp,
                                                           t->d_it);
-        dense_adam_kernel<<<1, kAdamThreads, 0, s>>>(d_part, deepfm_train_ctas(B), t->blob_floats, t->blob[0],
-                                                     t->blob[1], t->blob[2], t->hp, t->d_it);
-        g_launch_count += 5;
-      } else if (wd) {
-        w.b.B = B;
-        w.b.movie_id = rows.movie + off; w.b.user_id = rows.user + off; w.b.hist = rows.rated + off;
-        w.b.movie_genre = rows.mgenre + (size_t)off * 3; w.b.user_genre = rows.ugenre + (size_t)off * 5;
-        w.b.numerics = rows.numerics + (size_t)off * kNumNumerics;
-        w.label = rows.label + off;
-        step_labels = w.label;
-        CUDA_TRY(launch_widendeep_train_step(w, s));
-        table_grad_kernel<<<(kWideDeepTables * B + 127) / 128, 128, 0, s>>>(d_trow, d_gemb, kWideDeepTables * B, EP,
-                                                                            t->tab[3]);
-        table_grad_kernel<<<(B + 127) / 128, 128, 0, s>>>(d_frow, d_fgrad, B, 1, t->fo[3]);
-        table_adam_kernel<false><<<adam_blocks, 256, 0, s>>>(t->tab[0], t->tab[1], t->tab[2], t->tab[3],
-                                                             t->tab_floats, t->hp, t->d_it);
-        table_adam_kernel<true><<<fo_blocks, 256, 0, s>>>(t->fo[0], t->fo[1], t->fo[2], t->fo[3], t->onehot, t->hp,
-                                                          t->d_it);
-        dense_adam_kernel<<<1, kAdamThreads, 0, s>>>(d_part, widendeep_train_ctas(B), t->blob_floats, t->blob[0],
+        dense_adam_kernel<<<1, kAdamThreads, 0, s>>>(d_part, step_ctas(B), t->blob_floats, t->blob[0],
                                                      t->blob[1], t->blob[2], t->hp, t->d_it);
         g_launch_count += 5;
       } else {

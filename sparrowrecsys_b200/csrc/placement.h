@@ -1,6 +1,6 @@
 // placement.h - where the Keras tensors of the trainable models (NeuralCF's neural_cf_model_1 and two towers, DeepFM,
-// and EmbeddingMLP / Wide&Deep) live on the device, written once for the serving builders (build_ncf, build_deepfm,
-// build_embmlp in model.cu) and the
+// DeepFM_v2 and EmbeddingMLP / Wide&Deep) live on the device, written once for the serving builders (build_ncf,
+// build_deepfm, build_deepfm2, build_embmlp in model.cu) and the
 // trainer (srs_trainer_create, srs_trainer_get_weights in ncf_train.cu): the builders and the trainer scatter the
 // caller's host tensors through it, and the trainer gathers its weights back through it.  Also the by-name lookup of
 // the caller's tensors that both use.  Host code only.
@@ -81,7 +81,8 @@ struct TensorLookup {
 // Rows of a Dense tensor [rows][cols] in one zero-padded block of the Dense-weight blob or of the one-hot array
 struct Block {
   bool onehot;                   // false: the blob; true: the one-hot array, the [fm1_width] one-hot rows of DeepFM's
-                                 // dense_2/kernel or the [cross_buckets] wide rows of Wide&Deep's
+                                 // dense_2/kernel or DeepFM_v2's first_cat/kernel, or the [cross_buckets] wide rows of
+                                 // Wide&Deep's dense_2/kernel
   int at;                        // the block's first float
   int width;                     // floats per block row: the tensor's cols, zero padded
   std::vector<int> map;          // block row i holds tensor row map[i]; -1: a zero row
@@ -212,6 +213,60 @@ inline void point_into_blob(DeepFmParams* p, const float* blob) {
   p->blob = blob;
   p->W1 = blob + ly.W1; p->b1 = blob + ly.b1; p->W2 = blob + ly.W2; p->b2 = blob + ly.b2;
   p->wdeep = blob + ly.wdeep;
+}
+
+// DeepFM_v2: the four tables in field order (movieGenre1, movieId, userGenre1, userId: kDeepFm2Tables), the Dense
+// tensors in a DeepFm2Blob::of(EP) and first_cat/kernel's one-hot rows in their own [fm1_width] array, looked up in
+// the order the builder has always used.  Fills p's sizes and EP.
+inline Placement place_deepfm2(const srs_spec& s, int EP, DeepFm2Params* p) {
+  const int E = s.emb_dim, h0 = s.hidden[0], h1 = s.hidden[1], P = 64;
+  const int fm1 = 2 * s.n_genres + s.n_movies + s.n_users;
+  const DeepFm2Blob ly = DeepFm2Blob::of(EP);
+  const char* fields[4] = {"movieGenre1", "movieId", "userGenre1", "userId"};
+  const int64_t rows[4] = {s.n_genres, s.n_movies, s.n_genres, s.n_users};
+  Placement pl;
+  char name[64];
+  for (int f = 0; f < 4; ++f) {
+    snprintf(name, sizeof name, "%s_embedding", fields[f]);
+    place_table(pl, name, rows[f], E);
+  }
+  place_dense(pl, "first_cat/kernel", fm1, 1, {Block{true, 0, 1, iota_map(0, fm1, fm1)}});
+  place_dense(pl, "first_cat/bias", 1, 1, {Block{false, ly.first_cat_b, 1, iota_map(0, 1, 1)}});
+  place_dense(pl, "first_num/kernel", kNumNumerics, 1, {Block{false, ly.first_num, 1, iota_map(0, 7, kNumPad)}});
+  place_dense(pl, "first_num/bias", 1, 1, {Block{false, ly.first_num_b, 1, iota_map(0, 1, 1)}});
+  for (int f = 0; f < 4; ++f) {
+    snprintf(name, sizeof name, "proj_%s/kernel", fields[f]);
+    place_dense(pl, name, E, P, {Block{false, ly.proj + f * EP * P, P, iota_map(0, E, EP)}});
+    snprintf(name, sizeof name, "proj_%s/bias", fields[f]);
+    place_dense(pl, name, P, 1, {Block{false, ly.proj_b + f * P, 1, iota_map(0, P, P)}});
+  }
+  place_dense(pl, "proj_num/kernel", kNumNumerics, P, {Block{false, ly.proj_num, P, iota_map(0, 7, kNumPad)}});
+  place_dense(pl, "proj_num/bias", P, 1, {Block{false, ly.proj_num_b, 1, iota_map(0, P, P)}});
+  place_dense(pl, "deep/kernel", 5 * P, h0, {Block{false, ly.Wd, 32, iota_map(0, 5 * P, 5 * P)}});
+  place_dense(pl, "deep/bias", h0, 1, {Block{false, ly.bd, 1, iota_map(0, h0, 32)}});
+  place_dense(pl, "deep_1/kernel", h0, h1, {Block{false, ly.Wd1, 16, iota_map(0, h0, 32)}});
+  place_dense(pl, "deep_1/bias", h1, 1, {Block{false, ly.bd1, 1, iota_map(0, h1, 16)}});
+  // out/kernel: first | fm (64) | deep (h1), the deep rows padded to 16
+  place_dense(pl, "out/kernel", 1 + P + h1, 1, {Block{false, ly.wout, 1, iota_map(0, 1 + P + h1, 84)}});
+  place_dense(pl, "out/bias", 1, 1, {Block{false, ly.bout, 1, iota_map(0, 1, 1)}});
+  p->n_movies = s.n_movies; p->n_users = s.n_users; p->n_genres = s.n_genres; p->EP = EP;
+  return pl;
+}
+
+// p's tables (tables[k]: the k-th table of place_deepfm2's order) and Dense-weight pointers into a DeepFm2Blob on
+// the device
+inline void point_into_blob(DeepFm2Params* p, const float* const* tables, const float* blob) {
+  const DeepFm2Blob ly = DeepFm2Blob::of(p->EP);
+  p->mgenre = tables[0]; p->movie = tables[1]; p->ugenre = tables[2]; p->user = tables[3];
+  p->blob = blob;
+  p->first_num = blob + ly.first_num;
+  for (int f = 0; f < 4; ++f) {
+    p->proj[f] = blob + ly.proj + f * p->EP * 64;
+    p->proj_b[f] = blob + ly.proj_b + f * 64;
+  }
+  p->proj_num = blob + ly.proj_num; p->proj_num_b = blob + ly.proj_num_b;
+  p->Wd = blob + ly.Wd; p->bd = blob + ly.bd; p->Wd1 = blob + ly.Wd1; p->bd1 = blob + ly.bd1;
+  p->wout = blob + ly.wout;
 }
 
 // EmbeddingMLP and Wide&Deep: the ten tables (movieGenre1..3, userGenre1..5, movieId, userId: the order the

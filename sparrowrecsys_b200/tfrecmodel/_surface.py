@@ -67,14 +67,14 @@ class Surface:
 
     def fit(self, features, epochs: int = 5, batch_size: int = 12, seed: int = 0, validation_data=None,
             validation_split: float = 0.0, validation_freq: int = 1) -> dict:
-        """`model.fit(train_dataset, epochs=5)` (NeuralCF.py:91, DeepFM.py, WideNDeep.py:117): train from the weights `model` was
-        loaded with, then rebuild `model` from the trained weights.  Returns Keras's history dict, with the
-        `val_*` lists when `validation_data` or `validation_split` is given (`Trainer.fit`).  NeuralCF, DeepFM
-        and Wide&Deep only."""
-        if self.name not in ("neuralcf", "deepfm", "widendeep"):
+        """`model.fit(train_dataset, epochs=5)` (NeuralCF.py:91, DeepFM.py, WideNDeep.py:117,
+        DeepFM_v2.py:165): train from the weights `model` was loaded with, then rebuild `model` from the trained
+        weights.  Returns Keras's history dict, with the `val_*` lists when `validation_data` or
+        `validation_split` is given (`Trainer.fit`).  NeuralCF, DeepFM, Wide&Deep and DeepFM_v2 only."""
+        if self.name not in ("neuralcf", "deepfm", "widendeep", "deepfm_v2"):
             raise NotImplementedError("tfrecmodel.%s: fit is implemented for NeuralCF (tfrecmodel.neuralcf), "
-                                      "DeepFM (tfrecmodel.deepfm) and Wide&Deep (tfrecmodel.widendeep) only"
-                                      % self.name)
+                                      "DeepFM (tfrecmodel.deepfm), Wide&Deep (tfrecmodel.widendeep) and DeepFM_v2 "
+                                      "(tfrecmodel.deepfm_v2) only" % self.name)
         if self.model is None or self.weights is None:
             raise RuntimeError("tfrecmodel.%s: call load() before fit()" % self.name)
         from ..training import Trainer

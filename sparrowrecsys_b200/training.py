@@ -1,6 +1,6 @@
-"""`model.fit` of NeuralCF, DeepFM and Wide&Deep on the GPU (NeuralCF.py:74-91, DeepFM.py, WideNDeep.py:99-117:
-compile(loss='binary_crossentropy', optimizer='adam'), then fit(train_dataset, epochs=5) over make_csv_dataset batches
-of 12).
+"""`model.fit` of NeuralCF, DeepFM, Wide&Deep and DeepFM_v2 on the GPU (NeuralCF.py:74-91, DeepFM.py,
+WideNDeep.py:99-117, DeepFM_v2.py:158-165: compile(loss='binary_crossentropy', optimizer='adam'), then
+fit(train_dataset, epochs=5) over make_csv_dataset batches of 12).
 
     from sparrowrecsys_b200.training import Trainer
     tr = Trainer(spec, weights, device=0)                 # initial weights in Keras shapes
@@ -10,7 +10,7 @@ of 12).
     model = tr.to_model()                                 # a serving CTRModel built from the trained weights
 
 The forward, backward and Keras Adam run in the CUDA library (`srs_trainer_*`, include/srs_ctr.h; DESIGN.md
-sections 4.8, 4.9 and 4.18).  TF's shuffle (buffer 10 000, unseeded) cannot be reproduced, so `fit` takes a seed instead: the host
+sections 4.8, 4.9, 4.18 and 4.19).  TF's shuffle (buffer 10 000, unseeded) cannot be reproduced, so `fit` takes a seed instead: the host
 draws one `numpy.random.default_rng(seed).permutation(n)` per epoch and the library trains in that row order.
 """
 from __future__ import annotations
@@ -34,19 +34,19 @@ def epoch_orders(n: int, epochs: int, seed: int) -> np.ndarray:
 
 
 class Trainer:
-    """Trainable NeuralCF, DeepFM or Wide&Deep weights and Keras Adam's state on one GPU."""
+    """Trainable NeuralCF, DeepFM, Wide&Deep or DeepFM_v2 weights and Keras Adam's state on one GPU."""
 
-    MODELS = ("neuralcf", "deepfm", "widendeep")
+    MODELS = ("neuralcf", "deepfm", "widendeep", "deepfm_v2")
 
     def __init__(self, spec: ModelSpec, weights: Mapping[str, np.ndarray], device: int = 0,
                  adam: Optional[Mapping[str, float]] = None):
         """`weights`: the initial weights (canonical names, Keras shapes, float32 host arrays), e.g.
         `init_weights(spec, seed, for_test=False)` for an untrained model.  `adam`: Keras Adam's lr, beta_1,
         beta_2, epsilon (default: Keras's 0.001, 0.9, 0.999, 1e-7).  NotImplementedError for any model but
-        NeuralCF, DeepFM and Wide&Deep."""
+        NeuralCF, DeepFM, Wide&Deep and DeepFM_v2."""
         if spec.model not in self.MODELS:
-            raise NotImplementedError("fit is implemented for NeuralCF (neural_cf_model_1), DeepFM and Wide&Deep only, "
-                                      "not %r" % spec.model)
+            raise NotImplementedError("fit is implemented for NeuralCF (neural_cf_model_1), DeepFM, Wide&Deep and "
+                                      "DeepFM_v2 only, not %r" % spec.model)
         self.spec = spec
         self.device = int(device)
         self._h = None
@@ -67,7 +67,7 @@ class Trainer:
             hp = C.byref(_lib.SrsAdam(d["lr"], d["beta_1"], d["beta_2"], d["epsilon"]))
         h = C.c_void_p()
         sp = _spec_struct(spec)
-        _lib.check(self._lib.srs_trainer_create_ex(C.byref(sp), tensors, len(shapes), self.device, hp, C.byref(h)))
+        _lib.check(self._lib.srs_trainer_create_any(C.byref(sp), tensors, len(shapes), self.device, hp, C.byref(h)))
         self._h = h
 
     def close(self):
@@ -96,7 +96,7 @@ class Trainer:
             order=None, validation_data=None, validation_split: float = 0.0,
             validation_freq: int = 1) -> Dict[str, list]:
         """`model.fit(dataset, epochs)`: train on the rows of `features` (the model's `predict` columns: `movieId`,
-        `userId` for NeuralCF, also the 7 numerics, `movieGenre1` and `userGenre1` for DeepFM, the 7 numerics, all eight
+        `userId` for NeuralCF, also the 7 numerics, `movieGenre1` and `userGenre1` for DeepFM and DeepFM_v2, the 7 numerics, all eight
         genre columns and `userRatedMovie1` for Wide&Deep; labels default to
         `features["label"]`) in batches of `batch_size`, the last one partial.  The row order of epoch e is
         `epoch_orders(n, epochs, seed)[e]` unless `order` ([epochs][n], each a permutation) is given.  Returns
