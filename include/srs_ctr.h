@@ -413,8 +413,10 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
 int srs_trainer_create_ex(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
                           const srs_adam* hp, srs_trainer** out);
 /* srs_trainer_create for every kind this library can train; the list grows with the library, so a kind it rejects
- * today (SRS_ERR_INVALID) may be accepted by a later version.  Today: SRS_NEURALCF, SRS_DEEPFM, SRS_WIDENDEEP and
- * SRS_DEEPFM_V2 (its tensors as srs_model_create takes them).  Callers that rely on a fixed list use
+ * today (SRS_ERR_INVALID) may be accepted by a later version.  Today: SRS_NEURALCF, SRS_DEEPFM, SRS_WIDENDEEP,
+ * SRS_DEEPFM_V2 and SRS_DIEN (its tensors as srs_model_create takes them; DIEN's include the auxiliary head's group
+ * of eight, which its objective needs; it accepts emb_dim 1..32, hist_len 1..64, au_hidden 32 and hidden widths up
+ * to (128, 64), and trains through srs_trainer_fit_dien_host).  Callers that rely on a fixed list use
  * srs_trainer_create or srs_trainer_create_ex, whose lists do not change. */
 int srs_trainer_create_any(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
                            const srs_adam* hp, srs_trainer** out);
@@ -454,6 +456,22 @@ int srs_trainer_fit_validate_host(srs_trainer* tr, const srs_batch* batch, const
  * the serving CUDA-core forward over the trainer's arrays and folded into the metrics on the device.  Synchronous;
  * the checks and errors of srs_trainer_fit_host's rows, before any launch. */
 int srs_trainer_evaluate_host(srs_trainer* tr, const srs_batch* batch, const int32_t* labels, srs_eval_result* out);
+
+/* `model.fit` of DIEN (DIEN.py:296-304; DESIGN.md section 4.20): `epochs` epochs over the n = batch->B rows of
+ * `batch` (host: movie_id, user_id, movie_genre and user_genre (column 0 read), numerics and hist [n][hist_stride
+ * >= hist_len]) with their negatives neg_hist [n][neg_stride >= hist_len - 1] (NULL for hist_len 1) and labels [n]
+ * int32; epoch e trains rows order[e * n .. e * n + n) (a permutation of 0..n-1; the script's is file order) in
+ * batches of batch_size, the last one partial.  The objective of a batch is the SUM over its rows of final_loss_i
+ * = bce_i - 0.5 * mean_j aux_j (srs_dien_outputs_device), so dL/dz_i = sigmoid(z_i) - y_i; the GRU consumes the
+ * history mask, augru_h0 is not trained, the four tables take Keras's sparse Adam on every row and every other
+ * tensor ApplyAdam.  history (NULL or [epochs]) gets each epoch's {rows, batches, loss, auc, auc_value} as
+ * srs_dien_evaluate_host_batches reports them, over the steps' outputs before their updates.  Every check (ids,
+ * negatives, genres, labels, the order) runs before any launch, so a rejected call leaves the weights as they were;
+ * SRS_ERR_INVALID for a trainer of another kind, whose fit is srs_trainer_fit_host (and srs_trainer_fit_host,
+ * srs_trainer_fit_validate_host and srs_trainer_evaluate_host reject a DIEN trainer). */
+int srs_trainer_fit_dien_host(srs_trainer* tr, const srs_batch* batch, const int32_t* neg_hist, int32_t neg_stride,
+                              const int32_t* labels, const int32_t* order, int32_t batch_size, int32_t epochs,
+                              srs_dien_eval_result* history);
 
 /* Copy one trained tensor, in its Keras shape, to host memory `dst` (SRS_ERR_MISSING for an unknown name). */
 int srs_trainer_get_weights(const srs_trainer* tr, const char* name, float* dst);

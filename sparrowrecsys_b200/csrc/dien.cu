@@ -25,65 +25,12 @@
 // hist[t]: they are g_t and e(h_{t+1}) above, and the negative row e(neg[t-1]) is gathered beside x.  Lane
 // j owns unit j of both Dense32 layers; their weights (aux_pos_* / aux_neg_*, 2 (64 EP + 66) floats: 16.5 KB
 // at EP = 32) are staged after the sequence part.  The plain variant compiles without any of it.
-#include <cmath>
-
-#include "kernels.h"
+//
+// The per-row arithmetic (GRU, attention, AUGRU, auxiliary head) lives in dien_layers.cuh, which the training step
+// (dien_train.cu) shares.
+#include "dien_layers.cuh"
 
 namespace srs {
-
-constexpr int kDienRows = 32;     // rows per CTA tile
-
-template <int EP>
-struct DienBlob {                 // float offsets inside DienParams::seq (see model.cu::build_dien)
-  static constexpr int GW = 0;                       // gru kernel            [EP k][3][EP]
-  static constexpr int GU = GW + 3 * EP * EP;        // gru recurrent kernel  [EP k][3][EP]
-  static constexpr int AW = GU + 3 * EP * EP;        // attention Dense32     [EP k][32]
-  static constexpr int IW = AW + 32 * EP;            // augru input kernels   [3 g][EP k][EP]
-  static constexpr int HW = IW + 3 * EP * EP;        // augru hidden kernels  [3 g][EP k][EP]
-  static constexpr int SW = HW + 3 * EP * EP;        // augru act kernels     [3 g][EP k][EP]
-  static constexpr int BX = SW + 3 * EP * EP;        // gru input bias        [3][EP]
-  static constexpr int BH = BX + 3 * EP;             // gru recurrent bias    [3][EP]
-  static constexpr int BI = BH + 3 * EP;             // augru input bias      [3][EP]
-  static constexpr int BA = BI + 3 * EP;             // augru act bias        [3][EP]
-  static constexpr int H0 = BA + 3 * EP;             // augru initial state   [EP]
-  static constexpr int AB = H0 + EP;                 // attention Dense32 bias [32]
-  static constexpr int AO = AB + 32;                 // attention Dense1 kernel [32]
-  static constexpr int ABO = AO + 32;                // attention Dense1 bias  [1] (+3 pad)
-  static constexpr int TOTAL = ABO + 4;
-};
-
-template <int EP>
-struct DienAuxBlob {              // float offsets inside DienAuxView::w (see model.cu::build_dien)
-  static constexpr int PW = 0;                       // aux_pos_dense/kernel  [2EP k][32]: g_t rows, then e rows
-  static constexpr int NW = PW + 64 * EP;            // aux_neg_dense/kernel  [2EP k][32]
-  static constexpr int PB = NW + 64 * EP;            // aux_pos_dense/bias    [32]
-  static constexpr int NB = PB + 32;                 // aux_neg_dense/bias    [32]
-  static constexpr int PO = NB + 32;                 // aux_pos_out/kernel    [32]
-  static constexpr int NO = PO + 32;                 // aux_neg_out/kernel    [32]
-  static constexpr int POB = NO + 32;                // aux_pos_out/bias      [1]
-  static constexpr int NOB = POB + 1;                // aux_neg_out/bias      [1] (+2 pad)
-  static constexpr int TOTAL = POB + 4;
-};
-
-// pos_t + neg_t of one position: g = g_t, e = e(h_{t+1}), n = e(n_{t+1}), lane k holding element k
-template <int EP>
-__device__ __forceinline__ float dien_aux_step(const float* Sa, float g, float e, float n, int lane) {
-  using A = DienAuxBlob<EP>;
-  float ap = Sa[A::PB + lane], an = Sa[A::NB + lane];
-#pragma unroll
-  for (int k = 0; k < EP; ++k) {
-    const float gk = __shfl_sync(0xffffffffu, g, k);
-    const float ek = __shfl_sync(0xffffffffu, e, k);
-    const float nk = __shfl_sync(0xffffffffu, n, k);
-    ap = fmaf(gk, Sa[A::PW + k * 32 + lane], ap);
-    an = fmaf(gk, Sa[A::NW + k * 32 + lane], an);
-    ap = fmaf(ek, Sa[A::PW + (EP + k) * 32 + lane], ap);
-    an = fmaf(nk, Sa[A::NW + (EP + k) * 32 + lane], an);
-  }
-  const float pos = sigmoidf_acc(warp_sum(sigmoidf_acc(ap) * Sa[A::PO + lane]) + Sa[A::POB]);
-  const float neg = sigmoidf_acc(warp_sum(sigmoidf_acc(an) * Sa[A::NO + lane]) + Sa[A::NOB]);
-  return pos + neg;
-}
 
 template <int EP, bool AUX>
 __global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView b, DienAuxView ax) {
@@ -118,12 +65,6 @@ __global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView 
 
   // ---- interest evolution: one warp per row, lane = state element --------------------
   const int le = lane < EP ? lane : EP - 1;          // lanes >= EP mirror lane EP-1 (unused)
-  const float* gw = Sq + L::GW + le;
-  const float* gu = Sq + L::GU + le;
-  const float* aw = Sq + L::AW + lane;
-  const float* iw = Sq + L::IW + le;
-  const float* hw = Sq + L::HW + le;
-  const float* sw = Sq + L::SW + le;
   const float att_b = Sq[L::AB + lane], att_wo = Sq[L::AO + lane], att_bo = Sq[L::ABO];
   for (int r = warp; r < R; r += kThreads / 32) {
     const int row = row0 + r;
@@ -133,7 +74,7 @@ __global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView 
       continue;
     }
     // ids pass through float32 numeric columns before the Embedding layer (DIEN.py:96-105)
-    int cid = __float2int_rz(__int2float_rn(__ldg(b.movie_id + row)));
+    int cid = dien_id(__ldg(b.movie_id + row));
     cid = checked_id(cid, p.n_movies, b.err_flag);
     const float c = lane < EP ? __ldg(p.movie + (size_t)cid * EP + lane) : 0.f;
     const int32_t* hrow = b.hist + (size_t)row * b.hist_stride;
@@ -144,7 +85,7 @@ __global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView 
     for (int t = 0; t < p.T; ++t) {
       const int raw = hid_next;
       if (t + 1 < p.T) hid_next = __ldg(hrow + t + 1);
-      int hid = __float2int_rz(__int2float_rn(raw));
+      int hid = dien_id(raw);
       const bool valid = hid != 0;                         // Embedding(mask_zero=True) mask
       hid = checked_id(hid, p.n_movies, b.err_flag);
       const float x = lane < EP ? __ldg(p.movie + (size_t)hid * EP + lane) : 0.f;
@@ -152,72 +93,22 @@ __global__ void __launch_bounds__(kThreads) dien_kernel(DienParams p, BatchView 
       if constexpr (AUX) {
         if (t > 0) {
           g_prev = h;
-          int nid = __float2int_rz(__int2float_rn(__ldg(ax.neg + (size_t)row * ax.neg_stride + t - 1)));
+          int nid = dien_id(__ldg(ax.neg + (size_t)row * ax.neg_stride + t - 1));
           nid = checked_id(nid, p.n_movies, b.err_flag);
           xn = lane < EP ? __ldg(p.movie + (size_t)nid * EP + lane) : 0.f;
         }
       }
-      // -- GRU step (Keras: z | r | h, reset_after)
-      float xz = Sq[L::BX + le], xr = Sq[L::BX + EP + le], xh = Sq[L::BX + 2 * EP + le];
-      float rz = Sq[L::BH + le], rr = Sq[L::BH + EP + le], rh = Sq[L::BH + 2 * EP + le];
-#pragma unroll
-      for (int k = 0; k < EP; ++k) {
-        const float xk = __shfl_sync(0xffffffffu, x, k);
-        const float hk = __shfl_sync(0xffffffffu, h, k);
-        xz = fmaf(xk, gw[k * 3 * EP], xz);
-        xr = fmaf(xk, gw[k * 3 * EP + EP], xr);
-        xh = fmaf(xk, gw[k * 3 * EP + 2 * EP], xh);
-        rz = fmaf(hk, gu[k * 3 * EP], rz);
-        rr = fmaf(hk, gu[k * 3 * EP + EP], rr);
-        rh = fmaf(hk, gu[k * 3 * EP + 2 * EP], rh);
-      }
-      {
-        const float z = sigmoidf_acc(xz + rz);
-        const float rg = sigmoidf_acc(xr + rr);
-        const float hh = tanhf(xh + rg * rh);
-        const float hn = z * h + (1.f - z) * hh;
-        if (valid) h = hn;                                 // masked step: state and output carried
-      }
+      float gz, gr, ghh, grh;
+      const float hn = dien_gru_step<EP>(Sq, le, x, h, &gz, &gr, &ghh, &grh);
+      if (valid) h = hn;                                   // masked step: state and output carried
       if constexpr (AUX) {
-        if (t > 0) aux_row += dien_aux_step<EP>(Sa, g_prev, x, xn, lane);
+        float sp, sn, pos, neg;
+        if (t > 0) aux_row += dien_aux_step<EP>(Sa, g_prev, x, xn, lane, &sp, &sn, &pos, &neg);
       }
-      // -- attention score of position t
-      const float pc = h * c;
-      float a = att_b;
-#pragma unroll
-      for (int k = 0; k < EP; ++k) a = fmaf(__shfl_sync(0xffffffffu, pc, k), aw[k * 32], a);
-      a = sigmoidf_acc(a);
-      const float s = sigmoidf_acc(warp_sum(a * att_wo) + att_bo);
-      // -- AUGRU step: x = g_t (= h), state u
-      float pr = Sq[L::BI + le], pz = Sq[L::BI + EP + le], ph = Sq[L::BI + 2 * EP + le];
-#pragma unroll
-      for (int k = 0; k < EP; ++k) {
-        const float hk = __shfl_sync(0xffffffffu, h, k);
-        const float uk = __shfl_sync(0xffffffffu, u, k);
-        pr = fmaf(hk, iw[k * EP], pr);
-        pz = fmaf(hk, iw[EP * EP + k * EP], pz);
-        ph = fmaf(hk, iw[2 * EP * EP + k * EP], ph);
-        pr = fmaf(uk, hw[k * EP], pr);
-        pz = fmaf(uk, hw[EP * EP + k * EP], pz);
-      }
-      float ar = Sq[L::BA + le], az = Sq[L::BA + EP + le];
-#pragma unroll
-      for (int k = 0; k < EP; ++k) {
-        ar = fmaf(__shfl_sync(0xffffffffu, pr, k), sw[k * EP], ar);
-        az = fmaf(__shfl_sync(0xffffffffu, pz, k), sw[EP * EP + k * EP], az);
-      }
-      const float rg = sigmoidf_acc(ar), zg = sigmoidf_acc(az);
-      const float uz = u * zg;
-#pragma unroll
-      for (int k = 0; k < EP; ++k)
-        ph = fmaf(__shfl_sync(0xffffffffu, uz, k), hw[2 * EP * EP + k * EP], ph);
-      float ah = Sq[L::BA + 2 * EP + le];
-#pragma unroll
-      for (int k = 0; k < EP; ++k)
-        ah = fmaf(__shfl_sync(0xffffffffu, ph, k), sw[2 * EP * EP + k * EP], ah);
-      const float hn = tanhf(ah);
-      const float ra = s * rg;
-      u = (1.f - ra) * u + ra * hn;
+      float a;
+      const float s = dien_attention<EP>(Sq, lane, h * c, att_b, att_wo, att_bo, &a);
+      DienAugruStep st;
+      u = dien_augru_step<EP>(Sq, le, h, u, s, &st);
     }
     if (lane < EP) { xrow[OFF_C + lane] = c; xrow[OFF_ST + lane] = u; }
     if constexpr (AUX) {
@@ -247,24 +138,6 @@ static size_t dien_smem() {
   return (size_t)(kDienRows * ((5 * EP + kNumPad + 4) + 132 + 68) + DienBlob<EP>::TOTAL +
                   (AUX ? DienAuxBlob<EP>::TOTAL : 0)) *
          sizeof(float);
-}
-
-int dien_seq_floats(int EP) {
-  switch (EP) {
-    case 12: return DienBlob<12>::TOTAL;
-    case 16: return DienBlob<16>::TOTAL;
-    case 32: return DienBlob<32>::TOTAL;
-  }
-  return -1;
-}
-
-int dien_aux_floats(int EP) {
-  switch (EP) {
-    case 12: return DienAuxBlob<12>::TOTAL;
-    case 16: return DienAuxBlob<16>::TOTAL;
-    case 32: return DienAuxBlob<32>::TOTAL;
-  }
-  return -1;
 }
 
 template <int EP, bool AUX = false>

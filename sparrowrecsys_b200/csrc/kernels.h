@@ -303,7 +303,7 @@ struct DienParams {
   const float* user;       // [n_users][EP]
   const float* ugenre;     // [19][EP]
   const float* mgenre;     // [19][EP]
-  const float* seq;        // GRU + attention + AUGRU weights, layout dien.cu::DienBlob<EP>
+  const float* seq;        // GRU + attention + AUGRU weights, the sequence part of a DienLayout blob
   // top MLP, first kernel permuted to the tile order
   //   [userGenre1 | userId | augru state | candidate | movieGenre1] x EP, then 7 numerics + pad
   const float* W1;         // [KP = 5*EP + 8][128]
@@ -319,14 +319,98 @@ struct DienParams {
   int EP;
 };
 
+// The Dense weights of DIEN (a model's and a trainer's) as one blob, offsets in floats.  The sequence part
+// (DienParams::seq): gru/kernel and gru_recurrent/kernel [EP k][3][EP] (gates z | r | h), att_dense/kernel [EP][32],
+// the AUGRU's In, Hid and Act kernels [3 g][EP][EP] (gates r | z | h), the biases of the GRU's input and recurrent
+// side, of In and of Act [3][EP] each, augru_h0 [EP], att_dense/bias, att_out/kernel [32] and att_out/bias (+3 pad).
+// Then the auxiliary head (DienAuxView::w): aux_pos_dense/kernel and aux_neg_dense/kernel [2EP][32] (g_t rows, then
+// the item rows), their biases [32], aux_pos_out/kernel and aux_neg_out/kernel [32], the two output biases (+2
+// pad).  Then the top MLP: W1 [5EP + 8][128] in the tile order of dien.cu, b1 and a1 (prelu/alpha) [128], W2
+// [128][64], b2, a2 and w3 [64], b3 (+3 pad).  Widths past E, hidden widths and padding rows are zero; every array
+// starts at a multiple of 4 floats, the top MLP's at a multiple of 64.  dien_layers.cuh::DienBlob / DienAuxBlob name the same offsets at compile time.
+struct DienLayout {
+  int GW, GU, AW, IW, HW, SW, BX, BH, BI, BA, H0, AB, AO, ABO, seq;   // the sequence part; seq = its floats
+  int aux;                                                             // the auxiliary head's first float, and
+  int PW, NW, PB, NB, PO, NO, POB, NOB, aux_floats;                    //   its offsets relative to it
+  int W1, b1, a1, W2, b2, a2, w3, b3, floats;
+  __host__ __device__ static constexpr DienLayout of(int EP) {
+    DienLayout l{};
+    const int EE = EP * EP;
+    l.GW = 0;
+    l.GU = l.GW + 3 * EE;
+    l.AW = l.GU + 3 * EE;
+    l.IW = l.AW + 32 * EP;
+    l.HW = l.IW + 3 * EE;
+    l.SW = l.HW + 3 * EE;
+    l.BX = l.SW + 3 * EE;
+    l.BH = l.BX + 3 * EP;
+    l.BI = l.BH + 3 * EP;
+    l.BA = l.BI + 3 * EP;
+    l.H0 = l.BA + 3 * EP;
+    l.AB = l.H0 + EP;
+    l.AO = l.AB + 32;
+    l.ABO = l.AO + 32;
+    l.seq = l.ABO + 4;
+    l.aux = l.seq;
+    l.PW = 0;
+    l.NW = l.PW + 64 * EP;
+    l.PB = l.NW + 64 * EP;
+    l.NB = l.PB + 32;
+    l.PO = l.NB + 32;
+    l.NO = l.PO + 32;
+    l.POB = l.NO + 32;
+    l.NOB = l.POB + 1;
+    l.aux_floats = l.POB + 4;
+    l.W1 = (l.aux + l.aux_floats + 63) / 64 * 64;    // the top MLP's rows on 256-byte lines, as dense_layer reads them
+    l.b1 = l.W1 + (5 * EP + kNumPad) * 128;
+    l.a1 = l.b1 + 128;
+    l.W2 = l.a1 + 128;
+    l.b2 = l.W2 + 128 * 64;
+    l.a2 = l.b2 + 64;
+    l.w3 = l.a2 + 64;
+    l.b3 = l.w3 + 64;
+    l.floats = l.b3 + 4;
+    return l;
+  }
+};
+
+// ---- DIEN's training step (dien_train.cu; DESIGN.md section 4.20) ------------------------------------------------
+constexpr int kDienMaxT = 64;        // the longest history the step kernel trains (hist_len 1..64)
+constexpr int kDienTables = 4;       // embedding, userId_embedding, userGenre1_embedding, movieGenre1_embedding
+struct DienStepArgs {
+  DienParams p;            // the trainer's tables and Dense weights (DienLayout blob; p.b3 unused: read from blob)
+  const float* blob;       // the Dense-weight blob (b3 at DienLayout::b3, the auxiliary head at DienLayout::aux)
+  const int32_t* order;    // [B] the step's rows of the dataset
+  const int32_t* movie;    // the dataset [n]: movieId, userId, userGenre1 / movieGenre1 (column 0 of [n][5] / [n][3]
+  const int32_t* user;     //   after check), numerics [n][7], history [n][T], negatives [n][T - 1], labels [n]
+  const int32_t* ugenre;
+  const int32_t* mgenre;
+  const float* numerics;
+  const int32_t* hist;
+  const int32_t* neg;
+  const int32_t* label;
+  int B;
+  int64_t tab_row0[kDienTables];   // first row of each table in the trainer's table array
+  float* probs;            // [B] outputs of the step, before its update
+  float* logits;
+  float* aux;              // [B] each row's sum of pos_t + neg_t
+  int32_t* labels;         // [B] the step's labels in step order
+  int32_t* trow;           // [(2T + 3) B] table row of entry s * B + r, -1 = none (a missing genre)
+  float* gemb;             // [(2T + 3) B][EP] the entries' gradients
+  float* rec;              // [B][T][kDienRecSlots][32] per (row, position) inputs and deltas of the Dense products
+  float* part;             // [ctas][DienLayout::floats] per-CTA Dense gradient sums
+};
+int dien_train_ctas(int B);
+size_t dien_train_rec_floats(int B, int T);   // the floats of DienStepArgs::rec
+cudaError_t launch_dien_train_step(const DienStepArgs& a, cudaStream_t s);
+
 // ---- DIEN's auxiliary head (DIEN.py:261-292), the AUX variant of dien_kernel --------------------------
 struct DienAuxView {
-  const float* w;          // aux_pos_* / aux_neg_* weights, layout dien.cu::DienAuxBlob<EP>
+  const float* w;          // aux_pos_* / aux_neg_* weights, the auxiliary part of a DienLayout blob
   const int32_t* neg;      // [B][neg_stride] negtive_userRatedMovie2..T in graph order
   int neg_stride;
   float* aux;              // [B] out: sum over t of pos_t + neg_t
 };
-int dien_aux_floats(int EP);     // size of DienAuxView::w for a padded width, -1 if unsupported
 // the AUX variant of dien_kernel: probs / logits with the bits of launch_dien, plus aux[B]
 cudaError_t launch_dien_aux(const DienParams& p, const DienAuxView& a, const BatchView& b, cudaStream_t s);
 // final_loss[i] = bce(logits[i], labels[i]) - 0.5 * mean(aux[0..n)) in float32 (DIEN.py:287), the mean summed
@@ -346,7 +430,6 @@ cudaError_t launch_deepfm_tc(const DeepFmTcParams& p, const BatchView& b, cudaSt
 cudaError_t launch_deepfm2(const DeepFm2Params& p, const BatchView& b, cudaStream_t s);
 cudaError_t launch_din(const DinParams& p, const BatchView& b, cudaStream_t s);
 cudaError_t launch_dien(const DienParams& p, const BatchView& b, cudaStream_t s);
-int dien_seq_floats(int EP);     // size of DienParams::seq for a padded width, -1 if unsupported
 cudaError_t setup_dien_attributes();
 cudaError_t launch_fill_uniform(float* x, int64_t n, uint64_t seed, float lo, float hi,
                                 cudaStream_t s);

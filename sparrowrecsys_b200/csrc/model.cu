@@ -457,144 +457,34 @@ int build_din(Builder& B) {
   return B.status;
 }
 
-// ---- DIEN's auxiliary head (DIEN.py:261-292): an optional group of eight tensors, all or none; the blob
-// in the layout of dien.cu::DienAuxBlob<EP> ---------------------------------------------------------------
+// ---- DIEN (DIEN.py:154-292): one blob in the layout of kernels.h::DienLayout (placement.h::place_dien); the
+// auxiliary head's group of eight tensors is optional, all or none ----------------------------------------------
 const char* const kDienAuxNames[8] = {"aux_pos_dense/kernel", "aux_pos_dense/bias", "aux_pos_out/kernel",
                                       "aux_pos_out/bias",     "aux_neg_dense/kernel", "aux_neg_dense/bias",
                                       "aux_neg_out/kernel",   "aux_neg_out/bias"};
 
-int build_dien_aux(Builder& B) {
-  srs_model* m = B.m;
-  const int E = m->spec.emb_dim, EP = m->EP;
-  int present = 0;
-  for (const char* n : kDienAuxNames) present += B.by_name.count(n) ? 1 : 0;
-  if (present == 0) return SRS_OK;
-  const float* w[2][4];
-  for (int side = 0; side < 2; ++side) {
-    w[side][0] = B.host(kDienAuxNames[4 * side + 0], 2 * E, 32);
-    w[side][1] = B.host(kDienAuxNames[4 * side + 1], 32, 1);
-    w[side][2] = B.host(kDienAuxNames[4 * side + 2], 32, 1);
-    w[side][3] = B.host(kDienAuxNames[4 * side + 3], 1, 1);
-  }
-  if (B.status != SRS_OK) return B.status;
-  const int total = dien_aux_floats(EP);
-  if (total < 0) return fail(SRS_ERR_INVALID, "DIEN: unsupported padded width %d", EP);
-  std::vector<float> q((size_t)total, 0.f);
-  const int PW = 0, NW = 64 * EP, PB = 128 * EP, NB = PB + 32, PO = NB + 32, NO = PO + 32, POB = NO + 32;
-  for (int side = 0; side < 2; ++side) {
-    const int W = side ? NW : PW, Bs = side ? NB : PB, O = side ? NO : PO;
-    for (int k = 0; k < E; ++k)                  // concat order: hidden state rows, then embedding rows
-      for (int j = 0; j < 32; ++j) {
-        q[W + (size_t)k * 32 + j] = w[side][0][(size_t)k * 32 + j];
-        q[W + (size_t)(EP + k) * 32 + j] = w[side][0][(size_t)(E + k) * 32 + j];
-      }
-    for (int j = 0; j < 32; ++j) { q[Bs + j] = w[side][1][j]; q[O + j] = w[side][2][j]; }
-    q[POB + side] = w[side][3][0];
-  }
-  m->dien_aux.w = B.upload(q);
-  return B.status;
-}
-
-// ---- DIEN (DIEN.py:154-256): sequence-part blob in the layout of dien.cu::DienBlob<EP> ---------
 int build_dien(Builder& B) {
   srs_model* m = B.m;
   const srs_spec& s = m->spec;
-  const int E = s.emb_dim, EP = m->EP, T = s.hist_len, A = 32;
+  const int E = s.emb_dim, EP = m->EP, T = s.hist_len;
   if (E > 32) return fail(SRS_ERR_INVALID, "DIEN supports emb_dim <= 32");
-  if (s.au_hidden != A) return fail(SRS_ERR_INVALID, "DIEN attention width must be 32");
+  if (s.au_hidden != 32) return fail(SRS_ERR_INVALID, "DIEN attention width must be 32");
   if (s.n_hidden != 2 || s.hidden[0] > 128 || s.hidden[1] > 64 || s.hidden[0] < 1 || s.hidden[1] < 1)
     return fail(SRS_ERR_INVALID, "DIEN needs hidden widths <= (128, 64)");
   if (T < 1) return fail(SRS_ERR_INVALID, "hist_len must be >= 1");
-  const int h0 = s.hidden[0], h1 = s.hidden[1];
+  bool aux = false;
+  for (const char* n : kDienAuxNames) aux = aux || B.by_name.count(n);
   DienParams& p = m->dien;
-  p.movie = B.table("embedding", s.n_movies, E);
-  p.user = B.table("userId_embedding", s.n_users, E);
-  p.ugenre = B.table("userGenre1_embedding", s.n_genres, E);
-  p.mgenre = B.table("movieGenre1_embedding", s.n_genres, E);
-  const float* gk = B.host("gru/kernel", E, 3 * E);
-  const float* gr = B.host("gru_recurrent/kernel", E, 3 * E);
-  const float* gb = B.host("gru/bias", 2, 3 * E);
-  const float* ak = B.host("att_dense/kernel", E, A);
-  const float* ab = B.host("att_dense/bias", A, 1);
-  const float* ao = B.host("att_out/kernel", A, 1);
-  const float* aob = B.host("att_out/bias", 1, 1);
-  const char* gates[3] = {"r", "z", "h"};
-  const float *wi[3], *bi[3], *wh[3], *wa[3], *ba[3];
-  for (int g = 0; g < 3; ++g) {
-    char name[64];
-    snprintf(name, sizeof name, "augru_%s_input/kernel", gates[g]); wi[g] = B.host(name, E, E);
-    snprintf(name, sizeof name, "augru_%s_input/bias", gates[g]); bi[g] = B.host(name, E, 1);
-    snprintf(name, sizeof name, "augru_%s_hidden/kernel", gates[g]); wh[g] = B.host(name, E, E);
-    snprintf(name, sizeof name, "augru_%s_act/kernel", gates[g]); wa[g] = B.host(name, E, E);
-    snprintf(name, sizeof name, "augru_%s_act/bias", gates[g]); ba[g] = B.host(name, E, 1);
-  }
-  const float* u0 = B.host("augru_h0", 1, E);
-  const float* k1 = B.host("dense/kernel", 5 * E + 7, h0);
-  const float* b1 = B.host("dense/bias", h0, 1);
-  const float* a1 = B.host("prelu/alpha", h0, 1);
-  const float* k2 = B.host("dense_1/kernel", h0, h1);
-  const float* b2 = B.host("dense_1/bias", h1, 1);
-  const float* a2 = B.host("prelu_1/alpha", h1, 1);
-  const float* k3 = B.host("dense_2/kernel", h1, 1);
-  const float* b3 = B.host("dense_2/bias", 1, 1);
+  const Placement pl = place_dien(s, EP, aux, &p);
+  std::vector<float> blob(DienLayout::of(EP).floats, 0.f);
+  const float* tables[kDienTables];
+  place_host(B, pl, tables, blob.data(), nullptr);
   if (B.status != SRS_OK) return B.status;
-  const int total = dien_seq_floats(EP);
-  if (total < 0) return fail(SRS_ERR_INVALID, "DIEN: unsupported padded width %d", EP);
-  std::vector<float> q((size_t)total, 0.f);
-  const int EE = EP * EP;
-  const int GW = 0, GU = 3 * EE, AW = 6 * EE, IW = AW + 32 * EP, HW = IW + 3 * EE, SW = HW + 3 * EE,
-            BX = SW + 3 * EE, BH = BX + 3 * EP, BI = BH + 3 * EP, BA = BI + 3 * EP, H0 = BA + 3 * EP,
-            AB = H0 + EP, AO = AB + 32, ABO = AO + 32;
-  for (int k = 0; k < E; ++k)
-    for (int g = 0; g < 3; ++g)                 // Keras gate blocks z | r | h along the 3E axis
-      for (int e = 0; e < E; ++e) {
-        q[GW + (size_t)k * 3 * EP + g * EP + e] = gk[(size_t)k * 3 * E + g * E + e];
-        q[GU + (size_t)k * 3 * EP + g * EP + e] = gr[(size_t)k * 3 * E + g * E + e];
-      }
-  for (int g = 0; g < 3; ++g)
-    for (int e = 0; e < E; ++e) {
-      q[BX + g * EP + e] = gb[g * E + e];
-      q[BH + g * EP + e] = gb[3 * E + g * E + e];
-      q[BI + g * EP + e] = bi[g][e];
-      q[BA + g * EP + e] = ba[g][e];
-    }
-  for (int k = 0; k < E; ++k)
-    for (int j = 0; j < A; ++j) q[AW + (size_t)k * 32 + j] = ak[(size_t)k * A + j];
-  for (int g = 0; g < 3; ++g)
-    for (int k = 0; k < E; ++k)
-      for (int e = 0; e < E; ++e) {
-        q[IW + (size_t)g * EE + k * EP + e] = wi[g][(size_t)k * E + e];
-        q[HW + (size_t)g * EE + k * EP + e] = wh[g][(size_t)k * E + e];
-        q[SW + (size_t)g * EE + k * EP + e] = wa[g][(size_t)k * E + e];
-      }
-  for (int e = 0; e < E; ++e) q[H0 + e] = u0[e];
-  for (int j = 0; j < A; ++j) { q[AB + j] = ab[j]; q[AO + j] = ao[j]; }
-  q[ABO] = aob[0];
-  p.seq = B.upload(q);
-  // top kernel rows: [augru | candidate | user_profile | context] (DIEN.py:250); the blocks
-  // are DenseFeatures layers, sorted by column name inside (as in DIN)
-  const int up = 2 * E, ctx = 4 * E + 3;
-  std::vector<int> map;
-  append(map, iota_map(up + 1, E, EP));          // userGenre1 emb
-  append(map, iota_map(up + 1 + E, E, EP));      // userId emb
-  append(map, iota_map(0, E, EP));               // AUGRU final state
-  append(map, iota_map(E, E, EP));               // candidate emb
-  append(map, iota_map(ctx + 1, E, EP));         // movieGenre1 emb
-  const int nums[8] = {ctx, ctx + 1 + E, ctx + 2 + E, ctx + 3 + E, up, up + 1 + 2 * E, up + 2 + 2 * E, -1};
-  for (int j = 0; j < 8; ++j) map.push_back(nums[j]);
-  p.W1 = B.upload(B.permute(k1, h0, map, 128));
-  p.b1 = B.upload(B.padvec(b1, h0, 128));
-  p.a1 = B.upload(B.padvec(a1, h0, 128));
-  p.W2 = B.upload(B.permute(k2, h1, iota_map(0, h0, 128), 64));
-  p.b2 = B.upload(B.padvec(b2, h1, 64));
-  p.a2 = B.upload(B.padvec(a2, h1, 64));
-  p.w3 = B.upload(B.padvec(k3, h1, 64));
-  p.b3 = b3[0];
-  p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres;
-  p.T = T; p.EP = EP;
+  const float* d = B.upload(blob);
+  point_into_blob(&p, tables, d, blob.data());
+  m->dien_aux.w = aux && d ? d + DienLayout::of(EP).aux : nullptr;
   m->kernel_name = "dien_kernel";
-  if (B.status != SRS_OK) return B.status;
-  return build_dien_aux(B);
+  return B.status;
 }
 
 // ---- tensor-core DIN: shared-memory image ------------------------------------------------

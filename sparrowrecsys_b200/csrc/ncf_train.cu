@@ -1,8 +1,9 @@
 // ncf_train.cu - `model.fit` on the device: the C ABI's srs_trainer (include/srs_ctr.h), which trains NeuralCF
 // (neural_cf_model_1, NeuralCF.py:74-91; DESIGN.md section 4.8), DeepFM (DeepFM.py; section 4.9, its step kernel
 // in deepfm_train.cu), Wide&Deep (WideNDeep.py; section 4.18, its step kernel in widendeep_train.cu) and DeepFM_v2
-// (DeepFM_v2.py; section 4.19, its step kernel in deepfm2_train.cu), and the kernels the models share: dedupe, the
-// two forms of Adam, metrics.
+// (DeepFM_v2.py; section 4.19, its step kernel in deepfm2_train.cu) and DIEN (DIEN.py; section 4.20, its step kernel
+// in dien_train.cu, its fit in srs_trainer_fit_dien_host), and the kernels the models share: dedupe, the two forms of
+// Adam, metrics.
 //
 // NeuralCF's step of batch B_b (rows order[off .. off + B_b) of the uploaded dataset), five launches, no host sync:
 //   ncf_train_step_kernel  forward (the arithmetic of ncf_kernel) and backward, one thread per row; the Dense
@@ -26,6 +27,10 @@
 // four tables' entries and (width 1) over its one-hot entries, table_adam_kernel<false> over the four tables and
 // <true> over first_cat/kernel's one-hot rows, dense_adam_kernel, metrics_update_kernel; plus deepfm_permute_kernel
 // (it reads DeepFM's columns) once per epoch.
+// DIEN's step is six launches and no permute (the step kernel reads its rows through the order): dien_train_step_kernel,
+// table_grad_kernel over its (2T + 3) B entries, table_adam_kernel<false> over its four tables, dense_adam_kernel,
+// dien_final_loss_kernel (the batch's final_loss sum) and metrics_update_kernel (with the batch's own histogram);
+// plus launch_auc_value once per epoch.
 // No float atomics: every sum has a fixed order, so a fit is bitwise reproducible.
 //
 // Validation (srs_trainer_fit_validate_host) and srs_trainer_evaluate_host run the serving forward over the
@@ -300,6 +305,7 @@ struct srs_trainer {
   DeepFmParams fm{};                  //   (DeepFM)
   EmbMlpParams emb{};                 //   (Wide&Deep)
   DeepFm2Params fm2{};                //   (DeepFM_v2)
+  DienParams dien{};                  //   (DIEN: the step kernel's view; DIEN has no serving forward here)
   int64_t tab_floats = 0;             // (sum of the tables' rows) * EP
   float* tab[4] = {};                 // w, m, v, G   [rows][EP], padding zero
   float* blob[3] = {};                // w, m, v      [blob_floats]
@@ -439,11 +445,19 @@ cudaError_t eval_rows(const srs_trainer* t, const DeepFmRows& r, int n, float* p
   return launch_metrics_update(probs, logits, r.label, n, &em->cnt, &em->red, &em->loss, 1, s);
 }
 
+// A DIEN trainer at an entry point of the other models: its fit takes negatives and reports DIEN's own metrics
+int dien_rejected(const char* what) {
+  return failf(SRS_ERR_INVALID, "a DIEN trainer's %s is srs_trainer_fit_dien_host: DIEN trains on negatives and "
+               "reports its own loss, auc and auc_value (a trained model's evaluate is srs_dien_evaluate_host_batches)",
+               what);
+}
+
 // The trainer of any trainable kind (the entry points below check the kind against their own lists first)
 int trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
                    const srs_adam* hp, srs_trainer** out) {
   const srs_spec& s = *spec;
-  const bool fm = s.kind == SRS_DEEPFM, wd = s.kind == SRS_WIDENDEEP, fm2 = s.kind == SRS_DEEPFM_V2;
+  const bool fm = s.kind == SRS_DEEPFM, wd = s.kind == SRS_WIDENDEEP, fm2 = s.kind == SRS_DEEPFM_V2,
+             dien = s.kind == SRS_DIEN;
   if (s.emb_dim < 1 || s.emb_dim > 64) return failf(SRS_ERR_INVALID, "emb_dim must be in 1..64");
   if (s.n_movies < 1 || s.n_users < 1) return failf(SRS_ERR_INVALID, "empty vocabulary");
   int hmax = 0;
@@ -465,6 +479,15 @@ int trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_te
     if (s.n_genres < 1) return failf(SRS_ERR_INVALID, "empty genre vocabulary");
     if (s.hidden[0] < 1 || s.hidden[0] > 32 || s.hidden[1] < 1 || s.hidden[1] > 16)
       return failf(SRS_ERR_INVALID, "DeepFM_v2's hidden widths must be in 1..32 and 1..16");
+  } else if (dien) {
+    if (s.emb_dim > 32) return failf(SRS_ERR_INVALID, "DIEN's fit needs emb_dim in 1..32");
+    if (s.hist_len < 1 || s.hist_len > kDienMaxT)
+      return failf(SRS_ERR_INVALID, "DIEN's fit needs hist_len in 1..%d", kDienMaxT);
+    if (s.au_hidden != 32) return failf(SRS_ERR_INVALID, "DIEN's fit needs au_hidden 32");
+    if (s.n_hidden != 2) return failf(SRS_ERR_INVALID, "DIEN's fit needs exactly 2 hidden layers");
+    if (s.n_genres < 1) return failf(SRS_ERR_INVALID, "empty genre vocabulary");
+    if (s.hidden[0] < 1 || s.hidden[0] > 128 || s.hidden[1] < 1 || s.hidden[1] > 64)
+      return failf(SRS_ERR_INVALID, "DIEN's hidden widths must be in 1..128 and 1..64");
   } else {
     if (s.n_hidden < 1 || s.n_hidden > 3) return failf(SRS_ERR_INVALID, "1..3 hidden layers supported");
     for (int i = 0; i < s.n_hidden; ++i) {
@@ -500,6 +523,9 @@ int trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_te
     t->place = place_deepfm2(s, EP, &t->fm2);
     t->blob_floats = DeepFm2Blob::of(EP).floats;
     t->onehot = (int64_t)2 * s.n_genres + s.n_movies + s.n_users;
+  } else if (dien) {
+    t->place = place_dien(s, EP, true, &t->dien);   // the auxiliary head is part of the objective
+    t->blob_floats = DienLayout::of(EP).floats;
   } else {
     t->HP = hmax <= 16 ? 16 : 32;
     t->place = place_ncf(s, EP, t->HP, &t->ncf);
@@ -563,6 +589,10 @@ int trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_te
     for (int k = 0; k < kDeepFm2Tables; ++k) tables[k] = table(k);
     point_into_blob(&t->fm2, tables, t->blob[0]);
     t->fm2.first = t->fo[0];
+  } else if (dien) {
+    const float* tables[kDienTables];
+    for (int k = 0; k < kDienTables; ++k) tables[k] = table(k);
+    point_into_blob(&t->dien, tables, t->blob[0], blob.data());   // the step kernel reads b3 from the blob
   } else {
     t->ncf.movie = table(0);
     t->ncf.user = table(1);
@@ -604,9 +634,9 @@ int srs_trainer_create_any(const srs_spec* spec, const srs_tensor* tensors, int3
   if (!spec || !out) return failf(SRS_ERR_INVALID, "null argument");
   *out = nullptr;
   const int k = spec->kind;
-  if (k != SRS_NEURALCF && k != SRS_DEEPFM && k != SRS_WIDENDEEP && k != SRS_DEEPFM_V2)
-    return failf(SRS_ERR_INVALID, "fit is implemented for NeuralCF (neural_cf_model_1), DeepFM, Wide&Deep and "
-                 "DeepFM_v2 only");
+  if (k != SRS_NEURALCF && k != SRS_DEEPFM && k != SRS_WIDENDEEP && k != SRS_DEEPFM_V2 && k != SRS_DIEN)
+    return failf(SRS_ERR_INVALID, "fit is implemented for NeuralCF (neural_cf_model_1), DeepFM, Wide&Deep, "
+                 "DeepFM_v2 and DIEN only");
   return trainer_create(spec, tensors, n_tensors, device, hp, out);
 }
 
@@ -625,6 +655,7 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
                                   const srs_batch* val_batch, const int32_t* val_labels, int32_t val_freq,
                                   srs_eval_result* val_history) {
   if (!t || !batch || !labels || !order) return failf(SRS_ERR_INVALID, "null argument");
+  if (t->spec.kind == SRS_DIEN) return dien_rejected("fit");
   const bool fm = t->spec.kind == SRS_DEEPFM, wd = t->spec.kind == SRS_WIDENDEEP, fm2 = t->spec.kind == SRS_DEEPFM_V2;
   const int n = batch->B;
   if (n < 1) return failf(SRS_ERR_INVALID, "fit needs at least one row");
@@ -800,6 +831,7 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
 
 int srs_trainer_evaluate_host(srs_trainer* t, const srs_batch* batch, const int32_t* labels, srs_eval_result* out) {
   if (!t || !batch || !labels || !out) return failf(SRS_ERR_INVALID, "null argument");
+  if (t->spec.kind == SRS_DIEN) return dien_rejected("evaluate");
   const int n = batch->B;
   if (n < 1) return failf(SRS_ERR_INVALID, "evaluate needs at least one row");
   const int rc = check_rows(t, batch, labels, "");
@@ -824,6 +856,166 @@ int srs_trainer_evaluate_host(srs_trainer* t, const srs_batch* batch, const int3
   CUDA_TRY(cudaStreamSynchronize(s));
   if (met.cnt.err) return failf(SRS_ERR_INVALID, "evaluate produced a probability that is NaN or outside [0, 1]");
   metrics_summarise(met.cnt.hist, met.cnt.correct, met.loss, out, nullptr);
+  return SRS_OK;
+}
+
+int srs_trainer_fit_dien_host(srs_trainer* t, const srs_batch* batch, const int32_t* neg_hist, int32_t neg_stride,
+                              const int32_t* labels, const int32_t* order, int32_t batch_size, int32_t epochs,
+                              srs_dien_eval_result* history) {
+  if (!t || !batch || !labels || !order) return failf(SRS_ERR_INVALID, "null argument");
+  if (t->spec.kind != SRS_DIEN)
+    return failf(SRS_ERR_INVALID, "srs_trainer_fit_dien_host trains DIEN; this trainer's fit is srs_trainer_fit_host");
+  const srs_spec& sp = t->spec;
+  const int n = batch->B, T = sp.hist_len;
+  if (n < 1) return failf(SRS_ERR_INVALID, "fit needs at least one row");
+  if (batch_size < 1) return failf(SRS_ERR_INVALID, "batch_size must be at least 1");
+  if (epochs < 1) return failf(SRS_ERR_INVALID, "epochs must be at least 1");
+  // every check before the first launch: a rejected call leaves the trainer as it was
+  if (!batch->movie_id || !batch->user_id || !batch->movie_genre || !batch->user_genre || !batch->numerics ||
+      !batch->hist || batch->hist_stride < T)
+    return failf(SRS_ERR_INVALID, "DIEN needs movie_id, user_id, movie_genre, user_genre, numerics and hist "
+                 "[B][hist_stride >= %d]", T);
+  if (T > 1 && (!neg_hist || neg_stride < T - 1))
+    return failf(SRS_ERR_INVALID, "neg_hist [B][neg_stride >= %d] is required", T - 1);
+  // a numeric column's float32, as the kernels read it; |float(raw)| <= 2^31, which int64 holds (int may not)
+  auto as_id = [](int32_t raw) { return (int64_t)(float)raw; };
+  for (int i = 0; i < n; ++i) {
+    if (labels[i] != 0 && labels[i] != 1)
+      return failf(SRS_ERR_INVALID, "label of row %d is %d, not 0 or 1", i, labels[i]);
+    const int64_t m = as_id(batch->movie_id[i]);
+    if (m < 0 || m >= sp.n_movies)
+      return failf(SRS_ERR_RANGE, "movieId %d of row %d is outside [0, %d)", batch->movie_id[i], i, sp.n_movies);
+    if ((unsigned)batch->user_id[i] >= (unsigned)sp.n_users)
+      return failf(SRS_ERR_RANGE, "userId %d of row %d is outside [0, %d)", batch->user_id[i], i, sp.n_users);
+    if (batch->movie_genre[(size_t)i * 3] >= sp.n_genres)   // a negative genre is missing
+      return failf(SRS_ERR_RANGE, "movieGenre1 index %d of row %d is outside [0, %d)", batch->movie_genre[(size_t)i * 3],
+                   i, sp.n_genres);
+    if (batch->user_genre[(size_t)i * 5] >= sp.n_genres)
+      return failf(SRS_ERR_RANGE, "userGenre1 index %d of row %d is outside [0, %d)", batch->user_genre[(size_t)i * 5],
+                   i, sp.n_genres);
+    for (int k = 0; k < T; ++k) {
+      const int64_t h = as_id(batch->hist[(size_t)i * batch->hist_stride + k]);
+      if (h < 0 || h >= sp.n_movies)
+        return failf(SRS_ERR_RANGE, "history id %d (position %d) of row %d is outside [0, %d)",
+                     batch->hist[(size_t)i * batch->hist_stride + k], k, i, sp.n_movies);
+    }
+    for (int k = 0; k + 1 < T; ++k) {
+      const int64_t g = as_id(neg_hist[(size_t)i * neg_stride + k]);
+      if (g < 0 || g >= sp.n_movies)
+        return failf(SRS_ERR_RANGE, "negative movie id %d (position %d) of row %d is outside [0, %d)",
+                     neg_hist[(size_t)i * neg_stride + k], k + 2, i, sp.n_movies);
+    }
+  }
+  {
+    std::vector<char> seen(n);
+    for (int e = 0; e < epochs; ++e) {
+      std::fill(seen.begin(), seen.end(), 0);
+      for (int i = 0; i < n; ++i) {
+        const int r = order[(size_t)e * n + i];
+        if (r < 0 || r >= n || seen[r]) return failf(SRS_ERR_INVALID, "order of epoch %d is not a permutation of 0..%d", e, n - 1);
+        seen[r] = 1;
+      }
+    }
+  }
+  CUDA_TRY(cudaSetDevice(t->device));
+  const int EP = t->EP, Bmax = std::min(batch_size, n), K = (n + batch_size - 1) / batch_size;
+  const int n_ent = 2 * T + 3;                          // table entries per row
+  cudaStream_t s = t->stream;
+  Scratch sc;
+  int32_t *d_order, *d_movie, *d_user, *d_ug, *d_mg, *d_hist, *d_neg = nullptr, *d_label, *d_lab_b, *d_trow;
+  float *d_num, *d_probs, *d_logits, *d_aux, *d_final, *d_gemb, *d_rec, *d_part;
+  double *d_bloss, *d_auc, *d_aucsum;
+  unsigned long long* d_bhist;
+  MetricsState* d_met;
+  const size_t N = (size_t)n;
+  CUDA_TRY(sc.alloc(&d_order, (size_t)epochs * N));
+  CUDA_TRY(sc.alloc(&d_movie, N));
+  CUDA_TRY(sc.alloc(&d_user, N));
+  CUDA_TRY(sc.alloc(&d_ug, N));
+  CUDA_TRY(sc.alloc(&d_mg, N));
+  CUDA_TRY(sc.alloc(&d_num, N * kNumNumerics));
+  CUDA_TRY(sc.alloc(&d_hist, N * T));
+  if (T > 1) CUDA_TRY(sc.alloc(&d_neg, N * (T - 1)));
+  CUDA_TRY(sc.alloc(&d_label, N));
+  CUDA_TRY(sc.alloc(&d_lab_b, Bmax));
+  CUDA_TRY(sc.alloc(&d_probs, Bmax));
+  CUDA_TRY(sc.alloc(&d_logits, Bmax));
+  CUDA_TRY(sc.alloc(&d_aux, Bmax));
+  CUDA_TRY(sc.alloc(&d_final, Bmax));
+  CUDA_TRY(sc.alloc(&d_trow, (size_t)n_ent * Bmax));
+  CUDA_TRY(sc.alloc(&d_gemb, (size_t)n_ent * Bmax * EP));
+  CUDA_TRY(sc.alloc(&d_rec, dien_train_rec_floats(Bmax, T)));
+  CUDA_TRY(sc.alloc(&d_part, (size_t)dien_train_ctas(Bmax) * t->blob_floats));
+  CUDA_TRY(sc.alloc(&d_bloss, (size_t)epochs * K));
+  CUDA_TRY(sc.alloc(&d_auc, (size_t)K));
+  CUDA_TRY(sc.alloc(&d_aucsum, (size_t)epochs));
+  CUDA_TRY(sc.alloc(&d_bhist, (size_t)K * 2 * kMetBins));
+  CUDA_TRY(sc.alloc(&d_met, epochs));
+  CUDA_TRY(cudaMemcpyAsync(d_order, order, (size_t)epochs * N * 4, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_movie, batch->movie_id, N * 4, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_user, batch->user_id, N * 4, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpy2DAsync(d_ug, 4, batch->user_genre, 5 * 4, 4, N, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpy2DAsync(d_mg, 4, batch->movie_genre, 3 * 4, 4, N, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_num, batch->numerics, N * kNumNumerics * 4, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpy2DAsync(d_hist, (size_t)T * 4, batch->hist, (size_t)batch->hist_stride * 4, (size_t)T * 4, N,
+                             cudaMemcpyHostToDevice, s));
+  if (T > 1)
+    CUDA_TRY(cudaMemcpy2DAsync(d_neg, (size_t)(T - 1) * 4, neg_hist, (size_t)neg_stride * 4, (size_t)(T - 1) * 4, N,
+                               cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_label, labels, N * 4, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemsetAsync(d_met, 0, sizeof(MetricsState) * epochs, s));
+
+  int dev_sms = 132;
+  cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, t->device);
+  const int adam_blocks = (int)std::min<int64_t>((t->tab_floats + 255) / 256, (int64_t)dev_sms * 8);
+  DienStepArgs a{};
+  a.p = t->dien;
+  a.blob = t->blob[0];
+  a.movie = d_movie; a.user = d_user; a.ugenre = d_ug; a.mgenre = d_mg; a.numerics = d_num;
+  a.hist = d_hist; a.neg = d_neg; a.label = d_label;
+  for (int k = 0; k < kDienTables; ++k) a.tab_row0[k] = t->place[k].table_row;   // the tables come first
+  a.probs = d_probs; a.logits = d_logits; a.aux = d_aux; a.labels = d_lab_b;
+  a.trow = d_trow; a.gemb = d_gemb; a.rec = d_rec; a.part = d_part;
+  for (int e = 0; e < epochs; ++e) {
+    CUDA_TRY(cudaMemsetAsync(d_bhist, 0, (size_t)K * 2 * kMetBins * sizeof(unsigned long long), s));
+    for (int k = 0; k < K; ++k) {
+      const int off = k * batch_size, B = std::min(batch_size, n - off);
+      a.B = B;
+      a.order = d_order + (size_t)e * n + off;
+      CUDA_TRY(launch_dien_train_step(a, s));
+      table_grad_kernel<<<(n_ent * B + 127) / 128, 128, 0, s>>>(d_trow, d_gemb, n_ent * B, EP, t->tab[3]);
+      table_adam_kernel<false><<<adam_blocks, 256, 0, s>>>(t->tab[0], t->tab[1], t->tab[2], t->tab[3],
+                                                           t->tab_floats, t->hp, t->d_it);
+      dense_adam_kernel<<<1, kAdamThreads, 0, s>>>(d_part, dien_train_ctas(B), t->blob_floats, t->blob[0],
+                                                   t->blob[1], t->blob[2], t->hp, t->d_it);
+      g_launch_count += 3;
+      CUDA_TRY(cudaGetLastError());
+      CUDA_TRY(launch_dien_final_loss(d_logits, d_lab_b, d_aux, B, d_final, d_bloss + (size_t)e * K + k, s));
+      CUDA_TRY(launch_metrics_update(d_probs, d_logits, d_lab_b, B, &d_met[e].cnt, &d_met[e].red, nullptr, 0, s,
+                                      d_bhist + (size_t)k * 2 * kMetBins));
+    }
+    CUDA_TRY(launch_auc_value(d_bhist, K, d_auc, d_aucsum + e, s));
+  }
+  std::vector<MetricsState> met(epochs);
+  std::vector<double> bloss((size_t)epochs * K), aucsum(epochs);
+  CUDA_TRY(cudaMemcpyAsync(met.data(), d_met, sizeof(MetricsState) * epochs, cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(bloss.data(), d_bloss, bloss.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaMemcpyAsync(aucsum.data(), d_aucsum, aucsum.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  t->iterations += (int64_t)epochs * K;
+  for (int e = 0; e < epochs; ++e) {
+    if (met[e].cnt.err) return failf(SRS_ERR_INVALID, "epoch %d produced a probability that is NaN or outside [0, 1]", e);
+    if (!history) continue;
+    double loss = 0.0;                                   // the batches' final_loss sums, in batch order
+    for (int k = 0; k < K; ++k) loss += bloss[(size_t)e * K + k];
+    srs_eval_result r{};
+    metrics_summarise(met[e].cnt.hist, met[e].cnt.correct, loss, &r, nullptr);
+    history[e].rows = n;
+    history[e].batches = K;
+    history[e].loss = r.loss;
+    history[e].auc = r.roc_auc;
+    history[e].auc_value = aucsum[e] / (double)K;
+  }
   return SRS_OK;
 }
 

@@ -1,6 +1,6 @@
 // placement.h - where the Keras tensors of the trainable models (NeuralCF's neural_cf_model_1 and two towers, DeepFM,
-// DeepFM_v2 and EmbeddingMLP / Wide&Deep) live on the device, written once for the serving builders (build_ncf,
-// build_deepfm, build_deepfm2, build_embmlp in model.cu) and the
+// DeepFM_v2, EmbeddingMLP / Wide&Deep and DIEN) live on the device, written once for the serving builders (build_ncf,
+// build_deepfm, build_deepfm2, build_embmlp, build_dien in model.cu) and the
 // trainer (srs_trainer_create, srs_trainer_get_weights in ncf_train.cu): the builders and the trainer scatter the
 // caller's host tensors through it, and the trainer gathers its weights back through it.  Also the by-name lookup of
 // the caller's tensors that both use.  Host code only.
@@ -86,6 +86,7 @@ struct Block {
   int at;                        // the block's first float
   int width;                     // floats per block row: the tensor's cols, zero padded
   std::vector<int> map;          // block row i holds tensor row map[i]; -1: a zero row
+  int col0 = 0, ncols = 0;       // the block holds columns col0 .. col0 + ncols of those rows (ncols 0: all)
 };
 
 struct Placed {                  // one Keras tensor [rows][cols]
@@ -324,13 +325,106 @@ inline void point_into_blob(EmbMlpParams* p, const float* const* tables, const f
   p->w3 = blob + ly.w3; p->b3 = blob + ly.b3;
 }
 
+// DIEN: the four tables (embedding, userId_embedding, userGenre1_embedding, movieGenre1_embedding: kDienTables
+// order) and the Dense tensors in one DienLayout::of(EP) blob, looked up in the order the builder has always used;
+// `aux`: with the auxiliary head's group of eight (else its part of the blob stays zero).  The GRU's kernels and
+// biases keep Keras's z | r | h column blocks, each padded to EP.  Fills p's sizes, T and EP.
+inline Placement place_dien(const srs_spec& s, int EP, bool aux, DienParams* p) {
+  const int E = s.emb_dim, h0 = s.hidden[0], h1 = s.hidden[1], A = 32, EE = EP * EP;
+  const DienLayout ly = DienLayout::of(EP);
+  Placement pl;
+  place_table(pl, "embedding", s.n_movies, E);
+  place_table(pl, "userId_embedding", s.n_users, E);
+  place_table(pl, "userGenre1_embedding", s.n_genres, E);
+  place_table(pl, "movieGenre1_embedding", s.n_genres, E);
+  auto gates = [&](int at, int stride, std::vector<int> map) {   // a [.][3E] tensor's z | r | h blocks
+    std::vector<Block> b;
+    for (int g = 0; g < 3; ++g) b.push_back(Block{false, at + g * EP, stride, map, g * E, E});
+    return b;
+  };
+  place_dense(pl, "gru/kernel", E, 3 * E, gates(ly.GW, 3 * EP, iota_map(0, E, E)));
+  place_dense(pl, "gru_recurrent/kernel", E, 3 * E, gates(ly.GU, 3 * EP, iota_map(0, E, E)));
+  std::vector<Block> gb = gates(ly.BX, EP, {0}), gbh = gates(ly.BH, EP, {1});
+  gb.insert(gb.end(), gbh.begin(), gbh.end());
+  place_dense(pl, "gru/bias", 2, 3 * E, gb);
+  place_dense(pl, "att_dense/kernel", E, A, {Block{false, ly.AW, 32, iota_map(0, E, E)}});
+  place_dense(pl, "att_dense/bias", A, 1, {Block{false, ly.AB, 1, iota_map(0, A, A)}});
+  place_dense(pl, "att_out/kernel", A, 1, {Block{false, ly.AO, 1, iota_map(0, A, A)}});
+  place_dense(pl, "att_out/bias", 1, 1, {Block{false, ly.ABO, 1, iota_map(0, 1, 1)}});
+  const char* gate[3] = {"r", "z", "h"};
+  char name[64];
+  for (int g = 0; g < 3; ++g) {
+    snprintf(name, sizeof name, "augru_%s_input/kernel", gate[g]);
+    place_dense(pl, name, E, E, {Block{false, ly.IW + g * EE, EP, iota_map(0, E, E)}});
+    snprintf(name, sizeof name, "augru_%s_input/bias", gate[g]);
+    place_dense(pl, name, E, 1, {Block{false, ly.BI + g * EP, 1, iota_map(0, E, E)}});
+    snprintf(name, sizeof name, "augru_%s_hidden/kernel", gate[g]);
+    place_dense(pl, name, E, E, {Block{false, ly.HW + g * EE, EP, iota_map(0, E, E)}});
+    snprintf(name, sizeof name, "augru_%s_act/kernel", gate[g]);
+    place_dense(pl, name, E, E, {Block{false, ly.SW + g * EE, EP, iota_map(0, E, E)}});
+    snprintf(name, sizeof name, "augru_%s_act/bias", gate[g]);
+    place_dense(pl, name, E, 1, {Block{false, ly.BA + g * EP, 1, iota_map(0, E, E)}});
+  }
+  place_dense(pl, "augru_h0", 1, E, {Block{false, ly.H0, EP, {0}}});
+  // dense/kernel's rows are [augru | candidate | user_profile | context] (DIEN.py:250), the last two DenseFeatures
+  // layers sorted by column name inside; its tile rows are userGenre1 | userId | augru | candidate | movieGenre1,
+  // then the 7 numerics and one zero row
+  const int up = 2 * E, ctx = 4 * E + 3;
+  std::vector<int> map;
+  append(map, iota_map(up + 1, E, EP));
+  append(map, iota_map(up + 1 + E, E, EP));
+  append(map, iota_map(0, E, EP));
+  append(map, iota_map(E, E, EP));
+  append(map, iota_map(ctx + 1, E, EP));
+  for (int r : {ctx, ctx + 1 + E, ctx + 2 + E, ctx + 3 + E, up, up + 1 + 2 * E, up + 2 + 2 * E, -1}) map.push_back(r);
+  place_dense(pl, "dense/kernel", 5 * E + 7, h0, {Block{false, ly.W1, 128, map}});
+  place_dense(pl, "dense/bias", h0, 1, {Block{false, ly.b1, 1, iota_map(0, h0, 128)}});
+  place_dense(pl, "prelu/alpha", h0, 1, {Block{false, ly.a1, 1, iota_map(0, h0, 128)}});
+  place_dense(pl, "dense_1/kernel", h0, h1, {Block{false, ly.W2, 64, iota_map(0, h0, 128)}});
+  place_dense(pl, "dense_1/bias", h1, 1, {Block{false, ly.b2, 1, iota_map(0, h1, 64)}});
+  place_dense(pl, "prelu_1/alpha", h1, 1, {Block{false, ly.a2, 1, iota_map(0, h1, 64)}});
+  place_dense(pl, "dense_2/kernel", h1, 1, {Block{false, ly.w3, 1, iota_map(0, h1, 64)}});
+  place_dense(pl, "dense_2/bias", 1, 1, {Block{false, ly.b3, 1, iota_map(0, 1, 1)}});
+  if (aux) {                                   // [g_t | e] rows: E hidden-state rows, then E item rows
+    std::vector<int> amap = iota_map(0, E, EP);
+    append(amap, iota_map(E, E, EP));
+    for (int side = 0; side < 2; ++side) {
+      const char* sd = side ? "neg" : "pos";
+      snprintf(name, sizeof name, "aux_%s_dense/kernel", sd);
+      place_dense(pl, name, 2 * E, A, {Block{false, ly.aux + (side ? ly.NW : ly.PW), 32, amap}});
+      snprintf(name, sizeof name, "aux_%s_dense/bias", sd);
+      place_dense(pl, name, A, 1, {Block{false, ly.aux + (side ? ly.NB : ly.PB), 1, iota_map(0, A, A)}});
+      snprintf(name, sizeof name, "aux_%s_out/kernel", sd);
+      place_dense(pl, name, A, 1, {Block{false, ly.aux + (side ? ly.NO : ly.PO), 1, iota_map(0, A, A)}});
+      snprintf(name, sizeof name, "aux_%s_out/bias", sd);
+      place_dense(pl, name, 1, 1, {Block{false, ly.aux + (side ? ly.NOB : ly.POB), 1, iota_map(0, 1, 1)}});
+    }
+  }
+  p->n_movies = s.n_movies; p->n_users = s.n_users; p->n_genres = s.n_genres;
+  p->T = s.hist_len; p->EP = EP;
+  return pl;
+}
+
+// p's tables (tables[k]: the k-th table of place_dien's order) and Dense-weight pointers into a DienLayout blob on
+// the device; p->b3 from the host copy of the blob
+inline void point_into_blob(DienParams* p, const float* const* tables, const float* blob, const float* host_blob) {
+  const DienLayout ly = DienLayout::of(p->EP);
+  p->movie = tables[0]; p->user = tables[1]; p->ugenre = tables[2]; p->mgenre = tables[3];
+  p->seq = blob;
+  p->W1 = blob + ly.W1; p->b1 = blob + ly.b1; p->a1 = blob + ly.a1;
+  p->W2 = blob + ly.W2; p->b2 = blob + ly.b2; p->a2 = blob + ly.a2;
+  p->w3 = blob + ly.w3;
+  p->b3 = host_blob[ly.b3];
+}
+
 // a Dense tensor's data [rows][cols] into its blocks; what no block row takes stays as it was (zero)
 inline void scatter(const Placed& x, const float* src, float* blob, float* onehot) {
   for (const Block& k : x.blocks) {
     float* dst = (k.onehot ? onehot : blob) + k.at;
+    const int64_t n = k.ncols ? k.ncols : x.cols;
     for (size_t i = 0; i < k.map.size(); ++i)
       if (k.map[i] >= 0)
-        for (int64_t j = 0; j < x.cols; ++j) dst[i * k.width + j] = src[(size_t)k.map[i] * x.cols + j];
+        for (int64_t j = 0; j < n; ++j) dst[i * k.width + j] = src[(size_t)k.map[i] * x.cols + k.col0 + j];
   }
 }
 
@@ -338,9 +432,10 @@ inline void scatter(const Placed& x, const float* src, float* blob, float* oneho
 inline void gather(const Placed& x, const float* blob, const float* onehot, float* dst) {
   for (const Block& k : x.blocks) {
     const float* src = (k.onehot ? onehot : blob) + k.at;
+    const int64_t n = k.ncols ? k.ncols : x.cols;
     for (size_t i = 0; i < k.map.size(); ++i)
       if (k.map[i] >= 0)
-        for (int64_t j = 0; j < x.cols; ++j) dst[(size_t)k.map[i] * x.cols + j] = src[i * k.width + j];
+        for (int64_t j = 0; j < n; ++j) dst[(size_t)k.map[i] * x.cols + k.col0 + j] = src[i * k.width + j];
   }
 }
 

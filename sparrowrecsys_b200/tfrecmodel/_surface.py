@@ -70,11 +70,12 @@ class Surface:
         """`model.fit(train_dataset, epochs=5)` (NeuralCF.py:91, DeepFM.py, WideNDeep.py:117,
         DeepFM_v2.py:165): train from the weights `model` was loaded with, then rebuild `model` from the trained
         weights.  Returns Keras's history dict, with the `val_*` lists when `validation_data` or
-        `validation_split` is given (`Trainer.fit`).  NeuralCF, DeepFM, Wide&Deep and DeepFM_v2 only."""
-        if self.name not in ("neuralcf", "deepfm", "widendeep", "deepfm_v2"):
+        `validation_split` is given (`Trainer.fit`).  NeuralCF, DeepFM, Wide&Deep, DeepFM_v2 and DIEN only (DIEN: in
+        file order, without validation, its history {"loss", "auc", "auc_value"})."""
+        if self.name not in ("neuralcf", "deepfm", "widendeep", "deepfm_v2", "dien"):
             raise NotImplementedError("tfrecmodel.%s: fit is implemented for NeuralCF (tfrecmodel.neuralcf), "
-                                      "DeepFM (tfrecmodel.deepfm), Wide&Deep (tfrecmodel.widendeep) and DeepFM_v2 "
-                                      "(tfrecmodel.deepfm_v2) only" % self.name)
+                                      "DeepFM (tfrecmodel.deepfm), Wide&Deep (tfrecmodel.widendeep), DeepFM_v2 "
+                                      "(tfrecmodel.deepfm_v2) and DIEN (tfrecmodel.dien) only" % self.name)
         if self.model is None or self.weights is None:
             raise RuntimeError("tfrecmodel.%s: call load() before fit()" % self.name)
         from ..training import Trainer

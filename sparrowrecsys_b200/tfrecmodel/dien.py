@@ -7,8 +7,9 @@ stored weight (`augru_h0`) instead of a fresh random draw per call (:235-236).
     p = dien.predict(features)    # dict of 1-D columns -> float32 [N,1] (y_pred)
     y_pred, final_loss = dien.predict_outputs(features, batch_size=12)   # model.predict, both outputs (:312)
     dien.evaluate_outputs(features, batch_size=12)   # model.evaluate (:304) -> {"loss", "auc", "auc_value"}
+    history = dien.fit(train_features, epochs=5)     # model.fit (:300), in file order; rebuilds `model`
 
-The two-output calls need the auxiliary-head weights (`weights.init_aux_weights`) and the inputs
+The two-output calls and `fit` need the auxiliary-head weights (`weights.init_aux_weights`) and the inputs
 `negtive_userRatedMovie2..5` (`features.negative_history`) and `label`.
 """
 from ..weights import init_aux_weights, init_weights
@@ -59,6 +60,11 @@ def evaluate(features, batch_size=None):
 
 
 def fit(features, epochs=5, batch_size=12, seed=0):
-    """Not implemented for this model: `fit` covers NeuralCF (tfrecmodel.neuralcf) and DeepFM (tfrecmodel.deepfm)
-    only."""
-    return _surface.fit(features, epochs, batch_size, seed)
+    """`model.fit(train_dataset, epochs=5)` (DIEN.py:300): train from the loaded weights on the GPU, in file order
+    every epoch (the script's dataset has no shuffle; `seed` is not used), then rebuild `model` from the trained
+    weights; returns the history dict {"loss", "auc", "auc_value"} (one value per epoch).  `features` also carries
+    `negtive_userRatedMovie2..5` and `label`, as for `evaluate_outputs`."""
+    global model
+    history = _surface.fit(features, epochs, batch_size, seed)
+    model = _surface.model
+    return history

@@ -1,4 +1,4 @@
-"""`model.fit` of NeuralCF, DeepFM, Wide&Deep and DeepFM_v2 on the GPU (NeuralCF.py:74-91, DeepFM.py,
+"""`model.fit` of NeuralCF, DeepFM, Wide&Deep, DeepFM_v2 and DIEN on the GPU (NeuralCF.py:74-91, DeepFM.py,
 WideNDeep.py:99-117, DeepFM_v2.py:158-165: compile(loss='binary_crossentropy', optimizer='adam'), then
 fit(train_dataset, epochs=5) over make_csv_dataset batches of 12).
 
@@ -9,8 +9,11 @@ fit(train_dataset, epochs=5) over make_csv_dataset batches of 12).
     loss, accuracy, roc_auc, pr_auc = tr.evaluate(test_features)   # the current weights, no export
     model = tr.to_model()                                 # a serving CTRModel built from the trained weights
 
+DIEN (DIEN.py:296-304: compile(optimizer="adam"), fit over batches of 12 with no shuffle) trains in file order
+every epoch by default and reports its own history {"loss", "auc", "auc_value"} (section 4.20).
+
 The forward, backward and Keras Adam run in the CUDA library (`srs_trainer_*`, include/srs_ctr.h; DESIGN.md
-sections 4.8, 4.9, 4.18 and 4.19).  TF's shuffle (buffer 10 000, unseeded) cannot be reproduced, so `fit` takes a seed instead: the host
+sections 4.8, 4.9, 4.18, 4.19 and 4.20).  For the other models TF's shuffle (buffer 10 000, unseeded) cannot be reproduced, so `fit` takes a seed instead: the host
 draws one `numpy.random.default_rng(seed).permutation(n)` per epoch and the library trains in that row order.
 """
 from __future__ import annotations
@@ -21,10 +24,10 @@ from typing import Dict, Mapping, Optional
 import numpy as np
 
 from . import _lib
-from .features import encode_batch
+from .features import _as_ids, encode_batch, negative_history_keys
 from .model import CTRModel, _host_struct, _label_array, _spec_struct
 from .spec import ModelSpec
-from .weights import check_weights, weight_shapes
+from .weights import aux_weight_shapes, check_weights, weight_shapes
 
 
 def epoch_orders(n: int, epochs: int, seed: int) -> np.ndarray:
@@ -34,25 +37,26 @@ def epoch_orders(n: int, epochs: int, seed: int) -> np.ndarray:
 
 
 class Trainer:
-    """Trainable NeuralCF, DeepFM, Wide&Deep or DeepFM_v2 weights and Keras Adam's state on one GPU."""
+    """Trainable NeuralCF, DeepFM, Wide&Deep, DeepFM_v2 or DIEN weights and Keras Adam's state on one GPU."""
 
-    MODELS = ("neuralcf", "deepfm", "widendeep", "deepfm_v2")
+    MODELS = ("neuralcf", "deepfm", "widendeep", "deepfm_v2", "dien")
 
     def __init__(self, spec: ModelSpec, weights: Mapping[str, np.ndarray], device: int = 0,
                  adam: Optional[Mapping[str, float]] = None):
         """`weights`: the initial weights (canonical names, Keras shapes, float32 host arrays), e.g.
         `init_weights(spec, seed, for_test=False)` for an untrained model.  `adam`: Keras Adam's lr, beta_1,
-        beta_2, epsilon (default: Keras's 0.001, 0.9, 0.999, 1e-7).  NotImplementedError for any model but
-        NeuralCF, DeepFM, Wide&Deep and DeepFM_v2."""
+        beta_2, epsilon (default: Keras's 0.001, 0.9, 0.999, 1e-7).  DIEN's weights include the auxiliary head's
+        group (`weights.init_aux_weights`): its objective needs them.  NotImplementedError for any model but
+        NeuralCF, DeepFM, Wide&Deep, DeepFM_v2 and DIEN."""
         if spec.model not in self.MODELS:
-            raise NotImplementedError("fit is implemented for NeuralCF (neural_cf_model_1), DeepFM, Wide&Deep and "
-                                      "DeepFM_v2 only, not %r" % spec.model)
+            raise NotImplementedError("fit is implemented for NeuralCF (neural_cf_model_1), DeepFM, Wide&Deep, "
+                                      "DeepFM_v2 and DIEN only, not %r" % spec.model)
         self.spec = spec
         self.device = int(device)
         self._h = None
         self._lib = _lib.load()
         check_weights(spec, weights)
-        shapes = weight_shapes(spec)
+        shapes = _shapes(spec)
         tensors = (_lib.SrsTensor * len(shapes))()
         keep = []
         for i, (name, shape) in enumerate(shapes):
@@ -105,6 +109,12 @@ class Trainer:
         ValueError for an out-of-range id or genre, a label other than 0 / 1, or a bad order, KeyError for a
         missing column; the weights are then unchanged.
 
+        DIEN: `features` also carries `negtive_userRatedMovie2..T` (a missing one is a KeyError, as in
+        `CTRModel.dien_outputs`); the row order defaults to file order every epoch (DIEN.py's dataset has no
+        shuffle; `seed` is not used), an explicit `order` is still taken; the history is {"loss", "auc",
+        "auc_value"}, each epoch's as `CTRModel.dien_evaluate` defines them over the steps' outputs; validation is
+        not supported (NotImplementedError).
+
         Validation, as Keras's `fit`: `validation_data` is `(x_val, y_val)` or a feature dict with "label";
         otherwise `validation_split` = f in (0, 1) holds out the last floor(n * f) rows, taken before any
         shuffling (training then uses the first n - floor(n * f) rows, and `order` is over those).  The epochs e
@@ -112,6 +122,10 @@ class Trainer:
         on the validation rows (one batch, in file order), logged as "val_loss", "val_accuracy", "val_auc" and
         "val_auc_1" for those epochs only.  Validation changes no weight, no Adam state and no training log.  Its
         rows are checked like the training rows before anything runs."""
+        if self.spec.model == "dien":
+            if validation_data is not None or validation_split or validation_freq != 1:
+                raise NotImplementedError("DIEN's fit takes no validation: DIEN.py validates nothing during fit")
+            return self._fit_dien(features, labels, epochs, batch_size, order)
         res, vres, validated = self._fit(features, labels, epochs, batch_size, seed, order, validation_data,
                                          validation_split, validation_freq)
         out = _logs(res, "")
@@ -161,10 +175,37 @@ class Trainer:
         validated = [e for e in range(epochs) if val is not None and (e + 1) % validation_freq == 0]
         return list(hist[:epochs]), list(vhist[:epochs]), validated
 
+    def _fit_dien(self, features, labels, epochs, batch_size, order) -> Dict[str, list]:
+        """DIEN's fit: the rows, their negatives and labels to srs_trainer_fit_dien_host."""
+        keep = []
+        batch, lab, n = self._rows(features, labels, keep, "fit")
+        keys = negative_history_keys(self.spec.hist_len)
+        neg = np.empty((n, max(len(keys), 1)), np.int32)
+        for j, k in enumerate(keys):
+            neg[:, j] = _as_ids(features, k, self.spec.n_movies, "negative movie id")
+        neg = np.ascontiguousarray(neg[:, :len(keys)])
+        epochs, batch_size = int(epochs), int(batch_size)
+        if order is None:
+            order = np.tile(np.arange(n, dtype=np.int32), (epochs, 1))
+        order = np.ascontiguousarray(order, np.int32)
+        if order.shape != (epochs, n):
+            raise ValueError("order must be [epochs=%d][n=%d], got %s" % (epochs, n, order.shape))
+        hist = (_lib.SrsDienEvalResult * max(epochs, 1))()
+        _lib.check(self._lib.srs_trainer_fit_dien_host(
+            self._h, C.byref(batch), neg.ctypes.data if neg.size else None, neg.shape[1], lab.ctypes.data,
+            order.ctypes.data, batch_size, epochs, hist))
+        res = list(hist[:epochs])
+        return {"loss": [r.loss for r in res], "auc": [r.auc for r in res], "auc_value": [r.auc_value for r in res]}
+
     def evaluate(self, features: Mapping[str, object], labels=None):
         """`model.evaluate(x)` of the current weights: (loss, accuracy, roc_auc, pr_auc) over the rows of
         `features` in one batch, as `CTRModel.evaluate` of `to_model()` reports them (on CUDA cores), without
-        exporting the weights.  Errors as `fit`'s."""
+        exporting the weights.  Errors as `fit`'s.  DIEN: NotImplementedError, as `tfrecmodel.dien.evaluate`: its
+        Keras evaluate is `to_model().dien_evaluate`."""
+        if self.spec.model == "dien":
+            raise NotImplementedError("DIEN's Keras evaluate reports the loss with the auxiliary negative-sample term "
+                                      "and its AUC metrics, not the four compile metrics; use "
+                                      "Trainer.to_model().dien_evaluate")
         r = self.evaluate_result(features, labels)
         return r.loss, r.accuracy, r.roc_auc, r.pr_auc
 
@@ -200,7 +241,7 @@ class Trainer:
     def weights(self) -> Dict[str, np.ndarray]:
         """The current weights, canonical names and Keras shapes (float32 host arrays)."""
         out = {}
-        for name, shape in weight_shapes(self.spec):
+        for name, shape in _shapes(self.spec):
             a = np.empty(shape, np.float32)
             _lib.check(self._lib.srs_trainer_get_weights(self._h, name.encode(), a.ctypes.data))
             out[name] = a
@@ -209,6 +250,11 @@ class Trainer:
     def to_model(self, device: Optional[int] = None) -> CTRModel:
         """A serving `CTRModel` built from the current weights (the trainer is not shared with it)."""
         return CTRModel(self.spec, self.weights(), self.device if device is None else device)
+
+
+def _shapes(spec: ModelSpec):
+    """The trainer's tensors: the model's, and for DIEN the auxiliary head's group, which its objective needs."""
+    return weight_shapes(spec) + (aux_weight_shapes(spec) if spec.model == "dien" else [])
 
 
 def _logs(results, prefix: str) -> Dict[str, list]:

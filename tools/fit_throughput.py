@@ -1,14 +1,17 @@
-"""Time NeuralCF's, DeepFM's, Wide&Deep's or DeepFM_v2's `fit` on the GPU against the numpy oracle on the host.
+"""Time NeuralCF's, DeepFM's, Wide&Deep's, DeepFM_v2's or DIEN's `fit` on the GPU against the numpy oracle on the
+host.
 
-    python tools/fit_throughput.py [--model neuralcf|deepfm|widendeep|deepfm_v2] [--epochs 5] [--batch-sizes 12,4096]
+    python tools/fit_throughput.py [--model neuralcf|deepfm|widendeep|deepfm_v2|dien] [--epochs 5] [--batch-sizes 12,4096]
                                    [--cpu-epochs 1] [--validate [--repeats 5]] [--kernels 4096]
 
 Trains the reference script's run - the untrained model of `init_weights(default_spec(model), 0, for_test=False)`
 over the 88 827 rows of `tests/golden/<model>_trainset.npz` (Wide&Deep: `deepfm_trainset.npz` with the columns of
-`widendeep_samples.npz`; DeepFM_v2: `deepfm_trainset.npz`) - for `--epochs` epochs at each batch size, and reports
+`widendeep_samples.npz`; DeepFM_v2: `deepfm_trainset.npz`; DIEN: `deepfm_trainset.npz` with userRatedMovie1 of
+`widendeep_samples.npz`, userRatedMovie2..5 of `dien_train_samples.npz`, the auxiliary head's initial weights and
+the negatives of DIEN.py:49, in file order) - for `--epochs` epochs at each batch size, and reports
 the wall time of `Trainer.fit` (upload, every step, the history read-back) and µs per step.  The CPU column is the
 float32 oracle (`oracle.ncf_train.fit` / `oracle.deepfm_train.fit` / `oracle.widendeep_train.fit` /
-`oracle.deepfm_v2_train.fit`) over `--cpu-epochs` epochs at the same batch
+`oracle.deepfm_v2_train.fit` / `oracle.dien_train.fit`) over `--cpu-epochs` epochs at the same batch
 size, scaled to µs per step (`--cpu-epochs 0` leaves it out).  `--validate` adds the cost of validating on the
 22 440 rows of `tests/golden/dien_testset.npz` every epoch, next to the epoch time: `validation_s_per_epoch` from
 fits of `--val-epochs` one-step epochs (the first batch of rows) with and without validation, where the two validation
@@ -42,7 +45,7 @@ def card():
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=("neuralcf", "deepfm", "widendeep", "deepfm_v2"), default="neuralcf")
+    ap.add_argument("--model", choices=("neuralcf", "deepfm", "widendeep", "deepfm_v2", "dien"), default="neuralcf")
     ap.add_argument("--epochs", type=int, default=5)
     ap.add_argument("--batch-sizes", default="12,4096")
     ap.add_argument("--cpu-epochs", type=int, default=1)
@@ -52,13 +55,17 @@ def main():
     ap.add_argument("--repeats", type=int, default=5)
     ap.add_argument("--kernels", type=int, default=0, help="batch size of a per-kernel breakdown (0: none)")
     args = ap.parse_args()
-    from oracle import deepfm_train, deepfm_v2_train, ncf_train, widendeep_train
+    dien = args.model == "dien"
+    if dien and args.validate:
+        ap.error("DIEN's fit takes no validation")
+    from oracle import deepfm_train, deepfm_v2_train, dien_train, ncf_train, widendeep_train
     from sparrowrecsys_b200.spec import default_spec
     from sparrowrecsys_b200.training import Trainer
-    from sparrowrecsys_b200.weights import init_weights
+    from sparrowrecsys_b200.weights import init_aux_weights, init_weights
     golden = os.path.join(ROOT, "tests", "golden")
     wd = args.model == "widendeep"
-    z = np.load(os.path.join(golden, "%s_trainset.npz" % ("deepfm" if wd or args.model == "deepfm_v2" else args.model)))
+    z = np.load(os.path.join(golden, "%s_trainset.npz" % ("deepfm" if wd or args.model in ("deepfm_v2", "dien")
+                                                          else args.model)))
     if args.model == "neuralcf":
         feats = {k: z[k] for k in ("movieId", "userId", "label")}
     else:
@@ -66,13 +73,22 @@ def main():
     if wd:
         extra = np.load(os.path.join(golden, "widendeep_samples.npz"))
         feats.update({k[6:]: extra[k] for k in extra.files if k.startswith("train_")})
+    if dien:
+        from sparrowrecsys_b200.features import negative_history
+        feats["userRatedMovie1"] = np.load(os.path.join(golden, "widendeep_samples.npz"))["train_userRatedMovie1"]
+        feats.update(dict(np.load(os.path.join(golden, "dien_train_samples.npz"))))
+        feats.update(negative_history(feats, 5, 2020))
     n = len(feats["label"])
     spec = default_spec(args.model)
     W0 = init_weights(spec, 0, for_test=False)
+    if dien:
+        W0.update(init_aux_weights(spec, 0))
 
     def oracle_fit(orders, B):
         if args.model == "neuralcf":
             ncf_train.fit(W0, feats["movieId"], feats["userId"], feats["label"], orders, B, np.float32)
+        elif dien:
+            dien_train.fit(W0, dien_train.Rows.from_features(feats, 5), orders, B, np.float32)
         else:
             m = {"deepfm": deepfm_train, "widendeep": widendeep_train, "deepfm_v2": deepfm_v2_train}[args.model]
             m.fit(W0, m.Rows.from_features(feats), feats["label"], orders, B, np.float32)
@@ -113,7 +129,7 @@ def main():
             run.update({"gpu_epoch_s": plain / args.epochs, "validation_s_per_epoch": extra_small / args.val_epochs,
                         "validated_minus_plain_s_per_epoch": extra / args.epochs})
         if args.cpu_epochs:
-            orders = ncf_train.epoch_orders(n, args.cpu_epochs, 0)
+            orders = [np.arange(n)] * args.cpu_epochs if dien else ncf_train.epoch_orders(n, args.cpu_epochs, 0)
             t0 = time.perf_counter()
             oracle_fit(orders, B)
             cpu = time.perf_counter() - t0
