@@ -276,11 +276,14 @@ __device__ __forceinline__ void gather_row(float* dst, const float* __restrict__
   *reinterpret_cast<float4*>(dst + 4 * q) = v;
 }
 
-// Side features of a 32-row tile shared by the DIN-family CUDA-core kernels: the userGenre1,
-// userId and movieGenre1 embedding rows (DenseFeatures columns of the user-profile / context
-// layers, e.g. DIN.py:108-123) land at tile columns off_ug / off_u / off_mg, the 7 numerics
-// (+ one zero pad) at off_num.  Rows past the batch end and missing / OOV genres (-1) are zero;
-// an id outside its vocabulary latches the error flag.  NT: the CTA's thread count.
+// Side features of a 32-row tile shared by the DIN-family kernels: the userGenre1, userId and
+// movieGenre1 embedding rows (DenseFeatures columns of the user-profile / context layers, e.g.
+// DIN.py:108-123) land at tile columns off_ug / off_u / off_mg, the 7 numerics (+ one zero pad) at
+// off_num.  Rows past the batch end and missing / OOV genres (-1) are zero; an id outside its
+// vocabulary latches the error flag.  The ids are read here, the rows and numerics are copied by
+// cp.async (16-byte row chunks, 4-byte numerics, a zero fill where the row is zero) that is not
+// waited for: the caller waits for its cp.async groups (stage_wait) and passes a barrier before
+// the tile is read.  NT: the CTA's thread count.
 template <int EP, int R, int NT = kThreads>
 __device__ __forceinline__ void tile_side_features(float* __restrict__ Xs, int ldx, int row0,
                                                    const BatchView& b, const float* user,
@@ -288,6 +291,7 @@ __device__ __forceinline__ void tile_side_features(float* __restrict__ Xs, int l
                                                    int n_users, int n_genres, int off_ug, int off_u,
                                                    int off_mg, int off_num) {
   constexpr int Q = EP / 4;
+  const uint32_t xs = static_cast<uint32_t>(__cvta_generic_to_shared(Xs));
   for (int i = threadIdx.x; i < R * 3 * Q; i += NT) {
     const int q = i % Q;
     const int t = i / Q;
@@ -307,14 +311,22 @@ __device__ __forceinline__ void tile_side_features(float* __restrict__ Xs, int l
         table = slot == 0 ? ugenre : mgenre;
       }
     }
-    gather_row<EP>(Xs + r * ldx + off, table, id, q);
+    // source size 0 reads nothing (the address stays a valid row) and zero-fills the 16 bytes
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;"
+                 ::"r"(xs + 4u * (r * ldx + off + 4 * q)), "l"(table + (size_t)max(id, 0) * EP + 4 * q),
+                 "r"(id >= 0 ? 16u : 0u) : "memory");
   }
   for (int i = threadIdx.x; i < R * kNumPad; i += NT) {
     const int r = i / kNumPad, j = i % kNumPad;
     const int row = row0 + r;
-    float v = 0.f;
-    if (j < kNumNumerics && row < b.B) v = __ldg(b.numerics + row * kNumNumerics + j);
-    Xs[r * ldx + off_num + j] = v;
+    if (j < kNumNumerics) {
+      const bool in = row < b.B;
+      asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;"
+                   ::"r"(xs + 4u * (r * ldx + off_num + j)), "l"(b.numerics + (in ? row * kNumNumerics + j : 0)),
+                   "r"(in ? 4u : 0u) : "memory");
+    } else {
+      Xs[r * ldx + off_num + j] = 0.f;
+    }
   }
 }
 

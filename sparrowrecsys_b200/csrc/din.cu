@@ -129,6 +129,7 @@ __global__ void __launch_bounds__(kThreads) din_kernel(DinParams p, BatchView b)
     }
   }
   clk.lap(PH_AU_LOOP);
+  stage_wait();                                            // the side features' copies
   __syncthreads();
   clk.lap(PH_ROW_IMBALANCE);
 

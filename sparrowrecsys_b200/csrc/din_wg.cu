@@ -33,10 +33,13 @@
 // At E <= 32 the 112 KB MLP image is not resident beside the warpgroups' buffers: they share one region, the
 // image at its bottom and the buffers at its top, and the image bytes under the buffers (94 KB at G = 4,
 // R = 2) are copied again in each tile once its activation unit is done, W1^T's
-// part (if any) first on its own barrier so that W2^T's flies under Dense(128).  The shared tile
-// helpers that map threads generically (tile_side_features, stage_weights) use every warpgroup; dense_layer
-// and row_dot (E <= 64) map 256 threads, and only
-// warpgroups 0 and 1 issue the top MLP's Dense(128).  Shared memory: ~227 KB (E <= 32) / ~218 KB
+// part (if any) first on its own barrier so that W2^T's flies under Dense(128).  At E <= 32 a tile's inputs wait
+// on no CTA-wide barrier (after the CTA's first tile): each warpgroup copies the candidate rows of its own rows
+// and computes their activation-unit constants, and the side features, which only the top MLP reads, are copied
+// by cp.async that the walk's gather waits cover.  At E <= 64 the CTA copies them all between two barriers.
+// The shared tile helpers that map threads generically (tile_side_features, stage_weights) use every
+// warpgroup; dense_layer and row_dot (E <= 64) map 256 threads, and only warpgroups 0 and 1 issue the top
+// MLP's Dense(128).  Shared memory: ~227 KB (E <= 32) / ~218 KB
 // (E <= 64): one CTA per SM.
 #include "kernels.h"
 #include "wgmma.cuh"
@@ -301,6 +304,7 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
   constexpr int KS = EP / 16;                     // K steps per part (hi or lo)
   constexpr int CP = 8 * KB;                      // 16-byte chunks per split row
   constexpr int NCOPY = kWgPos * CP / 128;        // cp.async per thread per tile
+  constexpr int NR = (kWgRows + G - 1) / G;       // most rows of a tile a warpgroup owns
   constexpr int OFF_UG = 0, OFF_U = EP, OFF_POOL = 2 * EP, OFF_C = 3 * EP, OFF_MG = 4 * EP, OFF_NUM = 5 * EP;
   extern __shared__ uint8_t raw[];
   // top-MLP image (TC_MLP): resident part / this tile's reload of W1^T's and of W2^T's part landed
@@ -363,33 +367,38 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
       prefetch_l1(h + (n - 1) / 2);
       prefetch_l1(h + n - 1);
     }
-    tile_side_features<EP, kWgRows, NT>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users, p.n_genres,
-                                        OFF_UG, OFF_U, OFF_MG, OFF_NUM);
-    // candidate rows of the tile (ids pass through float32, DIN.py:95,125); rows past the batch end are zero
-    for (int i = tid; i < kWgRows * EP / 4; i += NT) {
-      const int r = i / (EP / 4), c4 = i % (EP / 4), row = row0 + r;
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (row < b.B) {
-        const int cid = checked_id(__float2int_rz(__int2float_rn(__ldg(b.movie_id + row))), p.n_movies, b.err_flag);
-        v = ldg4(p.movie + (size_t)cid * EP + 4 * c4);
-      } else {
-        *reinterpret_cast<float4*>(Xs + r * L::LDX + OFF_POOL + 4 * c4) = v;
+    if constexpr (!L::TC_MLP) {
+      // E <= 64: the tile's inputs by the whole CTA, between two CTA-wide barriers (DESIGN §4.1: the per-warpgroup
+      // flow below measured 1 % slower at cfg 5, whose walk of 44 items per warpgroup dominates the tile)
+      tile_side_features<EP, kWgRows, NT>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users, p.n_genres,
+                                          OFF_UG, OFF_U, OFF_MG, OFF_NUM);
+      // candidate rows of the tile (ids pass through float32, DIN.py:95,125); rows past the batch end are zero
+      for (int i = tid; i < kWgRows * EP / 4; i += NT) {
+        const int r = i / (EP / 4), c4 = i % (EP / 4), row = row0 + r;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (row < b.B) {
+          const int cid =
+              checked_id(__float2int_rz(__int2float_rn(__ldg(b.movie_id + row))), p.n_movies, b.err_flag);
+          v = ldg4(p.movie + (size_t)cid * EP + 4 * c4);
+        } else {
+          *reinterpret_cast<float4*>(Xs + r * L::LDX + OFF_POOL + 4 * c4) = v;
+        }
+        *reinterpret_cast<float4*>(Xs + r * L::LDX + OFF_C + 4 * c4) = v;
       }
-      *reinterpret_cast<float4*>(Xs + r * L::LDX + OFF_C + 4 * c4) = v;
-    }
-    stage_wait();
-    __syncthreads();
-    // activation-unit constant of every row: cst[r][j] = au_b[j] + sum_e c_r[e] (Wc - Wsub)[e][j]
-    for (int i = tid; i < kWgRows * 32; i += NT) {
-      const int r = i >> 5, j = i & 31;
-      const float* cv = Xs + r * L::LDX + OFF_C;
-      float acc = __ldg(p.au_b + j);
+      stage_wait();                               // the staged weights and the side features
+      __syncthreads();
+      // activation-unit constant of every row: cst[r][j] = au_b[j] + sum_e c_r[e] (Wc - Wsub)[e][j]
+      for (int i = tid; i < kWgRows * 32; i += NT) {
+        const int r = i >> 5, j = i & 31;
+        const float* cv = Xs + r * L::LDX + OFF_C;
+        float acc = __ldg(p.au_b + j);
   #pragma unroll 8
-      for (int e = 0; e < EP; ++e) acc = fmaf(cv[e], wc[e * 32 + j], acc);
-      cst_all[i] = acc;
+        for (int e = 0; e < EP; ++e) acc = fmaf(cv[e], wc[e * 32 + j], acc);
+        cst_all[i] = acc;
+      }
+      __syncthreads();
+      clk.lap(PH_TILE_INPUTS);
     }
-    __syncthreads();
-    clk.lap(PH_TILE_INPUTS);
     // rows of this warpgroup: q, q + G, ...; the valid ones are a prefix
     int nrows = 0;
     for (int r = q; r < kWgRows; r += G)
@@ -453,14 +462,55 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
       if (__any_sync(0xffffffffu, bad) && lane == 0 && b.err_flag) atomicExch(b.err_flag, 1);
     };
 
+    // E <= 32: tile inputs per warpgroup.  Warpgroup q's walk reads the candidate rows and activation-unit
+    // constants of its own rows only, so it copies and computes those alone and waits for itself; the side features
+    // are read by the top MLP only, so their copies are issued with the first gathers and waited for by the walk's
+    // first gather wait (or the wait before the top MLP).  The history ids are requested first, so that their round
+    // trip overlaps the others.
     int ids_next[R][NCOPY];
     {
       int ids0[R][NCOPY];
       load_ids(0, ids0);
       load_ids(1, ids_next);
+      if constexpr (L::TC_MLP) {
+        // candidate rows (ids pass through float32, DIN.py:95,125); rows past the batch end are zero.  Their commit
+        // group also holds the staged weights in the CTA's first tile.
+        for (int i = tw; i < NR * (EP / 4); i += 128) {
+          const int r = q + G * (i / (EP / 4)), c4 = i % (EP / 4), row = row0 + r;
+          if (r >= kWgRows) break;
+          const bool in = row < b.B;
+          const int cid =
+              in ? checked_id(__float2int_rz(__int2float_rn(__ldg(b.movie_id + row))), p.n_movies, b.err_flag) : 0;
+          cp_async16_zfill(Xs + r * L::LDX + OFF_C + 4 * c4, p.movie + (size_t)cid * EP + 4 * c4, in ? 16u : 0u);
+          if (!in)
+            *reinterpret_cast<float4*>(Xs + r * L::LDX + OFF_POOL + 4 * c4) = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        cp_async_commit();
+        tile_side_features<EP, kWgRows, NT>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users,
+                                            p.n_genres, OFF_UG, OFF_U, OFF_MG, OFF_NUM);
+      }
       gather(0, ids0);
     }
     cp_async_commit();
+    if constexpr (L::TC_MLP) {
+      cp_async_wait<1>();                         // the candidate rows (and in the first tile the staged weights)
+      // every warpgroup reads all of the staged weights: the CTA's first tile waits for the CTA, later ones for the
+      // warpgroup
+      if (tile == blockIdx.x) __syncthreads();
+      else named_sync(1 + q, 128);
+      // activation-unit constants of the warpgroup's rows: cst[r][j] = au_b[j] + sum_e c_r[e] (Wc - Wsub)[e][j]
+      for (int i = tw; i < NR * 32; i += 128) {
+        const int r = q + G * (i >> 5), j = i & 31;
+        if (r >= kWgRows) break;
+        const float* cv = Xs + r * L::LDX + OFF_C;
+        float acc = __ldg(p.au_b + j);
+  #pragma unroll 8
+        for (int e = 0; e < EP; ++e) acc = fmaf(cv[e], wc[e * 32 + j], acc);
+        cst_all[r * 32 + j] = acc;
+      }
+      named_sync(1 + q, 128);
+      clk.lap(PH_TILE_INPUTS);
+    }
     // per item row s: pooling operand at pb_s + s PB_BYTES, pooled lo sums at pool_lo + 32 s, W_r at + s B_BYTES
     const uint32_t pb_s = smem_u32(base + L::PB_OFF + q * L::PB_WG_BYTES);
     float* pool_lo = fs + L::F_WG + q * L::F_WG_STRIDE;
