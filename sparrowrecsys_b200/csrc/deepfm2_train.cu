@@ -1,5 +1,5 @@
 // deepfm2_train.cu - the forward / backward step of DeepFM_v2's `model.fit` (DeepFM_v2.py:158-165); the trainer
-// that drives it (permutation, dedupe, Adam, metrics) is srs_trainer in ncf_train.cu.  DESIGN.md section 4.19.
+// that drives it (permutation, dedupe, Adam, metrics) is srs_trainer in trainer.cu.  DESIGN.md section 4.19.
 //
 // deepfm2_train_step_kernel<EP>: one 32-row tile per CTA, 256 threads.  The forward is deepfm2_kernel's
 // (deepfm2_layers.cuh), so a step's outputs are the serving outputs bit for bit.  The backward runs on the same
@@ -47,7 +47,7 @@ __global__ void __launch_bounds__(kThreads) deepfm2_train_step_kernel(DeepFm2Ste
   float* dfs = firsts + R;                       // dL/dfirst
   float* dzs = dfs + R;                          // dL/dz
   const DeepFm2Blob ly = DeepFm2Blob::of(EP);
-  const BatchView& b = a.b;
+  const BatchView& b = a.io.b;
   const DeepFm2Params& p = a.p;
   const int tid = threadIdx.x;
   const int row0 = blockIdx.x * R;
@@ -66,7 +66,7 @@ __global__ void __launch_bounds__(kThreads) deepfm2_train_step_kernel(DeepFm2Ste
     const float pr = sigmoidf_acc(z);
     b.probs[row] = pr;
     b.logits[row] = z;
-    const float dz = (pr - (float)__ldg(a.label + row)) / (float)b.B;
+    const float dz = (pr - (float)__ldg(a.io.label + row)) / (float)b.B;
     dzs[r] = dz;
     dfs[r] = dz * __ldg(p.wout);
   });
@@ -111,9 +111,9 @@ __global__ void __launch_bounds__(kThreads) deepfm2_train_step_kernel(DeepFm2Ste
       case 2: id = __ldg(b.user_genre + row * 5); off = G + p.n_movies; break;
       default: id = __ldg(b.user_id + row); off = 2 * G + p.n_movies; break;
     }
-    a.trow[s * b.B + row] = id < 0 ? -1 : (int32_t)(a.tab_row0[s] + id);
-    a.frow[s * b.B + row] = id < 0 ? -1 : off + id;
-    a.fgrad[s * b.B + row] = dfs[r];
+    a.io.trow[s * b.B + row] = id < 0 ? -1 : (int32_t)(a.tab_row0[s] + id);
+    a.io.frow[s * b.B + row] = id < 0 ? -1 : off + id;
+    a.io.fgrad[s * b.B + row] = dfs[r];
   }
   // their gradients: row k of proj_f against each row's dF_f, one warp per (f, k), the proj row read once
   const int warp = tid >> 5, lane = tid & 31;
@@ -124,7 +124,7 @@ __global__ void __launch_bounds__(kThreads) deepfm2_train_step_kernel(DeepFm2Ste
       const float2 d = *reinterpret_cast<const float2*>(dF + r * LDF + f * kProj + 2 * lane);
       float g = fmaf(w.y, d.y, w.x * d.x);
       g = warp_sum(g);
-      if (lane == 0) a.gemb[((size_t)f * b.B + row0 + r) * EP + k] = g;
+      if (lane == 0) a.io.gemb[((size_t)f * b.B + row0 + r) * EP + k] = g;
     }
   }
 
@@ -169,21 +169,16 @@ __global__ void __launch_bounds__(kThreads) deepfm2_train_step_kernel(DeepFm2Ste
     } else if (dl) {
       for (int r = 0; r < nv; ++r) s += dl[r * ldd];
     }
-    a.part[(size_t)blockIdx.x * ly.floats + q] = s;
+    a.io.part[(size_t)blockIdx.x * ly.floats + q] = s;
   }
 }
 
 template <int EP>
-cudaError_t launch_step_t(const DeepFm2StepArgs& a, cudaStream_t s) {
+cudaError_t launch_step_t(const DeepFm2StepArgs* a, cudaStream_t s) {
   constexpr int smem = step_smem_floats<EP>() * (int)sizeof(float);
-  static bool attr_set = false;
-  if (!attr_set) {
-    const cudaError_t e = cudaFuncSetAttribute(deepfm2_train_step_kernel<EP>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
-  deepfm2_train_step_kernel<EP><<<deepfm2_train_ctas(a.b.B), kThreads, smem, s>>>(a);
+  if (!a)                                             // the opt-in on the current device, no launch
+    return cudaFuncSetAttribute(deepfm2_train_step_kernel<EP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  deepfm2_train_step_kernel<EP><<<deepfm2_train_ctas(a->io.b.B), kThreads, smem, s>>>(*a);
   ++g_launch_count;
   return cudaGetLastError();
 }
@@ -192,9 +187,9 @@ cudaError_t launch_step_t(const DeepFm2StepArgs& a, cudaStream_t s) {
 
 int deepfm2_train_ctas(int B) { return (B + kFm2StepRows - 1) / kFm2StepRows; }
 
-cudaError_t launch_deepfm2_train_step(const DeepFm2StepArgs& a, cudaStream_t s) {
+cudaError_t launch_deepfm2_train_step(int EP, const DeepFm2StepArgs* a, cudaStream_t s) {
 #define SRS_FM2_STEP_CASE(E_) \
-  if (a.p.EP == E_) return launch_step_t<E_>(a, s);
+  if (EP == E_) return launch_step_t<E_>(a, s);
   SRS_FM2_STEP_CASE(12) SRS_FM2_STEP_CASE(16) SRS_FM2_STEP_CASE(32) SRS_FM2_STEP_CASE(64)
 #undef SRS_FM2_STEP_CASE
   return cudaErrorInvalidValue;

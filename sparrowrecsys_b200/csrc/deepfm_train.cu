@@ -1,5 +1,5 @@
 // deepfm_train.cu - the forward / backward step of DeepFM's `model.fit` (DeepFM.py) and the per-epoch row
-// permutation; the trainer that drives them (dedupe, Adam, metrics) is srs_trainer in ncf_train.cu.
+// permutation; the trainer that drives them (dedupe, Adam, metrics) is srs_trainer in trainer.cu.
 // DESIGN.md section 4.9.
 //
 // deepfm_train_step_kernel<EP>: one 32-row tile per CTA, 256 threads.  The forward is deepfm_kernel's
@@ -38,7 +38,7 @@ __global__ void __launch_bounds__(kThreads) deepfm_train_step_kernel(DeepFmStepA
   float* D2 = D1 + R * LDH;                      // [R][LDH] delta of the second
   float* dzs = D2 + R * LDH;                     // [R]      dL/dz
   const DeepFmBlob ly = DeepFmBlob::of(EP);
-  const BatchView& b = a.b;
+  const BatchView& b = a.io.b;
   DeepFmParams p = a.p;
   deepfm_load_out<EP>(p);
   const int tid = threadIdx.x;
@@ -50,7 +50,7 @@ __global__ void __launch_bounds__(kThreads) deepfm_train_step_kernel(DeepFmStepA
     const float pr = sigmoidf_acc(z);
     b.probs[row] = pr;
     b.logits[row] = z;
-    dzs[r] = (pr - (float)__ldg(a.label + row)) / (float)b.B;
+    dzs[r] = (pr - (float)__ldg(a.io.label + row)) / (float)b.B;
   });
   __syncthreads();
   for (int i = tid; i < nv * 64; i += kThreads) {
@@ -80,12 +80,12 @@ __global__ void __launch_bounds__(kThreads) deepfm_train_step_kernel(DeepFmStepA
       case 2: id = __ldg(b.movie_genre + row * 3); break;
       default: id = __ldg(b.user_genre + row * 5); break;
     }
-    a.trow[s * b.B + row] = id < 0 ? -1 : (int32_t)(a.tab_row0[s] + id);
+    a.io.trow[s * b.B + row] = id < 0 ? -1 : (int32_t)(a.tab_row0[s] + id);
     if (s < 4) {                                 // the one-hot rows: movieGenre1 | movieId | userGenre1 | userId
       const int G = p.n_genres;                  // slot s: movieId, userId, movieGenre1, userGenre1
       const int off = s == 0 ? G : s == 1 ? 2 * G + p.n_movies : s == 2 ? 0 : G + p.n_movies;
-      a.frow[s * b.B + row] = id < 0 ? -1 : off + id;
-      a.fgrad[s * b.B + row] = dzs[r];
+      a.io.frow[s * b.B + row] = id < 0 ? -1 : off + id;
+      a.io.fgrad[s * b.B + row] = dzs[r];
     }
   }
   const float w0 = p.wdot[0], w1 = p.wdot[1], w2 = p.wdot[2], w3 = p.wdot[3];
@@ -112,7 +112,7 @@ __global__ void __launch_bounds__(kThreads) deepfm_train_step_kernel(DeepFmStepA
         g = fmaf(w[j], d1[j], g);
       }
     }
-    a.gemb[((size_t)s * b.B + row0 + r) * EP + k] = g;
+    a.io.gemb[((size_t)s * b.B + row0 + r) * EP + k] = g;
   }
 
   // Dense gradients of this CTA's rows: parameter q = sum over rows in row order of (input . delta)
@@ -133,26 +133,21 @@ __global__ void __launch_bounds__(kThreads) deepfm_train_step_kernel(DeepFmStepA
     } else if (dl) {
       for (int r = 0; r < nv; ++r) s += dl[r * ldd];
     }
-    a.part[(size_t)blockIdx.x * ly.floats + q] = s;
+    a.io.part[(size_t)blockIdx.x * ly.floats + q] = s;
   }
 }
 
 template <int EP>
-cudaError_t launch_step_t(const DeepFmStepArgs& a, cudaStream_t s) {
+cudaError_t launch_step_t(const DeepFmStepArgs* a, cudaStream_t s) {
   constexpr int smem = step_smem_floats<EP>() * (int)sizeof(float);
-  static bool attr_set = false;
-  if (!attr_set) {
-    const cudaError_t e = cudaFuncSetAttribute(deepfm_train_step_kernel<EP>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
-  deepfm_train_step_kernel<EP><<<deepfm_train_ctas(a.b.B), kThreads, smem, s>>>(a);
+  if (!a)                                             // the opt-in on the current device, no launch
+    return cudaFuncSetAttribute(deepfm_train_step_kernel<EP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  deepfm_train_step_kernel<EP><<<deepfm_train_ctas(a->io.b.B), kThreads, smem, s>>>(*a);
   ++g_launch_count;
   return cudaGetLastError();
 }
 
-__global__ void deepfm_permute_kernel(DeepFmRows src, DeepFmRows dst, const int32_t* __restrict__ order, int n) {
+__global__ void deepfm_permute_kernel(TrainRows src, TrainRows dst, const int32_t* __restrict__ order, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int r = order[i];
@@ -169,15 +164,15 @@ __global__ void deepfm_permute_kernel(DeepFmRows src, DeepFmRows dst, const int3
 
 int deepfm_train_ctas(int B) { return (B + kFm1Rows - 1) / kFm1Rows; }
 
-cudaError_t launch_deepfm_train_step(const DeepFmStepArgs& a, cudaStream_t s) {
+cudaError_t launch_deepfm_train_step(int EP, const DeepFmStepArgs* a, cudaStream_t s) {
 #define SRS_DEEPFM_TRAIN_CASE(E_) \
-  if (a.p.EP == E_) return launch_step_t<E_>(a, s);
+  if (EP == E_) return launch_step_t<E_>(a, s);
   SRS_DEEPFM_TRAIN_CASE(12) SRS_DEEPFM_TRAIN_CASE(16) SRS_DEEPFM_TRAIN_CASE(32) SRS_DEEPFM_TRAIN_CASE(64)
 #undef SRS_DEEPFM_TRAIN_CASE
   return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_deepfm_permute(const DeepFmRows& src, const DeepFmRows& dst, const int32_t* order, int n,
+cudaError_t launch_deepfm_permute(const TrainRows& src, const TrainRows& dst, const int32_t* order, int n,
                                   cudaStream_t s) {
   deepfm_permute_kernel<<<(n + 255) / 256, 256, 0, s>>>(src, dst, order, n);
   ++g_launch_count;

@@ -1,6 +1,6 @@
 // dien_train.cu - the forward / backward step of DIEN's `model.fit` (DIEN.py:296-304: compile(optimizer="adam"),
 // fit over batches of 12 in file order); the trainer that drives it (dedupe, Adam, metrics) is srs_trainer in
-// ncf_train.cu.  DESIGN.md section 4.20.
+// trainer.cu.  DESIGN.md section 4.20.
 //
 // dien_train_step_kernel<EP>: one 32-row tile per CTA, 256 threads, one warp per row and lane e on element e of
 // every state vector, as dien_kernel.  The objective is the sum over the batch of final_loss_i = bce_i - 0.5 *
@@ -460,16 +460,11 @@ __global__ void __launch_bounds__(kThreads) dien_train_step_kernel(DienStepArgs 
 }
 
 template <int EP>
-cudaError_t launch_step_t(const DienStepArgs& a, cudaStream_t s) {
+cudaError_t launch_step_t(const DienStepArgs* a, cudaStream_t s) {
   constexpr int smem = step_smem_floats<EP>() * (int)sizeof(float);
-  static bool attr_set = false;
-  if (!attr_set) {
-    const cudaError_t e = cudaFuncSetAttribute(dien_train_step_kernel<EP>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
-  dien_train_step_kernel<EP><<<dien_train_ctas(a.B), kThreads, smem, s>>>(a);
+  if (!a)                                             // the opt-in on the current device, no launch
+    return cudaFuncSetAttribute(dien_train_step_kernel<EP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  dien_train_step_kernel<EP><<<dien_train_ctas(a->B), kThreads, smem, s>>>(*a);
   ++g_launch_count;
   return cudaGetLastError();
 }
@@ -480,10 +475,10 @@ int dien_train_ctas(int B) { return (B + kDienRows - 1) / kDienRows; }
 
 size_t dien_train_rec_floats(int B, int T) { return (size_t)B * T * kDienRecSlots * 32; }
 
-cudaError_t launch_dien_train_step(const DienStepArgs& a, cudaStream_t s) {
-  if (a.B <= 0) return cudaSuccess;
+cudaError_t launch_dien_train_step(int EP, const DienStepArgs* a, cudaStream_t s) {
+  if (a && a->B <= 0) return cudaSuccess;
 #define SRS_DIEN_STEP_CASE(E_) \
-  if (a.p.EP == E_) return launch_step_t<E_>(a, s);
+  if (EP == E_) return launch_step_t<E_>(a, s);
   SRS_DIEN_STEP_CASE(12) SRS_DIEN_STEP_CASE(16) SRS_DIEN_STEP_CASE(32)
 #undef SRS_DIEN_STEP_CASE
   return cudaErrorInvalidValue;

@@ -1,4 +1,4 @@
-// kernels.h - what model.cu and ncf_train.cu need of the kernel files: the parameter blocks (device pointers into
+// kernels.h - what model.cu and trainer.cu need of the kernel files: the parameter blocks (device pointers into
 // the model's private weight layout) and launch entry points of the fused per-model forward kernels, of the
 // training steps, the ranking tail and the metrics.  The offline jobs' shared declarations are in hostcall.h.
 #pragma once
@@ -33,6 +33,40 @@ struct NcfParams {
   //            out kernel [1] @out_w, bias @out_b
   int w_off[6], b_off[6];
   int out_w, out_b;
+};
+
+// ---- NeuralCF's training step (ncf_train.cu; DESIGN.md section 4.8) --------------------------------------------
+struct NcfStepArgs {
+  const float* tab;        // [n_movies + n_users][EP]: movie rows, then user rows
+  const float* blob;       // Dense weights
+  const int32_t* movie;    // the dataset [n]
+  const int32_t* user;
+  const int32_t* label;
+  const int32_t* order;    // this step's rows [B]
+  int B, n_movies;
+  float* probs;            // [B] outputs of the step, before its update
+  float* logits;
+  int32_t* labels;         // [B] the step's labels, for the metrics
+  int32_t* trow;           // [2B] table row of each (movie, user) entry: movie r at r, user r at B + r
+  float* gemb;             // [2B][EP] the entries' embedding gradients
+  float* part;             // [ctas][blob_floats] per-CTA Dense gradient sums
+};
+int ncf_train_ctas(int B);
+// p: the trainer's NcfParams, for the instantiation <p.EP, p.HP> and the blob layout.  Each step launcher takes a
+// null `a` to opt its instantiation into the most dynamic shared memory it asks for, on the current device, instead
+// of launching (srs_trainer_create): the opt-in is per device.
+cudaError_t launch_ncf_train_step(const NcfStepArgs* a, const NcfParams& p, cudaStream_t s);
+
+// What the trainer hands each tile model's step (DeepFM, Wide&Deep, DeepFM_v2): the step's rows and where its
+// outputs go
+struct StepIO {
+  BatchView b;             // the step's B rows in order; probs / logits receive its outputs before the update
+  const int32_t* label;    // [B]
+  int32_t* trow;           // [n_ent B] table row of entry s * B + r (slot s), -1 = none (a missing genre)
+  float* gemb;             // [n_ent B][EP] the entries' gradients
+  int32_t* frow;           // [n_fent B] one-hot row of entry s * B + r, -1 = none (a missing genre)
+  float* fgrad;            // [n_fent B] its gradient
+  float* part;             // [ctas][blob floats] per-CTA Dense gradient sums
 };
 
 // ---- EmbeddingMLP / Wide&Deep (EmbeddingMLP.py:72-77, WideNDeep.py:101-107) --------
@@ -73,20 +107,15 @@ cudaError_t setup_embmlp_attributes();   // embmlp_kernel's dynamic shared memor
 
 // ---- Wide&Deep's training step (widendeep_train.cu; DESIGN.md section 4.18) ---------------------------------------
 constexpr int kWideDeepTables = 10;   // the kernel's slots: movieGenre1..3, movieId, userGenre1..5, userId
+// io: b.hist is userRatedMovie1 (stride 1); 10 table entries per row, and one one-hot entry, the row's wide row
+// (crossed bucket) with its dL/dz
 struct WideDeepStepArgs {
   EmbMlpParams p;          // the trainer's tables, Dense weights and wide rows
-  BatchView b;             // the step's B rows in order (hist: userRatedMovie1, stride 1); probs / logits receive
-                           // its outputs before the update
-  const int32_t* label;    // [B]
+  StepIO io;
   int64_t tab_row0[kWideDeepTables];   // first row of each slot's table in the trainer's table array
-  int32_t* trow;           // [10B] table row of entry s * B + r, -1 = none (a missing genre)
-  float* gemb;             // [10B][EP] the entries' gradients
-  int32_t* wrow;           // [B] wide row (crossed bucket) of row r
-  float* wgrad;            // [B] its gradient (the row's dL/dz)
-  float* part;             // [ctas][EmbMlpBlob::floats] per-CTA Dense gradient sums
 };
 int widendeep_train_ctas(int B);
-cudaError_t launch_widendeep_train_step(const WideDeepStepArgs& a, cudaStream_t s);
+cudaError_t launch_widendeep_train_step(int EP, const WideDeepStepArgs* a, cudaStream_t s);
 
 // ---- EmbeddingMLP / Wide&Deep on tensor cores (embmlp_tc.cu): E <= 12 ------------------------
 struct EmbMlpTcParams {
@@ -148,33 +177,29 @@ cudaError_t setup_deepfm_attributes();   // deepfm_kernel's (and deepfm2_kernel'
 
 // ---- DeepFM's training step (deepfm_train.cu; DESIGN.md section 4.9) ----------------------------
 constexpr int kDeepFmTables = 6;   // fm movieId, fm userId, fm movieGenre1, fm userGenre1, deep movieId, deep userId
+// io: 6 table entries per row (slot s in kDeepFmTables order), and 4 one-hot entries, rows of dense_2/kernel with
+// the row's dL/dz
 struct DeepFmStepArgs {
   DeepFmParams p;          // the trainer's tables and Dense weights
-  BatchView b;             // the step's B rows in order; probs / logits receive its outputs before the update
-  const int32_t* label;    // [B]
+  StepIO io;
   int64_t tab_row0[kDeepFmTables];   // first row of each table in the trainer's table array
-  int32_t* trow;           // [6B] table row of entry s * B + r (slot s in kDeepFmTables order), -1 = none
-  float* gemb;             // [6B][EP] the entries' gradients
-  int32_t* frow;           // [4B] one-hot row of dense_2/kernel of entry s * B + r, -1 = none (a missing genre)
-  float* fgrad;            // [4B] its gradient (the row's dL/dz)
-  float* part;             // [ctas][DeepFmBlob::floats] per-CTA Dense gradient sums
 };
 int deepfm_train_ctas(int B);
-cudaError_t launch_deepfm_train_step(const DeepFmStepArgs& a, cudaStream_t s);
-struct DeepFmRows {        // a DeepFM, DeepFM_v2 or Wide&Deep dataset on the device, in the srs_batch layout
-  int32_t* movie;          // [n]
+cudaError_t launch_deepfm_train_step(int EP, const DeepFmStepArgs* a, cudaStream_t s);
+struct TrainRows {         // a trainer's dataset on the device, in the srs_batch layout; a column the model does not
+  int32_t* movie;          //   read is null.  [n]
   int32_t* user;           // [n]
-  int32_t* mgenre;         // [n][3], column 0 read (DeepFM)
-  int32_t* ugenre;         // [n][5], column 0 read (DeepFM)
+  int32_t* mgenre;         // [n][3], column 0 read (DeepFM, DeepFM_v2)
+  int32_t* ugenre;         // [n][5], column 0 read (DeepFM, DeepFM_v2)
   float* numerics;         // [n][7]
   int32_t* label;          // [n]
-  int32_t* rated;          // [n] userRatedMovie1 (Wide&Deep; null otherwise)
+  int32_t* rated;          // [n] userRatedMovie1 (Wide&Deep)
 };
 // dst row i = src row order[i], i < n (genres: column 0 only)
-cudaError_t launch_deepfm_permute(const DeepFmRows& src, const DeepFmRows& dst, const int32_t* order, int n,
+cudaError_t launch_deepfm_permute(const TrainRows& src, const TrainRows& dst, const int32_t* order, int n,
                                   cudaStream_t s);
 // the same for Wide&Deep: every genre column and userRatedMovie1
-cudaError_t launch_widendeep_permute(const DeepFmRows& src, const DeepFmRows& dst, const int32_t* order, int n,
+cudaError_t launch_widendeep_permute(const TrainRows& src, const TrainRows& dst, const int32_t* order, int n,
                                      cudaStream_t s);
 
 // ---- DeepFM with the deep MLP on tensor cores (deepfm_tc.cu): emb_dim 13..16 --------------------
@@ -250,19 +275,15 @@ struct DeepFm2Blob {
 
 // ---- DeepFM_v2's training step (deepfm2_train.cu; DESIGN.md section 4.19) ----------------------------------------
 constexpr int kDeepFm2Tables = 4;   // movieGenre1, movieId, userGenre1, userId: the field order
+// io: 4 table entries per row (field s), and 4 one-hot entries, rows of first_cat/kernel with the row's
+// dL/dz * out/kernel[0]
 struct DeepFm2StepArgs {
   DeepFm2Params p;         // the trainer's tables, Dense weights and one-hot first_cat/kernel
-  BatchView b;             // the step's B rows in order; probs / logits receive its outputs before the update
-  const int32_t* label;    // [B]
+  StepIO io;
   int64_t tab_row0[kDeepFm2Tables];   // first row of each table in the trainer's table array
-  int32_t* trow;           // [4B] table row of entry s * B + r (field s), -1 = none (a missing genre)
-  float* gemb;             // [4B][EP] the entries' gradients
-  int32_t* frow;           // [4B] one-hot row of first_cat/kernel of entry s * B + r, -1 = none (a missing genre)
-  float* fgrad;            // [4B] its gradient (the row's dL/dz * out/kernel[0])
-  float* part;             // [ctas][DeepFm2Blob::floats] per-CTA Dense gradient sums
 };
 int deepfm2_train_ctas(int B);
-cudaError_t launch_deepfm2_train_step(const DeepFm2StepArgs& a, cudaStream_t s);
+cudaError_t launch_deepfm2_train_step(int EP, const DeepFm2StepArgs* a, cudaStream_t s);
 
 // ---- DIN (DIN.py:125-167) ------------------------------------------------------------
 struct DinParams {
@@ -402,7 +423,7 @@ struct DienStepArgs {
 };
 int dien_train_ctas(int B);
 size_t dien_train_rec_floats(int B, int T);   // the floats of DienStepArgs::rec
-cudaError_t launch_dien_train_step(const DienStepArgs& a, cudaStream_t s);
+cudaError_t launch_dien_train_step(int EP, const DienStepArgs* a, cudaStream_t s);
 
 // ---- DIEN's auxiliary head (DIEN.py:261-292), the AUX variant of dien_kernel --------------------------
 struct DienAuxView {

@@ -1,7 +1,7 @@
 // placement.h - where the Keras tensors of the trainable models (NeuralCF's neural_cf_model_1 and two towers, DeepFM,
 // DeepFM_v2, EmbeddingMLP / Wide&Deep and DIEN) live on the device, written once for the serving builders (build_ncf,
 // build_deepfm, build_deepfm2, build_embmlp, build_dien in model.cu) and the
-// trainer (srs_trainer_create, srs_trainer_get_weights in ncf_train.cu): the builders and the trainer scatter the
+// trainer (srs_trainer_create, srs_trainer_get_weights in trainer.cu): the builders and the trainer scatter the
 // caller's host tensors through it, and the trainer gathers its weights back through it.  Also the by-name lookup of
 // the caller's tensors that both use.  Host code only.
 #pragma once

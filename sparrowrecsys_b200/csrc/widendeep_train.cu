@@ -1,5 +1,5 @@
 // widendeep_train.cu - the forward / backward step of Wide&Deep's `model.fit` (WideNDeep.py:99-117) and the
-// per-epoch row permutation; the trainer that drives them (dedupe, Adam, metrics) is srs_trainer in ncf_train.cu.
+// per-epoch row permutation; the trainer that drives them (dedupe, Adam, metrics) is srs_trainer in trainer.cu.
 // DESIGN.md section 4.18.
 //
 // widendeep_train_step_kernel<EP>: one 32-row tile per CTA, 256 threads.  The forward is embmlp_kernel's
@@ -39,7 +39,7 @@ __global__ void __launch_bounds__(kThreads) widendeep_train_step_kernel(WideDeep
   float* W2s = D2 + R * LDH;
   float* dzs = W2s + 128 * 128;                  // dL/dz
   const EmbMlpBlob ly = EmbMlpBlob::of(EP);
-  const BatchView& b = a.b;
+  const BatchView& b = a.io.b;
   const EmbMlpParams& p = a.p;
   const int tid = threadIdx.x;
   const int row0 = blockIdx.x * R;
@@ -54,10 +54,10 @@ __global__ void __launch_bounds__(kThreads) widendeep_train_step_kernel(WideDeep
     const float pr = sigmoidf_acc(z);
     b.probs[row] = pr;
     b.logits[row] = z;
-    const float dz = (pr - (float)__ldg(a.label + row)) / (float)b.B;
+    const float dz = (pr - (float)__ldg(a.io.label + row)) / (float)b.B;
     dzs[r] = dz;
-    a.wrow[row] = bucket;
-    a.wgrad[row] = dz;
+    a.io.frow[row] = bucket;
+    a.io.fgrad[row] = dz;
   });
   __syncthreads();
   for (int i = tid; i < nv * 128; i += kThreads) {
@@ -86,7 +86,7 @@ __global__ void __launch_bounds__(kThreads) widendeep_train_step_kernel(WideDeep
     else if (s < 9) id = __ldg(b.user_genre + row * 5 + (s - 4));
     else id = __ldg(b.user_id + row);
     const bool missing = id < 0 || (s != 3 && s != 9 && id >= p.n_genres);
-    a.trow[s * b.B + row] = missing ? -1 : (int32_t)(a.tab_row0[s] + id);
+    a.io.trow[s * b.B + row] = missing ? -1 : (int32_t)(a.tab_row0[s] + id);
   }
   // their gradients: tile row q = s * EP + k of W1 against each row's delta1, one warp per q, W1's row read once
   const int warp = tid >> 5, lane = tid & 31;
@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(kThreads) widendeep_train_step_kernel(WideDeep
       const float4 d = *reinterpret_cast<const float4*>(D1 + r * LDH + 4 * lane);
       float g = fmaf(w.w, d.w, fmaf(w.z, d.z, fmaf(w.y, d.y, w.x * d.x)));
       g = warp_sum(g);
-      if (lane == 0) a.gemb[((size_t)s * b.B + row0 + r) * EP + k] = g;
+      if (lane == 0) a.io.gemb[((size_t)s * b.B + row0 + r) * EP + k] = g;
     }
   }
 
@@ -118,26 +118,21 @@ __global__ void __launch_bounds__(kThreads) widendeep_train_step_kernel(WideDeep
     } else if (dl) {
       for (int r = 0; r < nv; ++r) s += dl[r * ldd];
     }
-    a.part[(size_t)blockIdx.x * ly.floats + q] = s;
+    a.io.part[(size_t)blockIdx.x * ly.floats + q] = s;
   }
 }
 
 template <int EP>
-cudaError_t launch_step_t(const WideDeepStepArgs& a, cudaStream_t s) {
+cudaError_t launch_step_t(const WideDeepStepArgs* a, cudaStream_t s) {
   constexpr int smem = step_smem_floats<EP>() * (int)sizeof(float);
-  static bool attr_set = false;
-  if (!attr_set) {
-    const cudaError_t e = cudaFuncSetAttribute(widendeep_train_step_kernel<EP>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
-  widendeep_train_step_kernel<EP><<<widendeep_train_ctas(a.b.B), kThreads, smem, s>>>(a);
+  if (!a)                                             // the opt-in on the current device, no launch
+    return cudaFuncSetAttribute(widendeep_train_step_kernel<EP>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  widendeep_train_step_kernel<EP><<<widendeep_train_ctas(a->io.b.B), kThreads, smem, s>>>(*a);
   ++g_launch_count;
   return cudaGetLastError();
 }
 
-__global__ void widendeep_permute_kernel(DeepFmRows src, DeepFmRows dst, const int32_t* __restrict__ order, int n) {
+__global__ void widendeep_permute_kernel(TrainRows src, TrainRows dst, const int32_t* __restrict__ order, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int r = order[i];
@@ -157,15 +152,15 @@ __global__ void widendeep_permute_kernel(DeepFmRows src, DeepFmRows dst, const i
 
 int widendeep_train_ctas(int B) { return (B + kWdRows - 1) / kWdRows; }
 
-cudaError_t launch_widendeep_train_step(const WideDeepStepArgs& a, cudaStream_t s) {
+cudaError_t launch_widendeep_train_step(int EP, const WideDeepStepArgs* a, cudaStream_t s) {
 #define SRS_WD_STEP_CASE(E_) \
-  if (a.p.EP == E_) return launch_step_t<E_>(a, s);
+  if (EP == E_) return launch_step_t<E_>(a, s);
   SRS_WD_STEP_CASE(12) SRS_WD_STEP_CASE(16) SRS_WD_STEP_CASE(32) SRS_WD_STEP_CASE(64)
 #undef SRS_WD_STEP_CASE
   return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_widendeep_permute(const DeepFmRows& src, const DeepFmRows& dst, const int32_t* order, int n,
+cudaError_t launch_widendeep_permute(const TrainRows& src, const TrainRows& dst, const int32_t* order, int n,
                                      cudaStream_t s) {
   widendeep_permute_kernel<<<(n + 255) / 256, 256, 0, s>>>(src, dst, order, n);
   ++g_launch_count;

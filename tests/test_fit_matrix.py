@@ -1,8 +1,8 @@
 """`model.fit` at every step-kernel instantiation, hidden depth and padding edge against the float64 training oracle.
 
 NeuralCF's step is `ncf_train_step_kernel<EP, HP>` (EP in {12, 16, 32, 64}, HP in {16, 32}; csrc/ncf_train.cu) over
-1 to 3 hidden layers; it asks for more than 48 KiB of dynamic shared memory only when a shape needs it, and asks
-again when a later shape of the same instantiation needs more.  DeepFM's is `deepfm_train_step_kernel<EP>`
+1 to 3 hidden layers; the trainer (csrc/trainer.cu) opts it into its three-layer dynamic shared memory at create,
+which is above 48 KiB for some instantiations and covers every smaller shape.  DeepFM's is `deepfm_train_step_kernel<EP>`
 (csrc/deepfm_train.cu), with the serving `deepfm_kernel<EP>` for validation and `Trainer.evaluate`.  The trainer places
 its weights through the serving builders' placement (csrc/placement.h) and gathers its exports back through it, and
 its step kernels restate the layout's offsets.  The defects such code invites - a padded column read as data, the last real column or unit dropped, the wrong
@@ -256,9 +256,9 @@ def test_matrix_covers_depths_widths_and_batches():
 
 
 def test_matrix_crosses_the_shared_memory_opt_in_and_grows_it():
-    """`launch_step_t` opts a NeuralCF instantiation in above 48 KiB, and again when a later shape needs more than
-    it asked for: cases on both sides of 48 KiB, and an instantiation whose opted-in case is followed (in the order the
-    GPU tests run) by a larger one."""
+    """`srs_trainer_create` opts a NeuralCF instantiation in once, at its three-layer shared memory: cases on both
+    sides of 48 KiB, and an instantiation run at a shape that is followed (in the order the GPU tests run) by a larger
+    one, so that the create-time opt-in at the largest size covers each smaller shape."""
     ncf = [c for c in FIT_MATRIX if c.model == "neuralcf"]
     smem = [step_smem_bytes(c) for c in ncf]
     assert any(s <= OPT_IN_BYTES for s in smem) and any(s > OPT_IN_BYTES for s in smem), smem

@@ -1,4 +1,4 @@
-"""GPU checks of NeuralCF's `fit` (csrc/ncf_train.cu, DESIGN.md section 4.8) against the float64 / float32 oracle
+"""GPU checks of NeuralCF's `fit` (csrc/ncf_train.cu, csrc/trainer.cu, DESIGN.md section 4.8) against the float64 / float32 oracle
 (oracle/ncf_train.py) and the reference script's end-to-end known answer (tests/golden/neuralcf_fit.json)."""
 import json
 import os

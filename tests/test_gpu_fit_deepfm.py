@@ -1,4 +1,4 @@
-"""GPU checks of DeepFM's `fit` (csrc/deepfm_train.cu and the trainer in csrc/ncf_train.cu, DESIGN.md section 4.9)
+"""GPU checks of DeepFM's `fit` (csrc/deepfm_train.cu and the trainer in csrc/trainer.cu, DESIGN.md section 4.9)
 against the float64 / float32 oracle (oracle/deepfm_train.py) and the reference script's end-to-end known answer
 (tests/golden/deepfm_fit.json)."""
 import json

@@ -1,4 +1,4 @@
-"""GPU checks of DeepFM_v2's `fit` (csrc/deepfm2_train.cu and the trainer in csrc/ncf_train.cu, DESIGN.md section
+"""GPU checks of DeepFM_v2's `fit` (csrc/deepfm2_train.cu and the trainer in csrc/trainer.cu, DESIGN.md section
 4.19) against the float64 / float32 oracle (oracle/deepfm_v2_train.py) and the reference script's end-to-end known
 answer (tests/golden/deepfm_v2_fit.json)."""
 import json

@@ -1,4 +1,4 @@
-"""GPU checks of DIEN's `fit` (csrc/dien_train.cu and srs_trainer_fit_dien_host in csrc/ncf_train.cu, DESIGN.md
+"""GPU checks of DIEN's `fit` (csrc/dien_train.cu and srs_trainer_fit_dien_host in csrc/trainer.cu, DESIGN.md
 section 4.20) against the float64 / float32 oracle (oracle/dien_train.py)."""
 import ctypes as C
 import json

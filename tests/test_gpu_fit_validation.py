@@ -1,4 +1,4 @@
-"""GPU checks of validation during `fit` and of `Trainer.evaluate` (csrc/ncf_train.cu, DESIGN.md section 4.10):
+"""GPU checks of validation during `fit` and of `Trainer.evaluate` (csrc/trainer.cu, DESIGN.md section 4.10):
 validation is `evaluate` of the epoch's weights and changes nothing else, agrees with the float64 oracle's validated
 fit (oracle/fit_validation.py), and follows Keras's validation_split / validation_freq rules."""
 import ctypes as C

@@ -1,4 +1,4 @@
-"""GPU checks of Wide&Deep's `fit` (csrc/widendeep_train.cu and the trainer in csrc/ncf_train.cu, DESIGN.md section
+"""GPU checks of Wide&Deep's `fit` (csrc/widendeep_train.cu and the trainer in csrc/trainer.cu, DESIGN.md section
 4.18) against the float64 / float32 oracle (oracle/widendeep_train.py) and the reference script's end-to-end known
 answer (tests/golden/widendeep_fit.json)."""
 import json
