@@ -24,7 +24,8 @@ in numpy at `dtype` (float32 or float64):
   ApplyAdam's dense form.
 
 `defect` (mutants for the tests): "mask" ignores the mask in BPTT, "h0" trains augru_h0, "aux" drops the auxiliary
-head's gradient, "step" drops position 0's gradients, "mean" divides the objective by B.
+head's gradient, "step" drops position 0's gradients, "mean" divides the objective by B, "last" gives the embedding
+rows of history position T - 1 no gradient.
 """
 from __future__ import annotations
 
@@ -274,7 +275,7 @@ def gradients(W, r: Rows, y, dtype=np.float32, defect: Optional[str] = None):
         dh = np.where(m, dh * q["z"] + dmh @ U.T, dh).astype(dt)
     emb = g["embedding"]
     np.add.at(emb, r.mid, dC)
-    for t in range(T):
+    for t in range(T - 1 if defect == "last" else T):
         np.add.at(emb, r.hist[:, t], dX[:, t])
     for t in range(1, T):
         np.add.at(emb, r.neg[:, t - 1], dN[:, t - 1])

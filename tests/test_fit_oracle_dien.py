@@ -195,20 +195,6 @@ def test_create_and_create_ex_keep_their_lists_and_fit_dien_needs_a_trainer():
     assert lib.srs_trainer_fit_dien_host(None, None, None, 0, None, None, 12, 1, None) == _lib.SRS_ERR_INVALID
 
 
-def test_every_step_kernel_instantiation_has_a_gpu_matrix_case():
-    import re
-    from pathlib import Path
-    import test_gpu_fit_dien as G
-    src = (Path(__file__).resolve().parents[1] / "sparrowrecsys_b200" / "csrc" / "dien_train.cu").read_text()
-    eps = {int(x) for x in re.findall(r"SRS_DIEN_STEP_CASE\((\d+)\)", src)}
-    assert eps == {12, 16, 32}
-    round_ep = lambda E: 12 if E <= 12 else 16 if E <= 16 else 32
-    assert eps == {round_ep(c[0]) for c in G.MATRIX}
-    for ep in eps:                          # both edges of each instantiation's range
-        Es = {c[0] for c in G.MATRIX if round_ep(c[0]) == ep}
-        assert min(Es) <= {12: 1, 16: 13, 32: 17}[ep] and max(Es) == ep
-
-
 def test_trainer_refuses_dien_validation_without_a_device():
     from sparrowrecsys_b200.training import Trainer
     t = Trainer.__new__(Trainer)

@@ -3,7 +3,6 @@ the trainer ABI's up-front rejections for Wide&Deep (DESIGN.md section 4.18)."""
 import ctypes as C
 import json
 import os
-import re
 
 import numpy as np
 import pytest
@@ -14,7 +13,6 @@ from sparrowrecsys_b200.weights import init_weights
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = os.path.join(HERE, "golden")
-CSRC = os.path.join(os.path.dirname(HERE), "sparrowrecsys_b200", "csrc")
 
 
 def small_case(seed, B, hidden=(6, 5), E=3, Vm=7, Vu=9, cb=5):
@@ -307,22 +305,6 @@ def test_generator_reproduces_the_columns():
     import subprocess
     import sys
     subprocess.check_call([sys.executable, os.path.join(GOLDEN, "make_widendeep_train_golden.py"), "--check"])
-
-
-# ---- every step-kernel instantiation has a GPU case ---------------------------------------------------------------
-def round_ep(E):
-    """csrc/placement.h round_ep: an embedding width padded to the kernels' instantiations."""
-    return 12 if E <= 12 else 16 if E <= 16 else 32 if E <= 32 else 64
-
-
-def test_every_dispatched_step_instantiation_has_a_gpu_case():
-    with open(os.path.join(CSRC, "widendeep_train.cu")) as f:
-        dispatched = {int(e) for e in re.findall(r"SRS_WD_STEP_CASE\((\d+)\)", f.read())}
-    with open(os.path.join(HERE, "test_gpu_fit_widendeep.py")) as f:
-        m = re.search(r"^MATRIX_E = \(([\d, ]+)\)", f.read(), re.M)
-    covered = {round_ep(int(e)) for e in m.group(1).split(",") if e.strip()}
-    assert dispatched == {12, 16, 32, 64}
-    assert dispatched == covered
 
 
 # ---- the trainer ABI's rejections that need no device ----------------------------------------------------------

@@ -13,10 +13,10 @@ from sparrowrecsys_b200.weights import init_aux_weights, init_weights
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 SPREAD_MULTIPLE = 4.0          # GPU-to-float64 distance allowed, in units of the float32-to-float64 distance
-# two EP = 32 cases need more (DESIGN.md section 4.20): after one step the AUGRU's gate kernels sit in Adam's epsilon
-# regime, where a gradient's last bits decide the update; on an NVIDIA H100 80GB HBM3 at 700 W augru_z_act/kernel
-# measured 4.4x the float32 spread at T = 50 and augru_z_input/kernel 6.4x at batch 4096
-CASE_MULTIPLE = {(32, 50, 12, 12): 5.0, (32, 5, 4096, 4096): 7.0}
+# the batch-4096 case at EP = 32 needs more (DESIGN.md section 4.20): after one step the AUGRU's gate kernels sit in
+# Adam's epsilon regime, where a gradient's last bits decide the update; on an NVIDIA H100 80GB HBM3 at 700 W
+# augru_z_input/kernel measured 6.4x the float32 spread at batch 4096
+CASE_MULTIPLE = {(32, 5, 4096, 4096): 7.0}
 
 
 def _weights(spec, seed):
@@ -70,13 +70,11 @@ def _check_close(got, w64, w32, what):
     print("worst spread ratio", what, worst)
 
 
-# (E, T, hidden, n_movies, batch, rows, epochs): every EP (12, 16, 32) at both edges, T from 1 to 50, odd hidden
-# widths, a tiny vocabulary; 1, 2, 10 and 100 steps
+# (E, T, hidden, n_movies, batch, rows, epochs): long horizons and large batches at the reference shape, 100 steps
+# of one row, 100 of 12 and 33 rows, one and ten of 4096; tests/test_fit_matrix.py holds every EP, hidden width,
+# history length and padding edge to the same rule
 MATRIX = [(12, 5, (128, 64), 3000, 1, 100, 1), (10, 5, (128, 64), 3000, 12, 1200, 1),
           (16, 5, (128, 64), 3000, 33, 3300, 1), (10, 5, (128, 64), 3000, 4096, 40960, 1),
-          (10, 5, (128, 64), 3000, 12, 12, 1), (10, 5, (128, 64), 3000, 12, 24, 1), (10, 5, (128, 64), 3000, 33, 330, 1),
-          (1, 2, (7, 5), 50, 12, 24, 1), (12, 5, (128, 64), 3000, 1, 2, 1), (13, 9, (33, 17), 3000, 33, 40, 1),
-          (16, 1, (128, 64), 3000, 12, 24, 1), (17, 5, (128, 64), 8, 12, 36, 2), (32, 50, (65, 31), 3000, 12, 12, 1),
           (32, 5, (128, 64), 3000, 4096, 4096, 1)]
 
 
