@@ -875,7 +875,8 @@ extern "C" int srs_sample_split_by_timestamp_host(const int64_t* timestamp, int6
   if (!rows || !part_counts || !split_timestamp) return failf(SRS_ERR_INVALID, "null output");
   for (int64_t i = 0; i < n; ++i)
     if (timestamp[i] < -(1ll << 53) || timestamp[i] > (1ll << 53))
-      return failf(SRS_ERR_INVALID, "timestamp %lld is not exact as a double", (long long)timestamp[i]);
+      return failf(SRS_ERR_INVALID, "timestamp %lld outside -2^53..2^53, where a double is exact",
+                   (long long)timestamp[i]);
   HostCall r;
   PROPAGATE(r.begin(device));
   const int nn = (int)n;

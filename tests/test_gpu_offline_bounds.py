@@ -1,18 +1,25 @@
 """Every case of tests/test_offline_bounds.py's `BOUNDS` on the device against its oracle, bit for bit, and a repeat
 run giving the same bits."""
+import ctypes as C
+
 import numpy as np
 import pytest
 
 from oracle import als_cext as X
+from oracle import als_implicit_cext as XI
+from oracle import feature_job as FQ
 from oracle import feature_eng as F
 from oracle import graphemb as G
 from oracle import item2vec_cext as IX
 from oracle import lsh as H
+from sparrowrecsys_b200 import _lib
 from sparrowrecsys_b200 import collab
 from sparrowrecsys_b200 import embedding as E
 from sparrowrecsys_b200 import featureeng as FE
+from sparrowrecsys_b200 import featurejob as FJ
 
-from test_offline_bounds import BOUNDS, data, graph_transitions, i2v_oracle_input
+from test_offline_bounds import (BOUNDS, data, discretizer_splits, graph_transitions, i2v_oracle_input,
+                                 indexer_oracle, indexer_tokens, labels_csr, quantiles)
 
 pytestmark = pytest.mark.gpu
 
@@ -151,8 +158,134 @@ def _fe_oracle(d):
     return [out[c] for c in F.COLUMNS]
 
 
+def _p(a):
+    return a.ctypes.data
+
+
+def _fj_device(d):
+    op = d["op"]
+    if op == "quantile":
+        return [FJ.approx_quantile(d["values"], d["probs"], d["eps"])]
+    if op == "discretizer":
+        out = []
+        for N in d["buckets"]:
+            bz, b = FJ.QuantileDiscretizer(N, d["eps"]).fit_transform(d["values"])
+            out += [bz.splits, b]
+        return out
+    if op == "bucketize":
+        return [FJ.Bucketizer(s).transform(v) for s, v in d["runs"]]
+    if op == "scaler":
+        out = []
+        for v, fit in d["fits"]:
+            if fit is None:
+                m, x = FJ.MinMaxScaler().fit_transform(v)
+                out += [x, np.array([m.original_min, m.original_max])]
+            else:
+                out.append(FJ.MinMaxScalerModel(*fit).transform(v))
+        return out
+    if op == "ratings":
+        r = FJ.rating_features({"movieId": d["movie"], "rating": d["half"] * 0.5})
+        return [r[c] for c in ("movieId", "ratingCount", "avgRating", "ratingVar")]
+    if op == "indexer":                                # the raw ABI on word hashes: no 2^20 Python strings
+        tok, h = indexer_tokens(d), d["hashes"]
+        lw, lc = np.zeros(len(h), np.int32), np.zeros(len(h), np.int64)
+        _lib.check(_lib.load().srs_string_indexer_host(_p(tok), tok.size, _p(h), len(h), 0, _p(lw), _p(lc)))
+        return [lw, lc]
+    if op == "multi_hot":
+        r = FJ.multi_hot(d["ids"], d["genres"])
+        return [np.array(r["labels"]), r["counts"], r["movieId"], r["offsets"], r["indices"]]
+    if op == "split":
+        return [FJ.sample_split_rows(n, seed, frac, w) for n, seed, frac, w in d["runs"]]
+    if op == "ts_split":
+        out = []
+        for ts, seed, frac, eps in d["runs"]:
+            tr, te, split = FJ.sample_split_rows_by_timestamp(ts, seed, frac, eps)
+            out.append([tr, te, np.array([split])])
+        return out
+    raise KeyError(op)
+
+
+def _fj_oracle(d):
+    op = d["op"]
+    if op == "quantile":
+        return [quantiles(d["values"], d["probs"], d["eps"])]
+    if op == "discretizer":
+        out = []
+        for N in d["buckets"]:
+            s = discretizer_splits(d["values"], N, d["eps"])
+            out += [s, FQ.bucketize(s, d["values"])]
+        return out
+    if op == "bucketize":
+        return [FQ.bucketize(s, v) for s, v in d["runs"]]
+    if op == "scaler":
+        out = []
+        with np.errstate(over="ignore", invalid="ignore"):
+            for v, fit in d["fits"]:
+                if fit is None:
+                    x, lo, hi = FQ.min_max_scale(v)
+                    out += [x, np.array([lo, hi])]
+                else:
+                    out.append(FQ.min_max_scale(v, *fit)[0])
+        return out
+    if op == "ratings":
+        ids, n, avg, var = FQ.rating_features(d["movie"], d["half"])
+        return [ids, n, avg, var]
+    if op == "indexer":
+        return list(indexer_oracle(d))
+    if op == "multi_hot":
+        labels, counts, ids, off, idx = FQ.multi_hot(d["ids"], d["genres"])
+        return [np.array(labels), np.array(counts, np.int64), ids, off.astype(np.int32), idx]
+    if op == "split":
+        return [FQ.split_samples(n, seed, frac, w) for n, seed, frac, w in d["runs"]]
+    if op == "ts_split":
+        out = []
+        for ts, seed, frac, eps in d["runs"]:
+            tr, te, split = FQ.split_samples_by_timestamp(ts, seed, frac, eps)
+            out.append([tr.astype(np.int64), te.astype(np.int64), np.array([split])])
+        return out
+    raise KeyError(op)
+
+
+def _implicit_device(d):
+    r = {"userId": d["u"], "movieId": d["m"], "rating": d["r"]}
+    return [list(_fit_tuple(collab.als(r, implicit_prefs=True, **f))) for f in d["fits"]]
+
+
+def _fit_tuple(m):
+    return m.user_ids, m.user_factors, m.item_ids, m.item_factors
+
+
+def _implicit_oracle(d):
+    return [list(XI.fit(d["u"], d["m"], d["r"], **f)) for f in d["fits"]]
+
+
+def _ranking_device(d):
+    out = []
+    for pred, labels, ks, *_ in d["runs"]:
+        off, lab = labels_csr(labels)
+        n, L = pred.shape
+        for k in ks:
+            per, means = np.zeros((3, n)), np.zeros(3)
+            _lib.check(_lib.load().srs_ranking_metrics_host(_p(pred), n, L, _p(off), _p(lab if lab.size else off),
+                                                            k, 0, _p(per), _p(means)))
+            out += [means, per]
+    return out
+
+
+def _ranking_oracle(d):
+    out = []
+    for pred, labels, ks, *_ in d["runs"]:
+        off, lab = labels_csr(labels)
+        for k in ks:
+            means, per = XI.ranking_metrics(pred, off, lab, k)
+            out += [means, per]
+    return out
+
+
 RUNS = {"item2vec": (_i2v_device, _i2v_oracle), "graph": (_graph_device, _graph_oracle),
-        "lsh": (_lsh_device, _lsh_oracle), "featureeng": (_fe_device, _fe_oracle)}
+        "lsh": (_lsh_device, _lsh_oracle), "featureeng": (_fe_device, _fe_oracle),
+        "featurejob": (_fj_device, _fj_oracle), "als_implicit": (_implicit_device, _implicit_oracle),
+        "ranking_metrics": (_ranking_device, _ranking_oracle)}
 
 
 def _runs(name):

@@ -1,17 +1,20 @@
-"""The offline jobs at their bounds and tile edges (csrc/item2vec.cu, graphemb.cu, lsh.cu, als.cu, featureeng.cu).
+"""The offline jobs at their bounds and tile edges (csrc/item2vec.cu, graphemb.cu, lsh.cu, als.cu with implicit ALS
+and RankingMetrics, featureeng.cu, featurejob.cu, and hostcall.h's grid cap).
 
 `BOUNDS` names one case per (job, edge).  Each case builds its inputs here; its `reach` shows from the oracle alone,
 with no device, that the inputs reach the edge the case names, and returns the (bound, value) pairs it reaches.
 tests/test_gpu_offline_bounds.py runs every case on the device against its oracle, bit for bit, twice.
 
 The bounds come from the kernels' own constants: `test_every_bound_has_a_case` parses them, so a changed constant
-without a case at its new value fails.  The size bounds (21 000 000 ratings, kMaxWalkWords) are covered by the
-rejection one past them; the deepest Huffman case is the largest run.
+without a case at its new value fails.  The size bounds (21 000 000 ratings, kMaxWalkWords, featurejob.cu's
+kMaxValues) are covered by the rejection one past them; the deepest Huffman case is the largest run of the first
+jobs, and featurejob.cu's rating features run at 21 000 000 ratings and its StringIndexer at kMaxTokens.
 """
 from __future__ import annotations
 
 import ctypes as C
 import functools
+import math
 import os
 import re
 from typing import Callable, NamedTuple
@@ -20,6 +23,8 @@ import numpy as np
 import pytest
 
 from oracle import als as A
+from oracle import als_implicit as XP
+from oracle import feature_job as FQ
 from oracle import feature_eng as F
 from oracle import graphemb as G
 from oracle import item2vec as I
@@ -33,7 +38,8 @@ CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
 
 # ---- the kernels' constants --------------------------------------------------------------------------------------
 def constants(*files):
-    """name -> value of every `constexpr` integer in the given csrc files (simple integer expressions)."""
+    """name -> value of every `constexpr` integer in the given csrc files (simple integer expressions).  A name
+    defined in two files with two values raises ValueError rather than letting the last file win."""
     out = {}
     for f in files:
         with open(os.path.join(CSRC, f)) as fh:
@@ -44,13 +50,17 @@ def constants(*files):
             for k in sorted(out, key=len, reverse=True):
                 e = re.sub(r"\b%s\b" % k, str(out[k]), e)
             try:
-                out[name] = int(eval(e, {"__builtins__": {}}))
+                v = int(eval(e, {"__builtins__": {}}))
             except (NameError, SyntaxError):
-                pass
+                continue
+            if name in out and out[name] != v:
+                raise ValueError("%s is %d in %s but %d in an earlier file" % (name, v, f, out[name]))
+            out[name] = v
     return out
 
 
-K = constants("als.cu", "lsh.cu", "item2vec.cu", "featureeng.cu", "graphemb.cu")
+RATING_BOUND_FILES = ("als.cu", "featureeng.cu", "item2vec.cu", "featurejob.cu")
+K = constants("als.cu", "lsh.cu", "item2vec.cu", "featureeng.cu", "graphemb.cu", "featurejob.cu", "hostcall.h")
 
 
 class Case(NamedTuple):
@@ -470,6 +480,578 @@ def _fe_top_reach(d):
     return {("kMaxMovieSlots", top)}
 
 
+# ---- the FeatureEngineering job and the sample split (featurejob.cu) ---------------------------------------------
+# The values the cases are built at.  Literals rather than K: a constant moved without a case at its new value
+# fails test_every_bound_has_a_case.
+FJ_PROBS, FJ_BUCKETS, FJ_WORDS, FJ_TOKENS = 1 << 16, 10000, 1 << 20, (1 << 29) - 1
+FJ_WORDS_PER_ROW, FJ_PARTS, FJ_TOP_MOVIE, FJ_RATINGS = 256, 64, (1 << 24) - 1, 21000000
+GRID_BLOCKS = 132 * 64
+STRIDE_256, STRIDE_128 = GRID_BLOCKS * 256, GRID_BLOCKS * 128     # elements one grid covers at 256 / 128 threads
+SPLITS_THREADS = 1024                                              # fj_splits_kernel's one block
+# the tightest (n, eps) of the sweep in test_the_compress_segments_stay_under_their_cap.  2.0 * eps * n is
+# 1679.9999999999998 in double, so the host's floor(2 eps n) is 1 679 and its cap 1 689; the walk takes 1 682
+# segments, 3 more than that floor (2 more than the exact 1 680).  A cap without its slack of 8 (1 681) fails here.
+# At (3e6, 2e-4), where 2 eps n rounds to exactly 1 200, the walk's 1 202 segments fit even that cap.
+TIGHT_N, TIGHT_EPS = 3000000, 0.00028
+
+
+def seg_cap(n, eps):
+    """quantiles_of_keys' bound on fj_compress_kernel's segments."""
+    return min(n, int(2.0 * eps * n) + 8) + 2
+
+
+def compress_segments(n, eps):
+    """fj_compress_kernel's walk (oracle.feature_job.one_summary_segments), counted: (segments, heads)."""
+    e2 = 2.0 * float(eps)
+    T = e2 * n
+
+    def delta(j):
+        return 0 if j == 0 or j == n - 1 else int(math.floor(e2 * float(j + 1)))
+
+    ns = heads = 0
+    j = n - 1
+    while True:
+        d = delta(j)
+        x = T - float(d + 2)
+        t = int(math.ceil(x)) if x > 0 else 0
+        if 1 <= j <= n - 2 and t <= j - 1:
+            a, b = 1, j
+            while a < b:
+                mid = (a + b) // 2
+                if delta(mid) >= d:
+                    b = mid
+                else:
+                    a = mid + 1
+            count, stride = (j - max(a, t + 1)) // (t + 1) + 1, t + 1
+        else:
+            count, stride = 1, min(t, max(j - 1, 0)) + 1
+        ns, heads = ns + 1, heads + count
+        j -= count * stride
+        if j < 1:
+            return ns, heads
+
+
+def query_many(sampled, n, probs, eps):
+    """FQ.query_sampled at many probabilities, vectorised over the samples: the first sample but the last with
+    maxRank - targetError <= rank <= minRank + targetError, rank = ceil(p n), targetError = ceil(eps n)."""
+    v = np.array([s[0] for s in sampled], np.float64)
+    g = np.array([s[1] for s in sampled], np.int64)
+    d = np.array([s[2] for s in sampled], np.int64)
+    minr = np.cumsum(g)[:-1].astype(np.float64)
+    maxr = minr + d[:-1]
+    target = float(math.ceil(eps * n))
+    out = np.empty(len(probs))
+    for i, p in enumerate(np.asarray(probs, np.float64).tolist()):
+        if p <= eps:
+            out[i] = v[0]
+        elif p >= 1 - eps:
+            out[i] = v[-1]
+        else:
+            rank = float(math.ceil(p * n))
+            ok = (maxr - target <= rank) & (rank <= minr + target)
+            out[i] = v[int(np.argmax(ok))] if ok.any() else v[-1]
+    return out
+
+
+def quantiles(values, probs, eps):
+    """FQ.one_summary_quantiles, its query vectorised (query_many)."""
+    _, sampled, n = FQ.one_summary_samples(values, eps)
+    return query_many(sampled, n, probs, eps)
+
+
+def discretizer_splits(values, num_buckets, eps):
+    """FQ.discretizer_splits over `quantiles`."""
+    q = quantiles(values, FQ.discretizer_probabilities(num_buckets), eps)
+    q[0], q[-1] = -np.inf, np.inf
+    _, first = np.unique(q.view(np.uint64), return_index=True)
+    s = q[np.sort(first)]
+    assert len(s) >= 3 and np.all(s[:-1] < s[1:])
+    return s
+
+
+def _fj_probs():
+    """65 536 probabilities on 200 000 values with ties: 0, eps, 1 - eps, 1 and the doubles next to them, p with p n
+    an integer, the rest uniform."""
+    rng = np.random.default_rng(41)
+    n, eps = 200000, 0.01
+    x = np.round(rng.standard_normal(n) * 50)                         # about 700 distinct values
+    edges = []
+    for p in (0.0, eps, 1 - eps, 1.0):
+        edges += [p, np.nextafter(p, -1.0), np.nextafter(p, 2.0)]
+    edges = [p for p in edges if 0.0 <= p <= 1.0]
+    exact = np.arange(1, 2000) * 97 / n                                # p n = 97 k
+    rest = rng.random(FJ_PROBS - len(edges) - len(exact))
+    return dict(op="quantile", values=x, eps=eps, probs=np.r_[edges, exact, rest])
+
+
+def _fj_quantile_reach(d):
+    n, eps, p = len(d["values"]), d["eps"], d["probs"]
+    ns, heads = compress_segments(n, eps)
+    cap = seg_cap(n, eps)
+    assert ns <= cap
+    got = {("kMaxProbs", len(p)), ("segments_margin", cap - ns)}
+    if len(p) >= 2 * 128:
+        assert {0.0, 1.0, eps, 1 - eps} <= set(p.tolist())
+        assert np.any((p * n == np.floor(p * n)) & (p > eps) & (p < 1 - eps))
+    if n > STRIDE_256:
+        got.add(("keys_stride", 1))
+    if heads > STRIDE_256:                                             # fj_expand_kernel runs over the heads
+        got.add(("expand_stride", 1))
+    if eps == 0.0:
+        assert heads == n - 1
+        got.add(("every_value_a_head", 1))
+    if (n, eps) == (TIGHT_N, TIGHT_EPS):
+        assert ns - int(2.0 * eps * n) == 3, ns
+        got.add(("tightest_segments", ns))
+    return got
+
+
+def _fj_tight():
+    x = np.random.default_rng(42).integers(0, 1 << 40, TIGHT_N).astype(np.float64)
+    return dict(op="quantile", values=x, eps=TIGHT_EPS, probs=np.r_[0.0, 0.001, 0.25, 0.5, 0.8, 0.999, 1.0])
+
+
+def _fj_stride():
+    """n = 3 000 000 at eps = 0: every value but the minimum a head, so the keys and the expansion stride."""
+    rng = np.random.default_rng(43)
+    x = rng.standard_normal(3000000)
+    x[:4] = [-0.0, 0.0, np.inf, -np.inf]
+    x[4:1000] = 1.5                                                   # a run of equal values
+    return dict(op="quantile", values=x, eps=0.0, probs=np.r_[0.0, 1e-7, 1 / 3, 0.5, 0.8, 1 - 1e-7, 1.0])
+
+
+def _fj_discretizer_passes():
+    """Distinct values, so the split count is nq: num_buckets giving nq = 1023, 1024 and 1025, FJ_BUCKETS, and N
+    near both ends of the range."""
+    x = np.random.default_rng(44).permutation(100000).astype(np.float64) * 0.5
+    nq = lambda N: len(FQ.discretizer_probabilities(N))
+    want = []
+    for target in (SPLITS_THREADS - 1, SPLITS_THREADS, SPLITS_THREADS + 1):
+        want.append(next(N for N in range(target - 2, target + 1) if nq(N) == target))
+    Ns = want + [2, 3, 4, 5, 11, 9990, 9997, 9998, 9999, FJ_BUCKETS]
+    return dict(op="discretizer", values=x, eps=2.5e-5, buckets=Ns)
+
+
+def _fj_discretizer_duplicates():
+    """FJ_BUCKETS buckets over 100 000 values of about 600 distinct (rounded log-normal counts): `distinct` drops
+    most of the 10 001 quantiles, well past the first 1024."""
+    x = np.round(np.exp(np.random.default_rng(45).standard_normal(100000) * 2.0))
+    return dict(op="discretizer", values=x, eps=2.5e-5, buckets=[FJ_BUCKETS, SPLITS_THREADS])
+
+
+def _fj_discretizer_reach(d):
+    got = set()
+    for N in d["buckets"]:
+        nq = len(FQ.discretizer_probabilities(N))
+        s = discretizer_splits(d["values"], N, d["eps"])
+        got |= {("kMaxBuckets", N), ("nq", nq)}
+        if len(np.unique(d["values"])) == len(d["values"]):
+            assert len(s) == nq, (N, nq, len(s))
+        else:
+            dup = nq - len(s)
+            assert dup > SPLITS_THREADS or N < FJ_BUCKETS, dup
+            got.add(("dup_past_threads", int(dup > SPLITS_THREADS)))
+    return got
+
+
+def _fj_bucketize():
+    """FJ_BUCKETS + 1 splits (-inf, -0.0 and +inf among them); values on every split, on -0.0 and 0.0, at +-inf and
+    at the last split; more than one grid of values.  A second, small split set holds 0.0 instead of -0.0."""
+    rng = np.random.default_rng(46)
+    inner = np.sort(rng.choice(np.arange(-50000, 50000), FJ_BUCKETS - 1, replace=False)).astype(np.float64) / 8
+    inner[np.argmin(np.abs(inner))] = -0.0
+    splits = np.r_[-np.inf, inner, np.inf]
+    assert np.all(splits[:-1] < splits[1:]) and (np.signbit(splits) & (splits == 0)).any()
+    n = STRIDE_256 + 300001
+    v = rng.uniform(-7000, 7000, n)
+    v[:len(splits)] = splits
+    v[len(splits):len(splits) + 6] = [-0.0, 0.0, np.inf, -np.inf, -0.0, np.inf]
+    rng.shuffle(v)
+    small = np.array([-np.inf, -1.0, 0.0, 2.5, np.inf])
+    sv = np.array([-0.0, 0.0, -1.0, 2.5, np.inf, -np.inf, 1e300, -1e300, 3.0])
+    return dict(op="bucketize", runs=[(splits, v), (small, sv)])
+
+
+def _fj_bucketize_reach(d):
+    (splits, v), _ = d["runs"]
+    assert len(splits) == FJ_BUCKETS + 1 and np.isin(splits, v).all() and len(v) > STRIDE_256
+    b = FQ.bucketize(splits, v)
+    assert b.max() == len(splits) - 2 and b.min() == 0
+    return {("n_splits", len(splits)), ("bucket_stride", 1)}
+
+
+def _fj_scaler():
+    """-0.0 and 0.0 the two smallest of more than one grid of values; +-1e308 (a range of +inf: 0 and NaN); a fitted
+    min / max with values outside it."""
+    rng = np.random.default_rng(47)
+    n = STRIDE_256 + 12345
+    a = rng.uniform(0, 5, n)
+    a[[17, 4000]] = [-0.0, 0.0]
+    b = np.r_[1e308, -1e308, 0.0, 5.0, -1e308, 1e308, 1.0]
+    return dict(op="scaler", fits=[(a, None), (b, None), (a, (1.0, 3.5)), (b, (2.0, 2.0))])
+
+
+def _fj_scaler_reach(d):
+    a = d["fits"][0][0]
+    lo2 = a[np.argsort(FQ._total_order_keys(a), kind="stable")[:2]]
+    assert len(a) > STRIDE_256
+    with np.errstate(over="ignore", invalid="ignore"):
+        s = FQ.min_max_scale(d["fits"][1][0])[0]
+    assert np.isnan(s).any() and (s == 0).any()
+    return {("scale_stride", 1), ("scale_overflow", 1), ("signed_zero_min", int(np.signbit(lo2).tolist() == [True, False] and not lo2.any()))}
+
+
+# one movie of FJ_RATINGS - 1 ratings, a at 1 half-star and b at 10, and a one-rating movie at id 0.  Q = 81 a b is
+# below 2^53, but n S2 and S1^2 are not: Q formed in double - both products rounded, or either one fused (an FMA) -
+# gives another variance at this split
+RATING_SPLIT = (10500001, 10499998)
+
+
+def double_q_forms(N, S1, S2):
+    """Q = N S2 - S1^2 with double products: both rounded, and each of the two fused forms."""
+    both = float(N) * float(S2) - float(S1) * float(S1)
+    return both, float(N * S2 - int(float(S1) * float(S1))), float(int(float(N) * float(S2)) - S1 * S1)
+
+
+def _fj_ratings():
+    a, b = RATING_SPLIT
+    movie = np.r_[np.int32(0), np.full(a + b, 7, np.int32)]
+    half = np.r_[np.int8(6), np.ones(a, np.int8), np.full(b, 10, np.int8)]
+    p = np.random.default_rng(48).permutation(len(movie))
+    return dict(op="ratings", movie=movie[p], half=half[p])
+
+
+def _fj_ratings_reach(d):
+    m, h = d["movie"].astype(np.int64), d["half"].astype(np.int64)
+    n, s1, s2 = np.bincount(m), np.bincount(m, h).astype(np.int64), np.bincount(m, h * h).astype(np.int64)
+    N, S1, S2 = int(n[7]), int(s1[7]), int(s2[7])
+    Q = N * S2 - S1 * S1
+    assert Q == 81 * RATING_SPLIT[0] * RATING_SPLIT[1] and Q < 2 ** 53
+    den = float(4 * N * (N - 1))
+    assert all(float(Q) / den != q / den for q in double_q_forms(N, S1, S2))
+    assert np.isnan(FQ.rating_features(m, h)[3][0])                    # one rating: a null variance
+    return {("kMaxRatings", len(m)), ("rating_q_past_double", 1)}
+
+
+def _java_hash(s):
+    return F.java_string_hash(s)
+
+
+def trie_keys(hashes):
+    """FQ.trie_order_key, vectorised over int32 hashes."""
+    h = np.asarray(hashes, np.int64).astype(np.uint32).astype(np.uint64)
+    m = np.uint64(0xFFFFFFFF)
+    h = (h + (~(h << np.uint64(9)) & m)) & m
+    h ^= h >> np.uint64(14)
+    h = (h + (h << np.uint64(4))) & m
+    h ^= h >> np.uint64(10)
+    k = np.zeros_like(h)
+    for level in range(7):
+        k = (k << np.uint64(5)) | ((h >> np.uint64(5 * level)) & np.uint64(31))
+    return k
+
+
+def _fj_words():
+    """FJ_WORDS words: the first 4096 real strings, the rest random hashes with distinct trie keys; counts 1 and 2
+    (ties everywhere, so the trie order decides)."""
+    rng = np.random.default_rng(49)
+    strs = ["w%04d" % i for i in range(4096)]
+    h = np.array([_java_hash(s) for s in strs], np.int64)
+    extra = rng.integers(-2 ** 31, 2 ** 31, 2 * FJ_WORDS)
+    allh = np.r_[h, extra]
+    _, first = np.unique(trie_keys(allh), return_index=True)
+    keep = np.sort(first)
+    assert keep[:4096].tolist() == list(range(4096))
+    hashes = allh[keep[:FJ_WORDS]].astype(np.int32)
+    counts = rng.integers(1, 3, FJ_WORDS)
+    tok = rng.permutation(np.repeat(np.arange(FJ_WORDS, dtype=np.int32), counts))
+    return dict(op="indexer", tok=tok, hashes=hashes, strs=strs)
+
+
+def _fj_count_field():
+    """Two words, counts 2^29 - 2 and 1: FJ_TOKENS tokens, the count field full.  The lone word's trie key is the
+    smaller, so only the count field puts it second.  The tokens are built by the run (2 GiB)."""
+    h = np.array([_java_hash("Drama"), _java_hash("Film-Noir")], np.int32)
+    if trie_keys(h)[1] > trie_keys(h)[0]:
+        h = h[::-1].copy()
+    return dict(op="indexer", counts=[FJ_TOKENS - 1, 1], hashes=h, lone_at=123456789)
+
+
+def indexer_tokens(d):
+    if "tok" in d:
+        return d["tok"]
+    tok = np.zeros(sum(d["counts"]), np.int32)
+    tok[d["lone_at"]] = 1
+    return tok
+
+
+def indexer_oracle(d):
+    """The label order, (-count, trie key): FQ.string_indexer_labels' sort, on hashes."""
+    cnt = np.bincount(d["tok"], minlength=len(d["hashes"])) if "tok" in d else np.array(d["counts"], np.int64)
+    order = np.lexsort((trie_keys(d["hashes"]), -cnt)).astype(np.int32)
+    return order, cnt[order].astype(np.int64)
+
+
+def _fj_indexer_reach(d):
+    W, h = len(d["hashes"]), d["hashes"]
+    assert len(np.unique(trie_keys(h))) == W
+    sub = np.arange(0, 4096 if "strs" in d else W)
+    ks = trie_keys(h[sub])
+    assert ks.tolist() == [FQ.trie_order_key(int(x)) for x in h[sub].tolist()]
+    if "strs" in d:
+        assert FQ.hash_trie_keys(d["strs"]) == [d["strs"][i] for i in np.argsort(ks)]
+        cnt = np.bincount(d["tok"])
+        assert set(cnt.tolist()) == {1, 2}
+        return {("kMaxWords", W)}
+    assert sum(d["counts"]) == FJ_TOKENS and np.argmin(trie_keys(h)) == 1
+    return {("kMaxTokens", sum(d["counts"]))}
+
+
+def _fj_multi_hot():
+    """One movie of FJ_WORDS_PER_ROW genres listed in descending label order (fj_csr_kernel's insertion sort shifts
+    every element); 2 171 136 one-genre movies and their words, more than one grid at 256 threads (so fj_hist,
+    fj_row_iota, fj_row_len and fj_csr_kernel all stride), ids 0 and FJ_TOP_MOVIE."""
+    words = ["g%03d" % i for i in range(FJ_WORDS_PER_ROW)]
+    per = 66 * (np.arange(FJ_WORDS_PER_ROW) + 1)                      # word w in 66 (w + 1) one-genre movies
+    one = np.repeat(np.arange(FJ_WORDS_PER_ROW), per)
+    rng = np.random.default_rng(50)
+    n = len(one) + 1
+    ids = rng.choice(FJ_TOP_MOVIE - 1, n, replace=False) + 1
+    ids[:2] = [0, FJ_TOP_MOVIE]
+    genres = ["|".join(words)] + [words[w] for w in one.tolist()]      # the big movie: labels 255, 254, ..., 0
+    p = rng.permutation(n)
+    return dict(op="multi_hot", ids=ids[p].astype(np.int32), genres=[genres[i] for i in p.tolist()])
+
+
+def _fj_multi_hot_reach(d):
+    lens = np.array([g.count("|") + 1 for g in d["genres"]])
+    big = d["genres"][int(np.argmax(lens))].split("|")
+    labels, counts = FQ.string_indexer_labels([w for g in d["genres"] for w in g.split("|")])
+    index = {w: k for k, w in enumerate(labels)}
+    lab = [index[w] for w in big]
+    assert lab == sorted(lab, reverse=True) and len(set(counts)) == len(counts)
+    assert {0, FJ_TOP_MOVIE} <= set(d["ids"].tolist())
+    got = {("kMaxWordsPerRow", int(lens.max())), ("kMaxMovieId", FJ_TOP_MOVIE), ("kMaxMovieId", 0)}
+    if len(d["ids"]) > STRIDE_128:
+        got.add(("csr_stride", 1))
+    if len(d["ids"]) > STRIDE_256:
+        got.add(("row_stride", 1))                                    # fj_row_iota_kernel, fj_row_len_kernel
+    if lens.sum() > STRIDE_256:
+        got.add(("hist_stride", 1))                                   # fj_hist_kernel over the words
+    return got
+
+
+def _fj_split():
+    """FJ_PARTS weights from 1e-300 to 1e300, some 0; fraction 0 and 1; n = 1."""
+    w = 10.0 ** np.linspace(-300, 300, FJ_PARTS)
+    w[[3, 20, 40, 63]] = 0.0
+    w[[10, 50]] = [1.0, 1e300]
+    return dict(op="split", runs=[(300000, 11, 0.5, w), (300000, 12, 1.0, w), (300000, 13, 0.0, w),
+                                  (1, 14, 1.0, w), (200000, 15, 1.0, np.r_[1.0, 0.0, 2.0, 1e-300])])
+
+
+def _fj_split_reach(d):
+    got = {("kMaxParts", max(len(w) for *_, w in d["runs"]))}
+    for n, seed, frac, w in d["runs"]:
+        parts = FQ.split_samples(n, seed, frac, w)
+        assert all(len(p) == 0 for p, x in zip(parts, w) if x == 0)
+        got |= {("split_fraction", frac), ("split_n", min(n, 2))}
+        if frac == 0:
+            assert sum(len(p) for p in parts) == 0
+    return got
+
+
+def _fj_ts_split():
+    """Timestamps at +-2^53, negative; all equal (the test part empty); exactly one sampled row."""
+    rng = np.random.default_rng(51)
+    ts = rng.integers(-10 ** 12, 10 ** 12, 100000)
+    ts[:6] = [2 ** 53, -2 ** 53, 2 ** 53, -1, 0, 2 ** 53 - 1]
+    ts[6:5000] = 2 ** 53
+    u = FQ.stream_uniforms(61, 0, 1000)
+    one = float(np.sort(u)[1])                                         # exactly the smallest uniform passes
+    return dict(op="ts_split", runs=[(ts, 17, 0.5, 0.01), (ts, 18, 1.0, 0.0), (np.full(5000, -77), 19, 0.3, 0.05),
+                                     (np.arange(1000) - 500, 61, one, 0.05)])
+
+
+def _fj_ts_reach(d):
+    got = set()
+    for ts, seed, frac, eps in d["runs"]:
+        tr, te, split = FQ.split_samples_by_timestamp(ts, seed, frac, eps)
+        if len(tr) + len(te) == 1:
+            got.add(("ts_one_sampled", 1))
+        if len(set(ts.tolist())) == 1:
+            assert len(te) == 0
+            got.add(("ts_all_equal", 1))
+        if np.abs(ts).max() == 2 ** 53:
+            assert (ts < 0).any()
+            got.add(("ts_2_53", 1))
+    return got
+
+
+# ---- implicit ALS and RankingMetrics (als.cu) --------------------------------------------------------------------
+YTY_MEMBERS = (0, 1, 31, 32, 33, 64, 65, 2, 3, 5)                     # entities per YtY block (raw id mod blocks)
+
+
+def _block_ids(counts, base):
+    B = K["kYtyBlocks"]
+    assert len(counts) == B, (len(counts), B)
+    return np.concatenate([base + b + B * np.arange(c) for b, c in enumerate(counts)]).astype(np.int32)
+
+
+def _yty_tiles():
+    """Users and movies with YTY_MEMBERS entities in the kYtyBlocks YtY blocks; ranks 15 (nA 120, one tile), 16 (136, two)
+    and 64 (2080, 17).  Ratings include 0 and negatives."""
+    rng = np.random.default_rng(52)
+    users, movies = _block_ids(YTY_MEMBERS, 1000), _block_ids(YTY_MEMBERS[::-1], 5000)
+    u = np.r_[np.repeat(users, 6), rng.choice(users, len(movies))]
+    m = np.r_[rng.choice(movies, 6 * len(users)), movies]
+    r = rng.choice([-1.0, 0.0, 0.5, 1.0, 2.5, 4.0, 5.0], len(u)).astype(np.float32)
+    return dict(u=u.astype(np.int32), m=m.astype(np.int32), r=r,
+                fits=[dict(rank=k, max_iter=2, reg_param=0.05, alpha=a, seed=k) for k, a in ((15, 1.0), (16, 40.0),
+                                                                                            (64, 1.0))])
+
+
+def _yty_reach(d):
+    B = K["kYtyBlocks"]
+    got = set()
+    for ids, want in ((d["u"], YTY_MEMBERS), (d["m"], YTY_MEMBERS[::-1])):
+        per = np.bincount(np.unique(ids) % B, minlength=B)
+        assert per.tolist() == list(want), per
+        got |= {("yty_members", int(c)) for c in per} | {("kYtyBlocks", len(per))}
+    for f in d["fits"]:
+        nA = f["rank"] * (f["rank"] + 1) // 2
+        got.add(("yty_tiles", -(-nA // K["kYtyThreads"])))
+    return got
+
+
+def _implicit_chunks():
+    """Users and movies with 31, 32, 33, 64 and 65 ratings; zero and negative ratings at positions 0, 31 and 32 of
+    the 33- and 65-rating entities.  At alpha 0 and 40."""
+    counts = CHUNK_COUNTS[1:]
+    u, m, r = [], [], []
+    rng = np.random.default_rng(53)
+    for n, mv in zip(counts, range(2001, 2006)):
+        for usr in range(1, n + 1):
+            u.append(usr), m.append(mv), r.append(rng.integers(1, 11) / 2.0)
+    for n, usr in zip(counts, range(501, 506)):
+        for mv in range(1, n + 1):
+            u.append(usr), m.append(mv), r.append(rng.integers(1, 11) / 2.0)
+    u, m, r = np.array(u), np.array(m), np.array(r)
+    for usr, vals in ((505, (0.0, -2.0, 0.0)), (503, (-1.0, 0.0, -0.5))):
+        for mv, x in zip((1, 32, 33), vals):
+            r[(u == usr) & (m == mv)] = x
+    for mv, vals in ((2005, (-1.0, 0.0, -3.0)), (2003, (0.0, -4.0, 0.0))):
+        for usr, x in zip((1, 32, 33), vals):
+            r[(m == mv) & (u == usr)] = x
+    fits = [dict(rank=k, max_iter=2, reg_param=0.05, alpha=a, seed=k) for k in (8, 33) for a in (0.0, 40.0)]
+    return dict(u=u.astype(np.int32), m=m.astype(np.int32), r=r.astype(np.float32), fits=fits)
+
+
+def _implicit_chunks_reach(d):
+    _, _, by_movie, by_user = A.layouts(d["u"], d["m"], d["r"])
+    c = K["kChunk"]
+    got = {("implicit_alpha", f["alpha"]) for f in d["fits"]}
+    for side, (off, src, rr) in (("user", by_user), ("movie", by_movie)):
+        cnt = np.diff(off)
+        assert set(CHUNK_COUNTS[1:]) <= set(cnt.tolist()), side
+        got |= {("implicit_chunk", int(x)) for x in CHUNK_COUNTS[1:]}
+        for e in np.flatnonzero(np.isin(cnt, (c + 1, 2 * c + 1))):
+            rs = rr[off[e]:off[e + 1]]
+            nonpos = set(np.flatnonzero(rs <= 0).tolist())
+            assert {0, c - 1, c} <= nonpos, (side, e, nonpos)
+            assert (rs < 0).any() and (rs == 0).any()
+            got |= {("implicit_nonpos_at", p) for p in (0, c - 1, c)}
+            got |= {("implicit_n_plus", (j // c, int((rs[j:j + c] > 0).sum()))) for j in range(0, len(rs), c)}
+    return got
+
+
+RANK_L = (0, 1, 31, 32, 33, 64, 65)
+
+
+RANK_HITS = (0, 31, 32, 63, 64)                                      # either side of a 32-wide ballot
+
+
+def _ranking_lists():
+    """Per L in RANK_L, queries whose label sets have 1, 31, 32, 33, L + 3 and 40 distinct ids, one of 100 copies
+    of one id, and one empty.  Every set of two or more ids holds the predictions at RANK_HITS (those below L) and
+    at L - 1, among misses: its other ids are a few more predictions and ids never predicted.  The one-id sets are
+    the prediction at L - 1.  Per L, k in 1, L - 1, L, L + 1 and past every walk."""
+    rng = np.random.default_rng(54)
+    runs = []
+    for L in RANK_L:
+        named = sorted({i for i in RANK_HITS if i < L} | ({L - 1} if L else set()))
+        labels, preds = [], []
+        for q, size in enumerate((1, 31, 32, 33, L + 3, 100, 0, 40)):
+            pred = 100000 * (q + 1) + rng.permutation(1000)[:L]
+            if size == 0:
+                lab = pred[:0]
+            elif size in (1, 100):
+                lab = np.full(size, pred[L - 1] if L else 7)
+            else:
+                others = [i for i in rng.permutation(L)[:size // 4].tolist() if i not in named]
+                hit = pred[named + others][:size]
+                lab = np.r_[hit, 50 + np.arange(size - len(hit))]           # never predicted: misses
+                lab = np.r_[lab, lab[:size // 4]]                         # duplicates in the list
+            preds.append(pred), labels.append(rng.permutation(lab).astype(np.int32))
+        ks = sorted({k for k in (1, L - 1, L, L + 1, 200) if k >= 1})
+        runs.append((np.array(preds, np.int32).reshape(len(preds), L), labels, ks, named))
+    return dict(runs=runs)
+
+
+def labels_csr(labels):
+    off = np.zeros(len(labels) + 1, np.int32)
+    off[1:] = np.cumsum([len(x) for x in labels])
+    return off, (np.concatenate(labels) if labels else np.zeros(0)).astype(np.int32)
+
+
+def _ranking_lists_reach(d):
+    got = set()
+    for pred, labels, ks, named in d["runs"]:
+        L = pred.shape[1]
+        got.add(("rank_L", L))
+        for row, lab in zip(pred.tolist(), labels):
+            labset = set(lab.tolist())
+            dist = len(labset)
+            hits = [i for i, x in enumerate(row) if x in labset]
+            if len(lab) == 100 and dist == 1:
+                got.add(("rank_repeated_label", 100))
+            for k in ks:
+                steps = max(L, min(max(L, dist), k)) if dist else 0
+                got.add(("rank_steps", steps))
+            if dist == 0 or L == 0:
+                continue
+            if dist == 1:
+                assert hits == [L - 1], hits
+            else:
+                assert set(named) <= set(hits) and (len(hits) < L or L == 1), (L, dist, hits)
+                for p in hits:                                        # a hit with a miss before it
+                    if p == 0 or len(set(range(p)) - set(hits)):
+                        got.add(("rank_hit_at", p))
+            for k in ks:                                              # the walks see the hits
+                _, ndcg, ap = XP.query_metrics(row, lab, k)
+                assert ap > 0 and (ndcg > 0) == (min(hits) < min(max(L, dist), k)), (L, dist, k)
+            got.add(("rank_distinct", dist if dist <= 33 else "past_L" if dist > L else dist))
+        for k in ks:
+            got.add(("rank_k_vs_L", k - L if abs(k - L) <= 1 else "past" if k > 2 * L + 3 else "other"))
+    return got
+
+
+def _ranking_grid():
+    """67 585 and 140 000 queries: warps take a second and a third query (grid of 8448 blocks of 8 warps)."""
+    rng = np.random.default_rng(55)
+    runs = []
+    for n in (GRID_BLOCKS * K["kRankWarps"] + 1, 140000):
+        pred = rng.integers(0, 40, (n, 10)).astype(np.int32)
+        labels = [rng.integers(0, 40, int(c)).astype(np.int32) for c in rng.integers(0, 12, n)]
+        runs.append((pred, labels, [10]))
+    return dict(runs=runs)
+
+
+def _ranking_grid_reach(d):
+    per_trip = K["kMaxGridBlocks"] * K["kRankWarps"]
+    return {("rank_trips", -(-len(p) // per_trip)) for p, _, _ in d["runs"]}
+
+
 # ---- the table --------------------------------------------------------------------------------------------------
 BOUNDS = {
     "i2v_depth24_d64_w5_p1": Case("item2vec", lambda: _caterpillar(24, 64, 5, 1, 7), _i2v_reach),
@@ -490,6 +1072,23 @@ BOUNDS = {
     "als_fit_64_models": Case("als", _als_batched, _als_batched_reach),
     "featureeng_24_genres_windows_timestamps": Case("featureeng", _fe_genres, _fe_genres_reach),
     "featureeng_top_movie_id": Case("featureeng", _fe_top_movie, _fe_top_reach),
+    "fj_quantile_65536_probabilities": Case("featurejob", _fj_probs, _fj_quantile_reach),
+    "fj_quantile_tightest_segment_cap": Case("featurejob", _fj_tight, _fj_quantile_reach),
+    "fj_quantile_grid_stride_eps0": Case("featurejob", _fj_stride, _fj_quantile_reach),
+    "fj_discretizer_splits_kernel_passes": Case("featurejob", _fj_discretizer_passes, _fj_discretizer_reach),
+    "fj_discretizer_duplicates_past_1024": Case("featurejob", _fj_discretizer_duplicates, _fj_discretizer_reach),
+    "fj_bucketize_10001_splits_grid_stride": Case("featurejob", _fj_bucketize, _fj_bucketize_reach),
+    "fj_scaler_signed_zeros_overflow_stride": Case("featurejob", _fj_scaler, _fj_scaler_reach),
+    "fj_rating_features_max_ratings": Case("featurejob", _fj_ratings, _fj_ratings_reach),
+    "fj_string_indexer_max_words": Case("featurejob", _fj_words, _fj_indexer_reach),
+    "fj_string_indexer_count_field": Case("featurejob", _fj_count_field, _fj_indexer_reach),
+    "fj_multi_hot_256_words_top_ids_stride": Case("featurejob", _fj_multi_hot, _fj_multi_hot_reach),
+    "fj_split_64_parts": Case("featurejob", _fj_split, _fj_split_reach),
+    "fj_split_by_timestamp_edges": Case("featurejob", _fj_ts_split, _fj_ts_reach),
+    "als_implicit_yty_tiles": Case("als_implicit", _yty_tiles, _yty_reach),
+    "als_implicit_solve_chunks": Case("als_implicit", _implicit_chunks, _implicit_chunks_reach),
+    "ranking_lists_ballot_passes": Case("ranking_metrics", _ranking_lists, _ranking_lists_reach),
+    "ranking_grid_trips": Case("ranking_metrics", _ranking_grid, _ranking_grid_reach),
 }
 
 
@@ -531,6 +1130,32 @@ def test_every_bound_has_a_case():
     need |= {("kIdMask", K["kIdMask"]), ("kIdMask", K["kIdMask"] - 1), ("walk_length", 1), ("rec_nan", 1)}
     assert ("walk_depth", 24) in have or any(k == "walk_depth" and v >= 24 for k, v in have)
     assert any(k == "hub_row" and v >= 5000 for k, v in have)
+    # featurejob.cu
+    need |= {("kMaxProbs", K["kMaxProbs"]), ("kMaxBuckets", K["kMaxBuckets"]), ("nq", K["kMaxBuckets"] + 1)}
+    need |= {("kMaxBuckets", b) for b in (2, K["kMaxBuckets"] - 1)} | {("n_splits", K["kMaxBuckets"] + 1)}
+    need |= {("nq", q) for q in (SPLITS_THREADS - 1, SPLITS_THREADS, SPLITS_THREADS + 1)} | {("dup_past_threads", 1)}
+    need |= {("kMaxWords", K["kMaxWords"]), ("kMaxTokens", K["kMaxTokens"]), ("kMaxParts", K["kMaxParts"])}
+    need |= {("kMaxWordsPerRow", K["kMaxWordsPerRow"]), ("kMaxMovieId", K["kMaxMovieId"]), ("kMaxMovieId", 0)}
+    need |= {("kMaxRatings", K["kMaxRatings"]), ("rating_q_past_double", 1)}
+    need |= {("tightest_segments", compress_segments(TIGHT_N, TIGHT_EPS)[0]), ("every_value_a_head", 1)}
+    need |= {("segments_margin", seg_cap(TIGHT_N, TIGHT_EPS) - compress_segments(TIGHT_N, TIGHT_EPS)[0])}
+    assert GRID_BLOCKS == K["kMaxGridBlocks"]
+    need |= {("keys_stride", 1), ("expand_stride", 1), ("bucket_stride", 1), ("scale_stride", 1), ("csr_stride", 1),
+             ("row_stride", 1), ("hist_stride", 1)}
+    need |= {("scale_overflow", 1), ("signed_zero_min", 1)}
+    need |= {("split_fraction", f) for f in (0.0, 1.0)} | {("split_n", 1)}
+    need |= {("ts_one_sampled", 1), ("ts_all_equal", 1), ("ts_2_53", 1)}
+    # implicit ALS and RankingMetrics (als.cu)
+    t = K["kYtyThreads"]
+    need |= {("yty_tiles", v) for v in (1, 2, -(-(64 * 65 // 2) // t))}
+    need |= {("yty_members", v) for v in (0, 1, c - 1, c, c + 1, 2 * c, 2 * c + 1)} | {("kYtyBlocks", K["kYtyBlocks"])}
+    need |= {("implicit_chunk", v) for v in (c - 1, c, c + 1, 2 * c, 2 * c + 1)}
+    need |= {("implicit_nonpos_at", p) for p in (0, c - 1, c)}
+    need |= {("implicit_alpha", 0.0), ("implicit_alpha", 40.0)}
+    need |= {("rank_L", v) for v in (0, 1, 31, 32, 33, 64, 65)} | {("rank_repeated_label", 100)}
+    need |= {("rank_distinct", v) for v in (1, 31, 32, 33, "past_L")}
+    need |= {("rank_k_vs_L", v) for v in (-1, 0, 1, "past")} | {("rank_steps", v) for v in (31, 32, 33, 64, 65)}
+    need |= {("rank_hit_at", p) for p in RANK_HITS} | {("rank_trips", 2), ("rank_trips", 3)}
     assert need <= have, sorted(need - have)
     # the deepest case is the deepest code the rating bound allows: one level more needs more ratings than it takes
     assert sum(_deepest_counts(DEEPEST + 1)) > MAX_RATINGS >= sum(_deepest_counts(DEEPEST))
@@ -542,6 +1167,11 @@ def test_the_constants_are_parsed():
                  "kMaxTables", "kQueryWarps", "kMaxCode", "kMaxDim", "kMaxGenres", "kWindow", "kMaxMovieSlots",
                  "kIdMask", "kMaxWalkWords"):
         assert isinstance(K.get(name), int) and K[name] > 0, name
+    for name in ("kMaxValues", "kMaxProbs", "kMaxBuckets", "kMaxWords", "kMaxTokens", "kMaxWordsPerRow", "kMaxParts",
+                 "kMaxMovieId", "kMaxRatings", "kMaxGridBlocks", "kYtyThreads", "kYtyBlocks", "kRankWarps"):
+        assert isinstance(K.get(name), int) and K[name] > 0, name
+    assert K["kMaxGridBlocks"] == 132 * 64 and K["kMaxTokens"] == (1 << 29) - 1
+    assert {constants(f)["kMaxRatings"] for f in RATING_BOUND_FILES} == {MAX_RATINGS}
     assert K["kSrcPerBlock"] == K["kRecWarps"] * K["kSrcPerWarp"]
     assert K["kIdMask"] == K["kMaxMovieSlots"] - 1
 
@@ -668,3 +1298,173 @@ def test_one_past_each_bound_is_rejected_before_any_launch(name):
     msg = _lib.load().srs_last_error().decode()
     assert says in msg, msg
     assert launch_count() == n0
+
+
+# ---- featurejob.cu and RankingMetrics: one past each bound, before any launch, outputs untouched -----------------
+SENTINEL = -7
+
+
+def _fill(n, t):
+    return np.full(max(int(n), 1), SENTINEL, t)
+
+
+def _quantile_call(n=3, n_probs=2):
+    v, p, out = np.array([1.0, 2.0, 3.0]), np.full(max(n_probs, 1), 0.5), _fill(n_probs, np.float64)
+    return _lib.load().srs_approx_quantile_host(_p(v) if n <= 3 else None, n, _p(p), n_probs, 0.01, 0,
+                                                _p(out)), [out]
+
+
+def _discretizer_call(n=3, buckets=2):
+    v, splits, b, ns = np.array([1.0, 2.0, 3.0]), _fill(K["kMaxBuckets"] + 2, np.float64), _fill(3, np.int32), \
+        C.c_int32(SENTINEL)
+    rc = _lib.load().srs_quantile_discretizer_host(_p(v) if n <= 3 else None, n, buckets, 0.01, 0, _p(splits),
+                                                   C.byref(ns), _p(b))
+    return rc, [splits, b, np.array([ns.value])]
+
+
+def _bucketize_call(n=3, n_splits=3):
+    splits = np.r_[-np.inf, np.arange(max(n_splits - 2, 1)), np.inf][:n_splits]
+    v, out = np.array([0.5, 1.0, 0.0]), _fill(3, np.int32)
+    return _lib.load().srs_bucketize_host(_p(splits), n_splits, _p(v) if n <= 3 else None, n, 0, _p(out)), [out]
+
+
+def _scale_call(n):
+    out, mm = _fill(3, np.float64), _fill(2, np.float64)
+    return _lib.load().srs_minmax_scale_host(None, n, None, 0, _p(out), _p(mm)), [out, mm]
+
+
+def _split_call(n=10, n_parts=2):
+    w, rows, cnt = np.ones(n_parts), _fill(10, np.int32), _fill(n_parts, np.int64)
+    return _lib.load().srs_sample_split_host(n, 1, 0.5, _p(w), n_parts, 0, _p(rows), _p(cnt)), [rows, cnt]
+
+
+def _ts_split_call(n=3, ts=(1, 2, 3)):
+    t, rows, cnt, split = np.array(ts, np.int64), _fill(3, np.int32), _fill(2, np.int64), C.c_double(SENTINEL)
+    rc = _lib.load().srs_sample_split_by_timestamp_host(_p(t) if n <= 3 else None, n, 1, 0.5, 0.01, 0, _p(rows),
+                                                        _p(cnt), C.byref(split))
+    return rc, [rows, cnt, np.array([split.value])]
+
+
+def _ratings_call(n=2, movie=(1, 2)):
+    m, h = np.array(movie, np.int32), np.array([4, 6], np.int8)
+    ids, cnt, avg, var, nm = (_fill(4, np.int32), _fill(4, np.int64), _fill(4, np.float64), _fill(4, np.float64),
+                              C.c_int32(SENTINEL))
+    rc = _lib.load().srs_rating_features_host(_p(m) if n <= 2 else None, _p(h) if n <= 2 else None, n, 0, 4,
+                                              _p(ids), _p(cnt), _p(avg), _p(var), C.byref(nm))
+    return rc, [ids, cnt, avg, var, np.array([nm.value])]
+
+
+def _indexer_call(n_tok=2, W=2, hashes=(1, 2)):
+    tok, h = np.array([0, 1], np.int32), np.array(hashes, np.int32)
+    lw, lc = _fill(2, np.int32), _fill(2, np.int64)
+    rc = _lib.load().srs_string_indexer_host(_p(tok) if n_tok <= 2 else None, n_tok, _p(h), W, 0, _p(lw), _p(lc))
+    return rc, [lw, lc]
+
+
+def _multihot_call(row_len=1, movie=3):
+    ids, off = np.array([movie], np.int32), np.array([0, row_len], np.int32)
+    words, h = np.zeros(max(row_len, 1), np.int32), np.array([5], np.int32)
+    outs = [_fill(1, np.int32), _fill(1, np.int64), _fill(1, np.int32), _fill(2, np.int32), _fill(row_len, np.int32)]
+    rc = _lib.load().srs_genre_multihot_host(_p(ids), _p(off), _p(words), 1, _p(h), 1, 0, *[_p(o) for o in outs])
+    return rc, outs
+
+
+def _ranking_call(n_queries, pred_len):
+    means = _fill(3, np.float64)
+    return _lib.load().srs_ranking_metrics_host(None, n_queries, pred_len, None, None, 5, 0, None, _p(means)), [means]
+
+
+_VMAX = 2147483647 + 1                          # kMaxValues + 1, checked before any pointer is read
+FJ_REJECTIONS = {
+    "quantile values": (lambda: _quantile_call(n=_VMAX), "1..%d" % K["kMaxValues"]),
+    "discretizer values": (lambda: _discretizer_call(n=_VMAX), "1..%d" % K["kMaxValues"]),
+    "bucketize values": (lambda: _bucketize_call(n=_VMAX), "1..%d" % K["kMaxValues"]),
+    "scaler values": (lambda: _scale_call(_VMAX), "1..%d" % K["kMaxValues"]),
+    "split values": (lambda: _split_call(n=_VMAX), "1..%d" % K["kMaxValues"]),
+    "timestamp split values": (lambda: _ts_split_call(n=_VMAX), "1..%d" % K["kMaxValues"]),
+    "quantile probabilities": (lambda: _quantile_call(n_probs=K["kMaxProbs"] + 1), "1..%d" % K["kMaxProbs"]),
+    "discretizer one bucket": (lambda: _discretizer_call(buckets=1), "2..%d" % K["kMaxBuckets"]),
+    "discretizer buckets": (lambda: _discretizer_call(buckets=K["kMaxBuckets"] + 1), "2..%d" % K["kMaxBuckets"]),
+    "bucketize splits": (lambda: _bucketize_call(n_splits=K["kMaxBuckets"] + 2), "3..%d" % (K["kMaxBuckets"] + 1)),
+    "indexer words": (lambda: _indexer_call(W=K["kMaxWords"] + 1), "1..%d" % K["kMaxWords"]),
+    "indexer tokens": (lambda: _indexer_call(n_tok=K["kMaxTokens"] + 1), "1..%d" % K["kMaxTokens"]),
+    "indexer hash collision": (lambda: _indexer_call(hashes=(F.java_string_hash("Aa"), F.java_string_hash("BB"))),
+                               "share improve(hashCode)"),
+    "multi-hot words per row": (lambda: _multihot_call(row_len=K["kMaxWordsPerRow"] + 1),
+                                "1..%d" % K["kMaxWordsPerRow"]),
+    "multi-hot movie id": (lambda: _multihot_call(movie=K["kMaxMovieId"] + 1), "0..%d" % K["kMaxMovieId"]),
+    "rating features movie id": (lambda: _ratings_call(movie=(1, K["kMaxMovieId"] + 1)), "0..%d" % K["kMaxMovieId"]),
+    "rating features ratings": (lambda: _ratings_call(n=K["kMaxRatings"] + 1), "1..%d" % K["kMaxRatings"]),
+    "split parts": (lambda: _split_call(n_parts=K["kMaxParts"] + 1), "1..%d" % K["kMaxParts"]),
+    "timestamp past 2^53": (lambda: _ts_split_call(ts=(0, 2 ** 53 + 1, 5)), "-2^53..2^53"),
+    "ranking predictions": (lambda: _ranking_call(1 << 16, 1 << 15), "exceed 2147483647"),
+}
+
+
+@pytest.mark.parametrize("name", sorted(FJ_REJECTIONS))
+def test_featurejob_and_ranking_one_past_each_bound_rejected_before_any_launch(name):
+    from sparrowrecsys_b200.model import launch_count
+    call, says = FJ_REJECTIONS[name]
+    n0 = launch_count()
+    rc, outs = call()
+    assert rc in (_lib.SRS_ERR_INVALID, _lib.SRS_ERR_RANGE), rc
+    msg = _lib.load().srs_last_error().decode()
+    assert says in msg, msg
+    assert launch_count() == n0
+    for o in outs:
+        assert np.all(o == SENTINEL), (name, o)
+
+
+def test_the_hash_collision_is_the_oracles_too():
+    assert F.java_string_hash("Aa") == F.java_string_hash("BB") == 2112
+    with pytest.raises(ValueError):
+        FQ.hash_trie_keys(["Aa", "BB"])
+    with pytest.raises(ValueError):
+        FQ.string_indexer_labels(["Aa", "BB", "Aa"])
+
+
+# ---- the compress walk's segment cap -----------------------------------------------------------------------------
+def _sweep_points():
+    rng = np.random.default_rng(56)
+    ns = sorted({*range(1, 41), *np.unique(np.geomspace(41, 3e6, 40).astype(int)).tolist(), 3000000})
+    eps = [0.0, 1e-7, 1e-6, 1e-5, 1e-4, 2e-4, 5e-4, 1e-3, 1e-2, 0.1, 0.25, 0.5, 0.75, 1.0]
+    pts = [(n, e) for n in ns for e in eps]
+    pts += [(n, e * x) for n in ns[40::4] for e in (1 / (2 * math.sqrt(n)),) for x in (0.8, 0.9, 0.97, 1.0, 1.1)]
+    for _ in range(300):
+        n = int(rng.integers(1, 3000001))
+        pts.append((n, float(rng.random() / (2 * math.sqrt(n)) * rng.choice([1.0, 2.0]))))
+    return pts
+
+
+def test_the_compress_segments_stay_under_their_cap():
+    """fj_compress_kernel's segments under quantiles_of_keys' cap min(n, floor(2 eps n) + 8) + 2, for n from 1 to
+    3e6 and eps from 0 to 1 (near 1 / (2 sqrt n) the walk is longest against its cap), plus random draws.  The walk
+    takes one segment per run of delta (runs <= 2 eps n + 1) or per head, plus the ends: TIGHT_N, TIGHT_EPS takes
+    floor(2 eps n) + 3, the most seen, and the slack of 8 covers it."""
+    worst = 0.0
+    for n, e in _sweep_points():
+        ns, heads = compress_segments(n, e)
+        assert ns <= seg_cap(n, e), (n, e, ns)
+        assert ns - int(2.0 * e * n) <= 3, (n, e, ns)
+        if n <= 20000:
+            assert heads == len(FQ.one_summary_closed_form(n, e)) - (n > 1)
+        worst = max(worst, ns / seg_cap(n, e))
+    ns, _ = compress_segments(TIGHT_N, TIGHT_EPS)
+    assert ns - int(2.0 * TIGHT_EPS * TIGHT_N) == 3 and ns / seg_cap(TIGHT_N, TIGHT_EPS) >= worst
+
+
+def test_the_segment_count_matches_the_oracles_walk():
+    for n, e in ((1, 0.0), (2, 0.3), (1000, 0.0), (1000, 0.01), (5000, 0.002), (20001, 0.0035), (77, 1.0)):
+        heads = FQ.one_summary_segments(n, e)
+        assert compress_segments(n, e)[1] == len(heads) - (n > 1)
+
+
+def test_vectorised_query_matches_query_sampled():
+    rng = np.random.default_rng(57)
+    for n, eps in ((1, 0.0), (2, 0.5), (1000, 0.0), (3001, 0.01), (20000, 0.001)):
+        v = np.round(rng.standard_normal(n) * 30)
+        _, sampled, _ = FQ.one_summary_samples(v, eps)
+        p = np.r_[0.0, eps, 1 - eps, 1.0, np.nextafter(eps, 1.0), rng.random(200), np.arange(1, 50) / n]
+        p = p[(p >= 0) & (p <= 1)]
+        want = [FQ.query_sampled(sampled, n, float(x), eps) for x in p]
+        assert query_many(sampled, n, p, eps).tolist() == want
