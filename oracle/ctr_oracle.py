@@ -302,10 +302,15 @@ def din_history_keys(T):
     return sorted("userRatedMovie%d" % k for k in range(1, T + 1))
 
 
-def din_forward(spec, W, feats, dtype=np.float32):
+def din_forward(spec, W, feats, dtype=np.float32, defect=None, chunk=32):
     """DIN.py:125-167.  Sigmoid-gated *sum* pooling (no softmax), history id 0 is
     an ordinary table row (mask_zero has no numerical effect), ids pass through a
-    float32 numeric_column before the Embedding layer casts them back to int32."""
+    float32 numeric_column before the Embedding layer casts them back to int32.
+
+    `defect` (mutants for the tests; a kernel stages `chunk` positions at a time):
+    "last" leaves position T - 1 out of the pool, "chunk" a partial last chunk,
+    "pad" every padding position (id 0), and "alpha" reads position t's PReLU alpha
+    at t mod chunk."""
     E, T = spec.emb_dim, spec.hist_len
     cand_f = numeric(feats, "movieId", np.float32)                           # :95,125
     hist_f = np.concatenate([numeric(feats, k, np.float32) for k in din_history_keys(T)],
@@ -320,8 +325,17 @@ def din_forward(spec, W, feats, dtype=np.float32):
     Cr = np.repeat(C[:, None, :], T, axis=1)                                 # :139
     A = np.concatenate([H - Cr, H, Cr, H * Cr], axis=-1)                     # :141-147
     a = dense(A, W, "au_dense")                                              # :149
-    a = prelu(a, W["au_prelu/alpha"])                                        # :150 alpha [T,32]
+    alpha = W["au_prelu/alpha"]
+    if defect == "alpha":
+        alpha = alpha[np.arange(T) % chunk]
+    a = prelu(a, alpha)                                                      # :150 alpha [T,32]
     w = dense(a, W, "au_out", "sigmoid")[..., 0]                             # :151-152 [B,T]
+    if defect == "last":
+        w[:, T - 1] = 0
+    elif defect == "chunk":
+        w[:, T - T % chunk:] = 0
+    elif defect == "pad":
+        w[hist == 0] = 0
     pooled = (H * w[:, :, None]).sum(axis=1)                                 # :153-158
     uid = identity_ids(feats, "userId", spec.n_users)
     user_profile = np.concatenate([                                          # :108-114,127 sorted
@@ -343,7 +357,7 @@ def din_forward(spec, W, feats, dtype=np.float32):
     return sigmoid(z), z
 
 
-def dien_forward(spec, W, feats, dtype=np.float32):
+def dien_forward(spec, W, feats, dtype=np.float32, defect=None):
     """DIEN.py:154-256, the `y_pred` output (the auxiliary-loss head, :259-292, only feeds
     `add_loss` and is not part of the prediction).
 
@@ -364,7 +378,10 @@ def dien_forward(spec, W, feats, dtype=np.float32):
       r = s(Act_r(In_r(x) + Hid_r(u)));  z = s(Act_z(In_z(x) + Hid_z(u)))
       hn = tanh(Act_h(In_h(x) + Hid_h(u * z)));  a = s_t * r;  u' = (1 - a) * u + a * hn
     (`In` Dense with bias, `Hid` Dense without, `Act` Dense with bias and the activation).
-    Top (:250-256): [u_T | candidate | user_profile | context] -> 128 PReLU -> 64 PReLU -> 1."""
+    Top (:250-256): [u_T | candidate | user_profile | context] -> 128 PReLU -> 64 PReLU -> 1.
+
+    `defect` (mutants for the tests): "last" stops both recurrences before position T - 1,
+    "mask" runs the GRU over padding (id 0) as over any row."""
     E, T = spec.emb_dim, spec.hist_len
     cand_f = numeric(feats, "movieId", np.float32)                           # :96,154
     hist_f = np.concatenate([numeric(feats, k, np.float32) for k in din_history_keys(T)],
@@ -374,6 +391,9 @@ def dien_forward(spec, W, feats, dtype=np.float32):
     if cand.min() < 0 or max(cand.max(), hist.max()) >= spec.n_movies or hist.min() < 0:
         raise ValueError("movie id out of range")
     mask = hist_f != 0                                                       # Embedding.compute_mask
+    if defect == "mask":
+        mask[:] = True
+    steps = T - 1 if defect == "last" else T
     tab = W["embedding"].astype(dtype)
     X = tab[hist]                                                            # [B,T,E] :163
     C = tab[cand]                                                            # [B,E]   :164,167
@@ -382,7 +402,7 @@ def dien_forward(spec, W, feats, dtype=np.float32):
     bx, bh = W["gru/bias"].astype(dtype)
     h = np.zeros((B, E), dtype)
     G = np.zeros((B, T, E), dtype)
-    for t in range(T):                                                       # :169
+    for t in range(steps):                                                   # :169
         mx = X[:, t] @ K + bx
         mh = h @ U + bh
         z = sigmoid(mx[:, :E] + mh[:, :E])
@@ -397,7 +417,7 @@ def dien_forward(spec, W, feats, dtype=np.float32):
         pre = dense(x, W, "augru_%s_input" % g) + hid @ W["augru_%s_hidden/kernel" % g].astype(dtype)
         return dense(pre, W, "augru_%s_act" % g)
     u = np.repeat(W["augru_h0"].astype(dtype), B, axis=0)                    # :235-236 (stored)
-    for t in range(T):                                                       # :237-243
+    for t in range(steps):                                                   # :237-243
         x = G[:, t]
         r = sigmoid(gate("r", x, u))
         z = sigmoid(gate("z", x, u))

@@ -54,9 +54,10 @@ def neg_ids(spec, feats):
     return neg
 
 
-def aux_oracle(spec, W, feats):
+def aux_oracle(spec, W, feats, defect=None):
     """aux_row = sum_{t=1}^{T-1} pos_t + neg_t (DIEN.py:276-285): Dense32(sigmoid) then Dense1(sigmoid) over
-    [g_t | e(h_{t+1})] and [g_t | e(n_{t+1})], 1-based; no mask (the slices drop it)."""
+    [g_t | e(h_{t+1})] and [g_t | e(n_{t+1})], 1-based; no mask (the slices drop it).  `defect` "last" (a mutant
+    for the tests) leaves the sum's last step t = T - 1 out."""
     G, tab, hist = gru_outputs(spec, W, feats)
     neg = neg_ids(spec, feats)
     W64 = {k: v.astype(np.float64) for k, v in W.items() if k.startswith("aux_")}
@@ -65,7 +66,7 @@ def aux_oracle(spec, W, feats):
         x = np.concatenate([g, e], axis=1)                 # hidden state first (DIEN.py:278,282)
         return O.dense(O.dense(x, W64, "aux_%s_dense" % side, "sigmoid"), W64, "aux_%s_out" % side, "sigmoid")[:, 0]
     aux = np.zeros(hist.shape[0])
-    for t in range(1, spec.hist_len):                      # 0-based t: g_t = G[t-1], next item = position t
+    for t in range(1, spec.hist_len - (defect == "last")):  # 0-based t: g_t = G[t-1], next item = position t
         aux += head("pos", G[:, t - 1], tab[hist[:, t]]) + head("neg", G[:, t - 1], tab[neg[:, t - 1]])
     return aux
 
