@@ -130,8 +130,7 @@ const char* srs_last_error(void);
 int srs_model_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors,
                      int32_t device, srs_model** out);
 
-/* Same, with kernel-variant options "key=value;key=value": din_impl = tc | cudacore (rt and rtp,
- * the names of earlier tensor-core DIN kernels, select the tc kernel),
+/* Same, with kernel-variant options "key=value;key=value": din_impl = tc | cudacore,
  * embmlp_impl / deepfm_impl = tc | cudacore, zero_copy_scores = 0 | 1.  Unknown keys are ignored; a
  * forced variant that does not support the shape makes the call fail.  NULL / "" = the defaults
  * (which srs_model_kernel_name reports).  The environment variables SRS_DIN_IMPL, SRS_EMBMLP_IMPL,

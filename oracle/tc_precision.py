@@ -142,7 +142,7 @@ def _pad_rows(a, n):
 def din_tile_columns(E, EP):
     """Row of `dense/kernel` feeding each column of din_wg's top-MLP X tile
     [userGenre1 | userId | pooled | candidate | movieGenre1] (EP columns each, -1 = zero padding), and
-    the rows of the 7 numerics in NUMERIC_KEYS order (csrc/model.cu build_din)."""
+    the rows of the 7 numerics in NUMERIC_KEYS order (csrc/placement.h place_din)."""
     base = 3 + 4 * E
     starts = (1, 1 + E, 3 + 2 * E, 3 + 3 * E, base + 1)
     cols = np.full(5 * EP, -1, np.int64)
@@ -218,7 +218,7 @@ def din_forward(spec, W, feats, defect=None, row0=0):
 def embmlp_tile_columns(E):
     """Row of `dense/kernel` feeding each of embmlp_tc's 128 K columns (K = slot * 12 + e, slots
     movieGenre1..3, movieId, userGenre1..5, userId; -1 = zero), and the numerics' rows
-    (csrc/model.cu build_embmlp_tc)."""
+    (csrc/placement.h place_embmlp)."""
     starts = [1 + k * E for k in range(3)] + [1 + 3 * E] + [5 + 4 * E + k * E for k in range(5)] + [5 + 9 * E]
     cols = np.full(128, -1, np.int64)
     for slot, s in enumerate(starts):
@@ -249,7 +249,7 @@ def embmlp_forward(spec, W, feats, defect=None, row0=0):
 # ---- deepfm_tc_kernel ----------------------------------------------------------------------------------
 def deepfm_tile_columns(E):
     """Row of `dense/kernel` feeding each of deepfm_tc's 64 K columns ([deep movieId emb | deep userId emb],
-    16 each, then zeros), and the numerics' rows (csrc/model.cu build_deepfm_tc)."""
+    16 each, then zeros), and the numerics' rows (csrc/placement.h place_deepfm)."""
     cols = np.full(64, -1, np.int64)
     cols[:E] = 1 + np.arange(E)
     cols[16:16 + E] = 5 + E + np.arange(E)

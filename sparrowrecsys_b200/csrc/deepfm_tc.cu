@@ -69,7 +69,7 @@ __global__ void __launch_bounds__(128) deepfm_tc_kernel(const __grid_constant__ 
     const int u = 16 * warp + g + 8 * i;
     b1[i] = __ldg(p.b1 + u); b2[i] = __ldg(p.b2 + u); wdeep[i] = __ldg(p.wdeep + u);
 #pragma unroll
-    for (int n = 0; n < kNumNumerics; ++n) w1n[i][n] = __ldg(p.w1num + n * 64 + u);
+    for (int n = 0; n < kNumNumerics; ++n) w1n[i][n] = __ldg(p.w1_numerics + n * 64 + u);
   }
 
   const int n_sg = (b.B + kFtRows - 1) / kFtRows;

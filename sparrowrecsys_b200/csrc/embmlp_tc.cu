@@ -62,7 +62,7 @@ __global__ void __launch_bounds__(256, 1) embmlp_tc_kernel(const __grid_constant
     const int u = 64 * q + 16 * warp_w + g + 8 * i;
     b1[i] = __ldg(p.b1 + u); b2[i] = __ldg(p.b2 + u); w3[i] = __ldg(p.w3 + u);
 #pragma unroll
-    for (int n = 0; n < kNumNumerics; ++n) w1n[i][n] = __ldg(p.w1num + n * 128 + u);
+    for (int n = 0; n < kNumNumerics; ++n) w1n[i][n] = __ldg(p.w1_numerics + n * 128 + u);
   }
 
   const int n_sg = (b.B + kEtRows - 1) / kEtRows;

@@ -124,7 +124,8 @@ struct EmbMlpTcParams {
   const float* user;       // [n_users][12]
   const uint8_t* image;    // 128 KB: W1^T hi/lo, W2^T hi/lo as bf16 SW128 operand tiles
   const float* b1;         // [128]
-  const float* w1num;      // [8][128] rows of dense/kernel that multiply the 7 numerics
+  const float* w1_numerics;   // [8][128] the numerics' rows of EmbMlpBlob's W1 (rows 120..127, in the blob): the
+                              //   rows no MMA takes
   const float* b2;         // [128]
   const float* w3;         // [128]
   const float* wide;       // [cross_buckets] or nullptr
@@ -212,7 +213,8 @@ struct DeepFmTcParams {
   const float* deep_user;
   const uint8_t* image;    // 64 KB: W1^T hi/lo, W2^T hi/lo as [128][64] bf16 SW128 tiles
   const float* b1;         // [64]
-  const float* w1num;      // [8][64]
+  const float* w1_numerics;   // [8][64] the numerics' rows of DeepFmBlob's W1 (rows 32..39, in the blob): the
+                              //   rows no MMA takes
   const float* b2;         // [64]
   const float* first;      // [fm1_width]
   const float* wdeep;      // [64]
@@ -291,6 +293,7 @@ struct DinParams {
   const float* user;       // [n_users][EP]
   const float* ugenre;     // [19][EP]
   const float* mgenre;     // [19][EP]
+  // the Dense weights point into one DinBlob (below); au_bout and b3 are copies
   // activation unit, algebraically folded (DESIGN.md "DIN activation unit"):
   //   Dense32([h-c, h, c, h*c]) = h.(W_sub+W_h) + (h*c).W_prod + c.(W_c-W_sub) + b
   const float* au_wh;      // [EP][32]  W_sub + W_h
@@ -316,6 +319,37 @@ struct DinParams {
   const uint8_t* movie_split;  // din_wg.cu: [n_movies][EP x bf16 hi | EP x bf16 lo] (history rows)
   int max_ctas;                // din_wg.cu: CTAs per launch, 0 = one per 32-row tile (srs_model_set_sm_limit)
   const uint8_t* mlp_image;    // din_wg.cu, EP = 32: W1^T / W2^T bf16 hi / lo images (DinWgLayout<32>::IMG_*)
+};
+
+// The Dense weights of DIN as one blob, offsets in floats: au_dense/kernel's four row groups W_sub, W_h, W_c and
+// W_prod [EP][32] each (model creation folds them in place into wh = W_sub + W_h and wc = W_c - W_sub: DinParams'
+// au_wh and au_wc; wsub is then unused), au_dense/bias [32], au_prelu/alpha [T][32], au_out/kernel [32] and
+// au_out/bias; then the top MLP: W1 [5EP + 8][128] in the tile order of din.cu, b1 and a1 (prelu/alpha) [128],
+// W2 [128][64], b2, a2 and w3 [64], b3.  Widths past E, hidden widths and padding rows are zero; every array starts
+// on a 256-byte line (a multiple of 64 floats).
+struct DinBlob {
+  int wsub, wh, wc, wp, au_b, au_alpha, au_wout, au_bout, W1, b1, a1, W2, b2, a2, w3, b3, floats;
+  static DinBlob of(int EP, int T) {
+    DinBlob l;
+    l.wsub = 0;
+    l.wh = l.wsub + EP * 32;
+    l.wc = l.wh + EP * 32;
+    l.wp = l.wc + EP * 32;
+    l.au_b = l.wp + EP * 32;
+    l.au_alpha = l.au_b + 64;
+    l.au_wout = l.au_alpha + (T * 32 + 63) / 64 * 64;
+    l.au_bout = l.au_wout + 64;
+    l.W1 = l.au_bout + 64;
+    l.b1 = l.W1 + (5 * EP + kNumPad) * 128;
+    l.a1 = l.b1 + 128;
+    l.W2 = l.a1 + 128;
+    l.b2 = l.W2 + 128 * 64;
+    l.a2 = l.b2 + 64;
+    l.w3 = l.a2 + 64;
+    l.b3 = l.w3 + 64;
+    l.floats = l.b3 + 4;
+    return l;
+  }
 };
 
 // ---- DIEN (DIEN.py:154-256), CUDA-core kernel for E <= 32 -------------------------------------

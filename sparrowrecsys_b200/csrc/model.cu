@@ -204,7 +204,8 @@ namespace {
 
 struct Builder : TensorLookup {
   srs_model* m;
-  std::vector<float> din_w1, din_w2;    // the permuted DIN top-MLP weights build_din uploaded, for build_din_wg
+  std::vector<float> blob;    // the host copy of the Dense-weight blob build_embmlp, build_deepfm or build_din
+                              // uploaded, which the tensor-core builders make their operand images from
 
   Builder(srs_model* m, const srs_tensor* ts, int n) : TensorLookup(ts, n), m(m) {}
 
@@ -273,24 +274,6 @@ struct Builder : TensorLookup {
     }
     return d;
   }
-
-  // Dense kernel [K][N] -> [dev_rows][NP]: device row i takes reference row map[i]
-  // (-1 = zero row); columns zero padded to NP.
-  std::vector<float> permute(const float* ref, int N, const std::vector<int>& map, int NP) {
-    std::vector<float> out(map.size() * (size_t)NP, 0.f);
-    if (!ref) return out;
-    for (size_t i = 0; i < map.size(); ++i)
-      if (map[i] >= 0)
-        for (int j = 0; j < N; ++j) out[i * NP + j] = ref[(size_t)map[i] * N + j];
-    return out;
-  }
-
-  std::vector<float> padvec(const float* ref, int n, int np) {
-    std::vector<float> out(np, 0.f);
-    if (ref)
-      for (int i = 0; i < n; ++i) out[i] = ref[i];
-    return out;
-  }
 };
 
 // The tensors of a trainable model through its placement (placement.h): the Dense tensors scattered into the host
@@ -337,11 +320,12 @@ int build_embmlp(Builder& B) {
     return fail(SRS_ERR_INVALID, "EmbeddingMLP/W&D need two hidden layers of width <= 128");
   EmbMlpParams& p = m->emb;
   const Placement pl = place_embmlp(s, m->EP, &p);
-  std::vector<float> blob(EmbMlpBlob::of(m->EP).floats, 0.f), wide_rows(wide ? s.cross_buckets : 0, 0.f);
+  B.blob.assign(EmbMlpBlob::of(m->EP).floats, 0.f);
+  std::vector<float> wide_rows(wide ? s.cross_buckets : 0, 0.f);
   const float* tables[kWideDeepTables];
-  place_host(B, pl, tables, blob.data(), wide_rows.data());
+  place_host(B, pl, tables, B.blob.data(), wide_rows.data());
   if (B.status != SRS_OK) return B.status;
-  point_into_blob(&p, tables, B.upload(blob));
+  point_into_blob(&p, tables, B.upload(B.blob));
   p.wide = wide ? B.upload(wide_rows) : nullptr;
   m->kernel_name = wide ? "embmlp_kernel<wide&deep>" : "embmlp_kernel";
   return B.status;
@@ -355,16 +339,17 @@ int build_deepfm(Builder& B) {
   DeepFmParams& p = m->fm;
   const Placement pl = place_deepfm(s, m->EP, &p);
   const DeepFmBlob ly = DeepFmBlob::of(m->EP);
-  std::vector<float> blob(ly.floats, 0.f), first((size_t)2 * s.n_genres + s.n_movies + s.n_users, 0.f);
+  B.blob.assign(ly.floats, 0.f);
+  std::vector<float> first((size_t)2 * s.n_genres + s.n_movies + s.n_users, 0.f);
   const float* tables[kDeepFmTables];
-  place_host(B, pl, tables, blob.data(), first.data());
+  place_host(B, pl, tables, B.blob.data(), first.data());
   if (B.status != SRS_OK) return B.status;
   p.fm_movie = tables[0]; p.fm_user = tables[1]; p.fm_mgenre = tables[2]; p.fm_ugenre = tables[3];
   p.deep_movie = tables[4]; p.deep_user = tables[5];
-  point_into_blob(&p, B.upload(blob));
+  point_into_blob(&p, B.upload(B.blob));
   p.first = B.upload(first);
-  for (int d = 0; d < 4; ++d) p.wdot[d] = blob[ly.wdot + d];
-  p.bout = blob[ly.bout];
+  for (int d = 0; d < 4; ++d) p.wdot[d] = B.blob[ly.wdot + d];
+  p.bout = B.blob[ly.bout];
   m->kernel_name = "deepfm_kernel";
   return B.status;
 }
@@ -391,68 +376,25 @@ int build_deepfm2(Builder& B) {
 int build_din(Builder& B) {
   srs_model* m = B.m;
   const srs_spec& s = m->spec;
-  const int E = s.emb_dim, EP = m->EP, T = s.hist_len, A = 32;
-  if (s.au_hidden != A) return fail(SRS_ERR_INVALID, "DIN activation-unit width must be 32");
+  const int EP = m->EP, T = s.hist_len;
+  if (s.au_hidden != 32) return fail(SRS_ERR_INVALID, "DIN activation-unit width must be 32");
   if (s.n_hidden != 2 || s.hidden[0] > 128 || s.hidden[1] > 64 || s.hidden[0] < 1 || s.hidden[1] < 1)
     return fail(SRS_ERR_INVALID, "DIN needs hidden widths <= (128, 64)");
   if (T < 1) return fail(SRS_ERR_INVALID, "hist_len must be >= 1");
-  const int h0 = s.hidden[0], h1 = s.hidden[1];
   DinParams& p = m->din;
-  p.movie = B.table("embedding", s.n_movies, E);
-  p.user = B.table("userId_embedding", s.n_users, E);
-  p.ugenre = B.table("userGenre1_embedding", s.n_genres, E);
-  p.mgenre = B.table("movieGenre1_embedding", s.n_genres, E);
-  const float* au = B.host("au_dense/kernel", 4 * E, A);
-  const float* aub = B.host("au_dense/bias", A, 1);
-  const float* alpha = B.host("au_prelu/alpha", T, A);
-  const float* auo = B.host("au_out/kernel", A, 1);
-  const float* auob = B.host("au_out/bias", 1, 1);
-  const float* k1 = B.host("dense/kernel", 5 * E + 7, h0);
-  const float* b1 = B.host("dense/bias", h0, 1);
-  const float* a1 = B.host("prelu/alpha", h0, 1);
-  const float* k2 = B.host("dense_1/kernel", h0, h1);
-  const float* b2 = B.host("dense_1/bias", h1, 1);
-  const float* a2 = B.host("prelu_1/alpha", h1, 1);
-  const float* k3 = B.host("dense_2/kernel", h1, 1);
-  const float* b3 = B.host("dense_2/bias", 1, 1);
+  const Placement pl = place_din(s, EP, &p);
+  const DinBlob ly = DinBlob::of(EP, T);
+  B.blob.assign(ly.floats, 0.f);
+  const float* tables[4];
+  place_host(B, pl, tables, B.blob.data(), nullptr);
   if (B.status != SRS_OK) return B.status;
-  // activation-unit fold: rows of au_dense/kernel are [h-c | h | c | h*c] blocks of E
-  std::vector<float> wh((size_t)EP * A, 0.f), wp((size_t)EP * A, 0.f), wc((size_t)EP * A, 0.f);
-  for (int e = 0; e < E; ++e)
-    for (int j = 0; j < A; ++j) {
-      const float w_sub = au[(size_t)e * A + j], w_h = au[(size_t)(E + e) * A + j];
-      const float w_c = au[(size_t)(2 * E + e) * A + j], w_p = au[(size_t)(3 * E + e) * A + j];
-      wh[(size_t)e * A + j] = w_sub + w_h;
-      wp[(size_t)e * A + j] = w_p;
-      wc[(size_t)e * A + j] = w_c - w_sub;
-    }
-  p.au_wh = B.upload(wh); p.au_wp = B.upload(wp); p.au_wc = B.upload(wc);
-  p.au_b = B.upload(std::vector<float>(aub, aub + A));
-  p.au_alpha = B.upload(std::vector<float>(alpha, alpha + (size_t)T * A));
-  p.au_wout = B.upload(std::vector<float>(auo, auo + A));
-  p.au_bout = auob[0];
-  // top kernel rows: [user_profile | pooled | candidate | context] (DIN.py:161-162)
-  const int base = 3 + 4 * E;
-  std::vector<int> map;
-  append(map, iota_map(1, E, EP));               // userGenre1 emb
-  append(map, iota_map(1 + E, E, EP));           // userId emb
-  append(map, iota_map(3 + 2 * E, E, EP));       // pooled behaviours
-  append(map, iota_map(3 + 3 * E, E, EP));       // candidate emb
-  append(map, iota_map(base + 1, E, EP));        // movieGenre1 emb
-  const int nums[8] = {base, base + 1 + E, base + 2 + E, base + 3 + E, 0, 1 + 2 * E, 2 + 2 * E, -1};
-  for (int j = 0; j < 8; ++j) map.push_back(nums[j]);
-  B.din_w1 = B.permute(k1, h0, map, 128);
-  B.din_w2 = B.permute(k2, h1, iota_map(0, h0, 128), 64);
-  p.W1 = B.upload(B.din_w1);
-  p.b1 = B.upload(B.padvec(b1, h0, 128));
-  p.a1 = B.upload(B.padvec(a1, h0, 128));
-  p.W2 = B.upload(B.din_w2);
-  p.b2 = B.upload(B.padvec(b2, h1, 64));
-  p.a2 = B.upload(B.padvec(a2, h1, 64));
-  p.w3 = B.upload(B.padvec(k3, h1, 64));
-  p.b3 = b3[0];
-  p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres;
-  p.T = T; p.EP = EP;
+  // the activation-unit fold (DESIGN.md "DIN activation unit"): W_sub + W_h and W_c - W_sub
+  float* w = B.blob.data();
+  for (int i = 0; i < EP * 32; ++i) {
+    w[ly.wh + i] += w[ly.wsub + i];
+    w[ly.wc + i] -= w[ly.wsub + i];
+  }
+  point_into_blob(&p, tables, B.upload(B.blob), B.blob.data());
   m->kernel_name = "din_kernel";
   return B.status;
 }
@@ -514,6 +456,16 @@ void write_sw128(uint8_t* dst, int rows, int kblocks, bool lo_part, F get, int k
         }
 }
 
+// The hi and lo halves of W^T (see write_sw128) for W, a [kn][ld] block of a placed host blob: image row u (of
+// `units`), column k (kblocks K blocks of 64 from k0) holds W[k][u], zero for u >= ld or k >= kn.  `chunks` and
+// `lo_chunk0` as write_sw128's `chunks` and the lo half's `chunk0`: a 32-wide K tail can hold both halves.
+void write_wt(uint8_t* hi, uint8_t* lo, const float* w, int kn, int ld, int units, int kblocks, int k0 = 0,
+              int chunks = 8, int lo_chunk0 = 0) {
+  auto get = [&](int u, int k) -> float { return u < ld && k < kn ? w[(size_t)k * ld + u] : 0.f; };
+  write_sw128(hi, units, kblocks, false, get, k0, 0, chunks);
+  write_sw128(lo, units, kblocks, true, get, k0, lo_chunk0, chunks);
+}
+
 // Tensor-core DIN kernel (din_wg.cu): the movie table pre-split into bf16 hi / lo rows and, for EP = 32,
 // the top MLP's operand images; every other tensor is the one build_din uploaded.
 int build_din_wg(Builder& B) {
@@ -521,20 +473,15 @@ int build_din_wg(Builder& B) {
   DinParams& p = m->din;
   if (m->EP == 32) {
     // W1^T over the 160 embedding columns of the tile: K blocks 0..63 and 64..127 as a hi and a lo image, then
-    // one tail block whose rows are [hi k 128..159 | lo k 128..159]; W2^T as a hi and a lo image.  Units are
-    // the MMA rows, zero-padded to 128 / 64 like the permuted fp32 weights build_din uploaded.  Offsets:
+    // one tail block whose rows are [hi k 128..159 | lo k 128..159]; W2^T as a hi and a lo image.  Offsets:
     // din_wg.cu::DinWgLayout::IMG_*
-    const std::vector<float>& w1 = B.din_w1;     // [5 * 32 + 8][128]
-    const std::vector<float>& w2 = B.din_w2;     // [128][64]
-    auto w1_get = [&](int u, int k) -> float { return w1[(size_t)k * 128 + u]; };
-    auto w2_get = [&](int u, int k) -> float { return w2[(size_t)k * 64 + u]; };
+    const DinBlob ly = DinBlob::of(32, m->spec.hist_len);
+    const float* w1 = B.blob.data() + ly.W1;
+    const float* w2 = B.blob.data() + ly.W2;
     std::vector<uint8_t> img(114688, 0);
-    write_sw128(img.data() + 0, 128, 2, false, w1_get);
-    write_sw128(img.data() + 32768, 128, 2, true, w1_get);
-    write_sw128(img.data() + 65536, 128, 1, false, w1_get, 128, 0, 4);
-    write_sw128(img.data() + 65536, 128, 1, true, w1_get, 128, 4, 4);
-    write_sw128(img.data() + 81920, 64, 2, false, w2_get);
-    write_sw128(img.data() + 98304, 64, 2, true, w2_get);
+    write_wt(img.data() + 0, img.data() + 32768, w1, 5 * 32, 128, 128, 2);
+    write_wt(img.data() + 65536, img.data() + 65536, w1, 5 * 32, 128, 128, 1, 128, 4, 4);
+    write_wt(img.data() + 81920, img.data() + 98304, w2, 128, 64, 64, 2);
     p.mlp_image = B.upload(img);
     if (B.status != SRS_OK) return B.status;
   }
@@ -551,43 +498,21 @@ int build_din_wg(Builder& B) {
   return B.status;
 }
 
-// Tensor-core EmbeddingMLP / W&D (E <= 12): operand images from the tensors build_embmlp validated.
+// Tensor-core EmbeddingMLP / W&D (E <= 12): operand images from the blob build_embmlp placed.
 int build_embmlp_tc(Builder& B) {
   srs_model* m = B.m;
   const srs_spec& s = m->spec;
-  const int E = s.emb_dim, h0 = s.hidden[0], h1 = s.hidden[1];
-  const float* k1 = B.host("dense/kernel", 7 + 10 * E, h0);
-  const float* k2 = B.host("dense_1/kernel", h0, h1);
-  const float* b3 = B.host("dense_2/bias", 1, 1);
-  if (B.status != SRS_OK) return B.status;
-  // K = slot * 12 + e; slot order of the kernel's gather: movieGenre1..3, movieId, userGenre1..5, userId
-  int slot_start[10];
-  for (int k = 0; k < 3; ++k) slot_start[k] = 1 + k * E;
-  slot_start[3] = 1 + 3 * E;
-  for (int k = 0; k < 5; ++k) slot_start[4 + k] = 5 + 4 * E + k * E;
-  slot_start[9] = 5 + 9 * E;
-  auto w1_get = [&](int j, int k) -> float {
-    const int slot = k / 12, e = k - slot * 12;
-    if (j >= h0 || slot >= 10 || e >= E) return 0.f;
-    return k1[(size_t)(slot_start[slot] + e) * h0 + j];
-  };
-  auto w2_get = [&](int j, int k) -> float { return (j < h1 && k < h0) ? k2[(size_t)k * h1 + j] : 0.f; };
+  const EmbMlpBlob ly = EmbMlpBlob::of(12);
+  // W1^T over K = slot * 12 + e (the ten slots; the numerics' rows stay out of the MMA), W2^T
   std::vector<uint8_t> img(131072, 0);
-  write_sw128(img.data() + 0, 128, 2, false, w1_get);
-  write_sw128(img.data() + 32768, 128, 2, true, w1_get);
-  write_sw128(img.data() + 65536, 128, 2, false, w2_get);
-  write_sw128(img.data() + 98304, 128, 2, true, w2_get);
-  const int nrows[7] = {0, 1 + 4 * E, 2 + 4 * E, 3 + 4 * E, 4 + 4 * E, 5 + 10 * E, 6 + 10 * E};
-  std::vector<float> w1num(8 * 128, 0.f);
-  for (int n = 0; n < 7; ++n)
-    for (int j = 0; j < h0; ++j) w1num[(size_t)n * 128 + j] = k1[(size_t)nrows[n] * h0 + j];
+  write_wt(img.data() + 0, img.data() + 32768, B.blob.data() + ly.W1, 10 * 12, 128, 128, 2);
+  write_wt(img.data() + 65536, img.data() + 98304, B.blob.data() + ly.W2, 128, 128, 128, 2);
   EmbMlpTcParams& p = m->emb_tc;
   const EmbMlpParams& v1 = m->emb;
   for (int k = 0; k < 8; ++k) p.genre[k] = v1.genre[k];
   p.movie = v1.movie; p.user = v1.user;
   p.image = B.upload(img);
-  p.b1 = v1.b1; p.b2 = v1.b2; p.w3 = v1.w3; p.wide = v1.wide; p.b3 = b3[0];
-  p.w1num = B.upload(w1num);
+  p.b1 = v1.b1; p.w1_numerics = v1.W1 + 10 * 12 * 128; p.b2 = v1.b2; p.w3 = v1.w3; p.wide = v1.wide; p.b3 = B.blob[ly.b3];
   p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres; p.cross_buckets = s.cross_buckets;
   p.num_sms = m->device_sms;
   m->use_emb_tc = true;
@@ -595,37 +520,22 @@ int build_embmlp_tc(Builder& B) {
   return B.status;
 }
 
-// Tensor-core DeepFM (emb_dim 13..16): operand images from the tensors build_deepfm validated.
+// Tensor-core DeepFM (emb_dim 13..16): operand images from the blob build_deepfm placed.
 int build_deepfm_tc(Builder& B) {
   srs_model* m = B.m;
   const srs_spec& s = m->spec;
-  const int E = s.emb_dim, h0 = s.hidden[0], h1 = s.hidden[1];
-  const float* k1 = B.host("dense/kernel", 7 + 2 * E, h0);
-  const float* k2 = B.host("dense_1/kernel", h0, h1);
-  if (B.status != SRS_OK) return B.status;
-  auto w1_get = [&](int j, int k) -> float {        // K = [deep movieId emb (16) | deep userId emb (16) | 0]
-    if (j >= h0 || k >= 32) return 0.f;
-    const int e = k & 15;
-    if (e >= E) return 0.f;
-    return k1[(size_t)((k < 16 ? 1 : 5 + E) + e) * h0 + j];
-  };
-  auto w2_get = [&](int j, int k) -> float { return (j < h1 && k < h0) ? k2[(size_t)k * h1 + j] : 0.f; };
+  const DeepFmBlob ly = DeepFmBlob::of(16);
+  // W1^T over K = [deep movieId emb (16) | deep userId emb (16) | 0] (the numerics' rows stay out of the MMA), W2^T;
+  // units 64..127 are zero
   std::vector<uint8_t> img(65536, 0);
-  write_sw128(img.data() + 0, 128, 1, false, w1_get);
-  write_sw128(img.data() + 16384, 128, 1, true, w1_get);
-  write_sw128(img.data() + 32768, 128, 1, false, w2_get);
-  write_sw128(img.data() + 49152, 128, 1, true, w2_get);
-  const int nrows[7] = {0, 1 + E, 2 + E, 3 + E, 4 + E, 5 + 2 * E, 6 + 2 * E};
-  std::vector<float> w1num(8 * 64, 0.f);
-  for (int n = 0; n < 7; ++n)
-    for (int j = 0; j < h0; ++j) w1num[(size_t)n * 64 + j] = k1[(size_t)nrows[n] * h0 + j];
+  write_wt(img.data() + 0, img.data() + 16384, B.blob.data() + ly.W1, 2 * 16, 64, 128, 1);
+  write_wt(img.data() + 32768, img.data() + 49152, B.blob.data() + ly.W2, 64, 64, 128, 1);
   DeepFmTcParams& p = m->fm_tc;
   const DeepFmParams& v1 = m->fm;
   p.fm_movie = v1.fm_movie; p.fm_user = v1.fm_user; p.fm_mgenre = v1.fm_mgenre; p.fm_ugenre = v1.fm_ugenre;
   p.deep_movie = v1.deep_movie; p.deep_user = v1.deep_user;
   p.image = B.upload(img);
-  p.b1 = v1.b1; p.b2 = v1.b2; p.first = v1.first; p.wdeep = v1.wdeep;
-  p.w1num = B.upload(w1num);
+  p.b1 = v1.b1; p.w1_numerics = v1.W1 + 2 * 16 * 64; p.b2 = v1.b2; p.first = v1.first; p.wdeep = v1.wdeep;
   for (int d = 0; d < 4; ++d) p.wdot[d] = v1.wdot[d];
   p.bout = v1.bout;
   p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres;
@@ -637,14 +547,14 @@ int build_deepfm_tc(Builder& B) {
 
 // Kernel variant of a model kind whose CUDA-core kernel build_* has built: the tensor-core one (its builder
 // `build_tc`) when the shape `fits` it and `by_default`.  The option `key` (environment variable `env`)
-// overrides: cudacore keeps the CUDA-core kernel; tc (and with `rt_alias`, rt / rtp: the names of the earlier
-// row-tile tensor-core DIN kernels) builds the tensor-core one, or fails loudly on a shape that does not fit.
+// overrides: cudacore keeps the CUDA-core kernel; tc builds the tensor-core one, or fails loudly on a shape that
+// does not fit.
 int choose_kernel(Builder& B, const char* key, const char* env, bool fits, bool by_default, const char* fit_rule,
-                  bool rt_alias, int (*build_tc)(Builder&)) {
+                  int (*build_tc)(Builder&)) {
   const char* impl = opt(key, env);
   bool tc = fits && by_default;
   if (impl && !strcmp(impl, "cudacore")) tc = false;
-  if (impl && (!strcmp(impl, "tc") || (rt_alias && (!strcmp(impl, "rt") || !strcmp(impl, "rtp"))))) {
+  if (impl && !strcmp(impl, "tc")) {
     if (!fits) return fail(SRS_ERR_INVALID, "%s=%s needs %s", env, impl, fit_rule);
     tc = true;
   }
@@ -1124,14 +1034,13 @@ int srs_model_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_
       // tensor cores for the reference shape (E <= 12)
       rc = build_embmlp(B);
       if (rc == SRS_OK)
-        rc = choose_kernel(B, "embmlp_impl", "SRS_EMBMLP_IMPL", m->EP == 12, true, "emb_dim <= 12", false,
-                           build_embmlp_tc);
+        rc = choose_kernel(B, "embmlp_impl", "SRS_EMBMLP_IMPL", m->EP == 12, true, "emb_dim <= 12", build_embmlp_tc);
       break;
     case SRS_DEEPFM:
       // tensor-core deep MLP when emb_dim pads to 16
       rc = build_deepfm(B);
       if (rc == SRS_OK)
-        rc = choose_kernel(B, "deepfm_impl", "SRS_DEEPFM_IMPL", m->EP == 16, true, "12 < emb_dim <= 16", false,
+        rc = choose_kernel(B, "deepfm_impl", "SRS_DEEPFM_IMPL", m->EP == 16, true, "12 < emb_dim <= 16",
                            build_deepfm_tc);
       break;
     case SRS_DEEPFM_V2: rc = build_deepfm2(B); break;
@@ -1143,7 +1052,7 @@ int srs_model_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_
       rc = build_din(B);
       if (rc == SRS_OK)
         rc = choose_kernel(B, "din_impl", "SRS_DIN_IMPL", m->EP == 32 || m->EP == 64, spec->hist_len > 8,
-                           "16 < emb_dim <= 64", true, build_din_wg);
+                           "16 < emb_dim <= 64", build_din_wg);
       break;
   }
   cudaError_t e = cudaSuccess;

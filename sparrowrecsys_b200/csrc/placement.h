@@ -1,9 +1,10 @@
-// placement.h - where the Keras tensors of the trainable models (NeuralCF's neural_cf_model_1 and two towers, DeepFM,
-// DeepFM_v2, EmbeddingMLP / Wide&Deep and DIEN) live on the device, written once for the serving builders (build_ncf,
-// build_deepfm, build_deepfm2, build_embmlp, build_dien in model.cu) and the
-// trainer (srs_trainer_create, srs_trainer_get_weights in trainer.cu): the builders and the trainer scatter the
-// caller's host tensors through it, and the trainer gathers its weights back through it.  Also the by-name lookup of
-// the caller's tensors that both use.  Host code only.
+// placement.h - where the Keras tensors of the serving models (NeuralCF's neural_cf_model_1 and two towers, DeepFM,
+// DeepFM_v2, EmbeddingMLP / Wide&Deep, DIN and DIEN) live on the device, written once for the serving builders
+// (build_ncf, build_deepfm, build_deepfm2, build_embmlp, build_din, build_dien in model.cu; the tensor-core builders
+// derive their operand images from the blobs placed here) and the trainer (srs_trainer_create,
+// srs_trainer_get_weights in trainer.cu): the builders and the trainer scatter the caller's host tensors through it,
+// and the trainer gathers its weights back through it.  Also the by-name lookup of the caller's tensors that both
+// use.  Host code only.
 #pragma once
 
 #include <stdint.h>
@@ -325,12 +326,80 @@ inline void point_into_blob(EmbMlpParams* p, const float* const* tables, const f
   p->w3 = blob + ly.w3; p->b3 = blob + ly.b3;
 }
 
+// The top MLP of DIN and DIEN (dense/kernel .. dense_2/bias with the PReLU alphas) at ly's offsets W1 .. b3.
+// dense/kernel's rows are the concat of the sequence output (DIN's pooled behaviours, DIEN's AUGRU state), the
+// candidate embedding and the user_profile and context DenseFeatures layers, each layer sorted by column name
+// inside; up, seq, cand and ctx are the first rows of the four.  Its tile rows are userGenre1 | userId | sequence |
+// candidate | movieGenre1, then the 7 numerics and one zero row.
+template <class Layout>
+inline void place_top_mlp(Placement& pl, const srs_spec& s, int EP, const Layout& ly, int up, int seq, int cand,
+                          int ctx) {
+  const int E = s.emb_dim, h0 = s.hidden[0], h1 = s.hidden[1];
+  std::vector<int> map;
+  append(map, iota_map(up + 1, E, EP));
+  append(map, iota_map(up + 1 + E, E, EP));
+  append(map, iota_map(seq, E, EP));
+  append(map, iota_map(cand, E, EP));
+  append(map, iota_map(ctx + 1, E, EP));
+  for (int r : {ctx, ctx + 1 + E, ctx + 2 + E, ctx + 3 + E, up, up + 1 + 2 * E, up + 2 + 2 * E, -1}) map.push_back(r);
+  place_dense(pl, "dense/kernel", 5 * E + 7, h0, {Block{false, ly.W1, 128, map}});
+  place_dense(pl, "dense/bias", h0, 1, {Block{false, ly.b1, 1, iota_map(0, h0, 128)}});
+  place_dense(pl, "prelu/alpha", h0, 1, {Block{false, ly.a1, 1, iota_map(0, h0, 128)}});
+  place_dense(pl, "dense_1/kernel", h0, h1, {Block{false, ly.W2, 64, iota_map(0, h0, 128)}});
+  place_dense(pl, "dense_1/bias", h1, 1, {Block{false, ly.b2, 1, iota_map(0, h1, 64)}});
+  place_dense(pl, "prelu_1/alpha", h1, 1, {Block{false, ly.a2, 1, iota_map(0, h1, 64)}});
+  place_dense(pl, "dense_2/kernel", h1, 1, {Block{false, ly.w3, 1, iota_map(0, h1, 64)}});
+  place_dense(pl, "dense_2/bias", 1, 1, {Block{false, ly.b3, 1, iota_map(0, 1, 1)}});
+}
+
+// DIN: the four tables (embedding, userId_embedding, userGenre1_embedding, movieGenre1_embedding) and the Dense
+// tensors in one DinBlob::of(EP, T), looked up in the order the builder has always used.  au_dense/kernel's four
+// E-row groups go unfolded into the blob's W_sub, W_h, W_c and W_prod blocks (build_din folds them).  Fills p's
+// sizes, T and EP.
+inline Placement place_din(const srs_spec& s, int EP, DinParams* p) {
+  const int E = s.emb_dim, T = s.hist_len, A = 32;
+  const DinBlob ly = DinBlob::of(EP, T);
+  Placement pl;
+  place_table(pl, "embedding", s.n_movies, E);
+  place_table(pl, "userId_embedding", s.n_users, E);
+  place_table(pl, "userGenre1_embedding", s.n_genres, E);
+  place_table(pl, "movieGenre1_embedding", s.n_genres, E);
+  // au_dense/kernel's rows are [h - c | h | c | h * c], E each (DIN.py:146-149)
+  const int au[4] = {ly.wsub, ly.wh, ly.wc, ly.wp};
+  std::vector<Block> aub;
+  for (int g = 0; g < 4; ++g) aub.push_back(Block{false, au[g], A, iota_map(g * E, E, EP)});
+  place_dense(pl, "au_dense/kernel", 4 * E, A, std::move(aub));
+  place_dense(pl, "au_dense/bias", A, 1, {Block{false, ly.au_b, 1, iota_map(0, A, A)}});
+  place_dense(pl, "au_prelu/alpha", T, A, {Block{false, ly.au_alpha, A, iota_map(0, T, T)}});
+  place_dense(pl, "au_out/kernel", A, 1, {Block{false, ly.au_wout, 1, iota_map(0, A, A)}});
+  place_dense(pl, "au_out/bias", 1, 1, {Block{false, ly.au_bout, 1, iota_map(0, 1, 1)}});
+  // dense/kernel's rows are [user_profile | pooled | candidate | context] (DIN.py:161-162)
+  place_top_mlp(pl, s, EP, ly, 0, 3 + 2 * E, 3 + 3 * E, 3 + 4 * E);
+  p->n_movies = s.n_movies; p->n_users = s.n_users; p->n_genres = s.n_genres;
+  p->T = T; p->EP = EP;
+  return pl;
+}
+
+// p's tables (tables[k]: the k-th table of place_din's order) and Dense-weight pointers into a folded DinBlob on
+// the device; p->au_bout and p->b3 from the host copy of the blob
+inline void point_into_blob(DinParams* p, const float* const* tables, const float* blob, const float* host_blob) {
+  const DinBlob ly = DinBlob::of(p->EP, p->T);
+  p->movie = tables[0]; p->user = tables[1]; p->ugenre = tables[2]; p->mgenre = tables[3];
+  p->au_wh = blob + ly.wh; p->au_wp = blob + ly.wp; p->au_wc = blob + ly.wc; p->au_b = blob + ly.au_b;
+  p->au_alpha = blob + ly.au_alpha; p->au_wout = blob + ly.au_wout;
+  p->au_bout = host_blob[ly.au_bout];
+  p->W1 = blob + ly.W1; p->b1 = blob + ly.b1; p->a1 = blob + ly.a1;
+  p->W2 = blob + ly.W2; p->b2 = blob + ly.b2; p->a2 = blob + ly.a2;
+  p->w3 = blob + ly.w3;
+  p->b3 = host_blob[ly.b3];
+}
+
 // DIEN: the four tables (embedding, userId_embedding, userGenre1_embedding, movieGenre1_embedding: kDienTables
 // order) and the Dense tensors in one DienLayout::of(EP) blob, looked up in the order the builder has always used;
 // `aux`: with the auxiliary head's group of eight (else its part of the blob stays zero).  The GRU's kernels and
 // biases keep Keras's z | r | h column blocks, each padded to EP.  Fills p's sizes, T and EP.
 inline Placement place_dien(const srs_spec& s, int EP, bool aux, DienParams* p) {
-  const int E = s.emb_dim, h0 = s.hidden[0], h1 = s.hidden[1], A = 32, EE = EP * EP;
+  const int E = s.emb_dim, A = 32, EE = EP * EP;
   const DienLayout ly = DienLayout::of(EP);
   Placement pl;
   place_table(pl, "embedding", s.n_movies, E);
@@ -366,25 +435,8 @@ inline Placement place_dien(const srs_spec& s, int EP, bool aux, DienParams* p) 
     place_dense(pl, name, E, 1, {Block{false, ly.BA + g * EP, 1, iota_map(0, E, E)}});
   }
   place_dense(pl, "augru_h0", 1, E, {Block{false, ly.H0, EP, {0}}});
-  // dense/kernel's rows are [augru | candidate | user_profile | context] (DIEN.py:250), the last two DenseFeatures
-  // layers sorted by column name inside; its tile rows are userGenre1 | userId | augru | candidate | movieGenre1,
-  // then the 7 numerics and one zero row
-  const int up = 2 * E, ctx = 4 * E + 3;
-  std::vector<int> map;
-  append(map, iota_map(up + 1, E, EP));
-  append(map, iota_map(up + 1 + E, E, EP));
-  append(map, iota_map(0, E, EP));
-  append(map, iota_map(E, E, EP));
-  append(map, iota_map(ctx + 1, E, EP));
-  for (int r : {ctx, ctx + 1 + E, ctx + 2 + E, ctx + 3 + E, up, up + 1 + 2 * E, up + 2 + 2 * E, -1}) map.push_back(r);
-  place_dense(pl, "dense/kernel", 5 * E + 7, h0, {Block{false, ly.W1, 128, map}});
-  place_dense(pl, "dense/bias", h0, 1, {Block{false, ly.b1, 1, iota_map(0, h0, 128)}});
-  place_dense(pl, "prelu/alpha", h0, 1, {Block{false, ly.a1, 1, iota_map(0, h0, 128)}});
-  place_dense(pl, "dense_1/kernel", h0, h1, {Block{false, ly.W2, 64, iota_map(0, h0, 128)}});
-  place_dense(pl, "dense_1/bias", h1, 1, {Block{false, ly.b2, 1, iota_map(0, h1, 64)}});
-  place_dense(pl, "prelu_1/alpha", h1, 1, {Block{false, ly.a2, 1, iota_map(0, h1, 64)}});
-  place_dense(pl, "dense_2/kernel", h1, 1, {Block{false, ly.w3, 1, iota_map(0, h1, 64)}});
-  place_dense(pl, "dense_2/bias", 1, 1, {Block{false, ly.b3, 1, iota_map(0, 1, 1)}});
+  // dense/kernel's rows are [augru | candidate | user_profile | context] (DIEN.py:250)
+  place_top_mlp(pl, s, EP, ly, 2 * E, 0, E, 4 * E + 3);
   if (aux) {                                   // [g_t | e] rows: E hidden-state rows, then E item rows
     std::vector<int> amap = iota_map(0, E, EP);
     append(amap, iota_map(E, E, EP));

@@ -398,11 +398,8 @@ def test_launch_counter_counts_kernels():
 
 
 # ---- DIN tensor-core kernel (csrc/din_wg.cu, warpgroup MMAs) vs CUDA-core kernel vs oracle ----
-#      the option values tc, rt and rtp all select it.  "tc" runs it with one CTA per 32-row tile;
-#      "rt" (the row-tile option value) runs it with the grid capped at SM_CAP CTAs, so that every CTA
+#      sm_cap 0 runs it with one CTA per 32-row tile; sm_cap 7 caps the grid at 7 CTAs, so that every CTA
 #      walks several tiles in its grid-stride loop.
-KERNEL_OF = {"tc": "din_wg_kernel", "rt": "din_wg_kernel"}
-SM_CAP = {"tc": 0, "rt": 7}
 
 @pytest.fixture
 def din_impl(monkeypatch):
@@ -414,15 +411,15 @@ def din_impl(monkeypatch):
 @pytest.mark.parametrize("E,T,B", [(32, 50, 4096), (32, 9, 100), (32, 31, 17), (32, 32, 16),
                                    (32, 33, 15), (20, 64, 333), (32, 65, 129), (32, 128, 257),
                                    (24, 100, 1), (32, 50, 4097)])
-@pytest.mark.parametrize("impl", ["tc", "rt"])
-def test_din_tensor_core_kernel(E, T, B, impl, din_impl):
+@pytest.mark.parametrize("sm_cap", [0, 7])
+def test_din_tensor_core_kernel(E, T, B, sm_cap, din_impl):
     spec = default_spec("din", emb_dim=E, hist_len=T, n_movies=27279, n_users=5000)
     W = init_weights(spec, E * 1000 + T)
     feats = synthetic_features(spec, B, seed=T)
-    din_impl(impl)
+    din_impl("tc")
     with _model(spec, W) as m:
-        assert m.kernel_name == KERNEL_OF[impl]
-        m.set_sm_limit(SM_CAP[impl])
+        assert m.kernel_name == "din_wg_kernel"
+        m.set_sm_limit(sm_cap)
         p_tc, z_tc = m.predict_with_logits(feats)
         p_tc2 = m.predict(feats)
     assert np.array_equal(p_tc, p_tc2)                       # deterministic
@@ -445,7 +442,7 @@ def test_din_row_tile_kernel_wide_embeddings(E, T, B, din_impl):
     spec = default_spec("din", emb_dim=E, hist_len=T, n_movies=50_000, n_users=5000)
     W = init_weights(spec, E * 1000 + T)
     feats = synthetic_features(spec, B, seed=T, uniform_history=(T == 200))
-    din_impl("rt")
+    din_impl("tc")
     with _model(spec, W) as m:
         assert m.kernel_name == "din_wg_kernel"
         p_rt, z_rt = m.predict_with_logits(feats)
@@ -462,7 +459,7 @@ def test_din_row_tile_kernel_wide_embeddings(E, T, B, din_impl):
 
 
 def test_din_row_tile_kernel_wide_row_independence(din_impl):
-    din_impl("rt")
+    din_impl("tc")
     spec = default_spec("din", emb_dim=64, hist_len=200, n_movies=300_000, n_users=5000)
     W = init_weights(spec, 7)
     B = 2 * 148 * 32 + 77
@@ -478,37 +475,37 @@ def test_din_row_tile_kernel_wide_row_independence(din_impl):
         assert np.array_equal(np.concatenate([lo, hi]), p)   # sharding invariant
 
 
-@pytest.mark.parametrize("impl", ["tc", "rt"])
-def test_din_tensor_core_row_independence(impl, din_impl):
-    din_impl(impl)
+@pytest.mark.parametrize("sm_cap", [0, 7])
+def test_din_tensor_core_row_independence(sm_cap, din_impl):
+    din_impl("tc")
     spec = baseline_spec("cfg3_din")
     W = init_weights(spec, 3)
     B = 8192 + 5
     feats = synthetic_features(spec, B, seed=3)
     perm = np.random.default_rng(1).permutation(B)
     with _model(spec, W) as m:
-        m.set_sm_limit(SM_CAP[impl])
+        m.set_sm_limit(sm_cap)
         p = m.predict(feats)[:, 0]
         pp = m.predict({k: v[perm] for k, v in feats.items()})[:, 0]
         assert np.array_equal(pp, p[perm])                   # bit-exact under row permutation
-        assert m.kernel_name == KERNEL_OF[impl]
+        assert m.kernel_name == "din_wg_kernel"
         lo = m.predict({k: v[:4099] for k, v in feats.items()})[:, 0]
         hi = m.predict({k: v[4099:] for k, v in feats.items()})[:, 0]
         assert np.array_equal(np.concatenate([lo, hi]), p)   # sharding invariant
 
 
-@pytest.mark.parametrize("impl", ["tc", "rt"])
-def test_din_tensor_core_large_magnitudes(impl, din_impl):
+@pytest.mark.parametrize("sm_cap", [0, 7])
+def test_din_tensor_core_large_magnitudes(sm_cap, din_impl):
     """Trained-scale weights: embeddings O(0.5), logits up to ~10 - the bf16x3 split must hold
     the 1e-4 target with margin where plain TF32/bf16 would not."""
-    din_impl(impl)
+    din_impl("tc")
     spec = baseline_spec("cfg3_din")
     W = init_weights(spec, 5)
     W["embedding"] = (W["embedding"] * 10).astype(np.float32)
     W["dense_2/kernel"] = (W["dense_2/kernel"] * 4).astype(np.float32)
     feats = synthetic_features(spec, 2048, seed=5)
     with _model(spec, W) as m:
-        m.set_sm_limit(SM_CAP[impl])
+        m.set_sm_limit(sm_cap)
         p, z = m.predict_with_logits(feats)
     po, zo = O.forward(spec, W, feats)
     assert np.abs(zo).max() > 2.0
@@ -592,7 +589,7 @@ def test_deepfm_tensor_core_kernel(E, B, monkeypatch):
         assert np.abs(m.predict(feats) - po).max() <= PROB_ATOL
 
 
-# ---- the tensor-core DIN kernel under an SM limit (option value rtp) -----------------------------
+# ---- the tensor-core DIN kernel under an SM limit ----------------------------------------------------
 # din_wg_kernel walks the batch's 32-row tiles in a grid-stride loop; the SM limit decides how many tiles a
 # CTA walks (1 SM: every tile of the batch on one CTA - buffer reuse across tiles, odd last tiles, one-row
 # tiles all get exercised).
@@ -604,7 +601,7 @@ def test_din_rtp_kernel(E, T, B, sms, din_impl):
     spec = default_spec("din", emb_dim=E, hist_len=T, n_movies=27279, n_users=5000)
     W = init_weights(spec, E * 1000 + T)
     feats = synthetic_features(spec, B, seed=T + B)
-    din_impl("rtp")
+    din_impl("tc")
     with _model(spec, W) as m:
         assert m.kernel_name == "din_wg_kernel"
         if sms:
@@ -625,7 +622,7 @@ def test_din_rtp_out_of_range_ids_latch_the_error_flag(din_impl):
     spec = default_spec("din", emb_dim=32, hist_len=50, n_movies=27279, n_users=5000)
     W = init_weights(spec, 1)
     feats = synthetic_features(spec, 300, seed=3)
-    din_impl("rtp")
+    din_impl("tc")
     with _model(spec, W) as m:
         d = m.to_device(feats)
         import torch
