@@ -642,6 +642,18 @@ int srs_als_fit_implicit_host(const int32_t* user_id, const int32_t* movie_id, c
                               int32_t movie_capacity, int32_t* user_ids, float* user_factors, int32_t* n_users,
                               int32_t* movie_ids, float* movie_factors, int32_t* n_movies, double alpha);
 
+/* ALS.fit with nonnegative = true (DESIGN.md section 4.21): srs_als_fit_host's arguments, layouts, init, order and
+ * normal equations - srs_als_fit_implicit_host's, with `alpha`, when implicit_prefs is 1 - but each entity's factor
+ * is Spark's NNLSSolver's: NNLS.solve (projected gradient with conjugate directions, at most max(400, 20 rank)
+ * iterations) on the full symmetric matrix with lambda on its diagonal, each x(i) >= 0, rounded to float.  There is
+ * no singular system: an all-zero system gives a zero factor.  implicit_prefs 0 or 1; checks, errors and outputs
+ * as srs_als_fit_host's, all before any device call.  Synchronous; the same inputs give the same bits. */
+int srs_als_fit_nonnegative_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
+                                 int64_t n_ratings, const srs_als_params* params, int32_t device,
+                                 int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids, float* user_factors,
+                                 int32_t* n_users, int32_t* movie_ids, float* movie_factors, int32_t* n_movies,
+                                 int32_t implicit_prefs, double alpha);
+
 /* Many ALS fits over one rating set in one pass (CrossValidator's fold x grid models, DESIGN.md section 4.15).
  * fold [n_ratings] gives each rating a fold in 0..n_folds-1 (2 <= n_folds <= 65536).  Model m of the n_models
  * (1..64) trains on the ratings outside fold models[m].exclude_fold (-1: on all of them) with its own rank,
@@ -664,6 +676,16 @@ int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* movie_id, cons
                            uint64_t seed, int32_t device, int32_t user_capacity, int32_t movie_capacity,
                            int32_t* user_ids, float* user_factors, int32_t* n_users, int32_t* movie_ids,
                            float* movie_factors, int32_t* n_movies);
+
+/* srs_als_fit_folds_host with a solver per model (DESIGN.md section 4.21): nonnegative [n_models], each 0 or 1
+ * (checked before any device call, SRS_ERR_INVALID).  A model whose flag is 0 gives srs_als_fit_folds_host's bits,
+ * and one whose flag is 1 gives srs_als_fit_nonnegative_host's explicit fit's bits on its training ratings. */
+int srs_als_fit_folds_nonnegative_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
+                                       const int32_t* fold, int64_t n_ratings, int32_t n_folds,
+                                       const srs_als_model* models, int32_t n_models, uint64_t seed, int32_t device,
+                                       int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
+                                       float* user_factors, int32_t* n_users, int32_t* movie_ids,
+                                       float* movie_factors, int32_t* n_movies, const int32_t* nonnegative);
 
 /* ALSModel.recommendForAll: for each of n_src source factors [n_src][rank] (host), the L = min(num, n_dst)
  * destinations of highest score, best first, in out_ids / out_scores [n_src][L].  The score is the float dot

@@ -52,7 +52,8 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_graph_embedding_host", "srs_lsh_transform_host", "srs_lsh_query_host", "srs_approx_quantile_host",
            "srs_quantile_discretizer_host", "srs_bucketize_host", "srs_minmax_scale_host", "srs_rating_features_host",
            "srs_string_indexer_host", "srs_genre_multihot_host", "srs_sample_split_host",
-           "srs_sample_split_by_timestamp_host", "srs_als_fit_implicit_host", "srs_ranking_metrics_host")
+           "srs_sample_split_by_timestamp_host", "srs_als_fit_implicit_host", "srs_ranking_metrics_host",
+           "srs_als_fit_nonnegative_host", "srs_als_fit_folds_nonnegative_host")
 
 _lib = None
 
@@ -271,6 +272,10 @@ def load():
     lib.srs_als_fit_folds_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
                                            C.c_void_p, C.c_int32, C.c_uint64, C.c_int32, C.c_int32, C.c_int32,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.srs_als_fit_nonnegative_host.restype = C.c_int
+    lib.srs_als_fit_nonnegative_host.argtypes = lib.srs_als_fit_host.argtypes + [C.c_int32, C.c_double]
+    lib.srs_als_fit_folds_nonnegative_host.restype = C.c_int
+    lib.srs_als_fit_folds_nonnegative_host.argtypes = lib.srs_als_fit_folds_host.argtypes + [C.c_void_p]
     lib.srs_als_recommend_host.restype = C.c_int
     lib.srs_als_recommend_host.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                            C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]

@@ -16,8 +16,11 @@ them.
 * `als(..., implicit_prefs=True, alpha=...)` is the estimator's implicit-feedback mode (`srs_als_fit_implicit_host`),
   and `ranking_metrics` / `AlsModel.ranking_metrics` are mllib's `RankingMetrics` - precision@k, NDCG@k and MAP -
   with the per-query values on the device (`srs_ranking_metrics_host`; DESIGN.md section 4.17).
+* `als(..., nonnegative=True)` is the estimator's `nonnegative` mode: every factor solved under x >= 0 by Spark's
+  NNLSSolver, explicit or implicit (`srs_als_fit_nonnegative_host`), and a model mapping of `als_folds` /
+  `cross_validate`'s grid may set "nonnegative" (`srs_als_fit_folds_nonnegative_host`; DESIGN.md section 4.21).
 
-    python -m sparrowrecsys_b200.collab ratings.csv [--cv | --implicit [--alpha A]]
+    python -m sparrowrecsys_b200.collab ratings.csv [--nonnegative] [--cv | --implicit [--alpha A]]
 """
 from __future__ import annotations
 
@@ -183,11 +186,13 @@ class AlsModel:
 
 
 def als(ratings: Mapping[str, np.ndarray], rank: int = 10, max_iter: int = 5, reg_param: float = 0.01,
-        seed: int = 0, device: int = 0, implicit_prefs: bool = False, alpha: float = 1.0) -> AlsModel:
+        seed: int = 0, device: int = 0, implicit_prefs: bool = False, alpha: float = 1.0,
+        nonnegative: bool = False) -> AlsModel:
     """ALS.fit on `ratings` (userId, movieId, rating; as `featureeng.load_ratings_csv` returns) on `device`:
     explicit feedback, or with `implicit_prefs` the implicit mode with confidence 1 + alpha |rating| and
-    preference [rating > 0] (DESIGN.md section 4.17).  Ratings are cast to float32 as Spark casts its rating
-    column.  The same inputs give the same bits."""
+    preference [rating > 0] (DESIGN.md section 4.17).  With `nonnegative` every factor is solved under x >= 0 by
+    Spark's NNLSSolver (DESIGN.md section 4.21).  Ratings are cast to float32 as Spark casts its rating column.  The
+    same inputs give the same bits."""
     user = np.ascontiguousarray(ratings["userId"], np.int32)
     movie = np.ascontiguousarray(ratings["movieId"], np.int32)
     rating = np.ascontiguousarray(ratings["rating"], np.float32)
@@ -202,7 +207,9 @@ def als(ratings: Mapping[str, np.ndarray], rank: int = 10, max_iter: int = 5, re
     nu, nm = C.c_int32(0), C.c_int32(0)
     args = (_p(user), _p(movie), _p(rating), n, C.byref(params), device, cu, cm, _p(uids), _p(uf), C.byref(nu),
             _p(mids), _p(mf), C.byref(nm))
-    if implicit_prefs:
+    if nonnegative:
+        _lib.check(_lib.load().srs_als_fit_nonnegative_host(*args, int(bool(implicit_prefs)), float(alpha)))
+    elif implicit_prefs:
         _lib.check(_lib.load().srs_als_fit_implicit_host(*args, float(alpha)))
     else:
         _lib.check(_lib.load().srs_als_fit_host(*args))
@@ -247,8 +254,9 @@ def als_folds(ratings: Mapping[str, np.ndarray], fold, n_folds: int, models: Seq
               device: int = 0) -> List[AlsModel]:
     """Many ALS.fit calls over one rating set in one device pass (`srs_als_fit_folds_host`).  `fold` [n] gives each
     row a fold in 0..n_folds-1; each of the (at most 64) `models` is a mapping with rank, max_iter, reg_param and
-    exclude_fold (-1: train on every row).  Model m trains on the rows outside its excluded fold, and its factors
-    are bit for bit `als` on those rows in input order with its settings and `seed`."""
+    exclude_fold (-1: train on every row), and optionally nonnegative (default False).  Model m trains on the rows
+    outside its excluded fold, and its factors are bit for bit `als` on those rows in input order with its settings
+    and `seed`."""
     user = np.ascontiguousarray(ratings["userId"], np.int32)
     movie = np.ascontiguousarray(ratings["movieId"], np.int32)
     rating = np.ascontiguousarray(ratings["rating"], np.float32)
@@ -266,9 +274,13 @@ def als_folds(ratings: Mapping[str, np.ndarray], fold, n_folds: int, models: Seq
     uids, mids = np.zeros((len(ranks), cu), np.int32), np.zeros((len(ranks), cm), np.int32)
     uf, mf = np.zeros(cu * sum(ranks), np.float32), np.zeros(cm * sum(ranks), np.float32)
     nu, nm = np.zeros(len(ranks), np.int32), np.zeros(len(ranks), np.int32)
-    _lib.check(_lib.load().srs_als_fit_folds_host(_p(user), _p(movie), _p(rating), _p(fold), n, int(n_folds), specs,
-                                                  M, int(seed) & _M64, device, cu, cm, _p(uids), _p(uf), _p(nu),
-                                                  _p(mids), _p(mf), _p(nm)))
+    args = (_p(user), _p(movie), _p(rating), _p(fold), n, int(n_folds), specs, M, int(seed) & _M64, device, cu, cm,
+            _p(uids), _p(uf), _p(nu), _p(mids), _p(mf), _p(nm))
+    nonneg = np.array([int(bool(p.get("nonnegative", False))) for p in models] or [0], np.int32)
+    if nonneg.any():
+        _lib.check(_lib.load().srs_als_fit_folds_nonnegative_host(*args, _p(nonneg)))
+    else:
+        _lib.check(_lib.load().srs_als_fit_folds_host(*args))
     out, r0 = [], 0
     for m, k in enumerate(ranks[:M]):
         U = uf[cu * r0:cu * (r0 + k)].reshape(cu, k)
@@ -312,7 +324,7 @@ def mae(labels, predictions) -> float:
 
 
 METRICS = {"rmse": rmse, "mse": mse, "mae": mae}
-_GRID_PARAMS = ("rank", "reg_param", "max_iter")
+_GRID_PARAMS = ("rank", "reg_param", "max_iter", "nonnegative")
 
 
 def fold_ids(n: int, num_folds: int, seed: int = 0) -> np.ndarray:
@@ -342,7 +354,7 @@ def k_fold(n: int, num_folds: int, seed: int = 0):
 
 def param_maps(param_grid) -> List[dict]:
     """ParamGridBuilder.build over an ordered list of (param, values) pairs (or a dict, in its order) of "rank",
-    "reg_param" and "max_iter": every combination, the first param varying fastest.  No params give one empty
+    "reg_param", "max_iter" and "nonnegative": every combination, the first param varying fastest.  No params give one empty
     map, as Spark's builder does; a param with no values gives none, which is an error here."""
     pairs = list(param_grid.items()) if isinstance(param_grid, Mapping) else [tuple(p) for p in param_grid]
     names = [p[0] for p in pairs]
@@ -407,17 +419,21 @@ class CrossValidation:
 
 def cross_validate(ratings: Mapping[str, np.ndarray], param_grid, num_folds: int = 10, metric: str = "rmse",
                    cold_start_strategy: str = "nan", seed: int = 0, rank: int = 10, max_iter: int = 5,
-                   reg_param: float = 0.01, als_seed: int = 0, device: int = 0) -> CrossValidation:
+                   reg_param: float = 0.01, als_seed: int = 0, device: int = 0,
+                   nonnegative: bool = False) -> CrossValidation:
     """CrossValidator(ALS, RegressionEvaluator(metric), param_grid, num_folds).fit(ratings) on the device.  Every
     fold x grid model is trained in batched passes of at most 64 models (`als_folds`); params not in the grid take
-    rank, max_iter and reg_param, and every fit uses `als_seed`.  Each model predicts its validation rows with
+    rank, max_iter, reg_param and nonnegative, and every fit uses `als_seed`.  Each model predicts its validation rows with
     `cold_start_strategy` ("nan", the estimator's default, makes a fold with a cold row score NaN), avg_metrics[p]
     is the fold-order sum over k, and the best point (`best_index`) is refit on all rows by `als`."""
     if metric not in METRICS:
         raise ValueError("metric must be one of %s, not %r" % (sorted(METRICS), metric))
     if cold_start_strategy not in ("drop", "nan"):
         raise ValueError("cold_start_strategy must be 'drop' or 'nan', not %r" % (cold_start_strategy,))
-    points = [dict(dict(rank=rank, max_iter=max_iter, reg_param=reg_param), **pm) for pm in param_maps(param_grid)]
+    base = dict(rank=rank, max_iter=max_iter, reg_param=reg_param)
+    if nonnegative:                                         # a call that never mentions it keeps today's maps
+        base["nonnegative"] = True
+    points = [dict(base, **pm) for pm in param_maps(param_grid)]
     k, P = int(num_folds), len(points)
     n = len(ratings["userId"])
     fold = fold_ids(n, k, seed)
@@ -436,7 +452,8 @@ def cross_validate(ratings: Mapping[str, np.ndarray], param_grid, num_folds: int
         fold_metrics.append(row)
     avg = average_metrics(fold_metrics)
     best = best_index(avg)
-    model = als(ratings, points[best]["rank"], points[best]["max_iter"], points[best]["reg_param"], als_seed, device)
+    model = als(ratings, points[best]["rank"], points[best]["max_iter"], points[best]["reg_param"], als_seed, device,
+                nonnegative=bool(points[best].get("nonnegative", False)))
     return CrossValidation(avg, fold_metrics, best, dict(points[best]), model, points, cold)
 
 
@@ -448,7 +465,8 @@ def _show(title, ids, rec, sc, rows=10):
 
 def main(argv=None) -> int:
     argv = list(sys.argv[1:] if argv is None else argv)
-    usage = "usage: python -m sparrowrecsys_b200.collab ratings.csv [--cv | --implicit [--alpha A]]\n"
+    usage = ("usage: python -m sparrowrecsys_b200.collab ratings.csv [--nonnegative] "
+             "[--cv | --implicit [--alpha A]]\n")
     alpha = 1.0
     if "--alpha" in argv:
         at = argv.index("--alpha")
@@ -461,8 +479,8 @@ def main(argv=None) -> int:
         if "--implicit" not in argv:
             sys.stderr.write(usage)
             return 2
-    cv, implicit = "--cv" in argv, "--implicit" in argv
-    args = [a for a in argv if a not in ("--cv", "--implicit")]
+    cv, implicit, nonneg = "--cv" in argv, "--implicit" in argv, "--nonnegative" in argv
+    args = [a for a in argv if a not in ("--cv", "--implicit", "--nonnegative")]
     if len(args) != 1 or (cv and implicit):                 # CrossValidator has no ranking evaluator
         sys.stderr.write(usage)
         return 2
@@ -471,7 +489,8 @@ def main(argv=None) -> int:
     train_rows, test_rows = random_split(len(r["userId"]), (0.8, 0.2), seed=0)
     train = {k: v[train_rows] for k, v in r.items()}
     test = {k: v[test_rows] for k, v in r.items()}
-    model = als(train, rank=10, max_iter=5, reg_param=0.01, seed=0, implicit_prefs=implicit, alpha=alpha)
+    model = als(train, rank=10, max_iter=5, reg_param=0.01, seed=0, implicit_prefs=implicit, alpha=alpha,
+                nonnegative=nonneg)
     for name, ids, f in (("itemFactors", model.item_ids, model.item_factors),
                          ("userFactors", model.user_ids, model.user_factors)):
         print(name)
@@ -494,7 +513,7 @@ def main(argv=None) -> int:
     _show("userSubsetRecs", *model.recommend_for_user_subset(users, 10))
     _show("movieSubSetRecs", *model.recommend_for_item_subset(movies, 10))
     if cv:                                                  # cv.fit(test): regParam grid [0.01], 10 folds
-        res = cross_validate(test, [("reg_param", [0.01])], num_folds=10)
+        res = cross_validate(test, [("reg_param", [0.01])], num_folds=10, nonnegative=nonneg)
         print("avgMetrics = %r" % res.avg_metrics)
         print("cold validation rows per fold = %r" % res.cold_rows)
     return 0

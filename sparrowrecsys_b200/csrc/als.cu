@@ -29,6 +29,10 @@
 // in block order, and als_solve_kernel<false, true> starts each entity's ata from YtY and adds each rating's
 // confidence and preference terms.
 //
+// srs_als_fit_nonnegative_host and srs_als_fit_folds_nonnegative_host (DESIGN.md section 4.21) are these fits with
+// Spark's nonnegative = true: als_solve_kernel<..., true> keeps the accumulation and replaces the Cholesky tail by
+// NNLS.solve on one warp (nnls_warp); a batched fit launches its NNLS models over their own slice of the model list.
+//
 // srs_ranking_metrics_host: RankingMetrics' per-query precision@k, NDCG@k and average precision, one warp per
 // query (ranking_metrics_kernel), over each query's labels sorted on the device; the means on the host.
 //
@@ -165,12 +169,161 @@ struct Implicit {
   double alpha;
 };
 
+// NNLS.solve's wall test: step dir(i) > x(i) (1 - 1e-14)
+constexpr double kWallShrink = 1.0 - 1e-14;
+
+// element (i, j) of the symmetric matrix whose upper triangle is the packed P
+__device__ __forceinline__ double nnls_sym(const double* P, int i, int j) {
+  return i <= j ? P[j * (j + 1) / 2 + i] : P[i * (i + 1) / 2 + j];
+}
+
+// row i of dgemv "N" (y = A v, beta 0): from 0, columns j ascending with v(j) != 0, y += (1.0 v(j)) A(i,j)
+__device__ __forceinline__ double nnls_row(const double* P, const double* v, int i, int k) {
+  double y = 0.0;
+  for (int j = 0; j < k; ++j) {
+    const double vj = v[j];
+    if (vj != 0.0) y = __dadd_rn(y, __dmul_rn(vj, nnls_sym(P, i, j)));
+  }
+  return y;
+}
+
+// NNLS.solve's stop(step, ndir, nx)
+__device__ __forceinline__ bool nnls_stop(double step, double ndir, double nx) {
+  return step != step || step < 1e-7 || step > 1e40 || ndir < __dmul_rn(1e-12, nx) || ndir < 1e-32;
+}
+
+// Spark's NNLS.solve(ata, atb) on one warp (DESIGN.md section 4.21): P the packed upper ata with lambda on its
+// diagonal, B atb, ws [5][k] doubles of shared scratch; out [k] = x(i).toFloat.  Lane t owns rows t and t + 32 of x,
+// res, grad and dir.  The vectors the sums read are published in ws; every lane runs each sequential sum (ddot
+// from 0, i ascending) and the step-7 scan over them, so the scalars are the same on every lane and need no
+// broadcast.  Each operation is one explicitly rounded intrinsic.
+__device__ void nnls_warp(const double* P, const double* B, double* ws, int k, float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  double* sx = ws;                                      // x
+  double* sg = ws + k;                                  // grad
+  double* sd = ws + 2 * k;                              // dir
+  double* sr = ws + 3 * k;                              // res
+  double* sa = ws + 4 * k;                              // A grad, then A dir
+  double x[2], b[2], ld[2], g[2], d[2];
+#pragma unroll
+  for (int q = 0; q < 2; ++q) {
+    const int i = lane + 32 * q;
+    x[q] = ld[q] = g[q] = d[q] = 0.0;
+    b[q] = i < k ? B[i] : 0.0;
+    if (i < k) sx[i] = 0.0;
+  }
+  const int iter_max = max(400, 20 * k);
+  double last_norm = 0.0;
+  int iterno = 0, last_wall = 0;
+  __syncwarp();
+  while (iterno < iter_max) {
+    // res = A x - atb; grad = res, zero where it points out of the orthant at a bound
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const int i = lane + 32 * q;
+      if (i < k) {
+        const double res = __dsub_rn(nnls_row(P, sx, i, k), b[q]);
+        g[q] = res > 0.0 && x[q] == 0.0 ? 0.0 : res;
+        sr[i] = res;
+        sg[i] = g[q];
+      }
+    }
+    __syncwarp();
+#pragma unroll
+    for (int q = 0; q < 2; ++q)
+      if (lane + 32 * q < k) sa[lane + 32 * q] = nnls_row(P, sg, lane + 32 * q, k);
+    __syncwarp();
+    double ngrad = 0.0, top = 0.0, den = 0.0, nx = 0.0;   // ddot(grad, grad), ddot(grad, res), ddot(A grad, grad), ddot(x, x)
+    for (int j = 0; j < k; ++j) {
+      const double gj = sg[j], xj = sx[j];
+      ngrad = __dadd_rn(ngrad, __dmul_rn(gj, gj));
+      top = __dadd_rn(top, __dmul_rn(gj, sr[j]));
+      den = __dadd_rn(den, __dmul_rn(sa[j], gj));
+      nx = __dadd_rn(nx, __dmul_rn(xj, xj));
+    }
+    double step = __ddiv_rn(top, __dadd_rn(den, 1e-20));
+    double ndir = ngrad;                                // ddot(grad, grad) again, the same bits
+    bool cg = false;
+    if (iterno > last_wall + 1) {                       // the conjugate direction dir = grad + (ngrad / lastNorm) lastDir
+      const double alpha = __ddiv_rn(ngrad, last_norm);
+      __syncwarp();                                     // sa is read
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        const int i = lane + 32 * q;
+        if (i < k) {
+          d[q] = alpha != 0.0 ? __dadd_rn(g[q], __dmul_rn(alpha, ld[q])) : g[q];   // daxpy returns for alpha 0
+          sd[i] = d[q];
+        }
+      }
+      __syncwarp();
+#pragma unroll
+      for (int q = 0; q < 2; ++q)
+        if (lane + 32 * q < k) sa[lane + 32 * q] = nnls_row(P, sd, lane + 32 * q, k);
+      __syncwarp();
+      double top2 = 0.0, den2 = 0.0, nd = 0.0;
+      for (int j = 0; j < k; ++j) {
+        const double dj = sd[j];
+        top2 = __dadd_rn(top2, __dmul_rn(dj, sr[j]));
+        den2 = __dadd_rn(den2, __dmul_rn(sa[j], dj));
+        nd = __dadd_rn(nd, __dmul_rn(dj, dj));
+      }
+      const double dstep = __ddiv_rn(top2, __dadd_rn(den2, 1e-20));
+      if (!nnls_stop(dstep, nd, nx)) {
+        step = dstep;
+        ndir = nd;
+        cg = true;
+      }
+    }
+    if (nnls_stop(step, ndir, nx)) break;
+    __syncwarp();                                       // sd is read
+    if (!cg)
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        const int i = lane + 32 * q;
+        d[q] = g[q];
+        if (i < k) sd[i] = g[q];
+      }
+    __syncwarp();
+    for (int j = 0; j < k; ++j) {                       // don't run through the walls: in order, each j sees the step
+      const double dj = sd[j], xj = sx[j];              // the ones before it left
+      if (__dmul_rn(step, dj) > xj) step = __ddiv_rn(xj, dj);
+    }
+    bool wall = false;
+#pragma unroll
+    for (int q = 0; q < 2; ++q)
+      if (lane + 32 * q < k) {
+        const double sdv = __dmul_rn(step, d[q]);
+        if (sdv > __dmul_rn(x[q], kWallShrink)) {
+          x[q] = 0.0;
+          wall = true;
+        } else {
+          x[q] = __dsub_rn(x[q], sdv);
+        }
+      }
+    if (__any_sync(kFull, wall)) last_wall = iterno;
+    __syncwarp();                                       // sx is read
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      if (lane + 32 * q < k) sx[lane + 32 * q] = x[q];
+      ld[q] = d[q];
+    }
+    last_norm = ngrad;
+    ++iterno;
+    __syncwarp();
+  }
+#pragma unroll
+  for (int q = 0; q < 2; ++q)
+    if (lane + 32 * q < k) out[lane + 32 * q] = __double2float_rn(x[q]);
+}
+
 // One block per entity (the blockIdx.x-th longest; batched: block b is model b % M's (b / M)-th longest entity):
 // NormalEquation.add over its ratings, then CholeskySolver.solve(ne, n * regParam) (dppsv "U": dpptrf, then
 // dpptrs's two dtpsv).  A batched model skips its excluded fold's ratings, so its n counts the rest; an entity with
 // none is not in that model and its block writes nothing but the count.  Implicit: ata starts as YtY, each rating
-// adds dspr(c1) and, when positive, daxpy(1 + c1) (c1 = alpha |r|), and n counts the positive ratings.
-template <bool kBatch, bool kImplicit = false>
+// adds dspr(c1) and, when positive, daxpy(1 + c1) (c1 = alpha |r|), and n counts the positive ratings.  Nonneg:
+// NNLSSolver.solve in place of the Cholesky tail - warp 0 runs NNLS.solve on the same system (nnls_warp, its
+// vectors in the staging area the accumulation no longer needs); there is no singular system.
+template <bool kBatch, bool kImplicit = false, bool kNonneg = false>
 __global__ void __launch_bounds__(kSolveThreads) als_solve_kernel(Side sd, const float* __restrict__ srcF,
                                                                   float* __restrict__ dstF, int k, double reg,
                                                                   unsigned long long* __restrict__ err,
@@ -278,6 +431,10 @@ __global__ void __launch_bounds__(kSolveThreads) als_solve_kernel(Side sd, const
   const double lambda = __dmul_rn((double)n_train, reg);
   if (tid < k) P[tid * (tid + 1) / 2 + tid] = __dadd_rn(P[tid * (tid + 1) / 2 + tid], lambda);
   __syncthreads();
+  if (kNonneg) {                                        // fillAtA's matrix is P read symmetrically
+    if (tid < 32) nnls_warp(P, B, reinterpret_cast<double*>(s_x), k, dstF + (size_t)ent * k);
+    return;
+  }
   // dpptrf "U": in step r, U(r,r) = sqrt(a(r,r) - ddot(U(0:r,r), U(0:r,r))), then for c > r
   // U(r,c) = (a(r,c) - U(0,r) U(0,c) - ... - U(r-1,r) U(r-1,c)) / U(r,r): dtpsv's element, subtracted in order
   const int c = tid;
@@ -653,9 +810,10 @@ int build_layouts(HostCall& c, const int32_t* user_id, const int32_t* movie_id, 
   return SRS_OK;
 }
 
-// srs_als_fit_host and srs_als_fit_implicit_host: every check, then the fit.  `alpha` null: explicit feedback.
+// srs_als_fit_host, srs_als_fit_implicit_host and srs_als_fit_nonnegative_host: every check, then the fit.
+// `alpha` null: explicit feedback; `nonneg`: NNLSSolver in place of CholeskySolver.
 int fit_single(const int32_t* user_id, const int32_t* movie_id, const float* rating, int64_t n_ratings,
-               const srs_als_params* params, const double* alpha, int32_t device, int32_t user_capacity,
+               const srs_als_params* params, const double* alpha, bool nonneg, int32_t device, int32_t user_capacity,
                int32_t movie_capacity, int32_t* user_ids, float* user_factors, int32_t* n_users, int32_t* movie_ids,
                float* movie_factors, int32_t* n_movies) {
   if (!n_users || !n_movies) return failf(SRS_ERR_INVALID, "null n_users or n_movies");
@@ -690,12 +848,13 @@ int fit_single(const int32_t* user_id, const int32_t* movie_id, const float* rat
   CUDA_TRY(cudaMemsetAsync(d_err, 0xff, sizeof(unsigned long long), s));
   const size_t sm = solve_smem(k);
   if (!alpha) {
+    auto* solve = nonneg ? als_solve_kernel<false, false, true> : als_solve_kernel<false>;
     for (int it = 0; it < hp.max_iter; ++it) {
-      als_solve_kernel<false><<<nM, kSolveThreads, sm, s>>>(L.movies, d_uf, d_mf, k, hp.reg_param, d_err, 2ull * it,
-                                                            Batch{}, Implicit{});
+      solve<<<nM, kSolveThreads, sm, s>>>(L.movies, d_uf, d_mf, k, hp.reg_param, d_err, 2ull * it, Batch{},
+                                          Implicit{});
       LAUNCHED();
-      als_solve_kernel<false><<<nU, kSolveThreads, sm, s>>>(L.users, d_mf, d_uf, k, hp.reg_param, d_err,
-                                                            2ull * it + 1, Batch{}, Implicit{});
+      solve<<<nU, kSolveThreads, sm, s>>>(L.users, d_mf, d_uf, k, hp.reg_param, d_err, 2ull * it + 1, Batch{},
+                                          Implicit{});
       LAUNCHED();
     }
   } else {
@@ -724,6 +883,7 @@ int fit_single(const int32_t* user_id, const int32_t* movie_id, const float* rat
     CUDA_TRY(sc.alloc(&d_part, (size_t)kYtyBlocks * nA)); CUDA_TRY(sc.alloc(&d_yty, nA));
     const dim3 yg((nA + kYtyThreads - 1) / kYtyThreads, kYtyBlocks);
     const Implicit im{d_yty, *alpha};
+    auto* solve = nonneg ? als_solve_kernel<false, true, true> : als_solve_kernel<false, true>;
     for (int it = 0; it < hp.max_iter; ++it)
       for (int half = 0; half < 2; ++half) {            // the movies from the users, then the users from the movies
         const bool to_users = half == 1;
@@ -733,9 +893,9 @@ int fit_single(const int32_t* user_id, const int32_t* movie_id, const float* rat
         LAUNCHED();
         als_yty_merge_kernel<<<grid_for(nA, 256), 256, 0, s>>>(d_part, nA, d_yty);
         LAUNCHED();
-        als_solve_kernel<false, true><<<to_users ? nU : nM, kSolveThreads, sm, s>>>(
-            to_users ? L.users : L.movies, src, to_users ? d_uf : d_mf, k, hp.reg_param, d_err, 2ull * it + half,
-            Batch{}, im);
+        solve<<<to_users ? nU : nM, kSolveThreads, sm, s>>>(to_users ? L.users : L.movies, src,
+                                                            to_users ? d_uf : d_mf, k, hp.reg_param, d_err,
+                                                            2ull * it + half, Batch{}, im);
         LAUNCHED();
       }
   }
@@ -767,7 +927,7 @@ extern "C" int srs_als_fit_host(const int32_t* user_id, const int32_t* movie_id,
                                 int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
                                 float* user_factors, int32_t* n_users, int32_t* movie_ids, float* movie_factors,
                                 int32_t* n_movies) {
-  return srs::fit_single(user_id, movie_id, rating, n_ratings, params, nullptr, device, user_capacity,
+  return srs::fit_single(user_id, movie_id, rating, n_ratings, params, nullptr, false, device, user_capacity,
                          movie_capacity, user_ids, user_factors, n_users, movie_ids, movie_factors, n_movies);
 }
 
@@ -776,18 +936,38 @@ extern "C" int srs_als_fit_implicit_host(const int32_t* user_id, const int32_t* 
                                          int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
                                          float* user_factors, int32_t* n_users, int32_t* movie_ids,
                                          float* movie_factors, int32_t* n_movies, double alpha) {
-  return srs::fit_single(user_id, movie_id, rating, n_ratings, params, &alpha, device, user_capacity,
+  return srs::fit_single(user_id, movie_id, rating, n_ratings, params, &alpha, false, device, user_capacity,
                          movie_capacity, user_ids, user_factors, n_users, movie_ids, movie_factors, n_movies);
+}
+
+extern "C" int srs_als_fit_nonnegative_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
+                                            int64_t n_ratings, const srs_als_params* params, int32_t device,
+                                            int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
+                                            float* user_factors, int32_t* n_users, int32_t* movie_ids,
+                                            float* movie_factors, int32_t* n_movies, int32_t implicit_prefs,
+                                            double alpha) {
+  if (implicit_prefs != 0 && implicit_prefs != 1) {
+    if (n_users) *n_users = 0;
+    if (n_movies) *n_movies = 0;
+    return srs::failf(SRS_ERR_INVALID, "implicit_prefs %d is not 0 or 1", implicit_prefs);
+  }
+  return srs::fit_single(user_id, movie_id, rating, n_ratings, params, implicit_prefs ? &alpha : nullptr, true,
+                         device, user_capacity, movie_capacity, user_ids, user_factors, n_users, movie_ids,
+                         movie_factors, n_movies);
 }
 
 using namespace srs;
 
-extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
-                                      const int32_t* fold, int64_t n_ratings, int32_t n_folds,
-                                      const srs_als_model* models, int32_t n_models, uint64_t seed, int32_t device,
-                                      int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
-                                      float* user_factors, int32_t* n_users, int32_t* movie_ids,
-                                      float* movie_factors, int32_t* n_movies) {
+namespace {
+
+// srs_als_fit_folds_host and srs_als_fit_folds_nonnegative_host: every check, then the batched fit.  `nonneg`
+// [n_models] (null: none) picks each model's solver; the NNLS models run in a launch of their own per half-step,
+// over their own slice of the model list.
+int fit_folds(const int32_t* user_id, const int32_t* movie_id, const float* rating, const int32_t* fold,
+              int64_t n_ratings, int32_t n_folds, const srs_als_model* models, const int32_t* nonneg,
+              int32_t n_models, uint64_t seed, int32_t device, int32_t user_capacity, int32_t movie_capacity,
+              int32_t* user_ids, float* user_factors, int32_t* n_users, int32_t* movie_ids, float* movie_factors,
+              int32_t* n_movies) {
   if (n_models < 1 || n_models > kMaxModels)
     return failf(SRS_ERR_INVALID, "n_models %d outside 1..%d", n_models, kMaxModels);
   if (!models || !n_users || !n_movies) return failf(SRS_ERR_INVALID, "null models, n_users or n_movies");
@@ -800,6 +980,8 @@ extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* mov
       return failf(rc, "model %d: %s", m, srs_last_error());
     if (md[m].exclude_fold < -1 || md[m].exclude_fold >= n_folds)
       return failf(SRS_ERR_INVALID, "model %d: exclude_fold %d outside -1..%d", m, md[m].exclude_fold, n_folds - 1);
+    if (nonneg && nonneg[m] != 0 && nonneg[m] != 1)
+      return failf(SRS_ERR_INVALID, "model %d: nonnegative %d is not 0 or 1", m, nonneg[m]);
   }
   PROPAGATE(check_ratings(user_id, movie_id, rating, n_ratings));
   if (!fold) return failf(SRS_ERR_INVALID, "null fold");
@@ -837,6 +1019,13 @@ extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* mov
     kmax = std::max(kmax, md[m].rank);
     half_steps = std::max(half_steps, 2 * md[m].max_iter);
   }
+  // slot[m]: model m's place in the device list - the Cholesky models first, then the M_nn NNLS models
+  std::vector<int> slot(M);
+  int M_nn = 0;
+  for (int m = 0; m < M; ++m) M_nn += nonneg && nonneg[m];
+  for (int m = 0, a = 0, b = M - M_nn; m < M; ++m) slot[m] = nonneg && nonneg[m] ? b++ : a++;
+  std::vector<BatchModel> dev_bm(M);
+  for (int m = 0; m < M; ++m) dev_bm[slot[m]] = bm[m];
   std::vector<float> init(uf_total);
   std::vector<int> drawn(kMaxRank + 1, -1);            // the first model of each rank
   for (int m = 0; m < M; ++m) {
@@ -859,29 +1048,41 @@ extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* mov
   CUDA_TRY(sc.alloc(&d_models, M)); CUDA_TRY(sc.alloc(&d_err, M));
   CUDA_TRY(cudaMemcpyAsync(d_fold, fold, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
   CUDA_TRY(cudaMemcpyAsync(d_uf, init.data(), sizeof(float) * uf_total, cudaMemcpyHostToDevice, s));
-  CUDA_TRY(cudaMemcpyAsync(d_models, bm.data(), sizeof(BatchModel) * M, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(d_models, dev_bm.data(), sizeof(BatchModel) * M, cudaMemcpyHostToDevice, s));
   CUDA_TRY(cudaMemsetAsync(d_err, 0xff, sizeof(unsigned long long) * M, s));
   als_key_kernel<<<G, T, 0, s>>>(L.d_bm, d_fold, n, d_fold_m);      // each layout's fold ids
   LAUNCHED();
   als_key_kernel<<<G, T, 0, s>>>(L.d_bu, d_fold, n, d_fold_u);
   LAUNCHED();
-  // one launch per half-step for every model: a model past its max_iter exits at once
+  // one launch per half-step for every Cholesky model and one for every NNLS model: a model past its max_iter
+  // exits at once
   const size_t sm = solve_smem(kmax);
+  const int M_ch = M - M_nn;
   for (int h = 0; h < half_steps; ++h) {
     const bool to_users = h & 1;
-    const Batch bt{d_models, to_users ? d_fold_u : d_fold_m, to_users ? d_cnt_u : d_cnt_m, M, to_users};
     const int nE = to_users ? nU : nM;
-    als_solve_kernel<true><<<(unsigned)((int64_t)nE * M), kSolveThreads, sm, s>>>(
-        to_users ? L.users : L.movies, to_users ? d_mf : d_uf, to_users ? d_uf : d_mf, 0, 0.0, d_err,
-        (unsigned long long)h, bt, Implicit{});
-    LAUNCHED();
+    int32_t* cnt = to_users ? d_cnt_u : d_cnt_m;
+    const int32_t* fd = to_users ? d_fold_u : d_fold_m;
+    if (M_ch > 0) {
+      als_solve_kernel<true><<<(unsigned)((int64_t)nE * M_ch), kSolveThreads, sm, s>>>(
+          to_users ? L.users : L.movies, to_users ? d_mf : d_uf, to_users ? d_uf : d_mf, 0, 0.0, d_err,
+          (unsigned long long)h, Batch{d_models, fd, cnt, M_ch, to_users}, Implicit{});
+      LAUNCHED();
+    }
+    if (M_nn > 0) {
+      als_solve_kernel<true, false, true><<<(unsigned)((int64_t)nE * M_nn), kSolveThreads, sm, s>>>(
+          to_users ? L.users : L.movies, to_users ? d_mf : d_uf, to_users ? d_uf : d_mf, 0, 0.0, d_err + M_ch,
+          (unsigned long long)h, Batch{d_models + M_ch, fd, cnt + (size_t)M_ch * nE, M_nn, to_users}, Implicit{});
+      LAUNCHED();
+    }
   }
   std::vector<unsigned long long> err(M);
   CUDA_TRY(cudaMemcpyAsync(err.data(), d_err, sizeof(unsigned long long) * M, cudaMemcpyDeviceToHost, s));
   CUDA_TRY(cudaStreamSynchronize(s));
   for (int m = 0; m < M; ++m) {
-    if (err[m] == ~0ull) continue;
-    const int hs = (int)(err[m] >> 32), ent = (int)(err[m] & 0xffffffffu);
+    const unsigned long long e = err[slot[m]];
+    if (e == ~0ull) continue;
+    const int hs = (int)(e >> 32), ent = (int)(e & 0xffffffffu);
     int32_t id = 0;
     CUDA_TRY(cudaMemcpy(&id, (hs & 1 ? L.d_uids : L.d_mids) + ent, sizeof(int32_t), cudaMemcpyDeviceToHost));
     return failf(SRS_ERR_INVALID,
@@ -902,13 +1103,13 @@ extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* mov
     const int k = md[m].rank;
     int32_t nu = 0, nm = 0;
     for (int u = 0; u < nU; ++u) {
-      if (!cnt_u[(size_t)m * nU + u]) continue;
+      if (!cnt_u[(size_t)slot[m] * nU + u]) continue;
       user_ids[(size_t)m * user_capacity + nu] = L.uid[u];
       std::copy_n(uf.data() + bm[m].user_off + (size_t)u * k, k, user_factors + uo + (size_t)nu * k);
       ++nu;
     }
     for (int e = 0; e < nM; ++e) {
-      if (!cnt_m[(size_t)m * nM + e]) continue;
+      if (!cnt_m[(size_t)slot[m] * nM + e]) continue;
       movie_ids[(size_t)m * movie_capacity + nm] = mid[e];
       std::copy_n(mf.data() + bm[m].movie_off + (size_t)e * k, k, movie_factors + mo + (size_t)nm * k);
       ++nm;
@@ -919,6 +1120,36 @@ extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* mov
     mo += (size_t)movie_capacity * k;
   }
   return SRS_OK;
+}
+
+}  // namespace
+
+extern "C" int srs_als_fit_folds_host(const int32_t* user_id, const int32_t* movie_id, const float* rating,
+                                      const int32_t* fold, int64_t n_ratings, int32_t n_folds,
+                                      const srs_als_model* models, int32_t n_models, uint64_t seed, int32_t device,
+                                      int32_t user_capacity, int32_t movie_capacity, int32_t* user_ids,
+                                      float* user_factors, int32_t* n_users, int32_t* movie_ids,
+                                      float* movie_factors, int32_t* n_movies) {
+  return fit_folds(user_id, movie_id, rating, fold, n_ratings, n_folds, models, nullptr, n_models, seed, device,
+                   user_capacity, movie_capacity, user_ids, user_factors, n_users, movie_ids, movie_factors, n_movies);
+}
+
+extern "C" int srs_als_fit_folds_nonnegative_host(const int32_t* user_id, const int32_t* movie_id,
+                                                  const float* rating, const int32_t* fold, int64_t n_ratings,
+                                                  int32_t n_folds, const srs_als_model* models, int32_t n_models,
+                                                  uint64_t seed, int32_t device, int32_t user_capacity,
+                                                  int32_t movie_capacity, int32_t* user_ids, float* user_factors,
+                                                  int32_t* n_users, int32_t* movie_ids, float* movie_factors,
+                                                  int32_t* n_movies, const int32_t* nonnegative) {
+  if (!nonnegative) {
+    if (n_users && n_models >= 1 && n_models <= kMaxModels)
+      for (int m = 0; m < n_models; ++m) n_users[m] = 0;
+    if (n_movies && n_models >= 1 && n_models <= kMaxModels)
+      for (int m = 0; m < n_models; ++m) n_movies[m] = 0;
+    return failf(SRS_ERR_INVALID, "null nonnegative");
+  }
+  return fit_folds(user_id, movie_id, rating, fold, n_ratings, n_folds, models, nonnegative, n_models, seed, device,
+                   user_capacity, movie_capacity, user_ids, user_factors, n_users, movie_ids, movie_factors, n_movies);
 }
 
 extern "C" int srs_als_recommend_host(const float* src_factors, int32_t n_src, const int32_t* dst_ids,
