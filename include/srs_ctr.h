@@ -609,6 +609,22 @@ int srs_lsh_query_host(const int32_t* ids, const float* vectors, int64_t n, int3
                        int32_t num_tables, double bucket_length, const double* keys, int32_t num_keys, int32_t k,
                        int32_t device, int32_t* out_ids, double* out_dist, int32_t* out_count);
 
+/* approxSimilarityJoin(datasetA, datasetB, threshold): every pair (a of A, b of B) whose bucket ids are equal in at
+ * least one table, once however many tables it collides in, with distance sqrt of the sum of (x_a - x_b)^2 in double,
+ * left to right, strictly below `threshold` (any double: NaN or <= 0 gives no pair, +inf every candidate).  The pairs
+ * are ordered by (id_a, id_b) ascending as signed ints.  A self-join passes the same arrays as A and B.  Each side
+ * passes srs_lsh_transform_host's checks, n_a and n_b are 0..2^31-1, ids are unique within each side (the message
+ * names the side and the id), capacity >= 0, n_pairs is non-null and the outputs are non-null when capacity > 0; all
+ * checked before any device call (SRS_ERR_INVALID).  With an empty side, *n_pairs = 0 and no device call is made.
+ * Otherwise *n_pairs = P, the number of pairs, is written after the counting pass, on SRS_OK and on SRS_ERR_RANGE
+ * (P > capacity), so that a caller can retry with capacity P; out_ids_a, out_ids_b and out_dist [P] are written only
+ * on SRS_OK.  Synchronous; the same inputs give the same bits. */
+int srs_lsh_similarity_join_host(const int32_t* ids_a, const float* vectors_a, int64_t n_a,
+                                 const int32_t* ids_b, const float* vectors_b, int64_t n_b, int32_t dim,
+                                 const double* unit_vectors, int32_t num_tables, double bucket_length,
+                                 double threshold, int32_t device, int64_t capacity,
+                                 int32_t* out_ids_a, int32_t* out_ids_b, double* out_dist, int64_t* n_pairs);
+
 /* ---- Collaborative filtering: CollaborativeFiltering.scala on the device (DESIGN.md section 4.13) ----
  * srs_als_fit_host is Spark ML's ALS.fit with explicit feedback: `max_iter` times, the movie factors and then the
  * user factors, each entity's from its double-precision normal equations (its ratings in ascending counterpart id,

@@ -53,7 +53,7 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_quantile_discretizer_host", "srs_bucketize_host", "srs_minmax_scale_host", "srs_rating_features_host",
            "srs_string_indexer_host", "srs_genre_multihot_host", "srs_sample_split_host",
            "srs_sample_split_by_timestamp_host", "srs_als_fit_implicit_host", "srs_ranking_metrics_host",
-           "srs_als_fit_nonnegative_host", "srs_als_fit_folds_nonnegative_host")
+           "srs_als_fit_nonnegative_host", "srs_als_fit_folds_nonnegative_host", "srs_lsh_similarity_join_host")
 
 _lib = None
 
@@ -297,6 +297,11 @@ def load():
     lib.srs_lsh_query_host.restype = C.c_int
     lib.srs_lsh_query_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_double,
                                        C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.srs_lsh_similarity_join_host.restype = C.c_int
+    lib.srs_lsh_similarity_join_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
+                                                 C.c_int32, C.c_void_p, C.c_int32, C.c_double, C.c_double, C.c_int32,
+                                                 C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.POINTER(C.c_int64)]
     V, I32, I64, F64 = C.c_void_p, C.c_int32, C.c_int64, C.c_double
     for name, args in (
             ("srs_approx_quantile_host", [V, I64, V, I32, F64, I32, V]),

@@ -14,8 +14,9 @@ The rest of the job (`:140-266`, DESIGN.md section 4.14; `oracle/graphemb.py` an
 
 * `item_transitions` and `random_walks` are DeepWalk's transition matrix and walks (`srs_item_transitions_host`,
   `srs_random_walks_host`); `graph_embedding` trains the same Word2Vec on the walks (`srs_graph_embedding_host`).
-* `BucketedRandomProjectionLSH(...).fit(vectors)` gives a model whose `transform` and `approx_nearest_neighbors`
-  run on the device (`srs_lsh_transform_host`, `srs_lsh_query_host`).
+* `BucketedRandomProjectionLSH(...).fit(vectors)` gives a model whose `transform`, `approx_nearest_neighbors` and
+  `approx_similarity_join` run on the device (`srs_lsh_transform_host`, `srs_lsh_query_host`,
+  `srs_lsh_similarity_join_host`).
 
     python -m sparrowrecsys_b200.embedding ratings.csv OUTDIR     # OUTDIR/item2vecEmb.csv, OUTDIR/userEmb.csv
     python -m sparrowrecsys_b200.embedding ratings.csv OUTDIR --graph --lsh   # also itemGraphEmb.csv, the LSH demo
@@ -303,6 +304,39 @@ class BucketedRandomProjectionLSHModel:
                                                   ocnt.ctypes.data))
         res = [(oid[i, :ocnt[i]].copy(), odist[i, :ocnt[i]].copy()) for i in range(Q)]
         return res[0] if single else res
+
+    def approx_similarity_join(self, ids_a, vectors_a, ids_b, vectors_b, threshold: float, device: int = 0):
+        """approxSimilarityJoin(datasetA, datasetB, threshold): every pair (a, b) sharing a bucket in at least one
+        table, once, with Euclidean distance < threshold, ordered by (id_a, id_b).  Ids must be unique within each
+        side; pass the same arrays twice for a self-join.  Returns (ids_a int32 [P], ids_b int32 [P], distances
+        float64 [P]), computed on the device."""
+        sides = []
+        for name, ids, vectors in (("a", ids_a, vectors_a), ("b", ids_b, vectors_b)):
+            x = _float32_rows(vectors, self.dim)
+            ids = np.ascontiguousarray(ids, np.int32)
+            if ids.shape != (x.shape[0],):
+                raise ValueError("ids_%s [n] expected for %d vectors" % (name, x.shape[0]))
+            u, counts = np.unique(ids, return_counts=True)
+            if np.any(counts > 1):
+                raise ValueError("ids_%s holds id %d more than once" % (name, u[np.argmax(counts > 1)]))
+            sides.append((ids, x))
+        (ia, xa), (ib, xb) = sides
+        fn = _lib.load().srs_lsh_similarity_join_host
+        P = C.c_int64(0)
+        capacity = min(len(ia) * len(ib), 1 << 20)
+        for _ in range(2):                       # a first guess at the size, then the size the library reported
+            oa, ob = np.zeros(max(capacity, 1), np.int32), np.zeros(max(capacity, 1), np.int32)
+            od = np.zeros(max(capacity, 1), np.float64)
+            rc = fn(ia.ctypes.data, xa.ctypes.data, len(ia), ib.ctypes.data, xb.ctypes.data, len(ib), self.dim,
+                    self.rand_unit_vectors.ctypes.data, self.rand_unit_vectors.shape[0], self.bucket_length,
+                    float(threshold), device, capacity, oa.ctypes.data, ob.ctypes.data, od.ctypes.data,
+                    C.byref(P))
+            if rc != _lib.SRS_ERR_RANGE:
+                break
+            capacity = P.value
+        _lib.check(rc)
+        n = P.value
+        return oa[:n].copy(), ob[:n].copy(), od[:n].copy()
 
 
 # the reference's sample key (Embedding.scala:250)
