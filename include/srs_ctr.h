@@ -795,6 +795,46 @@ int srs_sample_split_by_timestamp_host(const int64_t* timestamp, int64_t n, uint
                                        double relative_error, int32_t device, int32_t* rows, int64_t* part_counts,
                                        double* split_timestamp);
 
+/* ---- mllib BinaryClassificationMetrics (Spark 2.4.3; OFF/evaluate/Evaluator.scala; DESIGN.md section 4.22) ----
+ * One call takes n (score, label) pairs cut into n_sets score sets: set s is pairs set_off[s] .. set_off[s + 1]
+ * (set_off NULL: one set, n_sets 1).  Per set, as mllib with one partition:
+ *   a label > 0.5 is a positive (NaN is not); the thresholds are the distinct scores in Double.compare's
+ *   descending order, NaN first and 0.0 above -0.0; numBins > 0 with grouping = thresholds / numBins >= 2 merges
+ *   runs of `grouping` consecutive thresholds (the last run may be shorter), each keeping its first score; TP / FP
+ *   are the exact cumulative counts down the thresholds; precision = TP / (TP + FP) (1 when 0 / 0), recall = TP / P
+ *   (0 when P = 0), FPR = FP / N (0 when N = 0), F(beta) = (1 + b^2) * (p * r / (b^2 * p + r)) (0 when p + r = 0);
+ *   roc() = (0, 0), (FPR, recall)..., (1, 1); pr() = (0, first precision), (recall, precision)...; each area is the
+ *   sum of the trapezoids (x2 - x1) * (y2 + y1) / 2, added in a fixed order (the same inputs give the same bits).
+ * 1 <= n <= 2^31 - 1, every set non-empty (set_off[0] = 0, strictly increasing, set_off[n_sets] = n), num_bins >= 0;
+ * checked before any device call (SRS_ERR_INVALID).  The handle keeps each point's threshold and counts on
+ * `device` (24 bytes a point); a call peaks near 33 bytes a pair on the device (plus 16 for the host path's copy). */
+typedef struct srs_binary_metrics srs_binary_metrics;
+typedef struct srs_binary_summary {
+  int64_t n, positives, negatives, thresholds;   /* thresholds: the points after binning */
+  double area_under_roc, area_under_pr;
+} srs_binary_summary;
+#define SRS_BM_ROC 0          /* double [thresholds + 2][2]: (FPR, recall) */
+#define SRS_BM_PR 1           /* double [thresholds + 1][2]: (recall, precision) */
+#define SRS_BM_THRESHOLDS 2   /* double [thresholds] */
+#define SRS_BM_PRECISION 3    /* double [thresholds][2]: (threshold, value), and so for the next two */
+#define SRS_BM_RECALL 4
+#define SRS_BM_FMEASURE 5     /* at `beta`; at beta 0 a point with r = 0 < p is 0 / 0, NaN as in Spark */
+/* scores and labels [n] float64 on the host.  Synchronous. */
+int srs_binary_metrics_create_host(const double* scores, const double* labels, int64_t n, const int64_t* set_off,
+                                   int32_t n_sets, int32_t num_bins, int32_t device, srs_binary_metrics** out);
+/* scores [n] float32 and labels [n] int32 (positive when > 0) on `device`, e.g. what srs_predict_device wrote;
+ * read after the work queued on `stream`.  Returns when the work is done. */
+int srs_binary_metrics_create_device(const float* scores, const int32_t* labels, int64_t n, const int64_t* set_off,
+                                     int32_t n_sets, int32_t num_bins, int32_t device, void* stream,
+                                     srs_binary_metrics** out);
+void srs_binary_metrics_destroy(srs_binary_metrics* h);
+int srs_binary_metrics_summary(const srs_binary_metrics* h, int32_t set, srs_binary_summary* out);
+/* curve `which` (SRS_BM_*) of `set` into host dst, laid out as above; an unknown `which` or set is rejected
+ * without touching dst */
+int srs_binary_metrics_curve(const srs_binary_metrics* h, int32_t set, int32_t which, double beta, double* dst);
+/* the cumulative TP and FP [thresholds] int64 of `set` */
+int srs_binary_metrics_confusion(const srs_binary_metrics* h, int32_t set, int64_t* tp, int64_t* fp);
+
 #ifdef __cplusplus
 }
 #endif

@@ -53,7 +53,9 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_quantile_discretizer_host", "srs_bucketize_host", "srs_minmax_scale_host", "srs_rating_features_host",
            "srs_string_indexer_host", "srs_genre_multihot_host", "srs_sample_split_host",
            "srs_sample_split_by_timestamp_host", "srs_als_fit_implicit_host", "srs_ranking_metrics_host",
-           "srs_als_fit_nonnegative_host", "srs_als_fit_folds_nonnegative_host", "srs_lsh_similarity_join_host")
+           "srs_als_fit_nonnegative_host", "srs_als_fit_folds_nonnegative_host", "srs_lsh_similarity_join_host",
+           "srs_binary_metrics_create_host", "srs_binary_metrics_create_device", "srs_binary_metrics_destroy",
+           "srs_binary_metrics_summary", "srs_binary_metrics_curve", "srs_binary_metrics_confusion")
 
 _lib = None
 
@@ -104,6 +106,15 @@ class SrsAlsModel(C.Structure):
     """`srs_als_model` (include/srs_ctr.h): one model of a batched ALS fit."""
     _fields_ = [("rank", C.c_int32), ("max_iter", C.c_int32), ("reg_param", C.c_double),
                 ("exclude_fold", C.c_int32)]
+
+
+class SrsBinarySummary(C.Structure):
+    """`srs_binary_summary` (include/srs_ctr.h): one score set of BinaryClassificationMetrics."""
+    _fields_ = [("n", C.c_int64), ("positives", C.c_int64), ("negatives", C.c_int64), ("thresholds", C.c_int64),
+                ("area_under_roc", C.c_double), ("area_under_pr", C.c_double)]
+
+
+SRS_BM_ROC, SRS_BM_PR, SRS_BM_THRESHOLDS, SRS_BM_PRECISION, SRS_BM_RECALL, SRS_BM_FMEASURE = range(6)
 
 
 class SrsError(RuntimeError):
@@ -303,6 +314,18 @@ def load():
                                                  C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.POINTER(C.c_int64)]
     V, I32, I64, F64 = C.c_void_p, C.c_int32, C.c_int64, C.c_double
+    lib.srs_binary_metrics_create_host.restype = C.c_int
+    lib.srs_binary_metrics_create_host.argtypes = [V, V, I64, V, I32, I32, I32, C.POINTER(V)]
+    lib.srs_binary_metrics_create_device.restype = C.c_int
+    lib.srs_binary_metrics_create_device.argtypes = [V, V, I64, V, I32, I32, I32, V, C.POINTER(V)]
+    lib.srs_binary_metrics_destroy.restype = None
+    lib.srs_binary_metrics_destroy.argtypes = [V]
+    lib.srs_binary_metrics_summary.restype = C.c_int
+    lib.srs_binary_metrics_summary.argtypes = [V, I32, C.POINTER(SrsBinarySummary)]
+    lib.srs_binary_metrics_curve.restype = C.c_int
+    lib.srs_binary_metrics_curve.argtypes = [V, I32, I32, F64, V]
+    lib.srs_binary_metrics_confusion.restype = C.c_int
+    lib.srs_binary_metrics_confusion.argtypes = [V, I32, V, V]
     for name, args in (
             ("srs_approx_quantile_host", [V, I64, V, I32, F64, I32, V]),
             ("srs_quantile_discretizer_host", [V, I64, I32, F64, I32, V, C.POINTER(I32), V]),
