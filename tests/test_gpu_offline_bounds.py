@@ -1,6 +1,8 @@
-"""Every case of tests/test_offline_bounds.py's `BOUNDS` on the device against its oracle, bit for bit, and a repeat
-run giving the same bits."""
+"""Every case of tests/test_offline_bounds.py's `BOUNDS` on the device against its oracle, bit for bit (the binary
+metrics' areas within 1e-13 of the exactly rounded sum of the oracle's trapezoids), and a repeat run giving the same
+bits."""
 import ctypes as C
+import re
 
 import numpy as np
 import pytest
@@ -12,6 +14,8 @@ from oracle import feature_eng as F
 from oracle import graphemb as G
 from oracle import item2vec_cext as IX
 from oracle import lsh as H
+from oracle import lsh_join as LJ
+from oracle import als_nnls_cext as XN
 from sparrowrecsys_b200 import _lib
 from sparrowrecsys_b200 import collab
 from sparrowrecsys_b200 import embedding as E
@@ -19,7 +23,8 @@ from sparrowrecsys_b200 import featureeng as FE
 from sparrowrecsys_b200 import featurejob as FJ
 
 from test_offline_bounds import (BOUNDS, data, discretizer_splits, graph_transitions, i2v_oracle_input,
-                                 indexer_oracle, indexer_tokens, labels_csr, quantiles)
+                                 indexer_oracle, indexer_tokens, labels_csr, nnls_singular_oracle, quantiles,
+                                 segmented_metrics, set_curves)
 
 pytestmark = pytest.mark.gpu
 
@@ -282,10 +287,132 @@ def _ranking_oracle(d):
     return out
 
 
+AREA_TOL = 1e-13
+
+
+def _bm_summaries(m, S):
+    """Every set's n, positives, thresholds and both areas (one summary call per set, the struct reused)."""
+    f, h = m._lib.srs_binary_metrics_summary, m._h
+    out = _lib.SrsBinarySummary()
+    ref = C.byref(out)
+    n, P, T = np.empty(S, np.int64), np.empty(S, np.int64), np.empty(S, np.int64)
+    roc, pr = np.empty(S), np.empty(S)
+    for k in range(S):
+        _lib.check(f(h, k, ref))
+        n[k], P[k], T[k], roc[k], pr[k] = out.n, out.positives, out.thresholds, out.area_under_roc, out.area_under_pr
+    return [n, P, T, roc, pr]
+
+
+def _bm_device(d):
+    from sparrowrecsys_b200.evaluation import BinaryClassificationMetrics
+    out = []
+    for run in d["runs"]:
+        s, y, off = run["scores"], run["labels"], run["offsets"]
+        if run["path"] == "device":
+            import torch
+            s, y = torch.from_numpy(s).cuda(), torch.from_numpy(y).cuda()
+        with BinaryClassificationMetrics(s, y, 0, off) as m:
+            summaries = _bm_summaries(m, len(off) - 1)
+            assert summaries[2].min() >= 1                    # every set has a threshold; only then read curves
+            curves = [[m.thresholds(k), *m.confusions(k), m.roc(k), m.pr(k), m.precision_by_threshold(k),
+                       m.recall_by_threshold(k), m.f_measure_by_threshold(1.0, k)] for k in run["sample"]]
+            out.append([summaries, curves])
+    return out
+
+
+def _bm_oracle(d):
+    out = []
+    for run in d["runs"]:
+        R = segmented_metrics(run["scores"].astype(np.float64), run["labels"].astype(np.float64), run["offsets"])
+        out.append([[R["n"], R["positives"], np.diff(R["pt_off"]), R["area_roc"], R["area_pr"]],
+                    [set_curves(R, k) for k in run["sample"]]])
+    return out
+
+
+def _bm_same(got, want):
+    """Counts and curves bit for bit, each area within AREA_TOL."""
+    assert len(got) == len(want)
+    for (gs, gc), (ws, wc) in zip(got, want):
+        _same_all(gs[:3], ws[:3])
+        for g, w, what in ((gs[3], ws[3], "roc"), (gs[4], ws[4], "pr")):
+            err = np.abs(g - w)
+            assert err.max() <= AREA_TOL, (what, int(err.argmax()), err.max())
+        _same_all(gc, wc)
+
+
+def _join_device(d):
+    out = []
+    for run in d["runs"]:
+        model = E.BucketedRandomProjectionLSHModel(run["uv"], run["bl"])
+        out.append(list(model.approx_similarity_join(run["ids_a"], run["xa"], run["ids_b"], run["xb"],
+                                                     run["threshold"])))
+    return out
+
+
+def _join_oracle(d):
+    return [list(LJ.approx_similarity_join(run["ids_a"], run["xa"], run["ids_b"], run["xb"], run["uv"], run["bl"],
+                                           run["threshold"])) for run in d["runs"]]
+
+
+def _nnls_fits_device(d):
+    r = {"userId": d["u"], "movieId": d["m"], "rating": d["r"]}
+    return [list(_fit_tuple(collab.als(r, nonnegative=True, **f))) for f in d["fits"]]
+
+
+def _nnls_fits_oracle(d):
+    return [list(XN.fit(d["u"], d["m"], d["r"], **f)) for f in d["fits"]]
+
+
+def _nnls_batch_device(d):
+    r = {"userId": d["u"], "movieId": d["m"], "rating": d["r"]}
+    return [list(_fit_tuple(m)) for m in collab.als_folds(r, d["fold"], d["n_folds"], d["models"], seed=d["seed"])]
+
+
+def _nnls_batch_oracle(d):
+    """One C-oracle single fit per model on the rows outside its excluded fold: NNLS or Cholesky by its flag."""
+    out = []
+    for s in d["models"]:
+        rows = d["fold"] != s["exclude_fold"]
+        fit = XN.fit if s["nonnegative"] else X.fit
+        out.append(list(fit(d["u"][rows], d["m"][rows], d["r"][rows], rank=s["rank"], max_iter=s["max_iter"],
+                            reg_param=s["reg_param"], seed=d["seed"])))
+    return out
+
+
+def _nnls_singular_device(d):
+    out = []
+    r = {"userId": d["u"], "movieId": d["m"], "rating": d["r"]}
+    for models in d["orders"]:
+        try:
+            collab.als_folds(r, d["fold"], d["n_folds"], models, seed=d["seed"])
+            out.append("no error")
+        except ValueError as e:
+            hit = re.search(r"model \d+: singular normal equations for \w+ -?\d+ in iteration \d+", str(e))
+            out.append(hit.group(0) if hit else str(e))
+    return out
+
+
+def _nnls_device(d):
+    if "orders" in d:
+        return _nnls_singular_device(d)
+    return _nnls_batch_device(d) if "models" in d else _nnls_fits_device(d)
+
+
+def _nnls_oracle(d):
+    if "orders" in d:
+        return nnls_singular_oracle(d)
+    return _nnls_batch_oracle(d) if "models" in d else _nnls_fits_oracle(d)
+
+
+def _same_messages(got, want):
+    assert got == want
+
+
 RUNS = {"item2vec": (_i2v_device, _i2v_oracle), "graph": (_graph_device, _graph_oracle),
         "lsh": (_lsh_device, _lsh_oracle), "featureeng": (_fe_device, _fe_oracle),
         "featurejob": (_fj_device, _fj_oracle), "als_implicit": (_implicit_device, _implicit_oracle),
-        "ranking_metrics": (_ranking_device, _ranking_oracle)}
+        "ranking_metrics": (_ranking_device, _ranking_oracle), "binary_metrics": (_bm_device, _bm_oracle),
+        "lsh_join": (_join_device, _join_oracle), "als_nonnegative": (_nnls_device, _nnls_oracle)}
 
 
 def _runs(name):
@@ -298,10 +425,23 @@ def _runs(name):
     return RUNS[BOUNDS[name].job]
 
 
+def _compare(name):
+    """How a case's device output is held to its oracle's."""
+    job = BOUNDS[name].job
+    if job == "binary_metrics":
+        return _bm_same
+    if name == "als_nonnegative_singular_after_nnls":
+        return _same_messages
+    return _same_all
+
+
 @pytest.mark.parametrize("name", sorted(BOUNDS))
 def test_case_bit_equal_to_its_oracle_and_repeatable(name):
     d = data(name)
     device, oracle = _runs(name)
     got = device(d)
-    _same_all(got, oracle(d))
-    _same_all(device(d), got)
+    _compare(name)(got, oracle(d))
+    if name == "als_nonnegative_singular_after_nnls":
+        assert device(d) == got
+    else:
+        _same_all(device(d), got)

@@ -1,5 +1,6 @@
-"""The offline jobs at their bounds and tile edges (csrc/item2vec.cu, graphemb.cu, lsh.cu, als.cu with implicit ALS
-and RankingMetrics, featureeng.cu, featurejob.cu, and hostcall.h's grid cap).
+"""The offline jobs at their bounds and tile edges (csrc/item2vec.cu, graphemb.cu, lsh.cu with the similarity join,
+als.cu with implicit ALS, RankingMetrics and nonnegative ALS, featureeng.cu, featurejob.cu, binary_metrics.cu, and
+hostcall.h's grid cap).
 
 `BOUNDS` names one case per (job, edge).  Each case builds its inputs here; its `reach` shows from the oracle alone,
 with no device, that the inputs reach the edge the case names, and returns the (bound, value) pairs it reaches.
@@ -24,6 +25,8 @@ import pytest
 
 from oracle import als as A
 from oracle import als_implicit as XP
+from oracle import als_nnls as N
+from oracle import binary_metrics as BM
 from oracle import feature_job as FQ
 from oracle import feature_eng as F
 from oracle import graphemb as G
@@ -61,6 +64,7 @@ def constants(*files):
 
 RATING_BOUND_FILES = ("als.cu", "featureeng.cu", "item2vec.cu", "featurejob.cu")
 K = constants("als.cu", "lsh.cu", "item2vec.cu", "featureeng.cu", "graphemb.cu", "featurejob.cu", "hostcall.h")
+KB = constants("binary_metrics.cu", "hostcall.h")     # its own table: its kChunk (points) is not als.cu's (ratings)
 
 
 class Case(NamedTuple):
@@ -1052,6 +1056,516 @@ def _ranking_grid_reach(d):
     return {("rank_trips", -(-len(p) // per_trip)) for p, _, _ in d["runs"]}
 
 
+def trips(n, per_trip=STRIDE_256):
+    """Grid-stride trips of a 256-thread kernel launched through grid_for over n elements."""
+    return -(-int(n) // per_trip)
+
+
+# ---- BinaryClassificationMetrics (binary_metrics.cu) --------------------------------------------------------------
+def segmented_metrics(scores, labels, offsets):
+    """BM.BinaryMetrics (numBins 0) of every set at once, vectorised over the sets, for millions of sets.  Returns
+    per set n, positives and pt_off [n_sets + 1] (each set's points), per point (the sets' points one after another)
+    thresholds, tp, fp, precision, recall and FPR, each set's ROC and PR points (roc_off, pr_off) and their trapezoid
+    terms (roc_terms_off, pr_terms_off), and per set both areas (math.fsum of the terms)."""
+    s = np.ascontiguousarray(scores, np.float64)
+    off = np.asarray(offsets, np.int64)
+    S = len(off) - 1
+    sizes = np.diff(off)
+    sid = np.repeat(np.arange(S), sizes)
+    key = BM.descending_key(s)
+    order = np.lexsort((key, sid))                               # (set, threshold order), stable
+    k, p, g = key[order], BM.is_positive(labels)[order].astype(np.int64), sid[order]
+    starts = np.flatnonzero(np.r_[True, (k[1:] != k[:-1]) | (g[1:] != g[:-1])])
+    rpos = np.add.reduceat(p, starts)
+    rneg = np.diff(np.r_[starts, len(k)]) - rpos
+    T = np.bincount(g[starts], minlength=S)
+    pt_off = np.r_[0, np.cumsum(T)]
+    ctp, cfp = np.cumsum(rpos), np.cumsum(rneg)
+    first = pt_off[:-1]
+    tp = ctp - np.repeat(ctp[first] - rpos[first], T)
+    fp = cfp - np.repeat(cfp[first] - rneg[first], T)
+    P = tp[pt_off[1:] - 1]
+    Nn = sizes - P
+    Pr, Nr = np.repeat(P, T), np.repeat(Nn, T)
+    rec = np.where(Pr == 0, 0.0, tp.astype(np.float64) / np.maximum(Pr, 1).astype(np.float64))
+    fpr = np.where(Nr == 0, 0.0, fp.astype(np.float64) / np.maximum(Nr, 1).astype(np.float64))
+    prec = BM.precision(tp, fp)
+    idx = np.arange(S)
+    # ROC: (0, 0), (FPR, recall) per point, (1, 1); PR: (0, the first precision), (recall, precision) per point
+    roc_off, pr_off = pt_off + 2 * np.arange(S + 1), pt_off + np.arange(S + 1)
+    roc = np.empty((roc_off[-1], 2))
+    at = np.arange(len(tp)) + 2 * np.repeat(idx, T) + 1
+    roc[at] = np.stack([fpr, rec], 1)
+    roc[roc_off[:-1]] = 0.0
+    roc[roc_off[1:] - 1] = 1.0
+    pr = np.empty((pr_off[-1], 2))
+    pr[np.arange(len(tp)) + np.repeat(idx, T) + 1] = np.stack([rec, prec], 1)
+    pr[pr_off[:-1]] = np.stack([np.zeros(S), prec[first]], 1)
+
+    def terms(pts, poff):
+        t = BM.trapezoid_terms(pts)                            # consecutive pairs; drop those across two sets
+        keep = np.ones(len(t), bool)
+        keep[poff[1:-1] - 1] = False
+        return t[keep], poff - np.arange(S + 1)
+
+    roc_t, roc_toff = terms(roc, roc_off)
+    pr_t, pr_toff = terms(pr, pr_off)
+
+    def areas(t, toff):
+        cnt = np.diff(toff)
+        out = np.add.reduceat(t, toff[:-1]) if len(t) else np.zeros(S)
+        for i in np.flatnonzero(cnt > 64):                       # long sets: the exactly rounded sum
+            out[i] = math.fsum(t[toff[i]:toff[i + 1]])
+        return out
+
+    return dict(n=sizes, positives=P, pt_off=pt_off, thresholds=BM.key_score(k[starts]), tp=tp, fp=fp,
+                precision=prec, recall=rec, fpr=fpr, roc=roc, roc_off=roc_off, pr=pr, pr_off=pr_off,
+                roc_terms=roc_t, roc_terms_off=roc_toff, pr_terms=pr_t, pr_terms_off=pr_toff,
+                area_roc=areas(roc_t, roc_toff), area_pr=areas(pr_t, pr_toff))
+
+
+def set_curves(R, s):
+    """Set s's thresholds, tp, fp, ROC, PR, and precision, recall and F1 by threshold, from segmented_metrics."""
+    a, b = R["pt_off"][s], R["pt_off"][s + 1]
+    thr, prec, rec = R["thresholds"][a:b], R["precision"][a:b], R["recall"][a:b]
+    return [thr, R["tp"][a:b], R["fp"][a:b], R["roc"][R["roc_off"][s]:R["roc_off"][s + 1]],
+            R["pr"][R["pr_off"][s]:R["pr_off"][s + 1]], np.stack([thr, prec], 1), np.stack([thr, rec], 1),
+            np.stack([thr, BM.f_measure(prec, rec, 1.0)], 1)]
+
+
+def bm_curves(m):
+    """The same of BM.BinaryMetrics m."""
+    return [m.thresholds(), m.tp, m.fp, m.roc(), m.pr(), m.precision_by_threshold(), m.recall_by_threshold(),
+            m.f_measure_by_threshold(1.0)]
+
+
+def set_bits(n_sets):
+    """The set sort's bit count: the width of the largest set index, n_sets - 1."""
+    return max(1, int(n_sets - 1).bit_length())
+
+
+def _bm_run(scores, labels, sizes, path="host", rng=None):
+    """One call: the sets of `sizes` pairs.  Full curves are compared on a sample: the first and last sets, the sets
+    either side of each power of two, and a few drawn at random."""
+    S = len(sizes)
+    sample = {0, S - 1} | {v for b in range(1, 32) for v in ((1 << b) - 1, 1 << b) if v < S}
+    if rng is not None:
+        sample |= set(rng.integers(0, S, 8).tolist())
+    return dict(scores=scores, labels=labels, offsets=np.r_[0, np.cumsum(sizes)].astype(np.int64), path=path,
+                sample=sorted(sample))
+
+
+def _bm_two_grids():
+    """One set of exactly 2 GRID distinct double scores (STRIDE_256 = GRID), plus 5 000 pairs tied with them."""
+    rng = np.random.default_rng(60)
+    T = 2 * STRIDE_256
+    s = (rng.permutation(T) - T // 3) / 7.0
+    s = rng.permutation(np.r_[s, rng.choice(s, 5000)])
+    y = rng.choice([0.0, 1.0, 0.5, 0.7], len(s), p=[0.5, 0.4, 0.05, 0.05])
+    return dict(runs=[_bm_run(s, y, [len(s)])])
+
+
+def _bm_sets(counts, seed):
+    """Per n_sets in counts, sets of 1 to 3 pairs: scores on five levels with ties, NaN, -0.0 and 0.0."""
+    rng = np.random.default_rng(seed)
+    runs = []
+    for S in counts:
+        sizes = rng.integers(1, 4, S)
+        n = int(sizes.sum())
+        s = rng.integers(0, 5, n) / 4.0
+        s[rng.random(n) < 0.02] = np.nan
+        s[rng.random(n) < 0.02] = -0.0
+        y = rng.integers(0, 2, n).astype(np.float64)
+        runs.append(_bm_run(s, y, sizes, rng=rng))
+    return dict(runs=runs)
+
+
+BM_SET_T = (2047, 2048, 2049, 4096, 4097, 65536, 65537)             # thresholds per set: kChunk (2 048) edges, 32 and
+                                                                    # 33 chunks
+
+
+def _bm_chunk_sets():
+    """Adjacent sets of BM_SET_T distinct thresholds (and 10 % tied pairs), with sets of 1 to 3 pairs between some."""
+    rng = np.random.default_rng(61)
+    parts = []
+    for T in (3,) + BM_SET_T[:3] + (1,) + BM_SET_T[3:] + (2,):
+        v = rng.permutation(T) / T - 0.25
+        parts.append(rng.permutation(np.r_[v, rng.choice(v, T // 10)]))
+    s = np.concatenate(parts)
+    y = (rng.random(len(s)) < 0.3 + 0.4 * (s > 0.3)).astype(np.float64)
+    return dict(runs=[_bm_run(s, y, [len(p) for p in parts], rng=rng)])
+
+
+# float32 bit patterns with an even mantissa: in each pair (b, b + 1) only the last mantissa bit differs
+BM_F32_EVEN = (0x00000002, 0x00000010, 0x00800000, 0x3F7FFFFE, 0x3F800000, 0x3DCCCCCC, 0xBF800000, 0xC2C80000,
+               0x80000004, 0x7F7FFFFE, 0xFF7FFFFE)
+
+
+def _bm_f32_adjacent():
+    """Device path (float32 scores, int32 labels): each pair of BM_F32_EVEN with the smaller score first in input
+    order and the two labels different, beside +-inf, +-0, NaN and random float32 scores; two sets, the second the
+    first with its labels flipped."""
+    rng = np.random.default_rng(62)
+    bits = []
+    for b in BM_F32_EVEN:
+        lo, hi = (b, b + 1) if b < 0x80000000 else (b + 1, b)       # negative: b + 1 is the smaller
+        bits += [lo, hi]
+    pairs = np.array(bits, np.uint32).view(np.float32)
+    special = np.array([np.inf, -np.inf, 0.0, -0.0, np.nan, 1.0, -1.0], np.float32)
+    noise = rng.standard_normal(300).astype(np.float32)
+    s = np.r_[pairs, special, noise].astype(np.float32)
+    y = np.r_[np.tile([0, 1], len(BM_F32_EVEN)), rng.integers(0, 2, len(special) + len(noise))].astype(np.int32)
+    y[1::4] = 2                                                      # any label > 0 is a positive
+    return dict(runs=[_bm_run(np.r_[s, s], np.r_[y, 1 - np.minimum(y, 1)], [len(s), len(s)], path="device")],
+                n_pairs=len(BM_F32_EVEN))
+
+
+def _bm_reach(d):
+    got = set()
+    for run in d["runs"]:
+        s, off = run["scores"], run["offsets"]
+        S = len(off) - 1
+        R = segmented_metrics(s.astype(np.float64), run["labels"].astype(np.float64), off)
+        T = np.diff(R["pt_off"])
+        got |= {("bm_sets_trips", trips(S)), ("bm_points_trips", trips(len(R["tp"])))}
+        if S > 1:
+            got.add(("bm_set_bits", set_bits(S)))
+            assert (S - 1) >> (set_bits(S) - 1) == 1                    # the top set holds the top bit
+        for t in np.unique(T).tolist():
+            if t > 1000:
+                got |= {("bm_set_thresholds", t), ("bm_set_chunks", -(-t // KB["kChunk"]))}
+        if T.max() > STRIDE_256:
+            t = int(T.max())
+            got |= {("bm_curve_trips", trips(t)), ("bm_curve_trips", trips(t + 1))}
+            got.add(("bm_roc_end_trip", (t + 1) // STRIDE_256 + 1))    # ROC's (1, 1) is entry T + 1
+        if run["path"] == "device":
+            k = BM.descending_key(s.astype(np.float64))
+            n = d["n_pairs"]
+            lo, hi = s[0:2 * n:2].astype(np.float64), s[1:2 * n:2].astype(np.float64)
+            assert np.all(lo < hi)                                       # the smaller first in input order
+            x = k[0:2 * n:2] ^ k[1:2 * n:2]
+            normal = np.abs(lo) >= np.finfo(np.float32).tiny
+            assert np.all(x[normal] == np.uint64(1 << 29)) and normal.sum() >= 6
+            got.add(("bm_f32_last_bit", 29))
+    return got
+
+
+def test_segmented_metrics_match_binary_metrics_set_by_set():
+    """segmented_metrics against BM.BinaryMetrics on 3 000 small random sets with ties, NaN, +-0 and +-inf, and a
+    few long ones: every curve and trapezoid term bit for bit, and the areas."""
+    rng = np.random.default_rng(63)
+    sizes = np.r_[rng.integers(1, 12, 3000), 700, 3000, 1]
+    n = int(sizes.sum())
+    special = np.array([np.nan, 0.0, -0.0, np.inf, -np.inf, 0.5, 0.25])
+    s = np.where(rng.random(n) < 0.3, special[rng.integers(0, len(special), n)], rng.integers(0, 9, n) / 8.0)
+    s[-3000:] = rng.random(3000)
+    y = rng.choice([0.0, 1.0, 0.5, 0.7, np.nan, 2.0], n)
+    off = np.r_[0, np.cumsum(sizes)]
+    R = segmented_metrics(s, y, off)
+    for i in range(len(sizes)):
+        m = BM.BinaryMetrics(s[off[i]:off[i + 1]], y[off[i]:off[i + 1]])
+        assert (R["n"][i], R["positives"][i]) == (m.n, m.positives)
+        for a, b in zip(set_curves(R, i), bm_curves(m)):
+            assert a.shape == b.shape and np.array_equal(np.asarray(a).view(np.uint8), np.asarray(b).view(np.uint8))
+        rt = R["roc_terms"][R["roc_terms_off"][i]:R["roc_terms_off"][i + 1]]
+        pt = R["pr_terms"][R["pr_terms_off"][i]:R["pr_terms_off"][i + 1]]
+        assert np.array_equal(rt, BM.trapezoid_terms(m.roc())) and np.array_equal(pt, BM.trapezoid_terms(m.pr()))
+        assert abs(R["area_roc"][i] - m.area_under_roc()) <= 1e-13
+        assert abs(R["area_pr"][i] - m.area_under_pr()) <= 1e-13
+
+
+# ---- the LSH similarity join (lsh.cu) ------------------------------------------------------------------------------
+def _join(ids_a, xa, ids_b, xb, uv, bl, threshold):
+    return dict(ids_a=np.asarray(ids_a, np.int32), xa=np.asarray(xa, np.float32), ids_b=np.asarray(ids_b, np.int32),
+                xb=np.asarray(xb, np.float32), uv=np.asarray(uv, np.float64), bl=float(bl),
+                threshold=float(threshold))
+
+
+def join_buckets(run):
+    """Both sides' bucket ids, and per table each A row's run of equal ids among B's (np.searchsorted)."""
+    ha, hb = H.transform(run["xa"], run["uv"], run["bl"]), H.transform(run["xb"], run["uv"], run["bl"])
+    runs = []
+    for j in range(ha.shape[1]):
+        sb = np.sort(hb[:, j])
+        runs.append(np.searchsorted(sb, ha[:, j], "right") - np.searchsorted(sb, ha[:, j], "left"))
+    return ha, hb, runs
+
+
+def _join_keys_trips():
+    """n_b = 70 000, L = 64: n_b L = 4 480 000 (bucket) keys, three grid trips.  A is 500 near-copies of B rows,
+    bucket length 1e-4: few collisions beyond a row's own copy."""
+    rng = np.random.default_rng(70)
+    nb, na, D, L = 70000, 500, 4, 64
+    xb = rng.standard_normal((nb, D)).astype(np.float32)
+    xa = xb[rng.choice(nb, na, replace=False)] + rng.standard_normal((na, D)).astype(np.float32) * 1e-6
+    return dict(runs=[_join(rng.permutation(10 * na)[:na], xa, rng.permutation(2 * nb)[:nb] - nb, xb,
+                            H.fit(D, L, seed=70), 1e-4, 0.01)])
+
+
+def _join_runs_trips():
+    """n_a = 2 GRID + 0 rows of D = 1, L = 1: the runs kernel covers n_a + 1 entries in three trips, its sentinel
+    len[n_a] alone on the third.  B holds buckets 0 .. 2 999, one row each; all but 3 000 A rows fall in negative
+    buckets (empty runs, row 0 and row n_a - 1 among them)."""
+    rng = np.random.default_rng(71)
+    na, nb = 2 * STRIDE_256, 3000
+    xb = (np.arange(nb) + 0.5).astype(np.float32)[:, None]
+    xa = -(rng.integers(1, 1 << 20, na) + 0.5)
+    hits = rng.choice(np.arange(1, na - 1), 3000, replace=False)
+    xa[hits] = rng.integers(0, nb, 3000) + 0.25
+    return dict(runs=[_join(rng.permutation(na), xa[:, None], np.arange(nb) * 3, xb, [[1.0]], 1.0, 1.0)])
+
+
+JOIN_C = (1, 1055, 1056, 1057, 256 * 1056, 256 * 1056 + 1)          # kJoinSegments = 1 056 edges, tiles of 256
+JOIN_GROUPS = {1: [(1, 1)], 1055: [(5, 211)], 1056: [(32, 33)], 1057: [(7, 151)], 256 * 1056: [(512, 528)],
+               256 * 1056 + 1: [(512, 528), (1, 1)]}                # C = sum of a b over buckets of a A and b B rows
+
+
+def _join_segments():
+    """L = 3, D = 3, unit vectors e0, e1, e2 and bucket length 1: table j's bucket of a row is floor(x[j]).  Per
+    run, table 0 and table 2 have C_0 and C_2 candidates, buckets built from JOIN_GROUPS at rows 0, 1, ... on both
+    sides, so the groups of the two tables share pairs; table 1 has none (A in bucket -3, B in -4)."""
+    rng = np.random.default_rng(72)
+    runs = []
+    for c0, c2 in ((JOIN_C[0], JOIN_C[1]), (JOIN_C[2], JOIN_C[3]), (JOIN_C[4], JOIN_C[5])):
+        na = max(sum(a for a, _ in JOIN_GROUPS[c]) for c in (c0, c2)) + 7
+        nb = max(sum(b for _, b in JOIN_GROUPS[c]) for c in (c0, c2)) + 5
+        ba, bb = np.full((na, 3), -1.0), np.full((nb, 3), -2.0)
+        ba[:, 1], bb[:, 1] = -3.0, -4.0
+        for j, c in ((0, c0), (2, c2)):
+            ra = rb = 0
+            for g, (a, b) in enumerate(JOIN_GROUPS[c]):
+                ba[ra:ra + a, j], bb[rb:rb + b, j] = 10 * (g + 1), 10 * (g + 1)
+                ra, rb = ra + a, rb + b
+        xa = ba + 0.5 + (rng.random(ba.shape) - 0.5) * 0.4
+        xb = bb + 0.5 + (rng.random(bb.shape) - 0.5) * 0.4
+        runs.append(_join(rng.permutation(3 * na)[:na], xa, rng.permutation(3 * nb)[:nb], xb, np.eye(3), 1.0, 1e9))
+    return dict(runs=runs)
+
+
+def _join_extreme_ids():
+    """Ids INT32_MIN, -1, 0 and INT32_MAX on both sides, every pair in one bucket: the output order at the sign bit."""
+    rng = np.random.default_rng(73)
+    ext = np.array([-2 ** 31, -1, 0, 2 ** 31 - 1], np.int64)
+    mid = rng.choice(np.r_[np.arange(-2 ** 31 + 1, -2 ** 31 + 50), np.arange(1, 100), 2 ** 31 - 50 + np.arange(49)],
+                     60, replace=False)
+    ids_a, ids_b = rng.permutation(np.r_[ext, mid[:30]]), rng.permutation(np.r_[ext, mid[30:]])
+    xa, xb = rng.random((34, 2)), rng.random((34, 2))                    # nonnegative: every bucket id 0
+    return dict(runs=[_join(ids_a, xa, ids_b, xb, _nonneg_unit(2, 2, 73), 1e6, 1e9)])
+
+
+def _join_signed_zero():
+    """Bucket length 1e300 and coordinates +-1e-38, +-1 and 0 on unit vectors e0, e1 and (0.6, 0.8): quotients that
+    underflow to -0.0 and +0.0 (floor keeps the sign), and -1.  A -0.0 and a +0.0 are one bucket in every table."""
+    rng = np.random.default_rng(74)
+    vals = np.array([1e-38, -1e-38, 1.0, -1.0, 0.0], np.float32)
+    uv = np.array([[1.0, 0.0], [0.0, 1.0], [0.6, 0.8]])
+    return dict(runs=[_join(np.arange(300) * 2 - 299, rng.choice(vals, (300, 2)), np.arange(280) * 5 - 700,
+                            rng.choice(vals, (280, 2)), uv, 1e300, 10.0)])
+
+
+def _join_infinite():
+    """Bucket length 5e-324 (the smallest subnormal): coordinates +-1 give buckets +-inf, 0 gives 0 and 1e-30 a
+    finite one near 2e293."""
+    rng = np.random.default_rng(75)
+    vals = np.array([1.0, -1.0, 0.0, 1e-30, -1e-30], np.float32)
+    uv = np.array([[1.0, 0.0], [0.0, 1.0], [0.6, 0.8]])
+    return dict(runs=[_join(rng.permutation(1000)[:250], rng.choice(vals, (250, 2)), rng.permutation(1000)[:260],
+                            rng.choice(vals, (260, 2)), uv, 5e-324, 10.0)])
+
+
+def _join_reach(d):
+    got = set()
+    for run in d["runs"]:
+        ha, hb, runs = join_buckets(run)
+        na, nb, L = len(ha), len(hb), ha.shape[1]
+        C = [int(r.sum()) for r in runs]
+        assert sum(C) > 0
+        got |= {("join_hash_trips", trips(max(na, nb) * L)), ("join_keys_trips", trips(nb * L)),
+                ("join_runs_trips", trips(na + 1))}
+        if trips(na + 1) > 1:
+            got.add(("join_sentinel_trip", na // STRIDE_256 + 1))         # len[n_a] at r = n_a
+            assert runs[0][0] == 0 and runs[0][-1] == 0 and 1000 <= (runs[0] > 0).sum() <= 10000
+            got |= {("join_empty_run_at", "first"), ("join_empty_run_at", "last")}
+        if L == 3 and run["bl"] == 1.0:                                  # the segment runs
+            got |= {("join_C", c) for c in C}
+            assert C[1] == 0 and C[0] > 0 and C[2] > 0
+            got.add(("join_empty_table_between", 1))
+            both = (ha[:, None, 0] == hb[None, :, 0]) & (ha[:, None, 2] == hb[None, :, 2])
+            assert both.any()                                            # pairs the first-table rule removes
+            got.add(("join_first_table_removes", 1))
+        ids = set(run["ids_a"].tolist()) & set(run["ids_b"].tolist())
+        for v in (-2 ** 31, -1, 0, 2 ** 31 - 1):
+            if v in ids and run["bl"] == 1e6:
+                assert np.all(ha == ha[0, 0]) and np.all(hb == ha[0, 0])  # one bucket: every pair
+                got.add(("join_id", v))
+        zero_a, zero_b = ha == 0, hb == 0
+        if (zero_a & np.signbit(ha)).any() and (zero_b & ~np.signbit(hb)).any():
+            assert (zero_b & np.signbit(hb)).any() and (zero_a & ~np.signbit(ha)).any()
+            # a pair whose table-0 ids are -0.0 and +0.0 and that meets again in a later table
+            a0 = np.flatnonzero(zero_a[:, 0] & np.signbit(ha[:, 0]))
+            b0 = np.flatnonzero(zero_b[:, 0] & ~np.signbit(hb[:, 0]))
+            assert np.any(ha[a0][:, None, 1:] == hb[b0][None, :, 1:])
+            got.add(("join_signed_zero", 1))
+        for inf in (np.inf, -np.inf):
+            if (ha == inf).any():
+                assert any(((ha[:, j] == inf).sum() * (hb[:, j] == inf).sum()) > 0 for j in range(L))
+                got.add(("join_infinite_bucket", inf))
+    return got
+
+
+# ---- nonnegative ALS (als.cu's NNLS tail) --------------------------------------------------------------------------
+# rank -> (users, seed): 1 500 ratings of 200 movies drawn with the seed (as nnls_cases()["ill_conditioned"]), the
+# init at the same seed, regParam 1e-9: the first movie half-step has a movie that stops at iterMax = max(400, 20 k)
+NNLS_ITER_MAX = {19: (20, 6), 20: (40, 4), 21: (30, 8)}
+NNLS_REG = 1e-9
+# the rank-21 system of the batched fit, whose seed is 6: ratings drawn with seed 1, ids from 1 000
+NNLS_BATCH_21 = (30, 1, 1000)
+
+
+def nnls_ratings(users, seed, first_id=0):
+    rng = np.random.default_rng(seed)
+    u, m, r = rng.integers(0, users, 1500), rng.integers(0, 200, 1500), rng.integers(1, 11, 1500) / 2.0
+    return (u + first_id).astype(np.int32), (m + first_id).astype(np.int32), r.astype(np.float32)
+
+
+def nnls_first_half(u, m, r, k, seed):
+    """The first movie half-step (C oracle) with each movie's NNLS iterations, and its system (Am, B)."""
+    from oracle import als_cext as X
+    from oracle import als_nnls_cext as XN
+    uids, mids, by_movie, _ = A.layouts(u, m, r)
+    U = X.init_user_factors(uids, k, seed)
+    it = np.zeros(len(mids), np.int32)
+    out, _ = XN.solve_half(by_movie, U, uids, k, NNLS_REG, None, it)
+    Am, B = A.normal_equations(by_movie, U, k, NNLS_REG)
+    return out, it, np.triu(Am) + np.transpose(np.triu(Am, 1), (0, 2, 1)), B
+
+
+def movies_changed_by(Am, B, rule):
+    """The movies whose float32 factor changes when N.nnls runs under `rule` for iterMax instead of max(400, 20k)."""
+    x0, _ = N.nnls(Am, B)
+    keep = N.iter_max
+    N.iter_max = rule
+    try:
+        x1, _ = N.nnls(Am, B)
+    finally:
+        N.iter_max = keep
+    return int(np.any(x0.astype(np.float32) != x1.astype(np.float32), axis=1).sum())
+
+
+NNLS_RULES = {"20k": lambda k: 20 * k, "400": lambda k: 400}
+
+
+def iter_max_reach(u, m, r, k, seed, rules, exactly_one):
+    out, it, Am, B = nnls_first_half(u, m, r, k, seed)
+    assert (it == N.iter_max(k)).any() and (it < N.iter_max(k)).any(), (k, it.max())
+    x, its = N.nnls(Am, B)
+    assert np.array_equal(its, it) and np.array_equal(x.astype(np.float32).view(np.uint32), out.view(np.uint32))
+    got = {("nnls_iter_max", k)}
+    for name in rules:
+        assert NNLS_RULES[name](k) < N.iter_max(k)
+        changed = movies_changed_by(Am, B, NNLS_RULES[name])
+        assert changed == 1 if exactly_one else changed >= 1, (k, name, changed)
+        got.add(("nnls_iter_max_rule", name))
+    return got
+
+
+def _nnls_iter_max(k):
+    u, m, r = nnls_ratings(*NNLS_ITER_MAX[k])
+    return dict(u=u, m=m, r=r, fits=[dict(rank=k, max_iter=1, reg_param=NNLS_REG, seed=NNLS_ITER_MAX[k][1])])
+
+
+def _nnls_iter_max_reach(d):
+    k = d["fits"][0]["rank"]
+    rules = {19: ["20k"], 20: [], 21: ["400"]}[k]
+    return iter_max_reach(d["u"], d["m"], d["r"], k, d["fits"][0]["seed"], rules, True)
+
+
+NNLS_BATCH_RANKS = (1, 19, 21, 33, 64)
+
+
+def _nnls_batch(chol):
+    """kMaxModels models over three blocks of disjoint ids: the rank-19 iterMax system (fold 0), NNLS_BATCH_21 (fold
+    1) and 600 ratings in folds 0..2, where user 5000 rates only in fold 2 and movie 5000 is rated only in fold 1.
+    Ranks NNLS_BATCH_RANKS, max_iter 1 and 2, every excluded fold; models 0 and 1 are the iterMax systems (rank 19
+    without fold 1, rank 21 without fold 0).  `chol` holds the models fitted by Cholesky rather than NNLS."""
+    rng = np.random.default_rng(76)
+    u19, m19, r19 = nnls_ratings(*NNLS_ITER_MAX[19])
+    u21, m21, r21 = nnls_ratings(*NNLS_BATCH_21)
+    ue = np.r_[rng.integers(5001, 5040, 600), np.full(5, 5000), rng.integers(5001, 5040, 4)]
+    me = np.r_[rng.integers(5001, 5060, 600), rng.integers(5001, 5060, 5), np.full(4, 5000)]
+    re = rng.integers(0, 11, len(ue)) / 2.0
+    fe = np.r_[rng.integers(0, 3, 600), np.full(5, 2), np.full(4, 1)]
+    u, m = np.r_[u19, u21, ue].astype(np.int32), np.r_[m19, m21, me].astype(np.int32)
+    r = np.r_[r19, r21, re].astype(np.float32)
+    fold = np.r_[np.zeros(1500), np.ones(1500), fe].astype(np.int32)
+    models = [dict(rank=NNLS_BATCH_RANKS[i % 5], max_iter=1 + (i // 5) % 2, reg_param=(0.05, 0.01)[(i // 40) % 2],
+                   exclude_fold=(i // 10) % 4 - 1) for i in range(K["kMaxModels"])]
+    models[0] = dict(rank=19, max_iter=1, reg_param=NNLS_REG, exclude_fold=1)
+    models[1] = dict(rank=21, max_iter=1, reg_param=NNLS_REG, exclude_fold=0)
+    for i, spec in enumerate(models):
+        spec["nonnegative"] = i not in chol
+        if i in chol and spec["reg_param"] == NNLS_REG:
+            spec["reg_param"] = 0.05
+    return dict(u=u, m=m, r=r, fold=fold, n_folds=3, models=models, seed=NNLS_ITER_MAX[19][1])
+
+
+def _nnls_batch_reach(d):
+    ms = d["models"]
+    assert len(ms) == K["kMaxModels"] and {s["rank"] for s in ms} == set(NNLS_BATCH_RANKS)
+    assert {s["max_iter"] for s in ms} == {1, 2} and {s["exclude_fold"] for s in ms} == {-1, 0, 1, 2}
+    nn = sum(s["nonnegative"] for s in ms)
+    got = {("kMaxModels", len(ms)), ("nnls_batch_mix", (len(ms) - nn, nn))}
+    for s in ms:                                                     # an entity with no training rating
+        rows = d["fold"] != s["exclude_fold"]
+        if s["nonnegative"] and (len(np.unique(d["u"][rows])) < len(np.unique(d["u"]))
+                                 or len(np.unique(d["m"][rows])) < len(np.unique(d["m"]))):
+            got.add(("nnls_batch_untrained_entity", 1))
+    for i, k, (users, seed, first) in ((0, 19, NNLS_ITER_MAX[19] + (0,)), (1, 21, NNLS_BATCH_21)):
+        if ms[i]["nonnegative"] and ms[i]["reg_param"] == NNLS_REG:
+            assert ms[i]["rank"] == k and ms[i]["max_iter"] == 1
+            u, m, r = nnls_ratings(users, seed, first)
+            reach = iter_max_reach(u, m, r, k, d["seed"], {19: ["20k"], 21: ["400"]}[k], False)
+            got |= {("batch_" + a, b) for a, b in reach}
+    return got
+
+
+def _nnls_singular():
+    """singular_case() at regParam 0 in a batch of an NNLS model and a Cholesky model on the same rows, in both
+    orders: user 9's system is all zero, singular for Cholesky and not for NNLS."""
+    from test_als_oracle import singular_case
+    u, m, r = singular_case()
+    fold = (np.arange(len(u)) % 2).astype(np.int32)
+    spec = dict(rank=2, max_iter=1, reg_param=0.0, exclude_fold=-1)
+    return dict(u=u.astype(np.int32), m=m.astype(np.int32), r=r.astype(np.float32), fold=fold, n_folds=2, seed=0,
+                orders=[[dict(spec, nonnegative=True), dict(spec, nonnegative=False)],
+                        [dict(spec, nonnegative=False), dict(spec, nonnegative=True)]])
+
+
+def nnls_singular_oracle(d):
+    """Per order, the batched fit's message: the Cholesky model's index in the caller's order and its singular
+    entity, as the C oracle's single fit reports it; the NNLS single fit has no singular system."""
+    from oracle import als_cext as X
+    from oracle import als_nnls_cext as XN
+    out = []
+    for models in d["orders"]:
+        for i, s in enumerate(models):
+            kw = dict(rank=s["rank"], max_iter=s["max_iter"], reg_param=s["reg_param"], seed=d["seed"])
+            if s["nonnegative"]:
+                XN.fit(d["u"], d["m"], d["r"], **kw)
+                continue
+            with pytest.raises(A.SingularError) as e:
+                X.fit(d["u"], d["m"], d["r"], **kw)
+            out.append("model %d: singular normal equations for %s %d in iteration %d"
+                       % (i, e.value.side, e.value.entity_id, e.value.iteration))
+    return out
+
+
+def _nnls_singular_reach(d):
+    want = nnls_singular_oracle(d)
+    assert [w.split(":")[0] for w in want] == ["model 1", "model 0"]
+    return {("nnls_singular_after_nnls", 1)}
+
+
 # ---- the table --------------------------------------------------------------------------------------------------
 BOUNDS = {
     "i2v_depth24_d64_w5_p1": Case("item2vec", lambda: _caterpillar(24, 64, 5, 1, 7), _i2v_reach),
@@ -1089,6 +1603,29 @@ BOUNDS = {
     "als_implicit_solve_chunks": Case("als_implicit", _implicit_chunks, _implicit_chunks_reach),
     "ranking_lists_ballot_passes": Case("ranking_metrics", _ranking_lists, _ranking_lists_reach),
     "ranking_grid_trips": Case("ranking_metrics", _ranking_grid, _ranking_grid_reach),
+    "bm_two_grids_of_thresholds": Case("binary_metrics", _bm_two_grids, _bm_reach),
+    "bm_4194304_sets": Case("binary_metrics", lambda: _bm_sets([1 << 22], 64), _bm_reach),
+    "bm_4194305_sets": Case("binary_metrics", lambda: _bm_sets([(1 << 22) + 1], 65), _bm_reach),
+    "bm_2_3_65536_65537_sets": Case("binary_metrics", lambda: _bm_sets([2, 3, 1 << 16, (1 << 16) + 1], 66),
+                                    _bm_reach),
+    "bm_sets_at_chunk_edges": Case("binary_metrics", _bm_chunk_sets, _bm_reach),
+    "bm_float32_last_mantissa_bit": Case("binary_metrics", _bm_f32_adjacent, _bm_reach),
+    "lsh_join_keys_three_trips": Case("lsh_join", _join_keys_trips, _join_reach),
+    "lsh_join_runs_three_trips": Case("lsh_join", _join_runs_trips, _join_reach),
+    "lsh_join_segment_edges": Case("lsh_join", _join_segments, _join_reach),
+    "lsh_join_int32_extreme_ids": Case("lsh_join", _join_extreme_ids, _join_reach),
+    "lsh_join_signed_zero_buckets": Case("lsh_join", _join_signed_zero, _join_reach),
+    "lsh_join_infinite_buckets": Case("lsh_join", _join_infinite, _join_reach),
+    "als_nonnegative_iter_max_rank19": Case("als_nonnegative", lambda: _nnls_iter_max(19), _nnls_iter_max_reach),
+    "als_nonnegative_iter_max_rank20": Case("als_nonnegative", lambda: _nnls_iter_max(20), _nnls_iter_max_reach),
+    "als_nonnegative_iter_max_rank21": Case("als_nonnegative", lambda: _nnls_iter_max(21), _nnls_iter_max_reach),
+    "als_nonnegative_batch_64_nnls": Case("als_nonnegative", lambda: _nnls_batch(set()), _nnls_batch_reach),
+    "als_nonnegative_batch_1_cholesky_63_nnls": Case("als_nonnegative", lambda: _nnls_batch({37}),
+                                                     _nnls_batch_reach),
+    "als_nonnegative_batch_63_cholesky_1_nnls": Case("als_nonnegative",
+                                                     lambda: _nnls_batch(set(range(K["kMaxModels"])) - {1}),
+                                                     _nnls_batch_reach),
+    "als_nonnegative_singular_after_nnls": Case("als_nonnegative", _nnls_singular, _nnls_singular_reach),
 }
 
 
@@ -1156,6 +1693,27 @@ def test_every_bound_has_a_case():
     need |= {("rank_distinct", v) for v in (1, 31, 32, 33, "past_L")}
     need |= {("rank_k_vs_L", v) for v in (-1, 0, 1, "past")} | {("rank_steps", v) for v in (31, 32, 33, 64, 65)}
     need |= {("rank_hit_at", p) for p in RANK_HITS} | {("rank_trips", 2), ("rank_trips", 3)}
+    # binary_metrics.cu: grid trips, the set sort's bits, the area chunks and the float32 sort's first bit
+    assert STRIDE_256 == KB["kMaxGridBlocks"] * KB["kChunkThreads"]
+    cb = KB["kChunk"]
+    need |= {("bm_points_trips", 2), ("bm_curve_trips", 2), ("bm_curve_trips", 3), ("bm_roc_end_trip", 3),
+             ("bm_sets_trips", 2)}
+    need |= {("bm_set_bits", b) for b in (1, 2, 16, 17, 22, 23)}
+    need |= {("bm_set_thresholds", t) for t in (cb - 1, cb, cb + 1, 2 * cb, 2 * cb + 1, 32 * cb, 32 * cb + 1)}
+    need |= {("bm_set_chunks", c) for c in (1, 2, 3, 32, 33)} | {("bm_f32_last_bit", 29)}
+    # lsh.cu's join: grid trips, the segment walk, the sentinel, empty runs and tables, ids and bucket ids
+    G, TJ = K["kJoinSegments"], K["kJoinThreads"]
+    need |= {("join_C", c) for c in (1, G - 1, G, G + 1, TJ * G, TJ * G + 1)}
+    need |= {("join_keys_trips", 3), ("join_hash_trips", 3), ("join_runs_trips", 3), ("join_sentinel_trip", 3)}
+    need |= {("join_empty_run_at", "first"), ("join_empty_run_at", "last"), ("join_empty_table_between", 1),
+             ("join_first_table_removes", 1), ("join_signed_zero", 1)}
+    need |= {("join_id", v) for v in (-2 ** 31, -1, 0, 2 ** 31 - 1)}
+    need |= {("join_infinite_bucket", np.inf), ("join_infinite_bucket", -np.inf)}
+    # als.cu's NNLS: iterMax either side of max(400, 20 k), and the batched fit's NNLS slice
+    need |= {("nnls_iter_max", k) for k in (19, 20, 21)} | {("nnls_iter_max_rule", r) for r in ("20k", "400")}
+    need |= {("batch_nnls_iter_max", 19), ("batch_nnls_iter_max", 21), ("nnls_batch_untrained_entity", 1)}
+    need |= {("nnls_batch_mix", (0, K["kMaxModels"])), ("nnls_batch_mix", (1, K["kMaxModels"] - 1)),
+             ("nnls_batch_mix", (K["kMaxModels"] - 1, 1)), ("nnls_singular_after_nnls", 1)}
     assert need <= have, sorted(need - have)
     # the deepest case is the deepest code the rating bound allows: one level more needs more ratings than it takes
     assert sum(_deepest_counts(DEEPEST + 1)) > MAX_RATINGS >= sum(_deepest_counts(DEEPEST))
@@ -1174,6 +1732,13 @@ def test_the_constants_are_parsed():
     assert {constants(f)["kMaxRatings"] for f in RATING_BOUND_FILES} == {MAX_RATINGS}
     assert K["kSrcPerBlock"] == K["kRecWarps"] * K["kSrcPerWarp"]
     assert K["kIdMask"] == K["kMaxMovieSlots"] - 1
+    for name in ("kJoinThreads", "kJoinSegments"):
+        assert isinstance(K.get(name), int) and K[name] > 0, name
+    for name in ("kMaxPairs", "kChunk", "kChunkThreads", "kPerThread", "kMaxGridBlocks"):
+        assert isinstance(KB.get(name), int) and KB[name] > 0, name
+    assert KB["kPerThread"] * KB["kChunkThreads"] == KB["kChunk"] and KB["kMaxPairs"] == 2 ** 31 - 1
+    with pytest.raises(ValueError):                                    # two kChunk: 2 048 points, 32 ratings
+        constants("binary_metrics.cu", "als.cu")
 
 
 def test_vectorised_corpus_matches_chunk_corpus():
