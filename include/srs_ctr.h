@@ -835,6 +835,36 @@ int srs_binary_metrics_curve(const srs_binary_metrics* h, int32_t set, int32_t w
 /* the cumulative TP and FP [thresholds] int64 of `set` */
 int srs_binary_metrics_confusion(const srs_binary_metrics* h, int32_t set, int64_t* tp, int64_t* fp);
 
+/* ---- Similar movies (ON/recprocess/SimilarMovieProcess.java getRecList; DESIGN.md section 4.23) ----------------
+ * A catalogue holds n_movies movies in movies.csv order: distinct ids movie_id [n_movies], and movie m's genres
+ * genre[genre_off[m] .. genre_off[m + 1]) (genre_off [n_movies + 1], genre_off[0] = 0), each an index 0 ..
+ * n_genres - 1 (n_genres <= 64), distinct within a movie.  The ratings rating_movie / rating_score [n_ratings] (float,
+ * as Float.parseFloat reads them) in ratings.csv order give each movie Movie.addRating's running mean in double;
+ * ratings of other movies are ignored.  emb [n_emb][dim] are the rows of item2vecEmb.csv, row r the vector of
+ * movie emb_id[r] (the last row of an id wins; ids outside the catalogue are ignored).  n_emb 0 is a catalogue
+ * without vectors.  Every argument is checked before any device call (SRS_ERR_INVALID).  Synchronous. */
+typedef struct srs_similar_catalog srs_similar_catalog;
+int srs_similar_catalog_create_host(const int32_t* movie_id, int32_t n_movies, const int32_t* genre_off,
+                                    const int32_t* genre, int32_t n_genres, const int32_t* rating_movie,
+                                    const float* rating_score, int64_t n_ratings, const int32_t* emb_id,
+                                    const float* emb, int32_t n_emb, int32_t dim, int32_t device,
+                                    srs_similar_catalog** out);
+void srs_similar_catalog_destroy(srs_similar_catalog* catalog);
+#define SRS_SIMILAR_DEFAULT 0          /* calculateSimilarScore: 0.7 * genre overlap + 0.3 * averageRating / 5 */
+#define SRS_SIMILAR_EMB 1              /* the cosine of the two movies' vectors (-1 for a candidate without one) */
+#define SRS_SIMILAR_OK 0
+#define SRS_SIMILAR_UNKNOWN_MOVIE 1    /* not in the catalogue: an empty list, as the Java returns */
+#define SRS_SIMILAR_NO_EMBEDDING 2     /* model EMB and the query has no vector (the Java throws): an empty list */
+/* getRecList(movie_ids[q], size, model) for q < n_queries: the union of the top-100-by-rating lists of the query's
+ * genres minus the query, scored by `model`, ordered by score descending (Double.compare; NaN first, 0.0 above
+ * -0.0) and ties by movie id ascending, cut to size >= 1.  Host outputs: out_ids [n_queries][size] int32,
+ * out_scores [n_queries][size] double, out_count [n_queries] (entries past it are 0), out_status [n_queries]
+ * (SRS_SIMILAR_OK / _UNKNOWN_MOVIE / _NO_EMBEDDING).  An unknown id is a status, not an error.  Synchronous; the same
+ * inputs give the same bits. */
+int srs_similar_movies_host(const srs_similar_catalog* catalog, const int32_t* movie_ids, int32_t n_queries,
+                            int32_t size, int32_t model, int32_t* out_ids, double* out_scores, int32_t* out_count,
+                            int32_t* out_status);
+
 #ifdef __cplusplus
 }
 #endif

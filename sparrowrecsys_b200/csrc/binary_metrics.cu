@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "../../include/srs_ctr.h"
+#include "double_key.cuh"
 #include "hostcall.h"
 
 struct srs_binary_metrics {
@@ -54,18 +55,7 @@ constexpr int kPerThread = kChunk / kChunkThreads;
 #define BM_GRID_STRIDE(i, n) \
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < (n); i += (int64_t)gridDim.x * blockDim.x)
 
-// Spark's threshold order as an ascending unsigned key: Double.compare descending, every NaN one key (0, first)
-__device__ __forceinline__ uint64_t desc_key(double x) {
-  if (x != x) return 0;
-  uint64_t b;
-  memcpy(&b, &x, 8);
-  return (b >> 63) ? b : ~(b | (1ull << 63));
-}
-__device__ __forceinline__ double key_score(uint64_t k) {
-  if (k == 0) return __longlong_as_double(0x7ff8000000000000ll);
-  const uint64_t b = (k >> 63) ? k : ~k & ~(1ull << 63);
-  return __longlong_as_double((long long)b);
-}
+// Spark's threshold order is desc_key's (double_key.cuh): Double.compare descending, every NaN one key (0, first)
 
 // BinaryLabelCounter: a label > 0.5 is a positive (a NaN label is not)
 __device__ __forceinline__ uint32_t positive(double y) { return y > 0.5 ? 1u : 0u; }

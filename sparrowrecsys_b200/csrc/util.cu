@@ -1,4 +1,5 @@
 // util.cu - small device utilities around the forward path.
+#include "cosine.cuh"
 #include "hostcall.h"
 
 namespace srs {
@@ -108,29 +109,15 @@ cudaError_t launch_assemble_request(const int32_t* req, const void* movie_feats,
   return cudaGetLastError();
 }
 
-// Cosine similarity of one query against n candidates, one warp per candidate.
-// Reference: online/model/Embedding.java:33-47 - float products accumulated in double,
-// dot / (sqrt(n1) * sqrt(n2)).
+// Cosine similarity of one query against n candidates, one warp per candidate (cosine.cuh).
 __global__ void cosine_kernel(const float* __restrict__ q, const float* __restrict__ c, int n,
                               int dim, float* __restrict__ out) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (warp >= n) return;
-  const float* v = c + (size_t)warp * dim;
-  double dot = 0.0, n1 = 0.0, n2 = 0.0;
-  for (int k = lane; k < dim; k += 32) {
-    const float a = __ldg(q + k), bb = __ldg(v + k);
-    dot += (double)__fmul_rn(a, bb);
-    n1 += (double)__fmul_rn(a, a);
-    n2 += (double)__fmul_rn(bb, bb);
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    dot += __shfl_xor_sync(0xffffffffu, dot, o);
-    n1 += __shfl_xor_sync(0xffffffffu, n1, o);
-    n2 += __shfl_xor_sync(0xffffffffu, n2, o);
-  }
-  if (lane == 0) out[warp] = (float)(dot / (sqrt(n1) * sqrt(n2)));
+  double dot, n1, n2;
+  cosine_sums(q, c + (size_t)warp * dim, dim, lane, dot, n1, n2);
+  if (lane == 0) out[warp] = (float)cosine_value(dot, n1, n2);
 }
 
 cudaError_t launch_cosine(const float* q, const float* c, int n, int dim, float* out,
