@@ -30,7 +30,7 @@ constexpr uint32_t FS_DOTS = 26624;                      // f32 [32][4]
 constexpr uint32_t FS_ZP = 27136;                        // f32 [4][32]
 constexpr uint32_t FS_BYTES = 27648;
 
-__global__ void __launch_bounds__(128) deepfm_tc_kernel(const __grid_constant__ DeepFmTcParams p,
+__global__ void __launch_bounds__(128) deepfm_tc_kernel(const __grid_constant__ DeepFmParams p,
                                                         BatchView b) {
   extern __shared__ uint8_t raw[];
   __shared__ uint64_t wbar;
@@ -62,6 +62,8 @@ __global__ void __launch_bounds__(128) deepfm_tc_kernel(const __grid_constant__ 
   __syncthreads();
   const uint32_t s_img = smem_u32(img), s_x = smem_u32(sc + FS_X);
   bool weights_ready = false;
+  // the numerics' rows of W1 (DeepFmBlob at EP = 16: rows 32..39, after the deep pair), which no MMA takes
+  const float* w1_numerics = p.W1 + 2 * 16 * 64;
   // this thread's accumulator rows are units u_i = 16 warp + g + 8 i of both layers
   float b1[2], b2[2], wdeep[2], w1n[2][kNumNumerics];
 #pragma unroll
@@ -69,7 +71,7 @@ __global__ void __launch_bounds__(128) deepfm_tc_kernel(const __grid_constant__ 
     const int u = 16 * warp + g + 8 * i;
     b1[i] = __ldg(p.b1 + u); b2[i] = __ldg(p.b2 + u); wdeep[i] = __ldg(p.wdeep + u);
 #pragma unroll
-    for (int n = 0; n < kNumNumerics; ++n) w1n[i][n] = __ldg(p.w1_numerics + n * 64 + u);
+    for (int n = 0; n < kNumNumerics; ++n) w1n[i][n] = __ldg(w1_numerics + n * 64 + u);
   }
 
   const int n_sg = (b.B + kFtRows - 1) / kFtRows;
@@ -238,7 +240,7 @@ __global__ void __launch_bounds__(128) deepfm_tc_kernel(const __grid_constant__ 
 
 static size_t deepfm_tc_smem() { return 1024 + FIMG_BYTES + FS_BYTES; }
 
-cudaError_t launch_deepfm_tc(const DeepFmTcParams& p, const BatchView& b, cudaStream_t s) {
+cudaError_t launch_deepfm_tc(const DeepFmParams& p, const BatchView& b, cudaStream_t s) {
   if (b.B <= 0) return cudaSuccess;
   const int n_sg = (b.B + kFtRows - 1) / kFtRows;
   const int cap = 2 * p.num_sms;                         // two CTAs fit per SM

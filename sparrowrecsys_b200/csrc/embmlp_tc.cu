@@ -31,10 +31,11 @@ constexpr uint32_t ES_NUMS = 65536;                      // f32 [64][8]
 constexpr uint32_t ES_ZP = 67584;                        // f32 [4][64]
 constexpr uint32_t ES_BYTES = 68608;
 
-__global__ void __launch_bounds__(256, 1) embmlp_tc_kernel(const __grid_constant__ EmbMlpTcParams p,
+__global__ void __launch_bounds__(256, 1) embmlp_tc_kernel(const __grid_constant__ EmbMlpParams p,
                                                             BatchView b) {
   extern __shared__ uint8_t raw[];
   __shared__ uint64_t wbar;
+  __shared__ float b3;      // dense_2/bias from the blob, once per CTA (a register would stay live through the MMAs)
   const int tid = threadIdx.x, q = tid >> 7, tw = tid & 127, warp_w = tw >> 5;
   const int lane = tw & 31, g = lane >> 2, cq = lane & 3;
   uint8_t* base = raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
@@ -55,6 +56,8 @@ __global__ void __launch_bounds__(256, 1) embmlp_tc_kernel(const __grid_constant
   __syncthreads();
   const uint32_t s_img = smem_u32(img), s_x = smem_u32(sc + ES_X);
   bool weights_ready = false;
+  // the numerics' rows of W1 (EmbMlpBlob at EP = 12: rows 120..127, after the ten slots), which no MMA takes
+  const float* w1_numerics = p.W1 + 10 * 12 * 128;
   // this thread's accumulator rows are units u_i = 64 q + 16 warp_w + g + 8 i of both layers
   float b1[2], b2[2], w3[2], w1n[2][kNumNumerics];
 #pragma unroll
@@ -62,8 +65,9 @@ __global__ void __launch_bounds__(256, 1) embmlp_tc_kernel(const __grid_constant
     const int u = 64 * q + 16 * warp_w + g + 8 * i;
     b1[i] = __ldg(p.b1 + u); b2[i] = __ldg(p.b2 + u); w3[i] = __ldg(p.w3 + u);
 #pragma unroll
-    for (int n = 0; n < kNumNumerics; ++n) w1n[i][n] = __ldg(p.w1_numerics + n * 128 + u);
+    for (int n = 0; n < kNumNumerics; ++n) w1n[i][n] = __ldg(w1_numerics + n * 128 + u);
   }
+  if (tid == 0) b3 = __ldg(p.b3);                        // the layers' barriers order it before the Dense(1)
 
   const int n_sg = (b.B + kEtRows - 1) / kEtRows;
   for (int sg = blockIdx.x; sg < n_sg; sg += gridDim.x) {
@@ -178,7 +182,7 @@ __global__ void __launch_bounds__(256, 1) embmlp_tc_kernel(const __grid_constant
     if (tid < kEtRows) {
       const int row = row0 + tid;
       if (row < b.B) {
-        float z = p.b3 + ((zp[tid] + zp[kEtRows + tid]) + (zp[2 * kEtRows + tid] + zp[3 * kEtRows + tid]));
+        float z = b3 + ((zp[tid] + zp[kEtRows + tid]) + (zp[2 * kEtRows + tid] + zp[3 * kEtRows + tid]));
         if (p.wide) {
           const int mid = checked_id(__ldg(b.movie_id + row), p.n_movies, b.err_flag);
           const int rated = checked_id(__ldg(b.hist + (size_t)row * b.hist_stride), p.n_movies, b.err_flag);
@@ -195,7 +199,7 @@ __global__ void __launch_bounds__(256, 1) embmlp_tc_kernel(const __grid_constant
 
 static size_t embmlp_tc_smem() { return 1024 + EIMG_BYTES + ES_BYTES; }
 
-cudaError_t launch_embmlp_tc(const EmbMlpTcParams& p, const BatchView& b, cudaStream_t s) {
+cudaError_t launch_embmlp_tc(const EmbMlpParams& p, const BatchView& b, cudaStream_t s) {
   if (b.B <= 0) return cudaSuccess;
   const int n_sg = (b.B + kEtRows - 1) / kEtRows;
   const int grid = n_sg < p.num_sms ? n_sg : p.num_sms;

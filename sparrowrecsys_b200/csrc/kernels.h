@@ -83,6 +83,9 @@ struct EmbMlpParams {
   const float* wide;       // [cross_buckets] wide rows of dense_2 (nullptr for EmbeddingMLP)
   int n_movies, n_users, n_genres, cross_buckets;
   int EP;
+  const uint8_t* image;    // embmlp_tc.cu, EP = 12: W1^T hi / lo, W2^T hi / lo as bf16 SW128 operand tiles (128 KB);
+                           //   null: embmlp_kernel runs
+  int num_sms;             // embmlp_tc.cu: CTAs per launch at most, one per SM (srs_model_set_sm_limit)
 };
 
 // The Dense weights of EmbeddingMLP and Wide&Deep (a model's and a trainer's) as one blob, offsets in floats:
@@ -117,23 +120,6 @@ struct WideDeepStepArgs {
 int widendeep_train_ctas(int B);
 cudaError_t launch_widendeep_train_step(int EP, const WideDeepStepArgs* a, cudaStream_t s);
 
-// ---- EmbeddingMLP / Wide&Deep on tensor cores (embmlp_tc.cu): E <= 12 ------------------------
-struct EmbMlpTcParams {
-  const float* genre[8];   // [19][12]
-  const float* movie;      // [n_movies][12]
-  const float* user;       // [n_users][12]
-  const uint8_t* image;    // 128 KB: W1^T hi/lo, W2^T hi/lo as bf16 SW128 operand tiles
-  const float* b1;         // [128]
-  const float* w1_numerics;   // [8][128] the numerics' rows of EmbMlpBlob's W1 (rows 120..127, in the blob): the
-                              //   rows no MMA takes
-  const float* b2;         // [128]
-  const float* w3;         // [128]
-  const float* wide;       // [cross_buckets] or nullptr
-  float b3;
-  int n_movies, n_users, n_genres, cross_buckets;
-  int num_sms;
-};
-
 // ---- DeepFM (DeepFM.py:91-113) -----------------------------------------------------
 struct DeepFmParams {
   const float* fm_movie;   // [n_movies][EP]
@@ -149,10 +135,13 @@ struct DeepFmParams {
   const float* b2;
   const float* first;      // [fm1_width] one-hot rows of dense_2 (movieGenre1|movieId|userGenre1|userId)
   const float* wdeep;      // [64]
-  float wdot[4];           // dense_2's dot rows and bias: deepfm_kernel and the training step load them from the
-  float bout;              //   blob (deepfm_load_out), deepfm_tc_kernel takes them from here
+  float wdot[4];           // dense_2's dot rows and bias, copied from the blob by build_deepfm for deepfm_tc_kernel;
+  float bout;              //   deepfm_kernel and the training step load them from the blob (deepfm_load_out)
   int n_movies, n_users, n_genres;
   int EP;
+  const uint8_t* image;    // deepfm_tc.cu, EP = 16: W1^T hi / lo, W2^T hi / lo as [128][64] bf16 SW128 tiles (64 KB);
+                           //   null: deepfm_kernel runs
+  int num_sms;             // deepfm_tc.cu: CTAs per launch at most, two per SM (srs_model_set_sm_limit)
 };
 
 // The Dense weights of DeepFM (a model's and a trainer's) as one blob, offsets in floats: W1 [2EP + 8][64] and
@@ -202,27 +191,6 @@ cudaError_t launch_deepfm_permute(const TrainRows& src, const TrainRows& dst, co
 // the same for Wide&Deep: every genre column and userRatedMovie1
 cudaError_t launch_widendeep_permute(const TrainRows& src, const TrainRows& dst, const int32_t* order, int n,
                                      cudaStream_t s);
-
-// ---- DeepFM with the deep MLP on tensor cores (deepfm_tc.cu): emb_dim 13..16 --------------------
-struct DeepFmTcParams {
-  const float* fm_movie;   // [n_movies][16]
-  const float* fm_user;
-  const float* fm_mgenre;
-  const float* fm_ugenre;
-  const float* deep_movie;
-  const float* deep_user;
-  const uint8_t* image;    // 64 KB: W1^T hi/lo, W2^T hi/lo as [128][64] bf16 SW128 tiles
-  const float* b1;         // [64]
-  const float* w1_numerics;   // [8][64] the numerics' rows of DeepFmBlob's W1 (rows 32..39, in the blob): the
-                              //   rows no MMA takes
-  const float* b2;         // [64]
-  const float* first;      // [fm1_width]
-  const float* wdeep;      // [64]
-  float wdot[4];
-  float bout;
-  int n_movies, n_users, n_genres;
-  int num_sms;
-};
 
 // ---- DeepFM_v2 (DeepFM_v2.py:98-155) -----------------------------------------------
 struct DeepFm2Params {
@@ -479,9 +447,9 @@ cudaError_t launch_din_wg(const DinParams& p, const BatchView& b, cudaStream_t s
 cudaError_t launch_split_table(const float* src, void* dst, int64_t rows, int EP, cudaStream_t s);
 cudaError_t launch_ncf(const NcfParams& p, const BatchView& b, cudaStream_t s);
 cudaError_t launch_embmlp(const EmbMlpParams& p, const BatchView& b, cudaStream_t s);
-cudaError_t launch_embmlp_tc(const EmbMlpTcParams& p, const BatchView& b, cudaStream_t s);
+cudaError_t launch_embmlp_tc(const EmbMlpParams& p, const BatchView& b, cudaStream_t s);
 cudaError_t launch_deepfm(const DeepFmParams& p, const BatchView& b, cudaStream_t s);
-cudaError_t launch_deepfm_tc(const DeepFmTcParams& p, const BatchView& b, cudaStream_t s);
+cudaError_t launch_deepfm_tc(const DeepFmParams& p, const BatchView& b, cudaStream_t s);
 cudaError_t launch_deepfm2(const DeepFm2Params& p, const BatchView& b, cudaStream_t s);
 cudaError_t launch_din(const DinParams& p, const BatchView& b, cudaStream_t s);
 cudaError_t launch_dien(const DienParams& p, const BatchView& b, cudaStream_t s);

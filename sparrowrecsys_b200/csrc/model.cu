@@ -169,11 +169,6 @@ struct srs_model {
   DinParams din{};
   DienParams dien{};
   DienAuxView dien_aux{};            // DIEN's auxiliary-head weights (w == nullptr: built without them)
-  bool use_din_wg = false;           // din holds the parameters of din_wg_kernel
-  EmbMlpTcParams emb_tc{};
-  bool use_emb_tc = false;
-  DeepFmTcParams fm_tc{};
-  bool use_fm_tc = false;
   const char* kernel_name = "";
   int zero_copy_scores = -1;         // the zero_copy_scores option: 0 switches the latency path of srs_predict_host
                                      // off; 1 (experimental): kernels write the scores of every host batch
@@ -198,6 +193,8 @@ struct srs_metrics {
 
 namespace {
 inline int* slot_err(srs_model* m, const Slot& s) { return m->err_flag + 1 + (&s - m->slots); }
+// build_din_wg has given din the pre-split history table that din_wg_kernel gathers from (else din_kernel runs)
+inline bool runs_din_wg(const srs_model* m) { return m->din.movie_split != nullptr; }
 }  // namespace
 
 namespace {
@@ -493,7 +490,6 @@ int build_din_wg(Builder& B) {
   e = launch_split_table(p.movie, d_split, m->spec.n_movies, m->EP, nullptr);
   if (e != cudaSuccess) return fail(SRS_ERR_CUDA, "table split failed: %s", cudaGetErrorString(e));
   p.movie_split = static_cast<const uint8_t*>(d_split);
-  m->use_din_wg = true;
   m->kernel_name = "din_wg_kernel";
   return B.status;
 }
@@ -501,46 +497,28 @@ int build_din_wg(Builder& B) {
 // Tensor-core EmbeddingMLP / W&D (E <= 12): operand images from the blob build_embmlp placed.
 int build_embmlp_tc(Builder& B) {
   srs_model* m = B.m;
-  const srs_spec& s = m->spec;
   const EmbMlpBlob ly = EmbMlpBlob::of(12);
   // W1^T over K = slot * 12 + e (the ten slots; the numerics' rows stay out of the MMA), W2^T
   std::vector<uint8_t> img(131072, 0);
   write_wt(img.data() + 0, img.data() + 32768, B.blob.data() + ly.W1, 10 * 12, 128, 128, 2);
   write_wt(img.data() + 65536, img.data() + 98304, B.blob.data() + ly.W2, 128, 128, 128, 2);
-  EmbMlpTcParams& p = m->emb_tc;
-  const EmbMlpParams& v1 = m->emb;
-  for (int k = 0; k < 8; ++k) p.genre[k] = v1.genre[k];
-  p.movie = v1.movie; p.user = v1.user;
-  p.image = B.upload(img);
-  p.b1 = v1.b1; p.w1_numerics = v1.W1 + 10 * 12 * 128; p.b2 = v1.b2; p.w3 = v1.w3; p.wide = v1.wide; p.b3 = B.blob[ly.b3];
-  p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres; p.cross_buckets = s.cross_buckets;
-  p.num_sms = m->device_sms;
-  m->use_emb_tc = true;
-  m->kernel_name = s.kind == SRS_WIDENDEEP ? "embmlp_tc_kernel<wide&deep>" : "embmlp_tc_kernel";
+  m->emb.image = B.upload(img);
+  m->emb.num_sms = m->device_sms;
+  m->kernel_name = m->spec.kind == SRS_WIDENDEEP ? "embmlp_tc_kernel<wide&deep>" : "embmlp_tc_kernel";
   return B.status;
 }
 
 // Tensor-core DeepFM (emb_dim 13..16): operand images from the blob build_deepfm placed.
 int build_deepfm_tc(Builder& B) {
   srs_model* m = B.m;
-  const srs_spec& s = m->spec;
   const DeepFmBlob ly = DeepFmBlob::of(16);
   // W1^T over K = [deep movieId emb (16) | deep userId emb (16) | 0] (the numerics' rows stay out of the MMA), W2^T;
   // units 64..127 are zero
   std::vector<uint8_t> img(65536, 0);
   write_wt(img.data() + 0, img.data() + 16384, B.blob.data() + ly.W1, 2 * 16, 64, 128, 1);
   write_wt(img.data() + 32768, img.data() + 49152, B.blob.data() + ly.W2, 64, 64, 128, 1);
-  DeepFmTcParams& p = m->fm_tc;
-  const DeepFmParams& v1 = m->fm;
-  p.fm_movie = v1.fm_movie; p.fm_user = v1.fm_user; p.fm_mgenre = v1.fm_mgenre; p.fm_ugenre = v1.fm_ugenre;
-  p.deep_movie = v1.deep_movie; p.deep_user = v1.deep_user;
-  p.image = B.upload(img);
-  p.b1 = v1.b1; p.w1_numerics = v1.W1 + 2 * 16 * 64; p.b2 = v1.b2; p.first = v1.first; p.wdeep = v1.wdeep;
-  for (int d = 0; d < 4; ++d) p.wdot[d] = v1.wdot[d];
-  p.bout = v1.bout;
-  p.n_movies = s.n_movies; p.n_users = s.n_users; p.n_genres = s.n_genres;
-  p.num_sms = m->device_sms;
-  m->use_fm_tc = true;
+  m->fm.image = B.upload(img);
+  m->fm.num_sms = m->device_sms;
   m->kernel_name = "deepfm_tc_kernel";
   return B.status;
 }
@@ -627,14 +605,14 @@ int launch(srs_model* m, const BatchView& v, cudaStream_t stream) {
     case SRS_TWOTOWERS: e = launch_ncf(m->ncf, v, stream); break;
     case SRS_EMBEDDINGMLP:
     case SRS_WIDENDEEP:
-      e = m->use_emb_tc ? launch_embmlp_tc(m->emb_tc, v, stream) : launch_embmlp(m->emb, v, stream);
+      e = m->emb.image ? launch_embmlp_tc(m->emb, v, stream) : launch_embmlp(m->emb, v, stream);
       break;
     case SRS_DEEPFM:
-      e = m->use_fm_tc ? launch_deepfm_tc(m->fm_tc, v, stream) : launch_deepfm(m->fm, v, stream);
+      e = m->fm.image ? launch_deepfm_tc(m->fm, v, stream) : launch_deepfm(m->fm, v, stream);
       break;
     case SRS_DEEPFM_V2: e = launch_deepfm2(m->fm2, v, stream); break;
     case SRS_DIN:
-      e = m->use_din_wg ? launch_din_wg(m->din, v, stream) : launch_din(m->din, v, stream);
+      e = runs_din_wg(m) ? launch_din_wg(m->din, v, stream) : launch_din(m->din, v, stream);
       break;
     case SRS_DIEN: e = launch_dien(m->dien, v, stream); break;
     default: return fail(SRS_ERR_INVALID, "unknown model kind");
@@ -1143,7 +1121,7 @@ int srs_predict_device_gather(srs_model* m, const srs_batch* b, srs_gather* gg, 
   rc = device_view(m, b, nullptr, nullptr, &v);          // gather_begin_step points the scores at the exchange
   if (rc != SRS_OK) return rc;
   CUDA_TRY(cudaSetDevice(m->device));
-  const bool in_kernel = m->spec.kind == SRS_DIN && m->use_din_wg;   // kernels ending in gather_signal_tail()
+  const bool in_kernel = m->spec.kind == SRS_DIN && runs_din_wg(m);   // kernels ending in gather_signal_tail()
   gather_begin_step(g, v, in_kernel);
   rc = launch(m, v, static_cast<cudaStream_t>(stream));
   if (rc != SRS_OK) return rc;
@@ -1246,8 +1224,8 @@ int srs_model_set_sm_limit(srs_model* m, int32_t n_sms) {
   if (!m) return fail(SRS_ERR_INVALID, "null model");
   const int n = (n_sms <= 0 || n_sms > m->device_sms) ? m->device_sms : n_sms;
   std::lock_guard<std::mutex> lock(m->mu);
-  m->emb_tc.num_sms = n;
-  m->fm_tc.num_sms = n;
+  m->emb.num_sms = n;
+  m->fm.num_sms = n;
   m->din.max_ctas = n < m->device_sms ? n : 0;
   return SRS_OK;
 }
@@ -1607,7 +1585,7 @@ int srs_debug_din_phases(const srs_model* m, uint64_t* out, int32_t n) {
   CUDA_TRY(cudaSetDevice(m->device));
   CUDA_TRY(cudaDeviceSynchronize());
   unsigned long long c[kDinPhases];
-  CUDA_TRY(m->use_din_wg ? din_wg_take_phases(c) : din_take_phases(c));
+  CUDA_TRY(runs_din_wg(m) ? din_wg_take_phases(c) : din_take_phases(c));
   for (int i = 0; i < kDinPhases; ++i) out[i] = c[i];
   return SRS_OK;
 }
