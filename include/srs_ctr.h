@@ -865,6 +865,37 @@ int srs_similar_movies_host(const srs_similar_catalog* catalog, const int32_t* m
                             int32_t size, int32_t model, int32_t* out_ids, double* out_scores, int32_t* out_count,
                             int32_t* out_status);
 
+/* ---- Multi-channel and embedding recall (SimilarMovieProcess.java:56-112; DESIGN.md section 4.24) -------------
+ * srs_similar_catalog_create_host with each movie's release_year [n_movies] as well (DataManager.parseReleaseYear:
+ * 0 where it fails), which multi-channel recall needs; srs_similar_catalog_create_host is this call with NULL.
+ * getMovies(size, sortBy) orders the movies of DataManager.movieMap, a HashMap<Integer, Movie>, whose iteration
+ * order (bucket (id ^ id >>> 16) & (capacity - 1) ascending, load order within a bucket) breaks ties.  When the
+ * load would treeify a bin (9 or more ids in one bucket of a table of 64 or more), which reorders it, the catalogue
+ * is still created but both recalls reject it (SRS_ERR_INVALID) before any device call. */
+int srs_similar_catalog_create_ex_host(const int32_t* movie_id, int32_t n_movies, const int32_t* genre_off,
+                                       const int32_t* genre, int32_t n_genres, const int32_t* rating_movie,
+                                       const float* rating_score, int64_t n_ratings, const int32_t* emb_id,
+                                       const float* emb, int32_t n_emb, int32_t dim, const int32_t* release_year,
+                                       int32_t device, srs_similar_catalog** out);
+#define SRS_SIMILAR_CANDIDATES_GENRE 0     /* candidateGenerator: the query's genres' top 100 by rating */
+#define SRS_SIMILAR_CANDIDATES_MULTIPLE 1  /* multipleRetrievalCandidates: the query's genres' top 20 by rating,
+                                              getMovies(100, "rating") and getMovies(100, "releaseYear") */
+/* srs_similar_movies_host with the candidates of `candidates` (GENRE: exactly srs_similar_movies_host).  MULTIPLE
+ * needs a catalogue created with release years; a query movie with no genres still gets the two global lists.
+ * The candidates are the union minus the query, ranked as srs_similar_movies_host ranks them. */
+int srs_similar_movies_candidates_host(const srs_similar_catalog* catalog, int32_t candidates,
+                                       const int32_t* movie_ids, int32_t n_queries, int32_t size, int32_t model,
+                                       int32_t* out_ids, double* out_scores, int32_t* out_count, int32_t* out_status);
+/* retrievalCandidatesByEmbedding(movie_ids[q], size): every movie of getMovies(10000, "rating"), the query itself
+ * included, scored by the emb ranker's cosine (-1 for a movie without a vector, NaN for a zero vector), in
+ * ascending Double.compare order (-1s first, NaN last; the Java's Map.Entry.comparingByValue(), so the least similar
+ * movies come first), ties by movie id, cut to size >= 1.  Outputs as srs_similar_movies_host's; an unknown id is
+ * SRS_SIMILAR_UNKNOWN_MOVIE and a query without a vector SRS_SIMILAR_NO_EMBEDDING (the Java returns null for both),
+ * each with an empty list.  Synchronous; the same inputs give the same bits. */
+int srs_similar_embedding_recall_host(const srs_similar_catalog* catalog, const int32_t* movie_ids,
+                                      int32_t n_queries, int32_t size, int32_t* out_ids, double* out_scores,
+                                      int32_t* out_count, int32_t* out_status);
+
 #ifdef __cplusplus
 }
 #endif
