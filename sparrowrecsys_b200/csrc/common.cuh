@@ -283,8 +283,11 @@ __device__ __forceinline__ void gather_row(float* dst, const float* __restrict__
 // vocabulary latches the error flag.  The ids are read here, the rows and numerics are copied by
 // cp.async (16-byte row chunks, 4-byte numerics, a zero fill where the row is zero) that is not
 // waited for: the caller waits for its cp.async groups (stage_wait) and passes a barrier before
-// the tile is read.  NT: the CTA's thread count.
-template <int EP, int R, int NT = kThreads>
+// the tile is read.  NT: the CTA's thread count.  kRowsL1: the rows are copied through L1 (cp.async.ca), which
+// din_wg_kernel wants (its gathers keep L1 for rows, and the 20 genre rows recur in every tile), instead of L2
+// only (.cg), which measured about 1 % faster for din_kernel.  Valid because no predict launch writes a table
+// that it gathers (L1 does not see other SMs' writes).
+template <int EP, int R, int NT = kThreads, bool kRowsL1 = false>
 __device__ __forceinline__ void tile_side_features(float* __restrict__ Xs, int ldx, int row0,
                                                    const BatchView& b, const float* user,
                                                    const float* ugenre, const float* mgenre,
@@ -312,9 +315,14 @@ __device__ __forceinline__ void tile_side_features(float* __restrict__ Xs, int l
       }
     }
     // source size 0 reads nothing (the address stays a valid row) and zero-fills the 16 bytes
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;"
-                 ::"r"(xs + 4u * (r * ldx + off + 4 * q)), "l"(table + (size_t)max(id, 0) * EP + 4 * q),
-                 "r"(id >= 0 ? 16u : 0u) : "memory");
+    if constexpr (kRowsL1)
+      asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;"
+                   ::"r"(xs + 4u * (r * ldx + off + 4 * q)), "l"(table + (size_t)max(id, 0) * EP + 4 * q),
+                   "r"(id >= 0 ? 16u : 0u) : "memory");
+    else
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;"
+                   ::"r"(xs + 4u * (r * ldx + off + 4 * q)), "l"(table + (size_t)max(id, 0) * EP + 4 * q),
+                   "r"(id >= 0 ? 16u : 0u) : "memory");
   }
   for (int i = threadIdx.x; i < R * kNumPad; i += NT) {
     const int r = i / kNumPad, j = i % kNumPad;

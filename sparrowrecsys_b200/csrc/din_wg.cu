@@ -370,8 +370,8 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
     if constexpr (!L::TC_MLP) {
       // E <= 64: the tile's inputs by the whole CTA, between two CTA-wide barriers (DESIGN §4.1: the per-warpgroup
       // flow below measured 1 % slower at cfg 5, whose walk of 44 items per warpgroup dominates the tile)
-      tile_side_features<EP, kWgRows, NT>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users, p.n_genres,
-                                          OFF_UG, OFF_U, OFF_MG, OFF_NUM);
+      tile_side_features<EP, kWgRows, NT, true>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users,
+                                                p.n_genres, OFF_UG, OFF_U, OFF_MG, OFF_NUM);
       // candidate rows of the tile (ids pass through float32, DIN.py:95,125); rows past the batch end are zero
       for (int i = tid; i < kWgRows * EP / 4; i += NT) {
         const int r = i / (EP / 4), c4 = i % (EP / 4), row = row0 + r;
@@ -419,7 +419,8 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
     const int n_items = (nrows + R - 1) / R * nch;
     // The history ids of an item are requested (into registers) two items before its rows are gathered,
     // so the HBM latency of the ids is not on the item chain.  Whether a slot is live is decided from its
-    // position, never from the id value: every live id goes through the range check.
+    // position, never from the id value: every live id goes through the range check.  The ids are read once
+    // and take no L1 line (ldg_stream): L1 stays with the embedding rows the gathers read again (DESIGN §4.1).
     // With one chunk per row (T <= 64) the item is the pair: no division
     auto item_pair = [&](int k) { return nch == 1 ? k : k / nch; };
     auto item_ch = [&](int k) { return nch == 1 ? 0 : k % nch; };
@@ -434,7 +435,7 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
   #pragma unroll
         for (int n = 0; n < NCOPY; ++n) {
           const int pos = (tw + 128 * n) / CP;
-          ids[s][n] = pos < nts ? __ldg(hrow + pos) : 0;
+          ids[s][n] = pos < nts ? ldg_stream(hrow + pos) : 0;
         }
       }
     };
@@ -486,8 +487,8 @@ __global__ void __launch_bounds__(DinWgLayout<EP>::THREADS, 1) din_wg_kernel(Din
             *reinterpret_cast<float4*>(Xs + r * L::LDX + OFF_POOL + 4 * c4) = make_float4(0.f, 0.f, 0.f, 0.f);
         }
         cp_async_commit();
-        tile_side_features<EP, kWgRows, NT>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users,
-                                            p.n_genres, OFF_UG, OFF_U, OFF_MG, OFF_NUM);
+        tile_side_features<EP, kWgRows, NT, true>(Xs, L::LDX, row0, b, p.user, p.ugenre, p.mgenre, p.n_users,
+                                                  p.n_genres, OFF_UG, OFF_U, OFF_MG, OFF_NUM);
       }
       gather(0, ids0);
     }

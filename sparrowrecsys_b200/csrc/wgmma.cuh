@@ -196,14 +196,25 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
 __device__ __forceinline__ void prefetch_l1(const void* p) {
   asm volatile("prefetch.global.L1 [%0];" ::"l"(p));
 }
+// read-only load that allocates no L1 line (L1::no_allocate): for a stream read once, so that it does not
+// evict the rows that cp_async16_zfill finds in L1
+__device__ __forceinline__ int ldg_stream(const int* p) {
+  int v;
+  asm("ld.global.nc.L1::no_allocate.b32 %0, [%1];" : "=r"(v) : "l"(p));
+  return v;
+}
 
 // ---- cp.async, named barriers --------------------------------------------------------------
 __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
-// copies the first src_bytes (0 or 16) of src and zero-fills the rest of the 16 bytes; 0 reads nothing
+// copies the first src_bytes (0 or 16) of src and zero-fills the rest of the 16 bytes; 0 reads nothing.
+// The source goes through L1 (.ca): the embedding rows it copies are gathered by id, and a few ids (the
+// padding row, popular movies) recur across a CTA's tiles, so a row read once is served from L1 after that
+// instead of queueing with every other SM on the same L2 line.  L1 is not coherent with other SMs' writes:
+// this is valid because no predict launch writes a table that it gathers.
 __device__ __forceinline__ void cp_async16_zfill(void* dst, const void* src, uint32_t src_bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(src_bytes)
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(src_bytes)
                : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }

@@ -3,10 +3,15 @@
     python tools/din_phases.py [--batches 64] [--launches 400]
 
 Prints, for din_wg_kernel (din_impl=tc) and din_kernel (din_impl=cudacore):
-  * the share of cycles per phase (srs::DinPhase, csrc/common.cuh), from a phase-timing build of the
-    library (-DSRS_DIN_PHASES) compiled into a temporary directory - the in-tree library is untouched;
+  * the share of cycles per phase (srs::DinPhase, csrc/common.cuh) on bench's inputs, from a phase-timing
+    build of the library (-DSRS_DIN_PHASES) compiled into a temporary directory - the in-tree library is
+    untouched;
   * the kernel time per batch with CUDA events over many launches of the in-tree library, in bench.py's
-    default mode (two streams, each launch capped to SMs / 2 CTAs) and on a single stream;
+    default mode (two streams, each launch capped to SMs / 2 CTAs) and on a single stream, for four sets
+    of history ids with the same shapes and the same number of row gathers (INPUTS): bench's Zipf ids
+    with 0-padded histories, Zipf ids with every history full, and uniform ids padded and full.  Zipf
+    ids and padding make a few table rows hot (half of bench's history positions read row 0); uniform
+    full histories spread the reads over the whole table, so the sets show what reuse of rows costs;
   * the card name and power limit.
 Needs a GPU.
 """
@@ -24,17 +29,23 @@ sys.path.insert(0, ROOT)
 PHASES = ["tile inputs", "W_r / folded column", "gather issue", "gather wait", "AU MMA", "gate", "pooling",
           "AU position loop", "row imbalance", "top MLP", "image wait"]
 IMPLS = (("tc", "din_wg_kernel"), ("cudacore", "din_kernel"))
+# name -> synthetic_features options; the first is bench's inputs
+INPUTS = (("zipf, padded", {}),
+          ("zipf, full", {"pad_history": False}),
+          ("uniform, padded", {"uniform_history": True}),
+          ("uniform, full", {"uniform_history": True, "pad_history": False}))
 
 
-def make_ring(n_batches, B, seed=1):
-    """n_batches distinct cfg 3 batches in HBM (together larger than the L2), and a cfg 3 model per impl."""
+def make_ring(n_batches, B, seed=1, **history):
+    """n_batches distinct cfg 3 batches in HBM (together larger than the L2), and a cfg 3 model per impl.
+    `history`: synthetic_features' options for the history ids (INPUTS)."""
     import torch
     from sparrowrecsys_b200.features import synthetic_features
     from sparrowrecsys_b200.spec import baseline_spec
     from sparrowrecsys_b200.weights import init_weights
     spec = baseline_spec("cfg3_din")
     W = init_weights(spec, 2)
-    feats = synthetic_features(spec, n_batches * B, seed=seed)
+    feats = synthetic_features(spec, n_batches * B, seed=seed, **history)
     batches = [{k: v[i * B:(i + 1) * B] for k, v in feats.items()} for i in range(n_batches)]
     return spec, W, batches, torch
 
@@ -65,10 +76,10 @@ def phases(args):
     print(json.dumps(out))
 
 
-def timing(args):
+def timing(args, history):
     """Kernel time per batch of the in-tree library: CUDA events around `launches` launches."""
     from sparrowrecsys_b200.model import CTRModel
-    spec, W, batches, torch = make_ring(args.batches, args.batch)
+    spec, W, batches, torch = make_ring(args.batches, args.batch, **history)
     n_sms = torch.cuda.get_device_properties(0).multi_processor_count
     res = {}
     for impl, name in IMPLS:
@@ -130,7 +141,8 @@ def main():
     from sparrowrecsys_b200 import build
     build.build()
     print(json.dumps({"card": card()}))
-    print(json.dumps({"kernel_time": timing(args)}))
+    for name, history in INPUTS:
+        print(json.dumps({"kernel_time": timing(args, history), "history": name}))
     with tempfile.TemporaryDirectory(prefix="srs_din_phases_") as tmp:
         lib = build.build(defines=["SRS_DIN_PHASES"], out_dir=tmp)
         env = dict(os.environ, SRS_CTR_LIB=lib)
