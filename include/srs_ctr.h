@@ -896,6 +896,37 @@ int srs_similar_embedding_recall_host(const srs_similar_catalog* catalog, const 
                                       int32_t n_queries, int32_t size, int32_t* out_ids, double* out_scores,
                                       int32_t* out_count, int32_t* out_status);
 
+/* ---- Recommended for you (ON/recprocess/RecForYouProcess.java getRecList; DESIGN.md section 4.25) -------------
+ * A user table holds DataManager.userMap: every distinct user id of rating_user [n_ratings] (the userId column of
+ * ratings.csv's 4-field lines, whether or not the movie is known), and each user's vector from the userEmb.csv rows
+ * emb [n_emb][dim], row r the vector of user emb_user[r] (the last row of a user wins; rows of users outside the
+ * table are ignored).  n_emb 0 is a table without vectors.  Every argument is checked before any device call
+ * (SRS_ERR_INVALID).  Synchronous. */
+typedef struct srs_recforyou_users srs_recforyou_users;
+int srs_recforyou_users_create_host(const int32_t* rating_user, int64_t n_ratings, const int32_t* emb_user,
+                                    const float* emb, int32_t n_emb, int32_t dim, int32_t device,
+                                    srs_recforyou_users** out);
+void srs_recforyou_users_destroy(srs_recforyou_users* users);
+#define SRS_RECFORYOU_DEFAULT 0        /* any other model string: candidates.size() - i for candidate i */
+#define SRS_RECFORYOU_EMB 1            /* "emb": the cosine of the user's and the movie's vectors (-1 for a missing
+                                          vector or unequal dimensions) */
+#define SRS_RECFORYOU_NEURALCF 2       /* "nerualcf" (sic): the served NeuralCF or two-tower model's output on
+                                          (userId, movieId), widened to double */
+#define SRS_RECFORYOU_OK 0
+#define SRS_RECFORYOU_UNKNOWN_USER 1   /* not in the user table: an empty list, as the Java returns */
+#define SRS_RECFORYOU_MODEL_RANGE 2    /* NEURALCF and the user, or a candidate, is outside the model's vocabulary
+                                          (TF-Serving rejects the request and the Java throws): an empty list */
+/* getRecList(user_ids[q], size, ranker) for q < n_users: the candidates are getMovies(800, "rating") of `catalog`
+ * (a catalogue whose HashMap order is unknown - see srs_similar_catalog_create_ex_host - is rejected), scored by
+ * `ranker`, ordered by score descending (Double.compare; NaN first) and ties by movie id ascending, cut to
+ * size >= 1.  `model` is read only by NEURALCF, which needs an SRS_NEURALCF or SRS_TWOTOWERS model; the catalogue, the
+ * user table and the model must be on one device.  Host outputs as srs_similar_movies_host's: out_ids
+ * [n_users][size] int32, out_scores [n_users][size] double, out_count [n_users] (entries past it are 0), out_status
+ * [n_users] (SRS_RECFORYOU_*).  Synchronous; the same inputs give the same bits. */
+int srs_recforyou_host(const srs_similar_catalog* catalog, const srs_recforyou_users* users, const srs_model* model,
+                       int32_t ranker, const int32_t* user_ids, int32_t n_users, int32_t size, int32_t* out_ids,
+                       double* out_scores, int32_t* out_count, int32_t* out_status);
+
 #ifdef __cplusplus
 }
 #endif

@@ -58,7 +58,8 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_binary_metrics_summary", "srs_binary_metrics_curve", "srs_binary_metrics_confusion",
            "srs_similar_catalog_create_host", "srs_similar_movies_host", "srs_similar_catalog_destroy",
            "srs_similar_catalog_create_ex_host", "srs_similar_movies_candidates_host",
-           "srs_similar_embedding_recall_host")
+           "srs_similar_embedding_recall_host", "srs_recforyou_users_create_host", "srs_recforyou_users_destroy",
+           "srs_recforyou_host")
 
 _lib = None
 
@@ -121,6 +122,8 @@ SRS_BM_ROC, SRS_BM_PR, SRS_BM_THRESHOLDS, SRS_BM_PRECISION, SRS_BM_RECALL, SRS_B
 SRS_SIMILAR_DEFAULT, SRS_SIMILAR_EMB = 0, 1
 SRS_SIMILAR_OK, SRS_SIMILAR_UNKNOWN_MOVIE, SRS_SIMILAR_NO_EMBEDDING = 0, 1, 2
 SRS_SIMILAR_CANDIDATES_GENRE, SRS_SIMILAR_CANDIDATES_MULTIPLE = 0, 1
+SRS_RECFORYOU_DEFAULT, SRS_RECFORYOU_EMB, SRS_RECFORYOU_NEURALCF = 0, 1, 2
+SRS_RECFORYOU_OK, SRS_RECFORYOU_UNKNOWN_USER, SRS_RECFORYOU_MODEL_RANGE = 0, 1, 2
 
 
 class SrsError(RuntimeError):
@@ -345,6 +348,12 @@ def load():
     lib.srs_similar_movies_candidates_host.argtypes = [V, I32, V, I32, I32, I32, V, V, V, V]
     lib.srs_similar_embedding_recall_host.restype = C.c_int
     lib.srs_similar_embedding_recall_host.argtypes = [V, V, I32, I32, V, V, V, V]
+    lib.srs_recforyou_users_create_host.restype = C.c_int
+    lib.srs_recforyou_users_create_host.argtypes = [V, I64, V, V, I32, I32, I32, C.POINTER(V)]
+    lib.srs_recforyou_users_destroy.restype = None
+    lib.srs_recforyou_users_destroy.argtypes = [V]
+    lib.srs_recforyou_host.restype = C.c_int
+    lib.srs_recforyou_host.argtypes = [V, V, V, I32, V, I32, I32, V, V, V, V]
     for name, args in (
             ("srs_approx_quantile_host", [V, I64, V, I32, F64, I32, V]),
             ("srs_quantile_discretizer_host", [V, I64, I32, F64, I32, V, C.POINTER(I32), V]),

@@ -1,6 +1,7 @@
 // cosine.cuh - Embedding.calculateSimilarity (online/model/Embedding.java:33-47) for one warp: float products
 // accumulated in double, dot / (sqrt(n1) * sqrt(n2)).  util.cu's cosine_kernel (one query against n candidates)
-// and similar.cu's emb ranker (each query against its genre candidates) share it.
+// and similar.cu's emb ranker (each query against its genre candidates) share it; recforyou.cu's emb ranker takes
+// the same sums one at a time (warp_product_sum).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -24,6 +25,18 @@ __device__ __forceinline__ void cosine_sums(const float* __restrict__ q, const f
     n1 += __shfl_xor_sync(0xffffffffu, n1, o);
     n2 += __shfl_xor_sync(0xffffffffu, n2, o);
   }
+}
+
+// One of cosine_sums' three sums alone, sum of (double)(a[k] * b[k]): the same lane split and xor tree, so the same
+// bits as the matching total of cosine_sums (a == b gives a squared norm).  recforyou.cu forms the norms once per
+// call and only the dot per pair.  All 32 lanes must call it.
+__device__ __forceinline__ double warp_product_sum(const float* __restrict__ a, const float* __restrict__ b, int dim,
+                                                   int lane) {
+  double s = 0.0;
+  for (int k = lane; k < dim; k += 32) s += (double)__fmul_rn(__ldg(a + k), __ldg(b + k));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  return s;
 }
 
 __device__ __forceinline__ double cosine_value(double dot, double n1, double n2) {

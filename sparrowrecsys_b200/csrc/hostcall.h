@@ -158,4 +158,21 @@ int word2vec_fit(HostCall& c, const int32_t* d_words, const uint32_t* d_keys, co
                  const srs_item2vec_params& hp, const char* what, int32_t capacity, int32_t* vocab_ids,
                  float* vectors, int32_t* vocab_size);
 
+// ---- similar.cu and model.cu: what recforyou.cu reads of a catalogue and of a model (no copies) --------------------
+struct SimilarCatalogView {
+  int32_t device, n_movies, dim;
+  bool hash_order;                     // getMovies' order is known (no HashMap bin treeified)
+  const int32_t* movie_id;             // [n_movies] by load-order slot
+  const float* emb;                    // [n_emb][dim] movie vectors
+  const int32_t* emb_row;              // [n_movies] the movie's row of emb, -1 for none
+  int32_t n_rec;                       // entries of rec
+  const int32_t* rec;                  // getMovies(800, "rating"): slots, in that order
+};
+SimilarCatalogView similar_catalog_view(const srs_similar_catalog* h);
+struct ModelView {
+  int32_t kind, device;                // srs_spec.kind and the model's device
+  const NcfParams* ncf;                // the placed NeuralCF / two-tower weights (other kinds: unset)
+};
+ModelView model_view(const srs_model* m);
+
 }  // namespace srs

@@ -185,6 +185,8 @@ struct srs_model {
   std::mutex mu;
 };
 
+srs::ModelView srs::model_view(const srs_model* m) { return {m->spec.kind, m->device, &m->ncf}; }
+
 // srs_metrics_*: one allocation on the device
 struct srs_metrics {
   int device = 0;

@@ -14,7 +14,8 @@
 //             lists (and whose first kMultiGenreTop entries) hold it;
 //   getMovies DataManager.movieMap's HashMap iteration order (the table length simulated on the host, a stable
 //             radix sort of the slots by bucket), then stable radix sorts of that order by desc_key(average) and
-//             by release year descending: the top kGlobalTop of each and the first kPool by rating, in id order.
+//             by release year descending: the top kGlobalTop of each, the first kPool by rating, in id order, and
+//             the first kRecForYou by rating in that order (recforyou.cu's candidates).
 // Query (srs_similar_movies_candidates_host): sim_query_kernel, one block per query movie -
 //   candidates the entries of the query's genre lists (GENRE), or their first kMultiGenreTop entries and the two
 //             global top lists (MULTIPLE); an entry is kept unless it is the query or an earlier list of the
@@ -63,11 +64,13 @@ struct srs_similar_catalog {
   int32_t* rtop = nullptr;               // [n_top] getMovies(100, "rating"), slots
   int32_t* ytop = nullptr;               // [n_top] getMovies(100, "releaseYear"), slots
   int32_t* pool = nullptr;               // [n_pool] getMovies(10000, "rating"), slots in ascending movie id
+  int32_t n_rec = 0;                     // entries of rec
+  int32_t* rec = nullptr;                // [n_rec] getMovies(800, "rating"), slots in that order (RecForYouProcess)
   ~srs_similar_catalog() {
     cudaSetDevice(device);
     for (void* p : {(void*)ids_sorted, (void*)slot_sorted, (void*)movie_id, (void*)mask, (void*)listed, (void*)avg,
                     (void*)glist, (void*)gcnt, (void*)emb, (void*)emb_row, (void*)listed_multi, (void*)in_rtop,
-                    (void*)rtop, (void*)ytop, (void*)pool})
+                    (void*)rtop, (void*)ytop, (void*)pool, (void*)rec})
       cudaFree(p);
   }
 };
@@ -80,6 +83,7 @@ constexpr int kMaxGenres = 64;           // one bit each in a uint64 mask
 constexpr int kMultiGenreTop = 20;       // getMoviesByGenre(genre, 20, "rating"): SimilarMovieProcess.java:65
 constexpr int kGlobalTop = 100;          // getMovies(100, "rating" / "releaseYear"): :71, :76
 constexpr int kPool = 10000;             // getMovies(10000, "rating"): :96
+constexpr int kRecForYou = 800;          // getMovies(800, "rating"): RecForYouProcess.java:34-35
 constexpr int kThreads = 256;
 constexpr int kQueryThreads = 256;
 constexpr int kSegRating = -1, kSegYear = -2;   // sim_query_kernel's segments of the two global lists
@@ -595,6 +599,7 @@ int create(const int32_t* movie_id, int32_t n_movies, const int32_t* genre_off, 
   std::vector<int32_t> pool;
   if (nm && h->hash_order) {
     h->n_pool = std::min(nm, kPool);
+    h->n_rec = std::min(nm, kRecForYou);
     h->n_top = h->has_year ? std::min(nm, kGlobalTop) : 0;
     uint32_t *d_bucket, *d_bucket_sorted, *d_ykey = nullptr, *d_ykey_sorted = nullptr;
     int32_t *d_slot, *d_hm, *d_rorder, *d_year = nullptr, *d_yorder = nullptr;
@@ -621,6 +626,8 @@ int create(const int32_t* movie_id, int32_t n_movies, const int32_t* genre_off, 
     LAUNCHED();
     CUB_RUN(c, cub::DeviceRadixSort::SortPairs(tmp__, tb__, d_rkey, d_rkey_sorted, d_hm, d_rorder, nm, 0, 64, c.s));
     PROPAGATE(persist(&h->pool, h->n_pool));
+    PROPAGATE(persist(&h->rec, h->n_rec));
+    CUDA_TRY(cudaMemcpyAsync(h->rec, d_rorder, sizeof(int32_t) * h->n_rec, cudaMemcpyDeviceToDevice, c.s));
     pool.resize(h->n_pool);
     CUDA_TRY(cudaMemcpyAsync(pool.data(), d_rorder, sizeof(int32_t) * h->n_pool, cudaMemcpyDeviceToHost, c.s));
     if (h->has_year) {
@@ -777,6 +784,11 @@ int recall(const srs_similar_catalog* h, const int32_t* movie_ids, int32_t n_que
 }
 
 }  // namespace
+
+SimilarCatalogView similar_catalog_view(const srs_similar_catalog* h) {
+  return {h->device, h->n_movies, h->dim, h->hash_order, h->movie_id, h->emb, h->emb_row, h->n_rec, h->rec};
+}
+
 }  // namespace srs
 
 extern "C" int srs_similar_catalog_create_host(const int32_t* movie_id, int32_t n_movies, const int32_t* genre_off,
