@@ -926,6 +926,29 @@ void srs_recforyou_users_destroy(srs_recforyou_users* users);
 int srs_recforyou_host(const srs_similar_catalog* catalog, const srs_recforyou_users* users, const srs_model* model,
                        int32_t ranker, const int32_t* user_ids, int32_t n_users, int32_t size, int32_t* out_ids,
                        double* out_scores, int32_t* out_count, int32_t* out_status);
+/* ---- Recommended for you with every served CTR model (DESIGN.md section 4.26) ------------------------------------
+ * The user side of the serving feature store, the `uf:<userId>` hashes (RecForYouProcess.java:46-52), attached to a
+ * user table: row i is user_id[i]'s srs_user_row fields - user_genre [n][5] vocabulary indices (-1 missing; an index
+ * >= 19 is SRS_ERR_RANGE), user_numerics [n][3] (userAvgRating, userRatingCount, userRatingStddev) and hist [n][5],
+ * userRatedMovie1..5 in key order (the library places them at each model's history positions).  Rows of ids outside
+ * the table are ignored and a later row of an id replaces the earlier one; a table user without a row takes an empty
+ * hash's values (genres -1, numerics 0, history ids 0).  A second call replaces the whole uf: side.  Every argument
+ * is checked before any device call (SRS_ERR_INVALID).  Synchronous. */
+int srs_recforyou_users_set_features_host(srs_recforyou_users* users, int32_t n, const int32_t* user_id,
+                                          const int32_t* user_genre, const float* user_numerics,
+                                          const int32_t* hist);
+/* srs_recforyou_host's NEURALCF ranker with a model of any kind.  NeuralCF and two-tower models give
+ * srs_recforyou_host's results.  Every other kind scores user u's candidate c as srs_rank_user_host does with u's uf:
+ * row and the model's movie table (srs_model_set_movie_features), so it needs both (SRS_ERR_INVALID before any
+ * launch).  A user is SRS_RECFORYOU_MODEL_RANGE, with an empty list, when predict would reject one of its rows for
+ * range: its userId, a history id the model reads or (for every known user) a candidate outside the model, or a
+ * candidate past the movie table; such rows never reach the forward.  The rows of the other users go through the
+ * model's own forward kernel in chunks of a fixed byte budget, with the model's lock held.  Outputs as
+ * srs_recforyou_host's; the model, the user table and the catalogue must be on one device.  Synchronous; the same
+ * inputs give the same bits, wherever the chunks end. */
+int srs_recforyou_ctr_host(const srs_similar_catalog* catalog, const srs_recforyou_users* users, srs_model* model,
+                           const int32_t* user_ids, int32_t n_users, int32_t size, int32_t* out_ids,
+                           double* out_scores, int32_t* out_count, int32_t* out_status);
 
 #ifdef __cplusplus
 }

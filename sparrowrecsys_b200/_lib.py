@@ -59,7 +59,7 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_similar_catalog_create_host", "srs_similar_movies_host", "srs_similar_catalog_destroy",
            "srs_similar_catalog_create_ex_host", "srs_similar_movies_candidates_host",
            "srs_similar_embedding_recall_host", "srs_recforyou_users_create_host", "srs_recforyou_users_destroy",
-           "srs_recforyou_host")
+           "srs_recforyou_host", "srs_recforyou_users_set_features_host", "srs_recforyou_ctr_host")
 
 _lib = None
 
@@ -354,6 +354,10 @@ def load():
     lib.srs_recforyou_users_destroy.argtypes = [V]
     lib.srs_recforyou_host.restype = C.c_int
     lib.srs_recforyou_host.argtypes = [V, V, V, I32, V, I32, I32, V, V, V, V]
+    lib.srs_recforyou_users_set_features_host.restype = C.c_int
+    lib.srs_recforyou_users_set_features_host.argtypes = [V, I32, V, V, V, V]
+    lib.srs_recforyou_ctr_host.restype = C.c_int
+    lib.srs_recforyou_ctr_host.argtypes = [V, V, V, V, I32, I32, V, V, V, V]
     for name, args in (
             ("srs_approx_quantile_host", [V, I64, V, I32, F64, I32, V]),
             ("srs_quantile_discretizer_host", [V, I64, I32, F64, I32, V, C.POINTER(I32), V]),

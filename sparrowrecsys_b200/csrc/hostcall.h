@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <mutex>
 #include <vector>
 
 #include "../../include/srs_ctr.h"
@@ -172,7 +173,18 @@ SimilarCatalogView similar_catalog_view(const srs_similar_catalog* h);
 struct ModelView {
   int32_t kind, device;                // srs_spec.kind and the model's device
   const NcfParams* ncf;                // the placed NeuralCF / two-tower weights (other kinds: unset)
+  int32_t hist_cols;                   // history columns the forward reads: T (DIN, DIEN), 1 (W&D) or 0
+  int32_t n_users, n_movies;           // the model's id vocabularies
+  const void* movie_feats;             // srs_model_set_movie_features' table, [movie_feats_rows][8 words]; or null
+  int32_t movie_feats_rows;
 };
 ModelView model_view(const srs_model* m);
+// The model's own forward, as its predict calls run it: the kernel the model chose at creation, on `s`.  The caller
+// holds model_mutex(m) from before it reads the movie table until its last launch has finished.
+std::mutex& model_mutex(srs_model* m);
+size_t model_batch_bytes(const srs_model* m, size_t B);   // the packed batch of B rows (model.cu's slot layout)
+// the view of a packed batch of B rows at `block`, its scores to `probs` and its range errors to `err_flag`
+BatchView model_batch_view(const srs_model* m, uint8_t* block, size_t B, float* probs, int* err_flag);
+int model_launch(srs_model* m, const BatchView& v, cudaStream_t s);
 
 }  // namespace srs

@@ -461,10 +461,11 @@ cudaError_t launch_wgmma_selftest(const float* A, const float* B, float* D, int 
 cudaError_t launch_cosine(const float* q, const float* c, int n, int dim, float* out,
                           cudaStream_t s);
 cudaError_t launch_widen_u16(const uint16_t* src, int32_t* dst, int64_t n, cudaStream_t s);
-cudaError_t launch_assemble_request(const int32_t* req, const void* movie_feats, int n_table, int n, int hc,
-                                    int dense, int32_t* movie_id, int32_t* user_id, int32_t* hist,
-                                    int32_t* movie_genre, int32_t* user_genre, float* numerics, int* err_flag,
-                                    cudaStream_t s);
+// n_req user records of 9 + hc words x n_cand candidate ids -> n_req * n_cand packed rows, user-major (util.cu)
+cudaError_t launch_assemble_request(const int32_t* req, int n_req, const int32_t* cand, int n_cand,
+                                    const void* movie_feats, int n_table, int hc, int dense, int32_t* movie_id,
+                                    int32_t* user_id, int32_t* hist, int32_t* movie_genre, int32_t* user_genre,
+                                    float* numerics, int* err_flag, cudaStream_t s);
 // topk.cu: ranking = descending score, ties by position; min(k, n) results
 size_t topk_scratch_bytes(int n);
 cudaError_t launch_topk(const float* scores, int n, int k, int32_t* top_idx, float* top_scores,

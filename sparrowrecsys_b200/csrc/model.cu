@@ -185,7 +185,11 @@ struct srs_model {
   std::mutex mu;
 };
 
-srs::ModelView srs::model_view(const srs_model* m) { return {m->spec.kind, m->device, &m->ncf}; }
+srs::ModelView srs::model_view(const srs_model* m) {
+  return {m->spec.kind, m->device, &m->ncf, m->hist_cols, m->spec.n_users, m->spec.n_movies, m->movie_feats,
+          m->movie_feats_rows};
+}
+std::mutex& srs::model_mutex(srs_model* m) { return m->mu; }
 
 // srs_metrics_*: one allocation on the device
 struct srs_metrics {
@@ -966,6 +970,25 @@ int dien_stage_and_launch(srs_model* m, Slot& s, const srs_batch* b, const int32
 
 }  // namespace
 
+// ---- what recforyou.cu's CTR page runs of a model (hostcall.h) ------------------------
+size_t srs::model_batch_bytes(const srs_model* m, size_t B) { return packed_layout(m, B).total; }
+
+BatchView srs::model_batch_view(const srs_model* m, uint8_t* block, size_t B, float* probs, int* err_flag) {
+  const PackedLayout L = packed_layout(m, B);
+  BatchView v{};
+  v.B = (int)B; v.hist_stride = m->hist_cols;
+  v.movie_id = reinterpret_cast<const int32_t*>(block + L.movie);
+  v.user_id = reinterpret_cast<const int32_t*>(block + L.user);
+  v.hist = reinterpret_cast<const int32_t*>(block + L.hist);
+  v.movie_genre = reinterpret_cast<const int32_t*>(block + L.mg);
+  v.user_genre = reinterpret_cast<const int32_t*>(block + L.ug);
+  v.numerics = reinterpret_cast<const float*>(block + L.num);
+  v.probs = probs; v.logits = nullptr; v.err_flag = err_flag;
+  return v;
+}
+
+int srs::model_launch(srs_model* m, const BatchView& v, cudaStream_t s) { return launch(m, v, s); }
+
 // ======================================================================================
 extern "C" {
 
@@ -1337,9 +1360,10 @@ int srs_rank_user_host(srs_model* m, const srs_user_row* user, const int32_t* ca
   CUDA_TRY(cudaMemcpyAsync(s.d_req.p, h, (9 + (size_t)hc + (size_t)n) * 4, cudaMemcpyHostToDevice, s.stream));
   const PackedLayout L = packed_layout(m, (size_t)n);
   uint8_t* d = s.d_block.p;
-  CUDA_TRY(launch_assemble_request(s.d_req.p, m->movie_feats, m->movie_feats_rows, n, hc, dense_feats ? 1 : 0,
-                                   reinterpret_cast<int32_t*>(d + L.movie), reinterpret_cast<int32_t*>(d + L.user),
-                                   reinterpret_cast<int32_t*>(d + L.hist), reinterpret_cast<int32_t*>(d + L.mg),
+  CUDA_TRY(launch_assemble_request(s.d_req.p, 1, s.d_req.p + 9 + hc, n, m->movie_feats, m->movie_feats_rows, hc,
+                                   dense_feats ? 1 : 0, reinterpret_cast<int32_t*>(d + L.movie),
+                                   reinterpret_cast<int32_t*>(d + L.user), reinterpret_cast<int32_t*>(d + L.hist),
+                                   reinterpret_cast<int32_t*>(d + L.mg),
                                    reinterpret_cast<int32_t*>(d + L.ug), reinterpret_cast<float*>(d + L.num),
                                    slot_err(m, s), s.stream));
   rc = launch(m, staged_view(m, s, (size_t)n, L), s.stream);

@@ -133,6 +133,7 @@ class CTRModel:
         self._keep = [w for w in self._keep if not isinstance(w, np.ndarray)]  # host copies done
         self.hist_cols = spec.hist_len if spec.model in ("din", "dien") \
             else (1 if spec.model == "widendeep" else 0)
+        self.movie_table_rows = 0         # set_movie_table: the rows of the movie table in HBM
 
     # ---- constructors ------------------------------------------------------------
     @classmethod
@@ -351,6 +352,7 @@ class CTRModel:
             table.float_cols["movieRatingStddev"], table.int_cols["releaseYear"].astype(np.float32)], axis=1),
             np.float32)
         _lib.check(self._lib.srs_model_set_movie_features(self._h, n, genres.ctypes.data, nums.ctypes.data))
+        self.movie_table_rows = n
 
     def rank_user(self, user_id: int, user_fields: Mapping[str, object], candidate_ids, size: int,
                   return_scores: bool = False):

@@ -6,7 +6,10 @@ model)` (online/recprocess/RecForYouProcess.java:29-105), for many users per cal
 `similar.SimilarMovies` catalogue, whose getMovies(800, "rating") are the candidates; `recommend(user_ids, size,
 model, ctr_model)` answers every user in one device call (`srs_recforyou_host`) with the "emb" ranker, the
 "nerualcf" ranker (a NeuralCF or two-tower `CTRModel`) or the default one.  DESIGN.md section 4.25 gives the
-semantics; oracle/recforyou.py restates the Java.
+semantics; oracle/recforyou.py restates the Java.  With the users' `uf:` hashes attached (`set_user_features`,
+`srs_recforyou_users_set_features_host`) the "nerualcf" ranker takes every other CTR model too - DIN, DIEN, DeepFM,
+DeepFM_v2, EmbeddingMLP, Wide&Deep - with its movie table (`CTRModel.set_movie_table`), through
+`srs_recforyou_ctr_host` (DESIGN.md section 4.26).
 
     python -m sparrowrecsys_b200.recforyou movies.csv ratings.csv [--emb item2vecEmb.csv] [--user-emb userEmb.csv]
         [--model emb|nerualcf|default] [--savedmodel DIR [--savedmodel-kind neuralcf|twotowers]] --size N
@@ -57,6 +60,31 @@ class RecForYou:
         _lib.check(lib.srs_recforyou_users_create_host(p(users), users.shape[0], p(eid), p(emb), n_emb, dim,
                                                        self.device, C.byref(h)))
         self._h = h
+        self.users = np.unique(users)
+        self.has_user_features = False
+
+    def set_user_features(self, store) -> None:
+        """Attach the `uf:<userId>` hashes of `store` (a `featurestore.FeatureStore`) for every user of the table,
+        typed by `parse_user_features` as `CTRModel.rank_user` types them; a user without a hash takes an empty
+        hash's values.  Replaces what an earlier call attached."""
+        from .features import genre_to_index
+        from .featurestore import parse_user_features
+        ids, genres, nums, hist = [], [], [], []
+        for u in self.users.tolist():
+            fields = store.user_features(u)
+            if not fields:
+                continue
+            t = parse_user_features(fields)
+            ids.append(u)
+            genres.append([int(genre_to_index([t["userGenre%d" % (g + 1)]])[0]) for g in range(5)])
+            nums.append([t["userAvgRating"], np.float32(t["userRatingCount"]), t["userRatingStddev"]])
+            hist.append([t["userRatedMovie%d" % (k + 1)] for k in range(5)])
+        n = len(ids)
+        a = [np.ascontiguousarray(np.array(x, dt).reshape(shape)) for x, dt, shape in
+             ((ids, np.int32, (n,)), (genres, np.int32, (n, 5)), (nums, np.float32, (n, 3)),
+              (hist, np.int32, (n, 5)))]
+        _lib.check(_lib.load().srs_recforyou_users_set_features_host(self._h, n, *[x.ctypes.data for x in a]))
+        self.has_user_features = True
 
     def close(self) -> None:
         if getattr(self, "_h", None):
@@ -75,15 +103,26 @@ class RecForYou:
     def recommend_arrays(self, user_ids, size: int, model: str = "emb", ctr_model=None):
         """One device call for every user: (ids int32 [U, size], scores float64 [U, size], count int32 [U], status
         int32 [U]); row u's first count[u] entries are its list, the rest 0.  `model` is the Java's string: "emb" the
-        cosine ranker, "nerualcf" (sic) the served `ctr_model` (a NeuralCF or two-tower `CTRModel`), anything else
-        - "neuralcf" included - the default ranker."""
+        cosine ranker, "nerualcf" (sic) the served `ctr_model`, anything else - "neuralcf" included - the default
+        ranker.  A NeuralCF or two-tower `ctr_model` reads (userId, movieId) only; any other kind reads the users'
+        features (`set_user_features`) and its movie table (`CTRModel.set_movie_table`), and is ranked through
+        `srs_recforyou_ctr_host`."""
         if self._h is None or self.catalogue._h is None:
             raise ValueError("the user table or its catalogue is closed")
+        ctr = False
         if model == "emb":
             ranker, handle = _lib.SRS_RECFORYOU_EMB, None
         elif model == "nerualcf":
-            if ctr_model is None or ctr_model.spec.model not in ("neuralcf", "twotowers"):
-                raise ValueError("the nerualcf ranker needs a NeuralCF or two-tower CTRModel")
+            if ctr_model is None:
+                raise ValueError("the nerualcf ranker needs a CTRModel")
+            if ctr_model.spec.model not in ("neuralcf", "twotowers"):
+                if not self.has_user_features:
+                    raise ValueError("a %s model reads the users' uf: features: call set_user_features first"
+                                     % ctr_model.spec.model)
+                if not getattr(ctr_model, "movie_table_rows", 0):
+                    raise ValueError("a %s model reads movie features: call CTRModel.set_movie_table first"
+                                     % ctr_model.spec.model)
+                ctr = True
             ranker, handle = _lib.SRS_RECFORYOU_NEURALCF, ctr_model._h
         else:
             ranker, handle = _lib.SRS_RECFORYOU_DEFAULT, None
@@ -95,8 +134,12 @@ class RecForYou:
         out = (np.zeros((U, size), np.int32), np.zeros((U, size), np.float64), np.zeros(U, np.int32),
                np.zeros(U, np.int32))
         p = lambda a: a.ctypes.data
-        _lib.check(_lib.load().srs_recforyou_host(self.catalogue._h, self._h, handle, ranker, p(q), U, size,
-                                                  *map(p, out)))
+        if ctr:
+            _lib.check(_lib.load().srs_recforyou_ctr_host(self.catalogue._h, self._h, handle, p(q), U, size,
+                                                          *map(p, out)))
+        else:
+            _lib.check(_lib.load().srs_recforyou_host(self.catalogue._h, self._h, handle, ranker, p(q), U, size,
+                                                      *map(p, out)))
         return out
 
     def recommend(self, user_ids, size: int, model: str = "emb", ctr_model=None) -> List[SimilarList]:
