@@ -61,10 +61,12 @@ def ctr_score_fn(spec, W, dtype=np.float32):
 
 class RecForYou:
     """The page over `catalogue` (an oracle/similar_recall.RecallCatalogue), the ratings' userId column in file order
-    and the userEmb.csv rows (ids, vectors) in file order (or None); a vector list may be any length."""
+    and the userEmb.csv rows (ids, vectors) in file order (or None); a vector list may be any length.  `cosine(q, C)`
+    scores the emb ranker: `similar_movies.java_cosine_many` (the Java's order) or `warp_cosine_many` (the device's)."""
 
-    def __init__(self, catalogue, rating_user, user_emb_ids=None, user_emb=None):
+    def __init__(self, catalogue, rating_user, user_emb_ids=None, user_emb=None, cosine=S.java_cosine_many):
         self.cat = catalogue
+        self.cosine = cosine
         self.users = {int(u) for u in np.asarray(rating_user).tolist()}
         self.emb = {}
         if user_emb_ids is not None:
@@ -82,7 +84,7 @@ class RecForYou:
         if model == "emb":
             uv = self.emb.get(int(user_id))
             have = [c for c in cands if uv is not None and c in self.cat.emb and len(self.cat.emb[c]) == len(uv)]
-            s = dict(zip(have, S.java_cosine_many(uv, np.array([self.cat.emb[c] for c in have])) if have else []))
+            s = dict(zip(have, self.cosine(uv, np.array([self.cat.emb[c] for c in have])) if have else []))
             return [float(s[c]) if c in s else -1.0 for c in cands]
         if model == "nerualcf":
             if score_fn is None:

@@ -33,6 +33,19 @@ def read_history_keys(spec):
     return ["userRatedMovie1"] if spec.model == "widendeep" else []
 
 
+def history_positions(spec):
+    """The position of userRatedMovie1..5 among the model's history inputs, -1 where it does not read the key: DIN
+    and DIEN read `spec.history_keys(T)`, the keys userRatedMovie1..T in ASCII order (so from T = 10 on
+    userRatedMovie2 follows userRatedMovie1x); Wide&Deep reads userRatedMovie1; the others none."""
+    from sparrowrecsys_b200.spec import history_keys
+    if spec.model == "widendeep":
+        return [0, -1, -1, -1, -1]
+    if spec.model not in ("din", "dien"):
+        return [-1] * 5
+    keys = history_keys(spec.hist_len)
+    return [keys.index("userRatedMovie%d" % k) if k <= spec.hist_len else -1 for k in range(1, 6)]
+
+
 def feature_score_fn(spec, W, store, movie_table, dtype=np.float32):
     """score_fn of the "nerualcf" ranker (oracle/recforyou.RecForYou.rec_list) for a model over the `uf:` / `mf:`
     features of `store` (a featurestore.FeatureStore) and `movie_table` (a featurestore.MovieFeatureTable): the

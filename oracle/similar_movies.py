@@ -6,8 +6,10 @@
 * `getMoviesByGenre(genre, 100, "rating")` (DataManager.java:253-268): a stable sort of a copy of the genre's list
   by `Double.compare(m2.avg, m1.avg)`, first 100.
 * `candidateGenerator` (:39-49): the union of those lists over the movie's genres, minus the movie.
-* `calculateSimilarScore` (:145-159) in float64, or `Embedding.calculateSimilarity` (Embedding.java:33-47): float
-  products summed in double in index order; a candidate without a vector scores -1.
+* `calculateSimilarScore` (:145-159) in float64 - NaN, the Java's `(double) 0 / 0`, when neither movie has a genre -
+  or `Embedding.calculateSimilarity` (Embedding.java:33-47): float products summed in double in index order; a
+  candidate without a vector scores -1.  `cosine` (a constructor argument) sums in that order by default;
+  `warp_cosine_many` restates the device's lane order (csrc/cosine.cuh), which can differ in the last bit.
 * The ranking sorts by `Double.compare` descending; Java leaves tied scores in HashMap order, here they go by movie
   id ascending.
 Status: OK, UNKNOWN_MOVIE (empty list, as the Java), NO_EMBEDDING (the Java throws a NullPointerException on a query
@@ -61,11 +63,40 @@ def java_cosine_many(q, C):
         return dot / (np.sqrt(d1) * np.sqrt(d2))
 
 
+def _warp_sum(P):
+    """csrc/cosine.cuh's sum of each row of the float64 products P [n, dim]: lane l sums elements l, l + 32, ... in
+    order from +0.0, then an xor tree over offsets 16, 8, 4, 2, 1 (lane l adds lane l ^ o); every lane ends equal."""
+    s = np.zeros((P.shape[0], 32))
+    for k in range(0, P.shape[1], 32):
+        w = min(32, P.shape[1] - k)
+        s[:, :w] += P[:, k:k + w]
+    lanes = np.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        s = s + s[:, lanes ^ o]
+    return s[:, 0]
+
+
+def warp_cosine_many(q, C):
+    """The device's cosine of q and each row of C (csrc/cosine.cuh, one warp per pair): float products widened to
+    double, summed in lane order (`_warp_sum`), dot / (sqrt(n1) * sqrt(n2)).  The same bits as `java_cosine_many`
+    whenever the sums are exact; otherwise they may differ in the last bit."""
+    q = np.asarray(q, np.float32)
+    C = np.asarray(C, np.float32).reshape(-1, q.shape[0])
+    dot = _warp_sum((q[None, :] * C).astype(np.float64))
+    d2 = _warp_sum((C * C).astype(np.float64))
+    d1 = _warp_sum((q * q).astype(np.float64)[None, :])[0]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return dot / (np.sqrt(d1) * np.sqrt(d2))
+
+
 class Catalogue:
     """movie_ids in movies.csv order, genres[m] the list of movie m's genre strings, the ratings (movie id, score)
-    in ratings.csv order, and optionally the vector file's (ids, vectors) rows."""
+    in ratings.csv order, and optionally the vector file's (ids, vectors) rows.  `cosine(q, C)` scores the emb
+    ranker: `java_cosine_many` (the Java's order) or `warp_cosine_many` (the device's)."""
 
-    def __init__(self, movie_ids, genres, rating_movie, rating_score, emb_ids=None, emb=None):
+    def __init__(self, movie_ids, genres, rating_movie, rating_score, emb_ids=None, emb=None,
+                 cosine=java_cosine_many):
+        self.cosine = cosine
         self.ids = [int(x) for x in movie_ids]
         self.genres = [list(g) for g in genres]
         self.slot = {}
@@ -109,7 +140,8 @@ class Catalogue:
 
     def similar_score(self, m, c):
         same = sum(1 for g in self.genres[m] if g in self.genres[c])
-        genre_similarity = same / (len(self.genres[m]) + len(self.genres[c])) / 2
+        sizes = len(self.genres[m]) + len(self.genres[c])
+        genre_similarity = same / sizes / 2 if sizes else float("nan")     # Java's (double) 0 / 0
         rating_score = self.avg[c] / 5
         return genre_similarity * 0.7 + rating_score * 0.3
 
@@ -123,7 +155,7 @@ class Catalogue:
         cands = self.candidates(m)
         if model == "emb":
             have = [c for c in cands if c in self.emb]
-            s = dict(zip(have, java_cosine_many(self.emb[m], np.array([self.emb[c] for c in have]))
+            s = dict(zip(have, self.cosine(self.emb[m], np.array([self.emb[c] for c in have]))
                          if have else []))
             scores = [float(s[c]) if c in s else -1.0 for c in cands]
         else:

@@ -98,8 +98,9 @@ class RecallCatalogue(S.Catalogue):
     """oracle/similar_movies.Catalogue plus each movie's release year (`release_year`, in load order, as
     `parse_release_year` gives it; None for none) and DataManager.getMovies."""
 
-    def __init__(self, movie_ids, genres, rating_movie, rating_score, emb_ids=None, emb=None, release_year=None):
-        super().__init__(movie_ids, genres, rating_movie, rating_score, emb_ids, emb)
+    def __init__(self, movie_ids, genres, rating_movie, rating_score, emb_ids=None, emb=None, release_year=None,
+                 cosine=S.java_cosine_many):
+        super().__init__(movie_ids, genres, rating_movie, rating_score, emb_ids, emb, cosine)
         self.year = None if release_year is None else [int(y) for y in release_year]
         self._sorted = {}
 
@@ -140,7 +141,7 @@ class RecallCatalogue(S.Catalogue):
         cands = self.multiple_candidates(m)
         if model == "emb":
             have = [c for c in cands if c in self.emb]
-            s = dict(zip(have, S.java_cosine_many(self.emb[m], np.array([self.emb[c] for c in have]))
+            s = dict(zip(have, self.cosine(self.emb[m], np.array([self.emb[c] for c in have]))
                          if have else []))
             scores = [float(s[c]) if c in s else -1.0 for c in cands]
         else:
@@ -159,7 +160,7 @@ class RecallCatalogue(S.Catalogue):
             return [], [], S.NO_EMBEDDING
         pool = self.get_movies(POOL, "rating")
         have = [c for c in pool if c in self.emb]
-        s = dict(zip(have, S.java_cosine_many(self.emb[m], np.array([self.emb[c] for c in have]))
+        s = dict(zip(have, self.cosine(self.emb[m], np.array([self.emb[c] for c in have]))
                      if have else []))
         items = sorted(((float(s[c]) if c in s else -1.0, self.ids[c]) for c in pool),
                        key=functools.cmp_to_key(lambda x, y: java_double_compare(x[0], y[0]) or

@@ -2,7 +2,8 @@
 (oracle/recforyou.py): the 5 000 users of the golden ratings with the emb and default rankers, the "nerualcf" ranker
 with the shipped NeuralCF and two-tower models and deeper synthetic ones (every score bit for bit the model's
 `predict` of that pair), users and candidates outside the model, a synthetic catalogue past 65 536 movies with 30 000
-users, the rejections and repeat calls."""
+users, the rejections and repeat calls.  Cosines are checked bit for bit against the oracle summing in the device's
+lane order (`warp_cosine_many`)."""
 import os
 
 import numpy as np
@@ -10,6 +11,7 @@ import pytest
 
 from conftest import load_golden_weights
 from oracle import recforyou as R
+from oracle import similar_movies as S
 from oracle.similar_recall import RecallCatalogue
 from sparrowrecsys_b200 import _lib
 from sparrowrecsys_b200.model import CTRModel
@@ -18,18 +20,20 @@ from sparrowrecsys_b200.recforyou import RecForYou
 from sparrowrecsys_b200.similar import SimilarMovies, genre_lists
 from sparrowrecsys_b200.spec import default_spec
 from sparrowrecsys_b200.weights import init_weights
+from test_gpu_similar import score_bits
 
 pytestmark = pytest.mark.gpu
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-COSINE_ATOL = 1e-6                      # test_gpu_parity.py::test_cosine_scores
 PROB_ATOL = 2e-5                        # test_gpu_parity.py: the CUDA path against the float64 forward
 
 
 def _oracle(movies, ratings, emb, uemb):
     cat = RecallCatalogue(movies["movieId"], genre_lists(list(movies["genres"])), ratings["movieId"],
-                          np.asarray(ratings["rating"], np.float32), *(emb if emb is not None else (None, None)))
-    return R.RecForYou(cat, ratings["userId"], *(uemb if uemb is not None else (None, None)))
+                          np.asarray(ratings["rating"], np.float32), *(emb if emb is not None else (None, None)),
+                          cosine=S.warp_cosine_many)
+    return R.RecForYou(cat, ratings["userId"], *(uemb if uemb is not None else (None, None)),
+                       cosine=S.warp_cosine_many)
 
 
 def _check_rows(out, orc, users, size, model, score_fn=None, rows=None):
@@ -42,12 +46,8 @@ def _check_rows(out, orc, users, size, model, score_fn=None, rows=None):
         assert count[q] == len(oi), (uid, count[q], len(oi))
         assert ids[q, :count[q]].tolist() == oi, (uid, model, size)
         assert not ids[q, count[q]:].any() and not scores[q, count[q]:].any()
-        if model == "emb":
-            d = scores[q, :count[q]] - np.array(osc, np.float64)
-            nan = np.isnan(np.array(osc, np.float64))
-            assert (np.isnan(scores[q, :count[q]]) == nan).all() and np.abs(d[~nan]).max(initial=0) < COSINE_ATOL
-        elif model != "nerualcf" or score_fn is not None:
-            assert scores[q, :count[q]].tobytes() == np.array(osc, np.float64).tobytes(), uid
+        if model != "nerualcf" or score_fn is not None:
+            assert scores[q, :count[q]].tobytes() == score_bits(osc), (uid, model, size)
 
 
 @pytest.fixture(scope="module")

@@ -2,7 +2,8 @@
 `SimilarMovies.retrieve_by_embedding`, csrc/similar.cu) against the oracle (oracle/similar_recall.py): the
 reference's 982 movies with the shipped vectors, a synthetic ML-20M-sized catalogue whose HashMap order is not id
 order, with tied years and ratings, vectorless and zero-vector movies, unknown and repeated queries, a table grown
-by treeifyBin's resizes, a treeified one, repeat calls, and the genre candidates left as they were."""
+by treeifyBin's resizes, a treeified one, repeat calls, and the genre candidates left as they were.  Every score is
+checked bit for bit: cosines against the oracle summing in the device's lane order (`warp_cosine_many`)."""
 import os
 
 import numpy as np
@@ -13,27 +14,23 @@ from oracle import similar_recall as R
 from sparrowrecsys_b200 import _lib
 from sparrowrecsys_b200.ranking import load_embeddings_csv
 from sparrowrecsys_b200.similar import SimilarMovies, data_manager_release_year, genre_lists
+from test_gpu_similar import score_bits
 
 pytestmark = pytest.mark.gpu
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-COSINE_ATOL = 1e-6                      # test_gpu_parity.py::test_cosine_scores
 
 
 def _oracle(movies, ratings, emb):
     return R.RecallCatalogue(movies["movieId"], genre_lists(list(movies["genres"])), ratings["movieId"],
                              np.asarray(ratings["rating"], np.float32), *(emb if emb is not None else (None, None)),
-                             release_year=[data_manager_release_year(t) for t in movies["title"]])
+                             release_year=[data_manager_release_year(t) for t in movies["title"]],
+                             cosine=S.warp_cosine_many)
 
 
-def _same_list(got_ids, got_scores, want_ids, want_scores, cosine, what):
+def _same_list(got_ids, got_scores, want_ids, want_scores, what):
     assert got_ids.tolist() == want_ids, what
-    if cosine:
-        g, w = np.asarray(got_scores), np.array(want_scores, np.float64)
-        assert np.array_equal(np.isnan(g), np.isnan(w)), what
-        assert np.abs(g[~np.isnan(g)] - w[~np.isnan(w)]).max(initial=0) < COSINE_ATOL, what
-    else:
-        assert np.asarray(got_scores).tobytes() == np.array(want_scores, np.float64).tobytes(), what
+    assert np.ascontiguousarray(got_scores).tobytes() == score_bits(want_scores), what
 
 
 def _check_multiple(dev, orc, queries, size, model):
@@ -41,7 +38,7 @@ def _check_multiple(dev, orc, queries, size, model):
     for q, mid in enumerate(np.asarray(queries).tolist()):
         oi, osc, ost = orc.rec_list(mid, size, model, "multiple")
         assert status[q] == ost and count[q] == len(oi), (mid, status[q], ost, count[q], len(oi))
-        _same_list(ids[q, :count[q]], scores[q, :count[q]], oi, osc, model == "emb", (mid, model, size))
+        _same_list(ids[q, :count[q]], scores[q, :count[q]], oi, osc, (mid, model, size))
         assert not ids[q, count[q]:].any() and not scores[q, count[q]:].any()
     return ids, scores, count, status
 
@@ -54,7 +51,7 @@ def _check_recall(dev, orc, queries, size, cache):
         oi, osc, ost = cache[mid]
         oi, osc = oi[:size], osc[:size]
         assert status[q] == ost and count[q] == len(oi), (mid, status[q], ost, count[q], len(oi))
-        _same_list(ids[q, :count[q]], scores[q, :count[q]], oi, osc, True, (mid, size))
+        _same_list(ids[q, :count[q]], scores[q, :count[q]], oi, osc, (mid, size))
         assert not ids[q, count[q]:].any() and not scores[q, count[q]:].any()
     return ids, scores, count, status
 
