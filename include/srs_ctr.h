@@ -393,7 +393,8 @@ int srs_dien_evaluate_host_batches(srs_model* m, int32_t n_batches, const srs_ba
  *             (1 - beta_2) G^2 with G = 0 off the batch, and every row is updated - not "lazy Adam".  All:
  *             w -= alpha m / (sqrt(v) + epsilon).
  * Every sum has a fixed order: the same weights, data and order give the same bits.
- * Supported: emb_dim 1..64; NeuralCF 1..3 hidden layers of width 1..32, DeepFM exactly 2 of width 1..64, Wide&Deep
+ * Supported: emb_dim 1..64; NeuralCF 1..3 hidden layers of width 1..32 (two towers: the same per tower, with
+ * final_dense), DeepFM exactly 2 of width 1..64, Wide&Deep
  * exactly 2 of width 1..128 and cross_buckets >= 1, DeepFM_v2 exactly 2 of widths 1..32 and 1..16, proj_dim 64 and
  * n_genres >= 1; any batch size >= 1. */
 typedef struct srs_adam {
@@ -412,10 +413,12 @@ int srs_trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t 
 int srs_trainer_create_ex(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
                           const srs_adam* hp, srs_trainer** out);
 /* srs_trainer_create for every kind this library can train; the list grows with the library, so a kind it rejects
- * today (SRS_ERR_INVALID) may be accepted by a later version.  Today: SRS_NEURALCF, SRS_DEEPFM, SRS_WIDENDEEP,
- * SRS_DEEPFM_V2 and SRS_DIEN (its tensors as srs_model_create takes them; DIEN's include the auxiliary head's group
- * of eight, which its objective needs; it accepts emb_dim 1..32, hist_len 1..64, au_hidden 32 and hidden widths up
- * to (128, 64), and trains through srs_trainer_fit_dien_host).  Callers that rely on a fixed list use
+ * today (SRS_ERR_INVALID) may be accepted by a later version.  Today: SRS_NEURALCF, SRS_TWOTOWERS, SRS_DEEPFM,
+ * SRS_WIDENDEEP, SRS_DEEPFM_V2 and SRS_DIEN (its tensors as srs_model_create takes them; DIEN's include the auxiliary
+ * head's group of eight, which its objective needs; it accepts emb_dim 1..32, hist_len 1..64, au_hidden 32 and hidden
+ * widths up to (128, 64), and trains through srs_trainer_fit_dien_host).  Two towers trains with NeuralCF's shapes
+ * (1..3 hidden layers of width 1..32 per tower) and only with final_dense = 1: without the final Dense the output is
+ * the raw Dot, on which binary cross-entropy is not defined (SRS_ERR_INVALID).  Callers that rely on a fixed list use
  * srs_trainer_create or srs_trainer_create_ex, whose lists do not change. */
 int srs_trainer_create_any(const srs_spec* spec, const srs_tensor* tensors, int32_t n_tensors, int32_t device,
                            const srs_adam* hp, srs_trainer** out);

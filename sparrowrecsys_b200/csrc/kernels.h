@@ -57,6 +57,12 @@ int ncf_train_ctas(int B);
 // of launching (srs_trainer_create): the opt-in is per device.
 cudaError_t launch_ncf_train_step(const NcfStepArgs* a, const NcfParams& p, cudaStream_t s);
 
+// ---- the two-tower model's training step (twotowers_train.cu; DESIGN.md section 4.27) -----------------------
+// NeuralCF's arguments and entries: movie r at r, user r at B + r.  p: the trainer's two-tower NcfParams (with its
+// final Dense); a null `a` opts the instantiation in, as launch_ncf_train_step.
+int twotowers_train_ctas(int B);
+cudaError_t launch_twotowers_train_step(const NcfStepArgs* a, const NcfParams& p, cudaStream_t s);
+
 // What the trainer hands each tile model's step (DeepFM, Wide&Deep, DeepFM_v2): the step's rows and where its
 // outputs go
 struct StepIO {

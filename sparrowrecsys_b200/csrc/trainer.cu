@@ -1,8 +1,9 @@
 // trainer.cu - `model.fit` on the device: the C ABI's srs_trainer (include/srs_ctr.h), which trains NeuralCF
 // (neural_cf_model_1, NeuralCF.py:74-91; DESIGN.md section 4.8), DeepFM (DeepFM.py; section 4.9), Wide&Deep
-// (WideNDeep.py; section 4.18), DeepFM_v2 (DeepFM_v2.py; section 4.19) and DIEN (DIEN.py; section 4.20, its fit in
-// srs_trainer_fit_dien_host), and the kernels the models share: dedupe and the two forms of Adam.  Each model's step
-// kernel is in its own file.
+// (WideNDeep.py; section 4.18), DeepFM_v2 (DeepFM_v2.py; section 4.19), DIEN (DIEN.py; section 4.20, its fit in
+// srs_trainer_fit_dien_host) and two towers (neural_cf_model_2 with its final Dense, NeuralCF.py:57-70; section
+// 4.27), and the kernels the models share: dedupe and the two forms of Adam.  Each model's step kernel is in its own
+// file.  Two towers runs NeuralCF's column of the table below with twotowers_train_step_kernel as its step.
 //
 // A step of B rows (rows order[off .. off + B) of the uploaded dataset) is these launches in this order, with no
 // host synchronisation; T is DIEN's hist_len:
@@ -26,8 +27,8 @@
 // table_grad_kernel dedupes each list (TF's _deduplicate_indexed_slices), table_adam_kernel applies Keras's sparse
 // Adam to EVERY table row and ApplyAdam to every one-hot row, dense_adam_kernel sums the partials in CTA order, applies
 // ApplyAdam to the Dense weights and advances the device-resident iteration counter.  The tile models read the
-// epoch's rows permuted once per epoch; NeuralCF and DIEN read the dataset through the order.  No float atomics:
-// every sum has a fixed order, so a fit is bitwise reproducible.
+// epoch's rows permuted once per epoch; NeuralCF, two towers and DIEN read the dataset through the order.  No float
+// atomics: every sum has a fixed order, so a fit is bitwise reproducible.
 //
 // Validation (srs_trainer_fit_validate_host) and srs_trainer_evaluate_host run the serving forward over the
 // trainer's arrays (ncf_kernel, deepfm_kernel, embmlp_kernel, deepfm2_kernel) and one metrics_update_kernel over all
@@ -200,6 +201,11 @@ int check_shape(const srs_spec& s) {
       if (s.hidden[0] < 1 || s.hidden[0] > 128 || s.hidden[1] < 1 || s.hidden[1] > 64)
         return failf(SRS_ERR_INVALID, "DIEN's hidden widths must be in 1..128 and 1..64");
       return SRS_OK;
+    case SRS_TWOTOWERS:
+      if (!s.final_dense)
+        return failf(SRS_ERR_INVALID, "the two-tower model trains only with its final Dense (final_dense): without it "
+                     "the output is the raw Dot, on which binary cross-entropy is not defined");
+      [[fallthrough]];
     default:
       if (s.n_hidden < 1 || s.n_hidden > 3) return failf(SRS_ERR_INVALID, "1..3 hidden layers supported");
       for (int i = 0; i < s.n_hidden; ++i)
@@ -313,14 +319,16 @@ cudaError_t eval_rows(const srs_trainer* t, const TrainRows& r, int n, float* pr
 }
 
 // The step of the trainer's model (not DIEN) over rows [off, off + B) of an epoch: the tile models read the
-// epoch's permuted rows, NeuralCF the dataset through `order` (the epoch's).  Points io.label at the step's labels.
+// epoch's permuted rows, NeuralCF and two towers the dataset through `order` (the epoch's).  Points io.label at the
+// step's labels.
 cudaError_t launch_step(const srs_trainer* t, const TrainRows& src, const TrainRows& rows, const int32_t* order,
                         int off, int B, int32_t* labels, StepIO& io, cudaStream_t s) {
-  if (t->spec.kind == SRS_NEURALCF) {
+  if (t->spec.kind == SRS_NEURALCF || t->spec.kind == SRS_TWOTOWERS) {
     const NcfStepArgs a{t->tab[0], t->blob[0], src.movie, src.user, src.label, order + off, B, t->spec.n_movies,
                         io.b.probs, io.b.logits, labels, io.trow, io.gemb, io.part};
     io.label = labels;
-    return launch_ncf_train_step(&a, t->ncf, s);
+    return t->spec.kind == SRS_TWOTOWERS ? launch_twotowers_train_step(&a, t->ncf, s)
+                                         : launch_ncf_train_step(&a, t->ncf, s);
   }
   io.b = view(rows, off, B, io.b.probs, io.b.logits, io.b.err_flag);
   io.label = rows.label + off;
@@ -468,12 +476,12 @@ int trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_te
       t->n_ent = 2 * s.hist_len + 3;
       t->ctas = dien_train_ctas;
       break;
-    default:
+    default:                                             // NeuralCF and two towers
       t->HP = *std::max_element(s.hidden, s.hidden + s.n_hidden) <= 16 ? 16 : 32;
       t->place = place_ncf(s, EP, t->HP, &t->ncf);
       t->blob_floats = t->ncf.blob_floats;
       t->n_ent = 2;
-      t->ctas = ncf_train_ctas;
+      t->ctas = s.kind == SRS_TWOTOWERS ? twotowers_train_ctas : ncf_train_ctas;
       break;
   }
   t->tab_floats = table_rows(t->place) * EP;
@@ -501,6 +509,7 @@ int trainer_create(const srs_spec* spec, const srs_tensor* tensors, int32_t n_te
       case SRS_WIDENDEEP: ce = launch_widendeep_train_step(EP, nullptr, nullptr); break;
       case SRS_DEEPFM_V2: ce = launch_deepfm2_train_step(EP, nullptr, nullptr); break;
       case SRS_DIEN: ce = launch_dien_train_step(EP, nullptr, nullptr); break;
+      case SRS_TWOTOWERS: ce = launch_twotowers_train_step(nullptr, t->ncf, nullptr); break;
       default: ce = launch_ncf_train_step(nullptr, t->ncf, nullptr); break;
     }
   }
@@ -596,9 +605,10 @@ int srs_trainer_create_any(const srs_spec* spec, const srs_tensor* tensors, int3
   if (!spec || !out) return failf(SRS_ERR_INVALID, "null argument");
   *out = nullptr;
   const int k = spec->kind;
-  if (k != SRS_NEURALCF && k != SRS_DEEPFM && k != SRS_WIDENDEEP && k != SRS_DEEPFM_V2 && k != SRS_DIEN)
-    return failf(SRS_ERR_INVALID, "fit is implemented for NeuralCF (neural_cf_model_1), DeepFM, Wide&Deep, "
-                 "DeepFM_v2 and DIEN only");
+  if (k != SRS_NEURALCF && k != SRS_TWOTOWERS && k != SRS_DEEPFM && k != SRS_WIDENDEEP && k != SRS_DEEPFM_V2 &&
+      k != SRS_DIEN)
+    return failf(SRS_ERR_INVALID, "fit is implemented for NeuralCF (neural_cf_model_1), two towers "
+                 "(neural_cf_model_2), DeepFM, Wide&Deep, DeepFM_v2 and DIEN only");
   return trainer_create(spec, tensors, n_tensors, device, hp, out);
 }
 

@@ -28,6 +28,8 @@ def evaluate(features, batch_size=None):
 
 
 def fit(features, epochs=5, batch_size=12, seed=0):
-    """Not implemented for this model: `fit` covers NeuralCF (tfrecmodel.neuralcf) and DeepFM (tfrecmodel.deepfm)
-    only."""
-    return _surface.fit(features, epochs, batch_size, seed)
+    """Not part of this surface: the `tfrecmodel.<name>.fit` calls restate each script's own `model.fit`, and
+    NeuralCF.py fits only its first model, neural_cf_model_1 (`tfrecmodel.neuralcf.fit`).  The two-tower model trains
+    on the GPU through `sparrowrecsys_b200.training.Trainer` (with its final Dense; DESIGN.md section 4.27)."""
+    raise NotImplementedError("tfrecmodel.twotowers: NeuralCF.py fits only neural_cf_model_1 (tfrecmodel.neuralcf."
+                              "fit); train the two-tower model with sparrowrecsys_b200.training.Trainer")

@@ -1,6 +1,7 @@
 """`model.fit` of NeuralCF, DeepFM, Wide&Deep, DeepFM_v2 and DIEN on the GPU (NeuralCF.py:74-91, DeepFM.py,
 WideNDeep.py:99-117, DeepFM_v2.py:158-165: compile(loss='binary_crossentropy', optimizer='adam'), then
-fit(train_dataset, epochs=5) over make_csv_dataset batches of 12).
+fit(train_dataset, epochs=5) over make_csv_dataset batches of 12), and of NeuralCF.py's second model, the two towers
+(neural_cf_model_2 with its final Dense), compiled and fitted as its first.
 
     from sparrowrecsys_b200.training import Trainer
     tr = Trainer(spec, weights, device=0)                 # initial weights in Keras shapes
@@ -13,7 +14,7 @@ DIEN (DIEN.py:296-304: compile(optimizer="adam"), fit over batches of 12 with no
 every epoch by default and reports its own history {"loss", "auc", "auc_value"} (section 4.20).
 
 The forward, backward and Keras Adam run in the CUDA library (`srs_trainer_*`, include/srs_ctr.h; DESIGN.md
-sections 4.8, 4.9, 4.18, 4.19 and 4.20).  For the other models TF's shuffle (buffer 10 000, unseeded) cannot be reproduced, so `fit` takes a seed instead: the host
+sections 4.8, 4.9, 4.18, 4.19, 4.20 and 4.27).  For the other models TF's shuffle (buffer 10 000, unseeded) cannot be reproduced, so `fit` takes a seed instead: the host
 draws one `numpy.random.default_rng(seed).permutation(n)` per epoch and the library trains in that row order.
 """
 from __future__ import annotations
@@ -37,20 +38,24 @@ def epoch_orders(n: int, epochs: int, seed: int) -> np.ndarray:
 
 
 class Trainer:
-    """Trainable NeuralCF, DeepFM, Wide&Deep, DeepFM_v2 or DIEN weights and Keras Adam's state on one GPU."""
+    """Trainable NeuralCF, two-tower, DeepFM, Wide&Deep, DeepFM_v2 or DIEN weights and Keras Adam's state on one
+    GPU."""
 
-    MODELS = ("neuralcf", "deepfm", "widendeep", "deepfm_v2", "dien")
+    MODELS = ("neuralcf", "twotowers", "deepfm", "widendeep", "deepfm_v2", "dien")
 
     def __init__(self, spec: ModelSpec, weights: Mapping[str, np.ndarray], device: int = 0,
                  adam: Optional[Mapping[str, float]] = None):
         """`weights`: the initial weights (canonical names, Keras shapes, float32 host arrays), e.g.
         `init_weights(spec, seed, for_test=False)` for an untrained model.  `adam`: Keras Adam's lr, beta_1,
         beta_2, epsilon (default: Keras's 0.001, 0.9, 0.999, 1e-7).  DIEN's weights include the auxiliary head's
-        group (`weights.init_aux_weights`): its objective needs them.  NotImplementedError for any model but
-        NeuralCF, DeepFM, Wide&Deep, DeepFM_v2 and DIEN."""
+        group (`weights.init_aux_weights`): its objective needs them.  The two towers train only with their final
+        Dense (`spec.final_dense`; without it the output is the raw Dot, which binary cross-entropy does not take:
+        ValueError).  NotImplementedError for any model but NeuralCF, two towers, DeepFM, Wide&Deep, DeepFM_v2
+        and DIEN."""
         if spec.model not in self.MODELS:
-            raise NotImplementedError("fit is implemented for NeuralCF (neural_cf_model_1), DeepFM, Wide&Deep, "
-                                      "DeepFM_v2 and DIEN only, not %r" % spec.model)
+            raise NotImplementedError("fit is implemented for NeuralCF (neural_cf_model_1), two towers "
+                                      "(neural_cf_model_2), DeepFM, Wide&Deep, DeepFM_v2 and DIEN only, not %r"
+                                      % spec.model)
         self.spec = spec
         self.device = int(device)
         self._h = None
@@ -100,7 +105,7 @@ class Trainer:
             order=None, validation_data=None, validation_split: float = 0.0,
             validation_freq: int = 1) -> Dict[str, list]:
         """`model.fit(dataset, epochs)`: train on the rows of `features` (the model's `predict` columns: `movieId`,
-        `userId` for NeuralCF, also the 7 numerics, `movieGenre1` and `userGenre1` for DeepFM and DeepFM_v2, the 7 numerics, all eight
+        `userId` for NeuralCF and two towers, also the 7 numerics, `movieGenre1` and `userGenre1` for DeepFM and DeepFM_v2, the 7 numerics, all eight
         genre columns and `userRatedMovie1` for Wide&Deep; labels default to
         `features["label"]`) in batches of `batch_size`, the last one partial.  The row order of epoch e is
         `epoch_orders(n, epochs, seed)[e]` unless `order` ([epochs][n], each a permutation) is given.  Returns
@@ -221,7 +226,7 @@ class Trainer:
         """(srs_batch over host arrays kept alive in `keep`, int32 labels, rows) of the model's columns."""
         lab = _label_array(features, labels)
         n = lab.shape[0]
-        if self.spec.model == "neuralcf":
+        if self.spec.model in ("neuralcf", "twotowers"):
             movie = _ids(features, "movieId")
             user = _ids(features, "userId")
             if movie.shape[0] != n or user.shape[0] != n:

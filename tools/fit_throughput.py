@@ -1,16 +1,18 @@
-"""Time NeuralCF's, DeepFM's, Wide&Deep's, DeepFM_v2's or DIEN's `fit` on the GPU against the numpy oracle on the
-host.
+"""Time NeuralCF's, the two towers', DeepFM's, Wide&Deep's, DeepFM_v2's or DIEN's `fit` on the GPU against the numpy
+oracle on the host.
 
-    python tools/fit_throughput.py [--model neuralcf|deepfm|widendeep|deepfm_v2|dien] [--epochs 5] [--batch-sizes 12,4096]
+    python tools/fit_throughput.py [--model neuralcf|twotowers|deepfm|widendeep|deepfm_v2|dien] [--epochs 5]
+                                   [--batch-sizes 12,4096]
                                    [--cpu-epochs 1] [--validate [--repeats 5]] [--kernels 4096]
 
 Trains the reference script's run - the untrained model of `init_weights(default_spec(model), 0, for_test=False)`
-over the 88 827 rows of `tests/golden/<model>_trainset.npz` (Wide&Deep: `deepfm_trainset.npz` with the columns of
+over the 88 827 rows of `tests/golden/<model>_trainset.npz` (two towers: `neuralcf_trainset.npz`, and the model is
+NeuralCF.py's neural_cf_model_2 with hidden_units [10, 10] and its final Dense; Wide&Deep: `deepfm_trainset.npz` with the columns of
 `widendeep_samples.npz`; DeepFM_v2: `deepfm_trainset.npz`; DIEN: `deepfm_trainset.npz` with userRatedMovie1 of
 `widendeep_samples.npz`, userRatedMovie2..5 of `dien_train_samples.npz`, the auxiliary head's initial weights and
 the negatives of DIEN.py:49, in file order) - for `--epochs` epochs at each batch size, and reports
 the wall time of `Trainer.fit` (upload, every step, the history read-back) and µs per step.  The CPU column is the
-float32 oracle (`oracle.ncf_train.fit` / `oracle.deepfm_train.fit` / `oracle.widendeep_train.fit` /
+float32 oracle (`oracle.ncf_train.fit` / `oracle.twotowers_train.fit` / `oracle.deepfm_train.fit` / `oracle.widendeep_train.fit` /
 `oracle.deepfm_v2_train.fit` / `oracle.dien_train.fit`) over `--cpu-epochs` epochs at the same batch
 size, scaled to µs per step (`--cpu-epochs 0` leaves it out).  `--validate` adds the cost of validating on the
 22 440 rows of `tests/golden/dien_testset.npz` every epoch, next to the epoch time: `validation_s_per_epoch` from
@@ -45,7 +47,7 @@ def card():
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=("neuralcf", "deepfm", "widendeep", "deepfm_v2", "dien"), default="neuralcf")
+    ap.add_argument("--model", choices=("neuralcf", "twotowers", "deepfm", "widendeep", "deepfm_v2", "dien"), default="neuralcf")
     ap.add_argument("--epochs", type=int, default=5)
     ap.add_argument("--batch-sizes", default="12,4096")
     ap.add_argument("--cpu-epochs", type=int, default=1)
@@ -58,15 +60,16 @@ def main():
     dien = args.model == "dien"
     if dien and args.validate:
         ap.error("DIEN's fit takes no validation")
-    from oracle import deepfm_train, deepfm_v2_train, dien_train, ncf_train, widendeep_train
+    from oracle import deepfm_train, deepfm_v2_train, dien_train, ncf_train, twotowers_train, widendeep_train
     from sparrowrecsys_b200.spec import default_spec
     from sparrowrecsys_b200.training import Trainer
     from sparrowrecsys_b200.weights import init_aux_weights, init_weights
     golden = os.path.join(ROOT, "tests", "golden")
     wd = args.model == "widendeep"
+    ids_only = args.model in ("neuralcf", "twotowers")          # the models that read movieId and userId only
     z = np.load(os.path.join(golden, "%s_trainset.npz" % ("deepfm" if wd or args.model in ("deepfm_v2", "dien")
-                                                          else args.model)))
-    if args.model == "neuralcf":
+                                                          else "neuralcf" if ids_only else args.model)))
+    if ids_only:
         feats = {k: z[k] for k in ("movieId", "userId", "label")}
     else:
         feats = dict(z)
@@ -79,14 +82,16 @@ def main():
         feats.update(dict(np.load(os.path.join(golden, "dien_train_samples.npz"))))
         feats.update(negative_history(feats, 5, 2020))
     n = len(feats["label"])
-    spec = default_spec(args.model)
+    spec = default_spec(args.model, hidden=(10, 10), final_dense=True) if args.model == "twotowers" \
+        else default_spec(args.model)
     W0 = init_weights(spec, 0, for_test=False)
     if dien:
         W0.update(init_aux_weights(spec, 0))
 
     def oracle_fit(orders, B):
-        if args.model == "neuralcf":
-            ncf_train.fit(W0, feats["movieId"], feats["userId"], feats["label"], orders, B, np.float32)
+        if ids_only:
+            m = ncf_train if args.model == "neuralcf" else twotowers_train
+            m.fit(W0, feats["movieId"], feats["userId"], feats["label"], orders, B, np.float32)
         elif dien:
             dien_train.fit(W0, dien_train.Rows.from_features(feats, 5), orders, B, np.float32)
         else:
@@ -99,7 +104,7 @@ def main():
     val = None
     if args.validate:
         t = np.load(os.path.join(golden, "dien_testset.npz"))
-        val = {k: t[k] for k in (("movieId", "userId", "label") if args.model == "neuralcf" else t.files)}
+        val = {k: t[k] for k in (("movieId", "userId", "label") if ids_only else t.files)}
         if wd:
             extra = np.load(os.path.join(golden, "widendeep_samples.npz"))
             val.update({k[5:]: extra[k] for k in extra.files if k.startswith("test_")})
