@@ -311,6 +311,21 @@ int srs_metrics_update_device(srs_metrics* mt, const float* probs, const float* 
  * a bad label or probability (the error stays until srs_metrics_reset) or if no row was folded. */
 int srs_metrics_result(srs_metrics* mt, srs_eval_result* out, int64_t* confusion);
 
+/* ---- Keras's sample weights (DESIGN.md section 4.28).  Row i carries a weight w_i >= 0, finite (a negative, NaN
+ * or infinite weight gives SRS_ERR_INVALID before any launch).  With weights, srs_eval_result's rows, positives and
+ * correct stay integer counts and its four doubles become Keras's weighted metrics:
+ *   loss      sum_i w_i l_i / rows (SUM_OVER_BATCH_SIZE: the row count, not the weights' sum), w_i l_i in float32;
+ *   accuracy  sum_i w_i [row i correct] / sum_i w_i, 0 when the weights sum to 0;
+ *   roc_auc, pr_auc   the same thresholds and formulas, TP/FP/TN/FN the sums of the rows' weights in double.
+ * The sums have a fixed order and use no float atomics: the same rows give the same bits on every run and every
+ * SM count.  All-ones weights give the unweighted result's bits. */
+
+/* srs_metrics_update_device with weights [n] float32 on the device.  A state folds either weighted or unweighted
+ * rows between resets (mixing gives SRS_ERR_INVALID); srs_metrics_result then reports the weighted metrics, and its
+ * `confusion` stays the integer counts.  The weights are not range-checked on the device. */
+int srs_metrics_update_weighted_device(srs_metrics* mt, const float* probs, const float* logits,
+                                       const int32_t* labels, const float* weights, int32_t n, void* stream);
+
 /* `model.evaluate(dataset)` over host batches: each batch is scored and folded into the metrics on the
  * device the way srs_predict_host_batches pipelines it (batch i on slot i % srs_num_slots()); only its
  * labels [B] int32 go in beside the features and no score comes back.  The loss sums of the batches are
@@ -321,6 +336,11 @@ int srs_metrics_result(srs_metrics* mt, srs_eval_result* out, int64_t* confusion
  * (its output is a raw dot, not a probability).  `out` is written only on success. */
 int srs_evaluate_host_batches(srs_model* m, int32_t n_batches, const srs_batch* batches,
                               const int32_t* const* labels, srs_eval_result* out);
+/* srs_evaluate_host_batches with sample weights: weights[i] [B] float32 (host) for batch i, each checked before any
+ * launch.  weights NULL: srs_evaluate_host_batches exactly.  Each batch's weighted sums are added in batch order. */
+int srs_evaluate_weighted_host_batches(srs_model* m, int32_t n_batches, const srs_batch* batches,
+                                       const int32_t* const* labels, const float* const* weights,
+                                       srs_eval_result* out);
 
 /* ---- DIEN's second output and its Keras evaluate.  The reference's DIEN is a two-output model,
  * `tf.keras.Model(inputs, outputs=[y_pred, auxiliary_loss_value])` (DIEN.py:296): `model.predict(dataset)`
@@ -458,6 +478,22 @@ int srs_trainer_fit_validate_host(srs_trainer* tr, const srs_batch* batch, const
  * the serving CUDA-core forward over the trainer's arrays and folded into the metrics on the device.  Synchronous;
  * the checks and errors of srs_trainer_fit_host's rows, before any launch. */
 int srs_trainer_evaluate_host(srs_trainer* tr, const srs_batch* batch, const int32_t* labels, srs_eval_result* out);
+
+/* srs_trainer_fit_validate_host with Keras's `fit(..., sample_weight=w)` (DESIGN.md section 4.28): weights [n] and
+ * val_weights [val_batch->B] (host float32, each NULL for none).  A step of B rows takes the loss sum_i w_i l_i / B,
+ * so dL/dz_i = (w_i (p_i - y_i)) / B; a row of weight 0 contributes no gradient but still counts in B, and every
+ * table row still takes Adam's decay.  history and val_history report the weighted metrics (as
+ * srs_metrics_update_weighted_device) when their weights are given.  Keras's class_weight is the caller's: it
+ * multiplies the training weights only.  The weights are checked with the rows, before any launch; NULL weights and
+ * val_weights give srs_trainer_fit_validate_host exactly, and all-ones weights its bits.  No extra launch per step. */
+int srs_trainer_fit_weighted_host(srs_trainer* tr, const srs_batch* batch, const int32_t* labels, const float* weights,
+                                  const int32_t* order, int32_t batch_size, int32_t epochs, srs_eval_result* history,
+                                  const srs_batch* val_batch, const int32_t* val_labels, const float* val_weights,
+                                  int32_t val_freq, srs_eval_result* val_history);
+
+/* srs_trainer_evaluate_host with weights [n] (host float32; NULL: srs_trainer_evaluate_host exactly). */
+int srs_trainer_evaluate_weighted_host(srs_trainer* tr, const srs_batch* batch, const int32_t* labels,
+                                       const float* weights, srs_eval_result* out);
 
 /* `model.fit` of DIEN (DIEN.py:296-304; DESIGN.md section 4.20): `epochs` epochs over the n = batch->B rows of
  * `batch` (host: movie_id, user_id, movie_genre and user_genre (column 0 read), numerics and hist [n][hist_stride

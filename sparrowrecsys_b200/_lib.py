@@ -47,6 +47,8 @@ EXPORTS = ("srs_abi_version", "srs_last_error", "srs_model_create", "srs_model_c
            "srs_dien_outputs_device", "srs_dien_outputs_host_batches", "srs_dien_evaluate_host_batches",
            "srs_trainer_create", "srs_trainer_create_ex", "srs_trainer_create_any", "srs_trainer_destroy", "srs_trainer_fit_host", "srs_trainer_get_weights",
            "srs_trainer_iterations", "srs_trainer_fit_validate_host", "srs_trainer_evaluate_host", "srs_trainer_fit_dien_host",
+           "srs_trainer_fit_weighted_host", "srs_trainer_evaluate_weighted_host", "srs_evaluate_weighted_host_batches",
+           "srs_metrics_update_weighted_device",
            "srs_featureeng_host", "srs_item2vec_host", "srs_user_embeddings_host", "srs_als_fit_host",
            "srs_als_fit_folds_host", "srs_als_recommend_host", "srs_item_transitions_host", "srs_random_walks_host",
            "srs_graph_embedding_host", "srs_lsh_transform_host", "srs_lsh_query_host", "srs_approx_quantile_host",
@@ -230,11 +232,18 @@ def load():
     lib.srs_metrics_update_device.restype = C.c_int
     lib.srs_metrics_update_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                               C.c_void_p]
+    lib.srs_metrics_update_weighted_device.restype = C.c_int
+    lib.srs_metrics_update_weighted_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                       C.c_int32, C.c_void_p]
     lib.srs_metrics_result.restype = C.c_int
     lib.srs_metrics_result.argtypes = [C.c_void_p, C.POINTER(SrsEvalResult), C.c_void_p]
     lib.srs_evaluate_host_batches.restype = C.c_int
     lib.srs_evaluate_host_batches.argtypes = [C.c_void_p, C.c_int32, C.POINTER(SrsBatch), C.POINTER(C.c_void_p),
                                               C.POINTER(SrsEvalResult)]
+    lib.srs_evaluate_weighted_host_batches.restype = C.c_int
+    lib.srs_evaluate_weighted_host_batches.argtypes = [C.c_void_p, C.c_int32, C.POINTER(SrsBatch),
+                                                       C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                                       C.POINTER(SrsEvalResult)]
     lib.srs_dien_outputs_device.restype = C.c_int
     lib.srs_dien_outputs_device.argtypes = [C.c_void_p, C.POINTER(SrsBatch), C.c_void_p, C.c_int32, C.c_void_p,
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -264,6 +273,13 @@ def load():
                                                   C.c_void_p, C.c_int32, C.POINTER(SrsEvalResult)]
     lib.srs_trainer_evaluate_host.restype = C.c_int
     lib.srs_trainer_evaluate_host.argtypes = [C.c_void_p, C.POINTER(SrsBatch), C.c_void_p, C.POINTER(SrsEvalResult)]
+    lib.srs_trainer_fit_weighted_host.restype = C.c_int
+    lib.srs_trainer_fit_weighted_host.argtypes = [C.c_void_p, C.POINTER(SrsBatch), C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.c_int32, C.c_int32, C.POINTER(SrsEvalResult), C.POINTER(SrsBatch),
+                                                  C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(SrsEvalResult)]
+    lib.srs_trainer_evaluate_weighted_host.restype = C.c_int
+    lib.srs_trainer_evaluate_weighted_host.argtypes = [C.c_void_p, C.POINTER(SrsBatch), C.c_void_p, C.c_void_p,
+                                                       C.POINTER(SrsEvalResult)]
     lib.srs_trainer_fit_dien_host.restype = C.c_int
     lib.srs_trainer_fit_dien_host.argtypes = [C.c_void_p, C.POINTER(SrsBatch), C.c_void_p, C.c_int32, C.c_void_p,
                                               C.c_void_p, C.c_int32, C.c_int32, C.POINTER(SrsDienEvalResult)]

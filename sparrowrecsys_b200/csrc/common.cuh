@@ -138,6 +138,17 @@ __device__ __forceinline__ float logit_bce(float x, int z) {
   return __fadd_rn(__fsub_rn(relu, xz), log1pf(expf(-fabsf(x))));
 }
 
+// A training step's dL/dz for a row of a batch of B with weight w: (w (p - y)) / B (Keras's SUM_OVER_BATCH_SIZE: the
+// denominator is B, not the weights' sum), and (p - y) / B when not `weighted`.  w = 1 gives the unweighted bits.
+__device__ __forceinline__ float row_dz(float p, int y, bool weighted, float w, int B) {
+  const float g = __fsub_rn(p, (float)y);
+  return __fdiv_rn(weighted ? __fmul_rn(w, g) : g, (float)B);
+}
+// the same with w = weight[row], weight null: unweighted
+__device__ __forceinline__ float row_dz(float p, int y, const float* weight, int row, int B) {
+  return row_dz(p, y, weight != nullptr, weight ? __ldg(weight + row) : 1.f, B);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

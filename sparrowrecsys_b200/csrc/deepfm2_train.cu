@@ -66,7 +66,7 @@ __global__ void __launch_bounds__(kThreads) deepfm2_train_step_kernel(DeepFm2Ste
     const float pr = sigmoidf_acc(z);
     b.probs[row] = pr;
     b.logits[row] = z;
-    const float dz = (pr - (float)__ldg(a.io.label + row)) / (float)b.B;
+    const float dz = row_dz(pr, __ldg(a.io.label + row), a.io.weight, row, b.B);
     dzs[r] = dz;
     dfs[r] = dz * __ldg(p.wout);
   });

@@ -50,7 +50,7 @@ __global__ void __launch_bounds__(kThreads) deepfm_train_step_kernel(DeepFmStepA
     const float pr = sigmoidf_acc(z);
     b.probs[row] = pr;
     b.logits[row] = z;
-    dzs[r] = (pr - (float)__ldg(a.io.label + row)) / (float)b.B;
+    dzs[r] = row_dz(pr, __ldg(a.io.label + row), a.io.weight, row, b.B);
   });
   __syncthreads();
   for (int i = tid; i < nv * 64; i += kThreads) {
@@ -156,6 +156,7 @@ __global__ void deepfm_permute_kernel(TrainRows src, TrainRows dst, const int32_
   dst.mgenre[(size_t)i * 3] = src.mgenre[(size_t)r * 3];
   dst.ugenre[(size_t)i * 5] = src.ugenre[(size_t)r * 5];
   dst.label[i] = src.label[r];
+  if (src.weight) dst.weight[i] = src.weight[r];
 #pragma unroll
   for (int j = 0; j < kNumNumerics; ++j) dst.numerics[(size_t)i * kNumNumerics + j] = src.numerics[(size_t)r * kNumNumerics + j];
 }

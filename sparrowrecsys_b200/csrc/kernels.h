@@ -50,6 +50,8 @@ struct NcfStepArgs {
   int32_t* trow;           // [2B] table row of each (movie, user) entry: movie r at r, user r at B + r
   float* gemb;             // [2B][EP] the entries' embedding gradients
   float* part;             // [ctas][blob_floats] per-CTA Dense gradient sums
+  const float* weight;     // the dataset's row weights [n] (DESIGN.md section 4.28); null: unweighted
+  float* weights;          // [B] the step's weights, for the metrics (written when weight is set)
 };
 int ncf_train_ctas(int B);
 // p: the trainer's NcfParams, for the instantiation <p.EP, p.HP> and the blob layout.  Each step launcher takes a
@@ -73,6 +75,7 @@ struct StepIO {
   int32_t* frow;           // [n_fent B] one-hot row of entry s * B + r, -1 = none (a missing genre)
   float* fgrad;            // [n_fent B] its gradient
   float* part;             // [ctas][blob floats] per-CTA Dense gradient sums
+  const float* weight;     // [B] the step's row weights (DESIGN.md section 4.28); null: unweighted
 };
 
 // ---- EmbeddingMLP / Wide&Deep (EmbeddingMLP.py:72-77, WideNDeep.py:101-107) --------
@@ -190,6 +193,7 @@ struct TrainRows {         // a trainer's dataset on the device, in the srs_batc
   float* numerics;         // [n][7]
   int32_t* label;          // [n]
   int32_t* rated;          // [n] userRatedMovie1 (Wide&Deep)
+  float* weight;           // [n] row weights (DESIGN.md section 4.28); null: unweighted, and not permuted
 };
 // dst row i = src row order[i], i < n (genres: column 0 only)
 cudaError_t launch_deepfm_permute(const TrainRows& src, const TrainRows& dst, const int32_t* order, int n,
@@ -510,6 +514,29 @@ struct MetricsState {                      // one history (srs_metrics, an epoch
 cudaError_t launch_metrics_update(const float* probs, const float* logits, const int32_t* labels, int n,
                                   MetricsCounters* cnt, MetricsReduce* red, double* loss_dst, int accumulate,
                                   cudaStream_t s, unsigned long long* own_hist = nullptr);
+// The weighted sums of Keras's metrics with sample weights w_i (DESIGN.md section 4.28), in double: hist is
+// MetricsCounters::hist with each row counted as w_i, correct = sum w_i [row correct], sum = sum w_i.  The loss
+// sum of a weighted update is sum w_i l_i, with w_i l_i rounded to float32 as Keras multiplies.
+struct MetricsWeighted {
+  double hist[2 * kMetBins];
+  double correct;
+  double sum;
+};
+constexpr int kMetWSums = 2 * kMetBins + 2;      // the doubles of MetricsWeighted
+static_assert(sizeof(MetricsWeighted) == kMetWSums * sizeof(double), "MetricsWeighted is an array of doubles");
+// The weighted update's per-CTA partials, summed by the last CTA in CTA order; launches sharing one must be
+// stream-ordered.  It needs no reset.
+struct MetricsWeightedReduce {
+  double partial[kMetMaxCtas][kMetWSums];
+};
+// launch_metrics_update with row weights w [n]: the integer counts and the error word as launch_metrics_update folds
+// them, the loss sum of w_i l_i into *loss_dst, and the weighted sums into *wdst (added to it when `accumulate`).
+// No float atomics: each CTA sums its rows' weights per bin in row order and the last CTA adds the CTA partials in
+// CTA order, so the result has the same bits on every run and does not depend on the SM count.  One launch.
+cudaError_t launch_metrics_update_weighted(const float* probs, const float* logits, const int32_t* labels,
+                                           const float* w, int n, MetricsCounters* cnt, MetricsReduce* red,
+                                           double* loss_dst, MetricsWeighted* wdst, MetricsWeightedReduce* wred,
+                                           int accumulate, cudaStream_t s);
 // DIEN's auc_value: `hist` holds K batch histograms [K][2 x 201] in batch order and is turned into their
 // prefix sums in place; auc[k] (K doubles) = the ROC AUC of batches 0..k in double, *sum_dst = their sum,
 // added in batch order.  Three launches on `s`.
@@ -517,6 +544,10 @@ cudaError_t launch_auc_value(unsigned long long* hist, int K, double* auc, doubl
 // host: the counts -> srs_eval_result (AUCs in double); `confusion` NULL or [4][200] tp, fp, tn, fn
 void metrics_summarise(const unsigned long long* hist, unsigned long long correct, double loss_sum,
                        srs_eval_result* out, int64_t* confusion);
+// the same with weights: rows, positives and correct from the counts, loss = loss_sum / rows (loss_sum = sum w l),
+// accuracy = div_no_nan(w.correct, w.sum) and the AUCs from the weighted bins
+void metrics_summarise_weighted(const unsigned long long* hist, unsigned long long correct, const MetricsWeighted& w,
+                                double loss_sum, srs_eval_result* out);
 
 extern int64_t g_launch_count;   // kernels launched by this library
 

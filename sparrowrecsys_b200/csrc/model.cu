@@ -2,6 +2,7 @@
 // device re-layout of the reference's weights), and the predict entry points.
 #include <cuda_runtime.h>
 
+#include <cfloat>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -146,6 +147,8 @@ struct Slot {
   PinnedBuffer<int32_t> h_req;      //   and its pinned copy
   Buffer<int32_t> d_labels;         // srs_evaluate_host_batches only (ensure_labels)
   Buffer<MetricsReduce> d_mred;     // the metrics kernel's CTA partials and ticket for this slot's stream
+  Buffer<float> d_weights;          // srs_evaluate_weighted_host_batches only (ensure_weights): the batch's weights
+  Buffer<MetricsWeightedReduce> d_wred;   //   and the weighted metrics' CTA partials for this slot's stream
   Buffer<int32_t> d_neg;            // srs_dien_*_host_batches only (ensure_dien): negative ids [B][T-1],
   Buffer<float> d_aux;              //   the auxiliary head's per-row sums [B]
   Buffer<float> d_final;            //   and final_loss [B]
@@ -180,6 +183,7 @@ struct srs_model {
   Slot slots[kSlots + 1];
   Buffer<MetricsCounters> eval_cnt;  // srs_evaluate_host_batches (ensure_eval): counts shared by the slots
   Buffer<double> eval_loss;          //   and one loss sum per batch, added in batch order on the host
+  Buffer<MetricsWeighted> eval_w;    //   and, weighted, one set of weighted sums per batch, added likewise
   Buffer<unsigned long long> eval_bhist;   // srs_dien_evaluate_host_batches (ensure_dien_eval): each batch's
   Buffer<double> eval_auc;                 //   own histogram, the prefix AUCs and (last entry) their sum
   std::mutex mu;
@@ -195,6 +199,9 @@ std::mutex& srs::model_mutex(srs_model* m) { return m->mu; }
 struct srs_metrics {
   int device = 0;
   MetricsState* d = nullptr;
+  MetricsWeighted* w = nullptr;        // the weighted sums (srs_metrics_update_weighted_device)
+  MetricsWeightedReduce* wred = nullptr;
+  int weighted = -1;                   // -1: nothing folded since the reset, 0: unweighted rows, 1: weighted rows
 };
 
 namespace {
@@ -854,10 +861,27 @@ int ensure_labels(Slot& s, int B) {
   return SRS_OK;
 }
 
-// srs_evaluate_host_batches: the model's shared counts and per-batch loss sums for n batches
-int ensure_eval(srs_model* m, int n) {
+// srs_evaluate_host_batches: the model's shared counts and per-batch loss sums (weighted: and weighted sums) for n
+// batches
+int ensure_eval(srs_model* m, int n, bool weighted) {
   CUDA_TRY(m->eval_cnt.grow(1, 1, [](int) { return sizeof(MetricsCounters); }));
   CUDA_TRY(m->eval_loss.grow(n, 64, [](int c) { return (size_t)c * sizeof(double); }));
+  if (weighted) CUDA_TRY(m->eval_w.grow(n, 64, [](int c) { return (size_t)c * sizeof(MetricsWeighted); }));
+  return SRS_OK;
+}
+
+// srs_evaluate_weighted_host_batches: the slot's weight staging and weighted-metrics scratch
+int ensure_weights(Slot& s, int B) {
+  CUDA_TRY(s.d_wred.grow(1, 1, [](int) { return sizeof(MetricsWeightedReduce); }));
+  CUDA_TRY(s.d_weights.grow(B, 1024, word_bytes));
+  return SRS_OK;
+}
+
+// Sample weights of a weighted evaluate or metrics update: finite and >= 0 (checked before any launch)
+int check_weights(const float* w, int B, int batch) {
+  for (int r = 0; r < B; ++r)
+    if (!(w[r] >= 0.f && w[r] <= FLT_MAX))
+      return fail(SRS_ERR_INVALID, "sample weight %g (batch %d, row %d) is not finite and >= 0", (double)w[r], batch, r);
   return SRS_OK;
 }
 
@@ -1382,10 +1406,15 @@ int srs_metrics_create(int32_t device, srs_metrics** out) {
   srs_metrics* mt = new srs_metrics();
   mt->device = device;
   cudaError_t e = cudaMalloc(&mt->d, sizeof(MetricsState));
+  if (e == cudaSuccess) e = cudaMalloc(&mt->w, sizeof(MetricsWeighted));
+  if (e == cudaSuccess) e = cudaMalloc(&mt->wred, sizeof(MetricsWeightedReduce));
   if (e == cudaSuccess) e = cudaMemset(mt->d, 0, sizeof(MetricsState));
+  if (e == cudaSuccess) e = cudaMemset(mt->w, 0, sizeof(MetricsWeighted));
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
     cudaFree(mt->d);
+    cudaFree(mt->w);
+    cudaFree(mt->wred);
     delete mt;
     return fail(SRS_ERR_CUDA, "metrics state allocation failed: %s", cudaGetErrorString(e));
   }
@@ -1397,6 +1426,8 @@ void srs_metrics_destroy(srs_metrics* mt) {
   if (!mt) return;
   cudaSetDevice(mt->device);
   cudaFree(mt->d);
+  cudaFree(mt->w);
+  cudaFree(mt->wred);
   delete mt;
 }
 
@@ -1404,17 +1435,32 @@ int srs_metrics_reset(srs_metrics* mt, void* stream) {
   if (!mt) return fail(SRS_ERR_INVALID, "null metrics state");
   CUDA_TRY(cudaSetDevice(mt->device));
   CUDA_TRY(cudaMemsetAsync(mt->d, 0, sizeof(MetricsState), static_cast<cudaStream_t>(stream)));
+  CUDA_TRY(cudaMemsetAsync(mt->w, 0, sizeof(MetricsWeighted), static_cast<cudaStream_t>(stream)));
+  mt->weighted = -1;
   return SRS_OK;
 }
 
 int srs_metrics_update_device(srs_metrics* mt, const float* probs, const float* logits, const int32_t* labels,
                               int32_t n, void* stream) {
+  return srs_metrics_update_weighted_device(mt, probs, logits, labels, nullptr, n, stream);
+}
+
+int srs_metrics_update_weighted_device(srs_metrics* mt, const float* probs, const float* logits,
+                                       const int32_t* labels, const float* weights, int32_t n, void* stream) {
   if (!mt) return fail(SRS_ERR_INVALID, "null metrics state");
   if (n < 1) return fail(SRS_ERR_INVALID, "n must be at least 1");
   if (!probs || !logits || !labels) return fail(SRS_ERR_INVALID, "probs, logits and labels are required");
+  const int weighted = weights != nullptr;
+  if (mt->weighted >= 0 && mt->weighted != weighted)
+    return fail(SRS_ERR_INVALID, "a metrics state folds either weighted or unweighted rows between resets");
   CUDA_TRY(cudaSetDevice(mt->device));
-  CUDA_TRY(launch_metrics_update(probs, logits, labels, n, &mt->d->cnt, &mt->d->red, &mt->d->loss, 1,
-                                 static_cast<cudaStream_t>(stream)));
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (weighted)
+    CUDA_TRY(launch_metrics_update_weighted(probs, logits, labels, weights, n, &mt->d->cnt, &mt->d->red,
+                                            &mt->d->loss, mt->w, mt->wred, 1, s));
+  else
+    CUDA_TRY(launch_metrics_update(probs, logits, labels, n, &mt->d->cnt, &mt->d->red, &mt->d->loss, 1, s));
+  mt->weighted = weighted;
   return SRS_OK;
 }
 
@@ -1430,6 +1476,11 @@ int srs_metrics_result(srs_metrics* mt, srs_eval_result* out, int64_t* confusion
   if (c.err & kMetErrProb) return fail(SRS_ERR_INVALID, "a probability is NaN or outside [0, 1]");
   srs_eval_result r{};
   metrics_summarise(c.hist, c.correct, loss, &r, confusion);
+  if (mt->weighted == 1) {                              // confusion stays the integer counts
+    MetricsWeighted w;
+    CUDA_TRY(cudaMemcpy(&w, mt->w, sizeof(w), cudaMemcpyDeviceToHost));
+    metrics_summarise_weighted(c.hist, c.correct, w, loss, &r);
+  }
   if (r.rows == 0) return fail(SRS_ERR_INVALID, "no rows have been folded into the metrics");
   *out = r;
   return SRS_OK;
@@ -1437,18 +1488,29 @@ int srs_metrics_result(srs_metrics* mt, srs_eval_result* out, int64_t* confusion
 
 int srs_evaluate_host_batches(srs_model* m, int32_t n, const srs_batch* batches, const int32_t* const* labels,
                               srs_eval_result* out) {
+  return srs_evaluate_weighted_host_batches(m, n, batches, labels, nullptr, out);
+}
+
+int srs_evaluate_weighted_host_batches(srs_model* m, int32_t n, const srs_batch* batches,
+                                       const int32_t* const* labels, const float* const* weights,
+                                       srs_eval_result* out) {
   if (!m) return fail(SRS_ERR_INVALID, "null model");
   if (n < 0 || (n > 0 && (!batches || !labels)) || !out) return fail(SRS_ERR_INVALID, "null argument");
   int rc = check_evaluable(m);
   if (rc != SRS_OK) return rc;
   rc = check_batches(m, n, batches, labels, "labels");
   if (rc != SRS_OK) return rc;
+  for (int i = 0; weights && i < n; ++i) {
+    if (batches[i].B > 0 && !weights[i]) return fail(SRS_ERR_INVALID, "weights of batch %d are null", i);
+    rc = check_weights(weights[i], batches[i].B, i);
+    if (rc != SRS_OK) return rc;
+  }
   int64_t rows = 0;
   for (int i = 0; i < n; ++i) rows += batches[i].B;
   if (rows == 0) return fail(SRS_ERR_INVALID, "evaluate needs at least one row");
   std::lock_guard<std::mutex> lock(m->mu);
   CUDA_TRY(cudaSetDevice(m->device));
-  rc = ensure_eval(m, n);
+  rc = ensure_eval(m, n, weights != nullptr);
   if (rc != SRS_OK) return rc;
   {
     Slot& s0 = m->slots[0];
@@ -1465,22 +1527,46 @@ int srs_evaluate_host_batches(srs_model* m, int32_t n, const srs_batch* batches,
     if (r != SRS_OK) return r;
     CUDA_TRY(cudaMemcpyAsync(s.d_labels.p, labels[i], (size_t)b->B * sizeof(int32_t), cudaMemcpyHostToDevice,
                              s.stream));
-    // the batch's loss sum goes to its own entry: the batch order, not the slot completion order, fixes the sum
-    CUDA_TRY(launch_metrics_update(s.d_probs.p, s.d_logits.p, s.d_labels.p, b->B, m->eval_cnt.p, s.d_mred.p,
-                                   m->eval_loss.p + i, 0, s.stream));
+    // the batch's loss sum (and weighted sums) go to its own entry: the batch order, not the slot completion order,
+    // fixes the sums
+    if (!weights) {
+      CUDA_TRY(launch_metrics_update(s.d_probs.p, s.d_logits.p, s.d_labels.p, b->B, m->eval_cnt.p, s.d_mred.p,
+                                     m->eval_loss.p + i, 0, s.stream));
+      return SRS_OK;
+    }
+    r = ensure_weights(s, b->B);
+    if (r != SRS_OK) return r;
+    CUDA_TRY(cudaMemcpyAsync(s.d_weights.p, weights[i], (size_t)b->B * sizeof(float), cudaMemcpyHostToDevice,
+                             s.stream));
+    CUDA_TRY(launch_metrics_update_weighted(s.d_probs.p, s.d_logits.p, s.d_labels.p, s.d_weights.p, b->B,
+                                            m->eval_cnt.p, s.d_mred.p, m->eval_loss.p + i, m->eval_w.p + i,
+                                            s.d_wred.p, 0, s.stream));
     return SRS_OK;
   });
   if (rc != SRS_OK) return rc;
   MetricsCounters c;
   std::vector<double> batch_loss((size_t)n);
+  std::vector<MetricsWeighted> batch_w(weights ? (size_t)n : 0);
   CUDA_TRY(cudaMemcpy(&c, m->eval_cnt.p, sizeof(c), cudaMemcpyDeviceToHost));
   CUDA_TRY(cudaMemcpy(batch_loss.data(), m->eval_loss.p, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost));
+  if (weights)
+    CUDA_TRY(cudaMemcpy(batch_w.data(), m->eval_w.p, (size_t)n * sizeof(MetricsWeighted), cudaMemcpyDeviceToHost));
   if (c.err & kMetErrLabel) return fail(SRS_ERR_INVALID, "a label is not 0 or 1");
   if (c.err & kMetErrProb) return fail(SRS_ERR_INVALID, "a probability is NaN or outside [0, 1]");
   double loss = 0.0;
-  for (int i = 0; i < n; ++i)
-    if (batches[i].B > 0) loss += batch_loss[(size_t)i];
-  metrics_summarise(c.hist, c.correct, loss, out, nullptr);
+  MetricsWeighted w{};
+  for (int i = 0; i < n; ++i) {
+    if (batches[i].B == 0) continue;
+    loss += batch_loss[(size_t)i];
+    if (!weights) continue;
+    const double* src = reinterpret_cast<const double*>(&batch_w[(size_t)i]);
+    double* dst = reinterpret_cast<double*>(&w);
+    for (int q = 0; q < kMetWSums; ++q) dst[q] += src[q];
+  }
+  if (weights)
+    metrics_summarise_weighted(c.hist, c.correct, w, loss, out);
+  else
+    metrics_summarise(c.hist, c.correct, loss, out, nullptr);
   return SRS_OK;
 }
 
@@ -1551,7 +1637,7 @@ int srs_dien_evaluate_host_batches(srs_model* m, int32_t n, const srs_batch* bat
   if (rows == 0) return fail(SRS_ERR_INVALID, "evaluate needs at least one row");
   std::lock_guard<std::mutex> lock(m->mu);
   CUDA_TRY(cudaSetDevice(m->device));
-  rc = ensure_eval(m, n);
+  rc = ensure_eval(m, n, false);
   if (rc == SRS_OK) rc = ensure_dien_eval(m, K);
   if (rc != SRS_OK) return rc;
   Slot& s0 = m->slots[0];

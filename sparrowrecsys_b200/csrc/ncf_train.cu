@@ -42,6 +42,7 @@ __global__ void __launch_bounds__(kTrainRows) ncf_train_step_kernel(NcfStepArgs 
   if (r < a.B) {
     const int row = __ldg(a.order + r);
     const int mid = __ldg(a.movie + row), uid = __ldg(a.user + row), y = __ldg(a.label + row);
+    const float w = a.weight ? __ldg(a.weight + row) : 1.f;   // the row's weight (1: unweighted)
     const float* mrow = a.tab + (size_t)mid * EP;
     const float* urow = a.tab + (size_t)(a.n_movies + uid) * EP;
     // forward: ncf_kernel's arithmetic for neural_cf_model_1
@@ -64,14 +65,15 @@ __global__ void __launch_bounds__(kTrainRows) ncf_train_step_kernel(NcfStepArgs 
     a.probs[r] = p;
     a.logits[r] = z;
     a.labels[r] = y;
+    if (a.weight) a.weights[r] = w;
 #pragma unroll
     for (int q = 0; q < EP / 4; ++q) {
       const float4 mv = ldg4(mrow + 4 * q), uv = ldg4(urow + 4 * q);
       rec[4 * q] = mv.x; rec[4 * q + 1] = mv.y; rec[4 * q + 2] = mv.z; rec[4 * q + 3] = mv.w;
       rec[EP + 4 * q] = uv.x; rec[EP + 4 * q + 1] = uv.y; rec[EP + 4 * q + 2] = uv.z; rec[EP + 4 * q + 3] = uv.w;
     }
-    // backward: dL/dz = (p - y) / B, relu' = [a > 0] = [h > 0]
-    const float dz = (p - (float)y) / (float)a.B;
+    // backward: dL/dz = (w (p - y)) / B (w = 1 unweighted), relu' = [a > 0] = [h > 0]
+    const float dz = row_dz(p, y, a.weight != nullptr, w, a.B);
     rec[RS - 1] = dz;
     float d[HP];
 #pragma unroll

@@ -30,6 +30,11 @@
 // epoch's rows permuted once per epoch; NeuralCF, two towers and DIEN read the dataset through the order.  No float
 // atomics: every sum has a fixed order, so a fit is bitwise reproducible.
 //
+// Sample weights (srs_trainer_fit_weighted_host, srs_trainer_evaluate_weighted_host; DESIGN.md section 4.28) add no
+// launch: the dataset's weight column is uploaded beside the labels, the step kernels scale dL/dz by it (NeuralCF and
+// two towers read weight[order[i]] and pass the step's weights on, the permute kernels carry it for the tile
+// models), and metrics_update_kernel's weighted instantiation replaces the unweighted one.
+//
 // Validation (srs_trainer_fit_validate_host) and srs_trainer_evaluate_host run the serving forward over the
 // trainer's arrays (ncf_kernel, deepfm_kernel, embmlp_kernel, deepfm2_kernel) and one metrics_update_kernel over all
 // the rows: two launches, with the bits of a CTRModel built from the exported weights.  The trainer's arrays hold the
@@ -37,6 +42,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cfloat>
 #include <vector>
 
 #include "../../include/srs_ctr.h"
@@ -215,10 +221,15 @@ int check_shape(const srs_spec& s) {
 }
 
 // The checks of rows the trainer reads (fit, validation, evaluate; DIEN has its own), all made before any launch.
-// `what` prefixes the messages: "" or "validation data: ".
-int check_rows(const srs_trainer* t, const srs_batch* batch, const int32_t* labels, const char* what) {
+// `what` prefixes the messages: "" or "validation data: ".  weights: null, or [n] each finite and >= 0.
+int check_rows(const srs_trainer* t, const srs_batch* batch, const int32_t* labels, const float* weights,
+               const char* what) {
   const srs_spec& sp = t->spec;
   const int n = batch->B;
+  for (int i = 0; weights && i < n; ++i)
+    if (!(weights[i] >= 0.f && weights[i] <= FLT_MAX))          // false for NaN
+      return failf(SRS_ERR_INVALID, "%ssample weight of row %d is %g: weights must be finite and >= 0", what, i,
+                   (double)weights[i]);
   if (!batch->movie_id || !batch->user_id) return failf(SRS_ERR_INVALID, "%smovie_id and user_id are required", what);
   if (t->genre_cols && (!batch->movie_genre || !batch->user_genre || !batch->numerics ||
                         (t->rated && (!batch->hist || batch->hist_stride < 1))))
@@ -254,8 +265,9 @@ int check_rows(const srs_trainer* t, const srs_batch* batch, const int32_t* labe
   return SRS_OK;
 }
 
-// n rows of the columns the trainer's model reads on the device; the others stay null
-cudaError_t alloc_rows(Scratch& sc, const srs_trainer* t, size_t n, TrainRows* r) {
+// n rows of the columns the trainer's model reads on the device, and the weights when `weighted`; the others stay
+// null
+cudaError_t alloc_rows(Scratch& sc, const srs_trainer* t, size_t n, bool weighted, TrainRows* r) {
   *r = TrainRows{};
   cudaError_t e = sc.alloc(&r->movie, n);
   if (e == cudaSuccess && t->rated) e = sc.alloc(&r->rated, n);
@@ -264,6 +276,7 @@ cudaError_t alloc_rows(Scratch& sc, const srs_trainer* t, size_t n, TrainRows* r
   if (e == cudaSuccess && t->genre_cols) e = sc.alloc(&r->ugenre, n * 5);
   if (e == cudaSuccess && t->genre_cols) e = sc.alloc(&r->numerics, n * kNumNumerics);
   if (e == cudaSuccess) e = sc.alloc(&r->label, n);
+  if (e == cudaSuccess && weighted) e = sc.alloc(&r->weight, n);
   return e;
 }
 
@@ -283,11 +296,13 @@ BatchView view(const TrainRows& r, int off, int B, float* probs, float* logits, 
   return b;
 }
 
-// batch->B rows on the device, uploaded on s: the columns the trainer's model reads, and the labels
-cudaError_t upload_rows(Scratch& sc, const srs_trainer* t, const srs_batch* b, const int32_t* labels, TrainRows* r,
-                        cudaStream_t s) {
+// batch->B rows on the device, uploaded on s: the columns the trainer's model reads, the labels and (not null) the
+// weights
+cudaError_t upload_rows(Scratch& sc, const srs_trainer* t, const srs_batch* b, const int32_t* labels,
+                        const float* weights, TrainRows* r, cudaStream_t s) {
   const size_t n = (size_t)b->B;
-  cudaError_t e = alloc_rows(sc, t, n, r);
+  cudaError_t e = alloc_rows(sc, t, n, weights != nullptr, r);
+  if (weights && e == cudaSuccess) e = cudaMemcpyAsync(r->weight, weights, n * 4, cudaMemcpyHostToDevice, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(r->movie, b->movie_id, n * 4, cudaMemcpyHostToDevice, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(r->user, b->user_id, n * 4, cudaMemcpyHostToDevice, s);
   if (e == cudaSuccess) e = cudaMemcpyAsync(r->label, labels, n * 4, cudaMemcpyHostToDevice, s);
@@ -303,9 +318,9 @@ cudaError_t upload_rows(Scratch& sc, const srs_trainer* t, const srs_batch* b, c
 }
 
 // `model.evaluate` of the trainer's current weights over n device rows, two launches on s: the serving forward, then
-// one metrics_update_kernel over all the rows into em
+// one metrics_update_kernel over all the rows into em (and, with r.weight, the weighted sums into wm through wred)
 cudaError_t eval_rows(const srs_trainer* t, const TrainRows& r, int n, float* probs, float* logits, int* err,
-                      MetricsState* em, cudaStream_t s) {
+                      MetricsState* em, MetricsWeighted* wm, MetricsWeightedReduce* wred, cudaStream_t s) {
   const BatchView b = view(r, 0, n, probs, logits, err);
   cudaError_t e;
   switch (t->spec.kind) {
@@ -315,23 +330,29 @@ cudaError_t eval_rows(const srs_trainer* t, const TrainRows& r, int n, float* pr
     default: e = launch_ncf(t->ncf, b, s); break;
   }
   if (e != cudaSuccess) return e;
+  if (r.weight)
+    return launch_metrics_update_weighted(probs, logits, r.label, r.weight, n, &em->cnt, &em->red, &em->loss, wm,
+                                          wred, 1, s);
   return launch_metrics_update(probs, logits, r.label, n, &em->cnt, &em->red, &em->loss, 1, s);
 }
 
 // The step of the trainer's model (not DIEN) over rows [off, off + B) of an epoch: the tile models read the
 // epoch's permuted rows, NeuralCF and two towers the dataset through `order` (the epoch's).  Points io.label at the
-// step's labels.
+// step's labels and, weighted, io.weight at the step's weights (NeuralCF and two towers: written by the step into
+// `weights`).
 cudaError_t launch_step(const srs_trainer* t, const TrainRows& src, const TrainRows& rows, const int32_t* order,
-                        int off, int B, int32_t* labels, StepIO& io, cudaStream_t s) {
+                        int off, int B, int32_t* labels, float* weights, StepIO& io, cudaStream_t s) {
   if (t->spec.kind == SRS_NEURALCF || t->spec.kind == SRS_TWOTOWERS) {
     const NcfStepArgs a{t->tab[0], t->blob[0], src.movie, src.user, src.label, order + off, B, t->spec.n_movies,
-                        io.b.probs, io.b.logits, labels, io.trow, io.gemb, io.part};
+                        io.b.probs, io.b.logits, labels, io.trow, io.gemb, io.part, src.weight, weights};
     io.label = labels;
+    io.weight = src.weight ? weights : nullptr;
     return t->spec.kind == SRS_TWOTOWERS ? launch_twotowers_train_step(&a, t->ncf, s)
                                          : launch_ncf_train_step(&a, t->ncf, s);
   }
   io.b = view(rows, off, B, io.b.probs, io.b.logits, io.b.err_flag);
   io.label = rows.label + off;
+  io.weight = rows.weight ? rows.weight + off : nullptr;
   switch (t->spec.kind) {
     case SRS_DEEPFM: {                                 // the tables come first in the placement
       DeepFmStepArgs a{t->fm, io, {}};
@@ -391,16 +412,19 @@ int check_orders(const int32_t* order, int n, int epochs) {
 }
 
 // A fit's device buffers that every model has: the order uploaded, each epoch's metrics state zeroed, and a
-// step's outputs and entry lists for up to Bmax rows
+// step's outputs and entry lists for up to Bmax rows; a weighted fit's weighted metrics and the step's weights
 struct FitBuffers {
   int32_t* order;                     // [epochs][n]
   MetricsState* met;                  // [epochs]
   int32_t* labels;                    // [Bmax] the step's labels (NeuralCF, DIEN: written by the step)
   StepIO io;                          // b.probs, b.logits, trow, gemb, part and (one-hot rows) frow, fgrad
+  MetricsWeighted* wmet;              // [epochs] weighted only, zeroed
+  MetricsWeightedReduce* wred;        //   its CTA partials (shared with validation: one stream)
+  float* weights;                     //   [Bmax] the step's weights (NeuralCF, two towers: written by the step)
 };
 
 cudaError_t alloc_fit(Scratch& sc, const srs_trainer* t, const int32_t* order, int n, int epochs, int Bmax,
-                      FitBuffers* f, cudaStream_t s) {
+                      bool weighted, FitBuffers* f, cudaStream_t s) {
   *f = FitBuffers{};
   const size_t ent = (size_t)t->n_ent * Bmax, fent = (size_t)t->n_fent * Bmax;
   cudaError_t e = sc.alloc(&f->order, (size_t)epochs * n);
@@ -415,6 +439,10 @@ cudaError_t alloc_fit(Scratch& sc, const srs_trainer* t, const int32_t* order, i
   if (e == cudaSuccess && fent) e = sc.alloc(&f->io.fgrad, fent);
   if (e == cudaSuccess) e = cudaMemcpyAsync(f->order, order, (size_t)epochs * n * 4, cudaMemcpyHostToDevice, s);
   if (e == cudaSuccess) e = cudaMemsetAsync(f->met, 0, sizeof(MetricsState) * epochs, s);
+  if (e == cudaSuccess && weighted) e = sc.alloc(&f->wmet, epochs);
+  if (e == cudaSuccess && weighted) e = sc.alloc(&f->wred, 1);
+  if (e == cudaSuccess && weighted) e = sc.alloc(&f->weights, Bmax);
+  if (e == cudaSuccess && weighted) e = cudaMemsetAsync(f->wmet, 0, sizeof(MetricsWeighted) * epochs, s);
   return e;
 }
 
@@ -626,40 +654,55 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
                                   int32_t batch_size, int32_t epochs, srs_eval_result* history,
                                   const srs_batch* val_batch, const int32_t* val_labels, int32_t val_freq,
                                   srs_eval_result* val_history) {
+  return srs_trainer_fit_weighted_host(t, batch, labels, nullptr, order, batch_size, epochs, history, val_batch,
+                                       val_labels, nullptr, val_freq, val_history);
+}
+
+int srs_trainer_fit_weighted_host(srs_trainer* t, const srs_batch* batch, const int32_t* labels, const float* weights,
+                                  const int32_t* order, int32_t batch_size, int32_t epochs, srs_eval_result* history,
+                                  const srs_batch* val_batch, const int32_t* val_labels, const float* val_weights,
+                                  int32_t val_freq, srs_eval_result* val_history) {
   if (!t || !batch || !labels || !order) return failf(SRS_ERR_INVALID, "null argument");
   if (t->spec.kind == SRS_DIEN) return dien_rejected("fit");
   const int n = batch->B;
   // every check before the first launch: a rejected call leaves the trainer as it was
   PROPAGATE(check_fit_sizes(n, batch_size, epochs));
-  PROPAGATE(check_rows(t, batch, labels, ""));
+  PROPAGATE(check_rows(t, batch, labels, weights, ""));
   PROPAGATE(check_orders(order, n, epochs));
   const int nv = val_batch ? val_batch->B : 0;         // validation rows; 0: no validation
   if (val_batch) {
     if (!val_labels) return failf(SRS_ERR_INVALID, "validation data: null labels");
     if (nv < 1) return failf(SRS_ERR_INVALID, "validation data: needs at least one row");
     if (val_freq < 1) return failf(SRS_ERR_INVALID, "validation_freq must be at least 1");
-    PROPAGATE(check_rows(t, val_batch, val_labels, "validation data: "));
+    PROPAGATE(check_rows(t, val_batch, val_labels, val_weights, "validation data: "));
   }
+  const bool vweighted = nv && val_weights;
   CUDA_TRY(cudaSetDevice(t->device));
   cudaStream_t s = t->stream;
   Scratch sc;
   FitBuffers f;
-  CUDA_TRY(alloc_fit(sc, t, order, n, epochs, std::min(batch_size, n), &f, s));
+  CUDA_TRY(alloc_fit(sc, t, order, n, epochs, std::min(batch_size, n), weights != nullptr, &f, s));
   TrainRows src{}, rows{};                             // the dataset, and (the tile models) the epoch's rows in order
-  CUDA_TRY(upload_rows(sc, t, batch, labels, &src, s));
-  if (t->permute) CUDA_TRY(alloc_rows(sc, t, n, &rows));
+  CUDA_TRY(upload_rows(sc, t, batch, labels, weights, &src, s));
+  if (t->permute) CUDA_TRY(alloc_rows(sc, t, n, weights != nullptr, &rows));
   CUDA_TRY(sc.alloc(&f.io.b.err_flag, 1));
   CUDA_TRY(cudaMemsetAsync(f.io.b.err_flag, 0, sizeof(int), s));
   // validation: its rows uploaded once, in file order; each validated epoch's metrics in its own state
   TrainRows vrows{};
   float *d_vprobs = nullptr, *d_vlogits = nullptr;
   MetricsState* d_vmet = nullptr;
+  MetricsWeighted* d_vwmet = nullptr;
   if (nv) {
-    CUDA_TRY(upload_rows(sc, t, val_batch, val_labels, &vrows, s));
+    CUDA_TRY(upload_rows(sc, t, val_batch, val_labels, vweighted ? val_weights : nullptr, &vrows, s));
     CUDA_TRY(sc.alloc(&d_vprobs, nv));
     CUDA_TRY(sc.alloc(&d_vlogits, nv));
     CUDA_TRY(sc.alloc(&d_vmet, epochs));
     CUDA_TRY(cudaMemsetAsync(d_vmet, 0, sizeof(MetricsState) * epochs, s));
+  }
+  if (vweighted) {
+    CUDA_TRY(sc.alloc(&d_vwmet, epochs));
+    CUDA_TRY(cudaMemsetAsync(d_vwmet, 0, sizeof(MetricsWeighted) * epochs, s));
+    if (!f.wred) CUDA_TRY(sc.alloc(&f.wred, 1));
   }
 
   int64_t steps = 0;
@@ -668,19 +711,30 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
     if (t->permute) CUDA_TRY(t->permute(src, rows, order_e, n, s));
     for (int off = 0; off < n; off += batch_size) {
       const int B = std::min(batch_size, n - off);
-      CUDA_TRY(launch_step(t, src, rows, order_e, off, B, f.labels, f.io, s));
+      CUDA_TRY(launch_step(t, src, rows, order_e, off, B, f.labels, f.weights, f.io, s));
       CUDA_TRY(update(t, f.io, B, s));
-      CUDA_TRY(launch_metrics_update(f.io.b.probs, f.io.b.logits, f.io.label, B, &f.met[e].cnt, &f.met[e].red,
-                                      &f.met[e].loss, 1, s));
+      if (f.io.weight)
+        CUDA_TRY(launch_metrics_update_weighted(f.io.b.probs, f.io.b.logits, f.io.label, f.io.weight, B,
+                                                &f.met[e].cnt, &f.met[e].red, &f.met[e].loss, &f.wmet[e], f.wred, 1,
+                                                s));
+      else
+        CUDA_TRY(launch_metrics_update(f.io.b.probs, f.io.b.logits, f.io.label, B, &f.met[e].cnt, &f.met[e].red,
+                                        &f.met[e].loss, 1, s));
       ++steps;
     }
     // after the epoch's last update, on the same stream: no host synchronisation
     if (nv && (e + 1) % val_freq == 0)
-      CUDA_TRY(eval_rows(t, vrows, nv, d_vprobs, d_vlogits, f.io.b.err_flag, &d_vmet[e], s));
+      CUDA_TRY(eval_rows(t, vrows, nv, d_vprobs, d_vlogits, f.io.b.err_flag, &d_vmet[e],
+                         d_vwmet ? &d_vwmet[e] : nullptr, f.wred, s));
   }
   std::vector<MetricsState> met(epochs), vmet(nv ? epochs : 0);
+  std::vector<MetricsWeighted> wmet(weights ? epochs : 0), vwmet(vweighted ? epochs : 0);
   CUDA_TRY(cudaMemcpyAsync(met.data(), f.met, sizeof(MetricsState) * epochs, cudaMemcpyDeviceToHost, s));
   if (nv) CUDA_TRY(cudaMemcpyAsync(vmet.data(), d_vmet, sizeof(MetricsState) * epochs, cudaMemcpyDeviceToHost, s));
+  if (weights)
+    CUDA_TRY(cudaMemcpyAsync(wmet.data(), f.wmet, sizeof(MetricsWeighted) * epochs, cudaMemcpyDeviceToHost, s));
+  if (vweighted)
+    CUDA_TRY(cudaMemcpyAsync(vwmet.data(), d_vwmet, sizeof(MetricsWeighted) * epochs, cudaMemcpyDeviceToHost, s));
   CUDA_TRY(cudaStreamSynchronize(s));
   t->iterations += steps;
   for (int e = 0; e < epochs; ++e) {
@@ -689,21 +743,32 @@ int srs_trainer_fit_validate_host(srs_trainer* t, const srs_batch* batch, const 
     if (validated && vmet[e].cnt.err)
       return failf(SRS_ERR_INVALID, "the validation of epoch %d produced a probability that is NaN or outside [0, 1]",
                    e);
-    if (history) metrics_summarise(met[e].cnt.hist, met[e].cnt.correct, met[e].loss, &history[e], nullptr);
+    if (history && weights)
+      metrics_summarise_weighted(met[e].cnt.hist, met[e].cnt.correct, wmet[e], met[e].loss, &history[e]);
+    else if (history)
+      metrics_summarise(met[e].cnt.hist, met[e].cnt.correct, met[e].loss, &history[e], nullptr);
     if (val_history) {
       val_history[e] = srs_eval_result{};
-      if (validated) metrics_summarise(vmet[e].cnt.hist, vmet[e].cnt.correct, vmet[e].loss, &val_history[e], nullptr);
+      if (validated && vweighted)
+        metrics_summarise_weighted(vmet[e].cnt.hist, vmet[e].cnt.correct, vwmet[e], vmet[e].loss, &val_history[e]);
+      else if (validated)
+        metrics_summarise(vmet[e].cnt.hist, vmet[e].cnt.correct, vmet[e].loss, &val_history[e], nullptr);
     }
   }
   return SRS_OK;
 }
 
 int srs_trainer_evaluate_host(srs_trainer* t, const srs_batch* batch, const int32_t* labels, srs_eval_result* out) {
+  return srs_trainer_evaluate_weighted_host(t, batch, labels, nullptr, out);
+}
+
+int srs_trainer_evaluate_weighted_host(srs_trainer* t, const srs_batch* batch, const int32_t* labels,
+                                       const float* weights, srs_eval_result* out) {
   if (!t || !batch || !labels || !out) return failf(SRS_ERR_INVALID, "null argument");
   if (t->spec.kind == SRS_DIEN) return dien_rejected("evaluate");
   const int n = batch->B;
   if (n < 1) return failf(SRS_ERR_INVALID, "evaluate needs at least one row");
-  PROPAGATE(check_rows(t, batch, labels, ""));
+  PROPAGATE(check_rows(t, batch, labels, weights, ""));
   CUDA_TRY(cudaSetDevice(t->device));
   cudaStream_t s = t->stream;
   Scratch sc;
@@ -711,19 +776,31 @@ int srs_trainer_evaluate_host(srs_trainer* t, const srs_batch* batch, const int3
   float *d_probs, *d_logits;
   int* d_err;
   MetricsState* d_met;
-  CUDA_TRY(upload_rows(sc, t, batch, labels, &rows, s));
+  MetricsWeighted* d_wmet = nullptr;
+  MetricsWeightedReduce* d_wred = nullptr;
+  CUDA_TRY(upload_rows(sc, t, batch, labels, weights, &rows, s));
   CUDA_TRY(sc.alloc(&d_probs, n));
   CUDA_TRY(sc.alloc(&d_logits, n));
   CUDA_TRY(sc.alloc(&d_err, 1));
   CUDA_TRY(sc.alloc(&d_met, 1));
   CUDA_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), s));
   CUDA_TRY(cudaMemsetAsync(d_met, 0, sizeof(MetricsState), s));
-  CUDA_TRY(eval_rows(t, rows, n, d_probs, d_logits, d_err, d_met, s));
+  if (weights) {
+    CUDA_TRY(sc.alloc(&d_wmet, 1));
+    CUDA_TRY(sc.alloc(&d_wred, 1));
+    CUDA_TRY(cudaMemsetAsync(d_wmet, 0, sizeof(MetricsWeighted), s));
+  }
+  CUDA_TRY(eval_rows(t, rows, n, d_probs, d_logits, d_err, d_met, d_wmet, d_wred, s));
   MetricsState met;
+  MetricsWeighted wmet;
   CUDA_TRY(cudaMemcpyAsync(&met, d_met, sizeof(met), cudaMemcpyDeviceToHost, s));
+  if (weights) CUDA_TRY(cudaMemcpyAsync(&wmet, d_wmet, sizeof(wmet), cudaMemcpyDeviceToHost, s));
   CUDA_TRY(cudaStreamSynchronize(s));
   if (met.cnt.err) return failf(SRS_ERR_INVALID, "evaluate produced a probability that is NaN or outside [0, 1]");
-  metrics_summarise(met.cnt.hist, met.cnt.correct, met.loss, out, nullptr);
+  if (weights)
+    metrics_summarise_weighted(met.cnt.hist, met.cnt.correct, wmet, met.loss, out);
+  else
+    metrics_summarise(met.cnt.hist, met.cnt.correct, met.loss, out, nullptr);
   return SRS_OK;
 }
 
@@ -778,9 +855,9 @@ int srs_trainer_fit_dien_host(srs_trainer* t, const srs_batch* batch, const int3
   cudaStream_t s = t->stream;
   Scratch sc;
   FitBuffers f;
-  CUDA_TRY(alloc_fit(sc, t, order, n, epochs, Bmax, &f, s));
+  CUDA_TRY(alloc_fit(sc, t, order, n, epochs, Bmax, false, &f, s));
   TrainRows src;                                       // movieId, userId and the labels
-  CUDA_TRY(upload_rows(sc, t, batch, labels, &src, s));
+  CUDA_TRY(upload_rows(sc, t, batch, labels, nullptr, &src, s));
   int32_t *d_ug, *d_mg, *d_hist, *d_neg = nullptr;
   float *d_num, *d_aux, *d_final, *d_rec;
   double *d_bloss, *d_auc, *d_aucsum;

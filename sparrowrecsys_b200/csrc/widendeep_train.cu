@@ -54,7 +54,7 @@ __global__ void __launch_bounds__(kThreads) widendeep_train_step_kernel(WideDeep
     const float pr = sigmoidf_acc(z);
     b.probs[row] = pr;
     b.logits[row] = z;
-    const float dz = (pr - (float)__ldg(a.io.label + row)) / (float)b.B;
+    const float dz = row_dz(pr, __ldg(a.io.label + row), a.io.weight, row, b.B);
     dzs[r] = dz;
     a.io.frow[row] = bucket;
     a.io.fgrad[row] = dz;
@@ -140,6 +140,7 @@ __global__ void widendeep_permute_kernel(TrainRows src, TrainRows dst, const int
   dst.user[i] = src.user[r];
   dst.rated[i] = src.rated[r];
   dst.label[i] = src.label[r];
+  if (src.weight) dst.weight[i] = src.weight[r];
 #pragma unroll
   for (int j = 0; j < 3; ++j) dst.mgenre[(size_t)i * 3 + j] = src.mgenre[(size_t)r * 3 + j];
 #pragma unroll

@@ -249,7 +249,8 @@ class CTRModel:
                                            top.ctypes.data))
         return idx, top
 
-    def evaluate(self, features: Mapping[str, object], labels=None, batch_size: Optional[int] = None):
+    def evaluate(self, features: Mapping[str, object], labels=None, batch_size: Optional[int] = None,
+                 sample_weight=None):
         """`model.evaluate(x)` of a model compiled as every reference script compiles it
         (loss='binary_crossentropy', metrics=['accuracy', AUC(curve='ROC'), AUC(curve='PR')]):
         returns (loss, accuracy, roc_auc, pr_auc), Keras's order.  `labels` defaults to
@@ -257,13 +258,18 @@ class CTRModel:
         (default: one) are scored and folded into the metrics on the device
         (`srs_evaluate_host_batches`); no score comes back.  ValueError for an out-of-range id, a bad
         label, a NaN or out-of-range probability, no rows, and the models evaluate does not cover
-        (DIEN; two towers without the final Dense)."""
-        r = self.evaluate_result(features, labels, batch_size)
+        (DIEN; two towers without the final Dense).  `sample_weight` ([N], Keras's `evaluate(...,
+        sample_weight=)`) gives the weighted metrics of DESIGN.md section 4.28; ValueError for a weight that is
+        negative, NaN or infinite or a length other than N (`training.sample_weights`)."""
+        r = self.evaluate_result(features, labels, batch_size, sample_weight)
         return r.loss, r.accuracy, r.roc_auc, r.pr_auc
 
-    def evaluate_result(self, features, labels=None, batch_size: Optional[int] = None) -> _lib.SrsEvalResult:
+    def evaluate_result(self, features, labels=None, batch_size: Optional[int] = None,
+                        sample_weight=None) -> _lib.SrsEvalResult:
         """`evaluate` with the counts: the `srs_eval_result` (rows, positives, correct and the four metrics)."""
+        from .training import sample_weights
         lab = _label_array(features, labels)
+        w = sample_weights(lab, sample_weight)
         enc = encode_batch(self.spec, features, narrow_ids=self.narrow_ids)
         n = enc.B
         if lab.shape[0] != n:
@@ -276,7 +282,11 @@ class CTRModel:
         structs = (_lib.SrsBatch * len(bounds))(*[_host_struct(enc.slice(lo, hi), keep) for lo, hi in bounds])
         lp = (C.c_void_p * len(bounds))(*[lab[lo:hi].ctypes.data for lo, hi in bounds])
         out = _lib.SrsEvalResult()
-        _lib.check(self._lib.srs_evaluate_host_batches(self._h, len(bounds), structs, lp, C.byref(out)))
+        if w is None:
+            _lib.check(self._lib.srs_evaluate_host_batches(self._h, len(bounds), structs, lp, C.byref(out)))
+            return out
+        wp = (C.c_void_p * len(bounds))(*[w[lo:hi].ctypes.data for lo, hi in bounds])
+        _lib.check(self._lib.srs_evaluate_weighted_host_batches(self._h, len(bounds), structs, lp, wp, C.byref(out)))
         return out
 
     # ---- DIEN's second output (DIEN.py:261-296) ---------------------------------------------------
@@ -458,16 +468,24 @@ class Metrics:
         import torch
         return (stream if stream is not None else torch.cuda.current_stream(self.device)).cuda_stream
 
-    def update_device(self, probs, logits, labels, stream=None):
+    def update_device(self, probs, logits, labels, stream=None, weights=None):
         """Fold n rows: `probs`, `logits` float32 and `labels` int32 CUDA tensors [n], asynchronous on
-        `stream` (a torch stream; default: torch's current stream)."""
+        `stream` (a torch stream; default: torch's current stream).  `weights` (float32 CUDA tensor [n]): Keras's
+        sample weights (DESIGN.md section 4.28); a state folds either weighted or unweighted rows between resets."""
         n = int(probs.numel())
-        for name, t, dt in (("probs", probs, "torch.float32"), ("logits", logits, "torch.float32"),
-                            ("labels", labels, "torch.int32")):
+        cols = [("probs", probs, "torch.float32"), ("logits", logits, "torch.float32"), ("labels", labels, "torch.int32")]
+        if weights is not None:
+            cols.append(("weights", weights, "torch.float32"))
+        for name, t, dt in cols:
             if str(t.dtype) != dt or not t.is_cuda or not t.is_contiguous() or int(t.numel()) != n:
                 raise ValueError("%s must be a contiguous %s CUDA tensor of %d elements" % (name, dt[6:], n))
-        _lib.check(self._lib.srs_metrics_update_device(self._h, probs.data_ptr(), logits.data_ptr(),
-                                                       labels.data_ptr(), n, self._stream(stream)))
+        if weights is None:
+            _lib.check(self._lib.srs_metrics_update_device(self._h, probs.data_ptr(), logits.data_ptr(),
+                                                           labels.data_ptr(), n, self._stream(stream)))
+        else:
+            _lib.check(self._lib.srs_metrics_update_weighted_device(self._h, probs.data_ptr(), logits.data_ptr(),
+                                                                    labels.data_ptr(), weights.data_ptr(), n,
+                                                                    self._stream(stream)))
 
     def reset(self, stream=None):
         _lib.check(self._lib.srs_metrics_reset(self._h, self._stream(stream)))

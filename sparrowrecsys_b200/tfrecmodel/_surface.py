@@ -59,14 +59,18 @@ class Surface:
             raise RuntimeError("tfrecmodel.%s: call load() before predict()" % self.name)
         return self.model.predict(features, batch_size)
 
-    def evaluate(self, features, batch_size: Optional[int] = None):
-        """(loss, accuracy, roc_auc, pr_auc) over the labelled rows (`features["label"]`)."""
+    def evaluate(self, features, batch_size: Optional[int] = None, sample_weight=None):
+        """(loss, accuracy, roc_auc, pr_auc) over the labelled rows (`features["label"]`), weighted by
+        `sample_weight` when given."""
         if self.model is None:
             raise RuntimeError("tfrecmodel.%s: call load() before evaluate()" % self.name)
-        return self.model.evaluate(features, batch_size=batch_size)
+        if sample_weight is None:
+            return self.model.evaluate(features, batch_size=batch_size)
+        return self.model.evaluate(features, batch_size=batch_size, sample_weight=sample_weight)
 
     def fit(self, features, epochs: int = 5, batch_size: int = 12, seed: int = 0, validation_data=None,
-            validation_split: float = 0.0, validation_freq: int = 1) -> dict:
+            validation_split: float = 0.0, validation_freq: int = 1, sample_weight=None,
+            class_weight=None) -> dict:
         """`model.fit(train_dataset, epochs=5)` (NeuralCF.py:91, DeepFM.py, WideNDeep.py:117,
         DeepFM_v2.py:165): train from the weights `model` was loaded with, then rebuild `model` from the trained
         weights.  Returns Keras's history dict, with the `val_*` lists when `validation_data` or
@@ -81,9 +85,11 @@ class Surface:
         from ..training import Trainer
         spec, device = self.model.spec, self.model.device
         with Trainer(spec, self.weights, device) as tr:
+            weighting = {} if sample_weight is None and class_weight is None else \
+                {"sample_weight": sample_weight, "class_weight": class_weight}
             history = tr.fit(features, epochs=epochs, batch_size=batch_size, seed=seed,
                              validation_data=validation_data, validation_split=validation_split,
-                             validation_freq=validation_freq)
+                             validation_freq=validation_freq, **weighting)
             trained = tr.weights()
         self.model.close()
         self.model = CTRModel(spec, trained, device)

@@ -23,8 +23,9 @@ def predict(features, batch_size=None):
     return _surface.predict(features, batch_size)
 
 
-def evaluate(features, batch_size=None):
-    return _surface.evaluate(features, batch_size)
+def evaluate(features, batch_size=None, sample_weight=None):
+    """`model.evaluate(x, sample_weight=...)`: (loss, accuracy, roc_auc, pr_auc), weighted when given."""
+    return _surface.evaluate(features, batch_size, sample_weight)
 
 
 def fit(features, epochs=5, batch_size=12, seed=0):

@@ -24,16 +24,19 @@ def predict(features, batch_size=None):
     return _surface.predict(features, batch_size)
 
 
-def evaluate(features, batch_size=None):
-    return _surface.evaluate(features, batch_size)
+def evaluate(features, batch_size=None, sample_weight=None):
+    """`model.evaluate(x, sample_weight=...)`: (loss, accuracy, roc_auc, pr_auc), weighted when given."""
+    return _surface.evaluate(features, batch_size, sample_weight)
 
 
-def fit(features, epochs=5, batch_size=12, seed=0, validation_data=None, validation_split=0.0, validation_freq=1):
+def fit(features, epochs=5, batch_size=12, seed=0, validation_data=None, validation_split=0.0, validation_freq=1,
+        sample_weight=None, class_weight=None):
     """`model.fit(train_dataset, epochs=5)`: train from the loaded weights on the GPU, then rebuild `model` from the
     trained weights; returns Keras's history dict {"loss", "accuracy", "auc", "auc_1"} (one value per epoch), plus
     "val_loss", "val_accuracy", "val_auc", "val_auc_1" for the validated epochs when `validation_data` or
-    `validation_split` is given (`Trainer.fit`)."""
+    `validation_split` is given (`Trainer.fit`).  `sample_weight` / `class_weight` as Keras's (`Trainer.fit`)."""
     global model
-    history = _surface.fit(features, epochs, batch_size, seed, validation_data, validation_split, validation_freq)
+    history = _surface.fit(features, epochs, batch_size, seed, validation_data, validation_split, validation_freq,
+                           sample_weight, class_weight)
     model = _surface.model
     return history

@@ -8,13 +8,14 @@ fit(train_dataset, epochs=5) over make_csv_dataset batches of 12), and of Neural
     history = tr.fit(train_features, epochs=5, batch_size=12, seed=0,
                      validation_data=test_features)       # optional: adds val_loss, val_accuracy, val_auc, val_auc_1
     loss, accuracy, roc_auc, pr_auc = tr.evaluate(test_features)   # the current weights, no export
+    tr.fit(train_features, sample_weight=w, class_weight={0: 1.0, 1: 3.0})   # Keras's per-row weights
     model = tr.to_model()                                 # a serving CTRModel built from the trained weights
 
 DIEN (DIEN.py:296-304: compile(optimizer="adam"), fit over batches of 12 with no shuffle) trains in file order
 every epoch by default and reports its own history {"loss", "auc", "auc_value"} (section 4.20).
 
 The forward, backward and Keras Adam run in the CUDA library (`srs_trainer_*`, include/srs_ctr.h; DESIGN.md
-sections 4.8, 4.9, 4.18, 4.19, 4.20 and 4.27).  For the other models TF's shuffle (buffer 10 000, unseeded) cannot be reproduced, so `fit` takes a seed instead: the host
+sections 4.8, 4.9, 4.18, 4.19, 4.20 and 4.27; sample weights 4.28).  For the other models TF's shuffle (buffer 10 000, unseeded) cannot be reproduced, so `fit` takes a seed instead: the host
 draws one `numpy.random.default_rng(seed).permutation(n)` per epoch and the library trains in that row order.
 """
 from __future__ import annotations
@@ -29,6 +30,46 @@ from .features import _as_ids, encode_batch, negative_history_keys
 from .model import CTRModel, _host_struct, _label_array, _spec_struct
 from .spec import ModelSpec
 from .weights import aux_weight_shapes, check_weights, weight_shapes
+
+
+def sample_weights(labels, sample_weight=None, class_weight=None) -> Optional[np.ndarray]:
+    """Keras's per-row weights (DESIGN.md section 4.28): w_i = sample_weight[i] * class_weight[label_i] in float32
+    (a factor that is not given is 1), or None when neither is given.  `sample_weight` is [n] (or [n, 1]) numeric;
+    `class_weight` maps the classes 0 and 1 to weights.  ValueError for a length other than the labels', a
+    class_weight key other than 0 or 1, or a weight (given or multiplied) that is negative, NaN or infinite."""
+    if sample_weight is None and class_weight is None:
+        return None
+    lab = np.asarray(labels).reshape(-1)
+    n = lab.shape[0]
+    w = np.ones(n, np.float32)
+    if sample_weight is not None:
+        sw = np.asarray(sample_weight)
+        if sw.ndim == 2 and sw.shape[1] == 1:
+            sw = sw[:, 0]
+        if sw.ndim != 1 or sw.shape[0] != n:
+            raise ValueError("sample_weight must be [%d] like the labels, got shape %s" % (n, sw.shape))
+        if sw.dtype.kind not in "biuf":
+            raise ValueError("sample_weight must be numeric")
+        with np.errstate(over="ignore"):
+            w = np.ascontiguousarray(sw, np.float32)
+    if class_weight is not None:
+        if not isinstance(class_weight, Mapping):
+            raise ValueError("class_weight must map the classes 0 and 1 to weights")
+        cw = np.ones(2, np.float32)
+        for k, v in class_weight.items():
+            if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or k not in (0, 1):
+                raise ValueError("class_weight keys must be the classes 0 and 1, got %r" % (k,))
+            with np.errstate(over="ignore"):
+                cw[int(k)] = np.float32(v)
+            if not (np.isfinite(cw[int(k)]) and cw[int(k)] >= 0):
+                raise ValueError("class_weight[%d] is %r: weights must be finite and >= 0" % (int(k), v))
+        with np.errstate(over="ignore", invalid="ignore"):
+            w = w * np.where(lab == 1, cw[1], cw[0]).astype(np.float32)
+    bad = ~(np.isfinite(w) & (w >= 0))
+    if bad.any():
+        i = int(np.argmax(bad))
+        raise ValueError("the weight of row %d is %r: weights must be finite and >= 0" % (i, float(w[i])))
+    return np.ascontiguousarray(w, np.float32)
 
 
 def epoch_orders(n: int, epochs: int, seed: int) -> np.ndarray:
@@ -103,7 +144,7 @@ class Trainer:
 
     def fit(self, features: Mapping[str, object], labels=None, epochs: int = 5, batch_size: int = 12, seed: int = 0,
             order=None, validation_data=None, validation_split: float = 0.0,
-            validation_freq: int = 1) -> Dict[str, list]:
+            validation_freq: int = 1, sample_weight=None, class_weight=None) -> Dict[str, list]:
         """`model.fit(dataset, epochs)`: train on the rows of `features` (the model's `predict` columns: `movieId`,
         `userId` for NeuralCF and two towers, also the 7 numerics, `movieGenre1` and `userGenre1` for DeepFM and DeepFM_v2, the 7 numerics, all eight
         genre columns and `userRatedMovie1` for Wide&Deep; labels default to
@@ -126,25 +167,35 @@ class Trainer:
         with (e + 1) % `validation_freq` == 0 end, after their last update, with `evaluate` of the current weights
         on the validation rows (one batch, in file order), logged as "val_loss", "val_accuracy", "val_auc" and
         "val_auc_1" for those epochs only.  Validation changes no weight, no Adam state and no training log.  Its
-        rows are checked like the training rows before anything runs."""
+        rows are checked like the training rows before anything runs.
+
+        Weights, as Keras's (DESIGN.md section 4.28): `sample_weight` [n] and `class_weight` {0: w0, 1: w1} weight
+        row i by sample_weight[i] * class_weight[label_i] (`sample_weights`).  A step's loss is then
+        sum w_i l_i / B, and the history's metrics are weighted.  `class_weight` applies to the training rows only;
+        `validation_data` may be `(x_val, y_val, val_sample_weight)`, and `validation_split` splits `sample_weight`
+        with the rows.  Weights are checked before anything runs.  DIEN: NotImplementedError (its loss carries the
+        auxiliary term)."""
         if self.spec.model == "dien":
+            if sample_weight is not None or class_weight is not None:
+                raise NotImplementedError("DIEN's fit takes no sample_weight or class_weight: its loss carries the "
+                                          "auxiliary negative-sample term")
             if validation_data is not None or validation_split or validation_freq != 1:
                 raise NotImplementedError("DIEN's fit takes no validation: DIEN.py validates nothing during fit")
             return self._fit_dien(features, labels, epochs, batch_size, order)
         res, vres, validated = self._fit(features, labels, epochs, batch_size, seed, order, validation_data,
-                                         validation_split, validation_freq)
+                                         validation_split, validation_freq, sample_weight, class_weight)
         out = _logs(res, "")
         if validated:
             out.update(_logs([vres[e] for e in validated], "val_"))
         return out
 
     def _fit(self, features, labels=None, epochs=5, batch_size=12, seed=0, order=None, validation_data=None,
-             validation_split=0.0, validation_freq=1):
+             validation_split=0.0, validation_freq=1, sample_weight=None, class_weight=None):
         """`fit`, returning the library's results: (the epochs' srs_eval_result, the validation's [epochs] with
         zeroed entries for epochs not validated, the validated epochs)."""
-        val = None
+        val, val_sw = None, None
         if validation_data is not None:
-            val = _validation_pair(validation_data)
+            val, val_sw = _validation_triple(validation_data)
         elif validation_split:
             split = float(validation_split)
             if not 0.0 < split < 1.0:
@@ -157,11 +208,15 @@ class Trainer:
                                  "validation_split=%r" % (n, validation_split))
             val = (_take(features, split_at, n), lab[split_at:])
             features, labels = _take(features, 0, split_at), lab[:split_at]
+            if sample_weight is not None:                     # split with the rows, checked over all n first
+                sw = sample_weights(lab, sample_weight)
+                sample_weight, val_sw = sw[:split_at], sw[split_at:]
         if isinstance(validation_freq, bool) or not isinstance(validation_freq, (int, np.integer)) \
                 or validation_freq < 1:
             raise ValueError("validation_freq must be an integer >= 1, got %r" % (validation_freq,))
         keep = []
         batch, lab, n = self._rows(features, labels, keep, "fit")
+        w = sample_weights(lab, sample_weight, class_weight)
         epochs, batch_size = int(epochs), int(batch_size)
         if order is None:
             order = epoch_orders(n, epochs, seed)
@@ -170,13 +225,20 @@ class Trainer:
             raise ValueError("order must be [epochs=%d][n=%d], got %s" % (epochs, n, order.shape))
         hist = (_lib.SrsEvalResult * max(epochs, 1))()
         vhist = (_lib.SrsEvalResult * max(epochs, 1))()
-        vbatch, vlab = None, None
+        vbatch, vlab, vw = None, None, None
         if val is not None:
             vb, vlab, _ = self._rows(val[0], val[1], keep, "validation")
             vbatch = C.byref(vb)
-        _lib.check(self._lib.srs_trainer_fit_validate_host(
-            self._h, C.byref(batch), lab.ctypes.data, order.ctypes.data, batch_size, epochs, hist, vbatch,
-            None if vlab is None else vlab.ctypes.data, int(validation_freq), vhist))
+            vw = sample_weights(vlab, val_sw)                 # class_weight is for the training rows only
+        if w is None and vw is None:
+            _lib.check(self._lib.srs_trainer_fit_validate_host(
+                self._h, C.byref(batch), lab.ctypes.data, order.ctypes.data, batch_size, epochs, hist, vbatch,
+                None if vlab is None else vlab.ctypes.data, int(validation_freq), vhist))
+        else:
+            _lib.check(self._lib.srs_trainer_fit_weighted_host(
+                self._h, C.byref(batch), lab.ctypes.data, None if w is None else w.ctypes.data, order.ctypes.data,
+                batch_size, epochs, hist, vbatch, None if vlab is None else vlab.ctypes.data,
+                None if vw is None else vw.ctypes.data, int(validation_freq), vhist))
         validated = [e for e in range(epochs) if val is not None and (e + 1) % validation_freq == 0]
         return list(hist[:epochs]), list(vhist[:epochs]), validated
 
@@ -202,24 +264,30 @@ class Trainer:
         res = list(hist[:epochs])
         return {"loss": [r.loss for r in res], "auc": [r.auc for r in res], "auc_value": [r.auc_value for r in res]}
 
-    def evaluate(self, features: Mapping[str, object], labels=None):
+    def evaluate(self, features: Mapping[str, object], labels=None, sample_weight=None):
         """`model.evaluate(x)` of the current weights: (loss, accuracy, roc_auc, pr_auc) over the rows of
         `features` in one batch, as `CTRModel.evaluate` of `to_model()` reports them (on CUDA cores), without
-        exporting the weights.  Errors as `fit`'s.  DIEN: NotImplementedError, as `tfrecmodel.dien.evaluate`: its
-        Keras evaluate is `to_model().dien_evaluate`."""
+        exporting the weights; weighted by `sample_weight` [n] when given (DESIGN.md section 4.28).  Errors as
+        `fit`'s.  DIEN: NotImplementedError, as `tfrecmodel.dien.evaluate`: its Keras evaluate is
+        `to_model().dien_evaluate`."""
         if self.spec.model == "dien":
             raise NotImplementedError("DIEN's Keras evaluate reports the loss with the auxiliary negative-sample term "
                                       "and its AUC metrics, not the four compile metrics; use "
                                       "Trainer.to_model().dien_evaluate")
-        r = self.evaluate_result(features, labels)
+        r = self.evaluate_result(features, labels, sample_weight)
         return r.loss, r.accuracy, r.roc_auc, r.pr_auc
 
-    def evaluate_result(self, features, labels=None) -> _lib.SrsEvalResult:
+    def evaluate_result(self, features, labels=None, sample_weight=None) -> _lib.SrsEvalResult:
         """`evaluate` with the counts: the `srs_eval_result` (rows, positives, correct and the four metrics)."""
         keep = []
         batch, lab, _ = self._rows(features, labels, keep, "evaluate")
+        w = sample_weights(lab, sample_weight)
         out = _lib.SrsEvalResult()
-        _lib.check(self._lib.srs_trainer_evaluate_host(self._h, C.byref(batch), lab.ctypes.data, C.byref(out)))
+        if w is None:
+            _lib.check(self._lib.srs_trainer_evaluate_host(self._h, C.byref(batch), lab.ctypes.data, C.byref(out)))
+        else:
+            _lib.check(self._lib.srs_trainer_evaluate_weighted_host(self._h, C.byref(batch), lab.ctypes.data,
+                                                                    w.ctypes.data, C.byref(out)))
         return out
 
     def _rows(self, features, labels, keep: list, what: str):
@@ -276,6 +344,15 @@ def _validation_pair(validation_data):
             and isinstance(validation_data[0], Mapping):
         return validation_data[0], validation_data[1]
     raise ValueError("validation_data must be (features, labels) or a feature dict with 'label'")
+
+
+def _validation_triple(validation_data):
+    """(features, labels, sample_weight or None) of `validation_data`: `_validation_pair`'s forms, or
+    `(x_val, y_val, val_sample_weight)`."""
+    if isinstance(validation_data, (tuple, list)) and len(validation_data) == 3 \
+            and isinstance(validation_data[0], Mapping):
+        return (validation_data[0], validation_data[1]), validation_data[2]
+    return _validation_pair(validation_data), None
 
 
 def _take(features, lo: int, hi: int) -> Dict[str, np.ndarray]:

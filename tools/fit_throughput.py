@@ -4,6 +4,7 @@ oracle on the host.
     python tools/fit_throughput.py [--model neuralcf|twotowers|deepfm|widendeep|deepfm_v2|dien] [--epochs 5]
                                    [--batch-sizes 12,4096]
                                    [--cpu-epochs 1] [--validate [--repeats 5]] [--kernels 4096]
+                                   [--sample-weight [--repeats 5]]
 
 Trains the reference script's run - the untrained model of `init_weights(default_spec(model), 0, for_test=False)`
 over the 88 827 rows of `tests/golden/<model>_trainset.npz` (two towers: `neuralcf_trainset.npz`, and the model is
@@ -19,7 +20,9 @@ size, scaled to µs per step (`--cpu-epochs 0` leaves it out).  `--validate` add
 fits of `--val-epochs` one-step epochs (the first batch of rows) with and without validation, where the two validation
 launches are a large part of each epoch, and `validated_minus_plain_s_per_epoch` from full-size fits (below the
 noise of a 7 403-step epoch).  Plain and validated fits alternate, `--repeats` pairs, medians.  `--kernels B` adds
-the device time of each kernel over one epoch at batch B (torch.profiler), per step.  Prints one JSON object with the card name and power limit read from nvidia-smi in the
+the device time of each kernel over one epoch at batch B (torch.profiler), per step.  `--sample-weight` adds the
+step time of a fit with Keras sample weights (DESIGN.md section 4.28; seeded weights in [0, 2) with every tenth row
+0) next to the unweighted one: `--repeats` alternating pairs of full fits, medians of µs per step.  Prints one JSON object with the card name and power limit read from nvidia-smi in the
 same run (and the model's name unless it is the default, NeuralCF).  Writes nothing.
 """
 import argparse
@@ -56,10 +59,14 @@ def main():
     ap.add_argument("--val-epochs", type=int, default=500)
     ap.add_argument("--repeats", type=int, default=5)
     ap.add_argument("--kernels", type=int, default=0, help="batch size of a per-kernel breakdown (0: none)")
+    ap.add_argument("--sample-weight", action="store_true",
+                    help="also time fits with per-row sample weights, alternating with unweighted ones")
     args = ap.parse_args()
     dien = args.model == "dien"
     if dien and args.validate:
         ap.error("DIEN's fit takes no validation")
+    if dien and args.sample_weight:
+        ap.error("DIEN's fit takes no sample weights")
     from oracle import deepfm_train, deepfm_v2_train, dien_train, ncf_train, twotowers_train, widendeep_train
     from sparrowrecsys_b200.spec import default_spec
     from sparrowrecsys_b200.training import Trainer
@@ -110,11 +117,17 @@ def main():
             val.update({k[5:]: extra[k] for k in extra.files if k.startswith("test_")})
         res["validation_rows"] = len(val["label"])
 
-    def timed_fit(B, validation_data=None, rows=None, epochs=args.epochs):
+    weights = None
+    if args.sample_weight:
+        weights = np.random.default_rng(7).uniform(0.0, 2.0, n).astype(np.float32)
+        weights[::10] = 0.0
+
+    def timed_fit(B, validation_data=None, rows=None, epochs=args.epochs, sample_weight=None):
         f = feats if rows is None else {k: v[:rows] for k, v in feats.items()}
         with Trainer(spec, W0) as tr:
             t0 = time.perf_counter()
-            hist = tr.fit(f, epochs=epochs, batch_size=B, seed=0, validation_data=validation_data)
+            hist = tr.fit(f, epochs=epochs, batch_size=B, seed=0, validation_data=validation_data,
+                          sample_weight=sample_weight)
             return time.perf_counter() - t0, hist
 
     def paired(B, **kw):
@@ -133,6 +146,13 @@ def main():
             _, extra_small = paired(B, rows=B, epochs=args.val_epochs)
             run.update({"gpu_epoch_s": plain / args.epochs, "validation_s_per_epoch": extra_small / args.val_epochs,
                         "validated_minus_plain_s_per_epoch": extra / args.epochs})
+        if weights is not None:                   # unweighted and weighted fits alternate
+            timed_fit(B, sample_weight=weights)   # warm-up of the weighted metrics kernel
+            pairs = [(timed_fit(B)[0], timed_fit(B, sample_weight=weights)[0]) for _ in range(args.repeats)]
+            plain = float(np.median([p for p, _ in pairs])) * 1e6 / steps
+            weighted = float(np.median([w for _, w in pairs])) * 1e6 / steps
+            run.update({"unweighted_us_per_step": plain, "weighted_us_per_step": weighted,
+                        "weighted_over_unweighted": weighted / plain})
         if args.cpu_epochs:
             orders = [np.arange(n)] * args.cpu_epochs if dien else ncf_train.epoch_orders(n, args.cpu_epochs, 0)
             t0 = time.perf_counter()
